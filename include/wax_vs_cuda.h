@@ -1,5 +1,5 @@
 /*
- * wax_vs_cuda.h -- C-ABI of libwaxvs_cuda.so: the B200 (sm_100a) brute-force vector scan + top-k
+ * wax_vs_cuda.h -- C-ABI of libwaxvs_cuda.so: the H100 (sm_90a) brute-force vector scan + top-k
  * that replaces WaxVectorSearch's Metal compute pipeline and CPU fallback behind the
  * `VectorSearchEngine` Swift protocol.
  *
@@ -300,7 +300,7 @@ int32_t wax_vs_debug_stream_read(wax_vs_engine *engine, uint32_t iters, float *o
 /* Tuning knobs for experiments ("variant", "ctas_per_sm", ...).  Unknown key -> WAX_VS_ERR_ARGUMENT. */
 int32_t wax_vs_debug_set_option(wax_vs_engine *engine, const char *key, int64_t value);
 
-/* Library build info: "waxvs_cuda <version> sm_100a ...". */
+/* Library build info: "waxvs_cuda <version> sm_90a ...". */
 const char *wax_vs_version(void);
 
 #ifdef __cplusplus

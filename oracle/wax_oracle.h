@@ -12,7 +12,7 @@
  *   known-answer the reference's tests hold for this path (tests/golden/reference_kats.json,
  *   transcribed with file:line) and nothing stronger exists upstream (SURVEY.md section 8c).
  *
- * What is restated (all paths relative to /root/reference):
+ * What is restated (all paths relative to the root of the Wax repository):
  *   - USearch metric formulas reached through VectorMetric.toUSearchMetric()
  *     (Sources/WaxVectorSearch/VectorMetric.swift:21-30): cos / ip / l2sq, as published in
  *     unum-cloud/USearch 2.23.0 include/usearch/index_plugins.hpp (metric_cos_gt, metric_ip_gt,

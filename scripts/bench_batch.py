@@ -14,8 +14,8 @@ ROOT = Path(__file__).resolve().parents[1]
 sys.path.insert(0, str(ROOT))
 from wax_b200 import CUDAVectorEngine, VectorMetric  # noqa: E402
 
-TF32_NOMINAL_TFLOPS = 1100.0   # dense TF32, B200 (B200_PROFILING.md nominal table; no measured TF32 peak is provided)
-BF16_NOMINAL_TFLOPS = 2250.0
+TF32_NOMINAL_TFLOPS = 495.0    # dense TF32, H100 SXM data sheet (used when no measured peak is present)
+BF16_NOMINAL_TFLOPS = 989.0    # dense BF16, H100 SXM data sheet
 try:
     _peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
 except Exception:  # noqa: BLE001
@@ -29,7 +29,7 @@ CONFIGS = [
          rows=10_000_000, dims=768, batch=256, k=100, normalize=False, seed=5),
 ]
 steps = int(sys.argv[1]) if len(sys.argv) > 1 else 5
-# nominations: "bf16" (default: kind::f16 MMAs over the bf16 shadow of the corpus) or "tf32" (from the fp32 corpus)
+# nominations: "bf16" (default: bf16 wgmmas over the bf16 shadow of the corpus) or "tf32" (from the fp32 corpus)
 nominate = sys.argv[2] if len(sys.argv) > 2 else "bf16"
 options = [kv.split("=") for kv in sys.argv[3:]]          # engine tuning options, e.g. batch_pair=1 batch_ares=0
 only = [int(v) for k, v in options if k == "only"]        # only=0 / only=1: run just that config

@@ -1,20 +1,21 @@
 #!/usr/bin/env python
 """CPU model (no GPU, no oracle): how often can level 1 of the batched path NOT prove a query of BASELINE configs[4]
-(10 M x 768 un-normalised rows, top-100 dot, 74 row slices of 135 135 rows) as a function of the nominee heap size per
+(10 M x 768 un-normalised rows, top-100 dot; on a 132-SM H100 two query groups share the SMs, 66 row slices of
+151 515 rows) as a function of the nominee heap size per
 (slice, query) and of the number of nominees the finish kernel re-scores?
 
 Scores of a unit query against uniform[-1,1]^768 rows are ~ N(0, 1/3); only the upper tail matters, so each slice's top-H
 scores are drawn from the exact order statistics (cumulative exponential spacings -> uniform order statistics -> normal
 quantiles).  The proof needs  s_k > max(max over slices of the slice's H-th best, the (R+1)-th nominee) + eps  with
 eps = 1.03 * 2^-7 * |q| * max|v| (+ accumulation slack), |q| = 1, max|v| ~ 16.  bf16 noise on the nominee ORDER is ignored
-(it adds a little): the measured rate with H = 16 was 6 of 6 144 (profiles/c5_proof_heap16_r02c.jsonl), the model says
-1-3 of 10 000; with H = 24 both are zero."""
+(it adds a little), so the model is a lower bound on the failure rate.  This is the Poisson tail argument behind the
+engine's heap-size cost model (enqueue_batch_tensor in wax_b200/csrc/waxvs_engine.cu)."""
 import sys
 
 import numpy as np
 from scipy.stats import norm
 
-S, n, k = 74, 135_135, 100
+S, n, k = 66, 151_515, 100
 sigma = np.sqrt(1 / 3)
 eps = (1.03 * 2 ** -7 * 1.01) * 1.0 * 16.0 + 768 * 2 ** -23 * 16
 trials = int(sys.argv[1]) if len(sys.argv) > 1 else 20_000

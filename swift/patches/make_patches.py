@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Generates swift/patches/*.patch: the call-site re-point of SURVEY.md section 8(f1) as unified diffs against the
-reference tree (christopherkarani/Wax at the revision under /root/reference).
+reference tree (a checkout of christopherkarani/Wax at the surveyed revision).
 
-    python swift/patches/make_patches.py [/root/reference]
+    python swift/patches/make_patches.py <path to the Wax checkout>
 
 What the patches do (nothing else of Wax is touched):
   * every closed enum that selects a vector engine gains `case cuda(CUDAVectorEngine)` under
@@ -15,9 +15,8 @@ What the patches do (nothing else of Wax is touched):
   * Package.swift gains the C module target `WaxVectorSearchCUDAC` (header + modulemap + `-lwaxvs_cuda`), Linux only,
     following the WaxCoreCompressionC precedent (Package.swift:54-73).
 
-The patches are mechanical rewrites of short, regular code (one-line switch arms); they are NOT compiled here -- this
-image has no Swift toolchain -- but `tests/test_swift_patches.py` checks that each applies cleanly (`git apply --check`)
-to a copy of the reference files and that applying them twice is rejected."""
+The patches are mechanical rewrites of short, regular code (one-line switch arms); they are NOT compiled (the project is built
+without a Swift toolchain); `git apply --check` against a Wax checkout shows that each applies cleanly."""
 from __future__ import annotations
 
 import difflib
@@ -26,7 +25,9 @@ import sys
 from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
-REF = Path(sys.argv[1]) if len(sys.argv) > 1 else Path("/root/reference")
+if len(sys.argv) != 2:
+    sys.exit("usage: python swift/patches/make_patches.py <path to a Wax checkout>")
+REF = Path(sys.argv[1])
 CUDA_IF, METAL_IF, ENDIF = "#if canImport(WaxVectorSearchCUDAC)", "#if canImport(Metal)", "#endif"
 
 

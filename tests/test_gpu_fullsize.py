@@ -94,7 +94,7 @@ def test_full_size_k72_and_k100_against_the_full_oracle_top100(oracle, full_engi
 
 def test_config2_full_size_batch_1024_top10_cosine(oracle, full_engine, c3_queries, c3_oracle_top100):
     """BASELINE configs[2] at its stated size: 10 M x 384, batch 1024, top-10 cosine through wax_vs_search_batch (the
-    tcgen05 nomination levels).  (1) the WHOLE batch equals the single-query fused scan on the GPU; (2) the sampled
+    wgmma nomination levels).  (1) the WHOLE batch equals the single-query fused scan on the GPU; (2) the sampled
     queries equal the streaming oracle -- ids and score bits in the kernels' accumulation order; (3) within 1e-4 and
     tie-aware order against the fp64 oracle."""
     t0, f0 = full_engine.batch_stats()

@@ -1,4 +1,4 @@
-"""wax_b200 -- B200-native (sm_100a) brute-force vector scan + top-k behind Wax's `VectorSearchEngine` surface.
+"""wax_b200 -- H100-native (sm_90a) brute-force vector scan + top-k behind Wax's `VectorSearchEngine` surface.
 
 Scope: the hot path named by BASELINE.json (SURVEY.md section 8) and nothing else.  The numeric work lives in
 libwaxvs_cuda.so (wax_b200/csrc, C-ABI in include/wax_vs_cuda.h); this package is the host-side mirror of

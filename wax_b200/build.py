@@ -1,4 +1,4 @@
-"""Build recipe for libwaxvs_cuda.so (sm_100a only, in-tree so the .so travels to the GPU box)."""
+"""Build recipe for libwaxvs_cuda.so (sm_90a only), written next to this file so the package imports from the tree."""
 from __future__ import annotations
 
 import os
@@ -13,7 +13,7 @@ LIB = PKG / "libwaxvs_cuda.so"
 SOURCES = ["waxvs_engine.cu"]
 HEADERS = ["waxvs_common.cuh", "waxvs_shard.cuh", "waxvs_scan.cuh", "waxvs_select.cuh", "waxvs_synth.cuh", "waxvs_batch.cuh"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-O3,-Wall",
     "-shared", "-cudart", "static",

@@ -1,15 +1,17 @@
 // waxvs_batch.cuh -- batched queries (BASELINE configs 3 and 5): a genuine dense contraction, so it runs on the
-// 5th-gen tensor cores.  score'[b][n] = sum_d Q[b][d] * V[n][d] as a skinny GEMM with tcgen05.mma kind::tf32:
+// Hopper tensor cores.  score'[b][n] = sum_d Q[b][d] * V[n][d] as a skinny GEMM with wgmma (tf32, or bf16 over a shadow):
 //
-//   A (M = 128 queries)  : TMA 2-D box [128 x 32 floats], 128-byte swizzle, K-major          (16 KB / k-block)
-//   B (N = 256 rows)     : TMA 2-D box [256 x 32 floats] of the row-major corpus, K-major     (32 KB / k-block)
-//   D                    : fp32 accumulators in TMEM, 128 lanes x 256 columns, double buffered (all 512 columns)
-//   warp roles           : warps 0-3 epilogue (thread t owns query t = TMEM lane t), warp 4 TMA producer,
-//                          warp 5 TMEM allocator + single-thread MMA issuer;  smem ring of 4 k-block stages.
+//   A (M = 128 queries)  : TMA 2-D box [128 rows x 128 bytes], 128-byte swizzle, K-major     (16 KB / k-block)
+//   B (N = 128 rows)     : TMA 2-D box [128 rows x 128 bytes] of the row-major corpus, K-major (16 KB / k-block)
+//   D                    : fp32 accumulators in the registers of one warpgroup, two m64n128 halves (128 per thread)
+//   warp roles           : warps 0-3 (one warpgroup) issue the wgmmas and run the epilogue (thread t owns query t),
+//                          warp 4 is the TMA producer;  smem ring of k-block stages (full / empty mbarriers).
 //
-// The score matrix (B x N, 40 GB at 1024 x 10 M) is never written: each epilogue thread scans its query's 256
-// accumulator columns straight out of TMEM (tcgen05.ld), scales by the row's cached 1/|v| (cosine) and keeps
-// the k' best (score', row) pairs of its row slice in a private max-heap (inserts are rare: O(k' ln(N/k'))).
+// The score matrix (B x N, 40 GB at 1024 x 10 M) is never written to global memory: the accumulators of a finished
+// tile are parked in a shared-memory score tile, the wgmmas of the NEXT tile are issued, and while the tensor cores
+// run them each epilogue thread scans its query's 128 scores of the parked tile, scales by the row's cached 1/|v|
+// (cosine) and keeps the k' best (score', row) pairs of its row slice in a private max-heap (inserts are rare:
+// O(k' ln(N/k'))).
 //
 // TF32 keeps 10 mantissa bits, which is not enough for the parity bar (scores within 1e-4, identical order),
 // so the tensor-core pass only NOMINATES candidates: batch_finish_kernel merges the slices' lists per query,
@@ -31,40 +33,41 @@
 
 namespace waxvs {
 
-constexpr int kBatchM = 128;            // queries per CTA  (UMMA M)
-constexpr int kBatchN = 256;            // corpus rows per tile (UMMA N)
+constexpr int kBatchM = 128;            // queries per CTA (two wgmma m64 halves)
+constexpr int kBatchN = 128;            // corpus rows per tile (wgmma N)
 constexpr int kBatchKBlock = 32;        // floats per k-block = one 128-byte swizzle atom
 constexpr int kBatchKBlockBf16 = 64;    // bf16 elements per k-block (the same 128 bytes)
-// Two shapes of the same kernel share the 227 KB of shared memory differently (template <STAGES, HEAP>):
-//   <4, 16>: four TMA stages (192 KB) + 16-entry nominee heaps (16 KB)  -- the pipeline is latency-bound on TMA
-//            (profiles/ncu_batch_tf32_r01b_summary.csv: 3 stages keep the tensor pipe 54 % busy), so the 4th stage
-//            matters; used whenever 16 nominees per slice are plenty (16 * slices >= 8 * k);
-//   <3, 64>: three stages + 64-entry heaps, for few slices or large k;
-//   <4, 24> (bf16 only: no scale area): four stages + 24-entry heaps, when k exceeds the slice count -- configs[4]'s
-//            top-100 over 74 slices left 1 query in 1 000 unproven with 16 nominees per slice (a slice that holds 16 rows
-//            within the bf16 bound of the 100th score), and every unproven query costs the batch a second pass.
-// PAIR = true is the cta_group::2 form: two CTAs of a cluster (two query groups, the same row slice) issue ONE
-// 256 x 256 x 8 MMA; each CTA stages only its own 128 query rows and HALF of the corpus tile (16 + 16 KB per
-// k-block instead of 16 + 32), so six stages fit where four did and the L2->SM traffic per SM drops by a third.
+// A launch shares the 227 KB of shared memory between the TMA ring (32 KB per stage; 16 KB when the queries are
+// resident), the resident queries (ARES: 16 KB per k-block), the 68 KB score tile and the nominee heaps (heap KB,
+// 16 / 24 / 32 / 64 entries).  Ring depth and heap size are launch parameters: larger heaps cost ring depth, so the
+// host picks the smallest heap that leaves the batch provable (see enqueue_batch_tensor).
 constexpr int kBatchRescore = 256;       // nominees of the union re-scored exactly per query (TF32 nominations)
 constexpr int kBatchRescoreMax = 1024;   // upper bound (BF16 nominations with larger k re-score more, see eps)
 constexpr uint32_t kBatchABytes = kBatchM * 128u;   // 16 KB
-constexpr uint32_t kBatchBBytes = kBatchN * 128u;   // 32 KB
+constexpr uint32_t kBatchBBytes = kBatchN * 128u;   // 16 KB
 constexpr uint32_t kBatchStageBytes = kBatchABytes + kBatchBBytes;
 constexpr int kBatchStageSlots = 8;      // staged nominees per epilogue thread before a forced flush
-__host__ __device__ constexpr uint32_t batch_stage_bytes(bool pair) { return kBatchABytes + (pair ? kBatchBBytes / 2 : kBatchBBytes); }
-__host__ __device__ constexpr uint32_t batch_smem_bytes(int stages, int heap, bool pair = false) {
-    return stages * batch_stage_bytes(pair) + 2048 /*scales*/ + 256 /*barriers*/ + kBatchStageSlots * kBatchM * 8 /*staging*/ +
+// Row stride of the score tile in floats: the padding makes the float2 fragment stores of a half-warp hit 32 banks.
+constexpr uint32_t kBatchScoreStride = kBatchN + 8;
+constexpr uint32_t kBatchScoreBytes = kBatchM * kBatchScoreStride * 4u;
+constexpr int kBatchMaxStages = 6;
+constexpr uint32_t kBatchSmemOptin = 227u * 1024u;
+// ares_kb = 0: the queries stream through the ring with the corpus; else ares_kb resident query k-blocks.
+__host__ __device__ constexpr uint32_t batch_smem_bytes(int stages, int heap, uint32_t ares_kb = 0) {
+    return ares_kb * kBatchABytes + stages * (ares_kb ? kBatchBBytes : kBatchStageBytes) + kBatchScoreBytes +
+           kBatchN * 4 /*scales*/ + 256 /*barriers*/ + kBatchStageSlots * kBatchM * 8 /*staging*/ +
            heap * kBatchM * 8 /*heaps*/ + 1024 /*align*/;
 }
-// ARES (queries resident in shared memory): `ares_kb` k-blocks of the 128 queries stay in shared memory for the whole
-// kernel (16 KB each: 6 k-blocks = 96 KB at 384 bf16 dims) and the ring stages carry the corpus only.
-__host__ __device__ constexpr uint32_t batch_ares_stage_bytes(bool pair) { return pair ? kBatchBBytes / 2 : kBatchBBytes; }
-__host__ __device__ constexpr uint32_t batch_ares_smem_bytes(int stages, int heap, bool pair, int ares_kb) {
-    return ares_kb * kBatchABytes + stages * batch_ares_stage_bytes(pair) + 256 + kBatchStageSlots * kBatchM * 8 +
-           heap * kBatchM * 8 + 1024;       // (bf16 only: no epilogue scale area)
+// deepest ring (<= kBatchMaxStages) that fits next to `heap`-entry heaps and `ares_kb` resident query k-blocks; 0 = none
+__host__ __device__ constexpr int batch_ring_stages(int heap, uint32_t ares_kb = 0) {
+    int st = kBatchMaxStages;
+    while (st > 0 && batch_smem_bytes(st, heap, ares_kb) > kBatchSmemOptin) --st;
+    return st;
 }
-constexpr int kBatchThreads = 192;
+static_assert(kBatchN == kBatchM, "the epilogue loads one row scale per thread");
+static_assert(batch_ring_stages(16) == 4 && batch_ring_stages(32) == 3 && batch_ring_stages(64) == 2,
+              "streamed-query shapes keep a useful ring next to every heap size");
+constexpr int kBatchThreads = 160;
 constexpr float kTf32Eps = 1.25f * 0x1p-9f;
 // BF16 nominations: both operands are ROUNDED to nearest; bf16 keeps 8 significand bits (7 stored), so the unit
 // round-off is 2^-8: |x~ - x| <= 2^-8 |x| each, |q~ v~ - q v| <= (2^-7 + 2^-16) |q v| termwise, hence
@@ -76,11 +79,12 @@ struct BatchParams {
     uint32_t n_rows, dims, n_queries;
     uint32_t groups;        // ceil(n_queries / 128)
     uint32_t slices;        // row slices; CTA b -> (group b % groups, slice b / groups)
-    uint32_t tiles_total;   // ceil(n_rows / 256)
-    uint32_t kprime;        // == HEAP of the kernel shape in use
+    uint32_t tiles_total;   // ceil(n_rows / 128)
+    uint32_t kprime;        // nominee heap entries per (slice, query): 16, 24, 32 or 64
+    uint32_t stages;        // TMA ring depth, 2 .. kBatchMaxStages (batch_ring_stages)
     int metric;             // kCosine or kDot
     const float *row_scale; // [n_rows] 1/|v| (cosine) or nullptr
-    uint64_t *heaps;        // [slices*groups][HEAP][128]: each CTA's heaps, dumped entry-major at the end
+    uint64_t *heaps;        // [slices*groups][kprime][128]: each CTA's heaps, dumped entry-major at the end
     uint32_t *tau_global;   // [n_queries] orderable(score') of the best k'-th nominee any slice has reached (0 = none)
     uint32_t no_insert;     // instrumentation: skip nominations (timing floor of the GEMM pipeline)
     // FILTER form (level 2): no heaps -- every row whose score' beats the query's FIXED threshold is appended to the
@@ -94,7 +98,7 @@ struct BatchParams {
     const uint32_t *allow_bits;
 };
 
-// ---- PTX wrappers (tcgen05 / TMA tensor) ---------------------------------------------------------------------
+// ---- PTX wrappers (TMA tensor loads, wgmma) ---------------------------------------------------------------------
 __device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int32_t c0,
                                             int32_t c1) {
     asm volatile(
@@ -109,51 +113,16 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap *map) {
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::tf32, one CTA.
-__device__ __forceinline__ void umma_tf32_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
+// CTA pair of a cluster (PAIR shapes): the same box lands at the same offset in the shared memory of both CTAs and
+// completes the transaction bytes on the mbarrier at the same offset in each.
+__device__ __forceinline__ void tma_load_2d_multicast(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int32_t c0,
+                                                      int32_t c1, uint16_t cta_mask) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(smem_dst)),
+        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
 }
-// kind::f16 (here: bf16 x bf16 -> fp32), one CTA: K = 16 elements = the same 32 bytes per MMA as tf32's K = 8.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// 32 lanes x 32 columns of 32-bit accumulators -> 32 registers (thread = lane, register j = column j).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ---- 2-CTA (cta_group::2) variants: the CTA pair of a cluster works as one 256-row MMA --------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -162,16 +131,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// TMA load issued by either CTA of the pair into its OWN shared memory; the transaction bytes are credited to the
-// LEADER CTA's mbarrier (peer bit of the shared::cluster address cleared, as cute::SM100_TMA_2SM_LOAD_2D does).
-__device__ __forceinline__ void tma_load_2d_pair(void *smem_dst, const CUtensorMap *map, uint64_t *bar, int32_t c0,
-                                                 int32_t c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-        : "memory");
 }
 // mbarrier.arrive on the barrier at the same offset in CTA `rank` of the cluster.
 __device__ __forceinline__ void mbar_arrive_remote(uint64_t *bar, uint32_t rank) {
@@ -182,70 +141,47 @@ __device__ __forceinline__ void mbar_arrive_remote(uint64_t *bar, uint32_t rank)
         "r"(rank)
         : "memory");
 }
-__device__ __forceinline__ void tcgen05_commit_pair(uint64_t *bar) {   // arrives on `bar` in BOTH CTAs of the pair
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"(static_cast<uint16_t>(3))
-        : "memory");
-}
-__device__ __forceinline__ void umma_tf32_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                  uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accesses of the accumulator registers across the asynchronous wgmmas.
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[64]) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void umma_bf16_ss_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                  uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// Shared-memory matrix descriptor, K-major, 128-byte swizzle (canonical layout ((8,n),2):((8,SBO),1) in 16-byte
-// units; rows 128 B apart, 8-row groups SBO = 1024 B apart).  Field layout: cute::UMMA::SmemDescriptor.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(const void *smem_tile) {
+// Shared-memory matrix descriptor for wgmma, K-major, 128-byte swizzle: rows 128 B apart, 8-row groups SBO = 1024 B
+// apart, LBO unused for swizzled K-major tiles.  Fields: start address >> 4 [0,14), LBO >> 4 [16,30), SBO >> 4 [32,46),
+// layout type [62,64) = 1 (SWIZZLE_128B).  The tile must be 1024-byte aligned; a K step of 32 bytes inside the swizzle
+// atom is +2 in the address field.
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(const void *smem_tile) {
     uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_u32(smem_tile) >> 4) & 0x3FFFu);  // start address  [0,14)
-    d |= static_cast<uint64_t>(1) << 16;                               // LBO (unused for swizzled K-major) [16,30)
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;                       // SBO [32,46)
-    d |= static_cast<uint64_t>(1) << 46;                               // descriptor version (Blackwell) [46,48)
-    d |= static_cast<uint64_t>(2) << 61;                               // layout type SWIZZLE_128B [61,64)
+    d |= static_cast<uint64_t>((smem_u32(smem_tile) >> 4) & 0x3FFFu);
+    d |= static_cast<uint64_t>(1) << 16;
+    d |= static_cast<uint64_t>(1024 >> 4) << 32;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = TF32, both K-major, M = 128, N = 256.
-__host__ __device__ constexpr uint32_t umma_idesc_tf32_m128_n256() {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
-}
-// cta_group::2: M = 256 (128 rows per CTA of the pair), N = 256.
-__host__ __device__ constexpr uint32_t umma_idesc_tf32_m256_n256() {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((256u >> 3) << 17) | ((256u >> 4) << 24);
-}
 
-// kind::f16 with A = B = BF16 (format 1), D = F32.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_m128_n256() {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((256u >> 3) << 17) | ((128u >> 4) << 24);
+// D (64 x 128 fp32, registers of the warpgroup) (+)= A (64 x K, smem) * B (128 x K, smem)^T for one 32-byte K step.
+__device__ __forceinline__ void wgmma_m64n128_tf32(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_m256_n256() {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((256u >> 3) << 17) | ((256u >> 4) << 24);
-}
-
-// max of three (FMNMX3 on sm_100; like fmaxf, a NaN input is dropped).
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-    float d;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-    return d;
+__device__ __forceinline__ void wgmma_m64n128_bf16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate));
 }
 
 // ---- per-thread nominee heap (max-heap on the ordering key: root = worst nominee) ----------------------------
@@ -257,16 +193,15 @@ __device__ __forceinline__ float nominee_score(uint64_t key) { return -from_orde
 
 // `heap` points at this thread's node 0 in shared memory; node i lives at heap[i * kBatchM] (entry-major, so the
 // 32 lanes of a warp touching the same level hit 32 different banks).  Returns the new root.
-template <int HEAP>
-__device__ __forceinline__ uint64_t heap_replace_root(uint64_t *heap, uint64_t x) {
+__device__ __forceinline__ uint64_t heap_replace_root(uint64_t *heap, uint32_t n, uint64_t x) {
     uint32_t i = 0;
 #pragma unroll 1
     for (;;) {
         const uint32_t l = 2 * i + 1;
-        if (l >= HEAP) break;
+        if (l >= n) break;
         const uint32_t r = l + 1;
         const uint64_t kl = heap[l * kBatchM];
-        const uint64_t kr = (r < HEAP) ? heap[r * kBatchM] : 0ull;
+        const uint64_t kr = (r < n) ? heap[r * kBatchM] : 0ull;
         const uint32_t c = (kr > kl) ? r : l;
         const uint64_t kc = (kr > kl) ? kr : kl;
         if (kc <= x) break;
@@ -344,13 +279,16 @@ __global__ void __launch_bounds__(256) shadow_bf16_kernel(const float *__restric
 }
 
 // ---- the tensor-core kernel ---------------------------------------------------------------------------------------
-// BF16: operands are bf16 (the corpus shadow + converted queries; 64 elements per 128-byte k-block, kind::f16 MMAs at
-//       twice the TF32 rate for the same bytes per cycle) -- nominations only, exactness comes from the finish kernel.
-// ARES: the CTA's 128 queries stay resident in shared memory (dims/64 bf16 k-blocks of 16 KB, loaded once), the ring
-//       stages carry only corpus tiles: a third less L2->SM and TMA->smem traffic per MMA.
+// BF16: operands are bf16 (the corpus shadow + converted queries; 64 elements per 128-byte k-block, wgmma k16 at twice
+//       the TF32 rate for the same bytes) -- nominations only, exactness comes from the finish kernel.
 // FILTER: the epilogue appends every row beating the query's fixed threshold to a per-query list instead of keeping
 //       the k' best in a heap (the filter level: complete by construction).
-template <int STAGES, int HEAP, bool PAIR, bool BF16 = false, bool ARES = false, bool FILTER = false>
+// ARES: the CTA's 128 queries stay resident in shared memory (num_kb k-blocks of 16 KB, loaded once); the ring stages
+//       carry only corpus tiles, which halves the TMA traffic per wgmma.
+// PAIR: a cluster of two CTAs (two query groups, the same row slice); each CTA loads HALF of every corpus tile and
+//       multicasts it into both CTAs' shared memory, so the pair reads each tile from L2 once instead of twice.  A
+//       stage is refilled only when the consumers of BOTH CTAs have released it.
+template <bool BF16, bool FILTER, bool ARES, bool PAIR>
 __global__ void __launch_bounds__(kBatchThreads, 1)
 batch_nominate_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c,
                       const BatchParams p) {
@@ -358,567 +296,264 @@ batch_nominate_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     // 1024-byte alignment for the 128B-swizzled tiles, computed as an OFFSET into the shared array so the compiler
     // keeps the shared address space (LDS/STS, not generic LD/ST).
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    constexpr uint32_t STAGE_BYTES = ARES ? batch_ares_stage_bytes(PAIR) : batch_stage_bytes(PAIR);
-    constexpr uint32_t B_OFF = ARES ? 0u : kBatchABytes;            // corpus tile offset inside a stage
-    constexpr uint32_t B_ROWS = PAIR ? kBatchN / 2 : kBatchN;       // corpus rows this CTA stages per tile
     constexpr uint32_t KB_ELEMS = BF16 ? kBatchKBlockBf16 : kBatchKBlock;   // elements per 128-byte k-block
+    constexpr uint32_t STAGE_BYTES = ARES ? kBatchBBytes : kBatchStageBytes;
+    constexpr uint32_t B_OFF = ARES ? 0u : kBatchABytes;                   // corpus tile offset inside a stage
     const uint32_t num_kb = p.dims / KB_ELEMS;
-    const uint32_t ares_bytes = ARES ? num_kb * kBatchABytes : 0u;   // resident queries: [kb][128 rows x 128 B]
-    uint8_t *a_res = smem;
-    uint8_t *stages = smem + ares_bytes;                               // [stage][A 16 KB | B 32 KB], 1024-aligned
-    // bf16 nominations never scale in the epilogue (the cosine shadow rows are pre-normalised): no scale area, which is
-    // what lets the <4 stages, 24-entry heaps> shape fit
-    constexpr uint32_t SCALE_BYTES = BF16 ? 0u : 2u * kBatchN * 4u;
-    float *scale_smem = reinterpret_cast<float *>(stages + STAGES * STAGE_BYTES);   // [2][256]
-    uint64_t *full = reinterpret_cast<uint64_t *>(stages + STAGES * STAGE_BYTES + SCALE_BYTES);   // [stages]
-    uint64_t *empty = full + STAGES;                                                   // [stages]
-    uint64_t *tmem_full = empty + STAGES;                                              // [2]
-    uint64_t *tmem_empty = tmem_full + 2;                                                    // [2]
-    uint64_t *a_full = tmem_empty + 2;                                                       // [1] (ARES)
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(a_full + 1);
-    uint64_t *stage_smem = reinterpret_cast<uint64_t *>(stages + STAGES * STAGE_BYTES + SCALE_BYTES + 256);  // [slots][128]
-    uint64_t *heap_smem = stage_smem + kBatchStageSlots * kBatchM;                                            // [64][128]
+    const uint32_t nst = p.stages, heap_n = p.kprime;
+    const uint32_t ares_bytes = ARES ? num_kb * kBatchABytes : 0u;
+    uint8_t *a_res = smem;                                                             // [kb][128 queries x 128 B]
+    uint8_t *stages = smem + ares_bytes;                                               // [stage][A 16 KB |] B 16 KB
+    float *score = reinterpret_cast<float *>(stages + nst * STAGE_BYTES);              // [128 queries][kBatchScoreStride]
+    float *scale_smem = score + kBatchM * kBatchScoreStride;                           // [128] 1/|v| of the parked tile
+    uint64_t *full = reinterpret_cast<uint64_t *>(scale_smem + kBatchN);               // [kBatchMaxStages]
+    uint64_t *empty = full + kBatchMaxStages;                                          // [kBatchMaxStages]
+    uint64_t *a_full = empty + kBatchMaxStages;                                        // [1] (ARES)
+    uint64_t *stage_smem = reinterpret_cast<uint64_t *>(reinterpret_cast<uint8_t *>(full) + 256);   // [slots][128]
+    uint64_t *heap_smem = stage_smem + kBatchStageSlots * kBatchM;                                   // [heap_n][128]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // PAIR: cluster c = (pair of groups c % (groups/2), slice c / (groups/2)); the CTA's rank picks the group.
     const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
     const uint32_t unit = PAIR ? blockIdx.x / 2u : blockIdx.x;
     const uint32_t units_per_slice = PAIR ? p.groups / 2u : p.groups;
     const uint32_t group = PAIR ? (unit % units_per_slice) * 2u + rank : unit % units_per_slice;
     const uint32_t slice = unit / units_per_slice;
-    const bool leader = rank == 0u;
     const uint32_t tile_lo = static_cast<uint32_t>(static_cast<uint64_t>(p.tiles_total) * slice / p.slices);
     const uint32_t tile_hi = static_cast<uint32_t>(static_cast<uint64_t>(p.tiles_total) * (slice + 1) / p.slices);
 
     if (warp == 4 && lane == 0) {
         tma_prefetch_desc(&tmap_q);
         tma_prefetch_desc(&tmap_c);
-        // PAIR: the leader's full[] collects both producers (its own expect_tx arrive + the peer's remote arrive) and
-        // its tmem_empty[] collects the 4 epilogue warps of both CTAs.
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], PAIR ? 2 : 1); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], PAIR ? 8 : 4); }
-        mbar_init(a_full, PAIR ? 2 : 1);
+        // full: the producer's expect_tx arrive + the TMA bytes (PAIR: half of the corpus bytes come from the peer's
+        // multicast); empty: one arrive per consumer warp of every CTA that writes into the stage
+        for (int s = 0; s < kBatchMaxStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], PAIR ? 8 : 4); }
+        mbar_init(a_full, 1);
         mbar_fence_init();
     }
-    if (warp == 5) {  // whole warp: allocate all 512 TMEM columns (2 accumulator buffers of 256)
-        if (PAIR) {
-            asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                         "r"(512)
-                         : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-        } else {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                         "r"(512)
-                         : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-    }
-    tcgen05_fence_before();
-    if (PAIR) cluster_sync_all(); else __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    if (PAIR) cluster_sync_all(); else __syncthreads();   // PAIR: the peer's barriers are initialised before any multicast
 
     if (warp == 4) {
         // ===== TMA producer =====
         if (lane == 0) {
-            if (ARES && tile_lo < tile_hi) {      // the CTA's queries, once: num_kb boxes of 128 rows x 128 B
-                if (PAIR) {
-                    if (leader) mbar_arrive_expect_tx(a_full, 2u * ares_bytes);
-                    else mbar_arrive_remote(a_full, 0u);
-                } else {
-                    mbar_arrive_expect_tx(a_full, ares_bytes);
-                }
-                for (uint32_t kb = 0; kb < num_kb; ++kb) {
-                    if (PAIR) tma_load_2d_pair(a_res + kb * kBatchABytes, &tmap_q, a_full, static_cast<int32_t>(kb * KB_ELEMS),
-                                               static_cast<int32_t>(group * kBatchM));
-                    else tma_load_2d(a_res + kb * kBatchABytes, &tmap_q, a_full, static_cast<int32_t>(kb * KB_ELEMS),
-                                     static_cast<int32_t>(group * kBatchM));
-                }
+            if (ARES && tile_lo < tile_hi) {      // the CTA's queries, once
+                mbar_arrive_expect_tx(a_full, ares_bytes);
+                for (uint32_t kb = 0; kb < num_kb; ++kb)
+                    tma_load_2d(a_res + kb * kBatchABytes, &tmap_q, a_full, static_cast<int32_t>(kb * KB_ELEMS),
+                                static_cast<int32_t>(group * kBatchM));
             }
             uint32_t stage = 0, phase = 0;
             for (uint32_t tile = tile_lo; tile < tile_hi; ++tile) {
                 for (uint32_t kb = 0; kb < num_kb; ++kb) {
                     mbar_wait_parity(&empty[stage], phase ^ 1u);
                     uint8_t *a = stages + stage * STAGE_BYTES;
-                    if (PAIR) {
-                        if (leader) mbar_arrive_expect_tx(&full[stage], 2u * STAGE_BYTES);   // both CTAs' bytes
-                        else mbar_arrive_remote(&full[stage], 0u);
-                        if (!ARES) tma_load_2d_pair(a, &tmap_q, &full[stage], static_cast<int32_t>(kb * KB_ELEMS),
-                                                    static_cast<int32_t>(group * kBatchM));
-                        tma_load_2d_pair(a + B_OFF, &tmap_c, &full[stage], static_cast<int32_t>(kb * KB_ELEMS),
-                                         static_cast<int32_t>(tile * kBatchN + rank * B_ROWS));
-                    } else {
-                        mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
-                        if (!ARES) tma_load_2d(a, &tmap_q, &full[stage], static_cast<int32_t>(kb * KB_ELEMS),
-                                               static_cast<int32_t>(group * kBatchM));
+                    mbar_arrive_expect_tx(&full[stage], STAGE_BYTES);
+                    if (!ARES)
+                        tma_load_2d(a, &tmap_q, &full[stage], static_cast<int32_t>(kb * KB_ELEMS), static_cast<int32_t>(group * kBatchM));
+                    if (PAIR)   // rows [64 rank, 64 rank + 64) of the tile, into both CTAs (same swizzle: 8-row atoms)
+                        tma_load_2d_multicast(a + B_OFF + rank * (kBatchBBytes / 2), &tmap_c, &full[stage],
+                                              static_cast<int32_t>(kb * KB_ELEMS),
+                                              static_cast<int32_t>(tile * kBatchN + rank * (kBatchN / 2)), 0x3);
+                    else
                         tma_load_2d(a + B_OFF, &tmap_c, &full[stage], static_cast<int32_t>(kb * KB_ELEMS),
                                     static_cast<int32_t>(tile * kBatchN));
-                    }
-                    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+                    if (++stage == nst) { stage = 0; phase ^= 1u; }
                 }
             }
         }
-    } else if (warp == 5) {
-        // ===== MMA issuer (one thread) =====
-        if (lane == 0 && leader) {      // PAIR: the leader CTA issues for both
-            constexpr uint32_t idesc = BF16 ? (PAIR ? umma_idesc_bf16_m256_n256() : umma_idesc_bf16_m128_n256())
-                                            : (PAIR ? umma_idesc_tf32_m256_n256() : umma_idesc_tf32_m128_n256());
-            if (ARES && tile_lo < tile_hi) { mbar_wait_parity(a_full, 0u); tcgen05_fence_after(); }
-            uint32_t stage = 0, phase = 0, t = 0;
-            for (uint32_t tile = tile_lo; tile < tile_hi; ++tile, ++t) {
-                const uint32_t acc = t & 1u, acc_phase = (t >> 1) & 1u;
-                mbar_wait_parity(&tmem_empty[acc], acc_phase ^ 1u);   // epilogue has drained this buffer
-                tcgen05_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * kBatchN;
-                for (uint32_t kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait_parity(&full[stage], phase);            // TMA bytes have landed
-                    tcgen05_fence_after();
-                    const uint8_t *a = stages + stage * STAGE_BYTES;
-                    const uint64_t da = umma_desc_k_sw128(ARES ? a_res + kb * kBatchABytes : a);
-                    const uint64_t db = umma_desc_k_sw128(a + B_OFF);
-#pragma unroll
-                    for (uint32_t j = 0; j < 4; ++j) {   // UMMA K = 8 tf32 / 16 bf16 = 32 bytes = +2 in the address field
-                        const uint32_t accum = (kb | j) != 0u ? 1u : 0u;
-                        if (BF16) {
-                            if (PAIR) umma_bf16_ss_pair(d_tmem, da + 2 * j, db + 2 * j, idesc, accum);
-                            else umma_bf16_ss(d_tmem, da + 2 * j, db + 2 * j, idesc, accum);
-                        } else {
-                            if (PAIR) umma_tf32_ss_pair(d_tmem, da + 2 * j, db + 2 * j, idesc, accum);
-                            else umma_tf32_ss(d_tmem, da + 2 * j, db + 2 * j, idesc, accum);
-                        }
-                    }
-                    if (PAIR) tcgen05_commit_pair(&empty[stage]);     // frees the stage in both CTAs
-                    else tcgen05_commit(&empty[stage]);               // frees the smem stage when the MMAs retire
-                    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-                }
-                if (PAIR) tcgen05_commit_pair(&tmem_full[acc]);       // accumulators complete -> both epilogues
-                else tcgen05_commit(&tmem_full[acc]);                 // accumulator complete -> epilogue
-            }
-        }
-    } else {
-        // ===== epilogue: thread t <-> query group*128 + t <-> TMEM lane t =====
-        // A nominee costs one compare against tau in the hot loop; winners are STAGED in shared memory and the
-        // whole warp flushes together (every lane sifts its own heap concurrently) so a lane's insert never idles
-        // the other 31.  tau is also shared across the slices of a query through tau_global: any slice's k'-th
-        // best is a valid filter for all of them (the union then holds >= k' nominees at or above it).
-        const uint32_t tid = threadIdx.x;                              // 0..127
-        const uint32_t q = group * kBatchM + tid;
-        const bool q_valid = q < p.n_queries && !p.no_insert;
-        uint64_t *heap = heap_smem + tid;
-        if (!FILTER) for (uint32_t i = 0; i < HEAP; ++i) heap[i * kBatchM] = WAXVS_KEY_NONE;
-        uint64_t root = WAXVS_KEY_NONE;                               // heap[0]: this slice's k'-th best so far
-        float tau = -INFINITY;
-        if (FILTER && q_valid) tau = __ldg(p.tau_fixed + q);          // never changes: the list is a pure filter
-        uint64_t *stage = stage_smem + tid;                           // slot i at stage[i * 128]
-        uint32_t cnt = 0;
-        bool improved = false;
-        auto flush = [&]() {
-            if (FILTER) {                                             // staged rows -> the query's global list
-                if (cnt) {
-                    const uint32_t base = atomicAdd(p.cand_count + q, cnt);
-                    for (uint32_t i = 0; i < cnt; ++i)
-                        if (base + i < p.cand_cap)
-                            p.cand_rows[static_cast<size_t>(q) * p.cand_cap + base + i] = static_cast<uint32_t>(stage[i * kBatchM]);
-                }
-                cnt = 0;
-                return;
-            }
-            for (uint32_t i = 0; i < cnt; ++i) {
-                const uint64_t x = stage[i * kBatchM];
-                if (x < root) { root = heap_replace_root<HEAP>(heap, x); improved = true; }
+        __syncwarp();
+        if (PAIR) cluster_sync_all();     // the peer may still multicast into / arrive on this CTA's shared memory
+        return;                           // the consumer warpgroup synchronises on named barrier 1 only
+    }
+
+    // ===== consumer warpgroup: wgmma issue + epilogue, thread t <-> query group*128 + t =====
+    // A nominee costs one compare against tau in the hot loop; winners are STAGED in shared memory and the
+    // whole warp flushes together (every lane sifts its own heap concurrently) so a lane's insert never idles
+    // the other 31.  tau is also shared across the slices of a query through tau_global: any slice's k'-th
+    // best is a valid filter for all of them (the union then holds >= k' nominees at or above it).
+    const uint32_t tid = threadIdx.x;                              // 0..127
+    const uint32_t q = group * kBatchM + tid;
+    const bool q_valid = q < p.n_queries && !p.no_insert;
+    uint64_t *heap = heap_smem + tid;
+    if (!FILTER) for (uint32_t i = 0; i < heap_n; ++i) heap[i * kBatchM] = WAXVS_KEY_NONE;
+    uint64_t root = WAXVS_KEY_NONE;                               // heap[0]: this slice's k'-th best so far
+    float tau = -INFINITY;
+    if (FILTER && q_valid) tau = __ldg(p.tau_fixed + q);          // never changes: the list is a pure filter
+    uint64_t *stage = stage_smem + tid;                           // slot i at stage[i * 128]
+    uint32_t cnt = 0;
+    bool improved = false;
+    auto flush = [&]() {
+        if (FILTER) {                                             // staged rows -> the query's global list
+            if (cnt) {
+                const uint32_t base = atomicAdd(p.cand_count + q, cnt);
+                for (uint32_t i = 0; i < cnt; ++i)
+                    if (base + i < p.cand_cap)
+                        p.cand_rows[static_cast<size_t>(q) * p.cand_cap + base + i] = static_cast<uint32_t>(stage[i * kBatchM]);
             }
             cnt = 0;
-            if (root != WAXVS_KEY_NONE) tau = fmaxf(tau, nominee_score(root));
-        };
-        const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
-        // The shared threshold is read one tile AHEAD (the L2 round trip of __ldcg would otherwise sit on every
-        // tile's critical path: with bf16 MMAs a tile lasts ~3000 cycles and the epilogue has no slack to hide it).
-        uint32_t g_next = 0;
-        uint32_t t = 0;
-        for (uint32_t tile = tile_lo; tile < tile_hi; ++tile, ++t) {
-            const uint32_t acc = t & 1u, acc_phase = (t >> 1) & 1u;
-            const uint32_t row0 = tile * kBatchN;
-            float *sc = scale_smem + acc * kBatchN;
-            if (!BF16 && p.row_scale) {
-#pragma unroll
-                for (uint32_t h = 0; h < 2; ++h) {
-                    const uint32_t r = row0 + tid + h * 128u;
-                    sc[tid + h * 128u] = (r < p.n_rows) ? __ldg(p.row_scale + r) : 0.0f;
-                }
-                asm volatile("bar.sync 1, 128;" ::: "memory");        // scales visible; previous use of sc[] finished
-            }
-            if (!FILTER && g_next) tau = fmaxf(tau, from_orderable_u32(g_next)); // adopt the best threshold any slice has published
-            mbar_wait_parity(&tmem_full[acc], acc_phase);
-            tcgen05_fence_after();
-            if (!FILTER && q_valid) g_next = __ldcg(p.tau_global + q); // consumed at the next tile
-            const uint32_t rows_here = min(static_cast<uint32_t>(kBatchN), p.n_rows - row0);
-#pragma unroll 1
-            for (uint32_t chunk = 0; chunk < kBatchN / 32; ++chunk) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_base + lane_base + acc * kBatchN + chunk * 32u, v);
-                if (chunk * 32u >= rows_here) continue;               // warp-uniform
-                // Hot path, branch-free: scale the 32 scores and take their max (max.f32 drops NaNs: FMNMX3, 17
-                // instructions for 32 values); only a chunk whose max beats tau (rare once the heap has warmed up)
-                // is examined column by column.  The rare path is deliberately COMPACT: the first version walked a
-                // fully unrolled max tree with the flush inlined at every leaf -- 200 KB of SASS, so every entry
-                // missed the instruction cache, which cost a quarter of the kernel once bf16 halved the MMA time.
-                float sv[32];
-                if (!BF16 && p.row_scale) {
-                    const float4 *sc4 = reinterpret_cast<const float4 *>(sc + chunk * 32u);
-#pragma unroll
-                    for (uint32_t j4 = 0; j4 < 8; ++j4) {
-                        const float4 w = sc4[j4];
-                        sv[4 * j4 + 0] = __uint_as_float(v[4 * j4 + 0]) * w.x;
-                        sv[4 * j4 + 1] = __uint_as_float(v[4 * j4 + 1]) * w.y;
-                        sv[4 * j4 + 2] = __uint_as_float(v[4 * j4 + 2]) * w.z;
-                        sv[4 * j4 + 3] = __uint_as_float(v[4 * j4 + 3]) * w.w;
-                    }
-                } else {
-#pragma unroll
-                    for (uint32_t j = 0; j < 32; ++j) sv[j] = __uint_as_float(v[j]);
-                }
-                float t11[11];
-#pragma unroll
-                for (uint32_t j = 0; j < 10; ++j) t11[j] = fmax3(sv[3 * j], sv[3 * j + 1], sv[3 * j + 2]);
-                t11[10] = fmaxf(sv[30], sv[31]);
-                const float u0 = fmax3(t11[0], t11[1], t11[2]), u1 = fmax3(t11[3], t11[4], t11[5]);
-                const float u2 = fmax3(t11[6], t11[7], t11[8]), u3 = fmaxf(t11[9], t11[10]);
-                const float cmax = fmaxf(fmax3(u0, u1, u2), u3);
-                if (cmax > tau && q_valid) {
-                    uint32_t mask = 0;
-#pragma unroll
-                    for (uint32_t j = 0; j < 32; ++j) mask |= (sv[j] > tau ? 1u : 0u) << j;
-                    const uint32_t cols = rows_here - chunk * 32u;                 // >= 1 here
-                    if (cols < 32u) mask &= (1u << cols) - 1u;
-                    // row0 + chunk * 32 is a multiple of 32: the chunk's 32 rows are exactly one word of the row filter
-                    if (p.allow_bits) mask &= __ldg(p.allow_bits + ((row0 + chunk * 32u) >> 5));
-                    while (mask) {
-                        if (cnt + __popc(mask) > kBatchStageSlots) flush();       // empties the slots, may raise tau
-                        uint32_t take = mask;
-                        if (__popc(mask) > kBatchStageSlots) {                     // warm-up only: lowest 8 set bits
-                            take = 0;
-#pragma unroll 1
-                            for (int i = 0; i < kBatchStageSlots; ++i) { const uint32_t bit = mask & (0u - mask); take |= bit; mask ^= bit; }
-                        } else {
-                            mask = 0;
-                        }
-#pragma unroll
-                        for (uint32_t j = 0; j < 32; ++j) {
-                            if ((take >> j) & 1u) {
-                                if (sv[j] > tau) { stage[cnt * kBatchM] = nominee_key(sv[j], row0 + chunk * 32u + j); ++cnt; }
-                            }
-                        }
-                    }
-                }
-            }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) {                                          // accumulator buffer is free again
-                if (PAIR) mbar_arrive_remote(&tmem_empty[acc], 0u);   // the leader's barrier gates the shared MMA
-                else mbar_arrive(&tmem_empty[acc]);
-            }
-            if (__any_sync(WAXVS_FULL_MASK, cnt >= kBatchStageSlots / 2)) {
-                flush();
-                if (!FILTER && improved && q_valid && root != WAXVS_KEY_NONE) {  // heap full: publish this slice's k'-th best
-                    atomicMax(p.tau_global + q, orderable_u32(nominee_score(root)));
-                    improved = false;
-                }
-            }
+            return;
         }
-        flush();
-        if (!FILTER) {
-            // dump this CTA's heaps (entry-major, coalesced) for batch_finish_kernel
-            uint64_t *dst = p.heaps + static_cast<size_t>(slice * p.groups + group) * HEAP * kBatchM + tid;
-            for (uint32_t i = 0; i < HEAP; ++i) dst[i * kBatchM] = heap[i * kBatchM];
+        for (uint32_t i = 0; i < cnt; ++i) {
+            const uint64_t x = stage[i * kBatchM];
+            if (x < root) { root = heap_replace_root(heap, heap_n, x); improved = true; }
         }
-    }
-    tcgen05_fence_before();
-    if (PAIR) cluster_sync_all(); else __syncthreads();   // PAIR: the peer may still arrive on / read this CTA's shared memory
-    if (warp == 5) {
-        tcgen05_fence_after();
-        if (PAIR) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-        else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
-    }
-}
+        cnt = 0;
+        if (root != WAXVS_KEY_NONE) tau = fmaxf(tau, nominee_score(root));
+    };
 
-
-// ---- TS + pair kernel: the queries live in TMEM ---------------------------------------------------------------------
-// Removes the shared-memory bandwidth bound of the SS shapes (DESIGN.md 4.5): the A operand (128 queries x dims
-// tf32 per CTA) is written ONCE into tensor memory (tcgen05.st, `dims` <= 384 columns) and every MMA reads it from
-// there (`tcgen05.mma ... [d], [a_tmem], b_desc`), so shared memory only carries the corpus: with the CTA pair each
-// CTA stages 32 rows x 32 floats = 4 KB per k-block per 128 MMA cycles (64 B/clk in + out instead of 192).
-//   TMEM columns: [0, dims) queries | [384, 448) accumulators 0 | [448, 512) accumulators 1   (N = 64 rows per tile)
-constexpr int kTsN = 64;                 // corpus rows per tile (UMMA N); each CTA of the pair stages half
-constexpr int kTsKbPerStage = 4;         // k-blocks per stage: 16 small MMAs per barrier round trip (a single thread
-                                         // cannot wait + commit every 128 cycles), so dims % 128 == 0
-constexpr int kTsStages = 6;
-constexpr uint32_t kTsBoxBytes = (kTsN / 2) * 128u;               // one k-block of this CTA's half tile: 4 KB
-constexpr uint32_t kTsStageBytes = kTsKbPerStage * kTsBoxBytes;  // 16 KB
-constexpr uint32_t kTsAccCol = 384;
-__host__ __device__ constexpr uint32_t batch_ts_smem_bytes(int heap) {
-    return kTsStages * kTsStageBytes + 2 * kTsN * 4 /*scales*/ + 1024 /*barriers*/ + kBatchStageSlots * kBatchM * 8 +
-           heap * kBatchM * 8 + 1024 /*align*/;
-}
-__host__ __device__ constexpr uint32_t umma_idesc_tf32_m256_n64() {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((64u >> 3) << 17) | ((256u >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32_ts_pair(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                                  uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-        "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-        "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-        : "memory");
-}
-
-template <int HEAP>
-__global__ void __launch_bounds__(kBatchThreads, 1)
-batch_tf32_ts_kernel(const __grid_constant__ CUtensorMap tmap_c, const float *__restrict__ queries, const BatchParams p) {
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t *stages = smem;                                                            // [stage][32 rows x 128 B]
-    float *scale_smem = reinterpret_cast<float *>(smem + kTsStages * kTsStageBytes);   // [2][64]
-    uint64_t *full = reinterpret_cast<uint64_t *>(scale_smem + 2 * kTsN);              // [stages]
-    uint64_t *empty = full + kTsStages;                                                // [stages]
-    uint64_t *tmem_full = empty + kTsStages;                                           // [2]
-    uint64_t *tmem_empty = tmem_full + 2;                                              // [2]
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tmem_empty + 2);
-    uint64_t *stage_smem = reinterpret_cast<uint64_t *>(smem + kTsStages * kTsStageBytes + 2 * kTsN * 4 + 1024);
-    uint64_t *heap_smem = stage_smem + kBatchStageSlots * kBatchM;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const uint32_t unit = blockIdx.x / 2u, units_per_slice = p.groups / 2u;
-    const uint32_t group = (unit % units_per_slice) * 2u + rank, slice = unit / units_per_slice;
-    const bool leader = rank == 0u;
-    const uint32_t tile_lo = static_cast<uint32_t>(static_cast<uint64_t>(p.tiles_total) * slice / p.slices);
-    const uint32_t tile_hi = static_cast<uint32_t>(static_cast<uint64_t>(p.tiles_total) * (slice + 1) / p.slices);
-    const uint32_t num_kb = p.dims / kBatchKBlock;
-
-    if (warp == 4 && lane == 0) {
-        tma_prefetch_desc(&tmap_c);
-        for (int s = 0; s < kTsStages; ++s) { mbar_init(&full[s], 2); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 8); }
-        mbar_fence_init();
-    }
-    if (warp == 5) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
-    __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp < 4) {
-        // queries -> TMEM: thread t writes query (group*128 + t) into lane t, columns [0, dims) (zeros if out of range)
-        const uint32_t q = group * kBatchM + threadIdx.x;
-        const float4 *src = reinterpret_cast<const float4 *>(queries + static_cast<size_t>(q) * p.dims);
-        const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
-        for (uint32_t c0 = 0; c0 < p.dims; c0 += 32u) {
-            uint32_t v[32];
+    // Scan rows [32 chunk, 32 chunk + 32) of the parked tile.  Hot path, branch-free: scale the 32 scores and take
+    // their max (fmaxf drops NaNs); only a chunk whose max beats tau (rare once the heap has warmed up) is examined
+    // column by column.  The rare path is deliberately COMPACT: a fully unrolled max tree with the flush inlined at
+    // every leaf is large enough to miss the instruction cache on every entry.
+    auto scan_chunk = [&](uint32_t row0, uint32_t rows_here, uint32_t chunk) {
+        if (chunk * 32u >= rows_here) return;                     // warp-uniform
+        const float4 *src = reinterpret_cast<const float4 *>(score + tid * kBatchScoreStride + chunk * 32u);
+        float sv[32];
+        if (!BF16 && p.row_scale) {
+            const float4 *sc4 = reinterpret_cast<const float4 *>(scale_smem + chunk * 32u);
 #pragma unroll
             for (uint32_t j4 = 0; j4 < 8; ++j4) {
-                float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (q < p.n_queries) x = __ldg(src + (c0 >> 2) + j4);
-                v[4 * j4 + 0] = __float_as_uint(x.x); v[4 * j4 + 1] = __float_as_uint(x.y);
-                v[4 * j4 + 2] = __float_as_uint(x.z); v[4 * j4 + 3] = __float_as_uint(x.w);
+                const float4 v = src[j4], w = sc4[j4];
+                sv[4 * j4 + 0] = v.x * w.x; sv[4 * j4 + 1] = v.y * w.y;
+                sv[4 * j4 + 2] = v.z * w.z; sv[4 * j4 + 3] = v.w * w.w;
             }
-            tmem_st_32x32(tmem_base + lane_base + c0, v);
-        }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-    }
-    tcgen05_fence_before();
-    cluster_sync_all();            // barriers initialised and both CTAs' queries resident before any MMA / remote arrive
-    tcgen05_fence_after();
-
-    if (warp == 4) {
-        // ===== TMA producer (both CTAs: each stages its half of the corpus tile) =====
-        if (lane == 0) {
-            uint32_t stage = 0, phase = 0;
-            for (uint32_t tile = tile_lo; tile < tile_hi; ++tile) {
-                for (uint32_t kb = 0; kb < num_kb; kb += kTsKbPerStage) {
-                    mbar_wait_parity(&empty[stage], phase ^ 1u);
-                    if (leader) mbar_arrive_expect_tx(&full[stage], 2u * kTsStageBytes);
-                    else mbar_arrive_remote(&full[stage], 0u);
+        } else {
 #pragma unroll
-                    for (uint32_t i = 0; i < kTsKbPerStage; ++i)
-                        tma_load_2d_pair(stages + stage * kTsStageBytes + i * kTsBoxBytes, &tmap_c, &full[stage],
-                                         static_cast<int32_t>((kb + i) * kBatchKBlock),
-                                         static_cast<int32_t>(tile * kTsN + rank * (kTsN / 2)));
-                    if (++stage == kTsStages) { stage = 0; phase ^= 1u; }
-                }
+            for (uint32_t j4 = 0; j4 < 8; ++j4) {
+                const float4 v = src[j4];
+                sv[4 * j4 + 0] = v.x; sv[4 * j4 + 1] = v.y; sv[4 * j4 + 2] = v.z; sv[4 * j4 + 3] = v.w;
             }
         }
-    } else if (warp == 5) {
-        // ===== MMA issuer: the leader CTA's single thread issues the 256-row MMAs for the pair =====
-        if (lane == 0 && leader) {
-            constexpr uint32_t idesc = umma_idesc_tf32_m256_n64();
-            uint32_t stage = 0, phase = 0, t = 0;
-            for (uint32_t tile = tile_lo; tile < tile_hi; ++tile, ++t) {
-                const uint32_t acc = t & 1u, acc_phase = (t >> 1) & 1u;
-                mbar_wait_parity(&tmem_empty[acc], acc_phase ^ 1u);
-                tcgen05_fence_after();
-                const uint32_t d_tmem = tmem_base + kTsAccCol + acc * kTsN;
-                for (uint32_t kb = 0; kb < num_kb; kb += kTsKbPerStage) {
-                    mbar_wait_parity(&full[stage], phase);
-                    tcgen05_fence_after();
+        float m[16];
 #pragma unroll
-                    for (uint32_t i = 0; i < kTsKbPerStage; ++i) {
-                        const uint64_t db = umma_desc_k_sw128(stages + stage * kTsStageBytes + i * kTsBoxBytes);
+        for (uint32_t j = 0; j < 16; ++j) m[j] = fmaxf(sv[j], sv[j + 16]);
 #pragma unroll
-                        for (uint32_t j = 0; j < kBatchKBlock / 8; ++j)   // A: 8 tf32 = 8 TMEM columns per K step
-                            umma_tf32_ts_pair(d_tmem, tmem_base + (kb + i) * kBatchKBlock + j * 8u, db + 2 * j, idesc,
-                                              (kb | i | j) != 0u ? 1u : 0u);
-                    }
-                    tcgen05_commit_pair(&empty[stage]);
-                    if (++stage == kTsStages) { stage = 0; phase ^= 1u; }
-                }
-                tcgen05_commit_pair(&tmem_full[acc]);
-            }
-        }
-    } else {
-        // ===== epilogue (same nomination scheme as batch_tf32_kernel, 64 columns per tile) =====
-        const uint32_t tid = threadIdx.x;
-        const uint32_t q = group * kBatchM + tid;
-        const bool q_valid = q < p.n_queries && !p.no_insert;
-        uint64_t *heap = heap_smem + tid;
-        for (uint32_t i = 0; i < HEAP; ++i) heap[i * kBatchM] = WAXVS_KEY_NONE;
-        uint64_t root = WAXVS_KEY_NONE;
-        float tau = -INFINITY;
-        uint64_t *stage = stage_smem + tid;
-        uint32_t cnt = 0;
-        bool improved = false;
-        auto flush = [&]() {
-            for (uint32_t i = 0; i < cnt; ++i) {
-                const uint64_t x = stage[i * kBatchM];
-                if (x < root) { root = heap_replace_root<HEAP>(heap, x); improved = true; }
-            }
-            cnt = 0;
-            if (root != WAXVS_KEY_NONE) tau = fmaxf(tau, nominee_score(root));
-        };
-        const uint32_t lane_base = static_cast<uint32_t>(warp * 32) << 16;
-        // the row scales of the NEXT tile are fetched while the current one is processed
-        float next_scale = 0.0f;
-        if (p.row_scale && tid < kTsN && tile_lo < tile_hi) {
-            const uint32_t r = tile_lo * kTsN + tid;
-            next_scale = (r < p.n_rows) ? __ldg(p.row_scale + r) : 0.0f;
-        }
-        uint32_t t = 0;
-        for (uint32_t tile = tile_lo; tile < tile_hi; ++tile, ++t) {
-            const uint32_t acc = t & 1u, acc_phase = (t >> 1) & 1u;
-            const uint32_t row0 = tile * kTsN;
-            float *sc = scale_smem + acc * kTsN;
-            if (p.row_scale && tid < kTsN) {
-                sc[tid] = next_scale;
-                const uint32_t r = row0 + kTsN + tid;
-                next_scale = (tile + 1 < tile_hi && r < p.n_rows) ? __ldg(p.row_scale + r) : 0.0f;
-            }
-            if (q_valid && (t & 7u) == 0u) {
-                const uint32_t g = __ldcg(p.tau_global + q);
-                if (g) tau = fmaxf(tau, from_orderable_u32(g));
-            }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
-            mbar_wait_parity(&tmem_full[acc], acc_phase);
-            tcgen05_fence_after();
-            const uint32_t rows_here = min(static_cast<uint32_t>(kTsN), p.n_rows - row0);
+        for (uint32_t w = 8; w >= 1; w >>= 1)
+#pragma unroll
+            for (uint32_t j = 0; j < w; ++j) m[j] = fmaxf(m[j], m[j + w]);
+        if (m[0] > tau && q_valid) {
+            uint32_t mask = 0;
+#pragma unroll
+            for (uint32_t j = 0; j < 32; ++j) mask |= (sv[j] > tau ? 1u : 0u) << j;
+            const uint32_t cols = rows_here - chunk * 32u;                 // >= 1 here
+            if (cols < 32u) mask &= (1u << cols) - 1u;
+            // row0 + chunk * 32 is a multiple of 32: the chunk's 32 rows are exactly one word of the row filter
+            if (p.allow_bits) mask &= __ldg(p.allow_bits + ((row0 + chunk * 32u) >> 5));
+            while (mask) {
+                if (cnt + __popc(mask) > kBatchStageSlots) flush();       // empties the slots, may raise tau
+                uint32_t take = mask;
+                if (__popc(mask) > kBatchStageSlots) {                     // warm-up only: lowest 8 set bits
+                    take = 0;
 #pragma unroll 1
-            for (uint32_t chunk = 0; chunk < kTsN / 32; ++chunk) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_base + lane_base + kTsAccCol + acc * kTsN + chunk * 32u, v);
-                if (chunk * 32u >= rows_here) continue;
-                float sv[32];
-                if (p.row_scale) {
-                    const float4 *sc4 = reinterpret_cast<const float4 *>(sc + chunk * 32u);
-#pragma unroll
-                    for (uint32_t j4 = 0; j4 < 8; ++j4) {
-                        const float4 w = sc4[j4];
-                        sv[4 * j4 + 0] = __uint_as_float(v[4 * j4 + 0]) * w.x;
-                        sv[4 * j4 + 1] = __uint_as_float(v[4 * j4 + 1]) * w.y;
-                        sv[4 * j4 + 2] = __uint_as_float(v[4 * j4 + 2]) * w.z;
-                        sv[4 * j4 + 3] = __uint_as_float(v[4 * j4 + 3]) * w.w;
-                    }
+                    for (int i = 0; i < kBatchStageSlots; ++i) { const uint32_t bit = mask & (0u - mask); take |= bit; mask ^= bit; }
                 } else {
-#pragma unroll
-                    for (uint32_t j = 0; j < 32; ++j) sv[j] = __uint_as_float(v[j]);
+                    mask = 0;
                 }
-                float m16[16], m8[8], m4[4], m2[2];
 #pragma unroll
-                for (uint32_t j = 0; j < 16; ++j) m16[j] = fmaxf(sv[j], sv[j + 16]);
-#pragma unroll
-                for (uint32_t j = 0; j < 8; ++j) m8[j] = fmaxf(m16[j], m16[j + 8]);
-#pragma unroll
-                for (uint32_t j = 0; j < 4; ++j) m4[j] = fmaxf(m8[j], m8[j + 4]);
-#pragma unroll
-                for (uint32_t j = 0; j < 2; ++j) m2[j] = fmaxf(m4[j], m4[j + 2]);
-                if (fmaxf(m2[0], m2[1]) > tau && q_valid) {
-                    auto leaf = [&](uint32_t j, float sj) {
-                        const uint32_t col = chunk * 32u + j;
-                        if (sj > tau && col < rows_here) {
-                            if (cnt == kBatchStageSlots) flush();
-                            stage[cnt * kBatchM] = nominee_key(sj, row0 + col);
-                            ++cnt;
-                        }
-                    };
-#pragma unroll
-                    for (uint32_t a = 0; a < 2; ++a) {
-                        if (!(m2[a] > tau)) continue;
-#pragma unroll
-                        for (uint32_t b = 0; b < 2; ++b) {
-                            const uint32_t i4 = a + 2 * b;
-                            if (!(m4[i4] > tau)) continue;
-#pragma unroll
-                            for (uint32_t c = 0; c < 2; ++c) {
-                                const uint32_t i8 = i4 + 4 * c;
-                                if (!(m8[i8] > tau)) continue;
-#pragma unroll
-                                for (uint32_t d = 0; d < 2; ++d) {
-                                    const uint32_t i16 = i8 + 8 * d;
-                                    if (!(m16[i16] > tau)) continue;
-                                    leaf(i16, sv[i16]);
-                                    leaf(i16 + 16, sv[i16 + 16]);
-                                }
-                            }
-                        }
+                for (uint32_t j = 0; j < 32; ++j) {
+                    if ((take >> j) & 1u) {
+                        if (sv[j] > tau) { stage[cnt * kBatchM] = nominee_key(sv[j], row0 + chunk * 32u + j); ++cnt; }
                     }
-                }
-            }
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_remote(&tmem_empty[acc], 0u);
-            if (__any_sync(WAXVS_FULL_MASK, cnt >= kBatchStageSlots / 2)) {
-                flush();
-                if (improved && q_valid && root != WAXVS_KEY_NONE) {
-                    atomicMax(p.tau_global + q, orderable_u32(nominee_score(root)));
-                    improved = false;
                 }
             }
         }
-        flush();
-        uint64_t *dst = p.heaps + static_cast<size_t>(slice * p.groups + group) * HEAP * kBatchM + tid;
-        for (uint32_t i = 0; i < HEAP; ++i) dst[i * kBatchM] = heap[i * kBatchM];
+    };
+    auto end_tile = [&]() {
+        if (__any_sync(WAXVS_FULL_MASK, cnt >= kBatchStageSlots / 2)) {
+            flush();
+            if (!FILTER && improved && q_valid && root != WAXVS_KEY_NONE) {  // heap full: publish this slice's k'-th best
+                atomicMax(p.tau_global + q, orderable_u32(nominee_score(root)));
+                improved = false;
+            }
+        }
+    };
+    auto release = [&](uint32_t s) {                              // this warp's wgmmas no longer read stage s
+        __syncwarp();
+        if (lane == 0) {
+            mbar_arrive(&empty[s]);
+            if (PAIR) mbar_arrive_remote(&empty[s], rank ^ 1u);  // the peer's producer also writes into this stage
+        }
+    };
+
+    float acc[2][64];                                             // [query half][fragment]
+    uint32_t ring = 0, phase = 0;
+    uint32_t prev_row0 = 0, prev_rows = 0;                        // the parked tile
+    bool parked = false;
+    uint32_t g_next = 0;
+    const uint32_t frag_row = static_cast<uint32_t>(warp) * 16u + (static_cast<uint32_t>(lane) >> 2);
+    const uint32_t frag_col = (static_cast<uint32_t>(lane) & 3u) * 2u;
+    if (ARES && tile_lo < tile_hi) mbar_wait_parity(a_full, 0u);
+    for (uint32_t tile = tile_lo; tile < tile_hi; ++tile) {
+        // (1) this tile's wgmmas, k-block by k-block; between k-blocks the parked tile's chunks are scanned
+        uint32_t held = 0;
+        for (uint32_t kb = 0; kb < num_kb; ++kb) {
+            mbar_wait_parity(&full[ring], phase);                 // TMA bytes have landed
+            const uint8_t *st = stages + ring * STAGE_BYTES;
+            const uint8_t *a = ARES ? a_res + kb * kBatchABytes : st;
+            const uint64_t da = wgmma_desc_k_sw128(a), da_hi = wgmma_desc_k_sw128(a + kBatchABytes / 2);
+            const uint64_t db = wgmma_desc_k_sw128(st + B_OFF);
+            __syncwarp();
+            wgmma_fence_operands(acc[0]); wgmma_fence_operands(acc[1]);
+            wgmma_fence();
+#pragma unroll
+            for (uint32_t j = 0; j < 4; ++j) {   // K = 8 tf32 / 16 bf16 = 32 bytes = +2 in the address field
+                const uint32_t accum = (kb | j) != 0u ? 1u : 0u;
+                if (BF16) {
+                    wgmma_m64n128_bf16(acc[0], da + 2 * j, db + 2 * j, accum);
+                    wgmma_m64n128_bf16(acc[1], da_hi + 2 * j, db + 2 * j, accum);
+                } else {
+                    wgmma_m64n128_tf32(acc[0], da + 2 * j, db + 2 * j, accum);
+                    wgmma_m64n128_tf32(acc[1], da_hi + 2 * j, db + 2 * j, accum);
+                }
+            }
+            wgmma_commit();
+            wgmma_fence_operands(acc[0]); wgmma_fence_operands(acc[1]);
+            if (kb > 0) { wgmma_wait<1>(); release(held); }      // the previous k-block's wgmmas have retired
+            held = ring;
+            if (++ring == nst) { ring = 0; phase ^= 1u; }
+            if (parked && kb < kBatchN / 32u) scan_chunk(prev_row0, prev_rows, kb);
+        }
+        if (parked) {
+            for (uint32_t c = num_kb; c < kBatchN / 32u; ++c) scan_chunk(prev_row0, prev_rows, c);
+            end_tile();
+        }
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc[0]); wgmma_fence_operands(acc[1]);
+        release(held);
+        // (2) park this tile: every thread has finished reading the previous one
+        const uint32_t row0 = tile * kBatchN;
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+#pragma unroll
+        for (uint32_t h = 0; h < 2; ++h) {
+            float *dst = score + (h * 64u + frag_row) * kBatchScoreStride + frag_col;
+#pragma unroll
+            for (uint32_t j = 0; j < 16; ++j) {
+                *reinterpret_cast<float2 *>(dst + 8u * j) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+                *reinterpret_cast<float2 *>(dst + 8u * kBatchScoreStride + 8u * j) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+            }
+        }
+        if (!BF16 && p.row_scale) {
+            const uint32_t r = row0 + tid;
+            scale_smem[tid] = (r < p.n_rows) ? __ldg(p.row_scale + r) : 0.0f;
+        }
+        asm volatile("bar.sync 1, 128;" ::: "memory");
+        // The shared threshold is read one tile AHEAD, so its L2 round trip is off the critical path.
+        if (!FILTER && g_next) tau = fmaxf(tau, from_orderable_u32(g_next)); // adopt the best threshold any slice has published
+        if (!FILTER && q_valid) g_next = __ldcg(p.tau_global + q);
+        prev_row0 = row0;
+        prev_rows = min(static_cast<uint32_t>(kBatchN), p.n_rows - row0);
+        parked = true;
     }
-    tcgen05_fence_before();
-    cluster_sync_all();
-    if (warp == 5) {
-        tcgen05_fence_after();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
+    if (parked) {
+        for (uint32_t c = 0; c < kBatchN / 32u; ++c) scan_chunk(prev_row0, prev_rows, c);
+        end_tile();
     }
+    flush();
+    if (!FILTER) {
+        // dump this CTA's heaps (entry-major, coalesced) for batch_finish_kernel
+        uint64_t *dst = p.heaps + static_cast<size_t>(slice * p.groups + group) * heap_n * kBatchM + tid;
+        for (uint32_t i = 0; i < heap_n; ++i) dst[i * kBatchM] = heap[i * kBatchM];
+    }
+    if (PAIR) cluster_sync_all();     // the peer may still multicast into / arrive on this CTA's shared memory
 }
 
 // ---- exact re-score + proof ------------------------------------------------------------------------------------------

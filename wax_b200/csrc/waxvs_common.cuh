@@ -1,4 +1,4 @@
-// waxvs_common.cuh -- shared device helpers for the B200 (sm_100a) vector-scan kernels.
+// waxvs_common.cuh -- shared device helpers for the H100 (sm_90a) vector-scan kernels.
 //
 // Ordering key.  Every candidate is a 64-bit key  (orderable(distance) << 32) | local_row  so that the
 // total order (distance ascending, row ascending) -- the order the oracle fixes, see

@@ -1,6 +1,6 @@
 // waxvs_engine.cu -- host side of libwaxvs_cuda.so: the engine object behind include/wax_vs_cuda.h.
 //
-// What it mirrors (all /root/reference paths): the state and behaviour of
+// What it mirrors (paths relative to the Wax repository root): the state and behaviour of
 //   actor MetalVectorEngine            Sources/WaxVectorSearch/MetalVectorEngine.swift:17-893
 // with USearchVectorEngine's metric coverage (USearchVectorEngine.swift:44-67) -- the corpus matrix resident
 // on the device (here: HBM, row-major fp32), a frameIds side array, a pool of per-search scratch contexts
@@ -124,19 +124,18 @@ struct Tuning {
     int l2_hint = 0;
     int ldg_ctas_per_sm = 4;
     int chunk_steps = -1;   // dynamic scheduling granularity of the TMA kernel: -1 auto (8 steps, fewer when the corpus gives
-                            // each warp only a few steps: 10 K rows = 2 500 steps over 1 184 warps), 0 = static round-robin
+                            // each warp only a few steps, e.g. 10 K rows x 4 rows per step = 2 500 steps over 1 056 warps), 0 = static round-robin
     int fused_k_max = 128;  // k <= this stays in the single fused launch (register lists); larger k: emit + radix select
-    int batch_tensor = 1;   // 1: batches take the tcgen05 TF32 nominate + exact re-score path when eligible
+    int batch_tensor = 1;   // 1: batches take the wgmma TF32 nominate + exact re-score path when eligible
     int batch_min = 4;      // smallest batch routed to the tensor path
     int time_overlap = 0;   // wax_vs_debug_time_search: alternate consecutive queries over two streams
-    int batch_pair = 0;     // 1: cta_group::2 CTA pairs for the SS shapes (validated; no net gain, see DESIGN 4.5)
-    int batch_ts = 0;       // 1: queries in TMEM + CTA pairs (dims <= 384, dims % 128 == 0)
+    int batch_pair = 0;     // 1: CTA pairs of a cluster share each corpus tile through a TMA multicast (needs >= 2 groups)
     uint32_t tma_max_dims = 4096;   // generic TMA shape up to this row length, the direct-load kernel above
     int batch_large_k = 1;  // batches with 128 < k <= 1024 take the tensor-core levels (0: loop the single-query emit + select path)
     int batch_heap = 0;     // 0 auto (cost model + adaptive bump), 16 / 24 / 32 / 64: nominee heap size per (slice, query) = kernel shape
     int batch_noinsert = 0; // instrumentation: GEMM pipeline only (results meaningless)
-    int batch_bf16 = 1;     // 1: nominate from a bf16 shadow of the corpus when HBM allows (kind::f16 MMAs, 2x the TF32 rate; +dims*2 B/row)
-    int batch_ares = 1;     // with batch_bf16: keep the CTA's queries resident in shared memory when they fit (dims <= 512)
+    int batch_bf16 = 1;     // 1: nominate from a bf16 shadow of the corpus when HBM allows (bf16 wgmma, 2x the TF32 rate; +dims*2 B/row)
+    int batch_ares = 1;     // with batch_bf16: keep the CTA's queries resident in shared memory when a 2-stage ring still fits
     int batch_rescore = 0;  // 0 auto; else nominees re-scored exactly per query (256, 512 or 1024)
     int batch_retry = 1;    // queries level 1 cannot prove go through the filter level (TF32, complete by construction) before an exact scan
     int filter_bf16 = 1;    // unproven queries first get a filter pass over the bf16 shadow (half the bytes of an exact scan)
@@ -146,7 +145,7 @@ struct Tuning {
     int tail_select = 1;    // TMA-staged kernels: radix-selection tail instead of pairwise list merges (same results)
     int shard_fused = 1;    // sharded search: exchange + merge inside the scan launch (0: separate 1-CTA launch)
     int single_shadow = 0;  // 1: single queries / batches below batch_min also take the bf16-shadow nominations
-                            // (half the HBM bytes per query: 1.19 vs 2.04 ms at 10 M x 384, same results); off by
+                            // (half the HBM bytes per query, same results); off by
                             // default: the plain single-query path is the fused fp32 scan BASELINE's north_star names
 };
 
@@ -188,7 +187,7 @@ struct SearchCtx {
 
 struct wax_vs_engine {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     size_t smem_optin = 0;
     uint32_t dims = 0;
     uint8_t similarity = 0;
@@ -415,19 +414,19 @@ static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0
         if (c == 1 || c == 2 || c == 3 || c == 4 || c == 6 || c == 8 || c == 12) C = c;   // unrolled shapes (12: the 1536-dim embeddings)
     }
     if (C == 0 && d < 32) return false;                  // a few floats per row: the direct-load kernel
-    if (C == 0 && d > e->tune.tma_max_dims) return false;   // very long rows: too few warps fit beside two stages; the
-                                                             // direct-load kernel streams them at 6.9 TB/s (sweep_long_r02t)
-    // rows per step / warps per CTA by row length (profiles/dims_sweep_r01_call17.json): keep a step at >= 4-12 KB
-    // and give short rows more warps (their bound is per-row instruction latency, not bytes in flight)
+    if (C == 0 && d > e->tune.tma_max_dims) return false;   // very long rows: too few warps fit beside two stages, the
+                                                             // direct-load kernel takes them
+    // Rows per step / warps per CTA by row length: keep a step at >= 4-12 KB and give short rows more warps (their bound
+    // is per-row instruction latency, not bytes in flight).  These defaults were chosen on B200, not re-tuned on H100; the
+    // `rows_per_step` / `warps` / `stages` options override them.
     int R, warps_default = 8;
     if (C == 0) {                                        // generic shape: run-time chunk count, query in shared memory
         // keep a step at >= 2-8 KB: short generic rows (dims < 128, 160, 300, 400, ...) take 8 or 4 rows per step and
-        // more warps, like the unrolled C <= 2 shapes (profiles/small_dims_sweep_r02*.jsonl)
-        // (long rows: as many rows as keep a step at <= 32 KB -- the few warps that then fit still hold ~190 KB in flight,
-        // profiles/small_dims_sweep_r02h.jsonl / sweep_big_r02i.jsonl: 1000 dims 6.1 -> 7.3 TB/s, 2048 dims 6.5 -> 7.3)
+        // more warps, like the unrolled C <= 2 shapes
+        // (long rows: as many rows as keep a step at <= 32 KB -- the few warps that then fit still hold ~190 KB in flight)
         int auto_r = d > 256 ? 4 : 8;
         if (d > 640) { auto_r = 8; while (auto_r > 1 && static_cast<size_t>(auto_r) * d * 4 > 32768) auto_r >>= 1; }
-        if (d > 3072) auto_r = 1;       // 12-16 KB rows: one per step keeps six warps in flight (3584: 7.36, 4096: 7.24 TB/s)
+        if (d > 3072) auto_r = 1;       // 12-16 KB rows: one per step keeps six warps in flight
         const int want_r = e->tune.rows_per_step;
         R = (want_r == 1 || want_r == 2 || want_r == 4 || want_r == 8) ? want_r : auto_r;
         if (R == 8) warps_default = 16;
@@ -440,13 +439,11 @@ static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0
         R = e->tune.rows_per_step == 4 || e->tune.rows_per_step == 8 ? e->tune.rows_per_step : (C <= 2 ? 8 : 4);
         if (C == 1) warps_default = 16;
         else if (C == 2) warps_default = 12;
-        // wide lists (33 <= k <= 128, four keys per lane): 16 warps per CTA spread the list upkeep and beat 8 warps up to
-        // a few GB of corpus (profiles/shape_sweep_r02.jsonl, k = 72: 72 vs 87 us at 174 K rows, 296 vs 315 us at
-        // 1.25 M, 555 vs 577 at 2.5 M; at 10 M rows the 8-warp shape's 48 KB in flight wins again)
+        // wide lists (33 <= k <= 128, four keys per lane): 16 warps per CTA spread the list upkeep; below 8 GB of corpus
+        // that won over 8 warps on B200, above it the 8-warp shape's 48 KB in flight did (chosen on B200, not re-tuned on H100)
         else if (mode == 1 && static_cast<uint64_t>(e->n_rows) * d * 4 < (8ull << 30)) warps_default = 16;
     }
-    // Default ring depth 2: measured best on B200 (profiles/sweep_r01_call2.json: ~48 KB in flight per SM beats
-    // deeper rings by 5-10 %).
+    // Default ring depth 2: ~48 KB in flight per SM for the 8-warp shapes (the `stages` option overrides it).
     const int stages = e->tune.stages > 0 ? e->tune.stages : 2;
     const size_t stage_bytes = static_cast<size_t>(R) * d * 4;
     const size_t query_bytes = C == 0 ? (static_cast<size_t>(d) * 4 + 512 + 32) : 0;
@@ -651,7 +648,7 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
         const int max_grid = e->tune.grid > 0 ? e->tune.grid : e->sm_count;
         grid = static_cast<int>(std::min<uint64_t>(max_grid, (steps + cfg.warps - 1) / cfg.warps));
         grid = std::max(std::min(grid, grid_cap), 1);
-        if (e->tune.chunk_steps < 0)     // auto: about two claims per warp at least (profiles/small_n_r02.jsonl), at most 8 steps
+        if (e->tune.chunk_steps < 0)     // auto: about two claims per warp at least, at most 8 steps
             p.chunk_steps = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>(8, steps / (static_cast<uint64_t>(grid) * cfg.warps * 2))));
         CUDA_TRY(launch_tma(e, p, grid, cfg, e->similarity, mode, stream));
     } else {
@@ -689,7 +686,7 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// batched path: tcgen05 TF32 nomination + exact re-score (waxvs_batch.cuh)
+// batched path: wgmma TF32 / bf16 nomination + exact re-score (waxvs_batch.cuh)
 static PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
     static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
     static std::once_flag once;
@@ -832,11 +829,27 @@ static cudaError_t launch_nominate(K kernel, uint32_t grid, uint32_t smem, bool 
     return cudaLaunchKernelEx(&cfg, kernel, map_q, map_c, bp);
 }
 
-// ring depth of the ARES shapes: what is left of the 227 KB after the resident queries
-static int ares_stages(bool pair, int heap, uint32_t num_kb, int want) {
-    int st = want;
-    while (st > 2 && batch_ares_smem_bytes(st, heap, pair, static_cast<int>(num_kb)) > 227u * 1024u) --st;
-    return batch_ares_smem_bytes(st, heap, pair, static_cast<int>(num_kb)) <= 227u * 1024u ? st : 0;
+// One launch of the nominate kernel in the form (bf16, filter, resident queries, CTA pair) the caller picked.
+static cudaError_t launch_nominate_form(bool bf16, bool filter, bool ares, bool pair, uint32_t grid, uint32_t smem,
+                                        cudaStream_t stream, const CUtensorMap &map_q, const CUtensorMap &map_c,
+                                        const BatchParams &bp) {
+#define WAXVS_NOM(BF, FI, AR, PR) return launch_nominate(batch_nominate_kernel<BF, FI, AR, PR>, grid, smem, PR, stream, map_q, map_c, bp)
+    if (filter) {
+        if (!bf16) WAXVS_NOM(false, true, false, false);
+        if (ares) WAXVS_NOM(true, true, true, false);
+        WAXVS_NOM(true, true, false, false);
+    }
+    if (!bf16) {
+        if (pair) WAXVS_NOM(false, false, false, true);
+        WAXVS_NOM(false, false, false, false);
+    }
+    if (ares) {
+        if (pair) WAXVS_NOM(true, false, true, true);
+        WAXVS_NOM(true, false, true, false);
+    }
+    if (pair) WAXVS_NOM(true, false, false, true);
+    WAXVS_NOM(true, false, false, false);
+#undef WAXVS_NOM
 }
 
 // P(X >= h) for X ~ Poisson(m): the chance that one row slice holds h or more of a query's "threatening" rows.
@@ -874,30 +887,16 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
         std::lock_guard<std::mutex> ag(e->attr_mu);
         if (!e->batch_attr_set) {
             auto chk = [&](cudaError_t r) { if (attr_err == cudaSuccess) attr_err = r; };
-            chk(set_smem_attr(batch_nominate_kernel<4, 16, false>, batch_smem_bytes(4, 16)));
-            chk(set_smem_attr(batch_nominate_kernel<3, 64, false>, batch_smem_bytes(3, 64)));
-            chk(set_smem_attr(batch_nominate_kernel<6, 16, true>, batch_smem_bytes(6, 16, true)));
-            chk(set_smem_attr(batch_nominate_kernel<4, 64, true>, batch_smem_bytes(4, 64, true)));
-            chk(set_smem_attr(batch_nominate_kernel<4, 16, false, true>, batch_smem_bytes(4, 16)));
-            chk(set_smem_attr(batch_nominate_kernel<3, 64, false, true>, batch_smem_bytes(3, 64)));
-            chk(set_smem_attr(batch_nominate_kernel<4, 24, false, true>, batch_smem_bytes(4, 24) - 2048u));
-            chk(set_smem_attr(batch_nominate_kernel<6, 16, true, true>, batch_smem_bytes(6, 16, true)));
-            chk(set_smem_attr(batch_nominate_kernel<4, 64, true, true>, batch_smem_bytes(4, 64, true)));
-            // ARES shapes: the ring depth is chosen at run time (<= the template's STAGES is what the kernel uses)
-            chk(set_smem_attr(batch_nominate_kernel<3, 16, false, true, true>, 227u * 1024u));
-            chk(set_smem_attr(batch_nominate_kernel<2, 16, false, true, true>, 227u * 1024u));
-            chk(set_smem_attr(batch_nominate_kernel<2, 64, false, true, true>, 227u * 1024u));
-            chk(set_smem_attr(batch_nominate_kernel<6, 16, true, true, true>, 227u * 1024u));
-            chk(set_smem_attr(batch_nominate_kernel<4, 16, true, true, true>, 227u * 1024u));
-            chk(set_smem_attr(batch_nominate_kernel<4, 64, true, true, true>, 227u * 1024u));
-            chk(set_smem_attr(batch_nominate_kernel<5, 32, true, true, true>, 227u * 1024u));
-            chk(set_smem_attr(batch_nominate_kernel<3, 24, false, true, true>, 227u * 1024u));
-            chk(set_smem_attr(batch_nominate_kernel<5, 32, true, true>, batch_smem_bytes(5, 32, true)));
-            chk(set_smem_attr(batch_tf32_ts_kernel<16>, batch_ts_smem_bytes(16)));
-            chk(set_smem_attr(batch_tf32_ts_kernel<64>, batch_ts_smem_bytes(64)));
-            chk(set_smem_attr(batch_nominate_kernel<4, 16, false, false, false, true>, batch_smem_bytes(4, 16)));
-            chk(set_smem_attr(batch_nominate_kernel<4, 16, false, true, false, true>, batch_smem_bytes(4, 16)));
-            chk(set_smem_attr(batch_nominate_kernel<3, 16, false, true, true, true>, 227u * 1024u));
+            // every form may use the whole opt-in shared memory; each launch asks for what its ring and heaps need
+            chk(set_smem_attr(batch_nominate_kernel<false, false, false, false>, kBatchSmemOptin));
+            chk(set_smem_attr(batch_nominate_kernel<false, false, false, true>, kBatchSmemOptin));
+            chk(set_smem_attr(batch_nominate_kernel<true, false, false, false>, kBatchSmemOptin));
+            chk(set_smem_attr(batch_nominate_kernel<true, false, false, true>, kBatchSmemOptin));
+            chk(set_smem_attr(batch_nominate_kernel<true, false, true, false>, kBatchSmemOptin));
+            chk(set_smem_attr(batch_nominate_kernel<true, false, true, true>, kBatchSmemOptin));
+            chk(set_smem_attr(batch_nominate_kernel<false, true, false, false>, kBatchSmemOptin));
+            chk(set_smem_attr(batch_nominate_kernel<true, true, false, false>, kBatchSmemOptin));
+            chk(set_smem_attr(batch_nominate_kernel<true, true, true, false>, kBatchSmemOptin));
             chk(set_smem_attr(filter_select_kernel, 16384 * 8));
             chk(set_smem_attr(batch_finish_kernel<kCosine>, (16384 + kBatchRescoreMax) * 8));
             chk(set_smem_attr(batch_finish_kernel<kDot>, (16384 + kBatchRescoreMax) * 8));
@@ -926,35 +925,29 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
     for (uint32_t q0 = 0; q0 < n_queries; q0 += max_groups * kBatchM) {
         const uint32_t nq = std::min<uint32_t>(n_queries - q0, max_groups * kBatchM);
         uint32_t groups = (nq + kBatchM - 1) / kBatchM;
-        // cta_group::2: CTA pairs (two query groups, one row slice) issue one 256-row MMA and each stages only half of
-        // the corpus tile.  Needs at least two groups; an odd group count is padded with an all-out-of-range group.
-        // TS shape: queries in TMEM + CTA pair (dims <= 384, dims % 128 == 0): shared memory carries only the corpus
-        const bool ts = !bf16 && !d_mask && e->tune.batch_ts != 0 && groups >= 2 && e->dims <= 384 && e->dims % 128u == 0;
-        bool pair = ts || (e->tune.batch_pair != 0 && groups >= 2);
-        const uint32_t tile_rows = ts ? static_cast<uint32_t>(kTsN) : static_cast<uint32_t>(kBatchN);
-        const uint32_t tiles_total = static_cast<uint32_t>((e->n_rows + tile_rows - 1) / tile_rows);
-        auto slices_for = [&](bool pr, uint32_t g) {
-            const uint32_t units = pr ? ((g + 1u) & ~1u) / 2u : g;                   // clusters (or CTAs) per slice
-            const uint32_t unit_slots = static_cast<uint32_t>(e->sm_count) / (pr ? 2u : 1u);
-            return std::max<uint32_t>(1, std::min<uint32_t>(unit_slots / units, tiles_total));
-        };
-        uint32_t slices = slices_for(pair, groups);
-        // Nominee heap size per (slice, query) = kernel shape.  TF32 / TS shapes: 16 entries when 16 nominees per slice
+        // CTA pairs (two query groups, one row slice, each CTA loads half of every corpus tile for both): needs at least
+        // two groups; an odd group count is padded with an all-out-of-range group.
+        const bool pair = e->tune.batch_pair != 0 && groups >= 2;
+        if (pair) groups = (groups + 1u) & ~1u;
+        const uint32_t tiles_total = static_cast<uint32_t>((e->n_rows + kBatchN - 1) / kBatchN);
+        const uint32_t units = pair ? groups / 2u : groups, unit_slots = static_cast<uint32_t>(e->sm_count) / (pair ? 2u : 1u);
+        uint32_t slices = std::max<uint32_t>(1, std::min<uint32_t>(unit_slots / units, tiles_total));
+        // Nominee heap size per (slice, query) = kernel shape.  TF32 shapes: 16 entries when 16 nominees per slice
         // comfortably cover k (16 * slices >= 8 k), else 64.  bf16 shapes (16 / 24 / 32 / 64): level 1 can prove a query
         // only if no slice holds `heap` rows scoring within the bf16 bound of the k-th result; with the corpus spread over
         // the slices those "threatening" rows (about 2.2 k of them for the bf16 bound on unit-scale embeddings) fall
-        // ~Poisson(m = 2.2 k / slices) per slice.  ONE unproven query costs its whole batch a second pass (DESIGN 4.5.2:
-        // k = 72 over 18 slices left 209 of 1024 queries unproven with 16 entries, none with 24 / 32), while 64-entry
-        // heaps cost a stage of the ring (8.6 vs 6.1-6.9 ms): the heap that minimises the expected cost is picked below.
+        // ~Poisson(m = 2.2 k / slices) per slice.  ONE unproven query costs its whole batch a second pass, while larger
+        // heaps cost ring stages (4 / 3 / 3 / 2): the heap that minimises the expected cost is picked below.
         const bool small_heap = e->tune.batch_heap == 16 || (e->tune.batch_heap == 0 && 16u * slices >= 8u * k_eff);
         uint32_t kprime = small_heap ? 16u : 64u;
-        if (bf16 && !ts) {
+        if (bf16) {
             uint32_t want = static_cast<uint32_t>(std::max(e->tune.batch_heap, 0));
             if (k_eff > 128u && want == 0u) want = 64u;       // large k: level 1 only has to NOMINATE k rows (filter level decides)
             if (want != 16u && want != 24u && want != 32u && want != 64u) {
                 // expected cost of a batch = the shape's relative time + P(some query of the batch is unproven) x one more
                 // pass.  Threatening rows per query: ~2.2 k (cosine, unit rows) / ~2.8 k (dot: the bound scales with the
-                // LARGEST row norm) -- calibrated on profiles/batch_k_sweep_r02p.jsonl and c5_proof_heap16_r02c.jsonl.
+                // LARGEST row norm).  The relative times of the heap sizes are guesses carried over from B200 (ring depths
+                // 4 / 3 / 3 / 2 on H100); they have not been measured on H100.
                 static const uint32_t ladder[4] = {16u, 24u, 32u, 64u};
                 static const double rel_time[4] = {1.00, 1.02, 1.10, 1.40};
                 const double m = (e->similarity == WAX_VS_DOT ? 2.8 : 2.2) * k_eff / slices;
@@ -963,99 +956,50 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
                 double best = 1e30;
                 uint32_t pick = 3u;
                 for (uint32_t i = 0; i < 4u; ++i) {
-                    if (ladder[i] == 24u && pair) continue;                     // 24: single-CTA shapes only
-                    if (ladder[i] == 32u && groups < 2u) continue;              // 32: cta_group::2 shapes only
                     const double p_fail = std::min(1.0, static_cast<double>(nq) * slices * poisson_tail(m, static_cast<int>(ladder[i])));
                     if (p_fail >= 1.0 && ladder[i] != 64u) continue;             // hopeless: every batch would pay a second pass
                     const double cost = rel_time[i] + 4.0 * p_fail;              // risk-averse: the model can be off
                     if (cost < best) { best = cost; pick = i; }
                 }
-                for (; bump > 0u && pick < 3u; --bump) {                         // the data overrules the model (see caller)
-                    ++pick;
-                    if (ladder[pick] == 24u && pair) ++pick;
-                    if (pick < 3u && ladder[pick] == 32u && groups < 2u) ++pick;
-                }
-                want = ladder[std::min(pick, 3u)];
+                pick = std::min(pick + bump, 3u);                                // the data overrules the model (see caller)
+                want = ladder[pick];
             }
-            if (want == 24u && pair) want = 32u;                       // 24: single-CTA shapes; 32: cta_group::2 shapes
-            if (want == 32u && groups < 2u) want = 64u;
-            if (want == 32u && !pair) { pair = true; slices = slices_for(true, groups); }
             kprime = want;
             if (used_heap) *used_heap = std::max(*used_heap, kprime);
         }
-        if (pair) groups = (groups + 1u) & ~1u;
-        // resident queries (bf16) when they leave room for a useful ring: >= 3 corpus stages (pair: >= 4 half-tile stages)
-        const uint32_t num_kb16 = e->dims / kBatchKBlockBf16;
-        const int ares_want = pair ? (kprime == 32u ? 5 : (kprime == 64u ? 4 : 6)) : (kprime == 64u ? 2 : 3);
-        const int ares_st = (bf16 && !ts && e->tune.batch_ares) ? ares_stages(pair, static_cast<int>(kprime), num_kb16, ares_want) : 0;
-        const bool ares = bf16 && !ts && ares_st >= (pair ? 4 : 2) && !(kprime >= 24u && ares_st < ares_want);
         slices = std::max<uint32_t>(1, std::min<uint32_t>(slices, 16384u / kprime));   // union fits the finish sort
         const uint32_t grid = groups * slices;
+        // resident queries (bf16) when a ring of at least two corpus stages still fits beside them
+        const uint32_t num_kb16 = e->dims / kBatchKBlockBf16;
+        const int ares_st = (bf16 && e->tune.batch_ares) ? batch_ring_stages(static_cast<int>(kprime), num_kb16) : 0;
+        const bool ares = ares_st >= 2;
+        const int stages = ares ? ares_st : batch_ring_stages(static_cast<int>(kprime));
         if ((rc = ensure_dev(&c->d_heaps, &c->heaps_cap, static_cast<size_t>(grid) * kBatchM * kprime, "nominee heaps"))) return rc;
         if ((rc = ensure_dev(&c->d_tau, &c->tau_cap, static_cast<size_t>(groups) * kBatchM, "shared thresholds"))) return rc;
         CUDA_TRY(cudaMemsetAsync(c->d_tau, 0, static_cast<size_t>(groups) * kBatchM * sizeof(uint32_t), stream));
         CUtensorMap map_q, map_c;
         const float *qbase = d_queries + static_cast<size_t>(q0) * e->dims;
-        const uint32_t c_box = ts ? kTsN / 2 : (pair ? kBatchN / 2 : kBatchN);
         if (bf16) {
             if ((rc = make_tensor_map(&map_q, c->d_queries_bf16 + static_cast<size_t>(q0) * e->dims, nq, e->dims, kBatchM, true))) return rc;
-            if ((rc = make_tensor_map(&map_c, e->d_shadow, e->n_rows, e->dims, c_box, true))) return rc;
+            if ((rc = make_tensor_map(&map_c, e->d_shadow, e->n_rows, e->dims, pair ? kBatchN / 2 : kBatchN, true))) return rc;
         } else {
             if ((rc = make_tensor_map(&map_q, qbase, nq, e->dims, kBatchM))) return rc;
-            if ((rc = make_tensor_map(&map_c, e->d_corpus, e->n_rows, e->dims, c_box))) return rc;
+            if ((rc = make_tensor_map(&map_c, e->d_corpus, e->n_rows, e->dims, pair ? kBatchN / 2 : kBatchN))) return rc;
         }
 
         BatchParams bp{};
         bp.n_rows = static_cast<uint32_t>(e->n_rows); bp.dims = e->dims; bp.n_queries = nq; bp.groups = groups;
         bp.slices = slices; bp.tiles_total = tiles_total; bp.kprime = kprime; bp.metric = e->similarity;
+        bp.stages = static_cast<uint32_t>(stages);
         // the cosine shadow rows are pre-normalised: no epilogue scaling on the bf16 path
         bp.row_scale = (e->similarity == WAX_VS_COSINE && !bf16) ? e->d_inv_norm : nullptr;
         bp.heaps = c->d_heaps;
         bp.tau_global = c->d_tau;
         bp.no_insert = e->tune.batch_noinsert ? 1u : 0u;
         bp.allow_bits = d_mask;
-        cudaError_t lerr = cudaSuccess;
-        if (ts) {
-            cudaLaunchConfig_t cfg{};
-            cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kBatchThreads); cfg.stream = stream;
-            cudaLaunchAttribute attr[1];
-            attr[0].id = cudaLaunchAttributeClusterDimension;
-            attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-            cfg.attrs = attr; cfg.numAttrs = 1;
-            if (small_heap) { cfg.dynamicSmemBytes = batch_ts_smem_bytes(16); lerr = cudaLaunchKernelEx(&cfg, batch_tf32_ts_kernel<16>, map_c, qbase, bp); }
-            else { cfg.dynamicSmemBytes = batch_ts_smem_bytes(64); lerr = cudaLaunchKernelEx(&cfg, batch_tf32_ts_kernel<64>, map_c, qbase, bp); }
-        } else if (bf16) {
-            const int kb = static_cast<int>(num_kb16);
-            const bool h16 = kprime == 16u;
-#define WAXVS_NOM(ST, HP, PR, AR, SMEM) lerr = launch_nominate(batch_nominate_kernel<ST, HP, PR, true, AR>, grid, (SMEM), PR, stream, map_q, map_c, bp)
-            if (ares && pair) {
-                if (kprime == 64u) WAXVS_NOM(4, 64, true, true, batch_ares_smem_bytes(4, 64, true, kb));
-                else if (kprime == 32u) WAXVS_NOM(5, 32, true, true, batch_ares_smem_bytes(5, 32, true, kb));
-                else if (ares_st >= 6) WAXVS_NOM(6, 16, true, true, batch_ares_smem_bytes(6, 16, true, kb));
-                else WAXVS_NOM(4, 16, true, true, batch_ares_smem_bytes(4, 16, true, kb));
-            } else if (ares) {
-                if (kprime == 64u) WAXVS_NOM(2, 64, false, true, batch_ares_smem_bytes(2, 64, false, kb));
-                else if (kprime == 24u) WAXVS_NOM(3, 24, false, true, batch_ares_smem_bytes(3, 24, false, kb));
-                else if (ares_st >= 3) WAXVS_NOM(3, 16, false, true, batch_ares_smem_bytes(3, 16, false, kb));
-                else WAXVS_NOM(2, 16, false, true, batch_ares_smem_bytes(2, 16, false, kb));
-            } else if (pair) {
-                if (h16) WAXVS_NOM(6, 16, true, false, batch_smem_bytes(6, 16, true));
-                else if (kprime == 32u) WAXVS_NOM(5, 32, true, false, batch_smem_bytes(5, 32, true));
-                else WAXVS_NOM(4, 64, true, false, batch_smem_bytes(4, 64, true));
-            } else {
-                if (kprime == 24u) WAXVS_NOM(4, 24, false, false, batch_smem_bytes(4, 24) - 2048u);
-                else if (h16) WAXVS_NOM(4, 16, false, false, batch_smem_bytes(4, 16));
-                else WAXVS_NOM(3, 64, false, false, batch_smem_bytes(3, 64));
-            }
-#undef WAXVS_NOM
-        } else if (pair) {
-            if (small_heap) lerr = launch_nominate(batch_nominate_kernel<6, 16, true>, grid, batch_smem_bytes(6, 16, true), true, stream, map_q, map_c, bp);
-            else lerr = launch_nominate(batch_nominate_kernel<4, 64, true>, grid, batch_smem_bytes(4, 64, true), true, stream, map_q, map_c, bp);
-        } else if (small_heap) {
-            lerr = launch_nominate(batch_nominate_kernel<4, 16, false>, grid, batch_smem_bytes(4, 16), false, stream, map_q, map_c, bp);
-        } else {
-            lerr = launch_nominate(batch_nominate_kernel<3, 64, false>, grid, batch_smem_bytes(3, 64), false, stream, map_q, map_c, bp);
-        }
+        const cudaError_t lerr = launch_nominate_form(bf16, false, ares, pair, grid,
+                                                      batch_smem_bytes(stages, static_cast<int>(kprime), ares ? num_kb16 : 0u),
+                                                      stream, map_q, map_c, bp);
         CUDA_TRY(lerr);
         CUDA_TRY(cudaGetLastError());
 
@@ -1175,7 +1119,7 @@ static int32_t sync_device_ids(wax_vs_engine *e, const uint64_t **out) {
 extern "C" {
 
 const char *wax_vs_last_error(void) { return g_last_error; }
-const char *wax_vs_version(void) { return "waxvs_cuda 0.1 sm_100a (fused scan+top-k; TMA bulk staging)"; }
+const char *wax_vs_version(void) { return "waxvs_cuda 0.1 sm_90a (fused scan+top-k; TMA bulk staging)"; }
 
 int32_t wax_vs_device_count(int32_t *out) {
     if (!out) return fail(WAX_VS_ERR_NULL, "out is NULL");
@@ -1670,19 +1614,13 @@ static int32_t enqueue_filter_level(wax_vs_engine *e, SearchCtx *c, const float 
         bp.cand_rows = c->d_cand_rows + static_cast<size_t>(q0) * cap;
         bp.cand_cap = cap;
         bp.allow_bits = d_mask;
-        if (bf16) {
-            const uint32_t num_kb = e->dims / kBatchKBlockBf16;
-            const int st = e->tune.batch_ares ? ares_stages(false, 16, num_kb, 3) : 0;
-            if (st >= 3)
-                CUDA_TRY(launch_nominate(batch_nominate_kernel<3, 16, false, true, true, true>, groups * slices,
-                                         batch_ares_smem_bytes(3, 16, false, static_cast<int>(num_kb)), false, stream, map_q, map_c, bp));
-            else
-                CUDA_TRY(launch_nominate(batch_nominate_kernel<4, 16, false, true, false, true>, groups * slices, batch_smem_bytes(4, 16),
-                                         false, stream, map_q, map_c, bp));
-        } else {
-            CUDA_TRY(launch_nominate(batch_nominate_kernel<4, 16, false, false, false, true>, groups * slices, batch_smem_bytes(4, 16),
-                                     false, stream, map_q, map_c, bp));
-        }
+        const uint32_t num_kb16 = e->dims / kBatchKBlockBf16;
+        const int ares_st = (bf16 && e->tune.batch_ares) ? batch_ring_stages(16, num_kb16) : 0;
+        const bool ares = ares_st >= 2;
+        const int stages = ares ? ares_st : batch_ring_stages(16);
+        bp.stages = static_cast<uint32_t>(stages);
+        CUDA_TRY(launch_nominate_form(bf16, true, ares, false, groups * slices, batch_smem_bytes(stages, 16, ares ? num_kb16 : 0u),
+                                      stream, map_q, map_c, bp));
         const dim3 rgrid(32, nq);
         if (e->similarity == WAX_VS_COSINE)
             filter_rescore_kernel<kCosine><<<rgrid, 256, 0, stream>>>(e->d_corpus, qbase, e->dims, bp.cand_count, bp.cand_rows, cap,
@@ -2672,7 +2610,7 @@ int32_t wax_vs_debug_stream_read(wax_vs_engine *e, uint32_t iters, float *out_be
     return WAX_VS_OK;
 }
 
-// Host <-> device transfer rates on this box, in GB/s, for `bytes` of pageable host memory (profiles/ingest_*.json):
+// Host <-> device transfer rates of this machine, in GB/s, for `bytes` of pageable host memory:
 //   [0] one-thread memcpy pageable -> pinned     [1] the staging copy with the engine's worker threads
 //   [2] DMA pinned -> HBM                         [3] DMA HBM -> pinned
 //   [4] upload pipeline pageable -> HBM           [5] download pipeline HBM -> pageable       [6] worker threads
@@ -2847,9 +2785,8 @@ int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value
     else if (!strcmp(key, "batch_large_k")) e->tune.batch_large_k = v;
     else if (!strcmp(key, "tma_max_dims")) e->tune.tma_max_dims = static_cast<uint32_t>(std::max(v, 0));
     else if (!strcmp(key, "batch_pair")) e->tune.batch_pair = v;
-    else if (!strcmp(key, "batch_ts")) e->tune.batch_ts = v;
-    else if (!strcmp(key, "batch_bf16")) { e->tune.batch_bf16 = v; e->shadow_unavailable = false; e->bf16_skip_batches = 0; }
     else if (!strcmp(key, "batch_ares")) e->tune.batch_ares = v;
+    else if (!strcmp(key, "batch_bf16")) { e->tune.batch_bf16 = v; e->shadow_unavailable = false; e->bf16_skip_batches = 0; }
     else if (!strcmp(key, "batch_rescore")) e->tune.batch_rescore = v;
     else if (!strcmp(key, "batch_retry")) e->tune.batch_retry = v;
     else if (!strcmp(key, "filter_cap")) e->tune.filter_cap = v;

@@ -119,9 +119,9 @@ __device__ __forceinline__ void finish_topk(const ScanParams &p, WarpTopK<E> &tk
     if (!s_last) return;
     __threadfence();
     tk.init();
-    // Block lists come from L2 (~1 us each if loaded one by one): fetch four at a time, then merge.
+    // Block lists come from L2 (a round trip each if loaded one by one): fetch four at a time, then merge.
     // (the merge loops are kept rolled: every inlined merge is ~150 instructions and this code runs once, so unrolled
-    // copies only buy instruction-cache misses -- the E = 4 tail was 80 us of them at 10 K rows)
+    // copies only buy instruction-cache misses)
     constexpr int U = (E == 1) ? 4 : 2;
 #pragma unroll 1
     for (uint32_t b0 = warp; b0 < gridDim.x; b0 += warps * U) {
@@ -164,9 +164,9 @@ __device__ __forceinline__ void finish_topk(const ScanParams &p, WarpTopK<E> &tk
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Selection tail (round 2).  The merge tail above costs one ~150-instruction bitonic merge per pair of lists: 7 per
-// CTA plus ~150 for the grid in the last CTA -- ~20 us at k = 10 and ~65 us at k = 72, which is most of a search over a
-// real (<= 174 K-row) Wax index.  Selection does not care about order: a block-wide MSB-first radix select (8 bits a
+// Selection tail.  The merge tail above costs one ~150-instruction bitonic merge per pair of lists: 7 per CTA plus one
+// per CTA of the grid in the last CTA -- a serial tail that is a large part of a search over a real (<= 174 K-row) Wax
+// index.  Selection does not care about order: a block-wide MSB-first radix select (8 bits a
 // pass, it stops as soon as the bin holding the k-th key holds one key) finds the k-th smallest key exactly, the keys
 // at or below it are the answer; only the final k are ranked (k x k compares) to come out sorted.
 struct SelectScratch {
@@ -418,7 +418,7 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         if (C == 0) {
             // Generic rows (dims < 128 or not one of the unrolled multiples of 128), several rows per step: chunk-outer /
             // row-inner, so a query chunk is read from shared memory once for the R rows (the row-outer form read it per row:
-            // twice the shared-memory traffic, 5.6 instead of 7.3 TB/s at 2560 dims).  Each row still sees its chunks in ascending
+            // twice the shared-memory traffic).  Each row still sees its chunks in ascending
             // order on its own accumulators: the same operations in the same order as the row-outer loop below.
             float a[R][4], b[R][4];
 #pragma unroll

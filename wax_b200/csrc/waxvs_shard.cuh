@@ -2,9 +2,9 @@
 //
 // SURVEY.md section 8(e): the corpus shards row-wise across the GPUs of a node, every rank scans its shard for the
 // replicated query and the per-shard top-k lists (k x 24 B per rank) are exchanged and merged under the same total
-// order (distance ascending, GLOBAL row ascending).  The reference has no distributed code; round 1 did this with
-// torch.distributed.all_gather_into_tensor + D2H + a numpy merge, which cost ~0.13 ms per query at 8 GPUs -- half a
-// 1.25 M-row scan.  Here the exchange is part of the scan kernel itself:
+// order (distance ascending, GLOBAL row ascending).  The reference has no distributed code.  An all-gather of the lists
+// + D2H + a host merge costs a sizeable part of a small shard's scan, so here the exchange is part of the scan kernel
+// itself:
 //
 //   * every rank owns a MAILBOX in its HBM (ShardMailbox); peers map it (CUDA IPC between the one-process-per-GPU
 //     ranks, plain peer access inside one process) and WRITE into it over NVLink / NVSwitch -- nobody ever reads
@@ -156,8 +156,8 @@ __global__ void __launch_bounds__(256) shard_exchange_kernel(const ShardParams s
 // Batched form of the same merge (sharded search_batch): `gathered` = [world][n_queries][k] candidates as an all-gather
 // of the ranks' per-query lists leaves them (every list sorted, padding valid = 0 last); out = [n_queries][k_out], the
 // k_out best of each query under (distance, GLOBAL row) -- the position rule of shard_exchange_cta, binary searches in
-// global memory.  One CTA per query.  Replaces the host-side numpy merge (7.6 ms per 1024 x 8 x 10 batch, ten times the
-// shard's tensor-core pass at 8 GPUs).
+// global memory.  One CTA per query.  Replaces a host-side numpy merge, which costs more than a shard's tensor-core
+// pass.
 __device__ __forceinline__ uint32_t cand_dist_key(const wax_vs_candidate &c) {
     return c.valid ? orderable_u32(c.distance) : WAXVS_UKEY_NONE;
 }

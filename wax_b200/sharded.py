@@ -103,9 +103,9 @@ class ShardedVectorEngine:
             self._comm_stream = torch.cuda.Stream(device=self.device)   # all-gather + D2H overlap the next scan
             # two scan streams: consecutive queries alternate, so one scan's tail overlaps the next one's prologue
             self._scan_streams = [torch.cuda.Stream(device=self.device) for _ in range(2)]
-            # Overlapping two scans pays when a shard is small (kernel tails/prologues overlap: +8 % at 7.7 GB,
-            # +15 % at 1.9 GB) and costs ~3 % when it is large (19 GB: twice the bytes in flight per SM), measured
-            # in profiles/bench_r01_n*_m*.json -- so alternate streams only below 12 GB per shard.
+            # Overlapping two scans pays when a shard is small (kernel tails/prologues overlap) and costs a little
+            # when it is large (twice the bytes in flight per SM).  The 12 GB threshold was chosen on B200 and has not
+            # been re-measured on H100.
             self._overlap_scans = (self.row_hi - self.row_lo) * self.dimensions * 4 < 12e9
             self.transport = "allgather"
             self.transport_note = ""
