@@ -293,6 +293,18 @@ int32_t wax_vs_debug_time_search_batch(wax_vs_engine *engine, uint32_t n_queries
                                        uint32_t warmup, uint32_t iters, float *out_ms_total,
                                        uint64_t *out_launches, uint32_t *out_unproven);
 
+/* Read-out of the batched path's nomination stage (tests): runs the tensor-core nomination + exact finish for
+   `n_queries` host queries and top_k <= 128 in the form the options select (batch_bf16, batch_ares, batch_pair,
+   batch_heap), optionally with a row filter (`allow_bits`: one bit per row, set = allowed; NULL = all rows).
+   out_scores [n_queries][count] receives every nomination score' the epilogue compared against its threshold (after
+   the cosine row scale); out_ok [n_queries] the proof flags; out_heaps [slices * groups][kprime][128] the nominee heaps
+   as dumped (key = (orderable(-score') << 32) | row); out_shape[7] = {bf16, resident queries, CTA pair, ring stages,
+   kprime, slices, groups}.  A batch that needs more than one launch -> WAX_VS_ERR_ARGUMENT; heaps_cap below the
+   heap entries -> WAX_VS_ERR_BUFFER with everything but the heaps written. */
+int32_t wax_vs_debug_batch_nominations(wax_vs_engine *engine, const float *queries, uint32_t n_queries, int64_t top_k,
+                                       const uint32_t *allow_bits, float *out_scores, uint32_t *out_ok,
+                                       uint64_t *out_heaps, uint64_t heaps_cap, uint32_t *out_shape);
+
 /* Streaming-read ceiling on the same box: a plain coalesced LDG.128 read of the live corpus bytes, best of
    `iters` (milliseconds, and the bytes read).  Context for the roofline fraction (SURVEY.md section 8d). */
 int32_t wax_vs_debug_stream_read(wax_vs_engine *engine, uint32_t iters, float *out_best_ms, uint64_t *out_bytes);

@@ -9,7 +9,22 @@ from wax_b200 import CUDAVectorEngine, VectorMetric
 pytestmark = pytest.mark.gpu
 
 
+# Cosine over rows whose norms spread over 1e-3 .. 1e3: the TF32 epilogue's per-row 1/|v| and the pre-normalised bf16
+# shadow rows then differ from row to row (synthetic cosine corpora are unit rows, where a misplaced scale is invisible).
+MIXED = "cosine_mixed_norms"
+
+
+def _metric(metric):
+    return VectorMetric.cosine if metric == MIXED else metric
+
+
 def _engine(oracle, metric, n, dims, seed, normalize=True):
+    if metric == MIXED:
+        corpus = oracle.synth_rows(seed, 0, n, dims, normalize=True)
+        corpus *= np.float32(10.0) ** np.random.default_rng(seed).uniform(-3, 3, (n, 1)).astype(np.float32)
+        eng = CUDAVectorEngine(VectorMetric.cosine, dims)
+        eng.add_batch(list(range(n)), corpus)
+        return eng
     eng = CUDAVectorEngine(metric, dims)
     eng.fill_synthetic(seed, n, normalize=normalize)
     return eng
@@ -25,7 +40,7 @@ def _single(eng, qs, k):
 @pytest.mark.parametrize("dims,n,b,k", [(384, 100_003, 5, 10), (384, 100_003, 129, 10), (384, 50_000, 300, 72),
                                         (768, 30_001, 64, 100), (128, 70_000, 17, 32), (32, 9_999, 8, 1),
                                         (384, 255, 6, 10), (384, 257, 6, 10), (384, 1, 4, 10), (1024, 20_000, 33, 10)])
-@pytest.mark.parametrize("metric", [VectorMetric.cosine, VectorMetric.dot])
+@pytest.mark.parametrize("metric", [VectorMetric.cosine, VectorMetric.dot, MIXED])
 @pytest.mark.parametrize("bf16", [1, 0])
 def test_batch_equals_single_query_path(oracle, metric, dims, n, b, k, bf16):
     eng = _engine(oracle, metric, n, dims, seed=900 + dims, normalize=(metric is VectorMetric.cosine))
@@ -42,7 +57,7 @@ def test_batch_equals_single_query_path(oracle, metric, dims, n, b, k, bf16):
         assert f1 - f0 <= max(1, b // 50), f"{f1 - f0} of {b} queries fell back to the exact path"
     # and the single-query path is itself bit-exact against the oracle (spot check one query)
     corpus = eng.read_rows(0, n)
-    r, d, s = oracle.search(metric.value, corpus, qs[0], k, mode=oracle.ACC_F32_TREE, threads=4)
+    r, d, s = oracle.search(_metric(metric).value, corpus, qs[0], k, mode=oracle.ACC_F32_TREE, threads=4)
     assert [g[0] for g in got[0]] == r.tolist()
     assert np.array_equal(np.float32([g[1] for g in got[0]]).view(np.uint32), s.view(np.uint32))
 
@@ -86,6 +101,30 @@ def test_batch_edge_rows_and_mutation_invalidates_norm_cache(oracle):
     assert 8 not in [i for i, _ in eng.search_batch(qs, 4000)[0]]
 
 
+def test_batch_edge_rows_and_mutation_invalidates_norm_cache_dot(oracle):
+    """The same edge rows and mutations for dot, whose proof bound scales with the corpus' max |v| (cached with the
+    norms): overwriting a row with a larger norm must raise that bound, so the level-1 proofs it allowed are refused."""
+    dims = 384
+    corpus = oracle.synth_rows(80, 0, 4000, dims)
+    corpus[7] = 0.0
+    corpus[8, 5] = np.nan
+    corpus[9, 6] = np.inf
+    eng = CUDAVectorEngine(VectorMetric.dot, dims)
+    eng.add_batch(list(range(4000)), corpus)
+    qs = oracle.synth_rows(81, 0, 6, dims)
+    assert eng.search_batch(qs, 10) == _single(eng, qs, 10)
+    ok_before = eng.batch_nominations(qs, 10)["ok"]
+    assert ok_before.sum() >= 3, ok_before          # unit rows: max|v| = 1 proves most queries at level 1
+    eng.add(11, corpus[11] * np.float32(1000.0))
+    ok_after = eng.batch_nominations(qs, 10)["ok"]
+    assert ok_after.sum() == 0, ok_after            # max|v| = 1000 now: eps ~ 8 |q|, nothing is provable
+    eng.add_batch([5000, 5001], np.stack([qs[0], qs[1] * np.float32(3.0)]))
+    eng.remove(3)
+    got = eng.search_batch(qs, 10)
+    assert got == _single(eng, qs, 10)
+    assert 8 not in [i for i, _ in eng.search_batch(qs, 4000)[0]]
+
+
 def test_ineligible_batches_use_the_loop(oracle):
     eng = _engine(oracle, VectorMetric.l2, 5000, 384, seed=5)
     qs = oracle.synth_rows(82, 0, 9, 384)
@@ -99,7 +138,7 @@ def test_ineligible_batches_use_the_loop(oracle):
 
 @pytest.mark.parametrize("dims,n,b,k", [(384, 100_003, 256, 10), (384, 100_003, 300, 10), (768, 30_001, 200, 100),
                                         (384, 50_000, 1024, 72), (128, 257, 129, 10)])
-@pytest.mark.parametrize("metric", [VectorMetric.cosine, VectorMetric.dot])
+@pytest.mark.parametrize("metric", [VectorMetric.cosine, VectorMetric.dot, MIXED])
 def test_cta_pair_mode_equals_single_query_path(oracle, metric, dims, n, b, k):
     """CTA-pair shape (two CTAs of a cluster, one row slice; each loads half of every corpus tile and multicasts it
     into both): same nominees -> same proof -> identical results."""
@@ -119,7 +158,7 @@ def test_cta_pair_mode_equals_single_query_path(oracle, metric, dims, n, b, k):
 @pytest.mark.parametrize("dims,n,b,k", [(384, 100_003, 256, 10), (384, 100_003, 300, 10), (768, 30_001, 200, 100),
                                         (384, 50_000, 1024, 72), (128, 257, 129, 10), (64, 9_999, 8, 1),
                                         (512, 40_000, 140, 32), (384, 1, 4, 10), (1024, 20_000, 33, 10)])
-@pytest.mark.parametrize("metric", [VectorMetric.cosine, VectorMetric.dot])
+@pytest.mark.parametrize("metric", [VectorMetric.cosine, VectorMetric.dot, MIXED])
 @pytest.mark.parametrize("pair,ares", [(0, 1), (0, 0), (1, 1), (1, 0)])
 def test_bf16_shadow_nominations_equal_single_query_path(oracle, metric, dims, n, b, k, pair, ares):
     """bf16 nominations (bf16 wgmmas over a bf16 shadow of the corpus, queries resident in shared memory or

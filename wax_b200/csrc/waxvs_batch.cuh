@@ -96,6 +96,8 @@ struct BatchParams {
     // filtered batches (wax_vs_search_batch_filtered): 1 bit per row, set = the row may be returned; nullptr = all rows.
     // Consulted only on the rare path (a chunk of 32 rows that holds a score above the query's threshold).
     const uint32_t *allow_bits;
+    // DUMP forms only (wax_vs_debug_batch_nominations): [n_queries][n_rows] every score' the epilogue compares with tau
+    float *dump_scores;
 };
 
 // ---- PTX wrappers (TMA tensor loads, wgmma) ---------------------------------------------------------------------
@@ -214,7 +216,11 @@ __device__ __forceinline__ uint64_t heap_replace_root(uint64_t *heap, uint32_t n
 
 // ---- row norms (cached per corpus version) --------------------------------------------------------------------
 // One warp per row, same accumulation order as the scan kernels.  inv_norm = 1/sqrt(sum v^2) (0 for a zero
-// row); max_norm_bits = max over finite rows of sqrt(sum v^2) as float bits (positive floats order as uints).
+// row); max_norm_bits = max over rows with finite components of |v| as float bits (positive floats order as uints).
+// A row of finite components whose sum v^2 overflows (|v| >= ~1.8e19) still has finite exact dot scores, so it must
+// count towards the dot bound: its norm is recomputed with scaling, max|x| * sqrt(sum (x / max|x|)^2) (+inf when |v|
+// itself exceeds FLT_MAX, which makes the proof refuse).  Rows holding inf or NaN are left out: their exact scores are
+// never finite, so they are never returned.
 __global__ void __launch_bounds__(256) row_norms_kernel(const float *corpus, uint32_t n_rows, uint32_t dims,
                                                         float *inv_norm, uint32_t *max_norm_bits) {
     const int lane = threadIdx.x & 31;
@@ -242,7 +248,26 @@ __global__ void __launch_bounds__(256) row_norms_kernel(const float *corpus, uin
         const float s = warp_butterfly_sum(__fadd_rn(__fadd_rn(b0, b1), __fadd_rn(b2, b3)));
         const float nrm = __fsqrt_rn(s);
         if (lane == 0) inv_norm[row] = (s == 0.0f) ? 0.0f : __fdiv_rn(1.0f, nrm);
-        if (finite_f32(nrm)) local_max = fmaxf(local_max, nrm);
+        if (finite_f32(nrm)) {
+            local_max = fmaxf(local_max, nrm);
+        } else {                                                  // warp-uniform: s is the butterfly sum
+            float m = 0.0f;
+            bool bad = false;
+            for (uint32_t i = lane; i < dims; i += 32u) {
+                const float x = __ldg(v + i);
+                bad |= !finite_f32(x);
+                m = fmaxf(m, fabsf(x));
+            }
+            if (!__any_sync(WAXVS_FULL_MASK, bad)) {
+                for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(WAXVS_FULL_MASK, m, o));
+                float t = 0.0f;
+                for (uint32_t i = lane; i < dims; i += 32u) {
+                    const float y = __fdiv_rn(__ldg(v + i), m);
+                    t = __fmaf_rn(y, y, t);
+                }
+                local_max = fmaxf(local_max, m * __fsqrt_rn(warp_butterfly_sum(t)));
+            }
+        }
     }
     if (lane == 0 && local_max > 0.0f) atomicMax(max_norm_bits, __float_as_uint(local_max));
 }
@@ -288,7 +313,9 @@ __global__ void __launch_bounds__(256) shadow_bf16_kernel(const float *__restric
 // PAIR: a cluster of two CTAs (two query groups, the same row slice); each CTA loads HALF of every corpus tile and
 //       multicasts it into both CTAs' shared memory, so the pair reads each tile from L2 once instead of twice.  A
 //       stage is refilled only when the consumers of BOTH CTAs have released it.
-template <bool BF16, bool FILTER, bool ARES, bool PAIR>
+// DUMP: test read-out (wax_vs_debug_batch_nominations) -- every scanned score' is also written to p.dump_scores.  A
+//       template parameter, so the production forms compile exactly as without it.
+template <bool BF16, bool FILTER, bool ARES, bool PAIR, bool DUMP = false>
 __global__ void __launch_bounds__(kBatchThreads, 1)
 batch_nominate_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c,
                       const BatchParams p) {
@@ -422,6 +449,12 @@ batch_nominate_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
                 const float4 v = src[j4];
                 sv[4 * j4 + 0] = v.x; sv[4 * j4 + 1] = v.y; sv[4 * j4 + 2] = v.z; sv[4 * j4 + 3] = v.w;
             }
+        }
+        if (DUMP && q < p.n_queries) {
+            float *d = p.dump_scores + static_cast<size_t>(q) * p.n_rows + row0 + chunk * 32u;
+#pragma unroll
+            for (uint32_t j = 0; j < 32; ++j)
+                if (chunk * 32u + j < rows_here) d[j] = sv[j];
         }
         float m[16];
 #pragma unroll

@@ -829,6 +829,28 @@ static cudaError_t launch_nominate(K kernel, uint32_t grid, uint32_t smem, bool 
     return cudaLaunchKernelEx(&cfg, kernel, map_q, map_c, bp);
 }
 
+// The heap forms with the score read-out (wax_vs_debug_batch_nominations); `set_attr`: allow the whole opt-in smem.
+static cudaError_t launch_nominate_dump(bool bf16, bool ares, bool pair, uint32_t grid, uint32_t smem, cudaStream_t stream,
+                                        const CUtensorMap &map_q, const CUtensorMap &map_c, const BatchParams &bp) {
+#define WAXVS_NOM(BF, AR, PR)                                                                                          \
+    do {                                                                                                               \
+        const cudaError_t err = set_smem_attr(batch_nominate_kernel<BF, false, AR, PR, true>, kBatchSmemOptin);        \
+        if (err != cudaSuccess) return err;                                                                            \
+        return launch_nominate(batch_nominate_kernel<BF, false, AR, PR, true>, grid, smem, PR, stream, map_q, map_c, bp); \
+    } while (0)
+    if (!bf16) {
+        if (pair) WAXVS_NOM(false, false, true);
+        WAXVS_NOM(false, false, false);
+    }
+    if (ares) {
+        if (pair) WAXVS_NOM(true, true, true);
+        WAXVS_NOM(true, true, false);
+    }
+    if (pair) WAXVS_NOM(true, false, true);
+    WAXVS_NOM(true, false, false);
+#undef WAXVS_NOM
+}
+
 // One launch of the nominate kernel in the form (bf16, filter, resident queries, CTA pair) the caller picked.
 static cudaError_t launch_nominate_form(bool bf16, bool filter, bool ares, bool pair, uint32_t grid, uint32_t smem,
                                         cudaStream_t stream, const CUtensorMap &map_q, const CUtensorMap &map_c,
@@ -864,12 +886,18 @@ static double poisson_tail(double m, int h) {
 // Enqueue the tensor-core nomination + exact finish for n_queries device-resident queries.  d_ok[i] = 1 when
 // query i's result is proven exact; the caller sends the others to the filter level, then to enqueue_search.
 // allow_bf16 = false forces TF32 nominations (adaptive level choice).  *used_bf16 reports what ran; d_tau_star
-// (optional) receives each query's threshold for the filter level.
+// (optional) receives each query's threshold for the filter level.  `dump` (tests only, one launch at most) runs the
+// same shape with the score read-out and reports the shape.
+struct NominationDump {
+    float *d_scores;        // [n_queries][n_rows]
+    uint32_t shape[7];      // bf16, ares, pair, stages, kprime, slices, groups
+};
 static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float *d_queries, uint32_t n_queries,
                                     uint32_t k_eff, uint64_t row_offset, wax_vs_candidate *d_out, uint32_t *d_ok,
                                     const uint64_t *d_ids, cudaStream_t stream, uint64_t *launches,
                                     bool allow_bf16 = true, bool *used_bf16 = nullptr, float *d_tau_star = nullptr,
-                                    const uint32_t *d_mask = nullptr, uint32_t *used_heap = nullptr) {
+                                    const uint32_t *d_mask = nullptr, uint32_t *used_heap = nullptr,
+                                    NominationDump *dump = nullptr) {
     int32_t rc = ensure_norms(e, stream);
     if (rc) return rc;
     bool bf16 = allow_bf16 && batch_bf16_wanted(e);
@@ -882,6 +910,8 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
     // fewer query groups share the SMs and a large batch is split into several launches
     uint32_t max_groups = static_cast<uint32_t>(e->sm_count);
     if (k_eff > 128u) max_groups = std::max<uint32_t>(1u, max_groups / ((k_eff * 115u / 100u + 63u) / 64u));
+    if (dump && n_queries > max_groups * kBatchM)
+        return fail(WAX_VS_ERR_ARGUMENT, "the nomination read-out covers one launch: at most %u queries", max_groups * kBatchM);
     cudaError_t attr_err = cudaSuccess;
     {   // per function and per DEVICE: once per engine
         std::lock_guard<std::mutex> ag(e->attr_mu);
@@ -997,9 +1027,16 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
         bp.tau_global = c->d_tau;
         bp.no_insert = e->tune.batch_noinsert ? 1u : 0u;
         bp.allow_bits = d_mask;
-        const cudaError_t lerr = launch_nominate_form(bf16, false, ares, pair, grid,
-                                                      batch_smem_bytes(stages, static_cast<int>(kprime), ares ? num_kb16 : 0u),
-                                                      stream, map_q, map_c, bp);
+        const uint32_t smem = batch_smem_bytes(stages, static_cast<int>(kprime), ares ? num_kb16 : 0u);
+        cudaError_t lerr;
+        if (dump) {
+            bp.dump_scores = dump->d_scores;
+            const uint32_t shape[7] = {bf16, ares, pair, static_cast<uint32_t>(stages), kprime, slices, groups};
+            std::copy(shape, shape + 7, dump->shape);
+            lerr = launch_nominate_dump(bf16, ares, pair, grid, smem, stream, map_q, map_c, bp);
+        } else {
+            lerr = launch_nominate_form(bf16, false, ares, pair, grid, smem, stream, map_q, map_c, bp);
+        }
         CUDA_TRY(lerr);
         CUDA_TRY(cudaGetLastError());
 
@@ -2763,6 +2800,56 @@ int32_t wax_vs_debug_time_search_batch(wax_vs_engine *e, uint32_t n_queries, int
         for (uint32_t i = 0; i < n_queries; ++i) bad += c->h_ok[i] ? 0u : 1u;
         *out_unproven = bad;
     }
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_debug_batch_nominations(wax_vs_engine *e, const float *queries, uint32_t n_queries, int64_t top_k,
+                                       const uint32_t *allow_bits, float *out_scores, uint32_t *out_ok,
+                                       uint64_t *out_heaps, uint64_t heaps_cap, uint32_t *out_shape) {
+    if (!e || !queries || !out_scores || !out_ok || !out_shape) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    DeviceGuard g(e->device);
+    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    const uint32_t k_eff = static_cast<uint32_t>(std::min<uint64_t>(clamp_topk(top_k), std::max<uint64_t>(e->n_rows, 1)));
+    if (n_queries == 0 || e->n_rows == 0 || k_eff > 128u || e->dims % kBatchKBlock != 0 || e->dims > 8192 ||
+        (e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT))
+        return fail(WAX_VS_ERR_UNSUPPORTED, "batch of %u queries, k=%u, dims=%u has no tensor-core nomination pass",
+                    n_queries, k_eff, e->dims);
+    SearchCtx *c = nullptr;
+    int32_t rc = ctx_acquire(e, &c);
+    if (rc) return rc;
+    struct Rel { wax_vs_engine *e; SearchCtx *c; float *d_scores; ~Rel() { if (d_scores) cudaFree(d_scores); ctx_release(e, c); } }
+        rel{e, c, nullptr};
+    const size_t qfloats = static_cast<size_t>(n_queries) * e->dims;
+    const size_t n_scores = static_cast<size_t>(n_queries) * e->n_rows;
+    if ((rc = ensure_dev(&c->d_queries, &c->d_queries_cap, qfloats, "query buffer"))) return rc;
+    if ((rc = ensure_dev(&c->d_out, &c->d_out_cap, static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
+    if ((rc = ensure_dev(&c->d_ok, &c->ok_cap, static_cast<size_t>(n_queries), "proof flags"))) return rc;
+    CUDA_TRY(cudaMalloc(&rel.d_scores, n_scores * sizeof(float)));
+    CUDA_TRY(cudaMemsetAsync(rel.d_scores, 0xFF, n_scores * sizeof(float), c->stream));   // NaN payload: "never written"
+    CUDA_TRY(cudaMemcpyAsync(c->d_queries, queries, qfloats * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    const uint32_t *d_mask = nullptr;
+    if (allow_bits) {
+        const size_t words = static_cast<size_t>((e->n_rows + 31) / 32);
+        if ((rc = ensure_dev(&c->d_mask, &c->mask_cap, words, "row filter"))) return rc;
+        CUDA_TRY(cudaMemcpyAsync(c->d_mask, allow_bits, words * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+        d_mask = c->d_mask;
+    }
+    NominationDump dump{};
+    dump.d_scores = rel.d_scores;
+    uint64_t launches = 0;
+    rc = enqueue_batch_tensor(e, c, c->d_queries, n_queries, k_eff, 0, c->d_out, c->d_ok, nullptr, c->stream, &launches,
+                              true, nullptr, nullptr, d_mask, nullptr, &dump);
+    if (rc) { cudaStreamSynchronize(c->stream); return rc; }
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    std::copy(dump.shape, dump.shape + 7, out_shape);
+    CUDA_TRY(cudaMemcpy(out_scores, rel.d_scores, n_scores * sizeof(float), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(out_ok, c->d_ok, n_queries * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    const uint64_t n_heap = static_cast<uint64_t>(dump.shape[5]) * dump.shape[6] * dump.shape[4] * kBatchM;
+    if (!out_heaps || heaps_cap < n_heap)
+        return fail(WAX_VS_ERR_BUFFER, "the heaps need %llu entries (%llu given)", static_cast<unsigned long long>(n_heap),
+                    static_cast<unsigned long long>(heaps_cap));
+    CUDA_TRY(cudaMemcpy(out_heaps, c->d_heaps, n_heap * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     return WAX_VS_OK;
 }
 

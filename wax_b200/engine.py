@@ -464,6 +464,37 @@ class CUDAVectorEngine:
                                                       C.byref(ms), C.byref(launches), C.byref(bad)))
         return ms.value, launches.value, bad.value
 
+    def batch_nominations(self, queries, top_k: int, allow_rows=None):
+        """Read-out of the batched path's nomination stage (wax_vs_debug_batch_nominations), in the form the options
+        select.  Returns a dict: scores [n_queries, count] fp32 (every score' compared against the threshold; never
+        written entries keep the 0xFFFFFFFF NaN payload), ok [n_queries], heaps [slices*groups, kprime, 128] uint64 and
+        the launch shape (bf16, ares, pair, stages, kprime, slices, groups).  `allow_rows`: optional row filter."""
+        q = np.ascontiguousarray(queries, dtype=np.float32).reshape(-1, self.dimensions)
+        nq, n = q.shape[0], self.count
+        scores = np.empty((nq, n), np.float32)
+        ok = np.empty(nq, np.uint32)
+        shape = np.zeros(7, np.uint32)
+        bits = None
+        if allow_rows is not None:
+            mask = np.zeros(((n + 31) // 32) * 32, bool)
+            mask[np.asarray(allow_rows, np.int64)] = True
+            bits = (mask.reshape(-1, 32).astype(np.uint64) << np.arange(32, dtype=np.uint64)).sum(1).astype(np.uint32)
+        u32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
+        heaps = np.empty(0, np.uint64)
+        for _ in range(2):     # the first call reports how many heap entries the shape it picked needs
+            rc = L.lib().wax_vs_debug_batch_nominations(
+                self._h, q.ctypes.data_as(C.POINTER(C.c_float)), nq, int(top_k), None if bits is None else u32(bits),
+                scores.ctypes.data_as(C.POINTER(C.c_float)), u32(ok),
+                heaps.ctypes.data_as(C.POINTER(C.c_uint64)) if heaps.size else None, heaps.size, u32(shape))
+            if rc != L.ERR_BUFFER or heaps.size:
+                break
+            heaps = np.empty(int(shape[5]) * int(shape[6]) * int(shape[4]) * 128, np.uint64)
+        _check(rc)
+        names = ("bf16", "ares", "pair", "stages", "kprime", "slices", "groups")
+        out = {name: int(v) for name, v in zip(names, shape)}
+        out.update(scores=scores, ok=ok, heaps=heaps.reshape(out["slices"] * out["groups"], out["kprime"], 128))
+        return out
+
     def stream_read_gbs(self, iters: int = 5) -> float:
         """Plain coalesced read of the corpus bytes: the box's streaming-read ceiling in GB/s."""
         ms, nbytes = C.c_float(0), C.c_uint64(0)
