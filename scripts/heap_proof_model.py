@@ -9,7 +9,7 @@ scores are drawn from the exact order statistics (cumulative exponential spacing
 quantiles).  The proof needs  s_k > max(max over slices of the slice's H-th best, the (R+1)-th nominee) + eps  with
 eps = 1.03 * 2^-7 * |q| * max|v| (+ accumulation slack), |q| = 1, max|v| ~ 16.  bf16 noise on the nominee ORDER is ignored
 (it adds a little), so the model is a lower bound on the failure rate.  This is the Poisson tail argument behind the
-engine's heap-size cost model (enqueue_batch_tensor in wax_b200/csrc/waxvs_engine.cu)."""
+engine's heap-size cost model (pick_heap in wax_b200/csrc/waxvs_engine.cu)."""
 import sys
 
 import numpy as np

@@ -68,6 +68,38 @@ struct DeviceGuard {
     ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
+// An owned allocation of `cap` elements: device memory, or (PINNED) mapped + portable host memory that kernels may write
+// results straight into (host delivery) from any device.  ensure(n) grows it without keeping the contents; the memory
+// goes back on release() or destruction, which must run while the owner's device is current.
+template <typename T, bool PINNED>
+struct Buf {
+    T *p = nullptr;
+    size_t cap = 0;     // elements
+    Buf() = default;
+    Buf(const Buf &) = delete;
+    Buf &operator=(const Buf &) = delete;
+    ~Buf() { release(); }
+    operator T *() const { return p; }
+    void release() {
+        if (p) PINNED ? cudaFreeHost(p) : cudaFree(p);
+        p = nullptr;
+        cap = 0;
+    }
+    int32_t ensure(size_t n, const char *what) {
+        if (n <= cap) return WAX_VS_OK;
+        release();
+        const cudaError_t err = PINNED ? cudaHostAlloc(reinterpret_cast<void **>(&p), n * sizeof(T), cudaHostAllocMapped | cudaHostAllocPortable)
+                                       : cudaMalloc(&p, n * sizeof(T));
+        if (err != cudaSuccess)
+            return fail(WAX_VS_ERR_CUDA, PINNED ? "failed to allocate pinned %s (%zu bytes): %s" : "failed to allocate %s (%zu bytes): %s",
+                        what, n * sizeof(T), cudaGetErrorString(cudaGetLastError()));
+        cap = n;
+        return WAX_VS_OK;
+    }
+};
+template <typename T> using DevBuf = Buf<T, false>;
+template <typename T> using PinnedBuf = Buf<T, true>;
+
 // ---------------------------------------------------------------------------------------------------------
 // id -> row: open addressing, linear probing.  Replaces frameIds.firstIndex(of:) (MetalVectorEngine.swift:334,385,426).
 struct IdMap {
@@ -153,36 +185,41 @@ struct Tuning {
 struct SearchCtx {
     cudaStream_t stream = nullptr;
     bool own_stream = false;
-    float *d_queries = nullptr; size_t d_queries_cap = 0;        // floats
-    wax_vs_candidate *d_out = nullptr; size_t d_out_cap = 0;      // candidates
-    float *h_queries = nullptr; size_t h_queries_cap = 0;        // pinned
-    wax_vs_candidate *h_out = nullptr; size_t h_out_cap = 0;      // pinned
-    uint64_t *d_block_keys = nullptr; size_t block_keys_cap = 0;  // u64
-    uint32_t *d_ticket = nullptr;
-    uint32_t *d_dist_keys = nullptr; size_t dist_keys_cap = 0;    // large-k path
-    SelectState *d_select = nullptr;
-    uint64_t *d_sel_keys = nullptr;                               // 16384 u64
+    DevBuf<float> d_queries;
+    DevBuf<wax_vs_candidate> d_out;
+    PinnedBuf<float> h_queries;
+    PinnedBuf<wax_vs_candidate> h_out;
+    DevBuf<uint64_t> d_block_keys;
+    DevBuf<uint32_t> d_ticket;
+    DevBuf<uint32_t> d_dist_keys;                  // large-k path
+    DevBuf<SelectState> d_select;
+    DevBuf<uint64_t> d_sel_keys;                   // 16384 u64
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    uint64_t *d_heaps = nullptr; size_t heaps_cap = 0;            // batched path: nominee heaps
-    uint32_t *d_ok = nullptr; size_t ok_cap = 0;                  // batched path: per-query proof flags
-    uint32_t *h_ok = nullptr; size_t h_ok_cap = 0;                // pinned
-    uint32_t *d_tau = nullptr; size_t tau_cap = 0;                // batched path: shared per-query thresholds
-    __nv_bfloat16 *d_queries_bf16 = nullptr; size_t queries_bf16_cap = 0;   // batched bf16 path: converted queries
-    float *d_retry_q = nullptr; size_t retry_q_cap = 0;           // bf16 -> TF32 retry: compacted queries
-    wax_vs_candidate *d_retry_out = nullptr; size_t retry_out_cap = 0;
-    uint32_t *d_retry_ok = nullptr; size_t retry_ok_cap = 0;
-    float *d_tau_star = nullptr; size_t tau_star_cap = 0;         // level 1 -> filter level: per-query thresholds
-    float *h_tau_star = nullptr; size_t h_tau_star_cap = 0;       // pinned
-    float *d_filter_tau = nullptr; size_t filter_tau_cap = 0;     // compacted thresholds of the unproven queries
-    float *h_filter_tau = nullptr; size_t h_filter_tau_cap = 0;   // pinned
-    uint32_t *d_cand_count = nullptr; size_t cand_count_cap = 0;
-    uint32_t *d_cand_rows = nullptr; size_t cand_rows_cap = 0;
-    uint64_t *d_cand_keys = nullptr; size_t cand_keys_cap = 0;
-    uint32_t *d_mask = nullptr; size_t mask_cap = 0;              // filtered search: row bitset / listed rows
-    uint64_t *d_gather_keys = nullptr; size_t gather_cap = 0;     // filtered search: keys of the listed rows
-    wax_vs_candidate *d_shard_local = nullptr;                    // sharded search: this rank's list before the exchange [kShardKCap]
-    unsigned long long *h_flag = nullptr;                         // mapped pinned: host-delivery completion flag
-    unsigned long long host_seq = 0;                              // last value the flag was asked to take
+    DevBuf<uint64_t> d_heaps;                      // batched path: nominee heaps
+    DevBuf<uint32_t> d_ok;                         // batched path: per-query proof flags
+    PinnedBuf<uint32_t> h_ok;
+    DevBuf<uint32_t> d_tau;                        // batched path: shared per-query thresholds
+    DevBuf<__nv_bfloat16> d_queries_bf16;          // batched bf16 path: converted queries
+    DevBuf<float> d_retry_q;                       // bf16 -> TF32 retry: compacted queries
+    DevBuf<wax_vs_candidate> d_retry_out;
+    DevBuf<uint32_t> d_retry_ok;
+    DevBuf<float> d_tau_star;                      // level 1 -> filter level: per-query thresholds
+    PinnedBuf<float> h_tau_star;
+    DevBuf<float> d_filter_tau;                    // compacted thresholds of the unproven queries
+    PinnedBuf<float> h_filter_tau;
+    DevBuf<uint32_t> d_cand_count;
+    DevBuf<uint32_t> d_cand_rows;
+    DevBuf<uint64_t> d_cand_keys;
+    DevBuf<uint32_t> d_mask;                       // filtered search: row bitset / listed rows
+    DevBuf<uint64_t> d_gather_keys;                // filtered search: keys of the listed rows
+    DevBuf<wax_vs_candidate> d_shard_local;        // sharded search: this rank's list before the exchange [kShardKCap]
+    PinnedBuf<unsigned long long> h_flag;          // host-delivery completion flag
+    unsigned long long host_seq = 0;               // last value the flag was asked to take
+    ~SearchCtx() {                                 // the buffers release themselves
+        if (ev0) cudaEventDestroy(ev0);
+        if (ev1) cudaEventDestroy(ev1);
+        if (own_stream && stream) cudaStreamDestroy(stream);
+    }
 };
 
 struct wax_vs_engine {
@@ -205,7 +242,8 @@ struct wax_vs_engine {
     // binary search in it and bulk appends touch no hash table at all; the table is built only once an out-of-order id
     // arrives (and kept from then on).  Order-preserving removes and in-place upserts keep the array sorted.
     bool ids_sorted = true;
-    uint64_t *d_ids = nullptr; size_t d_ids_cap = 0; bool d_ids_dirty = true;
+    DevBuf<uint64_t> d_ids;
+    bool d_ids_dirty = true;
     std::mutex ids_mu;
 
     std::shared_mutex rw;  // readers: search / serialize; writer: mutators (AsyncReadWriteLock, :56-80)
@@ -216,12 +254,12 @@ struct wax_vs_engine {
     Tuning tune;
 
     // cached per corpus version for the batched path: 1/|v| per row and max |v|
-    float *d_inv_norm = nullptr; size_t inv_norm_cap = 0;
-    uint32_t *d_max_norm = nullptr;
+    DevBuf<float> d_inv_norm;
+    DevBuf<uint32_t> d_max_norm;
     uint64_t norms_rows = 0;       // rows [0, norms_rows) of d_inv_norm are valid (appends extend it, other mutations reset it)
     std::mutex norms_mu;
     // bf16 shadow of the corpus for the batched bf16 nominations (cached per corpus version, guarded by norms_mu)
-    __nv_bfloat16 *d_shadow = nullptr; size_t shadow_cap = 0;
+    DevBuf<__nv_bfloat16> d_shadow;
     uint64_t shadow_rows = 0;      // rows [0, shadow_rows) of d_shadow are valid; shadow_valid = covers every live row
     bool shadow_valid = false, shadow_unavailable = false;
     uint64_t batch_tensor_queries = 0, batch_fallback_queries = 0;   // instrumentation
@@ -241,14 +279,20 @@ struct wax_vs_engine {
         cudaEvent_t ev[2] = {nullptr, nullptr};
         uint8_t *pin[2] = {nullptr, nullptr};
         size_t pin_bytes = 0;
-        float *d_stage = nullptr; size_t d_stage_cap = 0;        // floats
-        uint32_t *d_index = nullptr; size_t d_index_cap = 0;     // u32
+        DevBuf<float> d_stage;
+        DevBuf<uint32_t> d_index;
         int threads = 1;
+        ~Ingest() {
+            for (int i = 0; i < 2; ++i) {
+                if (pin[i]) cudaFreeHost(pin[i]);
+                if (ev[i]) cudaEventDestroy(ev[i]);
+            }
+            if (stream) cudaStreamDestroy(stream);
+        }
     } ing;
     uint64_t ingest_h2d_bytes = 0, ingest_d2h_bytes = 0;         // instrumentation
     std::mutex ingest_mu;                                        // readers that use the staging (serialize)
     std::mutex attr_mu;            // cudaFuncSetAttribute bookkeeping (per engine = per device)
-    bool sort_attr_set = false, gather_attr_set = false, batch_attr_set = false;
     std::unordered_map<const void *, int> smem_granted;   // opt-in shared memory already granted, per kernel (attr_mu)
     // Device-path searches (wax_vs_search_device & co.) return while their kernels are still in flight on the
     // caller's stream.  Mutators must not touch the corpus under them: every mutator drains the device first when
@@ -267,13 +311,13 @@ struct wax_vs_engine {
         unsigned long long timeout_ns = 20ull * 1000 * 1000 * 1000;
         std::mutex mu;                            // one collective call at a time per rank: seq order = issue order
         SearchCtx *ctx = nullptr;                 // host entry point: stream + scratch
-        wax_vs_candidate *d_final = nullptr;      // [kShardKCap]
-        wax_vs_candidate *h_final = nullptr;      // mapped pinned [kShardKCap]: the kernel writes the merged result here
-        unsigned long long *h_flag = nullptr;     // mapped pinned: seq when h_final is complete
+        DevBuf<wax_vs_candidate> d_final;         // [kShardKCap]
+        PinnedBuf<wax_vs_candidate> h_final;      // [kShardKCap]: the kernel writes the merged result here
+        PinnedBuf<unsigned long long> h_flag;     // seq when h_final is complete
     } shard;
 };
 
-extern "C" { static void shard_teardown(wax_vs_engine *e, bool free_own); static void ingest_free(wax_vs_engine *e); }
+extern "C" { static void shard_teardown(wax_vs_engine *e, bool free_own); }
 
 // Called by every mutator after it has taken the write lock (and selected the device).
 static void drain_device_path(wax_vs_engine *e) {
@@ -289,58 +333,24 @@ static void invalidate_row_caches(wax_vs_engine *e, uint64_t keep_prefix) {
 
 // ---------------------------------------------------------------------------------------------------------
 // scratch contexts
-static void ctx_free(SearchCtx *c) {
-    if (!c) return;
-    if (c->d_queries) cudaFree(c->d_queries);
-    if (c->d_out) cudaFree(c->d_out);
-    if (c->h_queries) cudaFreeHost(c->h_queries);
-    if (c->h_out) cudaFreeHost(c->h_out);
-    if (c->d_block_keys) cudaFree(c->d_block_keys);
-    if (c->d_ticket) cudaFree(c->d_ticket);
-    if (c->d_dist_keys) cudaFree(c->d_dist_keys);
-    if (c->d_select) cudaFree(c->d_select);
-    if (c->d_sel_keys) cudaFree(c->d_sel_keys);
-    if (c->d_heaps) cudaFree(c->d_heaps);
-    if (c->d_ok) cudaFree(c->d_ok);
-    if (c->d_tau) cudaFree(c->d_tau);
-    if (c->d_queries_bf16) cudaFree(c->d_queries_bf16);
-    if (c->d_retry_q) cudaFree(c->d_retry_q);
-    if (c->d_retry_out) cudaFree(c->d_retry_out);
-    if (c->d_retry_ok) cudaFree(c->d_retry_ok);
-    if (c->d_tau_star) cudaFree(c->d_tau_star);
-    if (c->h_tau_star) cudaFreeHost(c->h_tau_star);
-    if (c->d_filter_tau) cudaFree(c->d_filter_tau);
-    if (c->h_filter_tau) cudaFreeHost(c->h_filter_tau);
-    if (c->d_cand_count) cudaFree(c->d_cand_count);
-    if (c->d_cand_rows) cudaFree(c->d_cand_rows);
-    if (c->d_cand_keys) cudaFree(c->d_cand_keys);
-    if (c->d_mask) cudaFree(c->d_mask);
-    if (c->d_gather_keys) cudaFree(c->d_gather_keys);
-    if (c->d_shard_local) cudaFree(c->d_shard_local);
-    if (c->h_flag) cudaFreeHost(c->h_flag);
-    if (c->h_ok) cudaFreeHost(c->h_ok);
-    if (c->ev0) cudaEventDestroy(c->ev0);
-    if (c->ev1) cudaEventDestroy(c->ev1);
-    if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
-    delete c;
-}
-
 static int32_t ctx_new(wax_vs_engine *e, SearchCtx **out, bool with_stream) {
     SearchCtx *c = new (std::nothrow) SearchCtx();
     if (!c) return fail(WAX_VS_ERR_CUDA, "out of host memory");
-    auto bail = [&](int32_t rc) { ctx_free(c); return rc; };
+    auto bail = [&](int32_t rc) { delete c; return rc; };
     if (with_stream) {
         if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess)
             return bail(fail(WAX_VS_ERR_CUDA, "cudaStreamCreate failed"));
         c->own_stream = true;
     }
-    c->block_keys_cap = static_cast<size_t>(std::max(e->sm_count * 8, 2048)) * 128;
-    if (cudaMalloc(&c->d_block_keys, c->block_keys_cap * sizeof(uint64_t)) != cudaSuccess ||
-        cudaMalloc(&c->d_ticket, 4 * sizeof(uint32_t)) != cudaSuccess ||      // [0] ticket, [1] work counter
+    const size_t block_keys = static_cast<size_t>(std::max(e->sm_count * 8, 2048)) * 128;
+    if (cudaMalloc(&c->d_block_keys.p, block_keys * sizeof(uint64_t)) != cudaSuccess ||
+        cudaMalloc(&c->d_ticket.p, 4 * sizeof(uint32_t)) != cudaSuccess ||      // [0] ticket, [1] work counter
         cudaMemset(c->d_ticket, 0, 4 * sizeof(uint32_t)) != cudaSuccess ||
         cudaEventCreate(&c->ev0) != cudaSuccess || cudaEventCreate(&c->ev1) != cudaSuccess)
         return bail(fail(WAX_VS_ERR_CUDA, "failed to allocate search scratch: %s",
                          cudaGetErrorString(cudaGetLastError())));
+    c->d_block_keys.cap = block_keys;
+    c->d_ticket.cap = 4;
     *out = c;
     return WAX_VS_OK;
 }
@@ -362,6 +372,20 @@ static void ctx_release(wax_vs_engine *e, SearchCtx *c) {
     std::lock_guard<std::mutex> g(e->pool_mu);
     e->pool.push_back(c);
 }
+// A pooled context held for the length of one call.  clears_trace: also detach the phase-trace buffer on the way out.
+struct CtxLease {
+    wax_vs_engine *e;
+    SearchCtx *c = nullptr;
+    bool clears_trace = false;
+    explicit CtxLease(wax_vs_engine *eng, bool clear_trace = false) : e(eng), clears_trace(clear_trace) {}
+    CtxLease(const CtxLease &) = delete;
+    CtxLease &operator=(const CtxLease &) = delete;
+    ~CtxLease() {
+        if (c) ctx_release(e, c);
+        if (clears_trace) e->debug_trace = nullptr;
+    }
+    int32_t acquire() { return ctx_acquire(e, &c); }
+};
 // The scratch context bound to a caller-owned stream (device-path entry points): find-or-create in ONE critical
 // section, so two threads that first use the same stream cannot both insert (and leak) a context.
 static int32_t ctx_for_stream(wax_vs_engine *e, void *cuda_stream, SearchCtx **out) {
@@ -375,28 +399,6 @@ static int32_t ctx_for_stream(wax_vs_engine *e, void *cuda_stream, SearchCtx **o
     e->stream_ctx[cuda_stream] = c;
     ++e->pool_allocs;
     *out = c;
-    return WAX_VS_OK;
-}
-
-template <typename T>
-static int32_t ensure_dev(T **p, size_t *cap, size_t need, const char *what) {
-    if (need <= *cap) return WAX_VS_OK;
-    if (*p) { cudaFree(*p); *p = nullptr; *cap = 0; }
-    if (cudaMalloc(p, need * sizeof(T)) != cudaSuccess)
-        return fail(WAX_VS_ERR_CUDA, "failed to allocate %s (%zu bytes): %s", what, need * sizeof(T),
-                    cudaGetErrorString(cudaGetLastError()));
-    *cap = need;
-    return WAX_VS_OK;
-}
-template <typename T>
-static int32_t ensure_pinned(T **p, size_t *cap, size_t need, const char *what) {
-    if (need <= *cap) return WAX_VS_OK;
-    if (*p) { cudaFreeHost(*p); *p = nullptr; *cap = 0; }
-    // mapped + portable: kernels may write results straight into it (host delivery), any device may use it
-    if (cudaHostAlloc(reinterpret_cast<void **>(p), need * sizeof(T), cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess)
-        return fail(WAX_VS_ERR_CUDA, "failed to allocate pinned %s (%zu bytes): %s", what, need * sizeof(T),
-                    cudaGetErrorString(cudaGetLastError()));
-    *cap = need;
     return WAX_VS_OK;
 }
 
@@ -544,6 +546,17 @@ static int32_t wait_host_flag(cudaStream_t stream, unsigned long long *flag_ptr,
     }
 }
 
+// n host queries -> pinned staging (c->h_queries) -> c->d_queries, on `stream`
+static int32_t stage_queries(wax_vs_engine *e, SearchCtx *c, const float *queries, uint32_t n, cudaStream_t stream) {
+    const size_t qfloats = static_cast<size_t>(n) * e->dims;
+    int32_t rc = c->d_queries.ensure(qfloats, "query buffer");
+    if (!rc) rc = c->h_queries.ensure(qfloats, "query staging");
+    if (rc) return rc;
+    memcpy(c->h_queries, queries, qfloats * sizeof(float));
+    CUDA_TRY(cudaMemcpyAsync(c->d_queries, c->h_queries, qfloats * sizeof(float), cudaMemcpyHostToDevice, stream));
+    return WAX_VS_OK;
+}
+
 // Host delivery (the synchronous host entry points, fused top-k only): h_query travels in the kernel parameters when the
 // kernel can take it (else it is copied H2D here), and the kernel stores the result into host_out + raises host_flag.
 struct HostDelivery {
@@ -564,7 +577,8 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
     if (shard) {
         if (k_eff > static_cast<uint32_t>(kShardKCap))
             return fail(WAX_VS_ERR_UNSUPPORTED, "sharded search supports top_k <= %d (got %u)", kShardKCap, k_eff);
-        if (!c->d_shard_local) CUDA_TRY(cudaMalloc(&c->d_shard_local, kShardKCap * sizeof(wax_vs_candidate)));
+        int32_t rc = c->d_shard_local.ensure(kShardKCap, "shard candidates");
+        if (rc) return rc;
         d_merged = d_out;
         d_out = c->d_shard_local;           // the scan produces the LOCAL list; the exchange writes d_merged
     }
@@ -574,15 +588,6 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
         shard_exchange_kernel<<<1, 256, 0, stream>>>(sp, d_out, k_eff);
         CUDA_TRY(cudaGetLastError());
         ++*launches;
-        return WAX_VS_OK;
-    };
-    auto stage_query = [&]() -> int32_t {            // host query -> pinned staging -> device, on `stream`
-        int32_t rc = ensure_dev(&c->d_queries, &c->d_queries_cap, static_cast<size_t>(e->dims), "query buffer");
-        if (!rc) rc = ensure_pinned(&c->h_queries, &c->h_queries_cap, static_cast<size_t>(e->dims), "query staging");
-        if (rc) return rc;
-        memcpy(c->h_queries, host->h_query, e->dims * sizeof(float));
-        CUDA_TRY(cudaMemcpyAsync(c->d_queries, c->h_queries, e->dims * sizeof(float), cudaMemcpyHostToDevice, stream));
-        d_query = c->d_queries;
         return WAX_VS_OK;
     };
     if (e->n_rows == 0) {
@@ -603,10 +608,10 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
     const bool emit = k_eff > static_cast<uint32_t>(e->tune.fused_k_max);
     const int mode = emit ? 2 : (k_eff <= 32 ? 0 : 1);
     if (emit) {
-        int32_t rc = ensure_dev(&c->d_dist_keys, &c->dist_keys_cap, static_cast<size_t>(e->n_rows), "distance keys");
+        int32_t rc = c->d_dist_keys.ensure(static_cast<size_t>(e->n_rows), "distance keys");
+        if (!rc) rc = c->d_select.ensure(1, "selection state");
+        if (!rc) rc = c->d_sel_keys.ensure(16384, "selected keys");
         if (rc) return rc;
-        if (!c->d_select) CUDA_TRY(cudaMalloc(&c->d_select, sizeof(SelectState)));
-        if (!c->d_sel_keys) CUDA_TRY(cudaMalloc(&c->d_sel_keys, 16384 * sizeof(uint64_t)));
         p.dist_keys = c->d_dist_keys;
     }
 
@@ -620,9 +625,9 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
             memcpy(p.query_inline, host->h_query, e->dims * sizeof(float));
             p.query = nullptr;
         } else {
-            int32_t rc = stage_query();
+            int32_t rc = stage_queries(e, c, host->h_query, 1, stream);
             if (rc) return rc;
-            p.query = d_query;
+            p.query = c->d_queries;
         }
     }
     if (host && host->host_out && !emit && !shard) {
@@ -641,7 +646,7 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
         if (fused_exchange) { p.shard = *shard; p.shard.final_out = d_merged; }
     }
     int grid;
-    const int grid_cap = static_cast<int>(c->block_keys_cap / 128);
+    const int grid_cap = static_cast<int>(c->d_block_keys.cap / 128);
     if (use_tma) {
         p.stages = static_cast<uint32_t>(cfg.stages);
         const uint64_t steps = (e->n_rows + cfg.R - 1) / cfg.R;
@@ -670,13 +675,7 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
         select_compact_kernel<<<sgrid, 512, 0, stream>>>(c->d_dist_keys, n, c->d_select, c->d_sel_keys, 16384);
         uint32_t pow2 = 64;
         while (pow2 < k_eff) pow2 <<= 1;
-        {   // opt-in shared-memory limits are per function AND per device: once per engine, not once per process
-            std::lock_guard<std::mutex> ag(e->attr_mu);
-            if (!e->sort_attr_set) {
-                CUDA_TRY(cudaFuncSetAttribute(select_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8));
-                e->sort_attr_set = true;
-            }
-        }
+        CUDA_TRY(grant_smem(e, select_sort_kernel, pow2 * sizeof(uint64_t)));
         select_sort_kernel<<<1, 1024, pow2 * sizeof(uint64_t), stream>>>(c->d_select, c->d_sel_keys, pow2, p);
         CUDA_TRY(cudaGetLastError());
         *launches += 3 + 2 * kSelectPasses;
@@ -737,13 +736,17 @@ static bool batch_tensor_eligible(const wax_vs_engine *e, uint32_t n_queries, ui
 // computed, the running max only grows); anything that moves or overwrites rows resets norms_rows to 0.
 static int32_t ensure_norms_locked(wax_vs_engine *e, cudaStream_t stream) {
     if (e->norms_rows == e->n_rows && e->d_inv_norm) return WAX_VS_OK;
-    if (static_cast<size_t>(e->n_rows) > e->inv_norm_cap || !e->d_inv_norm) {
-        e->norms_rows = 0;                                       // ensure_dev re-allocates: the cached prefix is gone
+    if (static_cast<size_t>(e->n_rows) > e->d_inv_norm.cap || !e->d_inv_norm) {
+        e->norms_rows = 0;                                       // ensure re-allocates: the cached prefix is gone
         const size_t want = static_cast<size_t>(std::max<uint64_t>(e->cap_rows, std::max<uint64_t>(e->n_rows, 1)));
-        int32_t rc = ensure_dev(&e->d_inv_norm, &e->inv_norm_cap, want, "row norms");
+        int32_t rc = e->d_inv_norm.ensure(want, "row norms");
         if (rc) return rc;
     }
-    if (!e->d_max_norm) { CUDA_TRY(cudaMalloc(&e->d_max_norm, sizeof(uint32_t))); e->norms_rows = 0; }
+    if (!e->d_max_norm) {
+        int32_t rc = e->d_max_norm.ensure(1, "max row norm");
+        if (rc) return rc;
+        e->norms_rows = 0;
+    }
     if (e->norms_rows > e->n_rows) e->norms_rows = 0;
     if (e->norms_rows == 0) CUDA_TRY(cudaMemsetAsync(e->d_max_norm, 0, sizeof(uint32_t), stream));
     const uint64_t first = e->norms_rows, count = e->n_rows - first;
@@ -777,8 +780,8 @@ static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream) {
     if (rc) return rc;
     const size_t need = static_cast<size_t>(e->n_rows) * e->dims;                                  // must hold
     const size_t pref = static_cast<size_t>(std::max<uint64_t>(e->cap_rows, e->n_rows)) * e->dims;   // would like
-    if (e->shadow_cap < need) {
-        if (e->d_shadow) { cudaFree(e->d_shadow); e->d_shadow = nullptr; e->shadow_cap = 0; }
+    if (e->d_shadow.cap < need) {
+        e->d_shadow.release();
         e->shadow_rows = 0; e->shadow_valid = false;
         size_t free_b = 0, total_b = 0;
         size_t want = pref;
@@ -788,12 +791,13 @@ static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream) {
         const bool info = cudaMemGetInfo(&free_b, &total_b) == cudaSuccess;
         const size_t headroom = std::max<size_t>(size_t(2) << 30, total_b / 10);
         if (info && free_b < bytes + headroom) { want = need; bytes = want * sizeof(__nv_bfloat16); }
-        if (!info || free_b < bytes + headroom || cudaMalloc(&e->d_shadow, bytes) != cudaSuccess) {
+        // allocated by hand, not through ensure(): running out here is not an error and sets no last error
+        if (!info || free_b < bytes + headroom || cudaMalloc(&e->d_shadow.p, bytes) != cudaSuccess) {
             cudaGetLastError();
             e->shadow_unavailable = true;      // stays off for this engine: TF32 nominations need no extra memory
             return WAX_VS_OK;
         }
-        e->shadow_cap = want;
+        e->d_shadow.cap = want;
     }
     if (e->shadow_rows > e->n_rows) e->shadow_rows = 0;
     const uint64_t first = e->shadow_rows, count = e->n_rows - first;
@@ -810,18 +814,17 @@ static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream) {
     return WAX_VS_OK;
 }
 
-template <typename K>
-static cudaError_t set_smem_attr(K kernel, uint32_t bytes) {
-    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
-}
-
-template <typename K>
-static cudaError_t launch_nominate(K kernel, uint32_t grid, uint32_t smem, bool pair, cudaStream_t stream,
-                                   const CUtensorMap &map_q, const CUtensorMap &map_c, const BatchParams &bp) {
+// One launch of the nominate kernel in one form; its opt-in shared memory is granted first.
+template <bool BF, bool FI, bool AR, bool PR, bool DUMP>
+static cudaError_t launch_nominate_inst(wax_vs_engine *e, uint32_t grid, uint32_t smem, cudaStream_t stream,
+                                        const CUtensorMap &map_q, const CUtensorMap &map_c, const BatchParams &bp) {
+    const auto kernel = batch_nominate_kernel<BF, FI, AR, PR, DUMP>;
+    const cudaError_t err = grant_smem(e, kernel, smem);
+    if (err != cudaSuccess) return err;
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kBatchThreads); cfg.stream = stream; cfg.dynamicSmemBytes = smem;
     cudaLaunchAttribute attr[1];
-    if (pair) {
+    if (PR) {
         attr[0].id = cudaLaunchAttributeClusterDimension;
         attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
         cfg.attrs = attr; cfg.numAttrs = 1;
@@ -829,37 +832,20 @@ static cudaError_t launch_nominate(K kernel, uint32_t grid, uint32_t smem, bool 
     return cudaLaunchKernelEx(&cfg, kernel, map_q, map_c, bp);
 }
 
-// The heap forms with the score read-out (wax_vs_debug_batch_nominations); `set_attr`: allow the whole opt-in smem.
-static cudaError_t launch_nominate_dump(bool bf16, bool ares, bool pair, uint32_t grid, uint32_t smem, cudaStream_t stream,
-                                        const CUtensorMap &map_q, const CUtensorMap &map_c, const BatchParams &bp) {
-#define WAXVS_NOM(BF, AR, PR)                                                                                          \
-    do {                                                                                                               \
-        const cudaError_t err = set_smem_attr(batch_nominate_kernel<BF, false, AR, PR, true>, kBatchSmemOptin);        \
-        if (err != cudaSuccess) return err;                                                                            \
-        return launch_nominate(batch_nominate_kernel<BF, false, AR, PR, true>, grid, smem, PR, stream, map_q, map_c, bp); \
-    } while (0)
-    if (!bf16) {
-        if (pair) WAXVS_NOM(false, false, true);
-        WAXVS_NOM(false, false, false);
-    }
-    if (ares) {
-        if (pair) WAXVS_NOM(true, true, true);
-        WAXVS_NOM(true, true, false);
-    }
-    if (pair) WAXVS_NOM(true, false, true);
-    WAXVS_NOM(true, false, false);
-#undef WAXVS_NOM
-}
-
-// One launch of the nominate kernel in the form (bf16, filter, resident queries, CTA pair) the caller picked.
-static cudaError_t launch_nominate_form(bool bf16, bool filter, bool ares, bool pair, uint32_t grid, uint32_t smem,
-                                        cudaStream_t stream, const CUtensorMap &map_q, const CUtensorMap &map_c,
-                                        const BatchParams &bp) {
-#define WAXVS_NOM(BF, FI, AR, PR) return launch_nominate(batch_nominate_kernel<BF, FI, AR, PR>, grid, smem, PR, stream, map_q, map_c, bp)
-    if (filter) {
-        if (!bf16) WAXVS_NOM(false, true, false, false);
-        if (ares) WAXVS_NOM(true, true, true, false);
-        WAXVS_NOM(true, true, false, false);
+// The nominate kernel in the form (bf16, filter, resident queries, CTA pair) a pass picked; DUMP: with the score
+// read-out (wax_vs_debug_batch_nominations).  These are all the forms there are: the filter level runs neither as CTA
+// pairs nor with the read-out, and TF32 queries always stream through the ring.
+template <bool DUMP>
+static cudaError_t launch_nominate(wax_vs_engine *e, bool bf16, bool filter, bool ares, bool pair, uint32_t grid,
+                                   uint32_t smem, cudaStream_t stream, const CUtensorMap &map_q, const CUtensorMap &map_c,
+                                   const BatchParams &bp) {
+#define WAXVS_NOM(BF, FI, AR, PR) return launch_nominate_inst<BF, FI, AR, PR, DUMP>(e, grid, smem, stream, map_q, map_c, bp)
+    if constexpr (!DUMP) {
+        if (filter) {
+            if (!bf16) WAXVS_NOM(false, true, false, false);
+            if (ares) WAXVS_NOM(true, true, true, false);
+            WAXVS_NOM(true, true, false, false);
+        }
     }
     if (!bf16) {
         if (pair) WAXVS_NOM(false, false, false, true);
@@ -874,6 +860,7 @@ static cudaError_t launch_nominate_form(bool bf16, bool filter, bool ares, bool 
 #undef WAXVS_NOM
 }
 
+// ---- nominee-heap policy (level 1) ----
 // P(X >= h) for X ~ Poisson(m): the chance that one row slice holds h or more of a query's "threatening" rows.
 static double poisson_tail(double m, int h) {
     double term = std::exp(-m);                      // P(X = 0)
@@ -883,11 +870,141 @@ static double poisson_tail(double m, int h) {
     return std::min(1.0, tail + t);
 }
 
-// Enqueue the tensor-core nomination + exact finish for n_queries device-resident queries.  d_ok[i] = 1 when
-// query i's result is proven exact; the caller sends the others to the filter level, then to enqueue_search.
-// allow_bf16 = false forces TF32 nominations (adaptive level choice).  *used_bf16 reports what ran; d_tau_star
-// (optional) receives each query's threshold for the filter level.  `dump` (tests only, one launch at most) runs the
-// same shape with the score read-out and reports the shape.
+// Nominee heap size per (slice, query) = kernel shape, for nq queries over `slices` row slices.  TF32 shapes: 16 entries
+// when 16 nominees per slice comfortably cover k (16 * slices >= 8 k), else 64.  bf16 shapes (16 / 24 / 32 / 64): level 1
+// can prove a query only if no slice holds `heap` rows scoring within the bf16 bound of the k-th result; with the corpus
+// spread over the slices those "threatening" rows (about 2.2 k of them for the bf16 bound on unit-scale embeddings) fall
+// ~Poisson(m = 2.2 k / slices) per slice.  ONE unproven query costs its whole batch a second pass, while larger heaps
+// cost ring stages (4 / 3 / 3 / 2): the heap that minimises the expected cost is picked, then raised by heap_bump.
+static uint32_t pick_heap(wax_vs_engine *e, bool bf16, uint32_t nq, uint32_t slices, uint32_t k_eff) {
+    const bool small_heap = e->tune.batch_heap == 16 || (e->tune.batch_heap == 0 && 16u * slices >= 8u * k_eff);
+    if (!bf16) return small_heap ? 16u : 64u;
+    uint32_t want = static_cast<uint32_t>(std::max(e->tune.batch_heap, 0));
+    if (k_eff > 128u && want == 0u) want = 64u;       // large k: level 1 only has to NOMINATE k rows (filter level decides)
+    if (want == 16u || want == 24u || want == 32u || want == 64u) return want;
+    // expected cost of a batch = the shape's relative time + P(some query of the batch is unproven) x one more
+    // pass.  Threatening rows per query: ~2.2 k (cosine, unit rows) / ~2.8 k (dot: the bound scales with the
+    // LARGEST row norm).  The relative times of the heap sizes are guesses carried over from B200 (ring depths
+    // 4 / 3 / 3 / 2 on H100); they have not been measured on H100.
+    static const uint32_t ladder[4] = {16u, 24u, 32u, 64u};
+    static const double rel_time[4] = {1.00, 1.02, 1.10, 1.40};
+    const double m = (e->similarity == WAX_VS_DOT ? 2.8 : 2.2) * k_eff / slices;
+    uint32_t bump = 0;
+    { std::lock_guard<std::mutex> pg(e->pool_mu); bump = e->heap_bump; }
+    double best = 1e30;
+    uint32_t pick = 3u;
+    for (uint32_t i = 0; i < 4u; ++i) {
+        const double p_fail = std::min(1.0, static_cast<double>(nq) * slices * poisson_tail(m, static_cast<int>(ladder[i])));
+        if (p_fail >= 1.0 && ladder[i] != 64u) continue;             // hopeless: every batch would pay a second pass
+        const double cost = rel_time[i] + 4.0 * p_fail;              // risk-averse: the model can be off
+        if (cost < best) { best = cost; pick = i; }
+    }
+    return ladder[std::min(pick + bump, 3u)];                         // the data overrules the model (below)
+}
+
+// After a level-1 batch that nominated from the bf16 shadow with k <= 128 (large k is expected to need the filter
+// level).  When more than a quarter of the batch is unproven (tightly clustered neighbours), the next 16 batches
+// nominate in TF32.  With the automatic heap size the data has the last word on it: unproven queries -> one size up
+// for `heap_backoff` batches; when that time-out ends one size down is probed again, and a failure during the probe
+// doubles the time-out.
+static void record_level1_outcome(wax_vs_engine *e, uint32_t n_queries, size_t unproven, uint32_t used_heap) {
+    std::lock_guard<std::mutex> pg(e->pool_mu);
+    if (unproven * 4 > n_queries) e->bf16_skip_batches = 16;
+    if (used_heap == 0u || e->tune.batch_heap != 0) return;
+    e->last_heap = used_heap;
+    if (unproven && used_heap < 64u) {
+        if (e->heap_probing) e->heap_backoff = std::min<uint32_t>(e->heap_backoff * 2u, 1u << 16);
+        e->heap_bump = std::min<uint32_t>(e->heap_bump + 1u, 3u);
+        e->heap_bump_ttl = e->heap_backoff;
+    }
+    e->heap_probing = false;
+    if (!unproven && e->heap_bump > 0 && e->heap_bump_ttl > 0 && --e->heap_bump_ttl == 0) {
+        --e->heap_bump;
+        e->heap_probing = true;
+        e->heap_bump_ttl = e->heap_bump ? e->heap_backoff : 0;
+    }
+}
+
+// ---- the tensor-core nomination pass of both levels ----
+// One launch of a pass: queries [q0, q0 + nq) in `groups` query groups, each over `slices` row slices.
+struct NominateChunk {
+    uint32_t q0, nq, groups, slices, kprime;
+    const float *queries;       // the launch's fp32 queries
+    bool ares, pair;
+    int stages;
+};
+
+// Enqueues one nomination pass over n_queries device queries on `stream`, in launches of at most max_groups query groups,
+// and owns what the levels share: the bf16 query conversion, the tensor maps, the ring shape and the common BatchParams.
+// The level supplies the heap size (heap(nq, slices) -> kprime), its own BatchParams fields (prepare(chunk, bp)) and
+// the launches that follow each nomination launch (finish(chunk)).  pair: CTA pairs when a launch has two query groups
+// or more; dump: the score read-out forms.
+template <typename Heap, typename Prepare, typename Finish>
+static int32_t enqueue_nominate_pass(wax_vs_engine *e, SearchCtx *c, const float *d_queries, uint32_t n_queries, bool bf16,
+                                     bool filter, bool pair, bool dump, uint32_t max_groups, const uint32_t *d_mask,
+                                     cudaStream_t stream, uint64_t *launches, Heap heap, Prepare prepare, Finish finish) {
+    int32_t rc;
+    // bf16 nominations: convert the queries once per call (n_queries x dims, tiny next to the corpus pass)
+    if (bf16) {
+        const size_t qn = static_cast<size_t>(n_queries) * e->dims;
+        if ((rc = c->d_queries_bf16.ensure(qn, "bf16 queries"))) return rc;
+        const int g = static_cast<int>(std::min<size_t>((qn / 4 + 255) / 256, static_cast<size_t>(e->sm_count) * 8));
+        shadow_bf16_kernel<<<std::max(g, 1), 256, 0, stream>>>(d_queries, nullptr, n_queries, e->dims, c->d_queries_bf16);
+        CUDA_TRY(cudaGetLastError());
+        ++*launches;
+    }
+    const uint32_t tiles_total = static_cast<uint32_t>((e->n_rows + kBatchN - 1) / kBatchN);
+    const uint32_t num_kb16 = e->dims / kBatchKBlockBf16;
+    for (uint32_t q0 = 0; q0 < n_queries; q0 += max_groups * kBatchM) {
+        NominateChunk ch{};
+        ch.q0 = q0;
+        ch.nq = std::min<uint32_t>(n_queries - q0, max_groups * kBatchM);
+        ch.queries = d_queries + static_cast<size_t>(q0) * e->dims;
+        ch.groups = (ch.nq + kBatchM - 1) / kBatchM;
+        // CTA pairs (two query groups, one row slice, each CTA loads half of every corpus tile for both): needs at least
+        // two groups; an odd group count is padded with an all-out-of-range group.
+        ch.pair = pair && ch.groups >= 2;
+        if (ch.pair) ch.groups = (ch.groups + 1u) & ~1u;
+        const uint32_t units = ch.pair ? ch.groups / 2u : ch.groups;
+        const uint32_t unit_slots = static_cast<uint32_t>(e->sm_count) / (ch.pair ? 2u : 1u);
+        ch.slices = std::max<uint32_t>(1, std::min<uint32_t>(unit_slots / units, tiles_total));
+        ch.kprime = heap(ch.nq, ch.slices);
+        ch.slices = std::max<uint32_t>(1, std::min<uint32_t>(ch.slices, 16384u / ch.kprime));   // union fits the finish sort
+        // resident queries (bf16) when a ring of at least two corpus stages still fits beside them
+        const int ares_st = (bf16 && e->tune.batch_ares) ? batch_ring_stages(static_cast<int>(ch.kprime), num_kb16) : 0;
+        ch.ares = ares_st >= 2;
+        ch.stages = ch.ares ? ares_st : batch_ring_stages(static_cast<int>(ch.kprime));
+        // bf16: the converted queries against the corpus shadow; TF32: the fp32 queries against the corpus
+        const void *qbase = bf16 ? static_cast<const void *>(c->d_queries_bf16 + static_cast<size_t>(q0) * e->dims) : ch.queries;
+        const void *cbase = bf16 ? static_cast<const void *>(e->d_shadow.p) : e->d_corpus;
+        CUtensorMap map_q, map_c;
+        if ((rc = make_tensor_map(&map_q, qbase, ch.nq, e->dims, kBatchM, bf16))) return rc;
+        if ((rc = make_tensor_map(&map_c, cbase, e->n_rows, e->dims, ch.pair ? kBatchN / 2 : kBatchN, bf16))) return rc;
+        BatchParams bp{};
+        bp.n_rows = static_cast<uint32_t>(e->n_rows); bp.dims = e->dims; bp.n_queries = ch.nq; bp.groups = ch.groups;
+        bp.slices = ch.slices; bp.tiles_total = tiles_total; bp.kprime = ch.kprime; bp.metric = e->similarity;
+        bp.stages = static_cast<uint32_t>(ch.stages);
+        // the cosine shadow rows are pre-normalised: no epilogue scaling on the bf16 path
+        bp.row_scale = (e->similarity == WAX_VS_COSINE && !bf16) ? e->d_inv_norm.p : nullptr;
+        bp.allow_bits = d_mask;
+        if ((rc = prepare(ch, bp))) return rc;
+        const uint32_t grid = ch.groups * ch.slices;
+        const uint32_t smem = batch_smem_bytes(ch.stages, static_cast<int>(ch.kprime), ch.ares ? num_kb16 : 0u);
+        const cudaError_t lerr = dump ? launch_nominate<true>(e, bf16, filter, ch.ares, ch.pair, grid, smem, stream, map_q, map_c, bp)
+                                      : launch_nominate<false>(e, bf16, filter, ch.ares, ch.pair, grid, smem, stream, map_q, map_c, bp);
+        CUDA_TRY(lerr);
+        CUDA_TRY(cudaGetLastError());
+        ++*launches;
+        if ((rc = finish(ch))) return rc;
+    }
+    return WAX_VS_OK;
+}
+
+// Level 1: the tensor-core nomination + exact finish for n_queries device-resident queries.  d_ok[i] = 1 when query i's
+// result is proven exact; the caller sends the others to the filter level, then to enqueue_search.  allow_bf16 = false
+// forces TF32 nominations (adaptive level choice).  *used_bf16 reports what ran; d_tau_star (optional) receives each
+// query's threshold for the filter level.  `dump` (tests only, one launch at most) runs the same shape with the score
+// read-out and reports the shape.
 struct NominationDump {
     float *d_scores;        // [n_queries][n_rows]
     uint32_t shape[7];      // bf16, ares, pair, stages, kprime, slices, groups
@@ -912,38 +1029,6 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
     if (k_eff > 128u) max_groups = std::max<uint32_t>(1u, max_groups / ((k_eff * 115u / 100u + 63u) / 64u));
     if (dump && n_queries > max_groups * kBatchM)
         return fail(WAX_VS_ERR_ARGUMENT, "the nomination read-out covers one launch: at most %u queries", max_groups * kBatchM);
-    cudaError_t attr_err = cudaSuccess;
-    {   // per function and per DEVICE: once per engine
-        std::lock_guard<std::mutex> ag(e->attr_mu);
-        if (!e->batch_attr_set) {
-            auto chk = [&](cudaError_t r) { if (attr_err == cudaSuccess) attr_err = r; };
-            // every form may use the whole opt-in shared memory; each launch asks for what its ring and heaps need
-            chk(set_smem_attr(batch_nominate_kernel<false, false, false, false>, kBatchSmemOptin));
-            chk(set_smem_attr(batch_nominate_kernel<false, false, false, true>, kBatchSmemOptin));
-            chk(set_smem_attr(batch_nominate_kernel<true, false, false, false>, kBatchSmemOptin));
-            chk(set_smem_attr(batch_nominate_kernel<true, false, false, true>, kBatchSmemOptin));
-            chk(set_smem_attr(batch_nominate_kernel<true, false, true, false>, kBatchSmemOptin));
-            chk(set_smem_attr(batch_nominate_kernel<true, false, true, true>, kBatchSmemOptin));
-            chk(set_smem_attr(batch_nominate_kernel<false, true, false, false>, kBatchSmemOptin));
-            chk(set_smem_attr(batch_nominate_kernel<true, true, false, false>, kBatchSmemOptin));
-            chk(set_smem_attr(batch_nominate_kernel<true, true, true, false>, kBatchSmemOptin));
-            chk(set_smem_attr(filter_select_kernel, 16384 * 8));
-            chk(set_smem_attr(batch_finish_kernel<kCosine>, (16384 + kBatchRescoreMax) * 8));
-            chk(set_smem_attr(batch_finish_kernel<kDot>, (16384 + kBatchRescoreMax) * 8));
-            e->batch_attr_set = attr_err == cudaSuccess;
-        }
-    }
-    if (attr_err != cudaSuccess) return fail(WAX_VS_ERR_CUDA, "cudaFuncSetAttribute failed: %s", cudaGetErrorString(attr_err));
-
-    // bf16 nominations: convert the queries once per call (n_queries x dims, tiny next to the corpus pass)
-    if (bf16) {
-        const size_t qn = static_cast<size_t>(n_queries) * e->dims;
-        if ((rc = ensure_dev(&c->d_queries_bf16, &c->queries_bf16_cap, qn, "bf16 queries"))) return rc;
-        const int g = static_cast<int>(std::min<size_t>((qn / 4 + 255) / 256, static_cast<size_t>(e->sm_count) * 8));
-        shadow_bf16_kernel<<<std::max(g, 1), 256, 0, stream>>>(d_queries, nullptr, n_queries, e->dims, c->d_queries_bf16);
-        CUDA_TRY(cudaGetLastError());
-        ++*launches;
-    }
     // how many nominees the finish kernel re-scores exactly: the (rescore+1)-th nominee bounds the rows it skips, and
     // the coarser bf16 bound needs more distance between it and the k-th result (DESIGN 4.5)
     uint32_t rescore = static_cast<uint32_t>(kBatchRescore);
@@ -952,114 +1037,48 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
     if (k_eff > 128u) rescore = static_cast<uint32_t>(kBatchRescoreMax);   // the finish kernel writes k re-scored nominees
     rescore = rescore <= 256u ? 256u : (rescore <= 512u ? 512u : static_cast<uint32_t>(kBatchRescoreMax));
 
-    for (uint32_t q0 = 0; q0 < n_queries; q0 += max_groups * kBatchM) {
-        const uint32_t nq = std::min<uint32_t>(n_queries - q0, max_groups * kBatchM);
-        uint32_t groups = (nq + kBatchM - 1) / kBatchM;
-        // CTA pairs (two query groups, one row slice, each CTA loads half of every corpus tile for both): needs at least
-        // two groups; an odd group count is padded with an all-out-of-range group.
-        const bool pair = e->tune.batch_pair != 0 && groups >= 2;
-        if (pair) groups = (groups + 1u) & ~1u;
-        const uint32_t tiles_total = static_cast<uint32_t>((e->n_rows + kBatchN - 1) / kBatchN);
-        const uint32_t units = pair ? groups / 2u : groups, unit_slots = static_cast<uint32_t>(e->sm_count) / (pair ? 2u : 1u);
-        uint32_t slices = std::max<uint32_t>(1, std::min<uint32_t>(unit_slots / units, tiles_total));
-        // Nominee heap size per (slice, query) = kernel shape.  TF32 shapes: 16 entries when 16 nominees per slice
-        // comfortably cover k (16 * slices >= 8 k), else 64.  bf16 shapes (16 / 24 / 32 / 64): level 1 can prove a query
-        // only if no slice holds `heap` rows scoring within the bf16 bound of the k-th result; with the corpus spread over
-        // the slices those "threatening" rows (about 2.2 k of them for the bf16 bound on unit-scale embeddings) fall
-        // ~Poisson(m = 2.2 k / slices) per slice.  ONE unproven query costs its whole batch a second pass, while larger
-        // heaps cost ring stages (4 / 3 / 3 / 2): the heap that minimises the expected cost is picked below.
-        const bool small_heap = e->tune.batch_heap == 16 || (e->tune.batch_heap == 0 && 16u * slices >= 8u * k_eff);
-        uint32_t kprime = small_heap ? 16u : 64u;
-        if (bf16) {
-            uint32_t want = static_cast<uint32_t>(std::max(e->tune.batch_heap, 0));
-            if (k_eff > 128u && want == 0u) want = 64u;       // large k: level 1 only has to NOMINATE k rows (filter level decides)
-            if (want != 16u && want != 24u && want != 32u && want != 64u) {
-                // expected cost of a batch = the shape's relative time + P(some query of the batch is unproven) x one more
-                // pass.  Threatening rows per query: ~2.2 k (cosine, unit rows) / ~2.8 k (dot: the bound scales with the
-                // LARGEST row norm).  The relative times of the heap sizes are guesses carried over from B200 (ring depths
-                // 4 / 3 / 3 / 2 on H100); they have not been measured on H100.
-                static const uint32_t ladder[4] = {16u, 24u, 32u, 64u};
-                static const double rel_time[4] = {1.00, 1.02, 1.10, 1.40};
-                const double m = (e->similarity == WAX_VS_DOT ? 2.8 : 2.2) * k_eff / slices;
-                uint32_t bump = 0;
-                { std::lock_guard<std::mutex> pg(e->pool_mu); bump = e->heap_bump; }
-                double best = 1e30;
-                uint32_t pick = 3u;
-                for (uint32_t i = 0; i < 4u; ++i) {
-                    const double p_fail = std::min(1.0, static_cast<double>(nq) * slices * poisson_tail(m, static_cast<int>(ladder[i])));
-                    if (p_fail >= 1.0 && ladder[i] != 64u) continue;             // hopeless: every batch would pay a second pass
-                    const double cost = rel_time[i] + 4.0 * p_fail;              // risk-averse: the model can be off
-                    if (cost < best) { best = cost; pick = i; }
-                }
-                pick = std::min(pick + bump, 3u);                                // the data overrules the model (see caller)
-                want = ladder[pick];
-            }
-            kprime = want;
-            if (used_heap) *used_heap = std::max(*used_heap, kprime);
-        }
-        slices = std::max<uint32_t>(1, std::min<uint32_t>(slices, 16384u / kprime));   // union fits the finish sort
-        const uint32_t grid = groups * slices;
-        // resident queries (bf16) when a ring of at least two corpus stages still fits beside them
-        const uint32_t num_kb16 = e->dims / kBatchKBlockBf16;
-        const int ares_st = (bf16 && e->tune.batch_ares) ? batch_ring_stages(static_cast<int>(kprime), num_kb16) : 0;
-        const bool ares = ares_st >= 2;
-        const int stages = ares ? ares_st : batch_ring_stages(static_cast<int>(kprime));
-        if ((rc = ensure_dev(&c->d_heaps, &c->heaps_cap, static_cast<size_t>(grid) * kBatchM * kprime, "nominee heaps"))) return rc;
-        if ((rc = ensure_dev(&c->d_tau, &c->tau_cap, static_cast<size_t>(groups) * kBatchM, "shared thresholds"))) return rc;
-        CUDA_TRY(cudaMemsetAsync(c->d_tau, 0, static_cast<size_t>(groups) * kBatchM * sizeof(uint32_t), stream));
-        CUtensorMap map_q, map_c;
-        const float *qbase = d_queries + static_cast<size_t>(q0) * e->dims;
-        if (bf16) {
-            if ((rc = make_tensor_map(&map_q, c->d_queries_bf16 + static_cast<size_t>(q0) * e->dims, nq, e->dims, kBatchM, true))) return rc;
-            if ((rc = make_tensor_map(&map_c, e->d_shadow, e->n_rows, e->dims, pair ? kBatchN / 2 : kBatchN, true))) return rc;
-        } else {
-            if ((rc = make_tensor_map(&map_q, qbase, nq, e->dims, kBatchM))) return rc;
-            if ((rc = make_tensor_map(&map_c, e->d_corpus, e->n_rows, e->dims, pair ? kBatchN / 2 : kBatchN))) return rc;
-        }
-
-        BatchParams bp{};
-        bp.n_rows = static_cast<uint32_t>(e->n_rows); bp.dims = e->dims; bp.n_queries = nq; bp.groups = groups;
-        bp.slices = slices; bp.tiles_total = tiles_total; bp.kprime = kprime; bp.metric = e->similarity;
-        bp.stages = static_cast<uint32_t>(stages);
-        // the cosine shadow rows are pre-normalised: no epilogue scaling on the bf16 path
-        bp.row_scale = (e->similarity == WAX_VS_COSINE && !bf16) ? e->d_inv_norm : nullptr;
+    auto heap = [&](uint32_t nq, uint32_t slices) { return pick_heap(e, bf16, nq, slices, k_eff); };
+    auto prepare = [&](const NominateChunk &ch, BatchParams &bp) -> int32_t {
+        const size_t slots = static_cast<size_t>(ch.groups) * kBatchM;
+        int32_t prc = c->d_heaps.ensure(slots * ch.slices * ch.kprime, "nominee heaps");
+        if (!prc) prc = c->d_tau.ensure(slots, "shared thresholds");
+        if (prc) return prc;
+        CUDA_TRY(cudaMemsetAsync(c->d_tau, 0, slots * sizeof(uint32_t), stream));
         bp.heaps = c->d_heaps;
         bp.tau_global = c->d_tau;
         bp.no_insert = e->tune.batch_noinsert ? 1u : 0u;
-        bp.allow_bits = d_mask;
-        const uint32_t smem = batch_smem_bytes(stages, static_cast<int>(kprime), ares ? num_kb16 : 0u);
-        cudaError_t lerr;
+        if (bf16 && used_heap) *used_heap = std::max(*used_heap, ch.kprime);
         if (dump) {
             bp.dump_scores = dump->d_scores;
-            const uint32_t shape[7] = {bf16, ares, pair, static_cast<uint32_t>(stages), kprime, slices, groups};
+            const uint32_t shape[7] = {bf16, ch.ares, ch.pair, static_cast<uint32_t>(ch.stages), ch.kprime, ch.slices, ch.groups};
             std::copy(shape, shape + 7, dump->shape);
-            lerr = launch_nominate_dump(bf16, ares, pair, grid, smem, stream, map_q, map_c, bp);
-        } else {
-            lerr = launch_nominate_form(bf16, false, ares, pair, grid, smem, stream, map_q, map_c, bp);
         }
-        CUDA_TRY(lerr);
-        CUDA_TRY(cudaGetLastError());
-
+        return WAX_VS_OK;
+    };
+    auto finish = [&](const NominateChunk &ch) -> int32_t {
         FinishParams fp{};
-        fp.corpus = e->d_corpus; fp.queries = qbase; fp.n_rows = bp.n_rows; fp.dims = e->dims; fp.n_queries = nq;
-        fp.groups = groups; fp.slices = slices; fp.kprime = kprime; fp.k = k_eff; fp.metric = e->similarity;
-        fp.heaps = c->d_heaps; fp.max_norm_bits = e->d_max_norm;
-        fp.out = d_out + static_cast<size_t>(q0) * k_eff; fp.ok = d_ok + q0;
+        fp.corpus = e->d_corpus; fp.queries = ch.queries; fp.n_rows = static_cast<uint32_t>(e->n_rows); fp.dims = e->dims;
+        fp.n_queries = ch.nq; fp.groups = ch.groups; fp.slices = ch.slices; fp.kprime = ch.kprime; fp.k = k_eff;
+        fp.metric = e->similarity; fp.heaps = c->d_heaps; fp.max_norm_bits = e->d_max_norm;
+        fp.out = d_out + static_cast<size_t>(ch.q0) * k_eff; fp.ok = d_ok + ch.q0;
         fp.frame_ids = d_ids; fp.id_base = e->id_base; fp.row_offset = row_offset;
         uint32_t pow2 = 512;
-        while (pow2 < slices * kprime) pow2 <<= 1;
+        while (pow2 < ch.slices * ch.kprime) pow2 <<= 1;
         fp.pow2_all = pow2;
         fp.rescore = rescore;
         fp.eps_rel = bf16 ? kBf16Eps : kTf32Eps;
-        fp.tau_star = d_tau_star ? d_tau_star + q0 : nullptr;
+        fp.tau_star = d_tau_star ? d_tau_star + ch.q0 : nullptr;
         fp.tau_stride = n_queries;
         const size_t fsmem = static_cast<size_t>(pow2 + rescore) * sizeof(uint64_t);
-        if (e->similarity == WAX_VS_COSINE) batch_finish_kernel<kCosine><<<nq, 512, fsmem, stream>>>(fp);
-        else batch_finish_kernel<kDot><<<nq, 512, fsmem, stream>>>(fp);
+        const auto kernel = e->similarity == WAX_VS_COSINE ? batch_finish_kernel<kCosine> : batch_finish_kernel<kDot>;
+        CUDA_TRY(grant_smem(e, kernel, fsmem));
+        kernel<<<ch.nq, 512, fsmem, stream>>>(fp);
         CUDA_TRY(cudaGetLastError());
-        *launches += 2;
-    }
-    return WAX_VS_OK;
+        ++*launches;
+        return WAX_VS_OK;
+    };
+    return enqueue_nominate_pass(e, c, d_queries, n_queries, bf16, false, e->tune.batch_pair != 0, dump != nullptr,
+                                 max_groups, d_mask, stream, launches, heap, prepare, finish);
 }
 
 static uint32_t clamp_topk(int64_t k) {  // MetalVectorEngine.swift:842-846
@@ -1084,7 +1103,7 @@ static int32_t set_capacity(wax_vs_engine *e, uint64_t rows) {
         // the bf16 shadow is derived data: give its HBM back before giving up (mutators hold the write lock)
         cudaGetLastError();
         if (e->d_shadow) {
-            cudaFree(e->d_shadow); e->d_shadow = nullptr; e->shadow_cap = 0; e->shadow_valid = false; e->shadow_rows = 0;
+            e->d_shadow.release(); e->shadow_valid = false; e->shadow_rows = 0;
             e->shadow_unavailable = true;
         }
         if (cudaMalloc(&n, bytes) != cudaSuccess)
@@ -1141,7 +1160,7 @@ static int32_t sync_device_ids(wax_vs_engine *e, const uint64_t **out) {
     std::lock_guard<std::mutex> g(e->ids_mu);
     if (e->ids_identity) { *out = nullptr; return WAX_VS_OK; }
     if (e->d_ids_dirty) {
-        int32_t rc = ensure_dev(&e->d_ids, &e->d_ids_cap, std::max<size_t>(e->ids.size(), 1), "frame ids");
+        int32_t rc = e->d_ids.ensure(std::max<size_t>(e->ids.size(), 1), "frame ids");
         if (rc) return rc;
         if (!e->ids.empty())
             CUDA_TRY(cudaMemcpy(e->d_ids, e->ids.data(), e->ids.size() * sizeof(uint64_t), cudaMemcpyHostToDevice));
@@ -1206,19 +1225,14 @@ int32_t wax_vs_create(uint32_t dimensions, uint8_t similarity, const int32_t *de
 
 void wax_vs_destroy(wax_vs_engine *e) {
     if (!e) return;
+    DeviceGuard g(e->device);      // the engine's own buffers go with `delete e`: on its device too
     {
         std::unique_lock<std::shared_mutex> w(e->rw);
-        DeviceGuard g(e->device);
         cudaDeviceSynchronize();
         shard_teardown(e, true);
-        ingest_free(e);
-        for (SearchCtx *c : e->pool) ctx_free(c);
-        for (auto &kv : e->stream_ctx) ctx_free(kv.second);
+        for (SearchCtx *c : e->pool) delete c;
+        for (auto &kv : e->stream_ctx) delete kv.second;
         if (e->d_corpus) cudaFree(e->d_corpus);
-        if (e->d_ids) cudaFree(e->d_ids);
-        if (e->d_inv_norm) cudaFree(e->d_inv_norm);
-        if (e->d_max_norm) cudaFree(e->d_max_norm);
-        if (e->d_shadow) cudaFree(e->d_shadow);
     }
     delete e;
 }
@@ -1324,19 +1338,6 @@ static int32_t shared_staging() {
     }
     return WAX_VS_OK;
 }
-static void ingest_free(wax_vs_engine *e) {
-    auto &g = e->ing;
-    for (int i = 0; i < 2; ++i) {
-        if (g.pin[i]) cudaFreeHost(g.pin[i]);
-        if (g.ev[i]) cudaEventDestroy(g.ev[i]);
-        g.pin[i] = nullptr; g.ev[i] = nullptr;
-    }
-    if (g.d_stage) cudaFree(g.d_stage);
-    if (g.d_index) cudaFree(g.d_index);
-    if (g.stream) cudaStreamDestroy(g.stream);
-    g = wax_vs_engine::Ingest();
-}
-
 static void parallel_memcpy(void *dst, const void *src, size_t bytes, int threads) {
     const size_t min_slice = size_t(2) << 20;
     int t = static_cast<int>(std::min<size_t>(static_cast<size_t>(std::max(threads, 1)), std::max<size_t>(1, bytes / min_slice)));
@@ -1495,8 +1496,8 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
     auto &ig = e->ing;
     if ((rc = ingest_init(e))) return rc;
     const uint64_t slab_rows = std::max<uint64_t>(1, std::min<uint64_t>(n, (size_t(256) << 20) / row_bytes));
-    if ((rc = ensure_dev(&ig.d_stage, &ig.d_stage_cap, static_cast<size_t>(slab_rows) * e->dims, "upsert staging"))) return rc;
-    if ((rc = ensure_dev(&ig.d_index, &ig.d_index_cap, static_cast<size_t>(slab_rows), "upsert targets"))) return rc;
+    if ((rc = ig.d_stage.ensure(static_cast<size_t>(slab_rows) * e->dims, "upsert staging"))) return rc;
+    if ((rc = ig.d_index.ensure(static_cast<size_t>(slab_rows), "upsert targets"))) return rc;
     for (uint64_t done = 0; done < n; done += slab_rows) {
         const uint64_t m = std::min(slab_rows, n - done);
         if ((rc = upload_bytes(e, ig.d_stage, rows + done * e->dims, m * row_bytes))) return rc;
@@ -1562,8 +1563,8 @@ int32_t wax_vs_remove_batch(wax_vs_engine *e, const uint64_t *frame_ids, uint64_
     const uint64_t moving = src.size();
     if (moving) {
         const uint64_t slab_rows = std::max<uint64_t>(1, std::min<uint64_t>(moving, (size_t(256) << 20) / row_bytes));
-        if ((rc = ensure_dev(&ig.d_stage, &ig.d_stage_cap, static_cast<size_t>(slab_rows) * e->dims, "compaction bounce buffer"))) return rc;
-        if ((rc = ensure_dev(&ig.d_index, &ig.d_index_cap, static_cast<size_t>(slab_rows), "compaction sources"))) return rc;
+        if ((rc = ig.d_stage.ensure(static_cast<size_t>(slab_rows) * e->dims, "compaction bounce buffer"))) return rc;
+        if ((rc = ig.d_index.ensure(static_cast<size_t>(slab_rows), "compaction sources"))) return rc;
         if ((rc = ingest_staging(e, slab_rows * sizeof(uint32_t)))) return rc;
         for (uint64_t done = 0; done < moving; done += slab_rows) {
             const uint64_t m = std::min(slab_rows, moving - done);
@@ -1613,71 +1614,59 @@ static int32_t enqueue_filter_level(wax_vs_engine *e, SearchCtx *c, const float 
                                     bool bf16 = false, const uint32_t *d_mask = nullptr) {
     int32_t rc = ensure_norms(e, stream);
     if (rc) return rc;
-    if (bf16) {
-        const size_t qn = static_cast<size_t>(n_queries) * e->dims;
-        if ((rc = ensure_dev(&c->d_queries_bf16, &c->queries_bf16_cap, qn, "bf16 queries"))) return rc;
-        const int g = static_cast<int>(std::min<size_t>((qn / 4 + 255) / 256, static_cast<size_t>(e->sm_count) * 8));
-        shadow_bf16_kernel<<<std::max(g, 1), 256, 0, stream>>>(d_queries, nullptr, n_queries, e->dims, c->d_queries_bf16);
-        CUDA_TRY(cudaGetLastError());
-        ++*launches;
-    }
     uint32_t cap = 64;                      // a power of two in [64, 16384], at least k
     while ((cap < static_cast<uint32_t>(std::max(e->tune.filter_cap, 64)) || cap < k_eff) && cap < 16384u) cap <<= 1;
-    if ((rc = ensure_dev(&c->d_cand_count, &c->cand_count_cap, static_cast<size_t>(n_queries), "filter counts"))) return rc;
-    if ((rc = ensure_dev(&c->d_cand_rows, &c->cand_rows_cap, static_cast<size_t>(n_queries) * cap, "filter candidates"))) return rc;
-    if ((rc = ensure_dev(&c->d_cand_keys, &c->cand_keys_cap, static_cast<size_t>(n_queries) * cap, "filter keys"))) return rc;
+    if ((rc = c->d_cand_count.ensure(static_cast<size_t>(n_queries), "filter counts"))) return rc;
+    if ((rc = c->d_cand_rows.ensure(static_cast<size_t>(n_queries) * cap, "filter candidates"))) return rc;
+    if ((rc = c->d_cand_keys.ensure(static_cast<size_t>(n_queries) * cap, "filter keys"))) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_cand_count, 0, static_cast<size_t>(n_queries) * sizeof(uint32_t), stream));
-    const uint32_t max_groups = static_cast<uint32_t>(e->sm_count);
-    const uint32_t tiles_total = static_cast<uint32_t>((e->n_rows + kBatchN - 1) / kBatchN);
-    for (uint32_t q0 = 0; q0 < n_queries; q0 += max_groups * kBatchM) {
-        const uint32_t nq = std::min<uint32_t>(n_queries - q0, max_groups * kBatchM);
-        const uint32_t groups = (nq + kBatchM - 1) / kBatchM;
-        const uint32_t slices = std::max<uint32_t>(1, std::min<uint32_t>(static_cast<uint32_t>(e->sm_count) / groups, tiles_total));
-        CUtensorMap map_q, map_c;
-        const float *qbase = d_queries + static_cast<size_t>(q0) * e->dims;
-        if (bf16) {
-            if ((rc = make_tensor_map(&map_q, c->d_queries_bf16 + static_cast<size_t>(q0) * e->dims, nq, e->dims, kBatchM, true))) return rc;
-            if ((rc = make_tensor_map(&map_c, e->d_shadow, e->n_rows, e->dims, kBatchN, true))) return rc;
-        } else {
-            if ((rc = make_tensor_map(&map_q, qbase, nq, e->dims, kBatchM))) return rc;
-            if ((rc = make_tensor_map(&map_c, e->d_corpus, e->n_rows, e->dims, kBatchN))) return rc;
-        }
-        BatchParams bp{};
-        bp.n_rows = static_cast<uint32_t>(e->n_rows); bp.dims = e->dims; bp.n_queries = nq; bp.groups = groups;
-        bp.slices = slices; bp.tiles_total = tiles_total; bp.kprime = 16; bp.metric = e->similarity;
-        bp.row_scale = (e->similarity == WAX_VS_COSINE && !bf16) ? e->d_inv_norm : nullptr;   // shadow rows are pre-normalised
-        bp.tau_fixed = d_tau + q0;
-        bp.cand_count = c->d_cand_count + q0;
-        bp.cand_rows = c->d_cand_rows + static_cast<size_t>(q0) * cap;
+    auto prepare = [&](const NominateChunk &ch, BatchParams &bp) -> int32_t {
+        bp.tau_fixed = d_tau + ch.q0;
+        bp.cand_count = c->d_cand_count + ch.q0;
+        bp.cand_rows = c->d_cand_rows + static_cast<size_t>(ch.q0) * cap;
         bp.cand_cap = cap;
-        bp.allow_bits = d_mask;
-        const uint32_t num_kb16 = e->dims / kBatchKBlockBf16;
-        const int ares_st = (bf16 && e->tune.batch_ares) ? batch_ring_stages(16, num_kb16) : 0;
-        const bool ares = ares_st >= 2;
-        const int stages = ares ? ares_st : batch_ring_stages(16);
-        bp.stages = static_cast<uint32_t>(stages);
-        CUDA_TRY(launch_nominate_form(bf16, true, ares, false, groups * slices, batch_smem_bytes(stages, 16, ares ? num_kb16 : 0u),
-                                      stream, map_q, map_c, bp));
-        const dim3 rgrid(32, nq);
-        if (e->similarity == WAX_VS_COSINE)
-            filter_rescore_kernel<kCosine><<<rgrid, 256, 0, stream>>>(e->d_corpus, qbase, e->dims, bp.cand_count, bp.cand_rows, cap,
-                                                                      c->d_cand_keys + static_cast<size_t>(q0) * cap);
-        else
-            filter_rescore_kernel<kDot><<<rgrid, 256, 0, stream>>>(e->d_corpus, qbase, e->dims, bp.cand_count, bp.cand_rows, cap,
-                                                                   c->d_cand_keys + static_cast<size_t>(q0) * cap);
+        return WAX_VS_OK;
+    };
+    auto finish = [&](const NominateChunk &ch) -> int32_t {
+        const uint32_t *count = c->d_cand_count + ch.q0;
+        uint64_t *keys = c->d_cand_keys + static_cast<size_t>(ch.q0) * cap;
+        const auto rescore = e->similarity == WAX_VS_COSINE ? filter_rescore_kernel<kCosine> : filter_rescore_kernel<kDot>;
+        rescore<<<dim3(32, ch.nq), 256, 0, stream>>>(e->d_corpus, ch.queries, e->dims, count,
+                                                     c->d_cand_rows + static_cast<size_t>(ch.q0) * cap, cap, keys);
         CUDA_TRY(cudaGetLastError());
         FilterSelectParams sp{};
-        sp.cand_count = bp.cand_count; sp.keys = c->d_cand_keys + static_cast<size_t>(q0) * cap; sp.cand_cap = cap; sp.k = k_eff;
-        sp.out = d_out + static_cast<size_t>(q0) * k_eff; sp.ok = d_ok + q0;
+        sp.cand_count = count; sp.keys = keys; sp.cand_cap = cap; sp.k = k_eff;
+        sp.out = d_out + static_cast<size_t>(ch.q0) * k_eff; sp.ok = d_ok + ch.q0;
         sp.frame_ids = d_ids; sp.id_base = e->id_base; sp.row_offset = row_offset;
-        filter_select_kernel<<<nq, 1024, static_cast<size_t>(cap) * sizeof(uint64_t), stream>>>(sp);
+        const size_t ssmem = static_cast<size_t>(cap) * sizeof(uint64_t);
+        CUDA_TRY(grant_smem(e, filter_select_kernel, ssmem));
+        filter_select_kernel<<<ch.nq, 1024, ssmem, stream>>>(sp);
         CUDA_TRY(cudaGetLastError());
-        *launches += 3;
+        *launches += 2;
+        return WAX_VS_OK;
+    };
+    return enqueue_nominate_pass(e, c, d_queries, n_queries, bf16, true, false, false, static_cast<uint32_t>(e->sm_count),
+                                 d_mask, stream, launches, [](uint32_t, uint32_t) { return 16u; }, prepare, finish);
+}
+
+// ---- search ---------------------------------------------------------------------------------------------------
+// The exact scan for n queries, one enqueue_search each on `stream`: query i (qs[i] when a list is given) reads
+// d_queries[i] and writes d_out[i].  sync_on_error: drain the stream before a failure is returned.
+static int32_t enqueue_scans(wax_vs_engine *e, SearchCtx *c, const float *d_queries, uint32_t n, const uint32_t *qs,
+                             uint32_t k_eff, uint64_t row_offset, wax_vs_candidate *d_out, const uint64_t *d_ids,
+                             cudaStream_t stream, uint64_t *launches, const uint32_t *d_mask, bool sync_on_error) {
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t qi = qs ? qs[i] : i;
+        const int32_t rc = enqueue_search(e, c, d_queries + static_cast<size_t>(qi) * e->dims, k_eff, row_offset,
+                                          d_out + static_cast<size_t>(qi) * k_eff, d_ids, stream, launches, d_mask);
+        if (rc) {
+            if (sync_on_error) cudaStreamSynchronize(stream);
+            return rc;
+        }
     }
     return WAX_VS_OK;
 }
 
-// ---- search ---------------------------------------------------------------------------------------------------
 // n_queries device-resident queries -> d_out[n_queries][k_eff] on c->stream: the tensor-core levels (bf16 shadow ->
 // TF32 retry -> exact scan, DESIGN 4.5.1) when the batch is eligible, else one fused scan per query.  The tensor
 // levels read their proof flags back, so they synchronise c->stream; the scan loop only enqueues.
@@ -1692,124 +1681,107 @@ static int32_t run_queries_on_device(wax_vs_engine *e, SearchCtx *c, const float
     }
     // below batch_min the tensor path only pays off through the bf16 shadow (single_shadow): never TF32 for one query
     if (tensor_path && !allow_bf16 && n_queries < static_cast<uint32_t>(std::max(e->tune.batch_min, 1))) tensor_path = false;
-    if (tensor_path) {
-        // Batched: one tensor-core pass over the corpus nominates, the finish kernel re-scores exactly and
-        // proves completeness; unproven queries (rare) are re-run on the exact single-query path below.
-        if ((rc = ensure_dev(&c->d_ok, &c->ok_cap, static_cast<size_t>(n_queries), "proof flags"))) return rc;
-        if ((rc = ensure_pinned(&c->h_ok, &c->h_ok_cap, static_cast<size_t>(n_queries), "proof flag staging"))) return rc;
-        if ((rc = ensure_dev(&c->d_tau_star, &c->tau_star_cap, static_cast<size_t>(n_queries) * 2, "filter thresholds"))) return rc;
-        if ((rc = ensure_pinned(&c->h_tau_star, &c->h_tau_star_cap, static_cast<size_t>(n_queries) * 2, "filter threshold staging"))) return rc;
-        bool used_bf16 = false;
-        uint32_t used_heap = 0;
-        rc = enqueue_batch_tensor(e, c, d_queries, n_queries, k_eff, row_offset, d_out, c->d_ok, d_ids, c->stream, launches,
-                                  allow_bf16, &used_bf16, c->d_tau_star, d_mask, &used_heap);
-        if (rc) { cudaStreamSynchronize(c->stream); return rc; }
-        CUDA_TRY(cudaMemcpyAsync(c->h_ok, c->d_ok, n_queries * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
-        CUDA_TRY(cudaMemcpyAsync(c->h_tau_star, c->d_tau_star, 2 * n_queries * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    if (!tensor_path)
+        return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_out, d_ids, c->stream, launches, d_mask, true);
+    // Batched: one tensor-core pass over the corpus nominates, the finish kernel re-scores exactly and
+    // proves completeness; unproven queries (rare) are re-run on the exact single-query path below.
+    if ((rc = c->d_ok.ensure(static_cast<size_t>(n_queries), "proof flags"))) return rc;
+    if ((rc = c->h_ok.ensure(static_cast<size_t>(n_queries), "proof flag staging"))) return rc;
+    if ((rc = c->d_tau_star.ensure(static_cast<size_t>(n_queries) * 2, "filter thresholds"))) return rc;
+    if ((rc = c->h_tau_star.ensure(static_cast<size_t>(n_queries) * 2, "filter threshold staging"))) return rc;
+    bool used_bf16 = false;
+    uint32_t used_heap = 0;
+    rc = enqueue_batch_tensor(e, c, d_queries, n_queries, k_eff, row_offset, d_out, c->d_ok, d_ids, c->stream, launches,
+                              allow_bf16, &used_bf16, c->d_tau_star, d_mask, &used_heap);
+    if (rc) { cudaStreamSynchronize(c->stream); return rc; }
+    CUDA_TRY(cudaMemcpyAsync(c->h_ok, c->d_ok, n_queries * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(c->h_tau_star, c->d_tau_star, 2 * n_queries * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    std::vector<uint32_t> unproven;
+    for (uint32_t qi = 0; qi < n_queries; ++qi) if (!c->h_ok[qi]) unproven.push_back(qi);
+    if (used_bf16 && k_eff <= 128u) record_level1_outcome(e, n_queries, unproven.size(), used_heap);
+    uint64_t retried = 0, retried_bf16 = 0;
+    // Level 2, the filter levels: the unproven queries that have a finite threshold, as one compacted sub-batch, get
+    // ONE more tensor-core pass that keeps no heap -- it lists every row above the query's fixed threshold (complete
+    // by construction).  First over the bf16 shadow when level 1 used it (half the bytes of an exact scan, so it pays
+    // even for a single query; its wider bound admits more candidates), then -- for the lists that overflowed, and
+    // only for sub-batches worth a tensor pass -- in TF32 over the fp32 corpus.  What is left takes the exact scan.
+    auto filter_pass = [&](std::vector<uint32_t> &todo, bool bf16lvl) -> int32_t {
+        const uint32_t nf = static_cast<uint32_t>(todo.size());
+        int32_t frc;
+        if ((frc = c->d_retry_q.ensure(static_cast<size_t>(nf) * e->dims, "filter-level queries"))) return frc;
+        if ((frc = c->d_retry_out.ensure(static_cast<size_t>(nf) * k_eff, "filter-level results"))) return frc;
+        if ((frc = c->d_retry_ok.ensure(static_cast<size_t>(nf), "filter-level flags"))) return frc;
+        if ((frc = c->d_filter_tau.ensure(static_cast<size_t>(nf), "filter-level thresholds"))) return frc;
+        if ((frc = c->h_filter_tau.ensure(static_cast<size_t>(nf), "filter-level threshold staging"))) return frc;
+        const float *taus = c->h_tau_star + (bf16lvl ? n_queries : 0u);      // [0]: TF32 bound, [1]: bf16 bound
+        for (uint32_t i = 0; i < nf; ++i) c->h_filter_tau[i] = taus[todo[i]];
+        CUDA_TRY(cudaMemcpyAsync(c->d_filter_tau, c->h_filter_tau, nf * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+        for (uint32_t i = 0; i < nf; ++i)
+            CUDA_TRY(cudaMemcpyAsync(c->d_retry_q + static_cast<size_t>(i) * e->dims,
+                                     d_queries + static_cast<size_t>(todo[i]) * e->dims, e->dims * sizeof(float),
+                                     cudaMemcpyDeviceToDevice, c->stream));
+        frc = enqueue_filter_level(e, c, c->d_retry_q, c->d_filter_tau, nf, k_eff, row_offset, c->d_retry_out,
+                                   c->d_retry_ok, d_ids, c->stream, launches, bf16lvl, d_mask);
+        if (frc) { cudaStreamSynchronize(c->stream); return frc; }
+        CUDA_TRY(cudaMemcpyAsync(c->h_ok, c->d_retry_ok, nf * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(cudaStreamSynchronize(c->stream));
-        std::vector<uint32_t> unproven;
-        for (uint32_t qi = 0; qi < n_queries; ++qi) if (!c->h_ok[qi]) unproven.push_back(qi);
-        if (used_bf16 && k_eff <= 128u && unproven.size() * 4 > n_queries) {   // (large k is expected to need the filter level)
-            std::lock_guard<std::mutex> pg(e->pool_mu);
-            e->bf16_skip_batches = 16;
-        }
-        if (used_bf16 && k_eff <= 128u && used_heap != 0u && e->tune.batch_heap == 0) {
-            // the data has the last word on the heap size: unproven queries -> one size up for `ttl` batches; when the
-            // time-out ends one size down is probed again, and a failure during the probe doubles the time-out
-            std::lock_guard<std::mutex> pg(e->pool_mu);
-            e->last_heap = used_heap;
-            if (!unproven.empty()) {
-                if (used_heap < 64u) {
-                    if (e->heap_probing) e->heap_backoff = std::min<uint32_t>(e->heap_backoff * 2u, 1u << 16);
-                    e->heap_bump = std::min<uint32_t>(e->heap_bump + 1u, 3u);
-                    e->heap_bump_ttl = e->heap_backoff;
-                }
-                e->heap_probing = false;
-            } else {
-                e->heap_probing = false;
-                if (e->heap_bump > 0 && e->heap_bump_ttl > 0 && --e->heap_bump_ttl == 0) {
-                    --e->heap_bump;
-                    e->heap_probing = true;
-                    e->heap_bump_ttl = e->heap_bump ? e->heap_backoff : 0;
-                }
-            }
-        }
-        uint64_t retried = 0, retried_bf16 = 0;
-        // Level 2, the filter levels: the unproven queries that have a finite threshold, as one compacted sub-batch, get
-        // ONE more tensor-core pass that keeps no heap -- it lists every row above the query's fixed threshold (complete
-        // by construction).  First over the bf16 shadow when level 1 used it (half the bytes of an exact scan, so it pays
-        // even for a single query; its wider bound admits more candidates), then -- for the lists that overflowed, and
-        // only for sub-batches worth a tensor pass -- in TF32 over the fp32 corpus.  What is left takes the exact scan.
-        auto filter_pass = [&](std::vector<uint32_t> &todo, bool bf16lvl) -> int32_t {
-            const uint32_t nf = static_cast<uint32_t>(todo.size());
-            int32_t frc;
-            if ((frc = ensure_dev(&c->d_retry_q, &c->retry_q_cap, static_cast<size_t>(nf) * e->dims, "filter-level queries"))) return frc;
-            if ((frc = ensure_dev(&c->d_retry_out, &c->retry_out_cap, static_cast<size_t>(nf) * k_eff, "filter-level results"))) return frc;
-            if ((frc = ensure_dev(&c->d_retry_ok, &c->retry_ok_cap, static_cast<size_t>(nf), "filter-level flags"))) return frc;
-            if ((frc = ensure_dev(&c->d_filter_tau, &c->filter_tau_cap, static_cast<size_t>(nf), "filter-level thresholds"))) return frc;
-            if ((frc = ensure_pinned(&c->h_filter_tau, &c->h_filter_tau_cap, static_cast<size_t>(nf), "filter-level threshold staging"))) return frc;
-            const float *taus = c->h_tau_star + (bf16lvl ? n_queries : 0u);      // [0]: TF32 bound, [1]: bf16 bound
-            for (uint32_t i = 0; i < nf; ++i) c->h_filter_tau[i] = taus[todo[i]];
-            CUDA_TRY(cudaMemcpyAsync(c->d_filter_tau, c->h_filter_tau, nf * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-            for (uint32_t i = 0; i < nf; ++i)
-                CUDA_TRY(cudaMemcpyAsync(c->d_retry_q + static_cast<size_t>(i) * e->dims,
-                                         d_queries + static_cast<size_t>(todo[i]) * e->dims, e->dims * sizeof(float),
+        std::vector<uint32_t> overflowed;
+        for (uint32_t i = 0; i < nf; ++i) {
+            if (c->h_ok[i])
+                CUDA_TRY(cudaMemcpyAsync(d_out + static_cast<size_t>(todo[i]) * k_eff,
+                                         c->d_retry_out + static_cast<size_t>(i) * k_eff, k_eff * sizeof(wax_vs_candidate),
                                          cudaMemcpyDeviceToDevice, c->stream));
-            frc = enqueue_filter_level(e, c, c->d_retry_q, c->d_filter_tau, nf, k_eff, row_offset, c->d_retry_out,
-                                       c->d_retry_ok, d_ids, c->stream, launches, bf16lvl, d_mask);
-            if (frc) { cudaStreamSynchronize(c->stream); return frc; }
-            CUDA_TRY(cudaMemcpyAsync(c->h_ok, c->d_retry_ok, nf * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
-            CUDA_TRY(cudaStreamSynchronize(c->stream));
-            std::vector<uint32_t> overflowed;
-            for (uint32_t i = 0; i < nf; ++i) {
-                if (c->h_ok[i])
-                    CUDA_TRY(cudaMemcpyAsync(d_out + static_cast<size_t>(todo[i]) * k_eff,
-                                             c->d_retry_out + static_cast<size_t>(i) * k_eff, k_eff * sizeof(wax_vs_candidate),
-                                             cudaMemcpyDeviceToDevice, c->stream));
-                else
-                    overflowed.push_back(todo[i]);
-            }
-            todo.swap(overflowed);
-            return WAX_VS_OK;
-        };
-        if (e->tune.batch_retry && !unproven.empty()) {
-            std::vector<uint32_t> todo, rest;
-            for (uint32_t qi : unproven)
-                ((std::isfinite(c->h_tau_star[qi]) && std::isfinite(c->h_tau_star[n_queries + qi])) ? todo : rest).push_back(qi);
-            if (!todo.empty() && used_bf16 && e->tune.filter_bf16) {
-                retried_bf16 = todo.size();
-                if ((rc = filter_pass(todo, true))) return rc;
-            }
-            if (todo.size() >= static_cast<size_t>(std::max(e->tune.batch_min, 1))) {
-                retried = todo.size();
-                if ((rc = filter_pass(todo, false))) return rc;
-            }
-            rest.insert(rest.end(), todo.begin(), todo.end());
-            std::sort(rest.begin(), rest.end());
-            unproven.swap(rest);
+            else
+                overflowed.push_back(todo[i]);
         }
-        for (uint32_t qi : unproven) {
-            rc = enqueue_search(e, c, d_queries + static_cast<size_t>(qi) * e->dims, k_eff, row_offset,
-                                d_out + static_cast<size_t>(qi) * k_eff, d_ids, c->stream, launches, d_mask);
-            if (rc) { cudaStreamSynchronize(c->stream); return rc; }
+        todo.swap(overflowed);
+        return WAX_VS_OK;
+    };
+    if (e->tune.batch_retry && !unproven.empty()) {
+        std::vector<uint32_t> todo, rest;
+        for (uint32_t qi : unproven)
+            ((std::isfinite(c->h_tau_star[qi]) && std::isfinite(c->h_tau_star[n_queries + qi])) ? todo : rest).push_back(qi);
+        if (!todo.empty() && used_bf16 && e->tune.filter_bf16) {
+            retried_bf16 = todo.size();
+            if ((rc = filter_pass(todo, true))) return rc;
         }
-        {
-            std::lock_guard<std::mutex> pg(e->pool_mu);
-            e->batch_tensor_queries += n_queries - unproven.size();
-            e->batch_fallback_queries += unproven.size();
-            if (used_bf16) e->batch_bf16_queries += n_queries;
-            else e->batch_tf32_queries += n_queries;
-            e->batch_retry_queries += retried;
-            e->batch_filter_bf16_queries += retried_bf16;
+        if (todo.size() >= static_cast<size_t>(std::max(e->tune.batch_min, 1))) {
+            retried = todo.size();
+            if ((rc = filter_pass(todo, false))) return rc;
         }
-    } else {
-        for (uint32_t qi = 0; qi < n_queries; ++qi) {
-            rc = enqueue_search(e, c, d_queries + static_cast<size_t>(qi) * e->dims, k_eff, row_offset,
-                                d_out + static_cast<size_t>(qi) * k_eff, d_ids, c->stream, launches, d_mask);
-            if (rc) { cudaStreamSynchronize(c->stream); return rc; }
-        }
+        rest.insert(rest.end(), todo.begin(), todo.end());
+        std::sort(rest.begin(), rest.end());
+        unproven.swap(rest);
     }
+    if ((rc = enqueue_scans(e, c, d_queries, static_cast<uint32_t>(unproven.size()), unproven.data(), k_eff, row_offset,
+                            d_out, d_ids, c->stream, launches, d_mask, true)))
+        return rc;
+    std::lock_guard<std::mutex> pg(e->pool_mu);
+    e->batch_tensor_queries += n_queries - unproven.size();
+    e->batch_fallback_queries += unproven.size();
+    if (used_bf16) e->batch_bf16_queries += n_queries;
+    else e->batch_tf32_queries += n_queries;
+    e->batch_retry_queries += retried;
+    e->batch_filter_bf16_queries += retried_bf16;
     return WAX_VS_OK;
+}
+
+// n_queries x k_eff candidates -> frame ids and scores, query qi's at qi * out_stride; out_n[qi] = how many were valid.
+// row -> frameId and distance -> score on the host, as MetalVectorEngine.swift:595-603 does.
+static void deliver_results(const wax_vs_engine *e, const wax_vs_candidate *cands, uint32_t n_queries, uint32_t k_eff,
+                            uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    for (uint32_t qi = 0; qi < n_queries; ++qi) {
+        uint32_t m = 0;
+        for (uint32_t i = 0; i < k_eff; ++i) {
+            const wax_vs_candidate &cd = cands[static_cast<size_t>(qi) * k_eff + i];
+            if (!cd.valid) continue;
+            out_ids[static_cast<size_t>(qi) * out_stride + m] = e->ids_identity ? e->id_base + cd.row : e->ids[cd.row];
+            out_scores[static_cast<size_t>(qi) * out_stride + m] = score_from_distance(e->similarity, cd.distance);
+            ++m;
+        }
+        out_n[qi] = m;
+    }
 }
 
 static int32_t search_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
@@ -1833,74 +1805,43 @@ static int32_t search_host(wax_vs_engine *e, const float *queries, uint32_t n_qu
 
     DeviceGuard g(e->device);
     if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    SearchCtx *c = nullptr;
-    int32_t rc = ctx_acquire(e, &c);
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
     if (rc) return rc;
-    struct Rel { wax_vs_engine *e; SearchCtx *c; ~Rel() { ctx_release(e, c); } } rel{e, c};
+    SearchCtx *c = lease.c;
 
-    const size_t qfloats = static_cast<size_t>(n_queries) * e->dims;
     const size_t ncand = static_cast<size_t>(n_queries) * k_eff;
+    if ((rc = c->d_out.ensure(ncand, "result buffer"))) return rc;
+    if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
+    uint64_t launches = 0;
+    bool delivered = false;
     // One query on the fused scan: the query rides in the kernel parameters and the kernel itself stores the result in
     // mapped host memory and raises a flag -- no H2D copy, no D2H copy, no stream synchronisation on the way.
     if (n_queries == 1 && e->tune.host_delivery && k_eff <= static_cast<uint32_t>(e->tune.fused_k_max) &&
         !batch_tensor_eligible(e, 1, k_eff)) {
-        if ((rc = ensure_dev(&c->d_out, &c->d_out_cap, ncand, "result buffer"))) return rc;
-        if ((rc = ensure_pinned(&c->h_out, &c->h_out_cap, ncand, "result staging"))) return rc;
         if (!c->h_flag) {
-            CUDA_TRY(cudaHostAlloc(reinterpret_cast<void **>(&c->h_flag), sizeof(unsigned long long), cudaHostAllocMapped | cudaHostAllocPortable));
+            if ((rc = c->h_flag.ensure(1, "completion flag"))) return rc;
             *c->h_flag = 0; c->host_seq = 0;
         }
         HostDelivery hd{queries, c->h_out, c->h_flag, ++c->host_seq};
-        uint64_t launches = 0;
         if ((rc = enqueue_search(e, c, nullptr, k_eff, 0, c->d_out, nullptr, c->stream, &launches, nullptr, nullptr, &hd))) {
             cudaStreamSynchronize(c->stream);
             return rc;
         }
-        if (hd.delivered) {
-            if ((rc = wait_host_flag(c->stream, c->h_flag, hd.seq, 30ull * 1000 * 1000 * 1000)) != WAX_VS_OK) {
-                cudaStreamSynchronize(c->stream);
-                return rc > 0 ? fail(WAX_VS_ERR_CUDA, "search reported a device-side error") : rc;
-            }
-        } else {
-            CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, ncand * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, c->stream));
-            CUDA_TRY(cudaStreamSynchronize(c->stream));
+        delivered = hd.delivered;
+        if (delivered && (rc = wait_host_flag(c->stream, c->h_flag, hd.seq, 30ull * 1000 * 1000 * 1000)) != WAX_VS_OK) {
+            cudaStreamSynchronize(c->stream);
+            return rc > 0 ? fail(WAX_VS_ERR_CUDA, "search reported a device-side error") : rc;
         }
-        uint32_t m = 0;
-        for (uint32_t i = 0; i < k_eff; ++i) {
-            const wax_vs_candidate &cd = c->h_out[i];
-            if (!cd.valid) continue;
-            out_ids[m] = e->ids_identity ? e->id_base + cd.row : e->ids[cd.row];
-            out_scores[m] = score_from_distance(e->similarity, cd.distance);
-            ++m;
-        }
-        out_n[0] = m;
-        return WAX_VS_OK;
+    } else {
+        if ((rc = stage_queries(e, c, queries, n_queries, c->stream))) return rc;
+        if ((rc = run_queries_on_device(e, c, c->d_queries, n_queries, k_eff, 0, c->d_out, nullptr, &launches))) return rc;
     }
-    if ((rc = ensure_dev(&c->d_queries, &c->d_queries_cap, qfloats, "query buffer"))) return rc;
-    if ((rc = ensure_pinned(&c->h_queries, &c->h_queries_cap, qfloats, "query staging"))) return rc;
-    if ((rc = ensure_dev(&c->d_out, &c->d_out_cap, ncand, "result buffer"))) return rc;
-    if ((rc = ensure_pinned(&c->h_out, &c->h_out_cap, ncand, "result staging"))) return rc;
-
-    memcpy(c->h_queries, queries, qfloats * sizeof(float));
-    CUDA_TRY(cudaMemcpyAsync(c->d_queries, c->h_queries, qfloats * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    uint64_t launches = 0;
-    if ((rc = run_queries_on_device(e, c, c->d_queries, n_queries, k_eff, 0, c->d_out, nullptr, &launches))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, ncand * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(cudaStreamSynchronize(c->stream));
-
-    // row -> frameId and distance -> score on the host, as MetalVectorEngine.swift:595-603 does.
-    for (uint32_t qi = 0; qi < n_queries; ++qi) {
-        uint32_t m = 0;
-        for (uint32_t i = 0; i < k_eff; ++i) {
-            const wax_vs_candidate &cd = c->h_out[static_cast<size_t>(qi) * k_eff + i];
-            if (!cd.valid) continue;
-            const uint64_t row = cd.row;
-            out_ids[static_cast<size_t>(qi) * out_stride + m] = e->ids_identity ? e->id_base + row : e->ids[row];
-            out_scores[static_cast<size_t>(qi) * out_stride + m] = score_from_distance(e->similarity, cd.distance);
-            ++m;
-        }
-        out_n[qi] = m;
+    if (!delivered) {
+        CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, ncand * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(cudaStreamSynchronize(c->stream));
     }
+    deliver_results(e, c->h_out, n_queries, k_eff, out_ids, out_scores, out_stride, out_n);
     return WAX_VS_OK;
 }
 
@@ -1929,13 +1870,8 @@ int32_t wax_vs_search_device(wax_vs_engine *e, const float *d_queries, uint32_t 
     const uint64_t *d_ids = nullptr;
     if ((rc = sync_device_ids(e, &d_ids))) return rc;
     uint64_t launches = 0;
-    for (uint32_t qi = 0; qi < n_queries; ++qi) {
-        rc = enqueue_search(e, c, d_queries + static_cast<size_t>(qi) * e->dims, k_eff, row_offset,
-                            d_candidates + static_cast<size_t>(qi) * k_eff, d_ids,
-                            static_cast<cudaStream_t>(cuda_stream), &launches);
-        if (rc) return rc;
-    }
-    return WAX_VS_OK;
+    return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_candidates, d_ids,
+                         static_cast<cudaStream_t>(cuda_stream), &launches, nullptr, false);
 }
 
 // Batched form of wax_vs_search_device: the tensor-core levels on the caller's stream for the rank's shard.  Unlike
@@ -1956,14 +1892,9 @@ int32_t wax_vs_search_batch_device(wax_vs_engine *e, const float *d_queries, uin
     const uint64_t *d_ids = nullptr;
     if ((rc = sync_device_ids(e, &d_ids))) return rc;
     uint64_t launches = 0;
-    if (k_eff > e->n_rows) {   // a shard smaller than k: the scan pads with invalid candidates, the tensor path does not
-        for (uint32_t qi = 0; qi < n_queries; ++qi) {
-            rc = enqueue_search(e, c, d_queries + static_cast<size_t>(qi) * e->dims, k_eff, row_offset,
-                                d_candidates + static_cast<size_t>(qi) * k_eff, d_ids, c->stream, &launches);
-            if (rc) return rc;
-        }
-        return WAX_VS_OK;
-    }
+    if (k_eff > e->n_rows)     // a shard smaller than k: the scan pads with invalid candidates, the tensor path does not
+        return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_candidates, d_ids, c->stream,
+                             &launches, nullptr, false);
     return run_queries_on_device(e, c, d_queries, n_queries, k_eff, row_offset, d_candidates, d_ids, &launches);
 }
 
@@ -2002,10 +1933,8 @@ static void shard_teardown(wax_vs_engine *e, bool free_own) {
     if (!free_own) return;
     if (sh.box[sh.rank]) cudaFree(sh.box[sh.rank]);
     sh.box[sh.rank] = nullptr;
-    if (sh.ctx) { ctx_free(sh.ctx); sh.ctx = nullptr; }
-    if (sh.d_final) { cudaFree(sh.d_final); sh.d_final = nullptr; }
-    if (sh.h_final) { cudaFreeHost(sh.h_final); sh.h_final = nullptr; }
-    if (sh.h_flag) { cudaFreeHost(sh.h_flag); sh.h_flag = nullptr; }
+    delete sh.ctx;             // the result buffers stay with the engine: a re-open reuses them
+    sh.ctx = nullptr;
     cudaGetLastError();
     sh.open = false;
     sh.seq = 0;
@@ -2023,23 +1952,20 @@ int32_t wax_vs_shard_open(wax_vs_engine *e, int32_t rank, int32_t world, uint64_
     auto &sh = e->shard;
     ShardMailbox *box = nullptr;
     CUDA_TRY(cudaMalloc(&box, sizeof(ShardMailbox)));
+    int32_t rc = sh.d_final.ensure(kShardKCap, "shard result");
+    if (!rc) rc = sh.h_final.ensure(kShardKCap, "shard result delivery");
+    if (!rc) rc = sh.h_flag.ensure(1, "shard completion flag");
+    if (rc) { cudaFree(box); return rc; }
     cudaError_t err = cudaMemset(box, 0, sizeof(ShardMailbox));
-    if (err == cudaSuccess) err = cudaMalloc(&sh.d_final, kShardKCap * sizeof(wax_vs_candidate));
-    if (err == cudaSuccess) err = cudaHostAlloc(&sh.h_final, kShardKCap * sizeof(wax_vs_candidate), cudaHostAllocMapped | cudaHostAllocPortable);
-    if (err == cudaSuccess) err = cudaHostAlloc(&sh.h_flag, sizeof(unsigned long long), cudaHostAllocMapped | cudaHostAllocPortable);
     if (err == cudaSuccess) err = cudaDeviceSynchronize();
     ShardHandle h{};
     if (err == cudaSuccess) err = cudaIpcGetMemHandle(&h.ipc, box);
     if (err != cudaSuccess) {
         cudaFree(box);
-        if (sh.d_final) { cudaFree(sh.d_final); sh.d_final = nullptr; }
-        if (sh.h_final) { cudaFreeHost(sh.h_final); sh.h_final = nullptr; }
-        if (sh.h_flag) { cudaFreeHost(sh.h_flag); sh.h_flag = nullptr; }
         return fail(WAX_VS_ERR_CUDA, "failed to create the shard mailbox: %s", cudaGetErrorString(err));
     }
     *sh.h_flag = 0;
-    int32_t rc = ctx_new(e, &sh.ctx, true);
-    if (rc) { cudaFree(box); return rc; }
+    if ((rc = ctx_new(e, &sh.ctx, true))) { cudaFree(box); return rc; }
     sh.rank = rank; sh.world = world; sh.row_offset = row_offset;
     sh.box[rank] = box;
     sh.open = true; sh.connected = (world == 1);
@@ -2142,6 +2068,46 @@ static int32_t shard_wait_host(wax_vs_engine *e, unsigned long long seq) {
     return rc;
 }
 
+// The host-path collective search of both entry points (caller: read lock, device selected, arguments checked): the
+// rank's fused scan, with the row bitset `*bits` below the top-k when the filtered form passes a non-empty one, the
+// in-kernel exchange and merge, and the merged list delivered into mapped host memory.
+static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t k_eff, const std::vector<uint32_t> *bits,
+                                 uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n) {
+    auto &sh = e->shard;
+    std::lock_guard<std::mutex> sg(sh.mu);      // one host-path collective at a time: it owns sh.ctx and h_final
+    SearchCtx *c = sh.ctx;
+    int32_t rc;
+    const uint64_t *d_ids = nullptr;
+    if ((rc = sync_device_ids(e, &d_ids))) return rc;
+    const bool masked = bits && !bits->empty();
+    if (masked) {
+        if ((rc = c->d_mask.ensure(bits->size(), "row filter"))) return rc;
+        CUDA_TRY(cudaMemcpyAsync(c->d_mask, bits->data(), bits->size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    }
+    ShardParams sp = shard_params_next(e);
+    sp.host_out = sh.h_final; sp.host_flag = sh.h_flag;      // mapped pinned: the kernel delivers the result itself
+    HostDelivery hd{query, nullptr, nullptr, 0};             // the query rides in the kernel parameters when it fits
+    uint64_t launches = 0;
+    if ((rc = enqueue_search(e, c, nullptr, k_eff, sh.row_offset, sh.d_final, d_ids, c->stream, &launches,
+                             masked ? c->d_mask.p : nullptr, &sp, &hd))) {
+        cudaStreamSynchronize(c->stream);
+        return rc;
+    }
+    if ((rc = shard_wait_host(e, sp.seq))) { cudaStreamSynchronize(c->stream); return rc; }
+    if (bits) CUDA_TRY(cudaStreamSynchronize(c->stream));   // `bits` must outlive its upload
+    uint32_t m = 0;
+    for (uint32_t i = 0; i < k_eff; ++i) {
+        const wax_vs_candidate &cd = sh.h_final[i];
+        if (cd.valid != 1u) continue;
+        if (m >= out_cap) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need more", out_cap);
+        out_ids[m] = cd.frame_id;
+        out_scores[m] = score_from_distance(e->similarity, cd.distance);
+        ++m;
+    }
+    *out_n = m;
+    return WAX_VS_OK;
+}
+
 int32_t wax_vs_shard_search(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k, uint64_t *out_ids,
                             float *out_scores, uint32_t out_cap, uint32_t *out_n) {
     if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
@@ -2157,32 +2123,7 @@ int32_t wax_vs_shard_search(wax_vs_engine *e, const float *query, uint32_t query
     if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
     DeviceGuard g(e->device);
     if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    auto &sh = e->shard;
-    std::lock_guard<std::mutex> sg(sh.mu);      // one host-path collective at a time: it owns sh.ctx and h_final
-    SearchCtx *c = sh.ctx;
-    int32_t rc;
-    const uint64_t *d_ids = nullptr;
-    if ((rc = sync_device_ids(e, &d_ids))) return rc;
-    ShardParams sp = shard_params_next(e);
-    sp.host_out = sh.h_final; sp.host_flag = sh.h_flag;      // mapped pinned: the kernel delivers the result itself
-    HostDelivery hd{query, nullptr, nullptr, 0};             // the query rides in the kernel parameters when it fits
-    uint64_t launches = 0;
-    if ((rc = enqueue_search(e, c, nullptr, k_eff, sh.row_offset, sh.d_final, d_ids, c->stream, &launches, nullptr, &sp, &hd))) {
-        cudaStreamSynchronize(c->stream);
-        return rc;
-    }
-    if ((rc = shard_wait_host(e, sp.seq))) { cudaStreamSynchronize(c->stream); return rc; }
-    uint32_t m = 0;
-    for (uint32_t i = 0; i < k_eff; ++i) {
-        const wax_vs_candidate &cd = sh.h_final[i];
-        if (cd.valid != 1u) continue;
-        if (m >= out_cap) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need more", out_cap);
-        out_ids[m] = cd.frame_id;
-        out_scores[m] = score_from_distance(e->similarity, cd.distance);
-        ++m;
-    }
-    *out_n = m;
-    return WAX_VS_OK;
+    return shard_search_host(e, query, k_eff, nullptr, out_ids, out_scores, out_cap, out_n);
 }
 
 // Device-timed sharded searches, strictly one query at a time on one stream (the same mode as wax_vs_debug_time_search):
@@ -2200,7 +2141,7 @@ int32_t wax_vs_debug_time_shard_search(wax_vs_engine *e, uint32_t n_queries, int
     SearchCtx *c = sh.ctx;
     const uint32_t k_eff = clamp_topk(top_k);
     int32_t rc;
-    if ((rc = ensure_dev(&c->d_queries, &c->d_queries_cap, static_cast<size_t>(n_queries) * e->dims, "query buffer"))) return rc;
+    if ((rc = c->d_queries.ensure(static_cast<size_t>(n_queries) * e->dims, "query buffer"))) return rc;
     synth_fill_kernel<<<(n_queries + 255) / 256, 256, 0, c->stream>>>(c->d_queries, n_queries, e->dims, seed, 0, 1);
     CUDA_TRY(cudaGetLastError());
     const uint64_t *d_ids = nullptr;
@@ -2293,36 +2234,26 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
 
     DeviceGuard g(e->device);
     if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    SearchCtx *c = nullptr;
-    int32_t rc = ctx_acquire(e, &c);
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
     if (rc) return rc;
-    struct Rel { wax_vs_engine *e; SearchCtx *c; ~Rel() { ctx_release(e, c); } } rel{e, c};
-    const size_t qfloats = static_cast<size_t>(n_queries) * e->dims;
+    SearchCtx *c = lease.c;
     const size_t ncand = static_cast<size_t>(n_queries) * k_eff;
-    if ((rc = ensure_dev(&c->d_queries, &c->d_queries_cap, qfloats, "query buffer"))) return rc;
-    if ((rc = ensure_pinned(&c->h_queries, &c->h_queries_cap, qfloats, "query staging"))) return rc;
-    if ((rc = ensure_dev(&c->d_out, &c->d_out_cap, ncand, "result buffer"))) return rc;
-    if ((rc = ensure_pinned(&c->h_out, &c->h_out_cap, ncand, "result staging"))) return rc;
-    memcpy(c->h_queries, queries, qfloats * sizeof(float));
-    CUDA_TRY(cudaMemcpyAsync(c->d_queries, c->h_queries, qfloats * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    if ((rc = stage_queries(e, c, queries, n_queries, c->stream))) return rc;
+    if ((rc = c->d_out.ensure(ncand, "result buffer"))) return rc;
+    if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
 
     uint64_t launches = 0;
     if (mode == 0 && listed.size() <= 16384) {
         // small allow-list: gather + exact score of the listed rows only, then one-CTA sorts
         std::sort(listed.begin(), listed.end());
         const uint32_t n = static_cast<uint32_t>(listed.size());
-        if ((rc = ensure_dev(&c->d_mask, &c->mask_cap, static_cast<size_t>(std::max<uint32_t>(n, 1)), "listed rows"))) return rc;
-        if ((rc = ensure_dev(&c->d_gather_keys, &c->gather_cap, static_cast<size_t>(std::max<uint32_t>(n, 1)) * n_queries, "gather keys"))) return rc;
+        if ((rc = c->d_mask.ensure(static_cast<size_t>(std::max<uint32_t>(n, 1)), "listed rows"))) return rc;
+        if ((rc = c->d_gather_keys.ensure(static_cast<size_t>(std::max<uint32_t>(n, 1)) * n_queries, "gather keys"))) return rc;
         CUDA_TRY(cudaMemcpyAsync(c->d_mask, listed.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
         uint32_t pow2 = 64;
         while (pow2 < n) pow2 <<= 1;
-        {
-            std::lock_guard<std::mutex> ag(e->attr_mu);
-            if (!e->gather_attr_set) {
-                CUDA_TRY(cudaFuncSetAttribute(gather_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8));
-                e->gather_attr_set = true;
-            }
-        }
+        CUDA_TRY(grant_smem(e, gather_sort_kernel, pow2 * sizeof(uint64_t)));
         const uint32_t gx = std::max<uint32_t>(1, std::min<uint32_t>((n + 31) / 32, static_cast<uint32_t>(e->sm_count) * 8));
         for (uint32_t q0 = 0; q0 < n_queries; q0 += 32768u) {       // grid.y limit
             const uint32_t nq = std::min<uint32_t>(n_queries - q0, 32768u);
@@ -2342,7 +2273,7 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
             launches += 2;
         }
     } else {
-        if ((rc = ensure_dev(&c->d_mask, &c->mask_cap, bits.size(), "row filter"))) return rc;
+        if ((rc = c->d_mask.ensure(bits.size(), "row filter"))) return rc;
         CUDA_TRY(cudaMemcpyAsync(c->d_mask, bits.data(), bits.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
         if (n_queries == 1) {
             rc = enqueue_search(e, c, c->d_queries, k_eff, 0, c->d_out, nullptr, c->stream, &launches, c->d_mask);
@@ -2353,17 +2284,7 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
     }
     CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, ncand * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));   // also keeps `bits` / `listed` alive until the copies are done
-    for (uint32_t qi = 0; qi < n_queries; ++qi) {
-        uint32_t m = 0;
-        for (uint32_t i = 0; i < k_eff; ++i) {
-            const wax_vs_candidate &cd = c->h_out[static_cast<size_t>(qi) * k_eff + i];
-            if (!cd.valid) continue;
-            out_ids[static_cast<size_t>(qi) * out_stride + m] = e->ids_identity ? e->id_base + cd.row : e->ids[cd.row];
-            out_scores[static_cast<size_t>(qi) * out_stride + m] = score_from_distance(e->similarity, cd.distance);
-            ++m;
-        }
-        out_n[qi] = m;
-    }
+    deliver_results(e, c->h_out, n_queries, k_eff, out_ids, out_scores, out_stride, out_n);
     return WAX_VS_OK;
 }
 
@@ -2403,38 +2324,7 @@ int32_t wax_vs_shard_search_filtered(wax_vs_engine *e, const float *query, uint3
     if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
     std::vector<uint32_t> bits, listed;
     if (e->n_rows) build_row_filter(e, frame_ids, n_ids, mode, bits, listed);
-    auto &sh = e->shard;
-    std::lock_guard<std::mutex> sg(sh.mu);      // one host-path collective at a time: it owns sh.ctx and h_final
-    SearchCtx *c = sh.ctx;
-    int32_t rc;
-    const uint64_t *d_ids = nullptr;
-    if ((rc = sync_device_ids(e, &d_ids))) return rc;
-    if (!bits.empty()) {
-        if ((rc = ensure_dev(&c->d_mask, &c->mask_cap, bits.size(), "row filter"))) return rc;
-        CUDA_TRY(cudaMemcpyAsync(c->d_mask, bits.data(), bits.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-    }
-    ShardParams sp = shard_params_next(e);
-    sp.host_out = sh.h_final; sp.host_flag = sh.h_flag;
-    HostDelivery hd{query, nullptr, nullptr, 0};
-    uint64_t launches = 0;
-    if ((rc = enqueue_search(e, c, nullptr, k_eff, sh.row_offset, sh.d_final, d_ids, c->stream, &launches,
-                             bits.empty() ? nullptr : c->d_mask, &sp, &hd))) {
-        cudaStreamSynchronize(c->stream);
-        return rc;
-    }
-    if ((rc = shard_wait_host(e, sp.seq))) { cudaStreamSynchronize(c->stream); return rc; }
-    CUDA_TRY(cudaStreamSynchronize(c->stream));   // `bits` must outlive its upload
-    uint32_t m = 0;
-    for (uint32_t i = 0; i < k_eff; ++i) {
-        const wax_vs_candidate &cd = sh.h_final[i];
-        if (cd.valid != 1u) continue;
-        if (m >= out_cap) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need more", out_cap);
-        out_ids[m] = cd.frame_id;
-        out_scores[m] = score_from_distance(e->similarity, cd.distance);
-        ++m;
-    }
-    *out_n = m;
-    return WAX_VS_OK;
+    return shard_search_host(e, query, k_eff, &bits, out_ids, out_scores, out_cap, out_n);
 }
 
 // ---- persistence ---------------------------------------------------------------------------------------------
@@ -2575,26 +2465,26 @@ int32_t wax_vs_debug_time_search(wax_vs_engine *e, uint32_t n_queries, int64_t t
     if (n_queries == 0) n_queries = 1;
     std::shared_lock<std::shared_mutex> r(e->rw);
     DeviceGuard g(e->device);
-    SearchCtx *c = nullptr;
-    int32_t rc = ctx_acquire(e, &c);
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
     if (rc) return rc;
-    struct Rel { wax_vs_engine *e; SearchCtx *c; ~Rel() { ctx_release(e, c); } } rel{e, c};
+    SearchCtx *c = lease.c;
     const uint32_t k_eff = clamp_topk(top_k);
     const size_t qfloats = static_cast<size_t>(n_queries) * e->dims;
-    if ((rc = ensure_dev(&c->d_queries, &c->d_queries_cap, qfloats, "query buffer"))) return rc;
-    if ((rc = ensure_dev(&c->d_out, &c->d_out_cap, static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
+    if ((rc = c->d_queries.ensure(qfloats, "query buffer"))) return rc;
+    if ((rc = c->d_out.ensure(static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
     // n_queries distinct unit queries (generator stream `seed`); step i searches query i mod n_queries.
     synth_fill_kernel<<<(n_queries + 255) / 256, 256, 0, c->stream>>>(c->d_queries, n_queries, e->dims, seed, 0, 1);
     CUDA_TRY(cudaGetLastError());
     uint64_t launches = 0;
     // time_overlap: consecutive (independent) queries alternate over two streams so that one scan's tail overlaps
     // the next one's prologue -- what the sharded engine does with search_many_async.
-    SearchCtx *c2 = nullptr;
+    CtxLease lease2(e);
     if (e->tune.time_overlap) {
-        if ((rc = ctx_acquire(e, &c2))) return rc;
-        if ((rc = ensure_dev(&c2->d_out, &c2->d_out_cap, static_cast<size_t>(n_queries) * k_eff, "result buffer"))) { ctx_release(e, c2); return rc; }
+        if ((rc = lease2.acquire())) return rc;
+        if ((rc = lease2.c->d_out.ensure(static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
     }
-    struct Rel2 { wax_vs_engine *e; SearchCtx *c; ~Rel2() { if (c) ctx_release(e, c); } } rel2{e, c2};
+    SearchCtx *c2 = lease2.c;
     for (uint32_t it = 0; it < warmup + iters; ++it) {
         if (it == warmup) {
             launches = 0;
@@ -2621,10 +2511,10 @@ int32_t wax_vs_debug_stream_read(wax_vs_engine *e, uint32_t iters, float *out_be
     if (!e || !out_best_ms || !out_bytes) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     DeviceGuard g(e->device);
-    SearchCtx *c = nullptr;
-    int32_t rc = ctx_acquire(e, &c);
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
     if (rc) return rc;
-    struct Rel { wax_vs_engine *e; SearchCtx *c; ~Rel() { ctx_release(e, c); } } rel{e, c};
+    SearchCtx *c = lease.c;
     const uint64_t bytes = e->n_rows * e->dims * sizeof(float) / 16 * 16;
     *out_bytes = bytes;
     *out_best_ms = 0.0f;
@@ -2659,7 +2549,7 @@ int32_t wax_vs_debug_transfer_probe(wax_vs_engine *e, uint64_t bytes, float *out
     int32_t rc = ingest_staging(e, bytes);
     if (rc) return rc;
     auto &ig = e->ing;
-    if ((rc = ensure_dev(&ig.d_stage, &ig.d_stage_cap, static_cast<size_t>((bytes + 3) / 4), "probe buffer"))) return rc;
+    if ((rc = ig.d_stage.ensure(static_cast<size_t>((bytes + 3) / 4), "probe buffer"))) return rc;
     std::vector<uint8_t> host(bytes, 1);
     auto secs = [](auto t0) { return std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count(); };
     uint8_t *probe_pin = nullptr;
@@ -2689,13 +2579,13 @@ int32_t wax_vs_debug_phase_trace(wax_vs_engine *e, int64_t top_k, uint32_t iters
     if (!e || !out5) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::unique_lock<std::shared_mutex> w(e->rw);
     DeviceGuard g(e->device);
-    SearchCtx *c = nullptr;
-    int32_t rc = ctx_acquire(e, &c);
+    CtxLease lease(e, true);     // also detaches the trace buffer
+    int32_t rc = lease.acquire();
     if (rc) return rc;
-    struct Rel { wax_vs_engine *e; SearchCtx *c; ~Rel() { ctx_release(e, c); e->debug_trace = nullptr; } } rel{e, c};
+    SearchCtx *c = lease.c;
     const uint32_t k_eff = clamp_topk(top_k);
-    if ((rc = ensure_dev(&c->d_queries, &c->d_queries_cap, static_cast<size_t>(e->dims), "query buffer"))) return rc;
-    if ((rc = ensure_dev(&c->d_out, &c->d_out_cap, static_cast<size_t>(k_eff), "result buffer"))) return rc;
+    if ((rc = c->d_queries.ensure(static_cast<size_t>(e->dims), "query buffer"))) return rc;
+    if ((rc = c->d_out.ensure(static_cast<size_t>(k_eff), "result buffer"))) return rc;
     synth_fill_kernel<<<1, 256, 0, c->stream>>>(c->d_queries, 1, e->dims, 99, 0, 1);
     unsigned long long *d_trace = nullptr;
     CUDA_TRY(cudaMalloc(&d_trace, 8 * sizeof(unsigned long long)));
@@ -2743,7 +2633,7 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "batch_retry_queries")) *out = e->batch_retry_queries;               // TF32 filter level
     else if (!strcmp(name, "batch_filter_bf16_queries")) *out = e->batch_filter_bf16_queries;   // bf16-shadow filter level
     else if (!strcmp(name, "shadow_bytes")) *out = e->shadow_valid ? e->shadow_rows * e->dims * sizeof(__nv_bfloat16) : 0;   // live rows
-    else if (!strcmp(name, "shadow_capacity_bytes")) *out = e->shadow_cap * sizeof(__nv_bfloat16);                            // HBM held
+    else if (!strcmp(name, "shadow_capacity_bytes")) *out = e->d_shadow.cap * sizeof(__nv_bfloat16);                          // HBM held
     else if (!strcmp(name, "shadow_unavailable")) *out = e->shadow_unavailable ? 1 : 0;   // bf16 shadow did not fit: TF32 level runs
     else if (!strcmp(name, "batch_tf32_queries")) *out = e->batch_tf32_queries;
     else if (!strcmp(name, "ingest_h2d_bytes")) *out = e->ingest_h2d_bytes;
@@ -2768,15 +2658,15 @@ int32_t wax_vs_debug_time_search_batch(wax_vs_engine *e, uint32_t n_queries, int
     const uint32_t k_eff = static_cast<uint32_t>(std::min<uint64_t>(clamp_topk(top_k), std::max<uint64_t>(e->n_rows, 1)));
     if (!batch_tensor_eligible(e, n_queries, k_eff))
         return fail(WAX_VS_ERR_UNSUPPORTED, "batch of %u queries, k=%u, dims=%u is not eligible for the tensor path", n_queries, k_eff, e->dims);
-    SearchCtx *c = nullptr;
-    int32_t rc = ctx_acquire(e, &c);
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
     if (rc) return rc;
-    struct Rel { wax_vs_engine *e; SearchCtx *c; ~Rel() { ctx_release(e, c); } } rel{e, c};
+    SearchCtx *c = lease.c;
     const size_t qfloats = static_cast<size_t>(n_queries) * e->dims;
-    if ((rc = ensure_dev(&c->d_queries, &c->d_queries_cap, qfloats, "query buffer"))) return rc;
-    if ((rc = ensure_dev(&c->d_out, &c->d_out_cap, static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
-    if ((rc = ensure_dev(&c->d_ok, &c->ok_cap, static_cast<size_t>(n_queries), "proof flags"))) return rc;
-    if ((rc = ensure_pinned(&c->h_ok, &c->h_ok_cap, static_cast<size_t>(n_queries), "proof flag staging"))) return rc;
+    if ((rc = c->d_queries.ensure(qfloats, "query buffer"))) return rc;
+    if ((rc = c->d_out.ensure(static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
+    if ((rc = c->d_ok.ensure(static_cast<size_t>(n_queries), "proof flags"))) return rc;
+    if ((rc = c->h_ok.ensure(static_cast<size_t>(n_queries), "proof flag staging"))) return rc;
     synth_fill_kernel<<<(n_queries + 255) / 256, 256, 0, c->stream>>>(c->d_queries, n_queries, e->dims, seed, 0, 1);
     CUDA_TRY(cudaGetLastError());
     if ((rc = ensure_norms(e, c->stream))) return rc;   // cached per corpus version: outside the timed region
@@ -2815,35 +2705,35 @@ int32_t wax_vs_debug_batch_nominations(wax_vs_engine *e, const float *queries, u
         (e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT))
         return fail(WAX_VS_ERR_UNSUPPORTED, "batch of %u queries, k=%u, dims=%u has no tensor-core nomination pass",
                     n_queries, k_eff, e->dims);
-    SearchCtx *c = nullptr;
-    int32_t rc = ctx_acquire(e, &c);
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
     if (rc) return rc;
-    struct Rel { wax_vs_engine *e; SearchCtx *c; float *d_scores; ~Rel() { if (d_scores) cudaFree(d_scores); ctx_release(e, c); } }
-        rel{e, c, nullptr};
+    SearchCtx *c = lease.c;
     const size_t qfloats = static_cast<size_t>(n_queries) * e->dims;
     const size_t n_scores = static_cast<size_t>(n_queries) * e->n_rows;
-    if ((rc = ensure_dev(&c->d_queries, &c->d_queries_cap, qfloats, "query buffer"))) return rc;
-    if ((rc = ensure_dev(&c->d_out, &c->d_out_cap, static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
-    if ((rc = ensure_dev(&c->d_ok, &c->ok_cap, static_cast<size_t>(n_queries), "proof flags"))) return rc;
-    CUDA_TRY(cudaMalloc(&rel.d_scores, n_scores * sizeof(float)));
-    CUDA_TRY(cudaMemsetAsync(rel.d_scores, 0xFF, n_scores * sizeof(float), c->stream));   // NaN payload: "never written"
+    if ((rc = c->d_queries.ensure(qfloats, "query buffer"))) return rc;
+    if ((rc = c->d_out.ensure(static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
+    if ((rc = c->d_ok.ensure(static_cast<size_t>(n_queries), "proof flags"))) return rc;
+    DevBuf<float> scores;
+    if ((rc = scores.ensure(n_scores, "nomination scores"))) return rc;
+    CUDA_TRY(cudaMemsetAsync(scores, 0xFF, n_scores * sizeof(float), c->stream));   // NaN payload: "never written"
     CUDA_TRY(cudaMemcpyAsync(c->d_queries, queries, qfloats * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     const uint32_t *d_mask = nullptr;
     if (allow_bits) {
         const size_t words = static_cast<size_t>((e->n_rows + 31) / 32);
-        if ((rc = ensure_dev(&c->d_mask, &c->mask_cap, words, "row filter"))) return rc;
+        if ((rc = c->d_mask.ensure(words, "row filter"))) return rc;
         CUDA_TRY(cudaMemcpyAsync(c->d_mask, allow_bits, words * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
         d_mask = c->d_mask;
     }
     NominationDump dump{};
-    dump.d_scores = rel.d_scores;
+    dump.d_scores = scores;
     uint64_t launches = 0;
     rc = enqueue_batch_tensor(e, c, c->d_queries, n_queries, k_eff, 0, c->d_out, c->d_ok, nullptr, c->stream, &launches,
                               true, nullptr, nullptr, d_mask, nullptr, &dump);
     if (rc) { cudaStreamSynchronize(c->stream); return rc; }
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     std::copy(dump.shape, dump.shape + 7, out_shape);
-    CUDA_TRY(cudaMemcpy(out_scores, rel.d_scores, n_scores * sizeof(float), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(out_scores, scores, n_scores * sizeof(float), cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(out_ok, c->d_ok, n_queries * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     const uint64_t n_heap = static_cast<uint64_t>(dump.shape[5]) * dump.shape[6] * dump.shape[4] * kBatchM;
     if (!out_heaps || heaps_cap < n_heap)
