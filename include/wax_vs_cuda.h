@@ -129,8 +129,12 @@ int32_t wax_vs_remove_batch(wax_vs_engine *engine, const uint64_t *frame_ids, ui
 int32_t wax_vs_search(wax_vs_engine *engine, const float *query, uint32_t query_len, int64_t top_k,
                       uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n);
 
-/* n_queries independent searches over one pass of the corpus (batched form of the above; results of
-   query i start at out_ids[i*out_stride], count out_n[i]).  out_stride >= min(clamp(top_k), N). */
+/* n_queries independent searches (batched form of the above; results of query i start at out_ids[i*out_stride],
+   count out_n[i]).  out_stride >= min(clamp(top_k), N).  Eligible batches share one tensor-core pass over the corpus
+   (results identical to n_queries calls of wax_vs_search): cosine and dot, and l2 when the option "batch_l2" is 1
+   (wax_vs_debug_set_option; default 0 for now), with dims % 32 == 0 and dims <= 8192, at least "batch_min" queries
+   (default 4) and k <= 128 (up to 1024 when the corpus holds at least 64 x k rows).  Other batches run one exact scan
+   per query. */
 int32_t wax_vs_search_batch(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
                             uint32_t query_len, int64_t top_k, uint64_t *out_ids, float *out_scores,
                             uint32_t out_stride, uint32_t *out_n);
@@ -297,7 +301,7 @@ int32_t wax_vs_debug_time_search_batch(wax_vs_engine *engine, uint32_t n_queries
    `n_queries` host queries and top_k <= 128 in the form the options select (batch_bf16, batch_ares, batch_pair,
    batch_heap), optionally with a row filter (`allow_bits`: one bit per row, set = allowed; NULL = all rows).
    out_scores [n_queries][count] receives every nomination score' the epilogue compared against its threshold (after
-   the cosine row scale); out_ok [n_queries] the proof flags; out_heaps [slices * groups][kprime][128] the nominee heaps
+   the cosine row scale; l2: score' = q.v - |v|^2 / 2, larger = nearer); out_ok [n_queries] the proof flags; out_heaps [slices * groups][kprime][128] the nominee heaps
    as dumped (key = (orderable(-score') << 32) | row); out_shape[7] = {bf16, resident queries, CTA pair, ring stages,
    kprime, slices, groups}.  A batch that needs more than one launch -> WAX_VS_ERR_ARGUMENT; heaps_cap below the
    heap entries -> WAX_VS_ERR_BUFFER with everything but the heaps written. */
@@ -309,7 +313,10 @@ int32_t wax_vs_debug_batch_nominations(wax_vs_engine *engine, const float *queri
    `iters` (milliseconds, and the bytes read).  Context for the roofline fraction (SURVEY.md section 8d). */
 int32_t wax_vs_debug_stream_read(wax_vs_engine *engine, uint32_t iters, float *out_best_ms, uint64_t *out_bytes);
 
-/* Tuning knobs for experiments ("variant", "ctas_per_sm", ...).  Unknown key -> WAX_VS_ERR_ARGUMENT. */
+/* Tuning knobs for experiments ("variant", "ctas_per_sm", ...).  Unknown key -> WAX_VS_ERR_ARGUMENT.
+   "batch_l2" (default 0): 1 lets l2 batches take the tensor-core levels of wax_vs_search_batch, _batch_filtered and
+   _batch_device (and wax_vs_debug_time_search_batch / wax_vs_debug_batch_nominations); 0 loops the exact scan.  The
+   default is to flip once the l2 levels have been measured on the H100. */
 int32_t wax_vs_debug_set_option(wax_vs_engine *engine, const char *key, int64_t value);
 
 /* Library build info: "waxvs_cuda <version> sm_90a ...". */

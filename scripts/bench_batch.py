@@ -27,12 +27,17 @@ CONFIGS = [
          dims=384, batch=1024, k=10, normalize=True, seed=2),
     dict(name="configs[4]: 10M x 768 fp32 (rows not normalised), batch 256, top-100 dot", metric=VectorMetric.dot,
          rows=10_000_000, dims=768, batch=256, k=100, normalize=False, seed=5),
+    # l2 on the tensor-core levels is opt-in (batch_l2) for now: the shapes of configs[2] and configs[4]
+    dict(name="10M x 384 fp32, batch 1024, top-10 l2", metric=VectorMetric.l2, rows=10_000_000, dims=384, batch=1024,
+         k=10, normalize=True, seed=2, options=dict(batch_l2=1)),
+    dict(name="10M x 768 fp32 (rows not normalised), batch 256, top-100 l2", metric=VectorMetric.l2, rows=10_000_000,
+         dims=768, batch=256, k=100, normalize=False, seed=5, options=dict(batch_l2=1)),
 ]
 steps = int(sys.argv[1]) if len(sys.argv) > 1 else 5
 # nominations: "bf16" (default: bf16 wgmmas over the bf16 shadow of the corpus) or "tf32" (from the fp32 corpus)
 nominate = sys.argv[2] if len(sys.argv) > 2 else "bf16"
 options = [kv.split("=") for kv in sys.argv[3:]]          # engine tuning options, e.g. batch_pair=1 batch_ares=0
-only = [int(v) for k, v in options if k == "only"]        # only=0 / only=1: run just that config
+only = [int(v) for k, v in options if k == "only"]        # only=0 .. only=3: run just that config (repeatable)
 options = [(k, v) for k, v in options if k != "only"]
 for ci, cfg in enumerate(CONFIGS):
     if only and ci not in only:
@@ -40,7 +45,8 @@ for ci, cfg in enumerate(CONFIGS):
     eng = CUDAVectorEngine(cfg["metric"], cfg["dims"])
     eng.fill_synthetic(cfg["seed"], cfg["rows"], normalize=cfg["normalize"])
     eng.set_option("batch_bf16", 1 if nominate == "bf16" else 0)
-    for k, v in options:
+    cfg_options = list(cfg.get("options", {}).items()) + options
+    for k, v in cfg_options:
         eng.set_option(k, int(v))
     ms, launches, bad = eng.time_search_batch(cfg["batch"], cfg["k"], steps, warmup=2)
     per = ms / steps
@@ -72,13 +78,14 @@ for ci, cfg in enumerate(CONFIGS):
                      "useful_flops_per_launch": flops,
                      "hbm_floor_ms": cfg["rows"] * cfg["dims"] * (2 if bf16 else 4) / 7.5e12 * 1e3},
         "shadow_gb": eng.counter("shadow_bytes") / 1e9, "tf32_retry_queries": eng.counter("batch_retry_queries"),
+        "filter_bf16_queries": eng.counter("batch_filter_bf16_queries"),
         "e2e": {"value": cfg["batch"] / e2e_s, "unit": "queries/s", "ms_per_batch": e2e_s * 1e3,
                 "h2d_bytes_per_step": int(qs.nbytes), "d2h_bytes_per_step": cfg["batch"] * cfg["k"] * 24,
                 "api": "wax_vs_search_batch (host queries -> host ids/scores arrays)"},
         "gpu_launches_per_batch": launches / steps, "unproven_queries_last_step": bad,
         "tensor_path_queries": t1 - t0, "exact_fallback_queries": f1 - f0,
         "single_query_path_ms": single_ms / 5, "speedup_vs_single_query_loop": (single_ms / 5) * cfg["batch"] / per,
-        "check_top1": res[0][0], "options": dict(options),
+        "check_top1": res[0][0], "options": dict(cfg_options),
     }
     print(json.dumps(line), flush=True)
     eng.close()

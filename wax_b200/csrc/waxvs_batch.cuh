@@ -82,7 +82,7 @@ struct BatchParams {
     uint32_t tiles_total;   // ceil(n_rows / 128)
     uint32_t kprime;        // nominee heap entries per (slice, query): 16, 24, 32 or 64
     uint32_t stages;        // TMA ring depth, 2 .. kBatchMaxStages (batch_ring_stages)
-    int metric;             // kCosine or kDot
+    int metric;             // kCosine, kDot or kL2
     const float *row_scale; // [n_rows] 1/|v| (cosine) or nullptr
     uint64_t *heaps;        // [slices*groups][kprime][128]: each CTA's heaps, dumped entry-major at the end
     uint32_t *tau_global;   // [n_queries] orderable(score') of the best k'-th nominee any slice has reached (0 = none)
@@ -98,6 +98,8 @@ struct BatchParams {
     const uint32_t *allow_bits;
     // DUMP forms only (wax_vs_debug_batch_nominations): [n_queries][n_rows] every score' the epilogue compares with tau
     float *dump_scores;
+    // L2 forms only: [n_rows] 0.5 * sum v^2 (row_norms_kernel<true>); score' = q.v - half_sq[row]
+    const float *half_sq;
 };
 
 // ---- PTX wrappers (TMA tensor loads, wgmma) ---------------------------------------------------------------------
@@ -221,8 +223,12 @@ __device__ __forceinline__ uint64_t heap_replace_root(uint64_t *heap, uint32_t n
 // count towards the dot bound: its norm is recomputed with scaling, max|x| * sqrt(sum (x / max|x|)^2) (+inf when |v|
 // itself exceeds FLT_MAX, which makes the proof refuse).  Rows holding inf or NaN are left out: their exact scores are
 // never finite, so they are never returned.
+// HALF_SQ (l2 engines): also half_sq[row] = 0.5 * sum v^2, the term the l2 nomination score subtracts (+inf when the
+// sum overflows: such a row's score' is -inf, and max|v| makes the proof refuse).
+template <bool HALF_SQ = false>
 __global__ void __launch_bounds__(256) row_norms_kernel(const float *corpus, uint32_t n_rows, uint32_t dims,
-                                                        float *inv_norm, uint32_t *max_norm_bits) {
+                                                        float *inv_norm, uint32_t *max_norm_bits,
+                                                        float *half_sq = nullptr) {
     const int lane = threadIdx.x & 31;
     const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
     const bool vec4 = (dims % 4u) == 0u;
@@ -248,6 +254,9 @@ __global__ void __launch_bounds__(256) row_norms_kernel(const float *corpus, uin
         const float s = warp_butterfly_sum(__fadd_rn(__fadd_rn(b0, b1), __fadd_rn(b2, b3)));
         const float nrm = __fsqrt_rn(s);
         if (lane == 0) inv_norm[row] = (s == 0.0f) ? 0.0f : __fdiv_rn(1.0f, nrm);
+        if constexpr (HALF_SQ) {
+            if (lane == 0) half_sq[row] = 0.5f * s;
+        }
         if (finite_f32(nrm)) {
             local_max = fmaxf(local_max, nrm);
         } else {                                                  // warp-uniform: s is the butterfly sum
@@ -315,7 +324,10 @@ __global__ void __launch_bounds__(256) shadow_bf16_kernel(const float *__restric
 //       stage is refilled only when the consumers of BOTH CTAs have released it.
 // DUMP: test read-out (wax_vs_debug_batch_nominations) -- every scanned score' is also written to p.dump_scores.  A
 //       template parameter, so the production forms compile exactly as without it.
-template <bool BF16, bool FILTER, bool ARES, bool PAIR, bool DUMP = false>
+// L2: the l2 nomination score score' = q.v - |v|^2 / 2 (p.half_sq, staged per parked tile where the cosine scales go).
+//       |q - v|^2 = |q|^2 - 2 (q.v - |v|^2 / 2), so a larger score' is a nearer row and the heaps, thresholds and
+//       staging work unchanged.  TF32 reads the fp32 rows, bf16 the raw-row shadow (as for dot).
+template <bool BF16, bool FILTER, bool ARES, bool PAIR, bool DUMP = false, bool L2 = false>
 __global__ void __launch_bounds__(kBatchThreads, 1)
 batch_nominate_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_c,
                       const BatchParams p) {
@@ -332,7 +344,7 @@ batch_nominate_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     uint8_t *a_res = smem;                                                             // [kb][128 queries x 128 B]
     uint8_t *stages = smem + ares_bytes;                                               // [stage][A 16 KB |] B 16 KB
     float *score = reinterpret_cast<float *>(stages + nst * STAGE_BYTES);              // [128 queries][kBatchScoreStride]
-    float *scale_smem = score + kBatchM * kBatchScoreStride;                           // [128] 1/|v| of the parked tile
+    float *scale_smem = score + kBatchM * kBatchScoreStride;                           // [128] 1/|v| (L2: |v|^2/2) of the parked tile
     uint64_t *full = reinterpret_cast<uint64_t *>(scale_smem + kBatchN);               // [kBatchMaxStages]
     uint64_t *empty = full + kBatchMaxStages;                                          // [kBatchMaxStages]
     uint64_t *a_full = empty + kBatchMaxStages;                                        // [1] (ARES)
@@ -435,7 +447,15 @@ batch_nominate_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
         if (chunk * 32u >= rows_here) return;                     // warp-uniform
         const float4 *src = reinterpret_cast<const float4 *>(score + tid * kBatchScoreStride + chunk * 32u);
         float sv[32];
-        if (!BF16 && p.row_scale) {
+        if constexpr (L2) {
+            const float4 *w4 = reinterpret_cast<const float4 *>(scale_smem + chunk * 32u);
+#pragma unroll
+            for (uint32_t j4 = 0; j4 < 8; ++j4) {
+                const float4 v = src[j4], w = w4[j4];
+                sv[4 * j4 + 0] = v.x - w.x; sv[4 * j4 + 1] = v.y - w.y;
+                sv[4 * j4 + 2] = v.z - w.z; sv[4 * j4 + 3] = v.w - w.w;
+            }
+        } else if (!BF16 && p.row_scale) {
             const float4 *sc4 = reinterpret_cast<const float4 *>(scale_smem + chunk * 32u);
 #pragma unroll
             for (uint32_t j4 = 0; j4 < 8; ++j4) {
@@ -564,7 +584,10 @@ batch_nominate_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
                 *reinterpret_cast<float2 *>(dst + 8u * kBatchScoreStride + 8u * j) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
             }
         }
-        if (!BF16 && p.row_scale) {
+        if constexpr (L2) {
+            const uint32_t r = row0 + tid;
+            scale_smem[tid] = (r < p.n_rows) ? __ldg(p.half_sq + r) : 0.0f;
+        } else if (!BF16 && p.row_scale) {
             const uint32_t r = row0 + tid;
             scale_smem[tid] = (r < p.n_rows) ? __ldg(p.row_scale + r) : 0.0f;
         }
@@ -752,6 +775,54 @@ struct FinishParams {
     uint32_t tau_stride;        // n_queries of the whole batch (distance between the two arrays)
 };
 
+// ---- the l2 proof and filter thresholds (batch_finish_kernel<kL2>) ----------------------------------------------------
+// Notation: a = |q|^2, D = |q - v|^2, h = q.v - |v|^2 / 2 (so D = a - 2 h), n = dims, u = 2^-24, M = max|v|, eps the
+// level's operand bound (kTf32Eps / kBf16Eps); a^, D^ the fp32 values the kernels compute.
+// (1) Nomination error.  score' = fl(acc - w): acc is the wgmma q.v, within (1.01 eps + n 2^-23) |q| r as for dot (r =
+//     |v|); w = 0.5 fl(sum v^2), whose n nonnegative terms pass through at most n / 128 + 7 roundings; the subtraction
+//     adds u (|acc| + w).  Hence |score' - h| <= E(r) = (1.01 eps + (n+1) 2^-23) |q| r + (n+2) u r^2, and E_M = E(M)
+//     bounds every row with finite components.
+// (2) Exact re-score error.  D^ holds the single-query bits: each term fl(q_i - v_i)^2 (two relative roundings) goes
+//     through an fma chain of ceil(n / 128) steps, a 2-level fadd tree and a 5-level butterfly, every term nonnegative:
+//     |D^ - D| <= gamma_(n/128 + 9) D <= delta D with delta = (n + 4) 2^-23.  |a^ - a| <= delta a the same way (one
+//     rounding fewer per term).  Products that underflow add at most ~n 2^-149 absolutely: the 1e-30 margins cover it.
+// (3) Level 1.  An excluded row x has score'_x <= tau, so h_x <= tau + E_M, a >= a^ (1 - delta) and
+//     D^_x >= (1 - delta) D_x >= (1 - delta) (a^ (1 - delta) - 2 (tau + E_M)).  When that exceeds D^_k, no excluded row
+//     can beat or tie the k-th result.  Every step rounds towards the weaker claim, then a relative 2^-20 and an
+//     absolute 1e-30 come off.
+// (4) Filter level.  A row with D^_x <= D^_k has D_x <= D^_k / (1 - delta), so h_x >= (a^ / (1 + delta) - D^_k /
+//     (1 - delta)) / 2 and score'_x >= that - E_M = tau*: a pass that lists every row with score' > tau* (lowered by the
+//     same margins as for cosine / dot) misses no true top-k row.
+// Anything non-finite refuses the proof and gives tau* = -inf, so the exact scan answers: queries far from the origin
+// next to their distances (|q| M large), or a row whose sum v^2 overflows (M covers it, so E_M overflows).
+__device__ __forceinline__ float l2_nomination_bound(float eps, float qn_hi, float m, float n) {   // E_M, rounded up
+    const float c = __fadd_ru(__fmul_ru(1.01f, eps), __fmul_ru(n + 1.0f, 0x1p-23f));
+    const float r2 = __fmul_ru(__fmul_ru(n + 2.0f, 0x1p-24f), __fmul_ru(m, m));
+    return __fadd_ru(__fadd_ru(__fmul_ru(__fmul_ru(c, qn_hi), m), r2), 1e-30f);
+}
+__device__ __forceinline__ void l2_proof(float a2, float sqrt_a2, float dk, float tau, float max_norm, uint32_t dims,
+                                         float eps_rel, bool excluded_any, uint32_t &ok, float &tau_star,
+                                         float &tau_star16) {
+    const float n = static_cast<float>(dims);
+    const float delta = (n + 4.0f) * 0x1p-23f;                       // exact (dims <= 8192)
+    const float one_m = __fsub_rd(1.0f, delta), one_p = __fadd_ru(1.0f, delta);
+    const float qn = __fmul_ru(sqrt_a2, one_p);                      // >= |q|
+    const float em = l2_nomination_bound(eps_rel, qn, max_norm, n);
+    const float a_lo = __fsub_rd(__fmul_rd(a2, one_m), 1e-30f);
+    float lhs = __fsub_rd(a_lo, __fmul_ru(2.0f, __fadd_ru(tau, em)));
+    lhs = __fsub_rd(__fmul_rd(__fmul_rd(lhs, one_m), __fsub_rd(1.0f, 0x1p-20f)), 1e-30f);
+    if (excluded_any && (!(lhs > dk) || !finite_f32(lhs) || !finite_f32(em) || !finite_f32(a2))) ok = 0;
+    const float a_lo_f = __fsub_rd(__fdiv_rd(a2, one_p), 1e-30f);
+    const float d_hi = __fadd_ru(__fdiv_ru(dk, one_m), 1e-30f);
+    auto threshold = [&](float eps) {
+        const float e = l2_nomination_bound(eps, qn, max_norm, n);
+        const float t = __fsub_rd(__fmul_rd(0.5f, __fsub_rd(a_lo_f, d_hi)), e);
+        return (finite_f32(t) && finite_f32(e) && finite_f32(a2)) ? t - fabsf(t) * 0x1p-20f - 1e-30f : -INFINITY;
+    };
+    tau_star = threshold(kTf32Eps);
+    tau_star16 = threshold(kBf16Eps);
+}
+
 // One CTA per query.  Union of the slices' nominee heaps -> best kBatchRescore by score' -> exact re-score ->
 // proof.  Rows that were never nominated have score' <= tau_excl = max over slices of that slice's final heap
 // root (a slice only ever filtered by its own root or by a root another slice had published); nominated rows
@@ -835,7 +906,13 @@ __global__ void __launch_bounds__(512, 2) batch_finish_kernel(const FinishParams
         while (n_exact < kpp && ek[n_exact] != WAXVS_KEY_NONE) ++n_exact;
         uint32_t ok = 1;
         float tau_star = -INFINITY, tau_star16 = -INFINITY;
-        if (n_exact >= p.k) {
+        if (n_exact >= p.k && METRIC == kL2) {
+            if constexpr (METRIC == kL2) {
+                const float dk = from_orderable_u32(static_cast<uint32_t>(ek[p.k - 1] >> 32));
+                l2_proof(s_a2, s_sqrt_a2, dk, tau, __uint_as_float(*p.max_norm_bits), p.dims, p.eps_rel, excluded_any,
+                         ok, tau_star, tau_star16);
+            }
+        } else if (n_exact >= p.k) {
             const float dk = from_orderable_u32(static_cast<uint32_t>(ek[p.k - 1] >> 32));
             const float qn = s_sqrt_a2;
             const float scale = METRIC == kCosine ? qn : qn * __uint_as_float(*p.max_norm_bits);

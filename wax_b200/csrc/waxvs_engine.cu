@@ -176,6 +176,8 @@ struct Tuning {
     int host_delivery = 1;  // host entry points: the kernel stores the result in mapped host memory + flag (no D2H copy / sync)
     int tail_select = 1;    // TMA-staged kernels: radix-selection tail instead of pairwise list merges (same results)
     int shard_fused = 1;    // sharded search: exchange + merge inside the scan launch (0: separate 1-CTA launch)
+    int batch_l2 = 0;       // 1: l2 batches take the tensor-core levels too (off: they loop the single-query path).  A staging
+                            // switch: the default flips once the l2 levels have H100 figures behind them
     int single_shadow = 0;  // 1: single queries / batches below batch_min also take the bf16-shadow nominations
                             // (half the HBM bytes per query, same results); off by
                             // default: the plain single-query path is the fused fp32 scan BASELINE's north_star names
@@ -253,10 +255,12 @@ struct wax_vs_engine {
     uint64_t pool_allocs = 0, pool_reuses = 0;
     Tuning tune;
 
-    // cached per corpus version for the batched path: 1/|v| per row and max |v|
+    // cached per corpus version for the batched path: 1/|v| per row and max |v|; l2 engines also |v|^2 / 2 per row
     DevBuf<float> d_inv_norm;
     DevBuf<uint32_t> d_max_norm;
-    uint64_t norms_rows = 0;       // rows [0, norms_rows) of d_inv_norm are valid (appends extend it, other mutations reset it)
+    DevBuf<float> d_half_sq;
+    uint64_t norms_rows = 0;       // rows [0, norms_rows) of d_inv_norm (and d_half_sq) are valid (appends extend it, other
+                                   // mutations reset it)
     std::mutex norms_mu;
     // bf16 shadow of the corpus for the batched bf16 nominations (cached per corpus version, guarded by norms_mu)
     DevBuf<__nv_bfloat16> d_shadow;
@@ -721,7 +725,8 @@ static bool batch_bf16_wanted(const wax_vs_engine *e);
 static bool batch_tensor_eligible(const wax_vs_engine *e, uint32_t n_queries, uint32_t k_eff) {
     const uint32_t min_batch = (e->tune.single_shadow && batch_bf16_wanted(e)) ? 1u : static_cast<uint32_t>(std::max(e->tune.batch_min, 1));
     return e->tune.batch_tensor && n_queries >= min_batch &&
-           (e->similarity == WAX_VS_COSINE || e->similarity == WAX_VS_DOT) && e->dims % kBatchKBlock == 0 &&
+           (e->similarity == WAX_VS_COSINE || e->similarity == WAX_VS_DOT || (e->similarity == WAX_VS_L2 && e->tune.batch_l2)) &&
+           e->dims % kBatchKBlock == 0 &&
            e->dims <= 8192 &&        // the proof's accumulation slack (dims * 2^-23) stays far below the operand bound
            k_eff >= 1 && e->n_rows >= 1 &&
            // 128 < k <= 1024 (the production candidate limit reaches 1 000, UnifiedSearch.swift:1195-1200): real batches
@@ -732,14 +737,18 @@ static bool batch_tensor_eligible(const wax_vs_engine *e, uint32_t n_queries, ui
                              e->n_rows >= 64ull * k_eff));   // smaller corpora: too few row slices to nominate k rows
 }
 
-// 1/|v| per row + max |v|, cached per corpus version.  Appends only extend the cache (rows [norms_rows, n_rows) are
-// computed, the running max only grows); anything that moves or overwrites rows resets norms_rows to 0.
+// 1/|v| per row + max |v| (l2 engines: and |v|^2 / 2 per row, in the same pass), cached per corpus version.  Appends only
+// extend the cache (rows [norms_rows, n_rows) are computed, the running max only grows); anything that moves or
+// overwrites rows resets norms_rows to 0.
 static int32_t ensure_norms_locked(wax_vs_engine *e, cudaStream_t stream) {
-    if (e->norms_rows == e->n_rows && e->d_inv_norm) return WAX_VS_OK;
-    if (static_cast<size_t>(e->n_rows) > e->d_inv_norm.cap || !e->d_inv_norm) {
+    const bool l2 = e->similarity == WAX_VS_L2;
+    if (e->norms_rows == e->n_rows && e->d_inv_norm && (!l2 || e->d_half_sq)) return WAX_VS_OK;
+    if (static_cast<size_t>(e->n_rows) > e->d_inv_norm.cap || !e->d_inv_norm ||
+        (l2 && (static_cast<size_t>(e->n_rows) > e->d_half_sq.cap || !e->d_half_sq))) {
         e->norms_rows = 0;                                       // ensure re-allocates: the cached prefix is gone
         const size_t want = static_cast<size_t>(std::max<uint64_t>(e->cap_rows, std::max<uint64_t>(e->n_rows, 1)));
         int32_t rc = e->d_inv_norm.ensure(want, "row norms");
+        if (!rc && l2) rc = e->d_half_sq.ensure(want, "row half squared norms");
         if (rc) return rc;
     }
     if (!e->d_max_norm) {
@@ -752,8 +761,13 @@ static int32_t ensure_norms_locked(wax_vs_engine *e, cudaStream_t stream) {
     const uint64_t first = e->norms_rows, count = e->n_rows - first;
     if (count) {
         const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 8, (count + 7) / 8));
-        row_norms_kernel<<<std::max(grid, 1), 256, 0, stream>>>(e->d_corpus + first * e->dims, static_cast<uint32_t>(count), e->dims,
-                                                                e->d_inv_norm + first, e->d_max_norm);
+        if (l2)
+            row_norms_kernel<true><<<std::max(grid, 1), 256, 0, stream>>>(e->d_corpus + first * e->dims, static_cast<uint32_t>(count),
+                                                                          e->dims, e->d_inv_norm + first, e->d_max_norm,
+                                                                          e->d_half_sq + first);
+        else
+            row_norms_kernel<<<std::max(grid, 1), 256, 0, stream>>>(e->d_corpus + first * e->dims, static_cast<uint32_t>(count), e->dims,
+                                                                    e->d_inv_norm + first, e->d_max_norm);
         CUDA_TRY(cudaGetLastError());
     }
     CUDA_TRY(cudaStreamSynchronize(stream));
@@ -815,10 +829,10 @@ static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream) {
 }
 
 // One launch of the nominate kernel in one form; its opt-in shared memory is granted first.
-template <bool BF, bool FI, bool AR, bool PR, bool DUMP>
+template <bool BF, bool FI, bool AR, bool PR, bool DUMP, bool L2>
 static cudaError_t launch_nominate_inst(wax_vs_engine *e, uint32_t grid, uint32_t smem, cudaStream_t stream,
                                         const CUtensorMap &map_q, const CUtensorMap &map_c, const BatchParams &bp) {
-    const auto kernel = batch_nominate_kernel<BF, FI, AR, PR, DUMP>;
+    const auto kernel = batch_nominate_kernel<BF, FI, AR, PR, DUMP, L2>;
     const cudaError_t err = grant_smem(e, kernel, smem);
     if (err != cudaSuccess) return err;
     cudaLaunchConfig_t cfg{};
@@ -834,12 +848,12 @@ static cudaError_t launch_nominate_inst(wax_vs_engine *e, uint32_t grid, uint32_
 
 // The nominate kernel in the form (bf16, filter, resident queries, CTA pair) a pass picked; DUMP: with the score
 // read-out (wax_vs_debug_batch_nominations).  These are all the forms there are: the filter level runs neither as CTA
-// pairs nor with the read-out, and TF32 queries always stream through the ring.
-template <bool DUMP>
-static cudaError_t launch_nominate(wax_vs_engine *e, bool bf16, bool filter, bool ares, bool pair, uint32_t grid,
-                                   uint32_t smem, cudaStream_t stream, const CUtensorMap &map_q, const CUtensorMap &map_c,
-                                   const BatchParams &bp) {
-#define WAXVS_NOM(BF, FI, AR, PR) return launch_nominate_inst<BF, FI, AR, PR, DUMP>(e, grid, smem, stream, map_q, map_c, bp)
+// pairs nor with the read-out, and TF32 queries always stream through the ring.  L2: the same forms with the l2 score.
+template <bool DUMP, bool L2>
+static cudaError_t launch_nominate_forms(wax_vs_engine *e, bool bf16, bool filter, bool ares, bool pair, uint32_t grid,
+                                         uint32_t smem, cudaStream_t stream, const CUtensorMap &map_q,
+                                         const CUtensorMap &map_c, const BatchParams &bp) {
+#define WAXVS_NOM(BF, FI, AR, PR) return launch_nominate_inst<BF, FI, AR, PR, DUMP, L2>(e, grid, smem, stream, map_q, map_c, bp)
     if constexpr (!DUMP) {
         if (filter) {
             if (!bf16) WAXVS_NOM(false, true, false, false);
@@ -858,6 +872,13 @@ static cudaError_t launch_nominate(wax_vs_engine *e, bool bf16, bool filter, boo
     if (pair) WAXVS_NOM(true, false, false, true);
     WAXVS_NOM(true, false, false, false);
 #undef WAXVS_NOM
+}
+template <bool DUMP>
+static cudaError_t launch_nominate(wax_vs_engine *e, bool l2, bool bf16, bool filter, bool ares, bool pair, uint32_t grid,
+                                   uint32_t smem, cudaStream_t stream, const CUtensorMap &map_q, const CUtensorMap &map_c,
+                                   const BatchParams &bp) {
+    return l2 ? launch_nominate_forms<DUMP, true>(e, bf16, filter, ares, pair, grid, smem, stream, map_q, map_c, bp)
+              : launch_nominate_forms<DUMP, false>(e, bf16, filter, ares, pair, grid, smem, stream, map_q, map_c, bp);
 }
 
 // ---- nominee-heap policy (level 1) ----
@@ -885,10 +906,11 @@ static uint32_t pick_heap(wax_vs_engine *e, bool bf16, uint32_t nq, uint32_t sli
     // expected cost of a batch = the shape's relative time + P(some query of the batch is unproven) x one more
     // pass.  Threatening rows per query: ~2.2 k (cosine, unit rows) / ~2.8 k (dot: the bound scales with the
     // LARGEST row norm).  The relative times of the heap sizes are guesses carried over from B200 (ring depths
-    // 4 / 3 / 3 / 2 on H100); they have not been measured on H100.
+    // 4 / 3 / 3 / 2 on H100); they have not been measured on H100.  l2 takes the dot figure: its bound has the same
+    // max-norm structure; that figure has not been measured for l2.
     static const uint32_t ladder[4] = {16u, 24u, 32u, 64u};
     static const double rel_time[4] = {1.00, 1.02, 1.10, 1.40};
-    const double m = (e->similarity == WAX_VS_DOT ? 2.8 : 2.2) * k_eff / slices;
+    const double m = (e->similarity == WAX_VS_COSINE ? 2.2 : 2.8) * k_eff / slices;
     uint32_t bump = 0;
     { std::lock_guard<std::mutex> pg(e->pool_mu); bump = e->heap_bump; }
     double best = 1e30;
@@ -955,6 +977,7 @@ static int32_t enqueue_nominate_pass(wax_vs_engine *e, SearchCtx *c, const float
     }
     const uint32_t tiles_total = static_cast<uint32_t>((e->n_rows + kBatchN - 1) / kBatchN);
     const uint32_t num_kb16 = e->dims / kBatchKBlockBf16;
+    const bool l2 = e->similarity == WAX_VS_L2;          // the l2 score: the forms subtract the cached |v|^2 / 2
     for (uint32_t q0 = 0; q0 < n_queries; q0 += max_groups * kBatchM) {
         NominateChunk ch{};
         ch.q0 = q0;
@@ -986,12 +1009,13 @@ static int32_t enqueue_nominate_pass(wax_vs_engine *e, SearchCtx *c, const float
         bp.stages = static_cast<uint32_t>(ch.stages);
         // the cosine shadow rows are pre-normalised: no epilogue scaling on the bf16 path
         bp.row_scale = (e->similarity == WAX_VS_COSINE && !bf16) ? e->d_inv_norm.p : nullptr;
+        bp.half_sq = l2 ? e->d_half_sq.p : nullptr;
         bp.allow_bits = d_mask;
         if ((rc = prepare(ch, bp))) return rc;
         const uint32_t grid = ch.groups * ch.slices;
         const uint32_t smem = batch_smem_bytes(ch.stages, static_cast<int>(ch.kprime), ch.ares ? num_kb16 : 0u);
-        const cudaError_t lerr = dump ? launch_nominate<true>(e, bf16, filter, ch.ares, ch.pair, grid, smem, stream, map_q, map_c, bp)
-                                      : launch_nominate<false>(e, bf16, filter, ch.ares, ch.pair, grid, smem, stream, map_q, map_c, bp);
+        const cudaError_t lerr = dump ? launch_nominate<true>(e, l2, bf16, filter, ch.ares, ch.pair, grid, smem, stream, map_q, map_c, bp)
+                                      : launch_nominate<false>(e, l2, bf16, filter, ch.ares, ch.pair, grid, smem, stream, map_q, map_c, bp);
         CUDA_TRY(lerr);
         CUDA_TRY(cudaGetLastError());
         ++*launches;
@@ -1070,7 +1094,9 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
         fp.tau_star = d_tau_star ? d_tau_star + ch.q0 : nullptr;
         fp.tau_stride = n_queries;
         const size_t fsmem = static_cast<size_t>(pow2 + rescore) * sizeof(uint64_t);
-        const auto kernel = e->similarity == WAX_VS_COSINE ? batch_finish_kernel<kCosine> : batch_finish_kernel<kDot>;
+        const auto kernel = e->similarity == WAX_VS_COSINE ? batch_finish_kernel<kCosine>
+                            : e->similarity == WAX_VS_DOT  ? batch_finish_kernel<kDot>
+                                                           : batch_finish_kernel<kL2>;
         CUDA_TRY(grant_smem(e, kernel, fsmem));
         kernel<<<ch.nq, 512, fsmem, stream>>>(fp);
         CUDA_TRY(cudaGetLastError());
@@ -1630,7 +1656,9 @@ static int32_t enqueue_filter_level(wax_vs_engine *e, SearchCtx *c, const float 
     auto finish = [&](const NominateChunk &ch) -> int32_t {
         const uint32_t *count = c->d_cand_count + ch.q0;
         uint64_t *keys = c->d_cand_keys + static_cast<size_t>(ch.q0) * cap;
-        const auto rescore = e->similarity == WAX_VS_COSINE ? filter_rescore_kernel<kCosine> : filter_rescore_kernel<kDot>;
+        const auto rescore = e->similarity == WAX_VS_COSINE ? filter_rescore_kernel<kCosine>
+                             : e->similarity == WAX_VS_DOT  ? filter_rescore_kernel<kDot>
+                                                            : filter_rescore_kernel<kL2>;
         rescore<<<dim3(32, ch.nq), 256, 0, stream>>>(e->d_corpus, ch.queries, e->dims, count,
                                                      c->d_cand_rows + static_cast<size_t>(ch.q0) * cap, cap, keys);
         CUDA_TRY(cudaGetLastError());
@@ -2702,7 +2730,7 @@ int32_t wax_vs_debug_batch_nominations(wax_vs_engine *e, const float *queries, u
     if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
     const uint32_t k_eff = static_cast<uint32_t>(std::min<uint64_t>(clamp_topk(top_k), std::max<uint64_t>(e->n_rows, 1)));
     if (n_queries == 0 || e->n_rows == 0 || k_eff > 128u || e->dims % kBatchKBlock != 0 || e->dims > 8192 ||
-        (e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT))
+        (e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT && !(e->similarity == WAX_VS_L2 && e->tune.batch_l2)))
         return fail(WAX_VS_ERR_UNSUPPORTED, "batch of %u queries, k=%u, dims=%u has no tensor-core nomination pass",
                     n_queries, k_eff, e->dims);
     CtxLease lease(e);
@@ -2768,6 +2796,7 @@ int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value
     else if (!strcmp(key, "batch_retry")) e->tune.batch_retry = v;
     else if (!strcmp(key, "filter_cap")) e->tune.filter_cap = v;
     else if (!strcmp(key, "filter_bf16")) e->tune.filter_bf16 = v;
+    else if (!strcmp(key, "batch_l2")) e->tune.batch_l2 = v;
     else if (!strcmp(key, "single_shadow")) e->tune.single_shadow = v;
     else if (!strcmp(key, "shard_fused")) e->tune.shard_fused = v;
     else if (!strcmp(key, "tail_select")) e->tune.tail_select = v;

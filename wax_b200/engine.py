@@ -262,6 +262,8 @@ class CUDAVectorEngine:
         return [[(int(ids[i, j]), float(scores[i, j])) for j in range(int(ns[i]))] for i in range(b)]
 
     def search_batch(self, vectors, top_k: int) -> List[List[Tuple[int, float]]]:
+        """`search` for a batch of queries (wax_vs_search_batch): the same answers as one call per query.  Cosine and dot
+        batches share one tensor-core pass over the corpus, l2 batches too once set_option("batch_l2", 1) is set."""
         ids, scores, ns = self.search_batch_arrays(vectors, top_k)
         return [[(int(ids[i, j]), float(scores[i, j])) for j in range(int(ns[i]))] for i in range(ids.shape[0])]
 

@@ -293,7 +293,7 @@ class ShardedVectorEngine:
     def search_batch_arrays(self, queries, top_k: int):
         """A batch of independent queries against the sharded corpus: every rank runs the batched tensor-core levels
         (wax_vs_search_batch_device: bf16-shadow nominations -> TF32 retry -> exact scan, results identical to
-        single-query scans) on its shard, ONE all-gather carries batch x k candidates per rank, ONE merge kernel
+        single-query scans; cosine and dot, l2 with the engine option batch_l2 = 1) on its shard, ONE all-gather carries batch x k candidates per rank, ONE merge kernel
         (wax_vs_merge_candidates_device) ranks them on the device.  `queries`: [batch, dims] host array or device tensor (identical on every rank).  Returns
         (ids [batch, k_eff] uint64, scores [batch, k_eff] float32, n_valid [batch] uint32)."""
         torch, dist = self._torch, self._dist
