@@ -159,6 +159,28 @@ int32_t wax_vs_search_batch_filtered(wax_vs_engine *engine, const float *queries
                                      int32_t mode, uint64_t *out_ids, float *out_scores, uint32_t out_stride,
                                      uint32_t *out_n);
 
+/* The batched form with one filter PER QUERY (a server batching requests that each carry their own frame filter):
+   query i searches under filter query_filter[i], or unfiltered for WAX_VS_NO_FILTER.  Filter f is the ids
+   frame_ids[filter_offsets[f] .. filter_offsets[f+1]) with mode filter_modes[f] (0 allow-list, 1 deny-list);
+   filters no query references are not resolved.  Results of query i start at out_ids[i*out_stride], count out_n[i];
+   out_stride >= max_i min(clamp(top_k), #allowed_i) (else WAX_VS_ERR_BUFFER).  Query i's answer is identical to
+   wax_vs_search_filtered under its filter (wax_vs_search when unfiltered): same ids, same order, same score bits.
+   Routing: allow-lists of <= 16 384 rows score only their listed rows (one batched gather for all such queries);
+   queries whose filter allows at least clamp(top_k) rows share the tensor-core levels (or a masked fused scan each),
+   every query consulting its own row bitset; the rest (deny-lists leaving fewer than k rows) scan one by one.  The
+   bitsets are built on the device from the resolved rows; one tensor pass holds at most the option
+   "filter_bitset_bytes" of them (default 2 GiB, one bitset is ceil(N/32) * 4 bytes), more filters run in several
+   sub-batches (counter "filter_bitset_passes").  Arguments are checked before the empty-engine early return:
+   WAX_VS_ERR_ARGUMENT for a mode other than 0 / 1, filter_offsets[0] != 0, decreasing offsets, or a query_filter
+   entry >= n_filters other than WAX_VS_NO_FILTER; WAX_VS_ERR_NULL for a NULL array (frame_ids may be NULL when
+   filter_offsets[n_filters] == 0, filter_modes when n_filters == 0).  Unknown and repeated ids are ignored. */
+#define WAX_VS_NO_FILTER 0xFFFFFFFFu
+int32_t wax_vs_search_batch_multi_filtered(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                           uint32_t query_len, int64_t top_k, const uint64_t *frame_ids,
+                                           const uint64_t *filter_offsets, const int32_t *filter_modes,
+                                           uint32_t n_filters, const uint32_t *query_filter, uint64_t *out_ids,
+                                           float *out_scores, uint32_t out_stride, uint32_t *out_n);
+
 /* Device-resident form used by the row-sharded engine: `d_queries` (n_queries x dims) and
    `d_candidates` (n_queries x k_eff entries, k_eff = min(clamp(top_k), 10000) -- NOT clipped to N, padding
    has valid = 0) are DEVICE pointers on the engine's device; the work is enqueued on `cuda_stream`
@@ -287,7 +309,8 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *engine, uint64_t *tensor_queries
 /* Named instrumentation counters: "batch_tensor_queries", "batch_fallback_queries", "batch_bf16_queries" (queries
    nominated from the bf16 shadow), "batch_retry_queries" (bf16-unproven queries retried on the TF32 nominations),
    "shadow_bytes" (HBM held by the bf16 shadow), "shadow_unavailable" (1 = the shadow did not fit in HBM, batches
-   nominate in TF32 at about half the rate), "batch_tf32_queries", "pool_allocs", "pool_reuses". */
+   nominate in TF32 at about half the rate), "batch_tf32_queries", "filter_bitset_passes" (sub-batches of per-query
+   filtered queries on the tensor-core class, wax_vs_search_batch_multi_filtered), "pool_allocs", "pool_reuses". */
 int32_t wax_vs_debug_counter(wax_vs_engine *engine, const char *name, uint64_t *out);
 
 /* Device-only timing of the batched path (n_queries synthetic unit queries per step, everything resident):
@@ -316,7 +339,9 @@ int32_t wax_vs_debug_stream_read(wax_vs_engine *engine, uint32_t iters, float *o
 /* Tuning knobs for experiments ("variant", "ctas_per_sm", ...).  Unknown key -> WAX_VS_ERR_ARGUMENT.
    "batch_l2" (default 0): 1 lets l2 batches take the tensor-core levels of wax_vs_search_batch, _batch_filtered and
    _batch_device (and wax_vs_debug_time_search_batch / wax_vs_debug_batch_nominations); 0 loops the exact scan.  The
-   default is to flip once the l2 levels have been measured on the H100. */
+   default is to flip once the l2 levels have been measured on the H100.
+   "filter_bitset_bytes" (default 2 GiB): device memory the row bitsets of one tensor pass of
+   wax_vs_search_batch_multi_filtered may use; at least one bitset always fits. */
 int32_t wax_vs_debug_set_option(wax_vs_engine *engine, const char *key, int64_t value);
 
 /* Library build info: "waxvs_cuda <version> sm_90a ...". */

@@ -17,6 +17,7 @@ LIB_PATH = PKG / "libwaxvs_cuda.so"
 OK, ERR_NULL, ERR_DIMENSION, ERR_CAPACITY, ERR_CUDA, ERR_FORMAT, ERR_ARGUMENT, ERR_BUFFER, ERR_UNSUPPORTED = (
     0, -1, -2, -3, -4, -5, -6, -7, -8)
 MAX_RESULTS = 10_000
+NO_FILTER = 0xFFFFFFFF          # WAX_VS_NO_FILTER: a query of wax_vs_search_batch_multi_filtered without a filter
 MAX_DIMENSIONS = 1_000_000
 SHARD_HANDLE_BYTES, SHARD_MAX_RANKS, SHARD_MAX_K = 128, 16, 128
 
@@ -49,6 +50,9 @@ SIGNATURES = {
                                                  _u64p, _f32p, C.c_uint32, _u32p]),
     "wax_vs_shard_search_filtered": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_int64, _u64p, C.c_uint64, C.c_int32, _u64p,
                                                  _f32p, C.c_uint32, _u32p]),
+    "wax_vs_search_batch_multi_filtered": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _u64p,
+                                                       C.POINTER(C.c_int32), C.c_uint32, _u32p, _u64p, _f32p, C.c_uint32,
+                                                       _u32p]),
     "wax_vs_search_batch": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _f32p,
                                         C.c_uint32, _u32p]),
     "wax_vs_search_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, C.c_uint64, C.c_void_p,

@@ -96,6 +96,10 @@ struct BatchParams {
     // filtered batches (wax_vs_search_batch_filtered): 1 bit per row, set = the row may be returned; nullptr = all rows.
     // Consulted only on the rare path (a chunk of 32 rows that holds a score above the query's threshold).
     const uint32_t *allow_bits;
+    // per-query filters (wax_vs_search_batch_multi_filtered): query q of the launch uses the bitset allow_bits +
+    // query_filter[q] * filter_words, or none for WAX_VS_NO_FILTER; nullptr = every query uses allow_bits
+    const uint32_t *query_filter;
+    uint32_t filter_words;
     // DUMP forms only (wax_vs_debug_batch_nominations): [n_queries][n_rows] every score' the epilogue compares with tau
     float *dump_scores;
     // L2 forms only: [n_rows] 0.5 * sum v^2 (row_norms_kernel<true>); score' = q.v - half_sq[row]
@@ -412,6 +416,12 @@ batch_nominate_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
     const uint32_t tid = threadIdx.x;                              // 0..127
     const uint32_t q = group * kBatchM + tid;
     const bool q_valid = q < p.n_queries && !p.no_insert;
+    // this query's row filter (padded queries never read query_filter: they nominate nothing)
+    const uint32_t *allow = p.allow_bits;
+    if (p.query_filter && q < p.n_queries) {
+        const uint32_t f = __ldg(p.query_filter + q);
+        allow = f == WAX_VS_NO_FILTER ? nullptr : p.allow_bits + static_cast<size_t>(f) * p.filter_words;
+    }
     uint64_t *heap = heap_smem + tid;
     if (!FILTER) for (uint32_t i = 0; i < heap_n; ++i) heap[i * kBatchM] = WAXVS_KEY_NONE;
     uint64_t root = WAXVS_KEY_NONE;                               // heap[0]: this slice's k'-th best so far
@@ -490,7 +500,7 @@ batch_nominate_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_c
             const uint32_t cols = rows_here - chunk * 32u;                 // >= 1 here
             if (cols < 32u) mask &= (1u << cols) - 1u;
             // row0 + chunk * 32 is a multiple of 32: the chunk's 32 rows are exactly one word of the row filter
-            if (p.allow_bits) mask &= __ldg(p.allow_bits + ((row0 + chunk * 32u) >> 5));
+            if (allow) mask &= __ldg(allow + ((row0 + chunk * 32u) >> 5));
             while (mask) {
                 if (cnt + __popc(mask) > kBatchStageSlots) flush();       // empties the slots, may raise tau
                 uint32_t take = mask;
@@ -704,13 +714,20 @@ __device__ __forceinline__ void block_bitonic_sort(uint64_t *sk, uint32_t pow2) 
 }
 
 // ---- small allow-lists: score only the listed rows (O(n_allow), not O(N)) --------------------------------------------
-// One warp per listed row, exact distance in the kernels' order; then one CTA sorts the keys.
+// One warp per listed row, exact distance in the kernels' order; then one CTA sorts the keys.  Query y of the launch
+// scores the rows rows_all[span[y].x .. span[y].x + span[y].y) of one concatenated list (queries under the same filter
+// point at the same span) into keys_all[y * key_stride ..].
 template <int METRIC>
 __global__ void __launch_bounds__(256) gather_score_kernel(const float *corpus, const float *queries, uint32_t dims,
-                                                           const uint32_t *rows, uint32_t n, uint64_t *keys_all) {
+                                                           const uint32_t *rows_all, const uint2 *span, uint32_t key_stride,
+                                                           uint64_t *keys_all) {
     const int lane = threadIdx.x & 31;
     const float *query = queries + static_cast<size_t>(blockIdx.y) * dims;     // grid.y = queries of a filtered batch
-    uint64_t *keys = keys_all + static_cast<size_t>(blockIdx.y) * n;
+    const uint2 sp = span[blockIdx.y];
+    const uint32_t *rows = rows_all + sp.x;
+    const uint32_t n = sp.y;
+    if (n == 0) return;
+    uint64_t *keys = keys_all + static_cast<size_t>(blockIdx.y) * key_stride;
     float a2 = 0.0f, sqrt_a2 = 0.0f;
     if (METRIC == kCosine) {
         float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
@@ -745,15 +762,53 @@ __global__ void __launch_bounds__(256) gather_score_kernel(const float *corpus, 
     }
 }
 
-__global__ void __launch_bounds__(1024) gather_sort_kernel(const uint64_t *keys_all, uint32_t n, uint32_t pow2, ScanParams p) {
+// One CTA per query sorts its span's keys (pow2 >= the longest span of the launch) and writes p.k candidates at
+// p.out + query * p.k; the slots past the span's length are invalid.
+__global__ void __launch_bounds__(1024) gather_sort_kernel(const uint64_t *keys_all, const uint2 *span, uint32_t key_stride,
+                                                           uint32_t pow2, ScanParams p) {
     extern __shared__ uint64_t gsk[];
-    const uint64_t *keys = keys_all + static_cast<size_t>(blockIdx.x) * n;     // one CTA per query
+    const uint64_t *keys = keys_all + static_cast<size_t>(blockIdx.x) * key_stride;
+    const uint32_t n = span[blockIdx.x].y;
     p.out += static_cast<size_t>(blockIdx.x) * p.k;
     for (uint32_t i = threadIdx.x; i < pow2; i += blockDim.x) gsk[i] = (i < n) ? keys[i] : WAXVS_KEY_NONE;
     __syncthreads();
     block_bitonic_sort(gsk, pow2);
     for (uint32_t i = threadIdx.x; i < p.k; i += blockDim.x)
         write_candidate(p, static_cast<int>(i), i < pow2 ? gsk[i] : WAXVS_KEY_NONE);
+}
+
+// ---- row filters: F bitsets of `words` words each, built on the device from the resolved rows ------------------------
+// spec (3F + 1 entries): [0, F]: running count of listed rows (filter f lists entries [spec[f], spec[f+1]));
+// [F + 1, 2F + 1): where filter f's rows start in `rows`; [2F + 1, 3F + 1): its mode (0 allow-list, 1 deny-list).
+// Pass 1 writes the background: 0 for an allow-list, all ones below n_rows for a deny-list.
+__global__ void __launch_bounds__(256) filter_bits_init_kernel(uint32_t *bits, uint32_t words, uint32_t n_rows,
+                                                               const uint64_t *spec, uint32_t n_filters) {
+    const size_t total = static_cast<size_t>(words) * n_filters;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const uint32_t f = static_cast<uint32_t>(i / words), w = static_cast<uint32_t>(i % words);
+        uint32_t v = 0u;
+        if (spec[2u * n_filters + 1u + f]) v = (w == words - 1u && (n_rows & 31u)) ? (1u << (n_rows & 31u)) - 1u : 0xFFFFFFFFu;
+        bits[i] = v;
+    }
+}
+// Pass 2 sets (allow-list) or clears (deny-list) the bit of every listed row.  The rows of one filter are distinct.
+__global__ void __launch_bounds__(256) filter_bits_apply_kernel(uint32_t *bits, uint32_t words, const uint32_t *rows,
+                                                                const uint64_t *spec, uint32_t n_filters) {
+    const uint64_t total = spec[n_filters];
+    for (uint64_t t = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x; t < total;
+         t += static_cast<uint64_t>(gridDim.x) * blockDim.x) {
+        uint32_t lo = 0, hi = n_filters - 1u;             // the last f with spec[f] <= t
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi + 1u) >> 1;
+            if (spec[mid] <= t) lo = mid; else hi = mid - 1u;
+        }
+        const uint32_t row = rows[spec[n_filters + 1u + lo] + (t - spec[lo])];
+        uint32_t *word = bits + static_cast<size_t>(lo) * words + (row >> 5);
+        const uint32_t b = 1u << (row & 31u);
+        if (spec[2u * n_filters + 1u + lo]) atomicAnd(word, ~b);
+        else atomicOr(word, b);
+    }
 }
 
 struct FinishParams {

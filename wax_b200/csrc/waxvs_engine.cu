@@ -181,6 +181,7 @@ struct Tuning {
     int single_shadow = 0;  // 1: single queries / batches below batch_min also take the bf16-shadow nominations
                             // (half the HBM bytes per query, same results); off by
                             // default: the plain single-query path is the fused fp32 scan BASELINE's north_star names
+    uint64_t filter_bitset_bytes = 2ull << 30;   // per-query filters: row bitsets one tensor pass may hold
 };
 
 // Per-search scratch: the analogue of TransientBuffers (MetalVectorEngine.swift:36-41, :84-117).
@@ -212,7 +213,12 @@ struct SearchCtx {
     DevBuf<uint32_t> d_cand_count;
     DevBuf<uint32_t> d_cand_rows;
     DevBuf<uint64_t> d_cand_keys;
-    DevBuf<uint32_t> d_mask;                       // filtered search: row bitset / listed rows
+    DevBuf<uint32_t> d_mask;                       // filtered search: row bitsets [filters][words]
+    DevBuf<uint32_t> d_filter_rows;                // filtered search: the filters' resolved rows, concatenated
+    DevBuf<uint64_t> d_filter_spec;                // filtered search: bitset builder spec (filter_bits_init_kernel)
+    DevBuf<uint32_t> d_query_filter;               // filtered search: each query's bitset index
+    DevBuf<uint32_t> d_retry_filter;               // filter level: bitset indices of the compacted queries
+    DevBuf<uint2> d_gather_span;                   // filtered search: each gathered query's span of d_filter_rows
     DevBuf<uint64_t> d_gather_keys;                // filtered search: keys of the listed rows
     DevBuf<wax_vs_candidate> d_shard_local;        // sharded search: this rank's list before the exchange [kShardKCap]
     PinnedBuf<unsigned long long> h_flag;          // host-delivery completion flag
@@ -268,6 +274,7 @@ struct wax_vs_engine {
     bool shadow_valid = false, shadow_unavailable = false;
     uint64_t batch_tensor_queries = 0, batch_fallback_queries = 0;   // instrumentation
     uint64_t batch_bf16_queries = 0, batch_retry_queries = 0, batch_tf32_queries = 0, batch_filter_bf16_queries = 0;
+    uint64_t filter_bitset_passes = 0;
     // Adaptive level choice: when more than a quarter of a batch fails the coarse bf16 bound (tightly clustered
     // neighbours), the next 16 batches nominate in TF32 straight away, then bf16 is probed again.
     uint32_t bf16_skip_batches = 0;
@@ -550,13 +557,21 @@ static int32_t wait_host_flag(cudaStream_t stream, unsigned long long *flag_ptr,
     }
 }
 
-// n host queries -> pinned staging (c->h_queries) -> c->d_queries, on `stream`
-static int32_t stage_queries(wax_vs_engine *e, SearchCtx *c, const float *queries, uint32_t n, cudaStream_t stream) {
+// n host queries -> pinned staging (c->h_queries) -> c->d_queries, on `stream`; order (optional): staged query j is
+// queries[order[j]]
+static int32_t stage_queries(wax_vs_engine *e, SearchCtx *c, const float *queries, uint32_t n, cudaStream_t stream,
+                             const uint32_t *order = nullptr) {
     const size_t qfloats = static_cast<size_t>(n) * e->dims;
     int32_t rc = c->d_queries.ensure(qfloats, "query buffer");
     if (!rc) rc = c->h_queries.ensure(qfloats, "query staging");
     if (rc) return rc;
-    memcpy(c->h_queries, queries, qfloats * sizeof(float));
+    if (order) {
+        for (uint32_t j = 0; j < n; ++j)
+            memcpy(c->h_queries + static_cast<size_t>(j) * e->dims, queries + static_cast<size_t>(order[j]) * e->dims,
+                   e->dims * sizeof(float));
+    } else {
+        memcpy(c->h_queries, queries, qfloats * sizeof(float));
+    }
     CUDA_TRY(cudaMemcpyAsync(c->d_queries, c->h_queries, qfloats * sizeof(float), cudaMemcpyHostToDevice, stream));
     return WAX_VS_OK;
 }
@@ -947,6 +962,19 @@ static void record_level1_outcome(wax_vs_engine *e, uint32_t n_queries, size_t u
     }
 }
 
+// ---- row filters of a batch ----
+// Filter f is the bitset bits + f * words (bit set = the row may be returned).  index: each query's filter
+// (WAX_VS_NO_FILTER = none), on the device and the same on the host; nullptr = every query uses `bits` (nullptr = none).
+struct RowFilter {
+    const uint32_t *bits = nullptr;
+    uint32_t words = 0;
+    const uint32_t *d_index = nullptr, *h_index = nullptr;
+    const uint32_t *mask(uint32_t qi) const {
+        if (!h_index) return bits;
+        return h_index[qi] == WAX_VS_NO_FILTER ? nullptr : bits + static_cast<size_t>(h_index[qi]) * words;
+    }
+};
+
 // ---- the tensor-core nomination pass of both levels ----
 // One launch of a pass: queries [q0, q0 + nq) in `groups` query groups, each over `slices` row slices.
 struct NominateChunk {
@@ -963,7 +991,7 @@ struct NominateChunk {
 // or more; dump: the score read-out forms.
 template <typename Heap, typename Prepare, typename Finish>
 static int32_t enqueue_nominate_pass(wax_vs_engine *e, SearchCtx *c, const float *d_queries, uint32_t n_queries, bool bf16,
-                                     bool filter, bool pair, bool dump, uint32_t max_groups, const uint32_t *d_mask,
+                                     bool filter, bool pair, bool dump, uint32_t max_groups, const RowFilter &rf,
                                      cudaStream_t stream, uint64_t *launches, Heap heap, Prepare prepare, Finish finish) {
     int32_t rc;
     // bf16 nominations: convert the queries once per call (n_queries x dims, tiny next to the corpus pass)
@@ -1010,7 +1038,9 @@ static int32_t enqueue_nominate_pass(wax_vs_engine *e, SearchCtx *c, const float
         // the cosine shadow rows are pre-normalised: no epilogue scaling on the bf16 path
         bp.row_scale = (e->similarity == WAX_VS_COSINE && !bf16) ? e->d_inv_norm.p : nullptr;
         bp.half_sq = l2 ? e->d_half_sq.p : nullptr;
-        bp.allow_bits = d_mask;
+        bp.allow_bits = rf.bits;
+        bp.query_filter = rf.d_index ? rf.d_index + ch.q0 : nullptr;     // indexed by the launch's queries
+        bp.filter_words = rf.words;
         if ((rc = prepare(ch, bp))) return rc;
         const uint32_t grid = ch.groups * ch.slices;
         const uint32_t smem = batch_smem_bytes(ch.stages, static_cast<int>(ch.kprime), ch.ares ? num_kb16 : 0u);
@@ -1037,7 +1067,7 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
                                     uint32_t k_eff, uint64_t row_offset, wax_vs_candidate *d_out, uint32_t *d_ok,
                                     const uint64_t *d_ids, cudaStream_t stream, uint64_t *launches,
                                     bool allow_bf16 = true, bool *used_bf16 = nullptr, float *d_tau_star = nullptr,
-                                    const uint32_t *d_mask = nullptr, uint32_t *used_heap = nullptr,
+                                    const RowFilter &rf = RowFilter{}, uint32_t *used_heap = nullptr,
                                     NominationDump *dump = nullptr) {
     int32_t rc = ensure_norms(e, stream);
     if (rc) return rc;
@@ -1104,7 +1134,7 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
         return WAX_VS_OK;
     };
     return enqueue_nominate_pass(e, c, d_queries, n_queries, bf16, false, e->tune.batch_pair != 0, dump != nullptr,
-                                 max_groups, d_mask, stream, launches, heap, prepare, finish);
+                                 max_groups, rf, stream, launches, heap, prepare, finish);
 }
 
 static uint32_t clamp_topk(int64_t k) {  // MetalVectorEngine.swift:842-846
@@ -1637,7 +1667,7 @@ int32_t wax_vs_remove(wax_vs_engine *e, uint64_t frame_id) {
 static int32_t enqueue_filter_level(wax_vs_engine *e, SearchCtx *c, const float *d_queries, const float *d_tau,
                                     uint32_t n_queries, uint32_t k_eff, uint64_t row_offset, wax_vs_candidate *d_out,
                                     uint32_t *d_ok, const uint64_t *d_ids, cudaStream_t stream, uint64_t *launches,
-                                    bool bf16 = false, const uint32_t *d_mask = nullptr) {
+                                    bool bf16 = false, const RowFilter &rf = RowFilter{}) {
     int32_t rc = ensure_norms(e, stream);
     if (rc) return rc;
     uint32_t cap = 64;                      // a power of two in [64, 16384], at least k
@@ -1674,19 +1704,20 @@ static int32_t enqueue_filter_level(wax_vs_engine *e, SearchCtx *c, const float 
         return WAX_VS_OK;
     };
     return enqueue_nominate_pass(e, c, d_queries, n_queries, bf16, true, false, false, static_cast<uint32_t>(e->sm_count),
-                                 d_mask, stream, launches, [](uint32_t, uint32_t) { return 16u; }, prepare, finish);
+                                 rf, stream, launches, [](uint32_t, uint32_t) { return 16u; }, prepare, finish);
 }
 
 // ---- search ---------------------------------------------------------------------------------------------------
 // The exact scan for n queries, one enqueue_search each on `stream`: query i (qs[i] when a list is given) reads
-// d_queries[i] and writes d_out[i].  sync_on_error: drain the stream before a failure is returned.
+// d_queries[i], writes d_out[i] and consults its own row filter.  sync_on_error: drain the stream before a failure is
+// returned.
 static int32_t enqueue_scans(wax_vs_engine *e, SearchCtx *c, const float *d_queries, uint32_t n, const uint32_t *qs,
                              uint32_t k_eff, uint64_t row_offset, wax_vs_candidate *d_out, const uint64_t *d_ids,
-                             cudaStream_t stream, uint64_t *launches, const uint32_t *d_mask, bool sync_on_error) {
+                             cudaStream_t stream, uint64_t *launches, const RowFilter &rf, bool sync_on_error) {
     for (uint32_t i = 0; i < n; ++i) {
         const uint32_t qi = qs ? qs[i] : i;
         const int32_t rc = enqueue_search(e, c, d_queries + static_cast<size_t>(qi) * e->dims, k_eff, row_offset,
-                                          d_out + static_cast<size_t>(qi) * k_eff, d_ids, stream, launches, d_mask);
+                                          d_out + static_cast<size_t>(qi) * k_eff, d_ids, stream, launches, rf.mask(qi));
         if (rc) {
             if (sync_on_error) cudaStreamSynchronize(stream);
             return rc;
@@ -1697,10 +1728,11 @@ static int32_t enqueue_scans(wax_vs_engine *e, SearchCtx *c, const float *d_quer
 
 // n_queries device-resident queries -> d_out[n_queries][k_eff] on c->stream: the tensor-core levels (bf16 shadow ->
 // TF32 retry -> exact scan, DESIGN 4.5.1) when the batch is eligible, else one fused scan per query.  The tensor
-// levels read their proof flags back, so they synchronise c->stream; the scan loop only enqueues.
+// levels read their proof flags back, so they synchronise c->stream; the scan loop only enqueues.  rf: the queries' row
+// filters (every level consults each query's own bitset, so the proof is a statement about its ALLOWED rows).
 static int32_t run_queries_on_device(wax_vs_engine *e, SearchCtx *c, const float *d_queries, uint32_t n_queries,
                                      uint32_t k_eff, uint64_t row_offset, wax_vs_candidate *d_out, const uint64_t *d_ids,
-                                     uint64_t *launches, const uint32_t *d_mask = nullptr) {
+                                     uint64_t *launches, const RowFilter &rf = RowFilter{}) {
     int32_t rc = WAX_VS_OK;
     bool tensor_path = batch_tensor_eligible(e, n_queries, k_eff), allow_bf16 = true;
     if (tensor_path) {
@@ -1710,7 +1742,7 @@ static int32_t run_queries_on_device(wax_vs_engine *e, SearchCtx *c, const float
     // below batch_min the tensor path only pays off through the bf16 shadow (single_shadow): never TF32 for one query
     if (tensor_path && !allow_bf16 && n_queries < static_cast<uint32_t>(std::max(e->tune.batch_min, 1))) tensor_path = false;
     if (!tensor_path)
-        return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_out, d_ids, c->stream, launches, d_mask, true);
+        return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_out, d_ids, c->stream, launches, rf, true);
     // Batched: one tensor-core pass over the corpus nominates, the finish kernel re-scores exactly and
     // proves completeness; unproven queries (rare) are re-run on the exact single-query path below.
     if ((rc = c->d_ok.ensure(static_cast<size_t>(n_queries), "proof flags"))) return rc;
@@ -1720,7 +1752,7 @@ static int32_t run_queries_on_device(wax_vs_engine *e, SearchCtx *c, const float
     bool used_bf16 = false;
     uint32_t used_heap = 0;
     rc = enqueue_batch_tensor(e, c, d_queries, n_queries, k_eff, row_offset, d_out, c->d_ok, d_ids, c->stream, launches,
-                              allow_bf16, &used_bf16, c->d_tau_star, d_mask, &used_heap);
+                              allow_bf16, &used_bf16, c->d_tau_star, rf, &used_heap);
     if (rc) { cudaStreamSynchronize(c->stream); return rc; }
     CUDA_TRY(cudaMemcpyAsync(c->h_ok, c->d_ok, n_queries * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(cudaMemcpyAsync(c->h_tau_star, c->d_tau_star, 2 * n_queries * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
@@ -1749,8 +1781,20 @@ static int32_t run_queries_on_device(wax_vs_engine *e, SearchCtx *c, const float
             CUDA_TRY(cudaMemcpyAsync(c->d_retry_q + static_cast<size_t>(i) * e->dims,
                                      d_queries + static_cast<size_t>(todo[i]) * e->dims, e->dims * sizeof(float),
                                      cudaMemcpyDeviceToDevice, c->stream));
+        // per-query filters: the compacted queries keep their bitsets, in the same order
+        RowFilter frf = rf;
+        std::vector<uint32_t> retry_index;
+        if (rf.h_index) {
+            retry_index.resize(nf);
+            for (uint32_t i = 0; i < nf; ++i) retry_index[i] = rf.h_index[todo[i]];
+            if ((frc = c->d_retry_filter.ensure(nf, "filter-level filter indices"))) return frc;
+            CUDA_TRY(cudaMemcpyAsync(c->d_retry_filter, retry_index.data(), nf * sizeof(uint32_t), cudaMemcpyHostToDevice,
+                                     c->stream));
+            frf.d_index = c->d_retry_filter;
+            frf.h_index = retry_index.data();
+        }
         frc = enqueue_filter_level(e, c, c->d_retry_q, c->d_filter_tau, nf, k_eff, row_offset, c->d_retry_out,
-                                   c->d_retry_ok, d_ids, c->stream, launches, bf16lvl, d_mask);
+                                   c->d_retry_ok, d_ids, c->stream, launches, bf16lvl, frf);
         if (frc) { cudaStreamSynchronize(c->stream); return frc; }
         CUDA_TRY(cudaMemcpyAsync(c->h_ok, c->d_retry_ok, nf * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -1783,7 +1827,7 @@ static int32_t run_queries_on_device(wax_vs_engine *e, SearchCtx *c, const float
         unproven.swap(rest);
     }
     if ((rc = enqueue_scans(e, c, d_queries, static_cast<uint32_t>(unproven.size()), unproven.data(), k_eff, row_offset,
-                            d_out, d_ids, c->stream, launches, d_mask, true)))
+                            d_out, d_ids, c->stream, launches, rf, true)))
         return rc;
     std::lock_guard<std::mutex> pg(e->pool_mu);
     e->batch_tensor_queries += n_queries - unproven.size();
@@ -1796,13 +1840,17 @@ static int32_t run_queries_on_device(wax_vs_engine *e, SearchCtx *c, const float
 }
 
 // n_queries x k_eff candidates -> frame ids and scores, query qi's at qi * out_stride; out_n[qi] = how many were valid.
-// row -> frameId and distance -> score on the host, as MetalVectorEngine.swift:595-603 does.
+// row -> frameId and distance -> score on the host, as MetalVectorEngine.swift:595-603 does.  Optional: order[j] = the
+// query candidate list j belongs to, k_of[j] = how many of its k_eff slots were written.
 static void deliver_results(const wax_vs_engine *e, const wax_vs_candidate *cands, uint32_t n_queries, uint32_t k_eff,
-                            uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    for (uint32_t qi = 0; qi < n_queries; ++qi) {
+                            uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n,
+                            const uint32_t *order = nullptr, const uint32_t *k_of = nullptr) {
+    for (uint32_t j = 0; j < n_queries; ++j) {
+        const uint32_t qi = order ? order[j] : j;
+        const uint32_t kq = k_of ? k_of[j] : k_eff;
         uint32_t m = 0;
-        for (uint32_t i = 0; i < k_eff; ++i) {
-            const wax_vs_candidate &cd = cands[static_cast<size_t>(qi) * k_eff + i];
+        for (uint32_t i = 0; i < kq; ++i) {
+            const wax_vs_candidate &cd = cands[static_cast<size_t>(j) * k_eff + i];
             if (!cd.valid) continue;
             out_ids[static_cast<size_t>(qi) * out_stride + m] = e->ids_identity ? e->id_base + cd.row : e->ids[cd.row];
             out_scores[static_cast<size_t>(qi) * out_stride + m] = score_from_distance(e->similarity, cd.distance);
@@ -1899,7 +1947,7 @@ int32_t wax_vs_search_device(wax_vs_engine *e, const float *d_queries, uint32_t 
     if ((rc = sync_device_ids(e, &d_ids))) return rc;
     uint64_t launches = 0;
     return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_candidates, d_ids,
-                         static_cast<cudaStream_t>(cuda_stream), &launches, nullptr, false);
+                         static_cast<cudaStream_t>(cuda_stream), &launches, RowFilter{}, false);
 }
 
 // Batched form of wax_vs_search_device: the tensor-core levels on the caller's stream for the rank's shard.  Unlike
@@ -1922,7 +1970,7 @@ int32_t wax_vs_search_batch_device(wax_vs_engine *e, const float *d_queries, uin
     uint64_t launches = 0;
     if (k_eff > e->n_rows)     // a shard smaller than k: the scan pads with invalid candidates, the tensor path does not
         return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_candidates, d_ids, c->stream,
-                             &launches, nullptr, false);
+                             &launches, RowFilter{}, false);
     return run_queries_on_device(e, c, d_queries, n_queries, k_eff, row_offset, d_candidates, d_ids, &launches);
 }
 
@@ -2096,33 +2144,42 @@ static int32_t shard_wait_host(wax_vs_engine *e, unsigned long long seq) {
     return rc;
 }
 
+static int32_t build_filter_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<uint64_t> &spec, uint32_t n_filters,
+                                 cudaStream_t stream, uint64_t *launches);
+
 // The host-path collective search of both entry points (caller: read lock, device selected, arguments checked): the
-// rank's fused scan, with the row bitset `*bits` below the top-k when the filtered form passes a non-empty one, the
-// in-kernel exchange and merge, and the merged list delivered into mapped host memory.
-static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t k_eff, const std::vector<uint32_t> *bits,
-                                 uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n) {
+// rank's fused scan, with the row filter `*rows` (the distinct rows the filtered form's ids resolved to, mode 0 allow /
+// 1 deny) below the top-k, the in-kernel exchange and merge, and the merged list delivered into mapped host memory.
+static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t k_eff, const std::vector<uint32_t> *rows,
+                                 int32_t mode, uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n) {
     auto &sh = e->shard;
     std::lock_guard<std::mutex> sg(sh.mu);      // one host-path collective at a time: it owns sh.ctx and h_final
     SearchCtx *c = sh.ctx;
     int32_t rc;
     const uint64_t *d_ids = nullptr;
     if ((rc = sync_device_ids(e, &d_ids))) return rc;
-    const bool masked = bits && !bits->empty();
-    if (masked) {
-        if ((rc = c->d_mask.ensure(bits->size(), "row filter"))) return rc;
-        CUDA_TRY(cudaMemcpyAsync(c->d_mask, bits->data(), bits->size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    uint64_t launches = 0;
+    const bool masked = rows && e->n_rows;
+    if (masked) {       // one bitset, built on the device from the resolved rows
+        // sized for every row of the shard (a bound on any filter's distinct rows), so that a later call never
+        // reallocates: cudaFree waits for the device, where the peers' scans may already wait for this rank
+        if ((rc = c->d_filter_rows.ensure(std::max<size_t>(e->n_rows, 1), "filter rows"))) return rc;
+        if (!rows->empty())
+            CUDA_TRY(cudaMemcpyAsync(c->d_filter_rows, rows->data(), rows->size() * sizeof(uint32_t), cudaMemcpyHostToDevice,
+                                     c->stream));
+        const std::vector<uint64_t> spec = {0, rows->size(), 0, static_cast<uint64_t>(mode)};
+        if ((rc = build_filter_bits(e, c, spec, 1, c->stream, &launches))) return rc;
     }
     ShardParams sp = shard_params_next(e);
     sp.host_out = sh.h_final; sp.host_flag = sh.h_flag;      // mapped pinned: the kernel delivers the result itself
     HostDelivery hd{query, nullptr, nullptr, 0};             // the query rides in the kernel parameters when it fits
-    uint64_t launches = 0;
     if ((rc = enqueue_search(e, c, nullptr, k_eff, sh.row_offset, sh.d_final, d_ids, c->stream, &launches,
                              masked ? c->d_mask.p : nullptr, &sp, &hd))) {
         cudaStreamSynchronize(c->stream);
         return rc;
     }
     if ((rc = shard_wait_host(e, sp.seq))) { cudaStreamSynchronize(c->stream); return rc; }
-    if (bits) CUDA_TRY(cudaStreamSynchronize(c->stream));   // `bits` must outlive its upload
+    if (masked) CUDA_TRY(cudaStreamSynchronize(c->stream));   // `rows` must outlive its upload
     uint32_t m = 0;
     for (uint32_t i = 0; i < k_eff; ++i) {
         const wax_vs_candidate &cd = sh.h_final[i];
@@ -2151,7 +2208,7 @@ int32_t wax_vs_shard_search(wax_vs_engine *e, const float *query, uint32_t query
     if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
     DeviceGuard g(e->device);
     if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    return shard_search_host(e, query, k_eff, nullptr, out_ids, out_scores, out_cap, out_n);
+    return shard_search_host(e, query, k_eff, nullptr, 0, out_ids, out_scores, out_cap, out_n);
 }
 
 // Device-timed sharded searches, strictly one query at a time on one stream (the same mode as wax_vs_debug_time_search):
@@ -2209,14 +2266,13 @@ int32_t wax_vs_merge_candidates_device(wax_vs_engine *e, const wax_vs_candidate 
 // The reference filters AFTER the engine call and over-fetches 3 x topK to compensate (UnifiedSearch.swift:58,
 // 371-442, 1195-1200, 1241-1258).  Here the filter is pushed below the top-k: a row bitset consulted only for rows
 // that would enter the list, or -- for small allow-lists -- a gather that scores only the listed rows.
-// frameIds -> rows of this engine (unknown ids are ignored), as a bitset (bit set = the row may be returned) and as the
-// list of rows the ids named.  Returns the number of rows that may be returned.
-static uint64_t build_row_filter(wax_vs_engine *e, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
-                                 std::vector<uint32_t> &bits, std::vector<uint32_t> &listed) {
+// frameIds -> the distinct rows of this engine they name, appended to `rows` (unknown and repeated ids are ignored).
+// `seen` is a zeroed scratch bitset of ceil(N / 32) words shared by all the filters of a call: only the words this
+// filter touched are cleared again, so no list is sorted and no bitset is rebuilt per filter.  Returns the rows appended.
+static uint64_t build_row_filter(wax_vs_engine *e, const uint64_t *frame_ids, uint64_t n_ids, std::vector<uint32_t> &seen,
+                                 std::vector<uint32_t> &rows) {
     const uint64_t n_rows = e->n_rows;
-    bits.assign((n_rows + 31) / 32, mode == 0 ? 0u : 0xFFFFFFFFu);
-    if (mode == 1 && (n_rows & 31u)) bits.back() = (1u << (n_rows & 31u)) - 1u;
-    listed.clear();
+    const size_t first = rows.size();
     std::lock_guard<std::mutex> g(e->ids_mu);   // the lazily built id map is shared by concurrent readers
     // (find_row builds the lazily constructed hash table when it is needed: serialised by ids_mu)
     for (uint64_t i = 0; i < n_ids; ++i) {
@@ -2230,22 +2286,69 @@ static uint64_t build_row_filter(wax_vs_engine *e, const uint64_t *frame_ids, ui
             row = f;
         }
         const uint32_t w = static_cast<uint32_t>(row >> 5), b = 1u << (row & 31u);
-        if (mode == 0) { if (!(bits[w] & b)) { bits[w] |= b; listed.push_back(static_cast<uint32_t>(row)); } }
-        else if (bits[w] & b) { bits[w] &= ~b; listed.push_back(static_cast<uint32_t>(row)); }
+        if (!(seen[w] & b)) { seen[w] |= b; rows.push_back(static_cast<uint32_t>(row)); }
     }
-    return mode == 0 ? listed.size() : n_rows - listed.size();
+    for (size_t i = first; i < rows.size(); ++i) seen[rows[i] >> 5] = 0u;
+    return rows.size() - first;
 }
 
-// One filter, n_queries queries.  Small allow-lists: gather + exact score of the listed rows only (grid.y = query), one
-// CTA per query sorts.  Otherwise the row bitset rides below the top-k: in the fused scan (one query, or a batch the
-// tensor path cannot take) or in the tensor-core levels (nominations, filter level and the exact fall-back all consult
-// the same bitset, so the completeness proof is a statement about the ALLOWED rows).
+// n_filters row bitsets of ceil(N / 32) words into c->d_mask on `stream`, from the resolved rows in c->d_filter_rows:
+// spec is filter_bits_init_kernel's (running row counts, where each filter's rows start, modes).  The host uploads
+// 4 bytes per listed row instead of N / 8 bytes per filter.  c->d_mask must not be reallocated while earlier
+// launches on `stream` still read it: callers size it first.
+static int32_t build_filter_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<uint64_t> &spec, uint32_t n_filters,
+                                 cudaStream_t stream, uint64_t *launches) {
+    const uint32_t words = static_cast<uint32_t>((e->n_rows + 31) / 32);
+    int32_t rc;
+    if ((rc = c->d_filter_spec.ensure(spec.size(), "filter spec"))) return rc;
+    if ((rc = c->d_mask.ensure(static_cast<size_t>(n_filters) * words, "row filters"))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_filter_spec, spec.data(), spec.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, stream));
+    const size_t total_words = static_cast<size_t>(n_filters) * words;
+    const int cap = e->sm_count * 8;
+    const int g1 = static_cast<int>(std::min<size_t>(cap, (total_words + 255) / 256));
+    filter_bits_init_kernel<<<std::max(g1, 1), 256, 0, stream>>>(c->d_mask, words, static_cast<uint32_t>(e->n_rows),
+                                                                 c->d_filter_spec, n_filters);
+    CUDA_TRY(cudaGetLastError());
+    ++*launches;
+    const uint64_t listed = spec[n_filters];
+    if (listed) {
+        const int g2 = static_cast<int>(std::min<uint64_t>(cap, (listed + 255) / 256));
+        filter_bits_apply_kernel<<<g2, 256, 0, stream>>>(c->d_mask, words, c->d_filter_rows, c->d_filter_spec, n_filters);
+        CUDA_TRY(cudaGetLastError());
+        ++*launches;
+    }
+    return WAX_VS_OK;
+}
+
+// n_queries queries, query i under filter query_filter[i] (WAX_VS_NO_FILTER: unfiltered); the single-filter entry
+// points are the case of one filter that every query names.  Every query referenced filter is resolved once; query i
+// asks for k_i = min(clamp(top_k), allowed_i) rows and falls in one of three classes:
+//  - gather: an allow-list of <= 16 384 rows -- exact scores of the listed rows only, all such queries in one batched
+//    gather over the concatenated lists, one CTA per query sorts;
+//  - tensor: allowed_i >= clamp(top_k), so the class shares one k -- run_queries_on_device with a bitset per query (the
+//    tensor-core levels, whose nominations, filter level and exact fall-back all consult the query's own bitset, so the
+//    completeness proof is a statement about ITS allowed rows; or one masked fused scan per query);
+//  - scan: the rest (deny-lists that leave fewer than k rows, an unfiltered query on a corpus below k), one masked fused
+//    scan each with its own k_i.
+// The bitsets are built on the device; a pass holds at most filter_bitset_bytes of them, more filters run in several
+// sub-batches (queries sorted by filter, so each filter's bitset is built once).
 static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                    int64_t top_k, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                                    int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                    const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
                                     uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
-    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    if (!e || !out_n || !filter_offsets || (n_filters && !filter_modes) || (n_queries && !query_filter))
+        return fail(WAX_VS_ERR_NULL, "NULL argument");
+    for (uint32_t f = 0; f < n_filters; ++f)
+        if (filter_modes[f] != 0 && filter_modes[f] != 1)
+            return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
+    if (filter_offsets[0] != 0) return fail(WAX_VS_ERR_ARGUMENT, "filter_offsets[0] must be 0");
+    for (uint32_t f = 0; f < n_filters; ++f)
+        if (filter_offsets[f + 1] < filter_offsets[f])
+            return fail(WAX_VS_ERR_ARGUMENT, "filter_offsets decrease at filter %u", f);
+    if (filter_offsets[n_filters] && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    for (uint32_t i = 0; i < n_queries; ++i)
+        if (query_filter[i] != WAX_VS_NO_FILTER && query_filter[i] >= n_filters)
+            return fail(WAX_VS_ERR_ARGUMENT, "query %u names filter %u of %u", i, query_filter[i], n_filters);
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
     if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
@@ -2253,12 +2356,50 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
     if (query_len != e->dims)
         return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
 
-    std::vector<uint32_t> bits, listed;
-    const uint64_t allowed = build_row_filter(e, frame_ids, n_ids, mode, bits, listed);
-    const uint32_t k_eff = static_cast<uint32_t>(std::min<uint64_t>(clamp_topk(top_k), allowed));
-    if (k_eff == 0) return WAX_VS_OK;
+    // (1) resolve each referenced filter once: filter f's distinct rows are rows[first[f] .. first[f] + count[f])
+    const uint64_t n_rows = e->n_rows;
+    const uint32_t words = static_cast<uint32_t>((n_rows + 31) / 32);
+    std::vector<uint64_t> first(n_filters, 0), count(n_filters, 0);
+    std::vector<uint8_t> referenced(n_filters, 0);
+    for (uint32_t i = 0; i < n_queries; ++i)
+        if (query_filter[i] != WAX_VS_NO_FILTER) referenced[query_filter[i]] = 1;
+    std::vector<uint32_t> rows, seen(words, 0u);
+    for (uint32_t f = 0; f < n_filters; ++f) {
+        if (!referenced[f]) continue;
+        first[f] = rows.size();
+        count[f] = build_row_filter(e, frame_ids + filter_offsets[f], filter_offsets[f + 1] - filter_offsets[f], seen, rows);
+    }
+    // (2) each query's k, (3) its class
+    const uint32_t limit = clamp_topk(top_k);
+    std::vector<uint32_t> tensor, gather, scan;                // query indices
+    std::vector<uint32_t> k_of_query(n_queries, 0);
+    uint32_t k_max = 0;
+    for (uint32_t i = 0; i < n_queries; ++i) {
+        const uint32_t f = query_filter[i];
+        const uint64_t allowed = f == WAX_VS_NO_FILTER ? n_rows : (filter_modes[f] == 0 ? count[f] : n_rows - count[f]);
+        const uint32_t k = static_cast<uint32_t>(std::min<uint64_t>(limit, allowed));
+        if (k == 0) continue;
+        k_of_query[i] = k;
+        k_max = std::max(k_max, k);
+        if (f != WAX_VS_NO_FILTER && filter_modes[f] == 0 && count[f] <= 16384) gather.push_back(i);
+        else if (allowed >= limit) tensor.push_back(i);
+        else scan.push_back(i);
+    }
+    if (k_max == 0) return WAX_VS_OK;
     if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
-    if (out_stride < k_eff) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, k_eff);
+    if (out_stride < k_max) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, k_max);
+    // staged order: the tensor class, the gather class, the scan class; the first and last sorted by filter so that a
+    // sub-batch names a run of consecutive filters (unfiltered queries last)
+    auto by_filter = [&](uint32_t a, uint32_t b) { return query_filter[a] < query_filter[b]; };
+    std::stable_sort(tensor.begin(), tensor.end(), by_filter);
+    std::stable_sort(scan.begin(), scan.end(), by_filter);
+    std::vector<uint32_t> order(tensor);
+    order.insert(order.end(), gather.begin(), gather.end());
+    order.insert(order.end(), scan.begin(), scan.end());
+    const uint32_t n_staged = static_cast<uint32_t>(order.size());
+    const uint32_t n_tensor = static_cast<uint32_t>(tensor.size()), n_gather = static_cast<uint32_t>(gather.size());
+    std::vector<uint32_t> k_of(n_staged);
+    for (uint32_t j = 0; j < n_staged; ++j) k_of[j] = k_of_query[order[j]];
 
     DeviceGuard g(e->device);
     if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
@@ -2266,67 +2407,142 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
     int32_t rc = lease.acquire();
     if (rc) return rc;
     SearchCtx *c = lease.c;
-    const size_t ncand = static_cast<size_t>(n_queries) * k_eff;
-    if ((rc = stage_queries(e, c, queries, n_queries, c->stream))) return rc;
+    const size_t ncand = static_cast<size_t>(n_staged) * k_max;       // staged query j's candidates at j * k_max
+    if ((rc = stage_queries(e, c, queries, n_staged, c->stream, order.data()))) return rc;
     if ((rc = c->d_out.ensure(ncand, "result buffer"))) return rc;
     if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
-
+    if ((rc = c->d_filter_rows.ensure(std::max<size_t>(rows.size(), 1), "filter rows"))) return rc;
+    if (!rows.empty())
+        CUDA_TRY(cudaMemcpyAsync(c->d_filter_rows, rows.data(), rows.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
     uint64_t launches = 0;
-    if (mode == 0 && listed.size() <= 16384) {
-        // small allow-list: gather + exact score of the listed rows only, then one-CTA sorts
-        std::sort(listed.begin(), listed.end());
-        const uint32_t n = static_cast<uint32_t>(listed.size());
-        if ((rc = c->d_mask.ensure(static_cast<size_t>(std::max<uint32_t>(n, 1)), "listed rows"))) return rc;
-        if ((rc = c->d_gather_keys.ensure(static_cast<size_t>(std::max<uint32_t>(n, 1)) * n_queries, "gather keys"))) return rc;
-        CUDA_TRY(cudaMemcpyAsync(c->d_mask, listed.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+
+    // gather class: one concatenated row list, a span per query; the sort grants shared memory for the longest list
+    if (n_gather) {
+        std::vector<uint2> spans(n_gather);
+        uint32_t longest = 1;
+        for (uint32_t j = 0; j < n_gather; ++j) {
+            const uint32_t f = query_filter[order[n_tensor + j]];
+            spans[j] = make_uint2(static_cast<uint32_t>(first[f]), static_cast<uint32_t>(count[f]));
+            longest = std::max(longest, spans[j].y);
+        }
+        if ((rc = c->d_gather_span.ensure(n_gather, "gather spans"))) return rc;
+        if ((rc = c->d_gather_keys.ensure(static_cast<size_t>(longest) * n_gather, "gather keys"))) return rc;
+        CUDA_TRY(cudaMemcpyAsync(c->d_gather_span, spans.data(), n_gather * sizeof(uint2), cudaMemcpyHostToDevice, c->stream));
         uint32_t pow2 = 64;
-        while (pow2 < n) pow2 <<= 1;
+        while (pow2 < longest) pow2 <<= 1;
         CUDA_TRY(grant_smem(e, gather_sort_kernel, pow2 * sizeof(uint64_t)));
-        const uint32_t gx = std::max<uint32_t>(1, std::min<uint32_t>((n + 31) / 32, static_cast<uint32_t>(e->sm_count) * 8));
-        for (uint32_t q0 = 0; q0 < n_queries; q0 += 32768u) {       // grid.y limit
-            const uint32_t nq = std::min<uint32_t>(n_queries - q0, 32768u);
+        const uint32_t gx = std::max<uint32_t>(1, std::min<uint32_t>((longest + 31) / 32, static_cast<uint32_t>(e->sm_count) * 8));
+        for (uint32_t q0 = 0; q0 < n_gather; q0 += 32768u) {       // grid.y limit
+            const uint32_t nq = std::min<uint32_t>(n_gather - q0, 32768u);
             const dim3 ggrid(gx, nq);
-            const float *dq = c->d_queries + static_cast<size_t>(q0) * e->dims;
-            uint64_t *keys = c->d_gather_keys + static_cast<size_t>(q0) * n;
+            const float *dq = c->d_queries + static_cast<size_t>(n_tensor + q0) * e->dims;
+            const uint2 *span = c->d_gather_span + q0;
+            uint64_t *keys = c->d_gather_keys + static_cast<size_t>(q0) * longest;
             switch (e->similarity) {
-                case WAX_VS_COSINE: gather_score_kernel<kCosine><<<ggrid, 256, 0, c->stream>>>(e->d_corpus, dq, e->dims, c->d_mask, n, keys); break;
-                case WAX_VS_DOT: gather_score_kernel<kDot><<<ggrid, 256, 0, c->stream>>>(e->d_corpus, dq, e->dims, c->d_mask, n, keys); break;
-                default: gather_score_kernel<kL2><<<ggrid, 256, 0, c->stream>>>(e->d_corpus, dq, e->dims, c->d_mask, n, keys); break;
+                case WAX_VS_COSINE: gather_score_kernel<kCosine><<<ggrid, 256, 0, c->stream>>>(e->d_corpus, dq, e->dims, c->d_filter_rows, span, longest, keys); break;
+                case WAX_VS_DOT: gather_score_kernel<kDot><<<ggrid, 256, 0, c->stream>>>(e->d_corpus, dq, e->dims, c->d_filter_rows, span, longest, keys); break;
+                default: gather_score_kernel<kL2><<<ggrid, 256, 0, c->stream>>>(e->d_corpus, dq, e->dims, c->d_filter_rows, span, longest, keys); break;
             }
             CUDA_TRY(cudaGetLastError());
             ScanParams sp{};
-            sp.k = k_eff; sp.out = c->d_out + static_cast<size_t>(q0) * k_eff; sp.id_base = e->id_base;
-            gather_sort_kernel<<<nq, 1024, pow2 * sizeof(uint64_t), c->stream>>>(keys, n, pow2, sp);
+            sp.k = k_max; sp.out = c->d_out + static_cast<size_t>(n_tensor + q0) * k_max; sp.id_base = e->id_base;
+            gather_sort_kernel<<<nq, 1024, pow2 * sizeof(uint64_t), c->stream>>>(keys, span, longest, pow2, sp);
             CUDA_TRY(cudaGetLastError());
             launches += 2;
         }
-    } else {
-        if ((rc = c->d_mask.ensure(bits.size(), "row filter"))) return rc;
-        CUDA_TRY(cudaMemcpyAsync(c->d_mask, bits.data(), bits.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-        if (n_queries == 1) {
-            rc = enqueue_search(e, c, c->d_queries, k_eff, 0, c->d_out, nullptr, c->stream, &launches, c->d_mask);
-            if (rc) { cudaStreamSynchronize(c->stream); return rc; }
-        } else if ((rc = run_queries_on_device(e, c, c->d_queries, n_queries, k_eff, 0, c->d_out, nullptr, &launches, c->d_mask))) {
-            return rc;
+    }
+
+    // tensor and scan classes: sub-batches whose bitsets fit the budget (at least one always does)
+    const uint64_t fit = std::max<uint64_t>(1, e->tune.filter_bitset_bytes / (static_cast<uint64_t>(words) * sizeof(uint32_t)));
+    uint64_t distinct = 0;
+    for (uint32_t f = 0; f < n_filters; ++f) distinct += referenced[f];
+    const uint32_t per_pass = static_cast<uint32_t>(std::min<uint64_t>(fit, std::max<uint64_t>(distinct, 1)));
+    // sized once for the largest pass: a later pass must not reallocate a buffer earlier launches still read
+    if ((rc = c->d_mask.ensure(static_cast<size_t>(per_pass) * words, "row filters"))) return rc;
+    if ((rc = c->d_filter_spec.ensure(3u * per_pass + 1u, "filter spec"))) return rc;
+    if ((rc = c->d_query_filter.ensure(std::max<uint32_t>(n_tensor, 1), "query filters"))) return rc;
+    std::vector<uint32_t> index(n_staged, WAX_VS_NO_FILTER);           // staged query -> bitset of its pass
+    uint64_t passes = 0;
+    auto run_class = [&](uint32_t j0, uint32_t j1, bool tensor_class) -> int32_t {
+        for (uint32_t s0 = j0; s0 < j1;) {
+            std::vector<uint32_t> which;                                // the pass's filters, in bitset order
+            uint32_t s1 = s0;
+            for (; s1 < j1; ++s1) {
+                const uint32_t f = query_filter[order[s1]];
+                if (f != WAX_VS_NO_FILTER && (which.empty() || which.back() != f)) {
+                    if (which.size() == per_pass) break;
+                    which.push_back(f);
+                }
+                index[s1] = f == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : static_cast<uint32_t>(which.size() - 1);
+            }
+            int32_t prc;
+            if (!which.empty()) {
+                const uint32_t nf = static_cast<uint32_t>(which.size());
+                std::vector<uint64_t> spec(3u * nf + 1u, 0);
+                for (uint32_t l = 0; l < nf; ++l) {
+                    spec[l + 1] = spec[l] + count[which[l]];
+                    spec[nf + 1 + l] = first[which[l]];
+                    spec[2u * nf + 1u + l] = static_cast<uint64_t>(filter_modes[which[l]]);
+                }
+                if ((prc = build_filter_bits(e, c, spec, nf, c->stream, &launches))) { cudaStreamSynchronize(c->stream); return prc; }
+            }
+            RowFilter rf{c->d_mask.p, words, nullptr, index.data() + s0};
+            const uint32_t nq = s1 - s0;
+            const float *dq = c->d_queries + static_cast<size_t>(s0) * e->dims;
+            wax_vs_candidate *dout = c->d_out + static_cast<size_t>(s0) * k_max;
+            if (tensor_class && nq > 1) {
+                CUDA_TRY(cudaMemcpyAsync(c->d_query_filter + s0, index.data() + s0, nq * sizeof(uint32_t), cudaMemcpyHostToDevice,
+                                         c->stream));
+                rf.d_index = c->d_query_filter + s0;
+                if ((prc = run_queries_on_device(e, c, dq, nq, k_max, 0, dout, nullptr, &launches, rf))) return prc;
+            } else {
+                for (uint32_t j = 0; j < nq; ++j) {
+                    prc = enqueue_search(e, c, dq + static_cast<size_t>(j) * e->dims, k_of[s0 + j], 0,
+                                         dout + static_cast<size_t>(j) * k_max, nullptr, c->stream, &launches, rf.mask(j));
+                    if (prc) { cudaStreamSynchronize(c->stream); return prc; }
+                }
+            }
+            if (tensor_class) ++passes;
+            s0 = s1;
         }
+        return WAX_VS_OK;
+    };
+    if ((rc = run_class(0, n_tensor, true))) return rc;
+    if ((rc = run_class(n_tensor + n_gather, n_staged, false))) return rc;
+    if (passes) {
+        std::lock_guard<std::mutex> pg(e->pool_mu);
+        e->filter_bitset_passes += passes;
     }
     CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, ncand * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(cudaStreamSynchronize(c->stream));   // also keeps `bits` / `listed` alive until the copies are done
-    deliver_results(e, c->h_out, n_queries, k_eff, out_ids, out_scores, out_stride, out_n);
+    CUDA_TRY(cudaStreamSynchronize(c->stream));   // also keeps the host arrays alive until their copies are done
+    deliver_results(e, c->h_out, n_staged, k_max, out_ids, out_scores, out_stride, out_n, order.data(), k_of.data());
     return WAX_VS_OK;
 }
 
 int32_t wax_vs_search_filtered(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k,
                                const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids,
                                float *out_scores, uint32_t out_cap, uint32_t *out_n) {
-    return search_filtered_host(e, query, 1, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores, out_cap, out_n);
+    const uint64_t offsets[2] = {0, n_ids};
+    const uint32_t query_filter = 0;
+    return search_filtered_host(e, query, 1, query_len, top_k, frame_ids, offsets, &mode, 1, &query_filter, out_ids,
+                                out_scores, out_cap, out_n);
 }
 
 int32_t wax_vs_search_batch_filtered(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                      int64_t top_k, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
                                      uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    return search_filtered_host(e, queries, n_queries, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores,
-                                out_stride, out_n);
+    const uint64_t offsets[2] = {0, n_ids};
+    const std::vector<uint32_t> query_filter(n_queries, 0u);
+    return search_filtered_host(e, queries, n_queries, query_len, top_k, frame_ids, offsets, &mode, 1, query_filter.data(),
+                                out_ids, out_scores, out_stride, out_n);
+}
+
+int32_t wax_vs_search_batch_multi_filtered(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                           int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                           const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                           uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    return search_filtered_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
+                                query_filter, out_ids, out_scores, out_stride, out_n);
 }
 
 // The row-sharded form: every rank passes the SAME ids; a rank resolves the ones its shard holds (the others are
@@ -2350,9 +2566,12 @@ int32_t wax_vs_shard_search_filtered(wax_vs_engine *e, const float *query, uint3
     if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
     DeviceGuard g(e->device);
     if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    std::vector<uint32_t> bits, listed;
-    if (e->n_rows) build_row_filter(e, frame_ids, n_ids, mode, bits, listed);
-    return shard_search_host(e, query, k_eff, &bits, out_ids, out_scores, out_cap, out_n);
+    std::vector<uint32_t> rows;
+    if (e->n_rows) {
+        std::vector<uint32_t> seen(static_cast<size_t>((e->n_rows + 31) / 32), 0u);
+        build_row_filter(e, frame_ids, n_ids, seen, rows);
+    }
+    return shard_search_host(e, query, k_eff, &rows, mode, out_ids, out_scores, out_cap, out_n);
 }
 
 // ---- persistence ---------------------------------------------------------------------------------------------
@@ -2664,6 +2883,7 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "shadow_capacity_bytes")) *out = e->d_shadow.cap * sizeof(__nv_bfloat16);                          // HBM held
     else if (!strcmp(name, "shadow_unavailable")) *out = e->shadow_unavailable ? 1 : 0;   // bf16 shadow did not fit: TF32 level runs
     else if (!strcmp(name, "batch_tf32_queries")) *out = e->batch_tf32_queries;
+    else if (!strcmp(name, "filter_bitset_passes")) *out = e->filter_bitset_passes;   // per-query filters: tensor sub-batches
     else if (!strcmp(name, "ingest_h2d_bytes")) *out = e->ingest_h2d_bytes;
     else if (!strcmp(name, "ingest_d2h_bytes")) *out = e->ingest_d2h_bytes;
     else if (!strcmp(name, "norms_rows")) *out = e->norms_rows;       // rows whose cached 1/|v| is valid
@@ -2704,7 +2924,7 @@ int32_t wax_vs_debug_time_search_batch(wax_vs_engine *e, uint32_t n_queries, int
         if (it == warmup) { launches = 0; CUDA_TRY(cudaEventRecord(c->ev0, c->stream)); }
         uint32_t used_heap = 0;
         rc = enqueue_batch_tensor(e, c, c->d_queries, n_queries, k_eff, 0, c->d_out, c->d_ok, nullptr, c->stream, &launches,
-                                  true, nullptr, nullptr, nullptr, &used_heap);
+                                  true, nullptr, nullptr, RowFilter{}, &used_heap);
         if (rc) { cudaStreamSynchronize(c->stream); return rc; }
         if (used_heap) { std::lock_guard<std::mutex> pg(e->pool_mu); e->last_heap = used_heap; }
     }
@@ -2757,7 +2977,7 @@ int32_t wax_vs_debug_batch_nominations(wax_vs_engine *e, const float *queries, u
     dump.d_scores = scores;
     uint64_t launches = 0;
     rc = enqueue_batch_tensor(e, c, c->d_queries, n_queries, k_eff, 0, c->d_out, c->d_ok, nullptr, c->stream, &launches,
-                              true, nullptr, nullptr, d_mask, nullptr, &dump);
+                              true, nullptr, nullptr, RowFilter{d_mask}, nullptr, &dump);
     if (rc) { cudaStreamSynchronize(c->stream); return rc; }
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     std::copy(dump.shape, dump.shape + 7, out_shape);
@@ -2797,6 +3017,7 @@ int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value
     else if (!strcmp(key, "filter_cap")) e->tune.filter_cap = v;
     else if (!strcmp(key, "filter_bf16")) e->tune.filter_bf16 = v;
     else if (!strcmp(key, "batch_l2")) e->tune.batch_l2 = v;
+    else if (!strcmp(key, "filter_bitset_bytes")) e->tune.filter_bitset_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
     else if (!strcmp(key, "single_shadow")) e->tune.single_shadow = v;
     else if (!strcmp(key, "shard_fused")) e->tune.shard_fused = v;
     else if (!strcmp(key, "tail_select")) e->tune.tail_select = v;

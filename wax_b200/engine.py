@@ -261,6 +261,39 @@ class CUDAVectorEngine:
                                                     ns.ctypes.data_as(C.POINTER(C.c_uint32))))
         return [[(int(ids[i, j]), float(scores[i, j])) for j in range(int(ns[i]))] for i in range(b)]
 
+    def search_batch_multi_filtered(self, vectors, top_k: int, filters: Sequence[Tuple[object, Sequence[int]]],
+                                    query_filter: Sequence[Optional[int]]) -> List[List[Tuple[int, float]]]:
+        """A batch of queries with one filter PER QUERY (wax_vs_search_batch_multi_filtered): query i searches under
+        filters[query_filter[i]], or unfiltered when that entry is None.  A filter is ("allow", ids) or ("deny", ids);
+        the mode may also be given as 0 / 1.  Query i's answer equals search_filtered under its filter (search when
+        unfiltered); the batch shares one pass over the corpus per group of filters that fits the bitset budget."""
+        qs = _as_rows(vectors, self.dimensions) if len(vectors) else np.zeros((0, self.dimensions), np.float32)
+        b = qs.shape[0]
+        if len(query_filter) != b:
+            raise ValueError(f"query_filter has {len(query_filter)} entries for {b} queries")
+        if b == 0:
+            return []
+        modes, lists = [], []
+        for mode, fids in filters:
+            modes.append({"allow": 0, "deny": 1}[mode] if isinstance(mode, str) else int(mode))
+            lists.append(np.ascontiguousarray(fids, dtype=np.uint64).reshape(-1))
+        offsets = np.zeros(len(lists) + 1, np.uint64)
+        offsets[1:] = np.cumsum([x.size for x in lists], dtype=np.uint64) if lists else []
+        fids = np.concatenate(lists) if lists else np.zeros(0, np.uint64)
+        modes_arr = np.asarray(modes, np.int32)
+        qf = np.asarray([L.NO_FILTER if f is None else int(f) for f in query_filter], np.uint32)
+        cap = _clamp_topk(top_k)
+        ids = np.zeros((b, cap), np.uint64)
+        scores = np.zeros((b, cap), np.float32)
+        ns = np.zeros(b, np.uint32)
+        _check(L.lib().wax_vs_search_batch_multi_filtered(
+            self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_k),
+            fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
+            offsets.ctypes.data_as(C.POINTER(C.c_uint64)), modes_arr.ctypes.data_as(C.POINTER(C.c_int32)), len(lists),
+            qf.ctypes.data_as(C.POINTER(C.c_uint32)), ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+            scores.ctypes.data_as(C.POINTER(C.c_float)), cap, ns.ctypes.data_as(C.POINTER(C.c_uint32))))
+        return [[(int(ids[i, j]), float(scores[i, j])) for j in range(int(ns[i]))] for i in range(b)]
+
     def search_batch(self, vectors, top_k: int) -> List[List[Tuple[int, float]]]:
         """`search` for a batch of queries (wax_vs_search_batch): the same answers as one call per query.  Cosine and dot
         batches share one tensor-core pass over the corpus, l2 batches too once set_option("batch_l2", 1) is set."""

@@ -167,6 +167,47 @@ public:
         return out;
     }
 
+    // One frame filter per query (each request of a batch carries its own SearchRequest.frameFilter):
+    // query q searches under filters[queryFilter[q]] (first = frameIds, second = allow), or unfiltered for
+    // WAX_VS_NO_FILTER (wax_vs_search_batch_multi_filtered).
+    std::vector<std::vector<Hit>> searchBatchMultiFiltered(const std::vector<std::vector<float>> &vectors, int64_t topK,
+                                                           const std::vector<std::pair<std::vector<uint64_t>, bool>> &filters,
+                                                           const std::vector<uint32_t> &queryFilter) const {
+        std::vector<std::vector<Hit>> out(vectors.size());
+        if (queryFilter.size() != vectors.size())
+            throw EncodingError("queryFilter has " + std::to_string(queryFilter.size()) + " entries for " +
+                                std::to_string(vectors.size()) + " queries");
+        if (vectors.empty()) return out;
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_)
+                throw EncodingError("vector dimension mismatch: expected " + std::to_string(dimensions_) + ", got " +
+                                    std::to_string(v.size()));
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        std::vector<uint64_t> frameIds, offsets(1, 0);
+        std::vector<int32_t> modes;
+        for (const auto &f : filters) {
+            frameIds.insert(frameIds.end(), f.first.begin(), f.first.end());
+            offsets.push_back(frameIds.size());
+            modes.push_back(f.second ? 0 : 1);
+        }
+        const uint32_t lim = static_cast<uint32_t>(topK < 1 ? 1 : (topK > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topK));
+        std::vector<uint64_t> ids(vectors.size() * lim);
+        std::vector<float> scores(vectors.size() * lim);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_multi_filtered(h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_, topK,
+                                                 frameIds.data(), offsets.data(), modes.data(),
+                                                 static_cast<uint32_t>(filters.size()), queryFilter.data(), ids.data(),
+                                                 scores.data(), lim, ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q) {
+            out[q].resize(ns[q]);
+            for (uint32_t i = 0; i < ns[q]; ++i) out[q][i] = {ids[q * lim + i], scores[q * lim + i]};
+        }
+        return out;
+    }
+
     // static load(from:metric:dimensions:) (MetalVectorEngine.swift:318-328): the committed blob (may be empty = none
     // committed yet), then the pending embedding mutations as ONE upsert batch (sequential semantics in the library).
     static CUDAVectorEngine *load(const std::vector<uint8_t> *committedBlob, const std::vector<uint64_t> &pendingIds,
