@@ -181,6 +181,40 @@ int32_t wax_vs_search_batch_multi_filtered(wax_vs_engine *engine, const float *q
                                            uint32_t n_filters, const uint32_t *query_filter, uint64_t *out_ids,
                                            float *out_scores, uint32_t out_stride, uint32_t *out_n);
 
+/* ---- grouped search: the best frames of the best groups (API EXTENSION over the reference) -------------------------
+   Wax's PhotoRAG and VideoRAG answer with the best PHOTOS / VIDEOS, each a root frame plus derived frames (regions, OCR,
+   captions, segments) with their own embeddings.  They over-fetch frames and group the hits on the host:
+   PhotoRAG searches topK = max(resultLimit, searchTopK = 200) (PhotoRAGOrchestrator.swift:244-257, PhotoRAGConfig.swift:74,78)
+   and keeps the best score per parentId ?? id (:264-308); VideoRAG fetches max(400, resultLimit x segmentLimitPerVideo x 8)
+   frames (VideoRAGOrchestrator.swift:252), groups them by root (:273-350) and keeps segmentLimitPerVideo segments per
+   video (VideoRAGTypes.swift:64-65; :406-440).  That over-fetch can return fewer groups than asked, or miss a group's
+   rows.  wax_vs_search_grouped is exact.
+
+   Groups: a row's group id is the id last given to its frame by wax_vs_set_groups, else the frame's own id -- so a root
+   frame left unset and its derived frames set to the root's id form one group (Wax's parentId ?? id).  Groups follow
+   their rows: an appended frame is its own group, an upsert keeps the frame's group, removes drop it.  MV2V has no place
+   for groups: wax_vs_deserialize and wax_vs_debug_fill_synthetic reset every row to its own group, and the caller
+   re-applies the grouping from its frame metadata (parentId) after loading. */
+#define WAX_VS_MAX_PER_GROUP 128
+/* Assign frames to groups (upsert): frame_ids[i] -> group_ids[i]; unknown frame ids are ignored, a later entry for the
+   same frame wins; *out_assigned (optional) = rows whose group was written.  A mutator (write lock). */
+int32_t wax_vs_set_groups(wax_vs_engine *engine, const uint64_t *frame_ids, const uint64_t *group_ids, uint64_t n,
+                          uint64_t *out_assigned);
+/* The best min(per_group, ...) frames of each of the clamp(top_groups) best groups, group-major.  The rows that take
+   part are the allowed rows with a finite distance, ranked by (distance, row); a group ranks by its best row (ties
+   between groups go to the lower row); the answer is the first min(clamp(top_groups), #groups taking part) groups, each
+   with its min(per_group, its rows taking part) best rows, best first.  Scores as wax_vs_search, bit for bit.
+   Filter as wax_vs_search_filtered; n_ids == 0 with mode 1 (deny nothing) = unfiltered.  out_groups[i] = group id of
+   entry i.  out_cap >= min(clamp(top_groups) * per_group, N) else WAX_VS_ERR_BUFFER.  Checked before the empty-engine
+   early return: per_group == 0, per_group > WAX_VS_MAX_PER_GROUP, clamp(top_groups) * per_group > WAX_VS_MAX_RESULTS or
+   a mode other than 0 / 1 -> WAX_VS_ERR_ARGUMENT; a NULL output, or NULL frame_ids with n_ids > 0 -> WAX_VS_ERR_NULL.
+   The first grouped search after a mutation or wax_vs_set_groups builds a device group index (about 12 bytes per row,
+   counter "group_index_builds"); later ones reuse it. */
+int32_t wax_vs_search_grouped(wax_vs_engine *engine, const float *query, uint32_t query_len, int64_t top_groups,
+                              uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                              uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_cap,
+                              uint32_t *out_n);
+
 /* Device-resident form used by the row-sharded engine: `d_queries` (n_queries x dims) and
    `d_candidates` (n_queries x k_eff entries, k_eff = min(clamp(top_k), 10000) -- NOT clipped to N, padding
    has valid = 0) are DEVICE pointers on the engine's device; the work is enqueued on `cuda_stream`
@@ -310,7 +344,8 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *engine, uint64_t *tensor_queries
    nominated from the bf16 shadow), "batch_retry_queries" (bf16-unproven queries retried on the TF32 nominations),
    "shadow_bytes" (HBM held by the bf16 shadow), "shadow_unavailable" (1 = the shadow did not fit in HBM, batches
    nominate in TF32 at about half the rate), "batch_tf32_queries", "filter_bitset_passes" (sub-batches of per-query
-   filtered queries on the tensor-core class, wax_vs_search_batch_multi_filtered), "pool_allocs", "pool_reuses". */
+   filtered queries on the tensor-core class, wax_vs_search_batch_multi_filtered), "group_index_builds" (device group
+   index builds of wax_vs_search_grouped), "pool_allocs", "pool_reuses". */
 int32_t wax_vs_debug_counter(wax_vs_engine *engine, const char *name, uint64_t *out);
 
 /* Device-only timing of the batched path (n_queries synthetic unit queries per step, everything resident):

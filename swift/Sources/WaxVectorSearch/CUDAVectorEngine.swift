@@ -132,6 +132,50 @@ public actor CUDAVectorEngine {
         }
     }
 
+    /// Assign frames to groups (wax_vs_set_groups): `frameIds[i]` -> `groupIds[i]`, e.g. a derived frame to its
+    /// `parentId`; unset frames are their own group.  Groups are not part of MV2V: re-apply them after `deserialize`.
+    @discardableResult
+    public func setGroups(frameIds: [UInt64], groupIds: [UInt64]) async throws -> Int {
+        guard frameIds.count == groupIds.count else {
+            throw WaxError.encodingError(reason: "setGroups: frameIds.count != groupIds.count")
+        }
+        guard !frameIds.isEmpty else { return 0 }
+        let handle = self.handle
+        let assigned: UInt64 = try await io.run {
+            var n: UInt64 = 0
+            let rc = wax_vs_set_groups(handle, frameIds, groupIds, UInt64(frameIds.count), &n)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return n
+        }
+        return Int(assigned)
+    }
+
+    /// The best `perGroup` frames of each of the `topGroups` best groups, exact (wax_vs_search_grouped): what PhotoRAG
+    /// (PhotoRAGOrchestrator.swift:244-308) and VideoRAG (VideoRAGOrchestrator.swift:252-440) now approximate by
+    /// over-fetching frames and grouping them by `parentId ?? id`.  `frameIds` / `allow` filter as `search(...allow:)`;
+    /// an empty deny-list (`allow == false`) is no filter.
+    public func searchGrouped(vector: [Float], topGroups: Int, perGroup: Int = 1, frameIds: [UInt64] = [],
+                              allow: Bool = false) async throws -> [(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])] {
+        let handle = self.handle
+        let cap = max(1, min(min(max(topGroups, 1), Self.maxResults) * max(perGroup, 1), Self.maxResults))
+        return try await io.run {
+            var ids = [UInt64](repeating: 0, count: cap)
+            var scores = [Float](repeating: 0, count: cap)
+            var groups = [UInt64](repeating: 0, count: cap)
+            var n: UInt32 = 0
+            let rc = wax_vs_search_grouped(handle, vector, UInt32(vector.count), Int64(topGroups), UInt32(max(perGroup, 0)),
+                                           frameIds, UInt64(frameIds.count), allow ? 0 : 1, &ids, &scores, &groups,
+                                           UInt32(cap), &n)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            var out: [(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])] = []
+            for i in 0..<Int(n) {
+                if out.last?.groupId != groups[i] { out.append((groups[i], [])) }
+                out[out.count - 1].hits.append((ids[i], scores[i]))
+            }
+            return out
+        }
+    }
+
     public func add(frameId: UInt64, vector: [Float]) async throws {
         try await addBatch(frameIds: [frameId], vectors: [vector])
     }

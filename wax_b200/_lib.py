@@ -19,6 +19,7 @@ OK, ERR_NULL, ERR_DIMENSION, ERR_CAPACITY, ERR_CUDA, ERR_FORMAT, ERR_ARGUMENT, E
 MAX_RESULTS = 10_000
 NO_FILTER = 0xFFFFFFFF          # WAX_VS_NO_FILTER: a query of wax_vs_search_batch_multi_filtered without a filter
 MAX_DIMENSIONS = 1_000_000
+MAX_PER_GROUP = 128             # WAX_VS_MAX_PER_GROUP: rows per group of wax_vs_search_grouped
 SHARD_HANDLE_BYTES, SHARD_MAX_RANKS, SHARD_MAX_K = 128, 16, 128
 
 
@@ -53,6 +54,9 @@ SIGNATURES = {
     "wax_vs_search_batch_multi_filtered": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _u64p,
                                                        C.POINTER(C.c_int32), C.c_uint32, _u32p, _u64p, _f32p, C.c_uint32,
                                                        _u32p]),
+    "wax_vs_set_groups": (C.c_int32, [_eng, _u64p, _u64p, C.c_uint64, _u64p]),
+    "wax_vs_search_grouped": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_int64, C.c_uint32, _u64p, C.c_uint64, C.c_int32,
+                                          _u64p, _f32p, _u64p, C.c_uint32, _u32p]),
     "wax_vs_search_batch": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _f32p,
                                         C.c_uint32, _u32p]),
     "wax_vs_search_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, C.c_uint64, C.c_void_p,

@@ -11,7 +11,8 @@ PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "libwaxvs_cuda.so"
 SOURCES = ["waxvs_engine.cu"]
-HEADERS = ["waxvs_common.cuh", "waxvs_shard.cuh", "waxvs_scan.cuh", "waxvs_select.cuh", "waxvs_synth.cuh", "waxvs_batch.cuh"]
+HEADERS = ["waxvs_common.cuh", "waxvs_shard.cuh", "waxvs_scan.cuh", "waxvs_select.cuh", "waxvs_synth.cuh", "waxvs_batch.cuh",
+           "waxvs_group.cuh"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -36,6 +36,9 @@
 #include "waxvs_synth.cuh"
 #include "waxvs_batch.cuh"
 
+#include "waxvs_group.cuh"
+
+#include <cub/cub.cuh>
 #include <cudaTypedefs.h>
 
 using namespace waxvs;
@@ -221,6 +224,13 @@ struct SearchCtx {
     DevBuf<uint2> d_gather_span;                   // filtered search: each gathered query's span of d_filter_rows
     DevBuf<uint64_t> d_gather_keys;                // filtered search: keys of the listed rows
     DevBuf<wax_vs_candidate> d_shard_local;        // sharded search: this rank's list before the exchange [kShardKCap]
+    DevBuf<unsigned long long> d_group_best;       // grouped search: each group's best (key, row)
+    DevBuf<uint32_t> d_group_keys;                 // grouped search: row-indexed keys of the groups' best rows
+    DevBuf<uint2> d_group_spans;                   // grouped search: CSR span of each selected group
+    PinnedBuf<uint2> h_group_spans;
+    DevBuf<ExpandItem> d_expand_items;             // grouped search: expansion work items, all levels
+    DevBuf<uint64_t> d_expand[3];                  // grouped search: expansion lists (two level buffers, the result)
+    PinnedBuf<uint64_t> h_expand;
     PinnedBuf<unsigned long long> h_flag;          // host-delivery completion flag
     unsigned long long host_seq = 0;               // last value the flag was asked to take
     ~SearchCtx() {                                 // the buffers release themselves
@@ -275,6 +285,20 @@ struct wax_vs_engine {
     uint64_t batch_tensor_queries = 0, batch_fallback_queries = 0;   // instrumentation
     uint64_t batch_bf16_queries = 0, batch_retry_queries = 0, batch_tf32_queries = 0, batch_filter_bf16_queries = 0;
     uint64_t filter_bitset_passes = 0;
+    // Groups (wax_vs_set_groups): groups[r] = row r's group id, kept aligned with `ids` by every mutator.  Empty while
+    // groups_set is false: then every row is its own group (group id = frame id) and nothing is stored.
+    bool groups_set = false;
+    std::vector<uint64_t> groups;
+    // Device group index for grouped search (waxvs_group.cuh), cached per corpus version and grouping: rows sorted by
+    // (group id, row) as perm + starts, and each row's dense group.  Every mutator and set_groups invalidate it; the first
+    // grouped search after that rebuilds it under group_mu (concurrent readers hold only the read lock).
+    struct GroupIndex {
+        DevBuf<uint32_t> perm, row_group, starts;
+        uint32_t n_groups = 0;
+        bool valid = false;
+    } gindex;
+    std::mutex group_mu;
+    uint64_t group_index_builds = 0;   // instrumentation (pool_mu)
     // Adaptive level choice: when more than a quarter of a batch fails the coarse bf16 bound (tightly clustered
     // neighbours), the next 16 batches nominate in TF32 straight away, then bf16 is probed again.
     uint32_t bf16_skip_batches = 0;
@@ -340,6 +364,7 @@ static void invalidate_row_caches(wax_vs_engine *e, uint64_t keep_prefix) {
     e->norms_rows = std::min(e->norms_rows, keep_prefix);
     e->shadow_rows = std::min(e->shadow_rows, keep_prefix);
     if (e->shadow_rows == 0) e->shadow_valid = false;
+    e->gindex.valid = false;           // appends too: the new rows need index entries
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -586,12 +611,38 @@ struct HostDelivery {
     bool delivered = false;             // out: the launched kernel will raise host_flag (else: copy d_out back yourself)
 };
 
+// Exact radix select (waxvs_select.cuh) of the k smallest (key << 32 | row) over a row-indexed key array of n entries
+// (WAXVS_UKEY_NONE = absent); p.k = k candidates go to p.out, best first, padding valid = 0.
+static int32_t enqueue_select(wax_vs_engine *e, SearchCtx *c, const uint32_t *keys, uint32_t n, uint32_t k,
+                              const ScanParams &p, cudaStream_t stream, uint64_t *launches) {
+    int32_t rc = c->d_select.ensure(1, "selection state");
+    if (!rc) rc = c->d_sel_keys.ensure(16384, "selected keys");
+    if (rc) return rc;
+    const int sgrid = std::max(1, std::min<int>(e->sm_count * 4, static_cast<int>((n + 511) / 512)));
+    select_init_kernel<<<1, 256, 0, stream>>>(c->d_select, k);
+    for (int pass = 0; pass < kSelectPasses; ++pass) {
+        select_hist_kernel<<<sgrid, 512, 0, stream>>>(keys, n, c->d_select, pass);
+        select_scan_kernel<<<1, 1024, 0, stream>>>(c->d_select, pass);
+    }
+    select_compact_kernel<<<sgrid, 512, 0, stream>>>(keys, n, c->d_select, c->d_sel_keys, 16384);
+    uint32_t pow2 = 64;
+    while (pow2 < k) pow2 <<= 1;
+    CUDA_TRY(grant_smem(e, select_sort_kernel, pow2 * sizeof(uint64_t)));
+    select_sort_kernel<<<1, 1024, pow2 * sizeof(uint64_t), stream>>>(c->d_select, c->d_sel_keys, pow2, p);
+    CUDA_TRY(cudaGetLastError());
+    *launches += 3 + 2 * kSelectPasses;
+    return WAX_VS_OK;
+}
+
 // `shard` (optional): the row-sharded form -- d_out receives the result MERGED over all ranks; the exchange runs inside
 // the scan launch when the kernel's shared-memory lists can hold the merge keys, else as one extra 1-CTA launch.
+// keys_only: run the emitting scan alone -- c->d_dist_keys receives every row's distance key (the masked rows'
+// WAXVS_UKEY_NONE) and the caller does its own selection (grouped search); d_out and k_eff are not used.
 static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_query, uint32_t k_eff,
                               uint64_t row_offset, wax_vs_candidate *d_out, const uint64_t *d_ids,
                               cudaStream_t stream, uint64_t *launches, const uint32_t *d_mask = nullptr,
-                              const ShardParams *shard = nullptr, const HostDelivery *host = nullptr) {
+                              const ShardParams *shard = nullptr, const HostDelivery *host = nullptr,
+                              bool keys_only = false) {
     wax_vs_candidate *d_merged = nullptr;
     if (shard) {
         if (k_eff > static_cast<uint32_t>(kShardKCap))
@@ -624,12 +675,10 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
     p.mask = d_mask;
     p.trace = e->debug_trace;
 
-    const bool emit = k_eff > static_cast<uint32_t>(e->tune.fused_k_max);
+    const bool emit = keys_only || k_eff > static_cast<uint32_t>(e->tune.fused_k_max);
     const int mode = emit ? 2 : (k_eff <= 32 ? 0 : 1);
     if (emit) {
         int32_t rc = c->d_dist_keys.ensure(static_cast<size_t>(e->n_rows), "distance keys");
-        if (!rc) rc = c->d_select.ensure(1, "selection state");
-        if (!rc) rc = c->d_sel_keys.ensure(16384, "selected keys");
         if (rc) return rc;
         p.dist_keys = c->d_dist_keys;
     }
@@ -683,21 +732,9 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
     }
     ++*launches;
 
-    if (emit) {
-        const uint32_t n = static_cast<uint32_t>(e->n_rows);
-        const int sgrid = std::max(1, std::min<int>(e->sm_count * 4, static_cast<int>((n + 511) / 512)));
-        select_init_kernel<<<1, 256, 0, stream>>>(c->d_select, k_eff);
-        for (int pass = 0; pass < kSelectPasses; ++pass) {
-            select_hist_kernel<<<sgrid, 512, 0, stream>>>(c->d_dist_keys, n, c->d_select, pass);
-            select_scan_kernel<<<1, 1024, 0, stream>>>(c->d_select, pass);
-        }
-        select_compact_kernel<<<sgrid, 512, 0, stream>>>(c->d_dist_keys, n, c->d_select, c->d_sel_keys, 16384);
-        uint32_t pow2 = 64;
-        while (pow2 < k_eff) pow2 <<= 1;
-        CUDA_TRY(grant_smem(e, select_sort_kernel, pow2 * sizeof(uint64_t)));
-        select_sort_kernel<<<1, 1024, pow2 * sizeof(uint64_t), stream>>>(c->d_select, c->d_sel_keys, pow2, p);
-        CUDA_TRY(cudaGetLastError());
-        *launches += 3 + 2 * kSelectPasses;
+    if (emit && !keys_only) {
+        int32_t rc = enqueue_select(e, c, c->d_dist_keys, static_cast<uint32_t>(e->n_rows), k_eff, p, stream, launches);
+        if (rc) return rc;
     }
     if (shard && !fused_exchange) return exchange_standalone();
     return WAX_VS_OK;
@@ -1508,6 +1545,7 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
     if (increasing) {
         // the common bulk-ingest case: every id is new and larger than all stored ones -- no lookups, no hash table
         e->ids.insert(e->ids.end(), frame_ids, frame_ids + n);
+        if (e->groups_set) e->groups.insert(e->groups.end(), frame_ids, frame_ids + n);   // a new frame is its own group
         for (uint64_t i = 0; i < n; ++i) target[i] = static_cast<uint32_t>(n0 + i);
         e->n_rows += n;
         e->map_valid = false;
@@ -1523,6 +1561,7 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
                     ensure_map(e);
                 }
                 e->ids.push_back(frame_ids[i]);
+                if (e->groups_set) e->groups.push_back(frame_ids[i]);    // an upsert of a known frame keeps its group
                 if (!e->ids_sorted) e->map.put(frame_ids[i], row);
                 else e->map_valid = false;
                 ++e->n_rows;
@@ -1642,8 +1681,12 @@ int32_t wax_vs_remove_batch(wax_vs_engine *e, const uint64_t *frame_ids, uint64_
     }
     tr.mark("compact matrix");
     // ids: one compaction, one hash rebuild (lazily, on the next lookup)
-    for (uint64_t j = 0; j < moving; ++j) e->ids[first + j] = e->ids[src[j]];
+    for (uint64_t j = 0; j < moving; ++j) {
+        e->ids[first + j] = e->ids[src[j]];
+        if (e->groups_set) e->groups[first + j] = e->groups[src[j]];
+    }
     e->ids.resize(new_n);
+    if (e->groups_set) e->groups.resize(new_n);
     e->n_rows = new_n;
     e->map_valid = false;
     e->d_ids_dirty = true;
@@ -2574,6 +2617,274 @@ int32_t wax_vs_shard_search_filtered(wax_vs_engine *e, const float *query, uint3
     return shard_search_host(e, query, k_eff, &rows, mode, out_ids, out_scores, out_cap, out_n);
 }
 
+// ---- grouped search (waxvs_group.cuh) -----------------------------------------------------------------------------
+// PhotoRAG and VideoRAG group frames by parentId ?? id on the host after over-fetching frames
+// (PhotoRAGOrchestrator.swift:244-308, VideoRAGOrchestrator.swift:252-350,406-440); here the grouping is exact and runs
+// on the device over the emitting scan's per-row distance keys.
+
+int32_t wax_vs_set_groups(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *group_ids, uint64_t n,
+                          uint64_t *out_assigned) {
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    if (out_assigned) *out_assigned = 0;
+    if (n == 0) return WAX_VS_OK;
+    if (!frame_ids || !group_ids) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    std::unique_lock<std::shared_mutex> w(e->rw);
+    DeviceGuard g(e->device);
+    drain_device_path(e);
+    if (!e->groups_set) {              // from implicit (every row its own group) to an explicit array
+        e->groups.resize(e->n_rows);
+        for (uint64_t r = 0; r < e->n_rows; ++r) e->groups[r] = e->ids_identity ? e->id_base + r : e->ids[r];
+        e->groups_set = true;
+    }
+    std::vector<uint32_t> written(static_cast<size_t>((e->n_rows + 31) / 32), 0u);
+    uint64_t assigned = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        uint64_t row;
+        if (e->ids_identity) {
+            if (frame_ids[i] < e->id_base || frame_ids[i] - e->id_base >= e->n_rows) continue;
+            row = frame_ids[i] - e->id_base;
+        } else {
+            const uint32_t f = find_row(e, frame_ids[i]);
+            if (f == 0xFFFFFFFFu) continue;              // unknown frame: ignored
+            row = f;
+        }
+        e->groups[row] = group_ids[i];                   // a later entry for the same frame wins
+        const uint32_t wd = static_cast<uint32_t>(row >> 5), b = 1u << (row & 31u);
+        if (!(written[wd] & b)) { written[wd] |= b; ++assigned; }
+    }
+    e->gindex.valid = false;
+    if (out_assigned) *out_assigned = assigned;
+    return WAX_VS_OK;
+}
+
+// The device group index of the current corpus and grouping, built on c's stream by the first grouped search after a
+// mutation or set_groups: (group id, row) pairs radix-sorted by CUB (stable, so each group's rows stay in row order),
+// group heads flagged and prefix-summed into dense group indices.  Readers hold the read lock; group_mu serialises the
+// build, and the build completes before the index is published.
+static int32_t ensure_group_index(wax_vs_engine *e, SearchCtx *c) {
+    std::lock_guard<std::mutex> lk(e->group_mu);
+    auto &gi = e->gindex;
+    if (gi.valid) return WAX_VS_OK;
+    const uint32_t n = static_cast<uint32_t>(e->n_rows);
+    cudaStream_t s = c->stream;
+    int32_t rc;
+    const uint64_t *d_ids = nullptr;
+    if (!e->groups_set && (rc = sync_device_ids(e, &d_ids))) return rc;
+    DevBuf<uint64_t> keys_in, keys_out, d_groups;
+    DevBuf<uint32_t> vals, incl;
+    DevBuf<uint8_t> temp;
+    size_t sort_bytes = 0, scan_bytes = 0;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys_in.p, keys_out.p, vals.p, gi.perm.p, static_cast<int>(n),
+                                             0, 64, s));
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, vals.p, incl.p, static_cast<int>(n), s));
+    if ((rc = keys_in.ensure(n, "group sort keys")) || (rc = keys_out.ensure(n, "sorted group keys")) ||
+        (rc = vals.ensure(n, "group sort rows")) || (rc = incl.ensure(n, "group numbering")) ||
+        (rc = temp.ensure(std::max<size_t>(std::max(sort_bytes, scan_bytes), 1), "group index scratch")) ||
+        (rc = gi.perm.ensure(n, "group index rows")) || (rc = gi.row_group.ensure(n, "group index groups")) ||
+        (rc = gi.starts.ensure(static_cast<size_t>(n) + 1, "group index starts")))
+        return rc;
+    if (e->groups_set) {
+        if ((rc = d_groups.ensure(n, "group ids"))) return rc;
+        CUDA_TRY(cudaMemcpyAsync(d_groups, e->groups.data(), static_cast<size_t>(n) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    }
+    const int grid = static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 8, (n + 255) / 256)));
+    group_sort_input_kernel<<<grid, 256, 0, s>>>(keys_in, vals, n, e->groups_set ? d_groups.p : nullptr, d_ids, e->id_base);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(temp.p, sort_bytes, keys_in.p, keys_out.p, vals.p, gi.perm.p, static_cast<int>(n),
+                                             0, 64, s));
+    group_heads_kernel<<<grid, 256, 0, s>>>(keys_out, n, vals);        // the row values are no longer needed
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cub::DeviceScan::InclusiveSum(temp.p, scan_bytes, vals.p, incl.p, static_cast<int>(n), s));
+    group_finish_kernel<<<grid, 256, 0, s>>>(gi.perm, incl, n, gi.row_group, gi.starts);
+    CUDA_TRY(cudaGetLastError());
+    uint32_t n_groups = 0;
+    CUDA_TRY(cudaMemcpyAsync(&n_groups, incl.p + (n - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    CUDA_TRY(cudaMemcpy(gi.starts.p + n_groups, &n, sizeof(uint32_t), cudaMemcpyHostToDevice));
+    gi.n_groups = n_groups;
+    gi.valid = true;
+    std::lock_guard<std::mutex> pg(e->pool_mu);
+    ++e->group_index_builds;
+    return WAX_VS_OK;
+}
+
+static float host_from_orderable(uint32_t k) {       // inverse of orderable_u32
+    const uint32_t u = k ^ ((k & 0x80000000u) ? 0x80000000u : 0xFFFFFFFFu);
+    float f;
+    memcpy(&f, &u, sizeof f);
+    return f;
+}
+
+int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_groups,
+                              uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                              uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_cap,
+                              uint32_t *out_n) {
+    if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    if (per_group == 0 || per_group > WAX_VS_MAX_PER_GROUP)
+        return fail(WAX_VS_ERR_ARGUMENT, "per_group must be in [1, %d] (got %u)", WAX_VS_MAX_PER_GROUP, per_group);
+    const uint32_t n_top = clamp_topk(top_groups);
+    if (static_cast<uint64_t>(n_top) * per_group > WAX_VS_MAX_RESULTS)
+        return fail(WAX_VS_ERR_ARGUMENT, "clamp(top_groups) x per_group = %llu exceeds %d",
+                    static_cast<unsigned long long>(n_top) * per_group, WAX_VS_MAX_RESULTS);
+    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
+    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    *out_n = 0;
+    if (e->n_rows == 0) return WAX_VS_OK;                // as wax_vs_search (:448)
+    if (!query) return fail(WAX_VS_ERR_NULL, "query is NULL");
+    if (query_len != e->dims)
+        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
+    const uint32_t n = static_cast<uint32_t>(e->n_rows);
+    const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(n_top) * per_group, n));
+    if (out_cap < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_cap, need);
+    const bool filtered = !(mode == 1 && n_ids == 0);
+    std::vector<uint32_t> rows;
+    if (filtered) {
+        std::vector<uint32_t> seen(static_cast<size_t>((n + 31) / 32), 0u);
+        build_row_filter(e, frame_ids, n_ids, seen, rows);
+        if (mode == 0 && rows.empty()) return WAX_VS_OK;                 // nothing allowed
+        if (mode == 1 && rows.size() == n) return WAX_VS_OK;             // everything denied
+    }
+    DeviceGuard g(e->device);
+    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
+    if (rc) return rc;
+    SearchCtx *c = lease.c;
+    cudaStream_t s = c->stream;
+    if ((rc = ensure_group_index(e, c))) return rc;
+    const auto &gi = e->gindex;
+    uint64_t launches = 0;
+
+    // (1) the emitting scan under the row filter: c->d_dist_keys
+    if ((rc = stage_queries(e, c, query, 1, s))) return rc;
+    if ((rc = c->d_out.ensure(n_top, "result buffer"))) return rc;
+    if ((rc = c->h_out.ensure(n_top, "result staging"))) return rc;
+    if (filtered) {
+        if ((rc = c->d_filter_rows.ensure(std::max<size_t>(rows.size(), 1), "filter rows"))) return rc;
+        if (!rows.empty())
+            CUDA_TRY(cudaMemcpyAsync(c->d_filter_rows, rows.data(), rows.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+        const std::vector<uint64_t> spec = {0, rows.size(), 0, static_cast<uint64_t>(mode)};
+        if ((rc = build_filter_bits(e, c, spec, 1, s, &launches))) { cudaStreamSynchronize(s); return rc; }
+    }
+    if ((rc = enqueue_search(e, c, c->d_queries, 1, 0, c->d_out, nullptr, s, &launches, filtered ? c->d_mask.p : nullptr,
+                             nullptr, nullptr, true))) {
+        cudaStreamSynchronize(s);
+        return rc;
+    }
+    // (2) each group's best row, written at that row of an otherwise empty key array
+    if ((rc = c->d_group_best.ensure(std::max<uint32_t>(gi.n_groups, 1), "group minima"))) return rc;
+    if ((rc = c->d_group_keys.ensure(n, "group keys"))) return rc;
+    CUDA_TRY(cudaMemsetAsync(c->d_group_best, 0xFF, static_cast<size_t>(gi.n_groups) * sizeof(unsigned long long), s));
+    const uint64_t reduce_warps = (static_cast<uint64_t>(n) + 32 * kReduceRun - 1) / (32 * kReduceRun);
+    const int rgrid = static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 16, (reduce_warps + 7) / 8)));
+    group_reduce_kernel<<<rgrid, 256, 0, s>>>(gi.perm, gi.row_group, c->d_dist_keys, n, c->d_group_best);
+    const int kgrid = static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 8, (n + 255) / 256)));
+    group_keys_kernel<<<kgrid, 256, 0, s>>>(gi.row_group, c->d_group_best, n, c->d_group_keys);
+    CUDA_TRY(cudaGetLastError());
+    launches += 2;
+    // (3) the top groups' best rows, in the total order
+    ScanParams sp{};
+    sp.k = n_top; sp.out = c->d_out;
+    if ((rc = enqueue_select(e, c, c->d_group_keys, n, n_top, sp, s, &launches))) { cudaStreamSynchronize(s); return rc; }
+    CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, n_top * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, s));
+    const uint64_t *h_keys = nullptr;                 // per_group > 1: [selected][per_group] keys, group-major
+    uint32_t n_sel = 0;
+    if (per_group > 1) {
+        // (4) expansion: each selected group's per_group best rows.  Level 0 sorts tiles of kExpandTile CSR positions,
+        // each later level merges kExpandTile / per_group of the previous level's lists, until one list per group is left.
+        if ((rc = c->d_group_spans.ensure(n_top, "group spans")) || (rc = c->h_group_spans.ensure(n_top, "group span staging")))
+            return rc;
+        group_spans_kernel<<<(n_top + 255) / 256, 256, 0, s>>>(c->d_out, n_top, gi.row_group, gi.starts, c->d_group_spans);
+        CUDA_TRY(cudaGetLastError());
+        ++launches;
+        CUDA_TRY(cudaMemcpyAsync(c->h_group_spans, c->d_group_spans, n_top * sizeof(uint2), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        while (n_sel < n_top && c->h_group_spans[n_sel].y > 0) ++n_sel;   // valid candidates come first
+        struct Pending { uint32_t group, lists, off; };
+        std::vector<std::vector<ExpandItem>> levels(1);
+        std::vector<Pending> pending;
+        uint64_t buf_keys[2] = {0, 0};
+        uint32_t off = 0;
+        for (uint32_t i = 0; i < n_sel; ++i) {
+            const uint2 sp_i = c->h_group_spans[i];
+            const uint32_t tiles = (sp_i.y + kExpandTile - 1) / kExpandTile;
+            if (tiles == 1) { levels[0].push_back({sp_i.x, sp_i.y, i * per_group, 1u}); continue; }
+            for (uint32_t t = 0; t < tiles; ++t)
+                levels[0].push_back({sp_i.x + t * kExpandTile, std::min(kExpandTile, sp_i.y - t * kExpandTile), off + t * per_group, 0u});
+            pending.push_back({i, tiles, off});
+            off += tiles * per_group;
+        }
+        buf_keys[0] = off;
+        const uint32_t fan = kExpandTile / per_group;
+        while (!pending.empty()) {
+            const size_t lv = levels.size();
+            levels.emplace_back();
+            std::vector<Pending> next;
+            off = 0;
+            for (const Pending &pd : pending) {
+                const uint32_t m = (pd.lists + fan - 1) / fan;
+                if (m == 1) { levels[lv].push_back({pd.off, pd.lists * per_group, pd.group * per_group, 1u}); continue; }
+                for (uint32_t t = 0; t < m; ++t)
+                    levels[lv].push_back({pd.off + t * fan * per_group, std::min(fan, pd.lists - t * fan) * per_group,
+                                          off + t * per_group, 0u});
+                next.push_back({pd.group, m, off});
+                off += m * per_group;
+            }
+            buf_keys[lv & 1] = std::max<uint64_t>(buf_keys[lv & 1], off);
+            pending.swap(next);
+        }
+        std::vector<ExpandItem> all;
+        for (const auto &lvl : levels) all.insert(all.end(), lvl.begin(), lvl.end());
+        const size_t n_res = static_cast<size_t>(std::max<uint32_t>(n_sel, 1)) * per_group;
+        if ((rc = c->d_expand_items.ensure(std::max<size_t>(all.size(), 1), "expansion items")) ||
+            (rc = c->d_expand[0].ensure(std::max<uint64_t>(buf_keys[0], 1), "expansion lists")) ||
+            (rc = c->d_expand[1].ensure(std::max<uint64_t>(buf_keys[1], 1), "expansion lists")) ||
+            (rc = c->d_expand[2].ensure(n_res, "expansion result")) || (rc = c->h_expand.ensure(n_res, "expansion staging")))
+            return rc;
+        if (!all.empty())
+            CUDA_TRY(cudaMemcpyAsync(c->d_expand_items, all.data(), all.size() * sizeof(ExpandItem), cudaMemcpyHostToDevice, s));
+        size_t first_item = 0;
+        for (size_t lv = 0; lv < levels.size(); ++lv) {
+            const uint32_t items = static_cast<uint32_t>(levels[lv].size());
+            if (items) {
+                group_expand_kernel<<<items, 1024, 0, s>>>(c->d_expand_items + first_item, lv == 0 ? 1u : 0u, gi.perm,
+                                                           c->d_dist_keys, lv ? c->d_expand[(lv - 1) & 1].p : nullptr,
+                                                           per_group, c->d_expand[lv & 1], c->d_expand[2]);
+                CUDA_TRY(cudaGetLastError());
+                ++launches;
+            }
+            first_item += items;
+        }
+        if (n_sel)
+            CUDA_TRY(cudaMemcpyAsync(c->h_expand, c->d_expand[2], static_cast<size_t>(n_sel) * per_group * sizeof(uint64_t),
+                                     cudaMemcpyDeviceToHost, s));
+        h_keys = c->h_expand;
+    }
+    CUDA_TRY(cudaStreamSynchronize(s));              // also keeps `rows` and the item list alive until their copies are done
+    // (5) delivery: row -> frame id and group id, distance -> score
+    auto deliver = [&](uint32_t m, uint32_t row, float d) {
+        const uint64_t id = e->ids_identity ? e->id_base + row : e->ids[row];
+        out_ids[m] = id;
+        out_scores[m] = score_from_distance(e->similarity, d);
+        out_groups[m] = e->groups_set ? e->groups[row] : id;
+    };
+    uint32_t m = 0;
+    if (per_group == 1) {
+        for (uint32_t i = 0; i < n_top; ++i)
+            if (c->h_out[i].valid) deliver(m++, static_cast<uint32_t>(c->h_out[i].row), c->h_out[i].distance);
+    } else {
+        for (uint32_t i = 0; i < n_sel; ++i)
+            for (uint32_t j = 0; j < per_group; ++j) {
+                const uint64_t key = h_keys[static_cast<size_t>(i) * per_group + j];
+                if (key == WAXVS_KEY_NONE) break;
+                deliver(m++, static_cast<uint32_t>(key), host_from_orderable(static_cast<uint32_t>(key >> 32)));
+            }
+    }
+    *out_n = m;
+    return WAX_VS_OK;
+}
+
 // ---- persistence ---------------------------------------------------------------------------------------------
 static uint64_t mv2v_length(const wax_vs_engine *e) {
     return 36ull + e->n_rows * e->dims * 4ull + 8ull + e->n_rows * 8ull;
@@ -2659,6 +2970,8 @@ int32_t wax_vs_deserialize(wax_vs_engine *e, const uint8_t *src, uint64_t len) {
     e->ids_sorted = true;
     for (uint64_t i = 1; i < count && e->ids_sorted; ++i) e->ids_sorted = e->ids[i] > e->ids[i - 1];
     e->d_ids_dirty = true;
+    e->groups_set = false;                  // MV2V has no groups: the caller re-applies them (wax_vs_set_groups)
+    e->groups.clear(); e->groups.shrink_to_fit();
     invalidate_row_caches(e, 0);
     return WAX_VS_OK;
 }
@@ -2693,6 +3006,8 @@ int32_t wax_vs_debug_fill_synthetic(wax_vs_engine *e, uint64_t seed, uint64_t fi
     e->ids_identity = true; e->id_base = id_base;
     e->map = IdMap(); e->map_valid = true; e->ids_sorted = true;
     e->d_ids_dirty = true;
+    e->groups_set = false;
+    e->groups.clear(); e->groups.shrink_to_fit();
     invalidate_row_caches(e, 0);
     return WAX_VS_OK;
 }
@@ -2884,6 +3199,7 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "shadow_unavailable")) *out = e->shadow_unavailable ? 1 : 0;   // bf16 shadow did not fit: TF32 level runs
     else if (!strcmp(name, "batch_tf32_queries")) *out = e->batch_tf32_queries;
     else if (!strcmp(name, "filter_bitset_passes")) *out = e->filter_bitset_passes;   // per-query filters: tensor sub-batches
+    else if (!strcmp(name, "group_index_builds")) *out = e->group_index_builds;       // grouped search: device index builds
     else if (!strcmp(name, "ingest_h2d_bytes")) *out = e->ingest_h2d_bytes;
     else if (!strcmp(name, "ingest_d2h_bytes")) *out = e->ingest_d2h_bytes;
     else if (!strcmp(name, "norms_rows")) *out = e->norms_rows;       // rows whose cached 1/|v| is valid

@@ -1,4 +1,5 @@
-// waxvs_select.cuh -- exact top-k for 32 < k <= 10 000 (the API clamp, MetalVectorEngine.swift:18,842-846).
+// waxvs_select.cuh -- exact top-k for 1 <= k <= 10 000 (the API clamp, MetalVectorEngine.swift:18,842-846): the scan
+// uses it for k > fused_k_max, grouped search (waxvs_group.cuh) for every k.
 //
 // The reference handles large k with the CPU heap over the full distance buffer
 // (MetalVectorEngine.swift:455,614-625,630-680: `N < 1000 || k > 256` -> host heap).  Here the scan kernel

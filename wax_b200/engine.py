@@ -294,6 +294,52 @@ class CUDAVectorEngine:
             scores.ctypes.data_as(C.POINTER(C.c_float)), cap, ns.ctypes.data_as(C.POINTER(C.c_uint32))))
         return [[(int(ids[i, j]), float(scores[i, j])) for j in range(int(ns[i]))] for i in range(b)]
 
+    def set_groups(self, frame_ids: Sequence[int], group_ids: Sequence[int]) -> int:
+        """Assign frames to groups (wax_vs_set_groups): frame_ids[i] -> group_ids[i], unknown frames ignored, a later
+        entry for the same frame wins.  A frame never assigned is its own group (Wax's parentId ?? id).  Returns how
+        many rows had their group written.  Groups are not serialized: re-apply them after deserialize()."""
+        fids = np.ascontiguousarray(frame_ids, dtype=np.uint64).reshape(-1)
+        gids = np.ascontiguousarray(group_ids, dtype=np.uint64).reshape(-1)
+        if fids.size != gids.size:
+            raise ValueError(f"set_groups: {fids.size} frame ids for {gids.size} group ids")
+        if fids.size == 0:
+            return 0
+        n = C.c_uint64(0)
+        _check(L.lib().wax_vs_set_groups(self._h, fids.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                         gids.ctypes.data_as(C.POINTER(C.c_uint64)), fids.size, C.byref(n)))
+        return n.value
+
+    def search_grouped(self, vector: Sequence[float], top_groups: int, per_group: int = 1,
+                       allow: Optional[Sequence[int]] = None,
+                       deny: Optional[Sequence[int]] = None) -> List[Tuple[int, List[Tuple[int, float]]]]:
+        """The best `per_group` frames of each of the `top_groups` best groups (wax_vs_search_grouped), exact:
+        [(group_id, [(frame_id, score), ...]), ...], groups best first (a group ranks by its best frame), frames best
+        first.  Optional frame filter as search_filtered (at most one of allow= / deny=).  Replaces the over-fetch +
+        host grouping of PhotoRAG / VideoRAG (PhotoRAGOrchestrator.swift:244-308, VideoRAGOrchestrator.swift:252-440)."""
+        if allow is not None and deny is not None:
+            raise ValueError("pass at most one of allow= / deny=")
+        fids = np.ascontiguousarray(allow if allow is not None else (deny if deny is not None else []),
+                                    dtype=np.uint64).reshape(-1)
+        mode = 0 if allow is not None else 1
+        q = np.ascontiguousarray(vector, dtype=np.float32).reshape(-1)
+        cap = max(1, min(_clamp_topk(top_groups) * max(int(per_group), 1), L.MAX_RESULTS))
+        ids = np.empty(cap, np.uint64)
+        scores = np.empty(cap, np.float32)
+        groups = np.empty(cap, np.uint64)
+        n = C.c_uint32(0)
+        _check(L.lib().wax_vs_search_grouped(self._h, q.ctypes.data_as(C.POINTER(C.c_float)), q.size, int(top_groups),
+                                             int(per_group), fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size
+                                             else None, fids.size, mode, ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                             scores.ctypes.data_as(C.POINTER(C.c_float)),
+                                             groups.ctypes.data_as(C.POINTER(C.c_uint64)), cap, C.byref(n)))
+        out: List[Tuple[int, List[Tuple[int, float]]]] = []
+        for i in range(n.value):
+            g = int(groups[i])
+            if not out or out[-1][0] != g:
+                out.append((g, []))
+            out[-1][1].append((int(ids[i]), float(scores[i])))
+        return out
+
     def search_batch(self, vectors, top_k: int) -> List[List[Tuple[int, float]]]:
         """`search` for a batch of queries (wax_vs_search_batch): the same answers as one call per query.  Cosine and dot
         batches share one tensor-core pass over the corpus, l2 batches too once set_option("batch_l2", 1) is set."""

@@ -208,6 +208,39 @@ public:
         return out;
     }
 
+    // Assign frames to groups (wax_vs_set_groups): frameIds[i] -> groupIds[i] (e.g. a derived frame to its parentId);
+    // a frame never assigned is its own group.  Groups are not serialized: re-apply them after deserialize().
+    uint64_t setGroups(const std::vector<uint64_t> &frameIds, const std::vector<uint64_t> &groupIds) {
+        if (frameIds.size() != groupIds.size()) throw EncodingError("setGroups: frameIds.count != groupIds.count");
+        uint64_t assigned = 0;
+        if (frameIds.empty()) return 0;
+        check(wax_vs_set_groups(h_, frameIds.data(), groupIds.data(), frameIds.size(), &assigned));
+        return assigned;
+    }
+
+    // The best perGroup frames of each of the topGroups best groups, exact (wax_vs_search_grouped), group-major:
+    // (groupId, hits best first), groups best first.  frameIds / allow filter as searchFiltered; an empty deny-list is
+    // no filter.
+    using Group = std::pair<uint64_t, std::vector<Hit>>;
+    std::vector<Group> searchGrouped(const std::vector<float> &vector, int64_t topGroups, uint32_t perGroup = 1,
+                                     const std::vector<uint64_t> &frameIds = {}, bool allow = false) const {
+        const int64_t lim = topGroups < 1 ? 1 : (topGroups > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topGroups);
+        const int64_t want = lim * (perGroup ? perGroup : 1);
+        const size_t cap = static_cast<size_t>(want > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : want);
+        std::vector<uint64_t> ids(cap), groups(cap);
+        std::vector<float> scores(cap);
+        uint32_t n = 0;
+        check(wax_vs_search_grouped(h_, vector.data(), static_cast<uint32_t>(vector.size()), topGroups, perGroup,
+                                    frameIds.data(), frameIds.size(), allow ? 0 : 1, ids.data(), scores.data(), groups.data(),
+                                    static_cast<uint32_t>(cap), &n));
+        std::vector<Group> out;
+        for (uint32_t i = 0; i < n; ++i) {
+            if (out.empty() || out.back().first != groups[i]) out.push_back({groups[i], {}});
+            out.back().second.push_back({ids[i], scores[i]});
+        }
+        return out;
+    }
+
     // static load(from:metric:dimensions:) (MetalVectorEngine.swift:318-328): the committed blob (may be empty = none
     // committed yet), then the pending embedding mutations as ONE upsert batch (sequential semantics in the library).
     static CUDAVectorEngine *load(const std::vector<uint8_t> *committedBlob, const std::vector<uint64_t> &pendingIds,
