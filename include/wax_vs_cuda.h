@@ -215,6 +215,24 @@ int32_t wax_vs_search_grouped(wax_vs_engine *engine, const float *query, uint32_
                               uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_cap,
                               uint32_t *out_n);
 
+/* The batched form (a server batching PhotoRAG / VideoRAG requests): n_queries queries under ONE filter (as
+   wax_vs_search_batch_filtered; n_ids == 0 with mode 1 = unfiltered).  Query i's answer is identical to
+   wax_vs_search_grouped for that query alone -- same frame ids, group ids, order and score bits -- group-major at
+   out_*[i * out_stride], count out_n[i]; out_stride >= min(clamp(top_groups) * per_group, N) else WAX_VS_ERR_BUFFER.
+   Same argument checks as wax_vs_search_grouped, before the empty-engine early return; n_queries == 0 returns OK.
+   How: each query's exact top-k_c rows, k_c = min(1024, max(128, 4 * clamp(top_groups))), come from the batched
+   filtered search (the tensor-core levels, or the gather of a small allow-list).  A group ranks by its best row, so the
+   first clamp(top_groups) distinct groups of that list are the top groups and their listed rows their best rows; a
+   selected group with fewer listed rows than per_group is scored exactly over its own rows.  A query whose list names
+   too few groups (one video's segments fill it) runs the single-query pipeline, as do whole batches the tensor-core
+   levels do not take (small batches, dims % 32 != 0, l2 without the option "batch_l2", clamp(top_groups) > 256,
+   deny-lists leaving fewer than k_c rows).  Counters: "grouped_batch_covered_queries", "grouped_batch_expanded_groups"
+   ((query, group) pairs scored over the group's rows), "grouped_batch_fallback_queries". */
+int32_t wax_vs_search_batch_grouped(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                    uint32_t query_len, int64_t top_groups, uint32_t per_group,
+                                    const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids,
+                                    float *out_scores, uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n);
+
 /* Device-resident form used by the row-sharded engine: `d_queries` (n_queries x dims) and
    `d_candidates` (n_queries x k_eff entries, k_eff = min(clamp(top_k), 10000) -- NOT clipped to N, padding
    has valid = 0) are DEVICE pointers on the engine's device; the work is enqueued on `cuda_stream`

@@ -176,6 +176,40 @@ public actor CUDAVectorEngine {
         }
     }
 
+    /// `searchGrouped` for a batch of queries under ONE filter (wax_vs_search_batch_grouped), for a server batching
+    /// PhotoRAG / VideoRAG requests: one answer per query, each identical to `searchGrouped` for that query alone.
+    public func searchBatchGrouped(vectors: [[Float]], topGroups: Int, perGroup: Int = 1, frameIds: [UInt64] = [],
+                                   allow: Bool = false) async throws
+        -> [[(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])]] {
+        guard !vectors.isEmpty else { return [] }
+        let dims = dimensions
+        for v in vectors where v.count != dims {
+            throw WaxError.encodingError(reason: "vector dimension mismatch: expected \(dims), got \(v.count)")
+        }
+        let handle = self.handle
+        let cap = max(1, min(min(max(topGroups, 1), Self.maxResults) * max(perGroup, 1), Self.maxResults))
+        return try await io.run {
+            var flat = [Float](); flat.reserveCapacity(vectors.count * dims)
+            for v in vectors { flat.append(contentsOf: v) }
+            var ids = [UInt64](repeating: 0, count: vectors.count * cap)
+            var scores = [Float](repeating: 0, count: vectors.count * cap)
+            var groups = [UInt64](repeating: 0, count: vectors.count * cap)
+            var counts = [UInt32](repeating: 0, count: vectors.count)
+            let rc = wax_vs_search_batch_grouped(handle, flat, UInt32(vectors.count), UInt32(dims), Int64(topGroups),
+                                                 UInt32(max(perGroup, 0)), frameIds, UInt64(frameIds.count), allow ? 0 : 1,
+                                                 &ids, &scores, &groups, UInt32(cap), &counts)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return (0..<vectors.count).map { q in
+                var out: [(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])] = []
+                for i in (q * cap)..<(q * cap + Int(counts[q])) {
+                    if out.last?.groupId != groups[i] { out.append((groups[i], [])) }
+                    out[out.count - 1].hits.append((ids[i], scores[i]))
+                }
+                return out
+            }
+        }
+    }
+
     public func add(frameId: UInt64, vector: [Float]) async throws {
         try await addBatch(frameIds: [frameId], vectors: [vector])
     }

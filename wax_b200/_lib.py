@@ -57,6 +57,8 @@ SIGNATURES = {
     "wax_vs_set_groups": (C.c_int32, [_eng, _u64p, _u64p, C.c_uint64, _u64p]),
     "wax_vs_search_grouped": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_int64, C.c_uint32, _u64p, C.c_uint64, C.c_int32,
                                           _u64p, _f32p, _u64p, C.c_uint32, _u32p]),
+    "wax_vs_search_batch_grouped": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, C.c_uint32, _u64p,
+                                                C.c_uint64, C.c_int32, _u64p, _f32p, _u64p, C.c_uint32, _u32p]),
     "wax_vs_search_batch": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _f32p,
                                         C.c_uint32, _u32p]),
     "wax_vs_search_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, C.c_uint64, C.c_void_p,

@@ -37,6 +37,7 @@
 #include "waxvs_batch.cuh"
 
 #include "waxvs_group.cuh"
+#include "waxvs_group_batch.cuh"
 
 #include <cub/cub.cuh>
 #include <cudaTypedefs.h>
@@ -231,6 +232,13 @@ struct SearchCtx {
     DevBuf<ExpandItem> d_expand_items;             // grouped search: expansion work items, all levels
     DevBuf<uint64_t> d_expand[3];                  // grouped search: expansion lists (two level buffers, the result)
     PinnedBuf<uint64_t> h_expand;
+    DevBuf<uint64_t> d_bg_keys;                    // batched grouped search: [query][top_groups][per_group] result keys
+    PinnedBuf<uint64_t> h_bg_keys;
+    DevBuf<uint32_t> d_bg_status;                  // batched grouped search: covered flag per query, then the expansion count
+    PinnedBuf<uint32_t> h_bg_status;
+    DevBuf<CoverExpand> d_bg_expand;               // batched grouped search: the groups to expand
+    PinnedBuf<CoverExpand> h_bg_expand;
+    DevBuf<ScoreItem> d_score_items;               // batched grouped search: expansion tiles (level 0)
     PinnedBuf<unsigned long long> h_flag;          // host-delivery completion flag
     unsigned long long host_seq = 0;               // last value the flag was asked to take
     ~SearchCtx() {                                 // the buffers release themselves
@@ -299,6 +307,7 @@ struct wax_vs_engine {
     } gindex;
     std::mutex group_mu;
     uint64_t group_index_builds = 0;   // instrumentation (pool_mu)
+    uint64_t grouped_batch_covered_queries = 0, grouped_batch_expanded_groups = 0, grouped_batch_fallback_queries = 0;
     // Adaptive level choice: when more than a quarter of a batch fails the coarse bf16 bound (tightly clustered
     // neighbours), the next 16 batches nominate in TF32 straight away, then bf16 is probed again.
     uint32_t bf16_skip_batches = 0;
@@ -2375,81 +2384,75 @@ static int32_t build_filter_bits(wax_vs_engine *e, SearchCtx *c, const std::vect
 //    scan each with its own k_i.
 // The bitsets are built on the device; a pass holds at most filter_bitset_bytes of them, more filters run in several
 // sub-batches (queries sorted by filter, so each filter's bitset is built once).
-static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                    int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                    const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                    uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    if (!e || !out_n || !filter_offsets || (n_filters && !filter_modes) || (n_queries && !query_filter))
-        return fail(WAX_VS_ERR_NULL, "NULL argument");
-    for (uint32_t f = 0; f < n_filters; ++f)
-        if (filter_modes[f] != 0 && filter_modes[f] != 1)
-            return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
-    if (filter_offsets[0] != 0) return fail(WAX_VS_ERR_ARGUMENT, "filter_offsets[0] must be 0");
-    for (uint32_t f = 0; f < n_filters; ++f)
-        if (filter_offsets[f + 1] < filter_offsets[f])
-            return fail(WAX_VS_ERR_ARGUMENT, "filter_offsets decrease at filter %u", f);
-    if (filter_offsets[n_filters] && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+// The filters of a call, resolved once: filter f's distinct rows are rows[first[f] .. first[f] + count[f]).
+struct FilterSet {
+    std::vector<uint32_t> rows;
+    std::vector<uint64_t> first, count;
+    std::vector<uint8_t> referenced;            // filters some query names (the others are not resolved)
+};
+static void resolve_filters(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *filter_offsets, uint32_t n_filters,
+                            const uint32_t *query_filter, uint32_t n_queries, FilterSet &fs) {
+    fs.first.assign(n_filters, 0);
+    fs.count.assign(n_filters, 0);
+    fs.referenced.assign(n_filters, 0);
     for (uint32_t i = 0; i < n_queries; ++i)
-        if (query_filter[i] != WAX_VS_NO_FILTER && query_filter[i] >= n_filters)
-            return fail(WAX_VS_ERR_ARGUMENT, "query %u names filter %u of %u", i, query_filter[i], n_filters);
-    std::shared_lock<std::shared_mutex> r(e->rw);
-    for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
-    if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
-    if (!queries) return fail(WAX_VS_ERR_NULL, "query is NULL");
-    if (query_len != e->dims)
-        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
-
-    // (1) resolve each referenced filter once: filter f's distinct rows are rows[first[f] .. first[f] + count[f])
-    const uint64_t n_rows = e->n_rows;
-    const uint32_t words = static_cast<uint32_t>((n_rows + 31) / 32);
-    std::vector<uint64_t> first(n_filters, 0), count(n_filters, 0);
-    std::vector<uint8_t> referenced(n_filters, 0);
-    for (uint32_t i = 0; i < n_queries; ++i)
-        if (query_filter[i] != WAX_VS_NO_FILTER) referenced[query_filter[i]] = 1;
-    std::vector<uint32_t> rows, seen(words, 0u);
+        if (query_filter[i] != WAX_VS_NO_FILTER) fs.referenced[query_filter[i]] = 1;
+    std::vector<uint32_t> seen(static_cast<size_t>((e->n_rows + 31) / 32), 0u);
     for (uint32_t f = 0; f < n_filters; ++f) {
-        if (!referenced[f]) continue;
-        first[f] = rows.size();
-        count[f] = build_row_filter(e, frame_ids + filter_offsets[f], filter_offsets[f + 1] - filter_offsets[f], seen, rows);
+        if (!fs.referenced[f]) continue;
+        fs.first[f] = fs.rows.size();
+        fs.count[f] = build_row_filter(e, frame_ids + filter_offsets[f], filter_offsets[f + 1] - filter_offsets[f], seen, fs.rows);
     }
-    // (2) each query's k, (3) its class
+}
+
+// Each query's k and class.  Staged query j is query order[j] and fills k_of[j] of its k_max candidate slots; the staged
+// order is the tensor class, the gather class, the scan class, the first and last sorted by filter so that a sub-batch
+// names a run of consecutive filters (unfiltered queries last).  Queries whose filter allows nothing are not staged.
+struct FilteredPlan {
+    std::vector<uint32_t> order, k_of;
+    uint32_t k_max = 0, n_tensor = 0, n_gather = 0;
+};
+static void plan_filtered(const wax_vs_engine *e, int64_t top_k, const int32_t *filter_modes, const uint32_t *query_filter,
+                          uint32_t n_queries, const FilterSet &fs, FilteredPlan &plan) {
+    const uint64_t n_rows = e->n_rows;
     const uint32_t limit = clamp_topk(top_k);
     std::vector<uint32_t> tensor, gather, scan;                // query indices
     std::vector<uint32_t> k_of_query(n_queries, 0);
     uint32_t k_max = 0;
     for (uint32_t i = 0; i < n_queries; ++i) {
         const uint32_t f = query_filter[i];
-        const uint64_t allowed = f == WAX_VS_NO_FILTER ? n_rows : (filter_modes[f] == 0 ? count[f] : n_rows - count[f]);
+        const uint64_t allowed = f == WAX_VS_NO_FILTER ? n_rows : (filter_modes[f] == 0 ? fs.count[f] : n_rows - fs.count[f]);
         const uint32_t k = static_cast<uint32_t>(std::min<uint64_t>(limit, allowed));
         if (k == 0) continue;
         k_of_query[i] = k;
         k_max = std::max(k_max, k);
-        if (f != WAX_VS_NO_FILTER && filter_modes[f] == 0 && count[f] <= 16384) gather.push_back(i);
+        if (f != WAX_VS_NO_FILTER && filter_modes[f] == 0 && fs.count[f] <= 16384) gather.push_back(i);
         else if (allowed >= limit) tensor.push_back(i);
         else scan.push_back(i);
     }
-    if (k_max == 0) return WAX_VS_OK;
-    if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
-    if (out_stride < k_max) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, k_max);
-    // staged order: the tensor class, the gather class, the scan class; the first and last sorted by filter so that a
-    // sub-batch names a run of consecutive filters (unfiltered queries last)
     auto by_filter = [&](uint32_t a, uint32_t b) { return query_filter[a] < query_filter[b]; };
     std::stable_sort(tensor.begin(), tensor.end(), by_filter);
     std::stable_sort(scan.begin(), scan.end(), by_filter);
-    std::vector<uint32_t> order(tensor);
-    order.insert(order.end(), gather.begin(), gather.end());
-    order.insert(order.end(), scan.begin(), scan.end());
-    const uint32_t n_staged = static_cast<uint32_t>(order.size());
-    const uint32_t n_tensor = static_cast<uint32_t>(tensor.size()), n_gather = static_cast<uint32_t>(gather.size());
-    std::vector<uint32_t> k_of(n_staged);
-    for (uint32_t j = 0; j < n_staged; ++j) k_of[j] = k_of_query[order[j]];
+    plan.order = tensor;
+    plan.order.insert(plan.order.end(), gather.begin(), gather.end());
+    plan.order.insert(plan.order.end(), scan.begin(), scan.end());
+    plan.k_of.resize(plan.order.size());
+    for (size_t j = 0; j < plan.order.size(); ++j) plan.k_of[j] = k_of_query[plan.order[j]];
+    plan.k_max = k_max;
+    plan.n_tensor = static_cast<uint32_t>(tensor.size());
+    plan.n_gather = static_cast<uint32_t>(gather.size());
+}
 
-    DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    CtxLease lease(e);
-    int32_t rc = lease.acquire();
-    if (rc) return rc;
-    SearchCtx *c = lease.c;
+// The planned queries on c->stream: staged query j's candidates land at c->d_out[j * k_max], on the device.  Stages the
+// queries (c->d_queries, staged order) and the filters' rows (c->d_filter_rows).  plan.k_max > 0.
+static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries, const int32_t *filter_modes,
+                            uint32_t n_filters, const uint32_t *query_filter, const FilterSet &fs, const FilteredPlan &plan) {
+    const std::vector<uint32_t> &order = plan.order, &k_of = plan.k_of, &rows = fs.rows;
+    const std::vector<uint64_t> &first = fs.first, &count = fs.count;
+    const uint32_t k_max = plan.k_max, n_tensor = plan.n_tensor, n_gather = plan.n_gather;
+    const uint32_t n_staged = static_cast<uint32_t>(order.size());
+    const uint32_t words = static_cast<uint32_t>((e->n_rows + 31) / 32);
+    int32_t rc;
     const size_t ncand = static_cast<size_t>(n_staged) * k_max;       // staged query j's candidates at j * k_max
     if ((rc = stage_queries(e, c, queries, n_staged, c->stream, order.data()))) return rc;
     if ((rc = c->d_out.ensure(ncand, "result buffer"))) return rc;
@@ -2498,7 +2501,7 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
     // tensor and scan classes: sub-batches whose bitsets fit the budget (at least one always does)
     const uint64_t fit = std::max<uint64_t>(1, e->tune.filter_bitset_bytes / (static_cast<uint64_t>(words) * sizeof(uint32_t)));
     uint64_t distinct = 0;
-    for (uint32_t f = 0; f < n_filters; ++f) distinct += referenced[f];
+    for (uint32_t f = 0; f < n_filters; ++f) distinct += fs.referenced[f];
     const uint32_t per_pass = static_cast<uint32_t>(std::min<uint64_t>(fit, std::max<uint64_t>(distinct, 1)));
     // sized once for the largest pass: a later pass must not reallocate a buffer earlier launches still read
     if ((rc = c->d_mask.ensure(static_cast<size_t>(per_pass) * words, "row filters"))) return rc;
@@ -2556,9 +2559,52 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
         std::lock_guard<std::mutex> pg(e->pool_mu);
         e->filter_bitset_passes += passes;
     }
+    return WAX_VS_OK;
+}
+
+static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                    int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                    const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                    uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    if (!e || !out_n || !filter_offsets || (n_filters && !filter_modes) || (n_queries && !query_filter))
+        return fail(WAX_VS_ERR_NULL, "NULL argument");
+    for (uint32_t f = 0; f < n_filters; ++f)
+        if (filter_modes[f] != 0 && filter_modes[f] != 1)
+            return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
+    if (filter_offsets[0] != 0) return fail(WAX_VS_ERR_ARGUMENT, "filter_offsets[0] must be 0");
+    for (uint32_t f = 0; f < n_filters; ++f)
+        if (filter_offsets[f + 1] < filter_offsets[f])
+            return fail(WAX_VS_ERR_ARGUMENT, "filter_offsets decrease at filter %u", f);
+    if (filter_offsets[n_filters] && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    for (uint32_t i = 0; i < n_queries; ++i)
+        if (query_filter[i] != WAX_VS_NO_FILTER && query_filter[i] >= n_filters)
+            return fail(WAX_VS_ERR_ARGUMENT, "query %u names filter %u of %u", i, query_filter[i], n_filters);
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
+    if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
+    if (!queries) return fail(WAX_VS_ERR_NULL, "query is NULL");
+    if (query_len != e->dims)
+        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
+    FilterSet fs;
+    resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, fs);
+    FilteredPlan plan;
+    plan_filtered(e, top_k, filter_modes, query_filter, n_queries, fs, plan);
+    const uint32_t k_max = plan.k_max, n_staged = static_cast<uint32_t>(plan.order.size());
+    if (k_max == 0) return WAX_VS_OK;
+    if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
+    if (out_stride < k_max) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, k_max);
+
+    DeviceGuard g(e->device);
+    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
+    if (rc) return rc;
+    SearchCtx *c = lease.c;
+    if ((rc = run_filtered(e, c, queries, filter_modes, n_filters, query_filter, fs, plan))) return rc;
+    const size_t ncand = static_cast<size_t>(n_staged) * k_max;
     CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, ncand * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));   // also keeps the host arrays alive until their copies are done
-    deliver_results(e, c->h_out, n_staged, k_max, out_ids, out_scores, out_stride, out_n, order.data(), k_of.data());
+    deliver_results(e, c->h_out, n_staged, k_max, out_ids, out_scores, out_stride, out_n, plan.order.data(), plan.k_of.data());
     return WAX_VS_OK;
 }
 
@@ -2715,43 +2761,106 @@ static float host_from_orderable(uint32_t k) {       // inverse of orderable_u32
     return f;
 }
 
-int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_groups,
-                              uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
-                              uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_cap,
-                              uint32_t *out_n) {
-    if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
+// Grouped argument checks, before the empty-engine early return (single and batched forms); *n_top = clamp(top_groups).
+static int32_t check_grouped_args(wax_vs_engine *e, bool outputs, int64_t top_groups, uint32_t per_group,
+                                  const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint32_t *n_top) {
+    if (!e || !outputs) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (per_group == 0 || per_group > WAX_VS_MAX_PER_GROUP)
         return fail(WAX_VS_ERR_ARGUMENT, "per_group must be in [1, %d] (got %u)", WAX_VS_MAX_PER_GROUP, per_group);
-    const uint32_t n_top = clamp_topk(top_groups);
-    if (static_cast<uint64_t>(n_top) * per_group > WAX_VS_MAX_RESULTS)
+    *n_top = clamp_topk(top_groups);
+    if (static_cast<uint64_t>(*n_top) * per_group > WAX_VS_MAX_RESULTS)
         return fail(WAX_VS_ERR_ARGUMENT, "clamp(top_groups) x per_group = %llu exceeds %d",
-                    static_cast<unsigned long long>(n_top) * per_group, WAX_VS_MAX_RESULTS);
+                    static_cast<unsigned long long>(*n_top) * per_group, WAX_VS_MAX_RESULTS);
     if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
     if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
-    std::shared_lock<std::shared_mutex> r(e->rw);
-    *out_n = 0;
-    if (e->n_rows == 0) return WAX_VS_OK;                // as wax_vs_search (:448)
-    if (!query) return fail(WAX_VS_ERR_NULL, "query is NULL");
-    if (query_len != e->dims)
-        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
-    const uint32_t n = static_cast<uint32_t>(e->n_rows);
-    const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(n_top) * per_group, n));
-    if (out_cap < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_cap, need);
-    const bool filtered = !(mode == 1 && n_ids == 0);
-    std::vector<uint32_t> rows;
-    if (filtered) {
-        std::vector<uint32_t> seen(static_cast<size_t>((n + 31) / 32), 0u);
-        build_row_filter(e, frame_ids, n_ids, seen, rows);
-        if (mode == 0 && rows.empty()) return WAX_VS_OK;                 // nothing allowed
-        if (mode == 1 && rows.size() == n) return WAX_VS_OK;             // everything denied
+    return WAX_VS_OK;
+}
+
+// Expansion plan: span i = (first CSR position, rows, result offset) gets its per_group best rows at its result offset.
+// Level 0 sorts tiles of kExpandTile CSR positions, each later level merges kExpandTile / per_group of the previous
+// level's lists, until one list per span is left (a span of one tile is final at level 0).  Level l > 0 reads the level
+// buffer (l - 1) & 1 and writes l & 1; buf_keys = the keys each buffer must hold.
+struct ExpandPlan {
+    std::vector<std::vector<ExpandItem>> levels;   // level 0: begin = CSR position
+    std::vector<uint32_t> tile_span;               // level-0 item -> its span
+    uint64_t buf_keys[2] = {0, 0};
+};
+static void plan_expansion(const std::vector<uint3> &spans, uint32_t per_group, ExpandPlan &plan) {
+    struct Pending { uint32_t dst, lists, off; };
+    plan.levels.assign(1, {});
+    plan.tile_span.clear();
+    plan.buf_keys[0] = plan.buf_keys[1] = 0;
+    std::vector<Pending> pending;
+    uint32_t off = 0;
+    for (uint32_t i = 0; i < static_cast<uint32_t>(spans.size()); ++i) {
+        const uint3 sp_i = spans[i];
+        const uint32_t tiles = (sp_i.y + kExpandTile - 1) / kExpandTile;
+        if (tiles == 1) {
+            plan.levels[0].push_back({sp_i.x, sp_i.y, sp_i.z, 1u});
+            plan.tile_span.push_back(i);
+            continue;
+        }
+        for (uint32_t t = 0; t < tiles; ++t) {
+            plan.levels[0].push_back({sp_i.x + t * kExpandTile, std::min(kExpandTile, sp_i.y - t * kExpandTile), off + t * per_group, 0u});
+            plan.tile_span.push_back(i);
+        }
+        pending.push_back({sp_i.z, tiles, off});
+        off += tiles * per_group;
     }
-    DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    CtxLease lease(e);
-    int32_t rc = lease.acquire();
-    if (rc) return rc;
-    SearchCtx *c = lease.c;
+    plan.buf_keys[0] = off;
+    const uint32_t fan = kExpandTile / per_group;
+    while (!pending.empty()) {
+        const size_t lv = plan.levels.size();
+        plan.levels.emplace_back();
+        std::vector<Pending> next;
+        off = 0;
+        for (const Pending &pd : pending) {
+            const uint32_t m = (pd.lists + fan - 1) / fan;
+            if (m == 1) { plan.levels[lv].push_back({pd.off, pd.lists * per_group, pd.dst, 1u}); continue; }
+            for (uint32_t t = 0; t < m; ++t)
+                plan.levels[lv].push_back({pd.off + t * fan * per_group, std::min(fan, pd.lists - t * fan) * per_group,
+                                           off + t * per_group, 0u});
+            next.push_back({pd.dst, m, off});
+            off += m * per_group;
+        }
+        plan.buf_keys[lv & 1] = std::max<uint64_t>(plan.buf_keys[lv & 1], off);
+        pending.swap(next);
+    }
+}
+
+// Grouped delivery: row -> frame id and group id, distance -> score, as entry m of the outputs.
+static void deliver_group_row(const wax_vs_engine *e, uint32_t row, float d, uint32_t m, uint64_t *out_ids, float *out_scores,
+                              uint64_t *out_groups) {
+    const uint64_t id = e->ids_identity ? e->id_base + row : e->ids[row];
+    out_ids[m] = id;
+    out_scores[m] = score_from_distance(e->similarity, d);
+    out_groups[m] = e->groups_set ? e->groups[row] : id;
+}
+// n_slots groups of per_group keys (dist_key << 32 | row), group-major, each group's list ending at its first
+// WAXVS_KEY_NONE -> entries; returns how many.
+static uint32_t deliver_group_keys(const wax_vs_engine *e, const uint64_t *keys, uint32_t n_slots, uint32_t per_group,
+                                   uint64_t *out_ids, float *out_scores, uint64_t *out_groups) {
+    uint32_t m = 0;
+    for (uint32_t i = 0; i < n_slots; ++i)
+        for (uint32_t j = 0; j < per_group; ++j) {
+            const uint64_t key = keys[static_cast<size_t>(i) * per_group + j];
+            if (key == WAXVS_KEY_NONE) break;
+            deliver_group_row(e, static_cast<uint32_t>(key), host_from_orderable(static_cast<uint32_t>(key >> 32)), m++, out_ids,
+                              out_scores, out_groups);
+        }
+    return m;
+}
+
+// One grouped search under the caller's read lock and scratch context (re-taking the shared lock inside a batch could
+// wait behind a queued writer): the host query, the filter's resolved rows (nullptr: unfiltered; the filter allows some
+// row), the answer at out_* and *out_n.  The arguments are checked by the caller.
+static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, uint32_t n_top, uint32_t per_group,
+                           const std::vector<uint32_t> *rows, int32_t mode, uint64_t *out_ids, float *out_scores,
+                           uint64_t *out_groups, uint32_t *out_n) {
+    const uint32_t n = static_cast<uint32_t>(e->n_rows);
+    const bool filtered = rows != nullptr;
     cudaStream_t s = c->stream;
+    int32_t rc;
     if ((rc = ensure_group_index(e, c))) return rc;
     const auto &gi = e->gindex;
     uint64_t launches = 0;
@@ -2761,10 +2870,10 @@ int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t que
     if ((rc = c->d_out.ensure(n_top, "result buffer"))) return rc;
     if ((rc = c->h_out.ensure(n_top, "result staging"))) return rc;
     if (filtered) {
-        if ((rc = c->d_filter_rows.ensure(std::max<size_t>(rows.size(), 1), "filter rows"))) return rc;
-        if (!rows.empty())
-            CUDA_TRY(cudaMemcpyAsync(c->d_filter_rows, rows.data(), rows.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-        const std::vector<uint64_t> spec = {0, rows.size(), 0, static_cast<uint64_t>(mode)};
+        if ((rc = c->d_filter_rows.ensure(std::max<size_t>(rows->size(), 1), "filter rows"))) return rc;
+        if (!rows->empty())
+            CUDA_TRY(cudaMemcpyAsync(c->d_filter_rows, rows->data(), rows->size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+        const std::vector<uint64_t> spec = {0, rows->size(), 0, static_cast<uint64_t>(mode)};
         if ((rc = build_filter_bits(e, c, spec, 1, s, &launches))) { cudaStreamSynchronize(s); return rc; }
     }
     if ((rc = enqueue_search(e, c, c->d_queries, 1, 0, c->d_out, nullptr, s, &launches, filtered ? c->d_mask.p : nullptr,
@@ -2788,11 +2897,9 @@ int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t que
     sp.k = n_top; sp.out = c->d_out;
     if ((rc = enqueue_select(e, c, c->d_group_keys, n, n_top, sp, s, &launches))) { cudaStreamSynchronize(s); return rc; }
     CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, n_top * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, s));
-    const uint64_t *h_keys = nullptr;                 // per_group > 1: [selected][per_group] keys, group-major
     uint32_t n_sel = 0;
     if (per_group > 1) {
-        // (4) expansion: each selected group's per_group best rows.  Level 0 sorts tiles of kExpandTile CSR positions,
-        // each later level merges kExpandTile / per_group of the previous level's lists, until one list per group is left.
+        // (4) expansion: each selected group's per_group best rows (plan_expansion)
         if ((rc = c->d_group_spans.ensure(n_top, "group spans")) || (rc = c->h_group_spans.ensure(n_top, "group span staging")))
             return rc;
         group_spans_kernel<<<(n_top + 255) / 256, 256, 0, s>>>(c->d_out, n_top, gi.row_group, gi.starts, c->d_group_spans);
@@ -2801,52 +2908,23 @@ int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t que
         CUDA_TRY(cudaMemcpyAsync(c->h_group_spans, c->d_group_spans, n_top * sizeof(uint2), cudaMemcpyDeviceToHost, s));
         CUDA_TRY(cudaStreamSynchronize(s));
         while (n_sel < n_top && c->h_group_spans[n_sel].y > 0) ++n_sel;   // valid candidates come first
-        struct Pending { uint32_t group, lists, off; };
-        std::vector<std::vector<ExpandItem>> levels(1);
-        std::vector<Pending> pending;
-        uint64_t buf_keys[2] = {0, 0};
-        uint32_t off = 0;
-        for (uint32_t i = 0; i < n_sel; ++i) {
-            const uint2 sp_i = c->h_group_spans[i];
-            const uint32_t tiles = (sp_i.y + kExpandTile - 1) / kExpandTile;
-            if (tiles == 1) { levels[0].push_back({sp_i.x, sp_i.y, i * per_group, 1u}); continue; }
-            for (uint32_t t = 0; t < tiles; ++t)
-                levels[0].push_back({sp_i.x + t * kExpandTile, std::min(kExpandTile, sp_i.y - t * kExpandTile), off + t * per_group, 0u});
-            pending.push_back({i, tiles, off});
-            off += tiles * per_group;
-        }
-        buf_keys[0] = off;
-        const uint32_t fan = kExpandTile / per_group;
-        while (!pending.empty()) {
-            const size_t lv = levels.size();
-            levels.emplace_back();
-            std::vector<Pending> next;
-            off = 0;
-            for (const Pending &pd : pending) {
-                const uint32_t m = (pd.lists + fan - 1) / fan;
-                if (m == 1) { levels[lv].push_back({pd.off, pd.lists * per_group, pd.group * per_group, 1u}); continue; }
-                for (uint32_t t = 0; t < m; ++t)
-                    levels[lv].push_back({pd.off + t * fan * per_group, std::min(fan, pd.lists - t * fan) * per_group,
-                                          off + t * per_group, 0u});
-                next.push_back({pd.group, m, off});
-                off += m * per_group;
-            }
-            buf_keys[lv & 1] = std::max<uint64_t>(buf_keys[lv & 1], off);
-            pending.swap(next);
-        }
+        std::vector<uint3> spans(n_sel);
+        for (uint32_t i = 0; i < n_sel; ++i) spans[i] = make_uint3(c->h_group_spans[i].x, c->h_group_spans[i].y, i * per_group);
+        ExpandPlan plan;
+        plan_expansion(spans, per_group, plan);
         std::vector<ExpandItem> all;
-        for (const auto &lvl : levels) all.insert(all.end(), lvl.begin(), lvl.end());
+        for (const auto &lvl : plan.levels) all.insert(all.end(), lvl.begin(), lvl.end());
         const size_t n_res = static_cast<size_t>(std::max<uint32_t>(n_sel, 1)) * per_group;
         if ((rc = c->d_expand_items.ensure(std::max<size_t>(all.size(), 1), "expansion items")) ||
-            (rc = c->d_expand[0].ensure(std::max<uint64_t>(buf_keys[0], 1), "expansion lists")) ||
-            (rc = c->d_expand[1].ensure(std::max<uint64_t>(buf_keys[1], 1), "expansion lists")) ||
+            (rc = c->d_expand[0].ensure(std::max<uint64_t>(plan.buf_keys[0], 1), "expansion lists")) ||
+            (rc = c->d_expand[1].ensure(std::max<uint64_t>(plan.buf_keys[1], 1), "expansion lists")) ||
             (rc = c->d_expand[2].ensure(n_res, "expansion result")) || (rc = c->h_expand.ensure(n_res, "expansion staging")))
             return rc;
         if (!all.empty())
             CUDA_TRY(cudaMemcpyAsync(c->d_expand_items, all.data(), all.size() * sizeof(ExpandItem), cudaMemcpyHostToDevice, s));
         size_t first_item = 0;
-        for (size_t lv = 0; lv < levels.size(); ++lv) {
-            const uint32_t items = static_cast<uint32_t>(levels[lv].size());
+        for (size_t lv = 0; lv < plan.levels.size(); ++lv) {
+            const uint32_t items = static_cast<uint32_t>(plan.levels[lv].size());
             if (items) {
                 group_expand_kernel<<<items, 1024, 0, s>>>(c->d_expand_items + first_item, lv == 0 ? 1u : 0u, gi.perm,
                                                            c->d_dist_keys, lv ? c->d_expand[(lv - 1) & 1].p : nullptr,
@@ -2859,29 +2937,233 @@ int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t que
         if (n_sel)
             CUDA_TRY(cudaMemcpyAsync(c->h_expand, c->d_expand[2], static_cast<size_t>(n_sel) * per_group * sizeof(uint64_t),
                                      cudaMemcpyDeviceToHost, s));
-        h_keys = c->h_expand;
+        CUDA_TRY(cudaStreamSynchronize(s));          // also keeps the item list alive until its copy is done
+        *out_n = deliver_group_keys(e, c->h_expand, n_sel, per_group, out_ids, out_scores, out_groups);
+        return WAX_VS_OK;
     }
-    CUDA_TRY(cudaStreamSynchronize(s));              // also keeps `rows` and the item list alive until their copies are done
+    CUDA_TRY(cudaStreamSynchronize(s));              // also keeps `rows` alive until its copy is done
     // (5) delivery: row -> frame id and group id, distance -> score
-    auto deliver = [&](uint32_t m, uint32_t row, float d) {
-        const uint64_t id = e->ids_identity ? e->id_base + row : e->ids[row];
-        out_ids[m] = id;
-        out_scores[m] = score_from_distance(e->similarity, d);
-        out_groups[m] = e->groups_set ? e->groups[row] : id;
-    };
     uint32_t m = 0;
-    if (per_group == 1) {
-        for (uint32_t i = 0; i < n_top; ++i)
-            if (c->h_out[i].valid) deliver(m++, static_cast<uint32_t>(c->h_out[i].row), c->h_out[i].distance);
-    } else {
-        for (uint32_t i = 0; i < n_sel; ++i)
-            for (uint32_t j = 0; j < per_group; ++j) {
-                const uint64_t key = h_keys[static_cast<size_t>(i) * per_group + j];
-                if (key == WAXVS_KEY_NONE) break;
-                deliver(m++, static_cast<uint32_t>(key), host_from_orderable(static_cast<uint32_t>(key >> 32)));
-            }
-    }
+    for (uint32_t i = 0; i < n_top; ++i)
+        if (c->h_out[i].valid)
+            deliver_group_row(e, static_cast<uint32_t>(c->h_out[i].row), c->h_out[i].distance, m++, out_ids, out_scores, out_groups);
     *out_n = m;
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_groups,
+                              uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                              uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_cap,
+                              uint32_t *out_n) {
+    uint32_t n_top = 0;
+    int32_t rc = check_grouped_args(e, out_n && out_ids && out_scores && out_groups, top_groups, per_group, frame_ids, n_ids,
+                                    mode, &n_top);
+    if (rc) return rc;
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    *out_n = 0;
+    if (e->n_rows == 0) return WAX_VS_OK;                // as wax_vs_search (:448)
+    if (!query) return fail(WAX_VS_ERR_NULL, "query is NULL");
+    if (query_len != e->dims)
+        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
+    const uint32_t n = static_cast<uint32_t>(e->n_rows);
+    const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(n_top) * per_group, n));
+    if (out_cap < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_cap, need);
+    const bool filtered = !(mode == 1 && n_ids == 0);
+    std::vector<uint32_t> rows;
+    if (filtered) {
+        std::vector<uint32_t> seen(static_cast<size_t>((n + 31) / 32), 0u);
+        build_row_filter(e, frame_ids, n_ids, seen, rows);
+        if (mode == 0 && rows.empty()) return WAX_VS_OK;                 // nothing allowed
+        if (mode == 1 && rows.size() == n) return WAX_VS_OK;             // everything denied
+    }
+    DeviceGuard g(e->device);
+    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    CtxLease lease(e);
+    if ((rc = lease.acquire())) return rc;
+    return grouped_one(e, lease.c, query, n_top, per_group, filtered ? &rows : nullptr, mode, out_ids, out_scores, out_groups,
+                       out_n);
+}
+
+// ---- batched grouped search (waxvs_group_batch.cuh) -----------------------------------------------------------------
+constexpr uint64_t kExpandBatchKeys = 1ull << 24;   // level-buffer keys one round of batched expansions may hold
+
+// The expansions the cover kernel listed, (query, slot, span) sorted, into the batch's result keys c->d_bg_keys: level 0
+// scores the CSR tiles for the item's query (group_score_tile_kernel), the later levels merge as the single query does.
+// Rounds of spans keep the level buffers within kExpandBatchKeys; the buffers are sized once for the largest round.
+static int32_t enqueue_batch_expansion(wax_vs_engine *e, SearchCtx *c, const CoverExpand *list, uint32_t n_list,
+                                       uint32_t n_top, uint32_t per_group, const uint32_t *d_mask, uint64_t *launches) {
+    struct Round { ExpandPlan plan; std::vector<uint32_t> span_query; };
+    std::vector<Round> rounds;
+    std::vector<uint3> spans;
+    std::vector<uint32_t> span_query;
+    uint64_t round_keys = 0;
+    auto close_round = [&]() {
+        rounds.emplace_back();
+        plan_expansion(spans, per_group, rounds.back().plan);
+        rounds.back().span_query.swap(span_query);
+        spans.clear();
+        round_keys = 0;
+    };
+    for (uint32_t i = 0; i < n_list; ++i) {
+        const CoverExpand &x = list[i];
+        const uint64_t keys = static_cast<uint64_t>((x.count + kExpandTile - 1) / kExpandTile) * per_group;
+        if (!spans.empty() && round_keys + keys > kExpandBatchKeys) close_round();
+        spans.push_back(make_uint3(x.begin, x.count, (x.query * n_top + x.slot) * per_group));
+        span_query.push_back(x.query);
+        round_keys += keys;
+    }
+    if (!spans.empty()) close_round();
+    std::vector<ScoreItem> tiles;
+    std::vector<ExpandItem> merges;
+    uint64_t buf[2] = {1, 1};
+    for (const Round &rd : rounds) {
+        for (size_t t = 0; t < rd.plan.levels[0].size(); ++t) {
+            const ExpandItem &it = rd.plan.levels[0][t];
+            tiles.push_back({rd.span_query[rd.plan.tile_span[t]], it.begin, it.count, it.dst_off, it.final_out});
+        }
+        for (size_t lv = 1; lv < rd.plan.levels.size(); ++lv)
+            merges.insert(merges.end(), rd.plan.levels[lv].begin(), rd.plan.levels[lv].end());
+        buf[0] = std::max(buf[0], rd.plan.buf_keys[0]);
+        buf[1] = std::max(buf[1], rd.plan.buf_keys[1]);
+    }
+    cudaStream_t s = c->stream;
+    int32_t rc;
+    if ((rc = c->d_score_items.ensure(std::max<size_t>(tiles.size(), 1), "expansion tiles")) ||
+        (rc = c->d_expand_items.ensure(std::max<size_t>(merges.size(), 1), "expansion items")) ||
+        (rc = c->d_expand[0].ensure(buf[0], "expansion lists")) || (rc = c->d_expand[1].ensure(buf[1], "expansion lists")))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_score_items, tiles.data(), tiles.size() * sizeof(ScoreItem), cudaMemcpyHostToDevice, s));
+    if (!merges.empty())
+        CUDA_TRY(cudaMemcpyAsync(c->d_expand_items, merges.data(), merges.size() * sizeof(ExpandItem), cudaMemcpyHostToDevice, s));
+    const auto score = e->similarity == WAX_VS_COSINE ? group_score_tile_kernel<kCosine>
+                       : e->similarity == WAX_VS_DOT  ? group_score_tile_kernel<kDot>
+                                                      : group_score_tile_kernel<kL2>;
+    size_t first_tile = 0, first_merge = 0;
+    for (const Round &rd : rounds) {
+        const uint32_t n0 = static_cast<uint32_t>(rd.plan.levels[0].size());
+        score<<<n0, 256, 0, s>>>(c->d_score_items + first_tile, e->d_corpus, c->d_queries, e->dims, e->gindex.perm, d_mask,
+                                  per_group, c->d_expand[0], c->d_bg_keys);
+        CUDA_TRY(cudaGetLastError());
+        ++*launches;
+        first_tile += n0;
+        for (size_t lv = 1; lv < rd.plan.levels.size(); ++lv) {
+            const uint32_t items = static_cast<uint32_t>(rd.plan.levels[lv].size());
+            group_expand_kernel<<<items, 1024, 0, s>>>(c->d_expand_items + first_merge, 0u, e->gindex.perm, nullptr,
+                                                       c->d_expand[(lv - 1) & 1], per_group, c->d_expand[lv & 1], c->d_bg_keys);
+            CUDA_TRY(cudaGetLastError());
+            ++*launches;
+            first_merge += items;
+        }
+    }
+    CUDA_TRY(cudaStreamSynchronize(s));              // also keeps the item lists alive until their copies are done
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_search_batch_grouped(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                    int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
+                                    int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
+                                    uint32_t out_stride, uint32_t *out_n) {
+    uint32_t n_top = 0;
+    int32_t rc = check_grouped_args(e, out_n && out_ids && out_scores && out_groups, top_groups, per_group, frame_ids, n_ids,
+                                    mode, &n_top);
+    if (rc) return rc;
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
+    if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
+    if (!queries) return fail(WAX_VS_ERR_NULL, "query is NULL");
+    if (query_len != e->dims)
+        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
+    const uint32_t n = static_cast<uint32_t>(e->n_rows);
+    const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(n_top) * per_group, n));
+    if (out_stride < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, need);
+    // one filter that every query names, resolved once (none when unfiltered)
+    const bool filtered = !(mode == 1 && n_ids == 0);
+    const uint64_t offsets[2] = {0, n_ids};
+    const std::vector<uint32_t> query_filter(n_queries, filtered ? 0u : WAX_VS_NO_FILTER);
+    FilterSet fs;
+    resolve_filters(e, frame_ids, offsets, filtered ? 1u : 0u, query_filter.data(), n_queries, fs);
+    if (filtered && mode == 0 && fs.rows.empty()) return WAX_VS_OK;              // nothing allowed
+    if (filtered && mode == 1 && fs.rows.size() == n) return WAX_VS_OK;          // everything denied
+    // The coverage level: each query's exact top-k_c rows, when the batch goes to the tensor-core levels or the gather
+    // class of the batched filtered search; every other batch runs the single-query pipeline per query.
+    const uint32_t k_c = std::min(kCoverMax, std::max(128u, 4u * n_top));
+    FilteredPlan plan;
+    bool cover = n_top <= kCoverMax / 4;
+    if (cover) {
+        plan_filtered(e, k_c, &mode, query_filter.data(), n_queries, fs, plan);
+        const uint32_t n_staged = static_cast<uint32_t>(plan.order.size());
+        cover = n_staged == n_queries && (plan.n_gather == n_staged ||
+                                          (plan.n_tensor == n_staged && batch_tensor_eligible(e, n_staged, plan.k_max)));
+    }
+    DeviceGuard g(e->device);
+    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    CtxLease lease(e);
+    if ((rc = lease.acquire())) return rc;
+    SearchCtx *c = lease.c;
+    cudaStream_t s = c->stream;
+    std::vector<uint32_t> crowded;                   // queries for the single-query pipeline
+    uint64_t covered = 0, expanded = 0, launches = 0;
+    if (!cover) {
+        for (uint32_t i = 0; i < n_queries; ++i) crowded.push_back(i);
+    } else {
+        if ((rc = ensure_group_index(e, c))) return rc;
+        if ((rc = run_filtered(e, c, queries, &mode, filtered ? 1u : 0u, query_filter.data(), fs, plan))) return rc;
+        const uint32_t nq = n_queries, slots = n_top * per_group;
+        const size_t nkeys = static_cast<size_t>(nq) * slots;
+        if ((rc = c->d_bg_keys.ensure(nkeys, "grouped batch keys")) || (rc = c->h_bg_keys.ensure(nkeys, "grouped batch staging")) ||
+            (rc = c->d_bg_status.ensure(nq + 1u, "grouped batch status")) ||
+            (rc = c->h_bg_status.ensure(nq + 1u, "grouped batch status staging")) ||
+            (rc = c->d_bg_expand.ensure(static_cast<size_t>(nq) * n_top, "grouped batch expansions")) ||
+            (rc = c->h_bg_expand.ensure(static_cast<size_t>(nq) * n_top, "grouped batch expansion staging")))
+            return rc;
+        CUDA_TRY(cudaMemsetAsync(c->d_bg_status + nq, 0, sizeof(uint32_t), s));
+        group_cover_kernel<<<nq, kCoverMax, 0, s>>>(c->d_out, plan.k_max, k_c, e->gindex.row_group, e->gindex.starts, n_top,
+                                                    per_group, c->d_bg_keys, c->d_bg_status, c->d_bg_expand, c->d_bg_status + nq);
+        CUDA_TRY(cudaGetLastError());
+        ++launches;
+        CUDA_TRY(cudaMemcpyAsync(c->h_bg_status, c->d_bg_status, (nq + 1u) * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        const uint32_t n_exp = c->h_bg_status[nq];
+        if (n_exp) {
+            CUDA_TRY(cudaMemcpyAsync(c->h_bg_expand, c->d_bg_expand, n_exp * sizeof(CoverExpand), cudaMemcpyDeviceToHost, s));
+            CUDA_TRY(cudaStreamSynchronize(s));
+            CoverExpand *list = c->h_bg_expand;      // appended in any order: sort for a reproducible launch plan
+            std::sort(list, list + n_exp, [](const CoverExpand &a, const CoverExpand &b) {
+                return a.query != b.query ? a.query < b.query : a.slot < b.slot;
+            });
+            if (filtered) {                          // the expansion consults the filter's bitset (rows staged by run_filtered)
+                const std::vector<uint64_t> spec = {0, fs.rows.size(), 0, static_cast<uint64_t>(mode)};
+                if ((rc = build_filter_bits(e, c, spec, 1, s, &launches))) { cudaStreamSynchronize(s); return rc; }
+            }
+            if ((rc = enqueue_batch_expansion(e, c, list, n_exp, n_top, per_group, filtered ? c->d_mask.p : nullptr, &launches))) {
+                cudaStreamSynchronize(s);
+                return rc;
+            }
+            expanded = n_exp;
+        }
+        CUDA_TRY(cudaMemcpyAsync(c->h_bg_keys, c->d_bg_keys, nkeys * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        for (uint32_t j = 0; j < nq; ++j) {
+            const uint32_t qi = plan.order[j];
+            if (!c->h_bg_status[j]) { crowded.push_back(qi); continue; }
+            const size_t o = static_cast<size_t>(qi) * out_stride;
+            out_n[qi] = deliver_group_keys(e, c->h_bg_keys + static_cast<size_t>(j) * slots, n_top, per_group, out_ids + o,
+                                           out_scores + o, out_groups + o);
+            ++covered;
+        }
+        std::sort(crowded.begin(), crowded.end());
+    }
+    // crowded queries (and batches the coverage level does not take): the single-query pipeline, same lock and context
+    for (uint32_t qi : crowded) {
+        const size_t o = static_cast<size_t>(qi) * out_stride;
+        if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group, filtered ? &fs.rows : nullptr,
+                              mode, out_ids + o, out_scores + o, out_groups + o, out_n + qi)))
+            return rc;
+    }
+    std::lock_guard<std::mutex> pg(e->pool_mu);
+    e->grouped_batch_covered_queries += covered;
+    e->grouped_batch_expanded_groups += expanded;
+    e->grouped_batch_fallback_queries += crowded.size();
     return WAX_VS_OK;
 }
 
@@ -3200,6 +3482,9 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "batch_tf32_queries")) *out = e->batch_tf32_queries;
     else if (!strcmp(name, "filter_bitset_passes")) *out = e->filter_bitset_passes;   // per-query filters: tensor sub-batches
     else if (!strcmp(name, "group_index_builds")) *out = e->group_index_builds;       // grouped search: device index builds
+    else if (!strcmp(name, "grouped_batch_covered_queries")) *out = e->grouped_batch_covered_queries;     // answered by the coverage level
+    else if (!strcmp(name, "grouped_batch_expanded_groups")) *out = e->grouped_batch_expanded_groups;     // (query, group) expansions
+    else if (!strcmp(name, "grouped_batch_fallback_queries")) *out = e->grouped_batch_fallback_queries;   // single-query pipeline
     else if (!strcmp(name, "ingest_h2d_bytes")) *out = e->ingest_h2d_bytes;
     else if (!strcmp(name, "ingest_d2h_bytes")) *out = e->ingest_d2h_bytes;
     else if (!strcmp(name, "norms_rows")) *out = e->norms_rows;       // rows whose cached 1/|v| is valid

@@ -340,6 +340,44 @@ class CUDAVectorEngine:
             out[-1][1].append((int(ids[i]), float(scores[i])))
         return out
 
+    def search_batch_grouped(self, vectors, top_groups: int, per_group: int = 1,
+                             allow: Optional[Sequence[int]] = None,
+                             deny: Optional[Sequence[int]] = None) -> List[List[Tuple[int, List[Tuple[int, float]]]]]:
+        """`search_grouped` for a batch of queries under ONE optional filter (wax_vs_search_batch_grouped): one
+        [(group_id, [(frame_id, score), ...]), ...] per query, each identical to search_grouped for that query alone.
+        The batch shares one tensor-core pass for its queries' top rows; crowded queries run the single-query path."""
+        if allow is not None and deny is not None:
+            raise ValueError("pass at most one of allow= / deny=")
+        fids = np.ascontiguousarray(allow if allow is not None else (deny if deny is not None else []),
+                                    dtype=np.uint64).reshape(-1)
+        mode = 0 if allow is not None else 1
+        qs = _as_rows(vectors, self.dimensions) if len(vectors) else np.zeros((0, self.dimensions), np.float32)
+        b = qs.shape[0]
+        if b == 0:
+            return []
+        cap = max(1, min(_clamp_topk(top_groups) * max(int(per_group), 1), L.MAX_RESULTS))
+        ids = np.empty((b, cap), np.uint64)
+        scores = np.empty((b, cap), np.float32)
+        groups = np.empty((b, cap), np.uint64)
+        ns = np.zeros(b, np.uint32)
+        _check(L.lib().wax_vs_search_batch_grouped(self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1],
+                                                   int(top_groups), int(per_group),
+                                                   fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
+                                                   fids.size, mode, ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                   scores.ctypes.data_as(C.POINTER(C.c_float)),
+                                                   groups.ctypes.data_as(C.POINTER(C.c_uint64)), cap,
+                                                   ns.ctypes.data_as(C.POINTER(C.c_uint32))))
+        result = []
+        for i in range(b):
+            out: List[Tuple[int, List[Tuple[int, float]]]] = []
+            for j in range(int(ns[i])):
+                g = int(groups[i, j])
+                if not out or out[-1][0] != g:
+                    out.append((g, []))
+                out[-1][1].append((int(ids[i, j]), float(scores[i, j])))
+            result.append(out)
+        return result
+
     def search_batch(self, vectors, top_k: int) -> List[List[Tuple[int, float]]]:
         """`search` for a batch of queries (wax_vs_search_batch): the same answers as one call per query.  Cosine and dot
         batches share one tensor-core pass over the corpus, l2 batches too once set_option("batch_l2", 1) is set."""

@@ -241,6 +241,37 @@ public:
         return out;
     }
 
+    // searchGrouped for a batch of queries under ONE filter (wax_vs_search_batch_grouped): one answer per query, each
+    // identical to searchGrouped for that query alone.
+    std::vector<std::vector<Group>> searchBatchGrouped(const std::vector<std::vector<float>> &vectors, int64_t topGroups,
+                                                       uint32_t perGroup = 1, const std::vector<uint64_t> &frameIds = {},
+                                                       bool allow = false) const {
+        std::vector<std::vector<Group>> out(vectors.size());
+        if (vectors.empty()) return out;
+        const int64_t lim = topGroups < 1 ? 1 : (topGroups > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topGroups);
+        const int64_t want = lim * (perGroup ? perGroup : 1);
+        const size_t cap = static_cast<size_t>(want > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : want);
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchGrouped: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        std::vector<uint64_t> ids(vectors.size() * cap), groups(vectors.size() * cap);
+        std::vector<float> scores(vectors.size() * cap);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_grouped(h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_, topGroups,
+                                          perGroup, frameIds.data(), frameIds.size(), allow ? 0 : 1, ids.data(),
+                                          scores.data(), groups.data(), static_cast<uint32_t>(cap), ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) {
+                const size_t j = q * cap + i;
+                if (out[q].empty() || out[q].back().first != groups[j]) out[q].push_back({groups[j], {}});
+                out[q].back().second.push_back({ids[j], scores[j]});
+            }
+        return out;
+    }
+
     // static load(from:metric:dimensions:) (MetalVectorEngine.swift:318-328): the committed blob (may be empty = none
     // committed yet), then the pending embedding mutations as ONE upsert batch (sequential semantics in the library).
     static CUDAVectorEngine *load(const std::vector<uint8_t> *committedBlob, const std::vector<uint64_t> &pendingIds,
