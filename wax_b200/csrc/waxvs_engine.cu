@@ -63,13 +63,14 @@ static int32_t fail(int32_t code, const char *fmt, ...) {
     } while (0)
 
 struct DeviceGuard {
-    int prev = -1;
+    int prev = -1, dev;
     bool ok = true;
-    explicit DeviceGuard(int dev) {
+    explicit DeviceGuard(int device) : dev(device) {
         if (cudaGetDevice(&prev) != cudaSuccess) { prev = -1; }
         if (prev != dev) ok = (cudaSetDevice(dev) == cudaSuccess);
     }
     ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+    int32_t error() const { return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", dev); }   // when !ok
 };
 
 // An owned allocation of `cap` elements: device memory, or (PINNED) mapped + portable host memory that kernels may write
@@ -1258,6 +1259,13 @@ static uint32_t find_row(wax_vs_engine *e, uint64_t id) {
     ensure_map(e);
     return e->map.find(id);
 }
+// frameId -> row (0xFFFFFFFF = absent) for implicit and explicit ids.  May build the hash table: the caller holds the
+// write lock or ids_mu.
+static uint32_t row_of(wax_vs_engine *e, uint64_t id) {
+    if (!e->ids_identity) return find_row(e, id);
+    return id >= e->id_base && id - e->id_base < e->n_rows ? static_cast<uint32_t>(id - e->id_base) : 0xFFFFFFFFu;
+}
+static uint64_t frame_id_of(const wax_vs_engine *e, uint64_t row) { return e->ids_identity ? e->id_base + row : e->ids[row]; }
 static int32_t sync_device_ids(wax_vs_engine *e, const uint64_t **out) {
     std::lock_guard<std::mutex> g(e->ids_mu);
     if (e->ids_identity) { *out = nullptr; return WAX_VS_OK; }
@@ -1633,14 +1641,9 @@ int32_t wax_vs_remove_batch(wax_vs_engine *e, const uint64_t *frame_ids, uint64_
     // which rows go
     std::vector<uint32_t> gone;
     gone.reserve(n);
-    if (e->ids_identity) {
-        for (uint64_t i = 0; i < n; ++i)
-            if (frame_ids[i] >= e->id_base && frame_ids[i] - e->id_base < e->n_rows) gone.push_back(static_cast<uint32_t>(frame_ids[i] - e->id_base));
-    } else {
-        for (uint64_t i = 0; i < n; ++i) {
-            const uint32_t r = find_row(e, frame_ids[i]);
-            if (r != 0xFFFFFFFFu) gone.push_back(r);                // :426 unknown id = no-op
-        }
+    for (uint64_t i = 0; i < n; ++i) {
+        const uint32_t r = row_of(e, frame_ids[i]);
+        if (r != 0xFFFFFFFFu) gone.push_back(r);                    // :426 unknown id = no-op
     }
     if (gone.empty()) return WAX_VS_OK;
     std::sort(gone.begin(), gone.end());
@@ -1904,12 +1907,20 @@ static void deliver_results(const wax_vs_engine *e, const wax_vs_candidate *cand
         for (uint32_t i = 0; i < kq; ++i) {
             const wax_vs_candidate &cd = cands[static_cast<size_t>(j) * k_eff + i];
             if (!cd.valid) continue;
-            out_ids[static_cast<size_t>(qi) * out_stride + m] = e->ids_identity ? e->id_base + cd.row : e->ids[cd.row];
+            out_ids[static_cast<size_t>(qi) * out_stride + m] = frame_id_of(e, cd.row);
             out_scores[static_cast<size_t>(qi) * out_stride + m] = score_from_distance(e->similarity, cd.distance);
             ++m;
         }
         out_n[qi] = m;
     }
+}
+
+// The query argument of the host-path search entry points (validate, :449, :830-833).
+static int32_t check_query(const wax_vs_engine *e, const float *query, uint32_t query_len) {
+    if (!query) return fail(WAX_VS_ERR_NULL, "query is NULL");
+    if (query_len != e->dims)
+        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
+    return WAX_VS_OK;
 }
 
 static int32_t search_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
@@ -1922,9 +1933,8 @@ static int32_t search_host(wax_vs_engine *e, const float *queries, uint32_t n_qu
         return WAX_VS_OK;
     }
     if (n_queries == 0) return WAX_VS_OK;
-    if (!queries) return fail(WAX_VS_ERR_NULL, "query is NULL");
-    if (query_len != e->dims)  // validate (:449, :830-833)
-        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
+    int32_t rc;
+    if ((rc = check_query(e, queries, query_len))) return rc;
     const uint32_t limit = clamp_topk(top_k);
     const uint32_t k_eff = static_cast<uint32_t>(std::min<uint64_t>(limit, e->n_rows));  // topKCount (:451)
     if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
@@ -1932,10 +1942,9 @@ static int32_t search_host(wax_vs_engine *e, const float *queries, uint32_t n_qu
         return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, k_eff);
 
     DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    if (!g.ok) return g.error();
     CtxLease lease(e);
-    int32_t rc = lease.acquire();
-    if (rc) return rc;
+    if ((rc = lease.acquire())) return rc;
     SearchCtx *c = lease.c;
 
     const size_t ncand = static_cast<size_t>(n_queries) * k_eff;
@@ -1989,7 +1998,7 @@ int32_t wax_vs_search_device(wax_vs_engine *e, const float *d_queries, uint32_t 
     if (!e || !d_queries || !d_candidates) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    if (!g.ok) return g.error();
     const uint32_t k_eff = clamp_topk(top_k);
     SearchCtx *c = nullptr;
     int32_t rc = ctx_for_stream(e, cuda_stream, &c);
@@ -2011,7 +2020,7 @@ int32_t wax_vs_search_batch_device(wax_vs_engine *e, const float *d_queries, uin
     if (n_queries == 0) return WAX_VS_OK;
     std::shared_lock<std::shared_mutex> r(e->rw);
     DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    if (!g.ok) return g.error();
     const uint32_t k_eff = clamp_topk(top_k);
     SearchCtx *c = nullptr;
     int32_t rc = ctx_for_stream(e, cuda_stream, &c);
@@ -2024,6 +2033,89 @@ int32_t wax_vs_search_batch_device(wax_vs_engine *e, const float *d_queries, uin
         return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_candidates, d_ids, c->stream,
                              &launches, RowFilter{}, false);
     return run_queries_on_device(e, c, d_queries, n_queries, k_eff, row_offset, d_candidates, d_ids, &launches);
+}
+
+// ---- filtered search (SURVEY.md section 8f-4) -------------------------------------------------------------------
+// The reference filters AFTER the engine call and over-fetches 3 x topK to compensate (UnifiedSearch.swift:58,
+// 371-442, 1195-1200, 1241-1258).  Here the filter is pushed below the top-k: a row bitset consulted only for rows
+// that would enter the list, or -- for small allow-lists -- a gather that scores only the listed rows.
+// frameIds -> the distinct rows of this engine they name, appended to `rows` (unknown and repeated ids are ignored).
+// `seen` is a zeroed scratch bitset of ceil(N / 32) words shared by all the filters of a call: only the words this
+// filter touched are cleared again, so no list is sorted and no bitset is rebuilt per filter.  Returns the rows appended.
+static uint64_t build_row_filter(wax_vs_engine *e, const uint64_t *frame_ids, uint64_t n_ids, std::vector<uint32_t> &seen,
+                                 std::vector<uint32_t> &rows) {
+    const size_t first = rows.size();
+    std::lock_guard<std::mutex> g(e->ids_mu);   // the lazily built id map is shared by concurrent readers
+    // (row_of builds the lazily constructed hash table when it is needed: serialised by ids_mu)
+    for (uint64_t i = 0; i < n_ids; ++i) {
+        const uint32_t row = row_of(e, frame_ids[i]);
+        if (row == 0xFFFFFFFFu) continue;
+        const uint32_t w = row >> 5, b = 1u << (row & 31u);
+        if (!(seen[w] & b)) { seen[w] |= b; rows.push_back(row); }
+    }
+    for (size_t i = first; i < rows.size(); ++i) seen[rows[i] >> 5] = 0u;
+    return rows.size() - first;
+}
+
+// The filters of a call, resolved once: filter f's distinct rows are rows[first[f] .. first[f] + count[f]).
+struct FilterSet {
+    std::vector<uint32_t> rows;
+    std::vector<uint64_t> first, count;
+    std::vector<uint8_t> referenced;            // filters some query names (the others are not resolved)
+};
+// query_filter = nullptr: every filter is resolved (the single-filter entry points).
+static void resolve_filters(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *filter_offsets, uint32_t n_filters,
+                            const uint32_t *query_filter, uint32_t n_queries, FilterSet &fs) {
+    fs.first.assign(n_filters, 0);
+    fs.count.assign(n_filters, 0);
+    fs.referenced.assign(n_filters, query_filter ? 0 : 1);
+    for (uint32_t i = 0; i < n_queries; ++i)
+        if (query_filter[i] != WAX_VS_NO_FILTER) fs.referenced[query_filter[i]] = 1;
+    std::vector<uint32_t> seen(static_cast<size_t>((e->n_rows + 31) / 32), 0u);
+    for (uint32_t f = 0; f < n_filters; ++f) {
+        if (!fs.referenced[f]) continue;
+        fs.first[f] = fs.rows.size();
+        fs.count[f] = build_row_filter(e, frame_ids + filter_offsets[f], filter_offsets[f + 1] - filter_offsets[f], seen, fs.rows);
+    }
+}
+
+// n_filters row bitsets of ceil(N / 32) words into c->d_mask on `stream`, from the resolved rows in c->d_filter_rows:
+// spec is filter_bits_init_kernel's (running row counts, where each filter's rows start, modes).  The host uploads
+// 4 bytes per listed row instead of N / 8 bytes per filter.  c->d_mask must not be reallocated while earlier
+// launches on `stream` still read it: callers size it first.
+static int32_t build_filter_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<uint64_t> &spec, uint32_t n_filters,
+                                 cudaStream_t stream, uint64_t *launches) {
+    const uint32_t words = static_cast<uint32_t>((e->n_rows + 31) / 32);
+    int32_t rc;
+    if ((rc = c->d_filter_spec.ensure(spec.size(), "filter spec"))) return rc;
+    if ((rc = c->d_mask.ensure(static_cast<size_t>(n_filters) * words, "row filters"))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_filter_spec, spec.data(), spec.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, stream));
+    const size_t total_words = static_cast<size_t>(n_filters) * words;
+    const int cap = e->sm_count * 8;
+    const int g1 = static_cast<int>(std::min<size_t>(cap, (total_words + 255) / 256));
+    filter_bits_init_kernel<<<std::max(g1, 1), 256, 0, stream>>>(c->d_mask, words, static_cast<uint32_t>(e->n_rows),
+                                                                 c->d_filter_spec, n_filters);
+    CUDA_TRY(cudaGetLastError());
+    ++*launches;
+    const uint64_t listed = spec[n_filters];
+    if (listed) {
+        const int g2 = static_cast<int>(std::min<uint64_t>(cap, (listed + 255) / 256));
+        filter_bits_apply_kernel<<<g2, 256, 0, stream>>>(c->d_mask, words, c->d_filter_rows, c->d_filter_spec, n_filters);
+        CUDA_TRY(cudaGetLastError());
+        ++*launches;
+    }
+    return WAX_VS_OK;
+}
+// The resolved rows into c->d_filter_rows on `stream`, after growing it to at least `reserve` rows; `rows` must outlive
+// the copy.  mode 0 (allow) / 1 (deny): also the bitset of `rows` as the one filter, into c->d_mask.
+static int32_t stage_filter_rows(wax_vs_engine *e, SearchCtx *c, const std::vector<uint32_t> &rows, size_t reserve,
+                                 int32_t mode, cudaStream_t stream, uint64_t *launches) {
+    int32_t rc;
+    if ((rc = c->d_filter_rows.ensure(std::max<size_t>(reserve, 1), "filter rows"))) return rc;
+    if (!rows.empty())
+        CUDA_TRY(cudaMemcpyAsync(c->d_filter_rows, rows.data(), rows.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+    if (mode < 0) return WAX_VS_OK;
+    return build_filter_bits(e, c, {0, rows.size(), 0, static_cast<uint64_t>(mode)}, 1, stream, launches);
 }
 
 // ---- row-sharded search: fused scan + NVLink exchange + merge (waxvs_shard.cuh; SURVEY.md section 8e) ---------------
@@ -2074,7 +2166,7 @@ int32_t wax_vs_shard_open(wax_vs_engine *e, int32_t rank, int32_t world, uint64_
         return fail(WAX_VS_ERR_ARGUMENT, "rank %d of %d: world must be 1..%d", rank, world, kShardMaxRanks);
     std::unique_lock<std::shared_mutex> w(e->rw);
     DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    if (!g.ok) return g.error();
     drain_device_path(e);
     shard_teardown(e, true);
     auto &sh = e->shard;
@@ -2111,7 +2203,7 @@ int32_t wax_vs_shard_connect(wax_vs_engine *e, const uint8_t *handles, int32_t n
     if (!sh.open) return fail(WAX_VS_ERR_ARGUMENT, "wax_vs_shard_open has not been called");
     if (n_handles != sh.world) return fail(WAX_VS_ERR_ARGUMENT, "expected %d handles, got %d", sh.world, n_handles);
     DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    if (!g.ok) return g.error();
     for (int r = 0; r < sh.world; ++r) {
         ShardHandle h;
         memcpy(&h, handles + static_cast<size_t>(r) * sizeof h, sizeof h);
@@ -2172,7 +2264,7 @@ int32_t wax_vs_shard_search_device(wax_vs_engine *e, const float *d_query, int64
     std::shared_lock<std::shared_mutex> r(e->rw);
     if (!e->shard.connected) return fail(WAX_VS_ERR_ARGUMENT, "the shard group is not connected (wax_vs_shard_open / _connect)");
     DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    if (!g.ok) return g.error();
     const uint32_t k_eff = clamp_topk(top_k);
     if (k_eff > static_cast<uint32_t>(kShardKCap))
         return fail(WAX_VS_ERR_UNSUPPORTED, "sharded search supports top_k <= %d (got %u)", kShardKCap, k_eff);
@@ -2196,31 +2288,37 @@ static int32_t shard_wait_host(wax_vs_engine *e, unsigned long long seq) {
     return rc;
 }
 
-static int32_t build_filter_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<uint64_t> &spec, uint32_t n_filters,
-                                 cudaStream_t stream, uint64_t *launches);
-
-// The host-path collective search of both entry points (caller: read lock, device selected, arguments checked): the
-// rank's fused scan, with the row filter `*rows` (the distinct rows the filtered form's ids resolved to, mode 0 allow /
+// The host-path collective search of both entry points, under the read lock it takes (caller: e and out_n checked, and
+// the filtered form's mode and ids): the rank's fused scan, with the row filter of `frame_ids` (filtered: mode 0 allow /
 // 1 deny) below the top-k, the in-kernel exchange and merge, and the merged list delivered into mapped host memory.
-static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t k_eff, const std::vector<uint32_t> *rows,
-                                 int32_t mode, uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n) {
+static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k, bool filtered,
+                                 const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids, float *out_scores,
+                                 uint32_t out_cap, uint32_t *out_n) {
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    *out_n = 0;
+    if (!e->shard.connected) return fail(WAX_VS_ERR_ARGUMENT, "the shard group is not connected (wax_vs_shard_open / _connect)");
+    int32_t rc;
+    if ((rc = check_query(e, query, query_len))) return rc;
+    const uint32_t k_eff = clamp_topk(top_k);
+    if (k_eff > static_cast<uint32_t>(kShardKCap))
+        return fail(WAX_VS_ERR_UNSUPPORTED, "sharded search supports top_k <= %d (got %u)", kShardKCap, k_eff);
+    if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    const bool masked = filtered && e->n_rows;
+    const uint64_t offsets[2] = {0, n_ids};
+    FilterSet fs;
+    if (masked) resolve_filters(e, frame_ids, offsets, 1, nullptr, 0, fs);
     auto &sh = e->shard;
     std::lock_guard<std::mutex> sg(sh.mu);      // one host-path collective at a time: it owns sh.ctx and h_final
     SearchCtx *c = sh.ctx;
-    int32_t rc;
     const uint64_t *d_ids = nullptr;
     if ((rc = sync_device_ids(e, &d_ids))) return rc;
     uint64_t launches = 0;
-    const bool masked = rows && e->n_rows;
     if (masked) {       // one bitset, built on the device from the resolved rows
         // sized for every row of the shard (a bound on any filter's distinct rows), so that a later call never
         // reallocates: cudaFree waits for the device, where the peers' scans may already wait for this rank
-        if ((rc = c->d_filter_rows.ensure(std::max<size_t>(e->n_rows, 1), "filter rows"))) return rc;
-        if (!rows->empty())
-            CUDA_TRY(cudaMemcpyAsync(c->d_filter_rows, rows->data(), rows->size() * sizeof(uint32_t), cudaMemcpyHostToDevice,
-                                     c->stream));
-        const std::vector<uint64_t> spec = {0, rows->size(), 0, static_cast<uint64_t>(mode)};
-        if ((rc = build_filter_bits(e, c, spec, 1, c->stream, &launches))) return rc;
+        if ((rc = stage_filter_rows(e, c, fs.rows, e->n_rows, mode, c->stream, &launches))) return rc;
     }
     ShardParams sp = shard_params_next(e);
     sp.host_out = sh.h_final; sp.host_flag = sh.h_flag;      // mapped pinned: the kernel delivers the result itself
@@ -2231,7 +2329,7 @@ static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t 
         return rc;
     }
     if ((rc = shard_wait_host(e, sp.seq))) { cudaStreamSynchronize(c->stream); return rc; }
-    if (masked) CUDA_TRY(cudaStreamSynchronize(c->stream));   // `rows` must outlive its upload
+    if (masked) CUDA_TRY(cudaStreamSynchronize(c->stream));   // fs.rows must outlive its upload
     uint32_t m = 0;
     for (uint32_t i = 0; i < k_eff; ++i) {
         const wax_vs_candidate &cd = sh.h_final[i];
@@ -2248,19 +2346,7 @@ static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t 
 int32_t wax_vs_shard_search(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k, uint64_t *out_ids,
                             float *out_scores, uint32_t out_cap, uint32_t *out_n) {
     if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    std::shared_lock<std::shared_mutex> r(e->rw);
-    *out_n = 0;
-    if (!e->shard.connected) return fail(WAX_VS_ERR_ARGUMENT, "the shard group is not connected (wax_vs_shard_open / _connect)");
-    if (!query) return fail(WAX_VS_ERR_NULL, "query is NULL");
-    if (query_len != e->dims)
-        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
-    const uint32_t k_eff = clamp_topk(top_k);
-    if (k_eff > static_cast<uint32_t>(kShardKCap))
-        return fail(WAX_VS_ERR_UNSUPPORTED, "sharded search supports top_k <= %d (got %u)", kShardKCap, k_eff);
-    if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
-    DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    return shard_search_host(e, query, k_eff, nullptr, 0, out_ids, out_scores, out_cap, out_n);
+    return shard_search_host(e, query, query_len, top_k, false, nullptr, 0, 0, out_ids, out_scores, out_cap, out_n);
 }
 
 // Device-timed sharded searches, strictly one query at a time on one stream (the same mode as wax_vs_debug_time_search):
@@ -2308,70 +2394,13 @@ int32_t wax_vs_merge_candidates_device(wax_vs_engine *e, const wax_vs_candidate 
         return fail(WAX_VS_ERR_ARGUMENT, "merge: world %u, k %u, k_out %u", world, k, k_out);
     if (n_queries == 0) return WAX_VS_OK;
     DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    if (!g.ok) return g.error();
     merge_gathered_kernel<<<n_queries, 128, 0, static_cast<cudaStream_t>(cuda_stream)>>>(d_gathered, world, n_queries, k, k_out, d_out);
     CUDA_TRY(cudaGetLastError());
     return WAX_VS_OK;
 }
 
-// ---- filtered search (SURVEY.md section 8f-4) -------------------------------------------------------------------
-// The reference filters AFTER the engine call and over-fetches 3 x topK to compensate (UnifiedSearch.swift:58,
-// 371-442, 1195-1200, 1241-1258).  Here the filter is pushed below the top-k: a row bitset consulted only for rows
-// that would enter the list, or -- for small allow-lists -- a gather that scores only the listed rows.
-// frameIds -> the distinct rows of this engine they name, appended to `rows` (unknown and repeated ids are ignored).
-// `seen` is a zeroed scratch bitset of ceil(N / 32) words shared by all the filters of a call: only the words this
-// filter touched are cleared again, so no list is sorted and no bitset is rebuilt per filter.  Returns the rows appended.
-static uint64_t build_row_filter(wax_vs_engine *e, const uint64_t *frame_ids, uint64_t n_ids, std::vector<uint32_t> &seen,
-                                 std::vector<uint32_t> &rows) {
-    const uint64_t n_rows = e->n_rows;
-    const size_t first = rows.size();
-    std::lock_guard<std::mutex> g(e->ids_mu);   // the lazily built id map is shared by concurrent readers
-    // (find_row builds the lazily constructed hash table when it is needed: serialised by ids_mu)
-    for (uint64_t i = 0; i < n_ids; ++i) {
-        uint64_t row;
-        if (e->ids_identity) {
-            if (frame_ids[i] < e->id_base || frame_ids[i] - e->id_base >= n_rows) continue;
-            row = frame_ids[i] - e->id_base;
-        } else {
-            const uint32_t f = find_row(e, frame_ids[i]);
-            if (f == 0xFFFFFFFFu) continue;
-            row = f;
-        }
-        const uint32_t w = static_cast<uint32_t>(row >> 5), b = 1u << (row & 31u);
-        if (!(seen[w] & b)) { seen[w] |= b; rows.push_back(static_cast<uint32_t>(row)); }
-    }
-    for (size_t i = first; i < rows.size(); ++i) seen[rows[i] >> 5] = 0u;
-    return rows.size() - first;
-}
-
-// n_filters row bitsets of ceil(N / 32) words into c->d_mask on `stream`, from the resolved rows in c->d_filter_rows:
-// spec is filter_bits_init_kernel's (running row counts, where each filter's rows start, modes).  The host uploads
-// 4 bytes per listed row instead of N / 8 bytes per filter.  c->d_mask must not be reallocated while earlier
-// launches on `stream` still read it: callers size it first.
-static int32_t build_filter_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<uint64_t> &spec, uint32_t n_filters,
-                                 cudaStream_t stream, uint64_t *launches) {
-    const uint32_t words = static_cast<uint32_t>((e->n_rows + 31) / 32);
-    int32_t rc;
-    if ((rc = c->d_filter_spec.ensure(spec.size(), "filter spec"))) return rc;
-    if ((rc = c->d_mask.ensure(static_cast<size_t>(n_filters) * words, "row filters"))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(c->d_filter_spec, spec.data(), spec.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, stream));
-    const size_t total_words = static_cast<size_t>(n_filters) * words;
-    const int cap = e->sm_count * 8;
-    const int g1 = static_cast<int>(std::min<size_t>(cap, (total_words + 255) / 256));
-    filter_bits_init_kernel<<<std::max(g1, 1), 256, 0, stream>>>(c->d_mask, words, static_cast<uint32_t>(e->n_rows),
-                                                                 c->d_filter_spec, n_filters);
-    CUDA_TRY(cudaGetLastError());
-    ++*launches;
-    const uint64_t listed = spec[n_filters];
-    if (listed) {
-        const int g2 = static_cast<int>(std::min<uint64_t>(cap, (listed + 255) / 256));
-        filter_bits_apply_kernel<<<g2, 256, 0, stream>>>(c->d_mask, words, c->d_filter_rows, c->d_filter_spec, n_filters);
-        CUDA_TRY(cudaGetLastError());
-        ++*launches;
-    }
-    return WAX_VS_OK;
-}
-
+// ---- batched filtered search ------------------------------------------------------------------------------------
 // n_queries queries, query i under filter query_filter[i] (WAX_VS_NO_FILTER: unfiltered); the single-filter entry
 // points are the case of one filter that every query names.  Every query referenced filter is resolved once; query i
 // asks for k_i = min(clamp(top_k), allowed_i) rows and falls in one of three classes:
@@ -2384,27 +2413,6 @@ static int32_t build_filter_bits(wax_vs_engine *e, SearchCtx *c, const std::vect
 //    scan each with its own k_i.
 // The bitsets are built on the device; a pass holds at most filter_bitset_bytes of them, more filters run in several
 // sub-batches (queries sorted by filter, so each filter's bitset is built once).
-// The filters of a call, resolved once: filter f's distinct rows are rows[first[f] .. first[f] + count[f]).
-struct FilterSet {
-    std::vector<uint32_t> rows;
-    std::vector<uint64_t> first, count;
-    std::vector<uint8_t> referenced;            // filters some query names (the others are not resolved)
-};
-static void resolve_filters(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *filter_offsets, uint32_t n_filters,
-                            const uint32_t *query_filter, uint32_t n_queries, FilterSet &fs) {
-    fs.first.assign(n_filters, 0);
-    fs.count.assign(n_filters, 0);
-    fs.referenced.assign(n_filters, 0);
-    for (uint32_t i = 0; i < n_queries; ++i)
-        if (query_filter[i] != WAX_VS_NO_FILTER) fs.referenced[query_filter[i]] = 1;
-    std::vector<uint32_t> seen(static_cast<size_t>((e->n_rows + 31) / 32), 0u);
-    for (uint32_t f = 0; f < n_filters; ++f) {
-        if (!fs.referenced[f]) continue;
-        fs.first[f] = fs.rows.size();
-        fs.count[f] = build_row_filter(e, frame_ids + filter_offsets[f], filter_offsets[f + 1] - filter_offsets[f], seen, fs.rows);
-    }
-}
-
 // Each query's k and class.  Staged query j is query order[j] and fills k_of[j] of its k_max candidate slots; the staged
 // order is the tensor class, the gather class, the scan class, the first and last sorted by filter so that a sub-batch
 // names a run of consecutive filters (unfiltered queries last).  Queries whose filter allows nothing are not staged.
@@ -2457,9 +2465,7 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
     if ((rc = stage_queries(e, c, queries, n_staged, c->stream, order.data()))) return rc;
     if ((rc = c->d_out.ensure(ncand, "result buffer"))) return rc;
     if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
-    if ((rc = c->d_filter_rows.ensure(std::max<size_t>(rows.size(), 1), "filter rows"))) return rc;
-    if (!rows.empty())
-        CUDA_TRY(cudaMemcpyAsync(c->d_filter_rows, rows.data(), rows.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    if ((rc = stage_filter_rows(e, c, rows, rows.size(), -1, c->stream, nullptr))) return rc;
     uint64_t launches = 0;
 
     // gather class: one concatenated row list, a span per query; the sort grants shared memory for the longest list
@@ -2582,9 +2588,8 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
     if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
-    if (!queries) return fail(WAX_VS_ERR_NULL, "query is NULL");
-    if (query_len != e->dims)
-        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
+    int32_t rc;
+    if ((rc = check_query(e, queries, query_len))) return rc;
     FilterSet fs;
     resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, fs);
     FilteredPlan plan;
@@ -2595,10 +2600,9 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
     if (out_stride < k_max) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, k_max);
 
     DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    if (!g.ok) return g.error();
     CtxLease lease(e);
-    int32_t rc = lease.acquire();
-    if (rc) return rc;
+    if ((rc = lease.acquire())) return rc;
     SearchCtx *c = lease.c;
     if ((rc = run_filtered(e, c, queries, filter_modes, n_filters, query_filter, fs, plan))) return rc;
     const size_t ncand = static_cast<size_t>(n_staged) * k_max;
@@ -2643,24 +2647,7 @@ int32_t wax_vs_shard_search_filtered(wax_vs_engine *e, const float *query, uint3
     if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
     if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
-    std::shared_lock<std::shared_mutex> r(e->rw);
-    *out_n = 0;
-    if (!e->shard.connected) return fail(WAX_VS_ERR_ARGUMENT, "the shard group is not connected (wax_vs_shard_open / _connect)");
-    if (!query) return fail(WAX_VS_ERR_NULL, "query is NULL");
-    if (query_len != e->dims)
-        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
-    const uint32_t k_eff = clamp_topk(top_k);
-    if (k_eff > static_cast<uint32_t>(kShardKCap))
-        return fail(WAX_VS_ERR_UNSUPPORTED, "sharded search supports top_k <= %d (got %u)", kShardKCap, k_eff);
-    if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
-    DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    std::vector<uint32_t> rows;
-    if (e->n_rows) {
-        std::vector<uint32_t> seen(static_cast<size_t>((e->n_rows + 31) / 32), 0u);
-        build_row_filter(e, frame_ids, n_ids, seen, rows);
-    }
-    return shard_search_host(e, query, k_eff, &rows, mode, out_ids, out_scores, out_cap, out_n);
+    return shard_search_host(e, query, query_len, top_k, true, frame_ids, n_ids, mode, out_ids, out_scores, out_cap, out_n);
 }
 
 // ---- grouped search (waxvs_group.cuh) -----------------------------------------------------------------------------
@@ -2679,23 +2666,16 @@ int32_t wax_vs_set_groups(wax_vs_engine *e, const uint64_t *frame_ids, const uin
     drain_device_path(e);
     if (!e->groups_set) {              // from implicit (every row its own group) to an explicit array
         e->groups.resize(e->n_rows);
-        for (uint64_t r = 0; r < e->n_rows; ++r) e->groups[r] = e->ids_identity ? e->id_base + r : e->ids[r];
+        for (uint64_t r = 0; r < e->n_rows; ++r) e->groups[r] = frame_id_of(e, r);
         e->groups_set = true;
     }
     std::vector<uint32_t> written(static_cast<size_t>((e->n_rows + 31) / 32), 0u);
     uint64_t assigned = 0;
     for (uint64_t i = 0; i < n; ++i) {
-        uint64_t row;
-        if (e->ids_identity) {
-            if (frame_ids[i] < e->id_base || frame_ids[i] - e->id_base >= e->n_rows) continue;
-            row = frame_ids[i] - e->id_base;
-        } else {
-            const uint32_t f = find_row(e, frame_ids[i]);
-            if (f == 0xFFFFFFFFu) continue;              // unknown frame: ignored
-            row = f;
-        }
+        const uint32_t row = row_of(e, frame_ids[i]);
+        if (row == 0xFFFFFFFFu) continue;                // unknown frame: ignored
         e->groups[row] = group_ids[i];                   // a later entry for the same frame wins
-        const uint32_t wd = static_cast<uint32_t>(row >> 5), b = 1u << (row & 31u);
+        const uint32_t wd = row >> 5, b = 1u << (row & 31u);
         if (!(written[wd] & b)) { written[wd] |= b; ++assigned; }
     }
     e->gindex.valid = false;
@@ -2761,21 +2741,6 @@ static float host_from_orderable(uint32_t k) {       // inverse of orderable_u32
     return f;
 }
 
-// Grouped argument checks, before the empty-engine early return (single and batched forms); *n_top = clamp(top_groups).
-static int32_t check_grouped_args(wax_vs_engine *e, bool outputs, int64_t top_groups, uint32_t per_group,
-                                  const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint32_t *n_top) {
-    if (!e || !outputs) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    if (per_group == 0 || per_group > WAX_VS_MAX_PER_GROUP)
-        return fail(WAX_VS_ERR_ARGUMENT, "per_group must be in [1, %d] (got %u)", WAX_VS_MAX_PER_GROUP, per_group);
-    *n_top = clamp_topk(top_groups);
-    if (static_cast<uint64_t>(*n_top) * per_group > WAX_VS_MAX_RESULTS)
-        return fail(WAX_VS_ERR_ARGUMENT, "clamp(top_groups) x per_group = %llu exceeds %d",
-                    static_cast<unsigned long long>(*n_top) * per_group, WAX_VS_MAX_RESULTS);
-    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
-    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
-    return WAX_VS_OK;
-}
-
 // Expansion plan: span i = (first CSR position, rows, result offset) gets its per_group best rows at its result offset.
 // Level 0 sorts tiles of kExpandTile CSR positions, each later level merges kExpandTile / per_group of the previous
 // level's lists, until one list per span is left (a span of one tile is final at level 0).  Level l > 0 reads the level
@@ -2827,11 +2792,26 @@ static void plan_expansion(const std::vector<uint3> &spans, uint32_t per_group, 
         pending.swap(next);
     }
 }
+// Levels >= 1 of `plan` on stream s, after the caller's level 0 (the caller sizes the level buffers c->d_expand[0..1]
+// from plan.buf_keys first): d_items = their items, in level order; each span's last list goes to `result`.  No level
+// >= 1 is empty: plan_expansion adds one only while spans are pending, and each pending span contributes an item.
+static int32_t enqueue_expand_merges(wax_vs_engine *e, SearchCtx *c, const ExpandPlan &plan, const ExpandItem *d_items,
+                                     uint32_t per_group, uint64_t *result, cudaStream_t s, uint64_t *launches) {
+    for (size_t lv = 1; lv < plan.levels.size(); ++lv) {
+        const uint32_t items = static_cast<uint32_t>(plan.levels[lv].size());
+        group_expand_kernel<<<items, 1024, 0, s>>>(d_items, 0u, e->gindex.perm, nullptr, c->d_expand[(lv - 1) & 1], per_group,
+                                                   c->d_expand[lv & 1], result);
+        CUDA_TRY(cudaGetLastError());
+        ++*launches;
+        d_items += items;
+    }
+    return WAX_VS_OK;
+}
 
 // Grouped delivery: row -> frame id and group id, distance -> score, as entry m of the outputs.
 static void deliver_group_row(const wax_vs_engine *e, uint32_t row, float d, uint32_t m, uint64_t *out_ids, float *out_scores,
                               uint64_t *out_groups) {
-    const uint64_t id = e->ids_identity ? e->id_base + row : e->ids[row];
+    const uint64_t id = frame_id_of(e, row);
     out_ids[m] = id;
     out_scores[m] = score_from_distance(e->similarity, d);
     out_groups[m] = e->groups_set ? e->groups[row] : id;
@@ -2870,11 +2850,10 @@ static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, u
     if ((rc = c->d_out.ensure(n_top, "result buffer"))) return rc;
     if ((rc = c->h_out.ensure(n_top, "result staging"))) return rc;
     if (filtered) {
-        if ((rc = c->d_filter_rows.ensure(std::max<size_t>(rows->size(), 1), "filter rows"))) return rc;
-        if (!rows->empty())
-            CUDA_TRY(cudaMemcpyAsync(c->d_filter_rows, rows->data(), rows->size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
-        const std::vector<uint64_t> spec = {0, rows->size(), 0, static_cast<uint64_t>(mode)};
-        if ((rc = build_filter_bits(e, c, spec, 1, s, &launches))) { cudaStreamSynchronize(s); return rc; }
+        if ((rc = stage_filter_rows(e, c, *rows, rows->size(), mode, s, &launches))) {
+            cudaStreamSynchronize(s);
+            return rc;
+        }
     }
     if ((rc = enqueue_search(e, c, c->d_queries, 1, 0, c->d_out, nullptr, s, &launches, filtered ? c->d_mask.p : nullptr,
                              nullptr, nullptr, true))) {
@@ -2922,18 +2901,15 @@ static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, u
             return rc;
         if (!all.empty())
             CUDA_TRY(cudaMemcpyAsync(c->d_expand_items, all.data(), all.size() * sizeof(ExpandItem), cudaMemcpyHostToDevice, s));
-        size_t first_item = 0;
-        for (size_t lv = 0; lv < plan.levels.size(); ++lv) {
-            const uint32_t items = static_cast<uint32_t>(plan.levels[lv].size());
-            if (items) {
-                group_expand_kernel<<<items, 1024, 0, s>>>(c->d_expand_items + first_item, lv == 0 ? 1u : 0u, gi.perm,
-                                                           c->d_dist_keys, lv ? c->d_expand[(lv - 1) & 1].p : nullptr,
-                                                           per_group, c->d_expand[lv & 1], c->d_expand[2]);
-                CUDA_TRY(cudaGetLastError());
-                ++launches;
-            }
-            first_item += items;
+        const uint32_t tiles = static_cast<uint32_t>(plan.levels[0].size());
+        if (tiles) {
+            group_expand_kernel<<<tiles, 1024, 0, s>>>(c->d_expand_items, 1u, gi.perm, c->d_dist_keys, nullptr, per_group,
+                                                       c->d_expand[0], c->d_expand[2]);
+            CUDA_TRY(cudaGetLastError());
+            ++launches;
         }
+        if ((rc = enqueue_expand_merges(e, c, plan, c->d_expand_items + tiles, per_group, c->d_expand[2], s, &launches)))
+            return rc;
         if (n_sel)
             CUDA_TRY(cudaMemcpyAsync(c->h_expand, c->d_expand[2], static_cast<size_t>(n_sel) * per_group * sizeof(uint64_t),
                                      cudaMemcpyDeviceToHost, s));
@@ -2949,39 +2925,6 @@ static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, u
             deliver_group_row(e, static_cast<uint32_t>(c->h_out[i].row), c->h_out[i].distance, m++, out_ids, out_scores, out_groups);
     *out_n = m;
     return WAX_VS_OK;
-}
-
-int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_groups,
-                              uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
-                              uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_cap,
-                              uint32_t *out_n) {
-    uint32_t n_top = 0;
-    int32_t rc = check_grouped_args(e, out_n && out_ids && out_scores && out_groups, top_groups, per_group, frame_ids, n_ids,
-                                    mode, &n_top);
-    if (rc) return rc;
-    std::shared_lock<std::shared_mutex> r(e->rw);
-    *out_n = 0;
-    if (e->n_rows == 0) return WAX_VS_OK;                // as wax_vs_search (:448)
-    if (!query) return fail(WAX_VS_ERR_NULL, "query is NULL");
-    if (query_len != e->dims)
-        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
-    const uint32_t n = static_cast<uint32_t>(e->n_rows);
-    const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(n_top) * per_group, n));
-    if (out_cap < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_cap, need);
-    const bool filtered = !(mode == 1 && n_ids == 0);
-    std::vector<uint32_t> rows;
-    if (filtered) {
-        std::vector<uint32_t> seen(static_cast<size_t>((n + 31) / 32), 0u);
-        build_row_filter(e, frame_ids, n_ids, seen, rows);
-        if (mode == 0 && rows.empty()) return WAX_VS_OK;                 // nothing allowed
-        if (mode == 1 && rows.size() == n) return WAX_VS_OK;             // everything denied
-    }
-    DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    CtxLease lease(e);
-    if ((rc = lease.acquire())) return rc;
-    return grouped_one(e, lease.c, query, n_top, per_group, filtered ? &rows : nullptr, mode, out_ids, out_scores, out_groups,
-                       out_n);
 }
 
 // ---- batched grouped search (waxvs_group_batch.cuh) -----------------------------------------------------------------
@@ -3046,44 +2989,54 @@ static int32_t enqueue_batch_expansion(wax_vs_engine *e, SearchCtx *c, const Cov
         CUDA_TRY(cudaGetLastError());
         ++*launches;
         first_tile += n0;
-        for (size_t lv = 1; lv < rd.plan.levels.size(); ++lv) {
-            const uint32_t items = static_cast<uint32_t>(rd.plan.levels[lv].size());
-            group_expand_kernel<<<items, 1024, 0, s>>>(c->d_expand_items + first_merge, 0u, e->gindex.perm, nullptr,
-                                                       c->d_expand[(lv - 1) & 1], per_group, c->d_expand[lv & 1], c->d_bg_keys);
-            CUDA_TRY(cudaGetLastError());
-            ++*launches;
-            first_merge += items;
-        }
+        if ((rc = enqueue_expand_merges(e, c, rd.plan, c->d_expand_items + first_merge, per_group, c->d_bg_keys, s, launches)))
+            return rc;
+        for (size_t lv = 1; lv < rd.plan.levels.size(); ++lv) first_merge += rd.plan.levels[lv].size();
     }
     CUDA_TRY(cudaStreamSynchronize(s));              // also keeps the item lists alive until their copies are done
     return WAX_VS_OK;
 }
 
-int32_t wax_vs_search_batch_grouped(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                    int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
-                                    int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
-                                    uint32_t out_stride, uint32_t *out_n) {
-    uint32_t n_top = 0;
-    int32_t rc = check_grouped_args(e, out_n && out_ids && out_scores && out_groups, top_groups, per_group, frame_ids, n_ids,
-                                    mode, &n_top);
-    if (rc) return rc;
+// Both grouped entry points: the arguments checked before the empty-engine early return, the filter resolved once (an
+// empty deny-list is none), then grouped_one, or with `batched` the batch pipeline -- a batch of one stays a batch.
+static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                   int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
+                                   int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
+                                   uint32_t out_stride, uint32_t *out_n, bool batched) {
+    if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    if (per_group == 0 || per_group > WAX_VS_MAX_PER_GROUP)
+        return fail(WAX_VS_ERR_ARGUMENT, "per_group must be in [1, %d] (got %u)", WAX_VS_MAX_PER_GROUP, per_group);
+    const uint32_t n_top = clamp_topk(top_groups);
+    if (static_cast<uint64_t>(n_top) * per_group > WAX_VS_MAX_RESULTS)
+        return fail(WAX_VS_ERR_ARGUMENT, "clamp(top_groups) x per_group = %llu exceeds %d",
+                    static_cast<unsigned long long>(n_top) * per_group, WAX_VS_MAX_RESULTS);
+    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
+    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
-    if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
-    if (!queries) return fail(WAX_VS_ERR_NULL, "query is NULL");
-    if (query_len != e->dims)
-        return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, query_len);
+    if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;      // as wax_vs_search (:448)
+    int32_t rc;
+    if ((rc = check_query(e, queries, query_len))) return rc;
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(n_top) * per_group, n));
     if (out_stride < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, need);
-    // one filter that every query names, resolved once (none when unfiltered)
     const bool filtered = !(mode == 1 && n_ids == 0);
     const uint64_t offsets[2] = {0, n_ids};
-    const std::vector<uint32_t> query_filter(n_queries, filtered ? 0u : WAX_VS_NO_FILTER);
     FilterSet fs;
-    resolve_filters(e, frame_ids, offsets, filtered ? 1u : 0u, query_filter.data(), n_queries, fs);
-    if (filtered && mode == 0 && fs.rows.empty()) return WAX_VS_OK;              // nothing allowed
-    if (filtered && mode == 1 && fs.rows.size() == n) return WAX_VS_OK;          // everything denied
+    if (filtered) {
+        resolve_filters(e, frame_ids, offsets, 1, nullptr, 0, fs);
+        if (mode == 0 && fs.rows.empty()) return WAX_VS_OK;                 // nothing allowed
+        if (mode == 1 && fs.rows.size() == n) return WAX_VS_OK;             // everything denied
+    }
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    CtxLease lease(e);
+    if ((rc = lease.acquire())) return rc;
+    SearchCtx *c = lease.c;
+    if (!batched)
+        return grouped_one(e, c, queries, n_top, per_group, filtered ? &fs.rows : nullptr, mode, out_ids, out_scores,
+                           out_groups, out_n);
+    const std::vector<uint32_t> query_filter(n_queries, filtered ? 0u : WAX_VS_NO_FILTER);
     // The coverage level: each query's exact top-k_c rows, when the batch goes to the tensor-core levels or the gather
     // class of the batched filtered search; every other batch runs the single-query pipeline per query.
     const uint32_t k_c = std::min(kCoverMax, std::max(128u, 4u * n_top));
@@ -3095,11 +3048,6 @@ int32_t wax_vs_search_batch_grouped(wax_vs_engine *e, const float *queries, uint
         cover = n_staged == n_queries && (plan.n_gather == n_staged ||
                                           (plan.n_tensor == n_staged && batch_tensor_eligible(e, n_staged, plan.k_max)));
     }
-    DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
-    CtxLease lease(e);
-    if ((rc = lease.acquire())) return rc;
-    SearchCtx *c = lease.c;
     cudaStream_t s = c->stream;
     std::vector<uint32_t> crowded;                   // queries for the single-query pipeline
     uint64_t covered = 0, expanded = 0, launches = 0;
@@ -3165,6 +3113,22 @@ int32_t wax_vs_search_batch_grouped(wax_vs_engine *e, const float *queries, uint
     e->grouped_batch_expanded_groups += expanded;
     e->grouped_batch_fallback_queries += crowded.size();
     return WAX_VS_OK;
+}
+
+int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_groups,
+                              uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                              uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_cap,
+                              uint32_t *out_n) {
+    return search_grouped_host(e, query, 1, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids, out_scores,
+                               out_groups, out_cap, out_n, false);
+}
+
+int32_t wax_vs_search_batch_grouped(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                    int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
+                                    int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
+                                    uint32_t out_stride, uint32_t *out_n) {
+    return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
+                               out_scores, out_groups, out_stride, out_n, true);
 }
 
 // ---- persistence ---------------------------------------------------------------------------------------------
@@ -3548,7 +3512,7 @@ int32_t wax_vs_debug_batch_nominations(wax_vs_engine *e, const float *queries, u
     if (!e || !queries || !out_scores || !out_ok || !out_shape) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     DeviceGuard g(e->device);
-    if (!g.ok) return fail(WAX_VS_ERR_CUDA, "failed to select CUDA device %d", e->device);
+    if (!g.ok) return g.error();
     const uint32_t k_eff = static_cast<uint32_t>(std::min<uint64_t>(clamp_topk(top_k), std::max<uint64_t>(e->n_rows, 1)));
     if (n_queries == 0 || e->n_rows == 0 || k_eff > 128u || e->dims % kBatchKBlock != 0 || e->dims > 8192 ||
         (e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT && !(e->similarity == WAX_VS_L2 && e->tune.batch_l2)))
