@@ -1,4 +1,4 @@
-"""Shared test helpers: a list-based model of the engine's mutation semantics, comparators."""
+"""Shared test helpers: a list-based model of the engine's mutation semantics, comparators, test corpora."""
 from __future__ import annotations
 
 import json
@@ -69,3 +69,37 @@ def assert_tie_aware_order(got_ids, ref_ids, ref_scores_f64, tol):
 
 def load_json(name):
     return json.loads((GOLDEN / name).read_text())
+
+
+def unit_rows(rng, n, dims):
+    x = rng.standard_normal((n, dims))
+    return (x / np.linalg.norm(x, axis=1, keepdims=True)).astype(np.float32)
+
+
+def hidden_winner(rng, dims, n, bf16, n_decoys, scale_log2=0):
+    """Dot query q and a corpus whose first 1 + n_decoys rows (one slice: the first tile) are the true best row (row 0)
+    and decoys.  q and the decoys have components exactly representable in bf16 (hence TF32), so their score' is exact
+    up to accumulation; the best row's components sit just below a TF32 rounding midpoint that lies just below a bf16
+    midpoint, so TF32 (rounded or truncated) loses ~2^-11 and bf16 ~2^-8 of every component: its score' drops below
+    every decoy, whose exact scores are spread over (0.1, 0.9) of that loss below the best score.  The other rows are
+    unrelated unit rows.  Rows 0..n_decoys are scaled by 2^scale_log2 (exact)."""
+    q = 1.0 + rng.integers(0, 4, dims) * 2.0 ** -7
+    lo = 1.0 + rng.integers(0, 4, dims) * 2.0 ** -7                     # the bf16 value the best row rounds down to
+    best = (lo + 2.0 ** -8 - 2.0 ** -11) * (1.0 - 2.0 ** -18)
+    s_best = q @ best
+    rounded = lo if bf16 else lo + 2.0 ** -8 - 2.0 ** -10                # the operand the tensor cores see
+    gap = s_best - q @ rounded
+    decoys = np.empty((n_decoys, dims))
+    for i, t in enumerate(np.linspace(0.9, 0.15, n_decoys)):
+        row = lo.copy()
+        for c in rng.permutation(dims):                                 # exact 2^-7 steps up to the target score
+            if q @ row >= s_best - t * gap:
+                break
+            row[c] += 2.0 ** -7
+        assert s_best - t * gap <= q @ row < s_best
+        decoys[i] = row
+    corpus = unit_rows(rng, n, dims)
+    corpus[0] = best
+    corpus[1:1 + n_decoys] = decoys
+    corpus[:1 + n_decoys] *= np.float32(2.0 ** scale_log2)
+    return q.astype(np.float32)[None, :], corpus

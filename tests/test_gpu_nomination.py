@@ -18,6 +18,7 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from helpers import hidden_winner as _hidden_winner, unit_rows as _unit
 from wax_b200 import CUDAVectorEngine, VectorMetric
 
 pytestmark = pytest.mark.gpu
@@ -60,11 +61,6 @@ def _engine(metric, corpus, opts):
     for key, value in opts.items():
         eng.set_option(key, value)
     return eng
-
-
-def _unit(rng, n, dims):
-    x = rng.standard_normal((n, dims))
-    return (x / np.linalg.norm(x, axis=1, keepdims=True)).astype(np.float32)
 
 
 def _worst(rng, n, dims):
@@ -231,35 +227,6 @@ def test_filtered_batch_never_nominates_a_disallowed_row(bf16):
     eng.set_option("batch_tensor", 0)
     assert got == [eng.search_filtered(q, 10, allow=ids.tolist()) for q in qs[:8]] + got[8:]
     eng.close()
-
-
-def _hidden_winner(rng, dims, n, bf16, n_decoys, scale_log2=0):
-    """Dot query q and a corpus whose first 1 + n_decoys rows (one slice: the first tile) are the true best row (row 0)
-    and decoys.  q and the decoys have components exactly representable in bf16 (hence TF32), so their score' is exact
-    up to accumulation; the best row's components sit just below a TF32 rounding midpoint that lies just below a bf16
-    midpoint, so TF32 (rounded or truncated) loses ~2^-11 and bf16 ~2^-8 of every component: its score' drops below
-    every decoy, whose exact scores are spread over (0.1, 0.9) of that loss below the best score.  The other rows are
-    unrelated unit rows.  Rows 0..n_decoys are scaled by 2^scale_log2 (exact)."""
-    q = 1.0 + rng.integers(0, 4, dims) * 2.0 ** -7
-    lo = 1.0 + rng.integers(0, 4, dims) * 2.0 ** -7                     # the bf16 value the best row rounds down to
-    best = (lo + 2.0 ** -8 - 2.0 ** -11) * (1.0 - 2.0 ** -18)
-    s_best = q @ best
-    rounded = lo if bf16 else lo + 2.0 ** -8 - 2.0 ** -10                # the operand the tensor cores see
-    gap = s_best - q @ rounded
-    decoys = np.empty((n_decoys, dims))
-    for i, t in enumerate(np.linspace(0.9, 0.15, n_decoys)):
-        row = lo.copy()
-        for c in rng.permutation(dims):                                 # exact 2^-7 steps up to the target score
-            if q @ row >= s_best - t * gap:
-                break
-            row[c] += 2.0 ** -7
-        assert s_best - t * gap <= q @ row < s_best
-        decoys[i] = row
-    corpus = _unit(rng, n, dims)
-    corpus[0] = best
-    corpus[1:1 + n_decoys] = decoys
-    corpus[:1 + n_decoys] *= np.float32(2.0 ** scale_log2)
-    return q.astype(np.float32)[None, :], corpus
 
 
 @pytest.mark.parametrize("bf16", [1, 0])

@@ -993,6 +993,14 @@ __global__ void __launch_bounds__(512, 2) batch_finish_kernel(const FinishParams
         } else if (excluded_any) {
             ok = 0;
         }
+        // The cosine / dot bounds scale with the fp32 |q|: once fl(|q|^2) is zero or subnormal they shrink to nothing
+        // while score' still carries its error; an overflowing |q|^2 leaves no finite bound, and a NaN or Inf component
+        // gives NaN scores', which are never nominated nor counted as excluded (cosine rows with |v|^2 = 0 still have
+        // distance 1 then).  Such a query is never proven and has no filter threshold: the exact scan answers it.
+        if (METRIC != kL2 && (!(s_a2 >= 0x1p-126f) || !finite_f32(s_a2))) {
+            ok = 0;
+            tau_star = tau_star16 = -INFINITY;
+        }
         p.ok[q] = ok;
         if (p.tau_star) { p.tau_star[q] = tau_star; p.tau_star[p.tau_stride + q] = tau_star16; }
     }
