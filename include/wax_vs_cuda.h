@@ -125,7 +125,10 @@ int32_t wax_vs_remove_batch(wax_vs_engine *engine, const uint64_t *frame_ids, ui
          cosine 1 - d with d = 1 - q.v/(|q||v|), ALWAYS divided by the in-kernel |q|;
          dot -(1 - q.v);  l2 -sum (q-v)^2
    out_ids / out_scores need room for out_cap entries, out_cap >= min(clamp(top_k), N) else
-   WAX_VS_ERR_BUFFER. */
+   WAX_VS_ERR_BUFFER.
+   Cosine / dot with k <= 32 on a corpus of at least 512 MiB (fp32) first nominate on the engine's bf16 copy of the
+   corpus (half the bytes), re-score the nominees exactly and prove the result; the fp32 scan answers only when that
+   proof fails.  Results are the fp32 scan's either way. */
 int32_t wax_vs_search(wax_vs_engine *engine, const float *query, uint32_t query_len, int64_t top_k,
                       uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n);
 
@@ -363,7 +366,9 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *engine, uint64_t *tensor_queries
    "shadow_bytes" (HBM held by the bf16 shadow), "shadow_unavailable" (1 = the shadow did not fit in HBM, batches
    nominate in TF32 at about half the rate), "batch_tf32_queries", "filter_bitset_passes" (sub-batches of per-query
    filtered queries on the tensor-core class, wax_vs_search_batch_multi_filtered), "group_index_builds" (device group
-   index builds of wax_vs_search_grouped), "pool_allocs", "pool_reuses". */
+   index builds of wax_vs_search_grouped), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
+   (single queries the bf16-shadow route answered / that the fp32 scan answered after a failed proof; read them while
+   no search is running). */
 int32_t wax_vs_debug_counter(wax_vs_engine *engine, const char *name, uint64_t *out);
 
 /* Device-only timing of the batched path (n_queries synthetic unit queries per step, everything resident):
@@ -394,7 +399,10 @@ int32_t wax_vs_debug_stream_read(wax_vs_engine *engine, uint32_t iters, float *o
    _batch_device (and wax_vs_debug_time_search_batch / wax_vs_debug_batch_nominations); 0 loops the exact scan.  The
    default is to flip once the l2 levels have been measured on the H100.
    "filter_bitset_bytes" (default 2 GiB): device memory the row bitsets of one tensor pass of
-   wax_vs_search_batch_multi_filtered may use; at least one bitset always fits. */
+   wax_vs_search_batch_multi_filtered may use; at least one bitset always fits.
+   "shadow_scan" (default 1): 0 sends every single query to the fp32 scan (the bf16-shadow route off);
+   "shadow_scan_min_bytes" (default 512 MiB): the smallest fp32 corpus that takes that route;
+   "shadow_rows_per_step" / "shadow_warps" / "shadow_stages" (0 = auto): the shape of its nominating scan. */
 int32_t wax_vs_debug_set_option(wax_vs_engine *engine, const char *key, int64_t value);
 
 /* Library build info: "waxvs_cuda <version> sm_90a ...". */

@@ -65,6 +65,7 @@ __host__ __device__ constexpr int batch_ring_stages(int heap, uint32_t ares_kb =
     return st;
 }
 static_assert(kBatchN == kBatchM, "the epilogue loads one row scale per thread");
+static_assert(kNomineeStride == kBatchM, "the shadow scan writes its nominees as one query's heap of one slice");
 static_assert(batch_ring_stages(16) == 4 && batch_ring_stages(32) == 3 && batch_ring_stages(64) == 2,
               "streamed-query shapes keep a useful ring next to every heap size");
 constexpr int kBatchThreads = 160;

@@ -183,10 +183,15 @@ struct Tuning {
     int shard_fused = 1;    // sharded search: exchange + merge inside the scan launch (0: separate 1-CTA launch)
     int batch_l2 = 0;       // 1: l2 batches take the tensor-core levels too (off: they loop the single-query path).  A staging
                             // switch: the default flips once the l2 levels have H100 figures behind them
-    int single_shadow = 0;  // 1: single queries / batches below batch_min also take the bf16-shadow nominations
-                            // (half the HBM bytes per query, same results); off by
-                            // default: the plain single-query path is the fused fp32 scan BASELINE's north_star names
+    int single_shadow = 0;  // 1: single queries / batches below batch_min take the tensor-core bf16-shadow nominations
+                            // (one query in a 128-query wgmma tile) instead of the shadow route of `shadow_scan`
     uint64_t filter_bitset_bytes = 2ull << 30;   // per-query filters: row bitsets one tensor pass may hold
+    int shadow_scan = 1;    // single queries (cosine / dot, k <= 32) nominate on the bf16 shadow with the streaming scan, then
+                            // an exact re-score + proof, the fp32 scan only when the proof fails (0: always the fp32 scan)
+    uint64_t shadow_scan_min_bytes = 512ull << 20;   // ... for fp32 corpora of at least this many bytes (smaller ones are
+                                                     // latency-bound: two more launches and a shadow do not pay; on
+                                                     // H100 at 384 dims the route breaks even near 380 MB, DESIGN 5)
+    int shadow_rows_per_step = 0, shadow_warps = 0, shadow_stages = 0;   // shape of the SHADOW form (0 auto)
 };
 
 // Per-search scratch: the analogue of TransientBuffers (MetalVectorEngine.swift:36-41, :84-117).
@@ -242,6 +247,9 @@ struct SearchCtx {
     DevBuf<ScoreItem> d_score_items;               // batched grouped search: expansion tiles (level 0)
     PinnedBuf<unsigned long long> h_flag;          // host-delivery completion flag
     unsigned long long host_seq = 0;               // last value the flag was asked to take
+    DevBuf<uint32_t> d_proof_count;                // shadow route: [0] proofs that held, [1] that failed (guarded scan) ...
+    PinnedBuf<uint32_t> h_proof_count;             // ... and their mapped host mirror
+    uint32_t seen_failed = 0;                      // h_proof_count[1] when the host last looked
     ~SearchCtx() {                                 // the buffers release themselves
         if (ev0) cudaEventDestroy(ev0);
         if (ev1) cudaEventDestroy(ev1);
@@ -312,6 +320,8 @@ struct wax_vs_engine {
     // Adaptive level choice: when more than a quarter of a batch fails the coarse bf16 bound (tightly clustered
     // neighbours), the next 16 batches nominate in TF32 straight away, then bf16 is probed again.
     uint32_t bf16_skip_batches = 0;
+    // Single queries: after a failed shadow proof the next kShadowSkipQueries eligible queries take the fp32 scan directly
+    uint32_t shadow_scan_skip = 0;
     // adaptive nominee-heap size (bf16 level 1): a batch that left queries unproven makes the next `heap_bump_ttl` batches
     // use one size more than the model picks; a failure right after probing back down doubles the time-out
     uint32_t heap_bump = 0, heap_bump_ttl = 0, heap_backoff = 256;
@@ -452,7 +462,9 @@ static int32_t ctx_for_stream(wax_vs_engine *e, void *cuda_stream, SearchCtx **o
 // kernel dispatch
 struct TmaConfig { int C, R, warps, stages; size_t smem; };
 
-static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0) {
+// esize: bytes per element of the rows streamed -- 4 for the corpus, 2 for the bf16 shadow (the SHADOW form, unrolled
+// shapes only).
+static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0, size_t esize = sizeof(float)) {
     const uint32_t d = e->dims;
     if (d % 4u != 0) return false;                      // rows must be 16-byte multiples for the bulk copy
     const size_t budget = (e->smem_optin ? e->smem_optin : 232448) - 4096;   // minus the kernels' static shared memory
@@ -461,6 +473,7 @@ static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0
         const int c = static_cast<int>(d / 128u);
         if (c == 1 || c == 2 || c == 3 || c == 4 || c == 6 || c == 8 || c == 12) C = c;   // unrolled shapes (12: the 1536-dim embeddings)
     }
+    if (esize != sizeof(float) && C == 0) return false;
     if (C == 0 && d < 32) return false;                  // a few floats per row: the direct-load kernel
     if (C == 0 && d > e->tune.tma_max_dims) return false;   // very long rows: too few warps fit beside two stages, the
                                                              // direct-load kernel takes them
@@ -468,7 +481,16 @@ static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0
     // is per-row instruction latency, not bytes in flight).  These defaults were chosen on B200, not re-tuned on H100; the
     // `rows_per_step` / `warps` / `stages` options override them.
     int R, warps_default = 8;
-    if (C == 0) {                                        // generic shape: run-time chunk count, query in shared memory
+    if (esize != sizeof(float)) {                        // the shadow form (bf16 rows: half the bytes of a corpus row)
+        // 16 warps, 3 stages of 2-6 KB: on H100 at 10 M x 384 (C = 3) rows 4 / warps 16 / stages 3 took 2.503 ms per
+        // query against 2.545 for the fp32 shape's bytes (rows 8 / warps 8 / stages 2), the best of eight shapes
+        // alternated in one run (DESIGN 4.1); the other C take the same ring, not measured separately.
+        // launch_shadow_scan has rows per step r_min .. r_max.
+        const int want_r = e->tune.shadow_rows_per_step;
+        const int r_min = C <= 2 ? 8 : (C <= 4 ? 4 : 2), r_max = C <= 3 ? 16 : 2 * r_min;
+        R = (want_r >= r_min && want_r <= r_max && (want_r & (want_r - 1)) == 0) ? want_r : r_min;
+        warps_default = 16;
+    } else if (C == 0) {                               // generic shape: run-time chunk count, query in shared memory
         // keep a step at >= 2-8 KB: short generic rows (dims < 128, 160, 300, 400, ...) take 8 or 4 rows per step and
         // more warps, like the unrolled C <= 2 shapes
         // (long rows: as many rows as keep a step at <= 32 KB -- the few warps that then fit still hold ~190 KB in flight)
@@ -491,14 +513,17 @@ static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0
         // that won over 8 warps on B200, above it the 8-warp shape's 48 KB in flight did (chosen on B200, not re-tuned on H100)
         else if (mode == 1 && static_cast<uint64_t>(e->n_rows) * d * 4 < (8ull << 30)) warps_default = 16;
     }
-    // Default ring depth 2: ~48 KB in flight per SM for the 8-warp shapes (the `stages` option overrides it).
-    const int stages = e->tune.stages > 0 ? e->tune.stages : 2;
-    const size_t stage_bytes = static_cast<size_t>(R) * d * 4;
+    // Default ring depth 2: ~48 KB in flight per SM for the 8-warp shapes (the `stages` option overrides it).  The shadow
+    // form has options of its own (shadow_*): it runs right before a guarded fp32 scan that keeps the fp32 shape.
+    const bool shadow = esize != sizeof(float);
+    const int want_stages = shadow ? e->tune.shadow_stages : e->tune.stages, want_warps = shadow ? e->tune.shadow_warps : e->tune.warps;
+    const int stages = want_stages > 0 ? want_stages : (shadow ? 3 : 2);
+    const size_t stage_bytes = static_cast<size_t>(R) * d * esize;
     const size_t query_bytes = C == 0 ? (static_cast<size_t>(d) * 4 + 512 + 32) : 0;
     auto smem_for = [&](int w) { return static_cast<size_t>(w) * stages * (stage_bytes + 8 + 4) + static_cast<size_t>(w) * 1024 + 16 + query_bytes; };
-    int warps = e->tune.warps ? e->tune.warps : warps_default;
+    int warps = want_warps ? want_warps : warps_default;
     warps = std::max(1, std::min(16, warps));
-    if (!e->tune.warps) while (warps > 2 && smem_for(warps) > budget) --warps;   // long rows: fewer warps per CTA
+    if (!want_warps) while (warps > 2 && smem_for(warps) > budget) --warps;   // long rows: fewer warps per CTA
     if (smem_for(warps) > budget) return false;
     cfg->C = C; cfg->R = R; cfg->warps = warps; cfg->stages = stages; cfg->smem = smem_for(warps);
     return true;
@@ -516,11 +541,11 @@ static cudaError_t grant_smem(wax_vs_engine *e, K kernel, size_t bytes) {
     return err;
 }
 
-template <int C, int R, int M, int E, bool EMIT>
+template <int C, int R, int M, int E, bool EMIT, bool SHADOW = false>
 static cudaError_t launch_tma_inst(wax_vs_engine *e, const ScanParams &p, int grid, const TmaConfig &cfg, cudaStream_t s) {
-    cudaError_t err = grant_smem(e, scan_tma_kernel<C, R, M, E, EMIT>, cfg.smem);
+    cudaError_t err = grant_smem(e, scan_tma_kernel<C, R, M, E, EMIT, SHADOW>, cfg.smem);
     if (err != cudaSuccess) return err;
-    scan_tma_kernel<C, R, M, E, EMIT><<<grid, cfg.warps * 32, cfg.smem, s>>>(p);
+    scan_tma_kernel<C, R, M, E, EMIT, SHADOW><<<grid, cfg.warps * 32, cfg.smem, s>>>(p);
     return cudaGetLastError();
 }
 // mode: 0 = fused list k <= 32, 1 = fused list k <= 128, 2 = emit distance keys
@@ -547,6 +572,19 @@ static cudaError_t launch_tma(wax_vs_engine *e, const ScanParams &p, int grid, c
     WAXVS_CASE(6, 2); WAXVS_CASE(6, 4); WAXVS_CASE(8, 2); WAXVS_CASE(8, 4);
     WAXVS_CASE(12, 1); WAXVS_CASE(12, 2);
     WAXVS_CASE(0, 1); WAXVS_CASE(0, 2); WAXVS_CASE(0, 4); WAXVS_CASE(0, 8);
+#undef WAXVS_CASE
+    return cudaErrorInvalidValue;
+}
+// The SHADOW form (nominating pass of the bf16-shadow route): cosine / dot, the unrolled shapes, k' nominees (E = 4).
+static cudaError_t launch_shadow_scan(wax_vs_engine *e, const ScanParams &p, int grid, const TmaConfig &cfg, int metric,
+                                      cudaStream_t s) {
+#define WAXVS_CASE(Cv, Rv)                                                                                          \
+    if (cfg.C == Cv && cfg.R == Rv)                                                                                 \
+        return metric == kCosine ? launch_tma_inst<Cv, Rv, kCosine, 4, false, true>(e, p, grid, cfg, s)            \
+                                 : launch_tma_inst<Cv, Rv, kDot, 4, false, true>(e, p, grid, cfg, s)
+    WAXVS_CASE(1, 8); WAXVS_CASE(1, 16); WAXVS_CASE(2, 8); WAXVS_CASE(2, 16);
+    WAXVS_CASE(3, 4); WAXVS_CASE(3, 8); WAXVS_CASE(3, 16); WAXVS_CASE(4, 4); WAXVS_CASE(4, 8);
+    WAXVS_CASE(6, 2); WAXVS_CASE(6, 4); WAXVS_CASE(8, 2); WAXVS_CASE(8, 4); WAXVS_CASE(12, 2); WAXVS_CASE(12, 4);
 #undef WAXVS_CASE
     return cudaErrorInvalidValue;
 }
@@ -644,15 +682,103 @@ static int32_t enqueue_select(wax_vs_engine *e, SearchCtx *c, const uint32_t *ke
     return WAX_VS_OK;
 }
 
+// Persistent grid of a TMA-staged scan over n_rows rows in the shape `cfg`; sets the ring depth and (auto) the dynamic
+// chunk size in p.
+static int tma_grid(const wax_vs_engine *e, const SearchCtx *c, const TmaConfig &cfg, ScanParams &p) {
+    p.stages = static_cast<uint32_t>(cfg.stages);
+    const uint64_t steps = (e->n_rows + cfg.R - 1) / cfg.R;
+    const int max_grid = e->tune.grid > 0 ? e->tune.grid : e->sm_count;
+    int grid = static_cast<int>(std::min<uint64_t>(max_grid, (steps + cfg.warps - 1) / cfg.warps));
+    grid = std::max(std::min(grid, static_cast<int>(c->d_block_keys.cap / 128)), 1);
+    if (e->tune.chunk_steps < 0)     // auto: about two claims per warp at least, at most 8 steps
+        p.chunk_steps = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>(8, steps / (static_cast<uint64_t>(grid) * cfg.warps * 2))));
+    return grid;
+}
+
+static bool batch_bf16_wanted(const wax_vs_engine *e);
+static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream);
+
+// ---- the bf16-shadow route of a single query (DESIGN 4.1) ----
+// The fp32 scan reads dims * 4 bytes per row and runs at the HBM read ceiling; the shadow holds the same rows in bf16.
+// Three launches on `stream`, no host round trip: the SHADOW form of the scan nominates the k' best rows by score', the
+// batched path's finish kernel (one query, one slice) re-scores them exactly in the scan's own order and proves that no
+// other row can beat or tie the k-th (DESIGN 4.5), and `p` -- the query's fp32 scan, launched next by the caller -- is
+// guarded by that proof: it returns at entry when the proof held, else it answers the query as it always does.
+constexpr uint32_t kShadowNominees = 128;     // k': every warp list of the SHADOW form holds this many
+constexpr uint32_t kShadowRescore = 256;
+constexpr uint32_t kShadowSkipQueries = 16;   // after a failed proof: eligible queries that take the fp32 scan directly
+// Nothing is enqueued (and p stays unguarded) when the route does not apply to this engine and query; the caller has
+// already checked the rest: one unsharded fused query with k <= 32 on an unrolled TMA shape.
+static bool shadow_route_applies(const wax_vs_engine *e) {
+    return e->tune.shadow_scan && (e->similarity == WAX_VS_COSINE || e->similarity == WAX_VS_DOT) && !e->debug_trace &&
+           batch_bf16_wanted(e) && e->n_rows * e->dims * sizeof(float) >= e->tune.shadow_scan_min_bytes;
+}
+static int32_t enqueue_shadow_route(wax_vs_engine *e, SearchCtx *c, ScanParams &p, cudaStream_t stream, uint64_t *launches) {
+    if (!shadow_route_applies(e)) return WAX_VS_OK;
+    TmaConfig cfg{};
+    if (!pick_tma_config(e, &cfg, 1, sizeof(__nv_bfloat16))) return WAX_VS_OK;
+    int32_t rc;
+    if (!c->h_proof_count) {
+        if ((rc = c->d_proof_count.ensure(2, "proof counts")) || (rc = c->h_proof_count.ensure(2, "proof count mirror"))) return rc;
+        CUDA_TRY(cudaMemsetAsync(c->d_proof_count, 0, 2 * sizeof(uint32_t), stream));
+        c->h_proof_count[0] = c->h_proof_count[1] = 0;
+        c->seen_failed = 0;
+    }
+    {
+        std::lock_guard<std::mutex> pg(e->pool_mu);
+        const uint32_t failed = *static_cast<volatile uint32_t *>(c->h_proof_count + 1);   // no synchronisation: may lag
+        if (failed != c->seen_failed) { c->seen_failed = failed; e->shadow_scan_skip = kShadowSkipQueries; }
+        if (e->shadow_scan_skip > 0) { --e->shadow_scan_skip; return WAX_VS_OK; }
+    }
+    if ((rc = ensure_shadow(e, stream))) return rc;
+    if (!e->shadow_valid) return WAX_VS_OK;
+    if ((rc = c->d_heaps.ensure(static_cast<size_t>(kShadowNominees) * kNomineeStride, "nominee keys")) ||
+        (rc = c->d_ok.ensure(1, "proof flags")) || (!p.query && (rc = c->d_queries.ensure(e->dims, "query buffer"))))
+        return rc;
+
+    ScanParams sp = p;
+    sp.corpus = reinterpret_cast<const float *>(e->d_shadow.p);
+    sp.k = kShadowNominees;
+    sp.out = nullptr; sp.host_out = nullptr; sp.host_flag = nullptr;
+    sp.nominees = c->d_heaps;
+    sp.query_store = p.query ? nullptr : c->d_queries.p;
+    sp.tail_select = e->tune.tail_select ? 1u : 0u;
+    sp.tail_smem_bytes = static_cast<uint32_t>(static_cast<size_t>(cfg.warps) * cfg.stages * cfg.R * e->dims * sizeof(__nv_bfloat16));
+    const int grid = tma_grid(e, c, cfg, sp);
+    CUDA_TRY(launch_shadow_scan(e, sp, grid, cfg, e->similarity, stream));
+
+    FinishParams fp{};
+    fp.corpus = e->d_corpus; fp.queries = p.query ? p.query : c->d_queries.p;
+    fp.n_rows = p.n_rows; fp.dims = e->dims; fp.n_queries = 1; fp.groups = 1; fp.slices = 1;
+    fp.kprime = kShadowNominees; fp.k = p.k; fp.metric = e->similarity;
+    fp.heaps = c->d_heaps; fp.max_norm_bits = e->d_max_norm;
+    fp.out = p.out; fp.ok = c->d_ok;
+    fp.frame_ids = p.frame_ids; fp.id_base = p.id_base; fp.row_offset = p.row_offset;
+    fp.pow2_all = 512; fp.rescore = kShadowRescore; fp.eps_rel = kBf16Eps;
+    const size_t fsmem = static_cast<size_t>(fp.pow2_all + fp.rescore) * sizeof(uint64_t);
+    const auto kernel = e->similarity == WAX_VS_COSINE ? batch_finish_kernel<kCosine> : batch_finish_kernel<kDot>;
+    CUDA_TRY(grant_smem(e, kernel, fsmem));
+    kernel<<<1, 512, fsmem, stream>>>(fp);
+    CUDA_TRY(cudaGetLastError());
+    *launches += 2;
+
+    p.proof_ok = c->d_ok;
+    p.proof_count = c->d_proof_count;
+    p.proof_count_host = c->h_proof_count;
+    return WAX_VS_OK;
+}
+
 // `shard` (optional): the row-sharded form -- d_out receives the result MERGED over all ranks; the exchange runs inside
 // the scan launch when the kernel's shared-memory lists can hold the merge keys, else as one extra 1-CTA launch.
 // keys_only: run the emitting scan alone -- c->d_dist_keys receives every row's distance key (the masked rows'
 // WAXVS_UKEY_NONE) and the caller does its own selection (grouped search); d_out and k_eff are not used.
+// shadow_route: the query may take the bf16-shadow route when it applies (enqueue_shadow_route) -- the single-query entry
+// points; the batched levels' exact fall-backs (queries a bf16 proof already refused) and the sharded search do not.
 static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_query, uint32_t k_eff,
                               uint64_t row_offset, wax_vs_candidate *d_out, const uint64_t *d_ids,
                               cudaStream_t stream, uint64_t *launches, const uint32_t *d_mask = nullptr,
                               const ShardParams *shard = nullptr, const HostDelivery *host = nullptr,
-                              bool keys_only = false) {
+                              bool keys_only = false, bool shadow_route = false) {
     wax_vs_candidate *d_merged = nullptr;
     if (shard) {
         if (k_eff > static_cast<uint32_t>(kShardKCap))
@@ -723,16 +849,14 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
         fused_exchange = e->tune.shard_fused != 0 && static_cast<size_t>(shard->world) * k_eff * sizeof(uint32_t) <= list_bytes;
         if (fused_exchange) { p.shard = *shard; p.shard.final_out = d_merged; }
     }
+    if (shadow_route && !shard && mode == 0 && use_tma && cfg.C > 0) {
+        int32_t rc = enqueue_shadow_route(e, c, p, stream, launches);
+        if (rc) return rc;
+    }
     int grid;
     const int grid_cap = static_cast<int>(c->d_block_keys.cap / 128);
     if (use_tma) {
-        p.stages = static_cast<uint32_t>(cfg.stages);
-        const uint64_t steps = (e->n_rows + cfg.R - 1) / cfg.R;
-        const int max_grid = e->tune.grid > 0 ? e->tune.grid : e->sm_count;
-        grid = static_cast<int>(std::min<uint64_t>(max_grid, (steps + cfg.warps - 1) / cfg.warps));
-        grid = std::max(std::min(grid, grid_cap), 1);
-        if (e->tune.chunk_steps < 0)     // auto: about two claims per warp at least, at most 8 steps
-            p.chunk_steps = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>(8, steps / (static_cast<uint64_t>(grid) * cfg.warps * 2))));
+        grid = tma_grid(e, c, cfg, p);
         CUDA_TRY(launch_tma(e, p, grid, cfg, e->similarity, mode, stream));
     } else {
         const int max_grid = e->tune.grid > 0 ? e->tune.grid : e->sm_count * e->tune.ldg_ctas_per_sm;
@@ -1765,14 +1889,16 @@ static int32_t enqueue_filter_level(wax_vs_engine *e, SearchCtx *c, const float 
 // ---- search ---------------------------------------------------------------------------------------------------
 // The exact scan for n queries, one enqueue_search each on `stream`: query i (qs[i] when a list is given) reads
 // d_queries[i], writes d_out[i] and consults its own row filter.  sync_on_error: drain the stream before a failure is
-// returned.
+// returned.  shadow_route: see enqueue_search (never for the exact fall-backs of the batched levels).
 static int32_t enqueue_scans(wax_vs_engine *e, SearchCtx *c, const float *d_queries, uint32_t n, const uint32_t *qs,
                              uint32_t k_eff, uint64_t row_offset, wax_vs_candidate *d_out, const uint64_t *d_ids,
-                             cudaStream_t stream, uint64_t *launches, const RowFilter &rf, bool sync_on_error) {
+                             cudaStream_t stream, uint64_t *launches, const RowFilter &rf, bool sync_on_error,
+                             bool shadow_route = false) {
     for (uint32_t i = 0; i < n; ++i) {
         const uint32_t qi = qs ? qs[i] : i;
         const int32_t rc = enqueue_search(e, c, d_queries + static_cast<size_t>(qi) * e->dims, k_eff, row_offset,
-                                          d_out + static_cast<size_t>(qi) * k_eff, d_ids, stream, launches, rf.mask(qi));
+                                          d_out + static_cast<size_t>(qi) * k_eff, d_ids, stream, launches, rf.mask(qi),
+                                          nullptr, nullptr, false, shadow_route);
         if (rc) {
             if (sync_on_error) cudaStreamSynchronize(stream);
             return rc;
@@ -1796,8 +1922,9 @@ static int32_t run_queries_on_device(wax_vs_engine *e, SearchCtx *c, const float
     }
     // below batch_min the tensor path only pays off through the bf16 shadow (single_shadow): never TF32 for one query
     if (tensor_path && !allow_bf16 && n_queries < static_cast<uint32_t>(std::max(e->tune.batch_min, 1))) tensor_path = false;
-    if (!tensor_path)
-        return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_out, d_ids, c->stream, launches, rf, true);
+    if (!tensor_path)       // one query (or a few): each its own scan, through the shadow route where it applies
+        return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_out, d_ids, c->stream, launches, rf, true,
+                             true);
     // Batched: one tensor-core pass over the corpus nominates, the finish kernel re-scores exactly and
     // proves completeness; unproven queries (rare) are re-run on the exact single-query path below.
     if ((rc = c->d_ok.ensure(static_cast<size_t>(n_queries), "proof flags"))) return rc;
@@ -1961,7 +2088,8 @@ static int32_t search_host(wax_vs_engine *e, const float *queries, uint32_t n_qu
             *c->h_flag = 0; c->host_seq = 0;
         }
         HostDelivery hd{queries, c->h_out, c->h_flag, ++c->host_seq};
-        if ((rc = enqueue_search(e, c, nullptr, k_eff, 0, c->d_out, nullptr, c->stream, &launches, nullptr, nullptr, &hd))) {
+        if ((rc = enqueue_search(e, c, nullptr, k_eff, 0, c->d_out, nullptr, c->stream, &launches, nullptr, nullptr, &hd,
+                                 false, true))) {
             cudaStreamSynchronize(c->stream);
             return rc;
         }
@@ -2008,7 +2136,7 @@ int32_t wax_vs_search_device(wax_vs_engine *e, const float *d_queries, uint32_t 
     if ((rc = sync_device_ids(e, &d_ids))) return rc;
     uint64_t launches = 0;
     return enqueue_scans(e, c, d_queries, n_queries, nullptr, k_eff, row_offset, d_candidates, d_ids,
-                         static_cast<cudaStream_t>(cuda_stream), &launches, RowFilter{}, false);
+                         static_cast<cudaStream_t>(cuda_stream), &launches, RowFilter{}, false, true);
 }
 
 // Batched form of wax_vs_search_device: the tensor-core levels on the caller's stream for the rank's shard.  Unlike
@@ -2547,10 +2675,11 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
                                          c->stream));
                 rf.d_index = c->d_query_filter + s0;
                 if ((prc = run_queries_on_device(e, c, dq, nq, k_max, 0, dout, nullptr, &launches, rf))) return prc;
-            } else {
+            } else {                // single queries (search_filtered) and the scan class: the single-query path
                 for (uint32_t j = 0; j < nq; ++j) {
                     prc = enqueue_search(e, c, dq + static_cast<size_t>(j) * e->dims, k_of[s0 + j], 0,
-                                         dout + static_cast<size_t>(j) * k_max, nullptr, c->stream, &launches, rf.mask(j));
+                                         dout + static_cast<size_t>(j) * k_max, nullptr, c->stream, &launches, rf.mask(j),
+                                         nullptr, nullptr, false, true);
                     if (prc) { cudaStreamSynchronize(c->stream); return prc; }
                 }
             }
@@ -3293,6 +3422,8 @@ int32_t wax_vs_debug_time_search(wax_vs_engine *e, uint32_t n_queries, int64_t t
         if ((rc = lease2.c->d_out.ensure(static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
     }
     SearchCtx *c2 = lease2.c;
+    // the shadow route's bf16 copy is cached per corpus version: bring it up to date outside the timed region
+    if (shadow_route_applies(e) && (rc = ensure_shadow(e, c->stream))) return rc;
     for (uint32_t it = 0; it < warmup + iters; ++it) {
         if (it == warmup) {
             launches = 0;
@@ -3304,7 +3435,8 @@ int32_t wax_vs_debug_time_search(wax_vs_engine *e, uint32_t n_queries, int64_t t
         SearchCtx *cc = (c2 && (it & 1u)) ? c2 : c;
         if (c2 && it == 0) { CUDA_TRY(cudaEventRecord(c->ev1, c->stream)); CUDA_TRY(cudaStreamWaitEvent(c2->stream, c->ev1, 0)); }  // queries ready
         rc = enqueue_search(e, cc, c->d_queries + static_cast<size_t>(qi) * e->dims, k_eff, 0,
-                            cc->d_out + static_cast<size_t>(qi) * k_eff, nullptr, cc->stream, &launches);
+                            cc->d_out + static_cast<size_t>(qi) * k_eff, nullptr, cc->stream, &launches, nullptr, nullptr,
+                            nullptr, false, true);
         if (rc) { cudaStreamSynchronize(c->stream); if (c2) cudaStreamSynchronize(c2->stream); return rc; }
     }
     if (c2) { CUDA_TRY(cudaEventRecord(c2->ev1, c2->stream)); CUDA_TRY(cudaStreamWaitEvent(c->stream, c2->ev1, 0)); }
@@ -3455,6 +3587,16 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "shadow_rows")) *out = e->shadow_rows;     // rows whose bf16 shadow is valid
     else if (!strcmp(name, "batch_heap_bump")) *out = e->heap_bump;          // sizes above the model's nominee-heap choice (adaptive)
     else if (!strcmp(name, "batch_last_heap")) *out = e->last_heap;          // nominee heap entries of the last bf16 level-1 launch
+    else if (!strcmp(name, "single_shadow_queries") || !strcmp(name, "single_shadow_fallbacks")) {
+        // single queries the shadow route answered / the fp32 scan answered after a failed proof, as the guarded scans
+        // counted them (contexts a concurrent call holds are not in the pool: read this when the engine is idle)
+        const int slot = !strcmp(name, "single_shadow_queries") ? 0 : 1;
+        uint64_t n = 0;
+        auto add = [&](const SearchCtx *c) { if (c->h_proof_count) n += *static_cast<volatile uint32_t *>(c->h_proof_count + slot); };
+        for (const SearchCtx *c : e->pool) add(c);
+        for (const auto &kv : e->stream_ctx) add(kv.second);
+        *out = n;
+    }
     else if (!strcmp(name, "pool_allocs")) *out = e->pool_allocs;
     else if (!strcmp(name, "pool_reuses")) *out = e->pool_reuses;
     else return fail(WAX_VS_ERR_ARGUMENT, "unknown counter '%s'", name);
@@ -3584,6 +3726,18 @@ int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value
     else if (!strcmp(key, "batch_l2")) e->tune.batch_l2 = v;
     else if (!strcmp(key, "filter_bitset_bytes")) e->tune.filter_bitset_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
     else if (!strcmp(key, "single_shadow")) e->tune.single_shadow = v;
+    else if (!strcmp(key, "shadow_scan")) {     // also closes the skip window, including failures not yet seen
+        std::lock_guard<std::mutex> pg(e->pool_mu);
+        e->tune.shadow_scan = v;
+        e->shadow_scan_skip = 0;
+        auto seen = [](SearchCtx *c) { if (c->h_proof_count) c->seen_failed = *static_cast<volatile uint32_t *>(c->h_proof_count + 1); };
+        for (SearchCtx *c : e->pool) seen(c);
+        for (auto &kv : e->stream_ctx) seen(kv.second);
+    }
+    else if (!strcmp(key, "shadow_rows_per_step")) e->tune.shadow_rows_per_step = v;
+    else if (!strcmp(key, "shadow_warps")) e->tune.shadow_warps = v;
+    else if (!strcmp(key, "shadow_stages")) e->tune.shadow_stages = v;
+    else if (!strcmp(key, "shadow_scan_min_bytes")) e->tune.shadow_scan_min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
     else if (!strcmp(key, "shard_fused")) e->tune.shard_fused = v;
     else if (!strcmp(key, "tail_select")) e->tune.tail_select = v;
     else if (!strcmp(key, "inline_query")) e->tune.inline_query = v;

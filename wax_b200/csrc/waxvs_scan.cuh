@@ -66,7 +66,19 @@ struct ScanParams {
                                 // grid stage -- %globaltimer nanoseconds
     ShardParams shard;          // shard.world > 0: `out` is this rank's local list and the last CTA goes on to exchange it
                                 // with the other ranks over NVLink and to merge (waxvs_shard.cuh): still the same launch
+    // The bf16-shadow route of a single query (DESIGN 4.1): the SHADOW form nominates, batch_finish_kernel re-scores and
+    // proves, then the fp32 form runs guarded by the proof.
+    uint64_t *nominees;         // SHADOW: [k][kNomineeStride] the nominee keys, laid out as batch_finish_kernel's heaps of
+                                // one query and one slice (entry 0 = the worst nominee, real only when all k are)
+    float *query_store;         // SHADOW, query in the parameters: CTA 0 also stores it here for the launches that follow
+    const uint32_t *proof_ok;   // fp32 cosine / dot, E = 1: non-null = guarded by the proof flag batch_finish_kernel wrote: when set
+                                // every CTA returns at entry (CTA 0 first delivers `out` to the host), else a plain scan
+    uint32_t *proof_count;      // guarded: [0] proofs that held, [1] that failed -- running counts on the device ...
+    uint32_t *proof_count_host; // ... mirrored into mapped pinned memory, read by the host without synchronising
 };
+
+// batch_finish_kernel reads entry e of query 0's heap of slice 0 at e * kBatchM (static_assert in waxvs_batch.cuh).
+constexpr int kNomineeStride = 128;
 
 __device__ __forceinline__ bool row_allowed(const ScanParams &p, uint32_t row) {
     return p.mask == nullptr || ((__ldg(p.mask + (row >> 5)) >> (row & 31u)) & 1u) != 0u;
@@ -87,9 +99,23 @@ __device__ __forceinline__ void write_candidate(const ScanParams &p, int slot, u
     if (p.host_out) p.host_out[slot] = c;
 }
 
+// The tails' output: result slot `slot` (0 = best) -- a candidate, or (SHADOW) a nominee key, the worst of the k in
+// entry 0 and slot i < k-1 in entry i+1.
+template <bool SHADOW>
+__device__ __forceinline__ void write_slot(const ScanParams &p, int slot, uint64_t key) {
+    if constexpr (SHADOW) p.nominees[static_cast<size_t>(slot == static_cast<int>(p.k) - 1 ? 0 : slot + 1) * kNomineeStride] = key;
+    else write_candidate(p, slot, key);
+}
+
+// bf16 x 4 (one uint2 of the shadow, element 0 in the low half) -> fp32, exactly.
+__device__ __forceinline__ float4 bf16x4_to_float4(uint2 u) {
+    return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u),
+                       __uint_as_float(u.y << 16), __uint_as_float(u.y & 0xFFFF0000u));
+}
+
 // CTA merge + grid merge + output.  Called by every thread of the CTA after the scan loop.
 // lists: shared [warps][E*32] u64;  block_keys: global [grid][E*32].
-template <int E>
+template <int E, bool SHADOW = false>
 __device__ __forceinline__ void finish_topk(const ScanParams &p, WarpTopK<E> &tk, uint64_t *lists, int warp,
                                             int lane, int warps) {
     const int k = static_cast<int>(p.k);
@@ -150,7 +176,7 @@ __device__ __forceinline__ void finish_topk(const ScanParams &p, WarpTopK<E> &tk
         }
 #pragma unroll
         for (int j = 0; j < E; ++j)
-            if (j * 32 + lane < k) write_candidate(p, j * 32 + lane, tk.key[j]);
+            if (j * 32 + lane < k) write_slot<SHADOW>(p, j * 32 + lane, tk.key[j]);
         if (lane == 0) { *p.ticket = 0u; if (p.work_counter) *p.work_counter = 0u; }
         if (p.host_flag && !p.shard.world) {          // result complete in host memory: tell the waiting caller
             __threadfence_system();
@@ -230,7 +256,7 @@ __device__ __forceinline__ uint64_t block_select_kth(ForEach for_each, uint32_t 
 
 // The selection tail: called by every thread of the CTA after the scan loop (the warps' register lists need not be
 // merged, or even sorted, for this).  scratch = the dynamic shared memory (the idle ring), p.tail_smem_bytes of it.
-template <int E>
+template <int E, bool SHADOW = false>
 __device__ __forceinline__ void finish_topk_select(const ScanParams &p, WarpTopK<E> &tk, unsigned char *scratch) {
     __shared__ SelectScratch ss;
     __shared__ uint32_t s_last2;
@@ -280,9 +306,9 @@ __device__ __forceinline__ void finish_topk_select(const ScanParams &p, WarpTopK
             const uint64_t key = ss.sel[i];
             uint32_t rank = 0;
             for (uint32_t j = 0; j < n_sel; ++j) rank += ss.sel[j] < key ? 1u : 0u;
-            write_candidate(p, static_cast<int>(rank), key);
+            write_slot<SHADOW>(p, static_cast<int>(rank), key);
         } else {
-            write_candidate(p, static_cast<int>(i), WAXVS_KEY_NONE);      // padding after the n_sel ranked entries
+            write_slot<SHADOW>(p, static_cast<int>(i), WAXVS_KEY_NONE);   // padding after the n_sel ranked entries
         }
     }
     if (p.host_flag && !p.shard.world) __threadfence_system();
@@ -304,11 +330,36 @@ __device__ __forceinline__ void finish_topk_select(const ScanParams &p, WarpTopK
 //   E      register-list slots per lane: fused top-k for k <= 32*E (E = 1: k <= 32, E = 4: k <= 128 -- the production
 //          candidateLimit of 72, UnifiedSearch.swift:1195-1200, stays in the single launch)
 //   EMIT   false: fused top-k;  true: write orderable distance keys for the large-k select path
-template <int C, int R, int METRIC, int E, bool EMIT>
+//   SHADOW true (C > 0, cosine / dot, E = 4, fused): the nominating pass of the bf16-shadow route.  p.corpus is the
+//          shadow (bf16 rows, cosine rows pre-scaled by 1/|v|): a lane reads chunk lane + 32c as one uint2 of 4 bf16
+//          where the fp32 form reads a float4, widens it exactly and FMAs it against the fp32 query -- one quantity per
+//          row, score' = q.v~ for both metrics, key make_key(-score', row) (= nominee_key).  Only the row is rounded,
+//          so kBf16Eps bounds |score' - score|.  Every warp keeps k (= 128) nominees, so the grid's k-th bounds every
+//          row left out; the tails write them for batch_finish_kernel (write_slot).  A NaN score' is never nominated.
+template <int C, int R, int METRIC, int E, bool EMIT, bool SHADOW = false>
 __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant__ ScanParams p) {
-    const int D4 = C > 0 ? 32 * C : static_cast<int>(p.dims / 4u);          // float4 per row
+    static_assert(!SHADOW || (C > 0 && METRIC != kL2 && !EMIT), "the shadow form covers the unrolled cosine / dot shapes");
+    if constexpr (!SHADOW && !EMIT && E == 1 && METRIC != kL2) {
+        if (p.proof_ok) {               // guarded launch after a shadow proof (batch_finish_kernel, same stream; k <= 32)
+            const bool proven = *p.proof_ok != 0u;
+            if (blockIdx.x == 0) {
+                if (threadIdx.x == 0) {
+                    const uint32_t n = ++p.proof_count[proven ? 0 : 1];
+                    *static_cast<volatile uint32_t *>(p.proof_count_host + (proven ? 0 : 1)) = n;
+                }
+                if (proven && p.host_flag) {      // the delivery the last CTA would otherwise do
+                    for (uint32_t i = threadIdx.x; i < p.k; i += blockDim.x) p.host_out[i] = p.out[i];
+                    __threadfence_system();
+                    __syncthreads();
+                    if (threadIdx.x == 0) st_release_sys_u64(p.host_flag, p.host_seq);
+                }
+            }
+            if (proven) return;
+        }
+    }
+    const int D4 = C > 0 ? 32 * C : static_cast<int>(p.dims / 4u);          // float4 (SHADOW: uint2) per row
     const int CN = C > 0 ? C : (D4 + 31) / 32;                               // chunks per lane
-    const uint32_t ROW_BYTES = C > 0 ? 512u * C : p.dims * 4u;
+    const uint32_t ROW_BYTES = C > 0 ? (SHADOW ? 256u : 512u) * C : p.dims * 4u;
     const uint32_t STAGE_BYTES = ROW_BYTES * R;
     constexpr int LANES_PER_ROW = 32 / R;
 
@@ -337,8 +388,12 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         __syncthreads();
     }
     auto qchunk = [&](int c) -> float4 { return C > 0 ? q[C > 0 ? c : 0] : qs[lane + 32 * c]; };
+    if constexpr (SHADOW) {             // the finish and the guarded scan read the query from device memory
+        if (p.query_store && p.query == nullptr && blockIdx.x == 0)
+            for (uint32_t i = threadIdx.x; i < p.dims; i += blockDim.x) p.query_store[i] = p.query_inline[i];
+    }
     float a2 = 0.0f, sqrt_a2 = 0.0f;
-    if (METRIC == kCosine) {
+    if (METRIC == kCosine && !SHADOW) {
         float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
 #pragma unroll
         for (int c = 0; c < CN; ++c) {
@@ -363,7 +418,9 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         const uint32_t bytes = rows * ROW_BYTES;
         stage_step[s] = step;                        // released to the warp by the mbarrier arrive below
         mbar_arrive_expect_tx(&bars[s], bytes);
-        const float *src = p.corpus + static_cast<size_t>(row0) * p.dims;
+        const void *src = SHADOW ? static_cast<const void *>(reinterpret_cast<const unsigned char *>(p.corpus) +
+                                                             static_cast<size_t>(row0) * ROW_BYTES)
+                                 : static_cast<const void *>(p.corpus + static_cast<size_t>(row0) * p.dims);
         if (p.use_l2_hint) bulk_copy_g2s_hint(ring + s * STAGE_BYTES, src, bytes, &bars[s], policy);
         else bulk_copy_g2s(ring + s * STAGE_BYTES, src, bytes, &bars[s]);
     };
@@ -460,7 +517,8 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
 #pragma unroll
             for (int c = 0; c < CN; ++c) {
                 if (C == 0 && lane + 32 * c >= D4) break;   // ragged last chunk (dims % 128 != 0): this lane has no element
-                const float4 v = tile[r * D4 + lane + 32 * c];
+                const float4 v = SHADOW ? bf16x4_to_float4(reinterpret_cast<const uint2 *>(tile)[r * D4 + lane + 32 * c])
+                                        : tile[r * D4 + lane + 32 * c];
                 const float4 qc = qchunk(c);
                 if (METRIC == kL2) {
                     const float dx = __fsub_rn(qc.x, v.x), dy = __fsub_rn(qc.y, v.y);
@@ -470,7 +528,7 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
                 } else {
                     a0 = __fmaf_rn(qc.x, v.x, a0); a1 = __fmaf_rn(qc.y, v.y, a1);
                     a2_ = __fmaf_rn(qc.z, v.z, a2_); a3 = __fmaf_rn(qc.w, v.w, a3);
-                    if (METRIC == kCosine) {
+                    if (METRIC == kCosine && !SHADOW) {
                         b0 = __fmaf_rn(v.x, v.x, b0); b1 = __fmaf_rn(v.y, v.y, b1);
                         b2 = __fmaf_rn(v.z, v.z, b2); b3 = __fmaf_rn(v.w, v.w, b3);
                     }
@@ -491,15 +549,17 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         if (++s == stages) { s = 0; parity ^= 1u; }
 
         warp_reduce_scatter<R>(sum0, lane);
-        if (METRIC == kCosine) warp_reduce_scatter<R>(sum1, lane);
+        if (METRIC == kCosine && !SHADOW) warp_reduce_scatter<R>(sum1, lane);
 
         const uint32_t my_row = step * R + (lane / LANES_PER_ROW);
         float d;
-        if (METRIC == kCosine) d = finish_cos(sum0[0], a2, sqrt_a2, sum1[0]);
+        if (SHADOW) d = -sum0[0];          // -score': the nominee key's distance
+        else if (METRIC == kCosine) d = finish_cos(sum0[0], a2, sqrt_a2, sum1[0]);
         else if (METRIC == kDot) d = finish_dot(sum0[0]);
         else d = finish_l2(sum0[0]);
         const bool leader = (lane % LANES_PER_ROW) == 0;
-        const bool ok = (my_row < p.n_rows) && finite_f32(d);
+        // SHADOW: a score' of +-inf still has its place in the order (only the exact re-score decides), NaN has none
+        const bool ok = (my_row < p.n_rows) && (SHADOW ? d == d : finite_f32(d));
 
         if (EMIT) {
             if (leader && my_row < p.n_rows)
@@ -530,8 +590,8 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
     if (p.trace && lane == 0) atomicMax(p.trace + 1, global_timer_ns());
     if (!EMIT) {
         if (E > 1) tk.flush(lane, k);
-        if (p.tail_select) finish_topk_select<E>(p, tk, smem);
-        else finish_topk<E>(p, tk, lists, warp, lane, warps);
+        if (p.tail_select) finish_topk_select<E, SHADOW>(p, tk, smem);
+        else finish_topk<E, SHADOW>(p, tk, lists, warp, lane, warps);
     }
 }
 
