@@ -390,6 +390,26 @@ int32_t wax_vs_debug_batch_nominations(wax_vs_engine *engine, const float *queri
                                        const uint32_t *allow_bits, float *out_scores, uint32_t *out_ok,
                                        uint64_t *out_heaps, uint64_t heaps_cap, uint32_t *out_shape);
 
+/* Read-out of the single-query bf16-shadow route's first two launches (tests): for one host query and top_k <= 32, the
+   SHADOW form of the scan nominates 128 rows from the bf16 shadow and the finish re-scores them exactly and proves the
+   result -- the route's own launch code, in the shape the options select (shadow_rows_per_step, shadow_warps,
+   shadow_stages, grid, chunk_steps, tail_select), whatever "shadow_scan", "shadow_scan_min_bytes" and the skip window
+   after a failed proof say; the proof counters are not touched.  `allow_bits`: optional row filter (one bit per row,
+   set = allowed).  out_keys[128] receives the nominee keys in the layout the finish reads (entry 0 = the worst of the
+   128, entries 1..127 = the best first; key = (orderable(-score') << 32) | row, padding 0xFFFFFFFFFFFFFFFF);
+   out_ok[1] the proof flag; out_result[min(top_k, count)] the finish's candidates (frame_id resolved); out_shape[7] =
+   {rows per 128-dim chunk C, rows per step, warps, stages, grid, chunk_steps (0 = static), tail_select}.
+   WAX_VS_ERR_UNSUPPORTED when the route cannot run: l2, dims not a multiple of 128 up to 1536, top_k > 32, no
+   shadow, an empty corpus or a requested shape whose ring does not fit. */
+int32_t wax_vs_debug_shadow_nominations(wax_vs_engine *engine, const float *query, int64_t top_k, const uint32_t *allow_bits,
+                                        uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
+                                        uint32_t *out_shape);
+
+/* The bf16 shadow of rows [first, first + n) (brought up to date first): dims bf16 bit patterns per row, cosine rows
+   pre-scaled by 1/|v|.  WAX_VS_ERR_UNSUPPORTED when the engine keeps no shadow (batch_bf16 = 0, dims % 64 != 0, or it
+   did not fit in device memory). */
+int32_t wax_vs_debug_read_shadow(wax_vs_engine *engine, uint64_t first, uint64_t n, uint16_t *dst);
+
 /* Streaming-read ceiling on the same box: a plain coalesced LDG.128 read of the live corpus bytes, best of
    `iters` (milliseconds, and the bytes read).  Context for the roofline fraction (SURVEY.md section 8d). */
 int32_t wax_vs_debug_stream_read(wax_vs_engine *engine, uint32_t iters, float *out_best_ms, uint64_t *out_bytes);

@@ -61,6 +61,8 @@ def test_argument_validation_without_a_device():
     assert L.wax_vs_create(4, 0, None, 0, None) == _lib.ERR_NULL
     assert L.wax_vs_device_count(None) == _lib.ERR_NULL
     assert L.wax_vs_count(None, None) == _lib.ERR_NULL
+    assert L.wax_vs_debug_shadow_nominations(None, None, 10, None, None, None, None, None) == _lib.ERR_NULL
+    assert L.wax_vs_debug_read_shadow(None, 0, 1, None) == _lib.ERR_NULL
     L.wax_vs_destroy(None)  # no-op
 
 

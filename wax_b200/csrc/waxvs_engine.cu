@@ -713,25 +713,13 @@ static bool shadow_route_applies(const wax_vs_engine *e) {
     return e->tune.shadow_scan && (e->similarity == WAX_VS_COSINE || e->similarity == WAX_VS_DOT) && !e->debug_trace &&
            batch_bf16_wanted(e) && e->n_rows * e->dims * sizeof(float) >= e->tune.shadow_scan_min_bytes;
 }
-static int32_t enqueue_shadow_route(wax_vs_engine *e, SearchCtx *c, ScanParams &p, cudaStream_t stream, uint64_t *launches) {
-    if (!shadow_route_applies(e)) return WAX_VS_OK;
-    TmaConfig cfg{};
-    if (!pick_tma_config(e, &cfg, 1, sizeof(__nv_bfloat16))) return WAX_VS_OK;
+// Launches 1 and 2 of the route for the query of `p` (the fp32 scan's parameters: query, filter, k, out, ids) in the
+// SHADOW shape `cfg`, over a valid shadow: the SHADOW form writes the kShadowNominees keys to c->d_heaps, the finish
+// re-scores them exactly into p.out and writes its proof flag to c->d_ok.  shape (optional, the read-out
+// wax_vs_debug_shadow_nominations): {C, R, warps, stages, grid, chunk_steps, tail_select} of the SHADOW launch.
+static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const ScanParams &p, const TmaConfig &cfg,
+                                          cudaStream_t stream, uint64_t *launches, uint32_t *shape = nullptr) {
     int32_t rc;
-    if (!c->h_proof_count) {
-        if ((rc = c->d_proof_count.ensure(2, "proof counts")) || (rc = c->h_proof_count.ensure(2, "proof count mirror"))) return rc;
-        CUDA_TRY(cudaMemsetAsync(c->d_proof_count, 0, 2 * sizeof(uint32_t), stream));
-        c->h_proof_count[0] = c->h_proof_count[1] = 0;
-        c->seen_failed = 0;
-    }
-    {
-        std::lock_guard<std::mutex> pg(e->pool_mu);
-        const uint32_t failed = *static_cast<volatile uint32_t *>(c->h_proof_count + 1);   // no synchronisation: may lag
-        if (failed != c->seen_failed) { c->seen_failed = failed; e->shadow_scan_skip = kShadowSkipQueries; }
-        if (e->shadow_scan_skip > 0) { --e->shadow_scan_skip; return WAX_VS_OK; }
-    }
-    if ((rc = ensure_shadow(e, stream))) return rc;
-    if (!e->shadow_valid) return WAX_VS_OK;
     if ((rc = c->d_heaps.ensure(static_cast<size_t>(kShadowNominees) * kNomineeStride, "nominee keys")) ||
         (rc = c->d_ok.ensure(1, "proof flags")) || (!p.query && (rc = c->d_queries.ensure(e->dims, "query buffer"))))
         return rc;
@@ -761,10 +749,69 @@ static int32_t enqueue_shadow_route(wax_vs_engine *e, SearchCtx *c, ScanParams &
     kernel<<<1, 512, fsmem, stream>>>(fp);
     CUDA_TRY(cudaGetLastError());
     *launches += 2;
+    if (shape) {
+        const uint32_t s[7] = {static_cast<uint32_t>(cfg.C), static_cast<uint32_t>(cfg.R), static_cast<uint32_t>(cfg.warps),
+                               static_cast<uint32_t>(cfg.stages), static_cast<uint32_t>(grid), sp.chunk_steps, sp.tail_select};
+        std::copy(s, s + 7, shape);
+    }
+    return WAX_VS_OK;
+}
 
+static int32_t enqueue_shadow_route(wax_vs_engine *e, SearchCtx *c, ScanParams &p, cudaStream_t stream, uint64_t *launches) {
+    if (!shadow_route_applies(e)) return WAX_VS_OK;
+    TmaConfig cfg{};
+    if (!pick_tma_config(e, &cfg, 1, sizeof(__nv_bfloat16))) return WAX_VS_OK;
+    int32_t rc;
+    if (!c->h_proof_count) {
+        if ((rc = c->d_proof_count.ensure(2, "proof counts")) || (rc = c->h_proof_count.ensure(2, "proof count mirror"))) return rc;
+        CUDA_TRY(cudaMemsetAsync(c->d_proof_count, 0, 2 * sizeof(uint32_t), stream));
+        c->h_proof_count[0] = c->h_proof_count[1] = 0;
+        c->seen_failed = 0;
+    }
+    {
+        std::lock_guard<std::mutex> pg(e->pool_mu);
+        const uint32_t failed = *static_cast<volatile uint32_t *>(c->h_proof_count + 1);   // no synchronisation: may lag
+        if (failed != c->seen_failed) { c->seen_failed = failed; e->shadow_scan_skip = kShadowSkipQueries; }
+        if (e->shadow_scan_skip > 0) { --e->shadow_scan_skip; return WAX_VS_OK; }
+    }
+    if ((rc = ensure_shadow(e, stream))) return rc;
+    if (!e->shadow_valid) return WAX_VS_OK;
+    if ((rc = enqueue_shadow_nominations(e, c, p, cfg, stream, launches))) return rc;
     p.proof_ok = c->d_ok;
     p.proof_count = c->d_proof_count;
     p.proof_count_host = c->h_proof_count;
+    return WAX_VS_OK;
+}
+
+// The scan parameters of one query (`d_query` on the device, or nullptr when place_host_query sets it); the caller sets
+// the tail, the delivery and the shard exchange.  Auto chunk_steps (0 here) is set by tma_grid.
+static ScanParams scan_params(const wax_vs_engine *e, SearchCtx *c, const float *d_query, uint32_t k_eff, uint64_t row_offset,
+                              wax_vs_candidate *d_out, const uint64_t *d_ids, const uint32_t *d_mask) {
+    ScanParams p{};
+    p.corpus = e->d_corpus; p.query = d_query;
+    p.n_rows = static_cast<uint32_t>(e->n_rows); p.dims = e->dims; p.k = k_eff;
+    p.block_keys = c->d_block_keys; p.ticket = c->d_ticket; p.out = d_out;
+    p.frame_ids = d_ids; p.id_base = e->id_base; p.row_offset = row_offset;
+    p.use_l2_hint = e->tune.l2_hint ? 1u : 0u;
+    p.chunk_steps = e->tune.chunk_steps > 0 ? static_cast<uint32_t>(e->tune.chunk_steps) : 0u;
+    p.work_counter = c->d_ticket + 1;
+    p.mask = d_mask;
+    p.trace = e->debug_trace;
+    return p;
+}
+
+// A host query: in the kernel parameters when the kernel can take it (inline_ok: a fused TMA-staged scan), else copied
+// to c->d_queries on `stream`.
+static int32_t place_host_query(wax_vs_engine *e, SearchCtx *c, ScanParams &p, const float *h_query, bool inline_ok,
+                                cudaStream_t stream) {
+    if (inline_ok && e->tune.inline_query != 0 && e->dims <= static_cast<uint32_t>(kInlineQueryFloats)) {
+        memcpy(p.query_inline, h_query, e->dims * sizeof(float));
+        p.query = nullptr;
+        return WAX_VS_OK;
+    }
+    int32_t rc = stage_queries(e, c, h_query, 1, stream);
+    if (rc) return rc;
+    p.query = c->d_queries;
     return WAX_VS_OK;
 }
 
@@ -800,17 +847,7 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
         CUDA_TRY(cudaMemsetAsync(d_out, 0, static_cast<size_t>(k_eff) * sizeof(wax_vs_candidate), stream));
         return shard ? exchange_standalone() : WAX_VS_OK;
     }
-    ScanParams p{};
-    p.corpus = e->d_corpus; p.query = d_query;
-    p.n_rows = static_cast<uint32_t>(e->n_rows); p.dims = e->dims; p.k = k_eff;
-    p.block_keys = c->d_block_keys; p.ticket = c->d_ticket; p.out = d_out;
-    p.frame_ids = d_ids; p.id_base = e->id_base; p.row_offset = row_offset;
-    p.use_l2_hint = e->tune.l2_hint ? 1u : 0u;
-    p.chunk_steps = e->tune.chunk_steps > 0 ? static_cast<uint32_t>(e->tune.chunk_steps) : 0u;   // auto: set below
-    p.work_counter = c->d_ticket + 1;
-    p.mask = d_mask;
-    p.trace = e->debug_trace;
-
+    ScanParams p = scan_params(e, c, d_query, k_eff, row_offset, d_out, d_ids, d_mask);
     const bool emit = keys_only || k_eff > static_cast<uint32_t>(e->tune.fused_k_max);
     const int mode = emit ? 2 : (k_eff <= 32 ? 0 : 1);
     if (emit) {
@@ -824,15 +861,8 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
     if (e->tune.variant == 1 && !use_tma)
         return fail(WAX_VS_ERR_UNSUPPORTED, "TMA-staged kernel does not support dims=%u", e->dims);
     if (host && host->h_query) {
-        const bool inline_ok = use_tma && !emit && e->tune.inline_query != 0 && e->dims <= static_cast<uint32_t>(kInlineQueryFloats);
-        if (inline_ok) {
-            memcpy(p.query_inline, host->h_query, e->dims * sizeof(float));
-            p.query = nullptr;
-        } else {
-            int32_t rc = stage_queries(e, c, host->h_query, 1, stream);
-            if (rc) return rc;
-            p.query = c->d_queries;
-        }
+        int32_t rc = place_host_query(e, c, p, host->h_query, use_tma && !emit, stream);
+        if (rc) return rc;
     }
     if (host && host->host_out && !emit && !shard) {
         p.host_out = host->host_out; p.host_flag = host->host_flag; p.host_seq = host->seq;
@@ -3695,6 +3725,65 @@ int32_t wax_vs_debug_batch_nominations(wax_vs_engine *e, const float *queries, u
         return fail(WAX_VS_ERR_BUFFER, "the heaps need %llu entries (%llu given)", static_cast<unsigned long long>(n_heap),
                     static_cast<unsigned long long>(heaps_cap));
     CUDA_TRY(cudaMemcpy(out_heaps, c->d_heaps, n_heap * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_debug_shadow_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
+                                        uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
+                                        uint32_t *out_shape) {
+    if (!e || !query || !out_keys || !out_ok || !out_result || !out_shape) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    const uint32_t k_eff = static_cast<uint32_t>(std::min<uint64_t>(clamp_topk(top_k), std::max<uint64_t>(e->n_rows, 1)));
+    TmaConfig cfg{};
+    if (e->n_rows == 0 || k_eff > 32u || (e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT) ||
+        !batch_bf16_wanted(e) || !pick_tma_config(e, &cfg, 1, sizeof(__nv_bfloat16)))
+        return fail(WAX_VS_ERR_UNSUPPORTED, "no bf16-shadow route for k=%u, dims=%u in this shape", k_eff, e->dims);
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
+    if (rc) return rc;
+    SearchCtx *c = lease.c;
+    if ((rc = ensure_shadow(e, c->stream))) return rc;
+    if (!e->shadow_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the bf16 shadow does not fit in device memory");
+    if ((rc = c->d_out.ensure(k_eff, "result buffer"))) return rc;
+    const uint32_t *d_mask = nullptr;
+    if (allow_bits) {
+        const size_t words = static_cast<size_t>((e->n_rows + 31) / 32);
+        if ((rc = c->d_mask.ensure(words, "row filter"))) return rc;
+        CUDA_TRY(cudaMemcpyAsync(c->d_mask, allow_bits, words * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+        d_mask = c->d_mask;
+    }
+    ScanParams p = scan_params(e, c, nullptr, k_eff, 0, c->d_out, nullptr, d_mask);
+    if ((rc = place_host_query(e, c, p, query, true, c->stream))) return rc;
+    uint64_t launches = 0;
+    if ((rc = enqueue_shadow_nominations(e, c, p, cfg, c->stream, &launches, out_shape))) {
+        cudaStreamSynchronize(c->stream);
+        return rc;
+    }
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    CUDA_TRY(cudaMemcpy2D(out_keys, sizeof(uint64_t), c->d_heaps, kNomineeStride * sizeof(uint64_t), sizeof(uint64_t),
+                          kShadowNominees, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(out_ok, c->d_ok, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(out_result, c->d_out, k_eff * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost));
+    for (uint32_t i = 0; i < k_eff; ++i)
+        if (out_result[i].valid) out_result[i].frame_id = frame_id_of(e, out_result[i].row);
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_debug_read_shadow(wax_vs_engine *e, uint64_t first, uint64_t n, uint16_t *dst) {
+    if (!e || !dst) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
+    if (!batch_bf16_wanted(e)) return fail(WAX_VS_ERR_UNSUPPORTED, "no bf16 shadow for dims=%u with these options", e->dims);
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
+    if (rc) return rc;
+    if ((rc = ensure_shadow(e, lease.c->stream))) return rc;
+    if (!e->shadow_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the bf16 shadow does not fit in device memory");
+    if (n) CUDA_TRY(cudaMemcpy(dst, e->d_shadow + first * e->dims, n * e->dims * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost));
     return WAX_VS_OK;
 }
 

@@ -335,7 +335,7 @@ __device__ __forceinline__ void finish_topk_select(const ScanParams &p, WarpTopK
 //          where the fp32 form reads a float4, widens it exactly and FMAs it against the fp32 query -- one quantity per
 //          row, score' = q.v~ for both metrics, key make_key(-score', row) (= nominee_key).  Only the row is rounded,
 //          so kBf16Eps bounds |score' - score|.  Every warp keeps k (= 128) nominees, so the grid's k-th bounds every
-//          row left out; the tails write them for batch_finish_kernel (write_slot).  A NaN score' is never nominated.
+//          row left out; the tails write them for batch_finish_kernel (write_slot).  A non-finite score' counts as +inf.
 template <int C, int R, int METRIC, int E, bool EMIT, bool SHADOW = false>
 __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant__ ScanParams p) {
     static_assert(!SHADOW || (C > 0 && METRIC != kL2 && !EMIT), "the shadow form covers the unrolled cosine / dot shapes");
@@ -557,9 +557,12 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         else if (METRIC == kCosine) d = finish_cos(sum0[0], a2, sqrt_a2, sum1[0]);
         else if (METRIC == kDot) d = finish_dot(sum0[0]);
         else d = finish_l2(sum0[0]);
+        // SHADOW: a non-finite score' bounds nothing -- a product q_i v~_i can overflow where q_i v_i does not (v~ rounded
+        // up), giving +-inf or inf - inf = NaN for a row whose exact score is finite.  Such a row is nominated first
+        // (score' = +inf), so the finish re-scores it; and as entry 0 it refuses the proof.
+        if (SHADOW && !finite_f32(d)) d = -INFINITY;
         const bool leader = (lane % LANES_PER_ROW) == 0;
-        // SHADOW: a score' of +-inf still has its place in the order (only the exact re-score decides), NaN has none
-        const bool ok = (my_row < p.n_rows) && (SHADOW ? d == d : finite_f32(d));
+        const bool ok = (my_row < p.n_rows) && (SHADOW || finite_f32(d));
 
         if (EMIT) {
             if (leader && my_row < p.n_rows)

@@ -614,6 +614,41 @@ class CUDAVectorEngine:
         out.update(scores=scores, ok=ok, heaps=heaps.reshape(out["slices"] * out["groups"], out["kprime"], 128))
         return out
 
+    def shadow_nominations(self, vector, top_k: int, allow_rows=None):
+        """Read-out of the single-query bf16-shadow route's nomination and finish (wax_vs_debug_shadow_nominations), in
+        the shape the options select.  Returns a dict: keys [128] uint64 nominee keys (entry 0 = the worst, entries
+        1..127 = the best first), ok (the proof flag), result [(frame_id, score)] of the finish (the search's scores,
+        padding dropped) and the launch shape (C, R, warps, stages, grid, chunk_steps, tail_select).  `allow_rows`:
+        optional row filter."""
+        q = np.ascontiguousarray(vector, dtype=np.float32).reshape(self.dimensions)
+        n = self.count
+        k = max(1, min(int(top_k), n))
+        keys = np.empty(128, np.uint64)
+        ok = C.c_uint32(0)
+        result = (L.Candidate * k)()
+        shape = np.zeros(7, np.uint32)
+        bits = None
+        if allow_rows is not None:
+            mask = np.zeros(((n + 31) // 32) * 32, bool)
+            mask[np.asarray(allow_rows, np.int64)] = True
+            bits = (mask.reshape(-1, 32).astype(np.uint64) << np.arange(32, dtype=np.uint64)).sum(1).astype(np.uint32)
+        u32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
+        _check(L.lib().wax_vs_debug_shadow_nominations(
+            self._h, q.ctypes.data_as(C.POINTER(C.c_float)), int(top_k), None if bits is None else u32(bits),
+            keys.ctypes.data_as(C.POINTER(C.c_uint64)), C.byref(ok), result, u32(shape)))
+        one = np.float32(1.0)
+        score = (lambda d: float(one - np.float32(d))) if self.metric is VectorMetric.cosine else (lambda d: float(-np.float32(d)))
+        names = ("C", "R", "warps", "stages", "grid", "chunk_steps", "tail_select")
+        out = {name: int(v) for name, v in zip(names, shape)}
+        out.update(keys=keys, ok=ok.value, result=[(int(c.frame_id), score(c.distance)) for c in result if c.valid])
+        return out
+
+    def read_shadow(self, first: int, n: int) -> np.ndarray:
+        """The bf16 shadow of rows [first, first + n) as uint16 bit patterns [n, dims] (wax_vs_debug_read_shadow)."""
+        out = np.empty((n, self.dimensions), np.uint16)
+        _check(L.lib().wax_vs_debug_read_shadow(self._h, first, n, out.ctypes.data_as(C.POINTER(C.c_uint16))))
+        return out
+
     def stream_read_gbs(self, iters: int = 5) -> float:
         """Plain coalesced read of the corpus bytes: the box's streaming-read ceiling in GB/s."""
         ms, nbytes = C.c_float(0), C.c_uint64(0)
