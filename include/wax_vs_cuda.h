@@ -236,6 +236,57 @@ int32_t wax_vs_search_batch_grouped(wax_vs_engine *engine, const float *queries,
                                     const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids,
                                     float *out_scores, uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n);
 
+/* ---- frame attributes: time-range and tag predicates below the top-k (API EXTENSION over the reference) -------------
+   Wax post-filters every hit in UnifiedSearch.passesFrameFilter (UnifiedSearch.swift:1241-1258): a timeRange
+   (SearchRequest.swift:90-105; TimeRange.contains: after inclusive, before exclusive) and the includeDeleted /
+   includeSuperseded / includeSurrogates flags; PhotoRAG and VideoRAG pass a timeRange into the same request
+   (PhotoRAGOrchestrator.swift:238-252, VideoRAGOrchestrator.swift:226-261) and skip superseded and deleted frames by hand
+   (:286, :318, :758).  Here each row carries a timestamp and a 64-bit tag mask, and a predicate over them is evaluated on
+   the device; the caller assigns the tag bits (INTEGRATION.md maps FrameMeta onto them).
+
+   A row never given attributes has timestamp 0 and tags 0.  Attributes follow their rows as groups do: an appended frame
+   gets the defaults, an upsert keeps the frame's attributes, removes drop them; MV2V has no place for them, so
+   wax_vs_deserialize and wax_vs_debug_fill_synthetic reset every row and the caller re-applies them after loading.  The
+   first where search after a mutation or wax_vs_set_attributes uploads a device copy (16 bytes per row, counter
+   "attribute_uploads"); later ones reuse it. */
+typedef struct wax_vs_where {
+    int64_t after;      /* timestamp >= after;  INT64_MIN = no lower bound                                  */
+    int64_t before;     /* timestamp <  before; INT64_MAX = no upper bound (a timestamp of INT64_MAX passes) */
+    uint64_t all_tags;  /* (tags & all_tags) == all_tags                                                    */
+    uint64_t no_tags;   /* (tags & no_tags)  == 0                                                           */
+} wax_vs_where;
+/* Set frames' attributes (upsert, as wax_vs_set_groups): frame_ids[i] -> timestamps[i], tags[i]; unknown frame ids are
+   ignored, a later entry for the same frame wins; timestamps or tags may be NULL to leave that column unchanged.
+   *out_assigned (optional) = distinct known frames named.  A mutator (write lock). */
+int32_t wax_vs_set_attributes(wax_vs_engine *engine, const uint64_t *frame_ids, const int64_t *timestamps,
+                              const uint64_t *tags, uint64_t n, uint64_t *out_assigned);
+/* wax_vs_search_batch_multi_filtered plus a predicate per query: query i searches the rows that pass
+   wheres[query_where[i]] AND its id filter query_filter[i] (either may be WAX_VS_NO_FILTER).  A predicate that admits
+   nothing (after >= before, all_tags overlapping no_tags) is valid and yields empty answers.  Query i's answer is
+   identical to wax_vs_search_batch_multi_filtered with an allow-list of exactly the frames passing both: same ids, same
+   order, same score bits.  The argument checks of multi_filtered run before the empty-engine early return, and a
+   query_where entry >= n_wheres other than WAX_VS_NO_FILTER -> WAX_VS_ERR_ARGUMENT; NULL wheres (n_wheres > 0) or
+   query_where (n_queries > 0) -> WAX_VS_ERR_NULL.  A single query is the batch of one.
+   How: the unit that gets a row filter is each distinct (where, id filter) pair.  An allow-list is tested against the
+   attributes on the host (O(listed)); otherwise one device pass counts the rows passing every predicate of the call,
+   windows of <= 16 384 rows (nothing of the deny-list among them) are listed by the device and scored as a gather, and
+   wider ones get a row bitset (the deny-list's, the predicate ANDed in on the device) for the tensor-core levels or the
+   masked scan, exactly as an id filter's. */
+int32_t wax_vs_search_batch_where(wax_vs_engine *engine, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                  int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                  const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                  const wax_vs_where *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                  uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n);
+/* wax_vs_search_batch_grouped with ONE predicate for the batch, ANDed with its id filter; NULL where ->
+   WAX_VS_ERR_NULL, otherwise the checks of wax_vs_search_batch_grouped.  Each answer is identical to
+   wax_vs_search_grouped under the allow-list of the passing frames: same frame ids, group ids, order and score bits.
+   n_queries == 1 runs the single-query grouped pipeline. */
+int32_t wax_vs_search_batch_grouped_where(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                          uint32_t query_len, int64_t top_groups, uint32_t per_group,
+                                          const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                                          const wax_vs_where *where, uint64_t *out_ids, float *out_scores,
+                                          uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n);
+
 /* Device-resident form used by the row-sharded engine: `d_queries` (n_queries x dims) and
    `d_candidates` (n_queries x k_eff entries, k_eff = min(clamp(top_k), 10000) -- NOT clipped to N, padding
    has valid = 0) are DEVICE pointers on the engine's device; the work is enqueued on `cuda_stream`
@@ -366,7 +417,7 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *engine, uint64_t *tensor_queries
    "shadow_bytes" (HBM held by the bf16 shadow), "shadow_unavailable" (1 = the shadow did not fit in HBM, batches
    nominate in TF32 at about half the rate), "batch_tf32_queries", "filter_bitset_passes" (sub-batches of per-query
    filtered queries on the tensor-core class, wax_vs_search_batch_multi_filtered), "group_index_builds" (device group
-   index builds of wax_vs_search_grouped), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
+   index builds of wax_vs_search_grouped), "attribute_uploads" (device attribute copies of the where searches), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
    (single queries the bf16-shadow route answered / that the fp32 scan answered after a failed proof; read them while
    no search is running). */
 int32_t wax_vs_debug_counter(wax_vs_engine *engine, const char *name, uint64_t *out);

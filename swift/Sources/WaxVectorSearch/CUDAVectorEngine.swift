@@ -210,6 +210,88 @@ public actor CUDAVectorEngine {
         }
     }
 
+    /// Frame attributes (wax_vs_set_attributes): a timestamp and a tag mask per frame, evaluated by `searchBatchWhere`
+    /// below the top-k in place of `UnifiedSearch.passesFrameFilter`'s time and flag clauses (INTEGRATION.md maps
+    /// `FrameMeta` onto them).  `nil` leaves that column unchanged; not part of MV2V: re-apply after `deserialize`.
+    @discardableResult
+    public func setAttributes(frameIds: [UInt64], timestamps: [Int64]?, tags: [UInt64]?) async throws -> Int {
+        guard timestamps.map({ $0.count == frameIds.count }) ?? true, tags.map({ $0.count == frameIds.count }) ?? true else {
+            throw WaxError.encodingError(reason: "setAttributes: column length != frameIds.count")
+        }
+        guard !frameIds.isEmpty else { return 0 }
+        let handle = self.handle
+        let assigned: UInt64 = try await io.run {
+            var n: UInt64 = 0
+            let rc = wax_vs_set_attributes(handle, frameIds, timestamps, tags, UInt64(frameIds.count), &n)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return n
+        }
+        return Int(assigned)
+    }
+
+    /// A batch whose query i searches the frames passing `wheres[queryWhere[i]]` (nil: every frame), exact
+    /// (wax_vs_search_batch_where).
+    public func searchBatchWhere(vectors: [[Float]], topK: Int, wheres: [wax_vs_where],
+                                 queryWhere: [Int?]) async throws -> [[(frameId: UInt64, score: Float)]] {
+        guard !vectors.isEmpty else { return [] }
+        let dims = dimensions
+        for v in vectors where v.count != dims {
+            throw WaxError.encodingError(reason: "vector dimension mismatch: expected \(dims), got \(v.count)")
+        }
+        let handle = self.handle
+        let cap = min(max(topK, 1), Self.maxResults)
+        return try await io.run {
+            var flat = [Float](); flat.reserveCapacity(vectors.count * dims)
+            for v in vectors { flat.append(contentsOf: v) }
+            let offsets: [UInt64] = [0]
+            let queryFilter = [UInt32](repeating: WAX_VS_NO_FILTER, count: vectors.count)
+            let qw = queryWhere.map { $0.map(UInt32.init) ?? WAX_VS_NO_FILTER }
+            var ids = [UInt64](repeating: 0, count: vectors.count * cap)
+            var scores = [Float](repeating: 0, count: vectors.count * cap)
+            var counts = [UInt32](repeating: 0, count: vectors.count)
+            let rc = wax_vs_search_batch_where(handle, flat, UInt32(vectors.count), UInt32(dims), Int64(topK), nil, offsets,
+                                               nil, 0, queryFilter, wheres, UInt32(wheres.count), qw, &ids, &scores,
+                                               UInt32(cap), &counts)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return (0..<vectors.count).map { q in (0..<Int(counts[q])).map { (ids[q * cap + $0], scores[q * cap + $0]) } }
+        }
+    }
+
+    /// `searchBatchGrouped` over the frames passing `where` and the optional filter (wax_vs_search_batch_grouped_where):
+    /// PhotoRAG / VideoRAG's `timeRange` and superseded / deleted skips below the top-k.
+    public func searchBatchGroupedWhere(vectors: [[Float]], topGroups: Int, perGroup: Int = 1, where predicate: wax_vs_where,
+                                        frameIds: [UInt64] = [], allow: Bool = false) async throws
+        -> [[(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])]] {
+        guard !vectors.isEmpty else { return [] }
+        let dims = dimensions
+        for v in vectors where v.count != dims {
+            throw WaxError.encodingError(reason: "vector dimension mismatch: expected \(dims), got \(v.count)")
+        }
+        let handle = self.handle
+        let cap = max(1, min(min(max(topGroups, 1), Self.maxResults) * max(perGroup, 1), Self.maxResults))
+        return try await io.run {
+            var flat = [Float](); flat.reserveCapacity(vectors.count * dims)
+            for v in vectors { flat.append(contentsOf: v) }
+            var w = predicate
+            var ids = [UInt64](repeating: 0, count: vectors.count * cap)
+            var scores = [Float](repeating: 0, count: vectors.count * cap)
+            var groups = [UInt64](repeating: 0, count: vectors.count * cap)
+            var counts = [UInt32](repeating: 0, count: vectors.count)
+            let rc = wax_vs_search_batch_grouped_where(handle, flat, UInt32(vectors.count), UInt32(dims), Int64(topGroups),
+                                                       UInt32(max(perGroup, 0)), frameIds, UInt64(frameIds.count),
+                                                       allow ? 0 : 1, &w, &ids, &scores, &groups, UInt32(cap), &counts)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return (0..<vectors.count).map { q in
+                var out: [(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])] = []
+                for i in (q * cap)..<(q * cap + Int(counts[q])) {
+                    if out.last?.groupId != groups[i] { out.append((groups[i], [])) }
+                    out[out.count - 1].hits.append((ids[i], scores[i]))
+                }
+                return out
+            }
+        }
+    }
+
     public func add(frameId: UInt64, vector: [Float]) async throws {
         try await addBatch(frameIds: [frameId], vectors: [vector])
     }

@@ -21,11 +21,17 @@ NO_FILTER = 0xFFFFFFFF          # WAX_VS_NO_FILTER: a query of wax_vs_search_bat
 MAX_DIMENSIONS = 1_000_000
 MAX_PER_GROUP = 128             # WAX_VS_MAX_PER_GROUP: rows per group of wax_vs_search_grouped
 SHARD_HANDLE_BYTES, SHARD_MAX_RANKS, SHARD_MAX_K = 128, 16, 128
+INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1   # wax_vs_where bounds meaning "no bound"
 
 
 class Candidate(C.Structure):
     """wax_vs_candidate (24 bytes)."""
     _fields_ = [("distance", C.c_float), ("valid", C.c_uint32), ("row", C.c_uint64), ("frame_id", C.c_uint64)]
+
+
+class Where(C.Structure):
+    """wax_vs_where (32 bytes)."""
+    _fields_ = [("after", C.c_int64), ("before", C.c_int64), ("all_tags", C.c_uint64), ("no_tags", C.c_uint64)]
 
 
 # Every symbol include/wax_vs_cuda.h declares, with its signature.  tests/test_abi.py checks this table
@@ -59,6 +65,13 @@ SIGNATURES = {
                                           _u64p, _f32p, _u64p, C.c_uint32, _u32p]),
     "wax_vs_search_batch_grouped": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, C.c_uint32, _u64p,
                                                 C.c_uint64, C.c_int32, _u64p, _f32p, _u64p, C.c_uint32, _u32p]),
+    "wax_vs_set_attributes": (C.c_int32, [_eng, _u64p, C.POINTER(C.c_int64), _u64p, C.c_uint64, _u64p]),
+    "wax_vs_search_batch_where": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _u64p,
+                                              C.POINTER(C.c_int32), C.c_uint32, _u32p, C.c_void_p, C.c_uint32, _u32p,
+                                              _u64p, _f32p, C.c_uint32, _u32p]),
+    "wax_vs_search_batch_grouped_where": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, C.c_uint32, _u64p,
+                                                      C.c_uint64, C.c_int32, C.c_void_p, _u64p, _f32p, _u64p, C.c_uint32,
+                                                      _u32p]),
     "wax_vs_search_batch": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _f32p,
                                         C.c_uint32, _u32p]),
     "wax_vs_search_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, C.c_uint64, C.c_void_p,

@@ -38,6 +38,7 @@
 
 #include "waxvs_group.cuh"
 #include "waxvs_group_batch.cuh"
+#include "waxvs_where.cuh"
 
 #include <cub/cub.cuh>
 #include <cudaTypedefs.h>
@@ -247,6 +248,8 @@ struct SearchCtx {
     DevBuf<ScoreItem> d_score_items;               // batched grouped search: expansion tiles (level 0)
     PinnedBuf<unsigned long long> h_flag;          // host-delivery completion flag
     unsigned long long host_seq = 0;               // last value the flag was asked to take
+    DevBuf<WhereItem> d_where_items;               // where search: predicates of the count / compaction / bitset launches
+    DevBuf<uint32_t> d_where_counts;               // where search: rows passing each predicate, then compaction cursors
     DevBuf<uint32_t> d_proof_count;                // shadow route: [0] proofs that held, [1] that failed (guarded scan) ...
     PinnedBuf<uint32_t> h_proof_count;             // ... and their mapped host mirror
     uint32_t seen_failed = 0;                      // h_proof_count[1] when the host last looked
@@ -316,6 +319,16 @@ struct wax_vs_engine {
     } gindex;
     std::mutex group_mu;
     uint64_t group_index_builds = 0;   // instrumentation (pool_mu)
+    // Frame attributes (wax_vs_set_attributes): attrs[r] = row r's (timestamp, tags), kept aligned with `ids` by every
+    // mutator exactly as `groups` is.  Empty while attrs_set is false: then every row has timestamp 0 and tags 0.
+    bool attrs_set = false;
+    std::vector<AttrRow> attrs;
+    // Device mirror (16 bytes per row) for the where predicates, a cache like the group index: every mutator and
+    // set_attributes invalidate it; the first search that needs it rebuilds it under attrs_mu and publishes it complete.
+    DevBuf<AttrRow> d_attrs;
+    bool attrs_dev_valid = false;
+    std::mutex attrs_mu;
+    uint64_t attribute_uploads = 0;    // instrumentation (pool_mu)
     uint64_t grouped_batch_covered_queries = 0, grouped_batch_expanded_groups = 0, grouped_batch_fallback_queries = 0;
     // Adaptive level choice: when more than a quarter of a batch fails the coarse bf16 bound (tightly clustered
     // neighbours), the next 16 batches nominate in TF32 straight away, then bf16 is probed again.
@@ -385,6 +398,7 @@ static void invalidate_row_caches(wax_vs_engine *e, uint64_t keep_prefix) {
     e->shadow_rows = std::min(e->shadow_rows, keep_prefix);
     if (e->shadow_rows == 0) e->shadow_valid = false;
     e->gindex.valid = false;           // appends too: the new rows need index entries
+    e->attrs_dev_valid = false;        // likewise the attribute mirror
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1717,6 +1731,7 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
         // the common bulk-ingest case: every id is new and larger than all stored ones -- no lookups, no hash table
         e->ids.insert(e->ids.end(), frame_ids, frame_ids + n);
         if (e->groups_set) e->groups.insert(e->groups.end(), frame_ids, frame_ids + n);   // a new frame is its own group
+        if (e->attrs_set) e->attrs.resize(e->attrs.size() + n, AttrRow{0, 0});               // ... and has no attributes
         for (uint64_t i = 0; i < n; ++i) target[i] = static_cast<uint32_t>(n0 + i);
         e->n_rows += n;
         e->map_valid = false;
@@ -1733,6 +1748,7 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
                 }
                 e->ids.push_back(frame_ids[i]);
                 if (e->groups_set) e->groups.push_back(frame_ids[i]);    // an upsert of a known frame keeps its group
+                if (e->attrs_set) e->attrs.push_back(AttrRow{0, 0});     // ... and its attributes
                 if (!e->ids_sorted) e->map.put(frame_ids[i], row);
                 else e->map_valid = false;
                 ++e->n_rows;
@@ -1850,9 +1866,11 @@ int32_t wax_vs_remove_batch(wax_vs_engine *e, const uint64_t *frame_ids, uint64_
     for (uint64_t j = 0; j < moving; ++j) {
         e->ids[first + j] = e->ids[src[j]];
         if (e->groups_set) e->groups[first + j] = e->groups[src[j]];
+        if (e->attrs_set) e->attrs[first + j] = e->attrs[src[j]];
     }
     e->ids.resize(new_n);
     if (e->groups_set) e->groups.resize(new_n);
+    if (e->attrs_set) e->attrs.resize(new_n);
     e->n_rows = new_n;
     e->map_valid = false;
     e->d_ids_dirty = true;
@@ -2220,6 +2238,14 @@ struct FilterSet {
     std::vector<uint32_t> rows;
     std::vector<uint64_t> first, count;
     std::vector<uint8_t> referenced;            // filters some query names (the others are not resolved)
+    // Where search only (empty otherwise): filter f's bitset is ANDed with preds[where[f]] unless that is WAX_VS_NO_FILTER,
+    // and then allows allowed[f] rows; the rows of the filters in `compact` (device_rows in all) are listed by the device
+    // after `rows`, each item's slot being where its rows start.
+    std::vector<uint32_t> where;
+    std::vector<uint64_t> allowed;
+    std::vector<WherePred> preds;
+    std::vector<WhereItem> compact;
+    uint64_t device_rows = 0;
 };
 // query_filter = nullptr: every filter is resolved (the single-filter entry points).
 static void resolve_filters(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *filter_offsets, uint32_t n_filters,
@@ -2558,6 +2584,88 @@ int32_t wax_vs_merge_candidates_device(wax_vs_engine *e, const wax_vs_candidate 
     return WAX_VS_OK;
 }
 
+// ---- frame attributes on the device (waxvs_where.cuh) --------------------------------------------------------------
+// The attribute mirror of the current corpus, built on c's stream by the first search after a mutation or
+// set_attributes that needs it.  Readers hold the read lock; attrs_mu serialises the build, which completes before the
+// mirror is published.
+static int32_t ensure_attributes(wax_vs_engine *e, SearchCtx *c) {
+    std::lock_guard<std::mutex> lk(e->attrs_mu);
+    if (e->attrs_dev_valid) return WAX_VS_OK;
+    const size_t n = static_cast<size_t>(e->n_rows);
+    int32_t rc;
+    if ((rc = e->d_attrs.ensure(std::max<size_t>(n, 1), "row attributes"))) return rc;
+    if (e->attrs_set) CUDA_TRY(cudaMemcpyAsync(e->d_attrs, e->attrs.data(), n * sizeof(AttrRow), cudaMemcpyHostToDevice, c->stream));
+    else CUDA_TRY(cudaMemsetAsync(e->d_attrs, 0, n * sizeof(AttrRow), c->stream));    // never set: timestamp 0, tags 0
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    e->attrs_dev_valid = true;
+    std::lock_guard<std::mutex> pg(e->pool_mu);
+    ++e->attribute_uploads;
+    return WAX_VS_OK;
+}
+
+static int where_grid(const wax_vs_engine *e, uint64_t threads) {
+    return static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 8,
+                                                                     (threads + kWhereThreads - 1) / kWhereThreads)));
+}
+
+// counts[i] = the rows passing preds[i]: one streaming pass per kWhereChunk predicates, read back once.
+static int32_t where_counts(wax_vs_engine *e, SearchCtx *c, const std::vector<WherePred> &preds, std::vector<uint32_t> &counts) {
+    const uint32_t m = static_cast<uint32_t>(preds.size()), n = static_cast<uint32_t>(e->n_rows);
+    counts.assign(m, 0u);
+    if (!m) return WAX_VS_OK;
+    int32_t rc;
+    if ((rc = ensure_attributes(e, c))) return rc;
+    if ((rc = c->d_where_items.ensure(m, "where predicates")) || (rc = c->d_where_counts.ensure(m, "where counts"))) return rc;
+    std::vector<WhereItem> items(m);
+    for (uint32_t i = 0; i < m; ++i) items[i] = WhereItem{preds[i], 0};
+    CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaMemsetAsync(c->d_where_counts, 0, m * sizeof(uint32_t), c->stream));
+    for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk)
+        where_count_kernel<<<where_grid(e, n), kWhereThreads, 0, c->stream>>>(e->d_attrs, n, c->d_where_items + i0,
+                                                                             std::min(kWhereChunk, m - i0), c->d_where_counts + i0);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(counts.data(), c->d_where_counts, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    return WAX_VS_OK;
+}
+
+// ANDs items[i].pred into bitset items[i].slot of c->d_mask on `stream` (after the filter builders wrote it).
+static int32_t apply_where_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereItem> &items, cudaStream_t stream,
+                                uint64_t *launches) {
+    const uint32_t m = static_cast<uint32_t>(items.size()), n = static_cast<uint32_t>(e->n_rows);
+    if (!m) return WAX_VS_OK;
+    const uint32_t words = (n + 31u) / 32u;
+    int32_t rc;
+    if ((rc = c->d_where_items.ensure(m, "where predicates"))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, stream));
+    for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
+        where_bits_kernel<<<where_grid(e, static_cast<uint64_t>(words) * 32u), kWhereThreads, 0, stream>>>(
+            e->d_attrs, n, words, c->d_mask, c->d_where_items + i0, std::min(kWhereChunk, m - i0));
+        ++*launches;
+    }
+    CUDA_TRY(cudaGetLastError());
+    return WAX_VS_OK;
+}
+
+// The rows of the narrow predicates (fs.compact) into c->d_filter_rows at their slots, on `stream`.
+static int32_t list_where_rows(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereItem> &items, cudaStream_t stream,
+                               uint64_t *launches) {
+    const uint32_t m = static_cast<uint32_t>(items.size()), n = static_cast<uint32_t>(e->n_rows);
+    if (!m) return WAX_VS_OK;
+    int32_t rc;
+    if ((rc = c->d_where_items.ensure(m, "where predicates")) || (rc = c->d_where_counts.ensure(m, "where cursors"))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaMemsetAsync(c->d_where_counts, 0, m * sizeof(uint32_t), stream));
+    for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
+        where_compact_kernel<<<where_grid(e, n), kWhereThreads, 0, stream>>>(e->d_attrs, n, c->d_where_items + i0,
+                                                                            std::min(kWhereChunk, m - i0),
+                                                                            c->d_where_counts + i0, c->d_filter_rows);
+        ++*launches;
+    }
+    CUDA_TRY(cudaGetLastError());
+    return WAX_VS_OK;
+}
+
 // ---- batched filtered search ------------------------------------------------------------------------------------
 // n_queries queries, query i under filter query_filter[i] (WAX_VS_NO_FILTER: unfiltered); the single-filter entry
 // points are the case of one filter that every query names.  Every query referenced filter is resolved once; query i
@@ -2587,7 +2695,8 @@ static void plan_filtered(const wax_vs_engine *e, int64_t top_k, const int32_t *
     uint32_t k_max = 0;
     for (uint32_t i = 0; i < n_queries; ++i) {
         const uint32_t f = query_filter[i];
-        const uint64_t allowed = f == WAX_VS_NO_FILTER ? n_rows : (filter_modes[f] == 0 ? fs.count[f] : n_rows - fs.count[f]);
+        uint64_t allowed = f == WAX_VS_NO_FILTER ? n_rows : (filter_modes[f] == 0 ? fs.count[f] : n_rows - fs.count[f]);
+        if (f != WAX_VS_NO_FILTER && !fs.where.empty() && fs.where[f] != WAX_VS_NO_FILTER) allowed = fs.allowed[f];
         const uint32_t k = static_cast<uint32_t>(std::min<uint64_t>(limit, allowed));
         if (k == 0) continue;
         k_of_query[i] = k;
@@ -2623,8 +2732,9 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
     if ((rc = stage_queries(e, c, queries, n_staged, c->stream, order.data()))) return rc;
     if ((rc = c->d_out.ensure(ncand, "result buffer"))) return rc;
     if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
-    if ((rc = stage_filter_rows(e, c, rows, rows.size(), -1, c->stream, nullptr))) return rc;
+    if ((rc = stage_filter_rows(e, c, rows, rows.size() + fs.device_rows, -1, c->stream, nullptr))) return rc;
     uint64_t launches = 0;
+    if ((rc = list_where_rows(e, c, fs.compact, c->stream, &launches))) { cudaStreamSynchronize(c->stream); return rc; }
 
     // gather class: one concatenated row list, a span per query; the sort grants shared memory for the longest list
     if (n_gather) {
@@ -2695,6 +2805,10 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
                     spec[2u * nf + 1u + l] = static_cast<uint64_t>(filter_modes[which[l]]);
                 }
                 if ((prc = build_filter_bits(e, c, spec, nf, c->stream, &launches))) { cudaStreamSynchronize(c->stream); return prc; }
+                std::vector<WhereItem> wbits;                           // where search: the predicates ANDed in
+                for (uint32_t l = 0; l < nf && !fs.where.empty(); ++l)
+                    if (fs.where[which[l]] != WAX_VS_NO_FILTER) wbits.push_back(WhereItem{fs.preds[fs.where[which[l]]], l});
+                if ((prc = apply_where_bits(e, c, wbits, c->stream, &launches))) { cudaStreamSynchronize(c->stream); return prc; }
             }
             RowFilter rf{c->d_mask.p, words, nullptr, index.data() + s0};
             const uint32_t nq = s1 - s0;
@@ -2727,10 +2841,10 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
     return WAX_VS_OK;
 }
 
-static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                    int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                    const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                    uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+// The argument checks of the per-query filtered entry points, run before the empty-engine early return.
+static int32_t check_filter_args(const wax_vs_engine *e, uint32_t n_queries, const uint64_t *frame_ids,
+                                 const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                 const uint32_t *query_filter, const uint32_t *out_n) {
     if (!e || !out_n || !filter_offsets || (n_filters && !filter_modes) || (n_queries && !query_filter))
         return fail(WAX_VS_ERR_NULL, "NULL argument");
     for (uint32_t f = 0; f < n_filters; ++f)
@@ -2744,16 +2858,40 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
     for (uint32_t i = 0; i < n_queries; ++i)
         if (query_filter[i] != WAX_VS_NO_FILTER && query_filter[i] >= n_filters)
             return fail(WAX_VS_ERR_ARGUMENT, "query %u names filter %u of %u", i, query_filter[i], n_filters);
+    return WAX_VS_OK;
+}
+
+// The planned queries run on c, their answers delivered to the caller's buffers (plan.k_max > 0).
+static int32_t deliver_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries, const int32_t *filter_modes,
+                                uint32_t n_filters, const uint32_t *query_filter, const FilterSet &fs,
+                                const FilteredPlan &plan, uint64_t *out_ids, float *out_scores, uint32_t out_stride,
+                                uint32_t *out_n) {
+    int32_t rc;
+    if ((rc = run_filtered(e, c, queries, filter_modes, n_filters, query_filter, fs, plan))) return rc;
+    const size_t ncand = static_cast<size_t>(plan.order.size()) * plan.k_max;
+    CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, ncand * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));   // also keeps the host arrays alive until their copies are done
+    deliver_results(e, c->h_out, static_cast<uint32_t>(plan.order.size()), plan.k_max, out_ids, out_scores, out_stride,
+                    out_n, plan.order.data(), plan.k_of.data());
+    return WAX_VS_OK;
+}
+
+static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                    int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                    const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                    uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    int32_t rc;
+    if ((rc = check_filter_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, out_n)))
+        return rc;
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
     if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
-    int32_t rc;
     if ((rc = check_query(e, queries, query_len))) return rc;
     FilterSet fs;
     resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, fs);
     FilteredPlan plan;
     plan_filtered(e, top_k, filter_modes, query_filter, n_queries, fs, plan);
-    const uint32_t k_max = plan.k_max, n_staged = static_cast<uint32_t>(plan.order.size());
+    const uint32_t k_max = plan.k_max;
     if (k_max == 0) return WAX_VS_OK;
     if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
     if (out_stride < k_max) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, k_max);
@@ -2762,13 +2900,8 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
     if (!g.ok) return g.error();
     CtxLease lease(e);
     if ((rc = lease.acquire())) return rc;
-    SearchCtx *c = lease.c;
-    if ((rc = run_filtered(e, c, queries, filter_modes, n_filters, query_filter, fs, plan))) return rc;
-    const size_t ncand = static_cast<size_t>(n_staged) * k_max;
-    CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, ncand * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(cudaStreamSynchronize(c->stream));   // also keeps the host arrays alive until their copies are done
-    deliver_results(e, c->h_out, n_staged, k_max, out_ids, out_scores, out_stride, out_n, plan.order.data(), plan.k_of.data());
-    return WAX_VS_OK;
+    return deliver_filtered(e, lease.c, queries, filter_modes, n_filters, query_filter, fs, plan, out_ids, out_scores,
+                            out_stride, out_n);
 }
 
 int32_t wax_vs_search_filtered(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k,
@@ -2795,6 +2928,140 @@ int32_t wax_vs_search_batch_multi_filtered(wax_vs_engine *e, const float *querie
                                            uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
     return search_filtered_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
                                 query_filter, out_ids, out_scores, out_stride, out_n);
+}
+
+// ---- where search: attribute predicates below the top-k (waxvs_where.cuh) -------------------------------------------
+// Query i searches the rows that pass wheres[query_where[i]] AND its id filter.  The unit that gets a row filter is the
+// distinct (where, id filter) pair some query names; a pair without a where is the id filter itself.  A pair with one
+// becomes an ordinary filter of the plan above:
+//  - allow-list AND where: the listed rows are tested against the host attribute arrays (O(listed)) -> an allow-list;
+//  - deny-list AND where, or the where alone: allowed = (rows passing, from one device count pass for all the call's
+//    predicates) - (listed rows passing).  When nothing listed passes and at most kWhereGatherRows rows do, the device
+//    lists them (the gather class); otherwise the filter's bitset is the deny-list's (mode 1, listing only the rows that
+//    pass) with the predicate ANDed in on the device, for the tensor and scan classes.
+constexpr uint64_t kWhereGatherRows = 16384;   // the gather class's largest allow-list (plan_filtered)
+
+static WherePred where_pred(const wax_vs_where &w) { return WherePred{w.after, w.before, w.all_tags, w.no_tags}; }
+
+// The listed rows that pass `w`, appended to `out`.
+static void host_rows_passing(const wax_vs_engine *e, const WherePred &w, const uint32_t *rows, uint64_t n,
+                              std::vector<uint32_t> &out) {
+    for (uint64_t i = 0; i < n; ++i) {
+        const AttrRow a = e->attrs_set ? e->attrs[rows[i]] : AttrRow{0, 0};
+        if (where_passes(w, a.ts, a.tags)) out.push_back(rows[i]);
+    }
+}
+
+// The pairs of a call as the filters of `fs` (modes[p], pair_of[i] = query i's pair or WAX_VS_NO_FILTER), from the
+// resolved id filters `ids`.  Runs the count pass on c's stream.
+static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_where *wheres, uint32_t n_wheres,
+                                const uint32_t *query_where, const int32_t *filter_modes, const uint32_t *query_filter,
+                                uint32_t n_queries, const FilterSet &ids, FilterSet &fs, std::vector<int32_t> &modes,
+                                std::vector<uint32_t> &pair_of) {
+    pair_of.assign(n_queries, WAX_VS_NO_FILTER);
+    std::unordered_map<uint64_t, uint32_t> index;
+    std::vector<std::pair<uint32_t, uint32_t>> pairs;              // (where, id filter)
+    for (uint32_t i = 0; i < n_queries; ++i) {
+        const uint32_t w = query_where[i], f = query_filter[i];
+        if (w == WAX_VS_NO_FILTER && f == WAX_VS_NO_FILTER) continue;
+        const auto ins = index.emplace((static_cast<uint64_t>(w) << 32) | f, static_cast<uint32_t>(pairs.size()));
+        if (ins.second) pairs.emplace_back(w, f);
+        pair_of[i] = ins.first->second;
+    }
+    // the predicates whose count the plan needs: those of pairs without an allow-list
+    std::vector<uint32_t> slot(n_wheres, WAX_VS_NO_FILTER);
+    std::vector<WherePred> counted;
+    for (const auto &pr : pairs)
+        if (pr.first != WAX_VS_NO_FILTER && (pr.second == WAX_VS_NO_FILTER || filter_modes[pr.second] == 1) &&
+            slot[pr.first] == WAX_VS_NO_FILTER) {
+            slot[pr.first] = static_cast<uint32_t>(counted.size());
+            counted.push_back(where_pred(wheres[pr.first]));
+        }
+    std::vector<uint32_t> passing;
+    int32_t rc;
+    if ((rc = where_counts(e, c, counted, passing))) return rc;
+    const uint32_t np = static_cast<uint32_t>(pairs.size());
+    fs.first.assign(np, 0);
+    fs.count.assign(np, 0);
+    fs.referenced.assign(np, 1);
+    fs.where.assign(np, WAX_VS_NO_FILTER);
+    fs.allowed.assign(np, 0);
+    modes.assign(np, 0);
+    std::vector<uint32_t> listed_by_device;
+    for (uint32_t p = 0; p < np; ++p) {
+        const uint32_t w = pairs[p].first, f = pairs[p].second;
+        const uint32_t *rows = f == WAX_VS_NO_FILTER ? nullptr : ids.rows.data() + ids.first[f];
+        const uint64_t n_listed = f == WAX_VS_NO_FILTER ? 0 : ids.count[f];
+        fs.first[p] = fs.rows.size();
+        if (w == WAX_VS_NO_FILTER) {                               // the id filter as it is
+            fs.rows.insert(fs.rows.end(), rows, rows + n_listed);
+            fs.count[p] = n_listed;
+            modes[p] = filter_modes[f];
+            continue;
+        }
+        const WherePred pred = where_pred(wheres[w]);
+        host_rows_passing(e, pred, rows, n_listed, fs.rows);
+        fs.count[p] = fs.rows.size() - fs.first[p];
+        if (f != WAX_VS_NO_FILTER && filter_modes[f] == 0) continue;          // allow-list AND where: an allow-list
+        const uint64_t pass = passing[slot[w]];
+        if (fs.count[p] == 0 && pass > 0 && pass <= kWhereGatherRows) {       // narrow: the device lists the rows
+            fs.count[p] = pass;
+            fs.compact.push_back(WhereItem{pred, 0});
+            listed_by_device.push_back(p);
+            continue;
+        }
+        modes[p] = 1;                                                         // deny the listed rows that pass ...
+        fs.where[p] = static_cast<uint32_t>(fs.preds.size());                 // ... within the rows that pass
+        fs.preds.push_back(pred);
+        fs.allowed[p] = pass - fs.count[p];
+    }
+    uint64_t at = fs.rows.size();                                             // device-listed rows follow the host's
+    for (size_t j = 0; j < listed_by_device.size(); ++j) {
+        const uint32_t p = listed_by_device[j];
+        fs.first[p] = at;
+        fs.compact[j].slot = at;
+        at += fs.count[p];
+    }
+    fs.device_rows = at - fs.rows.size();
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_search_batch_where(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                  int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                  const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                  const wax_vs_where *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                  uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    int32_t rc;
+    if ((rc = check_filter_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, out_n)))
+        return rc;
+    if ((n_wheres && !wheres) || (n_queries && !query_where)) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    for (uint32_t i = 0; i < n_queries; ++i)
+        if (query_where[i] != WAX_VS_NO_FILTER && query_where[i] >= n_wheres)
+            return fail(WAX_VS_ERR_ARGUMENT, "query %u names where %u of %u", i, query_where[i], n_wheres);
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
+    if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
+    if ((rc = check_query(e, queries, query_len))) return rc;
+    FilterSet ids;
+    resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, ids);
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    CtxLease lease(e);
+    if ((rc = lease.acquire())) return rc;
+    FilterSet fs;
+    std::vector<int32_t> modes;
+    std::vector<uint32_t> pair_of;
+    if ((rc = plan_where_pairs(e, lease.c, wheres, n_wheres, query_where, filter_modes, query_filter, n_queries, ids, fs,
+                               modes, pair_of)))
+        return rc;
+    FilteredPlan plan;
+    plan_filtered(e, top_k, modes.data(), pair_of.data(), n_queries, fs, plan);
+    if (plan.k_max == 0) return WAX_VS_OK;
+    if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
+    if (out_stride < plan.k_max)
+        return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, plan.k_max);
+    return deliver_filtered(e, lease.c, queries, modes.data(), static_cast<uint32_t>(modes.size()), pair_of.data(), fs, plan,
+                            out_ids, out_scores, out_stride, out_n);
 }
 
 // The row-sharded form: every rank passes the SAME ids; a rank resolves the ones its shard holds (the others are
@@ -2838,6 +3105,36 @@ int32_t wax_vs_set_groups(wax_vs_engine *e, const uint64_t *frame_ids, const uin
         if (!(written[wd] & b)) { written[wd] |= b; ++assigned; }
     }
     e->gindex.valid = false;
+    if (out_assigned) *out_assigned = assigned;
+    return WAX_VS_OK;
+}
+
+// Frame attributes (waxvs_where.cuh): the timestamp and tag columns the where predicates test.  Upsert by frame id as
+// set_groups: unknown ids are ignored, a later entry for the same frame wins, a NULL column is left as it is.
+int32_t wax_vs_set_attributes(wax_vs_engine *e, const uint64_t *frame_ids, const int64_t *timestamps, const uint64_t *tags,
+                              uint64_t n, uint64_t *out_assigned) {
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    if (out_assigned) *out_assigned = 0;
+    if (n == 0) return WAX_VS_OK;
+    if (!frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    std::unique_lock<std::shared_mutex> w(e->rw);
+    DeviceGuard g(e->device);
+    drain_device_path(e);
+    if (!e->attrs_set) {               // from implicit (every row 0, 0) to explicit arrays
+        e->attrs.assign(e->n_rows, AttrRow{0, 0});
+        e->attrs_set = true;
+    }
+    std::vector<uint32_t> written(static_cast<size_t>((e->n_rows + 31) / 32), 0u);
+    uint64_t assigned = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        const uint32_t row = row_of(e, frame_ids[i]);
+        if (row == 0xFFFFFFFFu) continue;                // unknown frame: ignored
+        if (timestamps) e->attrs[row].ts = timestamps[i];
+        if (tags) e->attrs[row].tags = tags[i];
+        const uint32_t wd = row >> 5, b = 1u << (row & 31u);
+        if (!(written[wd] & b)) { written[wd] |= b; ++assigned; }
+    }
+    e->attrs_dev_valid = false;
     if (out_assigned) *out_assigned = assigned;
     return WAX_VS_OK;
 }
@@ -2994,8 +3291,8 @@ static uint32_t deliver_group_keys(const wax_vs_engine *e, const uint64_t *keys,
 // wait behind a queued writer): the host query, the filter's resolved rows (nullptr: unfiltered; the filter allows some
 // row), the answer at out_* and *out_n.  The arguments are checked by the caller.
 static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, uint32_t n_top, uint32_t per_group,
-                           const std::vector<uint32_t> *rows, int32_t mode, uint64_t *out_ids, float *out_scores,
-                           uint64_t *out_groups, uint32_t *out_n) {
+                           const std::vector<uint32_t> *rows, int32_t mode, const WherePred *where, uint64_t *out_ids,
+                           float *out_scores, uint64_t *out_groups, uint32_t *out_n) {
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const bool filtered = rows != nullptr;
     cudaStream_t s = c->stream;
@@ -3009,7 +3306,8 @@ static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, u
     if ((rc = c->d_out.ensure(n_top, "result buffer"))) return rc;
     if ((rc = c->h_out.ensure(n_top, "result staging"))) return rc;
     if (filtered) {
-        if ((rc = stage_filter_rows(e, c, *rows, rows->size(), mode, s, &launches))) {
+        if ((rc = stage_filter_rows(e, c, *rows, rows->size(), mode, s, &launches)) ||
+            (where && (rc = apply_where_bits(e, c, {WhereItem{*where, 0}}, s, &launches)))) {
             cudaStreamSynchronize(s);
             return rc;
         }
@@ -3161,7 +3459,7 @@ static int32_t enqueue_batch_expansion(wax_vs_engine *e, SearchCtx *c, const Cov
 static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                    int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
                                    int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
-                                   uint32_t out_stride, uint32_t *out_n, bool batched) {
+                                   uint32_t out_stride, uint32_t *out_n, bool batched, const wax_vs_where *where = nullptr) {
     if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (per_group == 0 || per_group > WAX_VS_MAX_PER_GROUP)
         return fail(WAX_VS_ERR_ARGUMENT, "per_group must be in [1, %d] (got %u)", WAX_VS_MAX_PER_GROUP, per_group);
@@ -3179,22 +3477,44 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(n_top) * per_group, n));
     if (out_stride < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, need);
-    const bool filtered = !(mode == 1 && n_ids == 0);
+    const bool filtered = where || !(mode == 1 && n_ids == 0);
     const uint64_t offsets[2] = {0, n_ids};
     FilterSet fs;
     if (filtered) {
         resolve_filters(e, frame_ids, offsets, 1, nullptr, 0, fs);
-        if (mode == 0 && fs.rows.empty()) return WAX_VS_OK;                 // nothing allowed
-        if (mode == 1 && fs.rows.size() == n) return WAX_VS_OK;             // everything denied
+        if (!where && mode == 0 && fs.rows.empty()) return WAX_VS_OK;                 // nothing allowed
+        if (!where && mode == 1 && fs.rows.size() == n) return WAX_VS_OK;             // everything denied
     }
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
     CtxLease lease(e);
     if ((rc = lease.acquire())) return rc;
     SearchCtx *c = lease.c;
+    // where (wax_vs_search_batch_grouped_where): the filter becomes an allow-list of the listed rows that pass, or the
+    // deny-list's rows that pass (mode 1) with the predicate ANDed into every bitset built from it (where_bits)
+    WherePred pred{};
+    bool where_bits = false;
+    if (where) {
+        pred = where_pred(*where);
+        std::vector<uint32_t> kept;
+        host_rows_passing(e, pred, fs.rows.data(), fs.rows.size(), kept);
+        fs.rows.swap(kept);
+        fs.count[0] = fs.rows.size();
+        if (mode == 0 && fs.rows.empty()) return WAX_VS_OK;                           // nothing allowed
+        if (mode == 1) {
+            std::vector<uint32_t> pass;
+            if ((rc = where_counts(e, c, {pred}, pass))) return rc;
+            if (pass[0] == fs.rows.size()) return WAX_VS_OK;                          // nothing passes but denied rows
+            fs.where.assign(1, 0);
+            fs.preds.assign(1, pred);
+            fs.allowed.assign(1, pass[0] - fs.rows.size());
+            where_bits = true;
+        }
+    }
+    const WherePred *row_where = where_bits ? &pred : nullptr;
     if (!batched)
-        return grouped_one(e, c, queries, n_top, per_group, filtered ? &fs.rows : nullptr, mode, out_ids, out_scores,
-                           out_groups, out_n);
+        return grouped_one(e, c, queries, n_top, per_group, filtered ? &fs.rows : nullptr, mode, row_where, out_ids,
+                           out_scores, out_groups, out_n);
     const std::vector<uint32_t> query_filter(n_queries, filtered ? 0u : WAX_VS_NO_FILTER);
     // The coverage level: each query's exact top-k_c rows, when the batch goes to the tensor-core levels or the gather
     // class of the batched filtered search; every other batch runs the single-query pipeline per query.
@@ -3240,7 +3560,11 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
             });
             if (filtered) {                          // the expansion consults the filter's bitset (rows staged by run_filtered)
                 const std::vector<uint64_t> spec = {0, fs.rows.size(), 0, static_cast<uint64_t>(mode)};
-                if ((rc = build_filter_bits(e, c, spec, 1, s, &launches))) { cudaStreamSynchronize(s); return rc; }
+                if ((rc = build_filter_bits(e, c, spec, 1, s, &launches)) ||
+                    (row_where && (rc = apply_where_bits(e, c, {WhereItem{pred, 0}}, s, &launches)))) {
+                    cudaStreamSynchronize(s);
+                    return rc;
+                }
             }
             if ((rc = enqueue_batch_expansion(e, c, list, n_exp, n_top, per_group, filtered ? c->d_mask.p : nullptr, &launches))) {
                 cudaStreamSynchronize(s);
@@ -3264,7 +3588,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     for (uint32_t qi : crowded) {
         const size_t o = static_cast<size_t>(qi) * out_stride;
         if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group, filtered ? &fs.rows : nullptr,
-                              mode, out_ids + o, out_scores + o, out_groups + o, out_n + qi)))
+                              mode, row_where, out_ids + o, out_scores + o, out_groups + o, out_n + qi)))
             return rc;
     }
     std::lock_guard<std::mutex> pg(e->pool_mu);
@@ -3288,6 +3612,15 @@ int32_t wax_vs_search_batch_grouped(wax_vs_engine *e, const float *queries, uint
                                     uint32_t out_stride, uint32_t *out_n) {
     return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
                                out_scores, out_groups, out_stride, out_n, true);
+}
+
+int32_t wax_vs_search_batch_grouped_where(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                          int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
+                                          int32_t mode, const wax_vs_where *where, uint64_t *out_ids, float *out_scores,
+                                          uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n) {
+    if (!where) return fail(WAX_VS_ERR_NULL, "where is NULL");
+    return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
+                               out_scores, out_groups, out_stride, out_n, n_queries > 1, where);
 }
 
 // ---- persistence ---------------------------------------------------------------------------------------------
@@ -3377,6 +3710,8 @@ int32_t wax_vs_deserialize(wax_vs_engine *e, const uint8_t *src, uint64_t len) {
     e->d_ids_dirty = true;
     e->groups_set = false;                  // MV2V has no groups: the caller re-applies them (wax_vs_set_groups)
     e->groups.clear(); e->groups.shrink_to_fit();
+    e->attrs_set = false;                   // nor attributes: the caller re-applies them (wax_vs_set_attributes)
+    e->attrs.clear(); e->attrs.shrink_to_fit();
     invalidate_row_caches(e, 0);
     return WAX_VS_OK;
 }
@@ -3413,6 +3748,8 @@ int32_t wax_vs_debug_fill_synthetic(wax_vs_engine *e, uint64_t seed, uint64_t fi
     e->d_ids_dirty = true;
     e->groups_set = false;
     e->groups.clear(); e->groups.shrink_to_fit();
+    e->attrs_set = false;
+    e->attrs.clear(); e->attrs.shrink_to_fit();
     invalidate_row_caches(e, 0);
     return WAX_VS_OK;
 }
@@ -3608,6 +3945,7 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "batch_tf32_queries")) *out = e->batch_tf32_queries;
     else if (!strcmp(name, "filter_bitset_passes")) *out = e->filter_bitset_passes;   // per-query filters: tensor sub-batches
     else if (!strcmp(name, "group_index_builds")) *out = e->group_index_builds;       // grouped search: device index builds
+    else if (!strcmp(name, "attribute_uploads")) *out = e->attribute_uploads;         // where search: attribute mirror builds
     else if (!strcmp(name, "grouped_batch_covered_queries")) *out = e->grouped_batch_covered_queries;     // answered by the coverage level
     else if (!strcmp(name, "grouped_batch_expanded_groups")) *out = e->grouped_batch_expanded_groups;     // (query, group) expansions
     else if (!strcmp(name, "grouped_batch_fallback_queries")) *out = e->grouped_batch_fallback_queries;   // single-query pipeline

@@ -1,0 +1,138 @@
+// waxvs_where.cuh -- frame attributes on the device: the time-range and tag predicates of wax_vs_search_batch_where and
+// wax_vs_search_batch_grouped_where.
+//
+// Wax post-filters every vector hit on the frame's metadata (UnifiedSearch.passesFrameFilter,
+// Sources/Wax/UnifiedSearch/UnifiedSearch.swift:1241-1258): a timeRange (TimeRange.contains, SearchRequest.swift:90-105:
+// after inclusive, before exclusive) and the status / supersededBy / kind flags.  Here each row carries two columns, a
+// timestamp and a 64-bit tag mask (16 bytes per row, AttrRow), and a predicate (WherePred) is evaluated on the device in
+// one streaming pass; what it produces feeds the row-filter machinery of the filtered search unchanged:
+//   where_count_kernel:   how many rows pass each predicate of a call (sizes the plan: k_i and the query classes);
+//   where_bits_kernel:    ANDs a predicate into a row bitset the filter builders made (filter_bits_*_kernel), a warp per
+//                         32-row word, one ballot per predicate;
+//   where_compact_kernel: lists the rows passing a narrow predicate into the concatenated filter rows (the gather class).
+// All three read each row's 16 bytes once per launch and test every predicate of the launch against it in registers;
+// the predicates of a launch (at most kWhereChunk) sit in shared memory.
+#pragma once
+#include <cstdint>
+
+namespace waxvs {
+
+// Row attributes as the device mirror holds them (16 bytes, one LDG.128 per row).
+struct alignas(16) AttrRow {
+    int64_t ts;
+    uint64_t tags;
+};
+
+// wax_vs_where, field for field.
+struct WherePred {
+    int64_t after, before;
+    uint64_t all_tags, no_tags;
+};
+
+// One predicate of a launch and what it applies to: the bitset index (where_bits_kernel) or the first slot of its rows in
+// the concatenated list (where_compact_kernel); unused by where_count_kernel.
+struct WhereItem {
+    WherePred pred;
+    uint64_t slot;
+};
+
+constexpr uint32_t kWhereChunk = 256;     // predicates per launch (shared memory: 10 KiB of items, 8 KiB of counts)
+constexpr uint32_t kWhereThreads = 256;
+
+// TimeRange.contains with INT64_MAX as "no upper bound" (a timestamp of INT64_MAX then passes), and the two tag tests.
+__host__ __device__ __forceinline__ bool where_passes(const WherePred &w, int64_t ts, uint64_t tags) {
+    return ts >= w.after && (ts < w.before || w.before == INT64_MAX) && (tags & w.all_tags) == w.all_tags &&
+           (tags & w.no_tags) == 0u;
+}
+
+__device__ __forceinline__ AttrRow load_attr(const AttrRow *attrs, uint32_t row) {
+    const longlong2 v = __ldg(reinterpret_cast<const longlong2 *>(attrs) + row);
+    return AttrRow{v.x, static_cast<uint64_t>(v.y)};
+}
+
+__device__ __forceinline__ void stage_items(WhereItem *s_items, const WhereItem *items, uint32_t n_items) {
+    uint64_t *dst = reinterpret_cast<uint64_t *>(s_items);
+    const uint64_t *src = reinterpret_cast<const uint64_t *>(items);
+    for (uint32_t i = threadIdx.x; i < n_items * (sizeof(WhereItem) / 8); i += blockDim.x) dst[i] = src[i];
+}
+
+// counts[i] += rows of [0, n) passing items[i].pred, i < n_items <= kWhereChunk.  Each warp adds its ballots' popcounts to
+// its own shared counters (no atomics), the CTA sums them and issues one global atomic per (CTA, predicate).
+__global__ void __launch_bounds__(kWhereThreads) where_count_kernel(const AttrRow *__restrict__ attrs, uint32_t n,
+                                                                    const WhereItem *__restrict__ items, uint32_t n_items,
+                                                                    uint32_t *__restrict__ counts) {
+    __shared__ WhereItem s_items[kWhereChunk];
+    __shared__ uint32_t s_count[kWhereThreads / 32][kWhereChunk];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    stage_items(s_items, items, n_items);
+    for (uint32_t i = threadIdx.x; i < (kWhereThreads / 32) * kWhereChunk; i += blockDim.x) (&s_count[0][0])[i] = 0u;
+    __syncthreads();
+    const uint32_t stride = gridDim.x * blockDim.x;
+    for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += stride) {     // warp-uniform bounds
+        const uint32_t row = base + threadIdx.x;
+        const bool live = row < n;
+        const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
+        for (uint32_t i = 0; i < n_items; ++i) {
+            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && where_passes(s_items[i].pred, a.ts, a.tags));
+            if (lane == 0) s_count[warp][i] += __popc(b);
+        }
+    }
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < n_items; i += blockDim.x) {
+        uint32_t sum = 0;
+#pragma unroll
+        for (uint32_t w = 0; w < kWhereThreads / 32; ++w) sum += s_count[w][i];
+        if (sum) atomicAdd(counts + i, sum);
+    }
+}
+
+// bits[items[i].slot * words + word] &= the predicate's ballot over the word's 32 rows (rows >= n fail).  A warp owns a
+// word, so the read-modify-write needs no atomic; a bitset is named by at most one item of a launch.
+__global__ void __launch_bounds__(kWhereThreads) where_bits_kernel(const AttrRow *__restrict__ attrs, uint32_t n,
+                                                                   uint32_t words, uint32_t *__restrict__ bits,
+                                                                   const WhereItem *__restrict__ items, uint32_t n_items) {
+    __shared__ WhereItem s_items[kWhereChunk];
+    const uint32_t lane = threadIdx.x & 31u;
+    stage_items(s_items, items, n_items);
+    __syncthreads();
+    const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
+    for (uint32_t word = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; word < words; word += warps) {
+        const uint32_t row = (word << 5) + lane;
+        const bool live = row < n;
+        const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
+        for (uint32_t i = 0; i < n_items; ++i) {
+            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && where_passes(s_items[i].pred, a.ts, a.tags));
+            if (lane == 0 && b != 0xFFFFFFFFu) bits[s_items[i].slot * words + word] &= b;
+        }
+    }
+}
+
+// The rows passing items[i].pred, written to rows_out[items[i].slot + j] for j < the predicate's count (cursor[i], zeroed
+// by the caller, ends at that count).  The order within a list is arbitrary: the gather class sorts by (distance, row).
+__global__ void __launch_bounds__(kWhereThreads) where_compact_kernel(const AttrRow *__restrict__ attrs, uint32_t n,
+                                                                      const WhereItem *__restrict__ items, uint32_t n_items,
+                                                                      uint32_t *__restrict__ cursor,
+                                                                      uint32_t *__restrict__ rows_out) {
+    __shared__ WhereItem s_items[kWhereChunk];
+    const uint32_t lane = threadIdx.x & 31u;
+    stage_items(s_items, items, n_items);
+    __syncthreads();
+    const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
+    const uint32_t below = (1u << lane) - 1u;
+    for (uint32_t word = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; word < (n + 31u) / 32u; word += warps) {
+        const uint32_t row = (word << 5) + lane;
+        const bool live = row < n;
+        const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
+        for (uint32_t i = 0; i < n_items; ++i) {
+            const bool pass = live && where_passes(s_items[i].pred, a.ts, a.tags);
+            const uint32_t b = __ballot_sync(0xFFFFFFFFu, pass);
+            if (!b) continue;
+            uint32_t at = 0;
+            if (lane == 0) at = atomicAdd(cursor + i, static_cast<uint32_t>(__popc(b)));
+            at = __shfl_sync(0xFFFFFFFFu, at, 0);
+            if (pass) rows_out[s_items[i].slot + at + __popc(b & below)] = row;
+        }
+    }
+}
+
+}  // namespace waxvs

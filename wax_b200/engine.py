@@ -16,6 +16,7 @@ Everything numeric happens in libwaxvs_cuda.so; nothing here computes a distance
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import enum
 import threading
 from typing import Iterable, List, Optional, Sequence, Tuple
@@ -102,6 +103,25 @@ def is_normalized_l2(vector: Sequence[float], tolerance: float = 1e-3) -> bool:
     for x in v:
         s = np.float32(s + x * x)
     return bool(abs(np.float32(np.sqrt(s)) - np.float32(1)) <= np.float32(tolerance))
+
+
+@dataclasses.dataclass(frozen=True)
+class Where:
+    """A predicate on a frame's attributes (wax_vs_where): timestamp in [after, before) -- TimeRange.contains,
+    SearchRequest.swift:90-105 -- with every bit of all_tags set and no bit of no_tags.  The defaults bound nothing
+    (before = INT64_MAX lets a timestamp of INT64_MAX pass)."""
+    after: int = L.INT64_MIN
+    before: int = L.INT64_MAX
+    all_tags: int = 0
+    no_tags: int = 0
+
+    def passes(self, timestamp: int, tags: int) -> bool:
+        """The predicate on the host, as the device evaluates it."""
+        return (self.after <= timestamp and (timestamp < self.before or self.before == L.INT64_MAX)
+                and (tags & self.all_tags) == self.all_tags and (tags & self.no_tags) == 0)
+
+    def to_c(self) -> "L.Where":
+        return L.Where(int(self.after), int(self.before), int(self.all_tags), int(self.no_tags))
 
 
 def _clamp_topk(top_k: int) -> int:
@@ -367,6 +387,113 @@ class CUDAVectorEngine:
                                                    scores.ctypes.data_as(C.POINTER(C.c_float)),
                                                    groups.ctypes.data_as(C.POINTER(C.c_uint64)), cap,
                                                    ns.ctypes.data_as(C.POINTER(C.c_uint32))))
+        result = []
+        for i in range(b):
+            out: List[Tuple[int, List[Tuple[int, float]]]] = []
+            for j in range(int(ns[i])):
+                g = int(groups[i, j])
+                if not out or out[-1][0] != g:
+                    out.append((g, []))
+                out[-1][1].append((int(ids[i, j]), float(scores[i, j])))
+            result.append(out)
+        return result
+
+    # -- frame attributes: time-range and tag predicates below the top-k
+    def set_attributes(self, frame_ids: Sequence[int], timestamps: Optional[Sequence[int]] = None,
+                       tags: Optional[Sequence[int]] = None) -> int:
+        """Set frames' timestamp and tag mask (wax_vs_set_attributes): upsert by frame id, unknown frames ignored, a later
+        entry for the same frame wins; a column passed as None is left unchanged.  A frame never given attributes has
+        timestamp 0 and tags 0.  Attributes are not serialized: re-apply them after deserialize().  Returns the number of
+        distinct known frames named."""
+        fids = np.ascontiguousarray(frame_ids, dtype=np.uint64).reshape(-1)
+        ts = None if timestamps is None else np.ascontiguousarray(timestamps, dtype=np.int64).reshape(-1)
+        tg = None if tags is None else np.ascontiguousarray(tags, dtype=np.uint64).reshape(-1)
+        for name, col in (("timestamps", ts), ("tags", tg)):
+            if col is not None and col.size != fids.size:
+                raise ValueError(f"set_attributes: {fids.size} frame ids for {col.size} {name}")
+        if fids.size == 0:
+            return 0
+        n = C.c_uint64(0)
+        _check(L.lib().wax_vs_set_attributes(
+            self._h, fids.ctypes.data_as(C.POINTER(C.c_uint64)),
+            ts.ctypes.data_as(C.POINTER(C.c_int64)) if ts is not None else None,
+            tg.ctypes.data_as(C.POINTER(C.c_uint64)) if tg is not None else None, fids.size, C.byref(n)))
+        return n.value
+
+    def search_where(self, vector: Sequence[float], top_k: int, where: "Where", allow: Optional[Sequence[int]] = None,
+                     deny: Optional[Sequence[int]] = None) -> List[Tuple[int, float]]:
+        """The best `top_k` frames passing `where` (and the optional id filter allow= / deny=): the batch of one of
+        search_batch_where."""
+        if allow is not None and deny is not None:
+            raise ValueError("pass at most one of allow= / deny=")
+        filters = [("allow", allow)] if allow is not None else ([("deny", deny)] if deny is not None else [])
+        return self.search_batch_where([vector], top_k, [where], [0], filters, [0 if filters else None])[0]
+
+    def search_batch_where(self, vectors, top_k: int, wheres: Sequence["Where"], query_where: Sequence[Optional[int]],
+                           filters: Optional[Sequence[Tuple[object, Sequence[int]]]] = None,
+                           query_filter: Optional[Sequence[Optional[int]]] = None) -> List[List[Tuple[int, float]]]:
+        """search_batch_multi_filtered plus a predicate per query (wax_vs_search_batch_where): query i searches the frames
+        passing wheres[query_where[i]] AND filters[query_filter[i]] (None = no predicate / no id filter).  Its answer
+        equals search_batch_multi_filtered with an allow-list of exactly those frames, score bits included."""
+        qs = _as_rows(vectors, self.dimensions) if len(vectors) else np.zeros((0, self.dimensions), np.float32)
+        b = qs.shape[0]
+        filters = list(filters or [])
+        if query_filter is None:
+            query_filter = [None] * b
+        if len(query_where) != b or len(query_filter) != b:
+            raise ValueError(f"query_where / query_filter need {b} entries")
+        if b == 0:
+            return []
+        modes, lists = [], []
+        for mode, fids in filters:
+            modes.append({"allow": 0, "deny": 1}[mode] if isinstance(mode, str) else int(mode))
+            lists.append(np.ascontiguousarray(fids, dtype=np.uint64).reshape(-1))
+        offsets = np.zeros(len(lists) + 1, np.uint64)
+        offsets[1:] = np.cumsum([x.size for x in lists], dtype=np.uint64) if lists else []
+        fids = np.concatenate(lists) if lists else np.zeros(0, np.uint64)
+        modes_arr = np.asarray(modes, np.int32)
+        qf = np.asarray([L.NO_FILTER if f is None else int(f) for f in query_filter], np.uint32)
+        qw = np.asarray([L.NO_FILTER if w is None else int(w) for w in query_where], np.uint32)
+        warr = (L.Where * max(len(wheres), 1))(*[w.to_c() for w in wheres])
+        cap = _clamp_topk(top_k)
+        ids = np.zeros((b, cap), np.uint64)
+        scores = np.zeros((b, cap), np.float32)
+        ns = np.zeros(b, np.uint32)
+        _check(L.lib().wax_vs_search_batch_where(
+            self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_k),
+            fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
+            offsets.ctypes.data_as(C.POINTER(C.c_uint64)), modes_arr.ctypes.data_as(C.POINTER(C.c_int32)), len(lists),
+            qf.ctypes.data_as(C.POINTER(C.c_uint32)), C.cast(warr, C.c_void_p), len(wheres),
+            qw.ctypes.data_as(C.POINTER(C.c_uint32)), ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+            scores.ctypes.data_as(C.POINTER(C.c_float)), cap, ns.ctypes.data_as(C.POINTER(C.c_uint32))))
+        return [[(int(ids[i, j]), float(scores[i, j])) for j in range(int(ns[i]))] for i in range(b)]
+
+    def search_batch_grouped_where(self, vectors, top_groups: int, per_group: int, where: "Where",
+                                   allow: Optional[Sequence[int]] = None,
+                                   deny: Optional[Sequence[int]] = None) -> List[List[Tuple[int, List[Tuple[int, float]]]]]:
+        """search_batch_grouped over the frames passing `where` AND the optional id filter
+        (wax_vs_search_batch_grouped_where); each answer equals search_grouped under the allow-list of those frames."""
+        if allow is not None and deny is not None:
+            raise ValueError("pass at most one of allow= / deny=")
+        fids = np.ascontiguousarray(allow if allow is not None else (deny if deny is not None else []),
+                                    dtype=np.uint64).reshape(-1)
+        mode = 0 if allow is not None else 1
+        qs = _as_rows(vectors, self.dimensions) if len(vectors) else np.zeros((0, self.dimensions), np.float32)
+        b = qs.shape[0]
+        if b == 0:
+            return []
+        cap = max(1, min(_clamp_topk(top_groups) * max(int(per_group), 1), L.MAX_RESULTS))
+        ids = np.empty((b, cap), np.uint64)
+        scores = np.empty((b, cap), np.float32)
+        groups = np.empty((b, cap), np.uint64)
+        ns = np.zeros(b, np.uint32)
+        w = where.to_c()
+        _check(L.lib().wax_vs_search_batch_grouped_where(
+            self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_groups), int(per_group),
+            fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None, fids.size, mode,
+            C.cast(C.pointer(w), C.c_void_p), ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+            scores.ctypes.data_as(C.POINTER(C.c_float)), groups.ctypes.data_as(C.POINTER(C.c_uint64)), cap,
+            ns.ctypes.data_as(C.POINTER(C.c_uint32))))
         result = []
         for i in range(b):
             out: List[Tuple[int, List[Tuple[int, float]]]] = []

@@ -272,6 +272,80 @@ public:
         return out;
     }
 
+    // Frame attributes (wax_vs_set_attributes): timestamps / tags per frame, upsert; a null column is left unchanged.
+    // Not serialized: re-apply them after deserialize().
+    uint64_t setAttributes(const std::vector<uint64_t> &frameIds, const std::vector<int64_t> *timestamps,
+                           const std::vector<uint64_t> *tags) {
+        if ((timestamps && timestamps->size() != frameIds.size()) || (tags && tags->size() != frameIds.size()))
+            throw EncodingError("setAttributes: column length != frameIds.count");
+        uint64_t assigned = 0;
+        if (frameIds.empty()) return 0;
+        check(wax_vs_set_attributes(h_, frameIds.data(), timestamps ? timestamps->data() : nullptr,
+                                    tags ? tags->data() : nullptr, frameIds.size(), &assigned));
+        return assigned;
+    }
+
+    // A batch whose query i searches the frames passing wheres[queryWhere[i]] (WAX_VS_NO_FILTER: none)
+    // (wax_vs_search_batch_where; no id filters here -- the C call takes them too).
+    std::vector<std::vector<Hit>> searchBatchWhere(const std::vector<std::vector<float>> &vectors, int64_t topK,
+                                                   const std::vector<wax_vs_where> &wheres,
+                                                   const std::vector<uint32_t> &queryWhere) const {
+        std::vector<std::vector<Hit>> out(vectors.size());
+        if (vectors.empty()) return out;
+        if (queryWhere.size() != vectors.size()) throw EncodingError("searchBatchWhere: queryWhere.count != vectors.count");
+        const uint32_t lim = static_cast<uint32_t>(topK < 1 ? 1 : (topK > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topK));
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchWhere: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        const uint64_t offsets[1] = {0};
+        const std::vector<uint32_t> queryFilter(vectors.size(), WAX_VS_NO_FILTER);
+        std::vector<uint64_t> ids(vectors.size() * lim);
+        std::vector<float> scores(vectors.size() * lim);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_where(h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_, topK, nullptr,
+                                        offsets, nullptr, 0, queryFilter.data(), wheres.data(),
+                                        static_cast<uint32_t>(wheres.size()), queryWhere.data(), ids.data(), scores.data(),
+                                        lim, ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) out[q].push_back({ids[q * lim + i], scores[q * lim + i]});
+        return out;
+    }
+
+    // searchBatchGrouped over the frames passing `where` and the optional filter (wax_vs_search_batch_grouped_where).
+    std::vector<std::vector<Group>> searchBatchGroupedWhere(const std::vector<std::vector<float>> &vectors,
+                                                            int64_t topGroups, uint32_t perGroup, const wax_vs_where &where,
+                                                            const std::vector<uint64_t> &frameIds = {},
+                                                            bool allow = false) const {
+        std::vector<std::vector<Group>> out(vectors.size());
+        if (vectors.empty()) return out;
+        const int64_t lim = topGroups < 1 ? 1 : (topGroups > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topGroups);
+        const int64_t want = lim * (perGroup ? perGroup : 1);
+        const size_t cap = static_cast<size_t>(want > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : want);
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchGroupedWhere: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        std::vector<uint64_t> ids(vectors.size() * cap), groups(vectors.size() * cap);
+        std::vector<float> scores(vectors.size() * cap);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_grouped_where(h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_,
+                                                topGroups, perGroup, frameIds.data(), frameIds.size(), allow ? 0 : 1,
+                                                &where, ids.data(), scores.data(), groups.data(),
+                                                static_cast<uint32_t>(cap), ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) {
+                const size_t j = q * cap + i;
+                if (out[q].empty() || out[q].back().first != groups[j]) out[q].push_back({groups[j], {}});
+                out[q].back().second.push_back({ids[j], scores[j]});
+            }
+        return out;
+    }
+
     // static load(from:metric:dimensions:) (MetalVectorEngine.swift:318-328): the committed blob (may be empty = none
     // committed yet), then the pending embedding mutations as ONE upsert batch (sequential semantics in the library).
     static CUDAVectorEngine *load(const std::vector<uint8_t> *committedBlob, const std::vector<uint64_t> &pendingIds,
