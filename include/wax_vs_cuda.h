@@ -418,8 +418,9 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *engine, uint64_t *tensor_queries
    nominate in TF32 at about half the rate), "batch_tf32_queries", "filter_bitset_passes" (sub-batches of per-query
    filtered queries on the tensor-core class, wax_vs_search_batch_multi_filtered), "group_index_builds" (device group
    index builds of wax_vs_search_grouped), "attribute_uploads" (device attribute copies of the where searches), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
-   (single queries the bf16-shadow route answered / that the fp32 scan answered after a failed proof; read them while
-   no search is running). */
+   (single queries the shadow route answered / that the fp32 scan answered after a failed proof, either shadow; read them
+   while no search is running), "single_int8_queries" (single queries whose route nominated from the int8 shadow),
+   "int8_shadow_bytes" / "int8_shadow_rows" (HBM held by the int8 shadow's live rows, codes and scales / rows it covers). */
 int32_t wax_vs_debug_counter(wax_vs_engine *engine, const char *name, uint64_t *out);
 
 /* Device-only timing of the batched path (n_queries synthetic unit queries per step, everything resident):
@@ -461,6 +462,23 @@ int32_t wax_vs_debug_shadow_nominations(wax_vs_engine *engine, const float *quer
    did not fit in device memory). */
 int32_t wax_vs_debug_read_shadow(wax_vs_engine *engine, uint64_t first, uint64_t n, uint16_t *dst);
 
+/* The int8 form of wax_vs_debug_shadow_nominations: the same read-out with the INT8 form of the scan nominating from the
+   int8 shadow, in the shape the options select (int8_rows_per_step, int8_warps, int8_stages, grid, chunk_steps,
+   tail_select), and the finish proving with that shadow's measured bound -- whatever "int8_scan_min_bytes" and the
+   bound's size say (a corpus whose bound is coarser than the bf16 one is read out too: the search would take the bf16
+   route).  Nominee keys carry score' = s * (q . c).  WAX_VS_ERR_UNSUPPORTED as for the bf16 read-out, or when the int8
+   shadow does not fit in device memory. */
+int32_t wax_vs_debug_int8_nominations(wax_vs_engine *engine, const float *query, int64_t top_k, const uint32_t *allow_bits,
+                                      uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
+                                      uint32_t *out_shape);
+
+/* The int8 shadow of rows [first, first + n) (brought up to date first): dst_codes[n][dims] the stored bytes (code + 128;
+   cosine rows pre-scaled by 1/|v| before coding), dst_scales[n] each row's scale s, *out_rho_max the measured bound:
+   >= ||v^ - s (byte - 128)||_2 for every row, +inf when a row is not finite.  WAX_VS_ERR_UNSUPPORTED for l2, dims not a
+   multiple of 128 up to 1536, or when the int8 shadow does not fit in device memory. */
+int32_t wax_vs_debug_read_int8_shadow(wax_vs_engine *engine, uint64_t first, uint64_t n, uint8_t *dst_codes,
+                                      float *dst_scales, float *out_rho_max);
+
 /* Streaming-read ceiling on the same box: a plain coalesced LDG.128 read of the live corpus bytes, best of
    `iters` (milliseconds, and the bytes read).  Context for the roofline fraction (SURVEY.md section 8d). */
 int32_t wax_vs_debug_stream_read(wax_vs_engine *engine, uint32_t iters, float *out_best_ms, uint64_t *out_bytes);
@@ -473,7 +491,10 @@ int32_t wax_vs_debug_stream_read(wax_vs_engine *engine, uint32_t iters, float *o
    wax_vs_search_batch_multi_filtered may use; at least one bitset always fits.
    "shadow_scan" (default 1): 0 sends every single query to the fp32 scan (the bf16-shadow route off);
    "shadow_scan_min_bytes" (default 512 MiB): the smallest fp32 corpus that takes that route;
-   "shadow_rows_per_step" / "shadow_warps" / "shadow_stages" (0 = auto): the shape of its nominating scan. */
+   "shadow_rows_per_step" / "shadow_warps" / "shadow_stages" (0 = auto): the shape of its nominating scan;
+   "int8_scan_min_bytes" (default 512 MiB): the smallest fp32 corpus whose route nominates from the int8 shadow (when it
+   fits and its measured bound is no coarser than the bf16 one); setting it also retries an int8 shadow that did not fit;
+   "int8_rows_per_step" / "int8_warps" / "int8_stages" (0 = auto): the shape of the INT8 nominating scan. */
 int32_t wax_vs_debug_set_option(wax_vs_engine *engine, const char *key, int64_t value);
 
 /* Library build info: "waxvs_cuda <version> sm_90a ...". */

@@ -1,16 +1,18 @@
 #!/usr/bin/env python
-"""Single-query bf16-shadow route against the fp32 scan (DESIGN 4.1) -- companion of bench.py, same conventions:
+"""Single-query shadow route against the fp32 scan (DESIGN 4.1) -- companion of bench.py, same conventions:
 device-only times (queries resident in HBM, CUDA events on the launching stream inside the library), one query in
-flight.  In one process and one engine the fp32 scan (option shadow_scan = 0) and the default route alternate, round by
-round, so that both see the same clocks and the same HBM.
+flight.  In one process and one engine the fp32 scan (option shadow_scan = 0), the route on the bf16 shadow
+(int8_scan_min_bytes out of reach) and the route on the int8 shadow alternate, round by round, so that all three see the
+same clocks and the same HBM.
 
     python scripts/bench_shadow_scan.py [--rounds 5] [--steps 50] [--out FILE] [--sweep] [--tune]
 
-Reports ms per query of both routes, their ratio and the spread over the rounds, the fallbacks counted, GB/s over the
-SHADOW bytes (what the route reads: rows * dims * 2 per query, plus the re-scored nominees) against the same run's plain
-read of the fp32 corpus (stream_read_gbs), the cost of the first search after fill_synthetic and after a remove (the
-shadow builds then), k = 1 / 10 / 32, 10 M x 768 dot, and with --sweep the corpus sizes 10 K .. 10 M that set the
-route's size threshold.  --tune alternates shapes of the SHADOW form (rows per step, warps, ring depth) on 10 M x 384.
+Reports ms per query of the three arms, their ratios and the spread over the rounds, the fallbacks counted, GB/s over
+the shadow bytes (what a route reads: rows * dims * 2 per query for bf16, rows * (dims + 4) for int8 codes and scales)
+against the same run's plain read of the fp32 corpus (stream_read_gbs), the cost of the first search after
+fill_synthetic and after a remove (the shadow builds then), k = 1 / 10 / 32, 10 M x 768 dot, and with --sweep the corpus
+sizes 10 K .. 10 M that set the size thresholds.  --tune alternates shapes of the INT8 form (rows per step, warps, ring
+depth) on 10 M x 384.
 Prints one JSON line (and writes it to --out)."""
 import argparse
 import json
@@ -26,6 +28,7 @@ sys.path.insert(0, str(ROOT))
 from wax_b200 import CUDAVectorEngine, VectorMetric  # noqa: E402
 
 N_DISTINCT, SEED = 64, 1002
+DEFAULT_INT8_MIN = 512 << 20     # the engine's default int8_scan_min_bytes (waxvs_engine.cu Tuning)
 
 
 def gpu_info():
@@ -46,22 +49,36 @@ def counts(eng):
     return eng.counter("single_shadow_queries"), eng.counter("single_shadow_fallbacks")
 
 
-def alternate(eng, k, rounds, steps):
-    """rounds x (fp32 scan, default route), steps device-timed queries each."""
-    fp32, route, launches = [], [], None
-    q0, f0 = counts(eng)
+NO_INT8 = 1 << 62          # int8_scan_min_bytes that keeps every corpus on the bf16 shadow
+
+
+def alternate(eng, k, rounds, steps, int8_min=0):
+    """rounds x (fp32 scan, bf16 route, int8 route), steps device-timed queries each; int8_min: the engine's
+    int8_scan_min_bytes for the int8 arm (the default threshold, or 0 below it)."""
+    arms = {"fp32": [], "bf16": [], "int8": []}
+    seen = {a: [0, 0, 0] for a in arms}           # route queries, fallbacks, int8 nominations
+    launches = {}
     for _ in range(rounds):
-        eng.set_option("shadow_scan", 0)
-        fp32.append(per_query_ms(eng, k, steps)[0])
-        eng.set_option("shadow_scan", 1)
-        ms, launches = per_query_ms(eng, k, steps)
-        route.append(ms)
-    q1, f1 = counts(eng)
-    m_fp32, m_route = float(np.median(fp32)), float(np.median(route))
-    return {"k": k, "fp32_ms": m_fp32, "route_ms": m_route, "speedup": m_fp32 / m_route,
-            "fp32_ms_rounds": fp32, "route_ms_rounds": route,
-            "route_spread_pct": (max(route) - min(route)) / m_route * 100, "fp32_spread_pct": (max(fp32) - min(fp32)) / m_fp32 * 100,
-            "route_launches_per_query": launches, "route_queries": q1 - q0, "fallbacks": f1 - f0}
+        for arm in arms:
+            eng.set_option("shadow_scan", 0 if arm == "fp32" else 1)
+            eng.set_option("int8_scan_min_bytes", NO_INT8 if arm == "bf16" else int8_min)
+            (q0, f0), i0 = counts(eng), eng.counter("single_int8_queries")
+            ms, launches[arm] = per_query_ms(eng, k, steps)
+            (q1, f1), i1 = counts(eng), eng.counter("single_int8_queries")
+            arms[arm].append(ms)
+            seen[arm] = [seen[arm][0] + q1 - q0, seen[arm][1] + f1 - f0, seen[arm][2] + i1 - i0]
+    eng.set_option("shadow_scan", 1)
+    eng.set_option("int8_scan_min_bytes", int8_min)
+    med = {a: float(np.median(t)) for a, t in arms.items()}
+    out = {"k": k, "fp32_ms": med["fp32"], "bf16_ms": med["bf16"], "int8_ms": med["int8"],
+           "int8_vs_bf16": med["bf16"] / med["int8"], "int8_vs_fp32": med["fp32"] / med["int8"]}
+    for a, t in arms.items():
+        out[f"{a}_ms_rounds"] = t
+        out[f"{a}_spread_pct"] = (max(t) - min(t)) / med[a] * 100
+        out[f"{a}_launches_per_query"] = launches[a]
+    for a in ("bf16", "int8"):
+        out[f"{a}_route_queries"], out[f"{a}_fallbacks"], out[f"{a}_int8_nominations"] = seen[a]
+    return out
 
 
 def first_search_ms(eng, dims, seed):
@@ -80,12 +97,13 @@ def headline(args):
     out["first_search_after_fill_ms"] = first_search_ms(eng, dims, 1)          # norms + shadow build
     out["steady_search_ms"] = float(np.median([first_search_ms(eng, dims, 2 + i) for i in range(5)]))
     eng.time_search(10, 20, warmup=0, n_queries=N_DISTINCT, seed=SEED)           # settle
-    out["k"] = [alternate(eng, k, args.rounds, args.steps) for k in (10, 1, 32)]
+    out["k"] = [alternate(eng, k, args.rounds, args.steps, int8_min=DEFAULT_INT8_MIN) for k in (10, 1, 32)]
     read = eng.stream_read_gbs(5)
     r10 = out["k"][0]
-    shadow_bytes = rows * dims * 2
     out["stream_read_gbs"] = read
-    out["route_gbs_on_shadow_bytes"] = shadow_bytes / (r10["route_ms"] * 1e-3) / 1e9
+    out["bf16_gbs_on_shadow_bytes"] = rows * dims * 2 / (r10["bf16_ms"] * 1e-3) / 1e9
+    out["int8_gbs_on_shadow_bytes"] = rows * (dims + 4) / (r10["int8_ms"] * 1e-3) / 1e9     # codes + scales
+    out["int8_frac_of_stream_read"] = out["int8_gbs_on_shadow_bytes"] / read
     out["fp32_gbs_on_corpus_bytes"] = rows * dims * 4 / (r10["fp32_ms"] * 1e-3) / 1e9
     eng.remove(123)
     out["first_search_after_remove_ms"] = first_search_ms(eng, dims, 3)        # shadow rebuild
@@ -97,10 +115,10 @@ def headline(args):
 
 
 def tune(eng, args):
-    """Shapes of the SHADOW form (its own options: the guarded fp32 scan keeps its shape), alternated round by round;
+    """Shapes of the INT8 form (its own options: the guarded fp32 scan keeps its shape), alternated round by round;
     0 = the engine's default."""
-    shapes = [(0, 0, 0), (8, 8, 3), (8, 12, 2), (8, 16, 2), (4, 16, 2), (4, 16, 3), (16, 8, 2), (4, 12, 3)]
-    cands = [dict(shadow_rows_per_step=r, shadow_warps=w, shadow_stages=s) for r, w, s in shapes]
+    shapes = [(0, 0, 0), (8, 16, 2), (8, 16, 4), (8, 12, 3), (16, 16, 2), (16, 8, 3), (4, 16, 3), (4, 16, 4)]
+    cands = [dict(int8_rows_per_step=r, int8_warps=w, int8_stages=s) for r, w, s in shapes]
     times, proven, failed = [[] for _ in cands], [0] * len(cands), [0] * len(cands)
     for _ in range(args.rounds):
         for i, c in enumerate(cands):
@@ -122,7 +140,7 @@ def dot768(args):
     eng = CUDAVectorEngine(VectorMetric.dot, dims)
     eng.fill_synthetic(5, rows, normalize=False)
     eng.time_search(10, 10, warmup=0, n_queries=N_DISTINCT, seed=SEED)
-    out = alternate(eng, 10, args.rounds, args.steps)
+    out = alternate(eng, 10, args.rounds, args.steps, int8_min=DEFAULT_INT8_MIN)
     out["workload"] = f"{rows} x {dims} fp32 dot (rows not normalised)"
     eng.close()
     return out
@@ -135,9 +153,10 @@ def sweep(args):
         eng.fill_synthetic(2, rows)
         eng.set_option("shadow_scan_min_bytes", 0)
         eng.time_search(10, 10, warmup=0, n_queries=N_DISTINCT, seed=SEED)
-        r = alternate(eng, 10, args.rounds, args.steps)
-        res.append({"rows": rows, "fp32_mb": rows * 384 * 4 / 2**20, "fp32_ms": r["fp32_ms"], "route_ms": r["route_ms"],
-                    "speedup": r["speedup"], "fallbacks": r["fallbacks"]})
+        r = alternate(eng, 10, args.rounds, args.steps, int8_min=0)
+        res.append({"rows": rows, "fp32_mb": rows * 384 * 4 / 2**20, "fp32_ms": r["fp32_ms"], "bf16_ms": r["bf16_ms"],
+                    "int8_ms": r["int8_ms"], "int8_vs_bf16": r["int8_vs_bf16"], "int8_vs_fp32": r["int8_vs_fp32"],
+                    "int8_fallbacks": r["int8_fallbacks"], "int8_nominations": r["int8_int8_nominations"]})
         eng.close()
     return res
 

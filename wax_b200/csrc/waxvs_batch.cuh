@@ -317,6 +317,65 @@ __global__ void __launch_bounds__(256) shadow_bf16_kernel(const float *__restric
     }
 }
 
+// ---- int8 shadow of the corpus (the single-query route, DESIGN 4.1; cached per corpus version like the bf16 one) -------
+// One warp per row.  v^ = the row as the bf16 shadow takes it (cosine: fl(v_i / |v|) through the cached 1/|v|, dot: v);
+// s = fl(max |v^_i| / 127) and c_i = rne(v^_i / s) in [-127, 127] (0 when s == 0), stored biased: dst byte c_i + 128 (the
+// scan widens it with one PRMT, int8x4_to_float4); scale[row] = s.  The bound is MEASURED from what was stored:
+// rho = ||v^ - s c||_2 in fp64 (s c_i is exact there), rounded up to fp32 with a relative 2^-40 on top for the fp64 sum, so
+// |q.v^ - s (q.c)| <= |q| rho for every query.  A row with a non-finite v^_i or s gives rho = +inf.  Every warp raises
+// *rho_max_bits (fp32 bits: nonnegative floats order as uints) once with the largest rho of its rows.
+// dims % 128 == 0 and dims <= 128 * kInt8MaxChunks (the unrolled scan shapes): a lane holds its chunks of the row in
+// registers between the max and the codes.
+constexpr uint32_t kInt8MaxChunks = 12;
+__global__ void __launch_bounds__(256) shadow_int8_kernel(const float *__restrict__ src, const float *__restrict__ scale_in,
+                                                          uint64_t n_rows, uint32_t dims, uint32_t *__restrict__ dst,
+                                                          float *__restrict__ scale, uint32_t *rho_max_bits) {
+    const int lane = threadIdx.x & 31;
+    const uint64_t warps = (static_cast<uint64_t>(gridDim.x) * blockDim.x) >> 5;
+    const uint32_t d4 = dims >> 2, cn = d4 / 32u;
+    uint32_t local_max = 0;                              // fp32 bits of the largest rho of this warp's rows
+    for (uint64_t row = (static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; row < n_rows; row += warps) {
+        const float4 *v4 = reinterpret_cast<const float4 *>(src) + row * d4;
+        const float w = scale_in ? __ldg(scale_in + row) : 1.0f;
+        float4 x[kInt8MaxChunks];
+        float m = 0.0f;
+        bool bad = false;
+#pragma unroll
+        for (uint32_t c = 0; c < kInt8MaxChunks; ++c) {
+            if (c >= cn) break;
+            x[c] = __ldcs(v4 + lane + 32u * c);
+            if (scale_in) { x[c].x *= w; x[c].y *= w; x[c].z *= w; x[c].w *= w; }
+            bad |= !finite_f32(x[c].x) || !finite_f32(x[c].y) || !finite_f32(x[c].z) || !finite_f32(x[c].w);
+            m = fmaxf(m, fmaxf(fmaxf(fabsf(x[c].x), fabsf(x[c].y)), fmaxf(fabsf(x[c].z), fabsf(x[c].w))));
+        }
+        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(WAXVS_FULL_MASK, m, o));
+        bad = __any_sync(WAXVS_FULL_MASK, bad);
+        const float s = __fdiv_rn(m, 127.0f);
+        double r2 = 0.0;
+#pragma unroll
+        for (uint32_t c = 0; c < kInt8MaxChunks; ++c) {
+            if (c >= cn) break;
+            const float xs[4] = {x[c].x, x[c].y, x[c].z, x[c].w};
+            uint32_t packed = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                int code = 0;
+                if (s > 0.0f && !bad) code = max(-127, min(127, __float2int_rn(__fdiv_rn(xs[j], s))));
+                packed |= static_cast<uint32_t>(code + 128) << (8 * j);
+                const double e = static_cast<double>(xs[j]) - static_cast<double>(s) * static_cast<double>(code);
+                r2 = fma(e, e, r2);
+            }
+            dst[row * d4 + lane + 32u * c] = packed;
+        }
+        for (int o = 16; o > 0; o >>= 1) r2 += __shfl_xor_sync(WAXVS_FULL_MASK, r2, o);
+        float rho = __double2float_ru(sqrt(r2) * (1.0 + 0x1p-40));
+        if (bad || !finite_f32(s) || !finite_f32(rho)) rho = INFINITY;
+        if (lane == 0) scale[row] = s;
+        local_max = max(local_max, __float_as_uint(rho));
+    }
+    if (lane == 0 && local_max) atomicMax(rho_max_bits, local_max);
+}
+
 // ---- the tensor-core kernel ---------------------------------------------------------------------------------------
 // BF16: operands are bf16 (the corpus shadow + converted queries; 64 elements per 128-byte k-block, wgmma k16 at twice
 //       the TF32 rate for the same bytes) -- nominations only, exactness comes from the finish kernel.

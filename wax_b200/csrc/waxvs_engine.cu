@@ -193,6 +193,10 @@ struct Tuning {
                                                      // latency-bound: two more launches and a shadow do not pay; on
                                                      // H100 at 384 dims the route breaks even near 380 MB, DESIGN 5)
     int shadow_rows_per_step = 0, shadow_warps = 0, shadow_stages = 0;   // shape of the SHADOW form (0 auto)
+    uint64_t int8_scan_min_bytes = 512ull << 20;   // the route nominates from the int8 shadow (half the bytes of the bf16
+                                                   // one) for fp32 corpora of at least this many bytes whose measured int8
+                                                   // bound is no coarser than the bf16 one (DESIGN 4.1, 5)
+    int int8_rows_per_step = 0, int8_warps = 0, int8_stages = 0;   // shape of the INT8 form (0 auto)
 };
 
 // Per-search scratch: the analogue of TransientBuffers (MetalVectorEngine.swift:36-41, :84-117).
@@ -302,6 +306,18 @@ struct wax_vs_engine {
     DevBuf<__nv_bfloat16> d_shadow;
     uint64_t shadow_rows = 0;      // rows [0, shadow_rows) of d_shadow are valid; shadow_valid = covers every live row
     bool shadow_valid = false, shadow_unavailable = false;
+    // int8 shadow of the corpus for the single-query route only (DESIGN 4.1; same cache rules, guarded by norms_mu): four
+    // biased codes per word, one scale per row (padded to whole scan steps) and the measured bound rho_max (fp32 bits on
+    // the device; read back once per build together with max|v|, giving the bound the finish uses)
+    DevBuf<uint32_t> d_int8;
+    DevBuf<float> d_int8_scale;
+    DevBuf<uint32_t> d_int8_rho;
+    uint64_t int8_rows = 0;        // rows [0, int8_rows) are valid; int8_valid = covers every live row
+    bool int8_valid = false, int8_unavailable = false;
+    bool int8_coarse = false;      // the last build measured a bound too coarse for the route: none is built again until
+                                   // the rows are rewritten (invalidate_row_caches with no prefix) or int8_scan_min_bytes is set
+    float int8_rho_max = 0.0f, int8_eps_rel = INFINITY;   // rho_max, and rho_max / M rounded up (M = 1 cosine, max|v| dot)
+    uint64_t single_int8_queries = 0;                     // single queries nominated from the int8 shadow (pool_mu)
     uint64_t batch_tensor_queries = 0, batch_fallback_queries = 0;   // instrumentation
     uint64_t batch_bf16_queries = 0, batch_retry_queries = 0, batch_tf32_queries = 0, batch_filter_bf16_queries = 0;
     uint64_t filter_bitset_passes = 0;
@@ -397,6 +413,9 @@ static void invalidate_row_caches(wax_vs_engine *e, uint64_t keep_prefix) {
     e->norms_rows = std::min(e->norms_rows, keep_prefix);
     e->shadow_rows = std::min(e->shadow_rows, keep_prefix);
     if (e->shadow_rows == 0) e->shadow_valid = false;
+    e->int8_rows = std::min(e->int8_rows, keep_prefix);   // a kept prefix keeps rho_max too: still an upper bound
+    e->int8_valid = false;
+    if (keep_prefix == 0) e->int8_coarse = false;
     e->gindex.valid = false;           // appends too: the new rows need index entries
     e->attrs_dev_valid = false;        // likewise the attribute mirror
 }
@@ -476,8 +495,8 @@ static int32_t ctx_for_stream(wax_vs_engine *e, void *cuda_stream, SearchCtx **o
 // kernel dispatch
 struct TmaConfig { int C, R, warps, stages; size_t smem; };
 
-// esize: bytes per element of the rows streamed -- 4 for the corpus, 2 for the bf16 shadow (the SHADOW form, unrolled
-// shapes only).
+// esize: bytes per element of the rows streamed -- 4 for the corpus, 2 for the bf16 shadow (the SHADOW form), 1 for the
+// int8 shadow (the INT8 form; its stages also hold the step's row scales) -- the shadow forms on unrolled shapes only.
 static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0, size_t esize = sizeof(float)) {
     const uint32_t d = e->dims;
     if (d % 4u != 0) return false;                      // rows must be 16-byte multiples for the bulk copy
@@ -495,7 +514,14 @@ static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0
     // is per-row instruction latency, not bytes in flight).  These defaults were chosen on B200, not re-tuned on H100; the
     // `rows_per_step` / `warps` / `stages` options override them.
     int R, warps_default = 8;
-    if (esize != sizeof(float)) {                        // the shadow form (bf16 rows: half the bytes of a corpus row)
+    if (esize == 1) {                                    // the INT8 form (a quarter of the bytes of a corpus row)
+        // steps of ~3 KB like the best bf16 shape, 16 warps, 3 stages (DESIGN 4.1); launch_int8_scan has rows per step
+        // r_lo .. r_hi, r_def by default
+        const int want_r = e->tune.int8_rows_per_step;
+        const int r_def = C <= 3 ? 8 : 4, r_lo = C == 3 ? 4 : r_def, r_hi = C <= 3 ? 16 : (C <= 6 ? 8 : 4);
+        R = (want_r >= r_lo && want_r <= r_hi && (want_r & (want_r - 1)) == 0) ? want_r : r_def;
+        warps_default = 16;
+    } else if (esize != sizeof(float)) {                 // the shadow form (bf16 rows: half the bytes of a corpus row)
         // 16 warps, 3 stages of 2-6 KB: on H100 at 10 M x 384 (C = 3) rows 4 / warps 16 / stages 3 took 2.503 ms per
         // query against 2.545 for the fp32 shape's bytes (rows 8 / warps 8 / stages 2), the best of eight shapes
         // alternated in one run (DESIGN 4.1); the other C take the same ring, not measured separately.
@@ -529,10 +555,11 @@ static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0
     }
     // Default ring depth 2: ~48 KB in flight per SM for the 8-warp shapes (the `stages` option overrides it).  The shadow
     // form has options of its own (shadow_*): it runs right before a guarded fp32 scan that keeps the fp32 shape.
-    const bool shadow = esize != sizeof(float);
-    const int want_stages = shadow ? e->tune.shadow_stages : e->tune.stages, want_warps = shadow ? e->tune.shadow_warps : e->tune.warps;
+    const bool shadow = esize != sizeof(float), int8 = esize == 1;
+    const int want_stages = int8 ? e->tune.int8_stages : shadow ? e->tune.shadow_stages : e->tune.stages;
+    const int want_warps = int8 ? e->tune.int8_warps : shadow ? e->tune.shadow_warps : e->tune.warps;
     const int stages = want_stages > 0 ? want_stages : (shadow ? 3 : 2);
-    const size_t stage_bytes = static_cast<size_t>(R) * d * esize;
+    const size_t stage_bytes = static_cast<size_t>(R) * d * esize + (int8 ? static_cast<size_t>(R) * 4 : 0);   // + scales
     const size_t query_bytes = C == 0 ? (static_cast<size_t>(d) * 4 + 512 + 32) : 0;
     auto smem_for = [&](int w) { return static_cast<size_t>(w) * stages * (stage_bytes + 8 + 4) + static_cast<size_t>(w) * 1024 + 16 + query_bytes; };
     int warps = want_warps ? want_warps : warps_default;
@@ -555,11 +582,11 @@ static cudaError_t grant_smem(wax_vs_engine *e, K kernel, size_t bytes) {
     return err;
 }
 
-template <int C, int R, int M, int E, bool EMIT, bool SHADOW = false>
+template <int C, int R, int M, int E, bool EMIT, bool SHADOW = false, bool INT8 = false>
 static cudaError_t launch_tma_inst(wax_vs_engine *e, const ScanParams &p, int grid, const TmaConfig &cfg, cudaStream_t s) {
-    cudaError_t err = grant_smem(e, scan_tma_kernel<C, R, M, E, EMIT, SHADOW>, cfg.smem);
+    cudaError_t err = grant_smem(e, scan_tma_kernel<C, R, M, E, EMIT, SHADOW, INT8>, cfg.smem);
     if (err != cudaSuccess) return err;
-    scan_tma_kernel<C, R, M, E, EMIT, SHADOW><<<grid, cfg.warps * 32, cfg.smem, s>>>(p);
+    scan_tma_kernel<C, R, M, E, EMIT, SHADOW, INT8><<<grid, cfg.warps * 32, cfg.smem, s>>>(p);
     return cudaGetLastError();
 }
 // mode: 0 = fused list k <= 32, 1 = fused list k <= 128, 2 = emit distance keys
@@ -599,6 +626,19 @@ static cudaError_t launch_shadow_scan(wax_vs_engine *e, const ScanParams &p, int
     WAXVS_CASE(1, 8); WAXVS_CASE(1, 16); WAXVS_CASE(2, 8); WAXVS_CASE(2, 16);
     WAXVS_CASE(3, 4); WAXVS_CASE(3, 8); WAXVS_CASE(3, 16); WAXVS_CASE(4, 4); WAXVS_CASE(4, 8);
     WAXVS_CASE(6, 2); WAXVS_CASE(6, 4); WAXVS_CASE(8, 2); WAXVS_CASE(8, 4); WAXVS_CASE(12, 2); WAXVS_CASE(12, 4);
+#undef WAXVS_CASE
+    return cudaErrorInvalidValue;
+}
+// The INT8 form (nominating pass of the int8-shadow route): the shapes pick_tma_config gives it.
+static cudaError_t launch_int8_scan(wax_vs_engine *e, const ScanParams &p, int grid, const TmaConfig &cfg, int metric,
+                                   cudaStream_t s) {
+#define WAXVS_CASE(Cv, Rv)                                                                                          \
+    if (cfg.C == Cv && cfg.R == Rv)                                                                                 \
+        return metric == kCosine ? launch_tma_inst<Cv, Rv, kCosine, 4, false, true, true>(e, p, grid, cfg, s)      \
+                                 : launch_tma_inst<Cv, Rv, kDot, 4, false, true, true>(e, p, grid, cfg, s)
+    WAXVS_CASE(1, 8); WAXVS_CASE(1, 16); WAXVS_CASE(2, 8); WAXVS_CASE(2, 16);
+    WAXVS_CASE(3, 4); WAXVS_CASE(3, 8); WAXVS_CASE(3, 16); WAXVS_CASE(4, 4); WAXVS_CASE(4, 8);
+    WAXVS_CASE(6, 4); WAXVS_CASE(6, 8); WAXVS_CASE(8, 4); WAXVS_CASE(12, 4);
 #undef WAXVS_CASE
     return cudaErrorInvalidValue;
 }
@@ -711,6 +751,7 @@ static int tma_grid(const wax_vs_engine *e, const SearchCtx *c, const TmaConfig 
 
 static bool batch_bf16_wanted(const wax_vs_engine *e);
 static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream);
+static int32_t ensure_int8_shadow(wax_vs_engine *e, cudaStream_t stream, bool keep_coarse = false);
 
 // ---- the bf16-shadow route of a single query (DESIGN 4.1) ----
 // The fp32 scan reads dims * 4 bytes per row and runs at the HBM read ceiling; the shadow holds the same rows in bf16.
@@ -723,31 +764,54 @@ constexpr uint32_t kShadowRescore = 256;
 constexpr uint32_t kShadowSkipQueries = 16;   // after a failed proof: eligible queries that take the fp32 scan directly
 // Nothing is enqueued (and p stays unguarded) when the route does not apply to this engine and query; the caller has
 // already checked the rest: one unsharded fused query with k <= 32 on an unrolled TMA shape.
+// (batch_bf16 and dims % 64 == 0 as for the bf16 nominations, but not whether the bf16 shadow fitted: when it did not,
+// the int8 form still runs on its own shadow, and the bf16 form finds no shadow and leaves the query to the fp32 scan)
 static bool shadow_route_applies(const wax_vs_engine *e) {
     return e->tune.shadow_scan && (e->similarity == WAX_VS_COSINE || e->similarity == WAX_VS_DOT) && !e->debug_trace &&
-           batch_bf16_wanted(e) && e->n_rows * e->dims * sizeof(float) >= e->tune.shadow_scan_min_bytes;
+           e->tune.batch_bf16 != 0 && e->dims % kBatchKBlockBf16 == 0 &&
+           e->n_rows * e->dims * sizeof(float) >= e->tune.shadow_scan_min_bytes;
 }
+// The int8 form of the route (DESIGN 4.1) is taken instead of the bf16 one for fp32 corpora of at least
+// int8_scan_min_bytes whose int8 shadow fits and whose measured bound is no coarser than the bf16 one (rho_max / M <=
+// kBf16Eps: a corpus with outlier dimensions coarsens its rows' scales and keeps the bf16 route, which proves for it).
+// Call with the route applying; builds the int8 shadow when the size rule holds (a corpus found too coarse builds none
+// until its rows are rewritten, see ensure_int8_shadow).  *use: take the int8 form.
+static int32_t int8_route_selected(wax_vs_engine *e, cudaStream_t stream, bool *use) {
+    *use = false;
+    TmaConfig cfg{};
+    if (e->n_rows * e->dims * sizeof(float) < e->tune.int8_scan_min_bytes || !pick_tma_config(e, &cfg, 1, 1)) return WAX_VS_OK;
+    const int32_t rc = ensure_int8_shadow(e, stream);
+    if (rc) return rc;
+    *use = e->int8_valid && e->int8_eps_rel <= kBf16Eps;
+    return WAX_VS_OK;
+}
+
 // Launches 1 and 2 of the route for the query of `p` (the fp32 scan's parameters: query, filter, k, out, ids) in the
-// SHADOW shape `cfg`, over a valid shadow: the SHADOW form writes the kShadowNominees keys to c->d_heaps, the finish
-// re-scores them exactly into p.out and writes its proof flag to c->d_ok.  shape (optional, the read-out
-// wax_vs_debug_shadow_nominations): {C, R, warps, stages, grid, chunk_steps, tail_select} of the SHADOW launch.
+// SHADOW (int8: INT8) shape `cfg`, over a valid shadow: the nominating form writes the kShadowNominees keys to c->d_heaps,
+// the finish re-scores them exactly into p.out and writes its proof flag to c->d_ok.  shape (optional, the read-outs
+// wax_vs_debug_shadow_nominations / wax_vs_debug_int8_nominations): {C, R, warps, stages, grid, chunk_steps, tail_select}
+// of the nominating launch.
 static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const ScanParams &p, const TmaConfig &cfg,
-                                          cudaStream_t stream, uint64_t *launches, uint32_t *shape = nullptr) {
+                                          cudaStream_t stream, uint64_t *launches, uint32_t *shape = nullptr,
+                                          bool int8 = false) {
     int32_t rc;
     if ((rc = c->d_heaps.ensure(static_cast<size_t>(kShadowNominees) * kNomineeStride, "nominee keys")) ||
         (rc = c->d_ok.ensure(1, "proof flags")) || (!p.query && (rc = c->d_queries.ensure(e->dims, "query buffer"))))
         return rc;
 
     ScanParams sp = p;
-    sp.corpus = reinterpret_cast<const float *>(e->d_shadow.p);
+    sp.corpus = int8 ? reinterpret_cast<const float *>(e->d_int8.p) : reinterpret_cast<const float *>(e->d_shadow.p);
+    sp.row_scale = int8 ? e->d_int8_scale.p : nullptr;
     sp.k = kShadowNominees;
     sp.out = nullptr; sp.host_out = nullptr; sp.host_flag = nullptr;
     sp.nominees = c->d_heaps;
     sp.query_store = p.query ? nullptr : c->d_queries.p;
     sp.tail_select = e->tune.tail_select ? 1u : 0u;
-    sp.tail_smem_bytes = static_cast<uint32_t>(static_cast<size_t>(cfg.warps) * cfg.stages * cfg.R * e->dims * sizeof(__nv_bfloat16));
+    sp.tail_smem_bytes = static_cast<uint32_t>(static_cast<size_t>(cfg.warps) * cfg.stages * cfg.R * e->dims *
+                                               (int8 ? 1 : sizeof(__nv_bfloat16)));
     const int grid = tma_grid(e, c, cfg, sp);
-    CUDA_TRY(launch_shadow_scan(e, sp, grid, cfg, e->similarity, stream));
+    if (int8) CUDA_TRY(launch_int8_scan(e, sp, grid, cfg, e->similarity, stream));
+    else CUDA_TRY(launch_shadow_scan(e, sp, grid, cfg, e->similarity, stream));
 
     FinishParams fp{};
     fp.corpus = e->d_corpus; fp.queries = p.query ? p.query : c->d_queries.p;
@@ -756,7 +820,7 @@ static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const 
     fp.heaps = c->d_heaps; fp.max_norm_bits = e->d_max_norm;
     fp.out = p.out; fp.ok = c->d_ok;
     fp.frame_ids = p.frame_ids; fp.id_base = p.id_base; fp.row_offset = p.row_offset;
-    fp.pow2_all = 512; fp.rescore = kShadowRescore; fp.eps_rel = kBf16Eps;
+    fp.pow2_all = 512; fp.rescore = kShadowRescore; fp.eps_rel = int8 ? e->int8_eps_rel : kBf16Eps;
     const size_t fsmem = static_cast<size_t>(fp.pow2_all + fp.rescore) * sizeof(uint64_t);
     const auto kernel = e->similarity == WAX_VS_COSINE ? batch_finish_kernel<kCosine> : batch_finish_kernel<kDot>;
     CUDA_TRY(grant_smem(e, kernel, fsmem));
@@ -774,7 +838,7 @@ static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const 
 static int32_t enqueue_shadow_route(wax_vs_engine *e, SearchCtx *c, ScanParams &p, cudaStream_t stream, uint64_t *launches) {
     if (!shadow_route_applies(e)) return WAX_VS_OK;
     TmaConfig cfg{};
-    if (!pick_tma_config(e, &cfg, 1, sizeof(__nv_bfloat16))) return WAX_VS_OK;
+    if (!pick_tma_config(e, &cfg, 1, sizeof(__nv_bfloat16))) return WAX_VS_OK;   // the unrolled shapes: both forms have them
     int32_t rc;
     if (!c->h_proof_count) {
         if ((rc = c->d_proof_count.ensure(2, "proof counts")) || (rc = c->h_proof_count.ensure(2, "proof count mirror"))) return rc;
@@ -788,9 +852,16 @@ static int32_t enqueue_shadow_route(wax_vs_engine *e, SearchCtx *c, ScanParams &
         if (failed != c->seen_failed) { c->seen_failed = failed; e->shadow_scan_skip = kShadowSkipQueries; }
         if (e->shadow_scan_skip > 0) { --e->shadow_scan_skip; return WAX_VS_OK; }
     }
-    if ((rc = ensure_shadow(e, stream))) return rc;
-    if (!e->shadow_valid) return WAX_VS_OK;
-    if ((rc = enqueue_shadow_nominations(e, c, p, cfg, stream, launches))) return rc;
+    bool int8 = false;
+    if ((rc = int8_route_selected(e, stream, &int8))) return rc;
+    if (int8) {
+        if (!pick_tma_config(e, &cfg, 1, 1)) return WAX_VS_OK;
+    } else {
+        if ((rc = ensure_shadow(e, stream))) return rc;
+        if (!e->shadow_valid) return WAX_VS_OK;
+    }
+    if ((rc = enqueue_shadow_nominations(e, c, p, cfg, stream, launches, nullptr, int8))) return rc;
+    if (int8) { std::lock_guard<std::mutex> pg(e->pool_mu); ++e->single_int8_queries; }
     p.proof_ok = c->d_ok;
     p.proof_count = c->d_proof_count;
     p.proof_count_host = c->h_proof_count;
@@ -1055,6 +1126,93 @@ static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream) {
     CUDA_TRY(cudaStreamSynchronize(stream));
     e->shadow_rows = e->n_rows;
     e->shadow_valid = true;
+    return WAX_VS_OK;
+}
+
+// int8 shadow of the corpus for the single-query route (shadow_int8_kernel; cosine rows pre-scaled by 1/|v| as in the bf16
+// shadow): built lazily, extended by appends (which can only raise rho_max), kept over a remove's untouched prefix, rebuilt
+// after overwrites; the same HBM headroom rule as ensure_shadow.  Returns WAX_VS_OK with e->int8_valid == false when it
+// does not fit (the route then stays on the bf16 shadow; counter "int8_shadow_bytes" = 0).  The build synchronises
+// `stream` and reads rho_max and max|v| back: int8_eps_rel = rho_max / M rounded up (M = 1 for cosine, whose rows are
+// pre-scaled, and max|v| for dot), so that the finish's eps_rel * |q| * M is at least |q| rho_max.
+// Memory: the bf16 shadow comes first.  Unless it already holds the live rows (or was refused), the int8 shadow reserves
+// what ensure_shadow would allocate next to the same free memory -- its capacity size when that fits the headroom rule,
+// else the live rows -- so that it never leaves the bf16 shadow, and with it the route's bf16 form and the batched bf16
+// nominations, less room than they would have without it.
+// A corpus whose bound is too coarse for the route (int8_eps_rel > kBf16Eps: outlier dimensions) gives its int8 shadow
+// back right after the build and builds none again (int8_coarse) until its rows are rewritten: appends can only raise
+// rho_max.  keep_coarse (the read-outs) keeps such a shadow; the route never uses it.
+static int32_t ensure_int8_shadow(wax_vs_engine *e, cudaStream_t stream, bool keep_coarse) {
+    std::lock_guard<std::mutex> g(e->norms_mu);
+    if ((e->int8_valid && e->int8_rows == e->n_rows) || e->int8_unavailable || (e->int8_coarse && !keep_coarse))
+        return WAX_VS_OK;
+    int32_t rc = ensure_norms_locked(e, stream);
+    if (rc) return rc;
+    if ((rc = e->d_int8_rho.ensure(1, "int8 shadow bound"))) return rc;
+    const size_t words = e->dims / 4;
+    const uint64_t need = e->n_rows, pref = std::max<uint64_t>(e->cap_rows, e->n_rows);
+    auto scale_entries = [](uint64_t rows) { return static_cast<size_t>((rows + 15) / 16 * 16); };   // whole steps (R <= 16)
+    if (e->d_int8.cap < need * words || e->d_int8_scale.cap < scale_entries(need)) {
+        e->d_int8.release(); e->d_int8_scale.release();
+        e->int8_rows = 0; e->int8_valid = false;
+        size_t free_b = 0, total_b = 0;
+        uint64_t want = pref;
+        auto bytes_for = [&](uint64_t rows) { return rows * words * sizeof(uint32_t) + scale_entries(rows) * sizeof(float); };
+        const bool info = cudaMemGetInfo(&free_b, &total_b) == cudaSuccess;
+        const size_t headroom = std::max<size_t>(size_t(2) << 30, total_b / 10);
+        size_t reserve = 0;                    // the bf16 shadow's allocation to come (see above)
+        if (batch_bf16_wanted(e) && e->d_shadow.cap < static_cast<size_t>(need) * e->dims) {
+            const size_t b_need = static_cast<size_t>(need) * e->dims * sizeof(__nv_bfloat16);
+            const size_t b_pref = static_cast<size_t>(pref) * e->dims * sizeof(__nv_bfloat16);
+            reserve = free_b >= b_pref + headroom ? b_pref : (free_b >= b_need + headroom ? b_need : 0);
+        }
+        if (info && free_b < bytes_for(want) + reserve + headroom) want = need;
+        // allocated by hand, not through ensure(): running out here is not an error and sets no last error
+        if (!info || free_b < bytes_for(want) + reserve + headroom ||
+            cudaMalloc(&e->d_int8.p, want * words * sizeof(uint32_t)) != cudaSuccess ||
+            cudaMalloc(&e->d_int8_scale.p, scale_entries(want) * sizeof(float)) != cudaSuccess) {
+            cudaGetLastError();
+            e->d_int8.release(); e->d_int8_scale.release();
+            e->int8_unavailable = true;        // stays off until int8_scan_min_bytes is set again
+            return WAX_VS_OK;
+        }
+        e->d_int8.cap = want * words;
+        e->d_int8_scale.cap = scale_entries(want);
+        CUDA_TRY(cudaMemsetAsync(e->d_int8_scale, 0, scale_entries(want) * sizeof(float), stream));   // the step padding
+    }
+    if (e->int8_rows > e->n_rows) e->int8_rows = 0;
+    if (e->int8_rows == 0) CUDA_TRY(cudaMemsetAsync(e->d_int8_rho, 0, sizeof(uint32_t), stream));
+    const uint64_t first = e->int8_rows, count = e->n_rows - first;
+    if (count) {
+        const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 8, (count + 7) / 8));
+        shadow_int8_kernel<<<std::max(grid, 1), 256, 0, stream>>>(e->d_corpus + first * e->dims,
+                                                                  e->similarity == WAX_VS_COSINE ? e->d_inv_norm + first : nullptr,
+                                                                  count, e->dims, e->d_int8 + first * words,
+                                                                  e->d_int8_scale + first, e->d_int8_rho);
+        CUDA_TRY(cudaGetLastError());
+    }
+    uint32_t bits[2] = {0, 0};
+    CUDA_TRY(cudaMemcpyAsync(&bits[0], e->d_int8_rho, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(&bits[1], e->d_max_norm, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));
+    float rho, m;
+    memcpy(&rho, &bits[0], sizeof rho);
+    memcpy(&m, &bits[1], sizeof m);
+    if (e->similarity == WAX_VS_COSINE) m = 1.0f;
+    const float q = rho / m;               // rounded up: one ulp up unless exact
+    e->int8_rho_max = rho;
+    // (a non-finite max|v| leaves the finish no finite bound either way: no int8 route then)
+    e->int8_eps_rel = (std::isfinite(q) && std::isfinite(m) && m > 0.0f)
+                          ? (static_cast<double>(q) * m >= rho ? q : std::nextafter(q, INFINITY)) : INFINITY;
+    e->int8_rows = e->n_rows;
+    e->int8_valid = true;
+    if (e->int8_eps_rel > kBf16Eps) {          // too coarse for the route (above)
+        e->int8_coarse = true;
+        if (!keep_coarse) {                    // nothing holds it: it was not valid for these rows before this call
+            e->d_int8.release(); e->d_int8_scale.release();
+            e->int8_rows = 0; e->int8_valid = false;
+        }
+    }
     return WAX_VS_OK;
 }
 
@@ -1376,6 +1534,10 @@ static int32_t set_capacity(wax_vs_engine *e, uint64_t rows) {
         if (e->d_shadow) {
             e->d_shadow.release(); e->shadow_valid = false; e->shadow_rows = 0;
             e->shadow_unavailable = true;
+        }
+        if (e->d_int8) {                       // likewise the int8 shadow
+            e->d_int8.release(); e->d_int8_scale.release(); e->int8_valid = false; e->int8_rows = 0;
+            e->int8_unavailable = true;
         }
         if (cudaMalloc(&n, bytes) != cudaSuccess)
             return fail(WAX_VS_ERR_CUDA, "Failed to resize vectors buffer (%zu bytes): %s", bytes,
@@ -3789,8 +3951,12 @@ int32_t wax_vs_debug_time_search(wax_vs_engine *e, uint32_t n_queries, int64_t t
         if ((rc = lease2.c->d_out.ensure(static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
     }
     SearchCtx *c2 = lease2.c;
-    // the shadow route's bf16 copy is cached per corpus version: bring it up to date outside the timed region
-    if (shadow_route_applies(e) && (rc = ensure_shadow(e, c->stream))) return rc;
+    // the shadow route's int8 or bf16 copy is cached per corpus version: bring it up to date outside the timed region
+    if (shadow_route_applies(e)) {
+        bool int8 = false;
+        if ((rc = int8_route_selected(e, c->stream, &int8))) return rc;
+        if (!int8 && (rc = ensure_shadow(e, c->stream))) return rc;
+    }
     for (uint32_t it = 0; it < warmup + iters; ++it) {
         if (it == warmup) {
             launches = 0;
@@ -3953,6 +4119,9 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "ingest_d2h_bytes")) *out = e->ingest_d2h_bytes;
     else if (!strcmp(name, "norms_rows")) *out = e->norms_rows;       // rows whose cached 1/|v| is valid
     else if (!strcmp(name, "shadow_rows")) *out = e->shadow_rows;     // rows whose bf16 shadow is valid
+    else if (!strcmp(name, "int8_shadow_bytes")) *out = e->int8_valid ? e->int8_rows * (e->dims + sizeof(float)) : 0;   // codes + scales
+    else if (!strcmp(name, "int8_shadow_rows")) *out = e->int8_rows;  // rows whose int8 shadow is valid
+    else if (!strcmp(name, "single_int8_queries")) *out = e->single_int8_queries;   // single queries nominated from it
     else if (!strcmp(name, "batch_heap_bump")) *out = e->heap_bump;          // sizes above the model's nominee-heap choice (adaptive)
     else if (!strcmp(name, "batch_last_heap")) *out = e->last_heap;          // nominee heap entries of the last bf16 level-1 launch
     else if (!strcmp(name, "single_shadow_queries") || !strcmp(name, "single_shadow_fallbacks")) {
@@ -4066,24 +4235,32 @@ int32_t wax_vs_debug_batch_nominations(wax_vs_engine *e, const float *queries, u
     return WAX_VS_OK;
 }
 
-int32_t wax_vs_debug_shadow_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
-                                        uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
-                                        uint32_t *out_shape) {
+// wax_vs_debug_shadow_nominations (int8 = false) and wax_vs_debug_int8_nominations (int8 = true)
+static int32_t debug_route_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
+                                       uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
+                                       uint32_t *out_shape, bool int8) {
     if (!e || !query || !out_keys || !out_ok || !out_result || !out_shape) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     const uint32_t k_eff = static_cast<uint32_t>(std::min<uint64_t>(clamp_topk(top_k), std::max<uint64_t>(e->n_rows, 1)));
     TmaConfig cfg{};
     if (e->n_rows == 0 || k_eff > 32u || (e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT) ||
-        !batch_bf16_wanted(e) || !pick_tma_config(e, &cfg, 1, sizeof(__nv_bfloat16)))
-        return fail(WAX_VS_ERR_UNSUPPORTED, "no bf16-shadow route for k=%u, dims=%u in this shape", k_eff, e->dims);
+        (int8 ? (e->tune.batch_bf16 == 0 || e->dims % kBatchKBlockBf16 != 0) : !batch_bf16_wanted(e)) ||
+        !pick_tma_config(e, &cfg, 1, int8 ? 1 : sizeof(__nv_bfloat16)))
+        return fail(WAX_VS_ERR_UNSUPPORTED, "no %s-shadow route for k=%u, dims=%u in this shape", int8 ? "int8" : "bf16",
+                    k_eff, e->dims);
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
     CtxLease lease(e);
     int32_t rc = lease.acquire();
     if (rc) return rc;
     SearchCtx *c = lease.c;
-    if ((rc = ensure_shadow(e, c->stream))) return rc;
-    if (!e->shadow_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the bf16 shadow does not fit in device memory");
+    if (int8) {
+        if ((rc = ensure_int8_shadow(e, c->stream, true))) return rc;
+        if (!e->int8_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the int8 shadow does not fit in device memory");
+    } else {
+        if ((rc = ensure_shadow(e, c->stream))) return rc;
+        if (!e->shadow_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the bf16 shadow does not fit in device memory");
+    }
     if ((rc = c->d_out.ensure(k_eff, "result buffer"))) return rc;
     const uint32_t *d_mask = nullptr;
     if (allow_bits) {
@@ -4095,7 +4272,7 @@ int32_t wax_vs_debug_shadow_nominations(wax_vs_engine *e, const float *query, in
     ScanParams p = scan_params(e, c, nullptr, k_eff, 0, c->d_out, nullptr, d_mask);
     if ((rc = place_host_query(e, c, p, query, true, c->stream))) return rc;
     uint64_t launches = 0;
-    if ((rc = enqueue_shadow_nominations(e, c, p, cfg, c->stream, &launches, out_shape))) {
+    if ((rc = enqueue_shadow_nominations(e, c, p, cfg, c->stream, &launches, out_shape, int8))) {
         cudaStreamSynchronize(c->stream);
         return rc;
     }
@@ -4106,6 +4283,41 @@ int32_t wax_vs_debug_shadow_nominations(wax_vs_engine *e, const float *query, in
     CUDA_TRY(cudaMemcpy(out_result, c->d_out, k_eff * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost));
     for (uint32_t i = 0; i < k_eff; ++i)
         if (out_result[i].valid) out_result[i].frame_id = frame_id_of(e, out_result[i].row);
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_debug_shadow_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
+                                        uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
+                                        uint32_t *out_shape) {
+    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, false);
+}
+
+int32_t wax_vs_debug_int8_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
+                                      uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
+                                      uint32_t *out_shape) {
+    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, true);
+}
+
+int32_t wax_vs_debug_read_int8_shadow(wax_vs_engine *e, uint64_t first, uint64_t n, uint8_t *dst_codes, float *dst_scales,
+                                      float *out_rho_max) {
+    if (!e || !dst_codes || !dst_scales || !out_rho_max) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
+    TmaConfig cfg{};
+    if ((e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT) || !pick_tma_config(e, &cfg, 1, 1))
+        return fail(WAX_VS_ERR_UNSUPPORTED, "no int8 shadow for dims=%u with this metric", e->dims);
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
+    if (rc) return rc;
+    if ((rc = ensure_int8_shadow(e, lease.c->stream, true))) return rc;
+    if (!e->int8_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the int8 shadow does not fit in device memory");
+    if (n) {
+        CUDA_TRY(cudaMemcpy(dst_codes, e->d_int8 + first * (e->dims / 4), n * e->dims, cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(dst_scales, e->d_int8_scale + first, n * sizeof(float), cudaMemcpyDeviceToHost));
+    }
+    *out_rho_max = e->int8_rho_max;
     return WAX_VS_OK;
 }
 
@@ -4165,6 +4377,14 @@ int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value
     else if (!strcmp(key, "shadow_warps")) e->tune.shadow_warps = v;
     else if (!strcmp(key, "shadow_stages")) e->tune.shadow_stages = v;
     else if (!strcmp(key, "shadow_scan_min_bytes")) e->tune.shadow_scan_min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
+    else if (!strcmp(key, "int8_scan_min_bytes")) {     // also lets an int8 shadow that did not fit be tried again
+        e->tune.int8_scan_min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
+        e->int8_unavailable = false;
+        e->int8_coarse = false;
+    }
+    else if (!strcmp(key, "int8_rows_per_step")) e->tune.int8_rows_per_step = v;
+    else if (!strcmp(key, "int8_warps")) e->tune.int8_warps = v;
+    else if (!strcmp(key, "int8_stages")) e->tune.int8_stages = v;
     else if (!strcmp(key, "shard_fused")) e->tune.shard_fused = v;
     else if (!strcmp(key, "tail_select")) e->tune.tail_select = v;
     else if (!strcmp(key, "inline_query")) e->tune.inline_query = v;

@@ -75,6 +75,7 @@ struct ScanParams {
                                 // every CTA returns at entry (CTA 0 first delivers `out` to the host), else a plain scan
     uint32_t *proof_count;      // guarded: [0] proofs that held, [1] that failed -- running counts on the device ...
     uint32_t *proof_count_host; // ... mirrored into mapped pinned memory, read by the host without synchronising
+    const float *row_scale;     // INT8: [rows, padded to whole steps] the scale s of each int8 shadow row
 };
 
 // batch_finish_kernel reads entry e of query 0's heap of slice 0 at e * kBatchM (static_assert in waxvs_batch.cuh).
@@ -111,6 +112,16 @@ __device__ __forceinline__ void write_slot(const ScanParams &p, int slot, uint64
 __device__ __forceinline__ float4 bf16x4_to_float4(uint2 u) {
     return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u),
                        __uint_as_float(u.y << 16), __uint_as_float(u.y & 0xFFFF0000u));
+}
+
+// 4 biased int8 (one uint32 of the int8 shadow, byte b = c + 128, element 0 in the low byte) -> fp32 c, exactly: PRMT the
+// byte under the exponent of 2^23 (0x4B0000bb = 2^23 + b), then subtract 2^23 + 128.
+__device__ __forceinline__ float4 int8x4_to_float4(uint32_t u) {
+    constexpr float kBias = 8388736.0f;     // 2^23 + 128
+    return make_float4(__fsub_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7650)), kBias),
+                       __fsub_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7651)), kBias),
+                       __fsub_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7652)), kBias),
+                       __fsub_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7653)), kBias));
 }
 
 // CTA merge + grid merge + output.  Called by every thread of the CTA after the scan loop.
@@ -336,9 +347,15 @@ __device__ __forceinline__ void finish_topk_select(const ScanParams &p, WarpTopK
 //          row, score' = q.v~ for both metrics, key make_key(-score', row) (= nominee_key).  Only the row is rounded,
 //          so kBf16Eps bounds |score' - score|.  Every warp keeps k (= 128) nominees, so the grid's k-th bounds every
 //          row left out; the tails write them for batch_finish_kernel (write_slot).  A non-finite score' counts as +inf.
-template <int C, int R, int METRIC, int E, bool EMIT, bool SHADOW = false>
+//   INT8   (with SHADOW) the nominating pass of the int8-shadow route: p.corpus holds the rows as biased int8 codes c (one
+//          byte per element, ROW_BYTES = 128 C) and p.row_scale each row's scale s.  A lane reads chunk lane + 32c as one
+//          uint32 of 4 codes, widens them exactly (int8x4_to_float4) and FMAs them against the same fp32 query registers;
+//          the row's sum is multiplied once by s: score' = s (q.c).  The R scales of a step ride in the same stage behind
+//          the rows (a second bulk copy on the same mbarrier), so R >= 4 keeps that copy 16-byte aligned.
+template <int C, int R, int METRIC, int E, bool EMIT, bool SHADOW = false, bool INT8 = false>
 __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant__ ScanParams p) {
     static_assert(!SHADOW || (C > 0 && METRIC != kL2 && !EMIT), "the shadow form covers the unrolled cosine / dot shapes");
+    static_assert(!INT8 || (SHADOW && R >= 4), "the int8 form is a shadow form with 16-byte scale copies");
     if constexpr (!SHADOW && !EMIT && E == 1 && METRIC != kL2) {
         if (p.proof_ok) {               // guarded launch after a shadow proof (batch_finish_kernel, same stream; k <= 32)
             const bool proven = *p.proof_ok != 0u;
@@ -357,10 +374,10 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
             if (proven) return;
         }
     }
-    const int D4 = C > 0 ? 32 * C : static_cast<int>(p.dims / 4u);          // float4 (SHADOW: uint2) per row
+    const int D4 = C > 0 ? 32 * C : static_cast<int>(p.dims / 4u);          // float4 (SHADOW: uint2, INT8: uint32) per row
     const int CN = C > 0 ? C : (D4 + 31) / 32;                               // chunks per lane
-    const uint32_t ROW_BYTES = C > 0 ? (SHADOW ? 256u : 512u) * C : p.dims * 4u;
-    const uint32_t STAGE_BYTES = ROW_BYTES * R;
+    const uint32_t ROW_BYTES = C > 0 ? (INT8 ? 128u : SHADOW ? 256u : 512u) * C : p.dims * 4u;
+    const uint32_t STAGE_BYTES = ROW_BYTES * R + (INT8 ? R * 4u : 0u);       // INT8: the step's scales behind its rows
     constexpr int LANES_PER_ROW = 32 / R;
 
     extern __shared__ __align__(128) unsigned char smem[];
@@ -417,12 +434,14 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         const uint32_t rows = min(static_cast<uint32_t>(R), p.n_rows - row0);
         const uint32_t bytes = rows * ROW_BYTES;
         stage_step[s] = step;                        // released to the warp by the mbarrier arrive below
-        mbar_arrive_expect_tx(&bars[s], bytes);
+        mbar_arrive_expect_tx(&bars[s], bytes + (INT8 ? R * 4u : 0u));
         const void *src = SHADOW ? static_cast<const void *>(reinterpret_cast<const unsigned char *>(p.corpus) +
                                                              static_cast<size_t>(row0) * ROW_BYTES)
                                  : static_cast<const void *>(p.corpus + static_cast<size_t>(row0) * p.dims);
         if (p.use_l2_hint) bulk_copy_g2s_hint(ring + s * STAGE_BYTES, src, bytes, &bars[s], policy);
         else bulk_copy_g2s(ring + s * STAGE_BYTES, src, bytes, &bars[s]);
+        // the scale array is padded to whole steps: a ragged last step still copies R scales
+        if constexpr (INT8) bulk_copy_g2s(ring + s * STAGE_BYTES + R * ROW_BYTES, p.row_scale + row0, R * 4u, &bars[s]);
     };
 
     // Step sequence of this warp.  Static: gwarp, gwarp + total_warps, ...  Dynamic (chunk_steps > 0, fused
@@ -470,6 +489,9 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         mbar_wait_parity(&bars[s], parity);
         const uint32_t step = stage_step[s];
         const float4 *tile = reinterpret_cast<const float4 *>(ring + s * STAGE_BYTES);
+        // INT8: the scale of the row this lane finishes after the reduce-scatter, read before the stage is refilled
+        const float row_s = INT8 ? reinterpret_cast<const float *>(ring + s * STAGE_BYTES + R * ROW_BYTES)[lane / LANES_PER_ROW]
+                                 : 1.0f;
 
         float sum0[R], sum1[R];
         if (C == 0) {
@@ -517,7 +539,8 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
 #pragma unroll
             for (int c = 0; c < CN; ++c) {
                 if (C == 0 && lane + 32 * c >= D4) break;   // ragged last chunk (dims % 128 != 0): this lane has no element
-                const float4 v = SHADOW ? bf16x4_to_float4(reinterpret_cast<const uint2 *>(tile)[r * D4 + lane + 32 * c])
+                const float4 v = INT8 ? int8x4_to_float4(reinterpret_cast<const uint32_t *>(tile)[r * D4 + lane + 32 * c])
+                               : SHADOW ? bf16x4_to_float4(reinterpret_cast<const uint2 *>(tile)[r * D4 + lane + 32 * c])
                                         : tile[r * D4 + lane + 32 * c];
                 const float4 qc = qchunk(c);
                 if (METRIC == kL2) {
@@ -553,7 +576,8 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
 
         const uint32_t my_row = step * R + (lane / LANES_PER_ROW);
         float d;
-        if (SHADOW) d = -sum0[0];          // -score': the nominee key's distance
+        if (INT8) d = -__fmul_rn(row_s, sum0[0]);   // -score' = -s (q.c)
+        else if (SHADOW) d = -sum0[0];     // -score': the nominee key's distance
         else if (METRIC == kCosine) d = finish_cos(sum0[0], a2, sqrt_a2, sum1[0]);
         else if (METRIC == kDot) d = finish_dot(sum0[0]);
         else d = finish_l2(sum0[0]);

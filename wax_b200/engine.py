@@ -747,6 +747,14 @@ class CUDAVectorEngine:
         1..127 = the best first), ok (the proof flag), result [(frame_id, score)] of the finish (the search's scores,
         padding dropped) and the launch shape (C, R, warps, stages, grid, chunk_steps, tail_select).  `allow_rows`:
         optional row filter."""
+        return self._route_nominations(L.lib().wax_vs_debug_shadow_nominations, vector, top_k, allow_rows)
+
+    def int8_nominations(self, vector, top_k: int, allow_rows=None):
+        """shadow_nominations for the int8 form of the route (wax_vs_debug_int8_nominations): the INT8 scan nominates
+        from the int8 shadow in the shape the int8_* options select and the finish proves with its measured bound."""
+        return self._route_nominations(L.lib().wax_vs_debug_int8_nominations, vector, top_k, allow_rows)
+
+    def _route_nominations(self, fn, vector, top_k: int, allow_rows):
         q = np.ascontiguousarray(vector, dtype=np.float32).reshape(self.dimensions)
         n = self.count
         k = max(1, min(int(top_k), n))
@@ -760,7 +768,7 @@ class CUDAVectorEngine:
             mask[np.asarray(allow_rows, np.int64)] = True
             bits = (mask.reshape(-1, 32).astype(np.uint64) << np.arange(32, dtype=np.uint64)).sum(1).astype(np.uint32)
         u32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
-        _check(L.lib().wax_vs_debug_shadow_nominations(
+        _check(fn(
             self._h, q.ctypes.data_as(C.POINTER(C.c_float)), int(top_k), None if bits is None else u32(bits),
             keys.ctypes.data_as(C.POINTER(C.c_uint64)), C.byref(ok), result, u32(shape)))
         one = np.float32(1.0)
@@ -775,6 +783,16 @@ class CUDAVectorEngine:
         out = np.empty((n, self.dimensions), np.uint16)
         _check(L.lib().wax_vs_debug_read_shadow(self._h, first, n, out.ctypes.data_as(C.POINTER(C.c_uint16))))
         return out
+
+    def read_int8_shadow(self, first: int, n: int):
+        """The int8 shadow of rows [first, first + n) (wax_vs_debug_read_int8_shadow): (codes [n, dims] uint8 as stored,
+        i.e. code + 128; scales [n] float32; rho_max, the measured bound of the whole shadow)."""
+        codes = np.empty((n, self.dimensions), np.uint8)
+        scales = np.empty(n, np.float32)
+        rho = C.c_float(0.0)
+        _check(L.lib().wax_vs_debug_read_int8_shadow(self._h, first, n, codes.ctypes.data_as(C.POINTER(C.c_uint8)),
+                                                     scales.ctypes.data_as(C.POINTER(C.c_float)), C.byref(rho)))
+        return codes, scales, float(rho.value)
 
     def stream_read_gbs(self, iters: int = 5) -> float:
         """Plain coalesced read of the corpus bytes: the box's streaming-read ceiling in GB/s."""
