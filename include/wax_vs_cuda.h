@@ -420,7 +420,8 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *engine, uint64_t *tensor_queries
    index builds of wax_vs_search_grouped), "attribute_uploads" (device attribute copies of the where searches), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
    (single queries the shadow route answered / that the fp32 scan answered after a failed proof, either shadow; read them
    while no search is running), "single_int8_queries" (single queries whose route nominated from the int8 shadow),
-   "int8_shadow_bytes" / "int8_shadow_rows" (HBM held by the int8 shadow's live rows, codes and scales / rows it covers). */
+   "int8_shadow_bytes" / "int8_shadow_rows" (HBM held by the int8 shadow's live rows, codes and scales / rows it covers),
+   "single_u4_queries", "u4_shadow_bytes" / "u4_shadow_rows" (the same for the 4-bit shadow). */
 int32_t wax_vs_debug_counter(wax_vs_engine *engine, const char *name, uint64_t *out);
 
 /* Device-only timing of the batched path (n_queries synthetic unit queries per step, everything resident):
@@ -479,6 +480,23 @@ int32_t wax_vs_debug_int8_nominations(wax_vs_engine *engine, const float *query,
 int32_t wax_vs_debug_read_int8_shadow(wax_vs_engine *engine, uint64_t first, uint64_t n, uint8_t *dst_codes,
                                       float *dst_scales, float *out_rho_max);
 
+/* The 4-bit form of wax_vs_debug_shadow_nominations: the U4 form of the scan nominates from the 4-bit shadow in the shape
+   the options select (u4_rows_per_step, u4_warps, u4_stages, grid, chunk_steps) and the grid-wide re-score proves --
+   whatever "u4_scan_min_bytes" and the demotion say.  Every CTA of the scan writes its best 256 keys: out_keys takes
+   out_shape[4] * 256 of them (unordered, padding 0xFFFF...; WAX_VS_ERR_BUFFER when keys_cap is smaller), score' =
+   fl(fl(s_q h) (2 sum c_q u - 15 sum c_q)).  out_bound[3] = {rho_max of the shadow, rho_q of this query's int8 coding,
+   tau_excl: the score' no left-out row exceeds, -inf when no row was left out}. */
+int32_t wax_vs_debug_u4_nominations(wax_vs_engine *engine, const float *query, int64_t top_k, const uint32_t *allow_bits,
+                                    uint64_t *out_keys, uint64_t keys_cap, uint32_t *out_ok, wax_vs_candidate *out_result,
+                                    uint32_t *out_shape, float *out_bound);
+
+/* The 4-bit shadow of rows [first, first + n) (brought up to date first): dst_codes[n][dims / 2] the stored bytes (byte b of
+   word w: element 8w + b in the low nibble, 8w + 4 + b in the high one; cosine rows pre-scaled by 1/|v| before coding),
+   dst_half_steps[n] each row's half step h (the row decodes to h (2u - 15)), *out_rho_max the measured bound as for int8.
+   WAX_VS_ERR_UNSUPPORTED as for the int8 read-out. */
+int32_t wax_vs_debug_read_u4_shadow(wax_vs_engine *engine, uint64_t first, uint64_t n, uint8_t *dst_codes,
+                                    float *dst_half_steps, float *out_rho_max);
+
 /* Streaming-read ceiling on the same box: a plain coalesced LDG.128 read of the live corpus bytes, best of
    `iters` (milliseconds, and the bytes read).  Context for the roofline fraction (SURVEY.md section 8d). */
 int32_t wax_vs_debug_stream_read(wax_vs_engine *engine, uint32_t iters, float *out_best_ms, uint64_t *out_bytes);
@@ -494,7 +512,11 @@ int32_t wax_vs_debug_stream_read(wax_vs_engine *engine, uint32_t iters, float *o
    "shadow_rows_per_step" / "shadow_warps" / "shadow_stages" (0 = auto): the shape of its nominating scan;
    "int8_scan_min_bytes" (default 512 MiB): the smallest fp32 corpus whose route nominates from the int8 shadow (when it
    fits and its measured bound is no coarser than the bf16 one); setting it also retries an int8 shadow that did not fit;
-   "int8_rows_per_step" / "int8_warps" / "int8_stages" (0 = auto): the shape of the INT8 nominating scan. */
+   "int8_rows_per_step" / "int8_warps" / "int8_stages" (0 = auto): the shape of the INT8 nominating scan;
+   "u4_scan_min_bytes" (default 2 GiB): the smallest fp32 corpus whose route nominates from the 4-bit shadow (when it
+   fits with a finite bound; a failed 4-bit proof sends the next 16 eligible queries, doubling, to the int8 form); setting
+   it also retries a 4-bit shadow that did not fit and ends a demotion;
+   "u4_rows_per_step" / "u4_warps" / "u4_stages" (0 = auto): the shape of the U4 nominating scan. */
 int32_t wax_vs_debug_set_option(wax_vs_engine *engine, const char *key, int64_t value);
 
 /* Library build info: "waxvs_cuda <version> sm_90a ...". */

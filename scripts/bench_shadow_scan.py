@@ -2,16 +2,17 @@
 """Single-query shadow route against the fp32 scan (DESIGN 4.1) -- companion of bench.py, same conventions:
 device-only times (queries resident in HBM, CUDA events on the launching stream inside the library), one query in
 flight.  In one process and one engine the fp32 scan (option shadow_scan = 0), the route on the bf16 shadow
-(int8_scan_min_bytes out of reach) and the route on the int8 shadow alternate, round by round, so that all three see the
-same clocks and the same HBM.
+(int8_scan_min_bytes out of reach), the route on the int8 shadow (u4_scan_min_bytes out of reach) and the route on the
+4-bit shadow alternate, round by round, so that all four see the same clocks and the same HBM.
 
     python scripts/bench_shadow_scan.py [--rounds 5] [--steps 50] [--out FILE] [--sweep] [--tune]
 
 Reports ms per query of the three arms, their ratios and the spread over the rounds, the fallbacks counted, GB/s over
-the shadow bytes (what a route reads: rows * dims * 2 per query for bf16, rows * (dims + 4) for int8 codes and scales)
+the shadow bytes (what a route reads: rows * dims * 2 per query for bf16, rows * (dims + 4) for int8 codes and scales,
+rows * (dims / 2 + 4) for 4-bit codes and half steps)
 against the same run's plain read of the fp32 corpus (stream_read_gbs), the cost of the first search after
 fill_synthetic and after a remove (the shadow builds then), k = 1 / 10 / 32, 10 M x 768 dot, and with --sweep the corpus
-sizes 10 K .. 10 M that set the size thresholds.  --tune alternates shapes of the INT8 form (rows per step, warps, ring
+sizes 10 K .. 10 M that set the size thresholds.  --tune alternates shapes of the U4 form (rows per step, warps, ring
 depth) on 10 M x 384.
 Prints one JSON line (and writes it to --out)."""
 import argparse
@@ -53,31 +54,35 @@ NO_INT8 = 1 << 62          # int8_scan_min_bytes that keeps every corpus on the 
 
 
 def alternate(eng, k, rounds, steps, int8_min=0):
-    """rounds x (fp32 scan, bf16 route, int8 route), steps device-timed queries each; int8_min: the engine's
-    int8_scan_min_bytes for the int8 arm (the default threshold, or 0 below it)."""
-    arms = {"fp32": [], "bf16": [], "int8": []}
-    seen = {a: [0, 0, 0] for a in arms}           # route queries, fallbacks, int8 nominations
+    """rounds x (fp32 scan, bf16 route, int8 route, 4-bit route), steps device-timed queries each; int8_min: the engine's
+    int8_scan_min_bytes / u4_scan_min_bytes for the int8 and u4 arms (the default threshold, or 0 below it)."""
+    arms = {"fp32": [], "bf16": [], "int8": [], "u4": []}
+    seen = {a: [0, 0, 0] for a in arms}           # route queries, fallbacks, nominations of the arm's own form
     launches = {}
     for _ in range(rounds):
         for arm in arms:
             eng.set_option("shadow_scan", 0 if arm == "fp32" else 1)
             eng.set_option("int8_scan_min_bytes", NO_INT8 if arm == "bf16" else int8_min)
-            (q0, f0), i0 = counts(eng), eng.counter("single_int8_queries")
+            eng.set_option("u4_scan_min_bytes", int8_min if arm == "u4" else NO_INT8)
+            own = "single_u4_queries" if arm == "u4" else "single_int8_queries"
+            (q0, f0), i0 = counts(eng), eng.counter(own)
             ms, launches[arm] = per_query_ms(eng, k, steps)
-            (q1, f1), i1 = counts(eng), eng.counter("single_int8_queries")
+            (q1, f1), i1 = counts(eng), eng.counter(own)
             arms[arm].append(ms)
             seen[arm] = [seen[arm][0] + q1 - q0, seen[arm][1] + f1 - f0, seen[arm][2] + i1 - i0]
     eng.set_option("shadow_scan", 1)
     eng.set_option("int8_scan_min_bytes", int8_min)
+    eng.set_option("u4_scan_min_bytes", int8_min)
     med = {a: float(np.median(t)) for a, t in arms.items()}
     out = {"k": k, "fp32_ms": med["fp32"], "bf16_ms": med["bf16"], "int8_ms": med["int8"],
-           "int8_vs_bf16": med["bf16"] / med["int8"], "int8_vs_fp32": med["fp32"] / med["int8"]}
+           "u4_ms": med["u4"], "int8_vs_bf16": med["bf16"] / med["int8"], "int8_vs_fp32": med["fp32"] / med["int8"],
+           "u4_vs_int8": med["int8"] / med["u4"]}
     for a, t in arms.items():
         out[f"{a}_ms_rounds"] = t
         out[f"{a}_spread_pct"] = (max(t) - min(t)) / med[a] * 100
         out[f"{a}_launches_per_query"] = launches[a]
-    for a in ("bf16", "int8"):
-        out[f"{a}_route_queries"], out[f"{a}_fallbacks"], out[f"{a}_int8_nominations"] = seen[a]
+    for a in ("bf16", "int8", "u4"):
+        out[f"{a}_route_queries"], out[f"{a}_fallbacks"], out[f"{a}_{'u4' if a == 'u4' else 'int8'}_nominations"] = seen[a]
     return out
 
 
@@ -104,6 +109,8 @@ def headline(args):
     out["bf16_gbs_on_shadow_bytes"] = rows * dims * 2 / (r10["bf16_ms"] * 1e-3) / 1e9
     out["int8_gbs_on_shadow_bytes"] = rows * (dims + 4) / (r10["int8_ms"] * 1e-3) / 1e9     # codes + scales
     out["int8_frac_of_stream_read"] = out["int8_gbs_on_shadow_bytes"] / read
+    out["u4_gbs_on_shadow_bytes"] = rows * (dims // 2 + 4) / (r10["u4_ms"] * 1e-3) / 1e9    # codes + half steps
+    out["u4_frac_of_stream_read"] = out["u4_gbs_on_shadow_bytes"] / read
     out["fp32_gbs_on_corpus_bytes"] = rows * dims * 4 / (r10["fp32_ms"] * 1e-3) / 1e9
     eng.remove(123)
     out["first_search_after_remove_ms"] = first_search_ms(eng, dims, 3)        # shadow rebuild
@@ -115,10 +122,10 @@ def headline(args):
 
 
 def tune(eng, args):
-    """Shapes of the INT8 form (its own options: the guarded fp32 scan keeps its shape), alternated round by round;
+    """Shapes of the U4 form (its own options: the guarded fp32 scan keeps its shape), alternated round by round;
     0 = the engine's default."""
-    shapes = [(0, 0, 0), (8, 16, 2), (8, 16, 4), (8, 12, 3), (16, 16, 2), (16, 8, 3), (4, 16, 3), (4, 16, 4)]
-    cands = [dict(int8_rows_per_step=r, int8_warps=w, int8_stages=s) for r, w, s in shapes]
+    shapes = [(0, 0, 0), (16, 16, 2), (16, 16, 4), (16, 12, 4), (16, 8, 6), (8, 16, 3), (8, 16, 4), (8, 16, 6)]
+    cands = [dict(u4_rows_per_step=r, u4_warps=w, u4_stages=s) for r, w, s in shapes]
     times, proven, failed = [[] for _ in cands], [0] * len(cands), [0] * len(cands)
     for _ in range(args.rounds):
         for i, c in enumerate(cands):
@@ -156,7 +163,9 @@ def sweep(args):
         r = alternate(eng, 10, args.rounds, args.steps, int8_min=0)
         res.append({"rows": rows, "fp32_mb": rows * 384 * 4 / 2**20, "fp32_ms": r["fp32_ms"], "bf16_ms": r["bf16_ms"],
                     "int8_ms": r["int8_ms"], "int8_vs_bf16": r["int8_vs_bf16"], "int8_vs_fp32": r["int8_vs_fp32"],
-                    "int8_fallbacks": r["int8_fallbacks"], "int8_nominations": r["int8_int8_nominations"]})
+                    "int8_fallbacks": r["int8_fallbacks"], "int8_nominations": r["int8_int8_nominations"],
+                    "u4_ms": r["u4_ms"], "u4_vs_int8": r["u4_vs_int8"], "u4_fallbacks": r["u4_fallbacks"],
+                    "u4_nominations": r["u4_u4_nominations"]})
         eng.close()
     return res
 

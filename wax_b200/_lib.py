@@ -110,6 +110,9 @@ SIGNATURES = {
     "wax_vs_debug_int8_nominations": (C.c_int32, [_eng, _f32p, C.c_int64, _u32p, _u64p, _u32p, C.POINTER(Candidate),
                                                   _u32p]),
     "wax_vs_debug_read_int8_shadow": (C.c_int32, [_eng, C.c_uint64, C.c_uint64, _u8p, _f32p, _f32p]),
+    "wax_vs_debug_u4_nominations": (C.c_int32, [_eng, _f32p, C.c_int64, _u32p, _u64p, C.c_uint64, _u32p,
+                                                C.POINTER(Candidate), _u32p, _f32p]),
+    "wax_vs_debug_read_u4_shadow": (C.c_int32, [_eng, C.c_uint64, C.c_uint64, _u8p, _f32p, _f32p]),
     "wax_vs_debug_stream_read": (C.c_int32, [_eng, C.c_uint32, _f32p, _u64p]),
     "wax_vs_debug_set_option": (C.c_int32, [_eng, C.c_char_p, C.c_int64]),
     "wax_vs_version": (C.c_char_p, []),

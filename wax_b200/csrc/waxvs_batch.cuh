@@ -376,6 +376,63 @@ __global__ void __launch_bounds__(256) shadow_int8_kernel(const float *__restric
     if (lane == 0 && local_max) atomicMax(rho_max_bits, local_max);
 }
 
+// ---- 4-bit shadow of the corpus (the single-query route, DESIGN 4.1; cached like the int8 one) ---------------------------
+// One warp per row, v^ as for the int8 shadow.  Sixteen mid-rise levels: h = fl(max |v^_i| / 16) is half a step, u_i =
+// clamp(floor(v^_i / 2h) + 8, 0, 15) and the row decodes to h (2 u_i - 15) (u_i = 8 when h == 0 or the row is not finite).
+// Two codes per byte in the order the scan's dp4a pair wants: byte b of word w holds element 8w + b in its low nibble and
+// element 8w + 4 + b in its high one.  half_step[row] = h.  The bound is measured from what was stored, as for int8: rho =
+// ||v^ - h (2u - 15)||_2 in fp64, rounded up; +inf for a non-finite row; *rho_max_bits raised once per warp.
+__global__ void __launch_bounds__(256) shadow_u4_kernel(const float *__restrict__ src, const float *__restrict__ scale_in,
+                                                        uint64_t n_rows, uint32_t dims, uint32_t *__restrict__ dst,
+                                                        float *__restrict__ half_step, uint32_t *rho_max_bits) {
+    const int lane = threadIdx.x & 31;
+    const uint64_t warps = (static_cast<uint64_t>(gridDim.x) * blockDim.x) >> 5;
+    const uint32_t d4 = dims >> 2, cn = d4 / 32u;
+    uint32_t local_max = 0;
+    for (uint64_t row = (static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; row < n_rows; row += warps) {
+        const float4 *v4 = reinterpret_cast<const float4 *>(src) + row * d4;
+        const float w = scale_in ? __ldg(scale_in + row) : 1.0f;
+        float4 x[kInt8MaxChunks];
+        float m = 0.0f;
+        bool bad = false;
+#pragma unroll
+        for (uint32_t c = 0; c < kInt8MaxChunks; ++c) {
+            if (c >= cn) break;
+            x[c] = __ldcs(v4 + lane + 32u * c);
+            if (scale_in) { x[c].x *= w; x[c].y *= w; x[c].z *= w; x[c].w *= w; }
+            bad |= !finite_f32(x[c].x) || !finite_f32(x[c].y) || !finite_f32(x[c].z) || !finite_f32(x[c].w);
+            m = fmaxf(m, fmaxf(fmaxf(fabsf(x[c].x), fabsf(x[c].y)), fmaxf(fabsf(x[c].z), fabsf(x[c].w))));
+        }
+        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(WAXVS_FULL_MASK, m, o));
+        bad = __any_sync(WAXVS_FULL_MASK, bad);
+        const float h = __fdiv_rn(m, 16.0f), step = __fmul_rn(2.0f, h);
+        double r2 = 0.0;
+#pragma unroll
+        for (uint32_t c = 0; c < kInt8MaxChunks; ++c) {
+            if (c >= cn) break;
+            const float xs[4] = {x[c].x, x[c].y, x[c].z, x[c].w};
+            uint32_t nibbles = 0;                        // this float4's codes, one per byte
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                int u = 8;
+                if (h > 0.0f && !bad) u = max(0, min(15, __float2int_rd(__fdiv_rn(xs[j], step)) + 8));
+                nibbles |= static_cast<uint32_t>(u) << (8 * j);
+                const double e = static_cast<double>(xs[j]) - static_cast<double>(h) * static_cast<double>(2 * u - 15);
+                r2 = fma(e, e, r2);
+            }
+            // float4 2w (an even lane) gives word w its low nibbles, float4 2w + 1 (the next lane) its high ones
+            const uint32_t high = __shfl_down_sync(WAXVS_FULL_MASK, nibbles, 1);
+            if ((lane & 1) == 0) dst[row * (d4 / 2u) + (lane >> 1) + 16u * c] = nibbles | (high << 4);
+        }
+        for (int o = 16; o > 0; o >>= 1) r2 += __shfl_xor_sync(WAXVS_FULL_MASK, r2, o);
+        float rho = __double2float_ru(sqrt(r2) * (1.0 + 0x1p-40));
+        if (bad || !finite_f32(h) || !finite_f32(rho)) rho = INFINITY;
+        if (lane == 0) half_step[row] = h;
+        local_max = max(local_max, __float_as_uint(rho));
+    }
+    if (lane == 0 && local_max) atomicMax(rho_max_bits, local_max);
+}
+
 // ---- the tensor-core kernel ---------------------------------------------------------------------------------------
 // BF16: operands are bf16 (the corpus shadow + converted queries; 64 elements per 128-byte k-block, wgmma k16 at twice
 //       the TF32 rate for the same bytes) -- nominations only, exactness comes from the finish kernel.
@@ -1069,6 +1126,110 @@ __global__ void __launch_bounds__(512, 2) batch_finish_kernel(const FinishParams
     sp.frame_ids = p.frame_ids; sp.id_base = p.id_base; sp.row_offset = p.row_offset;
     for (uint32_t i = threadIdx.x; i < p.k; i += blockDim.x)
         write_candidate(sp, static_cast<int>(i), i < p.rescore ? ek[i] : WAXVS_KEY_NONE);
+}
+
+// ---- the 4-bit route's exact re-score + proof, on the whole grid ----------------------------------------------------------
+// The U4 scan leaves kU4CtaNominees nominees per CTA -- thousands, where batch_finish_kernel's single CTA re-scores at
+// most kBatchRescoreMax: the 4-bit bound is sixteen times the int8 one.  One warp per nominee, four at a time, distances in
+// the scan's own order (exact_row_distance_x4: the fp32 scan's bits); every warp keeps the k best exact keys and the
+// scan's selection tail reduces them to p.out.  The CTA that finishes it proves what batch_finish_kernel proves for
+// cosine / dot: every row left out has score' <= tau (p.aux[0], see finish_u4_nominees), and
+//   |q.v^ - score'| <= |q| rho_max + rho_q (|v^| + rho_max)        (row coding, then query coding; DESIGN 4.1)
+// plus the two roundings of score' (under acc_slack), so the answer is exact when the exact k-th score exceeds
+// tau + that bound + the finish's slacks.  It then resets p.aux[0] for the next query.
+struct RescoreParams {
+    const float *corpus, *query;
+    uint32_t dims, k, n_nominees;
+    const uint64_t *nominees;
+    uint32_t *aux;                  // ScanParams::u4_aux, and [2]: the cut word this launch proved with
+    const uint32_t *max_norm_bits;
+    float rho_max;
+    uint64_t *block_keys;           // [grid][k] scratch
+    uint32_t *ticket;               // zero on entry, zero again on exit
+    uint32_t *work_counter;         // the U4 scan's claim counter (its tail has no last CTA): reset here for the next scan
+    wax_vs_candidate *out;          // [k]
+    uint32_t *ok;                   // 1 = proven exact, 0 = the fp32 scan must answer
+    const uint64_t *frame_ids;
+    uint64_t id_base, row_offset;
+    uint32_t tail_smem_bytes;
+};
+
+template <int METRIC>
+__global__ void __launch_bounds__(512, 1) shadow_rescore_kernel(const RescoreParams p) {
+    static_assert(METRIC == kCosine || METRIC == kDot, "the shadow route covers cosine and dot");
+    extern __shared__ __align__(16) unsigned char rsm[];
+    __shared__ float s_a2, s_sqrt_a2;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, warps = blockDim.x >> 5;
+    const int k = static_cast<int>(p.k);
+    if (warp == 0) {  // |q|^2 in the kernels' order
+        float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+        for (uint32_t base = 4u * lane; base < p.dims; base += 128u) {
+            const float4 x = __ldg(reinterpret_cast<const float4 *>(p.query + base));
+            s0 = __fmaf_rn(x.x, x.x, s0); s1 = __fmaf_rn(x.y, x.y, s1);
+            s2 = __fmaf_rn(x.z, x.z, s2); s3 = __fmaf_rn(x.w, x.w, s3);
+        }
+        const float a2 = warp_butterfly_sum(__fadd_rn(__fadd_rn(s0, s1), __fadd_rn(s2, s3)));
+        if (lane == 0) { s_a2 = a2; s_sqrt_a2 = __fsqrt_rn(a2); }
+    }
+    // the tail's parameters, in shared memory: a per-thread ScanParams would live in local memory (its inline query)
+    __shared__ ScanParams sp;
+    for (uint32_t i = threadIdx.x; i < sizeof(ScanParams) / 4u; i += blockDim.x) reinterpret_cast<uint32_t *>(&sp)[i] = 0u;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        sp.k = p.k; sp.block_keys = p.block_keys; sp.ticket = p.ticket; sp.out = p.out;
+        sp.frame_ids = p.frame_ids; sp.id_base = p.id_base; sp.row_offset = p.row_offset;
+        sp.tail_smem_bytes = p.tail_smem_bytes; sp.work_counter = p.work_counter;
+    }
+    __syncthreads();
+
+    WarpTopK<1> tk;
+    tk.init();
+    const uint32_t stride = gridDim.x * warps * 4u;
+    for (uint32_t i0 = (blockIdx.x * warps + warp) * 4u; i0 < p.n_nominees; i0 += stride) {   // warp-uniform
+        uint64_t nk[4];
+        const float *vp[4];
+        float d[4];
+#pragma unroll
+        for (uint32_t r = 0; r < 4; ++r) {
+            nk[r] = i0 + r < p.n_nominees ? p.nominees[i0 + r] : WAXVS_KEY_NONE;
+            vp[r] = p.corpus + static_cast<size_t>(nk[r] == WAXVS_KEY_NONE ? 0u : static_cast<uint32_t>(nk[r])) * p.dims;
+        }
+        exact_row_distance_x4<METRIC>(p.query, vp, p.dims, s_a2, s_sqrt_a2, lane, d);
+#pragma unroll
+        for (uint32_t r = 0; r < 4; ++r) {
+            if (nk[r] == WAXVS_KEY_NONE || !finite_f32(d[r])) continue;
+            const uint64_t x = make_key(d[r], static_cast<uint32_t>(nk[r]));
+            if (x < tk.thresh) tk.insert(x, lane, k);
+        }
+    }
+
+    if (!finish_topk_select<1>(sp, tk, rsm)) return;
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    const wax_vs_candidate kth = p.out[p.k - 1];
+    const uint32_t cut = p.aux[0];
+    const bool excluded_any = cut != WAXVS_UKEY_NONE;
+    const float tau = excluded_any ? -from_orderable_u32(cut) : -INFINITY;
+    const float rho_q = __uint_as_float(p.aux[1]);
+    uint32_t ok = 1;
+    if (kth.valid) {
+        const float dk = kth.distance, qn = s_sqrt_a2;
+        const float m = METRIC == kCosine ? 1.0f : __uint_as_float(*p.max_norm_bits);
+        const float scale = qn * m;
+        const float sk_exact = METRIC == kCosine ? (1.0f - dk) * qn : 1.0f - dk;
+        // |v^| <= 1.0001 for a cosine row (each element rounded twice), max|v| for dot
+        const float coding = qn * p.rho_max + rho_q * ((METRIC == kCosine ? 1.0001f : m) + p.rho_max);
+        const float acc_slack = static_cast<float>(p.dims) * 0x1p-23f * scale;      // as in batch_finish_kernel
+        const float ulp_slack = 0x1p-21f * fmaxf(1.0f, fabsf(dk)) * (METRIC == kCosine ? qn : 1.0f);
+        const float eps = coding * 1.01f + acc_slack + ulp_slack + 1e-30f;
+        if (excluded_any && (!(sk_exact > tau + eps) || !finite_f32(eps))) ok = 0;
+    } else if (excluded_any) {
+        ok = 0;
+    }
+    if (!(s_a2 >= 0x1p-126f) || !finite_f32(s_a2)) ok = 0;      // as in batch_finish_kernel: no bound from such a |q|
+    *p.ok = ok;
+    p.aux[0] = WAXVS_UKEY_NONE;
+    p.aux[2] = cut;                 // for wax_vs_debug_u4_nominations
 }
 
 // ---- filter level (level 2): exact re-score of EVERY candidate above the fixed threshold, then top-k ------------------

@@ -197,6 +197,11 @@ struct Tuning {
                                                    // one) for fp32 corpora of at least this many bytes whose measured int8
                                                    // bound is no coarser than the bf16 one (DESIGN 4.1, 5)
     int int8_rows_per_step = 0, int8_warps = 0, int8_stages = 0;   // shape of the INT8 form (0 auto)
+    uint64_t u4_scan_min_bytes = 2048ull << 20;    // ... and from the 4-bit shadow (half the bytes again) for fp32 corpora
+                                                   // of at least this many bytes, while its proofs hold (DESIGN 4.1, 5):
+                                                   // its re-score of thousands of nominees is a fixed cost, measured only
+                                                   // at 15 GB, so corpora of a GB or two stay on the int8 form
+    int u4_rows_per_step = 0, u4_warps = 0, u4_stages = 0;   // shape of the U4 form (0 auto)
 };
 
 // Per-search scratch: the analogue of TransientBuffers (MetalVectorEngine.swift:36-41, :84-117).
@@ -257,6 +262,9 @@ struct SearchCtx {
     DevBuf<uint32_t> d_proof_count;                // shadow route: [0] proofs that held, [1] that failed (guarded scan) ...
     PinnedBuf<uint32_t> h_proof_count;             // ... and their mapped host mirror
     uint32_t seen_failed = 0;                      // h_proof_count[1] when the host last looked
+    bool last_u4 = false;                          // the last route query enqueued here nominated from the 4-bit shadow
+    DevBuf<uint32_t> d_u4_aux;                     // 4-bit route: [0] cut key of the rows left out, [1] rho_q (ScanParams::u4_aux),
+                                                   // [2] the cut key the last re-score proved with (read-out)
     ~SearchCtx() {                                 // the buffers release themselves
         if (ev0) cudaEventDestroy(ev0);
         if (ev1) cudaEventDestroy(ev1);
@@ -309,15 +317,31 @@ struct wax_vs_engine {
     // int8 shadow of the corpus for the single-query route only (DESIGN 4.1; same cache rules, guarded by norms_mu): four
     // biased codes per word, one scale per row (padded to whole scan steps) and the measured bound rho_max (fp32 bits on
     // the device; read back once per build together with max|v|, giving the bound the finish uses)
-    DevBuf<uint32_t> d_int8;
-    DevBuf<float> d_int8_scale;
-    DevBuf<uint32_t> d_int8_rho;
-    uint64_t int8_rows = 0;        // rows [0, int8_rows) are valid; int8_valid = covers every live row
-    bool int8_valid = false, int8_unavailable = false;
-    bool int8_coarse = false;      // the last build measured a bound too coarse for the route: none is built again until
-                                   // the rows are rewritten (invalidate_row_caches with no prefix) or int8_scan_min_bytes is set
-    float int8_rho_max = 0.0f, int8_eps_rel = INFINITY;   // rho_max, and rho_max / M rounded up (M = 1 cosine, max|v| dot)
+    struct CodedShadow {
+        uint32_t bits = 8;             // per code: 8 (shadow_int8_kernel) or 4 (shadow_u4_kernel)
+        DevBuf<uint32_t> codes;
+        DevBuf<float> scale;
+        DevBuf<uint32_t> rho;
+        uint64_t rows = 0;             // rows [0, rows) are valid; valid = covers every live row
+        bool valid = false, unavailable = false;
+        bool coarse = false;           // the last build measured a bound too coarse for the route: none is built again until
+                                       // the rows are rewritten (invalidate_row_caches with no prefix) or its min_bytes option is set
+        float rho_max = 0.0f, eps_rel = INFINITY;   // rho_max, and rho_max / M rounded up (M = 1 cosine, max|v| dot)
+        void release() { codes.release(); scale.release(); rows = 0; valid = false; }
+        void invalidate(uint64_t keep_prefix) {     // a kept prefix keeps rho_max too: still an upper bound
+            rows = std::min(rows, keep_prefix);
+            valid = false;
+            if (keep_prefix == 0) coarse = false;
+        }
+    } i8, u4{4};
+    // The 4-bit shadow of the same route (16 levels, eight codes per word, one half step per row), same record and rules;
+    // its bound is 16 times the int8 one, so whether its nominees prove depends on the scores: a failed 4-bit proof sends
+    // the next u4_demote_window eligible queries to the int8 form (u4_demoted counts them down), and the window doubles
+    // when the first 4-bit query after it fails again.
+    uint32_t u4_demoted = 0, u4_demote_window = 16;
+    bool u4_probing = false;                              // the next 4-bit proof decides whether the window doubles
     uint64_t single_int8_queries = 0;                     // single queries nominated from the int8 shadow (pool_mu)
+    uint64_t single_u4_queries = 0;                       // ... from the 4-bit shadow (pool_mu)
     uint64_t batch_tensor_queries = 0, batch_fallback_queries = 0;   // instrumentation
     uint64_t batch_bf16_queries = 0, batch_retry_queries = 0, batch_tf32_queries = 0, batch_filter_bf16_queries = 0;
     uint64_t filter_bitset_passes = 0;
@@ -413,9 +437,8 @@ static void invalidate_row_caches(wax_vs_engine *e, uint64_t keep_prefix) {
     e->norms_rows = std::min(e->norms_rows, keep_prefix);
     e->shadow_rows = std::min(e->shadow_rows, keep_prefix);
     if (e->shadow_rows == 0) e->shadow_valid = false;
-    e->int8_rows = std::min(e->int8_rows, keep_prefix);   // a kept prefix keeps rho_max too: still an upper bound
-    e->int8_valid = false;
-    if (keep_prefix == 0) e->int8_coarse = false;
+    e->i8.invalidate(keep_prefix);
+    e->u4.invalidate(keep_prefix);
     e->gindex.valid = false;           // appends too: the new rows need index entries
     e->attrs_dev_valid = false;        // likewise the attribute mirror
 }
@@ -582,11 +605,11 @@ static cudaError_t grant_smem(wax_vs_engine *e, K kernel, size_t bytes) {
     return err;
 }
 
-template <int C, int R, int M, int E, bool EMIT, bool SHADOW = false, bool INT8 = false>
+template <int C, int R, int M, int E, bool EMIT, bool SHADOW = false, bool INT8 = false, bool U4 = false>
 static cudaError_t launch_tma_inst(wax_vs_engine *e, const ScanParams &p, int grid, const TmaConfig &cfg, cudaStream_t s) {
-    cudaError_t err = grant_smem(e, scan_tma_kernel<C, R, M, E, EMIT, SHADOW, INT8>, cfg.smem);
+    cudaError_t err = grant_smem(e, scan_tma_kernel<C, R, M, E, EMIT, SHADOW, INT8, U4>, cfg.smem);
     if (err != cudaSuccess) return err;
-    scan_tma_kernel<C, R, M, E, EMIT, SHADOW, INT8><<<grid, cfg.warps * 32, cfg.smem, s>>>(p);
+    scan_tma_kernel<C, R, M, E, EMIT, SHADOW, INT8, U4><<<grid, cfg.warps * 32, cfg.smem, s>>>(p);
     return cudaGetLastError();
 }
 // mode: 0 = fused list k <= 32, 1 = fused list k <= 128, 2 = emit distance keys
@@ -639,6 +662,28 @@ static cudaError_t launch_int8_scan(wax_vs_engine *e, const ScanParams &p, int g
     WAXVS_CASE(1, 8); WAXVS_CASE(1, 16); WAXVS_CASE(2, 8); WAXVS_CASE(2, 16);
     WAXVS_CASE(3, 4); WAXVS_CASE(3, 8); WAXVS_CASE(3, 16); WAXVS_CASE(4, 4); WAXVS_CASE(4, 8);
     WAXVS_CASE(6, 4); WAXVS_CASE(6, 8); WAXVS_CASE(8, 4); WAXVS_CASE(12, 4);
+#undef WAXVS_CASE
+    return cudaErrorInvalidValue;
+}
+// The U4 form (nominating pass of the 4-bit-shadow route): steps of ~3 KB (16 rows at 384 dims), 16 warps, 3 stages unless
+// the u4_* options say otherwise; launch_u4_scan has rows per step r_lo .. r_hi.
+static bool pick_u4_config(const wax_vs_engine *e, TmaConfig *cfg) {
+    if (!pick_tma_config(e, cfg, 1, 1)) return false;           // the unrolled shapes, as for the INT8 form
+    const int C = cfg->C, want_r = e->tune.u4_rows_per_step;
+    const int r_hi = C <= 3 ? 16 : (C <= 6 ? 8 : 4), r_lo = C <= 3 ? 8 : 4;
+    cfg->R = (want_r >= r_lo && want_r <= r_hi && (want_r & (want_r - 1)) == 0) ? want_r : r_hi;
+    cfg->stages = e->tune.u4_stages > 0 ? e->tune.u4_stages : 3;
+    cfg->warps = std::max(1, std::min(16, e->tune.u4_warps ? e->tune.u4_warps : 16));
+    const size_t stage_bytes = static_cast<size_t>(cfg->R) * (e->dims / 2 + 4);     // codes + half steps
+    cfg->smem = static_cast<size_t>(cfg->warps) * cfg->stages * (stage_bytes + 8 + 4) + static_cast<size_t>(cfg->warps) * 1024 + 16;
+    return cfg->smem <= (e->smem_optin ? e->smem_optin : 232448) - 4096;
+}
+// score' does not depend on the metric (cosine rows are pre-scaled in the shadow): one instantiation serves both.
+static cudaError_t launch_u4_scan(wax_vs_engine *e, const ScanParams &p, int grid, const TmaConfig &cfg, cudaStream_t s) {
+#define WAXVS_CASE(Cv, Rv) \
+    if (cfg.C == Cv && cfg.R == Rv) return launch_tma_inst<Cv, Rv, kDot, 4, false, true, false, true>(e, p, grid, cfg, s)
+    WAXVS_CASE(1, 8); WAXVS_CASE(1, 16); WAXVS_CASE(2, 8); WAXVS_CASE(2, 16); WAXVS_CASE(3, 8); WAXVS_CASE(3, 16);
+    WAXVS_CASE(4, 4); WAXVS_CASE(4, 8); WAXVS_CASE(6, 4); WAXVS_CASE(6, 8); WAXVS_CASE(8, 4); WAXVS_CASE(12, 4);
 #undef WAXVS_CASE
     return cudaErrorInvalidValue;
 }
@@ -751,7 +796,7 @@ static int tma_grid(const wax_vs_engine *e, const SearchCtx *c, const TmaConfig 
 
 static bool batch_bf16_wanted(const wax_vs_engine *e);
 static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream);
-static int32_t ensure_int8_shadow(wax_vs_engine *e, cudaStream_t stream, bool keep_coarse = false);
+static int32_t ensure_coded_shadow(wax_vs_engine *e, wax_vs_engine::CodedShadow &cs, cudaStream_t stream, bool keep_coarse = false);
 
 // ---- the bf16-shadow route of a single query (DESIGN 4.1) ----
 // The fp32 scan reads dims * 4 bytes per row and runs at the HBM read ceiling; the shadow holds the same rows in bf16.
@@ -775,14 +820,32 @@ static bool shadow_route_applies(const wax_vs_engine *e) {
 // int8_scan_min_bytes whose int8 shadow fits and whose measured bound is no coarser than the bf16 one (rho_max / M <=
 // kBf16Eps: a corpus with outlier dimensions coarsens its rows' scales and keeps the bf16 route, which proves for it).
 // Call with the route applying; builds the int8 shadow when the size rule holds (a corpus found too coarse builds none
-// until its rows are rewritten, see ensure_int8_shadow).  *use: take the int8 form.
+// until its rows are rewritten, see ensure_coded_shadow).  *use: take the int8 form.
 static int32_t int8_route_selected(wax_vs_engine *e, cudaStream_t stream, bool *use) {
     *use = false;
     TmaConfig cfg{};
     if (e->n_rows * e->dims * sizeof(float) < e->tune.int8_scan_min_bytes || !pick_tma_config(e, &cfg, 1, 1)) return WAX_VS_OK;
-    const int32_t rc = ensure_int8_shadow(e, stream);
+    const int32_t rc = ensure_coded_shadow(e, e->i8, stream);
     if (rc) return rc;
-    *use = e->int8_valid && e->int8_eps_rel <= kBf16Eps;
+    *use = e->i8.valid && e->i8.eps_rel <= kBf16Eps;
+    return WAX_VS_OK;
+}
+// The form the route takes for the next query, from what the engine observes: the 4-bit form for fp32 corpora of at least
+// u4_scan_min_bytes whose 4-bit shadow fits with a finite bound, unless a failed 4-bit proof has demoted the route
+// (`demoted`: the caller's reading of u4_demoted); else the int8 form by int8_route_selected; else the bf16 form.  Each is
+// the fastest form that proves on some corpus.  Builds the shadow of the form it selects, and no other.
+enum class RouteForm { kBf16, kInt8, kU4 };
+static int32_t select_route_form(wax_vs_engine *e, cudaStream_t stream, bool demoted, RouteForm *form) {
+    *form = RouteForm::kBf16;
+    TmaConfig cfg{};
+    int32_t rc;
+    if (!demoted && e->n_rows * e->dims * sizeof(float) >= e->tune.u4_scan_min_bytes && pick_u4_config(e, &cfg)) {
+        if ((rc = ensure_coded_shadow(e, e->u4, stream))) return rc;
+        if (e->u4.valid && std::isfinite(e->u4.eps_rel)) { *form = RouteForm::kU4; return WAX_VS_OK; }
+    }
+    bool int8 = false;
+    if ((rc = int8_route_selected(e, stream, &int8))) return rc;
+    if (int8) *form = RouteForm::kInt8;
     return WAX_VS_OK;
 }
 
@@ -793,15 +856,24 @@ static int32_t int8_route_selected(wax_vs_engine *e, cudaStream_t stream, bool *
 // of the nominating launch.
 static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const ScanParams &p, const TmaConfig &cfg,
                                           cudaStream_t stream, uint64_t *launches, uint32_t *shape = nullptr,
-                                          bool int8 = false) {
+                                          RouteForm form = RouteForm::kBf16) {
+    const bool int8 = form == RouteForm::kInt8, u4 = form == RouteForm::kU4;
     int32_t rc;
-    if ((rc = c->d_heaps.ensure(static_cast<size_t>(kShadowNominees) * kNomineeStride, "nominee keys")) ||
+    if (u4 && !c->d_u4_aux) {           // the cut word starts at "nothing cut"; every re-score leaves it so
+        if ((rc = c->d_u4_aux.ensure(3, "4-bit route state"))) return rc;
+        CUDA_TRY(cudaMemsetAsync(c->d_u4_aux, 0xFF, 3 * sizeof(uint32_t), stream));
+    }
+    // U4: up to kU4CtaNominees keys per CTA of the grid (tma_grid never exceeds sm_count or the grid option)
+    const size_t u4_keys = static_cast<size_t>(std::max(e->tune.grid, e->sm_count)) * kU4CtaNominees;
+    if ((rc = c->d_heaps.ensure(std::max(static_cast<size_t>(kShadowNominees) * kNomineeStride, u4 ? u4_keys : 0), "nominee keys")) ||
         (rc = c->d_ok.ensure(1, "proof flags")) || (!p.query && (rc = c->d_queries.ensure(e->dims, "query buffer"))))
         return rc;
 
     ScanParams sp = p;
-    sp.corpus = int8 ? reinterpret_cast<const float *>(e->d_int8.p) : reinterpret_cast<const float *>(e->d_shadow.p);
-    sp.row_scale = int8 ? e->d_int8_scale.p : nullptr;
+    sp.corpus = u4 ? reinterpret_cast<const float *>(e->u4.codes.p)
+                   : int8 ? reinterpret_cast<const float *>(e->i8.codes.p) : reinterpret_cast<const float *>(e->d_shadow.p);
+    sp.row_scale = u4 ? e->u4.scale.p : int8 ? e->i8.scale.p : nullptr;
+    sp.u4_aux = u4 ? c->d_u4_aux.p : nullptr;
     sp.k = kShadowNominees;
     sp.out = nullptr; sp.host_out = nullptr; sp.host_flag = nullptr;
     sp.nominees = c->d_heaps;
@@ -810,9 +882,23 @@ static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const 
     sp.tail_smem_bytes = static_cast<uint32_t>(static_cast<size_t>(cfg.warps) * cfg.stages * cfg.R * e->dims *
                                                (int8 ? 1 : sizeof(__nv_bfloat16)));
     const int grid = tma_grid(e, c, cfg, sp);
-    if (int8) CUDA_TRY(launch_int8_scan(e, sp, grid, cfg, e->similarity, stream));
+    if (u4) CUDA_TRY(launch_u4_scan(e, sp, grid, cfg, stream));
+    else if (int8) CUDA_TRY(launch_int8_scan(e, sp, grid, cfg, e->similarity, stream));
     else CUDA_TRY(launch_shadow_scan(e, sp, grid, cfg, e->similarity, stream));
 
+    if (u4) {           // every CTA's nominees, re-scored and proven on the whole grid
+        RescoreParams rp{};
+        rp.corpus = e->d_corpus; rp.query = p.query ? p.query : c->d_queries.p;
+        rp.dims = e->dims; rp.k = p.k; rp.n_nominees = static_cast<uint32_t>(grid) * kU4CtaNominees;
+        rp.nominees = c->d_heaps; rp.aux = c->d_u4_aux; rp.max_norm_bits = e->d_max_norm; rp.rho_max = e->u4.rho_max;
+        rp.block_keys = c->d_block_keys; rp.ticket = c->d_ticket; rp.work_counter = sp.work_counter; rp.out = p.out; rp.ok = c->d_ok;
+        rp.frame_ids = p.frame_ids; rp.id_base = p.id_base; rp.row_offset = p.row_offset;
+        rp.tail_smem_bytes = static_cast<uint32_t>(grid) * p.k * sizeof(uint64_t);      // <= 132 x 32 keys: no opt-in needed
+        if (rp.tail_smem_bytes > 48u * 1024u) rp.tail_smem_bytes = 0;                    // (a wider grid reads them from L2)
+        const auto kernel = e->similarity == WAX_VS_COSINE ? shadow_rescore_kernel<kCosine> : shadow_rescore_kernel<kDot>;
+        kernel<<<grid, 512, rp.tail_smem_bytes, stream>>>(rp);
+        CUDA_TRY(cudaGetLastError());
+    } else {
     FinishParams fp{};
     fp.corpus = e->d_corpus; fp.queries = p.query ? p.query : c->d_queries.p;
     fp.n_rows = p.n_rows; fp.dims = e->dims; fp.n_queries = 1; fp.groups = 1; fp.slices = 1;
@@ -820,12 +906,13 @@ static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const 
     fp.heaps = c->d_heaps; fp.max_norm_bits = e->d_max_norm;
     fp.out = p.out; fp.ok = c->d_ok;
     fp.frame_ids = p.frame_ids; fp.id_base = p.id_base; fp.row_offset = p.row_offset;
-    fp.pow2_all = 512; fp.rescore = kShadowRescore; fp.eps_rel = int8 ? e->int8_eps_rel : kBf16Eps;
+    fp.pow2_all = 512; fp.rescore = kShadowRescore; fp.eps_rel = int8 ? e->i8.eps_rel : kBf16Eps;
     const size_t fsmem = static_cast<size_t>(fp.pow2_all + fp.rescore) * sizeof(uint64_t);
     const auto kernel = e->similarity == WAX_VS_COSINE ? batch_finish_kernel<kCosine> : batch_finish_kernel<kDot>;
     CUDA_TRY(grant_smem(e, kernel, fsmem));
     kernel<<<1, 512, fsmem, stream>>>(fp);
     CUDA_TRY(cudaGetLastError());
+    }
     *launches += 2;
     if (shape) {
         const uint32_t s[7] = {static_cast<uint32_t>(cfg.C), static_cast<uint32_t>(cfg.R), static_cast<uint32_t>(cfg.warps),
@@ -846,22 +933,43 @@ static int32_t enqueue_shadow_route(wax_vs_engine *e, SearchCtx *c, ScanParams &
         c->h_proof_count[0] = c->h_proof_count[1] = 0;
         c->seen_failed = 0;
     }
+    bool demoted;
     {
         std::lock_guard<std::mutex> pg(e->pool_mu);
         const uint32_t failed = *static_cast<volatile uint32_t *>(c->h_proof_count + 1);   // no synchronisation: may lag
-        if (failed != c->seen_failed) { c->seen_failed = failed; e->shadow_scan_skip = kShadowSkipQueries; }
+        if (failed != c->seen_failed) {
+            c->seen_failed = failed;
+            if (c->last_u4) {           // a 4-bit proof failed (the fp32 scan answered): the int8 form for a while
+                if (e->u4_probing) e->u4_demote_window = std::min(e->u4_demote_window * 2, 1u << 20);
+                e->u4_demoted = e->u4_demote_window;
+            } else {
+                e->shadow_scan_skip = kShadowSkipQueries;
+            }
+        } else if (c->last_u4 && e->u4_probing) {        // the probe after a demotion held
+            e->u4_demote_window = 16;
+        }
+        if (c->last_u4) e->u4_probing = false;
+        c->last_u4 = false;
         if (e->shadow_scan_skip > 0) { --e->shadow_scan_skip; return WAX_VS_OK; }
+        demoted = e->u4_demoted > 0;
+        if (demoted && --e->u4_demoted == 0) e->u4_probing = true;
     }
-    bool int8 = false;
-    if ((rc = int8_route_selected(e, stream, &int8))) return rc;
-    if (int8) {
+    RouteForm form;
+    if ((rc = select_route_form(e, stream, demoted, &form))) return rc;
+    if (form == RouteForm::kU4) {
+        if (!pick_u4_config(e, &cfg)) return WAX_VS_OK;
+    } else if (form == RouteForm::kInt8) {
         if (!pick_tma_config(e, &cfg, 1, 1)) return WAX_VS_OK;
     } else {
         if ((rc = ensure_shadow(e, stream))) return rc;
         if (!e->shadow_valid) return WAX_VS_OK;
     }
-    if ((rc = enqueue_shadow_nominations(e, c, p, cfg, stream, launches, nullptr, int8))) return rc;
-    if (int8) { std::lock_guard<std::mutex> pg(e->pool_mu); ++e->single_int8_queries; }
+    if ((rc = enqueue_shadow_nominations(e, c, p, cfg, stream, launches, nullptr, form))) return rc;
+    c->last_u4 = form == RouteForm::kU4;
+    if (form != RouteForm::kBf16) {
+        std::lock_guard<std::mutex> pg(e->pool_mu);
+        ++(form == RouteForm::kU4 ? e->single_u4_queries : e->single_int8_queries);
+    }
     p.proof_ok = c->d_ok;
     p.proof_count = c->d_proof_count;
     p.proof_count_host = c->h_proof_count;
@@ -1131,30 +1239,31 @@ static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream) {
 
 // int8 shadow of the corpus for the single-query route (shadow_int8_kernel; cosine rows pre-scaled by 1/|v| as in the bf16
 // shadow): built lazily, extended by appends (which can only raise rho_max), kept over a remove's untouched prefix, rebuilt
-// after overwrites; the same HBM headroom rule as ensure_shadow.  Returns WAX_VS_OK with e->int8_valid == false when it
+// after overwrites; the same HBM headroom rule as ensure_shadow.  Returns WAX_VS_OK with cs.valid == false when it
 // does not fit (the route then stays on the bf16 shadow; counter "int8_shadow_bytes" = 0).  The build synchronises
-// `stream` and reads rho_max and max|v| back: int8_eps_rel = rho_max / M rounded up (M = 1 for cosine, whose rows are
+// `stream` and reads rho_max and max|v| back: eps_rel = rho_max / M rounded up (M = 1 for cosine, whose rows are
 // pre-scaled, and max|v| for dot), so that the finish's eps_rel * |q| * M is at least |q| rho_max.
 // Memory: the bf16 shadow comes first.  Unless it already holds the live rows (or was refused), the int8 shadow reserves
 // what ensure_shadow would allocate next to the same free memory -- its capacity size when that fits the headroom rule,
 // else the live rows -- so that it never leaves the bf16 shadow, and with it the route's bf16 form and the batched bf16
 // nominations, less room than they would have without it.
-// A corpus whose bound is too coarse for the route (int8_eps_rel > kBf16Eps: outlier dimensions) gives its int8 shadow
-// back right after the build and builds none again (int8_coarse) until its rows are rewritten: appends can only raise
+// A corpus whose bound is too coarse for the route (eps_rel > kBf16Eps: outlier dimensions) gives its int8 shadow
+// back right after the build and builds none again (coarse) until its rows are rewritten: appends can only raise
 // rho_max.  keep_coarse (the read-outs) keeps such a shadow; the route never uses it.
-static int32_t ensure_int8_shadow(wax_vs_engine *e, cudaStream_t stream, bool keep_coarse) {
+// The 4-bit shadow (cs.bits == 4, shadow_u4_kernel) follows the same rules with dims / 8 words per row; its bound is
+// coarser than the bf16 one by design, so only a non-finite bound makes it "coarse".
+static int32_t ensure_coded_shadow(wax_vs_engine *e, wax_vs_engine::CodedShadow &cs, cudaStream_t stream, bool keep_coarse) {
     std::lock_guard<std::mutex> g(e->norms_mu);
-    if ((e->int8_valid && e->int8_rows == e->n_rows) || e->int8_unavailable || (e->int8_coarse && !keep_coarse))
+    if ((cs.valid && cs.rows == e->n_rows) || cs.unavailable || (cs.coarse && !keep_coarse))
         return WAX_VS_OK;
     int32_t rc = ensure_norms_locked(e, stream);
     if (rc) return rc;
-    if ((rc = e->d_int8_rho.ensure(1, "int8 shadow bound"))) return rc;
-    const size_t words = e->dims / 4;
+    if ((rc = cs.rho.ensure(1, "coded shadow bound"))) return rc;
+    const size_t words = e->dims * cs.bits / 32;
     const uint64_t need = e->n_rows, pref = std::max<uint64_t>(e->cap_rows, e->n_rows);
     auto scale_entries = [](uint64_t rows) { return static_cast<size_t>((rows + 15) / 16 * 16); };   // whole steps (R <= 16)
-    if (e->d_int8.cap < need * words || e->d_int8_scale.cap < scale_entries(need)) {
-        e->d_int8.release(); e->d_int8_scale.release();
-        e->int8_rows = 0; e->int8_valid = false;
+    if (cs.codes.cap < need * words || cs.scale.cap < scale_entries(need)) {
+        cs.release();
         size_t free_b = 0, total_b = 0;
         uint64_t want = pref;
         auto bytes_for = [&](uint64_t rows) { return rows * words * sizeof(uint32_t) + scale_entries(rows) * sizeof(float); };
@@ -1169,30 +1278,29 @@ static int32_t ensure_int8_shadow(wax_vs_engine *e, cudaStream_t stream, bool ke
         if (info && free_b < bytes_for(want) + reserve + headroom) want = need;
         // allocated by hand, not through ensure(): running out here is not an error and sets no last error
         if (!info || free_b < bytes_for(want) + reserve + headroom ||
-            cudaMalloc(&e->d_int8.p, want * words * sizeof(uint32_t)) != cudaSuccess ||
-            cudaMalloc(&e->d_int8_scale.p, scale_entries(want) * sizeof(float)) != cudaSuccess) {
+            cudaMalloc(&cs.codes.p, want * words * sizeof(uint32_t)) != cudaSuccess ||
+            cudaMalloc(&cs.scale.p, scale_entries(want) * sizeof(float)) != cudaSuccess) {
             cudaGetLastError();
-            e->d_int8.release(); e->d_int8_scale.release();
-            e->int8_unavailable = true;        // stays off until int8_scan_min_bytes is set again
+            cs.release();
+            cs.unavailable = true;        // stays off until int8_scan_min_bytes is set again
             return WAX_VS_OK;
         }
-        e->d_int8.cap = want * words;
-        e->d_int8_scale.cap = scale_entries(want);
-        CUDA_TRY(cudaMemsetAsync(e->d_int8_scale, 0, scale_entries(want) * sizeof(float), stream));   // the step padding
+        cs.codes.cap = want * words;
+        cs.scale.cap = scale_entries(want);
+        CUDA_TRY(cudaMemsetAsync(cs.scale, 0, scale_entries(want) * sizeof(float), stream));   // the step padding
     }
-    if (e->int8_rows > e->n_rows) e->int8_rows = 0;
-    if (e->int8_rows == 0) CUDA_TRY(cudaMemsetAsync(e->d_int8_rho, 0, sizeof(uint32_t), stream));
-    const uint64_t first = e->int8_rows, count = e->n_rows - first;
+    if (cs.rows > e->n_rows) cs.rows = 0;
+    if (cs.rows == 0) CUDA_TRY(cudaMemsetAsync(cs.rho, 0, sizeof(uint32_t), stream));
+    const uint64_t first = cs.rows, count = e->n_rows - first;
     if (count) {
         const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 8, (count + 7) / 8));
-        shadow_int8_kernel<<<std::max(grid, 1), 256, 0, stream>>>(e->d_corpus + first * e->dims,
-                                                                  e->similarity == WAX_VS_COSINE ? e->d_inv_norm + first : nullptr,
-                                                                  count, e->dims, e->d_int8 + first * words,
-                                                                  e->d_int8_scale + first, e->d_int8_rho);
+        (cs.bits == 4 ? shadow_u4_kernel : shadow_int8_kernel)<<<std::max(grid, 1), 256, 0, stream>>>(
+            e->d_corpus + first * e->dims, e->similarity == WAX_VS_COSINE ? e->d_inv_norm + first : nullptr, count, e->dims,
+            cs.codes + first * words, cs.scale + first, cs.rho);
         CUDA_TRY(cudaGetLastError());
     }
     uint32_t bits[2] = {0, 0};
-    CUDA_TRY(cudaMemcpyAsync(&bits[0], e->d_int8_rho, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+    CUDA_TRY(cudaMemcpyAsync(&bits[0], cs.rho, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaMemcpyAsync(&bits[1], e->d_max_norm, sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
     CUDA_TRY(cudaStreamSynchronize(stream));
     float rho, m;
@@ -1200,17 +1308,16 @@ static int32_t ensure_int8_shadow(wax_vs_engine *e, cudaStream_t stream, bool ke
     memcpy(&m, &bits[1], sizeof m);
     if (e->similarity == WAX_VS_COSINE) m = 1.0f;
     const float q = rho / m;               // rounded up: one ulp up unless exact
-    e->int8_rho_max = rho;
+    cs.rho_max = rho;
     // (a non-finite max|v| leaves the finish no finite bound either way: no int8 route then)
-    e->int8_eps_rel = (std::isfinite(q) && std::isfinite(m) && m > 0.0f)
+    cs.eps_rel = (std::isfinite(q) && std::isfinite(m) && m > 0.0f)
                           ? (static_cast<double>(q) * m >= rho ? q : std::nextafter(q, INFINITY)) : INFINITY;
-    e->int8_rows = e->n_rows;
-    e->int8_valid = true;
-    if (e->int8_eps_rel > kBf16Eps) {          // too coarse for the route (above)
-        e->int8_coarse = true;
+    cs.rows = e->n_rows;
+    cs.valid = true;
+    if (cs.bits == 4 ? !std::isfinite(cs.eps_rel) : cs.eps_rel > kBf16Eps) {          // too coarse for the route (above)
+        cs.coarse = true;
         if (!keep_coarse) {                    // nothing holds it: it was not valid for these rows before this call
-            e->d_int8.release(); e->d_int8_scale.release();
-            e->int8_rows = 0; e->int8_valid = false;
+            cs.release();
         }
     }
     return WAX_VS_OK;
@@ -1535,10 +1642,8 @@ static int32_t set_capacity(wax_vs_engine *e, uint64_t rows) {
             e->d_shadow.release(); e->shadow_valid = false; e->shadow_rows = 0;
             e->shadow_unavailable = true;
         }
-        if (e->d_int8) {                       // likewise the int8 shadow
-            e->d_int8.release(); e->d_int8_scale.release(); e->int8_valid = false; e->int8_rows = 0;
-            e->int8_unavailable = true;
-        }
+        for (auto *cs : {&e->i8, &e->u4})      // likewise the int8 and 4-bit shadows
+            if (cs->codes) { cs->release(); cs->unavailable = true; }
         if (cudaMalloc(&n, bytes) != cudaSuccess)
             return fail(WAX_VS_ERR_CUDA, "Failed to resize vectors buffer (%zu bytes): %s", bytes,
                         cudaGetErrorString(cudaGetLastError()));
@@ -3953,9 +4058,9 @@ int32_t wax_vs_debug_time_search(wax_vs_engine *e, uint32_t n_queries, int64_t t
     SearchCtx *c2 = lease2.c;
     // the shadow route's int8 or bf16 copy is cached per corpus version: bring it up to date outside the timed region
     if (shadow_route_applies(e)) {
-        bool int8 = false;
-        if ((rc = int8_route_selected(e, c->stream, &int8))) return rc;
-        if (!int8 && (rc = ensure_shadow(e, c->stream))) return rc;
+        RouteForm form;
+        if ((rc = select_route_form(e, c->stream, false, &form))) return rc;
+        if (form == RouteForm::kBf16 && (rc = ensure_shadow(e, c->stream))) return rc;
     }
     for (uint32_t it = 0; it < warmup + iters; ++it) {
         if (it == warmup) {
@@ -4119,8 +4224,11 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "ingest_d2h_bytes")) *out = e->ingest_d2h_bytes;
     else if (!strcmp(name, "norms_rows")) *out = e->norms_rows;       // rows whose cached 1/|v| is valid
     else if (!strcmp(name, "shadow_rows")) *out = e->shadow_rows;     // rows whose bf16 shadow is valid
-    else if (!strcmp(name, "int8_shadow_bytes")) *out = e->int8_valid ? e->int8_rows * (e->dims + sizeof(float)) : 0;   // codes + scales
-    else if (!strcmp(name, "int8_shadow_rows")) *out = e->int8_rows;  // rows whose int8 shadow is valid
+    else if (!strcmp(name, "int8_shadow_bytes")) *out = e->i8.valid ? e->i8.rows * (e->dims + sizeof(float)) : 0;   // codes + scales
+    else if (!strcmp(name, "int8_shadow_rows")) *out = e->i8.rows;  // rows whose int8 shadow is valid
+    else if (!strcmp(name, "u4_shadow_bytes")) *out = e->u4.valid ? e->u4.rows * (e->dims / 2 + sizeof(float)) : 0;
+    else if (!strcmp(name, "u4_shadow_rows")) *out = e->u4.rows;
+    else if (!strcmp(name, "single_u4_queries")) *out = e->single_u4_queries;
     else if (!strcmp(name, "single_int8_queries")) *out = e->single_int8_queries;   // single queries nominated from it
     else if (!strcmp(name, "batch_heap_bump")) *out = e->heap_bump;          // sizes above the model's nominee-heap choice (adaptive)
     else if (!strcmp(name, "batch_last_heap")) *out = e->last_heap;          // nominee heap entries of the last bf16 level-1 launch
@@ -4235,19 +4343,22 @@ int32_t wax_vs_debug_batch_nominations(wax_vs_engine *e, const float *queries, u
     return WAX_VS_OK;
 }
 
-// wax_vs_debug_shadow_nominations (int8 = false) and wax_vs_debug_int8_nominations (int8 = true)
+// wax_vs_debug_shadow_nominations, wax_vs_debug_int8_nominations and wax_vs_debug_u4_nominations (keys_cap, out_bound: the
+// 4-bit form only -- its nominees are grid x kU4CtaNominees keys, and {rho_max, rho_q, tau_excl} go to out_bound)
 static int32_t debug_route_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
                                        uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
-                                       uint32_t *out_shape, bool int8) {
-    if (!e || !query || !out_keys || !out_ok || !out_result || !out_shape) return fail(WAX_VS_ERR_NULL, "NULL argument");
+                                       uint32_t *out_shape, RouteForm form, uint64_t keys_cap = 0, float *out_bound = nullptr) {
+    const bool u4 = form == RouteForm::kU4, int8 = form != RouteForm::kBf16;     // int8: a coded shadow
+    if (!e || !query || !out_keys || !out_ok || !out_result || !out_shape || (u4 && !out_bound))
+        return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     const uint32_t k_eff = static_cast<uint32_t>(std::min<uint64_t>(clamp_topk(top_k), std::max<uint64_t>(e->n_rows, 1)));
     TmaConfig cfg{};
     if (e->n_rows == 0 || k_eff > 32u || (e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT) ||
         (int8 ? (e->tune.batch_bf16 == 0 || e->dims % kBatchKBlockBf16 != 0) : !batch_bf16_wanted(e)) ||
-        !pick_tma_config(e, &cfg, 1, int8 ? 1 : sizeof(__nv_bfloat16)))
-        return fail(WAX_VS_ERR_UNSUPPORTED, "no %s-shadow route for k=%u, dims=%u in this shape", int8 ? "int8" : "bf16",
-                    k_eff, e->dims);
+        !(u4 ? pick_u4_config(e, &cfg) : pick_tma_config(e, &cfg, 1, int8 ? 1 : sizeof(__nv_bfloat16))))
+        return fail(WAX_VS_ERR_UNSUPPORTED, "no %s-shadow route for k=%u, dims=%u in this shape",
+                    u4 ? "4-bit" : int8 ? "int8" : "bf16", k_eff, e->dims);
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
     CtxLease lease(e);
@@ -4255,8 +4366,9 @@ static int32_t debug_route_nominations(wax_vs_engine *e, const float *query, int
     if (rc) return rc;
     SearchCtx *c = lease.c;
     if (int8) {
-        if ((rc = ensure_int8_shadow(e, c->stream, true))) return rc;
-        if (!e->int8_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the int8 shadow does not fit in device memory");
+        wax_vs_engine::CodedShadow &cs = u4 ? e->u4 : e->i8;
+        if ((rc = ensure_coded_shadow(e, cs, c->stream, true))) return rc;
+        if (!cs.valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the coded shadow does not fit in device memory");
     } else {
         if ((rc = ensure_shadow(e, c->stream))) return rc;
         if (!e->shadow_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the bf16 shadow does not fit in device memory");
@@ -4272,11 +4384,25 @@ static int32_t debug_route_nominations(wax_vs_engine *e, const float *query, int
     ScanParams p = scan_params(e, c, nullptr, k_eff, 0, c->d_out, nullptr, d_mask);
     if ((rc = place_host_query(e, c, p, query, true, c->stream))) return rc;
     uint64_t launches = 0;
-    if ((rc = enqueue_shadow_nominations(e, c, p, cfg, c->stream, &launches, out_shape, int8))) {
+    if ((rc = enqueue_shadow_nominations(e, c, p, cfg, c->stream, &launches, out_shape, form))) {
         cudaStreamSynchronize(c->stream);
         return rc;
     }
     CUDA_TRY(cudaStreamSynchronize(c->stream));
+    if (u4) {
+        const uint64_t n_keys = static_cast<uint64_t>(out_shape[4]) * kU4CtaNominees;
+        if (keys_cap < n_keys)
+            return fail(WAX_VS_ERR_BUFFER, "the nominees need %llu entries (%llu given)", static_cast<unsigned long long>(n_keys),
+                        static_cast<unsigned long long>(keys_cap));
+        CUDA_TRY(cudaMemcpy(out_keys, c->d_heaps, n_keys * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+        uint32_t aux[3];
+        CUDA_TRY(cudaMemcpy(aux, c->d_u4_aux, sizeof aux, cudaMemcpyDeviceToHost));
+        out_bound[0] = e->u4.rho_max;
+        memcpy(out_bound + 1, &aux[1], sizeof(float));
+        // the cut word as a score: -inf when no row was left out
+        if (aux[2] == 0xFFFFFFFFu) out_bound[2] = -INFINITY;
+        else { const uint32_t u = aux[2] ^ ((aux[2] & 0x80000000u) ? 0x80000000u : 0xFFFFFFFFu); float f; memcpy(&f, &u, 4); out_bound[2] = -f; }
+    } else
     CUDA_TRY(cudaMemcpy2D(out_keys, sizeof(uint64_t), c->d_heaps, kNomineeStride * sizeof(uint64_t), sizeof(uint64_t),
                           kShadowNominees, cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(out_ok, c->d_ok, sizeof(uint32_t), cudaMemcpyDeviceToHost));
@@ -4289,13 +4415,43 @@ static int32_t debug_route_nominations(wax_vs_engine *e, const float *query, int
 int32_t wax_vs_debug_shadow_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
                                         uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
                                         uint32_t *out_shape) {
-    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, false);
+    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, RouteForm::kBf16);
 }
 
 int32_t wax_vs_debug_int8_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
                                       uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
                                       uint32_t *out_shape) {
-    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, true);
+    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, RouteForm::kInt8);
+}
+
+int32_t wax_vs_debug_u4_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
+                                    uint64_t *out_keys, uint64_t keys_cap, uint32_t *out_ok, wax_vs_candidate *out_result,
+                                    uint32_t *out_shape, float *out_bound) {
+    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, RouteForm::kU4,
+                                   keys_cap, out_bound);
+}
+
+int32_t wax_vs_debug_read_u4_shadow(wax_vs_engine *e, uint64_t first, uint64_t n, uint8_t *dst_codes, float *dst_half_steps,
+                                    float *out_rho_max) {
+    if (!e || !dst_codes || !dst_half_steps || !out_rho_max) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
+    TmaConfig cfg{};
+    if ((e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT) || !pick_u4_config(e, &cfg))
+        return fail(WAX_VS_ERR_UNSUPPORTED, "no 4-bit shadow for dims=%u with this metric", e->dims);
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
+    if (rc) return rc;
+    if ((rc = ensure_coded_shadow(e, e->u4, lease.c->stream, true))) return rc;
+    if (!e->u4.valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the 4-bit shadow does not fit in device memory");
+    if (n) {
+        CUDA_TRY(cudaMemcpy(dst_codes, e->u4.codes + first * (e->dims / 8), n * e->dims / 2, cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(dst_half_steps, e->u4.scale + first, n * sizeof(float), cudaMemcpyDeviceToHost));
+    }
+    *out_rho_max = e->u4.rho_max;
+    return WAX_VS_OK;
 }
 
 int32_t wax_vs_debug_read_int8_shadow(wax_vs_engine *e, uint64_t first, uint64_t n, uint8_t *dst_codes, float *dst_scales,
@@ -4311,13 +4467,13 @@ int32_t wax_vs_debug_read_int8_shadow(wax_vs_engine *e, uint64_t first, uint64_t
     CtxLease lease(e);
     int32_t rc = lease.acquire();
     if (rc) return rc;
-    if ((rc = ensure_int8_shadow(e, lease.c->stream, true))) return rc;
-    if (!e->int8_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the int8 shadow does not fit in device memory");
+    if ((rc = ensure_coded_shadow(e, e->i8, lease.c->stream, true))) return rc;
+    if (!e->i8.valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the int8 shadow does not fit in device memory");
     if (n) {
-        CUDA_TRY(cudaMemcpy(dst_codes, e->d_int8 + first * (e->dims / 4), n * e->dims, cudaMemcpyDeviceToHost));
-        CUDA_TRY(cudaMemcpy(dst_scales, e->d_int8_scale + first, n * sizeof(float), cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(dst_codes, e->i8.codes + first * (e->dims / 4), n * e->dims, cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(dst_scales, e->i8.scale + first, n * sizeof(float), cudaMemcpyDeviceToHost));
     }
-    *out_rho_max = e->int8_rho_max;
+    *out_rho_max = e->i8.rho_max;
     return WAX_VS_OK;
 }
 
@@ -4379,9 +4535,18 @@ int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value
     else if (!strcmp(key, "shadow_scan_min_bytes")) e->tune.shadow_scan_min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
     else if (!strcmp(key, "int8_scan_min_bytes")) {     // also lets an int8 shadow that did not fit be tried again
         e->tune.int8_scan_min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
-        e->int8_unavailable = false;
-        e->int8_coarse = false;
+        e->i8.unavailable = false;
+        e->i8.coarse = false;
     }
+    else if (!strcmp(key, "u4_scan_min_bytes")) {       // also retries a 4-bit shadow that did not fit, and ends a demotion
+        e->tune.u4_scan_min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
+        e->u4.unavailable = false;
+        e->u4.coarse = false;
+        e->u4_demoted = 0; e->u4_demote_window = 16; e->u4_probing = false;
+    }
+    else if (!strcmp(key, "u4_rows_per_step")) e->tune.u4_rows_per_step = v;
+    else if (!strcmp(key, "u4_warps")) e->tune.u4_warps = v;
+    else if (!strcmp(key, "u4_stages")) e->tune.u4_stages = v;
     else if (!strcmp(key, "int8_rows_per_step")) e->tune.int8_rows_per_step = v;
     else if (!strcmp(key, "int8_warps")) e->tune.int8_warps = v;
     else if (!strcmp(key, "int8_stages")) e->tune.int8_stages = v;

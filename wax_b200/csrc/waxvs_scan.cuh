@@ -75,8 +75,12 @@ struct ScanParams {
                                 // every CTA returns at entry (CTA 0 first delivers `out` to the host), else a plain scan
     uint32_t *proof_count;      // guarded: [0] proofs that held, [1] that failed -- running counts on the device ...
     uint32_t *proof_count_host; // ... mirrored into mapped pinned memory, read by the host without synchronising
-    const float *row_scale;     // INT8: [rows, padded to whole steps] the scale s of each int8 shadow row
+    const float *row_scale;     // INT8: [rows, padded to whole steps] the scale s of each int8 shadow row; U4: the half step h
+    uint32_t *u4_aux;           // U4: [0] the smallest (key >> 32) any warp list or CTA selection cut rows at (every row left
+                                // out has a key at or above it; 0xFFFFFFFF on entry = nothing cut), [1] rho_q (fp32 bits)
 };
+
+constexpr uint32_t kU4CtaNominees = 256;    // U4: nominees every CTA writes (the best of its warps' lists)
 
 // batch_finish_kernel reads entry e of query 0's heap of slice 0 at e * kBatchM (static_assert in waxvs_batch.cuh).
 constexpr int kNomineeStride = 128;
@@ -122,6 +126,26 @@ __device__ __forceinline__ float4 int8x4_to_float4(uint32_t u) {
                        __fsub_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7651)), kBias),
                        __fsub_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7652)), kBias),
                        __fsub_rn(__uint_as_float(__byte_perm(u, 0x4B000000u, 0x7653)), kBias));
+}
+
+// Reduce-scatter of H integer partial sums over each half-warp (the U4 form: 16 lanes share a row): on exit v[0] of lane
+// L holds the 16-lane sum of entry (L & 15) / (16 / H) of its half.  Integer sums: exact in any order.
+template <int H>
+__device__ __forceinline__ void half_warp_reduce_scatter(int (&v)[H], int lane) {
+    static_assert(H == 1 || H == 2 || H == 4 || H == 8, "H must be a power of two <= 8");
+    int off = 8;
+#pragma unroll
+    for (int half = H / 2; half >= 1; half >>= 1, off >>= 1) {
+        const bool upper = (lane & off) != 0;
+#pragma unroll
+        for (int j = 0; j < half; ++j) {
+            const int send = upper ? v[j] : v[j + half];
+            const int keep = upper ? v[j + half] : v[j];
+            v[j] = keep + __shfl_xor_sync(WAXVS_FULL_MASK, send, off);
+        }
+    }
+#pragma unroll
+    for (; off >= 1; off >>= 1) v[0] += __shfl_xor_sync(WAXVS_FULL_MASK, v[0], off);
 }
 
 // CTA merge + grid merge + output.  Called by every thread of the CTA after the scan loop.
@@ -267,8 +291,9 @@ __device__ __forceinline__ uint64_t block_select_kth(ForEach for_each, uint32_t 
 
 // The selection tail: called by every thread of the CTA after the scan loop (the warps' register lists need not be
 // merged, or even sorted, for this).  scratch = the dynamic shared memory (the idle ring), p.tail_smem_bytes of it.
+// Returns true in the CTA that finished the grid stage (its threads have written the result, not yet synchronised).
 template <int E, bool SHADOW = false>
-__device__ __forceinline__ void finish_topk_select(const ScanParams &p, WarpTopK<E> &tk, unsigned char *scratch) {
+__device__ __forceinline__ bool finish_topk_select(const ScanParams &p, WarpTopK<E> &tk, unsigned char *scratch) {
     __shared__ SelectScratch ss;
     __shared__ uint32_t s_last2;
     const uint32_t tid = threadIdx.x, nthr = blockDim.x, k = p.k;
@@ -291,7 +316,7 @@ __device__ __forceinline__ void finish_topk_select(const ScanParams &p, WarpTopK
     if (p.trace && tid == 0) atomicMax(p.trace + 2, global_timer_ns());
     if (tid == 0) s_last2 = (atomicAdd(p.ticket, 1u) == gridDim.x - 1) ? 1u : 0u;
     __syncthreads();
-    if (!s_last2) return;
+    if (!s_last2) return false;
     __threadfence();
     if (p.trace && tid == 0) p.trace[3] = global_timer_ns();
     // ---- stage B (last CTA): the k smallest of the grid's gridDim.x * k keys, ranked, written out
@@ -331,6 +356,38 @@ __device__ __forceinline__ void finish_topk_select(const ScanParams &p, WarpTopK
         if (p.trace) p.trace[4] = global_timer_ns();
     }
     if (p.shard.world) shard_exchange_cta(p.shard, p.out, p.k, reinterpret_cast<uint32_t *>(scratch));
+    return true;
+}
+
+// The U4 form's tail: no grid stage.  Every CTA selects the kU4CtaNominees smallest keys of its warps' lists and writes
+// them to p.nominees[blockIdx.x * kU4CtaNominees ..] (unordered, NONE-padded); shadow_rescore_kernel re-scores them all.
+// A row that is not written was cut either by its warp's full list (key >= the list's last key) or by this selection
+// (key > the CTA's cut key): the smallest such key over the grid, in p.u4_aux[0], bounds the score' of every row left out.
+template <int E>
+__device__ __forceinline__ void finish_u4_nominees(const ScanParams &p, WarpTopK<E> &tk) {
+    __shared__ SelectScratch ss;
+    __shared__ uint32_t s_cut;
+    const uint32_t tid = threadIdx.x, nthr = blockDim.x;
+    if (tid == 0) s_cut = WAXVS_UKEY_NONE;
+    auto own_keys = [&](auto f) {
+#pragma unroll
+        for (int j = 0; j < E; ++j) f(tk.key[j]);
+    };
+    const uint64_t xa = block_select_kth(own_keys, kU4CtaNominees, &ss);     // synchronises: s_cut is initialised
+    if (tid == 0) ss.n_sel = 0;
+    __syncthreads();
+    uint64_t *mine = p.nominees + static_cast<size_t>(blockIdx.x) * kU4CtaNominees;
+#pragma unroll
+    for (int j = 0; j < E; ++j)
+        if (tk.key[j] != WAXVS_KEY_NONE && tk.key[j] <= xa) mine[atomicAdd(&ss.n_sel, 1u)] = tk.key[j];
+    if ((tid & 31u) == 0 && tk.thresh != WAXVS_KEY_NONE) atomicMin(&s_cut, static_cast<uint32_t>(tk.thresh >> 32));
+    __syncthreads();
+    for (uint32_t i = ss.n_sel + tid; i < kU4CtaNominees; i += nthr) mine[i] = WAXVS_KEY_NONE;
+    if (tid == 0) {
+        uint32_t cut = s_cut;
+        if (xa != WAXVS_KEY_NONE) cut = min(cut, static_cast<uint32_t>(xa >> 32));
+        if (cut != WAXVS_UKEY_NONE) atomicMin(p.u4_aux, cut);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -352,10 +409,20 @@ __device__ __forceinline__ void finish_topk_select(const ScanParams &p, WarpTopK
 //          uint32 of 4 codes, widens them exactly (int8x4_to_float4) and FMAs them against the same fp32 query registers;
 //          the row's sum is multiplied once by s: score' = s (q.c).  The R scales of a step ride in the same stage behind
 //          the rows (a second bulk copy on the same mbarrier), so R >= 4 keeps that copy 16-byte aligned.
-template <int C, int R, int METRIC, int E, bool EMIT, bool SHADOW = false, bool INT8 = false>
+//   U4     (with SHADOW, not INT8) the nominating pass of the 4-bit-shadow route: p.corpus holds the rows as 16-level
+//          codes u, two per byte (ROW_BYTES = 64 C; byte b of word w: element 8w + b in the low nibble, 8w + 4 + b in the
+//          high one), p.row_scale each row's half step h: the row decodes to h (2u - 15).  The query is coded once per
+//          launch to int8 (c_q = rne(q / s_q), s_q = max|q_i| / 127) and the row's sum is integer, two dp4a per word:
+//          score' = fl(fl(s_q h) (2 sum c_q u - 15 sum c_q)), exact but for those two roundings.  16 lanes share a row (C
+//          words each), the half-warps take the even and the odd rows of a step; for even C the odd half swaps its word
+//          pairs so that the two halves never read the same banks.  CTA 0 stores rho_q = ||q - s_q c_q|| (measured in
+//          fp64, rounded up; +inf for a non-finite query) in p.u4_aux[1]; the tail is finish_u4_nominees.
+template <int C, int R, int METRIC, int E, bool EMIT, bool SHADOW = false, bool INT8 = false, bool U4 = false>
 __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant__ ScanParams p) {
     static_assert(!SHADOW || (C > 0 && METRIC != kL2 && !EMIT), "the shadow form covers the unrolled cosine / dot shapes");
     static_assert(!INT8 || (SHADOW && R >= 4), "the int8 form is a shadow form with 16-byte scale copies");
+    static_assert(!U4 || (SHADOW && !INT8 && R >= 4 && E == 4), "the 4-bit form is a shadow form with 16-byte scale copies");
+    constexpr bool SCALED = INT8 || U4;     // the step's row scales ride behind its rows
     if constexpr (!SHADOW && !EMIT && E == 1 && METRIC != kL2) {
         if (p.proof_ok) {               // guarded launch after a shadow proof (batch_finish_kernel, same stream; k <= 32)
             const bool proven = *p.proof_ok != 0u;
@@ -376,8 +443,8 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
     }
     const int D4 = C > 0 ? 32 * C : static_cast<int>(p.dims / 4u);          // float4 (SHADOW: uint2, INT8: uint32) per row
     const int CN = C > 0 ? C : (D4 + 31) / 32;                               // chunks per lane
-    const uint32_t ROW_BYTES = C > 0 ? (INT8 ? 128u : SHADOW ? 256u : 512u) * C : p.dims * 4u;
-    const uint32_t STAGE_BYTES = ROW_BYTES * R + (INT8 ? R * 4u : 0u);       // INT8: the step's scales behind its rows
+    const uint32_t ROW_BYTES = C > 0 ? (U4 ? 64u : INT8 ? 128u : SHADOW ? 256u : 512u) * C : p.dims * 4u;
+    const uint32_t STAGE_BYTES = ROW_BYTES * R + (SCALED ? R * 4u : 0u);     // SCALED: the step's scales behind its rows
     constexpr int LANES_PER_ROW = 32 / R;
 
     extern __shared__ __align__(128) unsigned char smem[];
@@ -409,6 +476,59 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         if (p.query_store && p.query == nullptr && blockIdx.x == 0)
             for (uint32_t i = threadIdx.x; i < p.dims; i += blockDim.x) p.query_store[i] = p.query_inline[i];
     }
+    // U4: the query as int8 codes, in the words this lane reads of every row
+    constexpr int CU = U4 ? (C > 0 ? C : 1) : 1;
+    constexpr int H = U4 ? R / 2 : 1;                 // rows of a step per half-warp
+    const int hl = lane & 15, hh = lane >> 4;
+    int qlo[CU], qhi[CU], word_of[CU];
+    int q_code_sum = 0;
+    float s_q = 0.0f;
+    if constexpr (U4) {
+        float m = 0.0f;
+        bool bad = false;
+#pragma unroll
+        for (int c = 0; c < CU; ++c) {
+            bad |= !finite_f32(q[c].x) || !finite_f32(q[c].y) || !finite_f32(q[c].z) || !finite_f32(q[c].w);
+            m = fmaxf(m, fmaxf(fmaxf(fabsf(q[c].x), fabsf(q[c].y)), fmaxf(fabsf(q[c].z), fabsf(q[c].w))));
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(WAXVS_FULL_MASK, m, o));
+        bad = __any_sync(WAXVS_FULL_MASK, bad);
+        s_q = __fdiv_rn(m, 127.0f);
+        const bool code_it = !bad && s_q > 0.0f && finite_f32(s_q);
+        double r2 = 0.0;
+#pragma unroll
+        for (int c = 0; c < CU; ++c) {
+            word_of[c] = hl + 16 * ((C % 2 == 0) ? (c ^ hh) : c);
+            int packed[2];
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+                const float4 x4 = load_q(2 * word_of[c] + half);
+                const float xs[4] = {x4.x, x4.y, x4.z, x4.w};
+                uint32_t w = 0;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int code = code_it ? max(-127, min(127, __float2int_rn(__fdiv_rn(xs[j], s_q)))) : 0;
+                    w |= static_cast<uint32_t>(code & 0xFF) << (8 * j);
+                    const double e = static_cast<double>(xs[j]) - static_cast<double>(s_q) * static_cast<double>(code);
+                    r2 = fma(e, e, r2);
+                }
+                packed[half] = static_cast<int>(w);
+                q_code_sum = __dp4a(packed[half], 0x01010101, q_code_sum);
+            }
+            qlo[c] = packed[0]; qhi[c] = packed[1];
+        }
+#pragma unroll
+        for (int o = 8; o > 0; o >>= 1) {       // a half-warp holds every word of the query once
+            q_code_sum += __shfl_xor_sync(WAXVS_FULL_MASK, q_code_sum, o);
+            r2 += __shfl_xor_sync(WAXVS_FULL_MASK, r2, o);
+        }
+        if (blockIdx.x == 0 && threadIdx.x == 0) {
+            float rho_q = __double2float_ru(sqrt(r2) * (1.0 + 0x1p-40));
+            if (bad || !finite_f32(s_q) || !finite_f32(rho_q)) rho_q = INFINITY;
+            p.u4_aux[1] = __float_as_uint(rho_q);
+        }
+    }
     float a2 = 0.0f, sqrt_a2 = 0.0f;
     if (METRIC == kCosine && !SHADOW) {
         float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
@@ -434,14 +554,14 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         const uint32_t rows = min(static_cast<uint32_t>(R), p.n_rows - row0);
         const uint32_t bytes = rows * ROW_BYTES;
         stage_step[s] = step;                        // released to the warp by the mbarrier arrive below
-        mbar_arrive_expect_tx(&bars[s], bytes + (INT8 ? R * 4u : 0u));
+        mbar_arrive_expect_tx(&bars[s], bytes + (SCALED ? R * 4u : 0u));
         const void *src = SHADOW ? static_cast<const void *>(reinterpret_cast<const unsigned char *>(p.corpus) +
                                                              static_cast<size_t>(row0) * ROW_BYTES)
                                  : static_cast<const void *>(p.corpus + static_cast<size_t>(row0) * p.dims);
         if (p.use_l2_hint) bulk_copy_g2s_hint(ring + s * STAGE_BYTES, src, bytes, &bars[s], policy);
         else bulk_copy_g2s(ring + s * STAGE_BYTES, src, bytes, &bars[s]);
         // the scale array is padded to whole steps: a ragged last step still copies R scales
-        if constexpr (INT8) bulk_copy_g2s(ring + s * STAGE_BYTES + R * ROW_BYTES, p.row_scale + row0, R * 4u, &bars[s]);
+        if constexpr (SCALED) bulk_copy_g2s(ring + s * STAGE_BYTES + R * ROW_BYTES, p.row_scale + row0, R * 4u, &bars[s]);
     };
 
     // Step sequence of this warp.  Static: gwarp, gwarp + total_warps, ...  Dynamic (chunk_steps > 0, fused
@@ -490,11 +610,26 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         const uint32_t step = stage_step[s];
         const float4 *tile = reinterpret_cast<const float4 *>(ring + s * STAGE_BYTES);
         // INT8: the scale of the row this lane finishes after the reduce-scatter, read before the stage is refilled
-        const float row_s = INT8 ? reinterpret_cast<const float *>(ring + s * STAGE_BYTES + R * ROW_BYTES)[lane / LANES_PER_ROW]
-                                 : 1.0f;
+        // U4: a lane finishes row 2 (hl / (16 / H)) + hh of the step
+        const int my_in_step = U4 ? 2 * (hl / (16 / H)) + hh : lane / LANES_PER_ROW;
+        const float row_s = SCALED ? reinterpret_cast<const float *>(ring + s * STAGE_BYTES + R * ROW_BYTES)[my_in_step] : 1.0f;
 
         float sum0[R], sum1[R];
-        if (C == 0) {
+        int isum[H] = {};
+        if constexpr (U4) {
+            const uint32_t *tw = reinterpret_cast<const uint32_t *>(tile) + hh * 16 * C;
+#pragma unroll
+            for (int j = 0; j < H; ++j) {
+                int a = 0;
+#pragma unroll
+                for (int c = 0; c < CU; ++c) {
+                    const uint32_t w = tw[j * 32 * C + word_of[c]];
+                    a = __dp4a(static_cast<int>(w & 0x0F0F0F0Fu), qlo[c], a);
+                    a = __dp4a(static_cast<int>((w >> 4) & 0x0F0F0F0Fu), qhi[c], a);
+                }
+                isum[j] = a;
+            }
+        } else if (C == 0) {
             // Generic rows (dims < 128 or not one of the unrolled multiples of 128), several rows per step: chunk-outer /
             // row-inner, so a query chunk is read from shared memory once for the R rows (the row-outer form read it per row:
             // twice the shared-memory traffic).  Each row still sees its chunks in ascending
@@ -571,12 +706,14 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         ++consumed;
         if (++s == stages) { s = 0; parity ^= 1u; }
 
-        warp_reduce_scatter<R>(sum0, lane);
+        if constexpr (U4) half_warp_reduce_scatter<H>(isum, lane);
+        else warp_reduce_scatter<R>(sum0, lane);
         if (METRIC == kCosine && !SHADOW) warp_reduce_scatter<R>(sum1, lane);
 
-        const uint32_t my_row = step * R + (lane / LANES_PER_ROW);
+        const uint32_t my_row = step * R + my_in_step;
         float d;
-        if (INT8) d = -__fmul_rn(row_s, sum0[0]);   // -score' = -s (q.c)
+        if constexpr (U4) d = -__fmul_rn(__fmul_rn(s_q, row_s), static_cast<float>(2 * isum[0] - 15 * q_code_sum));   // -score'
+        else if (INT8) d = -__fmul_rn(row_s, sum0[0]);   // -score' = -s (q.c)
         else if (SHADOW) d = -sum0[0];     // -score': the nominee key's distance
         else if (METRIC == kCosine) d = finish_cos(sum0[0], a2, sqrt_a2, sum1[0]);
         else if (METRIC == kDot) d = finish_dot(sum0[0]);
@@ -585,7 +722,7 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
         // up), giving +-inf or inf - inf = NaN for a row whose exact score is finite.  Such a row is nominated first
         // (score' = +inf), so the finish re-scores it; and as entry 0 it refuses the proof.
         if (SHADOW && !finite_f32(d)) d = -INFINITY;
-        const bool leader = (lane % LANES_PER_ROW) == 0;
+        const bool leader = U4 ? (hl % (16 / H)) == 0 : (lane % LANES_PER_ROW) == 0;
         const bool ok = (my_row < p.n_rows) && (SHADOW || finite_f32(d));
 
         if (EMIT) {
@@ -617,7 +754,8 @@ __global__ void __launch_bounds__(512, 1) scan_tma_kernel(const __grid_constant_
     if (p.trace && lane == 0) atomicMax(p.trace + 1, global_timer_ns());
     if (!EMIT) {
         if (E > 1) tk.flush(lane, k);
-        if (p.tail_select) finish_topk_select<E, SHADOW>(p, tk, smem);
+        if constexpr (U4) finish_u4_nominees<E>(p, tk);
+        else if (p.tail_select) finish_topk_select<E, SHADOW>(p, tk, smem);
         else finish_topk<E, SHADOW>(p, tk, lists, warp, lane, warps);
     }
 }

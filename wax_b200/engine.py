@@ -754,11 +754,19 @@ class CUDAVectorEngine:
         from the int8 shadow in the shape the int8_* options select and the finish proves with its measured bound."""
         return self._route_nominations(L.lib().wax_vs_debug_int8_nominations, vector, top_k, allow_rows)
 
-    def _route_nominations(self, fn, vector, top_k: int, allow_rows):
+    def u4_nominations(self, vector, top_k: int, allow_rows=None):
+        """shadow_nominations for the 4-bit form of the route (wax_vs_debug_u4_nominations): the U4 scan nominates from
+        the 4-bit shadow in the shape the u4_* options select, every CTA writes its best 256 keys (keys [grid * 256],
+        unordered, padding 0xFFFF...), and the grid-wide re-score proves.  Also rho_max, rho_q (the measured row and
+        query coding bounds) and tau_excl (the score' no left-out row exceeds; -inf when none was left out)."""
+        return self._route_nominations(L.lib().wax_vs_debug_u4_nominations, vector, top_k, allow_rows, u4=True)
+
+    def _route_nominations(self, fn, vector, top_k: int, allow_rows, u4: bool = False):
         q = np.ascontiguousarray(vector, dtype=np.float32).reshape(self.dimensions)
         n = self.count
         k = max(1, min(int(top_k), n))
-        keys = np.empty(128, np.uint64)
+        keys = np.empty(256 * 1024 if u4 else 128, np.uint64)
+        bound = np.zeros(3, np.float32)
         ok = C.c_uint32(0)
         result = (L.Candidate * k)()
         shape = np.zeros(7, np.uint32)
@@ -768,14 +776,23 @@ class CUDAVectorEngine:
             mask[np.asarray(allow_rows, np.int64)] = True
             bits = (mask.reshape(-1, 32).astype(np.uint64) << np.arange(32, dtype=np.uint64)).sum(1).astype(np.uint32)
         u32 = lambda a: a.ctypes.data_as(C.POINTER(C.c_uint32))
-        _check(fn(
-            self._h, q.ctypes.data_as(C.POINTER(C.c_float)), int(top_k), None if bits is None else u32(bits),
-            keys.ctypes.data_as(C.POINTER(C.c_uint64)), C.byref(ok), result, u32(shape)))
+        if u4:
+            _check(fn(
+                self._h, q.ctypes.data_as(C.POINTER(C.c_float)), int(top_k), None if bits is None else u32(bits),
+                keys.ctypes.data_as(C.POINTER(C.c_uint64)), keys.size, C.byref(ok), result, u32(shape),
+                bound.ctypes.data_as(C.POINTER(C.c_float))))
+            keys = keys[:int(shape[4]) * 256]
+        else:
+            _check(fn(
+                self._h, q.ctypes.data_as(C.POINTER(C.c_float)), int(top_k), None if bits is None else u32(bits),
+                keys.ctypes.data_as(C.POINTER(C.c_uint64)), C.byref(ok), result, u32(shape)))
         one = np.float32(1.0)
         score = (lambda d: float(one - np.float32(d))) if self.metric is VectorMetric.cosine else (lambda d: float(-np.float32(d)))
         names = ("C", "R", "warps", "stages", "grid", "chunk_steps", "tail_select")
         out = {name: int(v) for name, v in zip(names, shape)}
         out.update(keys=keys, ok=ok.value, result=[(int(c.frame_id), score(c.distance)) for c in result if c.valid])
+        if u4:
+            out.update(rho_max=float(bound[0]), rho_q=float(bound[1]), tau_excl=float(bound[2]))
         return out
 
     def read_shadow(self, first: int, n: int) -> np.ndarray:
@@ -793,6 +810,19 @@ class CUDAVectorEngine:
         _check(L.lib().wax_vs_debug_read_int8_shadow(self._h, first, n, codes.ctypes.data_as(C.POINTER(C.c_uint8)),
                                                      scales.ctypes.data_as(C.POINTER(C.c_float)), C.byref(rho)))
         return codes, scales, float(rho.value)
+
+    def read_u4_shadow(self, first: int, n: int):
+        """The 4-bit shadow of rows [first, first + n) (wax_vs_debug_read_u4_shadow): (codes [n, dims] uint8 in 0..15,
+        unpacked to element order; half_steps [n] float32, a row decodes to h * (2 u - 15); rho_max of the whole shadow)."""
+        packed = np.empty((n, self.dimensions // 2), np.uint8)
+        half = np.empty(n, np.float32)
+        rho = C.c_float(0.0)
+        _check(L.lib().wax_vs_debug_read_u4_shadow(self._h, first, n, packed.ctypes.data_as(C.POINTER(C.c_uint8)),
+                                                   half.ctypes.data_as(C.POINTER(C.c_float)), C.byref(rho)))
+        # byte b of 4-byte word w: element 8w + b in the low nibble, 8w + 4 + b in the high one
+        w = packed.reshape(n, -1, 4)
+        codes = np.concatenate([w & 15, w >> 4], axis=2).reshape(n, self.dimensions)
+        return codes, half, float(rho.value)
 
     def stream_read_gbs(self, iters: int = 5) -> float:
         """Plain coalesced read of the corpus bytes: the box's streaming-read ceiling in GB/s."""
