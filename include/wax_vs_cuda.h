@@ -287,6 +287,70 @@ int32_t wax_vs_search_batch_grouped_where(wax_vs_engine *engine, const float *qu
                                           const wax_vs_where *where, uint64_t *out_ids, float *out_scores,
                                           uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n);
 
+/* ---- frame locations: PhotoRAG's location radius as a predicate below the top-k (API EXTENSION) ---------------------
+   PhotoRAG answers a location query with an allow-list (PhotoRAGOrchestrator.buildLocationAllowlist,
+   PhotoRAGOrchestrator.swift:788-854): the frames of every 0.01-degree bin (locationBins, :766-771, binned by
+   locationBin(from:), :868-875) in a box around the centre, passed as frameFilter beside the request's timeRange
+   (:238-257).  Here each row may carry its bins and the box is one more clause of a where, evaluated on the device.
+
+   Frame side: a row has a location, stored as its bins (Int(floor(lat * 100)), Int(floor(lon * 100)) in fp64, not
+   clamped; bins beyond int32 are stored saturated, and no box reaches past +-36 000), or has none, and then never passes
+   a location clause.  Locations follow their rows as attributes do: an appended frame has none, an upsert keeps the
+   frame's, removes drop them, wax_vs_deserialize and wax_vs_debug_fill_synthetic reset every row (MV2V has no place for
+   them).  The first where_near search after a mutation or wax_vs_set_locations uploads a device copy (8 bytes per row,
+   counter "location_uploads").
+
+   Query side, in fp64 as buildLocationAllowlist computes it: the centre clamped as PhotoCoordinate.init and the radius as
+   PhotoLocationQuery.init (PhotoRAGTypes.swift:33-57) with Swift's min / max (a NaN latitude becomes -90, a NaN radius
+   0); latDelta = r / 111000, lonDelta = min(180, r / max(1e-6, 111000 * cos(lat * pi / 180))); lat bins
+   floor((lat -+ latDelta) * 100) clamped to [-9000, 9000], lon bins floor((lon -+ lonDelta) * 100) not clamped; when
+   minLonBin > maxLonBin the lon bins are [minLonBin, 18000] and [-18000, maxLonBin].  There is no location clause where
+   Swift returns nil: radius <= 0, a bin count <= 0, or latBinCount * lonBinCount >= 100 000.  A row passes the clause
+   when its lat bin is in range and its lon bin in one of the lon ranges: exactly membership in the union of
+   locationBins[bin] over the box.
+   Two host-arithmetic notes: where Swift's Int(_:) would trap (a non-finite or out-of-range bin, e.g. an infinite
+   radius) the library returns WAX_VS_ERR_ARGUMENT; cos is the C library's, which Foundation uses on Linux too (on Darwin
+   it may differ in the last ulp, which moves a box edge only when lon +- lonDelta falls within an ulp of a bin edge). */
+typedef struct wax_vs_where_near {
+    wax_vs_where where;     /* the time and tag clauses                                  */
+    double latitude;        /* the centre, degrees                                       */
+    double longitude;
+    double radius_m;        /* metres; <= 0 or NaN: no location clause                   */
+} wax_vs_where_near;
+/* Set frames' locations (upsert, as wax_vs_set_attributes): frame_ids[i] -> (latitudes[i], longitudes[i]) in degrees; a
+   NaN pair clears the frame's location; any other non-finite coordinate -> WAX_VS_ERR_ARGUMENT and nothing is written.
+   Unknown frame ids are ignored, a later entry for the same frame wins; *out_assigned (optional) = distinct known frames
+   named.  A mutator (write lock). */
+int32_t wax_vs_set_locations(wax_vs_engine *engine, const uint64_t *frame_ids, const double *latitudes,
+                             const double *longitudes, uint64_t n, uint64_t *out_assigned);
+/* The query-side arithmetic above, on the host (no engine, no device): *out_active = 1 and out_box = {minLatBin,
+   maxLatBin, minLonBin, maxLonBin} for a box, *out_active = 0 and zeros for "no location clause"; WAX_VS_ERR_ARGUMENT
+   where Swift would trap. */
+int32_t wax_vs_location_box(double latitude, double longitude, double radius_m, int32_t out_box[4], int32_t *out_active);
+/* The frame-side rule, on the host, as wax_vs_set_locations stores it: *out_has = 0 (and zeros) for a NaN pair, else
+   out_bin = {latBin, lonBin}; WAX_VS_ERR_ARGUMENT for any other non-finite coordinate. */
+int32_t wax_vs_location_bin(double latitude, double longitude, int32_t out_bin[2], int32_t *out_has);
+/* wax_vs_search_batch_where with a location box in each predicate.  Query i's answer is identical to
+   wax_vs_search_batch_multi_filtered under an allow-list of exactly the frames that pass its time and tag clauses, lie in
+   its box and pass its id filter: same ids, order and score bits.  The argument checks of wax_vs_search_batch_where, and
+   the boxes' (WAX_VS_ERR_ARGUMENT), run before the empty-engine early return.  How: as wax_vs_search_batch_where, with
+   the box tested next to the time and tag clauses on the host (allow-lists) and in the location forms of the device
+   passes (count, listing, bitset AND); a call none of whose predicates has a box runs wax_vs_search_batch_where. */
+int32_t wax_vs_search_batch_where_near(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                       uint32_t query_len, int64_t top_k, const uint64_t *frame_ids,
+                                       const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                       const uint32_t *query_filter, const wax_vs_where_near *wheres, uint32_t n_wheres,
+                                       const uint32_t *query_where, uint64_t *out_ids, float *out_scores,
+                                       uint32_t out_stride, uint32_t *out_n);
+/* wax_vs_search_batch_grouped_where with ONE where_near predicate for the batch; each answer is identical to
+   wax_vs_search_grouped under the allow-list of the frames passing it and the id filter: same frame ids, group ids,
+   order and score bits. */
+int32_t wax_vs_search_batch_grouped_where_near(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                               uint32_t query_len, int64_t top_groups, uint32_t per_group,
+                                               const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                                               const wax_vs_where_near *where, uint64_t *out_ids, float *out_scores,
+                                               uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n);
+
 /* Device-resident form used by the row-sharded engine: `d_queries` (n_queries x dims) and
    `d_candidates` (n_queries x k_eff entries, k_eff = min(clamp(top_k), 10000) -- NOT clipped to N, padding
    has valid = 0) are DEVICE pointers on the engine's device; the work is enqueued on `cuda_stream`

@@ -292,6 +292,89 @@ public actor CUDAVectorEngine {
         }
     }
 
+    /// Frame locations in degrees (wax_vs_set_locations), for the frames PhotoRAG puts into `locationBins`: the engine
+    /// stores their 0.01° bins and `searchBatchWhereNear` tests PhotoRAG's location box below the top-k in place of
+    /// `buildLocationAllowlist`.  A NaN pair clears a location; not part of MV2V: re-apply after `deserialize`.
+    @discardableResult
+    public func setLocations(frameIds: [UInt64], latitudes: [Double], longitudes: [Double]) async throws -> Int {
+        guard latitudes.count == frameIds.count, longitudes.count == frameIds.count else {
+            throw WaxError.encodingError(reason: "setLocations: column length != frameIds.count")
+        }
+        guard !frameIds.isEmpty else { return 0 }
+        let handle = self.handle
+        let assigned: UInt64 = try await io.run {
+            var n: UInt64 = 0
+            let rc = wax_vs_set_locations(handle, frameIds, latitudes, longitudes, UInt64(frameIds.count), &n)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return n
+        }
+        return Int(assigned)
+    }
+
+    /// `searchBatchWhere` with PhotoRAG's location box in each predicate (wax_vs_search_batch_where_near).
+    public func searchBatchWhereNear(vectors: [[Float]], topK: Int, wheres: [wax_vs_where_near],
+                                     queryWhere: [Int?]) async throws -> [[(frameId: UInt64, score: Float)]] {
+        guard !vectors.isEmpty else { return [] }
+        let dims = dimensions
+        for v in vectors where v.count != dims {
+            throw WaxError.encodingError(reason: "vector dimension mismatch: expected \(dims), got \(v.count)")
+        }
+        let handle = self.handle
+        let cap = min(max(topK, 1), Self.maxResults)
+        return try await io.run {
+            var flat = [Float](); flat.reserveCapacity(vectors.count * dims)
+            for v in vectors { flat.append(contentsOf: v) }
+            let offsets: [UInt64] = [0]
+            let queryFilter = [UInt32](repeating: WAX_VS_NO_FILTER, count: vectors.count)
+            let qw = queryWhere.map { $0.map(UInt32.init) ?? WAX_VS_NO_FILTER }
+            var ids = [UInt64](repeating: 0, count: vectors.count * cap)
+            var scores = [Float](repeating: 0, count: vectors.count * cap)
+            var counts = [UInt32](repeating: 0, count: vectors.count)
+            let rc = wax_vs_search_batch_where_near(handle, flat, UInt32(vectors.count), UInt32(dims), Int64(topK), nil,
+                                                    offsets, nil, 0, queryFilter, wheres, UInt32(wheres.count), qw, &ids,
+                                                    &scores, UInt32(cap), &counts)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return (0..<vectors.count).map { q in (0..<Int(counts[q])).map { (ids[q * cap + $0], scores[q * cap + $0]) } }
+        }
+    }
+
+    /// `searchBatchGroupedWhere` with a location box (wax_vs_search_batch_grouped_where_near): PhotoRAG's location query
+    /// and `timeRange` below the top-k, without a frame allow-list.
+    public func searchBatchGroupedWhereNear(vectors: [[Float]], topGroups: Int, perGroup: Int = 1,
+                                            where predicate: wax_vs_where_near, frameIds: [UInt64] = [],
+                                            allow: Bool = false) async throws
+        -> [[(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])]] {
+        guard !vectors.isEmpty else { return [] }
+        let dims = dimensions
+        for v in vectors where v.count != dims {
+            throw WaxError.encodingError(reason: "vector dimension mismatch: expected \(dims), got \(v.count)")
+        }
+        let handle = self.handle
+        let cap = max(1, min(min(max(topGroups, 1), Self.maxResults) * max(perGroup, 1), Self.maxResults))
+        return try await io.run {
+            var flat = [Float](); flat.reserveCapacity(vectors.count * dims)
+            for v in vectors { flat.append(contentsOf: v) }
+            var w = predicate
+            var ids = [UInt64](repeating: 0, count: vectors.count * cap)
+            var scores = [Float](repeating: 0, count: vectors.count * cap)
+            var groups = [UInt64](repeating: 0, count: vectors.count * cap)
+            var counts = [UInt32](repeating: 0, count: vectors.count)
+            let rc = wax_vs_search_batch_grouped_where_near(handle, flat, UInt32(vectors.count), UInt32(dims),
+                                                            Int64(topGroups), UInt32(max(perGroup, 0)), frameIds,
+                                                            UInt64(frameIds.count), allow ? 0 : 1, &w, &ids, &scores,
+                                                            &groups, UInt32(cap), &counts)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return (0..<vectors.count).map { q in
+                var out: [(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])] = []
+                for i in (q * cap)..<(q * cap + Int(counts[q])) {
+                    if out.last?.groupId != groups[i] { out.append((groups[i], [])) }
+                    out[out.count - 1].hits.append((ids[i], scores[i]))
+                }
+                return out
+            }
+        }
+    }
+
     public func add(frameId: UInt64, vector: [Float]) async throws {
         try await addBatch(frameIds: [frameId], vectors: [vector])
     }

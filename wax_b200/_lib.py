@@ -34,9 +34,15 @@ class Where(C.Structure):
     _fields_ = [("after", C.c_int64), ("before", C.c_int64), ("all_tags", C.c_uint64), ("no_tags", C.c_uint64)]
 
 
+class WhereNear(C.Structure):
+    """wax_vs_where_near (56 bytes)."""
+    _fields_ = [("where", Where), ("latitude", C.c_double), ("longitude", C.c_double), ("radius_m", C.c_double)]
+
+
 # Every symbol include/wax_vs_cuda.h declares, with its signature.  tests/test_abi.py checks this table
 # against the header and against the built library.
 _f32p, _u64p, _u32p, _u8p = C.POINTER(C.c_float), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint8)
+_f64p = C.POINTER(C.c_double)
 _eng = C.c_void_p
 SIGNATURES = {
     "wax_vs_device_count": (C.c_int32, [C.POINTER(C.c_int32)]),
@@ -72,6 +78,15 @@ SIGNATURES = {
     "wax_vs_search_batch_grouped_where": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, C.c_uint32, _u64p,
                                                       C.c_uint64, C.c_int32, C.c_void_p, _u64p, _f32p, _u64p, C.c_uint32,
                                                       _u32p]),
+    "wax_vs_set_locations": (C.c_int32, [_eng, _u64p, _f64p, _f64p, C.c_uint64, _u64p]),
+    "wax_vs_location_box": (C.c_int32, [C.c_double, C.c_double, C.c_double, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "wax_vs_location_bin": (C.c_int32, [C.c_double, C.c_double, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "wax_vs_search_batch_where_near": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _u64p,
+                                                   C.POINTER(C.c_int32), C.c_uint32, _u32p, C.c_void_p, C.c_uint32,
+                                                   _u32p, _u64p, _f32p, C.c_uint32, _u32p]),
+    "wax_vs_search_batch_grouped_where_near": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, C.c_uint32,
+                                                           _u64p, C.c_uint64, C.c_int32, C.c_void_p, _u64p, _f32p, _u64p,
+                                                           C.c_uint32, _u32p]),
     "wax_vs_search_batch": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _f32p,
                                         C.c_uint32, _u32p]),
     "wax_vs_search_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, C.c_uint64, C.c_void_p,

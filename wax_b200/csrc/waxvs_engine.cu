@@ -259,6 +259,7 @@ struct SearchCtx {
     unsigned long long host_seq = 0;               // last value the flag was asked to take
     DevBuf<WhereItem> d_where_items;               // where search: predicates of the count / compaction / bitset launches
     DevBuf<uint32_t> d_where_counts;               // where search: rows passing each predicate, then compaction cursors
+    DevBuf<WhereNearItem> d_where_near_items;      // where_near search: the same launches' predicates with their boxes
     DevBuf<uint32_t> d_proof_count;                // shadow route: [0] proofs that held, [1] that failed (guarded scan) ...
     PinnedBuf<uint32_t> h_proof_count;             // ... and their mapped host mirror
     uint32_t seen_failed = 0;                      // h_proof_count[1] when the host last looked
@@ -369,6 +370,15 @@ struct wax_vs_engine {
     bool attrs_dev_valid = false;
     std::mutex attrs_mu;
     uint64_t attribute_uploads = 0;    // instrumentation (pool_mu)
+    // Frame locations (wax_vs_set_locations): locs[r] = row r's PhotoRAG bins, kept aligned with `ids` by every mutator
+    // exactly as `attrs` is.  Empty while locs_set is false: then no row has a location.  The device mirror (8 bytes
+    // per row) is the attribute mirror's twin: invalidated with it, rebuilt under attrs_mu by the first where_near search
+    // that needs it.
+    bool locs_set = false;
+    std::vector<LocRow> locs;
+    DevBuf<LocRow> d_locs;
+    bool locs_dev_valid = false;
+    uint64_t location_uploads = 0;     // instrumentation (pool_mu)
     uint64_t grouped_batch_covered_queries = 0, grouped_batch_expanded_groups = 0, grouped_batch_fallback_queries = 0;
     // Adaptive level choice: when more than a quarter of a batch fails the coarse bf16 bound (tightly clustered
     // neighbours), the next 16 batches nominate in TF32 straight away, then bf16 is probed again.
@@ -441,6 +451,7 @@ static void invalidate_row_caches(wax_vs_engine *e, uint64_t keep_prefix) {
     e->u4.invalidate(keep_prefix);
     e->gindex.valid = false;           // appends too: the new rows need index entries
     e->attrs_dev_valid = false;        // likewise the attribute mirror
+    e->locs_dev_valid = false;         // and the location mirror
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1999,6 +2010,7 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
         e->ids.insert(e->ids.end(), frame_ids, frame_ids + n);
         if (e->groups_set) e->groups.insert(e->groups.end(), frame_ids, frame_ids + n);   // a new frame is its own group
         if (e->attrs_set) e->attrs.resize(e->attrs.size() + n, AttrRow{0, 0});               // ... and has no attributes
+        if (e->locs_set) e->locs.resize(e->locs.size() + n, LocRow{kNoLocation, 0});         // ... nor a location
         for (uint64_t i = 0; i < n; ++i) target[i] = static_cast<uint32_t>(n0 + i);
         e->n_rows += n;
         e->map_valid = false;
@@ -2016,6 +2028,7 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
                 e->ids.push_back(frame_ids[i]);
                 if (e->groups_set) e->groups.push_back(frame_ids[i]);    // an upsert of a known frame keeps its group
                 if (e->attrs_set) e->attrs.push_back(AttrRow{0, 0});     // ... and its attributes
+                if (e->locs_set) e->locs.push_back(LocRow{kNoLocation, 0});   // ... and its location
                 if (!e->ids_sorted) e->map.put(frame_ids[i], row);
                 else e->map_valid = false;
                 ++e->n_rows;
@@ -2134,10 +2147,12 @@ int32_t wax_vs_remove_batch(wax_vs_engine *e, const uint64_t *frame_ids, uint64_
         e->ids[first + j] = e->ids[src[j]];
         if (e->groups_set) e->groups[first + j] = e->groups[src[j]];
         if (e->attrs_set) e->attrs[first + j] = e->attrs[src[j]];
+        if (e->locs_set) e->locs[first + j] = e->locs[src[j]];
     }
     e->ids.resize(new_n);
     if (e->groups_set) e->groups.resize(new_n);
     if (e->attrs_set) e->attrs.resize(new_n);
+    if (e->locs_set) e->locs.resize(new_n);
     e->n_rows = new_n;
     e->map_valid = false;
     e->d_ids_dirty = true;
@@ -2513,6 +2528,9 @@ struct FilterSet {
     std::vector<WherePred> preds;
     std::vector<WhereItem> compact;
     uint64_t device_rows = 0;
+    // Where_near search only (near true): boxes[j] is preds[j]'s location box, compact_boxes[j] compact[j]'s.
+    bool near = false;
+    std::vector<LocBox> boxes, compact_boxes;
 };
 // query_filter = nullptr: every filter is resolved (the single-filter entry points).
 static void resolve_filters(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *filter_offsets, uint32_t n_filters,
@@ -2853,13 +2871,28 @@ int32_t wax_vs_merge_candidates_device(wax_vs_engine *e, const wax_vs_candidate 
 
 // ---- frame attributes on the device (waxvs_where.cuh) --------------------------------------------------------------
 // The attribute mirror of the current corpus, built on c's stream by the first search after a mutation or
-// set_attributes that needs it.  Readers hold the read lock; attrs_mu serialises the build, which completes before the
-// mirror is published.
-static int32_t ensure_attributes(wax_vs_engine *e, SearchCtx *c) {
-    std::lock_guard<std::mutex> lk(e->attrs_mu);
-    if (e->attrs_dev_valid) return WAX_VS_OK;
+// set_attributes that needs it; with `locations`, the location mirror too (after a mutation or set_locations).  Readers
+// hold the read lock; attrs_mu serialises the builds, each of which completes before its mirror is published.
+static int32_t ensure_locations(wax_vs_engine *e, SearchCtx *c) {
+    if (e->locs_dev_valid) return WAX_VS_OK;
     const size_t n = static_cast<size_t>(e->n_rows);
     int32_t rc;
+    if ((rc = e->d_locs.ensure(std::max<size_t>(n, 1), "row locations"))) return rc;
+    const std::vector<LocRow> none(e->locs_set ? 0 : n, LocRow{kNoLocation, 0});            // never set: no row has one
+    CUDA_TRY(cudaMemcpyAsync(e->d_locs, e->locs_set ? e->locs.data() : none.data(), n * sizeof(LocRow),
+                             cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    e->locs_dev_valid = true;
+    std::lock_guard<std::mutex> pg(e->pool_mu);
+    ++e->location_uploads;
+    return WAX_VS_OK;
+}
+static int32_t ensure_attributes(wax_vs_engine *e, SearchCtx *c, bool locations = false) {
+    std::lock_guard<std::mutex> lk(e->attrs_mu);
+    int32_t rc;
+    if (locations && (rc = ensure_locations(e, c))) return rc;
+    if (e->attrs_dev_valid) return WAX_VS_OK;
+    const size_t n = static_cast<size_t>(e->n_rows);
     if ((rc = e->d_attrs.ensure(std::max<size_t>(n, 1), "row attributes"))) return rc;
     if (e->attrs_set) CUDA_TRY(cudaMemcpyAsync(e->d_attrs, e->attrs.data(), n * sizeof(AttrRow), cudaMemcpyHostToDevice, c->stream));
     else CUDA_TRY(cudaMemsetAsync(e->d_attrs, 0, n * sizeof(AttrRow), c->stream));    // never set: timestamp 0, tags 0
@@ -2875,34 +2908,66 @@ static int where_grid(const wax_vs_engine *e, uint64_t threads) {
                                                                      (threads + kWhereThreads - 1) / kWhereThreads)));
 }
 
-// counts[i] = the rows passing preds[i]: one streaming pass per kWhereChunk predicates, read back once.
-static int32_t where_counts(wax_vs_engine *e, SearchCtx *c, const std::vector<WherePred> &preds, std::vector<uint32_t> &counts) {
+// The location form's items: items[i] with boxes[i], staged into c->d_where_near_items on `stream`.
+static int32_t stage_near_items(SearchCtx *c, const std::vector<WhereItem> &items, const std::vector<LocBox> &boxes,
+                                cudaStream_t stream) {
+    const uint32_t m = static_cast<uint32_t>(items.size());
+    int32_t rc;
+    if ((rc = c->d_where_near_items.ensure(m, "where_near predicates"))) return rc;
+    std::vector<WhereNearItem> near(m);
+    for (uint32_t i = 0; i < m; ++i) near[i] = WhereNearItem{items[i].pred, items[i].slot, boxes[i]};
+    CUDA_TRY(cudaMemcpyAsync(c->d_where_near_items, near.data(), m * sizeof(WhereNearItem), cudaMemcpyHostToDevice, stream));
+    return WAX_VS_OK;
+}
+
+// counts[i] = the rows passing preds[i] (and with `boxes`, in boxes[i]): one streaming pass per kWhereChunk predicates,
+// read back once.
+static int32_t where_counts(wax_vs_engine *e, SearchCtx *c, const std::vector<WherePred> &preds, std::vector<uint32_t> &counts,
+                            const std::vector<LocBox> *boxes = nullptr) {
     const uint32_t m = static_cast<uint32_t>(preds.size()), n = static_cast<uint32_t>(e->n_rows);
     counts.assign(m, 0u);
     if (!m) return WAX_VS_OK;
     int32_t rc;
-    if ((rc = ensure_attributes(e, c))) return rc;
+    if ((rc = ensure_attributes(e, c, boxes != nullptr))) return rc;
     if ((rc = c->d_where_items.ensure(m, "where predicates")) || (rc = c->d_where_counts.ensure(m, "where counts"))) return rc;
     std::vector<WhereItem> items(m);
     for (uint32_t i = 0; i < m; ++i) items[i] = WhereItem{preds[i], 0};
-    CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemsetAsync(c->d_where_counts, 0, m * sizeof(uint32_t), c->stream));
-    for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk)
-        where_count_kernel<<<where_grid(e, n), kWhereThreads, 0, c->stream>>>(e->d_attrs, n, c->d_where_items + i0,
-                                                                             std::min(kWhereChunk, m - i0), c->d_where_counts + i0);
+    if (boxes) {
+        if ((rc = stage_near_items(c, items, *boxes, c->stream))) return rc;
+        for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk)
+            where_near_count_kernel<<<where_grid(e, n), kWhereThreads, 0, c->stream>>>(
+                e->d_attrs, e->d_locs, n, c->d_where_near_items + i0, std::min(kWhereChunk, m - i0), c->d_where_counts + i0);
+    } else {
+        CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, c->stream));
+        for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk)
+            where_count_kernel<<<where_grid(e, n), kWhereThreads, 0, c->stream>>>(e->d_attrs, n, c->d_where_items + i0,
+                                                                                 std::min(kWhereChunk, m - i0), c->d_where_counts + i0);
+    }
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(counts.data(), c->d_where_counts, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     return WAX_VS_OK;
 }
 
-// ANDs items[i].pred into bitset items[i].slot of c->d_mask on `stream` (after the filter builders wrote it).
+// ANDs items[i].pred (and with `boxes`, boxes[i]) into bitset items[i].slot of c->d_mask on `stream` (after the filter
+// builders wrote it).
 static int32_t apply_where_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereItem> &items, cudaStream_t stream,
-                                uint64_t *launches) {
+                                uint64_t *launches, const std::vector<LocBox> *boxes = nullptr) {
     const uint32_t m = static_cast<uint32_t>(items.size()), n = static_cast<uint32_t>(e->n_rows);
     if (!m) return WAX_VS_OK;
     const uint32_t words = (n + 31u) / 32u;
     int32_t rc;
+    if (boxes) {
+        if ((rc = stage_near_items(c, items, *boxes, stream))) return rc;
+        for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
+            where_near_bits_kernel<<<where_grid(e, static_cast<uint64_t>(words) * 32u), kWhereThreads, 0, stream>>>(
+                e->d_attrs, e->d_locs, n, words, c->d_mask, c->d_where_near_items + i0, std::min(kWhereChunk, m - i0));
+            ++*launches;
+        }
+        CUDA_TRY(cudaGetLastError());
+        return WAX_VS_OK;
+    }
     if ((rc = c->d_where_items.ensure(m, "where predicates"))) return rc;
     CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, stream));
     for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
@@ -2914,12 +2979,25 @@ static int32_t apply_where_bits(wax_vs_engine *e, SearchCtx *c, const std::vecto
     return WAX_VS_OK;
 }
 
-// The rows of the narrow predicates (fs.compact) into c->d_filter_rows at their slots, on `stream`.
+// The rows of the narrow predicates (fs.compact, with `boxes` fs.compact_boxes) into c->d_filter_rows at their slots, on
+// `stream`.
 static int32_t list_where_rows(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereItem> &items, cudaStream_t stream,
-                               uint64_t *launches) {
+                               uint64_t *launches, const std::vector<LocBox> *boxes = nullptr) {
     const uint32_t m = static_cast<uint32_t>(items.size()), n = static_cast<uint32_t>(e->n_rows);
     if (!m) return WAX_VS_OK;
     int32_t rc;
+    if (boxes) {
+        if ((rc = c->d_where_counts.ensure(m, "where cursors")) || (rc = stage_near_items(c, items, *boxes, stream))) return rc;
+        CUDA_TRY(cudaMemsetAsync(c->d_where_counts, 0, m * sizeof(uint32_t), stream));
+        for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
+            where_near_compact_kernel<<<where_grid(e, n), kWhereThreads, 0, stream>>>(
+                e->d_attrs, e->d_locs, n, c->d_where_near_items + i0, std::min(kWhereChunk, m - i0), c->d_where_counts + i0,
+                c->d_filter_rows);
+            ++*launches;
+        }
+        CUDA_TRY(cudaGetLastError());
+        return WAX_VS_OK;
+    }
     if ((rc = c->d_where_items.ensure(m, "where predicates")) || (rc = c->d_where_counts.ensure(m, "where cursors"))) return rc;
     CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, stream));
     CUDA_TRY(cudaMemsetAsync(c->d_where_counts, 0, m * sizeof(uint32_t), stream));
@@ -3001,7 +3079,10 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
     if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
     if ((rc = stage_filter_rows(e, c, rows, rows.size() + fs.device_rows, -1, c->stream, nullptr))) return rc;
     uint64_t launches = 0;
-    if ((rc = list_where_rows(e, c, fs.compact, c->stream, &launches))) { cudaStreamSynchronize(c->stream); return rc; }
+    if ((rc = list_where_rows(e, c, fs.compact, c->stream, &launches, fs.near ? &fs.compact_boxes : nullptr))) {
+        cudaStreamSynchronize(c->stream);
+        return rc;
+    }
 
     // gather class: one concatenated row list, a span per query; the sort grants shared memory for the longest list
     if (n_gather) {
@@ -3073,9 +3154,16 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
                 }
                 if ((prc = build_filter_bits(e, c, spec, nf, c->stream, &launches))) { cudaStreamSynchronize(c->stream); return prc; }
                 std::vector<WhereItem> wbits;                           // where search: the predicates ANDed in
+                std::vector<LocBox> wboxes;                             // ... and in where_near search their boxes
                 for (uint32_t l = 0; l < nf && !fs.where.empty(); ++l)
-                    if (fs.where[which[l]] != WAX_VS_NO_FILTER) wbits.push_back(WhereItem{fs.preds[fs.where[which[l]]], l});
-                if ((prc = apply_where_bits(e, c, wbits, c->stream, &launches))) { cudaStreamSynchronize(c->stream); return prc; }
+                    if (fs.where[which[l]] != WAX_VS_NO_FILTER) {
+                        wbits.push_back(WhereItem{fs.preds[fs.where[which[l]]], l});
+                        if (fs.near) wboxes.push_back(fs.boxes[fs.where[which[l]]]);
+                    }
+                if ((prc = apply_where_bits(e, c, wbits, c->stream, &launches, fs.near ? &wboxes : nullptr))) {
+                    cudaStreamSynchronize(c->stream);
+                    return prc;
+                }
             }
             RowFilter rf{c->d_mask.p, words, nullptr, index.data() + s0};
             const uint32_t nq = s1 - s0;
@@ -3210,21 +3298,28 @@ constexpr uint64_t kWhereGatherRows = 16384;   // the gather class's largest all
 
 static WherePred where_pred(const wax_vs_where &w) { return WherePred{w.after, w.before, w.all_tags, w.no_tags}; }
 
-// The listed rows that pass `w`, appended to `out`.
+// Whether row r lies in box b (a row without a location lies in no box).
+static bool host_loc_passes(const wax_vs_engine *e, const LocBox &b, uint32_t r) {
+    const LocRow l = e->locs_set ? e->locs[r] : LocRow{kNoLocation, 0};
+    return loc_passes(b, l.lat, l.lon);
+}
+
+// The listed rows that pass `w` (and lie in `box` unless that is nullptr), appended to `out`.
 static void host_rows_passing(const wax_vs_engine *e, const WherePred &w, const uint32_t *rows, uint64_t n,
-                              std::vector<uint32_t> &out) {
+                              std::vector<uint32_t> &out, const LocBox *box = nullptr) {
     for (uint64_t i = 0; i < n; ++i) {
         const AttrRow a = e->attrs_set ? e->attrs[rows[i]] : AttrRow{0, 0};
-        if (where_passes(w, a.ts, a.tags)) out.push_back(rows[i]);
+        if (where_passes(w, a.ts, a.tags) && (!box || host_loc_passes(e, *box, rows[i]))) out.push_back(rows[i]);
     }
 }
 
 // The pairs of a call as the filters of `fs` (modes[p], pair_of[i] = query i's pair or WAX_VS_NO_FILTER), from the
-// resolved id filters `ids`.  Runs the count pass on c's stream.
+// resolved id filters `ids`.  Runs the count pass on c's stream.  boxes (where_near search; nullptr otherwise): wheres[w]
+// also requires boxes[w], on the host for allow-lists and in the location forms of the kernels otherwise.
 static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_where *wheres, uint32_t n_wheres,
                                 const uint32_t *query_where, const int32_t *filter_modes, const uint32_t *query_filter,
                                 uint32_t n_queries, const FilterSet &ids, FilterSet &fs, std::vector<int32_t> &modes,
-                                std::vector<uint32_t> &pair_of) {
+                                std::vector<uint32_t> &pair_of, const LocBox *boxes = nullptr) {
     pair_of.assign(n_queries, WAX_VS_NO_FILTER);
     std::unordered_map<uint64_t, uint32_t> index;
     std::vector<std::pair<uint32_t, uint32_t>> pairs;              // (where, id filter)
@@ -3238,15 +3333,18 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_whe
     // the predicates whose count the plan needs: those of pairs without an allow-list
     std::vector<uint32_t> slot(n_wheres, WAX_VS_NO_FILTER);
     std::vector<WherePred> counted;
+    std::vector<LocBox> counted_boxes;
     for (const auto &pr : pairs)
         if (pr.first != WAX_VS_NO_FILTER && (pr.second == WAX_VS_NO_FILTER || filter_modes[pr.second] == 1) &&
             slot[pr.first] == WAX_VS_NO_FILTER) {
             slot[pr.first] = static_cast<uint32_t>(counted.size());
             counted.push_back(where_pred(wheres[pr.first]));
+            if (boxes) counted_boxes.push_back(boxes[pr.first]);
         }
     std::vector<uint32_t> passing;
     int32_t rc;
-    if ((rc = where_counts(e, c, counted, passing))) return rc;
+    if ((rc = where_counts(e, c, counted, passing, boxes ? &counted_boxes : nullptr))) return rc;
+    fs.near = boxes != nullptr;
     const uint32_t np = static_cast<uint32_t>(pairs.size());
     fs.first.assign(np, 0);
     fs.count.assign(np, 0);
@@ -3267,19 +3365,21 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_whe
             continue;
         }
         const WherePred pred = where_pred(wheres[w]);
-        host_rows_passing(e, pred, rows, n_listed, fs.rows);
+        host_rows_passing(e, pred, rows, n_listed, fs.rows, boxes ? &boxes[w] : nullptr);
         fs.count[p] = fs.rows.size() - fs.first[p];
         if (f != WAX_VS_NO_FILTER && filter_modes[f] == 0) continue;          // allow-list AND where: an allow-list
         const uint64_t pass = passing[slot[w]];
         if (fs.count[p] == 0 && pass > 0 && pass <= kWhereGatherRows) {       // narrow: the device lists the rows
             fs.count[p] = pass;
             fs.compact.push_back(WhereItem{pred, 0});
+            if (boxes) fs.compact_boxes.push_back(boxes[w]);
             listed_by_device.push_back(p);
             continue;
         }
         modes[p] = 1;                                                         // deny the listed rows that pass ...
         fs.where[p] = static_cast<uint32_t>(fs.preds.size());                 // ... within the rows that pass
         fs.preds.push_back(pred);
+        if (boxes) fs.boxes.push_back(boxes[w]);
         fs.allowed[p] = pass - fs.count[p];
     }
     uint64_t at = fs.rows.size();                                             // device-listed rows follow the host's
@@ -3293,18 +3393,14 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_whe
     return WAX_VS_OK;
 }
 
-int32_t wax_vs_search_batch_where(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                  int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                  const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                  const wax_vs_where *wheres, uint32_t n_wheres, const uint32_t *query_where,
-                                  uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+// Both batched where entry points after their argument checks; boxes as plan_where_pairs.
+static int32_t search_where_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                 int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                 const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                 const wax_vs_where *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                 uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n,
+                                 const LocBox *boxes) {
     int32_t rc;
-    if ((rc = check_filter_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, out_n)))
-        return rc;
-    if ((n_wheres && !wheres) || (n_queries && !query_where)) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    for (uint32_t i = 0; i < n_queries; ++i)
-        if (query_where[i] != WAX_VS_NO_FILTER && query_where[i] >= n_wheres)
-            return fail(WAX_VS_ERR_ARGUMENT, "query %u names where %u of %u", i, query_where[i], n_wheres);
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
     if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
@@ -3319,7 +3415,7 @@ int32_t wax_vs_search_batch_where(wax_vs_engine *e, const float *queries, uint32
     std::vector<int32_t> modes;
     std::vector<uint32_t> pair_of;
     if ((rc = plan_where_pairs(e, lease.c, wheres, n_wheres, query_where, filter_modes, query_filter, n_queries, ids, fs,
-                               modes, pair_of)))
+                               modes, pair_of, boxes)))
         return rc;
     FilteredPlan plan;
     plan_filtered(e, top_k, modes.data(), pair_of.data(), n_queries, fs, plan);
@@ -3329,6 +3425,181 @@ int32_t wax_vs_search_batch_where(wax_vs_engine *e, const float *queries, uint32
         return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, plan.k_max);
     return deliver_filtered(e, lease.c, queries, modes.data(), static_cast<uint32_t>(modes.size()), pair_of.data(), fs, plan,
                             out_ids, out_scores, out_stride, out_n);
+}
+
+// The argument checks of wax_vs_search_batch_where (and _near), before the empty-engine early return.
+static int32_t check_where_args(wax_vs_engine *e, uint32_t n_queries, const uint64_t *frame_ids,
+                                const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                const uint32_t *query_filter, const void *wheres, uint32_t n_wheres,
+                                const uint32_t *query_where, uint32_t *out_n) {
+    int32_t rc;
+    if ((rc = check_filter_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, out_n)))
+        return rc;
+    if ((n_wheres && !wheres) || (n_queries && !query_where)) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    for (uint32_t i = 0; i < n_queries; ++i)
+        if (query_where[i] != WAX_VS_NO_FILTER && query_where[i] >= n_wheres)
+            return fail(WAX_VS_ERR_ARGUMENT, "query %u names where %u of %u", i, query_where[i], n_wheres);
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_search_batch_where(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                  int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                  const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                  const wax_vs_where *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                  uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    int32_t rc;
+    if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
+                               n_wheres, query_where, out_n)))
+        return rc;
+    return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
+                             query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_stride, out_n, nullptr);
+}
+
+// ---- location predicates: PhotoRAG's location box beside the time and tag clauses (waxvs_where.cuh) -----------------
+constexpr double kSwiftPi = 3.141592653589793;   // Double.pi
+// Swift's min / max (the second operand wins only when it compares so; a NaN operand then loses to the first).
+static double swift_min(double x, double y) { return y < x ? y : x; }
+static double swift_max(double x, double y) { return y >= x ? y : x; }
+// Int(x) for x = floor(...): false where Swift traps (NaN, infinite or outside Int64).
+static bool swift_int(double x, int64_t *out) {
+    if (!(x >= -9223372036854775808.0 && x < 9223372036854775808.0)) return false;
+    *out = static_cast<int64_t>(x);
+    return true;
+}
+static int32_t saturate_bin(double x) {          // floor(v * 100) of a finite v; no box reaches past +-36 000
+    return x >= 2147483647.0 ? INT32_MAX : (x <= -2147483647.0 ? -INT32_MAX : static_cast<int32_t>(x));
+}
+
+// PhotoLocationQuery / PhotoCoordinate (PhotoRAGTypes.swift:33-57) and buildLocationAllowlist
+// (PhotoRAGOrchestrator.swift:788-854) in fp64: the box of bins, or *active = false where Swift returns nil (no location
+// clause; *box is then kNoLocBox).  out4 (optional) = {minLatBin, maxLatBin, minLonBin, maxLonBin} of an active box.
+static int32_t location_box(double lat, double lon, double radius_m, LocBox *box, bool *active, int32_t *out4 = nullptr) {
+    *box = kNoLocBox;
+    *active = false;
+    lat = swift_min(90.0, swift_max(-90.0, lat));
+    lon = swift_min(180.0, swift_max(-180.0, lon));
+    const double radius = swift_max(0.0, radius_m);
+    if (!(radius > 0)) return WAX_VS_OK;
+    const double lat_delta = radius / 111000.0;
+    const double lon_delta = swift_min(180.0, radius / swift_max(1e-6, 111000.0 * std::cos(lat * kSwiftPi / 180)));
+    int64_t b[4];
+    if (!swift_int(std::floor((lat - lat_delta) * 100.0), &b[0]) || !swift_int(std::floor((lat + lat_delta) * 100.0), &b[1]) ||
+        !swift_int(std::floor((lon - lon_delta) * 100.0), &b[2]) || !swift_int(std::floor((lon + lon_delta) * 100.0), &b[3]))
+        return fail(WAX_VS_ERR_ARGUMENT, "location box of (%g, %g, %g m) is not representable", lat, lon, radius_m);
+    const int64_t min_lat = std::max<int64_t>(-9000, b[0]), max_lat = std::min<int64_t>(9000, b[1]);
+    const int64_t min_lon = b[2], max_lon = b[3];                    // |bin| <= 36 000: lon in [-180, 180], delta <= 180
+    const int64_t lat_count = max_lat - min_lat + 1;
+    const int64_t lon_count = min_lon <= max_lon ? max_lon - min_lon + 1 : (18000 - min_lon) + (max_lon + 18000) + 1;
+    if (lat_count <= 0 || lon_count <= 0 || lat_count * lon_count >= 100000) return WAX_VS_OK;
+    const int32_t lo = static_cast<int32_t>(min_lon), hi = static_cast<int32_t>(max_lon);
+    *box = min_lon <= max_lon ? LocBox{static_cast<int32_t>(min_lat), static_cast<int32_t>(max_lat), lo, hi, 1, 0}
+                              : LocBox{static_cast<int32_t>(min_lat), static_cast<int32_t>(max_lat), lo, 18000, -18000, hi};
+    *active = true;
+    if (out4) {
+        out4[0] = static_cast<int32_t>(min_lat); out4[1] = static_cast<int32_t>(max_lat);
+        out4[2] = lo; out4[3] = hi;
+    }
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_location_box(double latitude, double longitude, double radius_m, int32_t out_box[4], int32_t *out_active) {
+    if (!out_box || !out_active) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    LocBox box;
+    bool active;
+    out_box[0] = out_box[1] = out_box[2] = out_box[3] = 0;
+    *out_active = 0;
+    int32_t rc;
+    if ((rc = location_box(latitude, longitude, radius_m, &box, &active, out_box))) return rc;
+    *out_active = active ? 1 : 0;
+    return WAX_VS_OK;
+}
+
+// locationBin(from:) (PhotoRAGOrchestrator.swift:868-875): a NaN pair is "no location"; any other non-finite coordinate
+// is an argument error.
+static int32_t location_bin(double lat, double lon, LocRow *out) {
+    if (std::isnan(lat) && std::isnan(lon)) { *out = LocRow{kNoLocation, 0}; return WAX_VS_OK; }
+    if (!std::isfinite(lat) || !std::isfinite(lon))
+        return fail(WAX_VS_ERR_ARGUMENT, "location (%g, %g) is not finite (a NaN pair clears a location)", lat, lon);
+    *out = LocRow{saturate_bin(std::floor(lat * 100.0)), saturate_bin(std::floor(lon * 100.0))};
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_location_bin(double latitude, double longitude, int32_t out_bin[2], int32_t *out_has) {
+    if (!out_bin || !out_has) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    LocRow l{kNoLocation, 0};
+    int32_t rc;
+    if ((rc = location_bin(latitude, longitude, &l))) return rc;
+    *out_has = l.lat != kNoLocation;
+    out_bin[0] = *out_has ? l.lat : 0;
+    out_bin[1] = *out_has ? l.lon : 0;
+    return WAX_VS_OK;
+}
+
+// Upsert by frame id as set_attributes; every coordinate pair is checked before anything is written.
+int32_t wax_vs_set_locations(wax_vs_engine *e, const uint64_t *frame_ids, const double *latitudes, const double *longitudes,
+                             uint64_t n, uint64_t *out_assigned) {
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    if (out_assigned) *out_assigned = 0;
+    if (n == 0) return WAX_VS_OK;
+    if (!frame_ids || !latitudes || !longitudes) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    std::vector<LocRow> bins(n);
+    int32_t rc;
+    for (uint64_t i = 0; i < n; ++i)
+        if ((rc = location_bin(latitudes[i], longitudes[i], &bins[i]))) return rc;
+    std::unique_lock<std::shared_mutex> w(e->rw);
+    DeviceGuard g(e->device);
+    drain_device_path(e);
+    if (!e->locs_set) {                // from implicit (no row has a location) to an explicit column
+        e->locs.assign(e->n_rows, LocRow{kNoLocation, 0});
+        e->locs_set = true;
+    }
+    std::vector<uint32_t> written(static_cast<size_t>((e->n_rows + 31) / 32), 0u);
+    uint64_t assigned = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        const uint32_t row = row_of(e, frame_ids[i]);
+        if (row == 0xFFFFFFFFu) continue;                // unknown frame: ignored
+        e->locs[row] = bins[i];                          // a later entry for the same frame wins
+        const uint32_t wd = row >> 5, b = 1u << (row & 31u);
+        if (!(written[wd] & b)) { written[wd] |= b; ++assigned; }
+    }
+    e->locs_dev_valid = false;
+    if (out_assigned) *out_assigned = assigned;
+    return WAX_VS_OK;
+}
+
+// The time and tag clauses of wheres[i] and their boxes; *any = some box is active.
+static int32_t split_near(const wax_vs_where_near *wheres, uint32_t n_wheres, std::vector<wax_vs_where> &plain,
+                          std::vector<LocBox> &boxes, bool *any) {
+    plain.resize(n_wheres);
+    boxes.resize(n_wheres);
+    *any = false;
+    for (uint32_t i = 0; i < n_wheres; ++i) {
+        plain[i] = wheres[i].where;
+        bool active;
+        int32_t rc;
+        if ((rc = location_box(wheres[i].latitude, wheres[i].longitude, wheres[i].radius_m, &boxes[i], &active))) return rc;
+        *any = *any || active;
+    }
+    return WAX_VS_OK;
+}
+
+// A call whose boxes are all "no location clause" is wax_vs_search_batch_where with the time and tag clauses.
+int32_t wax_vs_search_batch_where_near(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                       int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                       const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                       const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                       uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    int32_t rc;
+    if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
+                               n_wheres, query_where, out_n)))
+        return rc;
+    std::vector<wax_vs_where> plain;
+    std::vector<LocBox> boxes;
+    bool any;
+    if ((rc = split_near(wheres, n_wheres, plain, boxes, &any))) return rc;
+    return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
+                             query_filter, plain.data(), n_wheres, query_where, out_ids, out_scores, out_stride, out_n,
+                             any ? boxes.data() : nullptr);
 }
 
 // The row-sharded form: every rank passes the SAME ids; a rank resolves the ones its shard holds (the others are
@@ -3559,7 +3830,8 @@ static uint32_t deliver_group_keys(const wax_vs_engine *e, const uint64_t *keys,
 // row), the answer at out_* and *out_n.  The arguments are checked by the caller.
 static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, uint32_t n_top, uint32_t per_group,
                            const std::vector<uint32_t> *rows, int32_t mode, const WherePred *where, uint64_t *out_ids,
-                           float *out_scores, uint64_t *out_groups, uint32_t *out_n) {
+                           float *out_scores, uint64_t *out_groups, uint32_t *out_n,
+                           const std::vector<LocBox> *where_box = nullptr) {
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const bool filtered = rows != nullptr;
     cudaStream_t s = c->stream;
@@ -3574,7 +3846,7 @@ static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, u
     if ((rc = c->h_out.ensure(n_top, "result staging"))) return rc;
     if (filtered) {
         if ((rc = stage_filter_rows(e, c, *rows, rows->size(), mode, s, &launches)) ||
-            (where && (rc = apply_where_bits(e, c, {WhereItem{*where, 0}}, s, &launches)))) {
+            (where && (rc = apply_where_bits(e, c, {WhereItem{*where, 0}}, s, &launches, where_box)))) {
             cudaStreamSynchronize(s);
             return rc;
         }
@@ -3726,7 +3998,8 @@ static int32_t enqueue_batch_expansion(wax_vs_engine *e, SearchCtx *c, const Cov
 static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                    int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
                                    int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
-                                   uint32_t out_stride, uint32_t *out_n, bool batched, const wax_vs_where *where = nullptr) {
+                                   uint32_t out_stride, uint32_t *out_n, bool batched, const wax_vs_where *where = nullptr,
+                                   const LocBox *box = nullptr) {
     if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (per_group == 0 || per_group > WAX_VS_MAX_PER_GROUP)
         return fail(WAX_VS_ERR_ARGUMENT, "per_group must be in [1, %d] (got %u)", WAX_VS_MAX_PER_GROUP, per_group);
@@ -3761,19 +4034,23 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     // deny-list's rows that pass (mode 1) with the predicate ANDed into every bitset built from it (where_bits)
     WherePred pred{};
     bool where_bits = false;
+    const std::vector<LocBox> one_box(box ? 1 : 0, box ? *box : kNoLocBox);   // where_near: the predicate's box
+    const std::vector<LocBox> *pred_box = box ? &one_box : nullptr;
     if (where) {
         pred = where_pred(*where);
         std::vector<uint32_t> kept;
-        host_rows_passing(e, pred, fs.rows.data(), fs.rows.size(), kept);
+        host_rows_passing(e, pred, fs.rows.data(), fs.rows.size(), kept, box);
         fs.rows.swap(kept);
         fs.count[0] = fs.rows.size();
         if (mode == 0 && fs.rows.empty()) return WAX_VS_OK;                           // nothing allowed
         if (mode == 1) {
             std::vector<uint32_t> pass;
-            if ((rc = where_counts(e, c, {pred}, pass))) return rc;
+            if ((rc = where_counts(e, c, {pred}, pass, pred_box))) return rc;
             if (pass[0] == fs.rows.size()) return WAX_VS_OK;                          // nothing passes but denied rows
             fs.where.assign(1, 0);
             fs.preds.assign(1, pred);
+            fs.near = box != nullptr;
+            if (box) fs.boxes.assign(1, *box);
             fs.allowed.assign(1, pass[0] - fs.rows.size());
             where_bits = true;
         }
@@ -3781,7 +4058,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     const WherePred *row_where = where_bits ? &pred : nullptr;
     if (!batched)
         return grouped_one(e, c, queries, n_top, per_group, filtered ? &fs.rows : nullptr, mode, row_where, out_ids,
-                           out_scores, out_groups, out_n);
+                           out_scores, out_groups, out_n, pred_box);
     const std::vector<uint32_t> query_filter(n_queries, filtered ? 0u : WAX_VS_NO_FILTER);
     // The coverage level: each query's exact top-k_c rows, when the batch goes to the tensor-core levels or the gather
     // class of the batched filtered search; every other batch runs the single-query pipeline per query.
@@ -3828,7 +4105,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
             if (filtered) {                          // the expansion consults the filter's bitset (rows staged by run_filtered)
                 const std::vector<uint64_t> spec = {0, fs.rows.size(), 0, static_cast<uint64_t>(mode)};
                 if ((rc = build_filter_bits(e, c, spec, 1, s, &launches)) ||
-                    (row_where && (rc = apply_where_bits(e, c, {WhereItem{pred, 0}}, s, &launches)))) {
+                    (row_where && (rc = apply_where_bits(e, c, {WhereItem{pred, 0}}, s, &launches, pred_box)))) {
                     cudaStreamSynchronize(s);
                     return rc;
                 }
@@ -3855,7 +4132,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     for (uint32_t qi : crowded) {
         const size_t o = static_cast<size_t>(qi) * out_stride;
         if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group, filtered ? &fs.rows : nullptr,
-                              mode, row_where, out_ids + o, out_scores + o, out_groups + o, out_n + qi)))
+                              mode, row_where, out_ids + o, out_scores + o, out_groups + o, out_n + qi, pred_box)))
             return rc;
     }
     std::lock_guard<std::mutex> pg(e->pool_mu);
@@ -3888,6 +4165,22 @@ int32_t wax_vs_search_batch_grouped_where(wax_vs_engine *e, const float *queries
     if (!where) return fail(WAX_VS_ERR_NULL, "where is NULL");
     return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
                                out_scores, out_groups, out_stride, out_n, n_queries > 1, where);
+}
+
+// A predicate whose box is "no location clause" is wax_vs_search_batch_grouped_where with its time and tag clauses.
+int32_t wax_vs_search_batch_grouped_where_near(wax_vs_engine *e, const float *queries, uint32_t n_queries,
+                                               uint32_t query_len, int64_t top_groups, uint32_t per_group,
+                                               const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                                               const wax_vs_where_near *where, uint64_t *out_ids, float *out_scores,
+                                               uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n) {
+    if (!where) return fail(WAX_VS_ERR_NULL, "where is NULL");
+    LocBox box;
+    bool active;
+    int32_t rc;
+    if ((rc = location_box(where->latitude, where->longitude, where->radius_m, &box, &active))) return rc;
+    return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
+                               out_scores, out_groups, out_stride, out_n, n_queries > 1, &where->where,
+                               active ? &box : nullptr);
 }
 
 // ---- persistence ---------------------------------------------------------------------------------------------
@@ -3979,6 +4272,8 @@ int32_t wax_vs_deserialize(wax_vs_engine *e, const uint8_t *src, uint64_t len) {
     e->groups.clear(); e->groups.shrink_to_fit();
     e->attrs_set = false;                   // nor attributes: the caller re-applies them (wax_vs_set_attributes)
     e->attrs.clear(); e->attrs.shrink_to_fit();
+    e->locs_set = false;
+    e->locs.clear(); e->locs.shrink_to_fit();
     invalidate_row_caches(e, 0);
     return WAX_VS_OK;
 }
@@ -4017,6 +4312,8 @@ int32_t wax_vs_debug_fill_synthetic(wax_vs_engine *e, uint64_t seed, uint64_t fi
     e->groups.clear(); e->groups.shrink_to_fit();
     e->attrs_set = false;
     e->attrs.clear(); e->attrs.shrink_to_fit();
+    e->locs_set = false;
+    e->locs.clear(); e->locs.shrink_to_fit();
     invalidate_row_caches(e, 0);
     return WAX_VS_OK;
 }
@@ -4217,6 +4514,7 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "filter_bitset_passes")) *out = e->filter_bitset_passes;   // per-query filters: tensor sub-batches
     else if (!strcmp(name, "group_index_builds")) *out = e->group_index_builds;       // grouped search: device index builds
     else if (!strcmp(name, "attribute_uploads")) *out = e->attribute_uploads;         // where search: attribute mirror builds
+    else if (!strcmp(name, "location_uploads")) *out = e->location_uploads;           // where_near search: location mirror builds
     else if (!strcmp(name, "grouped_batch_covered_queries")) *out = e->grouped_batch_covered_queries;     // answered by the coverage level
     else if (!strcmp(name, "grouped_batch_expanded_groups")) *out = e->grouped_batch_expanded_groups;     // (query, group) expansions
     else if (!strcmp(name, "grouped_batch_fallback_queries")) *out = e->grouped_batch_fallback_queries;   // single-query pipeline

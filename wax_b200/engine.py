@@ -114,14 +114,50 @@ class Where:
     before: int = L.INT64_MAX
     all_tags: int = 0
     no_tags: int = 0
+    # PhotoRAG's location clause (wax_vs_where_near): (latitude, longitude, radius_m), the frames in the box of 0.01-degree
+    # bins buildLocationAllowlist would union (see location_box).  None: no location clause.
+    near: Optional[Tuple[float, float, float]] = None
 
-    def passes(self, timestamp: int, tags: int) -> bool:
-        """The predicate on the host, as the device evaluates it."""
-        return (self.after <= timestamp and (timestamp < self.before or self.before == L.INT64_MAX)
-                and (tags & self.all_tags) == self.all_tags and (tags & self.no_tags) == 0)
+    def passes(self, timestamp: int, tags: int, location: Optional[Tuple[int, int]] = None) -> bool:
+        """The predicate on the host, as the device evaluates it; `location` is the frame's (latBin, lonBin) or None."""
+        if not (self.after <= timestamp and (timestamp < self.before or self.before == L.INT64_MAX)
+                and (tags & self.all_tags) == self.all_tags and (tags & self.no_tags) == 0):
+            return False
+        box = None if self.near is None else location_box(*self.near)
+        if box is None:
+            return True
+        if location is None:
+            return False
+        lat_lo, lat_hi, lon_lo, lon_hi = box
+        lat_bin, lon_bin = location
+        lon_in = lon_lo <= lon_bin <= lon_hi if lon_lo <= lon_hi else (lon_lo <= lon_bin <= 18000 or -18000 <= lon_bin <= lon_hi)
+        return lat_lo <= lat_bin <= lat_hi and lon_in
 
     def to_c(self) -> "L.Where":
         return L.Where(int(self.after), int(self.before), int(self.all_tags), int(self.no_tags))
+
+    def to_c_near(self) -> "L.WhereNear":
+        lat, lon, radius = self.near if self.near is not None else (0.0, 0.0, 0.0)
+        return L.WhereNear(self.to_c(), float(lat), float(lon), float(radius))
+
+
+def location_box(latitude: float, longitude: float, radius_m: float) -> Optional[Tuple[int, int, int, int]]:
+    """PhotoRAG's box of bins for a location query (wax_vs_location_box): (minLatBin, maxLatBin, minLonBin, maxLonBin),
+    the lon bins wrapping as [minLonBin, 18000] and [-18000, maxLonBin] when minLonBin > maxLonBin, or None where
+    buildLocationAllowlist returns nil (no location clause).  Raises WaxError where Swift's Int(_:) would trap."""
+    box = (C.c_int32 * 4)()
+    active = C.c_int32(0)
+    _check(L.lib().wax_vs_location_box(float(latitude), float(longitude), float(radius_m), box, C.byref(active)))
+    return tuple(int(x) for x in box) if active.value else None
+
+
+def location_bin(latitude: float, longitude: float) -> Optional[Tuple[int, int]]:
+    """A frame's (latBin, lonBin) as set_locations stores it (wax_vs_location_bin): locationBin(from:); None for a NaN
+    pair (no location)."""
+    out = (C.c_int32 * 2)()
+    has = C.c_int32(0)
+    _check(L.lib().wax_vs_location_bin(float(latitude), float(longitude), out, C.byref(has)))
+    return (int(out[0]), int(out[1])) if has.value else None
 
 
 def _clamp_topk(top_k: int) -> int:
@@ -420,6 +456,26 @@ class CUDAVectorEngine:
             tg.ctypes.data_as(C.POINTER(C.c_uint64)) if tg is not None else None, fids.size, C.byref(n)))
         return n.value
 
+    def set_locations(self, frame_ids: Sequence[int], latitudes: Sequence[float], longitudes: Sequence[float]) -> int:
+        """Set frames' locations in degrees (wax_vs_set_locations): upsert by frame id, unknown frames ignored, a later
+        entry for the same frame wins, a NaN pair clears a location.  A frame never given one has none and passes no
+        location clause.  Locations are not serialized: re-apply them after deserialize().  Returns the number of
+        distinct known frames named."""
+        fids = np.ascontiguousarray(frame_ids, dtype=np.uint64).reshape(-1)
+        lat = np.ascontiguousarray(latitudes, dtype=np.float64).reshape(-1)
+        lon = np.ascontiguousarray(longitudes, dtype=np.float64).reshape(-1)
+        if lat.size != fids.size or lon.size != fids.size:
+            raise ValueError(f"set_locations: {fids.size} frame ids for {lat.size} latitudes and {lon.size} longitudes")
+        if fids.size == 0:
+            return 0
+        n = C.c_uint64(0)
+        _check(L.lib().wax_vs_set_locations(
+            self._h, fids.ctypes.data_as(C.POINTER(C.c_uint64)), lat.ctypes.data_as(C.POINTER(C.c_double)),
+            lon.ctypes.data_as(C.POINTER(C.c_double)), fids.size, C.byref(n)))
+        return n.value
+
+    location_box = staticmethod(location_box)
+
     def search_where(self, vector: Sequence[float], top_k: int, where: "Where", allow: Optional[Sequence[int]] = None,
                      deny: Optional[Sequence[int]] = None) -> List[Tuple[int, float]]:
         """The best `top_k` frames passing `where` (and the optional id filter allow= / deny=): the batch of one of
@@ -454,12 +510,17 @@ class CUDAVectorEngine:
         modes_arr = np.asarray(modes, np.int32)
         qf = np.asarray([L.NO_FILTER if f is None else int(f) for f in query_filter], np.uint32)
         qw = np.asarray([L.NO_FILTER if w is None else int(w) for w in query_where], np.uint32)
-        warr = (L.Where * max(len(wheres), 1))(*[w.to_c() for w in wheres])
+        near = any(w.near is not None for w in wheres)       # wax_vs_search_batch_where_near only when a box is asked
+        if near:
+            warr = (L.WhereNear * max(len(wheres), 1))(*[w.to_c_near() for w in wheres])
+        else:
+            warr = (L.Where * max(len(wheres), 1))(*[w.to_c() for w in wheres])
         cap = _clamp_topk(top_k)
         ids = np.zeros((b, cap), np.uint64)
         scores = np.zeros((b, cap), np.float32)
         ns = np.zeros(b, np.uint32)
-        _check(L.lib().wax_vs_search_batch_where(
+        entry = L.lib().wax_vs_search_batch_where_near if near else L.lib().wax_vs_search_batch_where
+        _check(entry(
             self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_k),
             fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
             offsets.ctypes.data_as(C.POINTER(C.c_uint64)), modes_arr.ctypes.data_as(C.POINTER(C.c_int32)), len(lists),
@@ -487,8 +548,10 @@ class CUDAVectorEngine:
         scores = np.empty((b, cap), np.float32)
         groups = np.empty((b, cap), np.uint64)
         ns = np.zeros(b, np.uint32)
-        w = where.to_c()
-        _check(L.lib().wax_vs_search_batch_grouped_where(
+        w = where.to_c() if where.near is None else where.to_c_near()
+        entry = L.lib().wax_vs_search_batch_grouped_where if where.near is None else \
+            L.lib().wax_vs_search_batch_grouped_where_near
+        _check(entry(
             self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_groups), int(per_group),
             fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None, fids.size, mode,
             C.cast(C.pointer(w), C.c_void_p), ids.ctypes.data_as(C.POINTER(C.c_uint64)),

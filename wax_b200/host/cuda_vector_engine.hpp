@@ -346,6 +346,79 @@ public:
         return out;
     }
 
+    // Frame locations in degrees (wax_vs_set_locations): upsert; a NaN pair clears a frame's location.  Not serialized:
+    // re-apply them after deserialize().
+    uint64_t setLocations(const std::vector<uint64_t> &frameIds, const std::vector<double> &latitudes,
+                          const std::vector<double> &longitudes) {
+        if (latitudes.size() != frameIds.size() || longitudes.size() != frameIds.size())
+            throw EncodingError("setLocations: column length != frameIds.count");
+        uint64_t assigned = 0;
+        if (frameIds.empty()) return 0;
+        check(wax_vs_set_locations(h_, frameIds.data(), latitudes.data(), longitudes.data(), frameIds.size(), &assigned));
+        return assigned;
+    }
+
+    // searchBatchWhere with PhotoRAG's location box in each predicate (wax_vs_search_batch_where_near).
+    std::vector<std::vector<Hit>> searchBatchWhereNear(const std::vector<std::vector<float>> &vectors, int64_t topK,
+                                                       const std::vector<wax_vs_where_near> &wheres,
+                                                       const std::vector<uint32_t> &queryWhere) const {
+        std::vector<std::vector<Hit>> out(vectors.size());
+        if (vectors.empty()) return out;
+        if (queryWhere.size() != vectors.size()) throw EncodingError("searchBatchWhereNear: queryWhere.count != vectors.count");
+        const uint32_t lim = static_cast<uint32_t>(topK < 1 ? 1 : (topK > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topK));
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchWhereNear: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        const uint64_t offsets[1] = {0};
+        const std::vector<uint32_t> queryFilter(vectors.size(), WAX_VS_NO_FILTER);
+        std::vector<uint64_t> ids(vectors.size() * lim);
+        std::vector<float> scores(vectors.size() * lim);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_where_near(h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_, topK,
+                                             nullptr, offsets, nullptr, 0, queryFilter.data(), wheres.data(),
+                                             static_cast<uint32_t>(wheres.size()), queryWhere.data(), ids.data(),
+                                             scores.data(), lim, ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) out[q].push_back({ids[q * lim + i], scores[q * lim + i]});
+        return out;
+    }
+
+    // searchBatchGroupedWhere with a location box (wax_vs_search_batch_grouped_where_near).
+    std::vector<std::vector<Group>> searchBatchGroupedWhereNear(const std::vector<std::vector<float>> &vectors,
+                                                                int64_t topGroups, uint32_t perGroup,
+                                                                const wax_vs_where_near &where,
+                                                                const std::vector<uint64_t> &frameIds = {},
+                                                                bool allow = false) const {
+        std::vector<std::vector<Group>> out(vectors.size());
+        if (vectors.empty()) return out;
+        const int64_t lim = topGroups < 1 ? 1 : (topGroups > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topGroups);
+        const int64_t want = lim * (perGroup ? perGroup : 1);
+        const size_t cap = static_cast<size_t>(want > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : want);
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchGroupedWhereNear: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        std::vector<uint64_t> ids(vectors.size() * cap), groups(vectors.size() * cap);
+        std::vector<float> scores(vectors.size() * cap);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_grouped_where_near(h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_,
+                                                     topGroups, perGroup, frameIds.data(), frameIds.size(), allow ? 0 : 1,
+                                                     &where, ids.data(), scores.data(), groups.data(),
+                                                     static_cast<uint32_t>(cap), ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) {
+                const size_t j = q * cap + i;
+                if (out[q].empty() || out[q].back().first != groups[j]) out[q].push_back({groups[j], {}});
+                out[q].back().second.push_back({ids[j], scores[j]});
+            }
+        return out;
+    }
+
     // static load(from:metric:dimensions:) (MetalVectorEngine.swift:318-328): the committed blob (may be empty = none
     // committed yet), then the pending embedding mutations as ONE upsert batch (sequential semantics in the library).
     static CUDAVectorEngine *load(const std::vector<uint8_t> *committedBlob, const std::vector<uint64_t> &pendingIds,
