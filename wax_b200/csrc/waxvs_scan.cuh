@@ -373,7 +373,9 @@ __device__ __forceinline__ void finish_u4_nominees(const ScanParams &p, WarpTopK
 #pragma unroll
         for (int j = 0; j < E; ++j) f(tk.key[j]);
     };
-    const uint64_t xa = block_select_kth(own_keys, kU4CtaNominees, &ss);     // synchronises: s_cut is initialised
+    // block_select_kth needs at least kU4CtaNominees keys in the CTA, NONE included; one warp holds only 32 E: then
+    // every real key is selected (the barrier below publishes s_cut)
+    const uint64_t xa = nthr * E >= kU4CtaNominees ? block_select_kth(own_keys, kU4CtaNominees, &ss) : WAXVS_KEY_NONE;
     if (tid == 0) ss.n_sel = 0;
     __syncthreads();
     uint64_t *mine = p.nominees + static_cast<size_t>(blockIdx.x) * kU4CtaNominees;
