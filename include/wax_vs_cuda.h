@@ -351,6 +351,47 @@ int32_t wax_vs_search_batch_grouped_where_near(wax_vs_engine *engine, const floa
                                                const wax_vs_where_near *where, uint64_t *out_ids, float *out_scores,
                                                uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n);
 
+/* ---- frame terms: Wax's metadataFilter as term clauses below the top-k (API EXTENSION) --------------------------------
+   MetadataFilter (SearchRequest.swift:130-145) requires exact key = value entries of meta.metadata.entries, TagPairs of
+   meta.tags and strings of meta.labels (UnifiedSearch.matches(metadataFilter:meta:), UnifiedSearch.swift:1215-1239).
+   Here each row may carry a set of 64-bit term ids, assigned by the caller (the bindings intern Wax's three kinds of
+   requirement exactly), and a where may require up to 32 of them.
+
+   Frame side: terms follow their rows as locations do: an appended frame has none, an upsert keeps the frame's set,
+   removes drop them, wax_vs_deserialize and wax_vs_debug_fill_synthetic reset every row (MV2V has no place for them, and
+   nothing is stored until the first wax_vs_set_terms).  The first where_terms search after a mutation or
+   wax_vs_set_terms builds a device inverted index (counters "term_index_builds", "term_index_bytes").
+
+   Query side: a row passes a where's term clause when its set holds every required id; an empty list is no clause, and
+   a row without terms passes no non-empty clause (Swift's answer for a nil meta.metadata). */
+/* Replace the whole term set of each named frame (upsert by frame id, as wax_vs_set_attributes): frame_ids[i] ->
+   terms[term_offsets[i] .. term_offsets[i + 1]).  Duplicate ids in a list are kept once, an empty list clears the set,
+   unknown frame ids are ignored and a later entry for the same frame wins; *out_assigned (optional) = distinct known
+   frames named.  NULL term_offsets, frame_ids (n > 0) or terms (a non-empty list) -> WAX_VS_ERR_NULL; offsets that do
+   not start at 0 or decrease -> WAX_VS_ERR_ARGUMENT, and nothing is written.  A mutator (write lock). */
+int32_t wax_vs_set_terms(wax_vs_engine *engine, const uint64_t *frame_ids, const uint64_t *term_offsets,
+                         const uint64_t *terms, uint64_t n, uint64_t *out_assigned);
+/* wax_vs_search_batch_where_near with a term clause in each where: where w requires
+   where_terms[where_term_offsets[w] .. where_term_offsets[w + 1]) (0 to 32 ids, duplicates allowed).  Query i's answer
+   is identical to wax_vs_search_batch_multi_filtered under an allow-list of exactly the frames that hold every required
+   id and pass the time, tag and location clauses and the id filter: same ids, order and score bits.  The argument checks
+   of wax_vs_search_batch_where_near, and NULL where_term_offsets or where_terms (some where has a term) ->
+   WAX_VS_ERR_NULL, offsets that do not start at 0 or decrease, or more than 32 ids in a where -> WAX_VS_ERR_ARGUMENT,
+   run before the empty-engine early return.  A call in which no where has a term runs wax_vs_search_batch_where_near.
+   How: wheres with terms and equal contents are one unit.  A (where, id filter) pair with terms is tested on the host
+   against an allow-list; otherwise the device resolves each required id's posting list, takes the rarest one's rows as
+   candidates (O(its length), never a pass over the corpus), checks the other terms, the where's clauses and a
+   deny-list on each, and counts the rows that pass: <= 16 384 rows are listed and scored as a gather, wider units get
+   their bits set in a row bitset under the filter_bitset_bytes split.  A call whose listed rows would pass 2^32 - 1
+   -> WAX_VS_ERR_CAPACITY.  Grouped search takes no term clause. */
+int32_t wax_vs_search_batch_where_terms(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                        uint32_t query_len, int64_t top_k, const uint64_t *frame_ids,
+                                        const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                        const uint32_t *query_filter, const wax_vs_where_near *wheres, uint32_t n_wheres,
+                                        const uint32_t *query_where, const uint64_t *where_term_offsets,
+                                        const uint64_t *where_terms, uint64_t *out_ids, float *out_scores,
+                                        uint32_t out_stride, uint32_t *out_n);
+
 /* Device-resident form used by the row-sharded engine: `d_queries` (n_queries x dims) and
    `d_candidates` (n_queries x k_eff entries, k_eff = min(clamp(top_k), 10000) -- NOT clipped to N, padding
    has valid = 0) are DEVICE pointers on the engine's device; the work is enqueued on `cuda_stream`
@@ -481,7 +522,8 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *engine, uint64_t *tensor_queries
    "shadow_bytes" (HBM held by the bf16 shadow), "shadow_unavailable" (1 = the shadow did not fit in HBM, batches
    nominate in TF32 at about half the rate), "batch_tf32_queries", "filter_bitset_passes" (sub-batches of per-query
    filtered queries on the tensor-core class, wax_vs_search_batch_multi_filtered), "group_index_builds" (device group
-   index builds of wax_vs_search_grouped), "attribute_uploads" (device attribute copies of the where searches), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
+   index builds of wax_vs_search_grouped), "attribute_uploads" (device attribute copies of the where searches),
+   "term_index_builds" / "term_index_bytes" (term index builds of the where_terms searches / HBM the index holds), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
    (single queries the shadow route answered / that the fp32 scan answered after a failed proof, either shadow; read them
    while no search is running), "single_int8_queries" (single queries whose route nominated from the int8 shadow),
    "int8_shadow_bytes" / "int8_shadow_rows" (HBM held by the int8 shadow's live rows, codes and scales / rows it covers),

@@ -338,6 +338,62 @@ public actor CUDAVectorEngine {
         }
     }
 
+    /// Frame term sets (wax_vs_set_terms): each named frame's whole set is replaced, an empty list clears it.  The caller
+    /// interns `("entry", key, value)`, `("tag", key, value)` and `("label", s)` exactly, so that `searchBatchWhereTerms`
+    /// is `matches(metadataFilter:meta:)` below the top-k.  Not part of MV2V: re-apply after `deserialize`.
+    @discardableResult
+    public func setTerms(frameIds: [UInt64], termLists: [[UInt64]]) async throws -> Int {
+        guard termLists.count == frameIds.count else {
+            throw WaxError.encodingError(reason: "setTerms: termLists.count != frameIds.count")
+        }
+        guard !frameIds.isEmpty else { return 0 }
+        let handle = self.handle
+        let assigned: UInt64 = try await io.run {
+            var offsets: [UInt64] = [0]
+            var flat = [UInt64]()
+            for t in termLists { flat.append(contentsOf: t); offsets.append(UInt64(flat.count)) }
+            var n: UInt64 = 0
+            let rc = wax_vs_set_terms(handle, frameIds, offsets, flat, UInt64(frameIds.count), &n)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return n
+        }
+        return Int(assigned)
+    }
+
+    /// `searchBatchWhereNear` with the term ids each where requires (wax_vs_search_batch_where_terms), at most 32 per
+    /// where: a session-scoped `wax_recall` without a frame allow-list.
+    public func searchBatchWhereTerms(vectors: [[Float]], topK: Int, wheres: [wax_vs_where_near], whereTerms: [[UInt64]],
+                                      queryWhere: [Int?]) async throws -> [[(frameId: UInt64, score: Float)]] {
+        guard !vectors.isEmpty else { return [] }
+        guard whereTerms.count == wheres.count else {
+            throw WaxError.encodingError(reason: "searchBatchWhereTerms: whereTerms.count != wheres.count")
+        }
+        let dims = dimensions
+        for v in vectors where v.count != dims {
+            throw WaxError.encodingError(reason: "vector dimension mismatch: expected \(dims), got \(v.count)")
+        }
+        let handle = self.handle
+        let cap = min(max(topK, 1), Self.maxResults)
+        return try await io.run {
+            var flat = [Float](); flat.reserveCapacity(vectors.count * dims)
+            for v in vectors { flat.append(contentsOf: v) }
+            var termOffsets: [UInt64] = [0]
+            var terms = [UInt64]()
+            for t in whereTerms { terms.append(contentsOf: t); termOffsets.append(UInt64(terms.count)) }
+            let offsets: [UInt64] = [0]
+            let queryFilter = [UInt32](repeating: WAX_VS_NO_FILTER, count: vectors.count)
+            let qw = queryWhere.map { $0.map(UInt32.init) ?? WAX_VS_NO_FILTER }
+            var ids = [UInt64](repeating: 0, count: vectors.count * cap)
+            var scores = [Float](repeating: 0, count: vectors.count * cap)
+            var counts = [UInt32](repeating: 0, count: vectors.count)
+            let rc = wax_vs_search_batch_where_terms(handle, flat, UInt32(vectors.count), UInt32(dims), Int64(topK), nil,
+                                                     offsets, nil, 0, queryFilter, wheres, UInt32(wheres.count), qw,
+                                                     termOffsets, terms, &ids, &scores, UInt32(cap), &counts)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return (0..<vectors.count).map { q in (0..<Int(counts[q])).map { (ids[q * cap + $0], scores[q * cap + $0]) } }
+        }
+    }
+
     /// `searchBatchGroupedWhere` with a location box (wax_vs_search_batch_grouped_where_near): PhotoRAG's location query
     /// and `timeRange` below the top-k, without a frame allow-list.
     public func searchBatchGroupedWhereNear(vectors: [[Float]], topGroups: Int, perGroup: Int = 1,

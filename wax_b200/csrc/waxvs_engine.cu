@@ -39,6 +39,7 @@
 #include "waxvs_group.cuh"
 #include "waxvs_group_batch.cuh"
 #include "waxvs_where.cuh"
+#include "waxvs_terms.cuh"
 
 #include <cub/cub.cuh>
 #include <cudaTypedefs.h>
@@ -260,6 +261,11 @@ struct SearchCtx {
     DevBuf<WhereItem> d_where_items;               // where search: predicates of the count / compaction / bitset launches
     DevBuf<uint32_t> d_where_counts;               // where search: rows passing each predicate, then compaction cursors
     DevBuf<WhereNearItem> d_where_near_items;      // where_near search: the same launches' predicates with their boxes
+    DevBuf<uint64_t> d_term_ids;                   // where_terms search: the call's distinct required term ids ...
+    DevBuf<TermSpan> d_term_spans;                 // ... their posting spans
+    DevBuf<TermUnit> d_term_units;                 // ... the units of term_filter_kernel
+    DevBuf<uint32_t> d_term_counts;                // ... their counts, then listing cursors
+    DevBuf<uint32_t> d_term_deny;                  // ... and their deny-lists' rows, each list ascending
     DevBuf<uint32_t> d_proof_count;                // shadow route: [0] proofs that held, [1] that failed (guarded scan) ...
     PinnedBuf<uint32_t> h_proof_count;             // ... and their mapped host mirror
     uint32_t seen_failed = 0;                      // h_proof_count[1] when the host last looked
@@ -379,6 +385,29 @@ struct wax_vs_engine {
     DevBuf<LocRow> d_locs;
     bool locs_dev_valid = false;
     uint64_t location_uploads = 0;     // instrumentation (pool_mu)
+    // Frame terms (wax_vs_set_terms): row r's sorted, distinct term ids are term_pool[term_refs[r].off, + .n), kept
+    // aligned with `ids` by every mutator exactly as `attrs` is.  A set_terms appends to the pool and repoints the row;
+    // term_garbage counts the pool entries no row points at, and the pool is compacted when they pass half of it.  Empty
+    // while terms_set is false: then no row has a term.
+    struct TermRef {
+        uint64_t off;
+        uint32_t n;
+    };
+    bool terms_set = false;
+    std::vector<TermRef> term_refs;
+    std::vector<uint64_t> term_pool;
+    uint64_t term_garbage = 0;
+    // Device inverted index for the term clauses (waxvs_terms.cuh), a cache like the group index: every mutator and
+    // set_terms invalidate it; the first where_terms search after that rebuilds it under term_mu.
+    struct TermIndex {
+        DevBuf<uint64_t> keys, start;
+        DevBuf<uint32_t> postings;
+        uint32_t n_terms = 0;
+        uint64_t n_postings = 0;
+        bool valid = false;
+    } tindex;
+    std::mutex term_mu;
+    uint64_t term_index_builds = 0;    // instrumentation (pool_mu)
     uint64_t grouped_batch_covered_queries = 0, grouped_batch_expanded_groups = 0, grouped_batch_fallback_queries = 0;
     // Adaptive level choice: when more than a quarter of a batch fails the coarse bf16 bound (tightly clustered
     // neighbours), the next 16 batches nominate in TF32 straight away, then bf16 is probed again.
@@ -452,6 +481,33 @@ static void invalidate_row_caches(wax_vs_engine *e, uint64_t keep_prefix) {
     e->gindex.valid = false;           // appends too: the new rows need index entries
     e->attrs_dev_valid = false;        // likewise the attribute mirror
     e->locs_dev_valid = false;         // and the location mirror
+    e->tindex.valid = false;           // and the term index
+}
+
+// The term pool rewritten in row order once more than half of it is garbage (set_terms, remove_batch).
+static void compact_term_pool(wax_vs_engine *e) {
+    if (e->term_garbage * 2 <= e->term_pool.size()) return;
+    std::vector<uint64_t> pool;
+    pool.reserve(e->term_pool.size() - e->term_garbage);
+    for (auto &t : e->term_refs) {
+        const uint64_t off = pool.size();
+        pool.insert(pool.end(), e->term_pool.begin() + t.off, e->term_pool.begin() + t.off + t.n);
+        t.off = t.n ? off : 0;
+    }
+    e->term_pool.swap(pool);
+    e->term_garbage = 0;
+}
+// No row has terms (deserialize, fill_synthetic): MV2V has no place for them.
+static void clear_terms(wax_vs_engine *e) {
+    e->terms_set = false;
+    e->term_refs.clear(); e->term_refs.shrink_to_fit();
+    e->term_pool.clear(); e->term_pool.shrink_to_fit();
+    e->term_garbage = 0;
+    auto &ti = e->tindex;              // the index goes with them (invalidate_row_caches would only mark it stale)
+    ti.keys.release(); ti.start.release(); ti.postings.release();
+    ti.n_terms = 0;
+    ti.n_postings = 0;
+    ti.valid = false;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -2011,6 +2067,7 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
         if (e->groups_set) e->groups.insert(e->groups.end(), frame_ids, frame_ids + n);   // a new frame is its own group
         if (e->attrs_set) e->attrs.resize(e->attrs.size() + n, AttrRow{0, 0});               // ... and has no attributes
         if (e->locs_set) e->locs.resize(e->locs.size() + n, LocRow{kNoLocation, 0});         // ... nor a location
+        if (e->terms_set) e->term_refs.resize(e->term_refs.size() + n, wax_vs_engine::TermRef{0, 0});   // ... nor terms
         for (uint64_t i = 0; i < n; ++i) target[i] = static_cast<uint32_t>(n0 + i);
         e->n_rows += n;
         e->map_valid = false;
@@ -2029,6 +2086,7 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
                 if (e->groups_set) e->groups.push_back(frame_ids[i]);    // an upsert of a known frame keeps its group
                 if (e->attrs_set) e->attrs.push_back(AttrRow{0, 0});     // ... and its attributes
                 if (e->locs_set) e->locs.push_back(LocRow{kNoLocation, 0});   // ... and its location
+                if (e->terms_set) e->term_refs.push_back(wax_vs_engine::TermRef{0, 0});   // ... and its terms
                 if (!e->ids_sorted) e->map.put(frame_ids[i], row);
                 else e->map_valid = false;
                 ++e->n_rows;
@@ -2143,16 +2201,23 @@ int32_t wax_vs_remove_batch(wax_vs_engine *e, const uint64_t *frame_ids, uint64_
     }
     tr.mark("compact matrix");
     // ids: one compaction, one hash rebuild (lazily, on the next lookup)
+    if (e->terms_set)
+        for (const uint32_t r : gone) e->term_garbage += e->term_refs[r].n;   // the removed rows' pool entries
     for (uint64_t j = 0; j < moving; ++j) {
         e->ids[first + j] = e->ids[src[j]];
         if (e->groups_set) e->groups[first + j] = e->groups[src[j]];
         if (e->attrs_set) e->attrs[first + j] = e->attrs[src[j]];
         if (e->locs_set) e->locs[first + j] = e->locs[src[j]];
+        if (e->terms_set) e->term_refs[first + j] = e->term_refs[src[j]];
     }
     e->ids.resize(new_n);
     if (e->groups_set) e->groups.resize(new_n);
     if (e->attrs_set) e->attrs.resize(new_n);
     if (e->locs_set) e->locs.resize(new_n);
+    if (e->terms_set) {
+        e->term_refs.resize(new_n);
+        compact_term_pool(e);
+    }
     e->n_rows = new_n;
     e->map_valid = false;
     e->d_ids_dirty = true;
@@ -2531,6 +2596,11 @@ struct FilterSet {
     // Where_near search only (near true): boxes[j] is preds[j]'s location box, compact_boxes[j] compact[j]'s.
     bool near = false;
     std::vector<LocBox> boxes, compact_boxes;
+    // Where_terms search only (plan_term_units): the narrow term units, whose rows the device lists at their slots after
+    // the compact rows, and the wide ones, whose rows the device sets in their filter's bitset; term_of[f] = filter f's
+    // wide unit in term_wide (empty, or WAX_VS_NO_FILTER, when it has none: its rows are the listed ones).
+    std::vector<TermUnit> term_list, term_wide;
+    std::vector<uint32_t> term_of;
 };
 // query_filter = nullptr: every filter is resolved (the single-filter entry points).
 static void resolve_filters(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *filter_offsets, uint32_t n_filters,
@@ -2903,6 +2973,77 @@ static int32_t ensure_attributes(wax_vs_engine *e, SearchCtx *c, bool locations 
     return WAX_VS_OK;
 }
 
+// The term index of the current corpus and term lists (waxvs_terms.cuh), built on c's stream by the first where_terms
+// search after a mutation or set_terms: the (term, row) pairs in row order, radix-sorted by term with CUB (stable, so
+// each posting list stays in ascending row order), the heads flagged and prefix-summed into term_keys / term_start.  The
+// sort takes an int item count (as the group index's), so more than 2^31 - 1 pairs is refused.  Readers hold the read
+// lock; term_mu serialises the build, which completes before the index is published.
+static int32_t ensure_term_index(wax_vs_engine *e, SearchCtx *c) {
+    std::lock_guard<std::mutex> lk(e->term_mu);
+    auto &ti = e->tindex;
+    if (ti.valid) return WAX_VS_OK;
+    uint64_t n_pairs = 0;
+    if (e->terms_set)
+        for (const auto &t : e->term_refs) n_pairs += t.n;
+    if (n_pairs > static_cast<uint64_t>(INT32_MAX))
+        return fail(WAX_VS_ERR_CAPACITY, "term index of %llu (term, row) pairs: at most %d are supported",
+                    static_cast<unsigned long long>(n_pairs), INT32_MAX);
+    const uint32_t P = static_cast<uint32_t>(n_pairs);
+    cudaStream_t s = c->stream;
+    int32_t rc;
+    uint32_t n_terms = 0;
+    if ((rc = ti.postings.ensure(std::max<uint32_t>(P, 1), "term postings"))) return rc;
+    if (P) {
+        std::vector<uint64_t> h_keys(P);
+        std::vector<uint32_t> h_rows(P);
+        for (uint64_t r = 0, at = 0; r < e->n_rows; ++r) {
+            const auto &t = e->term_refs[r];
+            for (uint32_t j = 0; j < t.n; ++j, ++at) {
+                h_keys[at] = e->term_pool[t.off + j];
+                h_rows[at] = static_cast<uint32_t>(r);
+            }
+        }
+        DevBuf<uint64_t> keys_in, keys_out;
+        DevBuf<uint32_t> rows_in, heads, incl;
+        DevBuf<uint8_t> temp;
+        size_t sort_bytes = 0, scan_bytes = 0;
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys_in.p, keys_out.p, rows_in.p, ti.postings.p,
+                                                 static_cast<int>(P), 0, 64, s));
+        CUDA_TRY(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, heads.p, incl.p, static_cast<int>(P), s));
+        if ((rc = keys_in.ensure(P, "term sort keys")) || (rc = keys_out.ensure(P, "sorted term keys")) ||
+            (rc = rows_in.ensure(P, "term sort rows")) || (rc = heads.ensure(P, "term heads")) ||
+            (rc = incl.ensure(P, "term numbering")) ||
+            (rc = temp.ensure(std::max<size_t>(std::max(sort_bytes, scan_bytes), 1), "term index scratch")))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(keys_in, h_keys.data(), static_cast<size_t>(P) * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+        CUDA_TRY(cudaMemcpyAsync(rows_in, h_rows.data(), static_cast<size_t>(P) * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(temp.p, sort_bytes, keys_in.p, keys_out.p, rows_in.p, ti.postings.p,
+                                                 static_cast<int>(P), 0, 64, s));
+        const int grid = static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 8, (P + 255) / 256)));
+        group_heads_kernel<<<grid, 256, 0, s>>>(keys_out, P, heads);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cub::DeviceScan::InclusiveSum(temp.p, scan_bytes, heads.p, incl.p, static_cast<int>(P), s));
+        CUDA_TRY(cudaMemcpyAsync(&n_terms, incl.p + (P - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if ((rc = ti.keys.ensure(n_terms, "term keys")) || (rc = ti.start.ensure(static_cast<size_t>(n_terms) + 1, "term starts")))
+            return rc;
+        term_index_finish_kernel<<<grid, 256, 0, s>>>(keys_out, incl, P, ti.keys, ti.start);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaStreamSynchronize(s));     // before the scratch goes
+    } else if ((rc = ti.keys.ensure(1, "term keys")) || (rc = ti.start.ensure(1, "term starts"))) {
+        return rc;
+    }
+    const uint64_t end = P;
+    CUDA_TRY(cudaMemcpyAsync(ti.start.p + n_terms, &end, sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    ti.n_terms = n_terms;
+    ti.n_postings = P;
+    ti.valid = true;
+    std::lock_guard<std::mutex> pg(e->pool_mu);
+    ++e->term_index_builds;
+    return WAX_VS_OK;
+}
+
 static int where_grid(const wax_vs_engine *e, uint64_t threads) {
     return static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 8,
                                                                      (threads + kWhereThreads - 1) / kWhereThreads)));
@@ -3011,6 +3152,33 @@ static int32_t list_where_rows(wax_vs_engine *e, SearchCtx *c, const std::vector
     return WAX_VS_OK;
 }
 
+// term_filter_kernel over `units` on `stream` (waxvs_terms.cuh): counting into c->d_term_counts (zeroed here) and, with
+// rows_out, listing each unit's rows at its slot; or, with bits, setting them in bitset `slot` of bits.  plan_term_units
+// sized c->d_term_units and c->d_term_counts for the call's largest launch, so no buffer an earlier launch reads moves.
+static int32_t launch_term_filter(wax_vs_engine *e, SearchCtx *c, const std::vector<TermUnit> &units, uint32_t *rows_out,
+                                  uint32_t *bits, cudaStream_t s, uint64_t *launches) {
+    const uint32_t n = static_cast<uint32_t>(units.size());
+    if (!n) return WAX_VS_OK;
+    int32_t rc;
+    if ((rc = c->d_term_units.ensure(n, "term units")) || (rc = c->d_term_counts.ensure(n, "term counts"))) return rc;
+    if (!bits) CUDA_TRY(cudaMemsetAsync(c->d_term_counts, 0, n * sizeof(uint32_t), s));
+    CUDA_TRY(cudaMemcpyAsync(c->d_term_units, units.data(), n * sizeof(TermUnit), cudaMemcpyHostToDevice, s));
+    const uint32_t words = static_cast<uint32_t>((e->n_rows + 31) / 32);
+    for (uint32_t u0 = 0; u0 < n; u0 += 65535u) {       // grid.y limit
+        const uint32_t nu = std::min<uint32_t>(n - u0, 65535u);
+        uint32_t longest = 1;
+        for (uint32_t j = u0; j < u0 + nu; ++j) longest = std::max(longest, units[j].spans[0].count);
+        const uint32_t spread = std::max<uint32_t>(4, static_cast<uint32_t>(e->sm_count) * 16 / nu);
+        const dim3 grid(std::min<uint32_t>((longest + kTermThreads - 1) / kTermThreads, spread), nu);
+        term_filter_kernel<<<grid, kTermThreads, 0, s>>>(e->tindex.postings, e->d_attrs, e->d_locs, c->d_term_deny,
+                                                         c->d_term_units + u0, bits ? nullptr : c->d_term_counts + u0,
+                                                         rows_out, bits, words);
+        CUDA_TRY(cudaGetLastError());
+        ++*launches;
+    }
+    return WAX_VS_OK;
+}
+
 // ---- batched filtered search ------------------------------------------------------------------------------------
 // n_queries queries, query i under filter query_filter[i] (WAX_VS_NO_FILTER: unfiltered); the single-filter entry
 // points are the case of one filter that every query names.  Every query referenced filter is resolved once; query i
@@ -3079,7 +3247,8 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
     if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
     if ((rc = stage_filter_rows(e, c, rows, rows.size() + fs.device_rows, -1, c->stream, nullptr))) return rc;
     uint64_t launches = 0;
-    if ((rc = list_where_rows(e, c, fs.compact, c->stream, &launches, fs.near ? &fs.compact_boxes : nullptr))) {
+    if ((rc = list_where_rows(e, c, fs.compact, c->stream, &launches, fs.near ? &fs.compact_boxes : nullptr)) ||
+        (rc = launch_term_filter(e, c, fs.term_list, c->d_filter_rows, nullptr, c->stream, &launches))) {
         cudaStreamSynchronize(c->stream);
         return rc;
     }
@@ -3148,7 +3317,8 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
                 const uint32_t nf = static_cast<uint32_t>(which.size());
                 std::vector<uint64_t> spec(3u * nf + 1u, 0);
                 for (uint32_t l = 0; l < nf; ++l) {
-                    spec[l + 1] = spec[l] + count[which[l]];
+                    const bool wide = !fs.term_of.empty() && fs.term_of[which[l]] != WAX_VS_NO_FILTER;
+                    spec[l + 1] = spec[l] + (wide ? 0 : count[which[l]]);     // a wide term unit lists nothing
                     spec[nf + 1 + l] = first[which[l]];
                     spec[2u * nf + 1u + l] = static_cast<uint64_t>(filter_modes[which[l]]);
                 }
@@ -3160,7 +3330,14 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
                         wbits.push_back(WhereItem{fs.preds[fs.where[which[l]]], l});
                         if (fs.near) wboxes.push_back(fs.boxes[fs.where[which[l]]]);
                     }
-                if ((prc = apply_where_bits(e, c, wbits, c->stream, &launches, fs.near ? &wboxes : nullptr))) {
+                std::vector<TermUnit> tbits;                            // where_terms search: wide units' rows
+                for (uint32_t l = 0; l < nf && !fs.term_of.empty(); ++l)
+                    if (fs.term_of[which[l]] != WAX_VS_NO_FILTER) {
+                        tbits.push_back(fs.term_wide[fs.term_of[which[l]]]);
+                        tbits.back().slot = l;
+                    }
+                if ((prc = apply_where_bits(e, c, wbits, c->stream, &launches, fs.near ? &wboxes : nullptr)) ||
+                    (prc = launch_term_filter(e, c, tbits, nullptr, c->d_mask, c->stream, &launches))) {
                     cudaStreamSynchronize(c->stream);
                     return prc;
                 }
@@ -3304,22 +3481,138 @@ static bool host_loc_passes(const wax_vs_engine *e, const LocBox &b, uint32_t r)
     return loc_passes(b, l.lat, l.lon);
 }
 
-// The listed rows that pass `w` (and lie in `box` unless that is nullptr), appended to `out`.
+// Whether row r holds every id of the sorted, distinct list `req` (a row without terms holds none).
+static bool host_terms_pass(const wax_vs_engine *e, const std::vector<uint64_t> &req, uint32_t r) {
+    if (req.empty()) return true;
+    if (!e->terms_set) return false;
+    const auto &t = e->term_refs[r];
+    const uint64_t *p = e->term_pool.data() + t.off;
+    return std::includes(p, p + t.n, req.begin(), req.end());
+}
+
+// The listed rows that pass `w` (and lie in `box` unless that is nullptr, and hold the terms `req` unless that is
+// nullptr), appended to `out`.
 static void host_rows_passing(const wax_vs_engine *e, const WherePred &w, const uint32_t *rows, uint64_t n,
-                              std::vector<uint32_t> &out, const LocBox *box = nullptr) {
+                              std::vector<uint32_t> &out, const LocBox *box = nullptr,
+                              const std::vector<uint64_t> *req = nullptr) {
     for (uint64_t i = 0; i < n; ++i) {
         const AttrRow a = e->attrs_set ? e->attrs[rows[i]] : AttrRow{0, 0};
-        if (where_passes(w, a.ts, a.tags) && (!box || host_loc_passes(e, *box, rows[i]))) out.push_back(rows[i]);
+        if (where_passes(w, a.ts, a.tags) && (!box || host_loc_passes(e, *box, rows[i])) &&
+            (!req || host_terms_pass(e, *req, rows[i])))
+            out.push_back(rows[i]);
     }
+}
+
+// The term units of a call (pairs[p] for p in units_p, whose where has terms and whose id filter is none or a
+// deny-list) on c's stream: the posting span of every distinct required id (one launch, one read-back), then one
+// term_filter_kernel launch counts each unit's rows from the postings of its rarest term (another read-back).  A unit
+// becomes an allow-list of its fs.count[p] rows: a narrow one (<= kWhereGatherRows) is listed by the device in
+// run_filtered at a slot from `at` on, as long as its count; a wide one gets its bits set in its bitset by the device,
+// under the sub-batch split of filter_bitset_bytes.  The lists are therefore bounded as the device-listed where rows
+// are, and no bitset is held outside that split.  A deny-list is checked by binary search in its rows, sorted, in
+// c->d_term_deny.  `at` ends past the last slot.
+static int32_t plan_term_units(wax_vs_engine *e, SearchCtx *c, const wax_vs_where *wheres, const LocBox *boxes,
+                               const std::vector<uint64_t> *terms, const FilterSet &ids,
+                               const std::vector<std::pair<uint32_t, uint32_t>> &pairs, const std::vector<uint32_t> &units_p,
+                               FilterSet &fs, uint64_t &at) {
+    int32_t rc;
+    if ((rc = ensure_term_index(e, c)) || (rc = ensure_attributes(e, c, boxes != nullptr))) return rc;
+    const auto &ti = e->tindex;
+    cudaStream_t s = c->stream;
+    std::vector<uint64_t> req;
+    for (const uint32_t p : units_p) req.insert(req.end(), terms[pairs[p].first].begin(), terms[pairs[p].first].end());
+    std::sort(req.begin(), req.end());
+    req.erase(std::unique(req.begin(), req.end()), req.end());
+    const uint32_t n_ids = static_cast<uint32_t>(req.size());
+    std::vector<TermSpan> spans(n_ids);
+    if ((rc = c->d_term_ids.ensure(n_ids, "required terms")) || (rc = c->d_term_spans.ensure(n_ids, "term spans"))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_term_ids, req.data(), n_ids * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    term_spans_kernel<<<std::max<uint32_t>(1, std::min<uint32_t>((n_ids + 255) / 256, e->sm_count * 8)), 256, 0, s>>>(
+        ti.keys, ti.start, ti.n_terms, c->d_term_ids, n_ids, c->d_term_spans);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(spans.data(), c->d_term_spans, n_ids * sizeof(TermSpan), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+
+    // the deny-lists of the units, each sorted, once per list
+    std::vector<uint32_t> deny_rows;
+    std::unordered_map<uint32_t, TermSpan> deny_of;
+    for (const uint32_t p : units_p) {
+        const uint32_t f = pairs[p].second;
+        if (f == WAX_VS_NO_FILTER || deny_of.count(f)) continue;
+        deny_of[f] = TermSpan{deny_rows.size(), static_cast<uint32_t>(ids.count[f]), 0};
+        deny_rows.insert(deny_rows.end(), ids.rows.begin() + ids.first[f], ids.rows.begin() + ids.first[f] + ids.count[f]);
+        std::sort(deny_rows.end() - ids.count[f], deny_rows.end());
+    }
+    if ((rc = c->d_term_deny.ensure(std::max<size_t>(deny_rows.size(), 1), "term deny-lists"))) return rc;
+    if (!deny_rows.empty())
+        CUDA_TRY(cudaMemcpyAsync(c->d_term_deny, deny_rows.data(), deny_rows.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+
+    // each unit's candidates are the postings of its rarest term; a term no row holds leaves the unit empty
+    std::vector<TermUnit> units;
+    std::vector<uint32_t> unit_pair;
+    for (const uint32_t p : units_p) {
+        const uint32_t w = pairs[p].first, f = pairs[p].second;
+        fs.first[p] = at;
+        fs.count[p] = 0;
+        TermUnit u{};
+        u.pred = where_pred(wheres[w]);
+        const LocBox box = boxes ? boxes[w] : kNoLocBox;
+        u.box = box;
+        u.has_box = box.lat_lo != kNoLocBox.lat_lo || box.lat_hi != kNoLocBox.lat_hi || box.lon_lo0 != kNoLocBox.lon_lo0 ||
+                    box.lon_hi0 != kNoLocBox.lon_hi0 || box.lon_lo1 != kNoLocBox.lon_lo1 || box.lon_hi1 != kNoLocBox.lon_hi1;
+        u.n_spans = static_cast<uint32_t>(terms[w].size());
+        u.deny = f == WAX_VS_NO_FILTER ? TermSpan{0, 0, 0} : deny_of[f];
+        uint32_t rarest = 0;
+        for (uint32_t j = 0; j < u.n_spans; ++j) {
+            u.spans[j] = spans[std::lower_bound(req.begin(), req.end(), terms[w][j]) - req.begin()];
+            if (u.spans[j].count < u.spans[rarest].count) rarest = j;
+        }
+        if (u.spans[rarest].count == 0) continue;
+        std::swap(u.spans[0], u.spans[rarest]);
+        units.push_back(u);
+        unit_pair.push_back(p);
+    }
+    const uint32_t n_units = static_cast<uint32_t>(units.size());
+    if (!n_units) return WAX_VS_OK;
+    // sized once for the largest launch of the call (run_filtered launches subsets of these units)
+    if ((rc = c->d_term_units.ensure(n_units, "term units")) || (rc = c->d_term_counts.ensure(n_units, "term counts")))
+        return rc;
+    uint64_t launches = 0;
+    if ((rc = launch_term_filter(e, c, units, nullptr, nullptr, s, &launches))) { cudaStreamSynchronize(s); return rc; }
+    std::vector<uint32_t> counts(n_units);
+    CUDA_TRY(cudaMemcpyAsync(counts.data(), c->d_term_counts, n_units * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    fs.term_of.assign(fs.count.size(), WAX_VS_NO_FILTER);
+    for (uint32_t j = 0; j < n_units; ++j) {
+        const uint32_t p = unit_pair[j];
+        fs.count[p] = counts[j];
+        if (counts[j] == 0) continue;
+        if (counts[j] <= kWhereGatherRows) {                 // narrow: listed at its slot (the gather class)
+            units[j].slot = at;
+            fs.first[p] = at;
+            at += counts[j];
+            fs.term_list.push_back(units[j]);
+        } else {                                             // wide: its bitset's bits (tensor class)
+            fs.term_of[p] = static_cast<uint32_t>(fs.term_wide.size());
+            fs.term_wide.push_back(units[j]);
+        }
+    }
+    if (at > UINT32_MAX)                                     // the gather spans hold 32-bit offsets
+        return fail(WAX_VS_ERR_CAPACITY, "the filters of one call list %llu rows, at most %u are supported",
+                    static_cast<unsigned long long>(at), UINT32_MAX);
+    return WAX_VS_OK;
 }
 
 // The pairs of a call as the filters of `fs` (modes[p], pair_of[i] = query i's pair or WAX_VS_NO_FILTER), from the
 // resolved id filters `ids`.  Runs the count pass on c's stream.  boxes (where_near search; nullptr otherwise): wheres[w]
-// also requires boxes[w], on the host for allow-lists and in the location forms of the kernels otherwise.
+// also requires boxes[w], on the host for allow-lists and in the location forms of the kernels otherwise.  terms
+// (where_terms search; nullptr otherwise): wheres[w] also requires the sorted, distinct ids terms[w]; a pair whose where
+// has some is tested on the host against an allow-list, and is a term unit (plan_term_units) otherwise.
 static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_where *wheres, uint32_t n_wheres,
                                 const uint32_t *query_where, const int32_t *filter_modes, const uint32_t *query_filter,
                                 uint32_t n_queries, const FilterSet &ids, FilterSet &fs, std::vector<int32_t> &modes,
-                                std::vector<uint32_t> &pair_of, const LocBox *boxes = nullptr) {
+                                std::vector<uint32_t> &pair_of, const LocBox *boxes = nullptr,
+                                const std::vector<uint64_t> *terms = nullptr) {
     pair_of.assign(n_queries, WAX_VS_NO_FILTER);
     std::unordered_map<uint64_t, uint32_t> index;
     std::vector<std::pair<uint32_t, uint32_t>> pairs;              // (where, id filter)
@@ -3336,7 +3629,7 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_whe
     std::vector<LocBox> counted_boxes;
     for (const auto &pr : pairs)
         if (pr.first != WAX_VS_NO_FILTER && (pr.second == WAX_VS_NO_FILTER || filter_modes[pr.second] == 1) &&
-            slot[pr.first] == WAX_VS_NO_FILTER) {
+            slot[pr.first] == WAX_VS_NO_FILTER && !(terms && !terms[pr.first].empty())) {
             slot[pr.first] = static_cast<uint32_t>(counted.size());
             counted.push_back(where_pred(wheres[pr.first]));
             if (boxes) counted_boxes.push_back(boxes[pr.first]);
@@ -3352,7 +3645,7 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_whe
     fs.where.assign(np, WAX_VS_NO_FILTER);
     fs.allowed.assign(np, 0);
     modes.assign(np, 0);
-    std::vector<uint32_t> listed_by_device;
+    std::vector<uint32_t> listed_by_device, term_units;
     for (uint32_t p = 0; p < np; ++p) {
         const uint32_t w = pairs[p].first, f = pairs[p].second;
         const uint32_t *rows = f == WAX_VS_NO_FILTER ? nullptr : ids.rows.data() + ids.first[f];
@@ -3365,7 +3658,12 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_whe
             continue;
         }
         const WherePred pred = where_pred(wheres[w]);
-        host_rows_passing(e, pred, rows, n_listed, fs.rows, boxes ? &boxes[w] : nullptr);
+        const bool has_terms = terms && !terms[w].empty();
+        if (has_terms && (f == WAX_VS_NO_FILTER || filter_modes[f] == 1)) {   // the device lists it from the postings
+            term_units.push_back(p);
+            continue;
+        }
+        host_rows_passing(e, pred, rows, n_listed, fs.rows, boxes ? &boxes[w] : nullptr, has_terms ? &terms[w] : nullptr);
         fs.count[p] = fs.rows.size() - fs.first[p];
         if (f != WAX_VS_NO_FILTER && filter_modes[f] == 0) continue;          // allow-list AND where: an allow-list
         const uint64_t pass = passing[slot[w]];
@@ -3389,17 +3687,18 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_whe
         fs.compact[j].slot = at;
         at += fs.count[p];
     }
+    if (!term_units.empty() && (rc = plan_term_units(e, c, wheres, boxes, terms, ids, pairs, term_units, fs, at))) return rc;
     fs.device_rows = at - fs.rows.size();
     return WAX_VS_OK;
 }
 
-// Both batched where entry points after their argument checks; boxes as plan_where_pairs.
+// The batched where entry points after their argument checks; boxes and terms as plan_where_pairs.
 static int32_t search_where_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                  int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
                                  const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
                                  const wax_vs_where *wheres, uint32_t n_wheres, const uint32_t *query_where,
                                  uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n,
-                                 const LocBox *boxes) {
+                                 const LocBox *boxes, const std::vector<uint64_t> *terms = nullptr) {
     int32_t rc;
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
@@ -3415,7 +3714,7 @@ static int32_t search_where_host(wax_vs_engine *e, const float *queries, uint32_
     std::vector<int32_t> modes;
     std::vector<uint32_t> pair_of;
     if ((rc = plan_where_pairs(e, lease.c, wheres, n_wheres, query_where, filter_modes, query_filter, n_queries, ids, fs,
-                               modes, pair_of, boxes)))
+                               modes, pair_of, boxes, terms)))
         return rc;
     FilteredPlan plan;
     plan_filtered(e, top_k, modes.data(), pair_of.data(), n_queries, fs, plan);
@@ -3600,6 +3899,110 @@ int32_t wax_vs_search_batch_where_near(wax_vs_engine *e, const float *queries, u
     return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
                              query_filter, plain.data(), n_wheres, query_where, out_ids, out_scores, out_stride, out_n,
                              any ? boxes.data() : nullptr);
+}
+
+// ---- term clauses: Wax's metadataFilter as required term ids, from an inverted index (waxvs_terms.cuh) ---------------
+// Offsets of n lists: start at 0, never decrease; with max_len, no list is longer.
+static int32_t check_term_offsets(const uint64_t *offsets, uint64_t n, const uint64_t *terms, uint64_t max_len,
+                                  const char *what) {
+    if (offsets[0] != 0) return fail(WAX_VS_ERR_ARGUMENT, "%s[0] must be 0", what);
+    for (uint64_t i = 0; i < n; ++i) {
+        if (offsets[i + 1] < offsets[i])
+            return fail(WAX_VS_ERR_ARGUMENT, "%s decrease at list %llu", what, static_cast<unsigned long long>(i));
+        if (offsets[i + 1] - offsets[i] > max_len)
+            return fail(WAX_VS_ERR_ARGUMENT, "%s: list %llu has %llu terms, at most %llu are allowed", what,
+                        static_cast<unsigned long long>(i), static_cast<unsigned long long>(offsets[i + 1] - offsets[i]),
+                        static_cast<unsigned long long>(max_len));
+    }
+    if (offsets[n] && !terms) return fail(WAX_VS_ERR_NULL, "term list is NULL");
+    return WAX_VS_OK;
+}
+
+// Replace each named frame's whole term set (upsert by frame id, as set_locations); every list is checked before anything
+// is written.  The new list goes to the end of the pool, the row is repointed, and the pool is compacted when more than
+// half of it is garbage.
+int32_t wax_vs_set_terms(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *term_offsets, const uint64_t *terms,
+                         uint64_t n, uint64_t *out_assigned) {
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    if (out_assigned) *out_assigned = 0;
+    if (!term_offsets) return fail(WAX_VS_ERR_NULL, "term_offsets is NULL");
+    if (n && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    int32_t rc;
+    if ((rc = check_term_offsets(term_offsets, n, terms, UINT32_MAX, "term_offsets"))) return rc;
+    if (n == 0) return WAX_VS_OK;
+    std::unique_lock<std::shared_mutex> w(e->rw);
+    DeviceGuard g(e->device);
+    drain_device_path(e);
+    if (!e->terms_set) {               // from implicit (no row has a term) to explicit lists
+        e->term_refs.assign(e->n_rows, wax_vs_engine::TermRef{0, 0});
+        e->terms_set = true;
+    }
+    std::vector<uint32_t> written(static_cast<size_t>((e->n_rows + 31) / 32), 0u);
+    std::vector<uint64_t> list;
+    uint64_t assigned = 0;
+    for (uint64_t i = 0; i < n; ++i) {
+        const uint32_t row = row_of(e, frame_ids[i]);
+        if (row == 0xFFFFFFFFu) continue;                // unknown frame: ignored
+        list.assign(terms + term_offsets[i], terms + term_offsets[i + 1]);
+        std::sort(list.begin(), list.end());
+        list.erase(std::unique(list.begin(), list.end()), list.end());
+        auto &ref = e->term_refs[row];                   // a later entry for the same frame wins
+        e->term_garbage += ref.n;
+        ref = wax_vs_engine::TermRef{list.empty() ? 0 : e->term_pool.size(), static_cast<uint32_t>(list.size())};
+        e->term_pool.insert(e->term_pool.end(), list.begin(), list.end());
+        const uint32_t wd = row >> 5, b = 1u << (row & 31u);
+        if (!(written[wd] & b)) { written[wd] |= b; ++assigned; }
+    }
+    compact_term_pool(e);
+    e->tindex.valid = false;
+    if (out_assigned) *out_assigned = assigned;
+    return WAX_VS_OK;
+}
+
+// A call none of whose wheres has a term runs wax_vs_search_batch_where_near.
+int32_t wax_vs_search_batch_where_terms(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                        int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                        const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                        const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                        const uint64_t *where_term_offsets, const uint64_t *where_terms,
+                                        uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    int32_t rc;
+    if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
+                               n_wheres, query_where, out_n)))
+        return rc;
+    if (!where_term_offsets) return fail(WAX_VS_ERR_NULL, "where_term_offsets is NULL");
+    if ((rc = check_term_offsets(where_term_offsets, n_wheres, where_terms, kMaxWhereTerms, "where_term_offsets"))) return rc;
+    if (where_term_offsets[n_wheres] == 0)
+        return wax_vs_search_batch_where_near(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets,
+                                              filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids,
+                                              out_scores, out_stride, out_n);
+    std::vector<wax_vs_where> plain;
+    std::vector<LocBox> boxes;
+    bool any;
+    if ((rc = split_near(wheres, n_wheres, plain, boxes, &any))) return rc;
+    std::vector<std::vector<uint64_t>> terms(n_wheres);
+    for (uint32_t w = 0; w < n_wheres; ++w) {
+        terms[w].assign(where_terms + where_term_offsets[w], where_terms + where_term_offsets[w + 1]);
+        std::sort(terms[w].begin(), terms[w].end());
+        terms[w].erase(std::unique(terms[w].begin(), terms[w].end()), terms[w].end());
+    }
+    // Wheres with terms and equal contents (clauses, box, required ids) are one: each query names the first of them, so
+    // a batch that scopes 1 024 queries to 16 sessions plans 16 units, not 1 024.
+    std::vector<uint32_t> canon(n_wheres);
+    std::unordered_map<std::string, uint32_t> first_of;
+    for (uint32_t w = 0; w < n_wheres; ++w) {
+        canon[w] = w;
+        if (terms[w].empty()) continue;
+        std::string key(reinterpret_cast<const char *>(&plain[w]), sizeof(wax_vs_where));
+        key.append(reinterpret_cast<const char *>(&boxes[w]), sizeof(LocBox));
+        key.append(reinterpret_cast<const char *>(terms[w].data()), terms[w].size() * sizeof(uint64_t));
+        canon[w] = first_of.emplace(std::move(key), w).first->second;
+    }
+    std::vector<uint32_t> qw(n_queries);
+    for (uint32_t i = 0; i < n_queries; ++i) qw[i] = query_where[i] == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : canon[query_where[i]];
+    return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
+                             query_filter, plain.data(), n_wheres, qw.data(), out_ids, out_scores, out_stride, out_n,
+                             any ? boxes.data() : nullptr, terms.data());
 }
 
 // The row-sharded form: every rank passes the SAME ids; a rank resolves the ones its shard holds (the others are
@@ -4274,6 +4677,7 @@ int32_t wax_vs_deserialize(wax_vs_engine *e, const uint8_t *src, uint64_t len) {
     e->attrs.clear(); e->attrs.shrink_to_fit();
     e->locs_set = false;
     e->locs.clear(); e->locs.shrink_to_fit();
+    clear_terms(e);
     invalidate_row_caches(e, 0);
     return WAX_VS_OK;
 }
@@ -4314,6 +4718,7 @@ int32_t wax_vs_debug_fill_synthetic(wax_vs_engine *e, uint64_t seed, uint64_t fi
     e->attrs.clear(); e->attrs.shrink_to_fit();
     e->locs_set = false;
     e->locs.clear(); e->locs.shrink_to_fit();
+    clear_terms(e);
     invalidate_row_caches(e, 0);
     return WAX_VS_OK;
 }
@@ -4515,6 +4920,9 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "group_index_builds")) *out = e->group_index_builds;       // grouped search: device index builds
     else if (!strcmp(name, "attribute_uploads")) *out = e->attribute_uploads;         // where search: attribute mirror builds
     else if (!strcmp(name, "location_uploads")) *out = e->location_uploads;           // where_near search: location mirror builds
+    else if (!strcmp(name, "term_index_builds")) *out = e->term_index_builds;         // where_terms search: term index builds
+    else if (!strcmp(name, "term_index_bytes"))                                       // ... and the HBM the index holds
+        *out = e->tindex.keys.cap * sizeof(uint64_t) + e->tindex.start.cap * sizeof(uint64_t) + e->tindex.postings.cap * sizeof(uint32_t);
     else if (!strcmp(name, "grouped_batch_covered_queries")) *out = e->grouped_batch_covered_queries;     // answered by the coverage level
     else if (!strcmp(name, "grouped_batch_expanded_groups")) *out = e->grouped_batch_expanded_groups;     // (query, group) expansions
     else if (!strcmp(name, "grouped_batch_fallback_queries")) *out = e->grouped_batch_fallback_queries;   // single-query pipeline

@@ -117,11 +117,18 @@ class Where:
     # PhotoRAG's location clause (wax_vs_where_near): (latitude, longitude, radius_m), the frames in the box of 0.01-degree
     # bins buildLocationAllowlist would union (see location_box).  None: no location clause.
     near: Optional[Tuple[float, float, float]] = None
+    # Term clause (wax_vs_search_batch_where_terms): up to 32 term ids the frame's set must all hold (see set_terms and
+    # TermDictionary).  Empty: no term clause.
+    terms: Tuple[int, ...] = ()
 
-    def passes(self, timestamp: int, tags: int, location: Optional[Tuple[int, int]] = None) -> bool:
-        """The predicate on the host, as the device evaluates it; `location` is the frame's (latBin, lonBin) or None."""
+    def passes(self, timestamp: int, tags: int, location: Optional[Tuple[int, int]] = None,
+               terms: Optional[Iterable[int]] = None) -> bool:
+        """The predicate on the host, as the device evaluates it; `location` is the frame's (latBin, lonBin) or None,
+        `terms` its term set or None (no terms)."""
         if not (self.after <= timestamp and (timestamp < self.before or self.before == L.INT64_MAX)
                 and (tags & self.all_tags) == self.all_tags and (tags & self.no_tags) == 0):
+            return False
+        if self.terms and not set(int(t) for t in self.terms) <= set(int(t) for t in (terms or ())):
             return False
         box = None if self.near is None else location_box(*self.near)
         if box is None:
@@ -139,6 +146,50 @@ class Where:
     def to_c_near(self) -> "L.WhereNear":
         lat, lon, radius = self.near if self.near is not None else (0.0, 0.0, 0.0)
         return L.WhereNear(self.to_c(), float(lat), float(lon), float(radius))
+
+
+class TermDictionary:
+    """Wax's metadata as term ids (the frame side of set_terms, the query side of Where(terms=...)), by exact interning:
+    ("entry", key, value) for meta.metadata.entries, ("tag", key, value) for meta.tags and ("label", s) for meta.labels
+    each get the next id, so two different requirements never share one and the term clause is exactly
+    UnifiedSearch.matches(metadataFilter:meta:).  A requirement no frame was ever given maps to UNKNOWN, an id the
+    dictionary never assigns, which therefore matches no frame."""
+    UNKNOWN = (1 << 64) - 1
+
+    def __init__(self) -> None:
+        self._ids: dict = {}
+        self._lock = threading.Lock()
+
+    def __len__(self) -> int:
+        return len(self._ids)
+
+    def intern(self, kind: str, *parts: str) -> int:
+        """The id of ("entry", key, value), ("tag", key, value) or ("label", s), assigned on first sight."""
+        if (kind, len(parts)) not in (("entry", 2), ("tag", 2), ("label", 1)):
+            raise ValueError(f"TermDictionary: {kind!r} with {len(parts)} parts")
+        key = (kind,) + tuple(str(p) for p in parts)
+        with self._lock:
+            return self._ids.setdefault(key, len(self._ids))
+
+    def lookup(self, kind: str, *parts: str) -> int:
+        """The id of an interned requirement, or UNKNOWN."""
+        return self._ids.get((kind,) + tuple(str(p) for p in parts), self.UNKNOWN)
+
+    def frame_terms(self, entries: Optional[dict] = None, tags: Iterable[Tuple[str, str]] = (),
+                    labels: Iterable[str] = ()) -> List[int]:
+        """A frame's term set: its metadata entries (None for a nil meta.metadata), TagPairs and labels."""
+        out = [self.intern("entry", k, v) for k, v in (entries or {}).items()]
+        out += [self.intern("tag", k, v) for k, v in tags]
+        out += [self.intern("label", s) for s in labels]
+        return out
+
+    def filter_terms(self, required_entries: Optional[dict] = None, required_tags: Iterable[Tuple[str, str]] = (),
+                     required_labels: Iterable[str] = ()) -> Tuple[int, ...]:
+        """A MetadataFilter's requirements as the term ids a Where requires (duplicates kept once)."""
+        ids = [self.lookup("entry", k, v) for k, v in (required_entries or {}).items()]
+        ids += [self.lookup("tag", k, v) for k, v in required_tags]
+        ids += [self.lookup("label", s) for s in required_labels]
+        return tuple(sorted(set(ids)))
 
 
 def location_box(latitude: float, longitude: float, radius_m: float) -> Optional[Tuple[int, int, int, int]]:
@@ -476,6 +527,24 @@ class CUDAVectorEngine:
 
     location_box = staticmethod(location_box)
 
+    def set_terms(self, frame_ids: Sequence[int], term_lists: Sequence[Sequence[int]]) -> int:
+        """Replace frames' term sets (wax_vs_set_terms): upsert by frame id, unknown frames ignored, a later entry for the
+        same frame wins, duplicate ids kept once, an empty list clears the set.  A frame never given terms has none and
+        passes no non-empty term clause.  Terms are not serialized: re-apply them after deserialize().  Returns the
+        number of distinct known frames named."""
+        fids = np.ascontiguousarray(frame_ids, dtype=np.uint64).reshape(-1)
+        if len(term_lists) != fids.size:
+            raise ValueError(f"set_terms: {fids.size} frame ids for {len(term_lists)} term lists")
+        offsets = np.zeros(fids.size + 1, np.uint64)
+        offsets[1:] = np.cumsum([len(t) for t in term_lists], dtype=np.uint64) if fids.size else []
+        flat = np.fromiter((int(x) for t in term_lists for x in t), dtype=np.uint64, count=int(offsets[-1]))
+        n = C.c_uint64(0)
+        _check(L.lib().wax_vs_set_terms(
+            self._h, fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
+            offsets.ctypes.data_as(C.POINTER(C.c_uint64)), flat.ctypes.data_as(C.POINTER(C.c_uint64)) if flat.size else None,
+            fids.size, C.byref(n)))
+        return n.value
+
     def search_where(self, vector: Sequence[float], top_k: int, where: "Where", allow: Optional[Sequence[int]] = None,
                      deny: Optional[Sequence[int]] = None) -> List[Tuple[int, float]]:
         """The best `top_k` frames passing `where` (and the optional id filter allow= / deny=): the batch of one of
@@ -510,7 +579,8 @@ class CUDAVectorEngine:
         modes_arr = np.asarray(modes, np.int32)
         qf = np.asarray([L.NO_FILTER if f is None else int(f) for f in query_filter], np.uint32)
         qw = np.asarray([L.NO_FILTER if w is None else int(w) for w in query_where], np.uint32)
-        near = any(w.near is not None for w in wheres)       # wax_vs_search_batch_where_near only when a box is asked
+        with_terms = any(len(w.terms) for w in wheres)       # wax_vs_search_batch_where_terms only when a term is asked
+        near = with_terms or any(w.near is not None for w in wheres)   # ... _where_near only when a box is
         if near:
             warr = (L.WhereNear * max(len(wheres), 1))(*[w.to_c_near() for w in wheres])
         else:
@@ -519,14 +589,22 @@ class CUDAVectorEngine:
         ids = np.zeros((b, cap), np.uint64)
         scores = np.zeros((b, cap), np.float32)
         ns = np.zeros(b, np.uint32)
-        entry = L.lib().wax_vs_search_batch_where_near if near else L.lib().wax_vs_search_batch_where
-        _check(entry(
-            self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_k),
-            fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
-            offsets.ctypes.data_as(C.POINTER(C.c_uint64)), modes_arr.ctypes.data_as(C.POINTER(C.c_int32)), len(lists),
-            qf.ctypes.data_as(C.POINTER(C.c_uint32)), C.cast(warr, C.c_void_p), len(wheres),
-            qw.ctypes.data_as(C.POINTER(C.c_uint32)), ids.ctypes.data_as(C.POINTER(C.c_uint64)),
-            scores.ctypes.data_as(C.POINTER(C.c_float)), cap, ns.ctypes.data_as(C.POINTER(C.c_uint32))))
+        head = (self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_k),
+                fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
+                offsets.ctypes.data_as(C.POINTER(C.c_uint64)), modes_arr.ctypes.data_as(C.POINTER(C.c_int32)), len(lists),
+                qf.ctypes.data_as(C.POINTER(C.c_uint32)), C.cast(warr, C.c_void_p), len(wheres),
+                qw.ctypes.data_as(C.POINTER(C.c_uint32)))
+        tail = (ids.ctypes.data_as(C.POINTER(C.c_uint64)), scores.ctypes.data_as(C.POINTER(C.c_float)), cap,
+                ns.ctypes.data_as(C.POINTER(C.c_uint32)))
+        if with_terms:
+            toff = np.zeros(len(wheres) + 1, np.uint64)
+            toff[1:] = np.cumsum([len(w.terms) for w in wheres], dtype=np.uint64)
+            tflat = np.fromiter((int(t) for w in wheres for t in w.terms), dtype=np.uint64, count=int(toff[-1]))
+            _check(L.lib().wax_vs_search_batch_where_terms(*head, toff.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                                           tflat.ctypes.data_as(C.POINTER(C.c_uint64)), *tail))
+        else:
+            entry = L.lib().wax_vs_search_batch_where_near if near else L.lib().wax_vs_search_batch_where
+            _check(entry(*head, *tail))
         return [[(int(ids[i, j]), float(scores[i, j])) for j in range(int(ns[i]))] for i in range(b)]
 
     def search_batch_grouped_where(self, vectors, top_groups: int, per_group: int, where: "Where",
@@ -536,6 +614,8 @@ class CUDAVectorEngine:
         (wax_vs_search_batch_grouped_where); each answer equals search_grouped under the allow-list of those frames."""
         if allow is not None and deny is not None:
             raise ValueError("pass at most one of allow= / deny=")
+        if where.terms:
+            raise ValueError("grouped search takes no term clause")
         fids = np.ascontiguousarray(allow if allow is not None else (deny if deny is not None else []),
                                     dtype=np.uint64).reshape(-1)
         mode = 0 if allow is not None else 1

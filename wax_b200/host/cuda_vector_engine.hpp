@@ -386,6 +386,55 @@ public:
         return out;
     }
 
+    // Frame term sets (wax_vs_set_terms): replace each named frame's set; an empty list clears it.  Not serialized:
+    // re-apply them after deserialize().
+    uint64_t setTerms(const std::vector<uint64_t> &frameIds, const std::vector<std::vector<uint64_t>> &termLists) {
+        if (termLists.size() != frameIds.size()) throw EncodingError("setTerms: termLists.count != frameIds.count");
+        std::vector<uint64_t> offsets(1, 0), flat;
+        for (const auto &t : termLists) {
+            flat.insert(flat.end(), t.begin(), t.end());
+            offsets.push_back(flat.size());
+        }
+        uint64_t assigned = 0;
+        check(wax_vs_set_terms(h_, frameIds.data(), offsets.data(), flat.data(), frameIds.size(), &assigned));
+        return assigned;
+    }
+
+    // searchBatchWhereNear with the term ids each where requires (wax_vs_search_batch_where_terms).
+    std::vector<std::vector<Hit>> searchBatchWhereTerms(const std::vector<std::vector<float>> &vectors, int64_t topK,
+                                                        const std::vector<wax_vs_where_near> &wheres,
+                                                        const std::vector<std::vector<uint64_t>> &whereTerms,
+                                                        const std::vector<uint32_t> &queryWhere) const {
+        std::vector<std::vector<Hit>> out(vectors.size());
+        if (vectors.empty()) return out;
+        if (queryWhere.size() != vectors.size()) throw EncodingError("searchBatchWhereTerms: queryWhere.count != vectors.count");
+        if (whereTerms.size() != wheres.size()) throw EncodingError("searchBatchWhereTerms: whereTerms.count != wheres.count");
+        const uint32_t lim = static_cast<uint32_t>(topK < 1 ? 1 : (topK > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topK));
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchWhereTerms: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        std::vector<uint64_t> termOffsets(1, 0), terms;
+        for (const auto &t : whereTerms) {
+            terms.insert(terms.end(), t.begin(), t.end());
+            termOffsets.push_back(terms.size());
+        }
+        const uint64_t offsets[1] = {0};
+        const std::vector<uint32_t> queryFilter(vectors.size(), WAX_VS_NO_FILTER);
+        std::vector<uint64_t> ids(vectors.size() * lim);
+        std::vector<float> scores(vectors.size() * lim);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_where_terms(h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_, topK,
+                                              nullptr, offsets, nullptr, 0, queryFilter.data(), wheres.data(),
+                                              static_cast<uint32_t>(wheres.size()), queryWhere.data(), termOffsets.data(),
+                                              terms.data(), ids.data(), scores.data(), lim, ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) out[q].push_back({ids[q * lim + i], scores[q * lim + i]});
+        return out;
+    }
+
     // searchBatchGroupedWhere with a location box (wax_vs_search_batch_grouped_where_near).
     std::vector<std::vector<Group>> searchBatchGroupedWhereNear(const std::vector<std::vector<float>> &vectors,
                                                                 int64_t topGroups, uint32_t perGroup,
