@@ -350,6 +350,33 @@ int32_t wax_vs_search_batch_grouped_where_near(wax_vs_engine *engine, const floa
                                                const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
                                                const wax_vs_where_near *where, uint64_t *out_ids, float *out_scores,
                                                uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n);
+/* wax_vs_search_batch_grouped with a where and an id filter of its own for each query (a server batching PhotoRAG /
+   VideoRAG requests from many sessions): query i searches the frames that pass the time, tag and location clauses of
+   wheres[query_where[i]] AND id filter query_filter[i] (either may be WAX_VS_NO_FILTER; both: unfiltered; filters as
+   wax_vs_search_batch_multi_filtered).  Its answer is identical to wax_vs_search_grouped for that query alone under an
+   allow-list of exactly those frames -- same frame ids, group ids, group-major order and score bits -- at
+   out_*[i * out_stride], count out_n[i].  top_groups and per_group hold for the whole batch.  A where whose box is "no
+   location clause" is a time and tag predicate; a where that admits nothing is valid and gives out_n[i] = 0.  There is no
+   term clause: grouped search takes none.  Checked before the empty-engine early return: the checks of
+   wax_vs_search_batch_where_near (filters, query_filter and query_where ranges, NULL arrays, the boxes) and the grouped
+   ones of wax_vs_search_batch_grouped (per_group, clamp(top_groups) * per_group, NULL outputs; out_stride >=
+   min(clamp(top_groups) * per_group, N) else WAX_VS_ERR_BUFFER).  n_queries == 0 returns OK; n_queries == 1 runs the
+   single-query grouped pipeline.
+   How: the (where, id filter) pairs are the units of wax_vs_search_batch_where, each query's exact top-k_c rows come from
+   that batched search, and the coverage level is wax_vs_search_batch_grouped's.  A selected group that must be scored
+   over its own rows is scored under its query's row bitset, rebuilt on the device in passes of at most
+   "filter_bitset_bytes" of distinct units (counter "grouped_batch_expansion_passes").  Crowded queries, and batches the
+   coverage level does not take (a mix of gather and tensor classes among them), run the single-query pipeline, each
+   under its own pair.  wax_vs_search_batch_grouped, _grouped_where and _grouped_where_near are the case of one pair for
+   every query. */
+int32_t wax_vs_search_batch_grouped_multi_where(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                                uint32_t query_len, int64_t top_groups, uint32_t per_group,
+                                                const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                                const int32_t *filter_modes, uint32_t n_filters,
+                                                const uint32_t *query_filter, const wax_vs_where_near *wheres,
+                                                uint32_t n_wheres, const uint32_t *query_where, uint64_t *out_ids,
+                                                float *out_scores, uint64_t *out_groups, uint32_t out_stride,
+                                                uint32_t *out_n);
 
 /* ---- frame terms: Wax's metadataFilter as term clauses below the top-k (API EXTENSION) --------------------------------
    MetadataFilter (SearchRequest.swift:130-145) requires exact key = value entries of meta.metadata.entries, TagPairs of

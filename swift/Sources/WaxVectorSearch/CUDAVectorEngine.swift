@@ -338,6 +338,60 @@ public actor CUDAVectorEngine {
         }
     }
 
+    /// `searchBatchGroupedWhere` with a where and an id filter of each request's own
+    /// (wax_vs_search_batch_grouped_multi_where): a server batching PhotoRAG / VideoRAG requests from many sessions.
+    /// Query i searches the frames passing `wheres[queryWhere[i]]` AND `filters[queryFilter[i]]` (nil: none; a filter is
+    /// its frame ids and whether they are an allow-list); each answer equals `searchGrouped` under the allow-list of
+    /// exactly those frames.
+    public func searchBatchGroupedMultiWhere(vectors: [[Float]], topGroups: Int, perGroup: Int = 1,
+                                             wheres: [wax_vs_where_near], queryWhere: [Int?],
+                                             filters: [(frameIds: [UInt64], allow: Bool)] = [],
+                                             queryFilter: [Int?]? = nil) async throws
+        -> [[(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])]] {
+        guard !vectors.isEmpty else { return [] }
+        let dims = dimensions
+        for v in vectors where v.count != dims {
+            throw WaxError.encodingError(reason: "vector dimension mismatch: expected \(dims), got \(v.count)")
+        }
+        let perQueryFilter = queryFilter ?? [Int?](repeating: nil, count: vectors.count)
+        guard queryWhere.count == vectors.count, perQueryFilter.count == vectors.count else {
+            throw WaxError.encodingError(reason: "searchBatchGroupedMultiWhere: queryWhere / queryFilter.count != vectors.count")
+        }
+        let handle = self.handle
+        let cap = max(1, min(min(max(topGroups, 1), Self.maxResults) * max(perGroup, 1), Self.maxResults))
+        return try await io.run {
+            var flat = [Float](); flat.reserveCapacity(vectors.count * dims)
+            for v in vectors { flat.append(contentsOf: v) }
+            var frameIds = [UInt64]()
+            var offsets: [UInt64] = [0]
+            var modes = [Int32]()
+            for f in filters {
+                frameIds.append(contentsOf: f.frameIds)
+                offsets.append(UInt64(frameIds.count))
+                modes.append(f.allow ? 0 : 1)
+            }
+            let qf = perQueryFilter.map { $0.map(UInt32.init) ?? WAX_VS_NO_FILTER }
+            let qw = queryWhere.map { $0.map(UInt32.init) ?? WAX_VS_NO_FILTER }
+            var ids = [UInt64](repeating: 0, count: vectors.count * cap)
+            var scores = [Float](repeating: 0, count: vectors.count * cap)
+            var groups = [UInt64](repeating: 0, count: vectors.count * cap)
+            var counts = [UInt32](repeating: 0, count: vectors.count)
+            let rc = wax_vs_search_batch_grouped_multi_where(handle, flat, UInt32(vectors.count), UInt32(dims),
+                                                             Int64(topGroups), UInt32(max(perGroup, 0)), frameIds, offsets,
+                                                             modes, UInt32(filters.count), qf, wheres, UInt32(wheres.count),
+                                                             qw, &ids, &scores, &groups, UInt32(cap), &counts)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return (0..<vectors.count).map { q in
+                var out: [(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])] = []
+                for i in (q * cap)..<(q * cap + Int(counts[q])) {
+                    if out.last?.groupId != groups[i] { out.append((groups[i], [])) }
+                    out[out.count - 1].hits.append((ids[i], scores[i]))
+                }
+                return out
+            }
+        }
+    }
+
     /// Frame term sets (wax_vs_set_terms): each named frame's whole set is replaced, an empty list clears it.  The caller
     /// interns `("entry", key, value)`, `("tag", key, value)` and `("label", s)` exactly, so that `searchBatchWhereTerms`
     /// is `matches(metadataFilter:meta:)` below the top-k.  Not part of MV2V: re-apply after `deserialize`.

@@ -409,6 +409,7 @@ struct wax_vs_engine {
     std::mutex term_mu;
     uint64_t term_index_builds = 0;    // instrumentation (pool_mu)
     uint64_t grouped_batch_covered_queries = 0, grouped_batch_expanded_groups = 0, grouped_batch_fallback_queries = 0;
+    uint64_t grouped_batch_expansion_passes = 0;
     // Adaptive level choice: when more than a quarter of a batch fails the coarse bf16 bound (tightly clustered
     // neighbours), the next 16 batches nominate in TF32 straight away, then bf16 is probed again.
     uint32_t bf16_skip_batches = 0;
@@ -3231,6 +3232,42 @@ static void plan_filtered(const wax_vs_engine *e, int64_t top_k, const int32_t *
     plan.n_gather = static_cast<uint32_t>(gather.size());
 }
 
+// The bitsets of the filters `which` (bitset l is filter which[l]'s) into c->d_mask on c->stream, from the rows
+// run_filtered staged in c->d_filter_rows: the listed rows in the filter's mode, then where search's predicate and box
+// ANDed in, and a wide term unit's rows set.  On an error the stream is synchronised.
+static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const int32_t *filter_modes, const FilterSet &fs,
+                               const std::vector<uint32_t> &which, uint64_t *launches) {
+    const uint32_t nf = static_cast<uint32_t>(which.size());
+    std::vector<uint64_t> spec(3u * nf + 1u, 0);
+    for (uint32_t l = 0; l < nf; ++l) {
+        const bool wide = !fs.term_of.empty() && fs.term_of[which[l]] != WAX_VS_NO_FILTER;
+        spec[l + 1] = spec[l] + (wide ? 0 : fs.count[which[l]]);       // a wide term unit lists nothing
+        spec[nf + 1 + l] = fs.first[which[l]];
+        spec[2u * nf + 1u + l] = static_cast<uint64_t>(filter_modes[which[l]]);
+    }
+    int32_t rc;
+    if ((rc = build_filter_bits(e, c, spec, nf, c->stream, launches))) { cudaStreamSynchronize(c->stream); return rc; }
+    std::vector<WhereItem> wbits;                               // where search: the predicates ANDed in
+    std::vector<LocBox> wboxes;                                 // ... and in where_near search their boxes
+    for (uint32_t l = 0; l < nf && !fs.where.empty(); ++l)
+        if (fs.where[which[l]] != WAX_VS_NO_FILTER) {
+            wbits.push_back(WhereItem{fs.preds[fs.where[which[l]]], l});
+            if (fs.near) wboxes.push_back(fs.boxes[fs.where[which[l]]]);
+        }
+    std::vector<TermUnit> tbits;                                // where_terms search: wide units' rows
+    for (uint32_t l = 0; l < nf && !fs.term_of.empty(); ++l)
+        if (fs.term_of[which[l]] != WAX_VS_NO_FILTER) {
+            tbits.push_back(fs.term_wide[fs.term_of[which[l]]]);
+            tbits.back().slot = l;
+        }
+    if ((rc = apply_where_bits(e, c, wbits, c->stream, launches, fs.near ? &wboxes : nullptr)) ||
+        (rc = launch_term_filter(e, c, tbits, nullptr, c->d_mask, c->stream, launches))) {
+        cudaStreamSynchronize(c->stream);
+        return rc;
+    }
+    return WAX_VS_OK;
+}
+
 // The planned queries on c->stream: staged query j's candidates land at c->d_out[j * k_max], on the device.  Stages the
 // queries (c->d_queries, staged order) and the filters' rows (c->d_filter_rows).  plan.k_max > 0.
 static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries, const int32_t *filter_modes,
@@ -3313,35 +3350,7 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
                 index[s1] = f == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : static_cast<uint32_t>(which.size() - 1);
             }
             int32_t prc;
-            if (!which.empty()) {
-                const uint32_t nf = static_cast<uint32_t>(which.size());
-                std::vector<uint64_t> spec(3u * nf + 1u, 0);
-                for (uint32_t l = 0; l < nf; ++l) {
-                    const bool wide = !fs.term_of.empty() && fs.term_of[which[l]] != WAX_VS_NO_FILTER;
-                    spec[l + 1] = spec[l] + (wide ? 0 : count[which[l]]);     // a wide term unit lists nothing
-                    spec[nf + 1 + l] = first[which[l]];
-                    spec[2u * nf + 1u + l] = static_cast<uint64_t>(filter_modes[which[l]]);
-                }
-                if ((prc = build_filter_bits(e, c, spec, nf, c->stream, &launches))) { cudaStreamSynchronize(c->stream); return prc; }
-                std::vector<WhereItem> wbits;                           // where search: the predicates ANDed in
-                std::vector<LocBox> wboxes;                             // ... and in where_near search their boxes
-                for (uint32_t l = 0; l < nf && !fs.where.empty(); ++l)
-                    if (fs.where[which[l]] != WAX_VS_NO_FILTER) {
-                        wbits.push_back(WhereItem{fs.preds[fs.where[which[l]]], l});
-                        if (fs.near) wboxes.push_back(fs.boxes[fs.where[which[l]]]);
-                    }
-                std::vector<TermUnit> tbits;                            // where_terms search: wide units' rows
-                for (uint32_t l = 0; l < nf && !fs.term_of.empty(); ++l)
-                    if (fs.term_of[which[l]] != WAX_VS_NO_FILTER) {
-                        tbits.push_back(fs.term_wide[fs.term_of[which[l]]]);
-                        tbits.back().slot = l;
-                    }
-                if ((prc = apply_where_bits(e, c, wbits, c->stream, &launches, fs.near ? &wboxes : nullptr)) ||
-                    (prc = launch_term_filter(e, c, tbits, nullptr, c->d_mask, c->stream, &launches))) {
-                    cudaStreamSynchronize(c->stream);
-                    return prc;
-                }
-            }
+            if (!which.empty() && (prc = build_pass_bits(e, c, filter_modes, fs, which, &launches))) return prc;
             RowFilter rf{c->d_mask.p, words, nullptr, index.data() + s0};
             const uint32_t nq = s1 - s0;
             const float *dq = c->d_queries + static_cast<size_t>(s0) * e->dims;
@@ -4329,11 +4338,13 @@ static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, u
 // ---- batched grouped search (waxvs_group_batch.cuh) -----------------------------------------------------------------
 constexpr uint64_t kExpandBatchKeys = 1ull << 24;   // level-buffer keys one round of batched expansions may hold
 
-// The expansions the cover kernel listed, (query, slot, span) sorted, into the batch's result keys c->d_bg_keys: level 0
-// scores the CSR tiles for the item's query (group_score_tile_kernel), the later levels merge as the single query does.
-// Rounds of spans keep the level buffers within kExpandBatchKeys; the buffers are sized once for the largest round.
+// The expansions the cover kernel listed, in a reproducible order, into the batch's result keys c->d_bg_keys: level 0
+// scores the CSR tiles for the item's query (group_score_tile_kernel) under bitset query_slot[query] of c->d_mask
+// (WAX_VS_NO_FILTER: unfiltered), the later levels merge as the single query does.  Rounds of spans keep the level
+// buffers within kExpandBatchKeys; the buffers are sized once for the largest round.
 static int32_t enqueue_batch_expansion(wax_vs_engine *e, SearchCtx *c, const CoverExpand *list, uint32_t n_list,
-                                       uint32_t n_top, uint32_t per_group, const uint32_t *d_mask, uint64_t *launches) {
+                                       uint32_t n_top, uint32_t per_group, const std::vector<uint32_t> &query_slot,
+                                       uint64_t *launches) {
     struct Round { ExpandPlan plan; std::vector<uint32_t> span_query; };
     std::vector<Round> rounds;
     std::vector<uint3> spans;
@@ -4361,7 +4372,8 @@ static int32_t enqueue_batch_expansion(wax_vs_engine *e, SearchCtx *c, const Cov
     for (const Round &rd : rounds) {
         for (size_t t = 0; t < rd.plan.levels[0].size(); ++t) {
             const ExpandItem &it = rd.plan.levels[0][t];
-            tiles.push_back({rd.span_query[rd.plan.tile_span[t]], it.begin, it.count, it.dst_off, it.final_out});
+            const uint32_t q = rd.span_query[rd.plan.tile_span[t]];
+            tiles.push_back({q, it.begin, it.count, it.dst_off, it.final_out, query_slot[q]});
         }
         for (size_t lv = 1; lv < rd.plan.levels.size(); ++lv)
             merges.insert(merges.end(), rd.plan.levels[lv].begin(), rd.plan.levels[lv].end());
@@ -4380,11 +4392,12 @@ static int32_t enqueue_batch_expansion(wax_vs_engine *e, SearchCtx *c, const Cov
     const auto score = e->similarity == WAX_VS_COSINE ? group_score_tile_kernel<kCosine>
                        : e->similarity == WAX_VS_DOT  ? group_score_tile_kernel<kDot>
                                                       : group_score_tile_kernel<kL2>;
+    const uint32_t words = static_cast<uint32_t>((e->n_rows + 31) / 32);
     size_t first_tile = 0, first_merge = 0;
     for (const Round &rd : rounds) {
         const uint32_t n0 = static_cast<uint32_t>(rd.plan.levels[0].size());
-        score<<<n0, 256, 0, s>>>(c->d_score_items + first_tile, e->d_corpus, c->d_queries, e->dims, e->gindex.perm, d_mask,
-                                  per_group, c->d_expand[0], c->d_bg_keys);
+        score<<<n0, 256, 0, s>>>(c->d_score_items + first_tile, e->d_corpus, c->d_queries, e->dims, e->gindex.perm,
+                                  c->d_mask.p, words, per_group, c->d_expand[0], c->d_bg_keys);
         CUDA_TRY(cudaGetLastError());
         ++*launches;
         first_tile += n0;
@@ -4396,13 +4409,9 @@ static int32_t enqueue_batch_expansion(wax_vs_engine *e, SearchCtx *c, const Cov
     return WAX_VS_OK;
 }
 
-// Both grouped entry points: the arguments checked before the empty-engine early return, the filter resolved once (an
-// empty deny-list is none), then grouped_one, or with `batched` the batch pipeline -- a batch of one stays a batch.
-static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                   int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
-                                   int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
-                                   uint32_t out_stride, uint32_t *out_n, bool batched, const wax_vs_where *where = nullptr,
-                                   const LocBox *box = nullptr) {
+// The grouped checks of every grouped entry point, before the empty-engine early return.
+static int32_t check_grouped_args(const wax_vs_engine *e, int64_t top_groups, uint32_t per_group, const uint64_t *out_ids,
+                                  const float *out_scores, const uint64_t *out_groups, const uint32_t *out_n) {
     if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (per_group == 0 || per_group > WAX_VS_MAX_PER_GROUP)
         return fail(WAX_VS_ERR_ARGUMENT, "per_group must be in [1, %d] (got %u)", WAX_VS_MAX_PER_GROUP, per_group);
@@ -4410,8 +4419,26 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     if (static_cast<uint64_t>(n_top) * per_group > WAX_VS_MAX_RESULTS)
         return fail(WAX_VS_ERR_ARGUMENT, "clamp(top_groups) x per_group = %llu exceeds %d",
                     static_cast<unsigned long long>(n_top) * per_group, WAX_VS_MAX_RESULTS);
-    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
-    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    return WAX_VS_OK;
+}
+
+// Every grouped entry point after its argument checks: query i searches the rows passing wheres[query_where[i]] (and
+// boxes[query_where[i]] unless boxes is nullptr) AND id filter query_filter[i], either of which may be WAX_VS_NO_FILTER.
+// The (where, id filter) pairs are the units of the where search (plan_where_pairs), planned by the batched filtered
+// search at k_c; a query no row passes answers nothing.  Without `batched`, or when the coverage level does not take the
+// batch, every query runs grouped_one.  The batch pipeline:
+//  - coverage: each staged query's exact top-k_c rows (run_filtered), then group_cover_kernel, when every staged query
+//    is in the gather class, or every one in the tensor class and the batch goes to the tensor-core levels;
+//  - expansion: the cover kernel's list sorted by (unit, query, group rank), in passes of at most filter_bitset_bytes
+//    of distinct units' bitsets (build_pass_bits, as run_filtered builds them), each item scored under its unit's;
+//  - crowded queries: grouped_one under the query's own pair (grouped_one_args).
+static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                   int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids,
+                                   const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                   const uint32_t *query_filter, const wax_vs_where *wheres, uint32_t n_wheres,
+                                   const uint32_t *query_where, const LocBox *boxes, uint64_t *out_ids, float *out_scores,
+                                   uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n, bool batched) {
+    const uint32_t n_top = clamp_topk(top_groups);
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
     if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;      // as wax_vs_search (:448)
@@ -4420,69 +4447,37 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(n_top) * per_group, n));
     if (out_stride < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, need);
-    const bool filtered = where || !(mode == 1 && n_ids == 0);
-    const uint64_t offsets[2] = {0, n_ids};
-    FilterSet fs;
-    if (filtered) {
-        resolve_filters(e, frame_ids, offsets, 1, nullptr, 0, fs);
-        if (!where && mode == 0 && fs.rows.empty()) return WAX_VS_OK;                 // nothing allowed
-        if (!where && mode == 1 && fs.rows.size() == n) return WAX_VS_OK;             // everything denied
-    }
+    FilterSet ids;
+    resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, ids);
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
     CtxLease lease(e);
     if ((rc = lease.acquire())) return rc;
     SearchCtx *c = lease.c;
-    // where (wax_vs_search_batch_grouped_where): the filter becomes an allow-list of the listed rows that pass, or the
-    // deny-list's rows that pass (mode 1) with the predicate ANDed into every bitset built from it (where_bits)
-    WherePred pred{};
-    bool where_bits = false;
-    const std::vector<LocBox> one_box(box ? 1 : 0, box ? *box : kNoLocBox);   // where_near: the predicate's box
-    const std::vector<LocBox> *pred_box = box ? &one_box : nullptr;
-    if (where) {
-        pred = where_pred(*where);
-        std::vector<uint32_t> kept;
-        host_rows_passing(e, pred, fs.rows.data(), fs.rows.size(), kept, box);
-        fs.rows.swap(kept);
-        fs.count[0] = fs.rows.size();
-        if (mode == 0 && fs.rows.empty()) return WAX_VS_OK;                           // nothing allowed
-        if (mode == 1) {
-            std::vector<uint32_t> pass;
-            if ((rc = where_counts(e, c, {pred}, pass, pred_box))) return rc;
-            if (pass[0] == fs.rows.size()) return WAX_VS_OK;                          // nothing passes but denied rows
-            fs.where.assign(1, 0);
-            fs.preds.assign(1, pred);
-            fs.near = box != nullptr;
-            if (box) fs.boxes.assign(1, *box);
-            fs.allowed.assign(1, pass[0] - fs.rows.size());
-            where_bits = true;
-        }
-    }
-    const WherePred *row_where = where_bits ? &pred : nullptr;
-    if (!batched)
-        return grouped_one(e, c, queries, n_top, per_group, filtered ? &fs.rows : nullptr, mode, row_where, out_ids,
-                           out_scores, out_groups, out_n, pred_box);
-    const std::vector<uint32_t> query_filter(n_queries, filtered ? 0u : WAX_VS_NO_FILTER);
+    FilterSet fs;
+    std::vector<int32_t> modes;
+    std::vector<uint32_t> pair_of;
+    if ((rc = plan_where_pairs(e, c, wheres, n_wheres, query_where, filter_modes, query_filter, n_queries, ids, fs, modes,
+                               pair_of, boxes)))
+        return rc;
     // The coverage level: each query's exact top-k_c rows, when the batch goes to the tensor-core levels or the gather
     // class of the batched filtered search; every other batch runs the single-query pipeline per query.
     const uint32_t k_c = std::min(kCoverMax, std::max(128u, 4u * n_top));
     FilteredPlan plan;
-    bool cover = n_top <= kCoverMax / 4;
-    if (cover) {
-        plan_filtered(e, k_c, &mode, query_filter.data(), n_queries, fs, plan);
-        const uint32_t n_staged = static_cast<uint32_t>(plan.order.size());
-        cover = n_staged == n_queries && (plan.n_gather == n_staged ||
-                                          (plan.n_tensor == n_staged && batch_tensor_eligible(e, n_staged, plan.k_max)));
-    }
+    plan_filtered(e, k_c, modes.data(), pair_of.data(), n_queries, fs, plan);
+    const uint32_t nq = static_cast<uint32_t>(plan.order.size());    // the staged queries: some row passes
+    const bool cover = batched && nq > 0 && n_top <= kCoverMax / 4 &&
+                       (plan.n_gather == nq || (plan.n_tensor == nq && batch_tensor_eligible(e, nq, plan.k_max)));
     cudaStream_t s = c->stream;
     std::vector<uint32_t> crowded;                   // queries for the single-query pipeline
-    uint64_t covered = 0, expanded = 0, launches = 0;
+    uint64_t covered = 0, expanded = 0, expansion_passes = 0, launches = 0;
     if (!cover) {
-        for (uint32_t i = 0; i < n_queries; ++i) crowded.push_back(i);
+        crowded = plan.order;
     } else {
         if ((rc = ensure_group_index(e, c))) return rc;
-        if ((rc = run_filtered(e, c, queries, &mode, filtered ? 1u : 0u, query_filter.data(), fs, plan))) return rc;
-        const uint32_t nq = n_queries, slots = n_top * per_group;
+        if ((rc = run_filtered(e, c, queries, modes.data(), static_cast<uint32_t>(modes.size()), pair_of.data(), fs, plan)))
+            return rc;
+        const uint32_t slots = n_top * per_group;
         const size_t nkeys = static_cast<size_t>(nq) * slots;
         if ((rc = c->d_bg_keys.ensure(nkeys, "grouped batch keys")) || (rc = c->h_bg_keys.ensure(nkeys, "grouped batch staging")) ||
             (rc = c->d_bg_status.ensure(nq + 1u, "grouped batch status")) ||
@@ -4501,21 +4496,38 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
         if (n_exp) {
             CUDA_TRY(cudaMemcpyAsync(c->h_bg_expand, c->d_bg_expand, n_exp * sizeof(CoverExpand), cudaMemcpyDeviceToHost, s));
             CUDA_TRY(cudaStreamSynchronize(s));
+            std::vector<uint32_t> unit(nq);          // staged query -> its pair (WAX_VS_NO_FILTER, unfiltered, sorts last)
+            for (uint32_t j = 0; j < nq; ++j) unit[j] = pair_of[plan.order[j]];
             CoverExpand *list = c->h_bg_expand;      // appended in any order: sort for a reproducible launch plan
-            std::sort(list, list + n_exp, [](const CoverExpand &a, const CoverExpand &b) {
+            std::sort(list, list + n_exp, [&](const CoverExpand &a, const CoverExpand &b) {
+                if (unit[a.query] != unit[b.query]) return unit[a.query] < unit[b.query];
                 return a.query != b.query ? a.query < b.query : a.slot < b.slot;
             });
-            if (filtered) {                          // the expansion consults the filter's bitset (rows staged by run_filtered)
-                const std::vector<uint64_t> spec = {0, fs.rows.size(), 0, static_cast<uint64_t>(mode)};
-                if ((rc = build_filter_bits(e, c, spec, 1, s, &launches)) ||
-                    (row_where && (rc = apply_where_bits(e, c, {WhereItem{pred, 0}}, s, &launches, pred_box)))) {
+            // passes of at most `fit` distinct units' bitsets (run_filtered sized c->d_mask for at least as many); each
+            // pass ends in a synchronise, so the next one may rebuild the bitsets
+            const uint64_t words = (e->n_rows + 31) / 32;
+            const uint64_t fit = std::max<uint64_t>(1, e->tune.filter_bitset_bytes / (words * sizeof(uint32_t)));
+            std::vector<uint32_t> query_slot(nq, WAX_VS_NO_FILTER);
+            for (uint32_t i0 = 0; i0 < n_exp;) {
+                std::vector<uint32_t> which;         // the pass's units, in bitset order
+                uint32_t i1 = i0;
+                for (; i1 < n_exp; ++i1) {
+                    const uint32_t u = unit[list[i1].query];
+                    if (u != WAX_VS_NO_FILTER && (which.empty() || which.back() != u)) {
+                        if (which.size() == fit) break;
+                        which.push_back(u);
+                    }
+                    query_slot[list[i1].query] = u == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : static_cast<uint32_t>(which.size() - 1);
+                }
+                if (!which.empty()) {
+                    if ((rc = build_pass_bits(e, c, modes.data(), fs, which, &launches))) return rc;
+                    ++expansion_passes;
+                }
+                if ((rc = enqueue_batch_expansion(e, c, list + i0, i1 - i0, n_top, per_group, query_slot, &launches))) {
                     cudaStreamSynchronize(s);
                     return rc;
                 }
-            }
-            if ((rc = enqueue_batch_expansion(e, c, list, n_exp, n_top, per_group, filtered ? c->d_mask.p : nullptr, &launches))) {
-                cudaStreamSynchronize(s);
-                return rc;
+                i0 = i1;
             }
             expanded = n_exp;
         }
@@ -4529,36 +4541,76 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
                                            out_scores + o, out_groups + o);
             ++covered;
         }
-        std::sort(crowded.begin(), crowded.end());
     }
-    // crowded queries (and batches the coverage level does not take): the single-query pipeline, same lock and context
+    std::sort(crowded.begin(), crowded.end());
+    // crowded queries (and batches the coverage level does not take): the single-query pipeline, same lock and context,
+    // under the query's own pair as the one-filter grouped search takes it -- an id filter alone as it is, an allow-list
+    // as its rows that pass the where (plan_where_pairs listed them), a deny-list (or none) AND a where as the deny-list
+    // in mode 1 with the predicate and its box ANDed into the bitset
     for (uint32_t qi : crowded) {
+        const uint32_t p = pair_of[qi], w = query_where[qi], f = query_filter[qi];
+        const bool row_where = w != WAX_VS_NO_FILTER && (f == WAX_VS_NO_FILTER || filter_modes[f] == 1);
+        std::vector<uint32_t> rows;
+        int32_t mode = 1;
+        WherePred pred{};
+        std::vector<LocBox> box;
+        if (row_where) {
+            if (f != WAX_VS_NO_FILTER) rows.assign(ids.rows.begin() + ids.first[f], ids.rows.begin() + ids.first[f] + ids.count[f]);
+            pred = where_pred(wheres[w]);
+            if (boxes) box.assign(1, boxes[w]);
+        } else if (p != WAX_VS_NO_FILTER) {
+            rows.assign(fs.rows.begin() + fs.first[p], fs.rows.begin() + fs.first[p] + fs.count[p]);
+            mode = modes[p];
+        }
         const size_t o = static_cast<size_t>(qi) * out_stride;
-        if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group, filtered ? &fs.rows : nullptr,
-                              mode, row_where, out_ids + o, out_scores + o, out_groups + o, out_n + qi, pred_box)))
+        if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group,
+                              p == WAX_VS_NO_FILTER ? nullptr : &rows, mode, row_where ? &pred : nullptr, out_ids + o,
+                              out_scores + o, out_groups + o, out_n + qi, row_where && boxes ? &box : nullptr)))
             return rc;
     }
+    if (!batched) return WAX_VS_OK;
     std::lock_guard<std::mutex> pg(e->pool_mu);
     e->grouped_batch_covered_queries += covered;
     e->grouped_batch_expanded_groups += expanded;
     e->grouped_batch_fallback_queries += crowded.size();
+    e->grouped_batch_expansion_passes += expansion_passes;
     return WAX_VS_OK;
+}
+
+// The one-filter grouped entry points: one id filter (an empty deny-list is none) and at most one where (with `box`, its
+// active location box) for every query.
+static int32_t search_grouped_one_filter(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                         int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
+                                         int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
+                                         uint32_t out_stride, uint32_t *out_n, bool batched,
+                                         const wax_vs_where *where = nullptr, const LocBox *box = nullptr) {
+    int32_t rc;
+    if ((rc = check_grouped_args(e, top_groups, per_group, out_ids, out_scores, out_groups, out_n))) return rc;
+    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
+    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    const uint64_t offsets[2] = {0, n_ids};
+    const std::vector<uint32_t> query_filter(n_queries, mode == 1 && n_ids == 0 ? WAX_VS_NO_FILTER : 0u);
+    const std::vector<uint32_t> query_where(n_queries, where ? 0u : WAX_VS_NO_FILTER);
+    return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, offsets, &mode, 1,
+                               query_filter.data(), where, where ? 1u : 0u, query_where.data(), box, out_ids, out_scores,
+                               out_groups, out_stride, out_n, batched);
 }
 
 int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_groups,
                               uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
                               uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_cap,
                               uint32_t *out_n) {
-    return search_grouped_host(e, query, 1, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids, out_scores,
-                               out_groups, out_cap, out_n, false);
+    return search_grouped_one_filter(e, query, 1, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
+                                     out_scores, out_groups, out_cap, out_n, false);
 }
 
+// A batch of one stays a batch.
 int32_t wax_vs_search_batch_grouped(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                     int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
                                     int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
                                     uint32_t out_stride, uint32_t *out_n) {
-    return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
-                               out_scores, out_groups, out_stride, out_n, true);
+    return search_grouped_one_filter(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode,
+                                     out_ids, out_scores, out_groups, out_stride, out_n, true);
 }
 
 int32_t wax_vs_search_batch_grouped_where(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
@@ -4566,8 +4618,8 @@ int32_t wax_vs_search_batch_grouped_where(wax_vs_engine *e, const float *queries
                                           int32_t mode, const wax_vs_where *where, uint64_t *out_ids, float *out_scores,
                                           uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n) {
     if (!where) return fail(WAX_VS_ERR_NULL, "where is NULL");
-    return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
-                               out_scores, out_groups, out_stride, out_n, n_queries > 1, where);
+    return search_grouped_one_filter(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode,
+                                     out_ids, out_scores, out_groups, out_stride, out_n, n_queries > 1, where);
 }
 
 // A predicate whose box is "no location clause" is wax_vs_search_batch_grouped_where with its time and tag clauses.
@@ -4581,9 +4633,33 @@ int32_t wax_vs_search_batch_grouped_where_near(wax_vs_engine *e, const float *qu
     bool active;
     int32_t rc;
     if ((rc = location_box(where->latitude, where->longitude, where->radius_m, &box, &active))) return rc;
-    return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
-                               out_scores, out_groups, out_stride, out_n, n_queries > 1, &where->where,
-                               active ? &box : nullptr);
+    return search_grouped_one_filter(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode,
+                                     out_ids, out_scores, out_groups, out_stride, out_n, n_queries > 1, &where->where,
+                                     active ? &box : nullptr);
+}
+
+// A call whose boxes are all "no location clause" plans without the location forms, as wax_vs_search_batch_where.
+int32_t wax_vs_search_batch_grouped_multi_where(wax_vs_engine *e, const float *queries, uint32_t n_queries,
+                                                uint32_t query_len, int64_t top_groups, uint32_t per_group,
+                                                const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                                const int32_t *filter_modes, uint32_t n_filters,
+                                                const uint32_t *query_filter, const wax_vs_where_near *wheres,
+                                                uint32_t n_wheres, const uint32_t *query_where, uint64_t *out_ids,
+                                                float *out_scores, uint64_t *out_groups, uint32_t out_stride,
+                                                uint32_t *out_n) {
+    int32_t rc;
+    if ((rc = check_grouped_args(e, top_groups, per_group, out_ids, out_scores, out_groups, out_n)) ||
+        (rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
+                               n_wheres, query_where, out_n)))
+        return rc;
+    std::vector<wax_vs_where> plain;
+    std::vector<LocBox> boxes;
+    bool any;
+    if ((rc = split_near(wheres, n_wheres, plain, boxes, &any))) return rc;
+    return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, filter_offsets,
+                               filter_modes, n_filters, query_filter, plain.data(), n_wheres, query_where,
+                               any ? boxes.data() : nullptr, out_ids, out_scores, out_groups, out_stride, out_n,
+                               n_queries > 1);
 }
 
 // ---- persistence ---------------------------------------------------------------------------------------------
@@ -4926,6 +5002,7 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "grouped_batch_covered_queries")) *out = e->grouped_batch_covered_queries;     // answered by the coverage level
     else if (!strcmp(name, "grouped_batch_expanded_groups")) *out = e->grouped_batch_expanded_groups;     // (query, group) expansions
     else if (!strcmp(name, "grouped_batch_fallback_queries")) *out = e->grouped_batch_fallback_queries;   // single-query pipeline
+    else if (!strcmp(name, "grouped_batch_expansion_passes")) *out = e->grouped_batch_expansion_passes;   // bitset passes of the expansion
     else if (!strcmp(name, "ingest_h2d_bytes")) *out = e->ingest_h2d_bytes;
     else if (!strcmp(name, "ingest_d2h_bytes")) *out = e->ingest_d2h_bytes;
     else if (!strcmp(name, "norms_rows")) *out = e->norms_rows;       // rows whose cached 1/|v| is valid

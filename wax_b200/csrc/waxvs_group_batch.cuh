@@ -37,9 +37,10 @@ struct CoverExpand {
 };
 
 // Level-0 expansion work item: score CSR positions [begin, begin + count) (<= kExpandTile) for query `query` and keep
-// the per_group smallest keys at dst_off of the result (final_out = 1) or of the next level's input.
+// the per_group smallest keys at dst_off of the result (final_out = 1) or of the next level's input.  mask_slot: the
+// bitset of the query's row filter in the pass's masks, or WAX_VS_NO_FILTER (unfiltered).
 struct ScoreItem {
-    uint32_t query, begin, count, dst_off, final_out;
+    uint32_t query, begin, count, dst_off, final_out, mask_slot;
 };
 
 // One CTA of kCoverMax threads per query.  cands + q * k_list: the query's exact top-k_list rows, best first (invalid
@@ -116,19 +117,22 @@ __global__ void __launch_bounds__(kCoverMax) group_cover_kernel(const wax_vs_can
 }
 
 // Expansion level 0 for a batch: item `blockIdx.x` scores its CSR positions for its query, exactly (warp per row, the
-// kernels' operation order, so the bits equal the scan's); rows outside the filter (mask bit clear) or with a
-// non-finite distance drop out.  The tile is sorted in shared memory and its per_group best are kept.
+// kernels' operation order, so the bits equal the scan's); rows outside the item's filter (bit clear in bitset
+// mask_slot of `masks`, `words` words each) or with a non-finite distance drop out.  The tile is sorted in shared memory
+// and its per_group best are kept.
 template <int METRIC>
 __global__ void __launch_bounds__(256) group_score_tile_kernel(const ScoreItem *__restrict__ items, const float *corpus,
                                                                 const float *queries, uint32_t dims,
                                                                 const uint32_t *__restrict__ perm,
-                                                                const uint32_t *__restrict__ mask, uint32_t per_group,
+                                                                const uint32_t *__restrict__ masks, uint32_t words,
+                                                                uint32_t per_group,
                                                                 uint64_t *__restrict__ scratch_out,
                                                                 uint64_t *__restrict__ result) {
     __shared__ uint64_t sk[kExpandTile];
     const ScoreItem it = items[blockIdx.x];
     const int lane = threadIdx.x & 31;
     const float *query = queries + static_cast<size_t>(it.query) * dims;
+    const uint32_t *mask = it.mask_slot == WAX_VS_NO_FILTER ? nullptr : masks + static_cast<size_t>(it.mask_slot) * words;
     float a2 = 0.0f, sqrt_a2 = 0.0f;
     if (METRIC == kCosine) {
         a2 = query_sq_norm(query, dims, lane);

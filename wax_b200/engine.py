@@ -648,6 +648,61 @@ class CUDAVectorEngine:
             result.append(out)
         return result
 
+    def search_batch_grouped_multi_where(self, vectors, top_groups: int, per_group: int, wheres: Sequence["Where"],
+                                         query_where: Sequence[Optional[int]],
+                                         filters: Optional[Sequence[Tuple[object, Sequence[int]]]] = None,
+                                         query_filter: Optional[Sequence[Optional[int]]] = None
+                                         ) -> List[List[Tuple[int, List[Tuple[int, float]]]]]:
+        """search_batch_grouped with a where and an id filter of each query's own
+        (wax_vs_search_batch_grouped_multi_where): query i searches the frames passing wheres[query_where[i]] AND
+        filters[query_filter[i]] (None = no predicate / no id filter; arguments as search_batch_where).  Its answer, one
+        [(group_id, [(frame_id, score), ...]), ...], equals search_grouped under an allow-list of exactly those frames."""
+        if any(w.terms for w in wheres):
+            raise ValueError("grouped search takes no term clause")
+        qs = _as_rows(vectors, self.dimensions) if len(vectors) else np.zeros((0, self.dimensions), np.float32)
+        b = qs.shape[0]
+        filters = list(filters or [])
+        if query_filter is None:
+            query_filter = [None] * b
+        if len(query_where) != b or len(query_filter) != b:
+            raise ValueError(f"query_where / query_filter need {b} entries")
+        if b == 0:
+            return []
+        modes, lists = [], []
+        for mode, fids in filters:
+            modes.append({"allow": 0, "deny": 1}[mode] if isinstance(mode, str) else int(mode))
+            lists.append(np.ascontiguousarray(fids, dtype=np.uint64).reshape(-1))
+        offsets = np.zeros(len(lists) + 1, np.uint64)
+        offsets[1:] = np.cumsum([x.size for x in lists], dtype=np.uint64) if lists else []
+        fids = np.concatenate(lists) if lists else np.zeros(0, np.uint64)
+        modes_arr = np.asarray(modes, np.int32)
+        qf = np.asarray([L.NO_FILTER if f is None else int(f) for f in query_filter], np.uint32)
+        qw = np.asarray([L.NO_FILTER if w is None else int(w) for w in query_where], np.uint32)
+        warr = (L.WhereNear * max(len(wheres), 1))(*[w.to_c_near() for w in wheres])
+        cap = max(1, min(_clamp_topk(top_groups) * max(int(per_group), 1), L.MAX_RESULTS))
+        ids = np.empty((b, cap), np.uint64)
+        scores = np.empty((b, cap), np.float32)
+        groups = np.empty((b, cap), np.uint64)
+        ns = np.zeros(b, np.uint32)
+        _check(L.lib().wax_vs_search_batch_grouped_multi_where(
+            self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_groups), int(per_group),
+            fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
+            offsets.ctypes.data_as(C.POINTER(C.c_uint64)), modes_arr.ctypes.data_as(C.POINTER(C.c_int32)), len(lists),
+            qf.ctypes.data_as(C.POINTER(C.c_uint32)), C.cast(warr, C.c_void_p), len(wheres),
+            qw.ctypes.data_as(C.POINTER(C.c_uint32)), ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+            scores.ctypes.data_as(C.POINTER(C.c_float)), groups.ctypes.data_as(C.POINTER(C.c_uint64)), cap,
+            ns.ctypes.data_as(C.POINTER(C.c_uint32))))
+        result = []
+        for i in range(b):
+            out: List[Tuple[int, List[Tuple[int, float]]]] = []
+            for j in range(int(ns[i])):
+                g = int(groups[i, j])
+                if not out or out[-1][0] != g:
+                    out.append((g, []))
+                out[-1][1].append((int(ids[i, j]), float(scores[i, j])))
+            result.append(out)
+        return result
+
     def search_batch(self, vectors, top_k: int) -> List[List[Tuple[int, float]]]:
         """`search` for a batch of queries (wax_vs_search_batch): the same answers as one call per query.  Cosine and dot
         batches share one tensor-core pass over the corpus, l2 batches too once set_option("batch_l2", 1) is set."""

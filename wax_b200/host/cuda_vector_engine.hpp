@@ -346,6 +346,53 @@ public:
         return out;
     }
 
+    // searchBatchGroupedWhere with a where and an id filter of each query's own (wax_vs_search_batch_grouped_multi_where):
+    // query i searches the frames passing wheres[queryWhere[i]] AND filters[queryFilter[i]] (WAX_VS_NO_FILTER: none; a
+    // filter is (frame ids, allow)).
+    std::vector<std::vector<Group>> searchBatchGroupedMultiWhere(
+        const std::vector<std::vector<float>> &vectors, int64_t topGroups, uint32_t perGroup,
+        const std::vector<wax_vs_where_near> &wheres, const std::vector<uint32_t> &queryWhere,
+        const std::vector<std::pair<std::vector<uint64_t>, bool>> &filters = {},
+        const std::vector<uint32_t> &queryFilter = {}) const {
+        std::vector<std::vector<Group>> out(vectors.size());
+        if (vectors.empty()) return out;
+        if (queryWhere.size() != vectors.size() || (!queryFilter.empty() && queryFilter.size() != vectors.size()))
+            throw EncodingError("searchBatchGroupedMultiWhere: queryWhere / queryFilter.count != vectors.count");
+        const int64_t lim = topGroups < 1 ? 1 : (topGroups > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topGroups);
+        const int64_t want = lim * (perGroup ? perGroup : 1);
+        const size_t cap = static_cast<size_t>(want > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : want);
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchGroupedMultiWhere: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        std::vector<uint64_t> frameIds, offsets(1, 0);
+        std::vector<int32_t> modes;
+        for (const auto &f : filters) {
+            frameIds.insert(frameIds.end(), f.first.begin(), f.first.end());
+            offsets.push_back(frameIds.size());
+            modes.push_back(f.second ? 0 : 1);
+        }
+        const std::vector<uint32_t> noFilter(vectors.size(), WAX_VS_NO_FILTER);
+        const std::vector<uint32_t> &qf = queryFilter.empty() ? noFilter : queryFilter;
+        std::vector<uint64_t> ids(vectors.size() * cap), groups(vectors.size() * cap);
+        std::vector<float> scores(vectors.size() * cap);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_grouped_multi_where(
+            h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_, topGroups, perGroup, frameIds.data(),
+            offsets.data(), modes.data(), static_cast<uint32_t>(filters.size()), qf.data(), wheres.data(),
+            static_cast<uint32_t>(wheres.size()), queryWhere.data(), ids.data(), scores.data(), groups.data(),
+            static_cast<uint32_t>(cap), ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) {
+                const size_t j = q * cap + i;
+                if (out[q].empty() || out[q].back().first != groups[j]) out[q].push_back({groups[j], {}});
+                out[q].back().second.push_back({ids[j], scores[j]});
+            }
+        return out;
+    }
+
     // Frame locations in degrees (wax_vs_set_locations): upsert; a NaN pair clears a frame's location.  Not serialized:
     // re-apply them after deserialize().
     uint64_t setLocations(const std::vector<uint64_t> &frameIds, const std::vector<double> &latitudes,
