@@ -203,6 +203,40 @@ def test_batch_of_1024_and_many_pairs_over_three_bitsets():
         assert _bits(got[qi]) == _bits(want[qi]), qi
 
 
+def test_count_pass_chunks_with_and_without_a_box():
+    rng = np.random.default_rng(5350)
+    eng = CUDAVectorEngine(VectorMetric.cosine, DIMS)
+    eng.fill_synthetic(5351, N, id_base=40)
+    ids = np.arange(N, dtype=np.uint64) + 40
+    ts, tags = _attributes(rng, N)
+    eng.set_attributes(ids, ts, tags)
+    lat, lon, centres = _locations(rng, N)
+    eng.set_locations(ids, lat, lon)
+    index = PhotoIndex(ids, lat, lon)
+    # 300 wheres without an id filter, one count-pass predicate each: the first chunk of 256 has no box, the second
+    # has a box in each where; narrow and wide ones on both sides, so the listing and bitset passes see both too
+    plain = []
+    for _ in range(256):
+        a = int(rng.integers(0, N - 30_000))
+        span = int(rng.choice([2_000, 30_000]))
+        plain.append(Where(after=int(ts[a]), before=int(ts[a + span]), no_tags=DELETED))
+    boxed = [Where(near=(float(c[0]), float(c[1]), float(rng.choice([2_000.0, 120_000.0]))), no_tags=SUPERSEDED)
+             for c in centres[3:47]]
+    wheres = plain + boxed
+    b = len(wheres)
+    assert b > 256
+    sizes = [_allowed(w, None, ids, ts, tags, index).size for w in wheres]
+    for part in (sizes[:256], sizes[256:]):
+        assert min(part) <= 16384 < max(part)                                      # gather and bitset on each side
+    qs = np.asarray(rng.standard_normal((b, DIMS)), np.float32)
+    uploads = eng.counter("location_uploads")
+    got = eng.search_batch_where(qs, 10, wheres, list(range(b)))
+    assert eng.counter("location_uploads") == uploads + 1
+    want = _expected(eng, qs, 10, wheres, list(range(b)), [], [None] * b, ids, ts, tags, index)
+    for qi in range(b):
+        assert _bits(got[qi]) == _bits(want[qi]), qi
+
+
 def test_single_query_takes_the_shadow_route_under_the_near_bitset(oracle):
     n = 200_000
     rng = np.random.default_rng(5402)

@@ -258,9 +258,9 @@ struct SearchCtx {
     DevBuf<ScoreItem> d_score_items;               // batched grouped search: expansion tiles (level 0)
     PinnedBuf<unsigned long long> h_flag;          // host-delivery completion flag
     unsigned long long host_seq = 0;               // last value the flag was asked to take
-    DevBuf<WhereItem> d_where_items;               // where search: predicates of the count / compaction / bitset launches
+    DevBuf<WhereNearItem> d_where_items;           // where search: predicates of the count / compaction / bitset launches
+                                                   // (WhereItems in the plain form)
     DevBuf<uint32_t> d_where_counts;               // where search: rows passing each predicate, then compaction cursors
-    DevBuf<WhereNearItem> d_where_near_items;      // where_near search: the same launches' predicates with their boxes
     DevBuf<uint64_t> d_term_ids;                   // where_terms search: the call's distinct required term ids ...
     DevBuf<TermSpan> d_term_spans;                 // ... their posting spans
     DevBuf<TermUnit> d_term_units;                 // ... the units of term_filter_kernel
@@ -378,8 +378,8 @@ struct wax_vs_engine {
     uint64_t attribute_uploads = 0;    // instrumentation (pool_mu)
     // Frame locations (wax_vs_set_locations): locs[r] = row r's PhotoRAG bins, kept aligned with `ids` by every mutator
     // exactly as `attrs` is.  Empty while locs_set is false: then no row has a location.  The device mirror (8 bytes
-    // per row) is the attribute mirror's twin: invalidated with it, rebuilt under attrs_mu by the first where_near search
-    // that needs it.
+    // per row) is the attribute mirror's twin: invalidated with it, rebuilt under attrs_mu by the first launch that tests a
+    // box.
     bool locs_set = false;
     std::vector<LocRow> locs;
     DevBuf<LocRow> d_locs;
@@ -2586,17 +2586,13 @@ struct FilterSet {
     std::vector<uint32_t> rows;
     std::vector<uint64_t> first, count;
     std::vector<uint8_t> referenced;            // filters some query names (the others are not resolved)
-    // Where search only (empty otherwise): filter f's bitset is ANDed with preds[where[f]] unless that is WAX_VS_NO_FILTER,
-    // and then allows allowed[f] rows; the rows of the filters in `compact` (device_rows in all) are listed by the device
-    // after `rows`, each item's slot being where its rows start.
+    // Where search only (empty otherwise): filter f's bitset is ANDed with preds[where[f]] (its slot unused) unless that
+    // is WAX_VS_NO_FILTER, and then allows allowed[f] rows; the rows of the filters in `compact` (device_rows in all) are
+    // listed by the device after `rows`, each item's slot being where its rows start.  Every item carries its box.
     std::vector<uint32_t> where;
     std::vector<uint64_t> allowed;
-    std::vector<WherePred> preds;
-    std::vector<WhereItem> compact;
+    std::vector<WhereNearItem> preds, compact;
     uint64_t device_rows = 0;
-    // Where_near search only (near true): boxes[j] is preds[j]'s location box, compact_boxes[j] compact[j]'s.
-    bool near = false;
-    std::vector<LocBox> boxes, compact_boxes;
     // Where_terms search only (plan_term_units): the narrow term units, whose rows the device lists at their slots after
     // the compact rows, and the wide ones, whose rows the device sets in their filter's bitset; term_of[f] = filter f's
     // wide unit in term_wide (empty, or WAX_VS_NO_FILTER, when it has none: its rows are the listed ones).
@@ -3050,107 +3046,85 @@ static int where_grid(const wax_vs_engine *e, uint64_t threads) {
                                                                      (threads + kWhereThreads - 1) / kWhereThreads)));
 }
 
-// The location form's items: items[i] with boxes[i], staged into c->d_where_near_items on `stream`.
-static int32_t stage_near_items(SearchCtx *c, const std::vector<WhereItem> &items, const std::vector<LocBox> &boxes,
-                                cudaStream_t stream) {
-    const uint32_t m = static_cast<uint32_t>(items.size());
-    int32_t rc;
-    if ((rc = c->d_where_near_items.ensure(m, "where_near predicates"))) return rc;
-    std::vector<WhereNearItem> near(m);
-    for (uint32_t i = 0; i < m; ++i) near[i] = WhereNearItem{items[i].pred, items[i].slot, boxes[i]};
-    CUDA_TRY(cudaMemcpyAsync(c->d_where_near_items, near.data(), m * sizeof(WhereNearItem), cudaMemcpyHostToDevice, stream));
-    return WAX_VS_OK;
+// Whether b is a location clause (kNoLocBox is none; no box location_box builds equals it).
+static bool box_active(const LocBox &b) {
+    return b.lat_lo != kNoLocBox.lat_lo || b.lat_hi != kNoLocBox.lat_hi || b.lon_lo0 != kNoLocBox.lon_lo0 ||
+           b.lon_hi0 != kNoLocBox.lon_hi0 || b.lon_lo1 != kNoLocBox.lon_lo1 || b.lon_hi1 != kNoLocBox.lon_hi1;
 }
 
-// counts[i] = the rows passing preds[i] (and with `boxes`, in boxes[i]): one streaming pass per kWhereChunk predicates,
-// read back once.
-static int32_t where_counts(wax_vs_engine *e, SearchCtx *c, const std::vector<WherePred> &preds, std::vector<uint32_t> &counts,
-                            const std::vector<LocBox> *boxes = nullptr) {
-    const uint32_t m = static_cast<uint32_t>(preds.size()), n = static_cast<uint32_t>(e->n_rows);
+// One where pass over `items` on `stream`: the items staged in c->d_where_items, then launch(form, d_items, i0, count) for
+// each kWhereChunk of them (and ++*launches unless that is nullptr).  When some box is active the form is
+// std::true_type, the located kernels over the items with their boxes, after the location mirror is brought up;
+// otherwise it is std::false_type, the plain kernels over (pred, slot), which read no location.  kNoLocBox admits every
+// row, rows without a location included, so the two forms agree wherever both apply.
+extern "C++" {     // a template, inside the C API's block
+template <class Launch>
+static int32_t where_pass(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereNearItem> &items, cudaStream_t stream,
+                          uint64_t *launches, Launch launch) {
+    const uint32_t m = static_cast<uint32_t>(items.size());
+    if (!m) return WAX_VS_OK;
+    const bool located = std::any_of(items.begin(), items.end(), [](const WhereNearItem &it) { return box_active(it.box); });
+    int32_t rc;
+    if ((rc = ensure_attributes(e, c, located)) || (rc = c->d_where_items.ensure(m, "where predicates"))) return rc;
+    WhereItem *plain = reinterpret_cast<WhereItem *>(c->d_where_items.p);
+    if (located) {
+        CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereNearItem), cudaMemcpyHostToDevice, stream));
+    } else {
+        std::vector<WhereItem> h(m);
+        for (uint32_t i = 0; i < m; ++i) h[i] = WhereItem{items[i].pred, items[i].slot};
+        CUDA_TRY(cudaMemcpyAsync(plain, h.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, stream));
+    }
+    for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
+        if (located) launch(std::true_type{}, c->d_where_items.p + i0, i0, std::min(kWhereChunk, m - i0));
+        else launch(std::false_type{}, plain + i0, i0, std::min(kWhereChunk, m - i0));
+        if (launches) ++*launches;
+    }
+    CUDA_TRY(cudaGetLastError());
+    return WAX_VS_OK;
+}
+}  // extern "C++"
+
+// counts[i] = the rows passing items[i]: one streaming pass per kWhereChunk predicates, read back once.
+static int32_t where_counts(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereNearItem> &items,
+                            std::vector<uint32_t> &counts) {
+    const uint32_t m = static_cast<uint32_t>(items.size()), n = static_cast<uint32_t>(e->n_rows);
     counts.assign(m, 0u);
     if (!m) return WAX_VS_OK;
     int32_t rc;
-    if ((rc = ensure_attributes(e, c, boxes != nullptr))) return rc;
-    if ((rc = c->d_where_items.ensure(m, "where predicates")) || (rc = c->d_where_counts.ensure(m, "where counts"))) return rc;
-    std::vector<WhereItem> items(m);
-    for (uint32_t i = 0; i < m; ++i) items[i] = WhereItem{preds[i], 0};
+    if ((rc = c->d_where_counts.ensure(m, "where counts"))) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_where_counts, 0, m * sizeof(uint32_t), c->stream));
-    if (boxes) {
-        if ((rc = stage_near_items(c, items, *boxes, c->stream))) return rc;
-        for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk)
-            where_near_count_kernel<<<where_grid(e, n), kWhereThreads, 0, c->stream>>>(
-                e->d_attrs, e->d_locs, n, c->d_where_near_items + i0, std::min(kWhereChunk, m - i0), c->d_where_counts + i0);
-    } else {
-        CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, c->stream));
-        for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk)
-            where_count_kernel<<<where_grid(e, n), kWhereThreads, 0, c->stream>>>(e->d_attrs, n, c->d_where_items + i0,
-                                                                                 std::min(kWhereChunk, m - i0), c->d_where_counts + i0);
-    }
-    CUDA_TRY(cudaGetLastError());
+    if ((rc = where_pass(e, c, items, c->stream, nullptr, [&](auto located, const auto *d_items, uint32_t i0, uint32_t count) {
+             where_count_kernel<decltype(located)::value><<<where_grid(e, n), kWhereThreads, 0, c->stream>>>(
+                 e->d_attrs, e->d_locs, n, d_items, count, c->d_where_counts + i0);
+         })))
+        return rc;
     CUDA_TRY(cudaMemcpyAsync(counts.data(), c->d_where_counts, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     return WAX_VS_OK;
 }
 
-// ANDs items[i].pred (and with `boxes`, boxes[i]) into bitset items[i].slot of c->d_mask on `stream` (after the filter
-// builders wrote it).
-static int32_t apply_where_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereItem> &items, cudaStream_t stream,
-                                uint64_t *launches, const std::vector<LocBox> *boxes = nullptr) {
-    const uint32_t m = static_cast<uint32_t>(items.size()), n = static_cast<uint32_t>(e->n_rows);
-    if (!m) return WAX_VS_OK;
-    const uint32_t words = (n + 31u) / 32u;
-    int32_t rc;
-    if (boxes) {
-        if ((rc = stage_near_items(c, items, *boxes, stream))) return rc;
-        for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
-            where_near_bits_kernel<<<where_grid(e, static_cast<uint64_t>(words) * 32u), kWhereThreads, 0, stream>>>(
-                e->d_attrs, e->d_locs, n, words, c->d_mask, c->d_where_near_items + i0, std::min(kWhereChunk, m - i0));
-            ++*launches;
-        }
-        CUDA_TRY(cudaGetLastError());
-        return WAX_VS_OK;
-    }
-    if ((rc = c->d_where_items.ensure(m, "where predicates"))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, stream));
-    for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
-        where_bits_kernel<<<where_grid(e, static_cast<uint64_t>(words) * 32u), kWhereThreads, 0, stream>>>(
-            e->d_attrs, n, words, c->d_mask, c->d_where_items + i0, std::min(kWhereChunk, m - i0));
-        ++*launches;
-    }
-    CUDA_TRY(cudaGetLastError());
-    return WAX_VS_OK;
+// ANDs items[i] into bitset items[i].slot of c->d_mask on `stream` (after the filter builders wrote it).
+static int32_t apply_where_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereNearItem> &items, cudaStream_t stream,
+                                uint64_t *launches) {
+    const uint32_t n = static_cast<uint32_t>(e->n_rows), words = (n + 31u) / 32u;
+    return where_pass(e, c, items, stream, launches, [&](auto located, const auto *d_items, uint32_t, uint32_t count) {
+        where_bits_kernel<decltype(located)::value><<<where_grid(e, static_cast<uint64_t>(words) * 32u), kWhereThreads, 0,
+                                                      stream>>>(e->d_attrs, e->d_locs, n, words, c->d_mask, d_items, count);
+    });
 }
 
-// The rows of the narrow predicates (fs.compact, with `boxes` fs.compact_boxes) into c->d_filter_rows at their slots, on
-// `stream`.
-static int32_t list_where_rows(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereItem> &items, cudaStream_t stream,
-                               uint64_t *launches, const std::vector<LocBox> *boxes = nullptr) {
+// The rows of the narrow predicates (fs.compact) into c->d_filter_rows at their slots, on `stream`.
+static int32_t list_where_rows(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereNearItem> &items, cudaStream_t stream,
+                               uint64_t *launches) {
     const uint32_t m = static_cast<uint32_t>(items.size()), n = static_cast<uint32_t>(e->n_rows);
     if (!m) return WAX_VS_OK;
     int32_t rc;
-    if (boxes) {
-        if ((rc = c->d_where_counts.ensure(m, "where cursors")) || (rc = stage_near_items(c, items, *boxes, stream))) return rc;
-        CUDA_TRY(cudaMemsetAsync(c->d_where_counts, 0, m * sizeof(uint32_t), stream));
-        for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
-            where_near_compact_kernel<<<where_grid(e, n), kWhereThreads, 0, stream>>>(
-                e->d_attrs, e->d_locs, n, c->d_where_near_items + i0, std::min(kWhereChunk, m - i0), c->d_where_counts + i0,
-                c->d_filter_rows);
-            ++*launches;
-        }
-        CUDA_TRY(cudaGetLastError());
-        return WAX_VS_OK;
-    }
-    if ((rc = c->d_where_items.ensure(m, "where predicates")) || (rc = c->d_where_counts.ensure(m, "where cursors"))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, stream));
+    if ((rc = c->d_where_counts.ensure(m, "where cursors"))) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_where_counts, 0, m * sizeof(uint32_t), stream));
-    for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
-        where_compact_kernel<<<where_grid(e, n), kWhereThreads, 0, stream>>>(e->d_attrs, n, c->d_where_items + i0,
-                                                                            std::min(kWhereChunk, m - i0),
-                                                                            c->d_where_counts + i0, c->d_filter_rows);
-        ++*launches;
-    }
-    CUDA_TRY(cudaGetLastError());
-    return WAX_VS_OK;
+    return where_pass(e, c, items, stream, launches, [&](auto located, const auto *d_items, uint32_t i0, uint32_t count) {
+        where_compact_kernel<decltype(located)::value><<<where_grid(e, n), kWhereThreads, 0, stream>>>(
+            e->d_attrs, e->d_locs, n, d_items, count, c->d_where_counts + i0, c->d_filter_rows);
+    });
 }
 
 // term_filter_kernel over `units` on `stream` (waxvs_terms.cuh): counting into c->d_term_counts (zeroed here) and, with
@@ -3247,12 +3221,11 @@ static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const int32_t *fi
     }
     int32_t rc;
     if ((rc = build_filter_bits(e, c, spec, nf, c->stream, launches))) { cudaStreamSynchronize(c->stream); return rc; }
-    std::vector<WhereItem> wbits;                               // where search: the predicates ANDed in
-    std::vector<LocBox> wboxes;                                 // ... and in where_near search their boxes
+    std::vector<WhereNearItem> wbits;                           // where search: the predicates ANDed in
     for (uint32_t l = 0; l < nf && !fs.where.empty(); ++l)
         if (fs.where[which[l]] != WAX_VS_NO_FILTER) {
-            wbits.push_back(WhereItem{fs.preds[fs.where[which[l]]], l});
-            if (fs.near) wboxes.push_back(fs.boxes[fs.where[which[l]]]);
+            wbits.push_back(fs.preds[fs.where[which[l]]]);
+            wbits.back().slot = l;
         }
     std::vector<TermUnit> tbits;                                // where_terms search: wide units' rows
     for (uint32_t l = 0; l < nf && !fs.term_of.empty(); ++l)
@@ -3260,7 +3233,7 @@ static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const int32_t *fi
             tbits.push_back(fs.term_wide[fs.term_of[which[l]]]);
             tbits.back().slot = l;
         }
-    if ((rc = apply_where_bits(e, c, wbits, c->stream, launches, fs.near ? &wboxes : nullptr)) ||
+    if ((rc = apply_where_bits(e, c, wbits, c->stream, launches)) ||
         (rc = launch_term_filter(e, c, tbits, nullptr, c->d_mask, c->stream, launches))) {
         cudaStreamSynchronize(c->stream);
         return rc;
@@ -3284,7 +3257,7 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
     if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
     if ((rc = stage_filter_rows(e, c, rows, rows.size() + fs.device_rows, -1, c->stream, nullptr))) return rc;
     uint64_t launches = 0;
-    if ((rc = list_where_rows(e, c, fs.compact, c->stream, &launches, fs.near ? &fs.compact_boxes : nullptr)) ||
+    if ((rc = list_where_rows(e, c, fs.compact, c->stream, &launches)) ||
         (rc = launch_term_filter(e, c, fs.term_list, c->d_filter_rows, nullptr, c->stream, &launches))) {
         cudaStreamSynchronize(c->stream);
         return rc;
@@ -3484,7 +3457,16 @@ constexpr uint64_t kWhereGatherRows = 16384;   // the gather class's largest all
 
 static WherePred where_pred(const wax_vs_where &w) { return WherePred{w.after, w.before, w.all_tags, w.no_tags}; }
 
-// Whether row r lies in box b (a row without a location lies in no box).
+// A where as the host plans it: the time and tag clauses, the location box (kNoLocBox: no location clause) and the
+// sorted, distinct term ids a row must hold (none: no term clause).
+struct Clause {
+    WherePred pred;
+    LocBox box;
+    std::vector<uint64_t> terms;
+};
+static WhereNearItem where_item(const Clause &w) { return WhereNearItem{w.pred, 0, w.box}; }
+
+// Whether row r lies in box b (a row without a location lies in no active box).
 static bool host_loc_passes(const wax_vs_engine *e, const LocBox &b, uint32_t r) {
     const LocRow l = e->locs_set ? e->locs[r] : LocRow{kNoLocation, 0};
     return loc_passes(b, l.lat, l.lon);
@@ -3499,15 +3481,12 @@ static bool host_terms_pass(const wax_vs_engine *e, const std::vector<uint64_t> 
     return std::includes(p, p + t.n, req.begin(), req.end());
 }
 
-// The listed rows that pass `w` (and lie in `box` unless that is nullptr, and hold the terms `req` unless that is
-// nullptr), appended to `out`.
-static void host_rows_passing(const wax_vs_engine *e, const WherePred &w, const uint32_t *rows, uint64_t n,
-                              std::vector<uint32_t> &out, const LocBox *box = nullptr,
-                              const std::vector<uint64_t> *req = nullptr) {
+// The listed rows that pass every clause of `w`, appended to `out`.
+static void host_rows_passing(const wax_vs_engine *e, const Clause &w, const uint32_t *rows, uint64_t n,
+                              std::vector<uint32_t> &out) {
     for (uint64_t i = 0; i < n; ++i) {
         const AttrRow a = e->attrs_set ? e->attrs[rows[i]] : AttrRow{0, 0};
-        if (where_passes(w, a.ts, a.tags) && (!box || host_loc_passes(e, *box, rows[i])) &&
-            (!req || host_terms_pass(e, *req, rows[i])))
+        if (where_passes(w.pred, a.ts, a.tags) && host_loc_passes(e, w.box, rows[i]) && host_terms_pass(e, w.terms, rows[i]))
             out.push_back(rows[i]);
     }
 }
@@ -3519,17 +3498,16 @@ static void host_rows_passing(const wax_vs_engine *e, const WherePred &w, const 
 // run_filtered at a slot from `at` on, as long as its count; a wide one gets its bits set in its bitset by the device,
 // under the sub-batch split of filter_bitset_bytes.  The lists are therefore bounded as the device-listed where rows
 // are, and no bitset is held outside that split.  A deny-list is checked by binary search in its rows, sorted, in
-// c->d_term_deny.  `at` ends past the last slot.
-static int32_t plan_term_units(wax_vs_engine *e, SearchCtx *c, const wax_vs_where *wheres, const LocBox *boxes,
-                               const std::vector<uint64_t> *terms, const FilterSet &ids,
+// c->d_term_deny.  The location mirror is brought up when some unit has a box.  `at` ends past the last slot.
+static int32_t plan_term_units(wax_vs_engine *e, SearchCtx *c, const std::vector<Clause> &wheres, const FilterSet &ids,
                                const std::vector<std::pair<uint32_t, uint32_t>> &pairs, const std::vector<uint32_t> &units_p,
                                FilterSet &fs, uint64_t &at) {
     int32_t rc;
-    if ((rc = ensure_term_index(e, c)) || (rc = ensure_attributes(e, c, boxes != nullptr))) return rc;
+    if ((rc = ensure_term_index(e, c))) return rc;
     const auto &ti = e->tindex;
     cudaStream_t s = c->stream;
     std::vector<uint64_t> req;
-    for (const uint32_t p : units_p) req.insert(req.end(), terms[pairs[p].first].begin(), terms[pairs[p].first].end());
+    for (const uint32_t p : units_p) req.insert(req.end(), wheres[pairs[p].first].terms.begin(), wheres[pairs[p].first].terms.end());
     std::sort(req.begin(), req.end());
     req.erase(std::unique(req.begin(), req.end()), req.end());
     const uint32_t n_ids = static_cast<uint32_t>(req.size());
@@ -3559,30 +3537,32 @@ static int32_t plan_term_units(wax_vs_engine *e, SearchCtx *c, const wax_vs_wher
     // each unit's candidates are the postings of its rarest term; a term no row holds leaves the unit empty
     std::vector<TermUnit> units;
     std::vector<uint32_t> unit_pair;
+    bool located = false;
     for (const uint32_t p : units_p) {
-        const uint32_t w = pairs[p].first, f = pairs[p].second;
+        const Clause &w = wheres[pairs[p].first];
+        const uint32_t f = pairs[p].second;
         fs.first[p] = at;
         fs.count[p] = 0;
         TermUnit u{};
-        u.pred = where_pred(wheres[w]);
-        const LocBox box = boxes ? boxes[w] : kNoLocBox;
-        u.box = box;
-        u.has_box = box.lat_lo != kNoLocBox.lat_lo || box.lat_hi != kNoLocBox.lat_hi || box.lon_lo0 != kNoLocBox.lon_lo0 ||
-                    box.lon_hi0 != kNoLocBox.lon_hi0 || box.lon_lo1 != kNoLocBox.lon_lo1 || box.lon_hi1 != kNoLocBox.lon_hi1;
-        u.n_spans = static_cast<uint32_t>(terms[w].size());
+        u.pred = w.pred;
+        u.box = w.box;
+        u.has_box = box_active(w.box);
+        u.n_spans = static_cast<uint32_t>(w.terms.size());
         u.deny = f == WAX_VS_NO_FILTER ? TermSpan{0, 0, 0} : deny_of[f];
         uint32_t rarest = 0;
         for (uint32_t j = 0; j < u.n_spans; ++j) {
-            u.spans[j] = spans[std::lower_bound(req.begin(), req.end(), terms[w][j]) - req.begin()];
+            u.spans[j] = spans[std::lower_bound(req.begin(), req.end(), w.terms[j]) - req.begin()];
             if (u.spans[j].count < u.spans[rarest].count) rarest = j;
         }
         if (u.spans[rarest].count == 0) continue;
         std::swap(u.spans[0], u.spans[rarest]);
+        located = located || u.has_box;
         units.push_back(u);
         unit_pair.push_back(p);
     }
     const uint32_t n_units = static_cast<uint32_t>(units.size());
     if (!n_units) return WAX_VS_OK;
+    if ((rc = ensure_attributes(e, c, located))) return rc;
     // sized once for the largest launch of the call (run_filtered launches subsets of these units)
     if ((rc = c->d_term_units.ensure(n_units, "term units")) || (rc = c->d_term_counts.ensure(n_units, "term counts")))
         return rc;
@@ -3613,15 +3593,13 @@ static int32_t plan_term_units(wax_vs_engine *e, SearchCtx *c, const wax_vs_wher
 }
 
 // The pairs of a call as the filters of `fs` (modes[p], pair_of[i] = query i's pair or WAX_VS_NO_FILTER), from the
-// resolved id filters `ids`.  Runs the count pass on c's stream.  boxes (where_near search; nullptr otherwise): wheres[w]
-// also requires boxes[w], on the host for allow-lists and in the location forms of the kernels otherwise.  terms
-// (where_terms search; nullptr otherwise): wheres[w] also requires the sorted, distinct ids terms[w]; a pair whose where
-// has some is tested on the host against an allow-list, and is a term unit (plan_term_units) otherwise.
-static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_where *wheres, uint32_t n_wheres,
+// resolved id filters `ids`.  Runs the count pass on c's stream.  A pair's where is tested whole on the host against an
+// allow-list; otherwise a where with terms makes the pair a term unit (plan_term_units), and any other where is tested
+// on the device, its box with it.
+static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const std::vector<Clause> &wheres,
                                 const uint32_t *query_where, const int32_t *filter_modes, const uint32_t *query_filter,
                                 uint32_t n_queries, const FilterSet &ids, FilterSet &fs, std::vector<int32_t> &modes,
-                                std::vector<uint32_t> &pair_of, const LocBox *boxes = nullptr,
-                                const std::vector<uint64_t> *terms = nullptr) {
+                                std::vector<uint32_t> &pair_of) {
     pair_of.assign(n_queries, WAX_VS_NO_FILTER);
     std::unordered_map<uint64_t, uint32_t> index;
     std::vector<std::pair<uint32_t, uint32_t>> pairs;              // (where, id filter)
@@ -3633,20 +3611,17 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_whe
         pair_of[i] = ins.first->second;
     }
     // the predicates whose count the plan needs: those of pairs without an allow-list
-    std::vector<uint32_t> slot(n_wheres, WAX_VS_NO_FILTER);
-    std::vector<WherePred> counted;
-    std::vector<LocBox> counted_boxes;
+    std::vector<uint32_t> slot(wheres.size(), WAX_VS_NO_FILTER);
+    std::vector<WhereNearItem> counted;
     for (const auto &pr : pairs)
         if (pr.first != WAX_VS_NO_FILTER && (pr.second == WAX_VS_NO_FILTER || filter_modes[pr.second] == 1) &&
-            slot[pr.first] == WAX_VS_NO_FILTER && !(terms && !terms[pr.first].empty())) {
+            slot[pr.first] == WAX_VS_NO_FILTER && wheres[pr.first].terms.empty()) {
             slot[pr.first] = static_cast<uint32_t>(counted.size());
-            counted.push_back(where_pred(wheres[pr.first]));
-            if (boxes) counted_boxes.push_back(boxes[pr.first]);
+            counted.push_back(where_item(wheres[pr.first]));
         }
     std::vector<uint32_t> passing;
     int32_t rc;
-    if ((rc = where_counts(e, c, counted, passing, boxes ? &counted_boxes : nullptr))) return rc;
-    fs.near = boxes != nullptr;
+    if ((rc = where_counts(e, c, counted, passing))) return rc;
     const uint32_t np = static_cast<uint32_t>(pairs.size());
     fs.first.assign(np, 0);
     fs.count.assign(np, 0);
@@ -3666,27 +3641,23 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_whe
             modes[p] = filter_modes[f];
             continue;
         }
-        const WherePred pred = where_pred(wheres[w]);
-        const bool has_terms = terms && !terms[w].empty();
-        if (has_terms && (f == WAX_VS_NO_FILTER || filter_modes[f] == 1)) {   // the device lists it from the postings
+        if (!wheres[w].terms.empty() && (f == WAX_VS_NO_FILTER || filter_modes[f] == 1)) {   // listed from the postings
             term_units.push_back(p);
             continue;
         }
-        host_rows_passing(e, pred, rows, n_listed, fs.rows, boxes ? &boxes[w] : nullptr, has_terms ? &terms[w] : nullptr);
+        host_rows_passing(e, wheres[w], rows, n_listed, fs.rows);
         fs.count[p] = fs.rows.size() - fs.first[p];
         if (f != WAX_VS_NO_FILTER && filter_modes[f] == 0) continue;          // allow-list AND where: an allow-list
         const uint64_t pass = passing[slot[w]];
         if (fs.count[p] == 0 && pass > 0 && pass <= kWhereGatherRows) {       // narrow: the device lists the rows
             fs.count[p] = pass;
-            fs.compact.push_back(WhereItem{pred, 0});
-            if (boxes) fs.compact_boxes.push_back(boxes[w]);
+            fs.compact.push_back(where_item(wheres[w]));
             listed_by_device.push_back(p);
             continue;
         }
         modes[p] = 1;                                                         // deny the listed rows that pass ...
         fs.where[p] = static_cast<uint32_t>(fs.preds.size());                 // ... within the rows that pass
-        fs.preds.push_back(pred);
-        if (boxes) fs.boxes.push_back(boxes[w]);
+        fs.preds.push_back(where_item(wheres[w]));
         fs.allowed[p] = pass - fs.count[p];
     }
     uint64_t at = fs.rows.size();                                             // device-listed rows follow the host's
@@ -3696,18 +3667,17 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const wax_vs_whe
         fs.compact[j].slot = at;
         at += fs.count[p];
     }
-    if (!term_units.empty() && (rc = plan_term_units(e, c, wheres, boxes, terms, ids, pairs, term_units, fs, at))) return rc;
+    if (!term_units.empty() && (rc = plan_term_units(e, c, wheres, ids, pairs, term_units, fs, at))) return rc;
     fs.device_rows = at - fs.rows.size();
     return WAX_VS_OK;
 }
 
-// The batched where entry points after their argument checks; boxes and terms as plan_where_pairs.
+// The batched where entry points after their argument checks and the building of their clauses.
 static int32_t search_where_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                  int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
                                  const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                 const wax_vs_where *wheres, uint32_t n_wheres, const uint32_t *query_where,
-                                 uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n,
-                                 const LocBox *boxes, const std::vector<uint64_t> *terms = nullptr) {
+                                 const std::vector<Clause> &wheres, const uint32_t *query_where, uint64_t *out_ids,
+                                 float *out_scores, uint32_t out_stride, uint32_t *out_n) {
     int32_t rc;
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
@@ -3722,8 +3692,8 @@ static int32_t search_where_host(wax_vs_engine *e, const float *queries, uint32_
     FilterSet fs;
     std::vector<int32_t> modes;
     std::vector<uint32_t> pair_of;
-    if ((rc = plan_where_pairs(e, lease.c, wheres, n_wheres, query_where, filter_modes, query_filter, n_queries, ids, fs,
-                               modes, pair_of, boxes, terms)))
+    if ((rc = plan_where_pairs(e, lease.c, wheres, query_where, filter_modes, query_filter, n_queries, ids, fs, modes,
+                               pair_of)))
         return rc;
     FilteredPlan plan;
     plan_filtered(e, top_k, modes.data(), pair_of.data(), n_queries, fs, plan);
@@ -3759,8 +3729,10 @@ int32_t wax_vs_search_batch_where(wax_vs_engine *e, const float *queries, uint32
     if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
                                n_wheres, query_where, out_n)))
         return rc;
+    std::vector<Clause> clauses(n_wheres);
+    for (uint32_t w = 0; w < n_wheres; ++w) clauses[w] = Clause{where_pred(wheres[w]), kNoLocBox, {}};
     return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
-                             query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_stride, out_n, nullptr);
+                             query_filter, clauses, query_where, out_ids, out_scores, out_stride, out_n);
 }
 
 // ---- location predicates: PhotoRAG's location box beside the time and tag clauses (waxvs_where.cuh) -----------------
@@ -3875,23 +3847,19 @@ int32_t wax_vs_set_locations(wax_vs_engine *e, const uint64_t *frame_ids, const 
     return WAX_VS_OK;
 }
 
-// The time and tag clauses of wheres[i] and their boxes; *any = some box is active.
-static int32_t split_near(const wax_vs_where_near *wheres, uint32_t n_wheres, std::vector<wax_vs_where> &plain,
-                          std::vector<LocBox> &boxes, bool *any) {
-    plain.resize(n_wheres);
-    boxes.resize(n_wheres);
-    *any = false;
+// The clauses of wheres[0, n_wheres): the time and tag clauses and the location box of each, no terms.
+static int32_t near_clauses(const wax_vs_where_near *wheres, uint32_t n_wheres, std::vector<Clause> &clauses) {
+    clauses.resize(n_wheres);
     for (uint32_t i = 0; i < n_wheres; ++i) {
-        plain[i] = wheres[i].where;
+        clauses[i].pred = where_pred(wheres[i].where);
         bool active;
         int32_t rc;
-        if ((rc = location_box(wheres[i].latitude, wheres[i].longitude, wheres[i].radius_m, &boxes[i], &active))) return rc;
-        *any = *any || active;
+        if ((rc = location_box(wheres[i].latitude, wheres[i].longitude, wheres[i].radius_m, &clauses[i].box, &active)))
+            return rc;
     }
     return WAX_VS_OK;
 }
 
-// A call whose boxes are all "no location clause" is wax_vs_search_batch_where with the time and tag clauses.
 int32_t wax_vs_search_batch_where_near(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                        int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
                                        const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
@@ -3901,13 +3869,10 @@ int32_t wax_vs_search_batch_where_near(wax_vs_engine *e, const float *queries, u
     if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
                                n_wheres, query_where, out_n)))
         return rc;
-    std::vector<wax_vs_where> plain;
-    std::vector<LocBox> boxes;
-    bool any;
-    if ((rc = split_near(wheres, n_wheres, plain, boxes, &any))) return rc;
+    std::vector<Clause> clauses;
+    if ((rc = near_clauses(wheres, n_wheres, clauses))) return rc;
     return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
-                             query_filter, plain.data(), n_wheres, query_where, out_ids, out_scores, out_stride, out_n,
-                             any ? boxes.data() : nullptr);
+                             query_filter, clauses, query_where, out_ids, out_scores, out_stride, out_n);
 }
 
 // ---- term clauses: Wax's metadataFilter as required term ids, from an inverted index (waxvs_terms.cuh) ---------------
@@ -3968,7 +3933,6 @@ int32_t wax_vs_set_terms(wax_vs_engine *e, const uint64_t *frame_ids, const uint
     return WAX_VS_OK;
 }
 
-// A call none of whose wheres has a term runs wax_vs_search_batch_where_near.
 int32_t wax_vs_search_batch_where_terms(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                         int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
                                         const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
@@ -3981,37 +3945,31 @@ int32_t wax_vs_search_batch_where_terms(wax_vs_engine *e, const float *queries, 
         return rc;
     if (!where_term_offsets) return fail(WAX_VS_ERR_NULL, "where_term_offsets is NULL");
     if ((rc = check_term_offsets(where_term_offsets, n_wheres, where_terms, kMaxWhereTerms, "where_term_offsets"))) return rc;
-    if (where_term_offsets[n_wheres] == 0)
-        return wax_vs_search_batch_where_near(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets,
-                                              filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids,
-                                              out_scores, out_stride, out_n);
-    std::vector<wax_vs_where> plain;
-    std::vector<LocBox> boxes;
-    bool any;
-    if ((rc = split_near(wheres, n_wheres, plain, boxes, &any))) return rc;
-    std::vector<std::vector<uint64_t>> terms(n_wheres);
+    std::vector<Clause> clauses;
+    if ((rc = near_clauses(wheres, n_wheres, clauses))) return rc;
     for (uint32_t w = 0; w < n_wheres; ++w) {
-        terms[w].assign(where_terms + where_term_offsets[w], where_terms + where_term_offsets[w + 1]);
-        std::sort(terms[w].begin(), terms[w].end());
-        terms[w].erase(std::unique(terms[w].begin(), terms[w].end()), terms[w].end());
+        std::vector<uint64_t> &terms = clauses[w].terms;
+        terms.assign(where_terms + where_term_offsets[w], where_terms + where_term_offsets[w + 1]);
+        std::sort(terms.begin(), terms.end());
+        terms.erase(std::unique(terms.begin(), terms.end()), terms.end());
     }
     // Wheres with terms and equal contents (clauses, box, required ids) are one: each query names the first of them, so
     // a batch that scopes 1 024 queries to 16 sessions plans 16 units, not 1 024.
     std::vector<uint32_t> canon(n_wheres);
     std::unordered_map<std::string, uint32_t> first_of;
     for (uint32_t w = 0; w < n_wheres; ++w) {
+        const Clause &cl = clauses[w];
         canon[w] = w;
-        if (terms[w].empty()) continue;
-        std::string key(reinterpret_cast<const char *>(&plain[w]), sizeof(wax_vs_where));
-        key.append(reinterpret_cast<const char *>(&boxes[w]), sizeof(LocBox));
-        key.append(reinterpret_cast<const char *>(terms[w].data()), terms[w].size() * sizeof(uint64_t));
+        if (cl.terms.empty()) continue;
+        std::string key(reinterpret_cast<const char *>(&cl.pred), sizeof(WherePred));
+        key.append(reinterpret_cast<const char *>(&cl.box), sizeof(LocBox));
+        key.append(reinterpret_cast<const char *>(cl.terms.data()), cl.terms.size() * sizeof(uint64_t));
         canon[w] = first_of.emplace(std::move(key), w).first->second;
     }
     std::vector<uint32_t> qw(n_queries);
     for (uint32_t i = 0; i < n_queries; ++i) qw[i] = query_where[i] == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : canon[query_where[i]];
     return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
-                             query_filter, plain.data(), n_wheres, qw.data(), out_ids, out_scores, out_stride, out_n,
-                             any ? boxes.data() : nullptr, terms.data());
+                             query_filter, clauses, qw.data(), out_ids, out_scores, out_stride, out_n);
 }
 
 // The row-sharded form: every rank passes the SAME ids; a rank resolves the ones its shard holds (the others are
@@ -4239,11 +4197,11 @@ static uint32_t deliver_group_keys(const wax_vs_engine *e, const uint64_t *keys,
 
 // One grouped search under the caller's read lock and scratch context (re-taking the shared lock inside a batch could
 // wait behind a queued writer): the host query, the filter's resolved rows (nullptr: unfiltered; the filter allows some
-// row), the answer at out_* and *out_n.  The arguments are checked by the caller.
+// row) with `where` ANDed into its bitset (nullptr: none), the answer at out_* and *out_n.  The arguments are checked by
+// the caller.
 static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, uint32_t n_top, uint32_t per_group,
-                           const std::vector<uint32_t> *rows, int32_t mode, const WherePred *where, uint64_t *out_ids,
-                           float *out_scores, uint64_t *out_groups, uint32_t *out_n,
-                           const std::vector<LocBox> *where_box = nullptr) {
+                           const std::vector<uint32_t> *rows, int32_t mode, const Clause *where, uint64_t *out_ids,
+                           float *out_scores, uint64_t *out_groups, uint32_t *out_n) {
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const bool filtered = rows != nullptr;
     cudaStream_t s = c->stream;
@@ -4258,7 +4216,7 @@ static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, u
     if ((rc = c->h_out.ensure(n_top, "result staging"))) return rc;
     if (filtered) {
         if ((rc = stage_filter_rows(e, c, *rows, rows->size(), mode, s, &launches)) ||
-            (where && (rc = apply_where_bits(e, c, {WhereItem{*where, 0}}, s, &launches, where_box)))) {
+            (where && (rc = apply_where_bits(e, c, {where_item(*where)}, s, &launches)))) {
             cudaStreamSynchronize(s);
             return rc;
         }
@@ -4422,8 +4380,8 @@ static int32_t check_grouped_args(const wax_vs_engine *e, int64_t top_groups, ui
     return WAX_VS_OK;
 }
 
-// Every grouped entry point after its argument checks: query i searches the rows passing wheres[query_where[i]] (and
-// boxes[query_where[i]] unless boxes is nullptr) AND id filter query_filter[i], either of which may be WAX_VS_NO_FILTER.
+// Every grouped entry point after its argument checks: query i searches the rows passing wheres[query_where[i]] AND id
+// filter query_filter[i], either of which may be WAX_VS_NO_FILTER.
 // The (where, id filter) pairs are the units of the where search (plan_where_pairs), planned by the batched filtered
 // search at k_c; a query no row passes answers nothing.  Without `batched`, or when the coverage level does not take the
 // batch, every query runs grouped_one.  The batch pipeline:
@@ -4435,9 +4393,9 @@ static int32_t check_grouped_args(const wax_vs_engine *e, int64_t top_groups, ui
 static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                    int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids,
                                    const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
-                                   const uint32_t *query_filter, const wax_vs_where *wheres, uint32_t n_wheres,
-                                   const uint32_t *query_where, const LocBox *boxes, uint64_t *out_ids, float *out_scores,
-                                   uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n, bool batched) {
+                                   const uint32_t *query_filter, const std::vector<Clause> &wheres,
+                                   const uint32_t *query_where, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
+                                   uint32_t out_stride, uint32_t *out_n, bool batched) {
     const uint32_t n_top = clamp_topk(top_groups);
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
@@ -4457,8 +4415,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     FilterSet fs;
     std::vector<int32_t> modes;
     std::vector<uint32_t> pair_of;
-    if ((rc = plan_where_pairs(e, c, wheres, n_wheres, query_where, filter_modes, query_filter, n_queries, ids, fs, modes,
-                               pair_of, boxes)))
+    if ((rc = plan_where_pairs(e, c, wheres, query_where, filter_modes, query_filter, n_queries, ids, fs, modes, pair_of)))
         return rc;
     // The coverage level: each query's exact top-k_c rows, when the batch goes to the tensor-core levels or the gather
     // class of the batched filtered search; every other batch runs the single-query pipeline per query.
@@ -4552,20 +4509,16 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
         const bool row_where = w != WAX_VS_NO_FILTER && (f == WAX_VS_NO_FILTER || filter_modes[f] == 1);
         std::vector<uint32_t> rows;
         int32_t mode = 1;
-        WherePred pred{};
-        std::vector<LocBox> box;
         if (row_where) {
             if (f != WAX_VS_NO_FILTER) rows.assign(ids.rows.begin() + ids.first[f], ids.rows.begin() + ids.first[f] + ids.count[f]);
-            pred = where_pred(wheres[w]);
-            if (boxes) box.assign(1, boxes[w]);
         } else if (p != WAX_VS_NO_FILTER) {
             rows.assign(fs.rows.begin() + fs.first[p], fs.rows.begin() + fs.first[p] + fs.count[p]);
             mode = modes[p];
         }
         const size_t o = static_cast<size_t>(qi) * out_stride;
         if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group,
-                              p == WAX_VS_NO_FILTER ? nullptr : &rows, mode, row_where ? &pred : nullptr, out_ids + o,
-                              out_scores + o, out_groups + o, out_n + qi, row_where && boxes ? &box : nullptr)))
+                              p == WAX_VS_NO_FILTER ? nullptr : &rows, mode, row_where ? &wheres[w] : nullptr, out_ids + o,
+                              out_scores + o, out_groups + o, out_n + qi)))
             return rc;
     }
     if (!batched) return WAX_VS_OK;
@@ -4577,13 +4530,11 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     return WAX_VS_OK;
 }
 
-// The one-filter grouped entry points: one id filter (an empty deny-list is none) and at most one where (with `box`, its
-// active location box) for every query.
+// The one-filter grouped entry points: one id filter (an empty deny-list is none) and at most one where for every query.
 static int32_t search_grouped_one_filter(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                          int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
                                          int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
-                                         uint32_t out_stride, uint32_t *out_n, bool batched,
-                                         const wax_vs_where *where = nullptr, const LocBox *box = nullptr) {
+                                         uint32_t out_stride, uint32_t *out_n, bool batched, const Clause *where = nullptr) {
     int32_t rc;
     if ((rc = check_grouped_args(e, top_groups, per_group, out_ids, out_scores, out_groups, out_n))) return rc;
     if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
@@ -4591,9 +4542,11 @@ static int32_t search_grouped_one_filter(wax_vs_engine *e, const float *queries,
     const uint64_t offsets[2] = {0, n_ids};
     const std::vector<uint32_t> query_filter(n_queries, mode == 1 && n_ids == 0 ? WAX_VS_NO_FILTER : 0u);
     const std::vector<uint32_t> query_where(n_queries, where ? 0u : WAX_VS_NO_FILTER);
+    std::vector<Clause> wheres;
+    if (where) wheres.push_back(*where);
     return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, offsets, &mode, 1,
-                               query_filter.data(), where, where ? 1u : 0u, query_where.data(), box, out_ids, out_scores,
-                               out_groups, out_stride, out_n, batched);
+                               query_filter.data(), wheres, query_where.data(), out_ids, out_scores, out_groups, out_stride,
+                               out_n, batched);
 }
 
 int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_groups,
@@ -4618,27 +4571,24 @@ int32_t wax_vs_search_batch_grouped_where(wax_vs_engine *e, const float *queries
                                           int32_t mode, const wax_vs_where *where, uint64_t *out_ids, float *out_scores,
                                           uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n) {
     if (!where) return fail(WAX_VS_ERR_NULL, "where is NULL");
+    const Clause clause{where_pred(*where), kNoLocBox, {}};
     return search_grouped_one_filter(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode,
-                                     out_ids, out_scores, out_groups, out_stride, out_n, n_queries > 1, where);
+                                     out_ids, out_scores, out_groups, out_stride, out_n, n_queries > 1, &clause);
 }
 
-// A predicate whose box is "no location clause" is wax_vs_search_batch_grouped_where with its time and tag clauses.
 int32_t wax_vs_search_batch_grouped_where_near(wax_vs_engine *e, const float *queries, uint32_t n_queries,
                                                uint32_t query_len, int64_t top_groups, uint32_t per_group,
                                                const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
                                                const wax_vs_where_near *where, uint64_t *out_ids, float *out_scores,
                                                uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n) {
     if (!where) return fail(WAX_VS_ERR_NULL, "where is NULL");
-    LocBox box;
-    bool active;
+    std::vector<Clause> clause;
     int32_t rc;
-    if ((rc = location_box(where->latitude, where->longitude, where->radius_m, &box, &active))) return rc;
+    if ((rc = near_clauses(where, 1, clause))) return rc;
     return search_grouped_one_filter(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode,
-                                     out_ids, out_scores, out_groups, out_stride, out_n, n_queries > 1, &where->where,
-                                     active ? &box : nullptr);
+                                     out_ids, out_scores, out_groups, out_stride, out_n, n_queries > 1, &clause[0]);
 }
 
-// A call whose boxes are all "no location clause" plans without the location forms, as wax_vs_search_batch_where.
 int32_t wax_vs_search_batch_grouped_multi_where(wax_vs_engine *e, const float *queries, uint32_t n_queries,
                                                 uint32_t query_len, int64_t top_groups, uint32_t per_group,
                                                 const uint64_t *frame_ids, const uint64_t *filter_offsets,
@@ -4652,14 +4602,11 @@ int32_t wax_vs_search_batch_grouped_multi_where(wax_vs_engine *e, const float *q
         (rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
                                n_wheres, query_where, out_n)))
         return rc;
-    std::vector<wax_vs_where> plain;
-    std::vector<LocBox> boxes;
-    bool any;
-    if ((rc = split_near(wheres, n_wheres, plain, boxes, &any))) return rc;
+    std::vector<Clause> clauses;
+    if ((rc = near_clauses(wheres, n_wheres, clauses))) return rc;
     return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, filter_offsets,
-                               filter_modes, n_filters, query_filter, plain.data(), n_wheres, query_where,
-                               any ? boxes.data() : nullptr, out_ids, out_scores, out_groups, out_stride, out_n,
-                               n_queries > 1);
+                               filter_modes, n_filters, query_filter, clauses, query_where, out_ids, out_scores, out_groups,
+                               out_stride, out_n, n_queries > 1);
 }
 
 // ---- persistence ---------------------------------------------------------------------------------------------

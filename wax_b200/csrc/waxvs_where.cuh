@@ -1,5 +1,5 @@
-// waxvs_where.cuh -- frame attributes on the device: the time-range and tag predicates of wax_vs_search_batch_where and
-// wax_vs_search_batch_grouped_where.
+// waxvs_where.cuh -- frame attributes on the device: the time-range, tag and location predicates of the where searches
+// (wax_vs_search_batch_where and its _near, _terms and grouped forms).
 //
 // Wax post-filters every vector hit on the frame's metadata (UnifiedSearch.passesFrameFilter,
 // Sources/Wax/UnifiedSearch/UnifiedSearch.swift:1241-1258): a timeRange (TimeRange.contains, SearchRequest.swift:90-105:
@@ -13,12 +13,13 @@
 // All three read each row's 16 bytes once per launch and test every predicate of the launch against it in registers;
 // the predicates of a launch (at most kWhereChunk) sit in shared memory.
 //
-// The location forms (where_near_*_kernel, wax_vs_search_batch_where_near) add PhotoRAG's location box: each row also
-// carries its location bins (LocRow, 8 bytes, one 8-byte load per row beside the AttrRow's LDG.128), and each predicate
-// a box of bins (WhereNearItem) tested in registers next to the time and tag clauses.  They are kernels of their own, so
-// the three above keep their code exactly.
+// Each kernel has two forms, chosen by the host per launch.  The located form (kLocated = true) adds PhotoRAG's location
+// box: each row also carries its location bins (LocRow, 8 bytes, one 8-byte load per row beside the AttrRow's LDG.128),
+// and each predicate a box of bins (WhereNearItem) tested in registers next to the time and tag clauses.  The plain form
+// takes WhereItems, reads no location and ignores `locs`.
 #pragma once
 #include <cstdint>
+#include <type_traits>
 
 namespace waxvs {
 
@@ -41,107 +42,6 @@ struct WhereItem {
     uint64_t slot;
 };
 
-constexpr uint32_t kWhereChunk = 256;     // predicates per launch (shared memory: 10 KiB of items -- 16 KiB in the
-                                          // location forms -- and 8 KiB of counts)
-constexpr uint32_t kWhereThreads = 256;
-
-// TimeRange.contains with INT64_MAX as "no upper bound" (a timestamp of INT64_MAX then passes), and the two tag tests.
-__host__ __device__ __forceinline__ bool where_passes(const WherePred &w, int64_t ts, uint64_t tags) {
-    return ts >= w.after && (ts < w.before || w.before == INT64_MAX) && (tags & w.all_tags) == w.all_tags &&
-           (tags & w.no_tags) == 0u;
-}
-
-__device__ __forceinline__ AttrRow load_attr(const AttrRow *attrs, uint32_t row) {
-    const longlong2 v = __ldg(reinterpret_cast<const longlong2 *>(attrs) + row);
-    return AttrRow{v.x, static_cast<uint64_t>(v.y)};
-}
-
-__device__ __forceinline__ void stage_items(WhereItem *s_items, const WhereItem *items, uint32_t n_items) {
-    uint64_t *dst = reinterpret_cast<uint64_t *>(s_items);
-    const uint64_t *src = reinterpret_cast<const uint64_t *>(items);
-    for (uint32_t i = threadIdx.x; i < n_items * (sizeof(WhereItem) / 8); i += blockDim.x) dst[i] = src[i];
-}
-
-// counts[i] += rows of [0, n) passing items[i].pred, i < n_items <= kWhereChunk.  Each warp adds its ballots' popcounts to
-// its own shared counters (no atomics), the CTA sums them and issues one global atomic per (CTA, predicate).
-__global__ void __launch_bounds__(kWhereThreads) where_count_kernel(const AttrRow *__restrict__ attrs, uint32_t n,
-                                                                    const WhereItem *__restrict__ items, uint32_t n_items,
-                                                                    uint32_t *__restrict__ counts) {
-    __shared__ WhereItem s_items[kWhereChunk];
-    __shared__ uint32_t s_count[kWhereThreads / 32][kWhereChunk];
-    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    stage_items(s_items, items, n_items);
-    for (uint32_t i = threadIdx.x; i < (kWhereThreads / 32) * kWhereChunk; i += blockDim.x) (&s_count[0][0])[i] = 0u;
-    __syncthreads();
-    const uint32_t stride = gridDim.x * blockDim.x;
-    for (uint32_t base = blockIdx.x * blockDim.x; base < n; base += stride) {     // warp-uniform bounds
-        const uint32_t row = base + threadIdx.x;
-        const bool live = row < n;
-        const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
-        for (uint32_t i = 0; i < n_items; ++i) {
-            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && where_passes(s_items[i].pred, a.ts, a.tags));
-            if (lane == 0) s_count[warp][i] += __popc(b);
-        }
-    }
-    __syncthreads();
-    for (uint32_t i = threadIdx.x; i < n_items; i += blockDim.x) {
-        uint32_t sum = 0;
-#pragma unroll
-        for (uint32_t w = 0; w < kWhereThreads / 32; ++w) sum += s_count[w][i];
-        if (sum) atomicAdd(counts + i, sum);
-    }
-}
-
-// bits[items[i].slot * words + word] &= the predicate's ballot over the word's 32 rows (rows >= n fail).  A warp owns a
-// word, so the read-modify-write needs no atomic; a bitset is named by at most one item of a launch.
-__global__ void __launch_bounds__(kWhereThreads) where_bits_kernel(const AttrRow *__restrict__ attrs, uint32_t n,
-                                                                   uint32_t words, uint32_t *__restrict__ bits,
-                                                                   const WhereItem *__restrict__ items, uint32_t n_items) {
-    __shared__ WhereItem s_items[kWhereChunk];
-    const uint32_t lane = threadIdx.x & 31u;
-    stage_items(s_items, items, n_items);
-    __syncthreads();
-    const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
-    for (uint32_t word = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; word < words; word += warps) {
-        const uint32_t row = (word << 5) + lane;
-        const bool live = row < n;
-        const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
-        for (uint32_t i = 0; i < n_items; ++i) {
-            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && where_passes(s_items[i].pred, a.ts, a.tags));
-            if (lane == 0 && b != 0xFFFFFFFFu) bits[s_items[i].slot * words + word] &= b;
-        }
-    }
-}
-
-// The rows passing items[i].pred, written to rows_out[items[i].slot + j] for j < the predicate's count (cursor[i], zeroed
-// by the caller, ends at that count).  The order within a list is arbitrary: the gather class sorts by (distance, row).
-__global__ void __launch_bounds__(kWhereThreads) where_compact_kernel(const AttrRow *__restrict__ attrs, uint32_t n,
-                                                                      const WhereItem *__restrict__ items, uint32_t n_items,
-                                                                      uint32_t *__restrict__ cursor,
-                                                                      uint32_t *__restrict__ rows_out) {
-    __shared__ WhereItem s_items[kWhereChunk];
-    const uint32_t lane = threadIdx.x & 31u;
-    stage_items(s_items, items, n_items);
-    __syncthreads();
-    const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
-    const uint32_t below = (1u << lane) - 1u;
-    for (uint32_t word = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; word < (n + 31u) / 32u; word += warps) {
-        const uint32_t row = (word << 5) + lane;
-        const bool live = row < n;
-        const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
-        for (uint32_t i = 0; i < n_items; ++i) {
-            const bool pass = live && where_passes(s_items[i].pred, a.ts, a.tags);
-            const uint32_t b = __ballot_sync(0xFFFFFFFFu, pass);
-            if (!b) continue;
-            uint32_t at = 0;
-            if (lane == 0) at = atomicAdd(cursor + i, static_cast<uint32_t>(__popc(b)));
-            at = __shfl_sync(0xFFFFFFFFu, at, 0);
-            if (pass) rows_out[s_items[i].slot + at + __popc(b & below)] = row;
-        }
-    }
-}
-
-// ---- location forms ----------------------------------------------------------------------------------------------
 // A row's location as PhotoRAG bins it (locationBin(from:), PhotoRAGOrchestrator.swift:868-875): floor(lat * 100) and
 // floor(lon * 100), saturated to int32.  A row without a location has lat == kNoLocation, below every box.
 struct alignas(8) LocRow {
@@ -157,43 +57,66 @@ struct LocBox {
 };
 constexpr LocBox kNoLocBox{INT32_MIN, INT32_MAX, INT32_MIN, INT32_MAX, 1, 0};
 
-__host__ __device__ __forceinline__ bool loc_passes(const LocBox &b, int32_t lat, int32_t lon) {
-    return lat >= b.lat_lo && lat <= b.lat_hi && ((lon >= b.lon_lo0 && lon <= b.lon_hi0) || (lon >= b.lon_lo1 && lon <= b.lon_hi1));
-}
-
-// A WhereItem with its predicate's box (64 bytes).
+// A WhereItem with its predicate's box (64 bytes): the item of the located form.
 struct WhereNearItem {
     WherePred pred;
     uint64_t slot;
     LocBox box;
 };
+template <bool kLocated> using WhereItemOf = std::conditional_t<kLocated, WhereNearItem, WhereItem>;
 
-__device__ __forceinline__ void stage_near_items(WhereNearItem *s_items, const WhereNearItem *items, uint32_t n_items) {
-    uint64_t *dst = reinterpret_cast<uint64_t *>(s_items);
-    const uint64_t *src = reinterpret_cast<const uint64_t *>(items);
-    for (uint32_t i = threadIdx.x; i < n_items * (sizeof(WhereNearItem) / 8); i += blockDim.x) dst[i] = src[i];
+constexpr uint32_t kWhereChunk = 256;     // predicates per launch (shared memory: 10 KiB of items -- 16 KiB in the
+                                          // located form -- and 8 KiB of counts)
+constexpr uint32_t kWhereThreads = 256;
+
+// TimeRange.contains with INT64_MAX as "no upper bound" (a timestamp of INT64_MAX then passes), and the two tag tests.
+__host__ __device__ __forceinline__ bool where_passes(const WherePred &w, int64_t ts, uint64_t tags) {
+    return ts >= w.after && (ts < w.before || w.before == INT64_MAX) && (tags & w.all_tags) == w.all_tags &&
+           (tags & w.no_tags) == 0u;
 }
 
-// Row `row`'s location, or one in no box past the end.
+__host__ __device__ __forceinline__ bool loc_passes(const LocBox &b, int32_t lat, int32_t lon) {
+    return lat >= b.lat_lo && lat <= b.lat_hi && ((lon >= b.lon_lo0 && lon <= b.lon_hi0) || (lon >= b.lon_lo1 && lon <= b.lon_hi1));
+}
+
+__device__ __forceinline__ AttrRow load_attr(const AttrRow *attrs, uint32_t row) {
+    const longlong2 v = __ldg(reinterpret_cast<const longlong2 *>(attrs) + row);
+    return AttrRow{v.x, static_cast<uint64_t>(v.y)};
+}
+
+// Row `row`'s location, or one in no box past the end; the plain where form (kLocated = false) loads nothing.
+template <bool kLocated = true>
 __device__ __forceinline__ LocRow load_loc(const LocRow *locs, uint32_t row, bool live) {
-    if (!live) return LocRow{kNoLocation, 0};
+    if (!kLocated || !live) return LocRow{kNoLocation, 0};
     const int2 v = __ldg(reinterpret_cast<const int2 *>(locs) + row);
     return LocRow{v.x, v.y};
 }
 
-__device__ __forceinline__ bool near_passes(const WhereNearItem &it, const AttrRow &a, const LocRow &l) {
+__device__ __forceinline__ bool item_passes(const WhereItem &it, const AttrRow &a, const LocRow &) {
+    return where_passes(it.pred, a.ts, a.tags);
+}
+__device__ __forceinline__ bool item_passes(const WhereNearItem &it, const AttrRow &a, const LocRow &l) {
     return where_passes(it.pred, a.ts, a.tags) && loc_passes(it.box, l.lat, l.lon);
 }
 
-// where_count_kernel with each predicate's box.
-__global__ void __launch_bounds__(kWhereThreads) where_near_count_kernel(const AttrRow *__restrict__ attrs,
-                                                                         const LocRow *__restrict__ locs, uint32_t n,
-                                                                         const WhereNearItem *__restrict__ items,
-                                                                         uint32_t n_items, uint32_t *__restrict__ counts) {
-    __shared__ WhereNearItem s_items[kWhereChunk];
+template <class Item>
+__device__ __forceinline__ void stage_items(Item *s_items, const Item *items, uint32_t n_items) {
+    uint64_t *dst = reinterpret_cast<uint64_t *>(s_items);
+    const uint64_t *src = reinterpret_cast<const uint64_t *>(items);
+    for (uint32_t i = threadIdx.x; i < n_items * (sizeof(Item) / 8); i += blockDim.x) dst[i] = src[i];
+}
+
+// counts[i] += rows of [0, n) passing items[i], i < n_items <= kWhereChunk.  Each warp adds its ballots' popcounts to its
+// own shared counters (no atomics), the CTA sums them and issues one global atomic per (CTA, predicate).
+template <bool kLocated>
+__global__ void __launch_bounds__(kWhereThreads) where_count_kernel(const AttrRow *__restrict__ attrs,
+                                                                    const LocRow *__restrict__ locs, uint32_t n,
+                                                                    const WhereItemOf<kLocated> *__restrict__ items,
+                                                                    uint32_t n_items, uint32_t *__restrict__ counts) {
+    __shared__ WhereItemOf<kLocated> s_items[kWhereChunk];
     __shared__ uint32_t s_count[kWhereThreads / 32][kWhereChunk];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
-    stage_near_items(s_items, items, n_items);
+    stage_items(s_items, items, n_items);
     for (uint32_t i = threadIdx.x; i < (kWhereThreads / 32) * kWhereChunk; i += blockDim.x) (&s_count[0][0])[i] = 0u;
     __syncthreads();
     const uint32_t stride = gridDim.x * blockDim.x;
@@ -201,9 +124,9 @@ __global__ void __launch_bounds__(kWhereThreads) where_near_count_kernel(const A
         const uint32_t row = base + threadIdx.x;
         const bool live = row < n;
         const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
-        const LocRow l = load_loc(locs, row, live);
+        const LocRow l = load_loc<kLocated>(locs, row, live);
         for (uint32_t i = 0; i < n_items; ++i) {
-            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && near_passes(s_items[i], a, l));
+            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && item_passes(s_items[i], a, l));
             if (lane == 0) s_count[warp][i] += __popc(b);
         }
     }
@@ -216,38 +139,42 @@ __global__ void __launch_bounds__(kWhereThreads) where_near_count_kernel(const A
     }
 }
 
-// where_bits_kernel with each predicate's box.
-__global__ void __launch_bounds__(kWhereThreads) where_near_bits_kernel(const AttrRow *__restrict__ attrs,
-                                                                        const LocRow *__restrict__ locs, uint32_t n,
-                                                                        uint32_t words, uint32_t *__restrict__ bits,
-                                                                        const WhereNearItem *__restrict__ items,
-                                                                        uint32_t n_items) {
-    __shared__ WhereNearItem s_items[kWhereChunk];
+// bits[items[i].slot * words + word] &= the predicate's ballot over the word's 32 rows (rows >= n fail).  A warp owns a
+// word, so the read-modify-write needs no atomic; a bitset is named by at most one item of a launch.
+template <bool kLocated>
+__global__ void __launch_bounds__(kWhereThreads) where_bits_kernel(const AttrRow *__restrict__ attrs,
+                                                                   const LocRow *__restrict__ locs, uint32_t n,
+                                                                   uint32_t words, uint32_t *__restrict__ bits,
+                                                                   const WhereItemOf<kLocated> *__restrict__ items,
+                                                                   uint32_t n_items) {
+    __shared__ WhereItemOf<kLocated> s_items[kWhereChunk];
     const uint32_t lane = threadIdx.x & 31u;
-    stage_near_items(s_items, items, n_items);
+    stage_items(s_items, items, n_items);
     __syncthreads();
     const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
     for (uint32_t word = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; word < words; word += warps) {
         const uint32_t row = (word << 5) + lane;
         const bool live = row < n;
         const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
-        const LocRow l = load_loc(locs, row, live);
+        const LocRow l = load_loc<kLocated>(locs, row, live);
         for (uint32_t i = 0; i < n_items; ++i) {
-            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && near_passes(s_items[i], a, l));
+            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && item_passes(s_items[i], a, l));
             if (lane == 0 && b != 0xFFFFFFFFu) bits[s_items[i].slot * words + word] &= b;
         }
     }
 }
 
-// where_compact_kernel with each predicate's box.
-__global__ void __launch_bounds__(kWhereThreads) where_near_compact_kernel(const AttrRow *__restrict__ attrs,
-                                                                           const LocRow *__restrict__ locs, uint32_t n,
-                                                                           const WhereNearItem *__restrict__ items,
-                                                                           uint32_t n_items, uint32_t *__restrict__ cursor,
-                                                                           uint32_t *__restrict__ rows_out) {
-    __shared__ WhereNearItem s_items[kWhereChunk];
+// The rows passing items[i], written to rows_out[items[i].slot + j] for j < the predicate's count (cursor[i], zeroed by
+// the caller, ends at that count).  The order within a list is arbitrary: the gather class sorts by (distance, row).
+template <bool kLocated>
+__global__ void __launch_bounds__(kWhereThreads) where_compact_kernel(const AttrRow *__restrict__ attrs,
+                                                                      const LocRow *__restrict__ locs, uint32_t n,
+                                                                      const WhereItemOf<kLocated> *__restrict__ items,
+                                                                      uint32_t n_items, uint32_t *__restrict__ cursor,
+                                                                      uint32_t *__restrict__ rows_out) {
+    __shared__ WhereItemOf<kLocated> s_items[kWhereChunk];
     const uint32_t lane = threadIdx.x & 31u;
-    stage_near_items(s_items, items, n_items);
+    stage_items(s_items, items, n_items);
     __syncthreads();
     const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
     const uint32_t below = (1u << lane) - 1u;
@@ -255,9 +182,9 @@ __global__ void __launch_bounds__(kWhereThreads) where_near_compact_kernel(const
         const uint32_t row = (word << 5) + lane;
         const bool live = row < n;
         const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
-        const LocRow l = load_loc(locs, row, live);
+        const LocRow l = load_loc<kLocated>(locs, row, live);
         for (uint32_t i = 0; i < n_items; ++i) {
-            const bool pass = live && near_passes(s_items[i], a, l);
+            const bool pass = live && item_passes(s_items[i], a, l);
             const uint32_t b = __ballot_sync(0xFFFFFFFFu, pass);
             if (!b) continue;
             uint32_t at = 0;
