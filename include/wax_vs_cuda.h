@@ -478,11 +478,43 @@ int32_t wax_vs_merge_candidates_device(wax_vs_engine *engine, const wax_vs_candi
                                        uint32_t n_queries, uint32_t k, uint32_t k_out, wax_vs_candidate *d_out,
                                        void *cuda_stream);
 /* wax_vs_search_filtered over the whole sharded corpus: every rank passes the SAME frame_ids / mode; a rank resolves
-   the ids its own shard holds (the rest are unknown to it and ignored), its fused scan applies the row filter below
-   the top-k and the in-kernel exchange merges the ranks' lists.  Still one launch per query per rank. */
+   the ids its own shard holds (the rest are unknown to it and ignored), plans its shard as wax_vs_search_filtered
+   does (a short allow-list is gathered, anything else is a row filter in the fused scan) and the exchange merges the
+   ranks' lists.  Exactly one exchange per query per rank.  The no-clause case of wax_vs_shard_search_where. */
 int32_t wax_vs_shard_search_filtered(wax_vs_engine *engine, const float *query, uint32_t query_len, int64_t top_k,
                                      const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids,
                                      float *out_scores, uint32_t out_cap, uint32_t *out_n);
+/* Collective, fused transport, top_k <= WAX_VS_SHARD_MAX_K: one query under one where (time, tag and location clauses
+   of `where`, plus terms[0 .. n_terms) required, 0..32 ids) AND the id filter (frame_ids, n_ids, mode as
+   wax_vs_shard_search_filtered; n_ids == 0 with mode 1 = none).  Every rank passes the same arguments.  The answer is
+   the same on every rank and identical (ids, order, score bits) to wax_vs_search_batch_where_terms for that query on
+   one engine holding the whole corpus.  NULL where, out_n, frame_ids (n_ids > 0) or terms (n_terms > 0) ->
+   WAX_VS_ERR_NULL; a mode other than 0 / 1, more than 32 terms or a non-finite box -> WAX_VS_ERR_ARGUMENT; these checks
+   run before the engine is locked, so every rank fails alike before any rank joins the exchange.  top_k above
+   WAX_VS_SHARD_MAX_K -> WAX_VS_ERR_UNSUPPORTED.
+   How: each rank plans its shard as the where entry points do.  A unit of at most 16 384 rows is gathered, scored and
+   sorted, then exchanged by a one-CTA launch; a wider one is a row bitset in the fused scan, whose last CTA exchanges;
+   a shard where nothing passes exchanges padding.  A collective call never frees device memory or waits for the whole
+   device (a peer's exchange may be waiting for this rank on the same GPU): the rank's scratch is sized for its whole
+   shard, and superseded mirrors are released by the mutators, under the write lock. */
+int32_t wax_vs_shard_search_where(wax_vs_engine *engine, const float *query, uint32_t query_len, int64_t top_k,
+                                  const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                                  const wax_vs_where_near *where, const uint64_t *terms, uint32_t n_terms,
+                                  uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n);
+/* The rank-local half of a batched sharded where search, for any transport and any k up to 10 000.  Arguments are those
+   of wax_vs_search_batch_where_terms; where_term_offsets may be NULL when no where has a term.  d_queries is a device
+   pointer, as in wax_vs_search_batch_device.  Output: d_candidates [n_queries][clamp(top_k)] on the device.  Each list is
+   sorted by (distance, row_offset + local row), and padding has valid = 0 and comes last.  This is exactly the layout
+   that wax_vs_merge_candidates_device takes after an all-gather.  A query with no allowed row on this shard, and every
+   query of an empty shard, is all padding.  The argument checks of wax_vs_search_batch_where_terms, and NULL d_queries
+   or d_candidates -> WAX_VS_ERR_NULL, run before the empty-engine early return.  The call may synchronise cuda_stream,
+   as wax_vs_search_batch_device does. */
+int32_t wax_vs_search_batch_where_device(wax_vs_engine *engine, const float *d_queries, uint32_t n_queries, int64_t top_k,
+                                         const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                         const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                         const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                         const uint64_t *where_term_offsets, const uint64_t *where_terms,
+                                         uint64_t row_offset, wax_vs_candidate *d_candidates, void *cuda_stream);
 /* Device-resident form: d_query (dims floats) and d_candidates (clamp(top_k) merged entries, padding valid = 0) are
    device pointers; enqueued on `cuda_stream`, returns without synchronising. */
 int32_t wax_vs_shard_search_device(wax_vs_engine *engine, const float *d_query, int64_t top_k,

@@ -17,6 +17,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <map>
 #include <mutex>
 #include <new>
 #include <shared_mutex>
@@ -241,6 +242,7 @@ struct SearchCtx {
     DevBuf<uint32_t> d_retry_filter;               // filter level: bitset indices of the compacted queries
     DevBuf<uint2> d_gather_span;                   // filtered search: each gathered query's span of d_filter_rows
     DevBuf<uint64_t> d_gather_keys;                // filtered search: keys of the listed rows
+    DevBuf<uint32_t> d_order;                      // device-form where search: staged order, then each staged query's k
     DevBuf<wax_vs_candidate> d_shard_local;        // sharded search: this rank's list before the exchange [kShardKCap]
     DevBuf<unsigned long long> d_group_best;       // grouped search: each group's best (key, row)
     DevBuf<uint32_t> d_group_keys;                 // grouped search: row-indexed keys of the groups' best rows
@@ -399,12 +401,29 @@ struct wax_vs_engine {
     uint64_t term_garbage = 0;
     // Device inverted index for the term clauses (waxvs_terms.cuh), a cache like the group index: every mutator and
     // set_terms invalidate it; the first where_terms search after that rebuilds it under term_mu.
+    // Invalidation releases it (under the write lock), so a build only allocates: a build inside a sharded where search
+    // must not free device memory (reserve_shard_scratch).  For the same reason a shard rank keeps the build's scratch
+    // until then; other engines release it at the end of the build.
     struct TermIndex {
         DevBuf<uint64_t> keys, start;
         DevBuf<uint32_t> postings;
+        DevBuf<uint64_t> sort_keys, sorted_keys;   // build scratch
+        DevBuf<uint32_t> sort_rows, heads, numbering;
+        DevBuf<uint8_t> temp;
         uint32_t n_terms = 0;
         uint64_t n_postings = 0;
         bool valid = false;
+        void release_scratch() {
+            sort_keys.release(); sorted_keys.release(); sort_rows.release(); heads.release(); numbering.release();
+            temp.release();
+        }
+        void release() {
+            keys.release(); start.release(); postings.release();
+            release_scratch();
+            n_terms = 0;
+            n_postings = 0;
+            valid = false;
+        }
     } tindex;
     std::mutex term_mu;
     uint64_t term_index_builds = 0;    // instrumentation (pool_mu)
@@ -440,8 +459,6 @@ struct wax_vs_engine {
     } ing;
     uint64_t ingest_h2d_bytes = 0, ingest_d2h_bytes = 0;         // instrumentation
     std::mutex ingest_mu;                                        // readers that use the staging (serialize)
-    std::mutex attr_mu;            // cudaFuncSetAttribute bookkeeping (per engine = per device)
-    std::unordered_map<const void *, int> smem_granted;   // opt-in shared memory already granted, per kernel (attr_mu)
     // Device-path searches (wax_vs_search_device & co.) return while their kernels are still in flight on the
     // caller's stream.  Mutators must not touch the corpus under them: every mutator drains the device first when
     // this flag says something was enqueued since the last drain.
@@ -482,7 +499,17 @@ static void invalidate_row_caches(wax_vs_engine *e, uint64_t keep_prefix) {
     e->gindex.valid = false;           // appends too: the new rows need index entries
     e->attrs_dev_valid = false;        // likewise the attribute mirror
     e->locs_dev_valid = false;         // and the location mirror
-    e->tindex.valid = false;           // and the term index
+    e->tindex.release();               // and the term index
+    // The row-sized device buffers of the where mirrors and of the collective scratch go too, here under the write lock
+    // with the device drained: a sharded where search then only allocates them for the new row count, and never frees
+    // (reserve_shard_scratch).
+    e->d_attrs.release();
+    e->d_locs.release();
+    if (SearchCtx *c = e->shard.ctx) {
+        c->d_filter_rows.release();
+        c->d_mask.release();
+        c->d_term_deny.release();
+    }
 }
 
 // The term pool rewritten in row order once more than half of it is garbage (set_terms, remove_batch).
@@ -504,11 +531,7 @@ static void clear_terms(wax_vs_engine *e) {
     e->term_refs.clear(); e->term_refs.shrink_to_fit();
     e->term_pool.clear(); e->term_pool.shrink_to_fit();
     e->term_garbage = 0;
-    auto &ti = e->tindex;              // the index goes with them (invalidate_row_caches would only mark it stale)
-    ti.keys.release(); ti.start.release(); ti.postings.release();
-    ti.n_terms = 0;
-    ti.n_postings = 0;
-    ti.valid = false;
+    e->tindex.release();               // the index goes with them
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -663,10 +686,15 @@ static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0
 
 // The opt-in shared-memory limit is per function and per device: set it once per engine (= per device), and again
 // only if a larger ring is requested, instead of on every launch -- it costs more host time than a 10 K-row scan.
+// The opt-in dynamic shared memory of `kernel` on e's device, raised to at least `bytes`.  The attribute belongs to the
+// function on the device, not to an engine, so the grants are kept per (device, kernel) for the whole process: engines
+// that share a device (the ranks of a shard group in one process) only ever raise it, never lower it under another.
 template <typename K>
 static cudaError_t grant_smem(wax_vs_engine *e, K kernel, size_t bytes) {
-    std::lock_guard<std::mutex> g(e->attr_mu);
-    int &have = e->smem_granted[reinterpret_cast<const void *>(kernel)];
+    static std::mutex mu;
+    static std::map<std::pair<int, const void *>, int> granted;
+    std::lock_guard<std::mutex> g(mu);
+    int &have = granted[{e->device, reinterpret_cast<const void *>(kernel)}];
     if (have >= static_cast<int>(bytes)) return cudaSuccess;
     cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes));
     if (err == cudaSuccess) have = static_cast<int>(bytes);
@@ -1076,6 +1104,15 @@ static int32_t place_host_query(wax_vs_engine *e, SearchCtx *c, ScanParams &p, c
     return WAX_VS_OK;
 }
 
+// The stand-alone exchange of this rank's `local` list of k candidates (sorted, padding last), merged into sp.final_out.
+static int32_t enqueue_exchange(const ShardParams &sp, const wax_vs_candidate *local, uint32_t k, cudaStream_t stream,
+                                uint64_t *launches) {
+    shard_exchange_kernel<<<1, 256, 0, stream>>>(sp, local, k);
+    CUDA_TRY(cudaGetLastError());
+    ++*launches;
+    return WAX_VS_OK;
+}
+
 // `shard` (optional): the row-sharded form -- d_out receives the result MERGED over all ranks; the exchange runs inside
 // the scan launch when the kernel's shared-memory lists can hold the merge keys, else as one extra 1-CTA launch.
 // keys_only: run the emitting scan alone -- c->d_dist_keys receives every row's distance key (the masked rows'
@@ -1099,10 +1136,7 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
     auto exchange_standalone = [&]() -> int32_t {
         ShardParams sp = *shard;
         sp.final_out = d_merged;
-        shard_exchange_kernel<<<1, 256, 0, stream>>>(sp, d_out, k_eff);
-        CUDA_TRY(cudaGetLastError());
-        ++*launches;
-        return WAX_VS_OK;
+        return enqueue_exchange(sp, d_out, k_eff, stream, launches);
     };
     if (e->n_rows == 0) {
         CUDA_TRY(cudaMemsetAsync(d_out, 0, static_cast<size_t>(k_eff) * sizeof(wax_vs_candidate), stream));
@@ -2824,65 +2858,15 @@ static int32_t shard_wait_host(wax_vs_engine *e, unsigned long long seq) {
     return rc;
 }
 
-// The host-path collective search of both entry points, under the read lock it takes (caller: e and out_n checked, and
-// the filtered form's mode and ids): the rank's fused scan, with the row filter of `frame_ids` (filtered: mode 0 allow /
-// 1 deny) below the top-k, the in-kernel exchange and merge, and the merged list delivered into mapped host memory.
+struct Clause;
 static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k, bool filtered,
-                                 const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids, float *out_scores,
-                                 uint32_t out_cap, uint32_t *out_n) {
-    std::shared_lock<std::shared_mutex> r(e->rw);
-    *out_n = 0;
-    if (!e->shard.connected) return fail(WAX_VS_ERR_ARGUMENT, "the shard group is not connected (wax_vs_shard_open / _connect)");
-    int32_t rc;
-    if ((rc = check_query(e, query, query_len))) return rc;
-    const uint32_t k_eff = clamp_topk(top_k);
-    if (k_eff > static_cast<uint32_t>(kShardKCap))
-        return fail(WAX_VS_ERR_UNSUPPORTED, "sharded search supports top_k <= %d (got %u)", kShardKCap, k_eff);
-    if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
-    DeviceGuard g(e->device);
-    if (!g.ok) return g.error();
-    const bool masked = filtered && e->n_rows;
-    const uint64_t offsets[2] = {0, n_ids};
-    FilterSet fs;
-    if (masked) resolve_filters(e, frame_ids, offsets, 1, nullptr, 0, fs);
-    auto &sh = e->shard;
-    std::lock_guard<std::mutex> sg(sh.mu);      // one host-path collective at a time: it owns sh.ctx and h_final
-    SearchCtx *c = sh.ctx;
-    const uint64_t *d_ids = nullptr;
-    if ((rc = sync_device_ids(e, &d_ids))) return rc;
-    uint64_t launches = 0;
-    if (masked) {       // one bitset, built on the device from the resolved rows
-        // sized for every row of the shard (a bound on any filter's distinct rows), so that a later call never
-        // reallocates: cudaFree waits for the device, where the peers' scans may already wait for this rank
-        if ((rc = stage_filter_rows(e, c, fs.rows, e->n_rows, mode, c->stream, &launches))) return rc;
-    }
-    ShardParams sp = shard_params_next(e);
-    sp.host_out = sh.h_final; sp.host_flag = sh.h_flag;      // mapped pinned: the kernel delivers the result itself
-    HostDelivery hd{query, nullptr, nullptr, 0};             // the query rides in the kernel parameters when it fits
-    if ((rc = enqueue_search(e, c, nullptr, k_eff, sh.row_offset, sh.d_final, d_ids, c->stream, &launches,
-                             masked ? c->d_mask.p : nullptr, &sp, &hd))) {
-        cudaStreamSynchronize(c->stream);
-        return rc;
-    }
-    if ((rc = shard_wait_host(e, sp.seq))) { cudaStreamSynchronize(c->stream); return rc; }
-    if (masked) CUDA_TRY(cudaStreamSynchronize(c->stream));   // fs.rows must outlive its upload
-    uint32_t m = 0;
-    for (uint32_t i = 0; i < k_eff; ++i) {
-        const wax_vs_candidate &cd = sh.h_final[i];
-        if (cd.valid != 1u) continue;
-        if (m >= out_cap) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need more", out_cap);
-        out_ids[m] = cd.frame_id;
-        out_scores[m] = score_from_distance(e->similarity, cd.distance);
-        ++m;
-    }
-    *out_n = m;
-    return WAX_VS_OK;
-}
+                                 const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, const Clause *where,
+                                 uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n);
 
 int32_t wax_vs_shard_search(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k, uint64_t *out_ids,
                             float *out_scores, uint32_t out_cap, uint32_t *out_n) {
     if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    return shard_search_host(e, query, query_len, top_k, false, nullptr, 0, 0, out_ids, out_scores, out_cap, out_n);
+    return shard_search_host(e, query, query_len, top_k, false, nullptr, 0, 0, nullptr, out_ids, out_scores, out_cap, out_n);
 }
 
 // Device-timed sharded searches, strictly one query at a time on one stream (the same mode as wax_vs_debug_time_search):
@@ -3000,9 +2984,9 @@ static int32_t ensure_term_index(wax_vs_engine *e, SearchCtx *c) {
                 h_rows[at] = static_cast<uint32_t>(r);
             }
         }
-        DevBuf<uint64_t> keys_in, keys_out;
-        DevBuf<uint32_t> rows_in, heads, incl;
-        DevBuf<uint8_t> temp;
+        auto &keys_in = ti.sort_keys, &keys_out = ti.sorted_keys;
+        auto &rows_in = ti.sort_rows, &heads = ti.heads, &incl = ti.numbering;
+        auto &temp = ti.temp;
         size_t sort_bytes = 0, scan_bytes = 0;
         CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, keys_in.p, keys_out.p, rows_in.p, ti.postings.p,
                                                  static_cast<int>(P), 0, 64, s));
@@ -3027,6 +3011,7 @@ static int32_t ensure_term_index(wax_vs_engine *e, SearchCtx *c) {
         term_index_finish_kernel<<<grid, 256, 0, s>>>(keys_out, incl, P, ti.keys, ti.start);
         CUDA_TRY(cudaGetLastError());
         CUDA_TRY(cudaStreamSynchronize(s));     // before the scratch goes
+        if (!e->shard.open) ti.release_scratch();
     } else if ((rc = ti.keys.ensure(1, "term keys")) || (rc = ti.start.ensure(1, "term starts"))) {
         return rc;
     }
@@ -3241,10 +3226,23 @@ static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const int32_t *fi
     return WAX_VS_OK;
 }
 
-// The planned queries on c->stream: staged query j's candidates land at c->d_out[j * k_max], on the device.  Stages the
-// queries (c->d_queries, staged order) and the filters' rows (c->d_filter_rows).  plan.k_max > 0.
+// What run_filtered's candidates carry and where they go.  The defaults serve the host entry points, which map local rows
+// to frame ids themselves.  A shard reports global rows (row_offset + local row) and its frame ids (d_ids, nullptr for
+// identity ids); the device form's queries are on the device; the collective form (one query) exchanges its list with
+// the other ranks, merged into shard->final_out.
+struct FilteredTarget {
+    uint64_t row_offset = 0;
+    const uint64_t *d_ids = nullptr;
+    bool device_queries = false;
+    const ShardParams *shard = nullptr;
+};
+
+// The planned queries on c->stream: staged query j's candidates land at c->d_out[j * k_max], on the device (with
+// tgt.shard: this rank's list there, the merged one at tgt.shard->final_out).  Stages the queries (c->d_queries, staged
+// order; for device queries the order goes to c->d_order) and the filters' rows (c->d_filter_rows).  plan.k_max > 0.
 static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries, const int32_t *filter_modes,
-                            uint32_t n_filters, const uint32_t *query_filter, const FilterSet &fs, const FilteredPlan &plan) {
+                            uint32_t n_filters, const uint32_t *query_filter, const FilterSet &fs, const FilteredPlan &plan,
+                            const FilteredTarget &tgt = FilteredTarget{}) {
     const std::vector<uint32_t> &order = plan.order, &k_of = plan.k_of, &rows = fs.rows;
     const std::vector<uint64_t> &first = fs.first, &count = fs.count;
     const uint32_t k_max = plan.k_max, n_tensor = plan.n_tensor, n_gather = plan.n_gather;
@@ -3252,9 +3250,20 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
     const uint32_t words = static_cast<uint32_t>((e->n_rows + 31) / 32);
     int32_t rc;
     const size_t ncand = static_cast<size_t>(n_staged) * k_max;       // staged query j's candidates at j * k_max
-    if ((rc = stage_queries(e, c, queries, n_staged, c->stream, order.data()))) return rc;
+    if (tgt.device_queries) {
+        const size_t qfloats = static_cast<size_t>(n_staged) * e->dims;
+        if ((rc = c->d_queries.ensure(qfloats, "query buffer")) || (rc = c->d_order.ensure(2u * n_staged, "query order")))
+            return rc;
+        CUDA_TRY(cudaMemcpyAsync(c->d_order, order.data(), n_staged * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+        CUDA_TRY(cudaMemcpyAsync(c->d_order + n_staged, k_of.data(), n_staged * sizeof(uint32_t), cudaMemcpyHostToDevice,
+                                 c->stream));
+        const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (qfloats + 255) / 256)));
+        stage_query_rows_kernel<<<grid, 256, 0, c->stream>>>(queries, c->d_order, n_staged, e->dims, c->d_queries);
+        CUDA_TRY(cudaGetLastError());
+    } else if ((rc = stage_queries(e, c, queries, n_staged, c->stream, order.data()))) {
+        return rc;
+    }
     if ((rc = c->d_out.ensure(ncand, "result buffer"))) return rc;
-    if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
     if ((rc = stage_filter_rows(e, c, rows, rows.size() + fs.device_rows, -1, c->stream, nullptr))) return rc;
     uint64_t launches = 0;
     if ((rc = list_where_rows(e, c, fs.compact, c->stream, &launches)) ||
@@ -3293,10 +3302,12 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
             CUDA_TRY(cudaGetLastError());
             ScanParams sp{};
             sp.k = k_max; sp.out = c->d_out + static_cast<size_t>(n_tensor + q0) * k_max; sp.id_base = e->id_base;
+            sp.frame_ids = tgt.d_ids; sp.row_offset = tgt.row_offset;
             gather_sort_kernel<<<nq, 1024, pow2 * sizeof(uint64_t), c->stream>>>(keys, span, longest, pow2, sp);
             CUDA_TRY(cudaGetLastError());
             launches += 2;
         }
+        if (tgt.shard && (rc = enqueue_exchange(*tgt.shard, c->d_out, k_max, c->stream, &launches))) return rc;
     }
 
     // tensor and scan classes: sub-batches whose bitsets fit the budget (at least one always does)
@@ -3332,12 +3343,13 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
                 CUDA_TRY(cudaMemcpyAsync(c->d_query_filter + s0, index.data() + s0, nq * sizeof(uint32_t), cudaMemcpyHostToDevice,
                                          c->stream));
                 rf.d_index = c->d_query_filter + s0;
-                if ((prc = run_queries_on_device(e, c, dq, nq, k_max, 0, dout, nullptr, &launches, rf))) return prc;
+                if ((prc = run_queries_on_device(e, c, dq, nq, k_max, tgt.row_offset, dout, tgt.d_ids, &launches, rf)))
+                    return prc;
             } else {                // single queries (search_filtered) and the scan class: the single-query path
                 for (uint32_t j = 0; j < nq; ++j) {
-                    prc = enqueue_search(e, c, dq + static_cast<size_t>(j) * e->dims, k_of[s0 + j], 0,
-                                         dout + static_cast<size_t>(j) * k_max, nullptr, c->stream, &launches, rf.mask(j),
-                                         nullptr, nullptr, false, true);
+                    prc = enqueue_search(e, c, dq + static_cast<size_t>(j) * e->dims, k_of[s0 + j], tgt.row_offset,
+                                         tgt.shard ? tgt.shard->final_out : dout + static_cast<size_t>(j) * k_max, tgt.d_ids,
+                                         c->stream, &launches, rf.mask(j), tgt.shard, nullptr, false, true);
                     if (prc) { cudaStreamSynchronize(c->stream); return prc; }
                 }
             }
@@ -3381,8 +3393,9 @@ static int32_t deliver_filtered(wax_vs_engine *e, SearchCtx *c, const float *que
                                 const FilteredPlan &plan, uint64_t *out_ids, float *out_scores, uint32_t out_stride,
                                 uint32_t *out_n) {
     int32_t rc;
-    if ((rc = run_filtered(e, c, queries, filter_modes, n_filters, query_filter, fs, plan))) return rc;
     const size_t ncand = static_cast<size_t>(plan.order.size()) * plan.k_max;
+    if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
+    if ((rc = run_filtered(e, c, queries, filter_modes, n_filters, query_filter, fs, plan))) return rc;
     CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, ncand * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));   // also keeps the host arrays alive until their copies are done
     deliver_results(e, c->h_out, static_cast<uint32_t>(plan.order.size()), plan.k_max, out_ids, out_scores, out_stride,
@@ -3928,8 +3941,39 @@ int32_t wax_vs_set_terms(wax_vs_engine *e, const uint64_t *frame_ids, const uint
         if (!(written[wd] & b)) { written[wd] |= b; ++assigned; }
     }
     compact_term_pool(e);
-    e->tindex.valid = false;
+    e->tindex.release();
     if (out_assigned) *out_assigned = assigned;
+    return WAX_VS_OK;
+}
+
+// The clauses of wheres[0, n_wheres) with their term lists (offsets checked by the caller), and qw[i] = the where query
+// i names.  Wheres with terms and equal contents (clauses, box, required ids) are one: each query names the first of
+// them, so a batch that scopes 1 024 queries to 16 sessions plans 16 units, not 1 024.
+static int32_t term_clauses(const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                            uint32_t n_queries, const uint64_t *where_term_offsets, const uint64_t *where_terms,
+                            std::vector<Clause> &clauses, std::vector<uint32_t> &qw) {
+    int32_t rc;
+    if ((rc = check_term_offsets(where_term_offsets, n_wheres, where_terms, kMaxWhereTerms, "where_term_offsets"))) return rc;
+    if ((rc = near_clauses(wheres, n_wheres, clauses))) return rc;
+    for (uint32_t w = 0; w < n_wheres; ++w) {
+        std::vector<uint64_t> &terms = clauses[w].terms;
+        terms.assign(where_terms + where_term_offsets[w], where_terms + where_term_offsets[w + 1]);
+        std::sort(terms.begin(), terms.end());
+        terms.erase(std::unique(terms.begin(), terms.end()), terms.end());
+    }
+    std::vector<uint32_t> canon(n_wheres);
+    std::unordered_map<std::string, uint32_t> first_of;
+    for (uint32_t w = 0; w < n_wheres; ++w) {
+        const Clause &cl = clauses[w];
+        canon[w] = w;
+        if (cl.terms.empty()) continue;
+        std::string key(reinterpret_cast<const char *>(&cl.pred), sizeof(WherePred));
+        key.append(reinterpret_cast<const char *>(&cl.box), sizeof(LocBox));
+        key.append(reinterpret_cast<const char *>(cl.terms.data()), cl.terms.size() * sizeof(uint64_t));
+        canon[w] = first_of.emplace(std::move(key), w).first->second;
+    }
+    qw.resize(n_queries);
+    for (uint32_t i = 0; i < n_queries; ++i) qw[i] = query_where[i] == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : canon[query_where[i]];
     return WAX_VS_OK;
 }
 
@@ -3944,32 +3988,185 @@ int32_t wax_vs_search_batch_where_terms(wax_vs_engine *e, const float *queries, 
                                n_wheres, query_where, out_n)))
         return rc;
     if (!where_term_offsets) return fail(WAX_VS_ERR_NULL, "where_term_offsets is NULL");
-    if ((rc = check_term_offsets(where_term_offsets, n_wheres, where_terms, kMaxWhereTerms, "where_term_offsets"))) return rc;
     std::vector<Clause> clauses;
-    if ((rc = near_clauses(wheres, n_wheres, clauses))) return rc;
-    for (uint32_t w = 0; w < n_wheres; ++w) {
-        std::vector<uint64_t> &terms = clauses[w].terms;
-        terms.assign(where_terms + where_term_offsets[w], where_terms + where_term_offsets[w + 1]);
-        std::sort(terms.begin(), terms.end());
-        terms.erase(std::unique(terms.begin(), terms.end()), terms.end());
-    }
-    // Wheres with terms and equal contents (clauses, box, required ids) are one: each query names the first of them, so
-    // a batch that scopes 1 024 queries to 16 sessions plans 16 units, not 1 024.
-    std::vector<uint32_t> canon(n_wheres);
-    std::unordered_map<std::string, uint32_t> first_of;
-    for (uint32_t w = 0; w < n_wheres; ++w) {
-        const Clause &cl = clauses[w];
-        canon[w] = w;
-        if (cl.terms.empty()) continue;
-        std::string key(reinterpret_cast<const char *>(&cl.pred), sizeof(WherePred));
-        key.append(reinterpret_cast<const char *>(&cl.box), sizeof(LocBox));
-        key.append(reinterpret_cast<const char *>(cl.terms.data()), cl.terms.size() * sizeof(uint64_t));
-        canon[w] = first_of.emplace(std::move(key), w).first->second;
-    }
-    std::vector<uint32_t> qw(n_queries);
-    for (uint32_t i = 0; i < n_queries; ++i) qw[i] = query_where[i] == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : canon[query_where[i]];
+    std::vector<uint32_t> qw;
+    if ((rc = term_clauses(wheres, n_wheres, query_where, n_queries, where_term_offsets, where_terms, clauses, qw)))
+        return rc;
     return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
                              query_filter, clauses, qw.data(), out_ids, out_scores, out_stride, out_n);
+}
+
+// ---- sharded where search -----------------------------------------------------------------------------------------
+// The scratch of a collective where search on c, sized before the call plans anything for the bounds of one query on
+// this shard: one unit of at most n_rows listed rows, at most kWhereGatherRows gathered, kMaxWhereTerms required ids.
+// A buffer that grew during the call would free its old memory, and cudaFree waits for the whole device, where a peer's
+// exchange may already be waiting for this rank (ranks that share a GPU).  Mutators release the row-sized ones under the
+// write lock (invalidate_row_caches), so this only ever allocates.
+static int32_t reserve_shard_scratch(wax_vs_engine *e, SearchCtx *c) {
+    const size_t rows = std::max<size_t>(e->n_rows, 1), words = (rows + 31) / 32;
+    int32_t rc;
+    if ((rc = c->d_queries.ensure(e->dims, "query buffer")) || (rc = c->h_queries.ensure(e->dims, "query staging")) ||
+        (rc = c->d_out.ensure(kShardKCap, "result buffer")) || (rc = c->d_shard_local.ensure(kShardKCap, "shard candidates")) ||
+        (rc = c->d_filter_rows.ensure(rows, "filter rows")) || (rc = c->d_mask.ensure(words, "row filters")) ||
+        (rc = c->d_filter_spec.ensure(4, "filter spec")) || (rc = c->d_query_filter.ensure(1, "query filters")) ||
+        (rc = c->d_gather_span.ensure(1, "gather spans")) || (rc = c->d_gather_keys.ensure(kWhereGatherRows, "gather keys")) ||
+        (rc = c->d_where_items.ensure(1, "where predicates")) || (rc = c->d_where_counts.ensure(1, "where counts")) ||
+        (rc = c->d_term_ids.ensure(kMaxWhereTerms, "required terms")) ||
+        (rc = c->d_term_spans.ensure(kMaxWhereTerms, "term spans")) || (rc = c->d_term_units.ensure(1, "term units")) ||
+        (rc = c->d_term_counts.ensure(1, "term counts")) || (rc = c->d_term_deny.ensure(rows, "term deny-lists")))
+        return rc;
+    return WAX_VS_OK;
+}
+
+// The host-path collective search of the shard entry points, under the read lock it takes (caller: e and out_n checked,
+// and the filtered form's mode and ids, the where's clauses).  Without a filter or a where: the rank's fused scan, the
+// in-kernel exchange and merge, the merged list delivered into mapped host memory.  Otherwise the rank plans its shard
+// for the one query as the where entry points do (filtered: the id filter; `where`: its clauses) and runs the plan with
+// exactly one exchange: a gathered unit is exchanged by the stand-alone kernel, a row bitset rides in the fused scan, and
+// a shard where nothing passes exchanges padding.
+static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k, bool filtered,
+                                 const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, const Clause *where,
+                                 uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n) {
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    *out_n = 0;
+    if (!e->shard.connected) return fail(WAX_VS_ERR_ARGUMENT, "the shard group is not connected (wax_vs_shard_open / _connect)");
+    int32_t rc;
+    if ((rc = check_query(e, query, query_len))) return rc;
+    const uint32_t k_eff = clamp_topk(top_k);
+    if (k_eff > static_cast<uint32_t>(kShardKCap))
+        return fail(WAX_VS_ERR_UNSUPPORTED, "sharded search supports top_k <= %d (got %u)", kShardKCap, k_eff);
+    if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    auto &sh = e->shard;
+    std::lock_guard<std::mutex> sg(sh.mu);      // one host-path collective at a time: it owns sh.ctx and h_final
+    SearchCtx *c = sh.ctx;
+    const uint64_t *d_ids = nullptr;
+    if ((rc = sync_device_ids(e, &d_ids))) return rc;
+    uint64_t launches = 0;
+    const bool planned = filtered || where;
+    // the plan of the one query: pair (where 0 or none, id filter 0 or none); a deny-list of nothing is no filter
+    const std::vector<Clause> wheres(where ? 1 : 0, where ? *where : Clause{});
+    const uint32_t qw = where ? 0u : WAX_VS_NO_FILTER, qf = filtered && (mode == 0 || n_ids) ? 0u : WAX_VS_NO_FILTER;
+    const uint64_t offsets[2] = {0, n_ids};
+    FilterSet ids, fs;
+    std::vector<int32_t> modes;
+    std::vector<uint32_t> pair_of;
+    FilteredPlan plan;
+    if (planned && e->n_rows) {
+        resolve_filters(e, frame_ids, offsets, 1, &qf, 1, ids);
+        if ((rc = reserve_shard_scratch(e, c)) ||
+            (rc = plan_where_pairs(e, c, wheres, &qw, &mode, &qf, 1, ids, fs, modes, pair_of)))
+            return rc;
+        plan_filtered(e, k_eff, modes.data(), pair_of.data(), 1, fs, plan);
+    }
+    ShardParams sp = shard_params_next(e);
+    sp.host_out = sh.h_final; sp.host_flag = sh.h_flag;      // mapped pinned: the kernel delivers the result itself
+    if (!planned) {
+        HostDelivery hd{query, nullptr, nullptr, 0};             // the query rides in the kernel parameters when it fits
+        rc = enqueue_search(e, c, nullptr, k_eff, sh.row_offset, sh.d_final, d_ids, c->stream, &launches, nullptr, &sp, &hd);
+    } else if (plan.order.empty()) {                              // an empty shard, or nothing on it passes: padding
+        sp.final_out = sh.d_final;
+        if ((rc = c->d_shard_local.ensure(kShardKCap, "shard candidates"))) return rc;
+        CUDA_TRY(cudaMemsetAsync(c->d_shard_local, 0, k_eff * sizeof(wax_vs_candidate), c->stream));
+        rc = enqueue_exchange(sp, c->d_shard_local, k_eff, c->stream, &launches);
+    } else {                    // every rank exchanges k_eff entries, its list padded past its allowed rows
+        sp.final_out = sh.d_final;
+        plan.k_max = plan.k_of[0] = k_eff;
+        FilteredTarget tgt;
+        tgt.row_offset = sh.row_offset; tgt.d_ids = d_ids; tgt.shard = &sp;
+        rc = run_filtered(e, c, query, modes.data(), static_cast<uint32_t>(modes.size()), pair_of.data(), fs, plan, tgt);
+    }
+    if (rc) { cudaStreamSynchronize(c->stream); return rc; }
+    if ((rc = shard_wait_host(e, sp.seq))) { cudaStreamSynchronize(c->stream); return rc; }
+    if (planned) CUDA_TRY(cudaStreamSynchronize(c->stream));   // the host arrays must outlive their uploads
+    uint32_t m = 0;
+    for (uint32_t i = 0; i < k_eff; ++i) {
+        const wax_vs_candidate &cd = sh.h_final[i];
+        if (cd.valid != 1u) continue;
+        if (m >= out_cap) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need more", out_cap);
+        out_ids[m] = cd.frame_id;
+        out_scores[m] = score_from_distance(e->similarity, cd.distance);
+        ++m;
+    }
+    *out_n = m;
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_shard_search_where(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k,
+                                  const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, const wax_vs_where_near *where,
+                                  const uint64_t *terms, uint32_t n_terms, uint64_t *out_ids, float *out_scores,
+                                  uint32_t out_cap, uint32_t *out_n) {
+    if (!e || !out_n || !where) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
+    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    const uint64_t term_offsets[2] = {0, n_terms};
+    std::vector<Clause> clauses;
+    std::vector<uint32_t> qw;
+    const uint32_t q0 = 0;
+    int32_t rc;
+    if ((rc = term_clauses(where, 1, &q0, 1, term_offsets, terms, clauses, qw))) return rc;
+    return shard_search_host(e, query, query_len, top_k, true, frame_ids, n_ids, mode, &clauses[0], out_ids, out_scores,
+                             out_cap, out_n);
+}
+
+// The rank-local half of a batched sharded where search: the plan of wax_vs_search_batch_where_terms on this shard, run
+// on the caller's stream with global rows and frame ids, then each planned query's list scattered to its place in
+// d_candidates (every other slot is padding).
+int32_t wax_vs_search_batch_where_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries, int64_t top_k,
+                                         const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                         const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                         const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                         const uint64_t *where_term_offsets, const uint64_t *where_terms,
+                                         uint64_t row_offset, wax_vs_candidate *d_candidates, void *cuda_stream) {
+    int32_t rc;
+    uint32_t no_out_n = 0;                  // the checks of the host forms, which also test their out_n
+    if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
+                               n_wheres, query_where, &no_out_n)))
+        return rc;
+    if (!d_queries || !d_candidates) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    std::vector<Clause> clauses;
+    std::vector<uint32_t> qw;
+    if (where_term_offsets) {
+        rc = term_clauses(wheres, n_wheres, query_where, n_queries, where_term_offsets, where_terms, clauses, qw);
+    } else {
+        rc = near_clauses(wheres, n_wheres, clauses);
+        qw.assign(query_where, query_where + n_queries);
+    }
+    if (rc) return rc;
+    if (n_queries == 0) return WAX_VS_OK;
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    SearchCtx *c = nullptr;
+    if ((rc = ctx_for_stream(e, cuda_stream, &c))) return rc;
+    const uint32_t k_out = clamp_topk(top_k);
+    e->async_pending.store(true);
+    CUDA_TRY(cudaMemsetAsync(d_candidates, 0, static_cast<size_t>(n_queries) * k_out * sizeof(wax_vs_candidate), c->stream));
+    if (e->n_rows == 0) return WAX_VS_OK;
+    const uint64_t *d_ids = nullptr;
+    if ((rc = sync_device_ids(e, &d_ids))) return rc;
+    FilterSet ids, fs;
+    resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, ids);
+    std::vector<int32_t> modes;
+    std::vector<uint32_t> pair_of;
+    if ((rc = plan_where_pairs(e, c, clauses, qw.data(), filter_modes, query_filter, n_queries, ids, fs, modes, pair_of)))
+        return rc;
+    FilteredPlan plan;
+    plan_filtered(e, top_k, modes.data(), pair_of.data(), n_queries, fs, plan);
+    if (plan.k_max == 0) return WAX_VS_OK;
+    FilteredTarget tgt;
+    tgt.row_offset = row_offset; tgt.d_ids = d_ids; tgt.device_queries = true;
+    if ((rc = run_filtered(e, c, d_queries, modes.data(), static_cast<uint32_t>(modes.size()), pair_of.data(), fs, plan, tgt)))
+        return rc;
+    const uint32_t n_staged = static_cast<uint32_t>(plan.order.size());
+    const size_t total = static_cast<size_t>(n_staged) * plan.k_max;
+    const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (total + 255) / 256)));
+    scatter_candidates_kernel<<<grid, 256, 0, c->stream>>>(c->d_out, plan.k_max, c->d_order, c->d_order + n_staged, n_staged,
+                                                           k_out, d_candidates);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(c->stream));     // the host arrays of the plan must outlive their uploads
+    return WAX_VS_OK;
 }
 
 // The row-sharded form: every rank passes the SAME ids; a rank resolves the ones its shard holds (the others are
@@ -3981,7 +4178,8 @@ int32_t wax_vs_shard_search_filtered(wax_vs_engine *e, const float *query, uint3
     if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
     if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
-    return shard_search_host(e, query, query_len, top_k, true, frame_ids, n_ids, mode, out_ids, out_scores, out_cap, out_n);
+    return shard_search_host(e, query, query_len, top_k, true, frame_ids, n_ids, mode, nullptr, out_ids, out_scores, out_cap,
+                             out_n);
 }
 
 // ---- grouped search (waxvs_group.cuh) -----------------------------------------------------------------------------

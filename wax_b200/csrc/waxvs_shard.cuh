@@ -187,4 +187,31 @@ __global__ void __launch_bounds__(128) merge_gathered_kernel(const wax_vs_candid
     }
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// The device form of a batched where search (wax_vs_search_batch_where_device) stages and answers its queries in the
+// plan's order.  order[j] = the caller's query that staged query j is; k_of[j] = the slots of its list that were written.
+__global__ void __launch_bounds__(256) stage_query_rows_kernel(const float *__restrict__ queries,
+                                                               const uint32_t *__restrict__ order, uint32_t n,
+                                                               uint32_t dims, float *__restrict__ staged) {
+    const size_t total = static_cast<size_t>(n) * dims;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const uint32_t j = static_cast<uint32_t>(i / dims), d = static_cast<uint32_t>(i % dims);
+        staged[i] = queries[static_cast<size_t>(order[j]) * dims + d];
+    }
+}
+// Staged query j's first k_of[j] candidates (at staged + j * k_max) -> out[order[j]][0, k_of[j]) of k_out slots each.
+// The caller zeroed `out`, so every other slot is padding (valid = 0).  k_of[j] <= k_max <= k_out.
+__global__ void __launch_bounds__(256) scatter_candidates_kernel(const wax_vs_candidate *__restrict__ staged, uint32_t k_max,
+                                                                 const uint32_t *__restrict__ order,
+                                                                 const uint32_t *__restrict__ k_of, uint32_t n,
+                                                                 uint32_t k_out, wax_vs_candidate *__restrict__ out) {
+    const size_t total = static_cast<size_t>(n) * k_max;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const uint32_t j = static_cast<uint32_t>(i / k_max), s = static_cast<uint32_t>(i % k_max);
+        if (s < k_of[j]) out[static_cast<size_t>(order[j]) * k_out + s] = staged[i];
+    }
+}
+
 }  // namespace waxvs

@@ -211,6 +211,52 @@ def location_bin(latitude: float, longitude: float) -> Optional[Tuple[int, int]]
     return (int(out[0]), int(out[1])) if has.value else None
 
 
+class _WhereArgs:
+    """The id filters and wheres of a batched where search as the C ABI takes them (the pointers stay valid while this
+    object lives): filters[f] = ("allow" | "deny" | 0 | 1, ids), query_filter / query_where = per-query index or None."""
+
+    def __init__(self, wheres, query_where, filters, query_filter, b: int):
+        filters = list(filters or [])
+        if query_filter is None:
+            query_filter = [None] * b
+        if len(query_where) != b or len(query_filter) != b:
+            raise ValueError(f"query_where / query_filter need {b} entries")
+        modes, lists = [], []
+        for mode, fids in filters:
+            modes.append({"allow": 0, "deny": 1}[mode] if isinstance(mode, str) else int(mode))
+            lists.append(np.ascontiguousarray(fids, dtype=np.uint64).reshape(-1))
+        self.offsets = np.zeros(len(lists) + 1, np.uint64)
+        self.offsets[1:] = np.cumsum([x.size for x in lists], dtype=np.uint64) if lists else []
+        self.fids = np.concatenate(lists) if lists else np.zeros(0, np.uint64)
+        self.modes = np.asarray(modes, np.int32)
+        self.qf = np.asarray([L.NO_FILTER if f is None else int(f) for f in query_filter], np.uint32)
+        self.qw = np.asarray([L.NO_FILTER if w is None else int(w) for w in query_where], np.uint32)
+        self.n_wheres = len(wheres)
+        self.with_terms = any(len(w.terms) for w in wheres)     # wax_vs_search_batch_where_terms only when a term is asked
+        self.near = self.with_terms or any(w.near is not None for w in wheres)   # ... _where_near only when a box is
+        self.warr_near = (L.WhereNear * max(len(wheres), 1))(*[w.to_c_near() for w in wheres])
+        self.warr = self.warr_near if self.near else (L.Where * max(len(wheres), 1))(*[w.to_c() for w in wheres])
+        self.toff = np.zeros(len(wheres) + 1, np.uint64)
+        self.toff[1:] = np.cumsum([len(w.terms) for w in wheres], dtype=np.uint64) if wheres else []
+        self.tflat = np.fromiter((int(t) for w in wheres for t in w.terms), dtype=np.uint64, count=int(self.toff[-1]))
+
+    def filter_args(self):
+        """frame_ids, filter_offsets, filter_modes, n_filters, query_filter."""
+        return (self.fids.ctypes.data_as(C.POINTER(C.c_uint64)) if self.fids.size else None,
+                self.offsets.ctypes.data_as(C.POINTER(C.c_uint64)), self.modes.ctypes.data_as(C.POINTER(C.c_int32)),
+                self.modes.size, self.qf.ctypes.data_as(C.POINTER(C.c_uint32)))
+
+    def where_args(self, near: bool = False):
+        """wheres (wax_vs_where_near when the call needs them or `near`, else wax_vs_where), n_wheres, query_where."""
+        return (C.cast(self.warr_near if near else self.warr, C.c_void_p), self.n_wheres,
+                self.qw.ctypes.data_as(C.POINTER(C.c_uint32)))
+
+    def term_args(self):
+        """where_term_offsets, where_terms."""
+        return (self.toff.ctypes.data_as(C.POINTER(C.c_uint64)),
+                self.tflat.ctypes.data_as(C.POINTER(C.c_uint64)) if self.tflat.size else None)
+
+
 def _clamp_topk(top_k: int) -> int:
     """clampTopK (MetalVectorEngine.swift:842-846)."""
     return max(1, min(int(top_k), L.MAX_RESULTS))
@@ -562,48 +608,21 @@ class CUDAVectorEngine:
         equals search_batch_multi_filtered with an allow-list of exactly those frames, score bits included."""
         qs = _as_rows(vectors, self.dimensions) if len(vectors) else np.zeros((0, self.dimensions), np.float32)
         b = qs.shape[0]
-        filters = list(filters or [])
-        if query_filter is None:
-            query_filter = [None] * b
-        if len(query_where) != b or len(query_filter) != b:
-            raise ValueError(f"query_where / query_filter need {b} entries")
+        a = _WhereArgs(wheres, query_where, filters, query_filter, b)
         if b == 0:
             return []
-        modes, lists = [], []
-        for mode, fids in filters:
-            modes.append({"allow": 0, "deny": 1}[mode] if isinstance(mode, str) else int(mode))
-            lists.append(np.ascontiguousarray(fids, dtype=np.uint64).reshape(-1))
-        offsets = np.zeros(len(lists) + 1, np.uint64)
-        offsets[1:] = np.cumsum([x.size for x in lists], dtype=np.uint64) if lists else []
-        fids = np.concatenate(lists) if lists else np.zeros(0, np.uint64)
-        modes_arr = np.asarray(modes, np.int32)
-        qf = np.asarray([L.NO_FILTER if f is None else int(f) for f in query_filter], np.uint32)
-        qw = np.asarray([L.NO_FILTER if w is None else int(w) for w in query_where], np.uint32)
-        with_terms = any(len(w.terms) for w in wheres)       # wax_vs_search_batch_where_terms only when a term is asked
-        near = with_terms or any(w.near is not None for w in wheres)   # ... _where_near only when a box is
-        if near:
-            warr = (L.WhereNear * max(len(wheres), 1))(*[w.to_c_near() for w in wheres])
-        else:
-            warr = (L.Where * max(len(wheres), 1))(*[w.to_c() for w in wheres])
         cap = _clamp_topk(top_k)
         ids = np.zeros((b, cap), np.uint64)
         scores = np.zeros((b, cap), np.float32)
         ns = np.zeros(b, np.uint32)
-        head = (self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_k),
-                fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
-                offsets.ctypes.data_as(C.POINTER(C.c_uint64)), modes_arr.ctypes.data_as(C.POINTER(C.c_int32)), len(lists),
-                qf.ctypes.data_as(C.POINTER(C.c_uint32)), C.cast(warr, C.c_void_p), len(wheres),
-                qw.ctypes.data_as(C.POINTER(C.c_uint32)))
+        head = (self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_k), *a.filter_args(),
+                *a.where_args())
         tail = (ids.ctypes.data_as(C.POINTER(C.c_uint64)), scores.ctypes.data_as(C.POINTER(C.c_float)), cap,
                 ns.ctypes.data_as(C.POINTER(C.c_uint32)))
-        if with_terms:
-            toff = np.zeros(len(wheres) + 1, np.uint64)
-            toff[1:] = np.cumsum([len(w.terms) for w in wheres], dtype=np.uint64)
-            tflat = np.fromiter((int(t) for w in wheres for t in w.terms), dtype=np.uint64, count=int(toff[-1]))
-            _check(L.lib().wax_vs_search_batch_where_terms(*head, toff.ctypes.data_as(C.POINTER(C.c_uint64)),
-                                                           tflat.ctypes.data_as(C.POINTER(C.c_uint64)), *tail))
+        if a.with_terms:
+            _check(L.lib().wax_vs_search_batch_where_terms(*head, *a.term_args(), *tail))
         else:
-            entry = L.lib().wax_vs_search_batch_where_near if near else L.lib().wax_vs_search_batch_where
+            entry = L.lib().wax_vs_search_batch_where_near if a.near else L.lib().wax_vs_search_batch_where
             _check(entry(*head, *tail))
         return [[(int(ids[i, j]), float(scores[i, j])) for j in range(int(ns[i]))] for i in range(b)]
 
@@ -828,6 +847,29 @@ class CUDAVectorEngine:
                                                     idp, fids.size, 0 if allow is not None else 1,
                                                     ids.ctypes.data_as(C.POINTER(C.c_uint64)),
                                                     scores.ctypes.data_as(C.POINTER(C.c_float)), cap, C.byref(n)))
+        return [(int(ids[i]), float(scores[i])) for i in range(n.value)]
+
+    def shard_search_where(self, vector: Sequence[float], top_k: int, where: "Where", allow: Optional[Sequence[int]] = None,
+                           deny: Optional[Sequence[int]] = None) -> List[Tuple[int, float]]:
+        """COLLECTIVE where search (wax_vs_shard_search_where; every rank passes the same query, where and ids): the best
+        `top_k` frames of the whole sharded corpus that pass `where` (its time, tag, location and term clauses) and the
+        optional id filter; identical to search_where on one engine holding the whole corpus.  top_k <= 128."""
+        if allow is not None and deny is not None:
+            raise ValueError("pass at most one of allow= / deny=")
+        fids = np.ascontiguousarray(allow if allow is not None else (deny if deny is not None else []),
+                                    dtype=np.uint64).reshape(-1)
+        terms = np.ascontiguousarray([int(t) for t in where.terms], dtype=np.uint64)
+        w = where.to_c_near()
+        q = np.ascontiguousarray(vector, dtype=np.float32).reshape(-1)
+        cap = _clamp_topk(top_k)
+        ids = np.empty(cap, np.uint64)
+        scores = np.empty(cap, np.float32)
+        n = C.c_uint32(0)
+        _check(L.lib().wax_vs_shard_search_where(
+            self._h, q.ctypes.data_as(C.POINTER(C.c_float)), q.size, int(top_k),
+            fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None, fids.size, 0 if allow is not None else 1,
+            C.byref(w), terms.ctypes.data_as(C.POINTER(C.c_uint64)) if terms.size else None, terms.size,
+            ids.ctypes.data_as(C.POINTER(C.c_uint64)), scores.ctypes.data_as(C.POINTER(C.c_float)), cap, C.byref(n)))
         return [(int(ids[i]), float(scores[i])) for i in range(n.value)]
 
     def time_shard_search(self, top_k: int, iters: int, warmup: int = 3, n_queries: int = 1, seed: int = 7):

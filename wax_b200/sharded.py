@@ -457,6 +457,68 @@ class ShardedVectorEngine:
             raise InvalidToc("sharded filtered search needs the p2p-fused transport and top_k <= 128")
         return self.engine.shard_search_filtered(q, top_k, allow=allow, deny=deny)
 
+    # -- frame attributes and where search: the clauses ride below every rank's top-k, as in search_filtered
+    def set_attributes(self, frame_ids, timestamps=None, tags=None) -> int:
+        """CUDAVectorEngine.set_attributes on this rank's engine.  The full lists may be passed (ids this shard does not
+        hold are ignored) or only its own frames.  Returns this rank's assigned count."""
+        return self.engine.set_attributes(frame_ids, timestamps, tags)
+
+    def set_locations(self, frame_ids, latitudes, longitudes) -> int:
+        """CUDAVectorEngine.set_locations on this rank's engine (full lists or this rank's frames)."""
+        return self.engine.set_locations(frame_ids, latitudes, longitudes)
+
+    def set_terms(self, frame_ids, term_lists) -> int:
+        """CUDAVectorEngine.set_terms on this rank's engine (full lists or this rank's frames)."""
+        return self.engine.set_terms(frame_ids, term_lists)
+
+    def search_where(self, vector: Sequence[float], top_k: int, where, allow=None, deny=None) -> List[Tuple[int, float]]:
+        """The best `top_k` frames of the whole sharded corpus passing `where` and the optional id filter (collective:
+        same arguments on every rank); equal to CUDAVectorEngine.search_where on one engine holding the corpus.  The fused
+        transport with top_k <= 128 takes one exchange inside the scan (wax_vs_shard_search_where); otherwise the
+        batched device form runs for one query."""
+        q = np.ascontiguousarray(vector, dtype=np.float32).reshape(-1)
+        if q.size != self.dimensions:
+            from .engine import EncodingError
+            raise EncodingError(f"vector dimension mismatch: expected {self.dimensions}, got {q.size}")
+        if allow is not None and deny is not None:
+            raise ValueError("pass at most one of allow= / deny=")
+        if self.transport == "p2p-fused" and clamp_topk(top_k) <= 128:
+            return self.engine.shard_search_where(q, top_k, where, allow=allow, deny=deny)
+        filters = [("allow", allow)] if allow is not None else ([("deny", deny)] if deny is not None else [])
+        return self.search_batch_where(q.reshape(1, -1), top_k, [where], [0], filters, [0 if filters else None])[0]
+
+    def search_batch_where(self, vectors, top_k: int, wheres, query_where, filters=None,
+                           query_filter=None) -> List[List[Tuple[int, float]]]:
+        """CUDAVectorEngine.search_batch_where over the whole sharded corpus (collective): every rank plans its shard with
+        wax_vs_search_batch_where_device, ONE all-gather carries batch x k candidates per rank, ONE merge kernel ranks them
+        (wax_vs_merge_candidates_device) and ONE copy brings the answers to the host.  Any transport, k up to 10 000."""
+        from . import _lib as L
+        from .engine import _WhereArgs
+        torch, dist = self._torch, self._dist
+        qs = np.ascontiguousarray(vectors, dtype=np.float32).reshape(-1, self.dimensions)
+        b = qs.shape[0]
+        a = _WhereArgs(wheres, query_where, filters, query_filter, b)
+        if b == 0:
+            return []
+        k = clamp_topk(top_k)
+        d_qs = torch.from_numpy(qs).to(self.device)
+        local = torch.empty(b * k * 24, dtype=torch.uint8, device=self.device)
+        stream = torch.cuda.current_stream(self.device)
+        rc = L.lib().wax_vs_search_batch_where_device(self.engine.handle, C.c_void_p(d_qs.data_ptr()), b, k,
+                                                      *a.filter_args(), *a.where_args(near=True), *a.term_args(),
+                                                      self.row_lo, C.c_void_p(local.data_ptr()),
+                                                      C.c_void_p(stream.cuda_stream))
+        if rc != 0:
+            raise RuntimeError(f"wax_vs_search_batch_where_device rc={rc}: {L.last_error()}")
+        if self.world_size > 1:
+            gathered = torch.empty(self.world_size * b * k * 24, dtype=torch.uint8, device=self.device)
+            dist.all_gather_into_tensor(gathered, local, group=self.group)
+        else:
+            gathered = local
+        merged = self._merge_on_device(gathered, b, k, k, stream)
+        ids, scores, ns = self._unpack_merged(merged.cpu().numpy(), b, k)
+        return [[(int(ids[i, j]), float(scores[i, j])) for j in range(int(ns[i]))] for i in range(b)]
+
     def _search_fused(self, q: np.ndarray, top_k: int) -> List[Tuple[int, float]]:
         """wax_vs_shard_search: host query in, merged host result out; scan + NVLink exchange + merge in one launch."""
         return self.engine.shard_search(q, top_k)
