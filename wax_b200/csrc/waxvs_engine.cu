@@ -17,6 +17,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <limits>
 #include <map>
 #include <mutex>
 #include <new>
@@ -155,6 +156,10 @@ struct IdMap {
 };
 
 // ---------------------------------------------------------------------------------------------------------
+// The shadows the single-query route nominates from (DESIGN 4.1), in the order of their bytes per row: bf16 (the SHADOW
+// form of the scan), int8 (INT8) and 4-bit (U4).  Indexes the per-form tables, options, shadows and counters.
+enum RouteForm : int { kRouteBf16, kRouteInt8, kRouteU4, kRouteForms };
+
 struct Tuning {
     int variant = 0;      // 0 auto, 1 TMA-staged, 2 direct LDG
     int rows_per_step = 0;  // 0 auto
@@ -191,19 +196,18 @@ struct Tuning {
     uint64_t filter_bitset_bytes = 2ull << 30;   // per-query filters: row bitsets one tensor pass may hold
     int shadow_scan = 1;    // single queries (cosine / dot, k <= 32) nominate on the bf16 shadow with the streaming scan, then
                             // an exact re-score + proof, the fp32 scan only when the proof fails (0: always the fp32 scan)
-    uint64_t shadow_scan_min_bytes = 512ull << 20;   // ... for fp32 corpora of at least this many bytes (smaller ones are
-                                                     // latency-bound: two more launches and a shadow do not pay; on
-                                                     // H100 at 384 dims the route breaks even near 380 MB, DESIGN 5)
-    int shadow_rows_per_step = 0, shadow_warps = 0, shadow_stages = 0;   // shape of the SHADOW form (0 auto)
-    uint64_t int8_scan_min_bytes = 512ull << 20;   // the route nominates from the int8 shadow (half the bytes of the bf16
-                                                   // one) for fp32 corpora of at least this many bytes whose measured int8
-                                                   // bound is no coarser than the bf16 one (DESIGN 4.1, 5)
-    int int8_rows_per_step = 0, int8_warps = 0, int8_stages = 0;   // shape of the INT8 form (0 auto)
-    uint64_t u4_scan_min_bytes = 2048ull << 20;    // ... and from the 4-bit shadow (half the bytes again) for fp32 corpora
-                                                   // of at least this many bytes, while its proofs hold (DESIGN 4.1, 5):
-                                                   // its re-score of thousands of nominees is a fixed cost, measured only
-                                                   // at 15 GB, so corpora of a GB or two stay on the int8 form
-    int u4_rows_per_step = 0, u4_warps = 0, u4_stages = 0;   // shape of the U4 form (0 auto)
+    // Each form of the route, by RouteForm (options "<shadow|int8|u4>_scan_min_bytes", "_rows_per_step", "_warps",
+    // "_stages"): the smallest fp32 corpus it takes, and the shape of its nominating scan (0 auto).
+    struct Route { uint64_t min_bytes; int rows_per_step = 0, warps = 0, stages = 0; };
+    Route route[kRouteForms] = {
+        {512ull << 20},    // bf16: smaller corpora are latency-bound: two more launches and a shadow do not pay; on H100
+                           // at 384 dims the route breaks even near 380 MB (DESIGN 5)
+        {512ull << 20},    // int8 (half the bytes of the bf16 shadow), for corpora whose measured int8 bound is no coarser
+                           // than the bf16 one (DESIGN 4.1, 5)
+        {2048ull << 20},   // 4-bit (half the bytes again), while its proofs hold (DESIGN 4.1, 5): its re-score of
+                           // thousands of nominees is a fixed cost, measured only at 15 GB, so corpora of a GB or two
+                           // stay on the int8 form
+    };
 };
 
 // Per-search scratch: the analogue of TransientBuffers (MetalVectorEngine.swift:36-41, :84-117).
@@ -319,15 +323,12 @@ struct wax_vs_engine {
     uint64_t norms_rows = 0;       // rows [0, norms_rows) of d_inv_norm (and d_half_sq) are valid (appends extend it, other
                                    // mutations reset it)
     std::mutex norms_mu;
-    // bf16 shadow of the corpus for the batched bf16 nominations (cached per corpus version, guarded by norms_mu)
-    DevBuf<__nv_bfloat16> d_shadow;
-    uint64_t shadow_rows = 0;      // rows [0, shadow_rows) of d_shadow are valid; shadow_valid = covers every live row
-    bool shadow_valid = false, shadow_unavailable = false;
-    // int8 shadow of the corpus for the single-query route only (DESIGN 4.1; same cache rules, guarded by norms_mu): four
-    // biased codes per word, one scale per row (padded to whole scan steps) and the measured bound rho_max (fp32 bits on
-    // the device; read back once per build together with max|v|, giving the bound the finish uses)
-    struct CodedShadow {
-        uint32_t bits = 8;             // per code: 8 (shadow_int8_kernel) or 4 (shadow_u4_kernel)
+    // Shadows of the corpus, by RouteForm (cached per corpus version, guarded by norms_mu): bf16 (two values per word;
+    // also the batched bf16 nominations), int8 (four biased codes per word) and 4-bit (16 levels, eight codes per word)
+    // for the single-query route (DESIGN 4.1).  The coded two also hold one scale per row (the 4-bit one: a half step;
+    // padded to whole scan steps) and the measured bound rho_max (fp32 bits on the device; read back once per build
+    // together with max|v|, giving the bound the finish uses).
+    struct Shadow {
         DevBuf<uint32_t> codes;
         DevBuf<float> scale;
         DevBuf<uint32_t> rho;
@@ -335,22 +336,24 @@ struct wax_vs_engine {
         bool valid = false, unavailable = false;
         bool coarse = false;           // the last build measured a bound too coarse for the route: none is built again until
                                        // the rows are rewritten (invalidate_row_caches with no prefix) or its min_bytes option is set
-        float rho_max = 0.0f, eps_rel = INFINITY;   // rho_max, and rho_max / M rounded up (M = 1 cosine, max|v| dot)
+        float rho_max = 0.0f, eps_rel = INFINITY;   // rho_max, and rho_max / M rounded up (M = 1 cosine, max|v| dot);
+                                                    // bf16: eps_rel = kBf16Eps once built
         void release() { codes.release(); scale.release(); rows = 0; valid = false; }
-        void invalidate(uint64_t keep_prefix) {     // a kept prefix keeps rho_max too: still an upper bound
+        // A kept prefix keeps rho_max too: still an upper bound.  A shadow with a measured bound is no longer valid, so
+        // that its next use reads rho_max and max|v| back again; the bf16 one stays valid over a kept prefix
+        // (shadow_bytes reports the prefix).
+        void invalidate(uint64_t keep_prefix, bool measured_bound) {
             rows = std::min(rows, keep_prefix);
-            valid = false;
+            if (measured_bound || rows == 0) valid = false;
             if (keep_prefix == 0) coarse = false;
         }
-    } i8, u4{4};
-    // The 4-bit shadow of the same route (16 levels, eight codes per word, one half step per row), same record and rules;
-    // its bound is 16 times the int8 one, so whether its nominees prove depends on the scores: a failed 4-bit proof sends
-    // the next u4_demote_window eligible queries to the int8 form (u4_demoted counts them down), and the window doubles
-    // when the first 4-bit query after it fails again.
+    } shadows[kRouteForms];
+    // The 4-bit bound is 16 times the int8 one, so whether its nominees prove depends on the scores: a failed 4-bit proof
+    // sends the next u4_demote_window eligible queries to the int8 form (u4_demoted counts them down), and the window
+    // doubles when the first 4-bit query after it fails again.
     uint32_t u4_demoted = 0, u4_demote_window = 16;
     bool u4_probing = false;                              // the next 4-bit proof decides whether the window doubles
-    uint64_t single_int8_queries = 0;                     // single queries nominated from the int8 shadow (pool_mu)
-    uint64_t single_u4_queries = 0;                       // ... from the 4-bit shadow (pool_mu)
+    uint64_t single_route_queries[kRouteForms] = {};      // single queries nominated from each shadow (pool_mu)
     uint64_t batch_tensor_queries = 0, batch_fallback_queries = 0;   // instrumentation
     uint64_t batch_bf16_queries = 0, batch_retry_queries = 0, batch_tf32_queries = 0, batch_filter_bf16_queries = 0;
     uint64_t filter_bitset_passes = 0;
@@ -492,10 +495,7 @@ static void drain_device_path(wax_vs_engine *e) {
 // append keeps everything it had); 0 = rebuild from scratch on the next batched search.
 static void invalidate_row_caches(wax_vs_engine *e, uint64_t keep_prefix) {
     e->norms_rows = std::min(e->norms_rows, keep_prefix);
-    e->shadow_rows = std::min(e->shadow_rows, keep_prefix);
-    if (e->shadow_rows == 0) e->shadow_valid = false;
-    e->i8.invalidate(keep_prefix);
-    e->u4.invalidate(keep_prefix);
+    for (int f = 0; f < kRouteForms; ++f) e->shadows[f].invalidate(keep_prefix, f != kRouteBf16);
     e->gindex.valid = false;           // appends too: the new rows need index entries
     e->attrs_dev_valid = false;        // likewise the attribute mirror
     e->locs_dev_valid = false;         // and the location mirror
@@ -609,18 +609,28 @@ static int32_t ctx_for_stream(wax_vs_engine *e, void *cuda_stream, SearchCtx **o
 // kernel dispatch
 struct TmaConfig { int C, R, warps, stages; size_t smem; };
 
-// esize: bytes per element of the rows streamed -- 4 for the corpus, 2 for the bf16 shadow (the SHADOW form), 1 for the
-// int8 shadow (the INT8 form; its stages also hold the step's row scales) -- the shadow forms on unrolled shapes only.
-static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0, size_t esize = sizeof(float)) {
+// The unrolled shapes of the TMA scan: rows of C x 128 elements (12: the 1536-dim embeddings).
+constexpr int kUnrolledC[7] = {1, 2, 3, 4, 6, 8, 12};
+// Index in kUnrolledC of rows of d elements, -1 when no unrolled shape has them.
+static int unrolled_index(uint32_t d) {
+    for (int i = 0; i < 7; ++i)
+        if (d == 128u * kUnrolledC[i]) return i;
+    return -1;
+}
+// Dynamic shared memory a TMA-staged scan may take: the opt-in limit minus the kernels' static shared memory.
+static size_t tma_smem_budget(const wax_vs_engine *e) { return (e->smem_optin ? e->smem_optin : 232448) - 4096; }
+// ... and what a ring of `stages` steps of stage_bytes per warp takes (with each warp's barriers and list).
+static size_t tma_ring_smem(int warps, int stages, size_t stage_bytes) {
+    return static_cast<size_t>(warps) * stages * (stage_bytes + 8 + 4) + static_cast<size_t>(warps) * 1024 + 16;
+}
+
+// The fp32 scan's shape (the route's forms: pick_route_config).
+static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0) {
     const uint32_t d = e->dims;
     if (d % 4u != 0) return false;                      // rows must be 16-byte multiples for the bulk copy
-    const size_t budget = (e->smem_optin ? e->smem_optin : 232448) - 4096;   // minus the kernels' static shared memory
-    int C = 0;
-    if (d % 128u == 0) {
-        const int c = static_cast<int>(d / 128u);
-        if (c == 1 || c == 2 || c == 3 || c == 4 || c == 6 || c == 8 || c == 12) C = c;   // unrolled shapes (12: the 1536-dim embeddings)
-    }
-    if (esize != sizeof(float) && C == 0) return false;
+    const size_t budget = tma_smem_budget(e);
+    const int ci = unrolled_index(d);
+    const int C = ci < 0 ? 0 : kUnrolledC[ci];
     if (C == 0 && d < 32) return false;                  // a few floats per row: the direct-load kernel
     if (C == 0 && d > e->tune.tma_max_dims) return false;   // very long rows: too few warps fit beside two stages, the
                                                              // direct-load kernel takes them
@@ -628,23 +638,7 @@ static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0
     // is per-row instruction latency, not bytes in flight).  These defaults were chosen on B200, not re-tuned on H100; the
     // `rows_per_step` / `warps` / `stages` options override them.
     int R, warps_default = 8;
-    if (esize == 1) {                                    // the INT8 form (a quarter of the bytes of a corpus row)
-        // steps of ~3 KB like the best bf16 shape, 16 warps, 3 stages (DESIGN 4.1); launch_int8_scan has rows per step
-        // r_lo .. r_hi, r_def by default
-        const int want_r = e->tune.int8_rows_per_step;
-        const int r_def = C <= 3 ? 8 : 4, r_lo = C == 3 ? 4 : r_def, r_hi = C <= 3 ? 16 : (C <= 6 ? 8 : 4);
-        R = (want_r >= r_lo && want_r <= r_hi && (want_r & (want_r - 1)) == 0) ? want_r : r_def;
-        warps_default = 16;
-    } else if (esize != sizeof(float)) {                 // the shadow form (bf16 rows: half the bytes of a corpus row)
-        // 16 warps, 3 stages of 2-6 KB: on H100 at 10 M x 384 (C = 3) rows 4 / warps 16 / stages 3 took 2.503 ms per
-        // query against 2.545 for the fp32 shape's bytes (rows 8 / warps 8 / stages 2), the best of eight shapes
-        // alternated in one run (DESIGN 4.1); the other C take the same ring, not measured separately.
-        // launch_shadow_scan has rows per step r_min .. r_max.
-        const int want_r = e->tune.shadow_rows_per_step;
-        const int r_min = C <= 2 ? 8 : (C <= 4 ? 4 : 2), r_max = C <= 3 ? 16 : 2 * r_min;
-        R = (want_r >= r_min && want_r <= r_max && (want_r & (want_r - 1)) == 0) ? want_r : r_min;
-        warps_default = 16;
-    } else if (C == 0) {                               // generic shape: run-time chunk count, query in shared memory
+    if (C == 0) {                                      // generic shape: run-time chunk count, query in shared memory
         // keep a step at >= 2-8 KB: short generic rows (dims < 128, 160, 300, 400, ...) take 8 or 4 rows per step and
         // more warps, like the unrolled C <= 2 shapes
         // (long rows: as many rows as keep a step at <= 32 KB -- the few warps that then fit still hold ~190 KB in flight)
@@ -667,18 +661,14 @@ static bool pick_tma_config(const wax_vs_engine *e, TmaConfig *cfg, int mode = 0
         // that won over 8 warps on B200, above it the 8-warp shape's 48 KB in flight did (chosen on B200, not re-tuned on H100)
         else if (mode == 1 && static_cast<uint64_t>(e->n_rows) * d * 4 < (8ull << 30)) warps_default = 16;
     }
-    // Default ring depth 2: ~48 KB in flight per SM for the 8-warp shapes (the `stages` option overrides it).  The shadow
-    // form has options of its own (shadow_*): it runs right before a guarded fp32 scan that keeps the fp32 shape.
-    const bool shadow = esize != sizeof(float), int8 = esize == 1;
-    const int want_stages = int8 ? e->tune.int8_stages : shadow ? e->tune.shadow_stages : e->tune.stages;
-    const int want_warps = int8 ? e->tune.int8_warps : shadow ? e->tune.shadow_warps : e->tune.warps;
-    const int stages = want_stages > 0 ? want_stages : (shadow ? 3 : 2);
-    const size_t stage_bytes = static_cast<size_t>(R) * d * esize + (int8 ? static_cast<size_t>(R) * 4 : 0);   // + scales
+    // Default ring depth 2: ~48 KB in flight per SM for the 8-warp shapes (the `stages` option overrides it).  The route's
+    // forms have options of their own: they run right before a guarded fp32 scan that keeps the fp32 shape.
+    const int stages = e->tune.stages > 0 ? e->tune.stages : 2;
+    const size_t stage_bytes = static_cast<size_t>(R) * d * sizeof(float);
     const size_t query_bytes = C == 0 ? (static_cast<size_t>(d) * 4 + 512 + 32) : 0;
-    auto smem_for = [&](int w) { return static_cast<size_t>(w) * stages * (stage_bytes + 8 + 4) + static_cast<size_t>(w) * 1024 + 16 + query_bytes; };
-    int warps = want_warps ? want_warps : warps_default;
-    warps = std::max(1, std::min(16, warps));
-    if (!want_warps) while (warps > 2 && smem_for(warps) > budget) --warps;   // long rows: fewer warps per CTA
+    auto smem_for = [&](int w) { return tma_ring_smem(w, stages, stage_bytes) + query_bytes; };
+    int warps = std::max(1, std::min(16, e->tune.warps ? e->tune.warps : warps_default));
+    if (!e->tune.warps) while (warps > 2 && smem_for(warps) > budget) --warps;   // long rows: fewer warps per CTA
     if (smem_for(warps) > budget) return false;
     cfg->C = C; cfg->R = R; cfg->warps = warps; cfg->stages = stages; cfg->smem = smem_for(warps);
     return true;
@@ -735,54 +725,97 @@ static cudaError_t launch_tma(wax_vs_engine *e, const ScanParams &p, int grid, c
 #undef WAXVS_CASE
     return cudaErrorInvalidValue;
 }
-// The SHADOW form (nominating pass of the bf16-shadow route): cosine / dot, the unrolled shapes, k' nominees (E = 4).
-static cudaError_t launch_shadow_scan(wax_vs_engine *e, const ScanParams &p, int grid, const TmaConfig &cfg, int metric,
+// The nominating pass of the route (SHADOW form, INT8 / U4 for the coded shadows): cosine / dot, k' nominees (E = 4).
+// The 4-bit score' does not depend on the metric (cosine rows are pre-scaled in the shadow): one instantiation serves both.
+template <RouteForm F, int C, int R>
+static cudaError_t launch_route_cr(wax_vs_engine *e, const ScanParams &p, int grid, const TmaConfig &cfg, int metric,
+                                   cudaStream_t s) {
+    if constexpr (F == kRouteU4) {
+        return launch_tma_inst<C, R, kDot, 4, false, true, false, true>(e, p, grid, cfg, s);
+    } else {
+        return metric == kCosine ? launch_tma_inst<C, R, kCosine, 4, false, true, F == kRouteInt8>(e, p, grid, cfg, s)
+                                 : launch_tma_inst<C, R, kDot, 4, false, true, F == kRouteInt8>(e, p, grid, cfg, s);
+    }
+}
+// The (C, R) shapes compiled for each form of the route, listed once: launch_<form>_scan launches the form's scan in the
+// shape `cfg`, and with p = nullptr only tells whether that shape is compiled (cudaSuccess; pick_route_config takes a
+// rows_per_step option by it).
+#define WAXVS_CASE(Cv, Rv) \
+    if (cfg.C == Cv && cfg.R == Rv) return p ? launch_route_cr<F, Cv, Rv>(e, *p, grid, cfg, metric, s) : cudaSuccess
+static cudaError_t launch_shadow_scan(wax_vs_engine *e, const ScanParams *p, int grid, const TmaConfig &cfg, int metric,
                                       cudaStream_t s) {
-#define WAXVS_CASE(Cv, Rv)                                                                                          \
-    if (cfg.C == Cv && cfg.R == Rv)                                                                                 \
-        return metric == kCosine ? launch_tma_inst<Cv, Rv, kCosine, 4, false, true>(e, p, grid, cfg, s)            \
-                                 : launch_tma_inst<Cv, Rv, kDot, 4, false, true>(e, p, grid, cfg, s)
+    constexpr RouteForm F = kRouteBf16;
     WAXVS_CASE(1, 8); WAXVS_CASE(1, 16); WAXVS_CASE(2, 8); WAXVS_CASE(2, 16);
     WAXVS_CASE(3, 4); WAXVS_CASE(3, 8); WAXVS_CASE(3, 16); WAXVS_CASE(4, 4); WAXVS_CASE(4, 8);
     WAXVS_CASE(6, 2); WAXVS_CASE(6, 4); WAXVS_CASE(8, 2); WAXVS_CASE(8, 4); WAXVS_CASE(12, 2); WAXVS_CASE(12, 4);
-#undef WAXVS_CASE
     return cudaErrorInvalidValue;
 }
-// The INT8 form (nominating pass of the int8-shadow route): the shapes pick_tma_config gives it.
-static cudaError_t launch_int8_scan(wax_vs_engine *e, const ScanParams &p, int grid, const TmaConfig &cfg, int metric,
+static cudaError_t launch_int8_scan(wax_vs_engine *e, const ScanParams *p, int grid, const TmaConfig &cfg, int metric,
                                    cudaStream_t s) {
-#define WAXVS_CASE(Cv, Rv)                                                                                          \
-    if (cfg.C == Cv && cfg.R == Rv)                                                                                 \
-        return metric == kCosine ? launch_tma_inst<Cv, Rv, kCosine, 4, false, true, true>(e, p, grid, cfg, s)      \
-                                 : launch_tma_inst<Cv, Rv, kDot, 4, false, true, true>(e, p, grid, cfg, s)
+    constexpr RouteForm F = kRouteInt8;
     WAXVS_CASE(1, 8); WAXVS_CASE(1, 16); WAXVS_CASE(2, 8); WAXVS_CASE(2, 16);
     WAXVS_CASE(3, 4); WAXVS_CASE(3, 8); WAXVS_CASE(3, 16); WAXVS_CASE(4, 4); WAXVS_CASE(4, 8);
     WAXVS_CASE(6, 4); WAXVS_CASE(6, 8); WAXVS_CASE(8, 4); WAXVS_CASE(12, 4);
-#undef WAXVS_CASE
     return cudaErrorInvalidValue;
 }
-// The U4 form (nominating pass of the 4-bit-shadow route): steps of ~3 KB (16 rows at 384 dims), 16 warps, 3 stages unless
-// the u4_* options say otherwise; launch_u4_scan has rows per step r_lo .. r_hi.
-static bool pick_u4_config(const wax_vs_engine *e, TmaConfig *cfg) {
-    if (!pick_tma_config(e, cfg, 1, 1)) return false;           // the unrolled shapes, as for the INT8 form
-    const int C = cfg->C, want_r = e->tune.u4_rows_per_step;
-    const int r_hi = C <= 3 ? 16 : (C <= 6 ? 8 : 4), r_lo = C <= 3 ? 8 : 4;
-    cfg->R = (want_r >= r_lo && want_r <= r_hi && (want_r & (want_r - 1)) == 0) ? want_r : r_hi;
-    cfg->stages = e->tune.u4_stages > 0 ? e->tune.u4_stages : 3;
-    cfg->warps = std::max(1, std::min(16, e->tune.u4_warps ? e->tune.u4_warps : 16));
-    const size_t stage_bytes = static_cast<size_t>(cfg->R) * (e->dims / 2 + 4);     // codes + half steps
-    cfg->smem = static_cast<size_t>(cfg->warps) * cfg->stages * (stage_bytes + 8 + 4) + static_cast<size_t>(cfg->warps) * 1024 + 16;
-    return cfg->smem <= (e->smem_optin ? e->smem_optin : 232448) - 4096;
-}
-// score' does not depend on the metric (cosine rows are pre-scaled in the shadow): one instantiation serves both.
-static cudaError_t launch_u4_scan(wax_vs_engine *e, const ScanParams &p, int grid, const TmaConfig &cfg, cudaStream_t s) {
-#define WAXVS_CASE(Cv, Rv) \
-    if (cfg.C == Cv && cfg.R == Rv) return launch_tma_inst<Cv, Rv, kDot, 4, false, true, false, true>(e, p, grid, cfg, s)
+static cudaError_t launch_u4_scan(wax_vs_engine *e, const ScanParams *p, int grid, const TmaConfig &cfg, int metric,
+                                  cudaStream_t s) {
+    constexpr RouteForm F = kRouteU4;
     WAXVS_CASE(1, 8); WAXVS_CASE(1, 16); WAXVS_CASE(2, 8); WAXVS_CASE(2, 16); WAXVS_CASE(3, 8); WAXVS_CASE(3, 16);
     WAXVS_CASE(4, 4); WAXVS_CASE(4, 8); WAXVS_CASE(6, 4); WAXVS_CASE(6, 8); WAXVS_CASE(8, 4); WAXVS_CASE(12, 4);
-#undef WAXVS_CASE
     return cudaErrorInvalidValue;
 }
+#undef WAXVS_CASE
+
+// What differs between the forms of the single-query route (DESIGN 4.1), by RouteForm.
+struct RouteFormSpec {
+    const char *name;
+    uint32_t bits;            // per element of a shadow row
+    bool scaled;              // rows carry a scale (in the scan's stages too), and the shadow a measured bound
+    cudaError_t (*launch)(wax_vs_engine *, const ScanParams *, int, const TmaConfig &, int, cudaStream_t);   // its scan
+    int default_r[7];         // rows per step without the option, by C of kUnrolledC
+    int warps, stages;        // without the options
+    bool keep_warps;          // without the warps option the default is kept and a ring that does not fit refused (else
+                              // fewer warps until it fits)
+    bool grid_rescore;        // nominees: kU4CtaNominees per CTA, re-scored and proven on the whole grid by
+                              // shadow_rescore_kernel (else the kShadowNominees x kNomineeStride warp lists of one query,
+                              // re-scored and proven by batch_finish_kernel)
+    uint32_t tail_bytes;      // per element of the ring, the staging the scan's selection tail may use (the 4-bit form
+                              // has no selection tail and keeps the bf16 figure)
+    float max_eps_rel;        // the coarsest bound whose nominees the route takes
+};
+constexpr RouteFormSpec kRouteSpec[kRouteForms] = {
+    // bf16: 16 warps, 3 stages of 2-6 KB: on H100 at 10 M x 384 (C = 3) rows 4 / warps 16 / stages 3 took 2.503 ms per
+    // query against 2.545 for the fp32 shape's bytes (rows 8 / warps 8 / stages 2), the best of eight shapes alternated
+    // in one run (DESIGN 4.1); the other C take the same ring, not measured separately.
+    {"bf16", 16, false, launch_shadow_scan, {8, 8, 4, 4, 2, 2, 2}, 16, 3, false, false, 2, kBf16Eps},
+    // int8: steps of ~3 KB like the best bf16 shape, 16 warps, 3 stages (DESIGN 4.1)
+    {"int8", 8, true, launch_int8_scan, {8, 8, 8, 4, 4, 4, 4}, 16, 3, false, false, 1, kBf16Eps},
+    // 4-bit: steps of ~3 KB (16 rows at 384 dims), 16 warps, 3 stages; its bound is coarser than the bf16 one by design,
+    // so any finite one is taken
+    {"4-bit", 4, true, launch_u4_scan, {16, 16, 16, 8, 8, 4, 4}, 16, 3, true, true, 2, std::numeric_limits<float>::max()},
+};
+
+// The nominating scan's shape for a form of the route: the unrolled shapes only, its options or its defaults.
+static bool pick_route_config(const wax_vs_engine *e, RouteForm f, TmaConfig *cfg) {
+    const RouteFormSpec &fs = kRouteSpec[f];
+    const Tuning::Route &t = e->tune.route[f];
+    const int ci = unrolled_index(e->dims);
+    if (ci < 0) return false;
+    const int C = kUnrolledC[ci];
+    const bool listed = fs.launch(nullptr, nullptr, 0, TmaConfig{C, t.rows_per_step, 0, 0, 0}, 0, nullptr) == cudaSuccess;
+    const int R = listed ? t.rows_per_step : fs.default_r[ci];
+    const int stages = t.stages > 0 ? t.stages : fs.stages;
+    const size_t stage_bytes = static_cast<size_t>(R) * (e->dims * fs.bits / 8 + (fs.scaled ? sizeof(float) : 0));
+    const size_t budget = tma_smem_budget(e);
+    int warps = std::max(1, std::min(16, t.warps ? t.warps : fs.warps));
+    if (!t.warps && !fs.keep_warps) while (warps > 2 && tma_ring_smem(warps, stages, stage_bytes) > budget) --warps;
+    const size_t smem = tma_ring_smem(warps, stages, stage_bytes);
+    if (smem > budget) return false;
+    *cfg = TmaConfig{C, R, warps, stages, smem};
+    return true;
+}
+
 static cudaError_t launch_ldg(const ScanParams &p, int grid, int metric, int mode, cudaStream_t s) {
     switch (metric * 3 + mode) {
         case 0: scan_ldg_kernel<kCosine, 1, false><<<grid, 256, 0, s>>>(p); break;
@@ -892,101 +925,92 @@ static int tma_grid(const wax_vs_engine *e, const SearchCtx *c, const TmaConfig 
 
 static bool batch_bf16_wanted(const wax_vs_engine *e);
 static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream);
-static int32_t ensure_coded_shadow(wax_vs_engine *e, wax_vs_engine::CodedShadow &cs, cudaStream_t stream, bool keep_coarse = false);
+static int32_t ensure_coded_shadow(wax_vs_engine *e, RouteForm f, cudaStream_t stream, bool keep_coarse);
+// The shadow of form f, brought up to date when it fits (keep_coarse: see ensure_coded_shadow).
+static int32_t ensure_route_shadow(wax_vs_engine *e, RouteForm f, cudaStream_t stream, bool keep_coarse = false) {
+    return f == kRouteBf16 ? ensure_shadow(e, stream) : ensure_coded_shadow(e, f, stream, keep_coarse);
+}
 
-// ---- the bf16-shadow route of a single query (DESIGN 4.1) ----
-// The fp32 scan reads dims * 4 bytes per row and runs at the HBM read ceiling; the shadow holds the same rows in bf16.
-// Three launches on `stream`, no host round trip: the SHADOW form of the scan nominates the k' best rows by score', the
-// batched path's finish kernel (one query, one slice) re-scores them exactly in the scan's own order and proves that no
-// other row can beat or tie the k-th (DESIGN 4.5), and `p` -- the query's fp32 scan, launched next by the caller -- is
-// guarded by that proof: it returns at entry when the proof held, else it answers the query as it always does.
-constexpr uint32_t kShadowNominees = 128;     // k': every warp list of the SHADOW form holds this many
+// ---- the shadow route of a single query (DESIGN 4.1) ----
+// The fp32 scan reads dims * 4 bytes per row and runs at the HBM read ceiling; a shadow holds the same rows in fewer
+// bytes (bf16, int8 or 4-bit).  Three launches on `stream`, no host round trip: the form's nominating scan picks the best
+// rows by score', a re-score (the batched path's finish kernel, one query, one slice; the 4-bit form: a grid-wide one)
+// re-scores them exactly in the scan's own order and proves that no other row can beat or tie the k-th (DESIGN 4.5), and
+// `p` -- the query's fp32 scan, launched next by the caller -- is guarded by that proof: it returns at entry when the
+// proof held, else it answers the query as it always does.
+constexpr uint32_t kShadowNominees = 128;     // k': every warp list of the SHADOW and INT8 forms holds this many
 constexpr uint32_t kShadowRescore = 256;
 constexpr uint32_t kShadowSkipQueries = 16;   // after a failed proof: eligible queries that take the fp32 scan directly
 // Nothing is enqueued (and p stays unguarded) when the route does not apply to this engine and query; the caller has
 // already checked the rest: one unsharded fused query with k <= 32 on an unrolled TMA shape.
 // (batch_bf16 and dims % 64 == 0 as for the bf16 nominations, but not whether the bf16 shadow fitted: when it did not,
-// the int8 form still runs on its own shadow, and the bf16 form finds no shadow and leaves the query to the fp32 scan)
+// the coded forms still run on their own shadows, and the bf16 form finds no shadow and leaves the query to the fp32 scan)
 static bool shadow_route_applies(const wax_vs_engine *e) {
     return e->tune.shadow_scan && (e->similarity == WAX_VS_COSINE || e->similarity == WAX_VS_DOT) && !e->debug_trace &&
            e->tune.batch_bf16 != 0 && e->dims % kBatchKBlockBf16 == 0 &&
-           e->n_rows * e->dims * sizeof(float) >= e->tune.shadow_scan_min_bytes;
+           e->n_rows * e->dims * sizeof(float) >= e->tune.route[kRouteBf16].min_bytes;
 }
-// The int8 form of the route (DESIGN 4.1) is taken instead of the bf16 one for fp32 corpora of at least
-// int8_scan_min_bytes whose int8 shadow fits and whose measured bound is no coarser than the bf16 one (rho_max / M <=
-// kBf16Eps: a corpus with outlier dimensions coarsens its rows' scales and keeps the bf16 route, which proves for it).
-// Call with the route applying; builds the int8 shadow when the size rule holds (a corpus found too coarse builds none
-// until its rows are rewritten, see ensure_coded_shadow).  *use: take the int8 form.
-static int32_t int8_route_selected(wax_vs_engine *e, cudaStream_t stream, bool *use) {
+// The form the route takes for the next query, from what the engine observes: the first of the 4-bit, int8 and bf16
+// forms (each the fastest that proves on some corpus) whose min_bytes the fp32 corpus reaches, whose shape fits (*cfg)
+// and whose shadow fits with a bound no coarser than the form's max_eps_rel -- a corpus with outlier dimensions coarsens
+// the int8 rows' scales and keeps the bf16 form, which proves for it.  The 4-bit form is skipped while a failed 4-bit
+// proof has demoted the route (`demoted`: the caller's reading of u4_demoted).  Call with the route applying; builds the
+// shadows it tries (a corpus found too coarse builds none until its rows are rewritten, see ensure_coded_shadow).
+// *use = false: no form applies, the fp32 scan answers.
+static int32_t select_route_form(wax_vs_engine *e, cudaStream_t stream, bool demoted, bool *use, RouteForm *form,
+                                 TmaConfig *cfg) {
     *use = false;
-    TmaConfig cfg{};
-    if (e->n_rows * e->dims * sizeof(float) < e->tune.int8_scan_min_bytes || !pick_tma_config(e, &cfg, 1, 1)) return WAX_VS_OK;
-    const int32_t rc = ensure_coded_shadow(e, e->i8, stream);
-    if (rc) return rc;
-    *use = e->i8.valid && e->i8.eps_rel <= kBf16Eps;
-    return WAX_VS_OK;
-}
-// The form the route takes for the next query, from what the engine observes: the 4-bit form for fp32 corpora of at least
-// u4_scan_min_bytes whose 4-bit shadow fits with a finite bound, unless a failed 4-bit proof has demoted the route
-// (`demoted`: the caller's reading of u4_demoted); else the int8 form by int8_route_selected; else the bf16 form.  Each is
-// the fastest form that proves on some corpus.  Builds the shadow of the form it selects, and no other.
-enum class RouteForm { kBf16, kInt8, kU4 };
-static int32_t select_route_form(wax_vs_engine *e, cudaStream_t stream, bool demoted, RouteForm *form) {
-    *form = RouteForm::kBf16;
-    TmaConfig cfg{};
-    int32_t rc;
-    if (!demoted && e->n_rows * e->dims * sizeof(float) >= e->tune.u4_scan_min_bytes && pick_u4_config(e, &cfg)) {
-        if ((rc = ensure_coded_shadow(e, e->u4, stream))) return rc;
-        if (e->u4.valid && std::isfinite(e->u4.eps_rel)) { *form = RouteForm::kU4; return WAX_VS_OK; }
+    for (const RouteForm f : {kRouteU4, kRouteInt8, kRouteBf16}) {
+        if ((f == kRouteU4 && demoted) || e->n_rows * e->dims * sizeof(float) < e->tune.route[f].min_bytes ||
+            !pick_route_config(e, f, cfg))
+            continue;
+        if (const int32_t rc = ensure_route_shadow(e, f, stream)) return rc;
+        if (e->shadows[f].valid && e->shadows[f].eps_rel <= kRouteSpec[f].max_eps_rel) {
+            *use = true;
+            *form = f;
+            return WAX_VS_OK;
+        }
     }
-    bool int8 = false;
-    if ((rc = int8_route_selected(e, stream, &int8))) return rc;
-    if (int8) *form = RouteForm::kInt8;
     return WAX_VS_OK;
 }
 
-// Launches 1 and 2 of the route for the query of `p` (the fp32 scan's parameters: query, filter, k, out, ids) in the
-// SHADOW (int8: INT8) shape `cfg`, over a valid shadow: the nominating form writes the kShadowNominees keys to c->d_heaps,
-// the finish re-scores them exactly into p.out and writes its proof flag to c->d_ok.  shape (optional, the read-outs
-// wax_vs_debug_shadow_nominations / wax_vs_debug_int8_nominations): {C, R, warps, stages, grid, chunk_steps, tail_select}
-// of the nominating launch.
+// Launches 1 and 2 of the route for the query of `p` (the fp32 scan's parameters: query, filter, k, out, ids) in form f
+// and its shape `cfg`, over a valid shadow: the nominating scan writes its keys to c->d_heaps, the re-score writes the
+// exact result to p.out and its proof flag to c->d_ok.  shape (optional, the read-outs wax_vs_debug_*_nominations):
+// {C, R, warps, stages, grid, chunk_steps, tail_select} of the nominating launch.
 static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const ScanParams &p, const TmaConfig &cfg,
-                                          cudaStream_t stream, uint64_t *launches, uint32_t *shape = nullptr,
-                                          RouteForm form = RouteForm::kBf16) {
-    const bool int8 = form == RouteForm::kInt8, u4 = form == RouteForm::kU4;
+                                          cudaStream_t stream, uint64_t *launches, uint32_t *shape, RouteForm f) {
+    const RouteFormSpec &fs = kRouteSpec[f];
+    const wax_vs_engine::Shadow &sh = e->shadows[f];
     int32_t rc;
-    if (u4 && !c->d_u4_aux) {           // the cut word starts at "nothing cut"; every re-score leaves it so
+    if (fs.grid_rescore && !c->d_u4_aux) {           // the cut word starts at "nothing cut"; every re-score leaves it so
         if ((rc = c->d_u4_aux.ensure(3, "4-bit route state"))) return rc;
         CUDA_TRY(cudaMemsetAsync(c->d_u4_aux, 0xFF, 3 * sizeof(uint32_t), stream));
     }
-    // U4: up to kU4CtaNominees keys per CTA of the grid (tma_grid never exceeds sm_count or the grid option)
-    const size_t u4_keys = static_cast<size_t>(std::max(e->tune.grid, e->sm_count)) * kU4CtaNominees;
-    if ((rc = c->d_heaps.ensure(std::max(static_cast<size_t>(kShadowNominees) * kNomineeStride, u4 ? u4_keys : 0), "nominee keys")) ||
+    // grid_rescore: up to kU4CtaNominees keys per CTA of the grid (tma_grid never exceeds sm_count or the grid option)
+    const size_t cta_keys = static_cast<size_t>(std::max(e->tune.grid, e->sm_count)) * kU4CtaNominees;
+    if ((rc = c->d_heaps.ensure(std::max(static_cast<size_t>(kShadowNominees) * kNomineeStride, fs.grid_rescore ? cta_keys : 0), "nominee keys")) ||
         (rc = c->d_ok.ensure(1, "proof flags")) || (!p.query && (rc = c->d_queries.ensure(e->dims, "query buffer"))))
         return rc;
 
     ScanParams sp = p;
-    sp.corpus = u4 ? reinterpret_cast<const float *>(e->u4.codes.p)
-                   : int8 ? reinterpret_cast<const float *>(e->i8.codes.p) : reinterpret_cast<const float *>(e->d_shadow.p);
-    sp.row_scale = u4 ? e->u4.scale.p : int8 ? e->i8.scale.p : nullptr;
-    sp.u4_aux = u4 ? c->d_u4_aux.p : nullptr;
+    sp.corpus = reinterpret_cast<const float *>(sh.codes.p);
+    sp.row_scale = fs.scaled ? sh.scale.p : nullptr;
+    sp.u4_aux = fs.grid_rescore ? c->d_u4_aux.p : nullptr;
     sp.k = kShadowNominees;
     sp.out = nullptr; sp.host_out = nullptr; sp.host_flag = nullptr;
     sp.nominees = c->d_heaps;
     sp.query_store = p.query ? nullptr : c->d_queries.p;
     sp.tail_select = e->tune.tail_select ? 1u : 0u;
-    sp.tail_smem_bytes = static_cast<uint32_t>(static_cast<size_t>(cfg.warps) * cfg.stages * cfg.R * e->dims *
-                                               (int8 ? 1 : sizeof(__nv_bfloat16)));
+    sp.tail_smem_bytes = static_cast<uint32_t>(static_cast<size_t>(cfg.warps) * cfg.stages * cfg.R * e->dims * fs.tail_bytes);
     const int grid = tma_grid(e, c, cfg, sp);
-    if (u4) CUDA_TRY(launch_u4_scan(e, sp, grid, cfg, stream));
-    else if (int8) CUDA_TRY(launch_int8_scan(e, sp, grid, cfg, e->similarity, stream));
-    else CUDA_TRY(launch_shadow_scan(e, sp, grid, cfg, e->similarity, stream));
+    CUDA_TRY(fs.launch(e, &sp, grid, cfg, e->similarity, stream));
 
-    if (u4) {           // every CTA's nominees, re-scored and proven on the whole grid
+    if (fs.grid_rescore) {           // every CTA's nominees, re-scored and proven on the whole grid
         RescoreParams rp{};
         rp.corpus = e->d_corpus; rp.query = p.query ? p.query : c->d_queries.p;
         rp.dims = e->dims; rp.k = p.k; rp.n_nominees = static_cast<uint32_t>(grid) * kU4CtaNominees;
-        rp.nominees = c->d_heaps; rp.aux = c->d_u4_aux; rp.max_norm_bits = e->d_max_norm; rp.rho_max = e->u4.rho_max;
+        rp.nominees = c->d_heaps; rp.aux = c->d_u4_aux; rp.max_norm_bits = e->d_max_norm; rp.rho_max = sh.rho_max;
         rp.block_keys = c->d_block_keys; rp.ticket = c->d_ticket; rp.work_counter = sp.work_counter; rp.out = p.out; rp.ok = c->d_ok;
         rp.frame_ids = p.frame_ids; rp.id_base = p.id_base; rp.row_offset = p.row_offset;
         rp.tail_smem_bytes = static_cast<uint32_t>(grid) * p.k * sizeof(uint64_t);      // <= 132 x 32 keys: no opt-in needed
@@ -995,19 +1019,19 @@ static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const 
         kernel<<<grid, 512, rp.tail_smem_bytes, stream>>>(rp);
         CUDA_TRY(cudaGetLastError());
     } else {
-    FinishParams fp{};
-    fp.corpus = e->d_corpus; fp.queries = p.query ? p.query : c->d_queries.p;
-    fp.n_rows = p.n_rows; fp.dims = e->dims; fp.n_queries = 1; fp.groups = 1; fp.slices = 1;
-    fp.kprime = kShadowNominees; fp.k = p.k; fp.metric = e->similarity;
-    fp.heaps = c->d_heaps; fp.max_norm_bits = e->d_max_norm;
-    fp.out = p.out; fp.ok = c->d_ok;
-    fp.frame_ids = p.frame_ids; fp.id_base = p.id_base; fp.row_offset = p.row_offset;
-    fp.pow2_all = 512; fp.rescore = kShadowRescore; fp.eps_rel = int8 ? e->i8.eps_rel : kBf16Eps;
-    const size_t fsmem = static_cast<size_t>(fp.pow2_all + fp.rescore) * sizeof(uint64_t);
-    const auto kernel = e->similarity == WAX_VS_COSINE ? batch_finish_kernel<kCosine> : batch_finish_kernel<kDot>;
-    CUDA_TRY(grant_smem(e, kernel, fsmem));
-    kernel<<<1, 512, fsmem, stream>>>(fp);
-    CUDA_TRY(cudaGetLastError());
+        FinishParams fp{};
+        fp.corpus = e->d_corpus; fp.queries = p.query ? p.query : c->d_queries.p;
+        fp.n_rows = p.n_rows; fp.dims = e->dims; fp.n_queries = 1; fp.groups = 1; fp.slices = 1;
+        fp.kprime = kShadowNominees; fp.k = p.k; fp.metric = e->similarity;
+        fp.heaps = c->d_heaps; fp.max_norm_bits = e->d_max_norm;
+        fp.out = p.out; fp.ok = c->d_ok;
+        fp.frame_ids = p.frame_ids; fp.id_base = p.id_base; fp.row_offset = p.row_offset;
+        fp.pow2_all = 512; fp.rescore = kShadowRescore; fp.eps_rel = sh.eps_rel;
+        const size_t fsmem = static_cast<size_t>(fp.pow2_all + fp.rescore) * sizeof(uint64_t);
+        const auto kernel = e->similarity == WAX_VS_COSINE ? batch_finish_kernel<kCosine> : batch_finish_kernel<kDot>;
+        CUDA_TRY(grant_smem(e, kernel, fsmem));
+        kernel<<<1, 512, fsmem, stream>>>(fp);
+        CUDA_TRY(cudaGetLastError());
     }
     *launches += 2;
     if (shape) {
@@ -1020,8 +1044,6 @@ static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const 
 
 static int32_t enqueue_shadow_route(wax_vs_engine *e, SearchCtx *c, ScanParams &p, cudaStream_t stream, uint64_t *launches) {
     if (!shadow_route_applies(e)) return WAX_VS_OK;
-    TmaConfig cfg{};
-    if (!pick_tma_config(e, &cfg, 1, sizeof(__nv_bfloat16))) return WAX_VS_OK;   // the unrolled shapes: both forms have them
     int32_t rc;
     if (!c->h_proof_count) {
         if ((rc = c->d_proof_count.ensure(2, "proof counts")) || (rc = c->h_proof_count.ensure(2, "proof count mirror"))) return rc;
@@ -1050,21 +1072,15 @@ static int32_t enqueue_shadow_route(wax_vs_engine *e, SearchCtx *c, ScanParams &
         demoted = e->u4_demoted > 0;
         if (demoted && --e->u4_demoted == 0) e->u4_probing = true;
     }
-    RouteForm form;
-    if ((rc = select_route_form(e, stream, demoted, &form))) return rc;
-    if (form == RouteForm::kU4) {
-        if (!pick_u4_config(e, &cfg)) return WAX_VS_OK;
-    } else if (form == RouteForm::kInt8) {
-        if (!pick_tma_config(e, &cfg, 1, 1)) return WAX_VS_OK;
-    } else {
-        if ((rc = ensure_shadow(e, stream))) return rc;
-        if (!e->shadow_valid) return WAX_VS_OK;
-    }
+    bool use = false;
+    RouteForm form = kRouteBf16;
+    TmaConfig cfg{};
+    if ((rc = select_route_form(e, stream, demoted, &use, &form, &cfg)) || !use) return rc;
     if ((rc = enqueue_shadow_nominations(e, c, p, cfg, stream, launches, nullptr, form))) return rc;
-    c->last_u4 = form == RouteForm::kU4;
-    if (form != RouteForm::kBf16) {
+    c->last_u4 = form == kRouteU4;
+    {
         std::lock_guard<std::mutex> pg(e->pool_mu);
-        ++(form == RouteForm::kU4 ? e->single_u4_queries : e->single_int8_queries);
+        ++e->single_route_queries[form];
     }
     p.proof_ok = c->d_ok;
     p.proof_count = c->d_proof_count;
@@ -1292,111 +1308,111 @@ static int32_t ensure_norms(wax_vs_engine *e, cudaStream_t stream) {
 
 // The bf16 nominations want dims % 64 == 0 (whole 128-byte k-blocks of bf16).
 static bool batch_bf16_wanted(const wax_vs_engine *e) {
-    return e->tune.batch_bf16 != 0 && e->dims % kBatchKBlockBf16 == 0 && !e->shadow_unavailable;
+    return e->tune.batch_bf16 != 0 && e->dims % kBatchKBlockBf16 == 0 && !e->shadows[kRouteBf16].unavailable;
+}
+
+// 32-bit words per row of the form-f shadow, one scale per row padded to whole scan steps (R <= 16), and the bytes of
+// `rows` rows.
+static size_t shadow_words(const wax_vs_engine *e, RouteForm f) { return e->dims * kRouteSpec[f].bits / 32; }
+static size_t shadow_scale_entries(uint64_t rows) { return static_cast<size_t>((rows + 15) / 16 * 16); }
+static size_t shadow_bytes(const wax_vs_engine *e, RouteForm f, uint64_t rows) {
+    return rows * shadow_words(e, f) * sizeof(uint32_t) + (kRouteSpec[f].scaled ? shadow_scale_entries(rows) * sizeof(float) : 0);
+}
+// Room in the form-f shadow for the live rows (what it held is given back when it is too small).  Sized for the corpus
+// CAPACITY so that appends extend it in place; if only the live rows fit, that.  It must leave max(2 GiB, 10 % of the
+// device) free for scratch and growth, and a coded shadow also what the bf16 shadow will take (see ensure_coded_shadow).
+// Allocated by hand, not through ensure(): running out here is not an error and sets no last error; the shadow is
+// marked unavailable instead.
+static int32_t alloc_shadow(wax_vs_engine *e, RouteForm f, cudaStream_t stream) {
+    wax_vs_engine::Shadow &sh = e->shadows[f];
+    const bool scaled = kRouteSpec[f].scaled;
+    const size_t words = shadow_words(e, f);
+    const uint64_t need = e->n_rows, pref = std::max<uint64_t>(e->cap_rows, e->n_rows);
+    if (sh.codes.cap >= need * words && (!scaled || sh.scale.cap >= shadow_scale_entries(need))) return WAX_VS_OK;
+    sh.release();
+    size_t free_b = 0, total_b = 0;
+    const bool info = cudaMemGetInfo(&free_b, &total_b) == cudaSuccess;
+    const size_t headroom = std::max<size_t>(size_t(2) << 30, total_b / 10);
+    size_t reserve = 0;                    // the bf16 shadow's allocation to come
+    if (f != kRouteBf16 && batch_bf16_wanted(e) && e->shadows[kRouteBf16].codes.cap < need * shadow_words(e, kRouteBf16)) {
+        const size_t b_need = shadow_bytes(e, kRouteBf16, need), b_pref = shadow_bytes(e, kRouteBf16, pref);
+        reserve = free_b >= b_pref + headroom ? b_pref : (free_b >= b_need + headroom ? b_need : 0);
+    }
+    uint64_t want = pref;
+    if (info && free_b < shadow_bytes(e, f, want) + reserve + headroom) want = need;
+    if (!info || free_b < shadow_bytes(e, f, want) + reserve + headroom ||
+        cudaMalloc(&sh.codes.p, want * words * sizeof(uint32_t)) != cudaSuccess ||
+        (scaled && cudaMalloc(&sh.scale.p, shadow_scale_entries(want) * sizeof(float)) != cudaSuccess)) {
+        cudaGetLastError();
+        sh.release();
+        sh.unavailable = true;             // stays off until its option is set again (bf16: batch_bf16)
+        return WAX_VS_OK;
+    }
+    sh.codes.cap = want * words;
+    if (scaled) {
+        sh.scale.cap = shadow_scale_entries(want);
+        CUDA_TRY(cudaMemsetAsync(sh.scale, 0, sh.scale.cap * sizeof(float), stream));   // the step padding
+    }
+    return WAX_VS_OK;
 }
 
 // bf16 shadow of the corpus (cosine: rows pre-scaled by 1/|v|), cached per corpus version and extended incrementally
-// by appends like the norms.  Returns WAX_VS_OK with e->shadow_valid == false when the extra dims*2 bytes per row do
-// not fit in HBM (the caller then nominates in TF32 from the fp32 corpus; counter "shadow_unavailable").
+// by appends like the norms.  Returns WAX_VS_OK with valid == false when the extra dims*2 bytes per row do not fit in
+// HBM (the caller then nominates in TF32 from the fp32 corpus; counter "shadow_unavailable").
 static int32_t ensure_shadow(wax_vs_engine *e, cudaStream_t stream) {
     std::lock_guard<std::mutex> g(e->norms_mu);
-    if ((e->shadow_valid && e->shadow_rows == e->n_rows) || e->shadow_unavailable) return WAX_VS_OK;
+    wax_vs_engine::Shadow &sh = e->shadows[kRouteBf16];
+    if ((sh.valid && sh.rows == e->n_rows) || sh.unavailable) return WAX_VS_OK;
     int32_t rc = ensure_norms_locked(e, stream);
-    if (rc) return rc;
-    const size_t need = static_cast<size_t>(e->n_rows) * e->dims;                                  // must hold
-    const size_t pref = static_cast<size_t>(std::max<uint64_t>(e->cap_rows, e->n_rows)) * e->dims;   // would like
-    if (e->d_shadow.cap < need) {
-        e->d_shadow.release();
-        e->shadow_rows = 0; e->shadow_valid = false;
-        size_t free_b = 0, total_b = 0;
-        size_t want = pref;
-        size_t bytes = want * sizeof(__nv_bfloat16);
-        // keep headroom for scratch and growth: the shadow must leave max(2 GiB, 10 % of the device) free.  Sized for
-        // the corpus CAPACITY so that appends extend it in place; if only the live rows fit, take that.
-        const bool info = cudaMemGetInfo(&free_b, &total_b) == cudaSuccess;
-        const size_t headroom = std::max<size_t>(size_t(2) << 30, total_b / 10);
-        if (info && free_b < bytes + headroom) { want = need; bytes = want * sizeof(__nv_bfloat16); }
-        // allocated by hand, not through ensure(): running out here is not an error and sets no last error
-        if (!info || free_b < bytes + headroom || cudaMalloc(&e->d_shadow.p, bytes) != cudaSuccess) {
-            cudaGetLastError();
-            e->shadow_unavailable = true;      // stays off for this engine: TF32 nominations need no extra memory
-            return WAX_VS_OK;
-        }
-        e->d_shadow.cap = want;
-    }
-    if (e->shadow_rows > e->n_rows) e->shadow_rows = 0;
-    const uint64_t first = e->shadow_rows, count = e->n_rows - first;
+    if (rc || (rc = alloc_shadow(e, kRouteBf16, stream)) || sh.unavailable) return rc;
+    if (sh.rows > e->n_rows) sh.rows = 0;
+    const uint64_t first = sh.rows, count = e->n_rows - first;
     if (count) {
         const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 16, (count * (e->dims / 4) + 255) / 256));
         shadow_bf16_kernel<<<std::max(grid, 1), 256, 0, stream>>>(e->d_corpus + first * e->dims,
                                                                   e->similarity == WAX_VS_COSINE ? e->d_inv_norm + first : nullptr,
-                                                                  count, e->dims, e->d_shadow + first * e->dims);
+                                                                  count, e->dims,
+                                                                  reinterpret_cast<__nv_bfloat16 *>(sh.codes.p) + first * e->dims);
         CUDA_TRY(cudaGetLastError());
     }
     CUDA_TRY(cudaStreamSynchronize(stream));
-    e->shadow_rows = e->n_rows;
-    e->shadow_valid = true;
+    sh.rows = e->n_rows;
+    sh.valid = true;
+    sh.eps_rel = kBf16Eps;                 // the bound the finish proves bf16 nominees with
     return WAX_VS_OK;
 }
 
-// int8 shadow of the corpus for the single-query route (shadow_int8_kernel; cosine rows pre-scaled by 1/|v| as in the bf16
-// shadow): built lazily, extended by appends (which can only raise rho_max), kept over a remove's untouched prefix, rebuilt
-// after overwrites; the same HBM headroom rule as ensure_shadow.  Returns WAX_VS_OK with cs.valid == false when it
-// does not fit (the route then stays on the bf16 shadow; counter "int8_shadow_bytes" = 0).  The build synchronises
-// `stream` and reads rho_max and max|v| back: eps_rel = rho_max / M rounded up (M = 1 for cosine, whose rows are
-// pre-scaled, and max|v| for dot), so that the finish's eps_rel * |q| * M is at least |q| rho_max.
-// Memory: the bf16 shadow comes first.  Unless it already holds the live rows (or was refused), the int8 shadow reserves
+// int8 (f = kRouteInt8, shadow_int8_kernel) or 4-bit (kRouteU4, shadow_u4_kernel) shadow of the corpus for the
+// single-query route (cosine rows pre-scaled by 1/|v| as in the bf16 shadow): built lazily, extended by appends (which can
+// only raise rho_max), kept over a remove's untouched prefix, rebuilt after overwrites.  Returns WAX_VS_OK with
+// valid == false when it does not fit (the route then takes another form; counter "int8_shadow_bytes" /
+// "u4_shadow_bytes" = 0).  The build synchronises `stream` and reads rho_max and max|v| back: eps_rel = rho_max / M
+// rounded up (M = 1 for cosine, whose rows are pre-scaled, and max|v| for dot), so that the finish's eps_rel * |q| * M
+// is at least |q| rho_max.
+// Memory: the bf16 shadow comes first.  Unless it already holds the live rows (or was refused), a coded shadow reserves
 // what ensure_shadow would allocate next to the same free memory -- its capacity size when that fits the headroom rule,
 // else the live rows -- so that it never leaves the bf16 shadow, and with it the route's bf16 form and the batched bf16
 // nominations, less room than they would have without it.
-// A corpus whose bound is too coarse for the route (eps_rel > kBf16Eps: outlier dimensions) gives its int8 shadow
-// back right after the build and builds none again (coarse) until its rows are rewritten: appends can only raise
-// rho_max.  keep_coarse (the read-outs) keeps such a shadow; the route never uses it.
-// The 4-bit shadow (cs.bits == 4, shadow_u4_kernel) follows the same rules with dims / 8 words per row; its bound is
-// coarser than the bf16 one by design, so only a non-finite bound makes it "coarse".
-static int32_t ensure_coded_shadow(wax_vs_engine *e, wax_vs_engine::CodedShadow &cs, cudaStream_t stream, bool keep_coarse) {
+// A corpus whose bound is too coarse for the route (above the form's max_eps_rel: for int8, outlier dimensions; the
+// 4-bit bound is coarser than the bf16 one by design, so only a non-finite one) gives its shadow back right after the
+// build and builds none again (coarse) until its rows are rewritten: appends can only raise rho_max.  keep_coarse (the
+// read-outs) keeps such a shadow; the route never uses it.
+static int32_t ensure_coded_shadow(wax_vs_engine *e, RouteForm f, cudaStream_t stream, bool keep_coarse) {
     std::lock_guard<std::mutex> g(e->norms_mu);
+    wax_vs_engine::Shadow &cs = e->shadows[f];
     if ((cs.valid && cs.rows == e->n_rows) || cs.unavailable || (cs.coarse && !keep_coarse))
         return WAX_VS_OK;
     int32_t rc = ensure_norms_locked(e, stream);
     if (rc) return rc;
     if ((rc = cs.rho.ensure(1, "coded shadow bound"))) return rc;
-    const size_t words = e->dims * cs.bits / 32;
-    const uint64_t need = e->n_rows, pref = std::max<uint64_t>(e->cap_rows, e->n_rows);
-    auto scale_entries = [](uint64_t rows) { return static_cast<size_t>((rows + 15) / 16 * 16); };   // whole steps (R <= 16)
-    if (cs.codes.cap < need * words || cs.scale.cap < scale_entries(need)) {
-        cs.release();
-        size_t free_b = 0, total_b = 0;
-        uint64_t want = pref;
-        auto bytes_for = [&](uint64_t rows) { return rows * words * sizeof(uint32_t) + scale_entries(rows) * sizeof(float); };
-        const bool info = cudaMemGetInfo(&free_b, &total_b) == cudaSuccess;
-        const size_t headroom = std::max<size_t>(size_t(2) << 30, total_b / 10);
-        size_t reserve = 0;                    // the bf16 shadow's allocation to come (see above)
-        if (batch_bf16_wanted(e) && e->d_shadow.cap < static_cast<size_t>(need) * e->dims) {
-            const size_t b_need = static_cast<size_t>(need) * e->dims * sizeof(__nv_bfloat16);
-            const size_t b_pref = static_cast<size_t>(pref) * e->dims * sizeof(__nv_bfloat16);
-            reserve = free_b >= b_pref + headroom ? b_pref : (free_b >= b_need + headroom ? b_need : 0);
-        }
-        if (info && free_b < bytes_for(want) + reserve + headroom) want = need;
-        // allocated by hand, not through ensure(): running out here is not an error and sets no last error
-        if (!info || free_b < bytes_for(want) + reserve + headroom ||
-            cudaMalloc(&cs.codes.p, want * words * sizeof(uint32_t)) != cudaSuccess ||
-            cudaMalloc(&cs.scale.p, scale_entries(want) * sizeof(float)) != cudaSuccess) {
-            cudaGetLastError();
-            cs.release();
-            cs.unavailable = true;        // stays off until int8_scan_min_bytes is set again
-            return WAX_VS_OK;
-        }
-        cs.codes.cap = want * words;
-        cs.scale.cap = scale_entries(want);
-        CUDA_TRY(cudaMemsetAsync(cs.scale, 0, scale_entries(want) * sizeof(float), stream));   // the step padding
-    }
+    if ((rc = alloc_shadow(e, f, stream)) || cs.unavailable) return rc;
+    const size_t words = shadow_words(e, f);
     if (cs.rows > e->n_rows) cs.rows = 0;
     if (cs.rows == 0) CUDA_TRY(cudaMemsetAsync(cs.rho, 0, sizeof(uint32_t), stream));
     const uint64_t first = cs.rows, count = e->n_rows - first;
     if (count) {
         const int grid = static_cast<int>(std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 8, (count + 7) / 8));
-        (cs.bits == 4 ? shadow_u4_kernel : shadow_int8_kernel)<<<std::max(grid, 1), 256, 0, stream>>>(
+        (f == kRouteU4 ? shadow_u4_kernel : shadow_int8_kernel)<<<std::max(grid, 1), 256, 0, stream>>>(
             e->d_corpus + first * e->dims, e->similarity == WAX_VS_COSINE ? e->d_inv_norm + first : nullptr, count, e->dims,
             cs.codes + first * words, cs.scale + first, cs.rho);
         CUDA_TRY(cudaGetLastError());
@@ -1416,7 +1432,7 @@ static int32_t ensure_coded_shadow(wax_vs_engine *e, wax_vs_engine::CodedShadow 
                           ? (static_cast<double>(q) * m >= rho ? q : std::nextafter(q, INFINITY)) : INFINITY;
     cs.rows = e->n_rows;
     cs.valid = true;
-    if (cs.bits == 4 ? !std::isfinite(cs.eps_rel) : cs.eps_rel > kBf16Eps) {          // too coarse for the route (above)
+    if (cs.eps_rel > kRouteSpec[f].max_eps_rel) {          // too coarse for the route (above)
         cs.coarse = true;
         if (!keep_coarse) {                    // nothing holds it: it was not valid for these rows before this call
             cs.release();
@@ -1609,7 +1625,7 @@ static int32_t enqueue_nominate_pass(wax_vs_engine *e, SearchCtx *c, const float
         ch.stages = ch.ares ? ares_st : batch_ring_stages(static_cast<int>(ch.kprime));
         // bf16: the converted queries against the corpus shadow; TF32: the fp32 queries against the corpus
         const void *qbase = bf16 ? static_cast<const void *>(c->d_queries_bf16 + static_cast<size_t>(q0) * e->dims) : ch.queries;
-        const void *cbase = bf16 ? static_cast<const void *>(e->d_shadow.p) : e->d_corpus;
+        const void *cbase = bf16 ? static_cast<const void *>(e->shadows[kRouteBf16].codes.p) : e->d_corpus;
         CUtensorMap map_q, map_c;
         if ((rc = make_tensor_map(&map_q, qbase, ch.nq, e->dims, kBatchM, bf16))) return rc;
         if ((rc = make_tensor_map(&map_c, cbase, e->n_rows, e->dims, ch.pair ? kBatchN / 2 : kBatchN, bf16))) return rc;
@@ -1656,7 +1672,7 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
     bool bf16 = allow_bf16 && batch_bf16_wanted(e);
     if (bf16) {
         if ((rc = ensure_shadow(e, stream))) return rc;
-        bf16 = e->shadow_valid;
+        bf16 = e->shadows[kRouteBf16].valid;
     }
     if (used_bf16) *used_bf16 = bf16;
     // k > 128: the union of the slices' 64-entry heaps must hold k nominees with some room (slices >= 1.15 k / 64), so
@@ -1738,14 +1754,10 @@ static int32_t set_capacity(wax_vs_engine *e, uint64_t rows) {
     float *n = nullptr;
     const size_t bytes = static_cast<size_t>(rows) * e->dims * sizeof(float);
     if (cudaMalloc(&n, bytes) != cudaSuccess) {
-        // the bf16 shadow is derived data: give its HBM back before giving up (mutators hold the write lock)
+        // the shadows are derived data: give their HBM back before giving up (mutators hold the write lock)
         cudaGetLastError();
-        if (e->d_shadow) {
-            e->d_shadow.release(); e->shadow_valid = false; e->shadow_rows = 0;
-            e->shadow_unavailable = true;
-        }
-        for (auto *cs : {&e->i8, &e->u4})      // likewise the int8 and 4-bit shadows
-            if (cs->codes) { cs->release(); cs->unavailable = true; }
+        for (auto &sh : e->shadows)
+            if (sh.codes) { sh.release(); sh.unavailable = true; }
         if (cudaMalloc(&n, bytes) != cudaSuccess)
             return fail(WAX_VS_ERR_CUDA, "Failed to resize vectors buffer (%zu bytes): %s", bytes,
                         cudaGetErrorString(cudaGetLastError()));
@@ -4979,11 +4991,12 @@ int32_t wax_vs_debug_time_search(wax_vs_engine *e, uint32_t n_queries, int64_t t
         if ((rc = lease2.c->d_out.ensure(static_cast<size_t>(n_queries) * k_eff, "result buffer"))) return rc;
     }
     SearchCtx *c2 = lease2.c;
-    // the shadow route's int8 or bf16 copy is cached per corpus version: bring it up to date outside the timed region
+    // the shadow the route takes is cached per corpus version: bring it up to date outside the timed region
     if (shadow_route_applies(e)) {
-        RouteForm form;
-        if ((rc = select_route_form(e, c->stream, false, &form))) return rc;
-        if (form == RouteForm::kBf16 && (rc = ensure_shadow(e, c->stream))) return rc;
+        bool use = false;
+        RouteForm form = kRouteBf16;
+        TmaConfig cfg{};
+        if ((rc = select_route_form(e, c->stream, false, &use, &form, &cfg))) return rc;
     }
     for (uint32_t it = 0; it < warmup + iters; ++it) {
         if (it == warmup) {
@@ -5128,14 +5141,15 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *e, uint64_t *tensor_queries, uin
 int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) {
     if (!e || !name || !out) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::lock_guard<std::mutex> g(e->pool_mu);
+    const wax_vs_engine::Shadow &bf = e->shadows[kRouteBf16], &i8 = e->shadows[kRouteInt8], &u4 = e->shadows[kRouteU4];
     if (!strcmp(name, "batch_tensor_queries")) *out = e->batch_tensor_queries;
     else if (!strcmp(name, "batch_fallback_queries")) *out = e->batch_fallback_queries;
     else if (!strcmp(name, "batch_bf16_queries")) *out = e->batch_bf16_queries;
     else if (!strcmp(name, "batch_retry_queries")) *out = e->batch_retry_queries;               // TF32 filter level
     else if (!strcmp(name, "batch_filter_bf16_queries")) *out = e->batch_filter_bf16_queries;   // bf16-shadow filter level
-    else if (!strcmp(name, "shadow_bytes")) *out = e->shadow_valid ? e->shadow_rows * e->dims * sizeof(__nv_bfloat16) : 0;   // live rows
-    else if (!strcmp(name, "shadow_capacity_bytes")) *out = e->d_shadow.cap * sizeof(__nv_bfloat16);                          // HBM held
-    else if (!strcmp(name, "shadow_unavailable")) *out = e->shadow_unavailable ? 1 : 0;   // bf16 shadow did not fit: TF32 level runs
+    else if (!strcmp(name, "shadow_bytes")) *out = bf.valid ? bf.rows * e->dims * sizeof(__nv_bfloat16) : 0;   // live rows
+    else if (!strcmp(name, "shadow_capacity_bytes")) *out = bf.codes.cap * sizeof(uint32_t);                   // HBM held
+    else if (!strcmp(name, "shadow_unavailable")) *out = bf.unavailable ? 1 : 0;   // bf16 shadow did not fit: TF32 level runs
     else if (!strcmp(name, "batch_tf32_queries")) *out = e->batch_tf32_queries;
     else if (!strcmp(name, "filter_bitset_passes")) *out = e->filter_bitset_passes;   // per-query filters: tensor sub-batches
     else if (!strcmp(name, "group_index_builds")) *out = e->group_index_builds;       // grouped search: device index builds
@@ -5151,13 +5165,13 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "ingest_h2d_bytes")) *out = e->ingest_h2d_bytes;
     else if (!strcmp(name, "ingest_d2h_bytes")) *out = e->ingest_d2h_bytes;
     else if (!strcmp(name, "norms_rows")) *out = e->norms_rows;       // rows whose cached 1/|v| is valid
-    else if (!strcmp(name, "shadow_rows")) *out = e->shadow_rows;     // rows whose bf16 shadow is valid
-    else if (!strcmp(name, "int8_shadow_bytes")) *out = e->i8.valid ? e->i8.rows * (e->dims + sizeof(float)) : 0;   // codes + scales
-    else if (!strcmp(name, "int8_shadow_rows")) *out = e->i8.rows;  // rows whose int8 shadow is valid
-    else if (!strcmp(name, "u4_shadow_bytes")) *out = e->u4.valid ? e->u4.rows * (e->dims / 2 + sizeof(float)) : 0;
-    else if (!strcmp(name, "u4_shadow_rows")) *out = e->u4.rows;
-    else if (!strcmp(name, "single_u4_queries")) *out = e->single_u4_queries;
-    else if (!strcmp(name, "single_int8_queries")) *out = e->single_int8_queries;   // single queries nominated from it
+    else if (!strcmp(name, "shadow_rows")) *out = bf.rows;     // rows whose bf16 shadow is valid
+    else if (!strcmp(name, "int8_shadow_bytes")) *out = i8.valid ? i8.rows * (e->dims + sizeof(float)) : 0;   // codes + scales
+    else if (!strcmp(name, "int8_shadow_rows")) *out = i8.rows;  // rows whose int8 shadow is valid
+    else if (!strcmp(name, "u4_shadow_bytes")) *out = u4.valid ? u4.rows * (e->dims / 2 + sizeof(float)) : 0;
+    else if (!strcmp(name, "u4_shadow_rows")) *out = u4.rows;
+    else if (!strcmp(name, "single_u4_queries")) *out = e->single_route_queries[kRouteU4];
+    else if (!strcmp(name, "single_int8_queries")) *out = e->single_route_queries[kRouteInt8];   // single queries nominated from it
     else if (!strcmp(name, "batch_heap_bump")) *out = e->heap_bump;          // sizes above the model's nominee-heap choice (adaptive)
     else if (!strcmp(name, "batch_last_heap")) *out = e->last_heap;          // nominee heap entries of the last bf16 level-1 launch
     else if (!strcmp(name, "single_shadow_queries") || !strcmp(name, "single_shadow_fallbacks")) {
@@ -5276,31 +5290,25 @@ int32_t wax_vs_debug_batch_nominations(wax_vs_engine *e, const float *queries, u
 static int32_t debug_route_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
                                        uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
                                        uint32_t *out_shape, RouteForm form, uint64_t keys_cap = 0, float *out_bound = nullptr) {
-    const bool u4 = form == RouteForm::kU4, int8 = form != RouteForm::kBf16;     // int8: a coded shadow
-    if (!e || !query || !out_keys || !out_ok || !out_result || !out_shape || (u4 && !out_bound))
+    const RouteFormSpec &fs = kRouteSpec[form];
+    if (!e || !query || !out_keys || !out_ok || !out_result || !out_shape || (fs.grid_rescore && !out_bound))
         return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     const uint32_t k_eff = static_cast<uint32_t>(std::min<uint64_t>(clamp_topk(top_k), std::max<uint64_t>(e->n_rows, 1)));
     TmaConfig cfg{};
+    // (the coded forms also where the bf16 shadow did not fit, as in the route)
     if (e->n_rows == 0 || k_eff > 32u || (e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT) ||
-        (int8 ? (e->tune.batch_bf16 == 0 || e->dims % kBatchKBlockBf16 != 0) : !batch_bf16_wanted(e)) ||
-        !(u4 ? pick_u4_config(e, &cfg) : pick_tma_config(e, &cfg, 1, int8 ? 1 : sizeof(__nv_bfloat16))))
-        return fail(WAX_VS_ERR_UNSUPPORTED, "no %s-shadow route for k=%u, dims=%u in this shape",
-                    u4 ? "4-bit" : int8 ? "int8" : "bf16", k_eff, e->dims);
+        e->tune.batch_bf16 == 0 || e->dims % kBatchKBlockBf16 != 0 ||
+        (form == kRouteBf16 && e->shadows[kRouteBf16].unavailable) || !pick_route_config(e, form, &cfg))
+        return fail(WAX_VS_ERR_UNSUPPORTED, "no %s-shadow route for k=%u, dims=%u in this shape", fs.name, k_eff, e->dims);
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
     CtxLease lease(e);
     int32_t rc = lease.acquire();
     if (rc) return rc;
     SearchCtx *c = lease.c;
-    if (int8) {
-        wax_vs_engine::CodedShadow &cs = u4 ? e->u4 : e->i8;
-        if ((rc = ensure_coded_shadow(e, cs, c->stream, true))) return rc;
-        if (!cs.valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the coded shadow does not fit in device memory");
-    } else {
-        if ((rc = ensure_shadow(e, c->stream))) return rc;
-        if (!e->shadow_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the bf16 shadow does not fit in device memory");
-    }
+    if ((rc = ensure_route_shadow(e, form, c->stream, true))) return rc;
+    if (!e->shadows[form].valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the %s shadow does not fit in device memory", fs.name);
     if ((rc = c->d_out.ensure(k_eff, "result buffer"))) return rc;
     const uint32_t *d_mask = nullptr;
     if (allow_bits) {
@@ -5317,7 +5325,7 @@ static int32_t debug_route_nominations(wax_vs_engine *e, const float *query, int
         return rc;
     }
     CUDA_TRY(cudaStreamSynchronize(c->stream));
-    if (u4) {
+    if (fs.grid_rescore) {
         const uint64_t n_keys = static_cast<uint64_t>(out_shape[4]) * kU4CtaNominees;
         if (keys_cap < n_keys)
             return fail(WAX_VS_ERR_BUFFER, "the nominees need %llu entries (%llu given)", static_cast<unsigned long long>(n_keys),
@@ -5325,14 +5333,15 @@ static int32_t debug_route_nominations(wax_vs_engine *e, const float *query, int
         CUDA_TRY(cudaMemcpy(out_keys, c->d_heaps, n_keys * sizeof(uint64_t), cudaMemcpyDeviceToHost));
         uint32_t aux[3];
         CUDA_TRY(cudaMemcpy(aux, c->d_u4_aux, sizeof aux, cudaMemcpyDeviceToHost));
-        out_bound[0] = e->u4.rho_max;
+        out_bound[0] = e->shadows[form].rho_max;
         memcpy(out_bound + 1, &aux[1], sizeof(float));
         // the cut word as a score: -inf when no row was left out
         if (aux[2] == 0xFFFFFFFFu) out_bound[2] = -INFINITY;
         else { const uint32_t u = aux[2] ^ ((aux[2] & 0x80000000u) ? 0x80000000u : 0xFFFFFFFFu); float f; memcpy(&f, &u, 4); out_bound[2] = -f; }
-    } else
-    CUDA_TRY(cudaMemcpy2D(out_keys, sizeof(uint64_t), c->d_heaps, kNomineeStride * sizeof(uint64_t), sizeof(uint64_t),
-                          kShadowNominees, cudaMemcpyDeviceToHost));
+    } else {
+        CUDA_TRY(cudaMemcpy2D(out_keys, sizeof(uint64_t), c->d_heaps, kNomineeStride * sizeof(uint64_t), sizeof(uint64_t),
+                              kShadowNominees, cudaMemcpyDeviceToHost));
+    }
     CUDA_TRY(cudaMemcpy(out_ok, c->d_ok, sizeof(uint32_t), cudaMemcpyDeviceToHost));
     CUDA_TRY(cudaMemcpy(out_result, c->d_out, k_eff * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost));
     for (uint32_t i = 0; i < k_eff; ++i)
@@ -5343,82 +5352,66 @@ static int32_t debug_route_nominations(wax_vs_engine *e, const float *query, int
 int32_t wax_vs_debug_shadow_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
                                         uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
                                         uint32_t *out_shape) {
-    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, RouteForm::kBf16);
+    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, kRouteBf16);
 }
 
 int32_t wax_vs_debug_int8_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
                                       uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
                                       uint32_t *out_shape) {
-    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, RouteForm::kInt8);
+    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, kRouteInt8);
 }
 
 int32_t wax_vs_debug_u4_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
                                     uint64_t *out_keys, uint64_t keys_cap, uint32_t *out_ok, wax_vs_candidate *out_result,
                                     uint32_t *out_shape, float *out_bound) {
-    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, RouteForm::kU4,
+    return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, kRouteU4,
                                    keys_cap, out_bound);
+}
+
+// wax_vs_debug_read_shadow, wax_vs_debug_read_int8_shadow and wax_vs_debug_read_u4_shadow: rows [first, first + n) of the
+// form-f shadow, brought up to date first -- the stored codes, and for the coded forms each row's scale and rho_max.  The
+// bf16 shadow is read out whenever the engine keeps one, a coded one where the route could take its form.
+static int32_t debug_read_route_shadow(wax_vs_engine *e, RouteForm f, uint64_t first, uint64_t n, void *dst_codes,
+                                       float *dst_scales, float *out_rho_max) {
+    const RouteFormSpec &fs = kRouteSpec[f];
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
+    TmaConfig cfg{};
+    if (f == kRouteBf16 ? !batch_bf16_wanted(e)
+                        : (e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT) || !pick_route_config(e, f, &cfg))
+        return fail(WAX_VS_ERR_UNSUPPORTED, "no %s shadow for dims=%u with this metric and these options", fs.name, e->dims);
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    CtxLease lease(e);
+    int32_t rc = lease.acquire();
+    if (rc) return rc;
+    if ((rc = ensure_route_shadow(e, f, lease.c->stream, true))) return rc;
+    const wax_vs_engine::Shadow &sh = e->shadows[f];
+    if (!sh.valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the %s shadow does not fit in device memory", fs.name);
+    const size_t words = shadow_words(e, f);
+    if (n) {
+        CUDA_TRY(cudaMemcpy(dst_codes, sh.codes + first * words, n * words * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+        if (fs.scaled) CUDA_TRY(cudaMemcpy(dst_scales, sh.scale + first, n * sizeof(float), cudaMemcpyDeviceToHost));
+    }
+    if (fs.scaled) *out_rho_max = sh.rho_max;
+    return WAX_VS_OK;
 }
 
 int32_t wax_vs_debug_read_u4_shadow(wax_vs_engine *e, uint64_t first, uint64_t n, uint8_t *dst_codes, float *dst_half_steps,
                                     float *out_rho_max) {
     if (!e || !dst_codes || !dst_half_steps || !out_rho_max) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    std::shared_lock<std::shared_mutex> r(e->rw);
-    if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
-    TmaConfig cfg{};
-    if ((e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT) || !pick_u4_config(e, &cfg))
-        return fail(WAX_VS_ERR_UNSUPPORTED, "no 4-bit shadow for dims=%u with this metric", e->dims);
-    DeviceGuard g(e->device);
-    if (!g.ok) return g.error();
-    CtxLease lease(e);
-    int32_t rc = lease.acquire();
-    if (rc) return rc;
-    if ((rc = ensure_coded_shadow(e, e->u4, lease.c->stream, true))) return rc;
-    if (!e->u4.valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the 4-bit shadow does not fit in device memory");
-    if (n) {
-        CUDA_TRY(cudaMemcpy(dst_codes, e->u4.codes + first * (e->dims / 8), n * e->dims / 2, cudaMemcpyDeviceToHost));
-        CUDA_TRY(cudaMemcpy(dst_half_steps, e->u4.scale + first, n * sizeof(float), cudaMemcpyDeviceToHost));
-    }
-    *out_rho_max = e->u4.rho_max;
-    return WAX_VS_OK;
+    return debug_read_route_shadow(e, kRouteU4, first, n, dst_codes, dst_half_steps, out_rho_max);
 }
 
 int32_t wax_vs_debug_read_int8_shadow(wax_vs_engine *e, uint64_t first, uint64_t n, uint8_t *dst_codes, float *dst_scales,
                                       float *out_rho_max) {
     if (!e || !dst_codes || !dst_scales || !out_rho_max) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    std::shared_lock<std::shared_mutex> r(e->rw);
-    if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
-    TmaConfig cfg{};
-    if ((e->similarity != WAX_VS_COSINE && e->similarity != WAX_VS_DOT) || !pick_tma_config(e, &cfg, 1, 1))
-        return fail(WAX_VS_ERR_UNSUPPORTED, "no int8 shadow for dims=%u with this metric", e->dims);
-    DeviceGuard g(e->device);
-    if (!g.ok) return g.error();
-    CtxLease lease(e);
-    int32_t rc = lease.acquire();
-    if (rc) return rc;
-    if ((rc = ensure_coded_shadow(e, e->i8, lease.c->stream, true))) return rc;
-    if (!e->i8.valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the int8 shadow does not fit in device memory");
-    if (n) {
-        CUDA_TRY(cudaMemcpy(dst_codes, e->i8.codes + first * (e->dims / 4), n * e->dims, cudaMemcpyDeviceToHost));
-        CUDA_TRY(cudaMemcpy(dst_scales, e->i8.scale + first, n * sizeof(float), cudaMemcpyDeviceToHost));
-    }
-    *out_rho_max = e->i8.rho_max;
-    return WAX_VS_OK;
+    return debug_read_route_shadow(e, kRouteInt8, first, n, dst_codes, dst_scales, out_rho_max);
 }
 
 int32_t wax_vs_debug_read_shadow(wax_vs_engine *e, uint64_t first, uint64_t n, uint16_t *dst) {
     if (!e || !dst) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    std::shared_lock<std::shared_mutex> r(e->rw);
-    if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
-    if (!batch_bf16_wanted(e)) return fail(WAX_VS_ERR_UNSUPPORTED, "no bf16 shadow for dims=%u with these options", e->dims);
-    DeviceGuard g(e->device);
-    if (!g.ok) return g.error();
-    CtxLease lease(e);
-    int32_t rc = lease.acquire();
-    if (rc) return rc;
-    if ((rc = ensure_shadow(e, lease.c->stream))) return rc;
-    if (!e->shadow_valid) return fail(WAX_VS_ERR_UNSUPPORTED, "the bf16 shadow does not fit in device memory");
-    if (n) CUDA_TRY(cudaMemcpy(dst, e->d_shadow + first * e->dims, n * e->dims * sizeof(__nv_bfloat16), cudaMemcpyDeviceToHost));
-    return WAX_VS_OK;
+    return debug_read_route_shadow(e, kRouteBf16, first, n, dst, nullptr, nullptr);
 }
 
 int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value) {
@@ -5441,7 +5434,7 @@ int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value
     else if (!strcmp(key, "tma_max_dims")) e->tune.tma_max_dims = static_cast<uint32_t>(std::max(v, 0));
     else if (!strcmp(key, "batch_pair")) e->tune.batch_pair = v;
     else if (!strcmp(key, "batch_ares")) e->tune.batch_ares = v;
-    else if (!strcmp(key, "batch_bf16")) { e->tune.batch_bf16 = v; e->shadow_unavailable = false; e->bf16_skip_batches = 0; }
+    else if (!strcmp(key, "batch_bf16")) { e->tune.batch_bf16 = v; e->shadows[kRouteBf16].unavailable = false; e->bf16_skip_batches = 0; }
     else if (!strcmp(key, "batch_rescore")) e->tune.batch_rescore = v;
     else if (!strcmp(key, "batch_retry")) e->tune.batch_retry = v;
     else if (!strcmp(key, "filter_cap")) e->tune.filter_cap = v;
@@ -5457,27 +5450,27 @@ int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value
         for (SearchCtx *c : e->pool) seen(c);
         for (auto &kv : e->stream_ctx) seen(kv.second);
     }
-    else if (!strcmp(key, "shadow_rows_per_step")) e->tune.shadow_rows_per_step = v;
-    else if (!strcmp(key, "shadow_warps")) e->tune.shadow_warps = v;
-    else if (!strcmp(key, "shadow_stages")) e->tune.shadow_stages = v;
-    else if (!strcmp(key, "shadow_scan_min_bytes")) e->tune.shadow_scan_min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
+    else if (!strcmp(key, "shadow_rows_per_step")) e->tune.route[kRouteBf16].rows_per_step = v;
+    else if (!strcmp(key, "shadow_warps")) e->tune.route[kRouteBf16].warps = v;
+    else if (!strcmp(key, "shadow_stages")) e->tune.route[kRouteBf16].stages = v;
+    else if (!strcmp(key, "shadow_scan_min_bytes")) e->tune.route[kRouteBf16].min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
     else if (!strcmp(key, "int8_scan_min_bytes")) {     // also lets an int8 shadow that did not fit be tried again
-        e->tune.int8_scan_min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
-        e->i8.unavailable = false;
-        e->i8.coarse = false;
+        e->tune.route[kRouteInt8].min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
+        e->shadows[kRouteInt8].unavailable = false;
+        e->shadows[kRouteInt8].coarse = false;
     }
     else if (!strcmp(key, "u4_scan_min_bytes")) {       // also retries a 4-bit shadow that did not fit, and ends a demotion
-        e->tune.u4_scan_min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
-        e->u4.unavailable = false;
-        e->u4.coarse = false;
+        e->tune.route[kRouteU4].min_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
+        e->shadows[kRouteU4].unavailable = false;
+        e->shadows[kRouteU4].coarse = false;
         e->u4_demoted = 0; e->u4_demote_window = 16; e->u4_probing = false;
     }
-    else if (!strcmp(key, "u4_rows_per_step")) e->tune.u4_rows_per_step = v;
-    else if (!strcmp(key, "u4_warps")) e->tune.u4_warps = v;
-    else if (!strcmp(key, "u4_stages")) e->tune.u4_stages = v;
-    else if (!strcmp(key, "int8_rows_per_step")) e->tune.int8_rows_per_step = v;
-    else if (!strcmp(key, "int8_warps")) e->tune.int8_warps = v;
-    else if (!strcmp(key, "int8_stages")) e->tune.int8_stages = v;
+    else if (!strcmp(key, "u4_rows_per_step")) e->tune.route[kRouteU4].rows_per_step = v;
+    else if (!strcmp(key, "u4_warps")) e->tune.route[kRouteU4].warps = v;
+    else if (!strcmp(key, "u4_stages")) e->tune.route[kRouteU4].stages = v;
+    else if (!strcmp(key, "int8_rows_per_step")) e->tune.route[kRouteInt8].rows_per_step = v;
+    else if (!strcmp(key, "int8_warps")) e->tune.route[kRouteInt8].warps = v;
+    else if (!strcmp(key, "int8_stages")) e->tune.route[kRouteInt8].stages = v;
     else if (!strcmp(key, "shard_fused")) e->tune.shard_fused = v;
     else if (!strcmp(key, "tail_select")) e->tune.tail_select = v;
     else if (!strcmp(key, "inline_query")) e->tune.inline_query = v;
