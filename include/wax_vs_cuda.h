@@ -211,7 +211,7 @@ int32_t wax_vs_set_groups(wax_vs_engine *engine, const uint64_t *frame_ids, cons
    entry i.  out_cap >= min(clamp(top_groups) * per_group, N) else WAX_VS_ERR_BUFFER.  Checked before the empty-engine
    early return: per_group == 0, per_group > WAX_VS_MAX_PER_GROUP, clamp(top_groups) * per_group > WAX_VS_MAX_RESULTS or
    a mode other than 0 / 1 -> WAX_VS_ERR_ARGUMENT; a NULL output, or NULL frame_ids with n_ids > 0 -> WAX_VS_ERR_NULL.
-   The first grouped search after a mutation or wax_vs_set_groups builds a device group index (about 12 bytes per row,
+   The first grouped search after a mutation or wax_vs_set_groups builds a device group index (at most 20 bytes per row,
    counter "group_index_builds"); later ones reuse it. */
 int32_t wax_vs_search_grouped(wax_vs_engine *engine, const float *query, uint32_t query_len, int64_t top_groups,
                               uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
@@ -515,6 +515,57 @@ int32_t wax_vs_search_batch_where_device(wax_vs_engine *engine, const float *d_q
                                          const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
                                          const uint64_t *where_term_offsets, const uint64_t *where_terms,
                                          uint64_t row_offset, wax_vs_candidate *d_candidates, void *cuda_stream);
+
+/* ---- sharded grouped search: wax_vs_search_batch_grouped_multi_where over the row-sharded engine ------------------
+   Exact, in two exchanges of any transport (wax_b200/sharded.py).  G = clamp(top_groups), P = per_group.
+   Round 1: every rank's own grouped answer (wax_vs_shard_grouped_heads_device), all-gathered.
+   Merge 1: the global top G groups by their best rows (wax_vs_merge_group_heads_device).  P == 1 ends here.
+   Round 2: every rank's P best rows of each chosen group (wax_vs_shard_grouped_expand_device), all-gathered and merged
+   per (query, group) by wax_vs_merge_candidates_device(world, n_queries * G, P, P).
+   Each entry point uses the caller's stream and may synchronise it. */
+typedef struct wax_vs_group_candidate {   /* 32 bytes, naturally aligned */
+    float distance;     /* as wax_vs_candidate                                   */
+    uint32_t valid;     /* 1 = real row, 0 = padding (all fields zero)           */
+    uint64_t row;       /* global row = row_offset + local row                   */
+    uint64_t frame_id;
+    uint64_t group_id;
+} wax_vs_group_candidate;
+#define WAX_VS_SHARD_MAX_GROUPS 256        /* clamp(top_groups) of the sharded grouped form */
+/* Round 1.  d_heads = [n_queries][G][P] on the device: query i's answer of wax_vs_search_batch_grouped_multi_where on
+   this engine alone (same batch, wheres and id filters), group-major, groups best first, rows best first, with global
+   rows.  Padding has valid = 0 and is zeroed; an empty shard writes only padding.  Checked before the empty-engine early
+   return: the checks of wax_vs_search_batch_grouped_multi_where; clamp(top_groups) > WAX_VS_SHARD_MAX_GROUPS ->
+   WAX_VS_ERR_UNSUPPORTED; NULL d_queries or d_heads -> WAX_VS_ERR_NULL.  n_queries == 0 returns OK. */
+int32_t wax_vs_shard_grouped_heads_device(wax_vs_engine *engine, const float *d_queries, uint32_t n_queries,
+                                          int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids,
+                                          const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                          const uint32_t *query_filter, const wax_vs_where_near *wheres, uint32_t n_wheres,
+                                          const uint32_t *query_where, uint64_t row_offset, wax_vs_group_candidate *d_heads,
+                                          void *cuda_stream);
+/* Merge 1.  d_gathered = [world][n_queries][G][P], the ranks' d_heads in rank order (ascending row ranges) as an
+   all-gather leaves them.  d_chosen = [n_queries][G]: per query the union of the ranks' group heads (a group's first
+   row), the best head kept per group id, the first G by (distance, global row); padding (valid = 0, zeroed) last.  These
+   are the global top G groups, each as its best row.  world outside 1..WAX_VS_SHARD_MAX_RANKS, per_group outside
+   1..WAX_VS_MAX_PER_GROUP -> WAX_VS_ERR_ARGUMENT; clamp(top_groups) > WAX_VS_SHARD_MAX_GROUPS -> WAX_VS_ERR_UNSUPPORTED;
+   NULL pointers -> WAX_VS_ERR_NULL. */
+int32_t wax_vs_merge_group_heads_device(wax_vs_engine *engine, const wax_vs_group_candidate *d_gathered, uint32_t world,
+                                        uint32_t n_queries, int64_t top_groups, uint32_t per_group,
+                                        wax_vs_group_candidate *d_chosen, void *cuda_stream);
+/* Round 2.  d_rows = [n_queries][G][P] wax_vs_candidate: slot (i, s) holds this shard's best min(P, rows) rows of group
+   d_chosen[i][s] under query i's where and id filter, sorted by (distance, global row), padding last and zeroed.  A
+   group this rank listed in round 1 (d_own_heads, its own d_heads) is copied from there; a group it holds but did not
+   list is scored over its rows (counter "shard_grouped_expanded_groups"); any other slot is padding.  The filters and
+   wheres must be those of round 1.  The checks of wax_vs_shard_grouped_heads_device, and NULL d_chosen, d_own_heads or
+   d_rows -> WAX_VS_ERR_NULL, run before the empty-engine early return. */
+int32_t wax_vs_shard_grouped_expand_device(wax_vs_engine *engine, const float *d_queries, uint32_t n_queries,
+                                           int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids,
+                                           const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                           const uint32_t *query_filter, const wax_vs_where_near *wheres,
+                                           uint32_t n_wheres, const uint32_t *query_where,
+                                           const wax_vs_group_candidate *d_chosen,
+                                           const wax_vs_group_candidate *d_own_heads, uint64_t row_offset,
+                                           wax_vs_candidate *d_rows, void *cuda_stream);
+
 /* Device-resident form: d_query (dims floats) and d_candidates (clamp(top_k) merged entries, padding valid = 0) are
    device pointers; enqueued on `cuda_stream`, returns without synchronising. */
 int32_t wax_vs_shard_search_device(wax_vs_engine *engine, const float *d_query, int64_t top_k,

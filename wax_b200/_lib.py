@@ -21,6 +21,7 @@ NO_FILTER = 0xFFFFFFFF          # WAX_VS_NO_FILTER: a query of wax_vs_search_bat
 MAX_DIMENSIONS = 1_000_000
 MAX_PER_GROUP = 128             # WAX_VS_MAX_PER_GROUP: rows per group of wax_vs_search_grouped
 SHARD_HANDLE_BYTES, SHARD_MAX_RANKS, SHARD_MAX_K = 128, 16, 128
+SHARD_MAX_GROUPS = 256          # WAX_VS_SHARD_MAX_GROUPS: clamp(top_groups) of the sharded grouped search
 INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1   # wax_vs_where bounds meaning "no bound"
 
 
@@ -100,6 +101,15 @@ SIGNATURES = {
     "wax_vs_search_batch_where_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, _u64p, _u64p,
                                                      C.POINTER(C.c_int32), C.c_uint32, _u32p, C.c_void_p, C.c_uint32, _u32p,
                                                      _u64p, _u64p, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "wax_vs_shard_grouped_heads_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, C.c_uint32, _u64p, _u64p,
+                                                      C.POINTER(C.c_int32), C.c_uint32, _u32p, C.c_void_p, C.c_uint32,
+                                                      _u32p, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "wax_vs_merge_group_heads_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_uint32, C.c_int64, C.c_uint32,
+                                                    C.c_void_p, C.c_void_p]),
+    "wax_vs_shard_grouped_expand_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, C.c_uint32, _u64p, _u64p,
+                                                       C.POINTER(C.c_int32), C.c_uint32, _u32p, C.c_void_p, C.c_uint32,
+                                                       _u32p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
+                                                       C.c_void_p]),
     "wax_vs_search_batch": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _f32p,
                                         C.c_uint32, _u32p]),
     "wax_vs_search_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, C.c_uint64, C.c_void_p,

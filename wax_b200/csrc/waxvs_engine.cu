@@ -362,10 +362,12 @@ struct wax_vs_engine {
     bool groups_set = false;
     std::vector<uint64_t> groups;
     // Device group index for grouped search (waxvs_group.cuh), cached per corpus version and grouping: rows sorted by
-    // (group id, row) as perm + starts, and each row's dense group.  Every mutator and set_groups invalidate it; the first
-    // grouped search after that rebuilds it under group_mu (concurrent readers hold only the read lock).
+    // (group id, row) as perm + starts, each row's dense group and each dense group's id (ascending: the sharded grouped
+    // search looks groups up by id).  Every mutator and set_groups invalidate it; the first grouped search after that
+    // rebuilds it under group_mu (concurrent readers hold only the read lock).
     struct GroupIndex {
         DevBuf<uint32_t> perm, row_group, starts;
+        DevBuf<uint64_t> ids;
         uint32_t n_groups = 0;
         bool valid = false;
     } gindex;
@@ -432,6 +434,7 @@ struct wax_vs_engine {
     uint64_t term_index_builds = 0;    // instrumentation (pool_mu)
     uint64_t grouped_batch_covered_queries = 0, grouped_batch_expanded_groups = 0, grouped_batch_fallback_queries = 0;
     uint64_t grouped_batch_expansion_passes = 0;
+    uint64_t shard_grouped_expanded_groups = 0;
     // Adaptive level choice: when more than a quarter of a batch fails the coarse bf16 bound (tightly clustered
     // neighbours), the next 16 batches nominate in TF32 straight away, then bf16 is probed again.
     uint32_t bf16_skip_batches = 0;
@@ -3238,6 +3241,19 @@ static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const int32_t *fi
     return WAX_VS_OK;
 }
 
+// The filters' rows into c->d_filter_rows on c->stream, where build_pass_bits and the gather class read them: the
+// host-listed rows, then the rows the device lists (narrow where units, narrow term units).
+static int32_t stage_pair_rows(wax_vs_engine *e, SearchCtx *c, const FilterSet &fs, uint64_t *launches) {
+    int32_t rc;
+    if ((rc = stage_filter_rows(e, c, fs.rows, fs.rows.size() + fs.device_rows, -1, c->stream, nullptr))) return rc;
+    if ((rc = list_where_rows(e, c, fs.compact, c->stream, launches)) ||
+        (rc = launch_term_filter(e, c, fs.term_list, c->d_filter_rows, nullptr, c->stream, launches))) {
+        cudaStreamSynchronize(c->stream);
+        return rc;
+    }
+    return WAX_VS_OK;
+}
+
 // What run_filtered's candidates carry and where they go.  The defaults serve the host entry points, which map local rows
 // to frame ids themselves.  A shard reports global rows (row_offset + local row) and its frame ids (d_ids, nullptr for
 // identity ids); the device form's queries are on the device; the collective form (one query) exchanges its list with
@@ -3255,7 +3271,7 @@ struct FilteredTarget {
 static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries, const int32_t *filter_modes,
                             uint32_t n_filters, const uint32_t *query_filter, const FilterSet &fs, const FilteredPlan &plan,
                             const FilteredTarget &tgt = FilteredTarget{}) {
-    const std::vector<uint32_t> &order = plan.order, &k_of = plan.k_of, &rows = fs.rows;
+    const std::vector<uint32_t> &order = plan.order, &k_of = plan.k_of;
     const std::vector<uint64_t> &first = fs.first, &count = fs.count;
     const uint32_t k_max = plan.k_max, n_tensor = plan.n_tensor, n_gather = plan.n_gather;
     const uint32_t n_staged = static_cast<uint32_t>(order.size());
@@ -3276,13 +3292,8 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
         return rc;
     }
     if ((rc = c->d_out.ensure(ncand, "result buffer"))) return rc;
-    if ((rc = stage_filter_rows(e, c, rows, rows.size() + fs.device_rows, -1, c->stream, nullptr))) return rc;
     uint64_t launches = 0;
-    if ((rc = list_where_rows(e, c, fs.compact, c->stream, &launches)) ||
-        (rc = launch_term_filter(e, c, fs.term_list, c->d_filter_rows, nullptr, c->stream, &launches))) {
-        cudaStreamSynchronize(c->stream);
-        return rc;
-    }
+    if ((rc = stage_pair_rows(e, c, fs, &launches))) return rc;
 
     // gather class: one concatenated row list, a span per query; the sort grants shared memory for the longest list
     if (n_gather) {
@@ -4301,6 +4312,10 @@ static int32_t ensure_group_index(wax_vs_engine *e, SearchCtx *c) {
     CUDA_TRY(cudaMemcpyAsync(&n_groups, incl.p + (n - 1), sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     CUDA_TRY(cudaMemcpy(gi.starts.p + n_groups, &n, sizeof(uint32_t), cudaMemcpyHostToDevice));
+    if ((rc = gi.ids.ensure(n_groups, "group index ids"))) return rc;
+    group_ids_kernel<<<grid, 256, 0, s>>>(keys_out, gi.starts, n_groups, gi.ids);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(s));              // keys_out is released on return
     gi.n_groups = n_groups;
     gi.valid = true;
     std::lock_guard<std::mutex> pg(e->pool_mu);
@@ -4308,6 +4323,11 @@ static int32_t ensure_group_index(wax_vs_engine *e, SearchCtx *c) {
     return WAX_VS_OK;
 }
 
+static uint32_t host_orderable(float f) {            // orderable_u32 on the host
+    uint32_t u;
+    memcpy(&u, &f, sizeof u);
+    return u ^ ((u & 0x80000000u) ? 0xFFFFFFFFu : 0x80000000u);
+}
 static float host_from_orderable(uint32_t k) {       // inverse of orderable_u32
     const uint32_t u = k ^ ((k & 0x80000000u) ? 0x80000000u : 0xFFFFFFFFu);
     float f;
@@ -4407,11 +4427,12 @@ static uint32_t deliver_group_keys(const wax_vs_engine *e, const uint64_t *keys,
 
 // One grouped search under the caller's read lock and scratch context (re-taking the shared lock inside a batch could
 // wait behind a queued writer): the host query, the filter's resolved rows (nullptr: unfiltered; the filter allows some
-// row) with `where` ANDed into its bitset (nullptr: none), the answer at out_* and *out_n.  The arguments are checked by
-// the caller.
+// row) with `where` ANDed into its bitset (nullptr: none), the answer at out_* and *out_n -- or, with out_keys, as
+// n_top x per_group keys (dist_key << 32 | row, group-major, padded with WAXVS_KEY_NONE) there instead.  The arguments
+// are checked by the caller.
 static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, uint32_t n_top, uint32_t per_group,
                            const std::vector<uint32_t> *rows, int32_t mode, const Clause *where, uint64_t *out_ids,
-                           float *out_scores, uint64_t *out_groups, uint32_t *out_n) {
+                           float *out_scores, uint64_t *out_groups, uint32_t *out_n, uint64_t *out_keys = nullptr) {
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const bool filtered = rows != nullptr;
     cudaStream_t s = c->stream;
@@ -4490,10 +4511,21 @@ static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, u
             CUDA_TRY(cudaMemcpyAsync(c->h_expand, c->d_expand[2], static_cast<size_t>(n_sel) * per_group * sizeof(uint64_t),
                                      cudaMemcpyDeviceToHost, s));
         CUDA_TRY(cudaStreamSynchronize(s));          // also keeps the item list alive until its copy is done
+        if (out_keys) {
+            std::fill(out_keys, out_keys + static_cast<size_t>(n_top) * per_group, WAXVS_KEY_NONE);
+            std::copy(c->h_expand.p, c->h_expand.p + static_cast<size_t>(n_sel) * per_group, out_keys);
+            return WAX_VS_OK;
+        }
         *out_n = deliver_group_keys(e, c->h_expand, n_sel, per_group, out_ids, out_scores, out_groups);
         return WAX_VS_OK;
     }
     CUDA_TRY(cudaStreamSynchronize(s));              // also keeps `rows` alive until its copy is done
+    if (out_keys) {
+        for (uint32_t i = 0; i < n_top; ++i)
+            out_keys[i] = c->h_out[i].valid ? (static_cast<uint64_t>(host_orderable(c->h_out[i].distance)) << 32) | c->h_out[i].row
+                                            : WAXVS_KEY_NONE;
+        return WAX_VS_OK;
+    }
     // (5) delivery: row -> frame id and group id, distance -> score
     uint32_t m = 0;
     for (uint32_t i = 0; i < n_top; ++i)
@@ -4577,6 +4609,46 @@ static int32_t enqueue_batch_expansion(wax_vs_engine *e, SearchCtx *c, const Cov
     return WAX_VS_OK;
 }
 
+// The expansions `list` (query = an index of `unit`, which names the query's pair or WAX_VS_NO_FILTER, unfiltered) into
+// c->d_bg_keys [query][n_top][per_group], queries staged in c->d_queries in the same indexing and the pairs' rows in
+// c->d_filter_rows.  The list, appended in any order, is sorted by (unit, query, group rank) for a reproducible launch
+// plan and run in passes of at most `fit` distinct units' bitsets (build_pass_bits); each pass ends in a synchronise, so
+// the next one may rebuild the bitsets.
+static int32_t expand_in_passes(wax_vs_engine *e, SearchCtx *c, CoverExpand *list, uint32_t n_exp,
+                                const std::vector<uint32_t> &unit, const int32_t *modes, const FilterSet &fs,
+                                uint32_t n_top, uint32_t per_group, uint64_t *launches, uint64_t *passes) {
+    std::sort(list, list + n_exp, [&](const CoverExpand &a, const CoverExpand &b) {
+        if (unit[a.query] != unit[b.query]) return unit[a.query] < unit[b.query];
+        return a.query != b.query ? a.query < b.query : a.slot < b.slot;
+    });
+    const uint64_t words = (e->n_rows + 31) / 32;
+    const uint64_t fit = std::max<uint64_t>(1, e->tune.filter_bitset_bytes / (words * sizeof(uint32_t)));
+    std::vector<uint32_t> query_slot(unit.size(), WAX_VS_NO_FILTER);
+    int32_t rc;
+    for (uint32_t i0 = 0; i0 < n_exp;) {
+        std::vector<uint32_t> which;         // the pass's units, in bitset order
+        uint32_t i1 = i0;
+        for (; i1 < n_exp; ++i1) {
+            const uint32_t u = unit[list[i1].query];
+            if (u != WAX_VS_NO_FILTER && (which.empty() || which.back() != u)) {
+                if (which.size() == fit) break;
+                which.push_back(u);
+            }
+            query_slot[list[i1].query] = u == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : static_cast<uint32_t>(which.size() - 1);
+        }
+        if (!which.empty()) {
+            if ((rc = build_pass_bits(e, c, modes, fs, which, launches))) return rc;
+            ++*passes;
+        }
+        if ((rc = enqueue_batch_expansion(e, c, list + i0, i1 - i0, n_top, per_group, query_slot, launches))) {
+            cudaStreamSynchronize(c->stream);
+            return rc;
+        }
+        i0 = i1;
+    }
+    return WAX_VS_OK;
+}
+
 // The grouped checks of every grouped entry point, before the empty-engine early return.
 static int32_t check_grouped_args(const wax_vs_engine *e, int64_t top_groups, uint32_t per_group, const uint64_t *out_ids,
                                   const float *out_scores, const uint64_t *out_groups, const uint32_t *out_n) {
@@ -4600,12 +4672,19 @@ static int32_t check_grouped_args(const wax_vs_engine *e, int64_t top_groups, ui
 //  - expansion: the cover kernel's list sorted by (unit, query, group rank), in passes of at most filter_bitset_bytes
 //    of distinct units' bitsets (build_pass_bits, as run_filtered builds them), each item scored under its unit's;
 //  - crowded queries: grouped_one under the query's own pair (grouped_one_args).
+// With `heads` (the sharded round 1) the answers go to the device instead, as [query][n_top][per_group] records with
+// global rows: the covered queries' keys are converted there, the crowded queries' are uploaded into their slots; the
+// caller zeroed the records, and the host outputs are not used.
+struct ShardHeads {
+    uint64_t row_offset;
+    wax_vs_group_candidate *d_heads;
+};
 static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                    int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids,
                                    const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
                                    const uint32_t *query_filter, const std::vector<Clause> &wheres,
                                    const uint32_t *query_where, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
-                                   uint32_t out_stride, uint32_t *out_n, bool batched) {
+                                   uint32_t out_stride, uint32_t *out_n, bool batched, const ShardHeads *heads = nullptr) {
     const uint32_t n_top = clamp_topk(top_groups);
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
@@ -4614,7 +4693,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     if ((rc = check_query(e, queries, query_len))) return rc;
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(n_top) * per_group, n));
-    if (out_stride < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, need);
+    if (!heads && out_stride < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, need);
     FilterSet ids;
     resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, ids);
     DeviceGuard g(e->device);
@@ -4665,44 +4744,27 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
             CUDA_TRY(cudaStreamSynchronize(s));
             std::vector<uint32_t> unit(nq);          // staged query -> its pair (WAX_VS_NO_FILTER, unfiltered, sorts last)
             for (uint32_t j = 0; j < nq; ++j) unit[j] = pair_of[plan.order[j]];
-            CoverExpand *list = c->h_bg_expand;      // appended in any order: sort for a reproducible launch plan
-            std::sort(list, list + n_exp, [&](const CoverExpand &a, const CoverExpand &b) {
-                if (unit[a.query] != unit[b.query]) return unit[a.query] < unit[b.query];
-                return a.query != b.query ? a.query < b.query : a.slot < b.slot;
-            });
-            // passes of at most `fit` distinct units' bitsets (run_filtered sized c->d_mask for at least as many); each
-            // pass ends in a synchronise, so the next one may rebuild the bitsets
-            const uint64_t words = (e->n_rows + 31) / 32;
-            const uint64_t fit = std::max<uint64_t>(1, e->tune.filter_bitset_bytes / (words * sizeof(uint32_t)));
-            std::vector<uint32_t> query_slot(nq, WAX_VS_NO_FILTER);
-            for (uint32_t i0 = 0; i0 < n_exp;) {
-                std::vector<uint32_t> which;         // the pass's units, in bitset order
-                uint32_t i1 = i0;
-                for (; i1 < n_exp; ++i1) {
-                    const uint32_t u = unit[list[i1].query];
-                    if (u != WAX_VS_NO_FILTER && (which.empty() || which.back() != u)) {
-                        if (which.size() == fit) break;
-                        which.push_back(u);
-                    }
-                    query_slot[list[i1].query] = u == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : static_cast<uint32_t>(which.size() - 1);
-                }
-                if (!which.empty()) {
-                    if ((rc = build_pass_bits(e, c, modes.data(), fs, which, &launches))) return rc;
-                    ++expansion_passes;
-                }
-                if ((rc = enqueue_batch_expansion(e, c, list + i0, i1 - i0, n_top, per_group, query_slot, &launches))) {
-                    cudaStreamSynchronize(s);
-                    return rc;
-                }
-                i0 = i1;
-            }
+            if ((rc = expand_in_passes(e, c, c->h_bg_expand, n_exp, unit, modes.data(), fs, n_top, per_group, &launches,
+                                       &expansion_passes)))
+                return rc;
             expanded = n_exp;
         }
-        CUDA_TRY(cudaMemcpyAsync(c->h_bg_keys, c->d_bg_keys, nkeys * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+        if (heads) {
+            ShardRowInfo ri{heads->row_offset, e->id_base, nullptr, e->gindex.row_group, e->gindex.ids};
+            if ((rc = sync_device_ids(e, &ri.ids)) || (rc = c->d_order.ensure(nq, "query order"))) return rc;
+            CUDA_TRY(cudaMemcpyAsync(c->d_order, plan.order.data(), nq * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+            const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (nkeys + 255) / 256)));
+            shard_group_heads_kernel<<<grid, 256, 0, s>>>(c->d_bg_keys, nq, slots, c->d_order, c->d_bg_status, ri, heads->d_heads);
+            CUDA_TRY(cudaGetLastError());
+            ++launches;
+        } else {
+            CUDA_TRY(cudaMemcpyAsync(c->h_bg_keys, c->d_bg_keys, nkeys * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
+        }
         CUDA_TRY(cudaStreamSynchronize(s));
         for (uint32_t j = 0; j < nq; ++j) {
             const uint32_t qi = plan.order[j];
             if (!c->h_bg_status[j]) { crowded.push_back(qi); continue; }
+            if (heads) { ++covered; continue; }
             const size_t o = static_cast<size_t>(qi) * out_stride;
             out_n[qi] = deliver_group_keys(e, c->h_bg_keys + static_cast<size_t>(j) * slots, n_top, per_group, out_ids + o,
                                            out_scores + o, out_groups + o);
@@ -4724,6 +4786,26 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
         } else if (p != WAX_VS_NO_FILTER) {
             rows.assign(fs.rows.begin() + fs.first[p], fs.rows.begin() + fs.first[p] + fs.count[p]);
             mode = modes[p];
+        }
+        if (heads) {                                 // the answer's keys -> records, uploaded into the query's slots
+            const size_t slots = static_cast<size_t>(n_top) * per_group;
+            std::vector<uint64_t> keys(slots);
+            if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group,
+                                  p == WAX_VS_NO_FILTER ? nullptr : &rows, mode, row_where ? &wheres[w] : nullptr, nullptr,
+                                  nullptr, nullptr, nullptr, keys.data())))
+                return rc;
+            std::vector<wax_vs_group_candidate> recs(slots, wax_vs_group_candidate{});
+            for (size_t i = 0; i < slots; ++i) {
+                if (keys[i] == WAXVS_KEY_NONE) continue;
+                const uint32_t row = static_cast<uint32_t>(keys[i]);
+                const uint64_t id = frame_id_of(e, row);
+                recs[i] = wax_vs_group_candidate{host_from_orderable(static_cast<uint32_t>(keys[i] >> 32)), 1u,
+                                                 heads->row_offset + row, id, e->groups_set ? e->groups[row] : id};
+            }
+            CUDA_TRY(cudaMemcpyAsync(heads->d_heads + qi * slots, recs.data(), slots * sizeof(wax_vs_group_candidate),
+                                     cudaMemcpyHostToDevice, s));
+            CUDA_TRY(cudaStreamSynchronize(s));      // recs must outlive its copy
+            continue;
         }
         const size_t o = static_cast<size_t>(qi) * out_stride;
         if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group,
@@ -4817,6 +4899,160 @@ int32_t wax_vs_search_batch_grouped_multi_where(wax_vs_engine *e, const float *q
     return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, filter_offsets,
                                filter_modes, n_filters, query_filter, clauses, query_where, out_ids, out_scores, out_groups,
                                out_stride, out_n, n_queries > 1);
+}
+
+// ---- sharded grouped search (waxvs_group_batch.cuh, waxvs_shard.cuh) ------------------------------------------------
+// The checks of the sharded grouped entry points: those of wax_vs_search_batch_grouped_multi_where and the cap on the
+// groups, before the engine is locked, so every rank fails alike before any exchange.  Builds the clauses.
+static int32_t check_shard_grouped_args(wax_vs_engine *e, const float *d_queries, uint32_t n_queries, int64_t top_groups,
+                                        uint32_t per_group, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                        const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                        const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                        const void *d_out, std::vector<Clause> &clauses) {
+    uint64_t no_ids = 0;                    // the checks of the host forms, which also test their outputs
+    float no_scores = 0.0f;
+    uint32_t no_n = 0;
+    int32_t rc;
+    if ((rc = check_grouped_args(e, top_groups, per_group, &no_ids, &no_scores, &no_ids, &no_n)) ||
+        (rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
+                               n_wheres, query_where, &no_n)))
+        return rc;
+    if (clamp_topk(top_groups) > WAX_VS_SHARD_MAX_GROUPS)
+        return fail(WAX_VS_ERR_UNSUPPORTED, "sharded grouped search takes clamp(top_groups) <= %d (got %u)",
+                    WAX_VS_SHARD_MAX_GROUPS, clamp_topk(top_groups));
+    if (!d_queries || !d_out) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    return near_clauses(wheres, n_wheres, clauses);
+}
+
+// Round 1: this shard's wax_vs_search_batch_grouped_multi_where, delivered as records on the device (ShardHeads).  The
+// queries come to the host once, as the host form takes them.
+int32_t wax_vs_shard_grouped_heads_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries, int64_t top_groups,
+                                          uint32_t per_group, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                          const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                          const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                          uint64_t row_offset, wax_vs_group_candidate *d_heads, void *cuda_stream) {
+    std::vector<Clause> clauses;
+    int32_t rc;
+    if ((rc = check_shard_grouped_args(e, d_queries, n_queries, top_groups, per_group, frame_ids, filter_offsets,
+                                       filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, d_heads,
+                                       clauses)))
+        return rc;
+    if (n_queries == 0) return WAX_VS_OK;
+    const size_t slots = static_cast<size_t>(clamp_topk(top_groups)) * per_group;
+    std::vector<float> queries(static_cast<size_t>(n_queries) * e->dims);
+    {
+        DeviceGuard g(e->device);
+        if (!g.ok) return g.error();
+        const cudaStream_t s = static_cast<cudaStream_t>(cuda_stream);
+        CUDA_TRY(cudaMemsetAsync(d_heads, 0, n_queries * slots * sizeof(wax_vs_group_candidate), s));
+        CUDA_TRY(cudaMemcpyAsync(queries.data(), d_queries, queries.size() * sizeof(float), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+    }
+    std::vector<uint32_t> no_n(n_queries);
+    const ShardHeads heads{row_offset, d_heads};
+    return search_grouped_host(e, queries.data(), n_queries, e->dims, top_groups, per_group, frame_ids, filter_offsets,
+                               filter_modes, n_filters, query_filter, clauses, query_where, nullptr, nullptr, nullptr, 0,
+                               no_n.data(), n_queries > 1, &heads);
+}
+
+// Merge 1 (merge_group_heads_kernel): stateless, enqueued on the caller's stream.
+int32_t wax_vs_merge_group_heads_device(wax_vs_engine *e, const wax_vs_group_candidate *d_gathered, uint32_t world,
+                                        uint32_t n_queries, int64_t top_groups, uint32_t per_group,
+                                        wax_vs_group_candidate *d_chosen, void *cuda_stream) {
+    if (!e || !d_gathered || !d_chosen) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    if (world == 0 || world > WAX_VS_SHARD_MAX_RANKS)
+        return fail(WAX_VS_ERR_ARGUMENT, "world must be in [1, %d] (got %u)", WAX_VS_SHARD_MAX_RANKS, world);
+    if (per_group == 0 || per_group > WAX_VS_MAX_PER_GROUP)
+        return fail(WAX_VS_ERR_ARGUMENT, "per_group must be in [1, %d] (got %u)", WAX_VS_MAX_PER_GROUP, per_group);
+    const uint32_t n_top = clamp_topk(top_groups);
+    if (n_top > WAX_VS_SHARD_MAX_GROUPS)
+        return fail(WAX_VS_ERR_UNSUPPORTED, "sharded grouped search takes clamp(top_groups) <= %d (got %u)",
+                    WAX_VS_SHARD_MAX_GROUPS, n_top);
+    if (n_queries == 0) return WAX_VS_OK;
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    uint32_t pow2 = 32;
+    while (pow2 < world * n_top) pow2 <<= 1;
+    const size_t smem = static_cast<size_t>(pow2) * (sizeof(uint64_t) + 3 * sizeof(uint32_t));
+    CUDA_TRY(grant_smem(e, merge_group_heads_kernel, smem));
+    merge_group_heads_kernel<<<n_queries, 1024, smem, static_cast<cudaStream_t>(cuda_stream)>>>(d_gathered, world, n_queries,
+                                                                                              n_top, per_group, pow2, d_chosen);
+    CUDA_TRY(cudaGetLastError());
+    return WAX_VS_OK;
+}
+
+// Round 2 on the caller's stream: the lookup kernel copies the groups this rank listed and lists the ones it must score;
+// those run as the batched grouped search's expansions (expand_in_passes) under each query's (where, id filter) pair,
+// and their keys become records.
+int32_t wax_vs_shard_grouped_expand_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries,
+                                           int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids,
+                                           const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                           const uint32_t *query_filter, const wax_vs_where_near *wheres,
+                                           uint32_t n_wheres, const uint32_t *query_where,
+                                           const wax_vs_group_candidate *d_chosen,
+                                           const wax_vs_group_candidate *d_own_heads, uint64_t row_offset,
+                                           wax_vs_candidate *d_rows, void *cuda_stream) {
+    std::vector<Clause> clauses;
+    int32_t rc;
+    if ((rc = check_shard_grouped_args(e, d_queries, n_queries, top_groups, per_group, frame_ids, filter_offsets,
+                                       filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, d_rows,
+                                       clauses)))
+        return rc;
+    if (!d_chosen || !d_own_heads) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    if (n_queries == 0) return WAX_VS_OK;
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    SearchCtx *c = nullptr;
+    if ((rc = ctx_for_stream(e, cuda_stream, &c))) return rc;
+    const cudaStream_t s = c->stream;
+    const uint32_t n_top = clamp_topk(top_groups);
+    const size_t n_slots = static_cast<size_t>(n_queries) * n_top;
+    e->async_pending.store(true);
+    CUDA_TRY(cudaMemsetAsync(d_rows, 0, n_slots * per_group * sizeof(wax_vs_candidate), s));
+    if (e->n_rows == 0) return WAX_VS_OK;
+    if ((rc = ensure_group_index(e, c))) return rc;
+    const auto &gi = e->gindex;
+    if ((rc = c->d_bg_expand.ensure(n_slots, "grouped batch expansions")) ||
+        (rc = c->h_bg_expand.ensure(n_slots, "grouped batch expansion staging")) ||
+        (rc = c->d_bg_status.ensure(1, "grouped batch status")) || (rc = c->h_bg_status.ensure(1, "grouped batch status staging")))
+        return rc;
+    CUDA_TRY(cudaMemsetAsync(c->d_bg_status, 0, sizeof(uint32_t), s));
+    const uint64_t warps_per_cta = 256 / 32;
+    shard_group_lookup_kernel<<<static_cast<uint32_t>((n_slots + warps_per_cta - 1) / warps_per_cta), 256, 0, s>>>(
+        d_chosen, d_own_heads, n_queries, n_top, per_group, gi.ids, gi.n_groups, gi.starts, d_rows, c->d_bg_expand,
+        c->d_bg_status);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(c->h_bg_status, c->d_bg_status, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    const uint32_t n_exp = c->h_bg_status[0];
+    if (n_exp == 0) return WAX_VS_OK;
+    uint64_t launches = 1, passes = 0;
+    CUDA_TRY(cudaMemcpyAsync(c->h_bg_expand, c->d_bg_expand, n_exp * sizeof(CoverExpand), cudaMemcpyDeviceToHost, s));
+    // the call's (where, id filter) pairs, their rows staged as run_filtered stages them, the queries in caller order
+    FilterSet ids, fs;
+    resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, ids);
+    std::vector<int32_t> modes;
+    std::vector<uint32_t> pair_of;
+    if ((rc = plan_where_pairs(e, c, clauses, query_where, filter_modes, query_filter, n_queries, ids, fs, modes, pair_of)) ||
+        (rc = stage_pair_rows(e, c, fs, &launches)))
+        return rc;
+    const size_t qfloats = static_cast<size_t>(n_queries) * e->dims;
+    if ((rc = c->d_queries.ensure(qfloats, "query buffer")) ||
+        (rc = c->d_bg_keys.ensure(n_slots * per_group, "grouped batch keys")))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_queries, d_queries, qfloats * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    CUDA_TRY(cudaStreamSynchronize(s));              // the expansion list is on the host
+    if ((rc = expand_in_passes(e, c, c->h_bg_expand, n_exp, pair_of, modes.data(), fs, n_top, per_group, &launches, &passes)))
+        return rc;
+    ShardRowInfo ri{row_offset, e->id_base, nullptr, gi.row_group, gi.ids};
+    if ((rc = sync_device_ids(e, &ri.ids))) return rc;
+    shard_group_expanded_kernel<<<n_exp, 128, 0, s>>>(c->d_bg_expand, c->d_bg_keys, n_top, per_group, ri, d_rows);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(s));              // the host arrays of the plan must outlive their uploads
+    std::lock_guard<std::mutex> pg(e->pool_mu);
+    e->shard_grouped_expanded_groups += n_exp;
+    return WAX_VS_OK;
 }
 
 // ---- persistence ---------------------------------------------------------------------------------------------
@@ -5162,6 +5398,7 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "grouped_batch_expanded_groups")) *out = e->grouped_batch_expanded_groups;     // (query, group) expansions
     else if (!strcmp(name, "grouped_batch_fallback_queries")) *out = e->grouped_batch_fallback_queries;   // single-query pipeline
     else if (!strcmp(name, "grouped_batch_expansion_passes")) *out = e->grouped_batch_expansion_passes;   // bitset passes of the expansion
+    else if (!strcmp(name, "shard_grouped_expanded_groups")) *out = e->shard_grouped_expanded_groups;     // sharded round 2: groups scored
     else if (!strcmp(name, "ingest_h2d_bytes")) *out = e->ingest_h2d_bytes;
     else if (!strcmp(name, "ingest_d2h_bytes")) *out = e->ingest_d2h_bytes;
     else if (!strcmp(name, "norms_rows")) *out = e->norms_rows;       // rows whose cached 1/|v| is valid

@@ -49,6 +49,14 @@ __global__ void group_finish_kernel(const uint32_t *__restrict__ perm, const uin
     }
 }
 
+// ids[g] = the group id of dense group g (its run head in the sorted keys): ascending, so a group id's dense index is a
+// binary search away, and row r's group id is ids[row_group[r]].
+__global__ void group_ids_kernel(const uint64_t *__restrict__ sorted, const uint32_t *__restrict__ starts,
+                                 uint32_t n_groups, uint64_t *__restrict__ ids) {
+    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < n_groups; g += gridDim.x * blockDim.x)
+        ids[g] = sorted[starts[g]];
+}
+
 // ---- per query --------------------------------------------------------------------------------------------------------
 // best[g] (initialised to WAXVS_KEY_NONE) = min over g's rows of (dist_key << 32 | row); dropped rows do not take part.
 // Lane L of a warp reduces positions [base + 16 L, base + 16 L + 16): a finished run is flushed with one atomicMin, the

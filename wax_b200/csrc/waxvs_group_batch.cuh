@@ -169,4 +169,96 @@ __global__ void __launch_bounds__(256) group_score_tile_kernel(const ScoreItem *
     for (uint32_t i = threadIdx.x; i < per_group; i += blockDim.x) dst[i] = sk[i];
 }
 
+// ---- sharded grouped search (wax_vs_shard_grouped_heads_device / _expand_device) --------------------------------------
+// A rank's rows as the records the ranks exchange: global row, frame id (ids[row] or id_base + row) and group id
+// (group_ids[row_group[row]]).  key = dist_key << 32 | local row; WAXVS_KEY_NONE is padding (all zero).
+struct ShardRowInfo {
+    uint64_t row_offset, id_base;
+    const uint64_t *ids;                     // nullptr: identity ids
+    const uint32_t *row_group;
+    const uint64_t *group_ids;
+};
+__device__ __forceinline__ wax_vs_group_candidate shard_group_record(uint64_t key, const ShardRowInfo &ri) {
+    wax_vs_group_candidate c{};
+    if (key != WAXVS_KEY_NONE) {
+        const uint32_t row = static_cast<uint32_t>(key);
+        c.distance = from_orderable_u32(static_cast<uint32_t>(key >> 32));
+        c.valid = 1u;
+        c.row = ri.row_offset + row;
+        c.frame_id = ri.ids ? ri.ids[row] : ri.id_base + row;
+        c.group_id = ri.group_ids[ri.row_group[row]];
+    }
+    return c;
+}
+
+// Round 1: the covered staged queries' result keys ([staged][slots]) -> their caller slots of heads ([query][slots]);
+// staged query j is query order[j], covered when status[j] != 0 (the others are delivered by the host).
+__global__ void __launch_bounds__(256) shard_group_heads_kernel(const uint64_t *__restrict__ keys, uint32_t n_staged,
+                                                                uint32_t slots, const uint32_t *__restrict__ order,
+                                                                const uint32_t *__restrict__ status, const ShardRowInfo ri,
+                                                                wax_vs_group_candidate *__restrict__ heads) {
+    const size_t total = static_cast<size_t>(n_staged) * slots;
+    for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const uint32_t j = static_cast<uint32_t>(i / slots), s = static_cast<uint32_t>(i % slots);
+        if (status[j]) heads[static_cast<size_t>(order[j]) * slots + s] = shard_group_record(keys[i], ri);
+    }
+}
+
+// Round 2, one warp per chosen (query, slot) of [n_queries][n_top]: a group this rank listed for the query in round 1
+// (own heads) is copied into rows ([query][slot][per_group]); a group the shard holds (its id found among the index's
+// sorted group ids) is appended to `expand` with its CSR span; anything else stays padding (the caller zeroed `rows`).
+__global__ void __launch_bounds__(256) shard_group_lookup_kernel(const wax_vs_group_candidate *__restrict__ chosen,
+                                                                 const wax_vs_group_candidate *__restrict__ own,
+                                                                 uint32_t n_queries, uint32_t n_top, uint32_t per_group,
+                                                                 const uint64_t *__restrict__ group_ids, uint32_t n_groups,
+                                                                 const uint32_t *__restrict__ starts,
+                                                                 wax_vs_candidate *__restrict__ rows,
+                                                                 CoverExpand *__restrict__ expand,
+                                                                 uint32_t *__restrict__ n_expand) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t slot = (static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+    if (slot >= static_cast<uint64_t>(n_queries) * n_top) return;      // warp-uniform
+    const wax_vs_group_candidate ch = chosen[slot];
+    if (!ch.valid) return;
+    const uint32_t q = static_cast<uint32_t>(slot / n_top), s = static_cast<uint32_t>(slot % n_top);
+    const wax_vs_group_candidate *oq = own + static_cast<size_t>(q) * n_top * per_group;
+    uint32_t listed = 0xFFFFFFFFu;
+    for (uint32_t g0 = 0; g0 < n_top && listed == 0xFFFFFFFFu; g0 += 32) {
+        const uint32_t g = g0 + lane;
+        const bool hit = g < n_top && oq[static_cast<size_t>(g) * per_group].valid &&
+                         oq[static_cast<size_t>(g) * per_group].group_id == ch.group_id;
+        const uint32_t b = __ballot_sync(WAXVS_FULL_MASK, hit);
+        if (b) listed = g0 + __ffs(b) - 1;
+    }
+    if (listed != 0xFFFFFFFFu) {                                        // copy: already this shard's best rows
+        for (uint32_t j = lane; j < per_group; j += 32) {
+            const wax_vs_group_candidate h = oq[static_cast<size_t>(listed) * per_group + j];
+            if (h.valid) rows[slot * per_group + j] = wax_vs_candidate{h.distance, 1u, h.row, h.frame_id};
+        }
+        return;
+    }
+    if (lane) return;
+    uint32_t lo = 0, hi = n_groups;                                     // expansion: the group's rows on this shard
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (group_ids[mid] < ch.group_id) lo = mid + 1; else hi = mid;
+    }
+    if (lo < n_groups && group_ids[lo] == ch.group_id)
+        expand[atomicAdd(n_expand, 1u)] = CoverExpand{q, s, starts[lo], starts[lo + 1] - starts[lo]};
+}
+
+// Round 2: the expanded slots' keys ([query][slot][per_group] in keys) -> their candidate records in rows.
+__global__ void __launch_bounds__(128) shard_group_expanded_kernel(const CoverExpand *__restrict__ expand,
+                                                                   const uint64_t *__restrict__ keys, uint32_t n_top,
+                                                                   uint32_t per_group, const ShardRowInfo ri,
+                                                                   wax_vs_candidate *__restrict__ rows) {
+    const CoverExpand x = expand[blockIdx.x];
+    const size_t base = (static_cast<size_t>(x.query) * n_top + x.slot) * per_group;
+    for (uint32_t j = threadIdx.x; j < per_group; j += blockDim.x) {
+        const wax_vs_group_candidate c = shard_group_record(keys[base + j], ri);
+        rows[base + j] = wax_vs_candidate{c.distance, c.valid, c.row, c.frame_id};
+    }
+}
+
 }  // namespace waxvs

@@ -188,6 +188,109 @@ __global__ void __launch_bounds__(128) merge_gathered_kernel(const wax_vs_candid
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// Sharded grouped search, merge 1 (wax_vs_merge_group_heads_device): the ranks' round-1 answers gathered as
+// [world][n_queries][G][P] -> per query the global top G groups, each as its best row.  A group's head on a rank is its
+// best row there, so its global head is the best of its heads; a group is ranked by that head in (distance, GLOBAL row).
+// Each rank's heads are in that order and lower ranks hold lower rows, so (distance key, rank * G + slot) orders the
+// heads exactly as (distance, global row) does.
+constexpr uint32_t kShardMaxGroups = 256;   // = WAX_VS_SHARD_MAX_GROUPS: world * G <= 4 096 heads in shared memory
+
+// Sorts (key[i], val[i]) pairs ascending by key, then val (pow2 entries, every thread of the CTA).
+__device__ __forceinline__ void block_bitonic_sort_pairs(uint64_t *key, uint32_t *val, uint32_t pow2) {
+    for (uint32_t size = 2; size <= pow2; size <<= 1) {
+        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+            for (uint32_t i = threadIdx.x; i < pow2 / 2; i += blockDim.x) {
+                const uint32_t lo = (i / stride) * (2 * stride) + (i % stride), hi = lo + stride;
+                const bool asc = ((lo & size) == 0);
+                const uint64_t ka = key[lo], kb = key[hi];
+                const uint32_t va = val[lo], vb = val[hi];
+                const bool greater = ka > kb || (ka == kb && va > vb);
+                if (greater == asc) { key[lo] = kb; key[hi] = ka; val[lo] = vb; val[hi] = va; }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// One CTA per query; dynamic shared memory: pow2 * 20 bytes, pow2 = the power of two >= max(world * G, 32).
+__global__ void __launch_bounds__(1024) merge_group_heads_kernel(const wax_vs_group_candidate *__restrict__ gathered,
+                                                                 uint32_t world, uint32_t n_queries, uint32_t n_top,
+                                                                 uint32_t per_group, uint32_t pow2,
+                                                                 wax_vs_group_candidate *__restrict__ chosen) {
+    extern __shared__ uint64_t heads_smem[];
+    uint64_t *s_key = heads_smem;                                      // [pow2]
+    uint32_t *s_val = reinterpret_cast<uint32_t *>(heads_smem + pow2); // [pow2]
+    uint32_t *s_head = s_val + pow2;                                   // [pow2] head index at each ordered position
+    uint32_t *s_keep = s_head + pow2;                                  // [pow2] 1: the position is its group's best head
+    __shared__ uint32_t s_warp[32], s_total;
+    const uint32_t q = blockIdx.x, t = threadIdx.x, heads = world * n_top;
+    const size_t rank_stride = static_cast<size_t>(n_queries) * n_top * per_group;
+    auto head = [&](uint32_t i) -> const wax_vs_group_candidate & {
+        return gathered[(i / n_top) * rank_stride + (static_cast<size_t>(q) * n_top + i % n_top) * per_group];
+    };
+    // 1. every rank's heads in (distance, global row) order
+    uint32_t mine = 0;
+    for (uint32_t i = t; i < pow2; i += blockDim.x) {
+        const bool v = i < heads && head(i).valid;
+        s_key[i] = v ? orderable_u32(head(i).distance) : ~0ull;
+        s_val[i] = v ? i : 0xFFFFFFFFu;
+        mine += v;
+    }
+    for (uint32_t i = t; i < pow2; i += blockDim.x) s_keep[i] = 0;
+    if (t == 0) s_total = 0;
+    __syncthreads();
+    atomicAdd(&s_total, mine);
+    block_bitonic_sort_pairs(s_key, s_val, pow2);                       // ends in __syncthreads
+    const uint32_t valid = s_total;
+    // 2. by (group id, position): the first position of each group id is its best head
+    for (uint32_t p = t; p < pow2; p += blockDim.x) {
+        s_head[p] = s_val[p];
+        s_key[p] = p < valid ? head(s_val[p]).group_id : ~0ull;
+        s_val[p] = p < valid ? p : 0xFFFFFFFFu;
+    }
+    __syncthreads();
+    block_bitonic_sort_pairs(s_key, s_val, pow2);
+    for (uint32_t j = t; j < valid; j += blockDim.x)
+        if (j == 0 || s_key[j - 1] != s_key[j]) s_keep[s_val[j]] = 1u;
+    __syncthreads();
+    // 3. the kept heads' ranks: an exclusive scan over the ordered positions, each thread a run of `per` of them
+    const uint32_t per = (pow2 + blockDim.x - 1) / blockDim.x, lane = t & 31u, warp = t >> 5;
+    uint32_t local = 0;
+    for (uint32_t e = 0; e < per; ++e) {
+        const uint32_t p = t * per + e;
+        if (p < valid) local += s_keep[p];
+    }
+    uint32_t incl = local;
+    for (uint32_t o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(WAXVS_FULL_MASK, incl, o);
+        if (lane >= o) incl += y;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    if (warp == 0) {
+        const uint32_t nw = blockDim.x >> 5;
+        uint32_t w = lane < nw ? s_warp[lane] : 0u;
+        for (uint32_t o = 1; o < 32; o <<= 1) {
+            const uint32_t y = __shfl_up_sync(WAXVS_FULL_MASK, w, o);
+            if (lane >= o) w += y;
+        }
+        if (lane < nw) s_warp[lane] = w;                               // inclusive per warp
+    }
+    __syncthreads();
+    uint32_t rank = (warp ? s_warp[warp - 1] : 0u) + incl - local;
+    const uint32_t kept = s_warp[(blockDim.x >> 5) - 1];
+    wax_vs_group_candidate *out = chosen + static_cast<size_t>(q) * n_top;
+    for (uint32_t e = 0; e < per; ++e) {
+        const uint32_t p = t * per + e;
+        if (p < valid && s_keep[p]) {
+            if (rank < n_top) out[rank] = head(s_head[p]);
+            ++rank;
+        }
+    }
+    for (uint32_t s = kept + t; s < n_top; s += blockDim.x) out[s] = wax_vs_group_candidate{};
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // The device form of a batched where search (wax_vs_search_batch_where_device) stages and answers its queries in the
 // plan's order.  order[j] = the caller's query that staged query j is; k_of[j] = the slots of its list that were written.
 __global__ void __launch_bounds__(256) stage_query_rows_kernel(const float *__restrict__ queries,

@@ -26,6 +26,10 @@ import numpy as np
 
 CAND_DTYPE = np.dtype([("distance", "<f4"), ("valid", "<u4"), ("row", "<u8"), ("frame_id", "<u8")])
 assert CAND_DTYPE.itemsize == 24
+# wax_vs_group_candidate: a row of a rank's grouped answer, with its group id (sharded grouped search)
+GROUP_CAND_DTYPE = np.dtype([("distance", "<f4"), ("valid", "<u4"), ("row", "<u8"), ("frame_id", "<u8"),
+                             ("group_id", "<u8")])
+assert GROUP_CAND_DTYPE.itemsize == 32
 
 
 def shard_range(total_rows: int, world_size: int, rank: int) -> Tuple[int, int]:
@@ -518,6 +522,86 @@ class ShardedVectorEngine:
         merged = self._merge_on_device(gathered, b, k, k, stream)
         ids, scores, ns = self._unpack_merged(merged.cpu().numpy(), b, k)
         return [[(int(ids[i, j]), float(scores[i, j])) for j in range(int(ns[i]))] for i in range(b)]
+
+    # -- grouped search: the best frames of the top groups, exact, in two exchanges (DESIGN.md section 4.14)
+    def set_groups(self, frame_ids, group_ids) -> int:
+        """CUDAVectorEngine.set_groups on this rank's engine (full lists or this rank's frames).  Returns this rank's
+        assigned count."""
+        return self.engine.set_groups(frame_ids, group_ids)
+
+    def _all_gather(self, local):
+        """[world][local] bytes on the device: the ranks' buffers in rank order."""
+        if self.world_size == 1:
+            return local
+        gathered = self._torch.empty(self.world_size * local.numel(), dtype=self._torch.uint8, device=self.device)
+        self._dist.all_gather_into_tensor(gathered, local, group=self.group)
+        return gathered
+
+    def search_batch_grouped(self, vectors, top_groups: int, per_group: int = 1, wheres=None, query_where=None,
+                             filters=None, query_filter=None) -> List[List[Tuple[int, List[Tuple[int, float]]]]]:
+        """CUDAVectorEngine.search_batch_grouped_multi_where over the whole sharded corpus (collective, any transport;
+        arguments as there, wheres and filters optional; clamp(top_groups) <= 256).  Round 1: every rank's own grouped
+        answer (wax_vs_shard_grouped_heads_device), one all-gather, the global top groups by their best rows
+        (wax_vs_merge_group_heads_device).  per_group > 1 adds round 2: every rank's best rows of each chosen group
+        (wax_vs_shard_grouped_expand_device), a second all-gather and the per-group merge (wax_vs_merge_candidates_device).
+        One copy brings the answer to the host.  Equal, bit for bit, to the single engine's answer."""
+        from . import _lib as L
+        from .engine import _check, _WhereArgs
+        torch = self._torch
+        qs = np.ascontiguousarray(vectors, dtype=np.float32).reshape(-1, self.dimensions)
+        b = qs.shape[0]
+        wheres = list(wheres or [])
+        if any(w.terms for w in wheres):
+            raise ValueError("grouped search takes no term clause")
+        a = _WhereArgs(wheres, [None] * b if query_where is None else query_where, filters, query_filter, b)
+        if b == 0:
+            return []
+        g, p = clamp_topk(top_groups), max(int(per_group), 1)
+        lib, h = L.lib(), self.engine.handle
+        d_qs = torch.from_numpy(qs).to(self.device)
+        stream = torch.cuda.current_stream(self.device)
+        s = C.c_void_p(stream.cuda_stream)
+        fargs, wargs = a.filter_args(), a.where_args(near=True)
+        heads = torch.empty(b * g * p * GROUP_CAND_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
+        _check(lib.wax_vs_shard_grouped_heads_device(h, C.c_void_p(d_qs.data_ptr()), b, int(top_groups), int(per_group),
+                                                     *fargs, *wargs, self.row_lo, C.c_void_p(heads.data_ptr()), s))
+        gathered = self._all_gather(heads)
+        chosen = torch.empty(b * g * GROUP_CAND_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
+        _check(lib.wax_vs_merge_group_heads_device(h, C.c_void_p(gathered.data_ptr()), self.world_size, b, int(top_groups),
+                                                   int(per_group), C.c_void_p(chosen.data_ptr()), s))
+        sim = self.metric.to_vec_similarity()
+        if p == 1:
+            best = chosen.cpu().numpy().view(GROUP_CAND_DTYPE).reshape(b, g)
+            scores = score_from_distance(sim, best["distance"])
+            return [[(int(best["group_id"][i, j]), [(int(best["frame_id"][i, j]), float(scores[i, j]))])
+                     for j in range(g) if best["valid"][i, j]] for i in range(b)]
+        rows = torch.empty(b * g * p * CAND_DTYPE.itemsize, dtype=torch.uint8, device=self.device)
+        _check(lib.wax_vs_shard_grouped_expand_device(h, C.c_void_p(d_qs.data_ptr()), b, int(top_groups), int(per_group),
+                                                      *fargs, *wargs, C.c_void_p(chosen.data_ptr()),
+                                                      C.c_void_p(heads.data_ptr()), self.row_lo,
+                                                      C.c_void_p(rows.data_ptr()), s))
+        merged = self._merge_on_device(self._all_gather(rows), b * g, p, p, stream)
+        host = torch.cat([chosen, merged]).cpu().numpy()
+        groups = host[:chosen.numel()].view(GROUP_CAND_DTYPE).reshape(b, g)
+        best = host[chosen.numel():].view(CAND_DTYPE).reshape(b, g, p)
+        scores = score_from_distance(sim, best["distance"])
+        return [[(int(groups["group_id"][i, j]), [(int(best["frame_id"][i, j, m]), float(scores[i, j, m]))
+                                                   for m in range(p) if best["valid"][i, j, m]])
+                 for j in range(g) if groups["valid"][i, j]] for i in range(b)]
+
+    def search_grouped(self, vector: Sequence[float], top_groups: int, per_group: int = 1, where=None, allow=None,
+                       deny=None) -> List[Tuple[int, List[Tuple[int, float]]]]:
+        """search_batch_grouped for one query (collective): CUDAVectorEngine.search_grouped's answer over the whole sharded
+        corpus, under an optional where and at most one of allow= / deny=."""
+        q = np.ascontiguousarray(vector, dtype=np.float32).reshape(-1)
+        if q.size != self.dimensions:
+            from .engine import EncodingError
+            raise EncodingError(f"vector dimension mismatch: expected {self.dimensions}, got {q.size}")
+        if allow is not None and deny is not None:
+            raise ValueError("pass at most one of allow= / deny=")
+        filters = [("allow", allow)] if allow is not None else ([("deny", deny)] if deny is not None else [])
+        return self.search_batch_grouped(q.reshape(1, -1), top_groups, per_group, [] if where is None else [where],
+                                         [None if where is None else 0], filters, [0 if filters else None])[0]
 
     def _search_fused(self, q: np.ndarray, top_k: int) -> List[Tuple[int, float]]:
         """wax_vs_shard_search: host query in, merged host result out; scan + NVLink exchange + merge in one launch."""
