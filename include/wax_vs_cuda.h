@@ -59,7 +59,7 @@ enum { WAX_VS_COSINE = 0, WAX_VS_DOT = 1, WAX_VS_L2 = 2 };
 typedef struct wax_vs_candidate {
     float distance;     /* USearch-convention distance (ascending = better)                        */
     uint32_t valid;     /* 1 = real candidate, 0 = padding (fewer than k finite candidates)        */
-    uint64_t row;       /* global row = row_offset + local row: the cross-shard tie-break key      */
+    uint64_t row;       /* global row = row_offset + local row or row key: the cross-shard tie-break */
     uint64_t frame_id;
 } wax_vs_candidate;
 
@@ -112,6 +112,29 @@ int32_t wax_vs_remove(wax_vs_engine *engine, uint64_t frame_id);
    are ignored, surviving rows keep their relative order -- with one compaction of the matrix in HBM, one compaction
    of the id array and one id->row hash rebuild.  *out_removed (optional) = rows actually deleted. */
 int32_t wax_vs_remove_batch(wax_vs_engine *engine, const uint64_t *frame_ids, uint64_t n, uint64_t *out_removed);
+
+/* ---- row keys: the rank-local store of the row-sharded engine (DESIGN.md section 4.15) ------------------------------
+   A keyed engine holds one u64 key per row, the row's insertion sequence number in the whole sharded corpus; keys
+   strictly increase with the row.  The device entry points (wax_vs_search_device and every entry below it that takes a
+   row_offset or reports global rows) report row r as row_offset + key[r], so the ranks' candidates merge in the single
+   engine's position order wherever each row lives.  An engine becomes keyed by wax_vs_add_batch_keyed or
+   wax_vs_deserialize_rows; until then row r's key is r and everything behaves as before.  wax_vs_deserialize and
+   wax_vs_debug_fill_synthetic drop the keys.  On a keyed engine wax_vs_add_batch gives appended rows the keys after the
+   last one, an upsert keeps its row's key and wax_vs_remove_batch keeps the survivors' keys. */
+/* wax_vs_add_batch whose appended rows take the keys first_key, first_key + 1, ... in order of first appearance.
+   first_key not above the last row's key -> WAX_VS_ERR_ARGUMENT, before anything changes.  *out_appended (optional) =
+   rows appended (the batch's distinct new ids). */
+int32_t wax_vs_add_batch_keyed(wax_vs_engine *engine, const uint64_t *frame_ids, const float *rows, uint64_t n,
+                               uint32_t vector_len, uint64_t first_key, uint64_t *out_appended);
+/* out[i] = 1 when the engine holds frame_ids[i], else 0. */
+int32_t wax_vs_contains(wax_vs_engine *engine, const uint64_t *frame_ids, uint64_t n, uint8_t *out);
+/* Replace the contents with rows [first, first + n) of an MV2V blob, keyed first, first + 1, ...  The blob is checked
+   exactly as wax_vs_deserialize checks it (same codes and reasons); a row range outside it -> WAX_VS_ERR_ARGUMENT. */
+int32_t wax_vs_deserialize_rows(wax_vs_engine *engine, const uint8_t *src, uint64_t len, uint64_t first, uint64_t n);
+/* Copy rows [first, first + n) out: frame ids, vectors (n x dims) and keys (r for an engine without keys).  Each output
+   may be NULL.  A range outside the rows -> WAX_VS_ERR_ARGUMENT. */
+int32_t wax_vs_export_rows(wax_vs_engine *engine, uint64_t first, uint64_t n, uint64_t *out_ids, float *out_vectors,
+                           uint64_t *out_keys);
 
 /* ---- search ------------------------------------------------------------------------------------- */
 
@@ -423,7 +446,7 @@ int32_t wax_vs_search_batch_where_terms(wax_vs_engine *engine, const float *quer
    `d_candidates` (n_queries x k_eff entries, k_eff = min(clamp(top_k), 10000) -- NOT clipped to N, padding
    has valid = 0) are DEVICE pointers on the engine's device; the work is enqueued on `cuda_stream`
    (a cudaStream_t; NULL = legacy default stream) and the call returns without synchronising.
-   candidate.row = row_offset + local row.
+   candidate.row = row_offset + local row (row_offset + the row's key on a keyed engine).
    Ordering against mutators: the library remembers that device-path work was enqueued and every mutator
    (add / remove / reserve / deserialize / fill) drains the DEVICE (cudaDeviceSynchronize) under its write lock
    before it touches the corpus, so an in-flight scan never reads rows that are being moved. */
@@ -472,8 +495,8 @@ int32_t wax_vs_shard_search(wax_vs_engine *engine, const float *query, uint32_t 
                             uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n);
 /* Device-side merge for the sharded search_batch: d_gathered = [world][n_queries][k] candidates exactly as an
    all-gather of the ranks' wax_vs_search_batch_device outputs leaves them (rank-major; every per-query list sorted, padding
-   valid = 0 last); d_out = [n_queries][k_out] (k_out <= k), the k_out best of each query under (distance, GLOBAL row)
-   -- ranks must be ordered by ascending row ranges.  Enqueued on cuda_stream, no synchronisation. */
+   valid = 0 last); d_out = [n_queries][k_out] (k_out <= k), the k_out best of each query under (distance, GLOBAL row),
+   whichever rows each rank holds (contiguous ranges or keyed rows).  Enqueued on cuda_stream, no synchronisation. */
 int32_t wax_vs_merge_candidates_device(wax_vs_engine *engine, const wax_vs_candidate *d_gathered, uint32_t world,
                                        uint32_t n_queries, uint32_t k, uint32_t k_out, wax_vs_candidate *d_out,
                                        void *cuda_stream);
@@ -504,7 +527,7 @@ int32_t wax_vs_shard_search_where(wax_vs_engine *engine, const float *query, uin
 /* The rank-local half of a batched sharded where search, for any transport and any k up to 10 000.  Arguments are those
    of wax_vs_search_batch_where_terms; where_term_offsets may be NULL when no where has a term.  d_queries is a device
    pointer, as in wax_vs_search_batch_device.  Output: d_candidates [n_queries][clamp(top_k)] on the device.  Each list is
-   sorted by (distance, row_offset + local row), and padding has valid = 0 and comes last.  This is exactly the layout
+   sorted by (distance, global row), and padding has valid = 0 and comes last.  This is exactly the layout
    that wax_vs_merge_candidates_device takes after an all-gather.  A query with no allowed row on this shard, and every
    query of an empty shard, is all padding.  The argument checks of wax_vs_search_batch_where_terms, and NULL d_queries
    or d_candidates -> WAX_VS_ERR_NULL, run before the empty-engine early return.  The call may synchronise cuda_stream,
@@ -526,7 +549,7 @@ int32_t wax_vs_search_batch_where_device(wax_vs_engine *engine, const float *d_q
 typedef struct wax_vs_group_candidate {   /* 32 bytes, naturally aligned */
     float distance;     /* as wax_vs_candidate                                   */
     uint32_t valid;     /* 1 = real row, 0 = padding (all fields zero)           */
-    uint64_t row;       /* global row = row_offset + local row                   */
+    uint64_t row;       /* global row = row_offset + local row or row key        */
     uint64_t frame_id;
     uint64_t group_id;
 } wax_vs_group_candidate;
@@ -542,8 +565,8 @@ int32_t wax_vs_shard_grouped_heads_device(wax_vs_engine *engine, const float *d_
                                           const uint32_t *query_filter, const wax_vs_where_near *wheres, uint32_t n_wheres,
                                           const uint32_t *query_where, uint64_t row_offset, wax_vs_group_candidate *d_heads,
                                           void *cuda_stream);
-/* Merge 1.  d_gathered = [world][n_queries][G][P], the ranks' d_heads in rank order (ascending row ranges) as an
-   all-gather leaves them.  d_chosen = [n_queries][G]: per query the union of the ranks' group heads (a group's first
+/* Merge 1.  d_gathered = [world][n_queries][G][P], the ranks' d_heads in rank order as an all-gather leaves them (any
+   placement of rows on ranks).  d_chosen = [n_queries][G]: per query the union of the ranks' group heads (a group's first
    row), the best head kept per group id, the first G by (distance, global row); padding (valid = 0, zeroed) last.  These
    are the global top G groups, each as its best row.  world outside 1..WAX_VS_SHARD_MAX_RANKS, per_group outside
    1..WAX_VS_MAX_PER_GROUP -> WAX_VS_ERR_ARGUMENT; clamp(top_groups) > WAX_VS_SHARD_MAX_GROUPS -> WAX_VS_ERR_UNSUPPORTED;

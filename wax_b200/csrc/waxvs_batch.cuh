@@ -936,7 +936,7 @@ struct FinishParams {
     const uint32_t *max_norm_bits;
     wax_vs_candidate *out;      // [n_queries][k]
     uint32_t *ok;               // [n_queries] 1 = proven exact, 0 = re-run on the exact path
-    const uint64_t *frame_ids;
+    const uint64_t *frame_ids, *row_keys;
     uint64_t id_base, row_offset;
     uint32_t pow2_all;          // next pow2 >= slices*kprime
     uint32_t rescore;           // nominees re-scored exactly per query: a power of two in [256, kBatchRescoreMax]
@@ -1123,7 +1123,7 @@ __global__ void __launch_bounds__(512, 2) batch_finish_kernel(const FinishParams
     }
     ScanParams sp{};
     sp.out = p.out + static_cast<size_t>(q) * p.k;
-    sp.frame_ids = p.frame_ids; sp.id_base = p.id_base; sp.row_offset = p.row_offset;
+    sp.frame_ids = p.frame_ids; sp.id_base = p.id_base; sp.row_offset = p.row_offset; sp.row_keys = p.row_keys;
     for (uint32_t i = threadIdx.x; i < p.k; i += blockDim.x)
         write_candidate(sp, static_cast<int>(i), i < p.rescore ? ek[i] : WAXVS_KEY_NONE);
 }
@@ -1149,7 +1149,7 @@ struct RescoreParams {
     uint32_t *work_counter;         // the U4 scan's claim counter (its tail has no last CTA): reset here for the next scan
     wax_vs_candidate *out;          // [k]
     uint32_t *ok;                   // 1 = proven exact, 0 = the fp32 scan must answer
-    const uint64_t *frame_ids;
+    const uint64_t *frame_ids, *row_keys;
     uint64_t id_base, row_offset;
     uint32_t tail_smem_bytes;
 };
@@ -1177,7 +1177,7 @@ __global__ void __launch_bounds__(512, 1) shadow_rescore_kernel(const RescorePar
     __syncthreads();
     if (threadIdx.x == 0) {
         sp.k = p.k; sp.block_keys = p.block_keys; sp.ticket = p.ticket; sp.out = p.out;
-        sp.frame_ids = p.frame_ids; sp.id_base = p.id_base; sp.row_offset = p.row_offset;
+        sp.frame_ids = p.frame_ids; sp.id_base = p.id_base; sp.row_offset = p.row_offset; sp.row_keys = p.row_keys;
         sp.tail_smem_bytes = p.tail_smem_bytes; sp.work_counter = p.work_counter;
     }
     __syncthreads();
@@ -1284,7 +1284,7 @@ struct FilterSelectParams {
     uint32_t cand_cap, k;
     wax_vs_candidate *out;      // [n_queries][k]
     uint32_t *ok;               // [n_queries]: 1 = complete (the list did not overflow and holds >= k finite rows)
-    const uint64_t *frame_ids;
+    const uint64_t *frame_ids, *row_keys;
     uint64_t id_base, row_offset;
 };
 
@@ -1303,7 +1303,7 @@ __global__ void __launch_bounds__(1024) filter_select_kernel(const FilterSelectP
     if (threadIdx.x == 0) p.ok[q] = (total <= p.cand_cap && fsk[p.k - 1] != WAXVS_KEY_NONE) ? 1u : 0u;
     ScanParams sp{};
     sp.out = p.out + static_cast<size_t>(q) * p.k;
-    sp.frame_ids = p.frame_ids; sp.id_base = p.id_base; sp.row_offset = p.row_offset;
+    sp.frame_ids = p.frame_ids; sp.id_base = p.id_base; sp.row_offset = p.row_offset; sp.row_keys = p.row_keys;
     for (uint32_t i = threadIdx.x; i < p.k; i += blockDim.x) write_candidate(sp, static_cast<int>(i), fsk[i]);
 }
 

@@ -214,6 +214,8 @@ struct Tuning {
 struct SearchCtx {
     cudaStream_t stream = nullptr;
     bool own_stream = false;
+    const uint64_t *row_keys = nullptr;            // the engine's device row keys while a call that reports global rows
+                                                   // (device and shard entry points) holds this context; else nullptr
     DevBuf<float> d_queries;
     DevBuf<wax_vs_candidate> d_out;
     PinnedBuf<float> h_queries;
@@ -308,6 +310,13 @@ struct wax_vs_engine {
     DevBuf<uint64_t> d_ids;
     bool d_ids_dirty = true;
     std::mutex ids_mu;
+    // Row keys of a keyed shard (DESIGN 4.15): keys[r] is row r's insertion sequence number in the sharded corpus, strictly
+    // increasing with r, and the device entry points report row r as row_offset + keys[r].  Absent (keys_set false, a row
+    // is reported as row_offset + r) until wax_vs_add_batch_keyed or wax_vs_deserialize_rows runs.  Every mutator keeps
+    // keys aligned with `ids` and d_keys current.
+    bool keys_set = false;
+    std::vector<uint64_t> keys;
+    DevBuf<uint64_t> d_keys;
 
     std::shared_mutex rw;  // readers: search / serialize; writer: mutators (AsyncReadWriteLock, :56-80)
     std::mutex pool_mu;
@@ -490,6 +499,8 @@ struct wax_vs_engine {
 
 extern "C" { static void shard_teardown(wax_vs_engine *e, bool free_own); }
 
+static const uint64_t *device_row_keys(const wax_vs_engine *e) { return e->keys_set ? e->d_keys.p : nullptr; }
+
 // Called by every mutator after it has taken the write lock (and selected the device).
 static void drain_device_path(wax_vs_engine *e) {
     if (e->async_pending.exchange(false)) cudaDeviceSynchronize();
@@ -568,6 +579,7 @@ static int32_t ctx_acquire(wax_vs_engine *e, SearchCtx **out) {
             *out = e->pool.back();
             e->pool.pop_back();
             ++e->pool_reuses;
+            (*out)->row_keys = nullptr;
             return WAX_VS_OK;
         }
         ++e->pool_allocs;
@@ -593,15 +605,21 @@ struct CtxLease {
     int32_t acquire() { return ctx_acquire(e, &c); }
 };
 // The scratch context bound to a caller-owned stream (device-path entry points): find-or-create in ONE critical
-// section, so two threads that first use the same stream cannot both insert (and leak) a context.
+// section, so two threads that first use the same stream cannot both insert (and leak) a context.  These calls report
+// global rows, so the context carries the row keys.
 static int32_t ctx_for_stream(wax_vs_engine *e, void *cuda_stream, SearchCtx **out) {
     std::lock_guard<std::mutex> pg(e->pool_mu);
     auto it = e->stream_ctx.find(cuda_stream);
-    if (it != e->stream_ctx.end()) { *out = it->second; return WAX_VS_OK; }
+    if (it != e->stream_ctx.end()) {
+        *out = it->second;
+        (*out)->row_keys = device_row_keys(e);
+        return WAX_VS_OK;
+    }
     SearchCtx *c = nullptr;
     int32_t rc = ctx_new(e, &c, false);
     if (rc) return rc;
     c->stream = static_cast<cudaStream_t>(cuda_stream);
+    c->row_keys = device_row_keys(e);
     e->stream_ctx[cuda_stream] = c;
     ++e->pool_allocs;
     *out = c;
@@ -1015,7 +1033,7 @@ static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const 
         rp.dims = e->dims; rp.k = p.k; rp.n_nominees = static_cast<uint32_t>(grid) * kU4CtaNominees;
         rp.nominees = c->d_heaps; rp.aux = c->d_u4_aux; rp.max_norm_bits = e->d_max_norm; rp.rho_max = sh.rho_max;
         rp.block_keys = c->d_block_keys; rp.ticket = c->d_ticket; rp.work_counter = sp.work_counter; rp.out = p.out; rp.ok = c->d_ok;
-        rp.frame_ids = p.frame_ids; rp.id_base = p.id_base; rp.row_offset = p.row_offset;
+        rp.frame_ids = p.frame_ids; rp.id_base = p.id_base; rp.row_offset = p.row_offset; rp.row_keys = p.row_keys;
         rp.tail_smem_bytes = static_cast<uint32_t>(grid) * p.k * sizeof(uint64_t);      // <= 132 x 32 keys: no opt-in needed
         if (rp.tail_smem_bytes > 48u * 1024u) rp.tail_smem_bytes = 0;                    // (a wider grid reads them from L2)
         const auto kernel = e->similarity == WAX_VS_COSINE ? shadow_rescore_kernel<kCosine> : shadow_rescore_kernel<kDot>;
@@ -1028,7 +1046,7 @@ static int32_t enqueue_shadow_nominations(wax_vs_engine *e, SearchCtx *c, const 
         fp.kprime = kShadowNominees; fp.k = p.k; fp.metric = e->similarity;
         fp.heaps = c->d_heaps; fp.max_norm_bits = e->d_max_norm;
         fp.out = p.out; fp.ok = c->d_ok;
-        fp.frame_ids = p.frame_ids; fp.id_base = p.id_base; fp.row_offset = p.row_offset;
+        fp.frame_ids = p.frame_ids; fp.id_base = p.id_base; fp.row_offset = p.row_offset; fp.row_keys = p.row_keys;
         fp.pow2_all = 512; fp.rescore = kShadowRescore; fp.eps_rel = sh.eps_rel;
         const size_t fsmem = static_cast<size_t>(fp.pow2_all + fp.rescore) * sizeof(uint64_t);
         const auto kernel = e->similarity == WAX_VS_COSINE ? batch_finish_kernel<kCosine> : batch_finish_kernel<kDot>;
@@ -1099,7 +1117,7 @@ static ScanParams scan_params(const wax_vs_engine *e, SearchCtx *c, const float 
     p.corpus = e->d_corpus; p.query = d_query;
     p.n_rows = static_cast<uint32_t>(e->n_rows); p.dims = e->dims; p.k = k_eff;
     p.block_keys = c->d_block_keys; p.ticket = c->d_ticket; p.out = d_out;
-    p.frame_ids = d_ids; p.id_base = e->id_base; p.row_offset = row_offset;
+    p.frame_ids = d_ids; p.id_base = e->id_base; p.row_offset = row_offset; p.row_keys = c->row_keys;
     p.use_l2_hint = e->tune.l2_hint ? 1u : 0u;
     p.chunk_steps = e->tune.chunk_steps > 0 ? static_cast<uint32_t>(e->tune.chunk_steps) : 0u;
     p.work_counter = c->d_ticket + 1;
@@ -1716,7 +1734,7 @@ static int32_t enqueue_batch_tensor(wax_vs_engine *e, SearchCtx *c, const float 
         fp.n_queries = ch.nq; fp.groups = ch.groups; fp.slices = ch.slices; fp.kprime = ch.kprime; fp.k = k_eff;
         fp.metric = e->similarity; fp.heaps = c->d_heaps; fp.max_norm_bits = e->d_max_norm;
         fp.out = d_out + static_cast<size_t>(ch.q0) * k_eff; fp.ok = d_ok + ch.q0;
-        fp.frame_ids = d_ids; fp.id_base = e->id_base; fp.row_offset = row_offset;
+        fp.frame_ids = d_ids; fp.id_base = e->id_base; fp.row_offset = row_offset; fp.row_keys = c->row_keys;
         uint32_t pow2 = 512;
         while (pow2 < ch.slices * ch.kprime) pow2 <<= 1;
         fp.pow2_all = pow2;
@@ -1818,6 +1836,28 @@ static uint32_t row_of(wax_vs_engine *e, uint64_t id) {
     return id >= e->id_base && id - e->id_base < e->n_rows ? static_cast<uint32_t>(id - e->id_base) : 0xFFFFFFFFu;
 }
 static uint64_t frame_id_of(const wax_vs_engine *e, uint64_t row) { return e->ids_identity ? e->id_base + row : e->ids[row]; }
+// A keyed engine's device key column after a mutation (write lock held): rows [from, n_rows) changed.  A column that has
+// to grow is uploaded whole.
+static int32_t upload_row_keys(wax_vs_engine *e, uint64_t from) {
+    if (!e->keys_set || e->n_rows == 0) return WAX_VS_OK;
+    if (e->d_keys.cap < e->n_rows) {
+        int32_t rc = e->d_keys.ensure(std::max<size_t>(e->n_rows, e->cap_rows), "row keys");
+        if (rc) return rc;
+        from = 0;
+    }
+    if (from < e->n_rows)
+        CUDA_TRY(cudaMemcpy(e->d_keys + from, e->keys.data() + from, (e->n_rows - from) * sizeof(uint64_t),
+                            cudaMemcpyHostToDevice));
+    return WAX_VS_OK;
+}
+// From implicit keys (row r has key r) to an explicit column, before the first keyed mutation.
+static int32_t materialize_row_keys(wax_vs_engine *e) {
+    if (e->keys_set) return WAX_VS_OK;
+    e->keys.resize(e->n_rows);
+    for (uint64_t r = 0; r < e->n_rows; ++r) e->keys[r] = r;
+    e->keys_set = true;
+    return upload_row_keys(e, 0);
+}
 static int32_t sync_device_ids(wax_vs_engine *e, const uint64_t **out) {
     std::lock_guard<std::mutex> g(e->ids_mu);
     if (e->ids_identity) { *out = nullptr; return WAX_VS_OK; }
@@ -2087,20 +2127,30 @@ static int32_t download_bytes(wax_vs_engine *e, void *h_dst, const void *d_src, 
     return WAX_VS_OK;
 }
 
-int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const float *rows, uint64_t n,
-                         uint32_t vector_len) {
+// addBatch for wax_vs_add_batch (first_key nullptr) and wax_vs_add_batch_keyed.  The appended rows of a keyed engine take
+// the keys *first_key, *first_key + 1, ... (nullptr: the keys that follow the last one).
+static int32_t add_batch_rows(wax_vs_engine *e, const uint64_t *frame_ids, const float *rows, uint64_t n,
+                              uint32_t vector_len, const uint64_t *first_key, uint64_t *out_appended) {
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    if (out_appended) *out_appended = 0;
     if (n == 0) return WAX_VS_OK;  // guard !frameIds.isEmpty (:360)
     if (!frame_ids || !rows) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (vector_len != e->dims)     // :367-370
         return fail(WAX_VS_ERR_DIMENSION, "vector dimension mismatch: expected %u, got %u", e->dims, vector_len);
     IngestTrace tr("add_batch");
     std::unique_lock<std::shared_mutex> w(e->rw);
+    if (first_key && e->n_rows > 0) {
+        const uint64_t last = e->keys_set ? e->keys.back() : e->n_rows - 1;
+        if (*first_key <= last)
+            return fail(WAX_VS_ERR_ARGUMENT, "first key %llu is not above the last row key %llu",
+                        static_cast<unsigned long long>(*first_key), static_cast<unsigned long long>(last));
+    }
     DeviceGuard g(e->device);
     drain_device_path(e);
     tr.mark("lock+drain");
     int32_t rc = grow_for(e, e->n_rows + n);  // maxNewCount (:379-380)
     if (rc) return rc;
+    if (first_key && (rc = materialize_row_keys(e))) return rc;
     tr.mark("grow");
     materialize_ids(e);
     tr.mark("ids");
@@ -2146,6 +2196,12 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
         }
     }
     e->d_ids_dirty = true;
+    if (out_appended) *out_appended = e->n_rows - n0;
+    if (e->keys_set) {
+        const uint64_t base = first_key ? *first_key : (n0 ? e->keys.back() + 1 : 0);
+        for (uint64_t r = n0; r < e->n_rows; ++r) e->keys.push_back(base + (r - n0));
+        if ((rc = upload_row_keys(e, n0))) return rc;
+    }
     const size_t row_bytes = static_cast<size_t>(e->dims) * sizeof(float);
     tr.mark("resolve targets");
     if (pure_append) {
@@ -2179,8 +2235,28 @@ int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const floa
     return WAX_VS_OK;
 }
 
+int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const float *rows, uint64_t n,
+                         uint32_t vector_len) {
+    return add_batch_rows(e, frame_ids, rows, n, vector_len, nullptr, nullptr);
+}
+
+int32_t wax_vs_add_batch_keyed(wax_vs_engine *e, const uint64_t *frame_ids, const float *rows, uint64_t n,
+                               uint32_t vector_len, uint64_t first_key, uint64_t *out_appended) {
+    return add_batch_rows(e, frame_ids, rows, n, vector_len, &first_key, out_appended);
+}
+
 int32_t wax_vs_add(wax_vs_engine *e, uint64_t frame_id, const float *vector, uint32_t vector_len) {
     return wax_vs_add_batch(e, &frame_id, vector, 1, vector_len);
+}
+
+int32_t wax_vs_contains(wax_vs_engine *e, const uint64_t *frame_ids, uint64_t n, uint8_t *out) {
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    if (n == 0) return WAX_VS_OK;
+    if (!frame_ids || !out) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    std::lock_guard<std::mutex> g(e->ids_mu);     // row_of may build the id map
+    for (uint64_t i = 0; i < n; ++i) out[i] = row_of(e, frame_ids[i]) != 0xFFFFFFFFu;
+    return WAX_VS_OK;
 }
 
 // remove(frameId:) for a whole set of frames (MetalVectorEngine.swift:423-444 applied n times, as ONE pass): unknown ids
@@ -2259,8 +2335,10 @@ int32_t wax_vs_remove_batch(wax_vs_engine *e, const uint64_t *frame_ids, uint64_
         if (e->attrs_set) e->attrs[first + j] = e->attrs[src[j]];
         if (e->locs_set) e->locs[first + j] = e->locs[src[j]];
         if (e->terms_set) e->term_refs[first + j] = e->term_refs[src[j]];
+        if (e->keys_set) e->keys[first + j] = e->keys[src[j]];
     }
     e->ids.resize(new_n);
+    if (e->keys_set) e->keys.resize(new_n);
     if (e->groups_set) e->groups.resize(new_n);
     if (e->attrs_set) e->attrs.resize(new_n);
     if (e->locs_set) e->locs.resize(new_n);
@@ -2272,6 +2350,7 @@ int32_t wax_vs_remove_batch(wax_vs_engine *e, const uint64_t *frame_ids, uint64_
     e->map_valid = false;
     e->d_ids_dirty = true;
     invalidate_row_caches(e, first);           // rows below the first removed row did not move
+    if ((rc = upload_row_keys(e, first))) return rc;
     tr.mark("compact ids");
     if (out_removed) *out_removed = gone.size();
     return WAX_VS_OK;
@@ -2319,7 +2398,7 @@ static int32_t enqueue_filter_level(wax_vs_engine *e, SearchCtx *c, const float 
         FilterSelectParams sp{};
         sp.cand_count = count; sp.keys = keys; sp.cand_cap = cap; sp.k = k_eff;
         sp.out = d_out + static_cast<size_t>(ch.q0) * k_eff; sp.ok = d_ok + ch.q0;
-        sp.frame_ids = d_ids; sp.id_base = e->id_base; sp.row_offset = row_offset;
+        sp.frame_ids = d_ids; sp.id_base = e->id_base; sp.row_offset = row_offset; sp.row_keys = c->row_keys;
         const size_t ssmem = static_cast<size_t>(cap) * sizeof(uint64_t);
         CUDA_TRY(grant_smem(e, filter_select_kernel, ssmem));
         filter_select_kernel<<<ch.nq, 1024, ssmem, stream>>>(sp);
@@ -2897,6 +2976,7 @@ int32_t wax_vs_debug_time_shard_search(wax_vs_engine *e, uint32_t n_queries, int
     auto &sh = e->shard;
     std::lock_guard<std::mutex> sg(sh.mu);
     SearchCtx *c = sh.ctx;
+    c->row_keys = device_row_keys(e);
     const uint32_t k_eff = clamp_topk(top_k);
     int32_t rc;
     if ((rc = c->d_queries.ensure(static_cast<size_t>(n_queries) * e->dims, "query buffer"))) return rc;
@@ -3325,7 +3405,7 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
             CUDA_TRY(cudaGetLastError());
             ScanParams sp{};
             sp.k = k_max; sp.out = c->d_out + static_cast<size_t>(n_tensor + q0) * k_max; sp.id_base = e->id_base;
-            sp.frame_ids = tgt.d_ids; sp.row_offset = tgt.row_offset;
+            sp.frame_ids = tgt.d_ids; sp.row_offset = tgt.row_offset; sp.row_keys = c->row_keys;
             gather_sort_kernel<<<nq, 1024, pow2 * sizeof(uint64_t), c->stream>>>(keys, span, longest, pow2, sp);
             CUDA_TRY(cudaGetLastError());
             launches += 2;
@@ -4064,6 +4144,7 @@ static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t 
     auto &sh = e->shard;
     std::lock_guard<std::mutex> sg(sh.mu);      // one host-path collective at a time: it owns sh.ctx and h_final
     SearchCtx *c = sh.ctx;
+    c->row_keys = device_row_keys(e);
     const uint64_t *d_ids = nullptr;
     if ((rc = sync_device_ids(e, &d_ids))) return rc;
     uint64_t launches = 0;
@@ -4750,7 +4831,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
             expanded = n_exp;
         }
         if (heads) {
-            ShardRowInfo ri{heads->row_offset, e->id_base, nullptr, e->gindex.row_group, e->gindex.ids};
+            ShardRowInfo ri{heads->row_offset, e->id_base, nullptr, device_row_keys(e), e->gindex.row_group, e->gindex.ids};
             if ((rc = sync_device_ids(e, &ri.ids)) || (rc = c->d_order.ensure(nq, "query order"))) return rc;
             CUDA_TRY(cudaMemcpyAsync(c->d_order, plan.order.data(), nq * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
             const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (nkeys + 255) / 256)));
@@ -4800,7 +4881,8 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
                 const uint32_t row = static_cast<uint32_t>(keys[i]);
                 const uint64_t id = frame_id_of(e, row);
                 recs[i] = wax_vs_group_candidate{host_from_orderable(static_cast<uint32_t>(keys[i] >> 32)), 1u,
-                                                 heads->row_offset + row, id, e->groups_set ? e->groups[row] : id};
+                                                 heads->row_offset + (e->keys_set ? e->keys[row] : row), id,
+                                                 e->groups_set ? e->groups[row] : id};
             }
             CUDA_TRY(cudaMemcpyAsync(heads->d_heads + qi * slots, recs.data(), slots * sizeof(wax_vs_group_candidate),
                                      cudaMemcpyHostToDevice, s));
@@ -5045,7 +5127,7 @@ int32_t wax_vs_shard_grouped_expand_device(wax_vs_engine *e, const float *d_quer
     CUDA_TRY(cudaStreamSynchronize(s));              // the expansion list is on the host
     if ((rc = expand_in_passes(e, c, c->h_bg_expand, n_exp, pair_of, modes.data(), fs, n_top, per_group, &launches, &passes)))
         return rc;
-    ShardRowInfo ri{row_offset, e->id_base, nullptr, gi.row_group, gi.ids};
+    ShardRowInfo ri{row_offset, e->id_base, nullptr, device_row_keys(e), gi.row_group, gi.ids};
     if ((rc = sync_device_ids(e, &ri.ids))) return rc;
     shard_group_expanded_kernel<<<n_exp, 128, 0, s>>>(c->d_bg_expand, c->d_bg_keys, n_top, per_group, ri, d_rows);
     CUDA_TRY(cudaGetLastError());
@@ -5102,7 +5184,8 @@ int32_t wax_vs_serialize(wax_vs_engine *e, uint8_t *dst, uint64_t cap, uint64_t 
     return WAX_VS_OK;
 }
 
-int32_t wax_vs_deserialize(wax_vs_engine *e, const uint8_t *src, uint64_t len) {
+// deserialize for wax_vs_deserialize (all rows, no keys) and wax_vs_deserialize_rows (rows [first, first + n), keyed).
+static int32_t deserialize_rows(wax_vs_engine *e, const uint8_t *src, uint64_t len, bool all, uint64_t first, uint64_t n) {
     if (!e || !src) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::unique_lock<std::shared_mutex> w(e->rw);
     // Reason strings follow MetalVectorEngine.deserialize (:716-815) / VectorSerializer.decodeVecSegment (:84-157).
@@ -5127,19 +5210,31 @@ int32_t wax_vs_deserialize(wax_vs_engine *e, const uint8_t *src, uint64_t len) {
     if (len != 36 + vbytes + 8 + ibytes)
         return fail(WAX_VS_ERR_FORMAT, "vec segment length mismatch: expected %llu, got %llu",
                     static_cast<unsigned long long>(36 + vbytes + 8 + ibytes), static_cast<unsigned long long>(len));
+    if (all) first = 0, n = count;
+    else if (first > count || n > count - first)
+        return fail(WAX_VS_ERR_ARGUMENT, "rows [%llu, %llu + %llu) are outside the segment's %llu rows",
+                    static_cast<unsigned long long>(first), static_cast<unsigned long long>(first),
+                    static_cast<unsigned long long>(n), static_cast<unsigned long long>(count));
+    const size_t row_bytes = static_cast<size_t>(dims) * 4u;
     DeviceGuard g(e->device);
     drain_device_path(e);
-    int32_t rc = set_capacity(e, std::max<uint64_t>(count, 64));  // reservedCapacity = max(...) (:791-792)
+    int32_t rc = set_capacity(e, std::max<uint64_t>(n, 64));  // reservedCapacity = max(...) (:791-792)
     if (rc) return rc;
-    if (vbytes && (rc = upload_bytes(e, e->d_corpus, src + 36, vbytes))) return rc;  // :794-799, pinned double-buffered H2D
-    e->n_rows = count;
-    e->ids.resize(count);
-    if (count) memcpy(e->ids.data(), src + 36 + vbytes + 8, ibytes);  // :809-811
+    if (n && (rc = upload_bytes(e, e->d_corpus, src + 36 + first * row_bytes, n * row_bytes)))  // :794-799, pinned H2D
+        return rc;
+    e->n_rows = n;
+    e->ids.resize(n);
+    if (n) memcpy(e->ids.data(), src + 36 + vbytes + 8 + first * 8, n * 8);  // :809-811
     e->ids_identity = false;
     e->map_valid = false;
     e->ids_sorted = true;
-    for (uint64_t i = 1; i < count && e->ids_sorted; ++i) e->ids_sorted = e->ids[i] > e->ids[i - 1];
+    for (uint64_t i = 1; i < n && e->ids_sorted; ++i) e->ids_sorted = e->ids[i] > e->ids[i - 1];
     e->d_ids_dirty = true;
+    e->keys_set = !all;                     // a slice's rows keep their positions in the segment as keys
+    e->keys.resize(e->keys_set ? n : 0);
+    for (uint64_t i = 0; i < e->keys.size(); ++i) e->keys[i] = first + i;
+    e->keys.shrink_to_fit();
+    if ((rc = upload_row_keys(e, 0))) return rc;
     e->groups_set = false;                  // MV2V has no groups: the caller re-applies them (wax_vs_set_groups)
     e->groups.clear(); e->groups.shrink_to_fit();
     e->attrs_set = false;                   // nor attributes: the caller re-applies them (wax_vs_set_attributes)
@@ -5148,6 +5243,32 @@ int32_t wax_vs_deserialize(wax_vs_engine *e, const uint8_t *src, uint64_t len) {
     e->locs.clear(); e->locs.shrink_to_fit();
     clear_terms(e);
     invalidate_row_caches(e, 0);
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_deserialize(wax_vs_engine *e, const uint8_t *src, uint64_t len) {
+    return deserialize_rows(e, src, len, true, 0, 0);
+}
+
+int32_t wax_vs_deserialize_rows(wax_vs_engine *e, const uint8_t *src, uint64_t len, uint64_t first, uint64_t n) {
+    return deserialize_rows(e, src, len, false, first, n);
+}
+
+int32_t wax_vs_export_rows(wax_vs_engine *e, uint64_t first, uint64_t n, uint64_t *out_ids, float *out_vectors,
+                           uint64_t *out_keys) {
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
+    for (uint64_t i = 0; i < n; ++i) {
+        if (out_ids) out_ids[i] = frame_id_of(e, first + i);
+        if (out_keys) out_keys[i] = e->keys_set ? e->keys[first + i] : first + i;
+    }
+    if (out_vectors && n) {
+        DeviceGuard g(e->device);
+        if (!g.ok) return g.error();
+        std::lock_guard<std::mutex> ig(e->ingest_mu);             // one exporter at a time (as serialize)
+        return download_bytes(e, out_vectors, e->d_corpus + first * e->dims, n * e->dims * sizeof(float));
+    }
     return WAX_VS_OK;
 }
 
@@ -5181,6 +5302,8 @@ int32_t wax_vs_debug_fill_synthetic(wax_vs_engine *e, uint64_t seed, uint64_t fi
     e->ids_identity = true; e->id_base = id_base;
     e->map = IdMap(); e->map_valid = true; e->ids_sorted = true;
     e->d_ids_dirty = true;
+    e->keys_set = false;
+    e->keys.clear(); e->keys.shrink_to_fit();
     e->groups_set = false;
     e->groups.clear(); e->groups.shrink_to_fit();
     e->attrs_set = false;

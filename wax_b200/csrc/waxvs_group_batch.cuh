@@ -175,6 +175,7 @@ __global__ void __launch_bounds__(256) group_score_tile_kernel(const ScoreItem *
 struct ShardRowInfo {
     uint64_t row_offset, id_base;
     const uint64_t *ids;                     // nullptr: identity ids
+    const uint64_t *row_keys;                // keyed shard: global row = row_offset + row_keys[row] (nullptr: + row)
     const uint32_t *row_group;
     const uint64_t *group_ids;
 };
@@ -184,7 +185,7 @@ __device__ __forceinline__ wax_vs_group_candidate shard_group_record(uint64_t ke
         const uint32_t row = static_cast<uint32_t>(key);
         c.distance = from_orderable_u32(static_cast<uint32_t>(key >> 32));
         c.valid = 1u;
-        c.row = ri.row_offset + row;
+        c.row = ri.row_offset + (ri.row_keys ? ri.row_keys[row] : row);
         c.frame_id = ri.ids ? ri.ids[row] : ri.id_base + row;
         c.group_id = ri.group_ids[ri.row_group[row]];
     }

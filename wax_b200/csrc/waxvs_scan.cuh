@@ -45,6 +45,7 @@ struct ScanParams {
     const uint64_t *frame_ids;  // device ids or nullptr (then id = id_base + row)
     uint64_t id_base;
     uint64_t row_offset;        // added to the reported row (shard offset)
+    const uint64_t *row_keys;   // keyed shard: row r is reported as row_offset + row_keys[r] (nullptr = row_offset + r)
     uint32_t use_l2_hint;       // 1: evict-first policy on the corpus stream
     uint32_t chunk_steps;       // > 0: dynamic scheduling, warps claim chunks of this many steps from work_counter
     uint32_t *work_counter;     // zero on entry, zero again on exit (reset by the last CTA)
@@ -97,7 +98,7 @@ __device__ __forceinline__ void write_candidate(const ScanParams &p, int slot, u
         const uint32_t row = static_cast<uint32_t>(key);
         c.distance = from_orderable_u32(static_cast<uint32_t>(key >> 32));
         c.valid = 1;
-        c.row = p.row_offset + row;
+        c.row = p.row_offset + (p.row_keys ? p.row_keys[row] : row);
         c.frame_id = p.frame_ids ? p.frame_ids[row] : p.id_base + row;
     }
     p.out[slot] = c;

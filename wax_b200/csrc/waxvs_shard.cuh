@@ -13,9 +13,9 @@
 //     slot [seq % depth][rank] of EVERY rank's mailbox, fences at system scope, raises flag[slot][rank] = seq on every
 //     rank, then spins on its OWN mailbox until all `world` flags carry seq;
 //   * it merges the world x k candidates (every list is sorted: a candidate's final position is its index plus, for
-//     every other rank, a binary search of its distance in that rank's list -- upper bound for lower ranks, lower
-//     bound for higher ranks, which is exactly the (distance, global row) order because shards are contiguous and
-//     ascending by rank), writes the k best to the result buffer and, for the host entry point, straight into mapped
+//     every other rank, a binary search of its (distance, global row) pair in that rank's list; the rows are read only
+//     when distances tie, and padding is ordered by rank), writes the k best to the result buffer and, for the host
+//     entry point, straight into mapped
 //     pinned host memory followed by a host-visible flag: no collective launch, no D2H copy, no host merge;
 //   * slot reuse is guarded by acknowledgements (acks[r] = last seq rank r has finished reading from its own mailbox),
 //     so any number of queries may be in flight on any streams.
@@ -113,14 +113,18 @@ __device__ __noinline__ void shard_exchange_cta(const ShardParams &sh, const wax
     __syncthreads();
     for (uint32_t i = tid; i < total; i += nthr) {
         const uint32_t r = i / k, j = i % k, key = skeys[i];
+        const unsigned long long row = key == WAXVS_UKEY_NONE ? 0ull : ld_cg_u64(reinterpret_cast<const uint64_t *>(&mine->cands[slot][r][j]) + 1);
         uint32_t pos = j;
         for (uint32_t r2 = 0; r2 < sh.world && pos < k; ++r2) {
             if (r2 == r) continue;
             const uint32_t *lst = skeys + r2 * k;
             uint32_t lo = 0, hi = k;
-            while (lo < hi) {                       // lower ranks hold lower global rows: their equal distances come first
+            while (lo < hi) {                       // entries before (key, row); equal distances read the rows
                 const uint32_t mid = (lo + hi) >> 1, v = lst[mid];
-                const bool before = (r2 < r) ? (v <= key) : (v < key);
+                bool before = v < key;
+                if (v == key)
+                    before = key == WAXVS_UKEY_NONE ? r2 < r
+                                                    : ld_cg_u64(reinterpret_cast<const uint64_t *>(&mine->cands[slot][r2][mid]) + 1) < row;
                 if (before) lo = mid + 1; else hi = mid;
             }
             pos += lo;
@@ -157,9 +161,15 @@ __global__ void __launch_bounds__(256) shard_exchange_kernel(const ShardParams s
 // of the ranks' per-query lists leaves them (every list sorted, padding valid = 0 last); out = [n_queries][k_out], the
 // k_out best of each query under (distance, GLOBAL row) -- the position rule of shard_exchange_cta, binary searches in
 // global memory.  One CTA per query.  Replaces a host-side numpy merge, which costs more than a shard's tensor-core
-// pass.
+// pass.  The rule needs no order between the ranks' rows, so it holds for keyed shards, whose rows interleave.
 __device__ __forceinline__ uint32_t cand_dist_key(const wax_vs_candidate &c) {
     return c.valid ? orderable_u32(c.distance) : WAXVS_UKEY_NONE;
+}
+// Candidate (km, m) of rank o comes before candidate (key, c) of rank r: by distance, then global row; padding by rank.
+__device__ __forceinline__ bool cand_before(uint32_t km, const wax_vs_candidate &m, uint32_t o, uint32_t key,
+                                            const wax_vs_candidate &c, uint32_t r) {
+    if (km != key) return km < key;
+    return key == WAXVS_UKEY_NONE ? o < r : m.row < c.row;
 }
 __global__ void __launch_bounds__(128) merge_gathered_kernel(const wax_vs_candidate *__restrict__ gathered, uint32_t world,
                                                              uint32_t n_queries, uint32_t k, uint32_t k_out,
@@ -175,11 +185,10 @@ __global__ void __launch_bounds__(128) merge_gathered_kernel(const wax_vs_candid
         for (uint32_t o = 0; o < world; ++o) {
             if (o == r) continue;
             const wax_vs_candidate *lst = mine + o * rank_stride;
-            uint32_t lo = 0, hi = k;                 // lower ranks: entries <= key come first; higher ranks: entries < key
+            uint32_t lo = 0, hi = k;
             while (lo < hi) {
                 const uint32_t mid = (lo + hi) >> 1;
-                const uint32_t km = cand_dist_key(lst[mid]);
-                if (o < r ? km <= key : km < key) lo = mid + 1; else hi = mid;
+                if (cand_before(cand_dist_key(lst[mid]), lst[mid], o, key, c, r)) lo = mid + 1; else hi = mid;
             }
             pos += lo;
         }
@@ -191,8 +200,8 @@ __global__ void __launch_bounds__(128) merge_gathered_kernel(const wax_vs_candid
 // Sharded grouped search, merge 1 (wax_vs_merge_group_heads_device): the ranks' round-1 answers gathered as
 // [world][n_queries][G][P] -> per query the global top G groups, each as its best row.  A group's head on a rank is its
 // best row there, so its global head is the best of its heads; a group is ranked by that head in (distance, GLOBAL row).
-// Each rank's heads are in that order and lower ranks hold lower rows, so (distance key, rank * G + slot) orders the
-// heads exactly as (distance, global row) does.
+// The heads are sorted by their rows first, and then by (distance key, row rank), which is (distance, global row) for any
+// placement of rows on ranks.
 constexpr uint32_t kShardMaxGroups = 256;   // = WAX_VS_SHARD_MAX_GROUPS: world * G <= 4 096 heads in shared memory
 
 // Sorts (key[i], val[i]) pairs ascending by key, then val (pow2 entries, every thread of the CTA).
@@ -228,12 +237,12 @@ __global__ void __launch_bounds__(1024) merge_group_heads_kernel(const wax_vs_gr
     auto head = [&](uint32_t i) -> const wax_vs_group_candidate & {
         return gathered[(i / n_top) * rank_stride + (static_cast<size_t>(q) * n_top + i % n_top) * per_group];
     };
-    // 1. every rank's heads in (distance, global row) order
+    // 1. every rank's heads in (distance, global row) order: the rank of each head's row, then (distance key, row rank)
     uint32_t mine = 0;
     for (uint32_t i = t; i < pow2; i += blockDim.x) {
         const bool v = i < heads && head(i).valid;
-        s_key[i] = v ? orderable_u32(head(i).distance) : ~0ull;
-        s_val[i] = v ? i : 0xFFFFFFFFu;
+        s_key[i] = v ? head(i).row : ~0ull;
+        s_val[i] = i;
         mine += v;
     }
     for (uint32_t i = t; i < pow2; i += blockDim.x) s_keep[i] = 0;
@@ -241,6 +250,15 @@ __global__ void __launch_bounds__(1024) merge_group_heads_kernel(const wax_vs_gr
     __syncthreads();
     atomicAdd(&s_total, mine);
     block_bitonic_sort_pairs(s_key, s_val, pow2);                       // ends in __syncthreads
+    for (uint32_t p = t; p < pow2; p += blockDim.x) s_head[s_val[p]] = p;
+    __syncthreads();
+    for (uint32_t i = t; i < pow2; i += blockDim.x) {
+        const bool v = i < heads && head(i).valid;
+        s_key[i] = v ? (static_cast<uint64_t>(orderable_u32(head(i).distance)) << 32 | s_head[i]) : ~0ull;
+        s_val[i] = v ? i : 0xFFFFFFFFu;
+    }
+    __syncthreads();
+    block_bitonic_sort_pairs(s_key, s_val, pow2);
     const uint32_t valid = s_total;
     // 2. by (group id, position): the first position of each group id is its best head
     for (uint32_t p = t; p < pow2; p += blockDim.x) {

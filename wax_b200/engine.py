@@ -800,6 +800,53 @@ class CUDAVectorEngine:
     def reserve(self, rows: int) -> None:
         _check(L.lib().wax_vs_reserve(self._h, int(rows)))
 
+    # -- row keys: the rank-local store of the row-sharded engine (DESIGN.md section 4.15)
+    def add_batch_keyed(self, frame_ids: Sequence[int], vectors, first_key: int) -> int:
+        """add_batch whose appended rows take the keys first_key, first_key + 1, ... (wax_vs_add_batch_keyed); returns how
+        many rows it appended.  A first_key not above the last row's key raises WaxError."""
+        ids = np.ascontiguousarray(frame_ids, dtype=np.uint64).reshape(-1)
+        if ids.size == 0:
+            return 0
+        if ids.size != len(vectors):
+            raise EncodingError("addBatch: frameIds.count != vectors.count")
+        rows = _as_rows(vectors, self.dimensions)
+        appended = C.c_uint64(0)
+        _check(L.lib().wax_vs_add_batch_keyed(self._h, ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                              rows.ctypes.data_as(C.POINTER(C.c_float)), ids.size, rows.shape[1],
+                                              int(first_key), C.byref(appended)))
+        self._dirty = True
+        return appended.value
+
+    def contains(self, frame_ids: Sequence[int]) -> np.ndarray:
+        """[n] bool: whether this engine holds each frame id."""
+        ids = np.ascontiguousarray(frame_ids, dtype=np.uint64).reshape(-1)
+        out = np.zeros(ids.size, np.uint8)
+        if ids.size:
+            _check(L.lib().wax_vs_contains(self._h, ids.ctypes.data_as(C.POINTER(C.c_uint64)), ids.size,
+                                           out.ctypes.data_as(C.POINTER(C.c_uint8))))
+        return out.astype(bool)
+
+    def deserialize_rows(self, data: bytes, first: int, n: int) -> None:
+        """Replace the contents with rows [first, first + n) of an MV2V blob, keyed first, first + 1, ...
+        (wax_vs_deserialize_rows: the blob is checked as deserialize() checks it)."""
+        buf = np.frombuffer(data, np.uint8)
+        ptr = buf.ctypes.data_as(C.POINTER(C.c_uint8)) if buf.size else C.cast(C.c_char_p(b""), C.POINTER(C.c_uint8))
+        _check(L.lib().wax_vs_deserialize_rows(self._h, ptr, buf.size, int(first), int(n)))
+        self._dirty = False
+
+    def export_rows(self, first: int, n: int, vectors: bool = True):
+        """Rows [first, first + n): (frame ids uint64 [n], vectors float32 [n, dims] or None, keys uint64 [n])."""
+        ids, keys = np.empty(n, np.uint64), np.empty(n, np.uint64)
+        vecs = np.empty((n, self.dimensions), np.float32) if vectors else None
+        _check(L.lib().wax_vs_export_rows(self._h, int(first), int(n), ids.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                          vecs.ctypes.data_as(C.POINTER(C.c_float)) if vectors else None,
+                                          keys.ctypes.data_as(C.POINTER(C.c_uint64))))
+        return ids, vecs, keys
+
+    def row_keys(self) -> np.ndarray:
+        """Every row's key, in row order (the row itself on an engine without keys)."""
+        return self.export_rows(0, self.count, vectors=False)[2]
+
     # -- row-sharded search (wax_vs_shard_*; no reference counterpart, SURVEY.md section 8e) ------------------------------
     def shard_open(self, rank: int, world: int, row_offset: int) -> bytes:
         """Become rank `rank` of `world`: allocates this engine's mailbox and returns the handle blob the other ranks

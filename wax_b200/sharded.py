@@ -1,7 +1,8 @@
 """Row-sharded vector search across GPUs: one process (rank) per GPU, one CUDA engine per rank.
 
-Design (SURVEY.md section 8e; BASELINE.json north_star): contiguous row ranges per rank, the query
-replicated, the identical fused kernel on every shard, ONE exchange of the per-shard top-k candidates
+Design (SURVEY.md section 8e; BASELINE.json north_star): rows spread over the ranks (contiguous ranges for
+fill_synthetic, or keyed by insertion order for a corpus the collective corpus methods keep, DESIGN.md section 4.15), the
+query replicated, the identical fused kernel on every shard, ONE exchange of the per-shard top-k candidates
 (k x 24 B per rank) and a merge under the same total order (distance ascending, GLOBAL row ascending), so
 results do not depend on the shard count.  Nothing else is exchanged.
 
@@ -37,6 +38,74 @@ def shard_range(total_rows: int, world_size: int, rank: int) -> Tuple[int, int]:
     lo = (total_rows * rank) // world_size
     hi = (total_rows * (rank + 1)) // world_size
     return lo, hi
+
+
+# -- corpus planning (DESIGN.md section 4.15): pure functions, so that the tests can drive ranks without a process group.
+# A row's key is its insertion sequence number in the whole corpus; ordering rows by key is the single engine's row order.
+def fill_emptiest(counts: Sequence[int], m: int) -> np.ndarray:
+    """How many of m new rows each rank takes: the ranks with the fewest rows first, to one level (ties to lower ranks)."""
+    counts = np.asarray(counts, np.int64)
+    alloc = np.zeros(counts.size, np.int64)
+    if m <= 0:
+        return alloc
+    lo, hi = int(counts.min()), int(counts.max()) + m           # the largest level L with sum(max(0, L - count)) <= m
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        if int(np.maximum(mid - counts, 0).sum()) <= m:
+            lo = mid
+        else:
+            hi = mid - 1
+    alloc = np.maximum(lo - counts, 0)
+    rest = m - int(alloc.sum())                                 # fewer than the ranks at the level: one more each
+    at_level = np.flatnonzero(counts + alloc == lo)[:rest]
+    alloc[at_level] += 1
+    return alloc
+
+
+def plan_add_batch(frame_ids, owner, counts: Sequence[int], next_key: int):
+    """Where each item of a sharded add_batch goes.  `owner` [n]: the rank holding each id before the batch (-1: none);
+    `counts`: rows per rank; `next_key`: the first unused key.  Held ids are upserted by their owner.  The distinct new
+    ids, in order of first appearance, take the keys next_key, next_key + 1, ... and are split in contiguous chunks over
+    the ranks (fill_emptiest, chunks in rank order); every occurrence of an id goes where its first one goes.
+    Returns (dest [n] rank of each item, first_key [world] of each rank's chunk, appended [world], the next unused key)."""
+    ids = np.asarray(frame_ids, np.uint64).reshape(-1)
+    owner = np.asarray(owner, np.int64).reshape(-1)
+    dest = owner.copy()
+    new = np.flatnonzero(owner < 0)
+    uniq, first, inverse = np.unique(ids[new], return_index=True, return_inverse=True)
+    order = np.argsort(first, kind="stable")                    # distinct new ids in batch order
+    seq = np.empty(uniq.size, np.int64)
+    seq[order] = np.arange(uniq.size)                           # sequence number of each distinct new id
+    alloc = fill_emptiest(counts, uniq.size)
+    start = np.concatenate([[0], np.cumsum(alloc)[:-1]])
+    dest[new] = np.searchsorted(np.cumsum(alloc), seq[inverse.reshape(-1)], side="right")
+    return dest, int(next_key) + start, alloc, int(next_key) + uniq.size
+
+
+def plan_serialize(keys: Sequence[np.ndarray]) -> List[np.ndarray]:
+    """The MV2V position of every rank's rows: rows ordered by key, which is the single engine's order.  keys[r] = rank r's
+    keys in row order (strictly increasing)."""
+    flat = np.concatenate([np.asarray(k, np.uint64).reshape(-1) for k in keys] + [np.zeros(0, np.uint64)])
+    pos = np.empty(flat.size, np.int64)
+    pos[np.argsort(flat, kind="stable")] = np.arange(flat.size)
+    bounds = np.cumsum([0] + [len(k) for k in keys])
+    return [pos[bounds[r]:bounds[r + 1]] for r in range(len(keys))]
+
+
+def mv2v_header(similarity: int, dims: int, count: int) -> bytes:
+    """The 36-byte MV2V v1 encoding-2 header (MetalVectorEngine.swift:686-700)."""
+    return (b"MV2V" + np.uint16(1).tobytes() + bytes([2, similarity]) + np.uint32(dims).tobytes() +
+            np.uint64(count).tobytes() + np.uint64(count * dims * 4).tobytes() + bytes(8))
+
+
+def mv2v_count(blob) -> int:
+    """The row count an MV2V header states (0 when the blob is too short to hold one: the load then reports why)."""
+    return int(np.frombuffer(blob, np.uint64, 1, 12)[0]) if len(blob) >= 36 else 0
+
+
+def shard_counts(total_rows: int, world_size: int) -> np.ndarray:
+    """[world] rows of each shard_range."""
+    return np.diff([shard_range(total_rows, world_size, r)[0] for r in range(world_size)] + [total_rows]).astype(np.int64)
 
 
 def clamp_topk(top_k: int) -> int:
@@ -82,10 +151,15 @@ class ShardedVectorEngine:
     local_search: optional injection point used by the CPU (gloo) tests of the host-side logic -- a callable
     (query ndarray, k) -> ndarray[CAND_DTYPE] of length k.  In production it is None and the local step is
     wax_vs_search_device on the rank's GPU.
+
+    Two ways to hold a corpus: `total_rows` > 0 with fill_synthetic (contiguous row ranges), or an empty engine filled by
+    the collective corpus methods (add_batch, remove_batch, deserialize, ...; DESIGN.md section 4.15), which place rows
+    on any rank and key them by insertion order.  local_store: optional stand-in for the rank's engine in those methods
+    (the CPU tests); it needs count, contains, add_batch_keyed, remove_batch, deserialize_rows and export_rows.
     """
 
     def __init__(self, metric, dimensions: int, total_rows: int = 0, group=None,
-                 local_search: Optional[Callable[[np.ndarray, int], np.ndarray]] = None, device=None):
+                 local_search: Optional[Callable[[np.ndarray, int], np.ndarray]] = None, device=None, local_store=None):
         import torch
         import torch.distributed as dist
         self._torch, self._dist = torch, dist
@@ -96,11 +170,15 @@ class ShardedVectorEngine:
         self.dimensions = int(dimensions)
         self.total_rows = int(total_rows)
         self.row_lo, self.row_hi = shard_range(self.total_rows, self.world_size, self.rank)
+        # corpus bookkeeping, the same on every rank: rows per rank and the next unused row key
+        self._counts = shard_counts(self.total_rows, self.world_size)
+        self._next_key = self.total_rows
+        self._contiguous = self.world_size > 1 and self.total_rows > 0     # fill_synthetic's ranges: no corpus methods
         self._local_search = local_search
         self.engine = None
         self._bufs = {}
         self._comm_stream = None
-        if local_search is None:
+        if local_search is None and local_store is None:
             from .engine import CUDAVectorEngine
             self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
             self.engine = CUDAVectorEngine(metric, dimensions, device=self.device.index)
@@ -117,6 +195,7 @@ class ShardedVectorEngine:
         else:
             self.device = torch.device("cpu")
             self.transport = "allgather"
+            self.engine = local_store
 
     def _connect_peers(self) -> None:
         """Create this rank's mailbox, exchange the handles (one all-gather of 128 bytes per rank, the only use of
@@ -169,6 +248,145 @@ class ShardedVectorEngine:
         """Each rank generates its own shard on device; frameId = global row."""
         self.engine.fill_synthetic(seed, self.row_hi - self.row_lo, first_row=self.row_lo, id_base=self.row_lo,
                                    normalize=normalize)
+
+    # -- corpus: collective, every rank passes the same arguments (DESIGN.md section 4.15)
+    def _check_corpus_methods(self) -> None:
+        if self._contiguous:
+            from .engine import InvalidToc
+            raise InvalidToc("the corpus methods need an engine built without total_rows (this one holds contiguous "
+                             "ranges for fill_synthetic)")
+
+    def _sum_on_ranks(self, values: np.ndarray) -> np.ndarray:
+        """Element-wise sum of an int64 vector over the ranks (one all-reduce)."""
+        if self.world_size == 1:
+            return values
+        torch, dist = self._torch, self._dist
+        dev = self.device if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
+        t = torch.from_numpy(np.ascontiguousarray(values, np.int64)).to(dev)
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
+        return t.cpu().numpy()
+
+    def _gather_to_root(self, values: np.ndarray) -> Optional[np.ndarray]:
+        """[world, ...] on rank 0 (None elsewhere): every rank's equally shaped int64 array."""
+        if self.world_size == 1:
+            return values[None]
+        torch, dist = self._torch, self._dist
+        dev = self.device if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
+        t = torch.from_numpy(np.ascontiguousarray(values, np.int64)).to(dev)
+        parts = [torch.empty_like(t) for _ in range(self.world_size)] if self.rank == 0 else None
+        dist.gather(t, parts, dst=0, group=self.group)
+        return np.stack([p.cpu().numpy() for p in parts]) if self.rank == 0 else None
+
+    def _set_counts(self, counts: np.ndarray) -> None:
+        self._counts = np.asarray(counts, np.int64)
+        self.total_rows = int(self._counts.sum())
+
+    def count(self) -> int:
+        """vectorCount of the whole sharded corpus (the same on every rank)."""
+        return self.total_rows
+
+    def add_batch(self, frame_ids: Sequence[int], vectors) -> None:
+        """addBatch over the sharded corpus (collective): the same answer, row order and MV2V bytes as one engine given
+        the same history.  One all-reduce finds each id's owner; owned ids are upserted in place, the new ones go to the
+        ranks with the fewest rows (plan_add_batch)."""
+        self._check_corpus_methods()
+        ids = np.ascontiguousarray(frame_ids, dtype=np.uint64).reshape(-1)
+        if ids.size == 0:
+            return
+        from .engine import EncodingError, _as_rows
+        if ids.size != len(vectors):
+            raise EncodingError("addBatch: frameIds.count != vectors.count")
+        rows = _as_rows(vectors, self.dimensions)
+        held = np.zeros(ids.size + self.world_size, np.int64)
+        held[:ids.size] = np.where(self.engine.contains(ids), self.rank + 1, 0)
+        held[ids.size + self.rank] = self.engine.count
+        held = self._sum_on_ranks(held)
+        dest, first_key, appended, next_key = plan_add_batch(ids, held[:ids.size] - 1, held[ids.size:], self._next_key)
+        mine = np.flatnonzero(dest == self.rank)
+        if mine.size:
+            if mine.size == ids.size:                      # the whole batch (always at world 1): no copy
+                mine = slice(None)
+            got = self.engine.add_batch_keyed(ids[mine], rows[mine], int(first_key[self.rank]))
+            assert got == appended[self.rank], (got, appended[self.rank])
+        self._set_counts(held[ids.size:] + appended)
+        self._next_key = next_key
+
+    def add(self, frame_id: int, vector: Sequence[float]) -> None:
+        """add(frameId:vector:) over the sharded corpus (collective)."""
+        self.add_batch([frame_id], np.asarray(vector, np.float32).reshape(1, -1))
+
+    def remove_batch(self, frame_ids: Sequence[int]) -> int:
+        """remove(frameId:) for many frames over the sharded corpus (collective): every rank removes the ids it holds,
+        the survivors keep their keys.  Returns how many rows went, over all ranks."""
+        self._check_corpus_methods()
+        ids = np.ascontiguousarray(frame_ids, dtype=np.uint64).reshape(-1)
+        gone = np.zeros(self.world_size, np.int64)
+        gone[self.rank] = self.engine.remove_batch(ids) if ids.size else 0
+        gone = self._sum_on_ranks(gone)
+        self._set_counts(self._counts - gone)
+        return int(gone.sum())
+
+    def remove(self, frame_id: int) -> None:
+        """remove(frameId:) over the sharded corpus (collective)."""
+        self.remove_batch([frame_id])
+
+    def deserialize(self, data) -> None:
+        """Load an MV2V blob (collective, the same bytes on every rank): rank r loads the rows shard_range gives it, keyed
+        by their positions in the blob.  A blob deserialize() would refuse is refused on every rank alike."""
+        self._check_corpus_methods()
+        count = mv2v_count(data)
+        lo, hi = shard_range(count, self.world_size, self.rank)
+        self.engine.deserialize_rows(data, lo, hi - lo)
+        self._set_counts(shard_counts(count, self.world_size))
+        self._next_key = count
+
+    def serialize(self, chunk_rows: int = 1 << 16):
+        """MV2V bytes of the whole corpus on rank 0 (None on the others): what CUDAVectorEngine.serialize gives for the
+        same history.  Collective: the ranks gather their keys on rank 0, then send their rows in chunks of at most
+        `chunk_rows`, which rank 0 places by key (plan_serialize)."""
+        self._check_corpus_methods()
+        count, dims, root = self.engine.count, self.dimensions, self.rank == 0
+        counts = self._sum_on_ranks(np.eye(self.world_size, dtype=np.int64)[self.rank] * count)
+        width, total = int(counts.max()), int(counts.sum())
+        keys = np.zeros(width, np.uint64)
+        keys[:count] = self.engine.export_rows(0, count, vectors=False)[2]
+        all_keys = self._gather_to_root(keys.view(np.int64))
+        if root:
+            pos = plan_serialize([all_keys[r, :counts[r]].view(np.uint64) for r in range(self.world_size)])
+            out = bytearray(36 + total * dims * 4 + 8 + total * 8)
+            out[:36] = mv2v_header(self.metric.to_vec_similarity(), dims, total)
+            vbytes = total * dims * 4
+            vecs = np.frombuffer(out, np.float32, total * dims, 36).reshape(total, dims)
+            out[36 + vbytes:44 + vbytes] = np.uint64(total * 8).tobytes()
+            ids_out = np.frombuffer(out, np.uint64, total, 44 + vbytes)
+
+        def place(dst, ids, vec):
+            """Rows at MV2V positions `dst` (increasing: a rank's keys increase); a consecutive run is one slice copy."""
+            if dst.size and dst[-1] - dst[0] == dst.size - 1:
+                dst = slice(int(dst[0]), int(dst[-1]) + 1)
+            ids_out[dst], vecs[dst] = ids, vec
+
+        rec = (8 + 4 * dims + 7) // 8 * 8                          # one row on the wire: its id, then its vector
+        for first in range(0, width, max(1, int(chunk_rows))):
+            m = min(int(chunk_rows), width - first)
+            have = max(0, min(m, count - first))
+            ids, vec, _ = self.engine.export_rows(first, have) if have else (None, None, None)
+            if root and have:                                       # rank 0's own rows skip the wire
+                place(pos[0][first:first + have], ids, vec)
+            if self.world_size == 1:
+                continue
+            wire = np.zeros((m, rec), np.uint8)
+            if have and not root:
+                wire[:have, :8] = ids.view(np.uint8).reshape(have, 8)
+                wire[:have, 8:8 + 4 * dims] = vec.view(np.uint8).reshape(have, 4 * dims)
+            got = self._gather_to_root(wire.view(np.int64).reshape(-1))
+            if root:
+                got = got.view(np.uint8).reshape(self.world_size, m, rec)
+                for r in range(1, self.world_size):
+                    n_r = max(0, min(m, int(counts[r]) - first))
+                    place(pos[r][first:first + n_r], np.ascontiguousarray(got[r, :n_r, :8]).view(np.uint64).reshape(-1),
+                          np.ascontiguousarray(got[r, :n_r, 8:8 + 4 * dims]).view(np.float32))
+        return out if root else None
 
     # -- search
     def _buffers(self, k: int, slot: int = 0):
