@@ -71,9 +71,23 @@ int32_t wax_vs_device_count(int32_t *out);
 /* MetalVectorEngine.init(metric:dimensions:) (MetalVectorEngine.swift:153-274).  Unlike the Metal
    engine (cosine only, :163-165) all three metrics are supported, with USearchVectorEngine's
    semantics (USearchVectorEngine.swift:44-67; VectorMetric.swift:21-30).  `devices`/`n_devices`: the
-   CUDA ordinals to use; NULL/0 = current device.  This build places one engine on one device
-   (n_devices must be <= 1); row-sharding across GPUs is one engine per rank + wax_vs_search_device +
-   one all-gather (wax_b200/sharded.py). */
+   CUDA ordinals to use; NULL/0 = current device, 1 = that device.
+   n_devices >= 2 returns a MULTI-DEVICE handle: the corpus sharded by rows over n_devices shards, shard r on devices[r]
+   (DESIGN.md section 4.16).  Every answer it gives equals that of one engine with the same call history, bit for bit:
+   ids, order, score bits, counts, MV2V bytes, error codes and reasons.  It serves wax_vs_dimensions, _similarity,
+   _count, _reserve, _add, _add_batch, _remove, _remove_batch, _search, _search_batch, _search_filtered,
+   _search_batch_filtered, _search_batch_multi_filtered, _set_attributes, _set_locations, _set_terms,
+   _search_batch_where, _where_near, _where_terms, _set_groups, _search_grouped, _search_batch_grouped, _grouped_where,
+   _grouped_where_near, _grouped_multi_where, _serialized_length, _serialize, _deserialize, wax_vs_debug_set_option
+   (applied to every shard) and wax_vs_debug_counter (summed over the shards, plus "shard_rows.<r>": shard r's rows);
+   every other entry point (the rank-level shard_*, *_device, keyed and merge entries, the other debug_*) returns
+   WAX_VS_ERR_UNSUPPORTED naming itself.  Grouped search with clamp(top_groups) > WAX_VS_SHARD_MAX_GROUPS is refused as
+   the sharded grouped form refuses it.  An ordinal
+   may repeat ({0, 0, 0}): the shards then share that device, a test and debug configuration.  Checked before any
+   device query: n_devices > WAX_VS_SHARD_MAX_RANKS or a negative ordinal -> WAX_VS_ERR_ARGUMENT, NULL devices ->
+   WAX_VS_ERR_NULL.  Two distinct devices that cannot access each other's memory -> WAX_VS_ERR_UNSUPPORTED.
+   Multi-process and multi-node sharding is one engine per rank + wax_vs_search_device + one all-gather
+   (wax_b200/sharded.py). */
 int32_t wax_vs_create(uint32_t dimensions, uint8_t similarity, const int32_t *devices, int32_t n_devices,
                       wax_vs_engine **out);
 void wax_vs_destroy(wax_vs_engine *engine);

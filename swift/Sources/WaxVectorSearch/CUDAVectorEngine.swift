@@ -29,13 +29,20 @@ public actor CUDAVectorEngine {
         return wax_vs_device_count(&n) == WAX_VS_OK && n > 0
     }
 
-    public init(metric: VectorMetric, dimensions: Int) throws {
+    /// `devices`: the CUDA ordinals to use; empty = the current device.  Two or more make a multi-device handle: the
+    /// corpus sharded by rows, shard r on devices[r], every answer equal to one engine's (an ordinal may repeat: shards
+    /// then share that device, a test and debug configuration).
+    public init(metric: VectorMetric, dimensions: Int, devices: [Int32] = []) throws {
         guard dimensions > 0 else { throw WaxError.invalidToc(reason: "dimensions must be > 0") }
         guard dimensions <= Constants.maxEmbeddingDimensions else {
             throw WaxError.capacityExceeded(limit: UInt64(Constants.maxEmbeddingDimensions), requested: UInt64(dimensions))
         }
         var h: OpaquePointer?
-        let rc = wax_vs_create(UInt32(dimensions), metric.toVecSimilarity().rawValue, nil, 0, &h)
+        let rc = devices.isEmpty
+            ? wax_vs_create(UInt32(dimensions), metric.toVecSimilarity().rawValue, nil, 0, &h)
+            : devices.withUnsafeBufferPointer {
+                wax_vs_create(UInt32(dimensions), metric.toVecSimilarity().rawValue, $0.baseAddress, Int32($0.count), &h)
+            }
         guard rc == WAX_VS_OK, let h else { throw Self.error(rc) }   // catchable: callers fall back to USearch (WaxSession.swift:484-497)
         self.handle = h
         self.metric = metric

@@ -287,7 +287,10 @@ struct SearchCtx {
     }
 };
 
+struct MultiEngine;   // waxvs_multi.cuh
+
 struct wax_vs_engine {
+    MultiEngine *multi = nullptr;   // a multi-device handle (n_devices >= 2): its shards and state, else nullptr
     int device = 0;
     int sm_count = 132;
     size_t smem_optin = 0;
@@ -1872,6 +1875,8 @@ static int32_t sync_device_ids(wax_vs_engine *e, const uint64_t **out) {
     return WAX_VS_OK;
 }
 
+#include "waxvs_multi.cuh"
+
 // ---------------------------------------------------------------------------------------------------------
 // C-ABI
 extern "C" {
@@ -1896,8 +1901,14 @@ int32_t wax_vs_create(uint32_t dimensions, uint8_t similarity, const int32_t *de
     if (dimensions > WAX_VS_MAX_DIMENSIONS)                                           // :157-162
         return fail(WAX_VS_ERR_CAPACITY, "capacity exceeded: limit %d, requested %u", WAX_VS_MAX_DIMENSIONS, dimensions);
     if (similarity > 2) return fail(WAX_VS_ERR_ARGUMENT, "vec similarity must be 0..2 (got %u)", similarity);
-    if (n_devices > 1)
-        return fail(WAX_VS_ERR_UNSUPPORTED, "one engine drives one device; shard with one engine per rank (wax_vs_search_device)");
+    if (n_devices > 1) {               // a multi-device handle (waxvs_multi.cuh): its own checks come before any device query
+        if (n_devices > WAX_VS_SHARD_MAX_RANKS)
+            return fail(WAX_VS_ERR_ARGUMENT, "%d devices: a multi-device handle takes at most %d", n_devices, WAX_VS_SHARD_MAX_RANKS);
+        if (!devices) return fail(WAX_VS_ERR_NULL, "devices is NULL");
+        for (int32_t r = 0; r < n_devices; ++r)
+            if (devices[r] < 0) return fail(WAX_VS_ERR_ARGUMENT, "device ordinal %d is negative", devices[r]);
+        return multi_create(dimensions, similarity, devices, n_devices, out);
+    }
     int count = 0;
     if (cudaGetDeviceCount(&count) != cudaSuccess || count <= 0) {
         cudaGetLastError();
@@ -1927,6 +1938,7 @@ int32_t wax_vs_create(uint32_t dimensions, uint8_t similarity, const int32_t *de
 
 void wax_vs_destroy(wax_vs_engine *e) {
     if (!e) return;
+    if (e->multi) { multi_destroy(e->multi); delete e; return; }
     DeviceGuard g(e->device);      // the engine's own buffers go with `delete e`: on its device too
     {
         std::unique_lock<std::shared_mutex> w(e->rw);
@@ -1940,6 +1952,7 @@ void wax_vs_destroy(wax_vs_engine *e) {
 }
 
 int32_t wax_vs_dimensions(const wax_vs_engine *e, uint32_t *out) {
+    if (e && e->multi && out) { *out = e->dims; return WAX_VS_OK; }
     if (!e || !out) return fail(WAX_VS_ERR_NULL, "NULL argument");
     *out = e->dims;
     return WAX_VS_OK;
@@ -1950,6 +1963,7 @@ int32_t wax_vs_similarity(const wax_vs_engine *e, uint8_t *out) {
     return WAX_VS_OK;
 }
 int32_t wax_vs_count(wax_vs_engine *e, uint64_t *out) {
+    if (e && e->multi && out) { std::shared_lock<std::shared_mutex> r(e->multi->rw); *out = e->multi->total(); return WAX_VS_OK; }
     if (!e || !out) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     *out = e->n_rows;
@@ -1957,6 +1971,7 @@ int32_t wax_vs_count(wax_vs_engine *e, uint64_t *out) {
 }
 
 int32_t wax_vs_reserve(wax_vs_engine *e, uint64_t rows) {
+    if (e && e->multi) return multi_reserve(e->multi, rows);
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     if (rows > 0xFFFFFFFFull)
         return fail(WAX_VS_ERR_CAPACITY, "capacity exceeded: limit %llu, requested %llu", 0xFFFFFFFFull,
@@ -2237,11 +2252,13 @@ static int32_t add_batch_rows(wax_vs_engine *e, const uint64_t *frame_ids, const
 
 int32_t wax_vs_add_batch(wax_vs_engine *e, const uint64_t *frame_ids, const float *rows, uint64_t n,
                          uint32_t vector_len) {
+    if (e && e->multi) return multi_add_batch(e->multi, frame_ids, rows, n, e->dims, vector_len);
     return add_batch_rows(e, frame_ids, rows, n, vector_len, nullptr, nullptr);
 }
 
 int32_t wax_vs_add_batch_keyed(wax_vs_engine *e, const uint64_t *frame_ids, const float *rows, uint64_t n,
                                uint32_t vector_len, uint64_t first_key, uint64_t *out_appended) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_add_batch_keyed");
     return add_batch_rows(e, frame_ids, rows, n, vector_len, &first_key, out_appended);
 }
 
@@ -2250,6 +2267,7 @@ int32_t wax_vs_add(wax_vs_engine *e, uint64_t frame_id, const float *vector, uin
 }
 
 int32_t wax_vs_contains(wax_vs_engine *e, const uint64_t *frame_ids, uint64_t n, uint8_t *out) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_contains");
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     if (n == 0) return WAX_VS_OK;
     if (!frame_ids || !out) return fail(WAX_VS_ERR_NULL, "NULL argument");
@@ -2265,6 +2283,7 @@ int32_t wax_vs_contains(wax_vs_engine *e, const uint64_t *frame_ids, uint64_t n,
 // an HBM bounce buffer (gather kernel + copy back: destinations never overtake unread sources because rows only move
 // down and slabs go in ascending order), the id array is compacted once and the id->row hash rebuilt once.
 int32_t wax_vs_remove_batch(wax_vs_engine *e, const uint64_t *frame_ids, uint64_t n, uint64_t *out_removed) {
+    if (e && e->multi) return multi_remove_batch(e->multi, frame_ids, n, out_removed);
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     if (out_removed) *out_removed = 0;
     if (n == 0) return WAX_VS_OK;
@@ -2577,6 +2596,9 @@ static int32_t check_query(const wax_vs_engine *e, const float *query, uint32_t 
 static int32_t search_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                            int64_t top_k, uint64_t *out_ids, float *out_scores, uint32_t out_stride,
                            uint32_t *out_n) {
+    if (e && e->multi)
+        return multi_search(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_k, out_ids, out_scores,
+                            out_stride, out_n);
     if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     if (e->n_rows == 0) {  // guard vectorCount > 0 else { return [] } (:448) -- before validation, as the reference
@@ -2647,6 +2669,7 @@ int32_t wax_vs_search_batch(wax_vs_engine *e, const float *queries, uint32_t n_q
 
 int32_t wax_vs_search_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries, int64_t top_k,
                              uint64_t row_offset, wax_vs_candidate *d_candidates, void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_search_device");
     if (!e || !d_queries || !d_candidates) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     DeviceGuard g(e->device);
@@ -2668,6 +2691,7 @@ int32_t wax_vs_search_device(wax_vs_engine *e, const float *d_queries, uint32_t 
 // are re-run), so on return d_candidates is complete on `cuda_stream` order and usually already materialised.
 int32_t wax_vs_search_batch_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries, int64_t top_k,
                                    uint64_t row_offset, wax_vs_candidate *d_candidates, void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_search_batch_device");
     if (!e || !d_queries || !d_candidates) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (n_queries == 0) return WAX_VS_OK;
     std::shared_lock<std::shared_mutex> r(e->rw);
@@ -2825,6 +2849,7 @@ static void shard_teardown(wax_vs_engine *e, bool free_own) {
 }
 
 int32_t wax_vs_shard_open(wax_vs_engine *e, int32_t rank, int32_t world, uint64_t row_offset, uint8_t *out_handle) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_open");
     if (!e || !out_handle) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (world < 1 || world > kShardMaxRanks || rank < 0 || rank >= world)
         return fail(WAX_VS_ERR_ARGUMENT, "rank %d of %d: world must be 1..%d", rank, world, kShardMaxRanks);
@@ -2861,6 +2886,7 @@ int32_t wax_vs_shard_open(wax_vs_engine *e, int32_t rank, int32_t world, uint64_
 }
 
 int32_t wax_vs_shard_connect(wax_vs_engine *e, const uint8_t *handles, int32_t n_handles) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_connect");
     if (!e || !handles) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::unique_lock<std::shared_mutex> w(e->rw);
     auto &sh = e->shard;
@@ -2904,6 +2930,7 @@ int32_t wax_vs_shard_connect(wax_vs_engine *e, const uint8_t *handles, int32_t n
 }
 
 int32_t wax_vs_shard_close(wax_vs_engine *e) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_close");
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     std::unique_lock<std::shared_mutex> w(e->rw);
     DeviceGuard g(e->device);
@@ -2924,6 +2951,7 @@ static ShardParams shard_params_next(wax_vs_engine *e) {
 
 int32_t wax_vs_shard_search_device(wax_vs_engine *e, const float *d_query, int64_t top_k, wax_vs_candidate *d_candidates,
                                    void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_search_device");
     if (!e || !d_query || !d_candidates) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     if (!e->shard.connected) return fail(WAX_VS_ERR_ARGUMENT, "the shard group is not connected (wax_vs_shard_open / _connect)");
@@ -2959,6 +2987,7 @@ static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t 
 
 int32_t wax_vs_shard_search(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k, uint64_t *out_ids,
                             float *out_scores, uint32_t out_cap, uint32_t *out_n) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_search");
     if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
     return shard_search_host(e, query, query_len, top_k, false, nullptr, 0, 0, nullptr, out_ids, out_scores, out_cap, out_n);
 }
@@ -2968,6 +2997,7 @@ int32_t wax_vs_shard_search(wax_vs_engine *e, const float *query, uint32_t query
 // collective searches back to back, CUDA events around the `iters`.  Every rank must make the same call.
 int32_t wax_vs_debug_time_shard_search(wax_vs_engine *e, uint32_t n_queries, int64_t top_k, uint64_t seed, uint32_t warmup,
                                        uint32_t iters, float *out_ms_total, uint64_t *out_launches) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_time_shard_search");
     if (!e || !out_ms_total) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (n_queries == 0) n_queries = 1;
     std::shared_lock<std::shared_mutex> r(e->rw);
@@ -3004,13 +3034,15 @@ int32_t wax_vs_debug_time_shard_search(wax_vs_engine *e, uint32_t n_queries, int
 int32_t wax_vs_merge_candidates_device(wax_vs_engine *e, const wax_vs_candidate *d_gathered, uint32_t world,
                                        uint32_t n_queries, uint32_t k, uint32_t k_out, wax_vs_candidate *d_out,
                                        void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_merge_candidates_device");
     if (!e || !d_gathered || !d_out) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (world == 0 || world > 1024u || k == 0 || k_out == 0 || k_out > k)
         return fail(WAX_VS_ERR_ARGUMENT, "merge: world %u, k %u, k_out %u", world, k, k_out);
     if (n_queries == 0) return WAX_VS_OK;
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
-    merge_gathered_kernel<<<n_queries, 128, 0, static_cast<cudaStream_t>(cuda_stream)>>>(d_gathered, world, n_queries, k, k_out, d_out);
+    merge_gathered_kernel<<<n_queries, 128, 0, static_cast<cudaStream_t>(cuda_stream)>>>(
+        GatheredLists<wax_vs_candidate>{d_gathered, static_cast<size_t>(n_queries) * k}, world, n_queries, k, k_out, d_out);
     CUDA_TRY(cudaGetLastError());
     return WAX_VS_OK;
 }
@@ -3537,6 +3569,10 @@ static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint
 int32_t wax_vs_search_filtered(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k,
                                const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids,
                                float *out_scores, uint32_t out_cap, uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_filtered(e->multi->probe, query, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores, out_cap, out_n)) return rc;
+        return multi_search_filtered(e, query, 1, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores, out_cap, out_n);
+    }
     const uint64_t offsets[2] = {0, n_ids};
     const uint32_t query_filter = 0;
     return search_filtered_host(e, query, 1, query_len, top_k, frame_ids, offsets, &mode, 1, &query_filter, out_ids,
@@ -3546,6 +3582,10 @@ int32_t wax_vs_search_filtered(wax_vs_engine *e, const float *query, uint32_t qu
 int32_t wax_vs_search_batch_filtered(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                      int64_t top_k, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
                                      uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_batch_filtered(e->multi->probe, queries, n_queries, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores, out_stride, out_n)) return rc;
+        return multi_search_filtered(e, queries, n_queries, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores, out_stride, out_n);
+    }
     const uint64_t offsets[2] = {0, n_ids};
     const std::vector<uint32_t> query_filter(n_queries, 0u);
     return search_filtered_host(e, queries, n_queries, query_len, top_k, frame_ids, offsets, &mode, 1, query_filter.data(),
@@ -3556,6 +3596,10 @@ int32_t wax_vs_search_batch_multi_filtered(wax_vs_engine *e, const float *querie
                                            int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
                                            const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
                                            uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_batch_multi_filtered(e->multi->probe, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, out_ids, out_scores, out_stride, out_n)) return rc;
+        return multi_search_multi_filtered(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, out_ids, out_scores, out_stride, out_n);
+    }
     return search_filtered_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
                                 query_filter, out_ids, out_scores, out_stride, out_n);
 }
@@ -3841,6 +3885,10 @@ int32_t wax_vs_search_batch_where(wax_vs_engine *e, const float *queries, uint32
                                   const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
                                   const wax_vs_where *wheres, uint32_t n_wheres, const uint32_t *query_where,
                                   uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_batch_where(e->multi->probe, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_stride, out_n)) return rc;
+        return multi_search_batch_where(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_stride, out_n);
+    }
     int32_t rc;
     if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
                                n_wheres, query_where, out_n)))
@@ -3934,6 +3982,7 @@ int32_t wax_vs_location_bin(double latitude, double longitude, int32_t out_bin[2
 // Upsert by frame id as set_attributes; every coordinate pair is checked before anything is written.
 int32_t wax_vs_set_locations(wax_vs_engine *e, const uint64_t *frame_ids, const double *latitudes, const double *longitudes,
                              uint64_t n, uint64_t *out_assigned) {
+    if (e && e->multi) return multi_set(e->multi, out_assigned, [&](wax_vs_engine *s, uint64_t *got) { return wax_vs_set_locations(s, frame_ids, latitudes, longitudes, n, got); });
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     if (out_assigned) *out_assigned = 0;
     if (n == 0) return WAX_VS_OK;
@@ -3981,6 +4030,10 @@ int32_t wax_vs_search_batch_where_near(wax_vs_engine *e, const float *queries, u
                                        const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
                                        const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
                                        uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_batch_where_near(e->multi->probe, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_stride, out_n)) return rc;
+        return multi_search_where(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, nullptr, nullptr, out_ids, out_scores, out_stride, out_n);
+    }
     int32_t rc;
     if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
                                n_wheres, query_where, out_n)))
@@ -4013,6 +4066,7 @@ static int32_t check_term_offsets(const uint64_t *offsets, uint64_t n, const uin
 // half of it is garbage.
 int32_t wax_vs_set_terms(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *term_offsets, const uint64_t *terms,
                          uint64_t n, uint64_t *out_assigned) {
+    if (e && e->multi) return multi_set(e->multi, out_assigned, [&](wax_vs_engine *s, uint64_t *got) { return wax_vs_set_terms(s, frame_ids, term_offsets, terms, n, got); });
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     if (out_assigned) *out_assigned = 0;
     if (!term_offsets) return fail(WAX_VS_ERR_NULL, "term_offsets is NULL");
@@ -4086,6 +4140,10 @@ int32_t wax_vs_search_batch_where_terms(wax_vs_engine *e, const float *queries, 
                                         const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
                                         const uint64_t *where_term_offsets, const uint64_t *where_terms,
                                         uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_batch_where_terms(e->multi->probe, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, where_term_offsets, where_terms, out_ids, out_scores, out_stride, out_n)) return rc;
+        return multi_search_where(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, where_term_offsets, where_terms, out_ids, out_scores, out_stride, out_n);
+    }
     int32_t rc;
     if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
                                n_wheres, query_where, out_n)))
@@ -4201,6 +4259,7 @@ int32_t wax_vs_shard_search_where(wax_vs_engine *e, const float *query, uint32_t
                                   const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, const wax_vs_where_near *where,
                                   const uint64_t *terms, uint32_t n_terms, uint64_t *out_ids, float *out_scores,
                                   uint32_t out_cap, uint32_t *out_n) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_search_where");
     if (!e || !out_n || !where) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
     if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
@@ -4223,6 +4282,7 @@ int32_t wax_vs_search_batch_where_device(wax_vs_engine *e, const float *d_querie
                                          const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
                                          const uint64_t *where_term_offsets, const uint64_t *where_terms,
                                          uint64_t row_offset, wax_vs_candidate *d_candidates, void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_search_batch_where_device");
     int32_t rc;
     uint32_t no_out_n = 0;                  // the checks of the host forms, which also test their out_n
     if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
@@ -4279,6 +4339,7 @@ int32_t wax_vs_search_batch_where_device(wax_vs_engine *e, const float *d_querie
 int32_t wax_vs_shard_search_filtered(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k,
                                      const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids,
                                      float *out_scores, uint32_t out_cap, uint32_t *out_n) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_search_filtered");
     if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
     if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
@@ -4293,6 +4354,7 @@ int32_t wax_vs_shard_search_filtered(wax_vs_engine *e, const float *query, uint3
 
 int32_t wax_vs_set_groups(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *group_ids, uint64_t n,
                           uint64_t *out_assigned) {
+    if (e && e->multi) return multi_set(e->multi, out_assigned, [&](wax_vs_engine *s, uint64_t *got) { return wax_vs_set_groups(s, frame_ids, group_ids, n, got); });
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     if (out_assigned) *out_assigned = 0;
     if (n == 0) return WAX_VS_OK;
@@ -4323,6 +4385,7 @@ int32_t wax_vs_set_groups(wax_vs_engine *e, const uint64_t *frame_ids, const uin
 // set_groups: unknown ids are ignored, a later entry for the same frame wins, a NULL column is left as it is.
 int32_t wax_vs_set_attributes(wax_vs_engine *e, const uint64_t *frame_ids, const int64_t *timestamps, const uint64_t *tags,
                               uint64_t n, uint64_t *out_assigned) {
+    if (e && e->multi) return multi_set(e->multi, out_assigned, [&](wax_vs_engine *s, uint64_t *got) { return wax_vs_set_attributes(s, frame_ids, timestamps, tags, n, got); });
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     if (out_assigned) *out_assigned = 0;
     if (n == 0) return WAX_VS_OK;
@@ -4927,6 +4990,10 @@ int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t que
                               uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
                               uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_cap,
                               uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_grouped(e->multi->probe, query, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids, out_scores, out_groups, out_cap, out_n)) return rc;
+        return multi_search_grouped_one(e, query, 1, query_len, top_groups, per_group, frame_ids, n_ids, mode, nullptr, nullptr, out_ids, out_scores, out_groups, out_cap, out_n);
+    }
     return search_grouped_one_filter(e, query, 1, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
                                      out_scores, out_groups, out_cap, out_n, false);
 }
@@ -4936,6 +5003,10 @@ int32_t wax_vs_search_batch_grouped(wax_vs_engine *e, const float *queries, uint
                                     int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
                                     int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
                                     uint32_t out_stride, uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_batch_grouped(e->multi->probe, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids, out_scores, out_groups, out_stride, out_n)) return rc;
+        return multi_search_grouped_one(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, nullptr, nullptr, out_ids, out_scores, out_groups, out_stride, out_n);
+    }
     return search_grouped_one_filter(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode,
                                      out_ids, out_scores, out_groups, out_stride, out_n, true);
 }
@@ -4944,6 +5015,10 @@ int32_t wax_vs_search_batch_grouped_where(wax_vs_engine *e, const float *queries
                                           int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
                                           int32_t mode, const wax_vs_where *where, uint64_t *out_ids, float *out_scores,
                                           uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_batch_grouped_where(e->multi->probe, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, where, out_ids, out_scores, out_groups, out_stride, out_n)) return rc;
+        return multi_search_grouped_one(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, where, nullptr, out_ids, out_scores, out_groups, out_stride, out_n);
+    }
     if (!where) return fail(WAX_VS_ERR_NULL, "where is NULL");
     const Clause clause{where_pred(*where), kNoLocBox, {}};
     return search_grouped_one_filter(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode,
@@ -4955,6 +5030,10 @@ int32_t wax_vs_search_batch_grouped_where_near(wax_vs_engine *e, const float *qu
                                                const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
                                                const wax_vs_where_near *where, uint64_t *out_ids, float *out_scores,
                                                uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_batch_grouped_where_near(e->multi->probe, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, where, out_ids, out_scores, out_groups, out_stride, out_n)) return rc;
+        return multi_search_grouped_one(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, nullptr, where, out_ids, out_scores, out_groups, out_stride, out_n);
+    }
     if (!where) return fail(WAX_VS_ERR_NULL, "where is NULL");
     std::vector<Clause> clause;
     int32_t rc;
@@ -4971,6 +5050,10 @@ int32_t wax_vs_search_batch_grouped_multi_where(wax_vs_engine *e, const float *q
                                                 uint32_t n_wheres, const uint32_t *query_where, uint64_t *out_ids,
                                                 float *out_scores, uint64_t *out_groups, uint32_t out_stride,
                                                 uint32_t *out_n) {
+    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
+        if (const int32_t rc = wax_vs_search_batch_grouped_multi_where(e->multi->probe, queries, n_queries, query_len, top_groups, per_group, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_groups, out_stride, out_n)) return rc;
+        return multi_search_grouped(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_groups, per_group, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_groups, out_stride, out_n);
+    }
     int32_t rc;
     if ((rc = check_grouped_args(e, top_groups, per_group, out_ids, out_scores, out_groups, out_n)) ||
         (rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
@@ -5013,6 +5096,7 @@ int32_t wax_vs_shard_grouped_heads_device(wax_vs_engine *e, const float *d_queri
                                           const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
                                           const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
                                           uint64_t row_offset, wax_vs_group_candidate *d_heads, void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_grouped_heads_device");
     std::vector<Clause> clauses;
     int32_t rc;
     if ((rc = check_shard_grouped_args(e, d_queries, n_queries, top_groups, per_group, frame_ids, filter_offsets,
@@ -5041,6 +5125,7 @@ int32_t wax_vs_shard_grouped_heads_device(wax_vs_engine *e, const float *d_queri
 int32_t wax_vs_merge_group_heads_device(wax_vs_engine *e, const wax_vs_group_candidate *d_gathered, uint32_t world,
                                         uint32_t n_queries, int64_t top_groups, uint32_t per_group,
                                         wax_vs_group_candidate *d_chosen, void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_merge_group_heads_device");
     if (!e || !d_gathered || !d_chosen) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (world == 0 || world > WAX_VS_SHARD_MAX_RANKS)
         return fail(WAX_VS_ERR_ARGUMENT, "world must be in [1, %d] (got %u)", WAX_VS_SHARD_MAX_RANKS, world);
@@ -5056,9 +5141,11 @@ int32_t wax_vs_merge_group_heads_device(wax_vs_engine *e, const wax_vs_group_can
     uint32_t pow2 = 32;
     while (pow2 < world * n_top) pow2 <<= 1;
     const size_t smem = static_cast<size_t>(pow2) * (sizeof(uint64_t) + 3 * sizeof(uint32_t));
-    CUDA_TRY(grant_smem(e, merge_group_heads_kernel, smem));
-    merge_group_heads_kernel<<<n_queries, 1024, smem, static_cast<cudaStream_t>(cuda_stream)>>>(d_gathered, world, n_queries,
-                                                                                              n_top, per_group, pow2, d_chosen);
+    using Gathered = GatheredLists<wax_vs_group_candidate>;
+    CUDA_TRY(grant_smem(e, merge_group_heads_kernel<Gathered>, smem));
+    merge_group_heads_kernel<<<n_queries, 1024, smem, static_cast<cudaStream_t>(cuda_stream)>>>(
+        Gathered{d_gathered, static_cast<size_t>(n_queries) * n_top * per_group}, world, n_queries, n_top, per_group, pow2,
+        d_chosen);
     CUDA_TRY(cudaGetLastError());
     return WAX_VS_OK;
 }
@@ -5074,6 +5161,7 @@ int32_t wax_vs_shard_grouped_expand_device(wax_vs_engine *e, const float *d_quer
                                            const wax_vs_group_candidate *d_chosen,
                                            const wax_vs_group_candidate *d_own_heads, uint64_t row_offset,
                                            wax_vs_candidate *d_rows, void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_grouped_expand_device");
     std::vector<Clause> clauses;
     int32_t rc;
     if ((rc = check_shard_grouped_args(e, d_queries, n_queries, top_groups, per_group, frame_ids, filter_offsets,
@@ -5143,6 +5231,7 @@ static uint64_t mv2v_length(const wax_vs_engine *e) {
 }
 
 int32_t wax_vs_serialized_length(wax_vs_engine *e, uint64_t *out) {
+    if (e && e->multi && out) { std::shared_lock<std::shared_mutex> r(e->multi->rw); *out = multi_mv2v_length(e->multi->total(), e->dims); return WAX_VS_OK; }
     if (!e || !out) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     *out = mv2v_length(e);
@@ -5150,6 +5239,7 @@ int32_t wax_vs_serialized_length(wax_vs_engine *e, uint64_t *out) {
 }
 
 int32_t wax_vs_serialize(wax_vs_engine *e, uint8_t *dst, uint64_t cap, uint64_t *out_len) {
+    if (e && e->multi) return multi_serialize(e->multi, e->dims, e->similarity, dst, cap, out_len);
     if (!e || !dst) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     const uint64_t need = mv2v_length(e);
@@ -5247,15 +5337,18 @@ static int32_t deserialize_rows(wax_vs_engine *e, const uint8_t *src, uint64_t l
 }
 
 int32_t wax_vs_deserialize(wax_vs_engine *e, const uint8_t *src, uint64_t len) {
+    if (e && e->multi) return multi_deserialize(e->multi, e->dims, e->similarity, src, len);
     return deserialize_rows(e, src, len, true, 0, 0);
 }
 
 int32_t wax_vs_deserialize_rows(wax_vs_engine *e, const uint8_t *src, uint64_t len, uint64_t first, uint64_t n) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_deserialize_rows");
     return deserialize_rows(e, src, len, false, first, n);
 }
 
 int32_t wax_vs_export_rows(wax_vs_engine *e, uint64_t first, uint64_t n, uint64_t *out_ids, float *out_vectors,
                            uint64_t *out_keys) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_export_rows");
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     std::shared_lock<std::shared_mutex> r(e->rw);
     if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
@@ -5274,6 +5367,7 @@ int32_t wax_vs_export_rows(wax_vs_engine *e, uint64_t first, uint64_t n, uint64_
 
 // ---- instrumentation ------------------------------------------------------------------------------------------
 int32_t wax_vs_debug_pool_stats(wax_vs_engine *e, uint64_t *allocations, uint64_t *reuses) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_pool_stats");
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     std::lock_guard<std::mutex> g(e->pool_mu);
     if (allocations) *allocations = e->pool_allocs;
@@ -5283,6 +5377,7 @@ int32_t wax_vs_debug_pool_stats(wax_vs_engine *e, uint64_t *allocations, uint64_
 
 int32_t wax_vs_debug_fill_synthetic(wax_vs_engine *e, uint64_t seed, uint64_t first_row, uint64_t rows,
                                     uint64_t id_base, int32_t normalize) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_fill_synthetic");
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     if (rows > 0xFFFFFFFFull) return fail(WAX_VS_ERR_CAPACITY, "capacity exceeded: limit %llu, requested %llu", 0xFFFFFFFFull, static_cast<unsigned long long>(rows));
     std::unique_lock<std::shared_mutex> w(e->rw);
@@ -5316,6 +5411,7 @@ int32_t wax_vs_debug_fill_synthetic(wax_vs_engine *e, uint64_t seed, uint64_t fi
 }
 
 int32_t wax_vs_debug_read_rows(wax_vs_engine *e, uint64_t first, uint64_t n, float *dst) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_read_rows");
     if (!e || !dst) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     if (first + n > e->n_rows) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
@@ -5326,6 +5422,7 @@ int32_t wax_vs_debug_read_rows(wax_vs_engine *e, uint64_t first, uint64_t n, flo
 
 int32_t wax_vs_debug_time_search(wax_vs_engine *e, uint32_t n_queries, int64_t top_k, uint64_t seed,
                                  uint32_t warmup, uint32_t iters, float *out_ms_total, uint64_t *out_launches) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_time_search");
     if (!e || !out_ms_total) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (n_queries == 0) n_queries = 1;
     std::shared_lock<std::shared_mutex> r(e->rw);
@@ -5381,6 +5478,7 @@ int32_t wax_vs_debug_time_search(wax_vs_engine *e, uint32_t n_queries, int64_t t
 }
 
 int32_t wax_vs_debug_stream_read(wax_vs_engine *e, uint32_t iters, float *out_best_ms, uint64_t *out_bytes) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_stream_read");
     if (!e || !out_best_ms || !out_bytes) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     DeviceGuard g(e->device);
@@ -5415,6 +5513,7 @@ int32_t wax_vs_debug_stream_read(wax_vs_engine *e, uint32_t iters, float *out_be
 //   [2] DMA pinned -> HBM                         [3] DMA HBM -> pinned
 //   [4] upload pipeline pageable -> HBM           [5] download pipeline HBM -> pageable       [6] worker threads
 int32_t wax_vs_debug_transfer_probe(wax_vs_engine *e, uint64_t bytes, float *out7) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_transfer_probe");
     if (!e || !out7) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::unique_lock<std::shared_mutex> w(e->rw);
     DeviceGuard g(e->device);
@@ -5449,6 +5548,7 @@ int32_t wax_vs_debug_transfer_probe(wax_vs_engine *e, uint64_t bytes, float *out
 // [2] -> the last CTA starts the grid stage, [3] -> result written (kernel end), [4] event-timed duration of the
 // launch on the stream (launch overhead = [4] - [3]).
 int32_t wax_vs_debug_phase_trace(wax_vs_engine *e, int64_t top_k, uint32_t iters, float *out5) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_phase_trace");
     if (!e || !out5) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::unique_lock<std::shared_mutex> w(e->rw);
     DeviceGuard g(e->device);
@@ -5490,6 +5590,7 @@ int32_t wax_vs_debug_phase_trace(wax_vs_engine *e, int64_t top_k, uint32_t iters
 }
 
 int32_t wax_vs_debug_batch_stats(wax_vs_engine *e, uint64_t *tensor_queries, uint64_t *fallback_queries) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_batch_stats");
     if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
     std::lock_guard<std::mutex> g(e->pool_mu);
     if (tensor_queries) *tensor_queries = e->batch_tensor_queries;
@@ -5498,6 +5599,7 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *e, uint64_t *tensor_queries, uin
 }
 
 int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) {
+    if (e && e->multi && name && out) return multi_counter(e->multi, name, out);
     if (!e || !name || !out) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::lock_guard<std::mutex> g(e->pool_mu);
     const wax_vs_engine::Shadow &bf = e->shadows[kRouteBf16], &i8 = e->shadows[kRouteInt8], &u4 = e->shadows[kRouteU4];
@@ -5553,6 +5655,7 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
 int32_t wax_vs_debug_time_search_batch(wax_vs_engine *e, uint32_t n_queries, int64_t top_k, uint64_t seed,
                                        uint32_t warmup, uint32_t iters, float *out_ms_total,
                                        uint64_t *out_launches, uint32_t *out_unproven) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_time_search_batch");
     if (!e || !out_ms_total) return fail(WAX_VS_ERR_NULL, "NULL argument");
     if (n_queries == 0) n_queries = 1;
     std::shared_lock<std::shared_mutex> r(e->rw);
@@ -5598,6 +5701,7 @@ int32_t wax_vs_debug_time_search_batch(wax_vs_engine *e, uint32_t n_queries, int
 int32_t wax_vs_debug_batch_nominations(wax_vs_engine *e, const float *queries, uint32_t n_queries, int64_t top_k,
                                        const uint32_t *allow_bits, float *out_scores, uint32_t *out_ok,
                                        uint64_t *out_heaps, uint64_t heaps_cap, uint32_t *out_shape) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_batch_nominations");
     if (!e || !queries || !out_scores || !out_ok || !out_shape) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::shared_lock<std::shared_mutex> r(e->rw);
     DeviceGuard g(e->device);
@@ -5712,18 +5816,21 @@ static int32_t debug_route_nominations(wax_vs_engine *e, const float *query, int
 int32_t wax_vs_debug_shadow_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
                                         uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
                                         uint32_t *out_shape) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_shadow_nominations");
     return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, kRouteBf16);
 }
 
 int32_t wax_vs_debug_int8_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
                                       uint64_t *out_keys, uint32_t *out_ok, wax_vs_candidate *out_result,
                                       uint32_t *out_shape) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_int8_nominations");
     return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, kRouteInt8);
 }
 
 int32_t wax_vs_debug_u4_nominations(wax_vs_engine *e, const float *query, int64_t top_k, const uint32_t *allow_bits,
                                     uint64_t *out_keys, uint64_t keys_cap, uint32_t *out_ok, wax_vs_candidate *out_result,
                                     uint32_t *out_shape, float *out_bound) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_u4_nominations");
     return debug_route_nominations(e, query, top_k, allow_bits, out_keys, out_ok, out_result, out_shape, kRouteU4,
                                    keys_cap, out_bound);
 }
@@ -5759,22 +5866,26 @@ static int32_t debug_read_route_shadow(wax_vs_engine *e, RouteForm f, uint64_t f
 
 int32_t wax_vs_debug_read_u4_shadow(wax_vs_engine *e, uint64_t first, uint64_t n, uint8_t *dst_codes, float *dst_half_steps,
                                     float *out_rho_max) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_read_u4_shadow");
     if (!e || !dst_codes || !dst_half_steps || !out_rho_max) return fail(WAX_VS_ERR_NULL, "NULL argument");
     return debug_read_route_shadow(e, kRouteU4, first, n, dst_codes, dst_half_steps, out_rho_max);
 }
 
 int32_t wax_vs_debug_read_int8_shadow(wax_vs_engine *e, uint64_t first, uint64_t n, uint8_t *dst_codes, float *dst_scales,
                                       float *out_rho_max) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_read_int8_shadow");
     if (!e || !dst_codes || !dst_scales || !out_rho_max) return fail(WAX_VS_ERR_NULL, "NULL argument");
     return debug_read_route_shadow(e, kRouteInt8, first, n, dst_codes, dst_scales, out_rho_max);
 }
 
 int32_t wax_vs_debug_read_shadow(wax_vs_engine *e, uint64_t first, uint64_t n, uint16_t *dst) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_read_shadow");
     if (!e || !dst) return fail(WAX_VS_ERR_NULL, "NULL argument");
     return debug_read_route_shadow(e, kRouteBf16, first, n, dst, nullptr, nullptr);
 }
 
 int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value) {
+    if (e && e->multi && key) return multi_set_option(e->multi, key, value);
     if (!e || !key) return fail(WAX_VS_ERR_NULL, "NULL argument");
     std::unique_lock<std::shared_mutex> w(e->rw);
     const int v = static_cast<int>(value);

@@ -171,20 +171,33 @@ __device__ __forceinline__ bool cand_before(uint32_t km, const wax_vs_candidate 
     if (km != key) return km < key;
     return key == WAXVS_UKEY_NONE ? o < r : m.row < c.row;
 }
-__global__ void __launch_bounds__(128) merge_gathered_kernel(const wax_vs_candidate *__restrict__ gathered, uint32_t world,
-                                                             uint32_t n_queries, uint32_t k, uint32_t k_out,
-                                                             wax_vs_candidate *__restrict__ out) {
+// How a merge finds rank r's records: one rank-major gathered buffer, as an all-gather leaves it ...
+template <class T>
+struct GatheredLists {
+    const T *base;
+    size_t rank_stride;                    // the records of one rank
+    __device__ __forceinline__ const T *operator()(uint32_t r) const { return base + r * rank_stride; }
+};
+// ... or a table of per-rank buffers, each on its rank's device and read here over peer memory (the multi-device handle,
+// waxvs_multi.cuh).  The table rides in the kernel parameters.
+template <class T>
+struct PeerLists {
+    const T *list[kShardMaxRanks];
+    __device__ __forceinline__ const T *operator()(uint32_t r) const { return list[r]; }
+};
+template <class Lists>
+__global__ void __launch_bounds__(128) merge_gathered_kernel(const Lists lists, uint32_t world, uint32_t n_queries, uint32_t k,
+                                                             uint32_t k_out, wax_vs_candidate *__restrict__ out) {
     const uint32_t q = blockIdx.x;
-    const size_t rank_stride = static_cast<size_t>(n_queries) * k;
-    const wax_vs_candidate *mine = gathered + static_cast<size_t>(q) * k;           // rank 0's list of this query
+    const size_t at = static_cast<size_t>(q) * k;                    // this query's list in every rank's buffer
     for (uint32_t t = threadIdx.x; t < world * k; t += blockDim.x) {
         const uint32_t r = t / k, j = t % k;
-        const wax_vs_candidate c = mine[r * rank_stride + j];
+        const wax_vs_candidate c = lists(r)[at + j];
         const uint32_t key = cand_dist_key(c);
         uint32_t pos = j;
         for (uint32_t o = 0; o < world; ++o) {
             if (o == r) continue;
-            const wax_vs_candidate *lst = mine + o * rank_stride;
+            const wax_vs_candidate *lst = lists(o) + at;
             uint32_t lo = 0, hi = k;
             while (lo < hi) {
                 const uint32_t mid = (lo + hi) >> 1;
@@ -222,9 +235,10 @@ __device__ __forceinline__ void block_bitonic_sort_pairs(uint64_t *key, uint32_t
 }
 
 // One CTA per query; dynamic shared memory: pow2 * 20 bytes, pow2 = the power of two >= max(world * G, 32).
-__global__ void __launch_bounds__(1024) merge_group_heads_kernel(const wax_vs_group_candidate *__restrict__ gathered,
-                                                                 uint32_t world, uint32_t n_queries, uint32_t n_top,
-                                                                 uint32_t per_group, uint32_t pow2,
+// `lists` finds rank r's [n_queries][G][P] records (GatheredLists or PeerLists).
+template <class Lists>
+__global__ void __launch_bounds__(1024) merge_group_heads_kernel(const Lists lists, uint32_t world, uint32_t n_queries,
+                                                                 uint32_t n_top, uint32_t per_group, uint32_t pow2,
                                                                  wax_vs_group_candidate *__restrict__ chosen) {
     extern __shared__ uint64_t heads_smem[];
     uint64_t *s_key = heads_smem;                                      // [pow2]
@@ -233,9 +247,8 @@ __global__ void __launch_bounds__(1024) merge_group_heads_kernel(const wax_vs_gr
     uint32_t *s_keep = s_head + pow2;                                  // [pow2] 1: the position is its group's best head
     __shared__ uint32_t s_warp[32], s_total;
     const uint32_t q = blockIdx.x, t = threadIdx.x, heads = world * n_top;
-    const size_t rank_stride = static_cast<size_t>(n_queries) * n_top * per_group;
     auto head = [&](uint32_t i) -> const wax_vs_group_candidate & {
-        return gathered[(i / n_top) * rank_stride + (static_cast<size_t>(q) * n_top + i % n_top) * per_group];
+        return lists(i / n_top)[(static_cast<size_t>(q) * n_top + i % n_top) * per_group];
     };
     // 1. every rank's heads in (distance, global row) order: the rank of each head's row, then (distance key, row rank)
     uint32_t mine = 0;

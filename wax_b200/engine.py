@@ -290,18 +290,25 @@ class CUDAVectorEngine:
         return L.lib().wax_vs_device_count(C.byref(n)) == L.OK and n.value > 0
 
     def __init__(self, metric: VectorMetric = VectorMetric.cosine, dimensions: int = 0,
-                 device: Optional[int] = None):     # init(metric:dimensions:) (:153)
+                 device: Optional[int] = None, devices: Optional[Sequence[int]] = None):   # init(metric:dimensions:) (:153)
+        """`devices` with two or more ordinals makes a multi-device handle: the corpus sharded by rows, shard r on
+        devices[r], every answer equal to one engine's (DESIGN.md section 4.16).  An ordinal may repeat: shards then
+        share that device (a test and debug configuration)."""
         if dimensions <= 0:
             raise InvalidToc("dimensions must be > 0")
         if dimensions > L.MAX_DIMENSIONS:
             raise CapacityExceeded(f"capacity exceeded: limit {L.MAX_DIMENSIONS}, requested {dimensions}")
+        if device is not None and devices is not None:
+            raise ValueError("pass at most one of device= / devices=")
         self.metric = metric
         self.dimensions = int(dimensions)
         self._dirty = False
         self._h = C.c_void_p()
-        devs = (C.c_int32 * 1)(device) if device is not None else None
+        if device is not None:
+            devices = [device]
+        devs = (C.c_int32 * len(devices))(*devices) if devices else None
         _check(L.lib().wax_vs_create(self.dimensions, metric.to_vec_similarity(), devs,
-                                     1 if device is not None else 0, C.byref(self._h)))
+                                     len(devices) if devices else 0, C.byref(self._h)))
         self._closed = False
         self._lock = threading.Lock()
 

@@ -32,6 +32,13 @@ public:
     CUDAVectorEngine(VectorMetric metric, uint32_t dimensions) : metric_(metric), dimensions_(dimensions) {
         check(wax_vs_create(dimensions, static_cast<uint8_t>(metric), nullptr, 0, &h_));
     }
+    // Two or more device ordinals: a multi-device handle, the corpus sharded by rows, shard r on devices[r] (an ordinal
+    // may repeat: shards then share that device, a test and debug configuration).  One ordinal: that device.
+    CUDAVectorEngine(VectorMetric metric, uint32_t dimensions, const std::vector<int32_t> &devices)
+        : metric_(metric), dimensions_(dimensions) {
+        check(wax_vs_create(dimensions, static_cast<uint8_t>(metric), devices.empty() ? nullptr : devices.data(),
+                            static_cast<int32_t>(devices.size()), &h_));
+    }
     ~CUDAVectorEngine() { wax_vs_destroy(h_); }
     CUDAVectorEngine(const CUDAVectorEngine &) = delete;
     CUDAVectorEngine &operator=(const CUDAVectorEngine &) = delete;
