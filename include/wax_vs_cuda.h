@@ -75,7 +75,7 @@ int32_t wax_vs_device_count(int32_t *out);
    n_devices >= 2 returns a MULTI-DEVICE handle: the corpus sharded by rows over n_devices shards, shard r on devices[r]
    (DESIGN.md section 4.16).  Every answer it gives equals that of one engine with the same call history, bit for bit:
    ids, order, score bits, counts, MV2V bytes, error codes and reasons.  It serves wax_vs_dimensions, _similarity,
-   _count, _reserve, _add, _add_batch, _remove, _remove_batch, _search, _search_batch, _search_filtered,
+   _count, _reserve, _add, _add_batch, _remove, _remove_batch, _rebalance, _search, _search_batch, _search_filtered,
    _search_batch_filtered, _search_batch_multi_filtered, _set_attributes, _set_locations, _set_terms,
    _search_batch_where, _where_near, _where_terms, _set_groups, _search_grouped, _search_batch_grouped, _grouped_where,
    _grouped_where_near, _grouped_multi_where, _serialized_length, _serialize, _deserialize, wax_vs_debug_set_option
@@ -126,6 +126,17 @@ int32_t wax_vs_remove(wax_vs_engine *engine, uint64_t frame_id);
    are ignored, surviving rows keep their relative order -- with one compaction of the matrix in HBM, one compaction
    of the id array and one id->row hash rebuild.  *out_removed (optional) = rows actually deleted. */
 int32_t wax_vs_remove_batch(wax_vs_engine *engine, const uint64_t *frame_ids, uint64_t n, uint64_t *out_removed);
+
+/* Even out the rows of a multi-device handle's shards, in place.  *out_moved (optional) = rows moved.
+   A mutator (DESIGN.md section 4.16): every shard ends with T / R or T / R + 1 of the T rows, the extra ones on the shards
+   that held the most, and each moved row takes its key, group, attributes, location and terms with it.  Nothing the
+   handle serves changes except "shard_rows.<r>": every answer still equals one engine's with the same call history, and
+   a later upsert or remove of a moved frame finds it where it now lives.  A balanced handle (max - min <= 1) moves
+   nothing and touches no shard.  One engine (n_devices <= 1) returns WAX_VS_OK with *out_moved = 0.  A failed
+   allocation (a receiving shard's growth, the staging) is found before that shard's rows change: WAX_VS_ERR_CUDA, every
+   earlier move complete, no row held twice or lost.  The merge works in slabs of the option "rebalance_slab_bytes"
+   (wax_vs_debug_set_option, default 256 MiB). */
+int32_t wax_vs_rebalance(wax_vs_engine *engine, uint64_t *out_moved);
 
 /* ---- row keys: the rank-local store of the row-sharded engine (DESIGN.md section 4.15) ------------------------------
    A keyed engine holds one u64 key per row, the row's insertion sequence number in the whole sharded corpus; keys

@@ -548,6 +548,20 @@ public actor CUDAVectorEngine {
         return Int(removed)
     }
 
+    /// A multi-device handle: even out the shards' rows in place, each row moving with its group, attributes, location
+    /// and terms.  Every answer stays the same, so the serialized bytes do too.  Returns the rows moved (0 on one engine).
+    @discardableResult
+    public func rebalance() async throws -> Int {
+        let handle = self.handle
+        let moved: UInt64 = try await io.run {
+            var moved: UInt64 = 0
+            let rc = wax_vs_rebalance(handle, &moved)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return moved
+        }
+        return Int(moved)
+    }
+
     public func serialize() async throws -> Data {
         let handle = self.handle
         return try await io.run {

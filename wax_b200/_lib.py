@@ -57,6 +57,7 @@ SIGNATURES = {
     "wax_vs_add_batch": (C.c_int32, [_eng, _u64p, _f32p, C.c_uint64, C.c_uint32]),
     "wax_vs_remove": (C.c_int32, [_eng, C.c_uint64]),
     "wax_vs_remove_batch": (C.c_int32, [_eng, _u64p, C.c_uint64, _u64p]),
+    "wax_vs_rebalance": (C.c_int32, [_eng, _u64p]),
     "wax_vs_add_batch_keyed": (C.c_int32, [_eng, _u64p, _f32p, C.c_uint64, C.c_uint32, C.c_uint64, _u64p]),
     "wax_vs_contains": (C.c_int32, [_eng, _u64p, C.c_uint64, _u8p]),
     "wax_vs_deserialize_rows": (C.c_int32, [_eng, _u8p, C.c_uint64, C.c_uint64, C.c_uint64]),

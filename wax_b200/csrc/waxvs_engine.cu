@@ -194,6 +194,7 @@ struct Tuning {
     int single_shadow = 0;  // 1: single queries / batches below batch_min take the tensor-core bf16-shadow nominations
                             // (one query in a 128-query wgmma tile) instead of the shadow route of `shadow_scan`
     uint64_t filter_bitset_bytes = 2ull << 30;   // per-query filters: row bitsets one tensor pass may hold
+    uint64_t rebalance_slab_bytes = 256ull << 20;   // a rebalance merge's slab and staging chunk (absorb_rows), each
     int shadow_scan = 1;    // single queries (cosine / dot, k <= 32) nominate on the bf16 shadow with the streaming scan, then
                             // an exact re-score + proof, the fp32 scan only when the proof fails (0: always the fp32 scan)
     // Each form of the route, by RouteForm (options "<shadow|int8|u4>_scan_min_bytes", "_rows_per_step", "_warps",
@@ -1875,6 +1876,8 @@ static int32_t sync_device_ids(wax_vs_engine *e, const uint64_t **out) {
     return WAX_VS_OK;
 }
 
+extern "C" { static int32_t absorb_rows(wax_vs_engine *e, wax_vs_engine *donor, uint64_t first, uint64_t n); }
+
 #include "waxvs_multi.cuh"
 
 // ---------------------------------------------------------------------------------------------------------
@@ -2377,6 +2380,121 @@ int32_t wax_vs_remove_batch(wax_vs_engine *e, const uint64_t *frame_ids, uint64_
 
 int32_t wax_vs_remove(wax_vs_engine *e, uint64_t frame_id) {
     return wax_vs_remove_batch(e, &frame_id, 1, nullptr);
+}
+
+// The receiving half of a rebalance move (multi_rebalance, DESIGN.md section 4.16): rows [first, first + n) of `donor`, a
+// run of increasing keys, merge into `e` by key together with their ids, keys, groups, attributes, locations and terms.
+// Every allocation (the receiver's growth, the bounce buffer, the staging, the key column) comes before a row changes,
+// so a failed allocation leaves `e` as it was.  Destination slabs are written top-down: own rows only move up and
+// incoming rows only move down, so a slab's sources lie in it or below it, and each slab is gathered into the bounce
+// buffer (merge_rows_kernel) before it is copied in place, as the compaction of remove_batch does.  The incoming rows of
+// one slab are one contiguous run of the donor's, staged on the receiver's device with cudaMemcpyPeerAsync (a
+// device-local copy when the two share a device): no kernel reads peer memory.  The donor is only read; the caller
+// drops the rows from it afterwards.
+static int32_t absorb_rows(wax_vs_engine *e, wax_vs_engine *donor, uint64_t first, uint64_t n) {
+    if (n == 0) return WAX_VS_OK;
+    IngestTrace tr("rebalance merge");
+    std::unique_lock<std::shared_mutex> w(e->rw);
+    std::shared_lock<std::shared_mutex> donor_lock(donor->rw);
+    if (!donor->keys_set || first + n > donor->n_rows || (!e->keys_set && e->n_rows))
+        return fail(WAX_VS_ERR_ARGUMENT, "rebalance: rows [%llu, +%llu) of a keyed shard expected",
+                    static_cast<unsigned long long>(first), static_cast<unsigned long long>(n));
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    drain_device_path(e);
+    const uint64_t n0 = e->n_rows, m = n0 + n;
+    const uint64_t *in_keys = donor->keys.data() + first;
+    // rows below the first incoming key keep their place; every destination row from f on has a tagged source
+    const uint64_t f = static_cast<uint64_t>(std::lower_bound(e->keys.begin(), e->keys.end(), in_keys[0]) - e->keys.begin());
+    const uint64_t total = m - f;
+    std::vector<uint64_t> src(total);
+    for (uint64_t t = 0, i = f, j = 0; t < total; ++t)
+        src[t] = j < n && (i == n0 || in_keys[j] < e->keys[i]) ? (kMergeIncoming | j++) : i++;
+    tr.mark("lock+drain+merge positions");
+
+    int32_t rc;
+    if ((rc = grow_for(e, m)) || (rc = ingest_init(e))) return rc;
+    auto &ig = e->ing;
+    const size_t row_bytes = static_cast<size_t>(e->dims) * sizeof(float);
+    const uint64_t slab_rows = std::max<uint64_t>(1, std::min<uint64_t>(total, e->tune.rebalance_slab_bytes / row_bytes));
+    DevBuf<float> incoming;
+    DevBuf<uint64_t> d_src;
+    if ((rc = ig.d_stage.ensure(static_cast<size_t>(slab_rows) * e->dims, "rebalance bounce buffer")) ||
+        (rc = incoming.ensure(static_cast<size_t>(std::min(slab_rows, n)) * e->dims, "rebalance staging")) ||
+        (rc = d_src.ensure(static_cast<size_t>(slab_rows), "rebalance sources")))
+        return rc;
+    uint64_t keys_from = f;
+    if (e->d_keys.cap < m) {                   // the last allocation: the whole key column is uploaded below
+        if ((rc = e->d_keys.ensure(std::max<size_t>(m, e->cap_rows), "row keys"))) return rc;
+        keys_from = 0;
+    }
+    tr.mark("grow+staging");
+
+    std::vector<uint64_t> tags;
+    for (uint64_t hi = total; hi > 0;) {
+        const uint64_t lo = hi > slab_rows ? hi - slab_rows : 0, len = hi - lo;
+        tags.assign(src.begin() + lo, src.begin() + hi);
+        uint64_t jlo = ~0ull, jhi = 0;         // the incoming run this slab takes
+        for (const uint64_t t : tags)
+            if (t & kMergeIncoming) { jlo = std::min(jlo, t & ~kMergeIncoming); jhi = std::max(jhi, (t & ~kMergeIncoming) + 1); }
+        if (jhi > jlo) {
+            CUDA_TRY(cudaMemcpyPeerAsync(incoming, e->device, donor->d_corpus + (first + jlo) * donor->dims, donor->device,
+                                         (jhi - jlo) * row_bytes, ig.stream));
+            for (uint64_t &t : tags) if (t & kMergeIncoming) t -= jlo;
+        }
+        CUDA_TRY(cudaMemcpyAsync(d_src, tags.data(), len * sizeof(uint64_t), cudaMemcpyHostToDevice, ig.stream));
+        const unsigned grid = static_cast<unsigned>(std::min<uint64_t>(len, static_cast<uint64_t>(e->sm_count) * 32));
+        merge_rows_kernel<<<grid, 128, 0, ig.stream>>>(ig.d_stage, e->d_corpus, incoming, d_src, len, e->dims);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaMemcpyAsync(e->d_corpus + (f + lo) * e->dims, ig.d_stage, len * row_bytes, cudaMemcpyDeviceToDevice,
+                                 ig.stream));
+        CUDA_TRY(cudaStreamSynchronize(ig.stream));          // tags / d_src / incoming are reused by the next slab
+        hi = lo;
+    }
+    tr.mark("merge matrix");
+
+    // The host columns in the same order.  A column set on one side only is materialised with the defaults the other
+    // side's rows answered with: group = own frame id, attributes {0, 0}, no location, no terms.
+    materialize_ids(e);
+    auto merge = [&](auto &col, auto incoming_of) {
+        auto tail = std::vector<typename std::decay_t<decltype(col)>::value_type>(total);
+        for (uint64_t t = 0; t < total; ++t)
+            tail[t] = (src[t] & kMergeIncoming) ? incoming_of(first + (src[t] & ~kMergeIncoming)) : col[src[t]];
+        col.resize(f);
+        col.insert(col.end(), tail.begin(), tail.end());
+    };
+    if ((e->groups_set || donor->groups_set) && !e->groups_set) { e->groups = e->ids; e->groups_set = true; }
+    if (donor->attrs_set && !e->attrs_set) { e->attrs.assign(n0, AttrRow{0, 0}); e->attrs_set = true; }
+    if (donor->locs_set && !e->locs_set) { e->locs.assign(n0, LocRow{kNoLocation, 0}); e->locs_set = true; }
+    if (donor->terms_set && !e->terms_set) { e->term_refs.assign(n0, wax_vs_engine::TermRef{0, 0}); e->terms_set = true; }
+    merge(e->ids, [&](uint64_t r) { return frame_id_of(donor, r); });
+    merge(e->keys, [&](uint64_t r) { return donor->keys[r]; });
+    e->keys_set = true;
+    if (e->groups_set) merge(e->groups, [&](uint64_t r) { return donor->groups_set ? donor->groups[r] : frame_id_of(donor, r); });
+    if (e->attrs_set) merge(e->attrs, [&](uint64_t r) { return donor->attrs_set ? donor->attrs[r] : AttrRow{0, 0}; });
+    if (e->locs_set) merge(e->locs, [&](uint64_t r) { return donor->locs_set ? donor->locs[r] : LocRow{kNoLocation, 0}; });
+    if (e->terms_set)
+        merge(e->term_refs, [&](uint64_t r) {
+            if (!donor->terms_set || donor->term_refs[r].n == 0) return wax_vs_engine::TermRef{0, 0};
+            const wax_vs_engine::TermRef t = donor->term_refs[r];
+            const uint64_t off = e->term_pool.size();
+            e->term_pool.insert(e->term_pool.end(), donor->term_pool.begin() + t.off, donor->term_pool.begin() + t.off + t.n);
+            return wax_vs_engine::TermRef{off, t.n};
+        });
+    e->n_rows = m;
+    e->ids_sorted = std::is_sorted(e->ids.begin(), e->ids.end());   // distinct ids: sorted = increasing
+    e->map_valid = false;
+    e->d_ids_dirty = true;
+    invalidate_row_caches(e, f);
+    rc = upload_row_keys(e, keys_from);
+    tr.mark("merge columns");
+    return rc;
+}
+
+int32_t wax_vs_rebalance(wax_vs_engine *e, uint64_t *out_moved) {
+    if (out_moved) *out_moved = 0;
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    return e->multi ? multi_rebalance(e->multi, out_moved) : WAX_VS_OK;   // one engine has nothing to even out
 }
 
 // Filter level (level 2 of the batched path): for queries level 1 could not prove.  One TF32 tensor-core pass in
@@ -5912,6 +6030,7 @@ int32_t wax_vs_debug_set_option(wax_vs_engine *e, const char *key, int64_t value
     else if (!strcmp(key, "filter_bf16")) e->tune.filter_bf16 = v;
     else if (!strcmp(key, "batch_l2")) e->tune.batch_l2 = v;
     else if (!strcmp(key, "filter_bitset_bytes")) e->tune.filter_bitset_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 0));
+    else if (!strcmp(key, "rebalance_slab_bytes")) e->tune.rebalance_slab_bytes = static_cast<uint64_t>(std::max<int64_t>(value, 1));
     else if (!strcmp(key, "single_shadow")) e->tune.single_shadow = v;
     else if (!strcmp(key, "shadow_scan")) {     // also closes the skip window, including failures not yet seen
         std::lock_guard<std::mutex> pg(e->pool_mu);

@@ -10,6 +10,8 @@
 //     wax_vs_search_batch_device for a batch), then device 0 waits on an event of each shard's stream and ONE merge
 //     launch reads the lists in place through peer memory (merge_gathered_kernel<PeerLists>), followed by one D2H copy
 //     and one synchronise;
+//   * rebalance: sharded.plan_rebalance (ported below unchanged) moves each donor's tail to the receivers, which merge
+//     the rows by key with their side columns (absorb_rows), so every answer stays the same;
 //   * threads: one persistent worker per shard lets the shards proceed concurrently through the entries that may
 //     synchronise (the batched levels, the mutators).  Each concurrent caller leases its own per-shard streams and
 //     buffers (MultiCtx), as CtxLease does for one engine.
@@ -319,6 +321,86 @@ static int32_t multi_remove_batch(MultiEngine *m, const uint64_t *frame_ids, uin
     for (int r = 0; r < m->n(); ++r) { m->rows[r] -= gone[r]; sum += gone[r]; }
     if (out_removed) *out_removed = sum;
     return rc;
+}
+
+// ---- rebalance ------------------------------------------------------------------------------------------------------
+struct MultiMove {
+    int donor, receiver;
+    uint64_t rows;
+};
+// sharded.plan_rebalance, ported unchanged: targets of T / R rows, the T % R extra rows to the shards that hold the most
+// (ties to lower shards); donors and receivers in shard order, each donor's tail dealt out in key order.
+static std::vector<MultiMove> multi_plan_rebalance(const std::vector<uint64_t> &counts) {
+    const size_t R = counts.size();
+    uint64_t total = 0;
+    for (uint64_t c : counts) total += c;
+    std::vector<uint64_t> target(R, total / R);
+    std::vector<size_t> order(R);
+    for (size_t r = 0; r < R; ++r) order[r] = r;
+    std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return counts[a] > counts[b]; });
+    for (uint64_t i = 0; i < total % R; ++i) ++target[order[i]];
+    std::vector<uint64_t> take(R);
+    for (size_t r = 0; r < R; ++r) take[r] = target[r] > counts[r] ? target[r] - counts[r] : 0;
+    std::vector<MultiMove> moves;
+    size_t r = 0;
+    for (size_t d = 0; d < R; ++d) {
+        for (uint64_t left = counts[d] > target[d] ? counts[d] - target[d] : 0; left;) {
+            while (take[r] == 0) ++r;
+            const uint64_t n = std::min(left, take[r]);
+            moves.push_back(MultiMove{static_cast<int>(d), static_cast<int>(r), n});
+            left -= n;
+            take[r] -= n;
+        }
+    }
+    return moves;
+}
+
+// Each receiver merges its incoming runs in move order on its own worker (absorb_rows), the receivers concurrently: a
+// shard is a donor or a receiver, never both, so the donors are only read meanwhile.  Then each donor drops the rows of
+// its completed moves, all from its tail, by wax_vs_remove_batch: a truncation, its rows [0, new_n) and their caches stay
+// valid.  A failed move changes nothing on its receiver, and its rows stay on the donor.
+static int32_t multi_rebalance(MultiEngine *m, uint64_t *out_moved) {
+    std::unique_lock<std::shared_mutex> w(m->rw);
+    const std::vector<MultiMove> moves = multi_plan_rebalance(m->rows);
+    if (moves.empty()) return WAX_VS_OK;
+    const int R = m->n();
+    std::vector<uint64_t> tail(m->rows), first(moves.size());   // tail[d]: where donor d's next run starts
+    for (const MultiMove &mv : moves) tail[mv.donor] -= mv.rows;
+    std::vector<std::vector<size_t>> into(R);
+    for (size_t i = 0; i < moves.size(); ++i) {
+        first[i] = tail[moves[i].donor];
+        tail[moves[i].donor] += moves[i].rows;
+        into[moves[i].receiver].push_back(i);
+    }
+    std::vector<int> receivers, donors;
+    for (int r = 0; r < R; ++r) if (!into[r].empty()) receivers.push_back(r);
+    std::vector<uint8_t> done(moves.size(), 0);
+    const int32_t rc = multi_run(m, receivers, [&](int r) -> int32_t {
+        for (size_t i : into[r]) {
+            if (const int32_t mrc = absorb_rows(m->shards[r], m->shards[moves[i].donor], first[i], moves[i].rows)) return mrc;
+            done[i] = 1;
+        }
+        return WAX_VS_OK;
+    });
+    const std::string why = rc ? wax_vs_last_error() : "";
+    std::vector<std::vector<uint64_t>> drop(R);
+    uint64_t moved = 0;
+    for (size_t i = 0; i < moves.size(); ++i) {
+        if (!done[i]) continue;
+        for (uint64_t row = first[i]; row < first[i] + moves[i].rows; ++row)
+            drop[moves[i].donor].push_back(frame_id_of(m->shards[moves[i].donor], row));
+        m->rows[moves[i].receiver] += moves[i].rows;
+        moved += moves[i].rows;
+    }
+    for (int d = 0; d < R; ++d) if (!drop[d].empty()) donors.push_back(d);
+    std::vector<uint64_t> gone(R, 0);
+    const int32_t drc = multi_run(m, donors, [&](int d) -> int32_t {
+        return wax_vs_remove_batch(m->shards[d], drop[d].data(), drop[d].size(), &gone[d]);
+    });
+    for (int d = 0; d < R; ++d) m->rows[d] -= gone[d];
+    if (out_moved) *out_moved = moved;
+    if (rc) return fail(rc, "%s", why.c_str());
+    return drc;
 }
 
 static int32_t multi_reserve(MultiEngine *m, uint64_t rows) {

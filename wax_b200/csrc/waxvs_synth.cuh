@@ -73,6 +73,26 @@ __global__ void __launch_bounds__(128) gather_rows_kernel(float *__restrict__ bo
     }
 }
 
+// Two-source row gather of the rebalance merge (absorb_rows): bounce row i <- incoming row (tag & ~kMergeIncoming) when the
+// tag has kMergeIncoming set, else corpus row tag.  float4 when the rows allow it.
+constexpr uint64_t kMergeIncoming = 1ull << 63;
+__global__ void __launch_bounds__(128) merge_rows_kernel(float *__restrict__ bounce, const float *__restrict__ corpus,
+                                                         const float *__restrict__ incoming, const uint64_t *__restrict__ tagged_src,
+                                                         uint64_t n, uint32_t dims) {
+    for (uint64_t row = blockIdx.x; row < n; row += gridDim.x) {
+        const uint64_t tag = tagged_src[row];
+        const float *s = (tag & kMergeIncoming) ? incoming + (tag & ~kMergeIncoming) * dims : corpus + tag * dims;
+        float *d = bounce + row * dims;
+        if ((dims & 3u) == 0u) {
+            const float4 *s4 = reinterpret_cast<const float4 *>(s);
+            float4 *d4 = reinterpret_cast<float4 *>(d);
+            for (uint32_t i = threadIdx.x; i < dims / 4u; i += blockDim.x) d4[i] = __ldcs(s4 + i);
+        } else {
+            for (uint32_t i = threadIdx.x; i < dims; i += blockDim.x) d[i] = s[i];
+        }
+    }
+}
+
 // Read-only streaming ceiling: every thread LDG.128s a grid-stride slice and folds it into one word.  Used by
 // bench.py to report what a plain coalesced read of the same bytes achieves on the same box (SURVEY 8d).
 __global__ void __launch_bounds__(512) stream_read_kernel(const uint4 *__restrict__ src, uint64_t n_vec,

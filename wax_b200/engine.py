@@ -804,6 +804,13 @@ class CUDAVectorEngine:
             self._dirty = True
         return gone.value
 
+    def rebalance(self) -> int:
+        """Even out the rows of a multi-device handle's shards in place (wax_vs_rebalance); returns how many rows moved.
+        Every answer stays the same, groups, attributes, locations and terms included.  0 on one engine."""
+        moved = C.c_uint64(0)
+        _check(L.lib().wax_vs_rebalance(self._h, C.byref(moved)))
+        return moved.value
+
     def reserve(self, rows: int) -> None:
         _check(L.lib().wax_vs_reserve(self._h, int(rows)))
 

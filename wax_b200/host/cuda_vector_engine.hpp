@@ -93,6 +93,13 @@ public:
         check(wax_vs_remove_batch(h_, frameIds.data(), frameIds.size(), &gone));
         return gone;
     }
+    // A multi-device handle: even out the shards' rows in place, every answer unchanged; returns how many rows moved
+    // (0 on one engine).
+    uint64_t rebalance() {
+        uint64_t moved = 0;
+        check(wax_vs_rebalance(h_, &moved));
+        return moved;
+    }
 
     // A batch of independent queries (no reference counterpart: VectorSearchEngine.swift:13 takes one vector).  Eligible
     // batches take the tensor-core levels; the results are identical to one search() per query.

@@ -62,6 +62,33 @@ def fill_emptiest(counts: Sequence[int], m: int) -> np.ndarray:
     return alloc
 
 
+def plan_rebalance(counts: Sequence[int]):
+    """How a rebalance evens out the ranks' rows.  Every rank gets T // R of the T rows; the T % R extra rows go to the
+    ranks that hold the most now (ties to lower ranks), which moves the fewest rows and leaves a balanced corpus alone.
+    A donor gives up its surplus from its tail (its highest keys), so it only truncates; donors and receivers are taken in
+    rank order, and a donor's tail is dealt out in key order, its lowest-key part to the first receiver with a deficit.
+    Returns (targets [world], moves [(donor, receiver, rows), ...])."""
+    counts = np.asarray(counts, np.int64).reshape(-1)
+    world, total = counts.size, int(counts.sum())
+    targets = np.full(world, total // world if world else 0, np.int64)
+    targets[np.argsort(-counts, kind="stable")[:total % world if world else 0]] += 1
+    give = np.maximum(counts - targets, 0)
+    take = np.maximum(targets - counts, 0)
+    moves = []
+    receivers = iter(np.flatnonzero(take).tolist())
+    r = next(receivers, None)
+    for d in np.flatnonzero(give).tolist():
+        left = int(give[d])
+        while left:
+            n = min(left, int(take[r]))
+            moves.append((d, r, n))
+            left -= n
+            take[r] -= n
+            if take[r] == 0:
+                r = next(receivers, None)
+    return targets, moves
+
+
 def plan_add_batch(frame_ids, owner, counts: Sequence[int], next_key: int):
     """Where each item of a sharded add_batch goes.  `owner` [n]: the rank holding each id before the batch (-1: none);
     `counts`: rows per rank; `next_key`: the first unused key.  Held ids are upserted by their owner.  The distinct new
