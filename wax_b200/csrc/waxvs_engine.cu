@@ -1876,7 +1876,51 @@ static int32_t sync_device_ids(wax_vs_engine *e, const uint64_t **out) {
     return WAX_VS_OK;
 }
 
-extern "C" { static int32_t absorb_rows(wax_vs_engine *e, wax_vs_engine *donor, uint64_t first, uint64_t n); }
+// A where as the host plans it: the time and tag clauses, the location box (kNoLocBox: no location clause) and the
+// sorted, distinct term ids a row must hold (none: no term clause).
+struct Clause {
+    WherePred pred;
+    LocBox box;
+    std::vector<uint64_t> terms;
+};
+
+// What a filtered, where or grouped search asks for.  Its entry point checks the arguments and builds it once (the
+// request_* builders); then it is only read, by one engine or concurrently by every shard of a multi-device handle.
+// Query i searches under id filter query_filter[i] and where query_where[i], either of which may be WAX_VS_NO_FILTER.
+// The arrays are the caller's, or the request's own storage for the forms with one filter or one where for every query
+// and for canonical term wheres, so a request is neither copied nor moved.
+struct SearchRequest {
+    const float *queries;                   // host memory; the device forms pass their queries beside the request
+    uint32_t n_queries, query_len;
+    int64_t top_k;                          // grouped search: top_groups
+    uint32_t per_group;                     // grouped search only
+    bool batched;                           // grouped search: the batch pipeline may take the queries
+    const uint64_t *frame_ids = nullptr;
+    const uint64_t *filter_offsets = nullptr;
+    const int32_t *filter_modes = nullptr;
+    uint32_t n_filters = 0;
+    const uint32_t *query_filter = nullptr;
+    std::vector<Clause> wheres;
+    const uint32_t *query_where = nullptr;  // nullptr: no where list, the filtered entry points (plan_request)
+    uint64_t one_offsets[2] = {0, 0};
+    int32_t one_mode = 0;
+    std::vector<uint32_t> filter_of, where_of;
+    SearchRequest(const float *q, uint32_t n, uint32_t len, int64_t k, uint32_t groups_of = 0, bool batch = false)
+        : queries(q), n_queries(n), query_len(len), top_k(k), per_group(groups_of), batched(batch) {}
+    SearchRequest(const SearchRequest &) = delete;
+    SearchRequest &operator=(const SearchRequest &) = delete;
+};
+
+extern "C" {
+static int32_t absorb_rows(wax_vs_engine *e, wax_vs_engine *donor, uint64_t first, uint64_t n);
+static int32_t search_where_device(wax_vs_engine *e, const SearchRequest &req, const float *d_queries, uint64_t row_offset,
+                                   wax_vs_candidate *d_candidates, void *cuda_stream);
+static int32_t grouped_heads_device(wax_vs_engine *e, const SearchRequest &req, const float *d_queries, uint64_t row_offset,
+                                    wax_vs_group_candidate *d_heads, void *cuda_stream);
+static int32_t grouped_expand_device(wax_vs_engine *e, const SearchRequest &req, const float *d_queries,
+                                     const wax_vs_group_candidate *d_chosen, const wax_vs_group_candidate *d_own_heads,
+                                     uint64_t row_offset, wax_vs_candidate *d_rows, void *cuda_stream);
+}
 
 #include "waxvs_multi.cuh"
 
@@ -3098,16 +3142,15 @@ static int32_t shard_wait_host(wax_vs_engine *e, unsigned long long seq) {
     return rc;
 }
 
-struct Clause;
-static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k, bool filtered,
-                                 const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, const Clause *where,
-                                 uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n);
+static int32_t shard_search_host(wax_vs_engine *e, const SearchRequest &req, uint64_t *out_ids, float *out_scores,
+                                 uint32_t out_cap, uint32_t *out_n);
 
 int32_t wax_vs_shard_search(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k, uint64_t *out_ids,
                             float *out_scores, uint32_t out_cap, uint32_t *out_n) {
     WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_search");
     if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    return shard_search_host(e, query, query_len, top_k, false, nullptr, 0, 0, nullptr, out_ids, out_scores, out_cap, out_n);
+    const SearchRequest req(query, 1, query_len, top_k);
+    return shard_search_host(e, req, out_ids, out_scores, out_cap, out_n);
 }
 
 // Device-timed sharded searches, strictly one query at a time on one stream (the same mode as wax_vs_debug_time_search):
@@ -3404,6 +3447,15 @@ struct FilteredPlan {
     std::vector<uint32_t> order, k_of;
     uint32_t k_max = 0, n_tensor = 0, n_gather = 0;
 };
+// What plan_request made of a request: the resolved id filters (`ids`; where lists only), the filters the plan runs
+// (`fs`: the request's id filters, or its (where, id filter) pairs) with their modes, query i's filter pair_of[i]
+// (WAX_VS_NO_FILTER: unfiltered), and each query's k and class.
+struct WherePlan {
+    FilterSet ids, fs;
+    std::vector<int32_t> modes;
+    std::vector<uint32_t> pair_of;
+    FilteredPlan plan;
+};
 static void plan_filtered(const wax_vs_engine *e, int64_t top_k, const int32_t *filter_modes, const uint32_t *query_filter,
                           uint32_t n_queries, const FilterSet &fs, FilteredPlan &plan) {
     const uint64_t n_rows = e->n_rows;
@@ -3439,15 +3491,16 @@ static void plan_filtered(const wax_vs_engine *e, int64_t top_k, const int32_t *
 // The bitsets of the filters `which` (bitset l is filter which[l]'s) into c->d_mask on c->stream, from the rows
 // run_filtered staged in c->d_filter_rows: the listed rows in the filter's mode, then where search's predicate and box
 // ANDed in, and a wide term unit's rows set.  On an error the stream is synchronised.
-static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const int32_t *filter_modes, const FilterSet &fs,
-                               const std::vector<uint32_t> &which, uint64_t *launches) {
+static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const WherePlan &wp, const std::vector<uint32_t> &which,
+                               uint64_t *launches) {
+    const FilterSet &fs = wp.fs;
     const uint32_t nf = static_cast<uint32_t>(which.size());
     std::vector<uint64_t> spec(3u * nf + 1u, 0);
     for (uint32_t l = 0; l < nf; ++l) {
         const bool wide = !fs.term_of.empty() && fs.term_of[which[l]] != WAX_VS_NO_FILTER;
         spec[l + 1] = spec[l] + (wide ? 0 : fs.count[which[l]]);       // a wide term unit lists nothing
         spec[nf + 1 + l] = fs.first[which[l]];
-        spec[2u * nf + 1u + l] = static_cast<uint64_t>(filter_modes[which[l]]);
+        spec[2u * nf + 1u + l] = static_cast<uint64_t>(wp.modes[which[l]]);
     }
     int32_t rc;
     if ((rc = build_filter_bits(e, c, spec, nf, c->stream, launches))) { cudaStreamSynchronize(c->stream); return rc; }
@@ -3498,9 +3551,11 @@ struct FilteredTarget {
 // The planned queries on c->stream: staged query j's candidates land at c->d_out[j * k_max], on the device (with
 // tgt.shard: this rank's list there, the merged one at tgt.shard->final_out).  Stages the queries (c->d_queries, staged
 // order; for device queries the order goes to c->d_order) and the filters' rows (c->d_filter_rows).  plan.k_max > 0.
-static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries, const int32_t *filter_modes,
-                            uint32_t n_filters, const uint32_t *query_filter, const FilterSet &fs, const FilteredPlan &plan,
+static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries, const WherePlan &wp,
                             const FilteredTarget &tgt = FilteredTarget{}) {
+    const FilterSet &fs = wp.fs;
+    const FilteredPlan &plan = wp.plan;
+    const uint32_t *query_filter = wp.pair_of.data();
     const std::vector<uint32_t> &order = plan.order, &k_of = plan.k_of;
     const std::vector<uint64_t> &first = fs.first, &count = fs.count;
     const uint32_t k_max = plan.k_max, n_tensor = plan.n_tensor, n_gather = plan.n_gather;
@@ -3566,7 +3621,7 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
     // tensor and scan classes: sub-batches whose bitsets fit the budget (at least one always does)
     const uint64_t fit = std::max<uint64_t>(1, e->tune.filter_bitset_bytes / (static_cast<uint64_t>(words) * sizeof(uint32_t)));
     uint64_t distinct = 0;
-    for (uint32_t f = 0; f < n_filters; ++f) distinct += fs.referenced[f];
+    for (const uint8_t r : fs.referenced) distinct += r;
     const uint32_t per_pass = static_cast<uint32_t>(std::min<uint64_t>(fit, std::max<uint64_t>(distinct, 1)));
     // sized once for the largest pass: a later pass must not reallocate a buffer earlier launches still read
     if ((rc = c->d_mask.ensure(static_cast<size_t>(per_pass) * words, "row filters"))) return rc;
@@ -3587,7 +3642,7 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
                 index[s1] = f == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : static_cast<uint32_t>(which.size() - 1);
             }
             int32_t prc;
-            if (!which.empty() && (prc = build_pass_bits(e, c, filter_modes, fs, which, &launches))) return prc;
+            if (!which.empty() && (prc = build_pass_bits(e, c, wp, which, &launches))) return prc;
             RowFilter rf{c->d_mask.p, words, nullptr, index.data() + s0};
             const uint32_t nq = s1 - s0;
             const float *dq = c->d_queries + static_cast<size_t>(s0) * e->dims;
@@ -3620,11 +3675,11 @@ static int32_t run_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries
     return WAX_VS_OK;
 }
 
-// The argument checks of the per-query filtered entry points, run before the empty-engine early return.
-static int32_t check_filter_args(const wax_vs_engine *e, uint32_t n_queries, const uint64_t *frame_ids,
-                                 const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
-                                 const uint32_t *query_filter, const uint32_t *out_n) {
-    if (!e || !out_n || !filter_offsets || (n_filters && !filter_modes) || (n_queries && !query_filter))
+// The request's per-query id filters: filter f lists frame_ids[filter_offsets[f], filter_offsets[f + 1]) as an
+// allow-list (mode 0) or a deny-list (mode 1), and query i names filter query_filter[i].
+static int32_t request_filters(SearchRequest &r, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                               const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter) {
+    if (!filter_offsets || (n_filters && !filter_modes) || (r.n_queries && !query_filter))
         return fail(WAX_VS_ERR_NULL, "NULL argument");
     for (uint32_t f = 0; f < n_filters; ++f)
         if (filter_modes[f] != 0 && filter_modes[f] != 1)
@@ -3634,92 +3689,47 @@ static int32_t check_filter_args(const wax_vs_engine *e, uint32_t n_queries, con
         if (filter_offsets[f + 1] < filter_offsets[f])
             return fail(WAX_VS_ERR_ARGUMENT, "filter_offsets decrease at filter %u", f);
     if (filter_offsets[n_filters] && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
-    for (uint32_t i = 0; i < n_queries; ++i)
+    for (uint32_t i = 0; i < r.n_queries; ++i)
         if (query_filter[i] != WAX_VS_NO_FILTER && query_filter[i] >= n_filters)
             return fail(WAX_VS_ERR_ARGUMENT, "query %u names filter %u of %u", i, query_filter[i], n_filters);
+    r.frame_ids = frame_ids;
+    r.filter_offsets = filter_offsets;
+    r.filter_modes = filter_modes;
+    r.n_filters = n_filters;
+    r.query_filter = query_filter;
+    return WAX_VS_OK;
+}
+
+// One id filter for every query.  With empty_deny_is_none a deny-list of no ids is no filter (the grouped and shard entry
+// points); otherwise it is a filter that denies no row (the filtered ones).  The answers are the same.
+static int32_t request_one_filter(SearchRequest &r, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                                  bool empty_deny_is_none) {
+    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
+    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    r.one_offsets[1] = n_ids;
+    r.one_mode = mode;
+    r.filter_of.assign(r.n_queries, empty_deny_is_none && mode == 1 && n_ids == 0 ? WAX_VS_NO_FILTER : 0u);
+    r.frame_ids = frame_ids;
+    r.filter_offsets = r.one_offsets;
+    r.filter_modes = &r.one_mode;
+    r.n_filters = 1;
+    r.query_filter = r.filter_of.data();
     return WAX_VS_OK;
 }
 
 // The planned queries run on c, their answers delivered to the caller's buffers (plan.k_max > 0).
-static int32_t deliver_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries, const int32_t *filter_modes,
-                                uint32_t n_filters, const uint32_t *query_filter, const FilterSet &fs,
-                                const FilteredPlan &plan, uint64_t *out_ids, float *out_scores, uint32_t out_stride,
-                                uint32_t *out_n) {
+static int32_t deliver_filtered(wax_vs_engine *e, SearchCtx *c, const float *queries, const WherePlan &wp,
+                                uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    const FilteredPlan &plan = wp.plan;
     int32_t rc;
     const size_t ncand = static_cast<size_t>(plan.order.size()) * plan.k_max;
     if ((rc = c->h_out.ensure(ncand, "result staging"))) return rc;
-    if ((rc = run_filtered(e, c, queries, filter_modes, n_filters, query_filter, fs, plan))) return rc;
+    if ((rc = run_filtered(e, c, queries, wp))) return rc;
     CUDA_TRY(cudaMemcpyAsync(c->h_out, c->d_out, ncand * sizeof(wax_vs_candidate), cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));   // also keeps the host arrays alive until their copies are done
     deliver_results(e, c->h_out, static_cast<uint32_t>(plan.order.size()), plan.k_max, out_ids, out_scores, out_stride,
                     out_n, plan.order.data(), plan.k_of.data());
     return WAX_VS_OK;
-}
-
-static int32_t search_filtered_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                    int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                    const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                    uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    int32_t rc;
-    if ((rc = check_filter_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, out_n)))
-        return rc;
-    std::shared_lock<std::shared_mutex> r(e->rw);
-    for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
-    if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
-    if ((rc = check_query(e, queries, query_len))) return rc;
-    FilterSet fs;
-    resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, fs);
-    FilteredPlan plan;
-    plan_filtered(e, top_k, filter_modes, query_filter, n_queries, fs, plan);
-    const uint32_t k_max = plan.k_max;
-    if (k_max == 0) return WAX_VS_OK;
-    if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
-    if (out_stride < k_max) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, k_max);
-
-    DeviceGuard g(e->device);
-    if (!g.ok) return g.error();
-    CtxLease lease(e);
-    if ((rc = lease.acquire())) return rc;
-    return deliver_filtered(e, lease.c, queries, filter_modes, n_filters, query_filter, fs, plan, out_ids, out_scores,
-                            out_stride, out_n);
-}
-
-int32_t wax_vs_search_filtered(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k,
-                               const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids,
-                               float *out_scores, uint32_t out_cap, uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_filtered(e->multi->probe, query, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores, out_cap, out_n)) return rc;
-        return multi_search_filtered(e, query, 1, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores, out_cap, out_n);
-    }
-    const uint64_t offsets[2] = {0, n_ids};
-    const uint32_t query_filter = 0;
-    return search_filtered_host(e, query, 1, query_len, top_k, frame_ids, offsets, &mode, 1, &query_filter, out_ids,
-                                out_scores, out_cap, out_n);
-}
-
-int32_t wax_vs_search_batch_filtered(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                     int64_t top_k, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
-                                     uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_batch_filtered(e->multi->probe, queries, n_queries, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores, out_stride, out_n)) return rc;
-        return multi_search_filtered(e, queries, n_queries, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores, out_stride, out_n);
-    }
-    const uint64_t offsets[2] = {0, n_ids};
-    const std::vector<uint32_t> query_filter(n_queries, 0u);
-    return search_filtered_host(e, queries, n_queries, query_len, top_k, frame_ids, offsets, &mode, 1, query_filter.data(),
-                                out_ids, out_scores, out_stride, out_n);
-}
-
-int32_t wax_vs_search_batch_multi_filtered(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                           int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                           const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                           uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_batch_multi_filtered(e->multi->probe, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, out_ids, out_scores, out_stride, out_n)) return rc;
-        return multi_search_multi_filtered(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, out_ids, out_scores, out_stride, out_n);
-    }
-    return search_filtered_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
-                                query_filter, out_ids, out_scores, out_stride, out_n);
 }
 
 // ---- where search: attribute predicates below the top-k (waxvs_where.cuh) -------------------------------------------
@@ -3735,13 +3745,6 @@ constexpr uint64_t kWhereGatherRows = 16384;   // the gather class's largest all
 
 static WherePred where_pred(const wax_vs_where &w) { return WherePred{w.after, w.before, w.all_tags, w.no_tags}; }
 
-// A where as the host plans it: the time and tag clauses, the location box (kNoLocBox: no location clause) and the
-// sorted, distinct term ids a row must hold (none: no term clause).
-struct Clause {
-    WherePred pred;
-    LocBox box;
-    std::vector<uint64_t> terms;
-};
 static WhereNearItem where_item(const Clause &w) { return WhereNearItem{w.pred, 0, w.box}; }
 
 // Whether row r lies in box b (a row without a location lies in no active box).
@@ -3950,52 +3953,104 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const std::vecto
     return WAX_VS_OK;
 }
 
-// The batched where entry points after their argument checks and the building of their clauses.
-static int32_t search_where_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                 int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                 const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                 const std::vector<Clause> &wheres, const uint32_t *query_where, uint64_t *out_ids,
-                                 float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+// The planning step of every filtered, where and grouped search on this engine: the request's id filters resolved to
+// rows, then its (where, id filter) pairs planned as the filters of wp.fs (plan_where_pairs, which runs the count pass
+// on c's stream), then each query's k at most clamp(k) and its class (plan_filtered; skipped with plan_queries = false,
+// as round 2 of the sharded grouped search needs no classes).  A request without a where list plans its id filters as
+// they are, in filter order.
+static int32_t plan_request(wax_vs_engine *e, SearchCtx *c, const SearchRequest &req, int64_t k, WherePlan &wp,
+                            bool plan_queries = true) {
+    if (req.query_where) {
+        resolve_filters(e, req.frame_ids, req.filter_offsets, req.n_filters, req.query_filter, req.n_queries, wp.ids);
+        if (const int32_t rc = plan_where_pairs(e, c, req.wheres, req.query_where, req.filter_modes, req.query_filter,
+                                                req.n_queries, wp.ids, wp.fs, wp.modes, wp.pair_of))
+            return rc;
+    } else {
+        resolve_filters(e, req.frame_ids, req.filter_offsets, req.n_filters, req.query_filter, req.n_queries, wp.fs);
+        wp.modes.assign(req.filter_modes, req.filter_modes + req.n_filters);
+        wp.pair_of.assign(req.query_filter, req.query_filter + req.n_queries);
+    }
+    if (plan_queries) plan_filtered(e, k, wp.modes.data(), wp.pair_of.data(), req.n_queries, wp.fs, wp.plan);
+    return WAX_VS_OK;
+}
+
+// The filtered and where entry points on one engine, after their argument checks.
+static int32_t search_where_host(wax_vs_engine *e, const SearchRequest &req, uint64_t *out_ids, float *out_scores,
+                                 uint32_t out_stride, uint32_t *out_n) {
     int32_t rc;
     std::shared_lock<std::shared_mutex> r(e->rw);
-    for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
-    if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;
-    if ((rc = check_query(e, queries, query_len))) return rc;
-    FilterSet ids;
-    resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, ids);
+    for (uint32_t i = 0; i < req.n_queries; ++i) out_n[i] = 0;
+    if (e->n_rows == 0 || req.n_queries == 0) return WAX_VS_OK;
+    if ((rc = check_query(e, req.queries, req.query_len))) return rc;
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
     CtxLease lease(e);
     if ((rc = lease.acquire())) return rc;
-    FilterSet fs;
-    std::vector<int32_t> modes;
-    std::vector<uint32_t> pair_of;
-    if ((rc = plan_where_pairs(e, lease.c, wheres, query_where, filter_modes, query_filter, n_queries, ids, fs, modes,
-                               pair_of)))
-        return rc;
-    FilteredPlan plan;
-    plan_filtered(e, top_k, modes.data(), pair_of.data(), n_queries, fs, plan);
-    if (plan.k_max == 0) return WAX_VS_OK;
+    WherePlan wp;
+    if ((rc = plan_request(e, lease.c, req, req.top_k, wp))) return rc;
+    const uint32_t k_max = wp.plan.k_max;
+    if (k_max == 0) return WAX_VS_OK;
     if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
-    if (out_stride < plan.k_max)
-        return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, plan.k_max);
-    return deliver_filtered(e, lease.c, queries, modes.data(), static_cast<uint32_t>(modes.size()), pair_of.data(), fs, plan,
-                            out_ids, out_scores, out_stride, out_n);
+    if (out_stride < k_max) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, k_max);
+    return deliver_filtered(e, lease.c, req.queries, wp, out_ids, out_scores, out_stride, out_n);
 }
 
-// The argument checks of wax_vs_search_batch_where (and _near), before the empty-engine early return.
-static int32_t check_where_args(wax_vs_engine *e, uint32_t n_queries, const uint64_t *frame_ids,
-                                const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
-                                const uint32_t *query_filter, const void *wheres, uint32_t n_wheres,
-                                const uint32_t *query_where, uint32_t *out_n) {
-    int32_t rc;
-    if ((rc = check_filter_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, out_n)))
-        return rc;
-    if ((n_wheres && !wheres) || (n_queries && !query_where)) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    for (uint32_t i = 0; i < n_queries; ++i)
+// The filtered and where entry points after their argument checks: on one engine, or across the shards of a
+// multi-device handle, which first zeroes out_n as one engine does.
+static int32_t search_where(wax_vs_engine *e, const SearchRequest &req, uint64_t *out_ids, float *out_scores,
+                            uint32_t out_stride, uint32_t *out_n) {
+    if (!e->multi) return search_where_host(e, req, out_ids, out_scores, out_stride, out_n);
+    for (uint32_t i = 0; i < req.n_queries; ++i) out_n[i] = 0;
+    return multi_search_where(e->multi, e->dims, e->similarity, req, out_ids, out_scores, out_stride, out_n);
+}
+
+// The request's per-query wheres: query i names where query_where[i] of n_wheres, whose clauses one of the builders
+// below makes.
+static int32_t request_where_list(SearchRequest &r, const void *wheres, uint32_t n_wheres, const uint32_t *query_where) {
+    if ((n_wheres && !wheres) || (r.n_queries && !query_where)) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    for (uint32_t i = 0; i < r.n_queries; ++i)
         if (query_where[i] != WAX_VS_NO_FILTER && query_where[i] >= n_wheres)
             return fail(WAX_VS_ERR_ARGUMENT, "query %u names where %u of %u", i, query_where[i], n_wheres);
+    r.query_where = query_where;
     return WAX_VS_OK;
+}
+
+// The time and tag clauses of wheres[0, n_wheres), no location, no terms.
+static void request_plain_clauses(SearchRequest &r, const wax_vs_where *wheres, uint32_t n_wheres) {
+    r.wheres.resize(n_wheres);
+    for (uint32_t w = 0; w < n_wheres; ++w) r.wheres[w] = Clause{where_pred(wheres[w]), kNoLocBox, {}};
+}
+
+// The request's where, if it has one, for every query.
+static void request_one_where(SearchRequest &r) {
+    r.where_of.assign(r.n_queries, r.wheres.empty() ? WAX_VS_NO_FILTER : 0u);
+    r.query_where = r.where_of.data();
+}
+
+int32_t wax_vs_search_filtered(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k,
+                               const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids,
+                               float *out_scores, uint32_t out_cap, uint32_t *out_n) {
+    return wax_vs_search_batch_filtered(e, query, 1, query_len, top_k, frame_ids, n_ids, mode, out_ids, out_scores, out_cap,
+                                        out_n);
+}
+
+int32_t wax_vs_search_batch_filtered(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                     int64_t top_k, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
+                                     uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(queries, n_queries, query_len, top_k);
+    const int32_t rc = request_one_filter(req, frame_ids, n_ids, mode, false);
+    return rc ? rc : search_where(e, req, out_ids, out_scores, out_stride, out_n);
+}
+
+int32_t wax_vs_search_batch_multi_filtered(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                           int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                           const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                           uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(queries, n_queries, query_len, top_k);
+    const int32_t rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter);
+    return rc ? rc : search_where(e, req, out_ids, out_scores, out_stride, out_n);
 }
 
 int32_t wax_vs_search_batch_where(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
@@ -4003,18 +4058,14 @@ int32_t wax_vs_search_batch_where(wax_vs_engine *e, const float *queries, uint32
                                   const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
                                   const wax_vs_where *wheres, uint32_t n_wheres, const uint32_t *query_where,
                                   uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_batch_where(e->multi->probe, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_stride, out_n)) return rc;
-        return multi_search_batch_where(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_stride, out_n);
-    }
+    if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(queries, n_queries, query_len, top_k);
     int32_t rc;
-    if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
-                               n_wheres, query_where, out_n)))
+    if ((rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
+        (rc = request_where_list(req, wheres, n_wheres, query_where)))
         return rc;
-    std::vector<Clause> clauses(n_wheres);
-    for (uint32_t w = 0; w < n_wheres; ++w) clauses[w] = Clause{where_pred(wheres[w]), kNoLocBox, {}};
-    return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
-                             query_filter, clauses, query_where, out_ids, out_scores, out_stride, out_n);
+    request_plain_clauses(req, wheres, n_wheres);
+    return search_where(e, req, out_ids, out_scores, out_stride, out_n);
 }
 
 // ---- location predicates: PhotoRAG's location box beside the time and tag clauses (waxvs_where.cuh) -----------------
@@ -4148,18 +4199,13 @@ int32_t wax_vs_search_batch_where_near(wax_vs_engine *e, const float *queries, u
                                        const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
                                        const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
                                        uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_batch_where_near(e->multi->probe, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_stride, out_n)) return rc;
-        return multi_search_where(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, nullptr, nullptr, out_ids, out_scores, out_stride, out_n);
-    }
+    if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(queries, n_queries, query_len, top_k);
     int32_t rc;
-    if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
-                               n_wheres, query_where, out_n)))
+    if ((rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
+        (rc = request_where_list(req, wheres, n_wheres, query_where)) || (rc = near_clauses(wheres, n_wheres, req.wheres)))
         return rc;
-    std::vector<Clause> clauses;
-    if ((rc = near_clauses(wheres, n_wheres, clauses))) return rc;
-    return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
-                             query_filter, clauses, query_where, out_ids, out_scores, out_stride, out_n);
+    return search_where(e, req, out_ids, out_scores, out_stride, out_n);
 }
 
 // ---- term clauses: Wax's metadataFilter as required term ids, from an inverted index (waxvs_terms.cuh) ---------------
@@ -4221,25 +4267,25 @@ int32_t wax_vs_set_terms(wax_vs_engine *e, const uint64_t *frame_ids, const uint
     return WAX_VS_OK;
 }
 
-// The clauses of wheres[0, n_wheres) with their term lists (offsets checked by the caller), and qw[i] = the where query
-// i names.  Wheres with terms and equal contents (clauses, box, required ids) are one: each query names the first of
-// them, so a batch that scopes 1 024 queries to 16 sessions plans 16 units, not 1 024.
-static int32_t term_clauses(const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
-                            uint32_t n_queries, const uint64_t *where_term_offsets, const uint64_t *where_terms,
-                            std::vector<Clause> &clauses, std::vector<uint32_t> &qw) {
+// The clauses of wheres[0, n_wheres) with their term lists.  With a where list, wheres with terms and equal contents
+// (clauses, box, required ids) are one: each query names the first of them, so a batch that scopes 1 024 queries to 16
+// sessions plans 16 units, not 1 024.
+static int32_t request_term_clauses(SearchRequest &r, const wax_vs_where_near *wheres, uint32_t n_wheres,
+                                    const uint64_t *where_term_offsets, const uint64_t *where_terms) {
     int32_t rc;
     if ((rc = check_term_offsets(where_term_offsets, n_wheres, where_terms, kMaxWhereTerms, "where_term_offsets"))) return rc;
-    if ((rc = near_clauses(wheres, n_wheres, clauses))) return rc;
+    if ((rc = near_clauses(wheres, n_wheres, r.wheres))) return rc;
     for (uint32_t w = 0; w < n_wheres; ++w) {
-        std::vector<uint64_t> &terms = clauses[w].terms;
+        std::vector<uint64_t> &terms = r.wheres[w].terms;
         terms.assign(where_terms + where_term_offsets[w], where_terms + where_term_offsets[w + 1]);
         std::sort(terms.begin(), terms.end());
         terms.erase(std::unique(terms.begin(), terms.end()), terms.end());
     }
+    if (!r.query_where) return WAX_VS_OK;
     std::vector<uint32_t> canon(n_wheres);
     std::unordered_map<std::string, uint32_t> first_of;
     for (uint32_t w = 0; w < n_wheres; ++w) {
-        const Clause &cl = clauses[w];
+        const Clause &cl = r.wheres[w];
         canon[w] = w;
         if (cl.terms.empty()) continue;
         std::string key(reinterpret_cast<const char *>(&cl.pred), sizeof(WherePred));
@@ -4247,8 +4293,10 @@ static int32_t term_clauses(const wax_vs_where_near *wheres, uint32_t n_wheres, 
         key.append(reinterpret_cast<const char *>(cl.terms.data()), cl.terms.size() * sizeof(uint64_t));
         canon[w] = first_of.emplace(std::move(key), w).first->second;
     }
-    qw.resize(n_queries);
-    for (uint32_t i = 0; i < n_queries; ++i) qw[i] = query_where[i] == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : canon[query_where[i]];
+    r.where_of.resize(r.n_queries);
+    for (uint32_t i = 0; i < r.n_queries; ++i)
+        r.where_of[i] = r.query_where[i] == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : canon[r.query_where[i]];
+    r.query_where = r.where_of.data();
     return WAX_VS_OK;
 }
 
@@ -4258,21 +4306,15 @@ int32_t wax_vs_search_batch_where_terms(wax_vs_engine *e, const float *queries, 
                                         const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
                                         const uint64_t *where_term_offsets, const uint64_t *where_terms,
                                         uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_batch_where_terms(e->multi->probe, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, where_term_offsets, where_terms, out_ids, out_scores, out_stride, out_n)) return rc;
-        return multi_search_where(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, where_term_offsets, where_terms, out_ids, out_scores, out_stride, out_n);
-    }
+    if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(queries, n_queries, query_len, top_k);
     int32_t rc;
-    if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
-                               n_wheres, query_where, out_n)))
+    if ((rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
+        (rc = request_where_list(req, wheres, n_wheres, query_where)))
         return rc;
     if (!where_term_offsets) return fail(WAX_VS_ERR_NULL, "where_term_offsets is NULL");
-    std::vector<Clause> clauses;
-    std::vector<uint32_t> qw;
-    if ((rc = term_clauses(wheres, n_wheres, query_where, n_queries, where_term_offsets, where_terms, clauses, qw)))
-        return rc;
-    return search_where_host(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets, filter_modes, n_filters,
-                             query_filter, clauses, qw.data(), out_ids, out_scores, out_stride, out_n);
+    if ((rc = request_term_clauses(req, wheres, n_wheres, where_term_offsets, where_terms))) return rc;
+    return search_where(e, req, out_ids, out_scores, out_stride, out_n);
 }
 
 // ---- sharded where search -----------------------------------------------------------------------------------------
@@ -4298,20 +4340,18 @@ static int32_t reserve_shard_scratch(wax_vs_engine *e, SearchCtx *c) {
 }
 
 // The host-path collective search of the shard entry points, under the read lock it takes (caller: e and out_n checked,
-// and the filtered form's mode and ids, the where's clauses).  Without a filter or a where: the rank's fused scan, the
-// in-kernel exchange and merge, the merged list delivered into mapped host memory.  Otherwise the rank plans its shard
-// for the one query as the where entry points do (filtered: the id filter; `where`: its clauses) and runs the plan with
-// exactly one exchange: a gathered unit is exchanged by the stand-alone kernel, a row bitset rides in the fused scan, and
-// a shard where nothing passes exchanges padding.
-static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_k, bool filtered,
-                                 const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, const Clause *where,
-                                 uint64_t *out_ids, float *out_scores, uint32_t out_cap, uint32_t *out_n) {
+// the request built).  A request without an id filter (wax_vs_shard_search): the rank's fused scan, the in-kernel
+// exchange and merge, the merged list delivered into mapped host memory.  Otherwise the rank plans its shard for the one
+// query as the where entry points do and runs the plan with exactly one exchange: a gathered unit is exchanged by the
+// stand-alone kernel, a row bitset rides in the fused scan, and a shard where nothing passes exchanges padding.
+static int32_t shard_search_host(wax_vs_engine *e, const SearchRequest &req, uint64_t *out_ids, float *out_scores,
+                                 uint32_t out_cap, uint32_t *out_n) {
     std::shared_lock<std::shared_mutex> r(e->rw);
     *out_n = 0;
     if (!e->shard.connected) return fail(WAX_VS_ERR_ARGUMENT, "the shard group is not connected (wax_vs_shard_open / _connect)");
     int32_t rc;
-    if ((rc = check_query(e, query, query_len))) return rc;
-    const uint32_t k_eff = clamp_topk(top_k);
+    if ((rc = check_query(e, req.queries, req.query_len))) return rc;
+    const uint32_t k_eff = clamp_topk(req.top_k);
     if (k_eff > static_cast<uint32_t>(kShardKCap))
         return fail(WAX_VS_ERR_UNSUPPORTED, "sharded search supports top_k <= %d (got %u)", kShardKCap, k_eff);
     if (!out_ids || !out_scores) return fail(WAX_VS_ERR_NULL, "output buffer is NULL");
@@ -4324,26 +4364,16 @@ static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t 
     const uint64_t *d_ids = nullptr;
     if ((rc = sync_device_ids(e, &d_ids))) return rc;
     uint64_t launches = 0;
-    const bool planned = filtered || where;
-    // the plan of the one query: pair (where 0 or none, id filter 0 or none); a deny-list of nothing is no filter
-    const std::vector<Clause> wheres(where ? 1 : 0, where ? *where : Clause{});
-    const uint32_t qw = where ? 0u : WAX_VS_NO_FILTER, qf = filtered && (mode == 0 || n_ids) ? 0u : WAX_VS_NO_FILTER;
-    const uint64_t offsets[2] = {0, n_ids};
-    FilterSet ids, fs;
-    std::vector<int32_t> modes;
-    std::vector<uint32_t> pair_of;
-    FilteredPlan plan;
-    if (planned && e->n_rows) {
-        resolve_filters(e, frame_ids, offsets, 1, &qf, 1, ids);
-        if ((rc = reserve_shard_scratch(e, c)) ||
-            (rc = plan_where_pairs(e, c, wheres, &qw, &mode, &qf, 1, ids, fs, modes, pair_of)))
-            return rc;
-        plan_filtered(e, k_eff, modes.data(), pair_of.data(), 1, fs, plan);
-    }
+    const bool planned = req.query_filter != nullptr;
+    WherePlan wp;
+    if (planned && e->n_rows &&
+        ((rc = reserve_shard_scratch(e, c)) || (rc = plan_request(e, c, req, k_eff, wp))))
+        return rc;
+    FilteredPlan &plan = wp.plan;
     ShardParams sp = shard_params_next(e);
     sp.host_out = sh.h_final; sp.host_flag = sh.h_flag;      // mapped pinned: the kernel delivers the result itself
     if (!planned) {
-        HostDelivery hd{query, nullptr, nullptr, 0};             // the query rides in the kernel parameters when it fits
+        HostDelivery hd{req.queries, nullptr, nullptr, 0};       // the query rides in the kernel parameters when it fits
         rc = enqueue_search(e, c, nullptr, k_eff, sh.row_offset, sh.d_final, d_ids, c->stream, &launches, nullptr, &sp, &hd);
     } else if (plan.order.empty()) {                              // an empty shard, or nothing on it passes: padding
         sp.final_out = sh.d_final;
@@ -4355,7 +4385,7 @@ static int32_t shard_search_host(wax_vs_engine *e, const float *query, uint32_t 
         plan.k_max = plan.k_of[0] = k_eff;
         FilteredTarget tgt;
         tgt.row_offset = sh.row_offset; tgt.d_ids = d_ids; tgt.shard = &sp;
-        rc = run_filtered(e, c, query, modes.data(), static_cast<uint32_t>(modes.size()), pair_of.data(), fs, plan, tgt);
+        rc = run_filtered(e, c, req.queries, wp, tgt);
     }
     if (rc) { cudaStreamSynchronize(c->stream); return rc; }
     if ((rc = shard_wait_host(e, sp.seq))) { cudaStreamSynchronize(c->stream); return rc; }
@@ -4379,68 +4409,42 @@ int32_t wax_vs_shard_search_where(wax_vs_engine *e, const float *query, uint32_t
                                   uint32_t out_cap, uint32_t *out_n) {
     WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_search_where");
     if (!e || !out_n || !where) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
-    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
+    SearchRequest req(query, 1, query_len, top_k);
     const uint64_t term_offsets[2] = {0, n_terms};
-    std::vector<Clause> clauses;
-    std::vector<uint32_t> qw;
-    const uint32_t q0 = 0;
     int32_t rc;
-    if ((rc = term_clauses(where, 1, &q0, 1, term_offsets, terms, clauses, qw))) return rc;
-    return shard_search_host(e, query, query_len, top_k, true, frame_ids, n_ids, mode, &clauses[0], out_ids, out_scores,
-                             out_cap, out_n);
+    if ((rc = request_one_filter(req, frame_ids, n_ids, mode, true)) ||
+        (rc = request_term_clauses(req, where, 1, term_offsets, terms)))
+        return rc;
+    request_one_where(req);
+    return shard_search_host(e, req, out_ids, out_scores, out_cap, out_n);
 }
 
-// The rank-local half of a batched sharded where search: the plan of wax_vs_search_batch_where_terms on this shard, run
-// on the caller's stream with global rows and frame ids, then each planned query's list scattered to its place in
-// d_candidates (every other slot is padding).
-int32_t wax_vs_search_batch_where_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries, int64_t top_k,
-                                         const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                         const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                         const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
-                                         const uint64_t *where_term_offsets, const uint64_t *where_terms,
-                                         uint64_t row_offset, wax_vs_candidate *d_candidates, void *cuda_stream) {
-    WAX_VS_MULTI_REFUSE(e, "wax_vs_search_batch_where_device");
-    int32_t rc;
-    uint32_t no_out_n = 0;                  // the checks of the host forms, which also test their out_n
-    if ((rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
-                               n_wheres, query_where, &no_out_n)))
-        return rc;
-    if (!d_queries || !d_candidates) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    std::vector<Clause> clauses;
-    std::vector<uint32_t> qw;
-    if (where_term_offsets) {
-        rc = term_clauses(wheres, n_wheres, query_where, n_queries, where_term_offsets, where_terms, clauses, qw);
-    } else {
-        rc = near_clauses(wheres, n_wheres, clauses);
-        qw.assign(query_where, query_where + n_queries);
-    }
-    if (rc) return rc;
+// The rank-local half of a batched sharded where search (wax_vs_search_batch_where_device, and each shard of a
+// multi-device handle): the request's plan on this shard, run on the caller's stream with global rows and frame ids,
+// then each planned query's list scattered to its place in d_candidates (every other slot is padding).
+static int32_t search_where_device(wax_vs_engine *e, const SearchRequest &req, const float *d_queries, uint64_t row_offset,
+                                   wax_vs_candidate *d_candidates, void *cuda_stream) {
+    const uint32_t n_queries = req.n_queries;
     if (n_queries == 0) return WAX_VS_OK;
     std::shared_lock<std::shared_mutex> r(e->rw);
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
     SearchCtx *c = nullptr;
+    int32_t rc;
     if ((rc = ctx_for_stream(e, cuda_stream, &c))) return rc;
-    const uint32_t k_out = clamp_topk(top_k);
+    const uint32_t k_out = clamp_topk(req.top_k);
     e->async_pending.store(true);
     CUDA_TRY(cudaMemsetAsync(d_candidates, 0, static_cast<size_t>(n_queries) * k_out * sizeof(wax_vs_candidate), c->stream));
     if (e->n_rows == 0) return WAX_VS_OK;
     const uint64_t *d_ids = nullptr;
     if ((rc = sync_device_ids(e, &d_ids))) return rc;
-    FilterSet ids, fs;
-    resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, ids);
-    std::vector<int32_t> modes;
-    std::vector<uint32_t> pair_of;
-    if ((rc = plan_where_pairs(e, c, clauses, qw.data(), filter_modes, query_filter, n_queries, ids, fs, modes, pair_of)))
-        return rc;
-    FilteredPlan plan;
-    plan_filtered(e, top_k, modes.data(), pair_of.data(), n_queries, fs, plan);
+    WherePlan wp;
+    if ((rc = plan_request(e, c, req, req.top_k, wp))) return rc;
+    const FilteredPlan &plan = wp.plan;
     if (plan.k_max == 0) return WAX_VS_OK;
     FilteredTarget tgt;
     tgt.row_offset = row_offset; tgt.d_ids = d_ids; tgt.device_queries = true;
-    if ((rc = run_filtered(e, c, d_queries, modes.data(), static_cast<uint32_t>(modes.size()), pair_of.data(), fs, plan, tgt)))
-        return rc;
+    if ((rc = run_filtered(e, c, d_queries, wp, tgt))) return rc;
     const uint32_t n_staged = static_cast<uint32_t>(plan.order.size());
     const size_t total = static_cast<size_t>(n_staged) * plan.k_max;
     const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (total + 255) / 256)));
@@ -4451,6 +4455,27 @@ int32_t wax_vs_search_batch_where_device(wax_vs_engine *e, const float *d_querie
     return WAX_VS_OK;
 }
 
+// The plan of wax_vs_search_batch_where_terms (or of _near, without term lists) on this rank's shard.
+int32_t wax_vs_search_batch_where_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries, int64_t top_k,
+                                         const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                         const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                         const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                         const uint64_t *where_term_offsets, const uint64_t *where_terms,
+                                         uint64_t row_offset, wax_vs_candidate *d_candidates, void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_search_batch_where_device");
+    if (!e) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(nullptr, n_queries, e->dims, top_k);
+    int32_t rc;
+    if ((rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
+        (rc = request_where_list(req, wheres, n_wheres, query_where)))
+        return rc;
+    if (!d_queries || !d_candidates) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    if ((rc = where_term_offsets ? request_term_clauses(req, wheres, n_wheres, where_term_offsets, where_terms)
+                                 : near_clauses(wheres, n_wheres, req.wheres)))
+        return rc;
+    return search_where_device(e, req, d_queries, row_offset, d_candidates, cuda_stream);
+}
+
 // The row-sharded form: every rank passes the SAME ids; a rank resolves the ones its shard holds (the others are
 // unknown to it and ignored), its fused scan consults the bitset below the top-k, and the usual in-kernel exchange
 // merges the ranks' lists -- the answer is the filtered top-k of the whole corpus, identical on every rank.
@@ -4459,10 +4484,11 @@ int32_t wax_vs_shard_search_filtered(wax_vs_engine *e, const float *query, uint3
                                      float *out_scores, uint32_t out_cap, uint32_t *out_n) {
     WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_search_filtered");
     if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
-    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
-    return shard_search_host(e, query, query_len, top_k, true, frame_ids, n_ids, mode, nullptr, out_ids, out_scores, out_cap,
-                             out_n);
+    SearchRequest req(query, 1, query_len, top_k);
+    const int32_t rc = request_one_filter(req, frame_ids, n_ids, mode, true);
+    if (rc) return rc;
+    request_one_where(req);
+    return shard_search_host(e, req, out_ids, out_scores, out_cap, out_n);
 }
 
 // ---- grouped search (waxvs_group.cuh) -----------------------------------------------------------------------------
@@ -4877,8 +4903,8 @@ static int32_t enqueue_batch_expansion(wax_vs_engine *e, SearchCtx *c, const Cov
 // plan and run in passes of at most `fit` distinct units' bitsets (build_pass_bits); each pass ends in a synchronise, so
 // the next one may rebuild the bitsets.
 static int32_t expand_in_passes(wax_vs_engine *e, SearchCtx *c, CoverExpand *list, uint32_t n_exp,
-                                const std::vector<uint32_t> &unit, const int32_t *modes, const FilterSet &fs,
-                                uint32_t n_top, uint32_t per_group, uint64_t *launches, uint64_t *passes) {
+                                const std::vector<uint32_t> &unit, const WherePlan &wp, uint32_t n_top,
+                                uint32_t per_group, uint64_t *launches, uint64_t *passes) {
     std::sort(list, list + n_exp, [&](const CoverExpand &a, const CoverExpand &b) {
         if (unit[a.query] != unit[b.query]) return unit[a.query] < unit[b.query];
         return a.query != b.query ? a.query < b.query : a.slot < b.slot;
@@ -4899,7 +4925,7 @@ static int32_t expand_in_passes(wax_vs_engine *e, SearchCtx *c, CoverExpand *lis
             query_slot[list[i1].query] = u == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : static_cast<uint32_t>(which.size() - 1);
         }
         if (!which.empty()) {
-            if ((rc = build_pass_bits(e, c, modes, fs, which, launches))) return rc;
+            if ((rc = build_pass_bits(e, c, wp, which, launches))) return rc;
             ++*passes;
         }
         if ((rc = enqueue_batch_expansion(e, c, list + i0, i1 - i0, n_top, per_group, query_slot, launches))) {
@@ -4911,21 +4937,19 @@ static int32_t expand_in_passes(wax_vs_engine *e, SearchCtx *c, CoverExpand *lis
     return WAX_VS_OK;
 }
 
-// The grouped checks of every grouped entry point, before the empty-engine early return.
-static int32_t check_grouped_args(const wax_vs_engine *e, int64_t top_groups, uint32_t per_group, const uint64_t *out_ids,
-                                  const float *out_scores, const uint64_t *out_groups, const uint32_t *out_n) {
-    if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    if (per_group == 0 || per_group > WAX_VS_MAX_PER_GROUP)
-        return fail(WAX_VS_ERR_ARGUMENT, "per_group must be in [1, %d] (got %u)", WAX_VS_MAX_PER_GROUP, per_group);
-    const uint32_t n_top = clamp_topk(top_groups);
-    if (static_cast<uint64_t>(n_top) * per_group > WAX_VS_MAX_RESULTS)
+// The request's grouped arguments: per_group in [1, WAX_VS_MAX_PER_GROUP], at most WAX_VS_MAX_RESULTS rows per query.
+static int32_t check_grouped_args(const SearchRequest &r) {
+    if (r.per_group == 0 || r.per_group > WAX_VS_MAX_PER_GROUP)
+        return fail(WAX_VS_ERR_ARGUMENT, "per_group must be in [1, %d] (got %u)", WAX_VS_MAX_PER_GROUP, r.per_group);
+    const uint32_t n_top = clamp_topk(r.top_k);
+    if (static_cast<uint64_t>(n_top) * r.per_group > WAX_VS_MAX_RESULTS)
         return fail(WAX_VS_ERR_ARGUMENT, "clamp(top_groups) x per_group = %llu exceeds %d",
-                    static_cast<unsigned long long>(n_top) * per_group, WAX_VS_MAX_RESULTS);
+                    static_cast<unsigned long long>(n_top) * r.per_group, WAX_VS_MAX_RESULTS);
     return WAX_VS_OK;
 }
 
-// Every grouped entry point after its argument checks: query i searches the rows passing wheres[query_where[i]] AND id
-// filter query_filter[i], either of which may be WAX_VS_NO_FILTER.
+// Every grouped entry point on one engine after its argument checks, `queries` being the request's on the host: query i
+// searches the rows passing wheres[query_where[i]] AND id filter query_filter[i], either of which may be WAX_VS_NO_FILTER.
 // The (where, id filter) pairs are the units of the where search (plan_where_pairs), planned by the batched filtered
 // search at k_c; a query no row passes answers nothing.  Without `batched`, or when the coverage level does not take the
 // batch, every query runs grouped_one.  The batch pipeline:
@@ -4941,40 +4965,32 @@ struct ShardHeads {
     uint64_t row_offset;
     wax_vs_group_candidate *d_heads;
 };
-static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                   int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids,
-                                   const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
-                                   const uint32_t *query_filter, const std::vector<Clause> &wheres,
-                                   const uint32_t *query_where, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
-                                   uint32_t out_stride, uint32_t *out_n, bool batched, const ShardHeads *heads = nullptr) {
-    const uint32_t n_top = clamp_topk(top_groups);
+static int32_t search_grouped_host(wax_vs_engine *e, const SearchRequest &req, const float *queries, uint64_t *out_ids,
+                                   float *out_scores, uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n,
+                                   const ShardHeads *heads = nullptr) {
+    const uint32_t n_queries = req.n_queries, per_group = req.per_group;
+    const uint32_t n_top = clamp_topk(req.top_k);
     std::shared_lock<std::shared_mutex> r(e->rw);
     for (uint32_t i = 0; i < n_queries; ++i) out_n[i] = 0;
     if (e->n_rows == 0 || n_queries == 0) return WAX_VS_OK;      // as wax_vs_search (:448)
     int32_t rc;
-    if ((rc = check_query(e, queries, query_len))) return rc;
+    if ((rc = check_query(e, queries, req.query_len))) return rc;
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(n_top) * per_group, n));
     if (!heads && out_stride < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, need);
-    FilterSet ids;
-    resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, ids);
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
     CtxLease lease(e);
     if ((rc = lease.acquire())) return rc;
     SearchCtx *c = lease.c;
-    FilterSet fs;
-    std::vector<int32_t> modes;
-    std::vector<uint32_t> pair_of;
-    if ((rc = plan_where_pairs(e, c, wheres, query_where, filter_modes, query_filter, n_queries, ids, fs, modes, pair_of)))
-        return rc;
     // The coverage level: each query's exact top-k_c rows, when the batch goes to the tensor-core levels or the gather
     // class of the batched filtered search; every other batch runs the single-query pipeline per query.
     const uint32_t k_c = std::min(kCoverMax, std::max(128u, 4u * n_top));
-    FilteredPlan plan;
-    plan_filtered(e, k_c, modes.data(), pair_of.data(), n_queries, fs, plan);
+    WherePlan wp;
+    if ((rc = plan_request(e, c, req, k_c, wp))) return rc;
+    const FilteredPlan &plan = wp.plan;
     const uint32_t nq = static_cast<uint32_t>(plan.order.size());    // the staged queries: some row passes
-    const bool cover = batched && nq > 0 && n_top <= kCoverMax / 4 &&
+    const bool cover = req.batched && nq > 0 && n_top <= kCoverMax / 4 &&
                        (plan.n_gather == nq || (plan.n_tensor == nq && batch_tensor_eligible(e, nq, plan.k_max)));
     cudaStream_t s = c->stream;
     std::vector<uint32_t> crowded;                   // queries for the single-query pipeline
@@ -4983,8 +4999,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
         crowded = plan.order;
     } else {
         if ((rc = ensure_group_index(e, c))) return rc;
-        if ((rc = run_filtered(e, c, queries, modes.data(), static_cast<uint32_t>(modes.size()), pair_of.data(), fs, plan)))
-            return rc;
+        if ((rc = run_filtered(e, c, queries, wp))) return rc;
         const uint32_t slots = n_top * per_group;
         const size_t nkeys = static_cast<size_t>(nq) * slots;
         if ((rc = c->d_bg_keys.ensure(nkeys, "grouped batch keys")) || (rc = c->h_bg_keys.ensure(nkeys, "grouped batch staging")) ||
@@ -5005,9 +5020,8 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
             CUDA_TRY(cudaMemcpyAsync(c->h_bg_expand, c->d_bg_expand, n_exp * sizeof(CoverExpand), cudaMemcpyDeviceToHost, s));
             CUDA_TRY(cudaStreamSynchronize(s));
             std::vector<uint32_t> unit(nq);          // staged query -> its pair (WAX_VS_NO_FILTER, unfiltered, sorts last)
-            for (uint32_t j = 0; j < nq; ++j) unit[j] = pair_of[plan.order[j]];
-            if ((rc = expand_in_passes(e, c, c->h_bg_expand, n_exp, unit, modes.data(), fs, n_top, per_group, &launches,
-                                       &expansion_passes)))
+            for (uint32_t j = 0; j < nq; ++j) unit[j] = wp.pair_of[plan.order[j]];
+            if ((rc = expand_in_passes(e, c, c->h_bg_expand, n_exp, unit, wp, n_top, per_group, &launches, &expansion_passes)))
                 return rc;
             expanded = n_exp;
         }
@@ -5038,22 +5052,23 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     // under the query's own pair as the one-filter grouped search takes it -- an id filter alone as it is, an allow-list
     // as its rows that pass the where (plan_where_pairs listed them), a deny-list (or none) AND a where as the deny-list
     // in mode 1 with the predicate and its box ANDed into the bitset
+    const FilterSet &ids = wp.ids, &fs = wp.fs;
     for (uint32_t qi : crowded) {
-        const uint32_t p = pair_of[qi], w = query_where[qi], f = query_filter[qi];
-        const bool row_where = w != WAX_VS_NO_FILTER && (f == WAX_VS_NO_FILTER || filter_modes[f] == 1);
+        const uint32_t p = wp.pair_of[qi], w = req.query_where[qi], f = req.query_filter[qi];
+        const bool row_where = w != WAX_VS_NO_FILTER && (f == WAX_VS_NO_FILTER || req.filter_modes[f] == 1);
         std::vector<uint32_t> rows;
         int32_t mode = 1;
         if (row_where) {
             if (f != WAX_VS_NO_FILTER) rows.assign(ids.rows.begin() + ids.first[f], ids.rows.begin() + ids.first[f] + ids.count[f]);
         } else if (p != WAX_VS_NO_FILTER) {
             rows.assign(fs.rows.begin() + fs.first[p], fs.rows.begin() + fs.first[p] + fs.count[p]);
-            mode = modes[p];
+            mode = wp.modes[p];
         }
         if (heads) {                                 // the answer's keys -> records, uploaded into the query's slots
             const size_t slots = static_cast<size_t>(n_top) * per_group;
             std::vector<uint64_t> keys(slots);
             if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group,
-                                  p == WAX_VS_NO_FILTER ? nullptr : &rows, mode, row_where ? &wheres[w] : nullptr, nullptr,
+                                  p == WAX_VS_NO_FILTER ? nullptr : &rows, mode, row_where ? &req.wheres[w] : nullptr, nullptr,
                                   nullptr, nullptr, nullptr, keys.data())))
                 return rc;
             std::vector<wax_vs_group_candidate> recs(slots, wax_vs_group_candidate{});
@@ -5072,11 +5087,11 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
         }
         const size_t o = static_cast<size_t>(qi) * out_stride;
         if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group,
-                              p == WAX_VS_NO_FILTER ? nullptr : &rows, mode, row_where ? &wheres[w] : nullptr, out_ids + o,
+                              p == WAX_VS_NO_FILTER ? nullptr : &rows, mode, row_where ? &req.wheres[w] : nullptr, out_ids + o,
                               out_scores + o, out_groups + o, out_n + qi)))
             return rc;
     }
-    if (!batched) return WAX_VS_OK;
+    if (!req.batched) return WAX_VS_OK;
     std::lock_guard<std::mutex> pg(e->pool_mu);
     e->grouped_batch_covered_queries += covered;
     e->grouped_batch_expanded_groups += expanded;
@@ -5085,35 +5100,33 @@ static int32_t search_grouped_host(wax_vs_engine *e, const float *queries, uint3
     return WAX_VS_OK;
 }
 
-// The one-filter grouped entry points: one id filter (an empty deny-list is none) and at most one where for every query.
-static int32_t search_grouped_one_filter(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                         int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
+// The grouped entry points after their argument checks: on one engine, or across the shards of a multi-device handle,
+// which first zeroes out_n as one engine does.
+static int32_t search_grouped(wax_vs_engine *e, const SearchRequest &req, uint64_t *out_ids, float *out_scores,
+                              uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n) {
+    if (!e->multi) return search_grouped_host(e, req, req.queries, out_ids, out_scores, out_groups, out_stride, out_n);
+    for (uint32_t i = 0; i < req.n_queries; ++i) out_n[i] = 0;
+    return multi_search_grouped(e->multi, e->dims, e->similarity, req, out_ids, out_scores, out_groups, out_stride, out_n);
+}
+
+// The one-filter grouped entry points, after their where (if any) went into req: the outputs, the grouped arguments,
+// one id filter (an empty deny-list is none) and at most one where for every query.
+static int32_t search_grouped_one_filter(wax_vs_engine *e, SearchRequest &req, const uint64_t *frame_ids, uint64_t n_ids,
                                          int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
-                                         uint32_t out_stride, uint32_t *out_n, bool batched, const Clause *where = nullptr) {
+                                         uint32_t out_stride, uint32_t *out_n) {
+    if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
     int32_t rc;
-    if ((rc = check_grouped_args(e, top_groups, per_group, out_ids, out_scores, out_groups, out_n))) return rc;
-    if (mode != 0 && mode != 1) return fail(WAX_VS_ERR_ARGUMENT, "filter mode must be 0 (allow-list) or 1 (deny-list)");
-    if (n_ids && !frame_ids) return fail(WAX_VS_ERR_NULL, "frame_ids is NULL");
-    const uint64_t offsets[2] = {0, n_ids};
-    const std::vector<uint32_t> query_filter(n_queries, mode == 1 && n_ids == 0 ? WAX_VS_NO_FILTER : 0u);
-    const std::vector<uint32_t> query_where(n_queries, where ? 0u : WAX_VS_NO_FILTER);
-    std::vector<Clause> wheres;
-    if (where) wheres.push_back(*where);
-    return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, offsets, &mode, 1,
-                               query_filter.data(), wheres, query_where.data(), out_ids, out_scores, out_groups, out_stride,
-                               out_n, batched);
+    if ((rc = check_grouped_args(req)) || (rc = request_one_filter(req, frame_ids, n_ids, mode, true))) return rc;
+    request_one_where(req);
+    return search_grouped(e, req, out_ids, out_scores, out_groups, out_stride, out_n);
 }
 
 int32_t wax_vs_search_grouped(wax_vs_engine *e, const float *query, uint32_t query_len, int64_t top_groups,
                               uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
                               uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_cap,
                               uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_grouped(e->multi->probe, query, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids, out_scores, out_groups, out_cap, out_n)) return rc;
-        return multi_search_grouped_one(e, query, 1, query_len, top_groups, per_group, frame_ids, n_ids, mode, nullptr, nullptr, out_ids, out_scores, out_groups, out_cap, out_n);
-    }
-    return search_grouped_one_filter(e, query, 1, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids,
-                                     out_scores, out_groups, out_cap, out_n, false);
+    SearchRequest req(query, 1, query_len, top_groups, per_group, false);
+    return search_grouped_one_filter(e, req, frame_ids, n_ids, mode, out_ids, out_scores, out_groups, out_cap, out_n);
 }
 
 // A batch of one stays a batch.
@@ -5121,26 +5134,18 @@ int32_t wax_vs_search_batch_grouped(wax_vs_engine *e, const float *queries, uint
                                     int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
                                     int32_t mode, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
                                     uint32_t out_stride, uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_batch_grouped(e->multi->probe, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, out_ids, out_scores, out_groups, out_stride, out_n)) return rc;
-        return multi_search_grouped_one(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, nullptr, nullptr, out_ids, out_scores, out_groups, out_stride, out_n);
-    }
-    return search_grouped_one_filter(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode,
-                                     out_ids, out_scores, out_groups, out_stride, out_n, true);
+    SearchRequest req(queries, n_queries, query_len, top_groups, per_group, true);
+    return search_grouped_one_filter(e, req, frame_ids, n_ids, mode, out_ids, out_scores, out_groups, out_stride, out_n);
 }
 
 int32_t wax_vs_search_batch_grouped_where(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
                                           int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
                                           int32_t mode, const wax_vs_where *where, uint64_t *out_ids, float *out_scores,
                                           uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_batch_grouped_where(e->multi->probe, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, where, out_ids, out_scores, out_groups, out_stride, out_n)) return rc;
-        return multi_search_grouped_one(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, where, nullptr, out_ids, out_scores, out_groups, out_stride, out_n);
-    }
     if (!where) return fail(WAX_VS_ERR_NULL, "where is NULL");
-    const Clause clause{where_pred(*where), kNoLocBox, {}};
-    return search_grouped_one_filter(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode,
-                                     out_ids, out_scores, out_groups, out_stride, out_n, n_queries > 1, &clause);
+    SearchRequest req(queries, n_queries, query_len, top_groups, per_group, n_queries > 1);
+    request_plain_clauses(req, where, 1);
+    return search_grouped_one_filter(e, req, frame_ids, n_ids, mode, out_ids, out_scores, out_groups, out_stride, out_n);
 }
 
 int32_t wax_vs_search_batch_grouped_where_near(wax_vs_engine *e, const float *queries, uint32_t n_queries,
@@ -5148,16 +5153,11 @@ int32_t wax_vs_search_batch_grouped_where_near(wax_vs_engine *e, const float *qu
                                                const uint64_t *frame_ids, uint64_t n_ids, int32_t mode,
                                                const wax_vs_where_near *where, uint64_t *out_ids, float *out_scores,
                                                uint64_t *out_groups, uint32_t out_stride, uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_batch_grouped_where_near(e->multi->probe, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, where, out_ids, out_scores, out_groups, out_stride, out_n)) return rc;
-        return multi_search_grouped_one(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode, nullptr, where, out_ids, out_scores, out_groups, out_stride, out_n);
-    }
     if (!where) return fail(WAX_VS_ERR_NULL, "where is NULL");
-    std::vector<Clause> clause;
-    int32_t rc;
-    if ((rc = near_clauses(where, 1, clause))) return rc;
-    return search_grouped_one_filter(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, n_ids, mode,
-                                     out_ids, out_scores, out_groups, out_stride, out_n, n_queries > 1, &clause[0]);
+    SearchRequest req(queries, n_queries, query_len, top_groups, per_group, n_queries > 1);
+    const int32_t rc = near_clauses(where, 1, req.wheres);
+    return rc ? rc
+              : search_grouped_one_filter(e, req, frame_ids, n_ids, mode, out_ids, out_scores, out_groups, out_stride, out_n);
 }
 
 int32_t wax_vs_search_batch_grouped_multi_where(wax_vs_engine *e, const float *queries, uint32_t n_queries,
@@ -5168,61 +5168,44 @@ int32_t wax_vs_search_batch_grouped_multi_where(wax_vs_engine *e, const float *q
                                                 uint32_t n_wheres, const uint32_t *query_where, uint64_t *out_ids,
                                                 float *out_scores, uint64_t *out_groups, uint32_t out_stride,
                                                 uint32_t *out_n) {
-    if (e && e->multi) {   // the probe engine's argument checks, then the multi-device form
-        if (const int32_t rc = wax_vs_search_batch_grouped_multi_where(e->multi->probe, queries, n_queries, query_len, top_groups, per_group, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_groups, out_stride, out_n)) return rc;
-        return multi_search_grouped(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_groups, per_group, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, out_ids, out_scores, out_groups, out_stride, out_n);
-    }
+    if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(queries, n_queries, query_len, top_groups, per_group, n_queries > 1);
     int32_t rc;
-    if ((rc = check_grouped_args(e, top_groups, per_group, out_ids, out_scores, out_groups, out_n)) ||
-        (rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
-                               n_wheres, query_where, out_n)))
+    if ((rc = check_grouped_args(req)) ||
+        (rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
+        (rc = request_where_list(req, wheres, n_wheres, query_where)) || (rc = near_clauses(wheres, n_wheres, req.wheres)))
         return rc;
-    std::vector<Clause> clauses;
-    if ((rc = near_clauses(wheres, n_wheres, clauses))) return rc;
-    return search_grouped_host(e, queries, n_queries, query_len, top_groups, per_group, frame_ids, filter_offsets,
-                               filter_modes, n_filters, query_filter, clauses, query_where, out_ids, out_scores, out_groups,
-                               out_stride, out_n, n_queries > 1);
+    return search_grouped(e, req, out_ids, out_scores, out_groups, out_stride, out_n);
 }
 
 // ---- sharded grouped search (waxvs_group_batch.cuh, waxvs_shard.cuh) ------------------------------------------------
-// The checks of the sharded grouped entry points: those of wax_vs_search_batch_grouped_multi_where and the cap on the
-// groups, before the engine is locked, so every rank fails alike before any exchange.  Builds the clauses.
-static int32_t check_shard_grouped_args(wax_vs_engine *e, const float *d_queries, uint32_t n_queries, int64_t top_groups,
-                                        uint32_t per_group, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                        const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                        const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
-                                        const void *d_out, std::vector<Clause> &clauses) {
-    uint64_t no_ids = 0;                    // the checks of the host forms, which also test their outputs
-    float no_scores = 0.0f;
-    uint32_t no_n = 0;
+// The checks of the sharded grouped entry points: those of wax_vs_search_batch_grouped_multi_where but the host outputs,
+// then the cap on the groups, before the engine is locked, so every rank fails alike before any exchange; then the
+// device pointers.  Builds the clauses.
+static int32_t request_shard_grouped(SearchRequest &req, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                     const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                     const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                     const float *d_queries, const void *d_out) {
     int32_t rc;
-    if ((rc = check_grouped_args(e, top_groups, per_group, &no_ids, &no_scores, &no_ids, &no_n)) ||
-        (rc = check_where_args(e, n_queries, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
-                               n_wheres, query_where, &no_n)))
+    if ((rc = check_grouped_args(req)) ||
+        (rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
+        (rc = request_where_list(req, wheres, n_wheres, query_where)))
         return rc;
-    if (clamp_topk(top_groups) > WAX_VS_SHARD_MAX_GROUPS)
+    if (clamp_topk(req.top_k) > WAX_VS_SHARD_MAX_GROUPS)
         return fail(WAX_VS_ERR_UNSUPPORTED, "sharded grouped search takes clamp(top_groups) <= %d (got %u)",
-                    WAX_VS_SHARD_MAX_GROUPS, clamp_topk(top_groups));
+                    WAX_VS_SHARD_MAX_GROUPS, clamp_topk(req.top_k));
     if (!d_queries || !d_out) return fail(WAX_VS_ERR_NULL, "NULL argument");
-    return near_clauses(wheres, n_wheres, clauses);
+    return near_clauses(wheres, n_wheres, req.wheres);
 }
 
-// Round 1: this shard's wax_vs_search_batch_grouped_multi_where, delivered as records on the device (ShardHeads).  The
-// queries come to the host once, as the host form takes them.
-int32_t wax_vs_shard_grouped_heads_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries, int64_t top_groups,
-                                          uint32_t per_group, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                          const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                          const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
-                                          uint64_t row_offset, wax_vs_group_candidate *d_heads, void *cuda_stream) {
-    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_grouped_heads_device");
-    std::vector<Clause> clauses;
-    int32_t rc;
-    if ((rc = check_shard_grouped_args(e, d_queries, n_queries, top_groups, per_group, frame_ids, filter_offsets,
-                                       filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, d_heads,
-                                       clauses)))
-        return rc;
+// Round 1 (wax_vs_shard_grouped_heads_device, and each shard of a multi-device handle): this shard's
+// search_grouped_host, delivered as records on the device (ShardHeads).  The queries come to the host once, as the host
+// form takes them.
+static int32_t grouped_heads_device(wax_vs_engine *e, const SearchRequest &req, const float *d_queries, uint64_t row_offset,
+                                    wax_vs_group_candidate *d_heads, void *cuda_stream) {
+    const uint32_t n_queries = req.n_queries;
     if (n_queries == 0) return WAX_VS_OK;
-    const size_t slots = static_cast<size_t>(clamp_topk(top_groups)) * per_group;
+    const size_t slots = static_cast<size_t>(clamp_topk(req.top_k)) * req.per_group;
     std::vector<float> queries(static_cast<size_t>(n_queries) * e->dims);
     {
         DeviceGuard g(e->device);
@@ -5234,9 +5217,20 @@ int32_t wax_vs_shard_grouped_heads_device(wax_vs_engine *e, const float *d_queri
     }
     std::vector<uint32_t> no_n(n_queries);
     const ShardHeads heads{row_offset, d_heads};
-    return search_grouped_host(e, queries.data(), n_queries, e->dims, top_groups, per_group, frame_ids, filter_offsets,
-                               filter_modes, n_filters, query_filter, clauses, query_where, nullptr, nullptr, nullptr, 0,
-                               no_n.data(), n_queries > 1, &heads);
+    return search_grouped_host(e, req, queries.data(), nullptr, nullptr, nullptr, 0, no_n.data(), &heads);
+}
+
+int32_t wax_vs_shard_grouped_heads_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries, int64_t top_groups,
+                                          uint32_t per_group, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                          const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                          const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                          uint64_t row_offset, wax_vs_group_candidate *d_heads, void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_grouped_heads_device");
+    if (!e) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(nullptr, n_queries, e->dims, top_groups, per_group, n_queries > 1);
+    const int32_t rc = request_shard_grouped(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
+                                             n_wheres, query_where, d_queries, d_heads);
+    return rc ? rc : grouped_heads_device(e, req, d_queries, row_offset, d_heads, cuda_stream);
 }
 
 // Merge 1 (merge_group_heads_kernel): stateless, enqueued on the caller's stream.
@@ -5268,33 +5262,22 @@ int32_t wax_vs_merge_group_heads_device(wax_vs_engine *e, const wax_vs_group_can
     return WAX_VS_OK;
 }
 
-// Round 2 on the caller's stream: the lookup kernel copies the groups this rank listed and lists the ones it must score;
-// those run as the batched grouped search's expansions (expand_in_passes) under each query's (where, id filter) pair,
-// and their keys become records.
-int32_t wax_vs_shard_grouped_expand_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries,
-                                           int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids,
-                                           const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
-                                           const uint32_t *query_filter, const wax_vs_where_near *wheres,
-                                           uint32_t n_wheres, const uint32_t *query_where,
-                                           const wax_vs_group_candidate *d_chosen,
-                                           const wax_vs_group_candidate *d_own_heads, uint64_t row_offset,
-                                           wax_vs_candidate *d_rows, void *cuda_stream) {
-    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_grouped_expand_device");
-    std::vector<Clause> clauses;
-    int32_t rc;
-    if ((rc = check_shard_grouped_args(e, d_queries, n_queries, top_groups, per_group, frame_ids, filter_offsets,
-                                       filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, d_rows,
-                                       clauses)))
-        return rc;
-    if (!d_chosen || !d_own_heads) return fail(WAX_VS_ERR_NULL, "NULL argument");
+// Round 2 on the caller's stream (wax_vs_shard_grouped_expand_device, and each shard of a multi-device handle): the
+// lookup kernel copies the groups this rank listed and lists the ones it must score; those run as the batched grouped
+// search's expansions (expand_in_passes) under each query's (where, id filter) pair, and their keys become records.
+static int32_t grouped_expand_device(wax_vs_engine *e, const SearchRequest &req, const float *d_queries,
+                                     const wax_vs_group_candidate *d_chosen, const wax_vs_group_candidate *d_own_heads,
+                                     uint64_t row_offset, wax_vs_candidate *d_rows, void *cuda_stream) {
+    const uint32_t n_queries = req.n_queries, per_group = req.per_group;
     if (n_queries == 0) return WAX_VS_OK;
     std::shared_lock<std::shared_mutex> r(e->rw);
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
     SearchCtx *c = nullptr;
+    int32_t rc;
     if ((rc = ctx_for_stream(e, cuda_stream, &c))) return rc;
     const cudaStream_t s = c->stream;
-    const uint32_t n_top = clamp_topk(top_groups);
+    const uint32_t n_top = clamp_topk(req.top_k);
     const size_t n_slots = static_cast<size_t>(n_queries) * n_top;
     e->async_pending.store(true);
     CUDA_TRY(cudaMemsetAsync(d_rows, 0, n_slots * per_group * sizeof(wax_vs_candidate), s));
@@ -5318,20 +5301,15 @@ int32_t wax_vs_shard_grouped_expand_device(wax_vs_engine *e, const float *d_quer
     uint64_t launches = 1, passes = 0;
     CUDA_TRY(cudaMemcpyAsync(c->h_bg_expand, c->d_bg_expand, n_exp * sizeof(CoverExpand), cudaMemcpyDeviceToHost, s));
     // the call's (where, id filter) pairs, their rows staged as run_filtered stages them, the queries in caller order
-    FilterSet ids, fs;
-    resolve_filters(e, frame_ids, filter_offsets, n_filters, query_filter, n_queries, ids);
-    std::vector<int32_t> modes;
-    std::vector<uint32_t> pair_of;
-    if ((rc = plan_where_pairs(e, c, clauses, query_where, filter_modes, query_filter, n_queries, ids, fs, modes, pair_of)) ||
-        (rc = stage_pair_rows(e, c, fs, &launches)))
-        return rc;
+    WherePlan wp;
+    if ((rc = plan_request(e, c, req, req.top_k, wp, false)) || (rc = stage_pair_rows(e, c, wp.fs, &launches))) return rc;
     const size_t qfloats = static_cast<size_t>(n_queries) * e->dims;
     if ((rc = c->d_queries.ensure(qfloats, "query buffer")) ||
         (rc = c->d_bg_keys.ensure(n_slots * per_group, "grouped batch keys")))
         return rc;
     CUDA_TRY(cudaMemcpyAsync(c->d_queries, d_queries, qfloats * sizeof(float), cudaMemcpyDeviceToDevice, s));
     CUDA_TRY(cudaStreamSynchronize(s));              // the expansion list is on the host
-    if ((rc = expand_in_passes(e, c, c->h_bg_expand, n_exp, pair_of, modes.data(), fs, n_top, per_group, &launches, &passes)))
+    if ((rc = expand_in_passes(e, c, c->h_bg_expand, n_exp, wp.pair_of, wp, n_top, per_group, &launches, &passes)))
         return rc;
     ShardRowInfo ri{row_offset, e->id_base, nullptr, device_row_keys(e), gi.row_group, gi.ids};
     if ((rc = sync_device_ids(e, &ri.ids))) return rc;
@@ -5341,6 +5319,24 @@ int32_t wax_vs_shard_grouped_expand_device(wax_vs_engine *e, const float *d_quer
     std::lock_guard<std::mutex> pg(e->pool_mu);
     e->shard_grouped_expanded_groups += n_exp;
     return WAX_VS_OK;
+}
+
+int32_t wax_vs_shard_grouped_expand_device(wax_vs_engine *e, const float *d_queries, uint32_t n_queries,
+                                           int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids,
+                                           const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                           const uint32_t *query_filter, const wax_vs_where_near *wheres,
+                                           uint32_t n_wheres, const uint32_t *query_where,
+                                           const wax_vs_group_candidate *d_chosen,
+                                           const wax_vs_group_candidate *d_own_heads, uint64_t row_offset,
+                                           wax_vs_candidate *d_rows, void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_shard_grouped_expand_device");
+    if (!e) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(nullptr, n_queries, e->dims, top_groups, per_group, n_queries > 1);
+    const int32_t rc = request_shard_grouped(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter, wheres,
+                                             n_wheres, query_where, d_queries, d_rows);
+    if (rc) return rc;
+    if (!d_chosen || !d_own_heads) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    return grouped_expand_device(e, req, d_queries, d_chosen, d_own_heads, row_offset, d_rows, cuda_stream);
 }
 
 // ---- persistence ---------------------------------------------------------------------------------------------

@@ -16,8 +16,10 @@
 //     synchronise (the batched levels, the mutators).  Each concurrent caller leases its own per-shard streams and
 //     buffers (MultiCtx), as CtxLease does for one engine.
 //
-// Included by waxvs_engine.cu after its helpers; each served public entry dispatches here in its first line, and every
-// other entry refuses a multi-device handle (multi_refuse).
+// Included by waxvs_engine.cu after its helpers.  Each served public entry dispatches here in its first line, but the
+// filtered, where and grouped ones, which first check their arguments and build their request (SearchRequest) exactly as
+// one engine does, then reach here through search_where / search_grouped.  Every other entry refuses a multi-device
+// handle (multi_refuse).
 #pragma once
 #include <condition_variable>
 #include <deque>
@@ -90,8 +92,6 @@ struct MultiCtx {
 struct MultiEngine {
     std::vector<int> devices;
     std::vector<wax_vs_engine *> shards;
-    wax_vs_engine *probe = nullptr;                // an empty engine on devices[0]: runs the argument checks of the
-                                                   // filtered, where and grouped entries exactly as one engine does
     std::vector<uint64_t> rows;                    // rows per shard
     uint64_t next_key = 0;                         // the first unused row key
     std::shared_mutex rw;                          // readers: searches / serialize; writer: mutators
@@ -184,7 +184,6 @@ static void multi_destroy(MultiEngine *m) {
     }
     for (MultiCtx *c : m->pool) delete c;
     for (wax_vs_engine *s : m->shards) wax_vs_destroy(s);
-    wax_vs_destroy(m->probe);
     delete m;
 }
 
@@ -222,9 +221,6 @@ static int32_t multi_create(uint32_t dims, uint8_t similarity, const int32_t *de
     h->device = devices[0]; h->dims = dims; h->similarity = similarity; h->multi = m;
     m->devices.assign(devices, devices + n);
     m->rows.assign(n, 0);
-    if (const int32_t rc = wax_vs_create(dims, similarity, devices, 1, &m->probe)) {
-        multi_destroy(m); h->multi = nullptr; delete h; return rc;
-    }
     for (int32_t r = 0; r < n; ++r) {
         wax_vs_engine *s = nullptr;
         const int32_t rc = wax_vs_create(dims, similarity, devices + r, 1, &s);
@@ -637,32 +633,27 @@ static int32_t multi_search(MultiEngine *m, uint32_t dims, uint8_t similarity, c
     return WAX_VS_OK;
 }
 
-// The filtered, where, where_near and where_terms forms, after the probe engine ran their argument checks (which also
-// zeroed out_n): every live shard plans its rows with wax_vs_search_batch_where_device and the lists merge as above.
-// One engine's buffer check needs max_i min(clamp(k), rows query i allows); the merged lists hold min(clamp(k), allowed
-// rows with a finite distance) valid entries per query, the same number whenever the allowed rows are finite.
-static int32_t multi_search_where(MultiEngine *m, uint32_t dims, uint8_t similarity, const float *queries, uint32_t n_queries,
-                                  uint32_t query_len, int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                  const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                  const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
-                                  const uint64_t *where_term_offsets, const uint64_t *where_terms, uint64_t *out_ids,
-                                  float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+// The filtered and where entry points, after their argument checks (search_where zeroed out_n): every live shard plans
+// its rows for the request (search_where_device) and the lists merge as above.  One engine's buffer check needs
+// max_i min(clamp(k), rows query i allows); the merged lists hold min(clamp(k), allowed rows with a finite distance)
+// valid entries per query, the same number whenever the allowed rows are finite.
+static int32_t multi_search_where(MultiEngine *m, uint32_t dims, uint8_t similarity, const SearchRequest &req,
+                                  uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    const uint32_t n_queries = req.n_queries;
     std::shared_lock<std::shared_mutex> r_lock(m->rw);
     if (m->total() == 0 || n_queries == 0) return WAX_VS_OK;
     int32_t rc;
-    if ((rc = multi_check_query(dims, queries, query_len))) return rc;
-    const uint32_t k = clamp_topk(top_k);
+    if ((rc = multi_check_query(dims, req.queries, req.query_len))) return rc;
+    const uint32_t k = clamp_topk(req.top_k);
     MultiLease lease(m);
     if ((rc = lease.acquire())) return rc;
     MultiCtx *c = lease.c;
     const std::vector<int> live = multi_live(m);
-    rc = multi_fan_out(m, c, live, queries, n_queries, dims, true, [&](int r, const float *dq, cudaStream_t s) -> int32_t {
+    rc = multi_fan_out(m, c, live, req.queries, n_queries, dims, true, [&](int r, const float *dq, cudaStream_t s) -> int32_t {
         MultiCtx::Part &p = c->part[r];
         int32_t prc;
         if ((prc = p.d_cands.ensure(static_cast<size_t>(n_queries) * k, "shard candidates"))) return prc;
-        return wax_vs_search_batch_where_device(m->shards[r], dq, n_queries, k, frame_ids, filter_offsets, filter_modes,
-                                                n_filters, query_filter, wheres, n_wheres, query_where, where_term_offsets,
-                                                where_terms, 0, p.d_cands, s);
+        return search_where_device(m->shards[r], req, dq, 0, p.d_cands, s);
     });
     if (rc) return rc;
     DeviceGuard g(c->part[0].device);
@@ -682,31 +673,14 @@ static int32_t multi_search_where(MultiEngine *m, uint32_t dims, uint8_t similar
     return WAX_VS_OK;
 }
 
-// The entry points' arguments in the form of wax_vs_search_batch_where_device / the grouped rounds: one filter for every
-// query, no where or one where for every query, a plain where as a where_near without a location clause.
-struct MultiClauses {
-    uint64_t offsets[2] = {0, 0};
-    std::vector<uint32_t> query_filter, query_where;
-    wax_vs_where_near near{};
-    void one_filter(uint64_t n_ids, uint32_t n_queries) { offsets[1] = n_ids; query_filter.assign(n_queries, 0u); }
-    void wheres(const wax_vs_where *w, const wax_vs_where_near *wn, uint32_t n_queries) {
-        query_where.assign(n_queries, w || wn ? 0u : WAX_VS_NO_FILTER);
-        if (w) near = wax_vs_where_near{*w, 0.0, 0.0, 0.0};
-        if (wn) near = *wn;
-    }
-};
-
 // Grouped search, the protocol of the sharded grouped form (DESIGN.md section 4.14) with the shards' buffers read in place
-// on device 0: round 1 (wax_vs_shard_grouped_heads_device) on every live shard, merge 1 (merge_group_heads_kernel over
-// PeerLists) on device 0; with per_group > 1 round 2 (wax_vs_shard_grouped_expand_device, reading d_chosen on device 0)
-// and the per-(query, group) merge of the rows.  After the probe engine ran the argument checks.
-static int32_t multi_search_grouped(MultiEngine *m, uint32_t dims, uint8_t similarity, const float *queries, uint32_t n_queries,
-                                    uint32_t query_len, int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids,
-                                    const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
-                                    const uint32_t *query_filter, const wax_vs_where_near *wheres, uint32_t n_wheres,
-                                    const uint32_t *query_where, uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
-                                    uint32_t out_stride, uint32_t *out_n) {
-    const uint32_t G = clamp_topk(top_groups), P = per_group;
+// on device 0: round 1 (grouped_heads_device) on every live shard, merge 1 (merge_group_heads_kernel over PeerLists) on
+// device 0; with per_group > 1 round 2 (grouped_expand_device, reading d_chosen on device 0) and the per-(query, group)
+// merge of the rows.  After the argument checks (search_grouped zeroed out_n).
+static int32_t multi_search_grouped(MultiEngine *m, uint32_t dims, uint8_t similarity, const SearchRequest &req,
+                                    uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_stride,
+                                    uint32_t *out_n) {
+    const uint32_t n_queries = req.n_queries, G = clamp_topk(req.top_k), P = req.per_group;
     if (G > WAX_VS_SHARD_MAX_GROUPS)
         return fail(WAX_VS_ERR_UNSUPPORTED, "sharded grouped search takes clamp(top_groups) <= %d (got %u)",
                     WAX_VS_SHARD_MAX_GROUPS, G);
@@ -714,7 +688,7 @@ static int32_t multi_search_grouped(MultiEngine *m, uint32_t dims, uint8_t simil
     const uint64_t total = m->total();
     if (total == 0 || n_queries == 0) return WAX_VS_OK;
     int32_t rc;
-    if ((rc = multi_check_query(dims, queries, query_len))) return rc;
+    if ((rc = multi_check_query(dims, req.queries, req.query_len))) return rc;
     const uint32_t need = static_cast<uint32_t>(std::min<uint64_t>(static_cast<uint64_t>(G) * P, total));
     if (out_stride < need) return fail(WAX_VS_ERR_BUFFER, "output buffers hold %u entries, need %u", out_stride, need);
     MultiLease lease(m);
@@ -722,13 +696,11 @@ static int32_t multi_search_grouped(MultiEngine *m, uint32_t dims, uint8_t simil
     MultiCtx *c = lease.c;
     const std::vector<int> live = multi_live(m);
     const size_t slots = static_cast<size_t>(n_queries) * G * P;
-    rc = multi_fan_out(m, c, live, queries, n_queries, dims, true, [&](int r, const float *dq, cudaStream_t s) -> int32_t {
+    rc = multi_fan_out(m, c, live, req.queries, n_queries, dims, true, [&](int r, const float *dq, cudaStream_t s) -> int32_t {
         MultiCtx::Part &p = c->part[r];
         int32_t prc;
         if ((prc = p.d_heads.ensure(slots, "group heads"))) return prc;
-        return wax_vs_shard_grouped_heads_device(m->shards[r], dq, n_queries, top_groups, P, frame_ids, filter_offsets,
-                                                 filter_modes, n_filters, query_filter, wheres, n_wheres, query_where, 0,
-                                                 p.d_heads, s);
+        return grouped_heads_device(m->shards[r], req, dq, 0, p.d_heads, s);
     });
     if (rc) return rc;
     MultiCtx::Part &p0 = c->part[0];
@@ -758,10 +730,7 @@ static int32_t multi_search_grouped(MultiEngine *m, uint32_t dims, uint8_t simil
             int32_t prc;
             if ((prc = p.d_cands.ensure(slots, "group rows"))) return prc;
             CUDA_TRY(cudaStreamWaitEvent(p.stream, c->chosen, 0));
-            if ((prc = wax_vs_shard_grouped_expand_device(m->shards[r], p.d_queries, n_queries, top_groups, P, frame_ids,
-                                                          filter_offsets, filter_modes, n_filters, query_filter, wheres,
-                                                          n_wheres, query_where, c->d_chosen, p.d_heads, 0, p.d_cands,
-                                                          p.stream)))
+            if ((prc = grouped_expand_device(m->shards[r], req, p.d_queries, c->d_chosen, p.d_heads, 0, p.d_cands, p.stream)))
                 return prc;
             CUDA_TRY(cudaEventRecord(p.done, p.stream));
             return WAX_VS_OK;
@@ -841,50 +810,4 @@ static int32_t multi_counter(MultiEngine *m, const char *name, uint64_t *out) {
     }
     *out = sum;
     return WAX_VS_OK;
-}
-
-// ---- the public entries' multi-device forms: the probe engine's argument checks, then the forms above ----------------
-static int32_t multi_search_filtered(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                     int64_t top_k, const uint64_t *frame_ids, uint64_t n_ids, int32_t mode, uint64_t *out_ids,
-                                     float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    MultiClauses a;
-    a.one_filter(n_ids, n_queries);
-    a.wheres(nullptr, nullptr, n_queries);
-    return multi_search_where(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_k, frame_ids, a.offsets, &mode, 1,
-                              a.query_filter.data(), nullptr, 0, a.query_where.data(), nullptr, nullptr, out_ids, out_scores,
-                              out_stride, out_n);
-}
-static int32_t multi_search_multi_filtered(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                           int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                           const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                           uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    MultiClauses a;
-    a.wheres(nullptr, nullptr, n_queries);
-    return multi_search_where(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_k, frame_ids, filter_offsets,
-                              filter_modes, n_filters, query_filter, nullptr, 0, a.query_where.data(), nullptr, nullptr,
-                              out_ids, out_scores, out_stride, out_n);
-}
-static int32_t multi_search_batch_where(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                        int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
-                                        const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
-                                        const wax_vs_where *wheres, uint32_t n_wheres, const uint32_t *query_where,
-                                        uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
-    std::vector<wax_vs_where_near> near(n_wheres);
-    for (uint32_t w = 0; w < n_wheres; ++w) near[w] = wax_vs_where_near{wheres[w], 0.0, 0.0, 0.0};   // no location clause
-    return multi_search_where(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_k, frame_ids, filter_offsets,
-                              filter_modes, n_filters, query_filter, near.data(), n_wheres, query_where, nullptr, nullptr,
-                              out_ids, out_scores, out_stride, out_n);
-}
-// One filter and at most one where for the whole batch (search_grouped, _batch_grouped, _grouped_where, _where_near).
-static int32_t multi_search_grouped_one(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
-                                        int64_t top_groups, uint32_t per_group, const uint64_t *frame_ids, uint64_t n_ids,
-                                        int32_t mode, const wax_vs_where *where, const wax_vs_where_near *where_near,
-                                        uint64_t *out_ids, float *out_scores, uint64_t *out_groups, uint32_t out_stride,
-                                        uint32_t *out_n) {
-    MultiClauses a;
-    a.one_filter(n_ids, n_queries);
-    a.wheres(where, where_near, n_queries);
-    return multi_search_grouped(e->multi, e->dims, e->similarity, queries, n_queries, query_len, top_groups, per_group,
-                                frame_ids, a.offsets, &mode, 1, a.query_filter.data(), &a.near, where || where_near ? 1 : 0,
-                                a.query_where.data(), out_ids, out_scores, out_groups, out_stride, out_n);
 }
