@@ -80,7 +80,7 @@ int32_t wax_vs_device_count(int32_t *out);
    _search_batch_where, _where_near, _where_terms, _set_groups, _search_grouped, _search_batch_grouped, _grouped_where,
    _grouped_where_near, _grouped_multi_where, _serialized_length, _serialize, _deserialize, wax_vs_debug_set_option
    (applied to every shard) and wax_vs_debug_counter (summed over the shards, plus "shard_rows.<r>": shard r's rows);
-   every other entry point (the rank-level shard_*, *_device, keyed and merge entries, the other debug_*) returns
+   every other entry point (the rank-level shard_*, *_device, keyed, export, absorb and merge entries, the other debug_*) returns
    WAX_VS_ERR_UNSUPPORTED naming itself.  Grouped search with clamp(top_groups) > WAX_VS_SHARD_MAX_GROUPS is refused as
    the sharded grouped form refuses it.  An ordinal
    may repeat ({0, 0, 0}): the shards then share that device, a test and debug configuration.  Checked before any
@@ -160,6 +160,59 @@ int32_t wax_vs_deserialize_rows(wax_vs_engine *engine, const uint8_t *src, uint6
    may be NULL.  A range outside the rows -> WAX_VS_ERR_ARGUMENT. */
 int32_t wax_vs_export_rows(wax_vs_engine *engine, uint64_t first, uint64_t n, uint64_t *out_ids, float *out_vectors,
                            uint64_t *out_keys);
+
+/* The rank-level halves of a rebalance of the multi-process engine (ShardedVectorEngine.rebalance, DESIGN.md section
+   4.15): a donor exports a run of its rows with their side columns, the receiver merges them by key.  The donor then
+   drops the rows with wax_vs_remove_batch of their ids. */
+/* Copy the vectors of rows [first, first + n) device-to-device into d_out (n x dims fp32 on the engine's device),
+   enqueued on cuda_stream (NULL = the legacy default stream): NCCL can send them from there without a host bounce.  A
+   later mutator of the engine waits for the copy.  A range outside the rows -> WAX_VS_ERR_ARGUMENT (as
+   wax_vs_export_rows); n == 0 is a no-op; d_out NULL -> WAX_VS_ERR_NULL. */
+int32_t wax_vs_export_rows_device(wax_vs_engine *engine, uint64_t first, uint64_t n, float *d_out, void *cuda_stream);
+
+/* One row's side columns (32 bytes): its group, its attributes and its location bins (lat_bin == WAX_VS_NO_LOCATION:
+   none, lon_bin 0). */
+typedef struct wax_vs_row_columns {
+    uint64_t group;
+    int64_t timestamp;
+    uint64_t tags;
+    int32_t lat_bin;
+    int32_t lon_bin;
+} wax_vs_row_columns;
+#define WAX_VS_NO_LOCATION (-2147483647 - 1)
+/* Bits of the columns an engine holds (set_groups, set_attributes, set_locations, set_terms have been called). */
+#define WAX_VS_COLUMN_GROUPS 1u
+#define WAX_VS_COLUMN_ATTRIBUTES 2u
+#define WAX_VS_COLUMN_LOCATIONS 4u
+#define WAX_VS_COLUMN_TERMS 8u
+
+/* The side columns of rows [first, first + n): out_columns[n] each row's group, attributes and location; the term
+   lists as out_term_offsets[n + 1] (from 0) into out_terms; *out_terms_len = the number of term ids in the rows (call
+   with out_terms NULL to size the buffer first); *out_set = the WAX_VS_COLUMN_* bits of the columns this engine holds.
+   A column the engine does not hold is exported as the defaults its rows answer with: group = own frame id,
+   attributes {0, 0}, no location, no terms.  Every output may be NULL.  Ids and keys come from wax_vs_export_rows.
+   A range outside the rows -> WAX_VS_ERR_ARGUMENT (as wax_vs_export_rows); out_terms with terms_cap below the term
+   ids -> WAX_VS_ERR_BUFFER. */
+int32_t wax_vs_export_columns(wax_vs_engine *engine, uint64_t first, uint64_t n, wax_vs_row_columns *out_columns,
+                              uint64_t *out_term_offsets, uint64_t *out_terms, uint64_t terms_cap, uint64_t *out_terms_len,
+                              uint32_t *out_set);
+
+/* Merge n rows into the engine by key: frame_ids[n], keys[n] (strictly increasing), d_vectors (n x dims fp32 on the
+   engine's device, complete when the call is made) and the side columns as wax_vs_export_columns gives them:
+   columns_set = the WAX_VS_COLUMN_* bits the source held, columns[n] (needed with the group, attribute or location
+   bit), term_offsets[n + 1] and terms (needed with the terms bit).  Every answer afterwards is that of an engine whose
+   rows, in key order, are its own and the incoming ones.  A column set on one side only is filled with the defaults
+   the other side's rows answered with; term lists are appended to the engine's term pool.  The merge works in slabs of
+   the option "rebalance_slab_bytes" written top-down, so it rewrites the rows above the first incoming key; every
+   allocation comes before a row changes (a failed one -> WAX_VS_ERR_CUDA, the engine untouched).  The row caches from
+   the first incoming key on are rebuilt by the next search that needs them.  Checked before anything changes, ->
+   WAX_VS_ERR_ARGUMENT with a reason: keys that do not strictly increase, a key or a frame id the engine already holds,
+   a frame id given twice, an engine that holds rows without keys, unknown column bits, term offsets that decrease or
+   a row's terms that do not strictly increase, d_vectors not device memory on the engine's device.  NULL pointers ->
+   WAX_VS_ERR_NULL.  n == 0 is a no-op. */
+int32_t wax_vs_absorb_rows(wax_vs_engine *engine, const uint64_t *frame_ids, const uint64_t *keys, const float *d_vectors,
+                           uint64_t n, uint32_t columns_set, const wax_vs_row_columns *columns,
+                           const uint64_t *term_offsets, const uint64_t *terms);
 
 /* ---- search ------------------------------------------------------------------------------------- */
 

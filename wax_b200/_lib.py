@@ -23,6 +23,9 @@ MAX_PER_GROUP = 128             # WAX_VS_MAX_PER_GROUP: rows per group of wax_vs
 SHARD_HANDLE_BYTES, SHARD_MAX_RANKS, SHARD_MAX_K = 128, 16, 128
 SHARD_MAX_GROUPS = 256          # WAX_VS_SHARD_MAX_GROUPS: clamp(top_groups) of the sharded grouped search
 INT64_MIN, INT64_MAX = -(1 << 63), (1 << 63) - 1   # wax_vs_where bounds meaning "no bound"
+NO_LOCATION = -(1 << 31)        # WAX_VS_NO_LOCATION: the lat_bin of a row without a location
+# WAX_VS_COLUMN_*: the side columns an engine holds (wax_vs_export_columns / wax_vs_absorb_rows)
+COLUMN_GROUPS, COLUMN_ATTRIBUTES, COLUMN_LOCATIONS, COLUMN_TERMS = 1, 2, 4, 8
 
 
 class Candidate(C.Structure):
@@ -62,6 +65,9 @@ SIGNATURES = {
     "wax_vs_contains": (C.c_int32, [_eng, _u64p, C.c_uint64, _u8p]),
     "wax_vs_deserialize_rows": (C.c_int32, [_eng, _u8p, C.c_uint64, C.c_uint64, C.c_uint64]),
     "wax_vs_export_rows": (C.c_int32, [_eng, C.c_uint64, C.c_uint64, _u64p, _f32p, _u64p]),
+    "wax_vs_export_rows_device": (C.c_int32, [_eng, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "wax_vs_export_columns": (C.c_int32, [_eng, C.c_uint64, C.c_uint64, C.c_void_p, _u64p, _u64p, C.c_uint64, _u64p, _u32p]),
+    "wax_vs_absorb_rows": (C.c_int32, [_eng, _u64p, _u64p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, _u64p, _u64p]),
     "wax_vs_search": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_int64, _u64p, _f32p, C.c_uint32, _u32p]),
     "wax_vs_search_filtered": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_int64, _u64p, C.c_uint64, C.c_int32, _u64p, _f32p,
                                            C.c_uint32, _u32p]),

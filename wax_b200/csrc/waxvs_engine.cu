@@ -2426,34 +2426,78 @@ int32_t wax_vs_remove(wax_vs_engine *e, uint64_t frame_id) {
     return wax_vs_remove_batch(e, &frame_id, 1, nullptr);
 }
 
-// The receiving half of a rebalance move (multi_rebalance, DESIGN.md section 4.16): rows [first, first + n) of `donor`, a
-// run of increasing keys, merge into `e` by key together with their ids, keys, groups, attributes, locations and terms.
-// Every allocation (the receiver's growth, the bounce buffer, the staging, the key column) comes before a row changes,
-// so a failed allocation leaves `e` as it was.  Destination slabs are written top-down: own rows only move up and
-// incoming rows only move down, so a slab's sources lie in it or below it, and each slab is gathered into the bounce
-// buffer (merge_rows_kernel) before it is copied in place, as the compaction of remove_batch does.  The incoming rows of
-// one slab are one contiguous run of the donor's, staged on the receiver's device with cudaMemcpyPeerAsync (a
-// device-local copy when the two share a device): no kernel reads peer memory.  The donor is only read; the caller
-// drops the rows from it afterwards.
-static int32_t absorb_rows(wax_vs_engine *e, wax_vs_engine *donor, uint64_t first, uint64_t n) {
-    if (n == 0) return WAX_VS_OK;
+// The source of a rebalance merge (absorb_body): n rows in strictly increasing key order, their vectors (n x dims fp32 on
+// device()) and their side columns.  set() is the WAX_VS_COLUMN_* bits of the columns the source holds; a column it does
+// not hold is answered with the defaults its rows have (group = own frame id, attributes {0, 0}, no location, no terms).
+static_assert(sizeof(wax_vs_row_columns) == 32 && WAX_VS_NO_LOCATION == kNoLocation, "wax_vs_row_columns layout");
+struct TermList {
+    const uint64_t *p;
+    uint32_t n;
+};
+// Rows [first, first + n) of another engine of this process (multi_rebalance), read under its read lock.
+struct DonorRows {
+    const wax_vs_engine *d;
+    uint64_t first, n;
+    const float *vectors() const { return d->d_corpus + first * d->dims; }
+    int device() const { return d->device; }
+    uint32_t set() const {
+        return (d->groups_set ? WAX_VS_COLUMN_GROUPS : 0u) | (d->attrs_set ? WAX_VS_COLUMN_ATTRIBUTES : 0u) |
+               (d->locs_set ? WAX_VS_COLUMN_LOCATIONS : 0u) | (d->terms_set ? WAX_VS_COLUMN_TERMS : 0u);
+    }
+    uint64_t key(uint64_t j) const { return d->keys[first + j]; }
+    uint64_t id(uint64_t j) const { return frame_id_of(d, first + j); }
+    uint64_t group(uint64_t j) const { return d->groups[first + j]; }
+    AttrRow attr(uint64_t j) const { return d->attrs[first + j]; }
+    LocRow loc(uint64_t j) const { return d->locs[first + j]; }
+    TermList terms(uint64_t j) const {
+        const wax_vs_engine::TermRef t = d->term_refs[first + j];
+        return TermList{d->term_pool.data() + t.off, t.n};
+    }
+};
+// Rows the caller hands over (wax_vs_absorb_rows), already checked.
+struct CallerRows {
+    const uint64_t *ids, *keys_;
+    const float *vecs;
+    int dev;
+    uint64_t n;
+    uint32_t columns_set;
+    const wax_vs_row_columns *cols;
+    const uint64_t *term_offsets, *term_ids;
+    const float *vectors() const { return vecs; }
+    int device() const { return dev; }
+    uint32_t set() const { return columns_set; }
+    uint64_t key(uint64_t j) const { return keys_[j]; }
+    uint64_t id(uint64_t j) const { return ids[j]; }
+    uint64_t group(uint64_t j) const { return cols[j].group; }
+    AttrRow attr(uint64_t j) const { return AttrRow{cols[j].timestamp, cols[j].tags}; }
+    LocRow loc(uint64_t j) const { return LocRow{cols[j].lat_bin, cols[j].lon_bin}; }
+    TermList terms(uint64_t j) const {
+        return TermList{term_ids + term_offsets[j], static_cast<uint32_t>(term_offsets[j + 1] - term_offsets[j])};
+    }
+};
+
+// The receiving half of a rebalance move (DESIGN.md sections 4.15 and 4.16): the rows of `in` merge into `e` by key
+// together with their ids, keys, groups, attributes, locations and terms.  The write lock of `e` is held and the rows
+// are checked.  Every allocation (the receiver's growth, the bounce buffer, the staging, the key column) comes before a
+// row changes, so a failed allocation leaves `e` as it was.  Destination slabs are written top-down: own rows only move
+// up and incoming rows only move down, so a slab's sources lie in it or below it, and each slab is gathered into the
+// bounce buffer (merge_rows_kernel) before it is copied in place, as the compaction of remove_batch does.  The incoming
+// rows of one slab are one contiguous run of the source's, staged on the receiver's device with cudaMemcpyPeerAsync (a
+// device-local copy when the two share a device): no kernel reads peer memory.  The source is only read.
+extern "C++" {                                 // the merge body is a template over its source
+template <class Src>
+static int32_t absorb_body(wax_vs_engine *e, const Src &in) {
     IngestTrace tr("rebalance merge");
-    std::unique_lock<std::shared_mutex> w(e->rw);
-    std::shared_lock<std::shared_mutex> donor_lock(donor->rw);
-    if (!donor->keys_set || first + n > donor->n_rows || (!e->keys_set && e->n_rows))
-        return fail(WAX_VS_ERR_ARGUMENT, "rebalance: rows [%llu, +%llu) of a keyed shard expected",
-                    static_cast<unsigned long long>(first), static_cast<unsigned long long>(n));
     DeviceGuard g(e->device);
     if (!g.ok) return g.error();
     drain_device_path(e);
-    const uint64_t n0 = e->n_rows, m = n0 + n;
-    const uint64_t *in_keys = donor->keys.data() + first;
+    const uint64_t n = in.n, n0 = e->n_rows, m = n0 + n;
     // rows below the first incoming key keep their place; every destination row from f on has a tagged source
-    const uint64_t f = static_cast<uint64_t>(std::lower_bound(e->keys.begin(), e->keys.end(), in_keys[0]) - e->keys.begin());
+    const uint64_t f = static_cast<uint64_t>(std::lower_bound(e->keys.begin(), e->keys.end(), in.key(0)) - e->keys.begin());
     const uint64_t total = m - f;
     std::vector<uint64_t> src(total);
     for (uint64_t t = 0, i = f, j = 0; t < total; ++t)
-        src[t] = j < n && (i == n0 || in_keys[j] < e->keys[i]) ? (kMergeIncoming | j++) : i++;
+        src[t] = j < n && (i == n0 || in.key(j) < e->keys[i]) ? (kMergeIncoming | j++) : i++;
     tr.mark("lock+drain+merge positions");
 
     int32_t rc;
@@ -2482,7 +2526,7 @@ static int32_t absorb_rows(wax_vs_engine *e, wax_vs_engine *donor, uint64_t firs
         for (const uint64_t t : tags)
             if (t & kMergeIncoming) { jlo = std::min(jlo, t & ~kMergeIncoming); jhi = std::max(jhi, (t & ~kMergeIncoming) + 1); }
         if (jhi > jlo) {
-            CUDA_TRY(cudaMemcpyPeerAsync(incoming, e->device, donor->d_corpus + (first + jlo) * donor->dims, donor->device,
+            CUDA_TRY(cudaMemcpyPeerAsync(incoming, e->device, in.vectors() + jlo * e->dims, in.device(),
                                          (jhi - jlo) * row_bytes, ig.stream));
             for (uint64_t &t : tags) if (t & kMergeIncoming) t -= jlo;
         }
@@ -2503,26 +2547,32 @@ static int32_t absorb_rows(wax_vs_engine *e, wax_vs_engine *donor, uint64_t firs
     auto merge = [&](auto &col, auto incoming_of) {
         auto tail = std::vector<typename std::decay_t<decltype(col)>::value_type>(total);
         for (uint64_t t = 0; t < total; ++t)
-            tail[t] = (src[t] & kMergeIncoming) ? incoming_of(first + (src[t] & ~kMergeIncoming)) : col[src[t]];
+            tail[t] = (src[t] & kMergeIncoming) ? incoming_of(src[t] & ~kMergeIncoming) : col[src[t]];
         col.resize(f);
         col.insert(col.end(), tail.begin(), tail.end());
     };
-    if ((e->groups_set || donor->groups_set) && !e->groups_set) { e->groups = e->ids; e->groups_set = true; }
-    if (donor->attrs_set && !e->attrs_set) { e->attrs.assign(n0, AttrRow{0, 0}); e->attrs_set = true; }
-    if (donor->locs_set && !e->locs_set) { e->locs.assign(n0, LocRow{kNoLocation, 0}); e->locs_set = true; }
-    if (donor->terms_set && !e->terms_set) { e->term_refs.assign(n0, wax_vs_engine::TermRef{0, 0}); e->terms_set = true; }
-    merge(e->ids, [&](uint64_t r) { return frame_id_of(donor, r); });
-    merge(e->keys, [&](uint64_t r) { return donor->keys[r]; });
+    const uint32_t set = in.set();
+    if ((set & WAX_VS_COLUMN_GROUPS) && !e->groups_set) { e->groups = e->ids; e->groups_set = true; }
+    if ((set & WAX_VS_COLUMN_ATTRIBUTES) && !e->attrs_set) { e->attrs.assign(n0, AttrRow{0, 0}); e->attrs_set = true; }
+    if ((set & WAX_VS_COLUMN_LOCATIONS) && !e->locs_set) { e->locs.assign(n0, LocRow{kNoLocation, 0}); e->locs_set = true; }
+    if ((set & WAX_VS_COLUMN_TERMS) && !e->terms_set) {
+        e->term_refs.assign(n0, wax_vs_engine::TermRef{0, 0});
+        e->terms_set = true;
+    }
+    merge(e->ids, [&](uint64_t j) { return in.id(j); });
+    merge(e->keys, [&](uint64_t j) { return in.key(j); });
     e->keys_set = true;
-    if (e->groups_set) merge(e->groups, [&](uint64_t r) { return donor->groups_set ? donor->groups[r] : frame_id_of(donor, r); });
-    if (e->attrs_set) merge(e->attrs, [&](uint64_t r) { return donor->attrs_set ? donor->attrs[r] : AttrRow{0, 0}; });
-    if (e->locs_set) merge(e->locs, [&](uint64_t r) { return donor->locs_set ? donor->locs[r] : LocRow{kNoLocation, 0}; });
+    if (e->groups_set) merge(e->groups, [&](uint64_t j) { return (set & WAX_VS_COLUMN_GROUPS) ? in.group(j) : in.id(j); });
+    if (e->attrs_set) merge(e->attrs, [&](uint64_t j) { return (set & WAX_VS_COLUMN_ATTRIBUTES) ? in.attr(j) : AttrRow{0, 0}; });
+    if (e->locs_set)
+        merge(e->locs, [&](uint64_t j) { return (set & WAX_VS_COLUMN_LOCATIONS) ? in.loc(j) : LocRow{kNoLocation, 0}; });
     if (e->terms_set)
-        merge(e->term_refs, [&](uint64_t r) {
-            if (!donor->terms_set || donor->term_refs[r].n == 0) return wax_vs_engine::TermRef{0, 0};
-            const wax_vs_engine::TermRef t = donor->term_refs[r];
+        merge(e->term_refs, [&](uint64_t j) {
+            if (!(set & WAX_VS_COLUMN_TERMS)) return wax_vs_engine::TermRef{0, 0};
+            const TermList t = in.terms(j);
+            if (t.n == 0) return wax_vs_engine::TermRef{0, 0};
             const uint64_t off = e->term_pool.size();
-            e->term_pool.insert(e->term_pool.end(), donor->term_pool.begin() + t.off, donor->term_pool.begin() + t.off + t.n);
+            e->term_pool.insert(e->term_pool.end(), t.p, t.p + t.n);
             return wax_vs_engine::TermRef{off, t.n};
         });
     e->n_rows = m;
@@ -2533,6 +2583,73 @@ static int32_t absorb_rows(wax_vs_engine *e, wax_vs_engine *donor, uint64_t firs
     rc = upload_row_keys(e, keys_from);
     tr.mark("merge columns");
     return rc;
+}
+}  // extern "C++"
+
+// Rows [first, first + n) of `donor`, another engine of this process, merge into `e` (multi_rebalance).  The donor is
+// only read; the caller drops the rows from it afterwards.
+static int32_t absorb_rows(wax_vs_engine *e, wax_vs_engine *donor, uint64_t first, uint64_t n) {
+    if (n == 0) return WAX_VS_OK;
+    std::unique_lock<std::shared_mutex> w(e->rw);
+    std::shared_lock<std::shared_mutex> donor_lock(donor->rw);
+    if (!donor->keys_set || first + n > donor->n_rows || (!e->keys_set && e->n_rows))
+        return fail(WAX_VS_ERR_ARGUMENT, "rebalance: rows [%llu, +%llu) of a keyed shard expected",
+                    static_cast<unsigned long long>(first), static_cast<unsigned long long>(n));
+    return absorb_body(e, DonorRows{donor, first, n});
+}
+
+int32_t wax_vs_absorb_rows(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *keys, const float *d_vectors,
+                           uint64_t n, uint32_t columns_set, const wax_vs_row_columns *columns,
+                           const uint64_t *term_offsets, const uint64_t *terms) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_absorb_rows");
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    if (n == 0) return WAX_VS_OK;
+    if (!frame_ids || !keys || !d_vectors) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    const uint32_t all = WAX_VS_COLUMN_GROUPS | WAX_VS_COLUMN_ATTRIBUTES | WAX_VS_COLUMN_LOCATIONS | WAX_VS_COLUMN_TERMS;
+    if (columns_set & ~all) return fail(WAX_VS_ERR_ARGUMENT, "absorb_rows: unknown column bits 0x%x", columns_set & ~all);
+    if ((columns_set & (WAX_VS_COLUMN_GROUPS | WAX_VS_COLUMN_ATTRIBUTES | WAX_VS_COLUMN_LOCATIONS)) && !columns)
+        return fail(WAX_VS_ERR_NULL, "columns is NULL");
+    if ((columns_set & WAX_VS_COLUMN_TERMS) && !term_offsets) return fail(WAX_VS_ERR_NULL, "term_offsets is NULL");
+    if ((columns_set & WAX_VS_COLUMN_TERMS) && term_offsets[n] && !terms) return fail(WAX_VS_ERR_NULL, "terms is NULL");
+    for (uint64_t j = 1; j < n; ++j)
+        if (keys[j] <= keys[j - 1])
+            return fail(WAX_VS_ERR_ARGUMENT, "absorb_rows: keys must strictly increase (row %llu)",
+                        static_cast<unsigned long long>(j));
+    if (columns_set & WAX_VS_COLUMN_TERMS) {
+        if (term_offsets[0] != 0) return fail(WAX_VS_ERR_ARGUMENT, "absorb_rows: term_offsets[0] must be 0");
+        for (uint64_t j = 0; j < n; ++j) {
+            if (term_offsets[j + 1] < term_offsets[j] || term_offsets[j + 1] - term_offsets[j] > 0xFFFFFFFFull)
+                return fail(WAX_VS_ERR_ARGUMENT, "absorb_rows: term_offsets must not decrease (row %llu)",
+                            static_cast<unsigned long long>(j));
+            for (uint64_t t = term_offsets[j] + 1; t < term_offsets[j + 1]; ++t)
+                if (terms[t] <= terms[t - 1])
+                    return fail(WAX_VS_ERR_ARGUMENT, "absorb_rows: row %llu's terms must strictly increase",
+                                static_cast<unsigned long long>(j));
+        }
+    }
+    {
+        std::vector<uint64_t> sorted(frame_ids, frame_ids + n);
+        std::sort(sorted.begin(), sorted.end());
+        const auto dup = std::adjacent_find(sorted.begin(), sorted.end());
+        if (dup != sorted.end())
+            return fail(WAX_VS_ERR_ARGUMENT, "absorb_rows: frame %llu appears twice", static_cast<unsigned long long>(*dup));
+    }
+    cudaPointerAttributes attr{};
+    if (cudaPointerGetAttributes(&attr, d_vectors) != cudaSuccess || attr.type != cudaMemoryTypeDevice ||
+        attr.device != e->device) {
+        cudaGetLastError();
+        return fail(WAX_VS_ERR_ARGUMENT, "absorb_rows: d_vectors is not memory on the engine's device %d", e->device);
+    }
+    std::unique_lock<std::shared_mutex> w(e->rw);
+    if (!e->keys_set && e->n_rows) return fail(WAX_VS_ERR_ARGUMENT, "absorb_rows: the engine holds rows without keys");
+    for (uint64_t j = 0; j < n; ++j)
+        if (std::binary_search(e->keys.begin(), e->keys.end(), keys[j]))
+            return fail(WAX_VS_ERR_ARGUMENT, "absorb_rows: key %llu is already held", static_cast<unsigned long long>(keys[j]));
+    for (uint64_t j = 0; j < n; ++j)
+        if (row_of(e, frame_ids[j]) != 0xFFFFFFFFu)
+            return fail(WAX_VS_ERR_ARGUMENT, "absorb_rows: frame %llu is already held",
+                        static_cast<unsigned long long>(frame_ids[j]));
+    return absorb_body(e, CallerRows{frame_ids, keys, d_vectors, e->device, n, columns_set, columns, term_offsets, terms});
 }
 
 int32_t wax_vs_rebalance(wax_vs_engine *e, uint64_t *out_moved) {
@@ -5476,6 +5593,55 @@ int32_t wax_vs_export_rows(wax_vs_engine *e, uint64_t first, uint64_t n, uint64_
         std::lock_guard<std::mutex> ig(e->ingest_mu);             // one exporter at a time (as serialize)
         return download_bytes(e, out_vectors, e->d_corpus + first * e->dims, n * e->dims * sizeof(float));
     }
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_export_rows_device(wax_vs_engine *e, uint64_t first, uint64_t n, float *d_out, void *cuda_stream) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_export_rows_device");
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
+    if (n == 0) return WAX_VS_OK;
+    if (!d_out) return fail(WAX_VS_ERR_NULL, "d_out is NULL");
+    DeviceGuard g(e->device);
+    if (!g.ok) return g.error();
+    e->async_pending.store(true);              // a mutator drains the copy before it moves a row
+    CUDA_TRY(cudaMemcpyAsync(d_out, e->d_corpus + first * e->dims, n * e->dims * sizeof(float), cudaMemcpyDeviceToDevice,
+                             static_cast<cudaStream_t>(cuda_stream)));
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_export_columns(wax_vs_engine *e, uint64_t first, uint64_t n, wax_vs_row_columns *out_columns,
+                              uint64_t *out_term_offsets, uint64_t *out_terms, uint64_t terms_cap, uint64_t *out_terms_len,
+                              uint32_t *out_set) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_export_columns");
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    std::shared_lock<std::shared_mutex> r(e->rw);
+    if (first > e->n_rows || n > e->n_rows - first) return fail(WAX_VS_ERR_ARGUMENT, "row range out of bounds");
+    uint64_t len = 0;
+    if (e->terms_set)
+        for (uint64_t i = first; i < first + n; ++i) len += e->term_refs[i].n;
+    if (out_terms && terms_cap < len)
+        return fail(WAX_VS_ERR_BUFFER, "terms_cap %llu < %llu term ids in the rows", static_cast<unsigned long long>(terms_cap),
+                    static_cast<unsigned long long>(len));
+    if (out_terms_len) *out_terms_len = len;
+    if (out_set)
+        *out_set = (e->groups_set ? WAX_VS_COLUMN_GROUPS : 0u) | (e->attrs_set ? WAX_VS_COLUMN_ATTRIBUTES : 0u) |
+                   (e->locs_set ? WAX_VS_COLUMN_LOCATIONS : 0u) | (e->terms_set ? WAX_VS_COLUMN_TERMS : 0u);
+    uint64_t pos = 0;
+    for (uint64_t j = 0; j < n; ++j) {
+        const uint64_t row = first + j;
+        if (out_columns) {
+            const AttrRow a = e->attrs_set ? e->attrs[row] : AttrRow{0, 0};
+            const LocRow l = e->locs_set ? e->locs[row] : LocRow{kNoLocation, 0};
+            out_columns[j] = wax_vs_row_columns{e->groups_set ? e->groups[row] : frame_id_of(e, row), a.ts, a.tags, l.lat, l.lon};
+        }
+        const wax_vs_engine::TermRef t = e->terms_set ? e->term_refs[row] : wax_vs_engine::TermRef{0, 0};
+        if (out_term_offsets) out_term_offsets[j] = pos;
+        if (out_terms && t.n) memcpy(out_terms + pos, e->term_pool.data() + t.off, t.n * sizeof(uint64_t));
+        pos += t.n;
+    }
+    if (out_term_offsets) out_term_offsets[n] = pos;
     return WAX_VS_OK;
 }
 

@@ -19,7 +19,7 @@ import ctypes as C
 import dataclasses
 import enum
 import threading
-from typing import Iterable, List, Optional, Sequence, Tuple
+from typing import Iterable, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -257,6 +257,20 @@ class _WhereArgs:
                 self.tflat.ctypes.data_as(C.POINTER(C.c_uint64)) if self.tflat.size else None)
 
 
+# wax_vs_row_columns: one row's group, attributes and location bins, as wax_vs_export_columns / wax_vs_absorb_rows take them
+ROW_COLUMNS_DTYPE = np.dtype([("group", "<u8"), ("timestamp", "<i8"), ("tags", "<u8"), ("lat_bin", "<i4"), ("lon_bin", "<i4")])
+assert ROW_COLUMNS_DTYPE.itemsize == 32
+
+
+class RowColumns(NamedTuple):
+    """The side columns of a run of rows (CUDAVectorEngine.export_columns): `set` = the L.COLUMN_* bits of the columns the
+    engine holds, `records` [n] ROW_COLUMNS_DTYPE, the term lists as `term_offsets` [n + 1] (from 0) into `terms`."""
+    set: int
+    records: np.ndarray
+    term_offsets: np.ndarray
+    terms: np.ndarray
+
+
 def _clamp_topk(top_k: int) -> int:
     """clampTopK (MetalVectorEngine.swift:842-846)."""
     return max(1, min(int(top_k), L.MAX_RESULTS))
@@ -302,6 +316,7 @@ class CUDAVectorEngine:
             raise ValueError("pass at most one of device= / devices=")
         self.metric = metric
         self.dimensions = int(dimensions)
+        self._device = device if device is not None else (devices[0] if devices else None)
         self._dirty = False
         self._h = C.c_void_p()
         if device is not None:
@@ -856,6 +871,55 @@ class CUDAVectorEngine:
                                           vecs.ctypes.data_as(C.POINTER(C.c_float)) if vectors else None,
                                           keys.ctypes.data_as(C.POINTER(C.c_uint64))))
         return ids, vecs, keys
+
+    def export_vectors(self, first: int, n: int):
+        """Rows [first, first + n)'s vectors as a new [n, dims] float32 torch tensor on the engine's device, copied device
+        to device on that device's current stream (wax_vs_export_rows_device)."""
+        import torch
+        dev = torch.device("cuda", torch.cuda.current_device() if self._device is None else self._device)
+        out = torch.empty((int(n), self.dimensions), dtype=torch.float32, device=dev)
+        _check(L.lib().wax_vs_export_rows_device(self._h, int(first), int(n), C.c_void_p(out.data_ptr()),
+                                                 C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        return out
+
+    def export_columns(self, first: int, n: int) -> RowColumns:
+        """The side columns of rows [first, first + n) (wax_vs_export_columns): a column the engine does not hold comes
+        as the defaults its rows answer with (group = own frame id, attributes 0, no location, no terms)."""
+        records = np.empty(int(n), ROW_COLUMNS_DTYPE)
+        offsets = np.empty(int(n) + 1, np.uint64)
+        length, bits = C.c_uint64(0), C.c_uint32(0)
+        _check(L.lib().wax_vs_export_columns(self._h, int(first), int(n), None, None, None, 0, C.byref(length), None))
+        terms = np.empty(length.value, np.uint64)
+        _check(L.lib().wax_vs_export_columns(self._h, int(first), int(n), records.ctypes.data_as(C.c_void_p),
+                                             offsets.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                             terms.ctypes.data_as(C.POINTER(C.c_uint64)), terms.size, C.byref(length),
+                                             C.byref(bits)))
+        return RowColumns(bits.value, records, offsets, terms)
+
+    def absorb_rows(self, frame_ids: Sequence[int], keys: Sequence[int], vectors, columns: Optional[RowColumns] = None) -> None:
+        """Merge rows into this engine by key (wax_vs_absorb_rows): frame ids, keys (strictly increasing), `vectors` a
+        [n, dims] float32 torch tensor on the engine's device, and the side columns export_columns gave (None: the source
+        held none).  The current stream of that device is synchronised first, so the vectors are complete."""
+        import torch
+        ids = np.ascontiguousarray(frame_ids, dtype=np.uint64).reshape(-1)
+        ks = np.ascontiguousarray(keys, dtype=np.uint64).reshape(-1)
+        if ids.size != ks.size or tuple(vectors.shape) != (ids.size, self.dimensions) or vectors.dtype != torch.float32:
+            raise ValueError(f"absorb_rows: {ids.size} ids, {ks.size} keys and vectors of shape {tuple(vectors.shape)} "
+                             f"({vectors.dtype})")
+        vecs = vectors.contiguous()
+        if vecs.is_cuda:
+            torch.cuda.current_stream(vecs.device).synchronize()
+        bits = 0 if columns is None else int(columns.set)
+        recs = None if columns is None else np.ascontiguousarray(columns.records, ROW_COLUMNS_DTYPE)
+        offs = None if columns is None else np.ascontiguousarray(columns.term_offsets, np.uint64)
+        terms = None if columns is None else np.ascontiguousarray(columns.terms, np.uint64)
+        _check(L.lib().wax_vs_absorb_rows(
+            self._h, ids.ctypes.data_as(C.POINTER(C.c_uint64)), ks.ctypes.data_as(C.POINTER(C.c_uint64)),
+            C.c_void_p(vecs.data_ptr()), ids.size, bits, recs.ctypes.data_as(C.c_void_p) if recs is not None else None,
+            offs.ctypes.data_as(C.POINTER(C.c_uint64)) if offs is not None else None,
+            terms.ctypes.data_as(C.POINTER(C.c_uint64)) if terms is not None and terms.size else None))
+        if ids.size:
+            self._dirty = True
 
     def row_keys(self) -> np.ndarray:
         """Every row's key, in row order (the row itself on an engine without keys)."""

@@ -182,7 +182,8 @@ class ShardedVectorEngine:
     Two ways to hold a corpus: `total_rows` > 0 with fill_synthetic (contiguous row ranges), or an empty engine filled by
     the collective corpus methods (add_batch, remove_batch, deserialize, ...; DESIGN.md section 4.15), which place rows
     on any rank and key them by insertion order.  local_store: optional stand-in for the rank's engine in those methods
-    (the CPU tests); it needs count, contains, add_batch_keyed, remove_batch, deserialize_rows and export_rows.
+    (the CPU tests); it needs count, contains, add_batch_keyed, remove_batch, deserialize_rows and export_rows, and for
+    rebalance export_vectors, export_columns and absorb_rows.
     """
 
     def __init__(self, metric, dimensions: int, total_rows: int = 0, group=None,
@@ -414,6 +415,108 @@ class ShardedVectorEngine:
                     place(pos[r][first:first + n_r], np.ascontiguousarray(got[r, :n_r, :8]).view(np.uint64).reshape(-1),
                           np.ascontiguousarray(got[r, :n_r, 8:8 + 4 * dims]).view(np.float32))
         return out if root else None
+
+    def rebalance(self, chunk_rows: Optional[int] = None) -> int:
+        """Even out the ranks' rows in place (collective, no arguments needed): every rank ends with the row count
+        plan_rebalance gives it, each moved row taking its key, group, attributes, location and terms with it, so every
+        answer, serialize() included, stays that of one engine with the same history.  Returns the rows moved, the same
+        on every rank.
+
+        One all-reduce of the ranks' row counts confirms the bookkeeping; a balanced corpus stops there.  Then, move by
+        move in plan order, the donor sends the next part of its tail (in key order) to the receiver point to point, in
+        chunks of at most `chunk_rows` rows (default: 256 MiB of vectors): a header, one fixed-width record per row (id,
+        key, group, attributes, location, term count), the vectors (a device tensor under NCCL, host memory under gloo)
+        and the term ids.  The receiver merges each chunk by key (absorb_rows), which rewrites its rows above the chunk's
+        first key; its extra device memory is one chunk plus the merge's slab buffers.  One all-reduce of the rows each
+        move delivered follows; each donor drops those rows.  A receiver that fails keeps what it merged before and
+        absorbs nothing more, the rest stays on the donors, and every rank raises the same error with the failing
+        rank's reason."""
+        self._check_corpus_methods()
+        torch, dist = self._torch, self._dist
+        from .engine import InvalidToc, ROW_COLUMNS_DTYPE, RowColumns
+        counts = self._sum_on_ranks(np.eye(self.world_size, dtype=np.int64)[self.rank] * self.engine.count)
+        if not np.array_equal(counts, self._counts):
+            raise InvalidToc(f"rebalance: the ranks hold {counts.tolist()} rows, the bookkeeping says {self._counts.tolist()}")
+        _, moves = plan_rebalance(counts)
+        if not moves:
+            return 0
+        dims = self.dimensions
+        chunk = max(1, int(chunk_rows) if chunk_rows else (256 << 20) // (4 * dims))
+        wire = self.device if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
+        rec = np.dtype([("id", "<u8"), ("key", "<u8"), ("cols", ROW_COLUMNS_DTYPE), ("n_terms", "<u8")])
+        tail = counts.copy()                                       # tail[d]: where donor d's next run starts
+        for d, _, rows in moves:
+            tail[d] -= rows
+        first = []
+        for d, _, rows in moves:
+            first.append(int(tail[d]))
+            tail[d] += rows
+        done = np.zeros(len(moves) + self.world_size, np.int64)    # rows each move delivered, then a failure flag per rank
+        failure = None
+        for i, (d, r, rows) in enumerate(moves):
+            if self.rank not in (d, r):
+                continue
+            for lo in range(0, rows, chunk):
+                m = min(chunk, rows - lo)
+                if self.rank == d:
+                    row = first[i] + lo
+                    ids, _, keys = self.engine.export_rows(row, m, vectors=False)
+                    cols = self.engine.export_columns(row, m)
+                    records = np.zeros(m, rec)
+                    records["id"], records["key"], records["cols"] = ids, keys, cols.records
+                    records["n_terms"] = np.diff(cols.term_offsets)
+                    head = np.array([cols.set, cols.terms.size], np.int64)
+                    dist.send(torch.from_numpy(head).to(wire), r, group=self.group)
+                    dist.send(torch.from_numpy(records.view(np.uint8).reshape(-1)).to(wire), r, group=self.group)
+                    dist.send(self.engine.export_vectors(row, m).to(wire), r, group=self.group)
+                    if cols.terms.size:
+                        dist.send(torch.from_numpy(cols.terms.view(np.int64)).to(wire), r, group=self.group)
+                    continue
+                head = torch.empty(2, dtype=torch.int64, device=wire)
+                dist.recv(head, d, group=self.group)
+                bits, n_terms = (int(x) for x in head.cpu())
+                raw = torch.empty(m * rec.itemsize, dtype=torch.uint8, device=wire)
+                dist.recv(raw, d, group=self.group)
+                vecs = torch.empty((m, dims), dtype=torch.float32, device=wire)
+                dist.recv(vecs, d, group=self.group)
+                terms = torch.empty(n_terms, dtype=torch.int64, device=wire)
+                if n_terms:
+                    dist.recv(terms, d, group=self.group)
+                if failure is not None:                            # drained, not merged: the rows stay on the donor
+                    continue
+                records = raw.cpu().numpy().view(rec)
+                offsets = np.zeros(m + 1, np.uint64)
+                offsets[1:] = np.cumsum(records["n_terms"])
+                try:
+                    self.engine.absorb_rows(records["id"], records["key"], vecs.to(self.device),
+                                            RowColumns(bits, records["cols"], offsets, terms.cpu().numpy().view(np.uint64)))
+                    done[i] += m
+                except Exception as exc:                           # noqa: BLE001 -- every rank re-raises it below
+                    failure = exc
+        if failure is not None:
+            done[len(moves) + self.rank] = 1
+        done = self._sum_on_ranks(done)
+        drop = []
+        for i, (d, r, rows) in enumerate(moves):
+            n_done = int(done[i])
+            if self.rank == d and n_done:
+                drop.append(self.engine.export_rows(first[i], n_done, vectors=False)[0])
+            counts[d] -= n_done
+            counts[r] += n_done
+        if drop:
+            self.engine.remove_batch(np.concatenate(drop))
+        self._set_counts(counts)
+        failed = np.flatnonzero(done[len(moves):])
+        if failed.size:
+            src = int(failed[0])
+            why = [(type(failure).__name__, str(failure)) if self.rank == src else None]
+            dist.broadcast_object_list(why, src=src if self.group is None else dist.get_global_rank(self.group, src),
+                                       group=self.group)
+            from . import engine as E
+            cls = getattr(E, why[0][0], None)
+            cls = cls if isinstance(cls, type) and issubclass(cls, E.WaxError) else RuntimeError
+            raise cls(f"rebalance: rank {src} could not absorb its rows: {why[0][1]}")
+        return int(done[:len(moves)].sum())
 
     # -- search
     def _buffers(self, k: int, slot: int = 0):
