@@ -72,8 +72,10 @@ constexpr int kBatchThreads = 160;
 constexpr float kTf32Eps = 1.25f * 0x1p-9f;
 // BF16 nominations: both operands are ROUNDED to nearest; bf16 keeps 8 significand bits (7 stored), so the unit
 // round-off is 2^-8: |x~ - x| <= 2^-8 |x| each, |q~ v~ - q v| <= (2^-7 + 2^-16) |q v| termwise, hence
-// |err| <= (2^-7 + 2^-16) sum |q_i v_i| <= (2^-7 + 2^-16) |q||v|; the fp32 accumulation adds O(dims * 2^-24) and the
-// pre-normalisation of the cosine shadow rows O(2^-23).  1.03 * 2^-7 covers all of it.
+// |err| <= (2^-7 + 2^-16) sum |q_i v_i| <= (2^-7 + 2^-16) |q||v|, and the pre-normalisation of the cosine shadow rows
+// adds O(2^-23).  1.03 * 2^-7 covers those two, not the fp32 accumulation: its spare (1.03 - 1 - 2^-9) 2^-7 ~ 2^-12.2
+// is below dims * 2^-24 beyond about 3 700 dims.  The proofs budget the accumulation on its own, as
+// acc_slack = dims 2^-23 |q||v| in batch_finish_kernel (and (n + 1) 2^-23 in l2_nomination_bound), for TF32 and bf16.
 constexpr float kBf16Eps = 1.03f * 0x1p-7f;
 
 struct BatchParams {

@@ -1279,7 +1279,7 @@ static bool batch_tensor_eligible(const wax_vs_engine *e, uint32_t n_queries, ui
     return e->tune.batch_tensor && n_queries >= min_batch &&
            (e->similarity == WAX_VS_COSINE || e->similarity == WAX_VS_DOT || (e->similarity == WAX_VS_L2 && e->tune.batch_l2)) &&
            e->dims % kBatchKBlock == 0 &&
-           e->dims <= 8192 &&        // the proof's accumulation slack (dims * 2^-23) stays far below the operand bound
+           e->dims <= 8192 &&        // the proof's accumulation slack (dims * 2^-23) stays below the operand bound
            k_eff >= 1 && e->n_rows >= 1 &&
            // 128 < k <= 1024 (the production candidate limit reaches 1 000, UnifiedSearch.swift:1195-1200): real batches
            // only.  Level 1 can rarely PROVE such a k (64 nominees per slice barely cover it) but its exactly re-scored
