@@ -741,6 +741,15 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *engine, uint64_t *tensor_queries
    "single_u4_queries", "u4_shadow_bytes" / "u4_shadow_rows" (the same for the 4-bit shadow). */
 int32_t wax_vs_debug_counter(wax_vs_engine *engine, const char *name, uint64_t *out);
 
+/* The form of the last fp32 scan this engine launched (the exact scan every search path ends in; tests): out[10] =
+   {kernel: 1 = TMA-staged, 2 = direct-load; C (rows of C x 128 elements, 0 = generic length), rows per step, warps,
+   stages (0 for the direct-load kernel); grid; chunk_steps (0 = static claims); mode: 0 = k <= 32 list, 1 = k <= 128
+   list, 2 = emit distance keys + radix select; tail: 0 = list merges (or none: emit), 1 = radix select over the grid's
+   keys staged in shared memory, 2 = radix select reading them from L2; query: 1 = in the kernel parameters, 0 = in
+   device memory}.  All zero before the first scan.  Read it while no search runs.  WAX_VS_ERR_UNSUPPORTED on a
+   multi-device handle. */
+int32_t wax_vs_debug_last_scan(wax_vs_engine *engine, uint32_t out[10]);
+
 /* Device-only timing of the batched path (n_queries synthetic unit queries per step, everything resident):
    total milliseconds of `iters` steps (CUDA events on the launching stream), kernel launches in the bracket and
    the number of queries of the last step whose proof did not complete (they would be re-run exactly). */

@@ -63,6 +63,9 @@ def test_argument_validation_without_a_device():
     assert L.wax_vs_count(None, None) == _lib.ERR_NULL
     assert L.wax_vs_debug_shadow_nominations(None, None, 10, None, None, None, None, None) == _lib.ERR_NULL
     assert L.wax_vs_debug_read_shadow(None, 0, 1, None) == _lib.ERR_NULL
+    out = (C.c_uint32 * 10)()
+    assert L.wax_vs_debug_last_scan(None, out) == _lib.ERR_NULL
+    assert L.wax_vs_debug_last_scan(None, None) == _lib.ERR_NULL
     L.wax_vs_destroy(None)  # no-op
 
 

@@ -258,7 +258,8 @@ def test_errors_equal_one_engines():
 REFUSED = ["wax_vs_add_batch_keyed", "wax_vs_contains", "wax_vs_search_device", "wax_vs_search_batch_device",
            "wax_vs_shard_open", "wax_vs_shard_close", "wax_vs_merge_candidates_device", "wax_vs_search_batch_where_device",
            "wax_vs_shard_search_where", "wax_vs_shard_grouped_expand_device", "wax_vs_shard_grouped_heads_device", "wax_vs_merge_group_heads_device", "wax_vs_deserialize_rows",
-           "wax_vs_export_rows", "wax_vs_debug_fill_synthetic", "wax_vs_debug_time_search", "wax_vs_debug_read_rows"]
+           "wax_vs_export_rows", "wax_vs_debug_fill_synthetic", "wax_vs_debug_time_search", "wax_vs_debug_read_rows",
+           "wax_vs_debug_last_scan"]
 
 
 def test_unserved_entries_are_refused_by_name():

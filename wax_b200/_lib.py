@@ -149,6 +149,7 @@ SIGNATURES = {
     "wax_vs_debug_phase_trace": (C.c_int32, [_eng, C.c_int64, C.c_uint32, _f32p]),
     "wax_vs_debug_batch_stats": (C.c_int32, [_eng, _u64p, _u64p]),
     "wax_vs_debug_counter": (C.c_int32, [_eng, C.c_char_p, _u64p]),
+    "wax_vs_debug_last_scan": (C.c_int32, [_eng, _u32p]),
     "wax_vs_debug_time_search_batch": (C.c_int32, [_eng, C.c_uint32, C.c_int64, C.c_uint64, C.c_uint32, C.c_uint32,
                                                    _f32p, _u64p, _u32p]),
     "wax_vs_debug_batch_nominations": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_int64, _u32p, _f32p, _u32p, _u64p,

@@ -367,6 +367,7 @@ struct wax_vs_engine {
     uint32_t u4_demoted = 0, u4_demote_window = 16;
     bool u4_probing = false;                              // the next 4-bit proof decides whether the window doubles
     uint64_t single_route_queries[kRouteForms] = {};      // single queries nominated from each shadow (pool_mu)
+    uint32_t last_scan[10] = {};                          // the form of the last fp32 scan launched (wax_vs_debug_last_scan; pool_mu)
     uint64_t batch_tensor_queries = 0, batch_fallback_queries = 0;   // instrumentation
     uint64_t batch_bf16_queries = 0, batch_retry_queries = 0, batch_tf32_queries = 0, batch_filter_bf16_queries = 0;
     uint64_t filter_bitset_passes = 0;
@@ -1231,6 +1232,16 @@ static int32_t enqueue_search(wax_vs_engine *e, SearchCtx *c, const float *d_que
         CUDA_TRY(launch_ldg(p, grid, e->similarity, mode, stream));
     }
     ++*launches;
+    {   // the form just launched, for wax_vs_debug_last_scan (the tail test is finish_topk_select's own)
+        const bool staged = static_cast<size_t>(grid) * k_eff * sizeof(uint64_t) <= p.tail_smem_bytes;
+        const uint32_t form[10] = {use_tma ? 1u : 2u, use_tma ? static_cast<uint32_t>(cfg.C) : 0u,
+                                   use_tma ? static_cast<uint32_t>(cfg.R) : 1u, use_tma ? static_cast<uint32_t>(cfg.warps) : 8u,
+                                   use_tma ? static_cast<uint32_t>(cfg.stages) : 0u, static_cast<uint32_t>(grid),
+                                   use_tma && !emit ? p.chunk_steps : 0u, static_cast<uint32_t>(mode),
+                                   p.tail_select ? (staged ? 1u : 2u) : 0u, p.query == nullptr ? 1u : 0u};
+        std::lock_guard<std::mutex> pg(e->pool_mu);
+        memcpy(e->last_scan, form, sizeof form);
+    }
 
     if (emit && !keys_only) {
         int32_t rc = enqueue_select(e, c, c->d_dist_keys, static_cast<uint32_t>(e->n_rows), k_eff, p, stream, launches);
@@ -5875,6 +5886,14 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *e, uint64_t *tensor_queries, uin
     std::lock_guard<std::mutex> g(e->pool_mu);
     if (tensor_queries) *tensor_queries = e->batch_tensor_queries;
     if (fallback_queries) *fallback_queries = e->batch_fallback_queries;
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_debug_last_scan(wax_vs_engine *e, uint32_t out[10]) {
+    WAX_VS_MULTI_REFUSE(e, "wax_vs_debug_last_scan");
+    if (!e || !out) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    std::lock_guard<std::mutex> g(e->pool_mu);
+    memcpy(out, e->last_scan, sizeof e->last_scan);
     return WAX_VS_OK;
 }
 

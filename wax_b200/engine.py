@@ -1068,6 +1068,16 @@ class CUDAVectorEngine:
         _check(L.lib().wax_vs_debug_counter(self._h, name.encode(), C.byref(v)))
         return v.value
 
+    def last_scan(self) -> dict:
+        """The form of the last fp32 scan this engine launched (wax_vs_debug_last_scan): kernel (1 = TMA-staged,
+        2 = direct-load), C, R, warps, stages, grid, chunk_steps (0 = static claims), mode (0 = k <= 32 list,
+        1 = k <= 128 list, 2 = emit + select), tail (0 = merge or none, 1 = select staged, 2 = select from L2) and
+        inline_query (1 = the query rode in the kernel parameters).  Read it while no search runs."""
+        out = np.zeros(10, np.uint32)
+        _check(L.lib().wax_vs_debug_last_scan(self._h, out.ctypes.data_as(C.POINTER(C.c_uint32))))
+        names = ("kernel", "C", "R", "warps", "stages", "grid", "chunk_steps", "mode", "tail", "inline_query")
+        return {name: int(v) for name, v in zip(names, out)}
+
     def time_search_batch(self, n_queries: int, top_k: int, iters: int, warmup: int = 2, seed: int = 7):
         """Device-only timing of the batched path. Returns (ms_total, launches, unproven_in_last_step)."""
         ms, launches, bad = C.c_float(0), C.c_uint64(0), C.c_uint32(0)
