@@ -77,8 +77,8 @@ int32_t wax_vs_device_count(int32_t *out);
    ids, order, score bits, counts, MV2V bytes, error codes and reasons.  It serves wax_vs_dimensions, _similarity,
    _count, _reserve, _add, _add_batch, _remove, _remove_batch, _rebalance, _search, _search_batch, _search_filtered,
    _search_batch_filtered, _search_batch_multi_filtered, _set_attributes, _set_locations, _set_terms,
-   _search_batch_where, _where_near, _where_terms, _set_groups, _search_grouped, _search_batch_grouped, _grouped_where,
-   _grouped_where_near, _grouped_multi_where, _serialized_length, _serialize, _deserialize, wax_vs_debug_set_option
+   _search_batch_where, _where_near, _where_terms, _where_groups, _set_groups, _search_grouped, _search_batch_grouped,
+   _grouped_where, _grouped_where_near, _grouped_multi_where, _grouped_multi_where_groups, _serialized_length, _serialize, _deserialize, wax_vs_debug_set_option
    (applied to every shard) and wax_vs_debug_counter (summed over the shards, plus "shard_rows.<r>": shard r's rows);
    every other entry point (the rank-level shard_*, *_device, keyed, export, absorb and merge entries, the other debug_*) returns
    WAX_VS_ERR_UNSUPPORTED naming itself.  Grouped search with clamp(top_groups) > WAX_VS_SHARD_MAX_GROUPS is refused as
@@ -520,6 +520,58 @@ int32_t wax_vs_search_batch_where_terms(wax_vs_engine *engine, const float *quer
                                         const uint64_t *where_terms, uint64_t *out_ids, float *out_scores,
                                         uint32_t out_stride, uint32_t *out_n);
 
+/* ---- group clauses: VideoRAG's video filter below the top-k (API EXTENSION) -----------------------------------------
+   VideoRAGQuery.videoIDs (VideoRAGTypes.swift:53) becomes FrameFilter(frameIds:), the union of segmentIdsByVideoID[v]
+   over the chosen videos, built in Swift on every request (VideoRAGOrchestrator.swift:239-247) and resolved id by id on
+   the host.  Here a where may name the groups instead: a row passes a where's group clause when its group is one of
+   the where's group ids.  A row's group is the one grouped search uses: the id last given to the frame by
+   wax_vs_set_groups, else the frame's own id (so with no set_groups the clause is a clause on frame ids); it follows the
+   frame through every mutator.  A clause lists 0 to 65 536 ids; duplicates are allowed, an id no row carries matches
+   nothing, and an empty list is no clause.  The clause is ANDed with the where's other clauses and the query's id
+   filter.  VideoRAG maps videoIDs to the roots of the chosen videos (the parentId its hits are grouped by).
+   How: wheres with equal contents are one unit.  A (where, id filter) pair with groups is tested on the host against an
+   allow-list; otherwise the device resolves each distinct group id of the call in the group index of grouped search
+   (built as grouped search builds it, counter "group_index_builds") and walks the rows of the unit's groups, or the
+   postings of its rarest term when that list is shorter than the group union -- O(rows of those groups), never a pass
+   over the corpus.  Each candidate is checked against the other clauses and a deny-list.  The rows that pass are counted:
+   <= 16 384 are listed and scored as a gather, wider units get their bits set in a row bitset under the
+   filter_bitset_bytes split.  Counters "where_group_units" (units planned on the device) and "where_group_rows_walked"
+   (the candidate positions their walks visit, once per unit and call). */
+/* wax_vs_search_batch_where_terms with a group clause in each where: where w requires one of
+   where_groups[where_group_offsets[w] .. where_group_offsets[w + 1]).  where_term_offsets may be NULL (no where has a
+   term).  Query i's answer is identical to wax_vs_search_batch_multi_filtered under an allow-list of exactly the frames
+   that pass every clause and the id filter: same ids, order and score bits.  Before the empty-engine early return: the
+   checks of wax_vs_search_batch_where_near, then NULL where_group_offsets, or NULL where_groups when some where has a
+   group -> WAX_VS_ERR_NULL, group offsets that do not start at 0 or decrease, or more than 65 536 ids in a where ->
+   WAX_VS_ERR_ARGUMENT, then the term checks of wax_vs_search_batch_where_terms.  A call in which no where has a group
+   runs wax_vs_search_batch_where_terms (term offsets given) or wax_vs_search_batch_where_near.  A call whose listed rows
+   would pass 2^32 - 1 -> WAX_VS_ERR_CAPACITY. */
+int32_t wax_vs_search_batch_where_groups(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                         uint32_t query_len, int64_t top_k, const uint64_t *frame_ids,
+                                         const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                         const uint32_t *query_filter, const wax_vs_where_near *wheres, uint32_t n_wheres,
+                                         const uint32_t *query_where, const uint64_t *where_term_offsets,
+                                         const uint64_t *where_terms, const uint64_t *where_group_offsets,
+                                         const uint64_t *where_groups, uint64_t *out_ids, float *out_scores,
+                                         uint32_t out_stride, uint32_t *out_n);
+/* wax_vs_search_batch_grouped_multi_where with a group clause in each where, as wax_vs_search_batch_where_groups takes
+   it (grouped search takes no term clause): VideoRAG's request -- the best segments of the best videos, among these
+   videos, inside this time window -- for many queries at once.  Query i's answer is identical to wax_vs_search_grouped
+   under an allow-list of exactly the frames that pass: same frame ids, group ids, group-major order and score bits.  The
+   checks of wax_vs_search_batch_grouped_multi_where, then the group checks of wax_vs_search_batch_where_groups, before
+   the empty-engine early return.  A call in which no where has a group runs wax_vs_search_batch_grouped_multi_where.
+   A selected group scored over its own rows, and a crowded query, is scored under its unit's row bitset, rebuilt on the
+   device. */
+int32_t wax_vs_search_batch_grouped_multi_where_groups(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                                       uint32_t query_len, int64_t top_groups, uint32_t per_group,
+                                                       const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                                       const int32_t *filter_modes, uint32_t n_filters,
+                                                       const uint32_t *query_filter, const wax_vs_where_near *wheres,
+                                                       uint32_t n_wheres, const uint32_t *query_where,
+                                                       const uint64_t *where_group_offsets, const uint64_t *where_groups,
+                                                       uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
+                                                       uint32_t out_stride, uint32_t *out_n);
+
 /* Device-resident form used by the row-sharded engine: `d_queries` (n_queries x dims) and
    `d_candidates` (n_queries x k_eff entries, k_eff = min(clamp(top_k), 10000) -- NOT clipped to N, padding
    has valid = 0) are DEVICE pointers on the engine's device; the work is enqueued on `cuda_stream`
@@ -734,7 +786,9 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *engine, uint64_t *tensor_queries
    nominate in TF32 at about half the rate), "batch_tf32_queries", "filter_bitset_passes" (sub-batches of per-query
    filtered queries on the tensor-core class, wax_vs_search_batch_multi_filtered), "group_index_builds" (device group
    index builds of wax_vs_search_grouped), "attribute_uploads" (device attribute copies of the where searches),
-   "term_index_builds" / "term_index_bytes" (term index builds of the where_terms searches / HBM the index holds), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
+   "term_index_builds" / "term_index_bytes" (term index builds of the where_terms searches / HBM the index holds),
+   "where_group_units" / "where_group_rows_walked" (units of the where_groups searches planned on the device / the
+   candidate positions they walk), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
    (single queries the shadow route answered / that the fp32 scan answered after a failed proof, either shadow; read them
    while no search is running), "single_int8_queries" (single queries whose route nominated from the int8 shadow),
    "int8_shadow_bytes" / "int8_shadow_rows" (HBM held by the int8 shadow's live rows, codes and scales / rows it covers),

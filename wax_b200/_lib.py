@@ -107,6 +107,13 @@ SIGNATURES = {
     "wax_vs_search_batch_where_terms": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _u64p,
                                                     C.POINTER(C.c_int32), C.c_uint32, _u32p, C.c_void_p, C.c_uint32,
                                                     _u32p, _u64p, _u64p, _u64p, _f32p, C.c_uint32, _u32p]),
+    "wax_vs_search_batch_where_groups": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _u64p,
+                                                     C.POINTER(C.c_int32), C.c_uint32, _u32p, C.c_void_p, C.c_uint32,
+                                                     _u32p, _u64p, _u64p, _u64p, _u64p, _u64p, _f32p, C.c_uint32, _u32p]),
+    "wax_vs_search_batch_grouped_multi_where_groups": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64,
+                                                                   C.c_uint32, _u64p, _u64p, C.POINTER(C.c_int32),
+                                                                   C.c_uint32, _u32p, C.c_void_p, C.c_uint32, _u32p,
+                                                                   _u64p, _u64p, _u64p, _f32p, _u64p, C.c_uint32, _u32p]),
     "wax_vs_shard_search_where": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_int64, _u64p, C.c_uint64, C.c_int32, C.c_void_p,
                                               _u64p, C.c_uint32, _u64p, _f32p, C.c_uint32, _u32p]),
     "wax_vs_search_batch_where_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, _u64p, _u64p,

@@ -42,6 +42,7 @@
 #include "waxvs_group_batch.cuh"
 #include "waxvs_where.cuh"
 #include "waxvs_terms.cuh"
+#include "waxvs_where_groups.cuh"
 
 #include <cub/cub.cuh>
 #include <cudaTypedefs.h>
@@ -275,6 +276,12 @@ struct SearchCtx {
     DevBuf<TermUnit> d_term_units;                 // ... the units of term_filter_kernel
     DevBuf<uint32_t> d_term_counts;                // ... their counts, then listing cursors
     DevBuf<uint32_t> d_term_deny;                  // ... and their deny-lists' rows, each list ascending
+    DevBuf<uint64_t> d_gw_ids;                     // where_groups search: the call's distinct group ids ...
+    DevBuf<GroupSpan> d_gw_resolved;               // ... their dense groups and CSR spans
+    DevBuf<GroupSpan> d_gw_spans;                  // ... each unit's groups, with their prefix
+    DevBuf<GroupUnit> d_gw_units;                  // ... the units of where_group_filter_kernel
+    DevBuf<uint32_t> d_gw_counts;                  // ... their counts, then listing cursors
+    DevBuf<uint32_t> d_gw_deny;                    // ... and their deny-lists' rows, each list ascending
     DevBuf<uint32_t> d_proof_count;                // shadow route: [0] proofs that held, [1] that failed (guarded scan) ...
     PinnedBuf<uint32_t> h_proof_count;             // ... and their mapped host mirror
     uint32_t seen_failed = 0;                      // h_proof_count[1] when the host last looked
@@ -387,6 +394,8 @@ struct wax_vs_engine {
     } gindex;
     std::mutex group_mu;
     uint64_t group_index_builds = 0;   // instrumentation (pool_mu)
+    uint64_t where_group_units = 0;        // where_groups search: units with a group clause planned on the device ...
+    uint64_t where_group_rows_walked = 0;  // ... and the candidate positions their walks visit (pool_mu)
     // Frame attributes (wax_vs_set_attributes): attrs[r] = row r's (timestamp, tags), kept aligned with `ids` by every
     // mutator exactly as `groups` is.  Empty while attrs_set is false: then every row has timestamp 0 and tags 0.
     bool attrs_set = false;
@@ -1888,11 +1897,12 @@ static int32_t sync_device_ids(wax_vs_engine *e, const uint64_t **out) {
 }
 
 // A where as the host plans it: the time and tag clauses, the location box (kNoLocBox: no location clause) and the
-// sorted, distinct term ids a row must hold (none: no term clause).
+// sorted, distinct term ids a row must hold (none: no term clause), and the group clause.
 struct Clause {
     WherePred pred;
     LocBox box;
     std::vector<uint64_t> terms;
+    std::vector<uint64_t> groups;      // sorted, distinct group ids, one of which the row's group must be (none: no clause)
 };
 
 // What a filtered, where or grouped search asks for.  Its entry point checks the arguments and builds it once (the
@@ -3040,6 +3050,11 @@ struct FilterSet {
     // wide unit in term_wide (empty, or WAX_VS_NO_FILTER, when it has none: its rows are the listed ones).
     std::vector<TermUnit> term_list, term_wide;
     std::vector<uint32_t> term_of;
+    // Where_groups search only (plan_group_units): filter f's group unit is group_units[group_of[f]] (empty, or
+    // WAX_VS_NO_FILTER, when it has none).  A unit of <= kWhereGatherRows rows (fs.count[f]) is listed by the device at its
+    // slot after the term units' rows; a wider one gets its bits set in its filter's bitset.
+    std::vector<GroupUnit> group_units;
+    std::vector<uint32_t> group_of;
 };
 // query_filter = nullptr: every filter is resolved (the single-filter entry points).
 static void resolve_filters(wax_vs_engine *e, const uint64_t *frame_ids, const uint64_t *filter_offsets, uint32_t n_filters,
@@ -3555,6 +3570,43 @@ static int32_t launch_term_filter(wax_vs_engine *e, SearchCtx *c, const std::vec
     return WAX_VS_OK;
 }
 
+constexpr uint64_t kWhereGatherRows = 16384;   // the gather class's largest allow-list (plan_filtered)
+
+// where_group_filter_kernel over `units` on `stream` (waxvs_where_groups.cuh), as launch_term_filter: counting into
+// c->d_gw_counts (zeroed here) and, with rows_out, listing each unit's rows at its slot; or, with bits, setting them in
+// bitset `slot` of bits.  plan_group_units sized c->d_gw_units and c->d_gw_counts for the call's largest launch and
+// staged the units' group spans in c->d_gw_spans and their deny-lists in c->d_gw_deny.
+static int32_t launch_group_filter(wax_vs_engine *e, SearchCtx *c, const std::vector<GroupUnit> &units, uint32_t *rows_out,
+                                   uint32_t *bits, cudaStream_t s, uint64_t *launches) {
+    const uint32_t n = static_cast<uint32_t>(units.size());
+    if (!n) return WAX_VS_OK;
+    int32_t rc;
+    if ((rc = c->d_gw_units.ensure(n, "group units")) || (rc = c->d_gw_counts.ensure(n, "group unit counts"))) return rc;
+    if (!bits) CUDA_TRY(cudaMemsetAsync(c->d_gw_counts, 0, n * sizeof(uint32_t), s));
+    CUDA_TRY(cudaMemcpyAsync(c->d_gw_units, units.data(), n * sizeof(GroupUnit), cudaMemcpyHostToDevice, s));
+    const uint32_t words = static_cast<uint32_t>((e->n_rows + 31) / 32);
+    for (uint32_t u0 = 0; u0 < n; u0 += 65535u) {       // grid.y limit
+        const uint32_t nu = std::min<uint32_t>(n - u0, 65535u);
+        uint32_t longest = 1;
+        for (uint32_t j = u0; j < u0 + nu; ++j) longest = std::max(longest, units[j].n_cand);
+        const uint32_t spread = std::max<uint32_t>(4, static_cast<uint32_t>(e->sm_count) * 16 / nu);
+        const dim3 grid(std::min<uint32_t>((longest + kTermThreads - 1) / kTermThreads, spread), nu);
+        where_group_filter_kernel<<<grid, kTermThreads, 0, s>>>(e->gindex.perm, e->gindex.row_group, e->tindex.postings,
+                                                                c->d_gw_spans, e->d_attrs, e->d_locs, c->d_gw_deny,
+                                                                c->d_gw_units + u0, bits ? nullptr : c->d_gw_counts + u0,
+                                                                rows_out, bits, words);
+        CUDA_TRY(cudaGetLastError());
+        ++*launches;
+    }
+    return WAX_VS_OK;
+}
+
+// Filter f's group unit when it is wide (its bits are set in its bitset, it lists nothing), else nullptr.
+static const GroupUnit *wide_group_unit(const FilterSet &fs, uint32_t f) {
+    if (fs.group_of.empty() || fs.group_of[f] == WAX_VS_NO_FILTER || fs.count[f] <= kWhereGatherRows) return nullptr;
+    return &fs.group_units[fs.group_of[f]];
+}
+
 // ---- batched filtered search ------------------------------------------------------------------------------------
 // n_queries queries, query i under filter query_filter[i] (WAX_VS_NO_FILTER: unfiltered); the single-filter entry
 // points are the case of one filter that every query names.  Every query referenced filter is resolved once; query i
@@ -3618,15 +3670,15 @@ static void plan_filtered(const wax_vs_engine *e, int64_t top_k, const int32_t *
 
 // The bitsets of the filters `which` (bitset l is filter which[l]'s) into c->d_mask on c->stream, from the rows
 // run_filtered staged in c->d_filter_rows: the listed rows in the filter's mode, then where search's predicate and box
-// ANDed in, and a wide term unit's rows set.  On an error the stream is synchronised.
+// ANDed in, and a wide term or group unit's rows set.  On an error the stream is synchronised.
 static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const WherePlan &wp, const std::vector<uint32_t> &which,
                                uint64_t *launches) {
     const FilterSet &fs = wp.fs;
     const uint32_t nf = static_cast<uint32_t>(which.size());
     std::vector<uint64_t> spec(3u * nf + 1u, 0);
     for (uint32_t l = 0; l < nf; ++l) {
-        const bool wide = !fs.term_of.empty() && fs.term_of[which[l]] != WAX_VS_NO_FILTER;
-        spec[l + 1] = spec[l] + (wide ? 0 : fs.count[which[l]]);       // a wide term unit lists nothing
+        const bool wide = (!fs.term_of.empty() && fs.term_of[which[l]] != WAX_VS_NO_FILTER) || wide_group_unit(fs, which[l]);
+        spec[l + 1] = spec[l] + (wide ? 0 : fs.count[which[l]]);       // a wide term or group unit lists nothing
         spec[nf + 1 + l] = fs.first[which[l]];
         spec[2u * nf + 1u + l] = static_cast<uint64_t>(wp.modes[which[l]]);
     }
@@ -3644,8 +3696,15 @@ static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const WherePlan &
             tbits.push_back(fs.term_wide[fs.term_of[which[l]]]);
             tbits.back().slot = l;
         }
+    std::vector<GroupUnit> gbits;                               // where_groups search: wide units' rows
+    for (uint32_t l = 0; l < nf; ++l)
+        if (const GroupUnit *u = wide_group_unit(fs, which[l])) {
+            gbits.push_back(*u);
+            gbits.back().slot = l;
+        }
     if ((rc = apply_where_bits(e, c, wbits, c->stream, launches)) ||
-        (rc = launch_term_filter(e, c, tbits, nullptr, c->d_mask, c->stream, launches))) {
+        (rc = launch_term_filter(e, c, tbits, nullptr, c->d_mask, c->stream, launches)) ||
+        (rc = launch_group_filter(e, c, gbits, nullptr, c->d_mask, c->stream, launches))) {
         cudaStreamSynchronize(c->stream);
         return rc;
     }
@@ -3653,12 +3712,16 @@ static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const WherePlan &
 }
 
 // The filters' rows into c->d_filter_rows on c->stream, where build_pass_bits and the gather class read them: the
-// host-listed rows, then the rows the device lists (narrow where units, narrow term units).
+// host-listed rows, then the rows the device lists (narrow where units, narrow term units, narrow group units).
 static int32_t stage_pair_rows(wax_vs_engine *e, SearchCtx *c, const FilterSet &fs, uint64_t *launches) {
     int32_t rc;
     if ((rc = stage_filter_rows(e, c, fs.rows, fs.rows.size() + fs.device_rows, -1, c->stream, nullptr))) return rc;
+    std::vector<GroupUnit> glist;
+    for (uint32_t f = 0; f < fs.group_of.size(); ++f)
+        if (fs.group_of[f] != WAX_VS_NO_FILTER && fs.count[f] && !wide_group_unit(fs, f)) glist.push_back(fs.group_units[fs.group_of[f]]);
     if ((rc = list_where_rows(e, c, fs.compact, c->stream, launches)) ||
-        (rc = launch_term_filter(e, c, fs.term_list, c->d_filter_rows, nullptr, c->stream, launches))) {
+        (rc = launch_term_filter(e, c, fs.term_list, c->d_filter_rows, nullptr, c->stream, launches)) ||
+        (rc = launch_group_filter(e, c, glist, c->d_filter_rows, nullptr, c->stream, launches))) {
         cudaStreamSynchronize(c->stream);
         return rc;
     }
@@ -3869,7 +3932,6 @@ static int32_t deliver_filtered(wax_vs_engine *e, SearchCtx *c, const float *que
 //    predicates) - (listed rows passing).  When nothing listed passes and at most kWhereGatherRows rows do, the device
 //    lists them (the gather class); otherwise the filter's bitset is the deny-list's (mode 1, listing only the rows that
 //    pass) with the predicate ANDed in on the device, for the tensor and scan classes.
-constexpr uint64_t kWhereGatherRows = 16384;   // the gather class's largest allow-list (plan_filtered)
 
 static WherePred where_pred(const wax_vs_where &w) { return WherePred{w.after, w.before, w.all_tags, w.no_tags}; }
 
@@ -3890,13 +3952,59 @@ static bool host_terms_pass(const wax_vs_engine *e, const std::vector<uint64_t> 
     return std::includes(p, p + t.n, req.begin(), req.end());
 }
 
+// Whether row r's group (its frame id while no set_groups was made) is one of the sorted, distinct list `groups`.
+static bool host_group_passes(const wax_vs_engine *e, const std::vector<uint64_t> &groups, uint32_t r) {
+    if (groups.empty()) return true;
+    return std::binary_search(groups.begin(), groups.end(), e->groups_set ? e->groups[r] : frame_id_of(e, r));
+}
+
 // The listed rows that pass every clause of `w`, appended to `out`.
 static void host_rows_passing(const wax_vs_engine *e, const Clause &w, const uint32_t *rows, uint64_t n,
                               std::vector<uint32_t> &out) {
     for (uint64_t i = 0; i < n; ++i) {
         const AttrRow a = e->attrs_set ? e->attrs[rows[i]] : AttrRow{0, 0};
-        if (where_passes(w.pred, a.ts, a.tags) && host_loc_passes(e, w.box, rows[i]) && host_terms_pass(e, w.terms, rows[i]))
+        if (where_passes(w.pred, a.ts, a.tags) && host_loc_passes(e, w.box, rows[i]) &&
+            host_terms_pass(e, w.terms, rows[i]) && host_group_passes(e, w.groups, rows[i]))
             out.push_back(rows[i]);
+    }
+}
+
+// The posting span of every distinct term id the wheres of pairs[p] (p in units_p) require, into `req` (sorted) and
+// `spans` (spans[j] is req[j]'s), on c's stream: the term index brought up, one launch, one read-back.
+static int32_t resolve_term_spans(wax_vs_engine *e, SearchCtx *c, const std::vector<Clause> &wheres,
+                                  const std::vector<std::pair<uint32_t, uint32_t>> &pairs,
+                                  const std::vector<uint32_t> &units_p, std::vector<uint64_t> &req,
+                                  std::vector<TermSpan> &spans) {
+    int32_t rc;
+    if ((rc = ensure_term_index(e, c))) return rc;
+    const auto &ti = e->tindex;
+    cudaStream_t s = c->stream;
+    for (const uint32_t p : units_p) req.insert(req.end(), wheres[pairs[p].first].terms.begin(), wheres[pairs[p].first].terms.end());
+    std::sort(req.begin(), req.end());
+    req.erase(std::unique(req.begin(), req.end()), req.end());
+    const uint32_t n_ids = static_cast<uint32_t>(req.size());
+    spans.assign(n_ids, TermSpan{0, 0, 0});
+    if ((rc = c->d_term_ids.ensure(n_ids, "required terms")) || (rc = c->d_term_spans.ensure(n_ids, "term spans"))) return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_term_ids, req.data(), n_ids * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    term_spans_kernel<<<std::max<uint32_t>(1, std::min<uint32_t>((n_ids + 255) / 256, e->sm_count * 8)), 256, 0, s>>>(
+        ti.keys, ti.start, ti.n_terms, c->d_term_ids, n_ids, c->d_term_spans);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(spans.data(), c->d_term_spans, n_ids * sizeof(TermSpan), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return WAX_VS_OK;
+}
+
+// The deny-lists of the units pairs[p] (p in units_p), each sorted, once per list: deny_of[f] = filter f's rows in
+// deny_rows.
+static void unit_deny_lists(const FilterSet &ids, const std::vector<std::pair<uint32_t, uint32_t>> &pairs,
+                            const std::vector<uint32_t> &units_p, std::vector<uint32_t> &deny_rows,
+                            std::unordered_map<uint32_t, TermSpan> &deny_of) {
+    for (const uint32_t p : units_p) {
+        const uint32_t f = pairs[p].second;
+        if (f == WAX_VS_NO_FILTER || deny_of.count(f)) continue;
+        deny_of[f] = TermSpan{deny_rows.size(), static_cast<uint32_t>(ids.count[f]), 0};
+        deny_rows.insert(deny_rows.end(), ids.rows.begin() + ids.first[f], ids.rows.begin() + ids.first[f] + ids.count[f]);
+        std::sort(deny_rows.end() - ids.count[f], deny_rows.end());
     }
 }
 
@@ -3912,33 +4020,14 @@ static int32_t plan_term_units(wax_vs_engine *e, SearchCtx *c, const std::vector
                                const std::vector<std::pair<uint32_t, uint32_t>> &pairs, const std::vector<uint32_t> &units_p,
                                FilterSet &fs, uint64_t &at) {
     int32_t rc;
-    if ((rc = ensure_term_index(e, c))) return rc;
-    const auto &ti = e->tindex;
     cudaStream_t s = c->stream;
     std::vector<uint64_t> req;
-    for (const uint32_t p : units_p) req.insert(req.end(), wheres[pairs[p].first].terms.begin(), wheres[pairs[p].first].terms.end());
-    std::sort(req.begin(), req.end());
-    req.erase(std::unique(req.begin(), req.end()), req.end());
-    const uint32_t n_ids = static_cast<uint32_t>(req.size());
-    std::vector<TermSpan> spans(n_ids);
-    if ((rc = c->d_term_ids.ensure(n_ids, "required terms")) || (rc = c->d_term_spans.ensure(n_ids, "term spans"))) return rc;
-    CUDA_TRY(cudaMemcpyAsync(c->d_term_ids, req.data(), n_ids * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
-    term_spans_kernel<<<std::max<uint32_t>(1, std::min<uint32_t>((n_ids + 255) / 256, e->sm_count * 8)), 256, 0, s>>>(
-        ti.keys, ti.start, ti.n_terms, c->d_term_ids, n_ids, c->d_term_spans);
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaMemcpyAsync(spans.data(), c->d_term_spans, n_ids * sizeof(TermSpan), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaStreamSynchronize(s));
+    std::vector<TermSpan> spans;
+    if ((rc = resolve_term_spans(e, c, wheres, pairs, units_p, req, spans))) return rc;
 
-    // the deny-lists of the units, each sorted, once per list
     std::vector<uint32_t> deny_rows;
     std::unordered_map<uint32_t, TermSpan> deny_of;
-    for (const uint32_t p : units_p) {
-        const uint32_t f = pairs[p].second;
-        if (f == WAX_VS_NO_FILTER || deny_of.count(f)) continue;
-        deny_of[f] = TermSpan{deny_rows.size(), static_cast<uint32_t>(ids.count[f]), 0};
-        deny_rows.insert(deny_rows.end(), ids.rows.begin() + ids.first[f], ids.rows.begin() + ids.first[f] + ids.count[f]);
-        std::sort(deny_rows.end() - ids.count[f], deny_rows.end());
-    }
+    unit_deny_lists(ids, pairs, units_p, deny_rows, deny_of);
     if ((rc = c->d_term_deny.ensure(std::max<size_t>(deny_rows.size(), 1), "term deny-lists"))) return rc;
     if (!deny_rows.empty())
         CUDA_TRY(cudaMemcpyAsync(c->d_term_deny, deny_rows.data(), deny_rows.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
@@ -4001,10 +4090,138 @@ static int32_t plan_term_units(wax_vs_engine *e, SearchCtx *c, const std::vector
     return WAX_VS_OK;
 }
 
+// The group units of a call (pairs[p] for p in units_p, whose where has groups and whose id filter is none or a
+// deny-list) on c's stream, planned as plan_term_units plans term units: the device group index brought up, every
+// distinct group id of the call resolved to its dense group and CSR span (one launch, one read-back), each unit's
+// groups and their prefix staged in c->d_gw_spans, then one where_group_filter_kernel launch counts each unit's rows
+// (another read-back).  A unit walks the rows of its groups, or the postings of its rarest term when that list is the
+// shorter; a unit none of whose groups (or some of whose terms) any row carries is empty and launches nothing.  A unit
+// becomes an allow-list of its fs.count[p] rows, listed by the device from `at` on (<= kWhereGatherRows) or set in its
+// bitset (wider).  `at` ends past the last slot.
+static int32_t ensure_group_index(wax_vs_engine *e, SearchCtx *c);
+static int32_t plan_group_units(wax_vs_engine *e, SearchCtx *c, const std::vector<Clause> &wheres, const FilterSet &ids,
+                                const std::vector<std::pair<uint32_t, uint32_t>> &pairs, const std::vector<uint32_t> &units_p,
+                                FilterSet &fs, uint64_t &at) {
+    int32_t rc;
+    if ((rc = ensure_group_index(e, c))) return rc;
+    const auto &gi = e->gindex;
+    cudaStream_t s = c->stream;
+    std::vector<uint64_t> req;
+    bool with_terms = false;
+    for (const uint32_t p : units_p) {
+        const Clause &w = wheres[pairs[p].first];
+        req.insert(req.end(), w.groups.begin(), w.groups.end());
+        with_terms = with_terms || !w.terms.empty();
+    }
+    std::sort(req.begin(), req.end());
+    req.erase(std::unique(req.begin(), req.end()), req.end());
+    const uint32_t n_ids = static_cast<uint32_t>(req.size());
+    std::vector<GroupSpan> resolved(n_ids);
+    if ((rc = c->d_gw_ids.ensure(n_ids, "where groups")) || (rc = c->d_gw_resolved.ensure(n_ids, "where group spans")))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_gw_ids, req.data(), n_ids * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    where_group_spans_kernel<<<std::max<uint32_t>(1, std::min<uint32_t>((n_ids + 255) / 256, e->sm_count * 8)), 256, 0, s>>>(
+        gi.ids, gi.starts, gi.n_groups, c->d_gw_ids, n_ids, c->d_gw_resolved);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(resolved.data(), c->d_gw_resolved, n_ids * sizeof(GroupSpan), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    std::vector<uint64_t> treq;
+    std::vector<TermSpan> tspans;
+    if (with_terms && (rc = resolve_term_spans(e, c, wheres, pairs, units_p, treq, tspans))) return rc;
+
+    std::vector<uint32_t> deny_rows;
+    std::unordered_map<uint32_t, TermSpan> deny_of;
+    unit_deny_lists(ids, pairs, units_p, deny_rows, deny_of);
+
+    // each unit's groups in ascending dense order (its ids are sorted, and dense groups follow the ids' order), those no
+    // row carries dropped, with the exclusive prefix of their row counts
+    std::vector<GroupSpan> gspans;
+    std::vector<GroupUnit> units;
+    std::vector<uint32_t> unit_pair;
+    bool located = false;
+    uint64_t walked = 0;
+    for (const uint32_t p : units_p) {
+        const Clause &w = wheres[pairs[p].first];
+        const uint32_t f = pairs[p].second;
+        fs.first[p] = at;
+        fs.count[p] = 0;
+        GroupUnit u{};
+        u.pred = w.pred;
+        u.box = w.box;
+        u.has_box = box_active(w.box);
+        u.deny = f == WAX_VS_NO_FILTER ? TermSpan{0, 0, 0} : deny_of[f];
+        u.gspan0 = gspans.size();
+        uint32_t rows = 0;
+        for (const uint64_t g : w.groups) {
+            GroupSpan gs = resolved[std::lower_bound(req.begin(), req.end(), g) - req.begin()];
+            if (gs.count == 0) continue;
+            gs.before = rows;
+            rows += gs.count;
+            gspans.push_back(gs);
+        }
+        u.n_gspans = static_cast<uint32_t>(gspans.size() - u.gspan0);
+        u.n_spans = static_cast<uint32_t>(w.terms.size());
+        uint32_t rarest = 0;
+        for (uint32_t j = 0; j < u.n_spans; ++j) {
+            u.spans[j] = tspans[std::lower_bound(treq.begin(), treq.end(), w.terms[j]) - treq.begin()];
+            if (u.spans[j].count < u.spans[rarest].count) rarest = j;
+        }
+        if (rows == 0 || (u.n_spans && u.spans[rarest].count == 0)) {
+            gspans.resize(u.gspan0);
+            continue;
+        }
+        if (u.n_spans) std::swap(u.spans[0], u.spans[rarest]);
+        u.walk_terms = u.n_spans && u.spans[0].count < rows;
+        u.n_cand = u.walk_terms ? u.spans[0].count : rows;
+        walked += u.n_cand;
+        located = located || u.has_box;
+        units.push_back(u);
+        unit_pair.push_back(p);
+    }
+    {
+        std::lock_guard<std::mutex> pg(e->pool_mu);
+        e->where_group_units += units_p.size();
+        e->where_group_rows_walked += walked;
+    }
+    const uint32_t n_units = static_cast<uint32_t>(units.size());
+    if (!n_units) return WAX_VS_OK;
+    if ((rc = ensure_attributes(e, c, located))) return rc;
+    // sized once for the largest launch of the call (run_filtered and grouped_one launch subsets of these units)
+    if ((rc = c->d_gw_spans.ensure(gspans.size(), "where group unit spans")) ||
+        (rc = c->d_gw_deny.ensure(std::max<size_t>(deny_rows.size(), 1), "where group deny-lists")) ||
+        (rc = c->d_gw_units.ensure(n_units, "group units")) || (rc = c->d_gw_counts.ensure(n_units, "group unit counts")))
+        return rc;
+    CUDA_TRY(cudaMemcpyAsync(c->d_gw_spans, gspans.data(), gspans.size() * sizeof(GroupSpan), cudaMemcpyHostToDevice, s));
+    if (!deny_rows.empty())
+        CUDA_TRY(cudaMemcpyAsync(c->d_gw_deny, deny_rows.data(), deny_rows.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
+    uint64_t launches = 0;
+    if ((rc = launch_group_filter(e, c, units, nullptr, nullptr, s, &launches))) { cudaStreamSynchronize(s); return rc; }
+    std::vector<uint32_t> counts(n_units);
+    CUDA_TRY(cudaMemcpyAsync(counts.data(), c->d_gw_counts, n_units * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    fs.group_of.assign(fs.count.size(), WAX_VS_NO_FILTER);
+    for (uint32_t j = 0; j < n_units; ++j) {
+        const uint32_t p = unit_pair[j];
+        fs.count[p] = counts[j];
+        if (counts[j] == 0) continue;
+        if (counts[j] <= kWhereGatherRows) {                 // narrow: listed at its slot (the gather class)
+            units[j].slot = at;
+            fs.first[p] = at;
+            at += counts[j];
+        }                                                    // wide: its bitset's bits (wide_group_unit)
+        fs.group_of[p] = static_cast<uint32_t>(fs.group_units.size());
+        fs.group_units.push_back(units[j]);
+    }
+    if (at > UINT32_MAX)                                     // the gather spans hold 32-bit offsets
+        return fail(WAX_VS_ERR_CAPACITY, "the filters of one call list %llu rows, at most %u are supported",
+                    static_cast<unsigned long long>(at), UINT32_MAX);
+    return WAX_VS_OK;
+}
+
 // The pairs of a call as the filters of `fs` (modes[p], pair_of[i] = query i's pair or WAX_VS_NO_FILTER), from the
 // resolved id filters `ids`.  Runs the count pass on c's stream.  A pair's where is tested whole on the host against an
-// allow-list; otherwise a where with terms makes the pair a term unit (plan_term_units), and any other where is tested
-// on the device, its box with it.
+// allow-list; otherwise a where with groups makes the pair a group unit (plan_group_units), one with terms a term unit
+// (plan_term_units), and any other where is tested on the device, its box with it.
 static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const std::vector<Clause> &wheres,
                                 const uint32_t *query_where, const int32_t *filter_modes, const uint32_t *query_filter,
                                 uint32_t n_queries, const FilterSet &ids, FilterSet &fs, std::vector<int32_t> &modes,
@@ -4024,7 +4241,7 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const std::vecto
     std::vector<WhereNearItem> counted;
     for (const auto &pr : pairs)
         if (pr.first != WAX_VS_NO_FILTER && (pr.second == WAX_VS_NO_FILTER || filter_modes[pr.second] == 1) &&
-            slot[pr.first] == WAX_VS_NO_FILTER && wheres[pr.first].terms.empty()) {
+            slot[pr.first] == WAX_VS_NO_FILTER && wheres[pr.first].terms.empty() && wheres[pr.first].groups.empty()) {
             slot[pr.first] = static_cast<uint32_t>(counted.size());
             counted.push_back(where_item(wheres[pr.first]));
         }
@@ -4038,7 +4255,7 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const std::vecto
     fs.where.assign(np, WAX_VS_NO_FILTER);
     fs.allowed.assign(np, 0);
     modes.assign(np, 0);
-    std::vector<uint32_t> listed_by_device, term_units;
+    std::vector<uint32_t> listed_by_device, term_units, group_units;
     for (uint32_t p = 0; p < np; ++p) {
         const uint32_t w = pairs[p].first, f = pairs[p].second;
         const uint32_t *rows = f == WAX_VS_NO_FILTER ? nullptr : ids.rows.data() + ids.first[f];
@@ -4048,6 +4265,10 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const std::vecto
             fs.rows.insert(fs.rows.end(), rows, rows + n_listed);
             fs.count[p] = n_listed;
             modes[p] = filter_modes[f];
+            continue;
+        }
+        if (!wheres[w].groups.empty() && (f == WAX_VS_NO_FILTER || filter_modes[f] == 1)) {  // listed from the group index
+            group_units.push_back(p);
             continue;
         }
         if (!wheres[w].terms.empty() && (f == WAX_VS_NO_FILTER || filter_modes[f] == 1)) {   // listed from the postings
@@ -4077,6 +4298,7 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const std::vecto
         at += fs.count[p];
     }
     if (!term_units.empty() && (rc = plan_term_units(e, c, wheres, ids, pairs, term_units, fs, at))) return rc;
+    if (!group_units.empty() && (rc = plan_group_units(e, c, wheres, ids, pairs, group_units, fs, at))) return rc;
     fs.device_rows = at - fs.rows.size();
     return WAX_VS_OK;
 }
@@ -4395,36 +4617,50 @@ int32_t wax_vs_set_terms(wax_vs_engine *e, const uint64_t *frame_ids, const uint
     return WAX_VS_OK;
 }
 
-// The clauses of wheres[0, n_wheres) with their term lists.  With a where list, wheres with terms and equal contents
-// (clauses, box, required ids) are one: each query names the first of them, so a batch that scopes 1 024 queries to 16
-// sessions plans 16 units, not 1 024.
-static int32_t request_term_clauses(SearchRequest &r, const wax_vs_where_near *wheres, uint32_t n_wheres,
-                                    const uint64_t *where_term_offsets, const uint64_t *where_terms) {
-    int32_t rc;
-    if ((rc = check_term_offsets(where_term_offsets, n_wheres, where_terms, kMaxWhereTerms, "where_term_offsets"))) return rc;
-    if ((rc = near_clauses(wheres, n_wheres, r.wheres))) return rc;
+// lists[offsets[w], offsets[w + 1]) of each where w, sorted and deduplicated, into (r.wheres[w].*field).
+static void request_id_lists(SearchRequest &r, uint32_t n_wheres, const uint64_t *offsets, const uint64_t *lists,
+                             std::vector<uint64_t> Clause::*field) {
     for (uint32_t w = 0; w < n_wheres; ++w) {
-        std::vector<uint64_t> &terms = r.wheres[w].terms;
-        terms.assign(where_terms + where_term_offsets[w], where_terms + where_term_offsets[w + 1]);
-        std::sort(terms.begin(), terms.end());
-        terms.erase(std::unique(terms.begin(), terms.end()), terms.end());
+        std::vector<uint64_t> &ids = r.wheres[w].*field;
+        ids.assign(lists + offsets[w], lists + offsets[w + 1]);
+        std::sort(ids.begin(), ids.end());
+        ids.erase(std::unique(ids.begin(), ids.end()), ids.end());
     }
-    if (!r.query_where) return WAX_VS_OK;
+}
+
+// With a where list, wheres with terms or groups and equal contents (clauses, box, required ids, group ids) are one:
+// each query names the first of them, so a batch that scopes 1 024 queries to 16 sessions plans 16 units, not 1 024.
+static void canonical_wheres(SearchRequest &r) {
+    if (!r.query_where) return;
+    const uint32_t n_wheres = static_cast<uint32_t>(r.wheres.size());
     std::vector<uint32_t> canon(n_wheres);
     std::unordered_map<std::string, uint32_t> first_of;
     for (uint32_t w = 0; w < n_wheres; ++w) {
         const Clause &cl = r.wheres[w];
         canon[w] = w;
-        if (cl.terms.empty()) continue;
+        if (cl.terms.empty() && cl.groups.empty()) continue;
+        const uint64_t n_terms = cl.terms.size();
         std::string key(reinterpret_cast<const char *>(&cl.pred), sizeof(WherePred));
         key.append(reinterpret_cast<const char *>(&cl.box), sizeof(LocBox));
+        key.append(reinterpret_cast<const char *>(&n_terms), sizeof(n_terms));
         key.append(reinterpret_cast<const char *>(cl.terms.data()), cl.terms.size() * sizeof(uint64_t));
+        key.append(reinterpret_cast<const char *>(cl.groups.data()), cl.groups.size() * sizeof(uint64_t));
         canon[w] = first_of.emplace(std::move(key), w).first->second;
     }
     r.where_of.resize(r.n_queries);
     for (uint32_t i = 0; i < r.n_queries; ++i)
         r.where_of[i] = r.query_where[i] == WAX_VS_NO_FILTER ? WAX_VS_NO_FILTER : canon[r.query_where[i]];
     r.query_where = r.where_of.data();
+}
+
+// The clauses of wheres[0, n_wheres) with their term lists, equal wheres made one (canonical_wheres).
+static int32_t request_term_clauses(SearchRequest &r, const wax_vs_where_near *wheres, uint32_t n_wheres,
+                                    const uint64_t *where_term_offsets, const uint64_t *where_terms) {
+    int32_t rc;
+    if ((rc = check_term_offsets(where_term_offsets, n_wheres, where_terms, kMaxWhereTerms, "where_term_offsets"))) return rc;
+    if ((rc = near_clauses(wheres, n_wheres, r.wheres))) return rc;
+    request_id_lists(r, n_wheres, where_term_offsets, where_terms, &Clause::terms);
+    canonical_wheres(r);
     return WAX_VS_OK;
 }
 
@@ -4442,6 +4678,57 @@ int32_t wax_vs_search_batch_where_terms(wax_vs_engine *e, const float *queries, 
         return rc;
     if (!where_term_offsets) return fail(WAX_VS_ERR_NULL, "where_term_offsets is NULL");
     if ((rc = request_term_clauses(req, wheres, n_wheres, where_term_offsets, where_terms))) return rc;
+    return search_where(e, req, out_ids, out_scores, out_stride, out_n);
+}
+
+// ---- group clauses: VideoRAG's videoIDs as "the row's group is one of these", from the group index -------------------
+// (waxvs_where_groups.cuh).  The group offsets of n_wheres wheres: not NULL, start at 0, never decrease, at most
+// kMaxWhereGroups ids in a where, and the ids not NULL when some where has one.  *any = some where has a group.
+static int32_t check_group_offsets(const uint64_t *offsets, uint32_t n_wheres, const uint64_t *groups, bool *any) {
+    if (!offsets) return fail(WAX_VS_ERR_NULL, "where_group_offsets is NULL");
+    if (offsets[0] != 0) return fail(WAX_VS_ERR_ARGUMENT, "where_group_offsets[0] must be 0");
+    for (uint32_t w = 0; w < n_wheres; ++w) {
+        if (offsets[w + 1] < offsets[w]) return fail(WAX_VS_ERR_ARGUMENT, "where_group_offsets decrease at where %u", w);
+        if (offsets[w + 1] - offsets[w] > kMaxWhereGroups)
+            return fail(WAX_VS_ERR_ARGUMENT, "where %u has %llu group ids, at most %u are allowed", w,
+                        static_cast<unsigned long long>(offsets[w + 1] - offsets[w]), kMaxWhereGroups);
+    }
+    if (offsets[n_wheres] && !groups) return fail(WAX_VS_ERR_NULL, "where_groups is NULL");
+    *any = offsets[n_wheres] != 0;
+    return WAX_VS_OK;
+}
+
+int32_t wax_vs_search_batch_where_groups(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                         int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                         const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                         const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                         const uint64_t *where_term_offsets, const uint64_t *where_terms,
+                                         const uint64_t *where_group_offsets, const uint64_t *where_groups,
+                                         uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n) {
+    if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(queries, n_queries, query_len, top_k);
+    int32_t rc;
+    bool any = false;
+    if ((rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
+        (rc = request_where_list(req, wheres, n_wheres, query_where)) ||
+        (rc = check_group_offsets(where_group_offsets, n_wheres, where_groups, &any)))
+        return rc;
+    if (!any)                          // no where has a group: the entry point without the clause
+        return where_term_offsets
+                   ? wax_vs_search_batch_where_terms(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets,
+                                                     filter_modes, n_filters, query_filter, wheres, n_wheres, query_where,
+                                                     where_term_offsets, where_terms, out_ids, out_scores, out_stride, out_n)
+                   : wax_vs_search_batch_where_near(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets,
+                                                    filter_modes, n_filters, query_filter, wheres, n_wheres, query_where,
+                                                    out_ids, out_scores, out_stride, out_n);
+    if (where_term_offsets) {
+        if ((rc = check_term_offsets(where_term_offsets, n_wheres, where_terms, kMaxWhereTerms, "where_term_offsets")))
+            return rc;
+    }
+    if ((rc = near_clauses(wheres, n_wheres, req.wheres))) return rc;
+    if (where_term_offsets) request_id_lists(req, n_wheres, where_term_offsets, where_terms, &Clause::terms);
+    request_id_lists(req, n_wheres, where_group_offsets, where_groups, &Clause::groups);
+    canonical_wheres(req);
     return search_where(e, req, out_ids, out_scores, out_stride, out_n);
 }
 
@@ -4843,12 +5130,13 @@ static uint32_t deliver_group_keys(const wax_vs_engine *e, const uint64_t *keys,
 
 // One grouped search under the caller's read lock and scratch context (re-taking the shared lock inside a batch could
 // wait behind a queued writer): the host query, the filter's resolved rows (nullptr: unfiltered; the filter allows some
-// row) with `where` ANDed into its bitset (nullptr: none), the answer at out_* and *out_n -- or, with out_keys, as
-// n_top x per_group keys (dist_key << 32 | row, group-major, padded with WAXVS_KEY_NONE) there instead.  The arguments
-// are checked by the caller.
+// row) with `where` ANDed into its bitset (nullptr: none) and the rows of a planned group unit set in it (nullptr: none;
+// then `rows` is empty, in mode 0), the answer at out_* and *out_n -- or, with out_keys, as n_top x per_group keys
+// (dist_key << 32 | row, group-major, padded with WAXVS_KEY_NONE) there instead.  The arguments are checked by the caller.
 static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, uint32_t n_top, uint32_t per_group,
                            const std::vector<uint32_t> *rows, int32_t mode, const Clause *where, uint64_t *out_ids,
-                           float *out_scores, uint64_t *out_groups, uint32_t *out_n, uint64_t *out_keys = nullptr) {
+                           float *out_scores, uint64_t *out_groups, uint32_t *out_n, uint64_t *out_keys = nullptr,
+                           const GroupUnit *unit = nullptr) {
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const bool filtered = rows != nullptr;
     cudaStream_t s = c->stream;
@@ -4862,8 +5150,14 @@ static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, u
     if ((rc = c->d_out.ensure(n_top, "result buffer"))) return rc;
     if ((rc = c->h_out.ensure(n_top, "result staging"))) return rc;
     if (filtered) {
+        std::vector<GroupUnit> unit_bits;
+        if (unit) {
+            unit_bits.push_back(*unit);
+            unit_bits.back().slot = 0;
+        }
         if ((rc = stage_filter_rows(e, c, *rows, rows->size(), mode, s, &launches)) ||
-            (where && (rc = apply_where_bits(e, c, {where_item(*where)}, s, &launches)))) {
+            (where && (rc = apply_where_bits(e, c, {where_item(*where)}, s, &launches))) ||
+            (rc = launch_group_filter(e, c, unit_bits, nullptr, c->d_mask, s, &launches))) {
             cudaStreamSynchronize(s);
             return rc;
         }
@@ -5178,17 +5472,21 @@ static int32_t search_grouped_host(wax_vs_engine *e, const SearchRequest &req, c
     std::sort(crowded.begin(), crowded.end());
     // crowded queries (and batches the coverage level does not take): the single-query pipeline, same lock and context,
     // under the query's own pair as the one-filter grouped search takes it -- an id filter alone as it is, an allow-list
-    // as its rows that pass the where (plan_where_pairs listed them), a deny-list (or none) AND a where as the deny-list
-    // in mode 1 with the predicate and its box ANDed into the bitset
+    // as its rows that pass the where (plan_where_pairs listed them), a group unit as its rows set in an empty bitset by
+    // the device, a deny-list (or none) AND any other where as the deny-list in mode 1 with the predicate and its box
+    // ANDed into the bitset
     const FilterSet &ids = wp.ids, &fs = wp.fs;
     for (uint32_t qi : crowded) {
-        const uint32_t p = wp.pair_of[qi], w = req.query_where[qi], f = req.query_filter[qi];
+        const uint32_t p = wp.pair_of[qi], f = req.query_filter[qi];
+        const GroupUnit *unit = p != WAX_VS_NO_FILTER && !fs.group_of.empty() && fs.group_of[p] != WAX_VS_NO_FILTER
+                                    ? &fs.group_units[fs.group_of[p]] : nullptr;
+        const uint32_t w = unit ? WAX_VS_NO_FILTER : req.query_where[qi];
         const bool row_where = w != WAX_VS_NO_FILTER && (f == WAX_VS_NO_FILTER || req.filter_modes[f] == 1);
         std::vector<uint32_t> rows;
-        int32_t mode = 1;
+        int32_t mode = unit ? 0 : 1;
         if (row_where) {
             if (f != WAX_VS_NO_FILTER) rows.assign(ids.rows.begin() + ids.first[f], ids.rows.begin() + ids.first[f] + ids.count[f]);
-        } else if (p != WAX_VS_NO_FILTER) {
+        } else if (p != WAX_VS_NO_FILTER && !unit) {
             rows.assign(fs.rows.begin() + fs.first[p], fs.rows.begin() + fs.first[p] + fs.count[p]);
             mode = wp.modes[p];
         }
@@ -5197,7 +5495,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const SearchRequest &req, c
             std::vector<uint64_t> keys(slots);
             if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group,
                                   p == WAX_VS_NO_FILTER ? nullptr : &rows, mode, row_where ? &req.wheres[w] : nullptr, nullptr,
-                                  nullptr, nullptr, nullptr, keys.data())))
+                                  nullptr, nullptr, nullptr, keys.data(), unit)))
                 return rc;
             std::vector<wax_vs_group_candidate> recs(slots, wax_vs_group_candidate{});
             for (size_t i = 0; i < slots; ++i) {
@@ -5216,7 +5514,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const SearchRequest &req, c
         const size_t o = static_cast<size_t>(qi) * out_stride;
         if ((rc = grouped_one(e, c, queries + static_cast<size_t>(qi) * e->dims, n_top, per_group,
                               p == WAX_VS_NO_FILTER ? nullptr : &rows, mode, row_where ? &req.wheres[w] : nullptr, out_ids + o,
-                              out_scores + o, out_groups + o, out_n + qi)))
+                              out_scores + o, out_groups + o, out_n + qi, nullptr, unit)))
             return rc;
     }
     if (!req.batched) return WAX_VS_OK;
@@ -5303,6 +5601,35 @@ int32_t wax_vs_search_batch_grouped_multi_where(wax_vs_engine *e, const float *q
         (rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
         (rc = request_where_list(req, wheres, n_wheres, query_where)) || (rc = near_clauses(wheres, n_wheres, req.wheres)))
         return rc;
+    return search_grouped(e, req, out_ids, out_scores, out_groups, out_stride, out_n);
+}
+
+int32_t wax_vs_search_batch_grouped_multi_where_groups(wax_vs_engine *e, const float *queries, uint32_t n_queries,
+                                                       uint32_t query_len, int64_t top_groups, uint32_t per_group,
+                                                       const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                                       const int32_t *filter_modes, uint32_t n_filters,
+                                                       const uint32_t *query_filter, const wax_vs_where_near *wheres,
+                                                       uint32_t n_wheres, const uint32_t *query_where,
+                                                       const uint64_t *where_group_offsets, const uint64_t *where_groups,
+                                                       uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
+                                                       uint32_t out_stride, uint32_t *out_n) {
+    if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(queries, n_queries, query_len, top_groups, per_group, n_queries > 1);
+    int32_t rc;
+    bool any = false;
+    if ((rc = check_grouped_args(req)) ||
+        (rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
+        (rc = request_where_list(req, wheres, n_wheres, query_where)) ||
+        (rc = check_group_offsets(where_group_offsets, n_wheres, where_groups, &any)))
+        return rc;
+    if (!any)                          // no where has a group: the entry point without the clause
+        return wax_vs_search_batch_grouped_multi_where(e, queries, n_queries, query_len, top_groups, per_group, frame_ids,
+                                                       filter_offsets, filter_modes, n_filters, query_filter, wheres,
+                                                       n_wheres, query_where, out_ids, out_scores, out_groups, out_stride,
+                                                       out_n);
+    if ((rc = near_clauses(wheres, n_wheres, req.wheres))) return rc;
+    request_id_lists(req, n_wheres, where_group_offsets, where_groups, &Clause::groups);
+    canonical_wheres(req);
     return search_grouped(e, req, out_ids, out_scores, out_groups, out_stride, out_n);
 }
 
@@ -5913,6 +6240,8 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "batch_tf32_queries")) *out = e->batch_tf32_queries;
     else if (!strcmp(name, "filter_bitset_passes")) *out = e->filter_bitset_passes;   // per-query filters: tensor sub-batches
     else if (!strcmp(name, "group_index_builds")) *out = e->group_index_builds;       // grouped search: device index builds
+    else if (!strcmp(name, "where_group_units")) *out = e->where_group_units;         // where_groups search: units planned ...
+    else if (!strcmp(name, "where_group_rows_walked")) *out = e->where_group_rows_walked;   // ... and the positions they walk
     else if (!strcmp(name, "attribute_uploads")) *out = e->attribute_uploads;         // where search: attribute mirror builds
     else if (!strcmp(name, "location_uploads")) *out = e->location_uploads;           // where_near search: location mirror builds
     else if (!strcmp(name, "term_index_builds")) *out = e->term_index_builds;         // where_terms search: term index builds

@@ -120,14 +120,22 @@ class Where:
     # Term clause (wax_vs_search_batch_where_terms): up to 32 term ids the frame's set must all hold (see set_terms and
     # TermDictionary).  Empty: no term clause.
     terms: Tuple[int, ...] = ()
+    # Group clause (wax_vs_search_batch_where_groups): up to 65 536 group ids, one of which must be the frame's group (its
+    # set_groups id, else its frame id) -- VideoRAG's videoIDs as the roots of the chosen videos.  Empty: no group clause.
+    groups: Tuple[int, ...] = ()
 
     def passes(self, timestamp: int, tags: int, location: Optional[Tuple[int, int]] = None,
-               terms: Optional[Iterable[int]] = None) -> bool:
+               terms: Optional[Iterable[int]] = None, group: Optional[int] = None) -> bool:
         """The predicate on the host, as the device evaluates it; `location` is the frame's (latBin, lonBin) or None,
-        `terms` its term set or None (no terms)."""
+        `terms` its term set or None (no terms), `group` its group id (required when the where has a group clause)."""
         if not (self.after <= timestamp and (timestamp < self.before or self.before == L.INT64_MAX)
                 and (tags & self.all_tags) == self.all_tags and (tags & self.no_tags) == 0):
             return False
+        if self.groups:
+            if group is None:
+                raise ValueError("Where.passes: a where with a group clause needs the frame's group")
+            if int(group) not in set(int(g) for g in self.groups):
+                return False
         if self.terms and not set(int(t) for t in self.terms) <= set(int(t) for t in (terms or ())):
             return False
         box = None if self.near is None else location_box(*self.near)
@@ -233,12 +241,15 @@ class _WhereArgs:
         self.qw = np.asarray([L.NO_FILTER if w is None else int(w) for w in query_where], np.uint32)
         self.n_wheres = len(wheres)
         self.with_terms = any(len(w.terms) for w in wheres)     # wax_vs_search_batch_where_terms only when a term is asked
-        self.near = self.with_terms or any(w.near is not None for w in wheres)   # ... _where_near only when a box is
+        self.with_groups = any(len(w.groups) for w in wheres)   # the _where_groups entries only when a group is asked
+        # ... _where_near only when a box is; the terms and groups entries always take wax_vs_where_near
+        self.near = self.with_terms or self.with_groups or any(w.near is not None for w in wheres)
         self.warr_near = (L.WhereNear * max(len(wheres), 1))(*[w.to_c_near() for w in wheres])
         self.warr = self.warr_near if self.near else (L.Where * max(len(wheres), 1))(*[w.to_c() for w in wheres])
         self.toff = np.zeros(len(wheres) + 1, np.uint64)
         self.toff[1:] = np.cumsum([len(w.terms) for w in wheres], dtype=np.uint64) if wheres else []
         self.tflat = np.fromiter((int(t) for w in wheres for t in w.terms), dtype=np.uint64, count=int(self.toff[-1]))
+        self.goff, self.gflat = group_offsets(wheres)
 
     def filter_args(self):
         """frame_ids, filter_offsets, filter_modes, n_filters, query_filter."""
@@ -255,6 +266,20 @@ class _WhereArgs:
         """where_term_offsets, where_terms."""
         return (self.toff.ctypes.data_as(C.POINTER(C.c_uint64)),
                 self.tflat.ctypes.data_as(C.POINTER(C.c_uint64)) if self.tflat.size else None)
+
+    def group_args(self):
+        """where_group_offsets, where_groups."""
+        return (self.goff.ctypes.data_as(C.POINTER(C.c_uint64)),
+                self.gflat.ctypes.data_as(C.POINTER(C.c_uint64)) if self.gflat.size else None)
+
+
+def group_offsets(wheres: Sequence["Where"]) -> Tuple[np.ndarray, np.ndarray]:
+    """The group clauses of `wheres` as the C ABI takes them: offsets [len(wheres) + 1] from 0, where w's ids being
+    ids[offsets[w]:offsets[w + 1]] in the order given (duplicates kept; the engine drops them)."""
+    offsets = np.zeros(len(wheres) + 1, np.uint64)
+    offsets[1:] = np.cumsum([len(w.groups) for w in wheres], dtype=np.uint64) if wheres else []
+    ids = np.fromiter((int(g) for w in wheres for g in w.groups), dtype=np.uint64, count=int(offsets[-1]))
+    return offsets, ids
 
 
 # wax_vs_row_columns: one row's group, attributes and location bins, as wax_vs_export_columns / wax_vs_absorb_rows take them
@@ -641,7 +666,10 @@ class CUDAVectorEngine:
                 *a.where_args())
         tail = (ids.ctypes.data_as(C.POINTER(C.c_uint64)), scores.ctypes.data_as(C.POINTER(C.c_float)), cap,
                 ns.ctypes.data_as(C.POINTER(C.c_uint32)))
-        if a.with_terms:
+        if a.with_groups:
+            terms = a.term_args() if a.with_terms else (None, None)
+            _check(L.lib().wax_vs_search_batch_where_groups(*head, *terms, *a.group_args(), *tail))
+        elif a.with_terms:
             _check(L.lib().wax_vs_search_batch_where_terms(*head, *a.term_args(), *tail))
         else:
             entry = L.lib().wax_vs_search_batch_where_near if a.near else L.lib().wax_vs_search_batch_where
@@ -662,6 +690,10 @@ class CUDAVectorEngine:
         mode = 0 if allow is not None else 1
         qs = _as_rows(vectors, self.dimensions) if len(vectors) else np.zeros((0, self.dimensions), np.float32)
         b = qs.shape[0]
+        if where.groups:               # one where and one id filter for every query (an empty deny-list is none)
+            filters = [] if allow is None and deny is None else [(mode, fids)]
+            one = None if not filters or (mode == 1 and fids.size == 0) else 0
+            return self.search_batch_grouped_multi_where(qs, top_groups, per_group, [where], [0] * b, filters, [one] * b)
         if b == 0:
             return []
         cap = max(1, min(_clamp_topk(top_groups) * max(int(per_group), 1), L.MAX_RESULTS))
@@ -725,14 +757,20 @@ class CUDAVectorEngine:
         scores = np.empty((b, cap), np.float32)
         groups = np.empty((b, cap), np.uint64)
         ns = np.zeros(b, np.uint32)
-        _check(L.lib().wax_vs_search_batch_grouped_multi_where(
-            self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_groups), int(per_group),
-            fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
-            offsets.ctypes.data_as(C.POINTER(C.c_uint64)), modes_arr.ctypes.data_as(C.POINTER(C.c_int32)), len(lists),
-            qf.ctypes.data_as(C.POINTER(C.c_uint32)), C.cast(warr, C.c_void_p), len(wheres),
-            qw.ctypes.data_as(C.POINTER(C.c_uint32)), ids.ctypes.data_as(C.POINTER(C.c_uint64)),
-            scores.ctypes.data_as(C.POINTER(C.c_float)), groups.ctypes.data_as(C.POINTER(C.c_uint64)), cap,
-            ns.ctypes.data_as(C.POINTER(C.c_uint32))))
+        head = (self._h, qs.ctypes.data_as(C.POINTER(C.c_float)), b, qs.shape[1], int(top_groups), int(per_group),
+                fids.ctypes.data_as(C.POINTER(C.c_uint64)) if fids.size else None,
+                offsets.ctypes.data_as(C.POINTER(C.c_uint64)), modes_arr.ctypes.data_as(C.POINTER(C.c_int32)), len(lists),
+                qf.ctypes.data_as(C.POINTER(C.c_uint32)), C.cast(warr, C.c_void_p), len(wheres),
+                qw.ctypes.data_as(C.POINTER(C.c_uint32)))
+        tail = (ids.ctypes.data_as(C.POINTER(C.c_uint64)), scores.ctypes.data_as(C.POINTER(C.c_float)),
+                groups.ctypes.data_as(C.POINTER(C.c_uint64)), cap, ns.ctypes.data_as(C.POINTER(C.c_uint32)))
+        if any(w.groups for w in wheres):   # wax_vs_search_batch_grouped_multi_where_groups only when a group is asked
+            goff, gflat = group_offsets(wheres)
+            _check(L.lib().wax_vs_search_batch_grouped_multi_where_groups(
+                *head, goff.ctypes.data_as(C.POINTER(C.c_uint64)),
+                gflat.ctypes.data_as(C.POINTER(C.c_uint64)) if gflat.size else None, *tail))
+        else:
+            _check(L.lib().wax_vs_search_batch_grouped_multi_where(*head, *tail))
         result = []
         for i in range(b):
             out: List[Tuple[int, List[Tuple[int, float]]]] = []

@@ -407,6 +407,58 @@ public:
         return out;
     }
 
+    // searchBatchGroupedMultiWhere with the group ids each where admits (wax_vs_search_batch_grouped_multi_where_groups):
+    // VideoRAG's request, the best segments of the best videos among the chosen ones, for many queries at once.
+    std::vector<std::vector<Group>> searchBatchGroupedMultiWhereGroups(
+        const std::vector<std::vector<float>> &vectors, int64_t topGroups, uint32_t perGroup,
+        const std::vector<wax_vs_where_near> &wheres, const std::vector<std::vector<uint64_t>> &whereGroups,
+        const std::vector<uint32_t> &queryWhere, const std::vector<std::pair<std::vector<uint64_t>, bool>> &filters = {},
+        const std::vector<uint32_t> &queryFilter = {}) const {
+        std::vector<std::vector<Group>> out(vectors.size());
+        if (vectors.empty()) return out;
+        if (queryWhere.size() != vectors.size() || (!queryFilter.empty() && queryFilter.size() != vectors.size()))
+            throw EncodingError("searchBatchGroupedMultiWhereGroups: queryWhere / queryFilter.count != vectors.count");
+        if (whereGroups.size() != wheres.size())
+            throw EncodingError("searchBatchGroupedMultiWhereGroups: whereGroups.count != wheres.count");
+        const int64_t lim = topGroups < 1 ? 1 : (topGroups > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topGroups);
+        const int64_t want = lim * (perGroup ? perGroup : 1);
+        const size_t cap = static_cast<size_t>(want > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : want);
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchGroupedMultiWhereGroups: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        std::vector<uint64_t> frameIds, offsets(1, 0), groupOffsets(1, 0), groupIds;
+        std::vector<int32_t> modes;
+        for (const auto &f : filters) {
+            frameIds.insert(frameIds.end(), f.first.begin(), f.first.end());
+            offsets.push_back(frameIds.size());
+            modes.push_back(f.second ? 0 : 1);
+        }
+        for (const auto &g : whereGroups) {
+            groupIds.insert(groupIds.end(), g.begin(), g.end());
+            groupOffsets.push_back(groupIds.size());
+        }
+        const std::vector<uint32_t> noFilter(vectors.size(), WAX_VS_NO_FILTER);
+        const std::vector<uint32_t> &qf = queryFilter.empty() ? noFilter : queryFilter;
+        std::vector<uint64_t> ids(vectors.size() * cap), groups(vectors.size() * cap);
+        std::vector<float> scores(vectors.size() * cap);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_grouped_multi_where_groups(
+            h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_, topGroups, perGroup, frameIds.data(),
+            offsets.data(), modes.data(), static_cast<uint32_t>(filters.size()), qf.data(), wheres.data(),
+            static_cast<uint32_t>(wheres.size()), queryWhere.data(), groupOffsets.data(), groupIds.data(), ids.data(),
+            scores.data(), groups.data(), static_cast<uint32_t>(cap), ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) {
+                const size_t j = q * cap + i;
+                if (out[q].empty() || out[q].back().first != groups[j]) out[q].push_back({groups[j], {}});
+                out[q].back().second.push_back({ids[j], scores[j]});
+            }
+        return out;
+    }
+
     // Frame locations in degrees (wax_vs_set_locations): upsert; a NaN pair clears a frame's location.  Not serialized:
     // re-apply them after deserialize().
     uint64_t setLocations(const std::vector<uint64_t> &frameIds, const std::vector<double> &latitudes,
@@ -491,6 +543,49 @@ public:
                                               nullptr, offsets, nullptr, 0, queryFilter.data(), wheres.data(),
                                               static_cast<uint32_t>(wheres.size()), queryWhere.data(), termOffsets.data(),
                                               terms.data(), ids.data(), scores.data(), lim, ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) out[q].push_back({ids[q * lim + i], scores[q * lim + i]});
+        return out;
+    }
+
+    // searchBatchWhereTerms with the group ids each where admits, one of which must be the frame's group
+    // (wax_vs_search_batch_where_groups): VideoRAG's videoIDs as the roots of the chosen videos.
+    std::vector<std::vector<Hit>> searchBatchWhereGroups(const std::vector<std::vector<float>> &vectors, int64_t topK,
+                                                         const std::vector<wax_vs_where_near> &wheres,
+                                                         const std::vector<std::vector<uint64_t>> &whereTerms,
+                                                         const std::vector<std::vector<uint64_t>> &whereGroups,
+                                                         const std::vector<uint32_t> &queryWhere) const {
+        std::vector<std::vector<Hit>> out(vectors.size());
+        if (vectors.empty()) return out;
+        if (queryWhere.size() != vectors.size()) throw EncodingError("searchBatchWhereGroups: queryWhere.count != vectors.count");
+        if (whereTerms.size() != wheres.size() || whereGroups.size() != wheres.size())
+            throw EncodingError("searchBatchWhereGroups: whereTerms / whereGroups.count != wheres.count");
+        const uint32_t lim = static_cast<uint32_t>(topK < 1 ? 1 : (topK > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topK));
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchWhereGroups: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        std::vector<uint64_t> termOffsets(1, 0), terms, groupOffsets(1, 0), groups;
+        for (const auto &t : whereTerms) {
+            terms.insert(terms.end(), t.begin(), t.end());
+            termOffsets.push_back(terms.size());
+        }
+        for (const auto &g : whereGroups) {
+            groups.insert(groups.end(), g.begin(), g.end());
+            groupOffsets.push_back(groups.size());
+        }
+        const uint64_t offsets[1] = {0};
+        const std::vector<uint32_t> queryFilter(vectors.size(), WAX_VS_NO_FILTER);
+        std::vector<uint64_t> ids(vectors.size() * lim);
+        std::vector<float> scores(vectors.size() * lim);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_where_groups(h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_, topK,
+                                               nullptr, offsets, nullptr, 0, queryFilter.data(), wheres.data(),
+                                               static_cast<uint32_t>(wheres.size()), queryWhere.data(), termOffsets.data(),
+                                               terms.data(), groupOffsets.data(), groups.data(), ids.data(), scores.data(),
+                                               lim, ns.data()));
         for (size_t q = 0; q < vectors.size(); ++q)
             for (uint32_t i = 0; i < ns[q]; ++i) out[q].push_back({ids[q * lim + i], scores[q * lim + i]});
         return out;

@@ -849,6 +849,8 @@ class ShardedVectorEngine:
         torch, dist = self._torch, self._dist
         qs = np.ascontiguousarray(vectors, dtype=np.float32).reshape(-1, self.dimensions)
         b = qs.shape[0]
+        if any(w.groups for w in wheres):
+            raise ValueError("the sharded engine takes no group clause")
         a = _WhereArgs(wheres, query_where, filters, query_filter, b)
         if b == 0:
             return []
@@ -901,6 +903,8 @@ class ShardedVectorEngine:
         wheres = list(wheres or [])
         if any(w.terms for w in wheres):
             raise ValueError("grouped search takes no term clause")
+        if any(w.groups for w in wheres):
+            raise ValueError("the sharded engine takes no group clause")
         a = _WhereArgs(wheres, [None] * b if query_where is None else query_where, filters, query_filter, b)
         if b == 0:
             return []
