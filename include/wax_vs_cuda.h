@@ -77,8 +77,9 @@ int32_t wax_vs_device_count(int32_t *out);
    ids, order, score bits, counts, MV2V bytes, error codes and reasons.  It serves wax_vs_dimensions, _similarity,
    _count, _reserve, _add, _add_batch, _remove, _remove_batch, _rebalance, _search, _search_batch, _search_filtered,
    _search_batch_filtered, _search_batch_multi_filtered, _set_attributes, _set_locations, _set_terms,
-   _search_batch_where, _where_near, _where_terms, _where_groups, _set_groups, _search_grouped, _search_batch_grouped,
-   _grouped_where, _grouped_where_near, _grouped_multi_where, _grouped_multi_where_groups, _serialized_length, _serialize, _deserialize, wax_vs_debug_set_option
+   _search_batch_where, _where_near, _where_terms, _where_groups, _where_roots, _set_groups, _set_root_tags, _search_grouped,
+   _search_batch_grouped, _grouped_where, _grouped_where_near, _grouped_multi_where, _grouped_multi_where_groups,
+   _grouped_multi_where_roots, _serialized_length, _serialize, _deserialize, wax_vs_debug_set_option
    (applied to every shard) and wax_vs_debug_counter (summed over the shards, plus "shard_rows.<r>": shard r's rows);
    every other entry point (the rank-level shard_*, *_device, keyed, export, absorb and merge entries, the other debug_*) returns
    WAX_VS_ERR_UNSUPPORTED naming itself.  Grouped search with clamp(top_groups) > WAX_VS_SHARD_MAX_GROUPS is refused as
@@ -572,6 +573,69 @@ int32_t wax_vs_search_batch_grouped_multi_where_groups(wax_vs_engine *engine, co
                                                        uint64_t *out_ids, float *out_scores, uint64_t *out_groups,
                                                        uint32_t out_stride, uint32_t *out_n);
 
+/* ---- root clauses: PhotoRAG's and VideoRAG's test on each hit's root below the top-k (API EXTENSION) -----------------
+   After ranking, both orchestrators drop every hit whose root (parentId ?? id) has no meta, is not kind == root, is
+   deleted or has supersededBy set (PhotoRAGOrchestrator.swift:280-286, VideoRAGOrchestrator.swift:314-318).  Re-ingesting
+   a photo or video supersedes the old root while its segments keep their embeddings, so a grouped search filtered that
+   way afterwards comes back short.  Here each group id may hold a 64-bit root-tag word, and a where may carry a root
+   clause on it, evaluated on the device below the top-k.
+
+   Group side: wax_vs_set_root_tags keeps a word per group id; a group never given one has the word 0.  A row's group is
+   the one grouped search and the group clause use (its wax_vs_set_groups id, else its frame id).  The words are keyed
+   by group, not by row: adds, upserts, removes, set_groups and rebalance leave them alone (a row that moves to another
+   group takes that group's word), and an id no row carries yet is kept for the rows that take it later.
+   wax_vs_deserialize clears them (MV2V has no place for them; the caller re-applies them).  The word is the caller's;
+   the bindings set bits such as IS_ROOT, DELETED and SUPERSEDED from the root's FrameMeta.
+
+   Query side: a row passes the clause when its group's word holds every bit of all_tags and none of no_tags; {0, 0} is
+   no clause.  The clause passes or fails all the rows of a group together, so grouped search returns the exact top
+   groups among the groups that pass.  PhotoRAG's test is all_tags = IS_ROOT, no_tags = DELETED | SUPERSEDED (a root
+   without meta never got IS_ROOT).
+   How: the first search with a root clause after a mutation, wax_vs_set_groups or wax_vs_set_root_tags builds a device
+   column of each row's word (8 bytes per row, from the group index of grouped search; counter "root_column_builds");
+   nothing is allocated before.  Every pass that tests a where (the count, listing and bitset passes, the term and group
+   units) has a rooted form that loads the row's word beside its attributes.  Listed rows are tested on the host. */
+typedef struct wax_vs_root_clause {
+    uint64_t all_tags;  /* (word & all_tags) == all_tags */
+    uint64_t no_tags;   /* (word & no_tags)  == 0        */
+} wax_vs_root_clause;
+/* Set groups' root-tag words (upsert by group id): group_ids[i] -> tags[i]; a later entry for the same id wins, and any
+   id is accepted, carried by a row or not.  *out_assigned (optional) = distinct group ids named.  NULL group_ids or tags
+   (n > 0) -> WAX_VS_ERR_NULL.  A mutator (write lock).  A multi-device handle keeps the whole table on every shard and
+   reports one engine's *out_assigned. */
+int32_t wax_vs_set_root_tags(wax_vs_engine *engine, const uint64_t *group_ids, const uint64_t *tags, uint64_t n,
+                             uint64_t *out_assigned);
+/* wax_vs_search_batch_where_groups with a root clause in each where: where w's is where_roots[w] (NULL: no where has
+   one).  Query i's answer is identical to wax_vs_search_batch_multi_filtered under an allow-list of exactly the frames
+   that pass every clause and the id filter: same ids, order and score bits.  The argument checks of
+   wax_vs_search_batch_where_groups (its term offsets when given, and the boxes) run before the empty-engine early
+   return.  A call in which no where has a root clause runs wax_vs_search_batch_where_groups. */
+int32_t wax_vs_search_batch_where_roots(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                        uint32_t query_len, int64_t top_k, const uint64_t *frame_ids,
+                                        const uint64_t *filter_offsets, const int32_t *filter_modes, uint32_t n_filters,
+                                        const uint32_t *query_filter, const wax_vs_where_near *wheres, uint32_t n_wheres,
+                                        const uint32_t *query_where, const uint64_t *where_term_offsets,
+                                        const uint64_t *where_terms, const uint64_t *where_group_offsets,
+                                        const uint64_t *where_groups, const wax_vs_root_clause *where_roots,
+                                        uint64_t *out_ids, float *out_scores, uint32_t out_stride, uint32_t *out_n);
+/* wax_vs_search_batch_grouped_multi_where_groups with a root clause in each where, as
+   wax_vs_search_batch_where_roots takes it: PhotoRAG's and VideoRAG's request -- the best frames of the best photos or
+   videos whose root is live -- with no over-fetch.  Query i's answer is identical to wax_vs_search_grouped under an
+   allow-list of exactly the frames that pass: same frame ids, group ids, group-major order and score bits; whenever at
+   least clamp(top_groups) groups pass, that many come back.  The checks of
+   wax_vs_search_batch_grouped_multi_where_groups (and the boxes) run before the empty-engine early return.  A call in
+   which no where has a root clause runs wax_vs_search_batch_grouped_multi_where_groups. */
+int32_t wax_vs_search_batch_grouped_multi_where_roots(wax_vs_engine *engine, const float *queries, uint32_t n_queries,
+                                                      uint32_t query_len, int64_t top_groups, uint32_t per_group,
+                                                      const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                                      const int32_t *filter_modes, uint32_t n_filters,
+                                                      const uint32_t *query_filter, const wax_vs_where_near *wheres,
+                                                      uint32_t n_wheres, const uint32_t *query_where,
+                                                      const uint64_t *where_group_offsets, const uint64_t *where_groups,
+                                                      const wax_vs_root_clause *where_roots, uint64_t *out_ids,
+                                                      float *out_scores, uint64_t *out_groups, uint32_t out_stride,
+                                                      uint32_t *out_n);
+
 /* Device-resident form used by the row-sharded engine: `d_queries` (n_queries x dims) and
    `d_candidates` (n_queries x k_eff entries, k_eff = min(clamp(top_k), 10000) -- NOT clipped to N, padding
    has valid = 0) are DEVICE pointers on the engine's device; the work is enqueued on `cuda_stream`
@@ -788,7 +852,7 @@ int32_t wax_vs_debug_batch_stats(wax_vs_engine *engine, uint64_t *tensor_queries
    index builds of wax_vs_search_grouped), "attribute_uploads" (device attribute copies of the where searches),
    "term_index_builds" / "term_index_bytes" (term index builds of the where_terms searches / HBM the index holds),
    "where_group_units" / "where_group_rows_walked" (units of the where_groups searches planned on the device / the
-   candidate positions they walk), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
+   candidate positions they walk), "root_column_builds" (root column builds of the where_roots searches), "pool_allocs", "pool_reuses", "single_shadow_queries" / "single_shadow_fallbacks"
    (single queries the shadow route answered / that the fp32 scan answered after a failed proof, either shadow; read them
    while no search is running), "single_int8_queries" (single queries whose route nominated from the int8 shadow),
    "int8_shadow_bytes" / "int8_shadow_rows" (HBM held by the int8 shadow's live rows, codes and scales / rows it covers),

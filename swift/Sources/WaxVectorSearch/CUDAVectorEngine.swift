@@ -459,6 +459,67 @@ public actor CUDAVectorEngine {
         }
     }
 
+    /// `searchBatchGroupedMultiWhereGroups` with a root clause in each where
+    /// (wax_vs_search_batch_grouped_multi_where_roots): PhotoRAG's and VideoRAG's request -- the best frames of the best
+    /// photos or videos whose root is live (`whereRoots[w]` = IS_ROOT, DELETED | SUPERSEDED on the root-tag word of the
+    /// frame's group) -- with no over-fetch and no filtering afterwards.
+    public func searchBatchGroupedMultiWhereRoots(vectors: [[Float]], topGroups: Int, perGroup: Int = 1,
+                                                  wheres: [wax_vs_where_near], whereGroups: [[UInt64]],
+                                                  whereRoots: [wax_vs_root_clause], queryWhere: [Int?],
+                                                  filters: [(frameIds: [UInt64], allow: Bool)] = [],
+                                                  queryFilter: [Int?]? = nil) async throws
+        -> [[(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])]] {
+        guard !vectors.isEmpty else { return [] }
+        let dims = dimensions
+        for v in vectors where v.count != dims {
+            throw WaxError.encodingError(reason: "vector dimension mismatch: expected \(dims), got \(v.count)")
+        }
+        let perQueryFilter = queryFilter ?? [Int?](repeating: nil, count: vectors.count)
+        guard queryWhere.count == vectors.count, perQueryFilter.count == vectors.count else {
+            throw WaxError.encodingError(reason: "searchBatchGroupedMultiWhereRoots: queryWhere / queryFilter.count != vectors.count")
+        }
+        guard whereGroups.count == wheres.count, whereRoots.count == wheres.count else {
+            throw WaxError.encodingError(reason: "searchBatchGroupedMultiWhereRoots: whereGroups / whereRoots.count != wheres.count")
+        }
+        let handle = self.handle
+        let cap = max(1, min(min(max(topGroups, 1), Self.maxResults) * max(perGroup, 1), Self.maxResults))
+        return try await io.run {
+            var flat = [Float](); flat.reserveCapacity(vectors.count * dims)
+            for v in vectors { flat.append(contentsOf: v) }
+            var frameIds = [UInt64]()
+            var offsets: [UInt64] = [0]
+            var modes = [Int32]()
+            for f in filters {
+                frameIds.append(contentsOf: f.frameIds)
+                offsets.append(UInt64(frameIds.count))
+                modes.append(f.allow ? 0 : 1)
+            }
+            var groupOffsets: [UInt64] = [0]
+            var groupIds = [UInt64]()
+            for g in whereGroups { groupIds.append(contentsOf: g); groupOffsets.append(UInt64(groupIds.count)) }
+            let qf = perQueryFilter.map { $0.map(UInt32.init) ?? WAX_VS_NO_FILTER }
+            let qw = queryWhere.map { $0.map(UInt32.init) ?? WAX_VS_NO_FILTER }
+            var ids = [UInt64](repeating: 0, count: vectors.count * cap)
+            var scores = [Float](repeating: 0, count: vectors.count * cap)
+            var groups = [UInt64](repeating: 0, count: vectors.count * cap)
+            var counts = [UInt32](repeating: 0, count: vectors.count)
+            let rc = wax_vs_search_batch_grouped_multi_where_roots(handle, flat, UInt32(vectors.count), UInt32(dims),
+                                                                   Int64(topGroups), UInt32(max(perGroup, 0)), frameIds,
+                                                                   offsets, modes, UInt32(filters.count), qf, wheres,
+                                                                   UInt32(wheres.count), qw, groupOffsets, groupIds,
+                                                                   whereRoots, &ids, &scores, &groups, UInt32(cap), &counts)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return (0..<vectors.count).map { q in
+                var out: [(groupId: UInt64, hits: [(frameId: UInt64, score: Float)])] = []
+                for i in (q * cap)..<(q * cap + Int(counts[q])) {
+                    if out.last?.groupId != groups[i] { out.append((groups[i], [])) }
+                    out[out.count - 1].hits.append((ids[i], scores[i]))
+                }
+                return out
+            }
+        }
+    }
+
     /// Frame term sets (wax_vs_set_terms): each named frame's whole set is replaced, an empty list clears it.  The caller
     /// interns `("entry", key, value)`, `("tag", key, value)` and `("label", s)` exactly, so that `searchBatchWhereTerms`
     /// is `matches(metadataFilter:meta:)` below the top-k.  Not part of MV2V: re-apply after `deserialize`.
@@ -550,6 +611,65 @@ public actor CUDAVectorEngine {
                                                       offsets, nil, 0, queryFilter, wheres, UInt32(wheres.count), qw,
                                                       termOffsets, terms, groupOffsets, groupIds, &ids, &scores,
                                                       UInt32(cap), &counts)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return (0..<vectors.count).map { q in (0..<Int(counts[q])).map { (ids[q * cap + $0], scores[q * cap + $0]) } }
+        }
+    }
+
+    /// Groups' root-tag words (wax_vs_set_root_tags): upsert by group id, the bits (IS_ROOT, DELETED, SUPERSEDED) set
+    /// from each root's `FrameMeta`; a group never given one has the word 0.  Keyed by group, so adds, removes and
+    /// `setGroups` leave them alone.  Not part of MV2V: re-apply after `deserialize`.
+    @discardableResult
+    public func setRootTags(groupIds: [UInt64], tags: [UInt64]) async throws -> Int {
+        guard groupIds.count == tags.count else {
+            throw WaxError.encodingError(reason: "setRootTags: groupIds.count != tags.count")
+        }
+        guard !groupIds.isEmpty else { return 0 }
+        let handle = self.handle
+        let assigned: UInt64 = try await io.run {
+            var n: UInt64 = 0
+            let rc = wax_vs_set_root_tags(handle, groupIds, tags, UInt64(groupIds.count), &n)
+            guard rc == WAX_VS_OK else { throw Self.error(rc) }
+            return n
+        }
+        return Int(assigned)
+    }
+
+    /// `searchBatchWhereGroups` with a root clause in each where (wax_vs_search_batch_where_roots): a frame passes when
+    /// its group's root-tag word holds every bit of `all_tags` and none of `no_tags` -- PhotoRAG's and VideoRAG's test
+    /// on each hit's root, below the top-k.
+    public func searchBatchWhereRoots(vectors: [[Float]], topK: Int, wheres: [wax_vs_where_near], whereTerms: [[UInt64]],
+                                      whereGroups: [[UInt64]], whereRoots: [wax_vs_root_clause], queryWhere: [Int?]) async throws
+        -> [[(frameId: UInt64, score: Float)]] {
+        guard !vectors.isEmpty else { return [] }
+        guard whereTerms.count == wheres.count, whereGroups.count == wheres.count, whereRoots.count == wheres.count else {
+            throw WaxError.encodingError(reason: "searchBatchWhereRoots: whereTerms / whereGroups / whereRoots.count != wheres.count")
+        }
+        let dims = dimensions
+        for v in vectors where v.count != dims {
+            throw WaxError.encodingError(reason: "vector dimension mismatch: expected \(dims), got \(v.count)")
+        }
+        let handle = self.handle
+        let cap = min(max(topK, 1), Self.maxResults)
+        return try await io.run {
+            var flat = [Float](); flat.reserveCapacity(vectors.count * dims)
+            for v in vectors { flat.append(contentsOf: v) }
+            var termOffsets: [UInt64] = [0]
+            var terms = [UInt64]()
+            for t in whereTerms { terms.append(contentsOf: t); termOffsets.append(UInt64(terms.count)) }
+            var groupOffsets: [UInt64] = [0]
+            var groupIds = [UInt64]()
+            for g in whereGroups { groupIds.append(contentsOf: g); groupOffsets.append(UInt64(groupIds.count)) }
+            let offsets: [UInt64] = [0]
+            let queryFilter = [UInt32](repeating: WAX_VS_NO_FILTER, count: vectors.count)
+            let qw = queryWhere.map { $0.map(UInt32.init) ?? WAX_VS_NO_FILTER }
+            var ids = [UInt64](repeating: 0, count: vectors.count * cap)
+            var scores = [Float](repeating: 0, count: vectors.count * cap)
+            var counts = [UInt32](repeating: 0, count: vectors.count)
+            let rc = wax_vs_search_batch_where_roots(handle, flat, UInt32(vectors.count), UInt32(dims), Int64(topK), nil,
+                                                     offsets, nil, 0, queryFilter, wheres, UInt32(wheres.count), qw,
+                                                     termOffsets, terms, groupOffsets, groupIds, whereRoots, &ids, &scores,
+                                                     UInt32(cap), &counts)
             guard rc == WAX_VS_OK else { throw Self.error(rc) }
             return (0..<vectors.count).map { q in (0..<Int(counts[q])).map { (ids[q * cap + $0], scores[q * cap + $0]) } }
         }

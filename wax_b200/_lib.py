@@ -43,6 +43,11 @@ class WhereNear(C.Structure):
     _fields_ = [("where", Where), ("latitude", C.c_double), ("longitude", C.c_double), ("radius_m", C.c_double)]
 
 
+class RootClause(C.Structure):
+    """wax_vs_root_clause (16 bytes)."""
+    _fields_ = [("all_tags", C.c_uint64), ("no_tags", C.c_uint64)]
+
+
 # Every symbol include/wax_vs_cuda.h declares, with its signature.  tests/test_abi.py checks this table
 # against the header and against the built library.
 _f32p, _u64p, _u32p, _u8p = C.POINTER(C.c_float), C.POINTER(C.c_uint64), C.POINTER(C.c_uint32), C.POINTER(C.c_uint8)
@@ -114,6 +119,16 @@ SIGNATURES = {
                                                                    C.c_uint32, _u64p, _u64p, C.POINTER(C.c_int32),
                                                                    C.c_uint32, _u32p, C.c_void_p, C.c_uint32, _u32p,
                                                                    _u64p, _u64p, _u64p, _f32p, _u64p, C.c_uint32, _u32p]),
+    "wax_vs_set_root_tags": (C.c_int32, [_eng, _u64p, _u64p, C.c_uint64, _u64p]),
+    "wax_vs_search_batch_where_roots": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64, _u64p, _u64p,
+                                                    C.POINTER(C.c_int32), C.c_uint32, _u32p, C.c_void_p, C.c_uint32,
+                                                    _u32p, _u64p, _u64p, _u64p, _u64p, C.c_void_p, _u64p, _f32p,
+                                                    C.c_uint32, _u32p]),
+    "wax_vs_search_batch_grouped_multi_where_roots": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_uint32, C.c_int64,
+                                                                  C.c_uint32, _u64p, _u64p, C.POINTER(C.c_int32),
+                                                                  C.c_uint32, _u32p, C.c_void_p, C.c_uint32, _u32p,
+                                                                  _u64p, _u64p, C.c_void_p, _u64p, _f32p, _u64p,
+                                                                  C.c_uint32, _u32p]),
     "wax_vs_shard_search_where": (C.c_int32, [_eng, _f32p, C.c_uint32, C.c_int64, _u64p, C.c_uint64, C.c_int32, C.c_void_p,
                                               _u64p, C.c_uint32, _u64p, _f32p, C.c_uint32, _u32p]),
     "wax_vs_search_batch_where_device": (C.c_int32, [_eng, C.c_void_p, C.c_uint32, C.c_int64, _u64p, _u64p,

@@ -13,7 +13,7 @@ LIB = PKG / "libwaxvs_cuda.so"
 SOURCES = ["waxvs_engine.cu"]
 HEADERS = ["waxvs_common.cuh", "waxvs_shard.cuh", "waxvs_scan.cuh", "waxvs_select.cuh", "waxvs_synth.cuh", "waxvs_batch.cuh",
            "waxvs_group.cuh", "waxvs_group_batch.cuh", "waxvs_where.cuh", "waxvs_terms.cuh",
-           "waxvs_where_groups.cuh", "waxvs_multi.cuh"]
+           "waxvs_where_groups.cuh", "waxvs_roots.cuh", "waxvs_multi.cuh"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -43,11 +43,18 @@
 #include "waxvs_where.cuh"
 #include "waxvs_terms.cuh"
 #include "waxvs_where_groups.cuh"
+#include "waxvs_roots.cuh"
 
 #include <cub/cub.cuh>
 #include <cudaTypedefs.h>
 
 using namespace waxvs;
+
+// The where items and the term and group-clause units as the host plans them: every clause, the root clause included.
+// Each launch stages the form its kernels take (where_pass, launch_term_filter, launch_group_filter).
+using WhereFull = Rooted<WhereNearItem>;
+using TermUnitR = Rooted<TermUnit>;
+using GroupUnitR = Rooted<GroupUnit>;
 
 // ---------------------------------------------------------------------------------------------------------
 // errors
@@ -268,18 +275,18 @@ struct SearchCtx {
     DevBuf<ScoreItem> d_score_items;               // batched grouped search: expansion tiles (level 0)
     PinnedBuf<unsigned long long> h_flag;          // host-delivery completion flag
     unsigned long long host_seq = 0;               // last value the flag was asked to take
-    DevBuf<WhereNearItem> d_where_items;           // where search: predicates of the count / compaction / bitset launches
-                                                   // (WhereItems in the plain form)
+    DevBuf<WhereFull> d_where_items;               // where search: predicates of the count / compaction / bitset launches
+                                                   // (in the launch's form: WhereItemOf<located, rooted>)
     DevBuf<uint32_t> d_where_counts;               // where search: rows passing each predicate, then compaction cursors
     DevBuf<uint64_t> d_term_ids;                   // where_terms search: the call's distinct required term ids ...
     DevBuf<TermSpan> d_term_spans;                 // ... their posting spans
-    DevBuf<TermUnit> d_term_units;                 // ... the units of term_filter_kernel
+    DevBuf<TermUnitR> d_term_units;                // ... the units of term_filter_kernel (in the launch's form)
     DevBuf<uint32_t> d_term_counts;                // ... their counts, then listing cursors
     DevBuf<uint32_t> d_term_deny;                  // ... and their deny-lists' rows, each list ascending
     DevBuf<uint64_t> d_gw_ids;                     // where_groups search: the call's distinct group ids ...
     DevBuf<GroupSpan> d_gw_resolved;               // ... their dense groups and CSR spans
     DevBuf<GroupSpan> d_gw_spans;                  // ... each unit's groups, with their prefix
-    DevBuf<GroupUnit> d_gw_units;                  // ... the units of where_group_filter_kernel
+    DevBuf<GroupUnitR> d_gw_units;                 // ... the units of where_group_filter_kernel (in the launch's form)
     DevBuf<uint32_t> d_gw_counts;                  // ... their counts, then listing cursors
     DevBuf<uint32_t> d_gw_deny;                    // ... and their deny-lists' rows, each list ascending
     DevBuf<uint32_t> d_proof_count;                // shadow route: [0] proofs that held, [1] that failed (guarded scan) ...
@@ -396,6 +403,18 @@ struct wax_vs_engine {
     uint64_t group_index_builds = 0;   // instrumentation (pool_mu)
     uint64_t where_group_units = 0;        // where_groups search: units with a group clause planned on the device ...
     uint64_t where_group_rows_walked = 0;  // ... and the candidate positions their walks visit (pool_mu)
+    // Root tags (wax_vs_set_root_tags): the caller's 64-bit word per group id, ids ascending with their words, keyed by
+    // group and not by row, so no row mutator touches them; deserialize clears them.  The device column col[r] = the word
+    // of row r's group (waxvs_roots.cuh) is a cache like the group index: every mutator, set_groups and set_root_tags
+    // invalidate it; the first search with a root clause after that rebuilds it under root_mu.  Nothing is allocated
+    // until then.
+    struct RootTags {
+        std::vector<uint64_t> ids, tags;
+        DevBuf<uint64_t> col;
+        bool col_valid = false;
+    } roots;
+    std::mutex root_mu;
+    uint64_t root_column_builds = 0;       // instrumentation (pool_mu)
     // Frame attributes (wax_vs_set_attributes): attrs[r] = row r's (timestamp, tags), kept aligned with `ids` by every
     // mutator exactly as `groups` is.  Empty while attrs_set is false: then every row has timestamp 0 and tags 0.
     bool attrs_set = false;
@@ -525,6 +544,7 @@ static void invalidate_row_caches(wax_vs_engine *e, uint64_t keep_prefix) {
     e->norms_rows = std::min(e->norms_rows, keep_prefix);
     for (int f = 0; f < kRouteForms; ++f) e->shadows[f].invalidate(keep_prefix, f != kRouteBf16);
     e->gindex.valid = false;           // appends too: the new rows need index entries
+    e->roots.col_valid = false;        // and the root column, read through it
     e->attrs_dev_valid = false;        // likewise the attribute mirror
     e->locs_dev_valid = false;         // and the location mirror
     e->tindex.release();               // and the term index
@@ -1897,12 +1917,13 @@ static int32_t sync_device_ids(wax_vs_engine *e, const uint64_t **out) {
 }
 
 // A where as the host plans it: the time and tag clauses, the location box (kNoLocBox: no location clause) and the
-// sorted, distinct term ids a row must hold (none: no term clause), and the group clause.
+// sorted, distinct term ids a row must hold (none: no term clause), the group clause and the root clause.
 struct Clause {
     WherePred pred;
     LocBox box;
     std::vector<uint64_t> terms;
     std::vector<uint64_t> groups;      // sorted, distinct group ids, one of which the row's group must be (none: no clause)
+    RootClause root{0, 0};             // the row's group's root-tag word must pass it ({0, 0}: no clause)
 };
 
 // What a filtered, where or grouped search asks for.  Its entry point checks the arguments and builds it once (the
@@ -3043,17 +3064,17 @@ struct FilterSet {
     // listed by the device after `rows`, each item's slot being where its rows start.  Every item carries its box.
     std::vector<uint32_t> where;
     std::vector<uint64_t> allowed;
-    std::vector<WhereNearItem> preds, compact;
+    std::vector<WhereFull> preds, compact;
     uint64_t device_rows = 0;
     // Where_terms search only (plan_term_units): the narrow term units, whose rows the device lists at their slots after
     // the compact rows, and the wide ones, whose rows the device sets in their filter's bitset; term_of[f] = filter f's
     // wide unit in term_wide (empty, or WAX_VS_NO_FILTER, when it has none: its rows are the listed ones).
-    std::vector<TermUnit> term_list, term_wide;
+    std::vector<TermUnitR> term_list, term_wide;
     std::vector<uint32_t> term_of;
     // Where_groups search only (plan_group_units): filter f's group unit is group_units[group_of[f]] (empty, or
     // WAX_VS_NO_FILTER, when it has none).  A unit of <= kWhereGatherRows rows (fs.count[f]) is listed by the device at its
     // slot after the term units' rows; a wider one gets its bits set in its filter's bitset.
-    std::vector<GroupUnit> group_units;
+    std::vector<GroupUnitR> group_units;
     std::vector<uint32_t> group_of;
 };
 // query_filter = nullptr: every filter is resolved (the single-filter entry points).
@@ -3468,40 +3489,61 @@ static bool box_active(const LocBox &b) {
            b.lon_hi0 != kNoLocBox.lon_hi0 || b.lon_lo1 != kNoLocBox.lon_lo1 || b.lon_hi1 != kNoLocBox.lon_hi1;
 }
 
-// One where pass over `items` on `stream`: the items staged in c->d_where_items, then launch(form, d_items, i0, count) for
-// each kWhereChunk of them (and ++*launches unless that is nullptr).  When some box is active the form is
-// std::true_type, the located kernels over the items with their boxes, after the location mirror is brought up;
-// otherwise it is std::false_type, the plain kernels over (pred, slot), which read no location.  kNoLocBox admits every
-// row, rows without a location included, so the two forms agree wherever both apply.
-extern "C++" {     // a template, inside the C API's block
-template <class Launch>
-static int32_t where_pass(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereNearItem> &items, cudaStream_t stream,
-                          uint64_t *launches, Launch launch) {
+// Whether c is a root clause ({0, 0} is none).
+static bool root_active(const RootClause &c) { return c.all_tags != 0u || c.no_tags != 0u; }
+
+static int32_t ensure_root_column(wax_vs_engine *e, SearchCtx *c);
+
+// One where pass over `items` on `stream`: the items staged in c->d_where_items in the pass's form, then launch(located,
+// rooted, d_items, i0, count) for each kWhereChunk of them (and ++*launches unless that is nullptr).  `located` is
+// std::true_type when some box is active, the located kernels over the items with their boxes, after the location
+// mirror is brought up; otherwise std::false_type, the plain kernels, which read no location.  kNoLocBox admits every
+// row, rows without a location included, so the two forms agree wherever both apply.  Likewise `rooted` is
+// std::true_type when some item has a root clause, after the root column is brought up, and the clause {0, 0} admits
+// every row.
+extern "C++" {     // templates, inside the C API's block
+template <bool kLocated, bool kRooted, class Launch>
+static int32_t where_pass_form(SearchCtx *c, const std::vector<WhereFull> &items, cudaStream_t stream, uint64_t *launches,
+                               Launch launch) {
+    using Item = WhereItemOf<kLocated, kRooted>;
     const uint32_t m = static_cast<uint32_t>(items.size());
-    if (!m) return WAX_VS_OK;
-    const bool located = std::any_of(items.begin(), items.end(), [](const WhereNearItem &it) { return box_active(it.box); });
-    int32_t rc;
-    if ((rc = ensure_attributes(e, c, located)) || (rc = c->d_where_items.ensure(m, "where predicates"))) return rc;
-    WhereItem *plain = reinterpret_cast<WhereItem *>(c->d_where_items.p);
-    if (located) {
-        CUDA_TRY(cudaMemcpyAsync(c->d_where_items, items.data(), m * sizeof(WhereNearItem), cudaMemcpyHostToDevice, stream));
-    } else {
-        std::vector<WhereItem> h(m);
-        for (uint32_t i = 0; i < m; ++i) h[i] = WhereItem{items[i].pred, items[i].slot};
-        CUDA_TRY(cudaMemcpyAsync(plain, h.data(), m * sizeof(WhereItem), cudaMemcpyHostToDevice, stream));
+    std::vector<Item> h(m);
+    for (uint32_t i = 0; i < m; ++i) {
+        h[i].pred = items[i].pred;
+        h[i].slot = items[i].slot;
+        if constexpr (kLocated) h[i].box = items[i].box;
+        if constexpr (kRooted) h[i].root = items[i].root;
     }
+    Item *d_items = reinterpret_cast<Item *>(c->d_where_items.p);
+    CUDA_TRY(cudaMemcpyAsync(d_items, h.data(), m * sizeof(Item), cudaMemcpyHostToDevice, stream));
     for (uint32_t i0 = 0; i0 < m; i0 += kWhereChunk) {
-        if (located) launch(std::true_type{}, c->d_where_items.p + i0, i0, std::min(kWhereChunk, m - i0));
-        else launch(std::false_type{}, plain + i0, i0, std::min(kWhereChunk, m - i0));
+        launch(std::bool_constant<kLocated>{}, std::bool_constant<kRooted>{}, d_items + i0, i0, std::min(kWhereChunk, m - i0));
         if (launches) ++*launches;
     }
     CUDA_TRY(cudaGetLastError());
     return WAX_VS_OK;
 }
+template <class Launch>
+static int32_t where_pass(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereFull> &items, cudaStream_t stream,
+                          uint64_t *launches, Launch launch) {
+    const uint32_t m = static_cast<uint32_t>(items.size());
+    if (!m) return WAX_VS_OK;
+    const bool located = std::any_of(items.begin(), items.end(), [](const WhereFull &it) { return box_active(it.box); });
+    const bool rooted = std::any_of(items.begin(), items.end(), [](const WhereFull &it) { return root_active(it.root); });
+    int32_t rc;
+    if ((rc = ensure_attributes(e, c, located)) || (rooted && (rc = ensure_root_column(e, c))) ||
+        (rc = c->d_where_items.ensure(m, "where predicates")))
+        return rc;
+    if (located)
+        return rooted ? where_pass_form<true, true>(c, items, stream, launches, launch)
+                      : where_pass_form<true, false>(c, items, stream, launches, launch);
+    return rooted ? where_pass_form<false, true>(c, items, stream, launches, launch)
+                  : where_pass_form<false, false>(c, items, stream, launches, launch);
+}
 }  // extern "C++"
 
 // counts[i] = the rows passing items[i]: one streaming pass per kWhereChunk predicates, read back once.
-static int32_t where_counts(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereNearItem> &items,
+static int32_t where_counts(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereFull> &items,
                             std::vector<uint32_t> &counts) {
     const uint32_t m = static_cast<uint32_t>(items.size()), n = static_cast<uint32_t>(e->n_rows);
     counts.assign(m, 0u);
@@ -3509,10 +3551,12 @@ static int32_t where_counts(wax_vs_engine *e, SearchCtx *c, const std::vector<Wh
     int32_t rc;
     if ((rc = c->d_where_counts.ensure(m, "where counts"))) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_where_counts, 0, m * sizeof(uint32_t), c->stream));
-    if ((rc = where_pass(e, c, items, c->stream, nullptr, [&](auto located, const auto *d_items, uint32_t i0, uint32_t count) {
-             where_count_kernel<decltype(located)::value><<<where_grid(e, n), kWhereThreads, 0, c->stream>>>(
-                 e->d_attrs, e->d_locs, n, d_items, count, c->d_where_counts + i0);
-         })))
+    if ((rc = where_pass(e, c, items, c->stream, nullptr,
+                         [&](auto located, auto rooted, const auto *d_items, uint32_t i0, uint32_t count) {
+                             where_count_kernel<decltype(located)::value, decltype(rooted)::value>
+                                 <<<where_grid(e, n), kWhereThreads, 0, c->stream>>>(e->d_attrs, e->d_locs, n, d_items, count,
+                                                                                    c->d_where_counts + i0, e->roots.col);
+                         })))
         return rc;
     CUDA_TRY(cudaMemcpyAsync(counts.data(), c->d_where_counts, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -3520,40 +3564,63 @@ static int32_t where_counts(wax_vs_engine *e, SearchCtx *c, const std::vector<Wh
 }
 
 // ANDs items[i] into bitset items[i].slot of c->d_mask on `stream` (after the filter builders wrote it).
-static int32_t apply_where_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereNearItem> &items, cudaStream_t stream,
+static int32_t apply_where_bits(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereFull> &items, cudaStream_t stream,
                                 uint64_t *launches) {
     const uint32_t n = static_cast<uint32_t>(e->n_rows), words = (n + 31u) / 32u;
-    return where_pass(e, c, items, stream, launches, [&](auto located, const auto *d_items, uint32_t, uint32_t count) {
-        where_bits_kernel<decltype(located)::value><<<where_grid(e, static_cast<uint64_t>(words) * 32u), kWhereThreads, 0,
-                                                      stream>>>(e->d_attrs, e->d_locs, n, words, c->d_mask, d_items, count);
+    return where_pass(e, c, items, stream, launches, [&](auto located, auto rooted, const auto *d_items, uint32_t, uint32_t count) {
+        where_bits_kernel<decltype(located)::value, decltype(rooted)::value>
+            <<<where_grid(e, static_cast<uint64_t>(words) * 32u), kWhereThreads, 0, stream>>>(
+                e->d_attrs, e->d_locs, n, words, c->d_mask, d_items, count, e->roots.col);
     });
 }
 
 // The rows of the narrow predicates (fs.compact) into c->d_filter_rows at their slots, on `stream`.
-static int32_t list_where_rows(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereNearItem> &items, cudaStream_t stream,
+static int32_t list_where_rows(wax_vs_engine *e, SearchCtx *c, const std::vector<WhereFull> &items, cudaStream_t stream,
                                uint64_t *launches) {
     const uint32_t m = static_cast<uint32_t>(items.size()), n = static_cast<uint32_t>(e->n_rows);
     if (!m) return WAX_VS_OK;
     int32_t rc;
     if ((rc = c->d_where_counts.ensure(m, "where cursors"))) return rc;
     CUDA_TRY(cudaMemsetAsync(c->d_where_counts, 0, m * sizeof(uint32_t), stream));
-    return where_pass(e, c, items, stream, launches, [&](auto located, const auto *d_items, uint32_t i0, uint32_t count) {
-        where_compact_kernel<decltype(located)::value><<<where_grid(e, n), kWhereThreads, 0, stream>>>(
-            e->d_attrs, e->d_locs, n, d_items, count, c->d_where_counts + i0, c->d_filter_rows);
+    return where_pass(e, c, items, stream, launches, [&](auto located, auto rooted, const auto *d_items, uint32_t i0, uint32_t count) {
+        where_compact_kernel<decltype(located)::value, decltype(rooted)::value><<<where_grid(e, n), kWhereThreads, 0, stream>>>(
+            e->d_attrs, e->d_locs, n, d_items, count, c->d_where_counts + i0, c->d_filter_rows, e->roots.col);
     });
 }
+
+// The term or group-clause units of a launch staged in `buf` on stream s, in the launch's form: as they are when some
+// unit has a root clause (*rooted = true; the root column is brought up first), else without their root clauses, the
+// unrooted form's units.
+extern "C++" {     // a template, inside the C API's block
+template <class Base>
+static int32_t stage_units(wax_vs_engine *e, SearchCtx *c, DevBuf<Rooted<Base>> &buf, const std::vector<Rooted<Base>> &units,
+                           cudaStream_t s, bool *rooted) {
+    const size_t n = units.size();
+    *rooted = std::any_of(units.begin(), units.end(), [](const Rooted<Base> &u) { return root_active(u.root); });
+    int32_t rc;
+    if (*rooted) {
+        if ((rc = ensure_root_column(e, c))) return rc;
+        CUDA_TRY(cudaMemcpyAsync(buf.p, units.data(), n * sizeof(Rooted<Base>), cudaMemcpyHostToDevice, s));
+        return WAX_VS_OK;
+    }
+    const std::vector<Base> plain(units.begin(), units.end());
+    CUDA_TRY(cudaMemcpyAsync(reinterpret_cast<Base *>(buf.p), plain.data(), n * sizeof(Base), cudaMemcpyHostToDevice, s));
+    return WAX_VS_OK;
+}
+}  // extern "C++"
 
 // term_filter_kernel over `units` on `stream` (waxvs_terms.cuh): counting into c->d_term_counts (zeroed here) and, with
 // rows_out, listing each unit's rows at its slot; or, with bits, setting them in bitset `slot` of bits.  plan_term_units
 // sized c->d_term_units and c->d_term_counts for the call's largest launch, so no buffer an earlier launch reads moves.
-static int32_t launch_term_filter(wax_vs_engine *e, SearchCtx *c, const std::vector<TermUnit> &units, uint32_t *rows_out,
+static int32_t launch_term_filter(wax_vs_engine *e, SearchCtx *c, const std::vector<TermUnitR> &units, uint32_t *rows_out,
                                   uint32_t *bits, cudaStream_t s, uint64_t *launches) {
     const uint32_t n = static_cast<uint32_t>(units.size());
     if (!n) return WAX_VS_OK;
     int32_t rc;
+    bool rooted;
     if ((rc = c->d_term_units.ensure(n, "term units")) || (rc = c->d_term_counts.ensure(n, "term counts"))) return rc;
     if (!bits) CUDA_TRY(cudaMemsetAsync(c->d_term_counts, 0, n * sizeof(uint32_t), s));
-    CUDA_TRY(cudaMemcpyAsync(c->d_term_units, units.data(), n * sizeof(TermUnit), cudaMemcpyHostToDevice, s));
+    if ((rc = stage_units(e, c, c->d_term_units, units, s, &rooted))) return rc;
     const uint32_t words = static_cast<uint32_t>((e->n_rows + 31) / 32);
     for (uint32_t u0 = 0; u0 < n; u0 += 65535u) {       // grid.y limit
         const uint32_t nu = std::min<uint32_t>(n - u0, 65535u);
@@ -3561,9 +3628,15 @@ static int32_t launch_term_filter(wax_vs_engine *e, SearchCtx *c, const std::vec
         for (uint32_t j = u0; j < u0 + nu; ++j) longest = std::max(longest, units[j].spans[0].count);
         const uint32_t spread = std::max<uint32_t>(4, static_cast<uint32_t>(e->sm_count) * 16 / nu);
         const dim3 grid(std::min<uint32_t>((longest + kTermThreads - 1) / kTermThreads, spread), nu);
-        term_filter_kernel<<<grid, kTermThreads, 0, s>>>(e->tindex.postings, e->d_attrs, e->d_locs, c->d_term_deny,
-                                                         c->d_term_units + u0, bits ? nullptr : c->d_term_counts + u0,
-                                                         rows_out, bits, words);
+        uint32_t *counts = bits ? nullptr : c->d_term_counts + u0;
+        if (rooted)
+            term_filter_kernel<true><<<grid, kTermThreads, 0, s>>>(e->tindex.postings, e->d_attrs, e->d_locs, c->d_term_deny,
+                                                                   c->d_term_units + u0, counts, rows_out, bits, words,
+                                                                   e->roots.col);
+        else
+            term_filter_kernel<false><<<grid, kTermThreads, 0, s>>>(e->tindex.postings, e->d_attrs, e->d_locs, c->d_term_deny,
+                                                                    reinterpret_cast<const TermUnit *>(c->d_term_units.p) + u0,
+                                                                    counts, rows_out, bits, words, nullptr);
         CUDA_TRY(cudaGetLastError());
         ++*launches;
     }
@@ -3576,14 +3649,15 @@ constexpr uint64_t kWhereGatherRows = 16384;   // the gather class's largest all
 // c->d_gw_counts (zeroed here) and, with rows_out, listing each unit's rows at its slot; or, with bits, setting them in
 // bitset `slot` of bits.  plan_group_units sized c->d_gw_units and c->d_gw_counts for the call's largest launch and
 // staged the units' group spans in c->d_gw_spans and their deny-lists in c->d_gw_deny.
-static int32_t launch_group_filter(wax_vs_engine *e, SearchCtx *c, const std::vector<GroupUnit> &units, uint32_t *rows_out,
+static int32_t launch_group_filter(wax_vs_engine *e, SearchCtx *c, const std::vector<GroupUnitR> &units, uint32_t *rows_out,
                                    uint32_t *bits, cudaStream_t s, uint64_t *launches) {
     const uint32_t n = static_cast<uint32_t>(units.size());
     if (!n) return WAX_VS_OK;
     int32_t rc;
+    bool rooted;
     if ((rc = c->d_gw_units.ensure(n, "group units")) || (rc = c->d_gw_counts.ensure(n, "group unit counts"))) return rc;
     if (!bits) CUDA_TRY(cudaMemsetAsync(c->d_gw_counts, 0, n * sizeof(uint32_t), s));
-    CUDA_TRY(cudaMemcpyAsync(c->d_gw_units, units.data(), n * sizeof(GroupUnit), cudaMemcpyHostToDevice, s));
+    if ((rc = stage_units(e, c, c->d_gw_units, units, s, &rooted))) return rc;
     const uint32_t words = static_cast<uint32_t>((e->n_rows + 31) / 32);
     for (uint32_t u0 = 0; u0 < n; u0 += 65535u) {       // grid.y limit
         const uint32_t nu = std::min<uint32_t>(n - u0, 65535u);
@@ -3591,10 +3665,15 @@ static int32_t launch_group_filter(wax_vs_engine *e, SearchCtx *c, const std::ve
         for (uint32_t j = u0; j < u0 + nu; ++j) longest = std::max(longest, units[j].n_cand);
         const uint32_t spread = std::max<uint32_t>(4, static_cast<uint32_t>(e->sm_count) * 16 / nu);
         const dim3 grid(std::min<uint32_t>((longest + kTermThreads - 1) / kTermThreads, spread), nu);
-        where_group_filter_kernel<<<grid, kTermThreads, 0, s>>>(e->gindex.perm, e->gindex.row_group, e->tindex.postings,
-                                                                c->d_gw_spans, e->d_attrs, e->d_locs, c->d_gw_deny,
-                                                                c->d_gw_units + u0, bits ? nullptr : c->d_gw_counts + u0,
-                                                                rows_out, bits, words);
+        uint32_t *counts = bits ? nullptr : c->d_gw_counts + u0;
+        if (rooted)
+            where_group_filter_kernel<true><<<grid, kTermThreads, 0, s>>>(
+                e->gindex.perm, e->gindex.row_group, e->tindex.postings, c->d_gw_spans, e->d_attrs, e->d_locs, c->d_gw_deny,
+                c->d_gw_units + u0, counts, rows_out, bits, words, e->roots.col);
+        else
+            where_group_filter_kernel<false><<<grid, kTermThreads, 0, s>>>(
+                e->gindex.perm, e->gindex.row_group, e->tindex.postings, c->d_gw_spans, e->d_attrs, e->d_locs, c->d_gw_deny,
+                reinterpret_cast<const GroupUnit *>(c->d_gw_units.p) + u0, counts, rows_out, bits, words, nullptr);
         CUDA_TRY(cudaGetLastError());
         ++*launches;
     }
@@ -3602,7 +3681,7 @@ static int32_t launch_group_filter(wax_vs_engine *e, SearchCtx *c, const std::ve
 }
 
 // Filter f's group unit when it is wide (its bits are set in its bitset, it lists nothing), else nullptr.
-static const GroupUnit *wide_group_unit(const FilterSet &fs, uint32_t f) {
+static const GroupUnitR *wide_group_unit(const FilterSet &fs, uint32_t f) {
     if (fs.group_of.empty() || fs.group_of[f] == WAX_VS_NO_FILTER || fs.count[f] <= kWhereGatherRows) return nullptr;
     return &fs.group_units[fs.group_of[f]];
 }
@@ -3684,21 +3763,21 @@ static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const WherePlan &
     }
     int32_t rc;
     if ((rc = build_filter_bits(e, c, spec, nf, c->stream, launches))) { cudaStreamSynchronize(c->stream); return rc; }
-    std::vector<WhereNearItem> wbits;                           // where search: the predicates ANDed in
+    std::vector<WhereFull> wbits;                               // where search: the predicates ANDed in
     for (uint32_t l = 0; l < nf && !fs.where.empty(); ++l)
         if (fs.where[which[l]] != WAX_VS_NO_FILTER) {
             wbits.push_back(fs.preds[fs.where[which[l]]]);
             wbits.back().slot = l;
         }
-    std::vector<TermUnit> tbits;                                // where_terms search: wide units' rows
+    std::vector<TermUnitR> tbits;                               // where_terms search: wide units' rows
     for (uint32_t l = 0; l < nf && !fs.term_of.empty(); ++l)
         if (fs.term_of[which[l]] != WAX_VS_NO_FILTER) {
             tbits.push_back(fs.term_wide[fs.term_of[which[l]]]);
             tbits.back().slot = l;
         }
-    std::vector<GroupUnit> gbits;                               // where_groups search: wide units' rows
+    std::vector<GroupUnitR> gbits;                              // where_groups search: wide units' rows
     for (uint32_t l = 0; l < nf; ++l)
-        if (const GroupUnit *u = wide_group_unit(fs, which[l])) {
+        if (const GroupUnitR *u = wide_group_unit(fs, which[l])) {
             gbits.push_back(*u);
             gbits.back().slot = l;
         }
@@ -3716,7 +3795,7 @@ static int32_t build_pass_bits(wax_vs_engine *e, SearchCtx *c, const WherePlan &
 static int32_t stage_pair_rows(wax_vs_engine *e, SearchCtx *c, const FilterSet &fs, uint64_t *launches) {
     int32_t rc;
     if ((rc = stage_filter_rows(e, c, fs.rows, fs.rows.size() + fs.device_rows, -1, c->stream, nullptr))) return rc;
-    std::vector<GroupUnit> glist;
+    std::vector<GroupUnitR> glist;
     for (uint32_t f = 0; f < fs.group_of.size(); ++f)
         if (fs.group_of[f] != WAX_VS_NO_FILTER && fs.count[f] && !wide_group_unit(fs, f)) glist.push_back(fs.group_units[fs.group_of[f]]);
     if ((rc = list_where_rows(e, c, fs.compact, c->stream, launches)) ||
@@ -3935,7 +4014,13 @@ static int32_t deliver_filtered(wax_vs_engine *e, SearchCtx *c, const float *que
 
 static WherePred where_pred(const wax_vs_where &w) { return WherePred{w.after, w.before, w.all_tags, w.no_tags}; }
 
-static WhereNearItem where_item(const Clause &w) { return WhereNearItem{w.pred, 0, w.box}; }
+static WhereFull where_item(const Clause &w) {
+    WhereFull it{};
+    it.pred = w.pred;
+    it.box = w.box;
+    it.root = w.root;
+    return it;
+}
 
 // Whether row r lies in box b (a row without a location lies in no active box).
 static bool host_loc_passes(const wax_vs_engine *e, const LocBox &b, uint32_t r) {
@@ -3958,13 +4043,24 @@ static bool host_group_passes(const wax_vs_engine *e, const std::vector<uint64_t
     return std::binary_search(groups.begin(), groups.end(), e->groups_set ? e->groups[r] : frame_id_of(e, r));
 }
 
+// Whether the root-tag word of row r's group (its frame id while no set_groups was made; 0 for a group never given
+// one) passes root clause rc.
+static bool host_root_passes(const wax_vs_engine *e, const RootClause &rc, uint32_t r) {
+    if (!root_active(rc)) return true;
+    const auto &ids = e->roots.ids;
+    const uint64_t g = e->groups_set ? e->groups[r] : frame_id_of(e, r);
+    const auto it = std::lower_bound(ids.begin(), ids.end(), g);
+    return root_passes(rc, it != ids.end() && *it == g ? e->roots.tags[it - ids.begin()] : 0u);
+}
+
 // The listed rows that pass every clause of `w`, appended to `out`.
 static void host_rows_passing(const wax_vs_engine *e, const Clause &w, const uint32_t *rows, uint64_t n,
                               std::vector<uint32_t> &out) {
     for (uint64_t i = 0; i < n; ++i) {
         const AttrRow a = e->attrs_set ? e->attrs[rows[i]] : AttrRow{0, 0};
         if (where_passes(w.pred, a.ts, a.tags) && host_loc_passes(e, w.box, rows[i]) &&
-            host_terms_pass(e, w.terms, rows[i]) && host_group_passes(e, w.groups, rows[i]))
+            host_terms_pass(e, w.terms, rows[i]) && host_group_passes(e, w.groups, rows[i]) &&
+            host_root_passes(e, w.root, rows[i]))
             out.push_back(rows[i]);
     }
 }
@@ -4033,7 +4129,7 @@ static int32_t plan_term_units(wax_vs_engine *e, SearchCtx *c, const std::vector
         CUDA_TRY(cudaMemcpyAsync(c->d_term_deny, deny_rows.data(), deny_rows.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, s));
 
     // each unit's candidates are the postings of its rarest term; a term no row holds leaves the unit empty
-    std::vector<TermUnit> units;
+    std::vector<TermUnitR> units;
     std::vector<uint32_t> unit_pair;
     bool located = false;
     for (const uint32_t p : units_p) {
@@ -4041,8 +4137,9 @@ static int32_t plan_term_units(wax_vs_engine *e, SearchCtx *c, const std::vector
         const uint32_t f = pairs[p].second;
         fs.first[p] = at;
         fs.count[p] = 0;
-        TermUnit u{};
+        TermUnitR u{};
         u.pred = w.pred;
+        u.root = w.root;
         u.box = w.box;
         u.has_box = box_active(w.box);
         u.n_spans = static_cast<uint32_t>(w.terms.size());
@@ -4136,7 +4233,7 @@ static int32_t plan_group_units(wax_vs_engine *e, SearchCtx *c, const std::vecto
     // each unit's groups in ascending dense order (its ids are sorted, and dense groups follow the ids' order), those no
     // row carries dropped, with the exclusive prefix of their row counts
     std::vector<GroupSpan> gspans;
-    std::vector<GroupUnit> units;
+    std::vector<GroupUnitR> units;
     std::vector<uint32_t> unit_pair;
     bool located = false;
     uint64_t walked = 0;
@@ -4145,8 +4242,9 @@ static int32_t plan_group_units(wax_vs_engine *e, SearchCtx *c, const std::vecto
         const uint32_t f = pairs[p].second;
         fs.first[p] = at;
         fs.count[p] = 0;
-        GroupUnit u{};
+        GroupUnitR u{};
         u.pred = w.pred;
+        u.root = w.root;
         u.box = w.box;
         u.has_box = box_active(w.box);
         u.deny = f == WAX_VS_NO_FILTER ? TermSpan{0, 0, 0} : deny_of[f];
@@ -4238,7 +4336,7 @@ static int32_t plan_where_pairs(wax_vs_engine *e, SearchCtx *c, const std::vecto
     }
     // the predicates whose count the plan needs: those of pairs without an allow-list
     std::vector<uint32_t> slot(wheres.size(), WAX_VS_NO_FILTER);
-    std::vector<WhereNearItem> counted;
+    std::vector<WhereFull> counted;
     for (const auto &pr : pairs)
         if (pr.first != WAX_VS_NO_FILTER && (pr.second == WAX_VS_NO_FILTER || filter_modes[pr.second] == 1) &&
             slot[pr.first] == WAX_VS_NO_FILTER && wheres[pr.first].terms.empty() && wheres[pr.first].groups.empty()) {
@@ -4628,8 +4726,9 @@ static void request_id_lists(SearchRequest &r, uint32_t n_wheres, const uint64_t
     }
 }
 
-// With a where list, wheres with terms or groups and equal contents (clauses, box, required ids, group ids) are one:
-// each query names the first of them, so a batch that scopes 1 024 queries to 16 sessions plans 16 units, not 1 024.
+// With a where list, wheres with terms or groups and equal contents (clauses, box, root clause, required ids, group ids)
+// are one: each query names the first of them, so a batch that scopes 1 024 queries to 16 sessions plans 16 units, not
+// 1 024.
 static void canonical_wheres(SearchRequest &r) {
     if (!r.query_where) return;
     const uint32_t n_wheres = static_cast<uint32_t>(r.wheres.size());
@@ -4642,6 +4741,7 @@ static void canonical_wheres(SearchRequest &r) {
         const uint64_t n_terms = cl.terms.size();
         std::string key(reinterpret_cast<const char *>(&cl.pred), sizeof(WherePred));
         key.append(reinterpret_cast<const char *>(&cl.box), sizeof(LocBox));
+        key.append(reinterpret_cast<const char *>(&cl.root), sizeof(RootClause));
         key.append(reinterpret_cast<const char *>(&n_terms), sizeof(n_terms));
         key.append(reinterpret_cast<const char *>(cl.terms.data()), cl.terms.size() * sizeof(uint64_t));
         key.append(reinterpret_cast<const char *>(cl.groups.data()), cl.groups.size() * sizeof(uint64_t));
@@ -4726,6 +4826,96 @@ int32_t wax_vs_search_batch_where_groups(wax_vs_engine *e, const float *queries,
             return rc;
     }
     if ((rc = near_clauses(wheres, n_wheres, req.wheres))) return rc;
+    if (where_term_offsets) request_id_lists(req, n_wheres, where_term_offsets, where_terms, &Clause::terms);
+    request_id_lists(req, n_wheres, where_group_offsets, where_groups, &Clause::groups);
+    canonical_wheres(req);
+    return search_where(e, req, out_ids, out_scores, out_stride, out_n);
+}
+
+// ---- root clauses: PhotoRAG's and VideoRAG's test on each hit's root, as a word per group (waxvs_roots.cuh) -----------
+// Upsert by group id: a later entry for the same id wins, and an id no row carries yet is kept for the rows that take it.
+// The table is keyed by group, so no row mutator touches it.  A multi-device handle keeps the whole table on every shard
+// (rebalance then has nothing to move) and reports one engine's count.
+int32_t wax_vs_set_root_tags(wax_vs_engine *e, const uint64_t *group_ids, const uint64_t *tags, uint64_t n,
+                             uint64_t *out_assigned) {
+    if (e && e->multi) {
+        const wax_vs_engine *first = e->multi->shards[0];
+        return multi_set(e->multi, out_assigned, [&](wax_vs_engine *s, uint64_t *got) {
+            return wax_vs_set_root_tags(s, group_ids, tags, n, s == first ? got : nullptr);
+        });
+    }
+    if (!e) return fail(WAX_VS_ERR_NULL, "engine is NULL");
+    if (out_assigned) *out_assigned = 0;
+    if (n == 0) return WAX_VS_OK;
+    if (!group_ids || !tags) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    // the call's distinct ids ascending, each with its last entry's word
+    std::vector<uint64_t> order(n);
+    for (uint64_t i = 0; i < n; ++i) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) { return group_ids[a] < group_ids[b]; });
+    std::vector<uint64_t> ids, words;
+    for (uint64_t i = 0; i < n; ++i) {
+        const uint64_t g = group_ids[order[i]];
+        if (!ids.empty() && ids.back() == g) words.back() = tags[order[i]];
+        else ids.push_back(g), words.push_back(tags[order[i]]);
+    }
+    std::unique_lock<std::shared_mutex> w(e->rw);
+    DeviceGuard g(e->device);
+    drain_device_path(e);
+    auto &rt = e->roots;
+    std::vector<uint64_t> m_ids, m_tags;            // the table merged with the call's entries, which win
+    m_ids.reserve(rt.ids.size() + ids.size());
+    m_tags.reserve(rt.ids.size() + ids.size());
+    size_t i = 0, j = 0;
+    while (i < rt.ids.size() || j < ids.size()) {
+        if (j == ids.size() || (i < rt.ids.size() && rt.ids[i] < ids[j])) {
+            m_ids.push_back(rt.ids[i]), m_tags.push_back(rt.tags[i]), ++i;
+        } else {
+            if (i < rt.ids.size() && rt.ids[i] == ids[j]) ++i;
+            m_ids.push_back(ids[j]), m_tags.push_back(words[j]), ++j;
+        }
+    }
+    rt.ids.swap(m_ids);
+    rt.tags.swap(m_tags);
+    rt.col_valid = false;
+    if (out_assigned) *out_assigned = ids.size();
+    return WAX_VS_OK;
+}
+
+// The root clauses of n_wheres wheres into r.wheres (NULL: none).  *any = some where has one.
+static void request_root_clauses(SearchRequest &r, const wax_vs_root_clause *roots, uint32_t n_wheres, bool *any) {
+    *any = false;
+    if (!roots) return;
+    for (uint32_t w = 0; w < n_wheres; ++w) {
+        r.wheres[w].root = RootClause{roots[w].all_tags, roots[w].no_tags};
+        *any = *any || root_active(r.wheres[w].root);
+    }
+}
+
+int32_t wax_vs_search_batch_where_roots(wax_vs_engine *e, const float *queries, uint32_t n_queries, uint32_t query_len,
+                                        int64_t top_k, const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                        const int32_t *filter_modes, uint32_t n_filters, const uint32_t *query_filter,
+                                        const wax_vs_where_near *wheres, uint32_t n_wheres, const uint32_t *query_where,
+                                        const uint64_t *where_term_offsets, const uint64_t *where_terms,
+                                        const uint64_t *where_group_offsets, const uint64_t *where_groups,
+                                        const wax_vs_root_clause *where_roots, uint64_t *out_ids, float *out_scores,
+                                        uint32_t out_stride, uint32_t *out_n) {
+    if (!e || !out_n) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(queries, n_queries, query_len, top_k);
+    int32_t rc;
+    bool any_group = false, any_root = false;
+    if ((rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
+        (rc = request_where_list(req, wheres, n_wheres, query_where)) ||
+        (rc = check_group_offsets(where_group_offsets, n_wheres, where_groups, &any_group)) ||
+        (where_term_offsets &&
+         (rc = check_term_offsets(where_term_offsets, n_wheres, where_terms, kMaxWhereTerms, "where_term_offsets"))) ||
+        (rc = near_clauses(wheres, n_wheres, req.wheres)))
+        return rc;
+    request_root_clauses(req, where_roots, n_wheres, &any_root);
+    if (!any_root)                     // no where has a root clause: the entry point without the clause
+        return wax_vs_search_batch_where_groups(e, queries, n_queries, query_len, top_k, frame_ids, filter_offsets,
+                                                filter_modes, n_filters, query_filter, wheres, n_wheres, query_where,
+                                                where_term_offsets, where_terms, where_group_offsets, where_groups, out_ids,
+                                                out_scores, out_stride, out_n);
     if (where_term_offsets) request_id_lists(req, n_wheres, where_term_offsets, where_terms, &Clause::terms);
     request_id_lists(req, n_wheres, where_group_offsets, where_groups, &Clause::groups);
     canonical_wheres(req);
@@ -4936,6 +5126,7 @@ int32_t wax_vs_set_groups(wax_vs_engine *e, const uint64_t *frame_ids, const uin
         if (!(written[wd] & b)) { written[wd] |= b; ++assigned; }
     }
     e->gindex.valid = false;
+    e->roots.col_valid = false;
     if (out_assigned) *out_assigned = assigned;
     return WAX_VS_OK;
 }
@@ -5023,6 +5214,39 @@ static int32_t ensure_group_index(wax_vs_engine *e, SearchCtx *c) {
     gi.valid = true;
     std::lock_guard<std::mutex> pg(e->pool_mu);
     ++e->group_index_builds;
+    return WAX_VS_OK;
+}
+
+// The root column of the current corpus, grouping and root tags (waxvs_roots.cuh), built on c's stream by the first
+// search with a root clause after a mutation, set_groups or set_root_tags: the group index brought up, the sorted table
+// uploaded, one root_column_kernel launch.  Readers hold the read lock; root_mu serialises the build, which completes
+// before the column is published.
+static int32_t ensure_root_column(wax_vs_engine *e, SearchCtx *c) {
+    int32_t rc;
+    if ((rc = ensure_group_index(e, c))) return rc;
+    std::lock_guard<std::mutex> lk(e->root_mu);
+    auto &rt = e->roots;
+    if (rt.col_valid) return WAX_VS_OK;
+    const auto &gi = e->gindex;
+    const uint32_t n_roots = static_cast<uint32_t>(rt.ids.size());
+    cudaStream_t s = c->stream;
+    DevBuf<uint64_t> d_ids, d_tags;
+    if ((rc = rt.col.ensure(std::max<uint64_t>(e->n_rows, 1), "root column")) ||
+        (rc = d_ids.ensure(std::max<uint32_t>(n_roots, 1), "root tag ids")) ||
+        (rc = d_tags.ensure(std::max<uint32_t>(n_roots, 1), "root tags")))
+        return rc;
+    if (n_roots) {
+        CUDA_TRY(cudaMemcpyAsync(d_ids, rt.ids.data(), n_roots * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+        CUDA_TRY(cudaMemcpyAsync(d_tags, rt.tags.data(), n_roots * sizeof(uint64_t), cudaMemcpyHostToDevice, s));
+    }
+    const uint64_t warps = (static_cast<uint64_t>(gi.n_groups) + 31) / 32;
+    const int grid = static_cast<int>(std::max<uint64_t>(1, std::min<uint64_t>(static_cast<uint64_t>(e->sm_count) * 8, (warps + 7) / 8)));
+    root_column_kernel<<<grid, 256, 0, s>>>(gi.ids, gi.starts, gi.perm, gi.n_groups, d_ids, d_tags, n_roots, rt.col);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaStreamSynchronize(s));              // the table is released on return
+    rt.col_valid = true;
+    std::lock_guard<std::mutex> pg(e->pool_mu);
+    ++e->root_column_builds;
     return WAX_VS_OK;
 }
 
@@ -5136,7 +5360,7 @@ static uint32_t deliver_group_keys(const wax_vs_engine *e, const uint64_t *keys,
 static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, uint32_t n_top, uint32_t per_group,
                            const std::vector<uint32_t> *rows, int32_t mode, const Clause *where, uint64_t *out_ids,
                            float *out_scores, uint64_t *out_groups, uint32_t *out_n, uint64_t *out_keys = nullptr,
-                           const GroupUnit *unit = nullptr) {
+                           const GroupUnitR *unit = nullptr) {
     const uint32_t n = static_cast<uint32_t>(e->n_rows);
     const bool filtered = rows != nullptr;
     cudaStream_t s = c->stream;
@@ -5150,7 +5374,7 @@ static int32_t grouped_one(wax_vs_engine *e, SearchCtx *c, const float *query, u
     if ((rc = c->d_out.ensure(n_top, "result buffer"))) return rc;
     if ((rc = c->h_out.ensure(n_top, "result staging"))) return rc;
     if (filtered) {
-        std::vector<GroupUnit> unit_bits;
+        std::vector<GroupUnitR> unit_bits;
         if (unit) {
             unit_bits.push_back(*unit);
             unit_bits.back().slot = 0;
@@ -5478,7 +5702,7 @@ static int32_t search_grouped_host(wax_vs_engine *e, const SearchRequest &req, c
     const FilterSet &ids = wp.ids, &fs = wp.fs;
     for (uint32_t qi : crowded) {
         const uint32_t p = wp.pair_of[qi], f = req.query_filter[qi];
-        const GroupUnit *unit = p != WAX_VS_NO_FILTER && !fs.group_of.empty() && fs.group_of[p] != WAX_VS_NO_FILTER
+        const GroupUnitR *unit = p != WAX_VS_NO_FILTER && !fs.group_of.empty() && fs.group_of[p] != WAX_VS_NO_FILTER
                                     ? &fs.group_units[fs.group_of[p]] : nullptr;
         const uint32_t w = unit ? WAX_VS_NO_FILTER : req.query_where[qi];
         const bool row_where = w != WAX_VS_NO_FILTER && (f == WAX_VS_NO_FILTER || req.filter_modes[f] == 1);
@@ -5628,6 +5852,38 @@ int32_t wax_vs_search_batch_grouped_multi_where_groups(wax_vs_engine *e, const f
                                                        n_wheres, query_where, out_ids, out_scores, out_groups, out_stride,
                                                        out_n);
     if ((rc = near_clauses(wheres, n_wheres, req.wheres))) return rc;
+    request_id_lists(req, n_wheres, where_group_offsets, where_groups, &Clause::groups);
+    canonical_wheres(req);
+    return search_grouped(e, req, out_ids, out_scores, out_groups, out_stride, out_n);
+}
+
+int32_t wax_vs_search_batch_grouped_multi_where_roots(wax_vs_engine *e, const float *queries, uint32_t n_queries,
+                                                      uint32_t query_len, int64_t top_groups, uint32_t per_group,
+                                                      const uint64_t *frame_ids, const uint64_t *filter_offsets,
+                                                      const int32_t *filter_modes, uint32_t n_filters,
+                                                      const uint32_t *query_filter, const wax_vs_where_near *wheres,
+                                                      uint32_t n_wheres, const uint32_t *query_where,
+                                                      const uint64_t *where_group_offsets, const uint64_t *where_groups,
+                                                      const wax_vs_root_clause *where_roots, uint64_t *out_ids,
+                                                      float *out_scores, uint64_t *out_groups, uint32_t out_stride,
+                                                      uint32_t *out_n) {
+    if (!e || !out_n || !out_ids || !out_scores || !out_groups) return fail(WAX_VS_ERR_NULL, "NULL argument");
+    SearchRequest req(queries, n_queries, query_len, top_groups, per_group, n_queries > 1);
+    int32_t rc;
+    bool any_group = false, any_root = false;
+    if ((rc = check_grouped_args(req)) ||
+        (rc = request_filters(req, frame_ids, filter_offsets, filter_modes, n_filters, query_filter)) ||
+        (rc = request_where_list(req, wheres, n_wheres, query_where)) ||
+        (rc = check_group_offsets(where_group_offsets, n_wheres, where_groups, &any_group)) ||
+        (rc = near_clauses(wheres, n_wheres, req.wheres)))
+        return rc;
+    request_root_clauses(req, where_roots, n_wheres, &any_root);
+    if (!any_root)                     // no where has a root clause: the entry point without the clause
+        return wax_vs_search_batch_grouped_multi_where_groups(e, queries, n_queries, query_len, top_groups, per_group,
+                                                              frame_ids, filter_offsets, filter_modes, n_filters,
+                                                              query_filter, wheres, n_wheres, query_where,
+                                                              where_group_offsets, where_groups, out_ids, out_scores,
+                                                              out_groups, out_stride, out_n);
     request_id_lists(req, n_wheres, where_group_offsets, where_groups, &Clause::groups);
     canonical_wheres(req);
     return search_grouped(e, req, out_ids, out_scores, out_groups, out_stride, out_n);
@@ -5901,6 +6157,8 @@ static int32_t deserialize_rows(wax_vs_engine *e, const uint8_t *src, uint64_t l
     e->locs_set = false;
     e->locs.clear(); e->locs.shrink_to_fit();
     clear_terms(e);
+    e->roots.ids.clear(); e->roots.ids.shrink_to_fit();   // nor root tags: the caller re-applies them (wax_vs_set_root_tags)
+    e->roots.tags.clear(); e->roots.tags.shrink_to_fit();
     invalidate_row_caches(e, 0);
     return WAX_VS_OK;
 }
@@ -6242,6 +6500,7 @@ int32_t wax_vs_debug_counter(wax_vs_engine *e, const char *name, uint64_t *out) 
     else if (!strcmp(name, "group_index_builds")) *out = e->group_index_builds;       // grouped search: device index builds
     else if (!strcmp(name, "where_group_units")) *out = e->where_group_units;         // where_groups search: units planned ...
     else if (!strcmp(name, "where_group_rows_walked")) *out = e->where_group_rows_walked;   // ... and the positions they walk
+    else if (!strcmp(name, "root_column_builds")) *out = e->root_column_builds;       // where_roots search: root column builds
     else if (!strcmp(name, "attribute_uploads")) *out = e->attribute_uploads;         // where search: attribute mirror builds
     else if (!strcmp(name, "location_uploads")) *out = e->location_uploads;           // where_near search: location mirror builds
     else if (!strcmp(name, "term_index_builds")) *out = e->term_index_builds;         // where_terms search: term index builds

@@ -85,19 +85,23 @@ __device__ __forceinline__ bool posting_has(const uint32_t *__restrict__ p, uint
 // Unit blockIdx.y's rows passing every clause: counted into counts[y] (zeroed by the caller), and with rows_out listed at
 // rows_out[units[y].slot + j], j < counts[y] (the order within a list is arbitrary: the gather class sorts by (distance,
 // row), the bitset builder sets bits), or with bits set in bits[units[y].slot * words ..] (counts may then be nullptr).
+// The rooted form (Rooted<TermUnit>) also tests the unit's root clause on the row's word in `roots`.
+template <bool kRooted>
 __global__ void __launch_bounds__(kTermThreads) term_filter_kernel(const uint32_t *__restrict__ postings,
                                                                    const AttrRow *__restrict__ attrs,
                                                                    const LocRow *__restrict__ locs,
                                                                    const uint32_t *__restrict__ deny_rows,
-                                                                   const TermUnit *__restrict__ units,
+                                                                   const RootedIf<TermUnit, kRooted> *__restrict__ units,
                                                                    uint32_t *__restrict__ counts,
                                                                    uint32_t *__restrict__ rows_out,
-                                                                   uint32_t *__restrict__ bits, uint32_t words) {
-    __shared__ TermUnit s;
+                                                                   uint32_t *__restrict__ bits, uint32_t words,
+                                                                   const uint64_t *__restrict__ roots) {
+    using Unit = RootedIf<TermUnit, kRooted>;
+    __shared__ Unit s;
     {
         uint64_t *dst = reinterpret_cast<uint64_t *>(&s);
         const uint64_t *src = reinterpret_cast<const uint64_t *>(units + blockIdx.y);
-        for (uint32_t i = threadIdx.x; i < sizeof(TermUnit) / 8; i += blockDim.x) dst[i] = src[i];
+        for (uint32_t i = threadIdx.x; i < sizeof(Unit) / 8; i += blockDim.x) dst[i] = src[i];
     }
     __syncthreads();
     const uint32_t lane = threadIdx.x & 31u, below = (1u << lane) - 1u;
@@ -115,6 +119,8 @@ __global__ void __launch_bounds__(kTermThreads) term_filter_kernel(const uint32_
                 const AttrRow a = load_attr(attrs, row);
                 pass = where_passes(s.pred, a.ts, a.tags);
             }
+            if constexpr (kRooted)
+                if (pass) pass = unit_root_passes(s, roots, row);
             if (pass && s.has_box) {
                 const LocRow l = load_loc(locs, row, true);
                 pass = loc_passes(s.box, l.lat, l.lon);

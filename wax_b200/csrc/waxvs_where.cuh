@@ -17,6 +17,11 @@
 // box: each row also carries its location bins (LocRow, 8 bytes, one 8-byte load per row beside the AttrRow's LDG.128),
 // and each predicate a box of bins (WhereNearItem) tested in registers next to the time and tag clauses.  The plain form
 // takes WhereItems, reads no location and ignores `locs`.
+//
+// Either form also has a rooted variant (kRooted = true) for PhotoRAG's and VideoRAG's root test: each row also carries
+// its group's root-tag word (one 8-byte load per row from the root column, waxvs_roots.cuh), and each item the where's
+// root clause (Rooted<Item>), tested in registers beside the others.  The unrooted forms load nothing and ignore `roots`.
+// The term and group-clause kernels (waxvs_terms.cuh, waxvs_where_groups.cuh) take the same variant of their units.
 #pragma once
 #include <cstdint>
 #include <type_traits>
@@ -63,10 +68,22 @@ struct WhereNearItem {
     uint64_t slot;
     LocBox box;
 };
-template <bool kLocated> using WhereItemOf = std::conditional_t<kLocated, WhereNearItem, WhereItem>;
+// A root clause (wax_vs_root_clause): the row's group's root-tag word holds every bit of all_tags and none of no_tags.
+// {0, 0} is no clause.
+struct RootClause {
+    uint64_t all_tags, no_tags;
+};
+
+// An item or unit of the rooted forms: the unrooted one with its where's root clause after it.
+template <class Base> struct Rooted : Base {
+    RootClause root;
+};
+template <class Base, bool kRooted> using RootedIf = std::conditional_t<kRooted, Rooted<Base>, Base>;
+template <bool kLocated, bool kRooted = false>
+using WhereItemOf = RootedIf<std::conditional_t<kLocated, WhereNearItem, WhereItem>, kRooted>;
 
 constexpr uint32_t kWhereChunk = 256;     // predicates per launch (shared memory: 10 KiB of items -- 16 KiB in the
-                                          // located form -- and 8 KiB of counts)
+                                          // located form, 4 KiB more rooted -- and 8 KiB of counts)
 constexpr uint32_t kWhereThreads = 256;
 
 // TimeRange.contains with INT64_MAX as "no upper bound" (a timestamp of INT64_MAX then passes), and the two tag tests.
@@ -92,11 +109,32 @@ __device__ __forceinline__ LocRow load_loc(const LocRow *locs, uint32_t row, boo
     return LocRow{v.x, v.y};
 }
 
-__device__ __forceinline__ bool item_passes(const WhereItem &it, const AttrRow &a, const LocRow &) {
+__host__ __device__ __forceinline__ bool root_passes(const RootClause &c, uint64_t root) {
+    return (root & c.all_tags) == c.all_tags && (root & c.no_tags) == 0u;
+}
+
+// Row `row`'s root-tag word, or 0 past the end; the unrooted forms load nothing.
+template <bool kRooted>
+__device__ __forceinline__ uint64_t load_root(const uint64_t *roots, uint32_t row, bool live) {
+    if (!kRooted || !live) return 0u;
+    return static_cast<uint64_t>(__ldg(reinterpret_cast<const unsigned long long *>(roots) + row));
+}
+
+__device__ __forceinline__ bool item_passes(const WhereItem &it, const AttrRow &a, const LocRow &, uint64_t) {
     return where_passes(it.pred, a.ts, a.tags);
 }
-__device__ __forceinline__ bool item_passes(const WhereNearItem &it, const AttrRow &a, const LocRow &l) {
+__device__ __forceinline__ bool item_passes(const WhereNearItem &it, const AttrRow &a, const LocRow &l, uint64_t) {
     return where_passes(it.pred, a.ts, a.tags) && loc_passes(it.box, l.lat, l.lon);
+}
+template <class Item>
+__device__ __forceinline__ bool item_passes(const Rooted<Item> &it, const AttrRow &a, const LocRow &l, uint64_t root) {
+    return item_passes(static_cast<const Item &>(it), a, l, root) && root_passes(it.root, root);
+}
+
+// A rooted term or group-clause unit's root clause on row `row` (waxvs_terms.cuh, waxvs_where_groups.cuh).
+template <class Unit>
+__device__ __forceinline__ bool unit_root_passes(const Rooted<Unit> &u, const uint64_t *roots, uint32_t row) {
+    return root_passes(u.root, load_root<true>(roots, row, true));
 }
 
 template <class Item>
@@ -108,12 +146,13 @@ __device__ __forceinline__ void stage_items(Item *s_items, const Item *items, ui
 
 // counts[i] += rows of [0, n) passing items[i], i < n_items <= kWhereChunk.  Each warp adds its ballots' popcounts to its
 // own shared counters (no atomics), the CTA sums them and issues one global atomic per (CTA, predicate).
-template <bool kLocated>
+template <bool kLocated, bool kRooted>
 __global__ void __launch_bounds__(kWhereThreads) where_count_kernel(const AttrRow *__restrict__ attrs,
                                                                     const LocRow *__restrict__ locs, uint32_t n,
-                                                                    const WhereItemOf<kLocated> *__restrict__ items,
-                                                                    uint32_t n_items, uint32_t *__restrict__ counts) {
-    __shared__ WhereItemOf<kLocated> s_items[kWhereChunk];
+                                                                    const WhereItemOf<kLocated, kRooted> *__restrict__ items,
+                                                                    uint32_t n_items, uint32_t *__restrict__ counts,
+                                                                    const uint64_t *__restrict__ roots) {
+    __shared__ WhereItemOf<kLocated, kRooted> s_items[kWhereChunk];
     __shared__ uint32_t s_count[kWhereThreads / 32][kWhereChunk];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     stage_items(s_items, items, n_items);
@@ -125,8 +164,9 @@ __global__ void __launch_bounds__(kWhereThreads) where_count_kernel(const AttrRo
         const bool live = row < n;
         const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
         const LocRow l = load_loc<kLocated>(locs, row, live);
+        const uint64_t root = load_root<kRooted>(roots, row, live);
         for (uint32_t i = 0; i < n_items; ++i) {
-            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && item_passes(s_items[i], a, l));
+            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && item_passes(s_items[i], a, l, root));
             if (lane == 0) s_count[warp][i] += __popc(b);
         }
     }
@@ -141,13 +181,13 @@ __global__ void __launch_bounds__(kWhereThreads) where_count_kernel(const AttrRo
 
 // bits[items[i].slot * words + word] &= the predicate's ballot over the word's 32 rows (rows >= n fail).  A warp owns a
 // word, so the read-modify-write needs no atomic; a bitset is named by at most one item of a launch.
-template <bool kLocated>
+template <bool kLocated, bool kRooted>
 __global__ void __launch_bounds__(kWhereThreads) where_bits_kernel(const AttrRow *__restrict__ attrs,
                                                                    const LocRow *__restrict__ locs, uint32_t n,
                                                                    uint32_t words, uint32_t *__restrict__ bits,
-                                                                   const WhereItemOf<kLocated> *__restrict__ items,
-                                                                   uint32_t n_items) {
-    __shared__ WhereItemOf<kLocated> s_items[kWhereChunk];
+                                                                   const WhereItemOf<kLocated, kRooted> *__restrict__ items,
+                                                                   uint32_t n_items, const uint64_t *__restrict__ roots) {
+    __shared__ WhereItemOf<kLocated, kRooted> s_items[kWhereChunk];
     const uint32_t lane = threadIdx.x & 31u;
     stage_items(s_items, items, n_items);
     __syncthreads();
@@ -157,8 +197,9 @@ __global__ void __launch_bounds__(kWhereThreads) where_bits_kernel(const AttrRow
         const bool live = row < n;
         const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
         const LocRow l = load_loc<kLocated>(locs, row, live);
+        const uint64_t root = load_root<kRooted>(roots, row, live);
         for (uint32_t i = 0; i < n_items; ++i) {
-            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && item_passes(s_items[i], a, l));
+            const uint32_t b = __ballot_sync(0xFFFFFFFFu, live && item_passes(s_items[i], a, l, root));
             if (lane == 0 && b != 0xFFFFFFFFu) bits[s_items[i].slot * words + word] &= b;
         }
     }
@@ -166,13 +207,14 @@ __global__ void __launch_bounds__(kWhereThreads) where_bits_kernel(const AttrRow
 
 // The rows passing items[i], written to rows_out[items[i].slot + j] for j < the predicate's count (cursor[i], zeroed by
 // the caller, ends at that count).  The order within a list is arbitrary: the gather class sorts by (distance, row).
-template <bool kLocated>
+template <bool kLocated, bool kRooted>
 __global__ void __launch_bounds__(kWhereThreads) where_compact_kernel(const AttrRow *__restrict__ attrs,
                                                                       const LocRow *__restrict__ locs, uint32_t n,
-                                                                      const WhereItemOf<kLocated> *__restrict__ items,
+                                                                      const WhereItemOf<kLocated, kRooted> *__restrict__ items,
                                                                       uint32_t n_items, uint32_t *__restrict__ cursor,
-                                                                      uint32_t *__restrict__ rows_out) {
-    __shared__ WhereItemOf<kLocated> s_items[kWhereChunk];
+                                                                      uint32_t *__restrict__ rows_out,
+                                                                      const uint64_t *__restrict__ roots) {
+    __shared__ WhereItemOf<kLocated, kRooted> s_items[kWhereChunk];
     const uint32_t lane = threadIdx.x & 31u;
     stage_items(s_items, items, n_items);
     __syncthreads();
@@ -183,8 +225,9 @@ __global__ void __launch_bounds__(kWhereThreads) where_compact_kernel(const Attr
         const bool live = row < n;
         const AttrRow a = live ? load_attr(attrs, row) : AttrRow{0, 0};
         const LocRow l = load_loc<kLocated>(locs, row, live);
+        const uint64_t root = load_root<kRooted>(roots, row, live);
         for (uint32_t i = 0; i < n_items; ++i) {
-            const bool pass = live && item_passes(s_items[i], a, l);
+            const bool pass = live && item_passes(s_items[i], a, l, root);
             const uint32_t b = __ballot_sync(0xFFFFFFFFu, pass);
             if (!b) continue;
             uint32_t at = 0;

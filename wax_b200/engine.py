@@ -123,14 +123,31 @@ class Where:
     # Group clause (wax_vs_search_batch_where_groups): up to 65 536 group ids, one of which must be the frame's group (its
     # set_groups id, else its frame id) -- VideoRAG's videoIDs as the roots of the chosen videos.  Empty: no group clause.
     groups: Tuple[int, ...] = ()
+    # Root clause (wax_vs_search_batch_where_roots): the root-tag word of the frame's group (see set_root_tags) must hold
+    # every bit of root_all_tags and none of root_no_tags -- PhotoRAG's and VideoRAG's test on each hit's root, e.g.
+    # root_all_tags = IS_ROOT, root_no_tags = DELETED | SUPERSEDED.  (0, 0): no root clause.
+    root_all_tags: int = 0
+    root_no_tags: int = 0
+
+    @property
+    def has_root_clause(self) -> bool:
+        return bool(self.root_all_tags or self.root_no_tags)
 
     def passes(self, timestamp: int, tags: int, location: Optional[Tuple[int, int]] = None,
-               terms: Optional[Iterable[int]] = None, group: Optional[int] = None) -> bool:
+               terms: Optional[Iterable[int]] = None, group: Optional[int] = None,
+               root_tags: Optional[int] = None) -> bool:
         """The predicate on the host, as the device evaluates it; `location` is the frame's (latBin, lonBin) or None,
-        `terms` its term set or None (no terms), `group` its group id (required when the where has a group clause)."""
+        `terms` its term set or None (no terms), `group` its group id (required when the where has a group clause),
+        `root_tags` its group's root-tag word (required when the where has a root clause; 0 for a group never given
+        one)."""
         if not (self.after <= timestamp and (timestamp < self.before or self.before == L.INT64_MAX)
                 and (tags & self.all_tags) == self.all_tags and (tags & self.no_tags) == 0):
             return False
+        if self.has_root_clause:
+            if root_tags is None:
+                raise ValueError("Where.passes: a where with a root clause needs the frame's group's root tags")
+            if (int(root_tags) & self.root_all_tags) != self.root_all_tags or int(root_tags) & self.root_no_tags:
+                return False
         if self.groups:
             if group is None:
                 raise ValueError("Where.passes: a where with a group clause needs the frame's group")
@@ -242,14 +259,16 @@ class _WhereArgs:
         self.n_wheres = len(wheres)
         self.with_terms = any(len(w.terms) for w in wheres)     # wax_vs_search_batch_where_terms only when a term is asked
         self.with_groups = any(len(w.groups) for w in wheres)   # the _where_groups entries only when a group is asked
-        # ... _where_near only when a box is; the terms and groups entries always take wax_vs_where_near
-        self.near = self.with_terms or self.with_groups or any(w.near is not None for w in wheres)
+        self.with_roots = any(w.has_root_clause for w in wheres)   # the _where_roots entries only when a root clause is
+        # ... _where_near only when a box is; the terms, groups and roots entries always take wax_vs_where_near
+        self.near = self.with_terms or self.with_groups or self.with_roots or any(w.near is not None for w in wheres)
         self.warr_near = (L.WhereNear * max(len(wheres), 1))(*[w.to_c_near() for w in wheres])
         self.warr = self.warr_near if self.near else (L.Where * max(len(wheres), 1))(*[w.to_c() for w in wheres])
         self.toff = np.zeros(len(wheres) + 1, np.uint64)
         self.toff[1:] = np.cumsum([len(w.terms) for w in wheres], dtype=np.uint64) if wheres else []
         self.tflat = np.fromiter((int(t) for w in wheres for t in w.terms), dtype=np.uint64, count=int(self.toff[-1]))
         self.goff, self.gflat = group_offsets(wheres)
+        self.roots = root_clauses(wheres)
 
     def filter_args(self):
         """frame_ids, filter_offsets, filter_modes, n_filters, query_filter."""
@@ -272,6 +291,10 @@ class _WhereArgs:
         return (self.goff.ctypes.data_as(C.POINTER(C.c_uint64)),
                 self.gflat.ctypes.data_as(C.POINTER(C.c_uint64)) if self.gflat.size else None)
 
+    def root_args(self):
+        """where_roots."""
+        return (C.cast(self.roots, C.c_void_p),)
+
 
 def group_offsets(wheres: Sequence["Where"]) -> Tuple[np.ndarray, np.ndarray]:
     """The group clauses of `wheres` as the C ABI takes them: offsets [len(wheres) + 1] from 0, where w's ids being
@@ -280,6 +303,11 @@ def group_offsets(wheres: Sequence["Where"]) -> Tuple[np.ndarray, np.ndarray]:
     offsets[1:] = np.cumsum([len(w.groups) for w in wheres], dtype=np.uint64) if wheres else []
     ids = np.fromiter((int(g) for w in wheres for g in w.groups), dtype=np.uint64, count=int(offsets[-1]))
     return offsets, ids
+
+
+def root_clauses(wheres: Sequence["Where"]) -> "C.Array":
+    """The root clauses of `wheres` as the C ABI takes them: one wax_vs_root_clause per where ((0, 0): none)."""
+    return (L.RootClause * max(len(wheres), 1))(*[L.RootClause(int(w.root_all_tags), int(w.root_no_tags)) for w in wheres])
 
 
 # wax_vs_row_columns: one row's group, attributes and location bins, as wax_vs_export_columns / wax_vs_absorb_rows take them
@@ -509,6 +537,22 @@ class CUDAVectorEngine:
                                          gids.ctypes.data_as(C.POINTER(C.c_uint64)), fids.size, C.byref(n)))
         return n.value
 
+    def set_root_tags(self, group_ids: Sequence[int], tags: Sequence[int]) -> int:
+        """Set groups' root-tag words (wax_vs_set_root_tags): upsert by group id, a later entry for the same id wins, and
+        an id no frame carries yet is kept for the frames that take it.  A group never given one has the word 0.  The
+        words are keyed by group, so adds, removes and set_groups leave them alone; they are not serialized: re-apply them
+        after deserialize().  Returns the number of distinct group ids named."""
+        gids = np.ascontiguousarray(group_ids, dtype=np.uint64).reshape(-1)
+        words = np.ascontiguousarray(tags, dtype=np.uint64).reshape(-1)
+        if gids.size != words.size:
+            raise ValueError(f"set_root_tags: {gids.size} group ids for {words.size} tag words")
+        if gids.size == 0:
+            return 0
+        n = C.c_uint64(0)
+        _check(L.lib().wax_vs_set_root_tags(self._h, gids.ctypes.data_as(C.POINTER(C.c_uint64)),
+                                            words.ctypes.data_as(C.POINTER(C.c_uint64)), gids.size, C.byref(n)))
+        return n.value
+
     def search_grouped(self, vector: Sequence[float], top_groups: int, per_group: int = 1,
                        allow: Optional[Sequence[int]] = None,
                        deny: Optional[Sequence[int]] = None) -> List[Tuple[int, List[Tuple[int, float]]]]:
@@ -666,7 +710,10 @@ class CUDAVectorEngine:
                 *a.where_args())
         tail = (ids.ctypes.data_as(C.POINTER(C.c_uint64)), scores.ctypes.data_as(C.POINTER(C.c_float)), cap,
                 ns.ctypes.data_as(C.POINTER(C.c_uint32)))
-        if a.with_groups:
+        if a.with_roots:
+            terms = a.term_args() if a.with_terms else (None, None)
+            _check(L.lib().wax_vs_search_batch_where_roots(*head, *terms, *a.group_args(), *a.root_args(), *tail))
+        elif a.with_groups:
             terms = a.term_args() if a.with_terms else (None, None)
             _check(L.lib().wax_vs_search_batch_where_groups(*head, *terms, *a.group_args(), *tail))
         elif a.with_terms:
@@ -690,7 +737,7 @@ class CUDAVectorEngine:
         mode = 0 if allow is not None else 1
         qs = _as_rows(vectors, self.dimensions) if len(vectors) else np.zeros((0, self.dimensions), np.float32)
         b = qs.shape[0]
-        if where.groups:               # one where and one id filter for every query (an empty deny-list is none)
+        if where.groups or where.has_root_clause:   # one where and one id filter for every query (an empty deny-list is none)
             filters = [] if allow is None and deny is None else [(mode, fids)]
             one = None if not filters or (mode == 1 and fids.size == 0) else 0
             return self.search_batch_grouped_multi_where(qs, top_groups, per_group, [where], [0] * b, filters, [one] * b)
@@ -764,11 +811,15 @@ class CUDAVectorEngine:
                 qw.ctypes.data_as(C.POINTER(C.c_uint32)))
         tail = (ids.ctypes.data_as(C.POINTER(C.c_uint64)), scores.ctypes.data_as(C.POINTER(C.c_float)),
                 groups.ctypes.data_as(C.POINTER(C.c_uint64)), cap, ns.ctypes.data_as(C.POINTER(C.c_uint32)))
-        if any(w.groups for w in wheres):   # wax_vs_search_batch_grouped_multi_where_groups only when a group is asked
-            goff, gflat = group_offsets(wheres)
-            _check(L.lib().wax_vs_search_batch_grouped_multi_where_groups(
-                *head, goff.ctypes.data_as(C.POINTER(C.c_uint64)),
-                gflat.ctypes.data_as(C.POINTER(C.c_uint64)) if gflat.size else None, *tail))
+        goff, gflat = group_offsets(wheres)
+        group_args = (goff.ctypes.data_as(C.POINTER(C.c_uint64)),
+                      gflat.ctypes.data_as(C.POINTER(C.c_uint64)) if gflat.size else None)
+        if any(w.has_root_clause for w in wheres):   # the _roots entry only when a root clause is asked
+            roots = root_clauses(wheres)
+            _check(L.lib().wax_vs_search_batch_grouped_multi_where_roots(*head, *group_args, C.cast(roots, C.c_void_p),
+                                                                         *tail))
+        elif any(w.groups for w in wheres):   # wax_vs_search_batch_grouped_multi_where_groups only when a group is asked
+            _check(L.lib().wax_vs_search_batch_grouped_multi_where_groups(*head, *group_args, *tail))
         else:
             _check(L.lib().wax_vs_search_batch_grouped_multi_where(*head, *tail))
         result = []

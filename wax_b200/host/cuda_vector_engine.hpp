@@ -459,6 +459,60 @@ public:
         return out;
     }
 
+    // searchBatchGroupedMultiWhereGroups with a root clause in each where (wax_vs_search_batch_grouped_multi_where_roots):
+    // PhotoRAG's and VideoRAG's request, the best frames of the best photos or videos whose root is live, with no
+    // over-fetch.  whereRoots[w] = {all_tags, no_tags} on the root-tag word of the frame's group ({0, 0}: none).
+    std::vector<std::vector<Group>> searchBatchGroupedMultiWhereRoots(
+        const std::vector<std::vector<float>> &vectors, int64_t topGroups, uint32_t perGroup,
+        const std::vector<wax_vs_where_near> &wheres, const std::vector<std::vector<uint64_t>> &whereGroups,
+        const std::vector<wax_vs_root_clause> &whereRoots, const std::vector<uint32_t> &queryWhere,
+        const std::vector<std::pair<std::vector<uint64_t>, bool>> &filters = {},
+        const std::vector<uint32_t> &queryFilter = {}) const {
+        std::vector<std::vector<Group>> out(vectors.size());
+        if (vectors.empty()) return out;
+        if (queryWhere.size() != vectors.size() || (!queryFilter.empty() && queryFilter.size() != vectors.size()))
+            throw EncodingError("searchBatchGroupedMultiWhereRoots: queryWhere / queryFilter.count != vectors.count");
+        if (whereGroups.size() != wheres.size() || whereRoots.size() != wheres.size())
+            throw EncodingError("searchBatchGroupedMultiWhereRoots: whereGroups / whereRoots.count != wheres.count");
+        const int64_t lim = topGroups < 1 ? 1 : (topGroups > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topGroups);
+        const int64_t want = lim * (perGroup ? perGroup : 1);
+        const size_t cap = static_cast<size_t>(want > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : want);
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchGroupedMultiWhereRoots: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        std::vector<uint64_t> frameIds, offsets(1, 0), groupOffsets(1, 0), groupIds;
+        std::vector<int32_t> modes;
+        for (const auto &f : filters) {
+            frameIds.insert(frameIds.end(), f.first.begin(), f.first.end());
+            offsets.push_back(frameIds.size());
+            modes.push_back(f.second ? 0 : 1);
+        }
+        for (const auto &g : whereGroups) {
+            groupIds.insert(groupIds.end(), g.begin(), g.end());
+            groupOffsets.push_back(groupIds.size());
+        }
+        const std::vector<uint32_t> noFilter(vectors.size(), WAX_VS_NO_FILTER);
+        const std::vector<uint32_t> &qf = queryFilter.empty() ? noFilter : queryFilter;
+        std::vector<uint64_t> ids(vectors.size() * cap), groups(vectors.size() * cap);
+        std::vector<float> scores(vectors.size() * cap);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_grouped_multi_where_roots(
+            h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_, topGroups, perGroup, frameIds.data(),
+            offsets.data(), modes.data(), static_cast<uint32_t>(filters.size()), qf.data(), wheres.data(),
+            static_cast<uint32_t>(wheres.size()), queryWhere.data(), groupOffsets.data(), groupIds.data(),
+            whereRoots.data(), ids.data(), scores.data(), groups.data(), static_cast<uint32_t>(cap), ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) {
+                const size_t j = q * cap + i;
+                if (out[q].empty() || out[q].back().first != groups[j]) out[q].push_back({groups[j], {}});
+                out[q].back().second.push_back({ids[j], scores[j]});
+            }
+        return out;
+    }
+
     // Frame locations in degrees (wax_vs_set_locations): upsert; a NaN pair clears a frame's location.  Not serialized:
     // re-apply them after deserialize().
     uint64_t setLocations(const std::vector<uint64_t> &frameIds, const std::vector<double> &latitudes,
@@ -586,6 +640,61 @@ public:
                                                static_cast<uint32_t>(wheres.size()), queryWhere.data(), termOffsets.data(),
                                                terms.data(), groupOffsets.data(), groups.data(), ids.data(), scores.data(),
                                                lim, ns.data()));
+        for (size_t q = 0; q < vectors.size(); ++q)
+            for (uint32_t i = 0; i < ns[q]; ++i) out[q].push_back({ids[q * lim + i], scores[q * lim + i]});
+        return out;
+    }
+
+    // Groups' root-tag words (wax_vs_set_root_tags): upsert by group id, e.g. IS_ROOT, DELETED and SUPERSEDED bits from
+    // each root's FrameMeta; a group never given one has the word 0.  Keyed by group, so row mutations leave them alone;
+    // not serialized: re-apply them after deserialize().
+    uint64_t setRootTags(const std::vector<uint64_t> &groupIds, const std::vector<uint64_t> &tags) {
+        if (groupIds.size() != tags.size()) throw EncodingError("setRootTags: groupIds.count != tags.count");
+        uint64_t assigned = 0;
+        if (groupIds.empty()) return 0;
+        check(wax_vs_set_root_tags(h_, groupIds.data(), tags.data(), groupIds.size(), &assigned));
+        return assigned;
+    }
+
+    // searchBatchWhereGroups with a root clause in each where (wax_vs_search_batch_where_roots): whereRoots[w] =
+    // {all_tags, no_tags} on the root-tag word of the frame's group ({0, 0}: none).
+    std::vector<std::vector<Hit>> searchBatchWhereRoots(const std::vector<std::vector<float>> &vectors, int64_t topK,
+                                                        const std::vector<wax_vs_where_near> &wheres,
+                                                        const std::vector<std::vector<uint64_t>> &whereTerms,
+                                                        const std::vector<std::vector<uint64_t>> &whereGroups,
+                                                        const std::vector<wax_vs_root_clause> &whereRoots,
+                                                        const std::vector<uint32_t> &queryWhere) const {
+        std::vector<std::vector<Hit>> out(vectors.size());
+        if (vectors.empty()) return out;
+        if (queryWhere.size() != vectors.size()) throw EncodingError("searchBatchWhereRoots: queryWhere.count != vectors.count");
+        if (whereTerms.size() != wheres.size() || whereGroups.size() != wheres.size() || whereRoots.size() != wheres.size())
+            throw EncodingError("searchBatchWhereRoots: whereTerms / whereGroups / whereRoots.count != wheres.count");
+        const uint32_t lim = static_cast<uint32_t>(topK < 1 ? 1 : (topK > WAX_VS_MAX_RESULTS ? WAX_VS_MAX_RESULTS : topK));
+        std::vector<float> flat;
+        flat.reserve(vectors.size() * dimensions_);
+        for (const auto &v : vectors) {
+            if (v.size() != dimensions_) throw EncodingError("searchBatchWhereRoots: vector dimension mismatch");
+            flat.insert(flat.end(), v.begin(), v.end());
+        }
+        std::vector<uint64_t> termOffsets(1, 0), terms, groupOffsets(1, 0), groups;
+        for (const auto &t : whereTerms) {
+            terms.insert(terms.end(), t.begin(), t.end());
+            termOffsets.push_back(terms.size());
+        }
+        for (const auto &g : whereGroups) {
+            groups.insert(groups.end(), g.begin(), g.end());
+            groupOffsets.push_back(groups.size());
+        }
+        const uint64_t offsets[1] = {0};
+        const std::vector<uint32_t> queryFilter(vectors.size(), WAX_VS_NO_FILTER);
+        std::vector<uint64_t> ids(vectors.size() * lim);
+        std::vector<float> scores(vectors.size() * lim);
+        std::vector<uint32_t> ns(vectors.size());
+        check(wax_vs_search_batch_where_roots(h_, flat.data(), static_cast<uint32_t>(vectors.size()), dimensions_, topK,
+                                              nullptr, offsets, nullptr, 0, queryFilter.data(), wheres.data(),
+                                              static_cast<uint32_t>(wheres.size()), queryWhere.data(), termOffsets.data(),
+                                              terms.data(), groupOffsets.data(), groups.data(), whereRoots.data(),
+                                              ids.data(), scores.data(), lim, ns.data()));
         for (size_t q = 0; q < vectors.size(); ++q)
             for (uint32_t i = 0; i < ns[q]; ++i) out[q].push_back({ids[q * lim + i], scores[q * lim + i]});
         return out;

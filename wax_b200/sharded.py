@@ -851,6 +851,8 @@ class ShardedVectorEngine:
         b = qs.shape[0]
         if any(w.groups for w in wheres):
             raise ValueError("the sharded engine takes no group clause")
+        if any(w.has_root_clause for w in wheres):
+            raise ValueError("the sharded engine takes no root clause")
         a = _WhereArgs(wheres, query_where, filters, query_filter, b)
         if b == 0:
             return []
@@ -905,6 +907,8 @@ class ShardedVectorEngine:
             raise ValueError("grouped search takes no term clause")
         if any(w.groups for w in wheres):
             raise ValueError("the sharded engine takes no group clause")
+        if any(w.has_root_clause for w in wheres):
+            raise ValueError("the sharded engine takes no root clause")
         a = _WhereArgs(wheres, [None] * b if query_where is None else query_where, filters, query_filter, b)
         if b == 0:
             return []
